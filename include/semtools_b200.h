@@ -346,6 +346,10 @@ int stb_debug_ticket_check(stb_ctx *ctx, uint64_t *device_value, uint64_t *host_
  * [0] first CTA start, [1] last scan end, [2] last CTA merge end, [3] final ticket,
  * [4] select done, [5] re-rank done. */
 int stb_debug_timestamps(stb_ctx *ctx, int reset, uint64_t out[8]);
+/* Rows the q8 tier's top-k prefilter passed on to the int8 codes, summed over the
+ * top-k launches since the last reset (reset != 0 zeroes the counter after reading it).
+ * Synchronises the context's stream. */
+int stb_debug_q4_refined(stb_ctx *ctx, int reset, uint64_t *refined);
 /* Test hook for K2: shadow build + wgmma GEMM on host inputs; out_full receives the
  * approximate cosine matrix [ceil(nq/128)*128][ceil(n/256)*256] (f32), out_submax (may be
  * NULL) the per-32-row maxima [ceil(nq/128)][ceil(n/256)*8][128]. */

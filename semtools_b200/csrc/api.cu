@@ -112,10 +112,16 @@ int stb_ctx_create(int device, void *cuda_stream, stb_ctx **out) {
     if ((rc = dev_reserve(&c->hist_dev, &one, 4096)) != STB_OK) goto fail;
     one = 0;
     if ((rc = dev_reserve(&c->tickets, &one, STB_TICKET_SLOTS)) != STB_OK) goto fail;
+    one = 0;
+    if ((rc = dev_reserve(&c->q4_thr, &one, STB_TICKET_SLOTS * STB_Q4_WORDS)) != STB_OK) goto fail;
+    one = 0;
+    if ((rc = dev_reserve(&c->q4_refined, &one, 1)) != STB_OK) goto fail;
   }
   if ((rc = dev_reserve(&c->hits_dev, &c->hits_cap, 1024)) != STB_OK) goto fail;
   if (cudaMemset(c->counters, 0, c->counters_cap * sizeof(unsigned int)) != cudaSuccess ||
       cudaMemset(c->tickets, 0, STB_TICKET_SLOTS * sizeof(unsigned long long)) != cudaSuccess ||
+      cudaMemset(c->q4_thr, 0, STB_TICKET_SLOTS * STB_Q4_WORDS * sizeof(unsigned long long)) != cudaSuccess ||
+      cudaMemset(c->q4_refined, 0, sizeof(unsigned long long)) != cudaSuccess ||
       cudaMemset(c->err_flag, 0, sizeof(int)) != cudaSuccess ||
       cudaMallocHost((void **)&c->q_pin, STB_D * sizeof(float)) != cudaSuccess ||
       cudaMallocHost((void **)&c->status_pin, 8 * sizeof(uint32_t)) != cudaSuccess ||
@@ -141,7 +147,7 @@ int stb_ctx_destroy(stb_ctx *c) {
   cudaFree(c->block_keys); cudaFree(c->counters); cudaFree(c->q_dev); cudaFree(c->hits_dev);
   cudaFree(c->status_dev); cudaFree(c->collect_rows); cudaFree(c->collect_count);
   cudaFree(c->collect_hits); cudaFree(c->ranges_dev); cudaFree(c->err_flag);
-  cudaFree(c->tickets);
+  cudaFree(c->tickets); cudaFree(c->q4_thr); cudaFree(c->q4_refined);
   cudaFree(c->dbg_dev); cudaFree(c->hist_dev); cudaFree(c->bq_tiles); cudaFree(c->b_submax); cudaFree(c->b_tilemax); cudaFree(c->b_cand);
   cudaFree(c->b_thr); cudaFree(c->b_cnt); cudaFree(c->b_keys);
   cudaFree(c->bq_dev); cudaFree(c->bh_dev); cudaFree(c->bs_dev); cudaFree(c->embed_off_dev); cudaFree(c->embed_ids_dev); cudaFree(c->embed_out_dev);
@@ -195,6 +201,19 @@ int stb_debug_ticket_check(stb_ctx *ctx, uint64_t *device_value, uint64_t *host_
   if (device_value) *device_value = dsum;          // sums over the counter ring
   if (host_value) *host_value = hsum;
   if (bad >= 0) { stb_set_error("ticket counter %d is %llu, host expects %llu", bad, v[bad], ctx->ticket_next[bad]); return STB_ERR_STATE; }
+  return STB_OK;
+}
+
+// Rows the q8 tier's prefilter passed on to the int8 codes, summed over the top-k launches since the
+// last reset.  Synchronises.
+int stb_debug_q4_refined(stb_ctx *ctx, int reset, uint64_t *refined) {
+  int rc = ctx_use(ctx);
+  if (rc) return rc;
+  unsigned long long v = 0;
+  STB_CUDA(cudaStreamSynchronize(ctx->stream));
+  STB_CUDA(cudaMemcpy(&v, ctx->q4_refined, sizeof(v), cudaMemcpyDeviceToHost));
+  if (reset) STB_CUDA(cudaMemset(ctx->q4_refined, 0, sizeof(v)));
+  if (refined) *refined = v;
   return STB_OK;
 }
 
@@ -299,6 +318,8 @@ int stb_corpus_destroy(stb_corpus *c) {
   cudaFree(c->shadow);
   cudaFree(c->q8);
   cudaFree(c->q8_scale);
+  cudaFree(c->q4);
+  cudaFree(c->q4_sr);
   cudaFree(c->rows);
   cudaGetLastError();
   delete c;
@@ -905,23 +926,33 @@ static int corpus_ensure_q8(stb_ctx *ctx, stb_corpus *c) {
   }
   uint64_t first = (c->q8 && c->q8_rows < c->n && !c->q8_bad) ? c->q8_rows : 0;      // valid prefix: convert only the new rows
   if (c->n > c->q8_cap_rows || !c->q8) {
-    uint8_t *np = nullptr;
+    // int8 codes + scales (260 B/row) and the top-k prefilter's nibble plane + {s, rho} (136 B/row)
+    uint8_t *np = nullptr, *pp = nullptr;
     float *ns = nullptr;
+    float2 *sp = nullptr;
     const uint64_t cap = std::max<uint64_t>(c->n, c->capacity);
     cudaError_t e = cudaMalloc((void **)&np, cap * 256ull);
     if (e == cudaSuccess) e = cudaMalloc((void **)&ns, cap * sizeof(float));
-    if (e != cudaSuccess) { cudaGetLastError(); cudaFree(np); stb_set_error("q8 tier: cannot allocate %llu MiB", (unsigned long long)(cap * 260 >> 20)); return STB_ERR_NOMEM; }
+    if (e == cudaSuccess) e = cudaMalloc((void **)&pp, cap * 128ull);
+    if (e == cudaSuccess) e = cudaMalloc((void **)&sp, cap * sizeof(float2));
+    if (e != cudaSuccess) {
+      cudaGetLastError(); cudaFree(np); cudaFree(ns); cudaFree(pp);
+      stb_set_error("q8 tier: cannot allocate %llu MiB", (unsigned long long)(cap * 396 >> 20));
+      return STB_ERR_NOMEM;
+    }
     if (c->q8 && first) {
       STB_CUDA(cudaMemcpyAsync(np, c->q8, first * 256ull, cudaMemcpyDeviceToDevice, ctx->stream));
       STB_CUDA(cudaMemcpyAsync(ns, c->q8_scale, first * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
+      STB_CUDA(cudaMemcpyAsync(pp, c->q4, first * 128ull, cudaMemcpyDeviceToDevice, ctx->stream));
+      STB_CUDA(cudaMemcpyAsync(sp, c->q4_sr, first * sizeof(float2), cudaMemcpyDeviceToDevice, ctx->stream));
       STB_CUDA(cudaStreamSynchronize(ctx->stream));
     } else first = 0;
-    cudaFree(c->q8); cudaFree(c->q8_scale);
-    c->q8 = np; c->q8_scale = ns; c->q8_cap_rows = cap;
+    cudaFree(c->q8); cudaFree(c->q8_scale); cudaFree(c->q4); cudaFree(c->q4_sr);
+    c->q8 = np; c->q8_scale = ns; c->q4 = pp; c->q4_sr = sp; c->q8_cap_rows = cap;
   }
   int rc;
   STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
-  if ((rc = stb_launch_q8_build(ctx, c->rows, first, c->n, c->q8, c->q8_scale, ctx->err_flag)) != STB_OK) return rc;
+  if ((rc = stb_launch_q8_build(ctx, c->rows, first, c->n, c->q8, c->q8_scale, c->q4, c->q4_sr, ctx->err_flag)) != STB_OK) return rc;
   int flag = 0;
   STB_CUDA(cudaMemcpyAsync(&flag, ctx->err_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));

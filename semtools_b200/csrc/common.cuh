@@ -51,6 +51,10 @@
 // the q8 tier always keeps K' = 128 candidates; beyond this top_k the gap between the k-th and
 // the 128th best is too small for its ~0.01 per-row error term to prove anything
 #define STB_Q8_MAX_K 16
+// the q8 tier's top-k scan skips a row whose 4-bit upper bound u4 (>= c - 1e-5) is below the proven
+// threshold T (<= c_k - 1e-5) by more than this: then c < c_k strictly (scan_topk.cu: stb_scan_q4)
+#define STB_Q4_SKIP_EPS 2.0e-5
+#define STB_Q4_WORDS 16     // threshold words per launch slot (>= STB_Q8_MAX_K)
 
 void stb_set_error(const char *fmt, ...);
 
@@ -81,6 +85,11 @@ struct stb_ctx {
   unsigned long long ticket_next[8];   // per slot: its value when the next launch using it starts
   unsigned long long topk_launches;    // picks the slot
   bool ticket_ring;                    // set by the first overlapped launch; until then every launch uses slot 0
+  // q8 tier prefilter (scan_topk.cu: stb_scan_q4): STB_TICKET_SLOTS x STB_Q4_WORDS tagged threshold words,
+  // one slot per launch in turn; the launch count is the tag
+  unsigned long long *q4_thr;
+  unsigned long long q4_launches;
+  unsigned long long *q4_refined;      // rows the prefilter passed on to the int8 codes (stb_debug_q4_refined)
   float *q_dev;             // 256 f32 staging for host queries
   stb_hit *hits_dev;        // result hits (top-k path)
   size_t hits_cap;
@@ -186,7 +195,9 @@ struct stb_corpus {
   // K1 tier q8: int8 codes [capacity][256] + per-row scale, built lazily / by stb_corpus_prepare
   uint8_t *q8;
   float *q8_scale;
-  uint64_t q8_rows;          // rows covered (== n when valid)
+  uint8_t *q4;               // ... its nibble plane [capacity][128] and per-row {s, rho} (top-k prefilter)
+  float2 *q4_sr;
+  uint64_t q8_rows;          // rows covered (== n when valid; also the plane's)
   uint64_t q8_cap_rows;
   int q8_bad;
   // per-tier bookkeeping: a reduced-width tier is skipped once it proves fewer than half of its
@@ -207,9 +218,9 @@ int stb_launch_scan_topk(stb_ctx *ctx, const stb_corpus *c, int tier, const floa
                          const uint64_t *ranges_dev, uint32_t n_ranges,
                          uint64_t n_virtual, stb_hit *out_hits_dev,
                          uint32_t *out_status_dev, const StbXchgArgs *xchg = nullptr, bool overlapped = false);
-// int8 codes + scales of rows [first_row, n_rows) (q8 tier)
+// int8 codes + scales, nibble plane + {s, rho} of rows [first_row, n_rows) (q8 tier)
 int stb_launch_q8_build(stb_ctx *ctx, const float *rows_dev, uint64_t first_row, uint64_t n_rows, uint8_t *out,
-                        float *scale, int *bad_flag_dev);
+                        float *scale, uint8_t *plane, float2 *sr, int *bad_flag_dev);
 // Largest top_k the fast path serves.
 uint32_t stb_scan_topk_max_k(void);
 // Collect path: every row whose approximate cosine >= cos_floor (or that cannot be

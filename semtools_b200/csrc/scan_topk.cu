@@ -8,7 +8,9 @@
 // HBM-bound: the only large traffic is the corpus matrix, 1 KiB per row, read
 // exactly once with 128-bit coalesced loads (8 lanes cover one 128-byte line of a
 // row; a warp instruction touches 4 full lines).  Everything else (query, K'
-// candidates per CTA, k results) is bytes.
+// candidates per CTA, k results) is bytes.  The narrower candidate tiers read less: the 16-bit
+// shadow 512 B per row; the q8 tier's top-k scan a 136 B/row 4-bit plane, plus the 260 B int8 codes
+// of the few rows whose 4-bit bound can still reach the k-th best (stb_scan_q4).
 //
 // Exactness: the streaming pass ranks rows by an fp32 approximate cosine and keeps
 // the best K' = 32*E per warp; the surviving K' of the whole grid are re-scored by
@@ -346,13 +348,34 @@ __device__ __forceinline__ void stb_scan_shadow(const ScanArgs &args, const uint
 // term folded into the score, so rows with a large scale are promoted instead of widening a
 // global margin.  A zero or unscorable query makes every score +inf: the proof fails and the
 // caller falls through to the f32 tiers.
-template <int U, int RANGES, class Sink>
-__device__ __forceinline__ void stb_scan_q8(const ScanArgs &args, const uint8_t *q8, const float *q8_scale, Sink &sink) {
-  const int lane = threadIdx.x & 31;
-  const int g = lane >> 3;   // row group inside the warp
-  const int j = lane & 7;    // this lane reads row bytes [16j, 16j+16) and [128+16j, 128+16j+16)
+// q16 of four query components (scaled by qs), split into a high and a low signed byte word
+__device__ __forceinline__ void stb_q16_words(float4 q, float qs, bool unusable, uint32_t &hw, uint32_t &lw, int &l1, int &sum) {
+  const float f[4] = {q.x, q.y, q.z, q.w};
+  hw = 0; lw = 0;
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    int v = unusable ? 0 : __float2int_rn(f[e] * qs);
+    v = max(-32639, min(32639, v));
+    l1 += abs(v);
+    sum += v;
+    const int lo = ((v + 128) & 255) - 128;               // signed low byte
+    const int hi = (v - lo) >> 8;                         // exact: v - lo is a multiple of 256
+    hw |= (uint32_t)(hi & 255) << (8 * e);
+    lw |= (uint32_t)(lo & 255) << (8 * e);
+  }
+}
+
+// The query as the q8 tier sees it (see stb_scan_q8); lane j holds the components of row bytes
+// [16j, 16j+16) and [128+16j, 128+16j+16).
+struct StbQ8Query {
+  uint32_t qhi[8], qlo[8];
+  float S, qs, inv_S, h_l1, e_q;
+  bool unusable;
+};
+__device__ __forceinline__ StbQ8Query stb_q8_query(const float *qf, int j) {
+  StbQ8Query Q;
   float4 q[8];
-  const float4 *q4 = reinterpret_cast<const float4 *>(args.q);
+  const float4 *q4 = reinterpret_cast<const float4 *>(qf);
 #pragma unroll
   for (int i = 0; i < 4; ++i) { q[i] = __ldg(q4 + 4 * j + i); q[4 + i] = __ldg(q4 + 32 + 4 * j + i); }
   const StbQueryNorm qn = stb_query_norm(q);
@@ -365,33 +388,59 @@ __device__ __forceinline__ void stb_scan_q8(const ScanArgs &args, const uint8_t 
   amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
   amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
   amax *= qn.rq;                                            // max |q^_i|
-  const bool q_unusable = qn.q_zero || qn.q_bad || !(amax > 0.f && amax <= 1.0001f);
-  const float S = q_unusable ? 1.f : 32639.0f / amax;
-  const float qs = qn.rq * S;
-  uint32_t qhi[8], qlo[8];
-  int l1 = 0;
+  Q.unusable = qn.q_zero || qn.q_bad || !(amax > 0.f && amax <= 1.0001f);
+  Q.S = Q.unusable ? 1.f : 32639.0f / amax;
+  Q.qs = qn.rq * Q.S;
+  int l1 = 0, sum = 0;
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const float f[4] = {q[i].x, q[i].y, q[i].z, q[i].w};
-    uint32_t hw = 0, lw = 0;
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      int v = q_unusable ? 0 : __float2int_rn(f[e] * qs);
-      v = max(-32639, min(32639, v));
-      l1 += abs(v);
-      const int lo = ((v + 128) & 255) - 128;               // signed low byte
-      const int hi = (v - lo) >> 8;                         // exact: v - lo is a multiple of 256
-      hw |= (uint32_t)(hi & 255) << (8 * e);
-      lw |= (uint32_t)(lo & 255) << (8 * e);
-    }
-    qhi[i] = hw; qlo[i] = lw;
-  }
+  for (int i = 0; i < 8; ++i) stb_q16_words(q[i], Q.qs, Q.unusable, Q.qhi[i], Q.qlo[i], l1, sum);
   l1 += __shfl_xor_sync(0xffffffffu, l1, 4);
   l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
   l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
-  const float inv_S = 1.0f / S;
-  const float h_l1 = 0.50025f * (float)l1 * inv_S;          // (0.5 + 3e-5 + fp slack) * ||q~||_1
-  const float e_q = 9.7f * inv_S;
+  Q.inv_S = 1.0f / Q.S;
+  Q.h_l1 = 0.50025f * (float)l1 * Q.inv_S;                  // (0.5 + 3e-5 + fp slack) * ||q~||_1
+  Q.e_q = 9.7f * Q.inv_S;
+  return Q;
+}
+
+// int8 dot products (group-reduced, every lane of the group holds them) and scales of U rows;
+// qhi / qlo: this lane's query words (StbQ8Query, or a copy in shared memory)
+template <int U>
+__device__ __forceinline__ void stb_q8_dots(const uint32_t *qhi, const uint32_t *qlo, const uint8_t *q8, const float *q8_scale,
+                                            const uint32_t (&row)[U], int j, int (&dot)[U], float (&sc_row)[U]) {
+  uint4 a[U][2];
+#pragma unroll
+  for (int u = 0; u < U; ++u) {
+    const uint8_t *p = q8 + (size_t)row[u] * 256 + (size_t)j * 16;
+    const float4 t0 = stb_ld_stream(reinterpret_cast<const float4 *>(p));
+    const float4 t1 = stb_ld_stream(reinterpret_cast<const float4 *>(p + 128));
+    a[u][0] = make_uint4(__float_as_uint(t0.x), __float_as_uint(t0.y), __float_as_uint(t0.z), __float_as_uint(t0.w));
+    a[u][1] = make_uint4(__float_as_uint(t1.x), __float_as_uint(t1.y), __float_as_uint(t1.z), __float_as_uint(t1.w));
+    sc_row[u] = __ldg(q8_scale + row[u]);                   // 8 lanes, one address
+  }
+#pragma unroll
+  for (int u = 0; u < U; ++u) {
+    int dh = 0, dl = 0;
+    const uint32_t w[8] = {a[u][0].x, a[u][0].y, a[u][0].z, a[u][0].w, a[u][1].x, a[u][1].y, a[u][1].z, a[u][1].w};
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      dh = __dp4a((int)w[i], (int)qhi[i], dh);
+      dl = __dp4a((int)w[i], (int)qlo[i], dl);
+    }
+    int d = dh * 256 + dl;
+    d += __shfl_xor_sync(0xffffffffu, d, 4);
+    d += __shfl_xor_sync(0xffffffffu, d, 2);
+    d += __shfl_xor_sync(0xffffffffu, d, 1);
+    dot[u] = d;
+  }
+}
+
+template <int U, int RANGES, class Sink>
+__device__ __forceinline__ void stb_scan_q8(const ScanArgs &args, const uint8_t *q8, const float *q8_scale, Sink &sink) {
+  const int lane = threadIdx.x & 31;
+  const int g = lane >> 3;   // row group inside the warp
+  const int j = lane & 7;
+  const StbQ8Query Q = stb_q8_query(args.q, j);
 
   constexpr uint64_t tile_rows = 4 * U;
   const uint64_t n_tiles = (args.n_virtual + tile_rows - 1) / tile_rows;
@@ -399,8 +448,8 @@ __device__ __forceinline__ void stb_scan_q8(const ScanArgs &args, const uint8_t 
   rmap.restart();
   stb_for_each_tile<RANGES, 2>(args, n_tiles, [&](uint64_t tile, bool first) {
     if (first) rmap.restart();
-    uint4 a[U][2];
     float sc_row[U];
+    int dot[U];
     uint32_t row[U];
     bool valid[U];
 #pragma unroll
@@ -409,28 +458,12 @@ __device__ __forceinline__ void stb_scan_q8(const ScanArgs &args, const uint8_t 
       valid[u] = v < args.n_virtual;
       const uint64_t vc = valid[u] ? v : (args.n_virtual - 1);
       row[u] = rmap.map(args, vc);
-      const uint8_t *p = q8 + (size_t)row[u] * 256 + (size_t)j * 16;
-      const float4 t0 = stb_ld_stream(reinterpret_cast<const float4 *>(p));
-      const float4 t1 = stb_ld_stream(reinterpret_cast<const float4 *>(p + 128));
-      a[u][0] = make_uint4(__float_as_uint(t0.x), __float_as_uint(t0.y), __float_as_uint(t0.z), __float_as_uint(t0.w));
-      a[u][1] = make_uint4(__float_as_uint(t1.x), __float_as_uint(t1.y), __float_as_uint(t1.z), __float_as_uint(t1.w));
-      sc_row[u] = __ldg(q8_scale + row[u]);                 // 8 lanes, one address
     }
+    stb_q8_dots<U>(Q.qhi, Q.qlo, q8, q8_scale, row, j, dot, sc_row);
     float sc[U];
 #pragma unroll
     for (int u = 0; u < U; ++u) {
-      int dh = 0, dl = 0;
-      const uint32_t w[8] = {a[u][0].x, a[u][0].y, a[u][0].z, a[u][0].w, a[u][1].x, a[u][1].y, a[u][1].z, a[u][1].w};
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        dh = __dp4a((int)w[i], (int)qhi[i], dh);
-        dl = __dp4a((int)w[i], (int)qlo[i], dl);
-      }
-      int dot = dh * 256 + dl;
-      dot += __shfl_xor_sync(0xffffffffu, dot, 4);
-      dot += __shfl_xor_sync(0xffffffffu, dot, 2);
-      dot += __shfl_xor_sync(0xffffffffu, dot, 1);
-      const float s = q_unusable ? CUDART_INF_F : fmaf(sc_row[u], fmaf((float)dot, inv_S, h_l1), e_q);
+      const float s = Q.unusable ? CUDART_INF_F : fmaf(sc_row[u], fmaf((float)dot[u], Q.inv_S, Q.h_l1), Q.e_q);
       sc[u] = valid[u] ? s : -CUDART_INF_F;
     }
     float s = -CUDART_INF_F;
@@ -442,12 +475,230 @@ __device__ __forceinline__ void stb_scan_q8(const ScanArgs &args, const uint8_t 
   });
 }
 
+// ---- the q8 tier's top-k scan: a 4-bit prefilter in front of the int8 codes --------------------
+// Beside the int8 codes the builder keeps a nibble plane, h_i = code_i >> 4 in [-8, 7] stored as
+// h_i + 8, two per byte (128 B/row), and per row {s, rho} with rho >= ||x^ - s (16 h + 7.5)||_2
+// (16 h + 7.5 is the midpoint of the 16 codes a nibble stands for).  Byte 16m + r of the plane
+// (m < 8, r < 16) holds component 32m + r in its low nibble and 32m + 16 + r in its high nibble,
+// so lane j of a row's 8-lane group reads one 16-byte chunk, and w & 0x0F0F0F0F and
+// (w >> 4) & 0x0F0F0F0F each line up with one query word.  With the query quantised exactly as
+// in stb_scan_q8 (q~ = q16 / S, |q^_i - q~_i| <= 0.6 / S):
+//     c  <=  q^ . x~ + rho  <=  s (16 q~ . h + 7.5 sum q~) + rho + (0.6 / S) ||x~||_1
+//     ||x~||_1 <= 16 ||x~||_2 <= 16 (1 + rho) <= 32.3        (rho <= 128 s <= 1.01)
+//     u4 = s (16 q16 . h + 7.5 sum q16) / S + rho + 19.4 / S          >=  c - 1e-5
+// (q16 . h = q16 . (h + 8) - 8 sum q16, exact in int32).  The coarse pass streams the plane and
+// {s, rho}, 136 B/row, and skips every row with u4 + STB_Q4_SKIP_EPS < T, where T is a proven
+// lower bound of this launch's k-th best exact cosine (below): a skipped row has c < c_k, so it
+// can neither be a result nor tie with one.  Every other row is queued per warp; each 32 queued
+// rows are scored from their int8 codes with the arithmetic of stb_scan_q8 and handed to the
+// sink, so the lists, drop bounds and completeness proof are the q8 tier's, over the rows that
+// were not skipped.
+// T: a refined row also has a lower bound l8 = s (dot / S - h_l1) - e_q - 2e-5 <= c - 1e-5, which
+// is max-ed into word (row mod k) of k words.  T = min of the k words is the l8 of k distinct
+// rows, so at least k rows have c >= T.  A word is u64 (tag << 32 | ordered l8) and the tag
+// identifies the launch: a later launch that shares the slot writes larger words, a word with
+// another tag reads as "no bound", so slots are never cleared and overlapped launches need no
+// ordering between them.  Warps re-read the words once per tile.
+#define STB_Q4_SCAN_U 8         // 8 rows x 1 LDG.128 per lane in flight (4 KiB per warp)
+#define STB_Q4_SPARE (32 * (STB_Q4_SCAN_U / 8 + 1))   // queued rows per warp: < 32 left over + one tile's worth ...
+#define STB_Q4_QUEUE (STB_Q4_SPARE + 4)                 // ... + a spare slot for lanes with nothing to store (16-B aligned)
+struct StbQ4Args {
+  const uint8_t *plane;          // [n][128] nibbles
+  const float2 *sr;              // [n] {s, rho}
+  unsigned long long *thr;       // the k threshold words of this launch
+  uint32_t tag;                  // this launch's tag (never 0)
+  uint32_t top_k;                // k >= 1 words
+  unsigned long long *refined;   // debug counter: rows refined from the int8 codes
+};
+
+template <int U, int RANGES, class Sink>
+__device__ __forceinline__ void stb_scan_q4(const ScanArgs &args, const uint8_t *q8, const float *q8_scale, const StbQ4Args &q4a,
+                                            uint32_t *wq, uint32_t *pw, Sink &sink) {
+  static_assert(U % 8 == 0 && STB_Q8_MAX_K <= 32, "each lane owns U / 8 rows of a tile; one lane per threshold word");
+  constexpr int P = U / 8;
+  const int lane = threadIdx.x & 31;
+  const int g = lane >> 3;   // row group inside the warp
+  const int j = lane & 7;    // this lane reads plane bytes [16j, 16j+16): components 32j .. 32j+31
+  const StbQ8Query Q = stb_q8_query(args.q, j);
+  // query words in shared memory (registers go to the loads in flight).  Plane chunk of lane j: word i
+  // (components 32j + 4i .. +3; i < 4 pairs with the low nibbles of chunk word i, else with the high
+  // nibbles of word i - 4) as hi / lo byte words at pw[(i * 8 + j) * 2 + {0, 1}]; the int8 codes' words
+  // (StbQ8Query) at pw[128 + 16 j + {0..7: hi, 8..15: lo}]
+  int sumq = 0;
+  {
+    const float4 *qv = reinterpret_cast<const float4 *>(args.q);
+    int l1 = 0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      uint32_t hw, lw;
+      stb_q16_words(__ldg(qv + 8 * j + i), Q.qs, Q.unusable, hw, lw, l1, sumq);
+      if (g == 0) {
+        *reinterpret_cast<uint2 *>(pw + (i * 8 + j) * 2) = make_uint2(hw, lw);
+        pw[128 + 16 * j + i] = Q.qhi[i];
+        pw[128 + 16 * j + 8 + i] = Q.qlo[i];
+      }
+    }
+    __syncwarp();
+  }
+  sumq += __shfl_xor_sync(0xffffffffu, sumq, 4);
+  sumq += __shfl_xor_sync(0xffffffffu, sumq, 2);
+  sumq += __shfl_xor_sync(0xffffffffu, sumq, 1);
+  const float A = 16.0f * Q.inv_S;
+  const float B = 7.5f * (float)sumq * Q.inv_S;
+  const float e_q4 = 19.4f * Q.inv_S;
+
+  const int kw = (int)q4a.top_k;
+  unsigned tcache = 0u;              // lane w < k: best ordered l8 of word w this warp knows (0: none)
+  float T = -CUDART_INF_F;
+  int qn = 0;                        // queued rows (warp-uniform)
+  unsigned refined = 0u;
+
+  auto refine = [&]() {              // the first 32 queue slots (0xffffffff: empty; slot 0 is never empty)
+    uint32_t row[8];
+    bool valid[8];
+#pragma unroll
+    for (int u = 0; u < 8; ++u) {
+      row[u] = wq[u * 4 + g];
+      valid[u] = row[u] != 0xffffffffu;
+      if (!valid[u]) row[u] = wq[0];
+    }
+    int dot[8];
+    float sc_row[8];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {          // two halves of 4 rows: the coarse pass's state stays in registers
+      const uint32_t rh[4] = {row[4 * h], row[4 * h + 1], row[4 * h + 2], row[4 * h + 3]};
+      int dh[4];
+      float sh[4];
+      stb_q8_dots<4>(pw + 128 + 16 * j, pw + 128 + 16 * j + 8, q8, q8_scale, rh, j, dh, sh);
+#pragma unroll
+      for (int u = 0; u < 4; ++u) { dot[4 * h + u] = dh[u]; sc_row[4 * h + u] = sh[u]; }
+    }
+    int d = 0;
+    float sc = 0.f;
+    uint32_t r = 0;
+    bool v = false;
+#pragma unroll
+    for (int u = 0; u < 8; ++u)
+      if (j == u) { d = dot[u]; sc = sc_row[u]; r = row[u]; v = valid[u]; }
+    const float s = !v ? -CUDART_INF_F : (Q.unusable ? CUDART_INF_F : fmaf(sc, fmaf((float)d, Q.inv_S, Q.h_l1), Q.e_q));
+    refined += (unsigned)__popc(__ballot_sync(0xffffffffu, v));
+    sink.template consume<32>(s, r);
+    if (Q.unusable) return;
+    // publish the lower bounds that beat the published value of their word (rare after the first tickets);
+    // the warp learns its own contributions with the next read
+    const unsigned o8 = stb_f2ord(fmaf(sc, fmaf((float)d, Q.inv_S, -Q.h_l1), -Q.e_q) - (float)STB_Q8_SCAN_EPS);
+    const int w = (int)(r % (uint32_t)kw);
+    const unsigned known = __shfl_sync(0xffffffffu, tcache, w);   // every lane takes part in the shuffle
+    if (v && o8 > known) atomicMax(q4a.thr + w, ((unsigned long long)q4a.tag << 32) | o8);
+  };
+
+  constexpr uint64_t tile_rows = 4 * U;
+  const uint64_t n_tiles = (args.n_virtual + tile_rows - 1) / tile_rows;
+  StbRowMap<RANGES> rmap;
+  rmap.restart();
+  stb_for_each_tile<RANGES, (64 / (4 * U) > 1 ? 64 / (4 * U) : 1)>(args, n_tiles, [&](uint64_t tile, bool first) {
+    if (first) rmap.restart();
+    // lane w < k: threshold word w as the other warps left it; issued with the tile's loads, folded in below
+    const unsigned long long tw = lane < kw ? __ldcg(q4a.thr + lane) : 0ull;
+    uint4 a[U];
+    uint32_t row[U];
+    bool valid[U];
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const uint64_t v = tile * tile_rows + (uint64_t)(u * 4 + g);
+      valid[u] = v < args.n_virtual;
+      const uint64_t vc = valid[u] ? v : (args.n_virtual - 1);
+      row[u] = rmap.map(args, vc);
+      const float4 t = stb_ld_stream(reinterpret_cast<const float4 *>(q4a.plane + (size_t)row[u] * 128 + (size_t)j * 16));
+      a[u] = make_uint4(__float_as_uint(t.x), __float_as_uint(t.y), __float_as_uint(t.z), __float_as_uint(t.w));
+    }
+    // lane j of group g owns rows u = 8p + j: their {s, rho} (the warp's 32 owned rows of one p are consecutive)
+    uint32_t my_row[P];
+    bool my_valid[P];
+    float2 sr[P];
+#pragma unroll
+    for (int p = 0; p < P; ++p) {
+      my_row[p] = row[8 * p];
+      my_valid[p] = valid[8 * p];
+#pragma unroll
+      for (int u = 1; u < 8; ++u)
+        if (j == u) { my_row[p] = row[8 * p + u]; my_valid[p] = valid[8 * p + u]; }
+      sr[p] = __ldg(q4a.sr + my_row[p]);
+    }
+    int dot[U];
+#pragma unroll
+    for (int u = 0; u < U; ++u) { dot[u] = 0; }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const uint2 ql = *reinterpret_cast<const uint2 *>(pw + (k * 8 + j) * 2);         // with the low nibbles
+      const uint2 qh = *reinterpret_cast<const uint2 *>(pw + ((4 + k) * 8 + j) * 2);   // with the high nibbles
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const uint32_t w = k == 0 ? a[u].x : (k == 1 ? a[u].y : (k == 2 ? a[u].z : a[u].w));
+        const int lo = (int)(w & 0x0F0F0F0Fu), hi = (int)((w >> 4) & 0x0F0F0F0Fu);
+        int dh = __dp4a(lo, (int)ql.x, 0), dl = __dp4a(lo, (int)ql.y, 0);
+        dh = __dp4a(hi, (int)qh.x, dh);
+        dl = __dp4a(hi, (int)qh.y, dl);
+        dot[u] += dh * 256 + dl;
+      }
+    }
+    if (lane < kw && (uint32_t)(tw >> 32) == q4a.tag) tcache = max(tcache, (unsigned)tw);
+    {
+      unsigned tmin = lane < kw ? tcache : 0xffffffffu;
+#pragma unroll
+      for (int off = 16; off > 0; off >>= 1) tmin = min(tmin, __shfl_xor_sync(0xffffffffu, tmin, off));
+      T = tmin ? stb_ord2f(tmin) : -CUDART_INF_F;
+    }
+#pragma unroll
+    for (int p = 0; p < P; ++p) {
+      // reduce-scatter over the 8-lane group (7 shuffles for 8 rows): lane j ends with row 8p + j
+      const int *x = dot + 8 * p;
+      int y4[4], y2[2];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int send = (j & 4) ? x[i] : x[i + 4], keep = (j & 4) ? x[i + 4] : x[i];
+        y4[i] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
+      }
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int send = (j & 2) ? y4[i] : y4[i + 2], keep = (j & 2) ? y4[i + 2] : y4[i];
+        y2[i] = keep + __shfl_xor_sync(0xffffffffu, send, 2);
+      }
+      const int send = (j & 1) ? y2[0] : y2[1], keep = (j & 1) ? y2[1] : y2[0];
+      const int D = keep + __shfl_xor_sync(0xffffffffu, send, 1) - 8 * sumq;   // q16 . h
+      const float u4 = fmaf(sr[p].x, fmaf((float)D, A, B), sr[p].y + e_q4);
+      const bool want = my_valid[p] && (Q.unusable || !(u4 + (float)STB_Q4_SKIP_EPS < T));
+      const unsigned m = __ballot_sync(0xffffffffu, want);
+      wq[want ? qn + __popc(m & ((1u << lane) - 1u)) : STB_Q4_SPARE] = my_row[p];
+      qn += __popc(m);
+    }
+    while (qn >= 32) {
+      __syncwarp();
+      refine();
+      uint32_t rest[P];
+#pragma unroll
+      for (int p = 0; p < P; ++p) rest[p] = (32 * (p + 1) + lane < qn) ? wq[32 * (p + 1) + lane] : 0u;
+      __syncwarp();
+#pragma unroll
+      for (int p = 0; p < P; ++p) wq[(32 * (p + 1) + lane < qn) ? 32 * p + lane : STB_Q4_SPARE] = rest[p];
+      qn -= 32;
+    }
+  });
+  if (qn > 0) {                      // the rest, with the empty slots marked
+    wq[lane >= qn ? lane : STB_Q4_SPARE] = 0xffffffffu;
+    __syncwarp();
+    refine();
+  }
+  if (lane == 0 && refined) atomicAdd(q4a.refined, (unsigned long long)refined);
+}
+
 // q8 builder: one warp per row; lane l owns elements 8l .. 8l+7.  Rows whose fp32 squared norm
 // is not a normal number set *bad_flag (the tier is then refused for this corpus, like the
 // 16-bit shadow); true zero rows get scale 0 and all-zero codes (score = the query's slack).
+// The same pass writes the nibble plane and {s, rho} of the top-k scan's prefilter (stb_scan_q4).
 __global__ void __launch_bounds__(256)
 stb_q8_build_kernel(const float4 *__restrict__ rows, uint64_t first_row, uint64_t n_rows, uint8_t *__restrict__ out,
-                    float *__restrict__ scale, int *bad_flag) {
+                    float *__restrict__ scale, uint8_t *__restrict__ plane, float2 *__restrict__ sr, int *bad_flag) {
   const int lane = threadIdx.x & 31;
   const uint64_t row = first_row + (uint64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
   if (row >= n_rows) return;
@@ -473,24 +724,43 @@ stb_q8_build_kernel(const float4 *__restrict__ rows, uint64_t first_row, uint64_
   for (int off = 16; off > 0; off >>= 1) am = fmaxf(am, __shfl_xor_sync(0xffffffffu, am, off));
   const float s = am * (1.0f / 127.0f);
   const float inv_s = am > 0.f ? 127.0f / am : 0.f;
-  uint32_t w0 = 0, w1 = 0;
+  uint32_t w0 = 0, w1 = 0, n0 = 0, n1 = 0;
+  float r2 = 0.f;
 #pragma unroll
   for (int e = 0; e < 4; ++e) {
     const int c0 = max(-127, min(127, __float2int_rn(x[e] * inv_s)));
     const int c1 = max(-127, min(127, __float2int_rn(x[4 + e] * inv_s)));
     w0 |= (uint32_t)(c0 & 255) << (8 * e);
     w1 |= (uint32_t)(c1 & 255) << (8 * e);
+    const int h0 = (c0 + 128) >> 4, h1 = (c1 + 128) >> 4;      // h + 8 in [0, 15]
+    n0 |= (uint32_t)h0 << (8 * e);
+    n1 |= (uint32_t)h1 << (8 * e);
+    // x^ - s (16 h + 7.5) with h = h0 - 8: the centre 16 h0 - 120.5 = (32 h0 - 241) / 2 is exact in fp32
+    const float d0 = x[e] - s * (0.5f * (float)(32 * h0 - 241));
+    const float d1 = x[4 + e] - s * (0.5f * (float)(32 * h1 - 241));
+    r2 = fmaf(d0, d0, fmaf(d1, d1, r2));
   }
   *reinterpret_cast<uint2 *>(out + row * 256 + (size_t)lane * 8) = make_uint2(w0, w1);
-  if (lane == 0) scale[row] = s;
+  // plane: lane 4m + t holds components 32m + 8t .. +7; t < 2 are the low nibbles of bytes 16m + 8t ..,
+  // t >= 2 the high nibbles of the same bytes (from lane + 2)
+  const uint32_t p0 = __shfl_down_sync(0xffffffffu, n0, 2), p1 = __shfl_down_sync(0xffffffffu, n1, 2);
+  if ((lane & 2) == 0)
+    *reinterpret_cast<uint2 *>(plane + row * 128 + (size_t)(lane >> 2) * 16 + (size_t)(lane & 1) * 8) = make_uint2(n0 | (p0 << 4), n1 | (p1 << 4));
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) r2 += __shfl_xor_sync(0xffffffffu, r2, off);
+  if (lane == 0) {
+    scale[row] = s;
+    // rounded up: 1e-4 relative covers the fp32 evaluation of the 256 differences and their sum
+    sr[row] = make_float2(s, sqrtf(r2) * 1.0001f + 1e-6f);
+  }
 }
 
 int stb_launch_q8_build(stb_ctx *ctx, const float *rows_dev, uint64_t first_row, uint64_t n_rows, uint8_t *out,
-                        float *scale, int *bad_flag_dev) {
+                        float *scale, uint8_t *plane, float2 *sr, int *bad_flag_dev) {
   if (first_row >= n_rows) return STB_OK;
   const unsigned blocks = (unsigned)((n_rows - first_row + 7) / 8);
   stb_q8_build_kernel<<<blocks, 256, 0, ctx->stream>>>(reinterpret_cast<const float4 *>(rows_dev), first_row, n_rows, out, scale,
-                                                       bad_flag_dev);
+                                                       plane, sr, bad_flag_dev);
   STB_CUDA(cudaGetLastError());
   ctx->kernel_launches++;
   return STB_OK;
@@ -610,6 +880,7 @@ struct TopkArgs {
   uint32_t early_trigger;    // overlapped launch: release the dependent launch at kernel start
   const uint8_t *q8;         // SRC == 2: int8 codes [n][256] ...
   const float *q8_scale;     //           ... and per-row scales [n]
+  StbQ4Args q4;              //           ... and the prefilter's copy, threshold words, debug counter
 };
 
 __device__ __forceinline__ unsigned long long stb_globaltimer() {
@@ -696,8 +967,13 @@ stb_scan_topk_kernel(const TopkArgs args) {
   if (args.early_trigger) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   TopSink<E> sink;
   sink.init();
-  if constexpr (SRC == 2) stb_scan_q8<U, RANGES>(args.scan, args.q8, args.q8_scale, sink);
-  else if constexpr (SRC == 1) stb_scan_shadow<U, RANGES>(args.scan, args.shadow, sink);
+  if constexpr (SRC == 2) {
+    // the refine queues live in the re-rank staging area, which is first used after the CTA merge
+    // (per warp: STB_Q4_QUEUE queued rows + 256 query words)
+    static_assert(STB_SCAN_WARPS * (STB_Q4_QUEUE + 256) <= 32 * STB_RR_STRIDE, "q4 scratch");
+    uint32_t *scratch = reinterpret_cast<uint32_t *>(srows) + (threadIdx.x >> 5) * (STB_Q4_QUEUE + 256);
+    stb_scan_q4<U, RANGES>(args.scan, args.q8, args.q8_scale, args.q4, scratch, scratch + STB_Q4_QUEUE, sink);
+  } else if constexpr (SRC == 1) stb_scan_shadow<U, RANGES>(args.scan, args.shadow, sink);
   else stb_scan_rows<U, RANGES>(args.scan, sink);
   STB_T_MAX(1);                      // last CTA leaves the scan loop
   // Programmatic dependent launch: the scan above reads only the corpus and the query,
@@ -1083,7 +1359,7 @@ static int stb_scan_ctas_per_sm_override() {
 
 template <int E, int RANGES, int SRC = 0, int EF = E>
 static int stb_launch_topk_t(stb_ctx *ctx, const TopkArgs &a_in, bool overlapped) {
-  constexpr int kU = SRC == 2 ? STB_Q8_SCAN_U : (SRC == 1 ? STB_SHADOW_SCAN_U : STB_SCAN_U);
+  constexpr int kU = SRC == 2 ? STB_Q4_SCAN_U : (SRC == 1 ? STB_SHADOW_SCAN_U : STB_SCAN_U);
   auto kern = stb_scan_topk_kernel<E, kU, RANGES, SRC, EF>;
   int occ = 0;
   STB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, STB_SCAN_THREADS, 0));
@@ -1181,7 +1457,21 @@ int stb_launch_scan_topk(stb_ctx *ctx, const stb_corpus *c, int tier, const floa
   a.shadow = c->shadow;
   a.q8 = c->q8;
   a.q8_scale = c->q8_scale;
-  if (tier == STB_TIER_Q8 && (top_k > STB_Q8_MAX_K || !c->q8)) { stb_set_error("scan_topk: q8 tier unavailable"); return STB_ERR_STATE; }
+  memset(&a.q4, 0, sizeof(a.q4));
+  if (tier == STB_TIER_Q8 && (top_k > STB_Q8_MAX_K || !c->q8 || !c->q4)) { stb_set_error("scan_topk: q8 tier unavailable"); return STB_ERR_STATE; }
+  if (tier == STB_TIER_Q8) {
+    // a fresh tag per launch, slots in turn (stb_scan_q4); after 2^32 launches the words are cleared once
+    if ((uint32_t)++ctx->q4_launches == 0) {
+      STB_CUDA(cudaMemsetAsync(ctx->q4_thr, 0, STB_TICKET_SLOTS * STB_Q4_WORDS * sizeof(unsigned long long), ctx->stream));
+      ++ctx->q4_launches;
+    }
+    a.q4.plane = c->q4;
+    a.q4.sr = c->q4_sr;
+    a.q4.thr = ctx->q4_thr + (ctx->q4_launches % STB_TICKET_SLOTS) * STB_Q4_WORDS;
+    a.q4.tag = (uint32_t)ctx->q4_launches;
+    a.q4.top_k = top_k > 0 ? top_k : 1;
+    a.q4.refined = ctx->q4_refined;
+  }
   if (tier == STB_TIER_H16 && !c->shadow) { stb_set_error("scan_topk: h16 tier unavailable"); return STB_ERR_STATE; }
   return n_ranges > 0 ? stb_launch_topk_r<1>(ctx, a, tier, top_k, overlapped) : stb_launch_topk_r<0>(ctx, a, tier, top_k, overlapped);
 }
