@@ -641,7 +641,7 @@ int stb_search(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t 
     float floor_cos = -INFINITY;
     if (n_hits == top_k) floor_cos = (float)(1.0 - ctx->hits_pin[top_k - 1].distance - 2.0 * STB_SCORE_EPS);
     uint64_t n_pass = 0;
-    if ((rc = collect_exact_sorted(ctx, corpus, floor_cos, has_max ? std::min(max_distance, 100.0) : 100.0,
+    if ((rc = collect_exact_sorted(ctx, corpus, floor_cos, has_max ? std::min(max_distance, STB_DEFAULT_MAX_DIST) : STB_DEFAULT_MAX_DIST,
                                    ranges_dev, n_loc, n_virtual, &n_pass)) != STB_OK) return rc;
     total = std::min<uint64_t>(n_pass, top_k);
     src_dev = ctx->collect_hits;
@@ -665,7 +665,7 @@ int stb_search(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t 
       }
     }
     float floor_cos = -INFINITY;
-    double limit = 100.0;
+    double limit = STB_DEFAULT_MAX_DIST;
     uint64_t n_pass = 0;
     bool done = false;
     if (threshold_all) {
@@ -677,7 +677,7 @@ int stb_search(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t 
       done = true;
     } else {
       if (has_max) {
-        limit = std::min(max_distance, 100.0);
+        limit = std::min(max_distance, STB_DEFAULT_MAX_DIST);
         if (!(max_distance == max_distance)) limit = -1.0;
       }
       // top_k beyond the register lists: histogram pass to find the score bin of the k-th

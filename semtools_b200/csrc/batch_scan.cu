@@ -553,6 +553,9 @@ stb_batch_finish_kernel(const FinishArgs a) {
   __shared__ int s_pass, s_alltiles;
   const uint32_t q = blockIdx.x;
   const int tid = threadIdx.x;
+  // launched with 256 threads (one per sub-tile key below); with the stride known the shared-memory
+  // sorts fit 64 registers, i.e. 4 CTAs per SM
+  __builtin_assume(blockDim.x == 256);
   // 1. merge the per-slice candidate tiles, keep the KSEL best
   const uint32_t n_in = a.n_slices * STB_BATCH_KSEL;     // <= STB_FINISH_KEYS
   int n_sort = 64;
@@ -562,19 +565,7 @@ stb_batch_finish_kernel(const FinishArgs a) {
   for (int i = tid; i < STB_D; i += 256) sqd[i] = (double)__ldg(a.queries + (size_t)q * STB_D + i);
   if (tid == 0) s_pass = 0;
   __syncthreads();
-  // in-place ascending sort (best first)
-  for (int kk = 2; kk <= n_sort; kk <<= 1)
-    for (int j = kk >> 1; j > 0; j >>= 1) {
-      for (int i = tid; i < n_sort; i += 256) {
-        int ixj = i ^ j;
-        if (ixj > i) {
-          uint64_t x = skeys[i], y = skeys[ixj];
-          bool up = ((i & kk) == 0);
-          if ((x > y) == up) { skeys[i] = y; skeys[ixj] = x; }
-        }
-      }
-      __syncthreads();
-    }
+  stb_cta_sort_keys_strided(skeys, n_sort);      // in place, ascending (best first)
   // 1b. the KSEL best sub-tiles all lie inside the KSEL best tiles (a tile's maximum is the
   //     maximum of its 8 sub-tiles): expand those tiles to their 8 sub-tile maxima, sort
   //     again and keep the KSEL best sub-tiles.
@@ -590,25 +581,11 @@ stb_batch_finish_kernel(const FinishArgs a) {
     __syncthreads();
     skeys[tid] = mykey;                                   // 256 threads -> 256 sub-tile keys
     __syncthreads();
-    for (int kk = 2; kk <= 256; kk <<= 1)
-      for (int j = kk >> 1; j > 0; j >>= 1) {
-        const int i = tid, ixj = i ^ j;
-        if (ixj > i) {
-          uint64_t x = skeys[i], y = skeys[ixj];
-          bool up = ((i & kk) == 0);
-          if ((x > y) == up) { skeys[i] = y; skeys[ixj] = x; }
-        }
-        __syncthreads();
-      }
+    stb_cta_sort_keys_strided(skeys, 256);
   }
-  if (tid == 0) {
-    double q2 = 0.0;
-    for (int i = 0; i < STB_D; ++i) q2 = fma(sqd[i], sqd[i], q2);
-    s_q2 = q2;
-  }
+  if (tid == 0) s_q2 = stb_canon_q2(sqd);
   __syncthreads();
-  // 2. exact canonical distance of every row of the selected sub-tiles (one thread per row,
-  //    f64 accumulation in index order == oracle orc_cosine_f32)
+  // 2. exact canonical distance of every row of the selected sub-tiles (one thread per row)
   const double q2 = s_q2;
   for (int c = tid; c < STB_BATCH_KSEL * STB_SUB; c += 256) {
     const uint64_t key = skeys[c / STB_SUB];
@@ -617,55 +594,21 @@ stb_batch_finish_kernel(const FinishArgs a) {
     if (key != STB_KEY_INVALID) {
       const uint64_t row = (uint64_t)stb_key_row(key) * STB_SUB + (c % STB_SUB);
       if (row < a.n_rows) {
-        const float4 *rp = a.rows + row * STB_ROW_F4;
-        double ab = 0.0, r2 = 0.0;
-#pragma unroll 8
-        for (int i = 0; i < STB_ROW_F4; ++i) {
-          const float4 v = __ldg(rp + i);
-          const double vx = (double)v.x, vy = (double)v.y, vz = (double)v.z, vw = (double)v.w;
-          ab = fma(sqd[4 * i + 0], vx, ab); r2 = fma(vx, vx, r2);
-          ab = fma(sqd[4 * i + 1], vy, ab); r2 = fma(vy, vy, r2);
-          ab = fma(sqd[4 * i + 2], vz, ab); r2 = fma(vz, vz, r2);
-          ab = fma(sqd[4 * i + 3], vw, ab); r2 = fma(vw, vw, r2);
-        }
-        double dist;
-        if (q2 == 0.0 && r2 == 0.0) dist = 0.0;
-        else if (ab == 0.0) dist = 1.0;
-        else {
-          double t = 1.0 - ab / (sqrt(q2) * sqrt(r2));
-          dist = t > 0.0 ? t : 0.0;
-        }
-        if (dist < 100.0) { d = dist; grow = a.row_base + row; atomicAdd(&s_pass, 1); }
+        double ab, r2;
+        stb_canon_dot<true>(sqd, a.rows + row * STB_ROW_F4, ab, r2);
+        const double dist = stb_canon_dist(ab, q2, r2);
+        if (dist < STB_DEFAULT_MAX_DIST) { d = dist; grow = a.row_base + row; atomicAdd(&s_pass, 1); }
       }
     }
     sd[c] = d; sr[c] = grow;
   }
   __syncthreads();
   // 3. sort the 1024 (distance,row) pairs
-  for (int kk = 2; kk <= 1024; kk <<= 1)
-    for (int j = kk >> 1; j > 0; j >>= 1) {
-      for (int i = tid; i < 1024; i += 256) {
-        int ixj = i ^ j;
-        if (ixj > i) {
-          bool up = ((i & kk) == 0);
-          bool gt = stb_hit_less(sd[ixj], sr[ixj], sd[i], sr[i]);
-          if (gt == up) {
-            double td = sd[i]; uint64_t tr = sr[i];
-            sd[i] = sd[ixj]; sr[i] = sr[ixj]; sd[ixj] = td; sr[ixj] = tr;
-          }
-        }
-      }
-      __syncthreads();
-    }
+  stb_cta_sort_hits(sd, sr, STB_BATCH_KSEL * STB_SUB);
   // 4. hits + completeness proof
   const uint32_t k = a.top_k;
   const uint32_t n_out = min((uint32_t)s_pass, k);
-  for (uint32_t i = tid; i < k; i += 256) {
-    stb_hit h;
-    h.distance = (i < n_out) ? sd[i] : CUDART_INF;
-    h.row = (i < n_out) ? sr[i] : 0xffffffffffffffffull;
-    a.out_hits[(size_t)q * k + i] = h;
-  }
+  stb_write_hits(a.out_hits + (size_t)q * k, sd, sr, n_out, k);
   if (tid == 0) {
     bool complete;
     if (s_alltiles && skeys[STB_BATCH_KSEL] == STB_KEY_INVALID) complete = true;   // every sub-tile was re-scored
@@ -855,10 +798,7 @@ stb_batch_finish2_kernel(const Finish2Args a) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint32_t k = a.top_k;
   auto give_up = [&]() {                               // the host answers this query through K1
-    for (uint32_t i = tid; i < k; i += 256) {
-      stb_hit h; h.distance = CUDART_INF; h.row = 0xffffffffffffffffull;
-      a.out_hits[(size_t)q * k + i] = h;
-    }
+    stb_write_hits(a.out_hits + (size_t)q * k, sd, sr, 0, k);
     if (tid == 0) { a.out_status[2 * q] = 0; a.out_status[2 * q + 1] = 0; }
   };
   // 1. segment counts -> offsets (n_seg <= 256: one thread per segment, warp scans + 8-entry fix-up)
@@ -906,16 +846,11 @@ stb_batch_finish2_kernel(const Finish2Args a) {
   if (m_all >= k) cut = stb_key_score(skeys[k - 1]) - 2.0f * (float)STB_BATCH_EPS;
   for (uint32_t i = tid; i < m_all; i += 256)
     if (stb_key_score(skeys[i]) >= cut) atomicMax(&s_m2, i + 1);
-  if (tid == 5 * 32) {
-    double q2 = 0.0;
-#pragma unroll 8
-    for (int i = 0; i < STB_D; ++i) q2 = fma(sqd[i], sqd[i], q2);
-    s_q2 = q2;
-  }
+  if (tid == 5 * 32) s_q2 = stb_canon_q2(sqd);
   __syncthreads();
   const uint32_t m2 = s_m2;
   if (m2 > STB_F2_RESCORE) { give_up(); return; }
-  // 4. exact canonical distances, 32 rows per pass (f64 accumulation in index order == orc_cosine_f32)
+  // 4. exact canonical distances, 32 rows per pass
   const double q2 = s_q2;
   for (uint32_t c0 = 0; c0 < m2; c0 += 32) {
     {
@@ -939,25 +874,10 @@ stb_batch_finish2_kernel(const Finish2Args a) {
       const int cl = warp * 8 + lane;
       const uint32_t ci = c0 + cl;
       if (ci < m2) {
-        const float4 *rp = reinterpret_cast<const float4 *>(srows + cl * STB_F2_STRIDE);
-        double ab = 0.0, r2 = 0.0;
-#pragma unroll 8
-        for (int i = 0; i < STB_ROW_F4; ++i) {
-          const float4 v = rp[i];
-          const double vx = (double)v.x, vy = (double)v.y, vz = (double)v.z, vw = (double)v.w;
-          ab = fma(sqd[4 * i + 0], vx, ab); r2 = fma(vx, vx, r2);
-          ab = fma(sqd[4 * i + 1], vy, ab); r2 = fma(vy, vy, r2);
-          ab = fma(sqd[4 * i + 2], vz, ab); r2 = fma(vz, vz, r2);
-          ab = fma(sqd[4 * i + 3], vw, ab); r2 = fma(vw, vw, r2);
-        }
-        double dist;
-        if (q2 == 0.0 && r2 == 0.0) dist = 0.0;
-        else if (ab == 0.0) dist = 1.0;
-        else {
-          const double t = 1.0 - ab / (sqrt(q2) * sqrt(r2));
-          dist = t > 0.0 ? t : 0.0;
-        }
-        if (dist < 100.0) { sd[ci] = dist; sr[ci] = a.row_base + (uint64_t)stb_key_row(skeys[ci]); atomicAdd(&s_pass, 1); }
+        double ab, r2;
+        stb_canon_dot<false>(sqd, reinterpret_cast<const float4 *>(srows + cl * STB_F2_STRIDE), ab, r2);
+        const double dist = stb_canon_dist(ab, q2, r2);
+        if (dist < STB_DEFAULT_MAX_DIST) { sd[ci] = dist; sr[ci] = a.row_base + (uint64_t)stb_key_row(skeys[ci]); atomicAdd(&s_pass, 1); }
         else { sd[ci] = CUDART_INF; sr[ci] = 0xffffffffffffffffull; }
       }
     }
@@ -968,28 +888,9 @@ stb_batch_finish2_kernel(const Finish2Args a) {
   while (n2 < m2) n2 <<= 1;
   for (uint32_t i = m2 + tid; i < n2; i += 256) { sd[i] = CUDART_INF; sr[i] = 0xffffffffffffffffull; }
   __syncthreads();
-  for (uint32_t kk = 2; kk <= n2; kk <<= 1)
-    for (uint32_t j = kk >> 1; j > 0; j >>= 1) {
-      for (uint32_t i = tid; i < n2; i += 256) {
-        const uint32_t ixj = i ^ j;
-        if (ixj > i) {
-          const bool up = ((i & kk) == 0);
-          const bool gt = stb_hit_less(sd[ixj], sr[ixj], sd[i], sr[i]);
-          if (gt == up) {
-            const double td = sd[i]; const uint64_t tr = sr[i];
-            sd[i] = sd[ixj]; sr[i] = sr[ixj]; sd[ixj] = td; sr[ixj] = tr;
-          }
-        }
-      }
-      __syncthreads();
-    }
+  stb_cta_sort_hits(sd, sr, n2);
   const uint32_t n_out = min((uint32_t)s_pass, k);
-  for (uint32_t i = tid; i < k; i += 256) {
-    stb_hit h;
-    h.distance = (i < n_out) ? sd[i] : CUDART_INF;
-    h.row = (i < n_out) ? sr[i] : 0xffffffffffffffffull;
-    a.out_hits[(size_t)q * k + i] = h;
-  }
+  stb_write_hits(a.out_hits + (size_t)q * k, sd, sr, n_out, k);
   if (tid == 0) { a.out_status[2 * q] = n_out; a.out_status[2 * q + 1] = 1u; }
 }
 

@@ -306,7 +306,12 @@ int stb_launch_batch_finish(stb_ctx *ctx, const uint64_t *cand, uint32_t n_slice
                             uint32_t *out_status, const float *submax, uint32_t q_pad);
 
 // ---- device helpers ---------------------------------------------------------------
+// The distance limit of a search without max_distance: max_distance.unwrap_or(100.0), strict.
+#define STB_DEFAULT_MAX_DIST 100.0
+
 #ifdef __CUDACC__
+#include <math_constants.h>
+
 // Monotone map float -> uint32 (larger float -> larger uint), total order with
 // -inf lowest; NaN never reaches it.
 __device__ __forceinline__ uint32_t stb_f2ord(float f) {
@@ -330,6 +335,91 @@ __device__ __forceinline__ uint32_t stb_key_row(uint64_t k) { return (uint32_t)k
 __device__ __forceinline__ bool stb_hit_less(double da, uint64_t ra, double db,
                                              uint64_t rb) {
   return (da < db) || (da == db && ra < rb);
+}
+
+// ---- the exact re-rank: canonical distance (oracle orc_cosine_f32), hit order, hit output ----
+// Every kernel that returns hits scores them with these, so the bits match the oracle's.
+// sqd: the query staged in f64 (exact conversion of the f32 components).
+
+// ||q||^2: f64 FMAs in index order.
+__device__ __forceinline__ double stb_canon_q2(const double *sqd) {
+  double q2 = 0.0;
+#pragma unroll 8
+  for (int i = 0; i < STB_D; ++i) q2 = fma(sqd[i], sqd[i], q2);
+  return q2;
+}
+
+// q . row and ||row||^2: f64 FMAs in index order, one rounding per step.  f32 x f32 products are
+// exact in f64, so this equals the oracle bit for bit.  LDG: the row is in global memory and read
+// through the read-only path; otherwise it is staged in shared memory.
+template <bool LDG>
+__device__ __forceinline__ void stb_canon_dot(const double *sqd, const float4 *row, double &ab, double &r2) {
+  ab = 0.0;
+  r2 = 0.0;
+#pragma unroll 8
+  for (int i = 0; i < STB_ROW_F4; ++i) {
+    const float4 v = LDG ? __ldg(row + i) : row[i];
+    const double vx = (double)v.x, vy = (double)v.y, vz = (double)v.z, vw = (double)v.w;
+    ab = fma(sqd[4 * i + 0], vx, ab); r2 = fma(vx, vx, r2);
+    ab = fma(sqd[4 * i + 1], vy, ab); r2 = fma(vy, vy, r2);
+    ab = fma(sqd[4 * i + 2], vz, ab); r2 = fma(vz, vz, r2);
+    ab = fma(sqd[4 * i + 3], vw, ab); r2 = fma(vw, vw, r2);
+  }
+}
+
+// Cosine distance: 0 when both vectors are zero, 1 when orthogonal, else max(0, 1 - ab / (|q| |r|)).
+// Callers keep a hit iff the result is strictly below their limit.
+__device__ __forceinline__ double stb_canon_dist(double ab, double q2, double r2) {
+  if (q2 == 0.0 && r2 == 0.0) return 0.0;
+  if (ab == 0.0) return 1.0;
+  const double t = 1.0 - ab / (sqrt(q2) * sqrt(r2));
+  return t > 0.0 ? t : 0.0;
+}
+
+// Ascending sort by (distance, row) of n (power of two) pairs in shared memory; any blockDim.x.
+__device__ __forceinline__ void stb_cta_sort_hits(double *sd, uint64_t *sr, uint32_t n) {
+  for (uint32_t kk = 2; kk <= n; kk <<= 1)
+    for (uint32_t j = kk >> 1; j > 0; j >>= 1) {
+      for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
+        const uint32_t ixj = i ^ j;
+        if (ixj > i) {
+          const bool up = ((i & kk) == 0);
+          const bool gt = stb_hit_less(sd[ixj], sr[ixj], sd[i], sr[i]);
+          if (gt == up) {
+            const double td = sd[i]; const uint64_t tr = sr[i];
+            sd[i] = sd[ixj]; sr[i] = sr[ixj]; sd[ixj] = td; sr[ixj] = tr;
+          }
+        }
+      }
+      __syncthreads();
+    }
+}
+
+// Ascending sort of n (power of two) keys in shared memory, thread-strided; any blockDim.x.
+__device__ __forceinline__ void stb_cta_sort_keys_strided(uint64_t *keys, uint32_t n) {
+  for (uint32_t kk = 2; kk <= n; kk <<= 1)
+    for (uint32_t j = kk >> 1; j > 0; j >>= 1) {
+      for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
+        const uint32_t ixj = i ^ j;
+        if (ixj > i) {
+          const uint64_t x = keys[i], y = keys[ixj];
+          const bool up = ((i & kk) == 0);
+          if ((x > y) == up) { keys[i] = y; keys[ixj] = x; }
+        }
+      }
+      __syncthreads();
+    }
+}
+
+// out[0, k): the first n_out sorted pairs, then (+inf, UINT64_MAX) padding, which merges as-is.
+__device__ __forceinline__ void stb_write_hits(stb_hit *out, const double *sd, const uint64_t *sr, uint32_t n_out,
+                                               uint32_t k) {
+  for (uint32_t i = threadIdx.x; i < k; i += blockDim.x) {
+    stb_hit h;
+    h.distance = (i < n_out) ? sd[i] : CUDART_INF;
+    h.row = (i < n_out) ? sr[i] : 0xffffffffffffffffull;
+    out[i] = h;
+  }
 }
 
 // Ascending bitonic sort of n keys (power of two, <= R*256) held in shared memory,

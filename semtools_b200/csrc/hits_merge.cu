@@ -26,28 +26,8 @@ stb_hits_merge_kernel(const stb_hit *lists, uint32_t total, uint32_t n_sort, uin
     }
   }
   __syncthreads();
-  for (uint32_t k = 2; k <= n_sort; k <<= 1) {
-    for (uint32_t j = k >> 1; j > 0; j >>= 1) {
-      for (uint32_t i = threadIdx.x; i < n_sort; i += blockDim.x) {
-        uint32_t ixj = i ^ j;
-        if (ixj > i) {
-          bool up = ((i & k) == 0);
-          bool gt = stb_hit_less(sd[ixj], sr[ixj], sd[i], sr[i]);
-          if (gt == up) {
-            double td = sd[i]; uint64_t tr = sr[i];
-            sd[i] = sd[ixj]; sr[i] = sr[ixj]; sd[ixj] = td; sr[ixj] = tr;
-          }
-        }
-      }
-      __syncthreads();
-    }
-  }
-  for (uint32_t i = threadIdx.x; i < top_k; i += blockDim.x) {
-    stb_hit h;
-    h.distance = (i < n_sort) ? sd[i] : CUDART_INF;
-    h.row = (i < n_sort) ? sr[i] : 0xffffffffffffffffull;
-    out[i] = h;
-  }
+  stb_cta_sort_hits(sd, sr, n_sort);
+  stb_write_hits(out, sd, sr, min(top_k, n_sort), top_k);
 }
 
 // Batched form: lists[n_lists][nq][per_list] -> out[nq][top_k]; one CTA per query.
@@ -68,27 +48,8 @@ stb_hits_merge_batch_kernel(const stb_hit *lists, uint32_t n_lists, uint32_t nq,
     sd[i] = d; sr[i] = r;
   }
   __syncthreads();
-  for (uint32_t k = 2; k <= n_sort; k <<= 1)
-    for (uint32_t j = k >> 1; j > 0; j >>= 1) {
-      for (uint32_t i = threadIdx.x; i < n_sort; i += blockDim.x) {
-        const uint32_t ixj = i ^ j;
-        if (ixj > i) {
-          const bool up = ((i & k) == 0);
-          const bool gt = stb_hit_less(sd[ixj], sr[ixj], sd[i], sr[i]);
-          if (gt == up) {
-            double td = sd[i]; uint64_t tr = sr[i];
-            sd[i] = sd[ixj]; sr[i] = sr[ixj]; sd[ixj] = td; sr[ixj] = tr;
-          }
-        }
-      }
-      __syncthreads();
-    }
-  for (uint32_t i = threadIdx.x; i < top_k; i += blockDim.x) {
-    stb_hit h;
-    h.distance = (i < n_sort) ? sd[i] : CUDART_INF;
-    h.row = (i < n_sort) ? sr[i] : 0xffffffffffffffffull;
-    out[(size_t)q * top_k + i] = h;
-  }
+  stb_cta_sort_hits(sd, sr, n_sort);
+  stb_write_hits(out + (size_t)q * top_k, sd, sr, min(top_k, n_sort), top_k);
 }
 
 // ---- sharded K2: exchange of the nq x k per-rank hits over NVLink peer memory -------------------
@@ -157,27 +118,8 @@ stb_batch_xchg_merge_kernel(const StbBatchXchgArgs a, uint32_t n_sort, stb_hit *
     sd[i] = d; sr[i] = r;
   }
   __syncthreads();
-  for (uint32_t k = 2; k <= n_sort; k <<= 1)
-    for (uint32_t j = k >> 1; j > 0; j >>= 1) {
-      for (uint32_t i = threadIdx.x; i < n_sort; i += blockDim.x) {
-        const uint32_t ixj = i ^ j;
-        if (ixj > i) {
-          const bool up = ((i & k) == 0);
-          const bool gt = stb_hit_less(sd[ixj], sr[ixj], sd[i], sr[i]);
-          if (gt == up) {
-            double td = sd[i]; uint64_t tr = sr[i];
-            sd[i] = sd[ixj]; sr[i] = sr[ixj]; sd[ixj] = td; sr[ixj] = tr;
-          }
-        }
-      }
-      __syncthreads();
-    }
-  for (uint32_t i = threadIdx.x; i < a.top_k; i += blockDim.x) {
-    stb_hit h;
-    h.distance = (i < n_sort) ? sd[i] : CUDART_INF;
-    h.row = (i < n_sort) ? sr[i] : 0xffffffffffffffffull;
-    out[(size_t)q * a.top_k + i] = h;
-  }
+  stb_cta_sort_hits(sd, sr, n_sort);
+  stb_write_hits(out + (size_t)q * a.top_k, sd, sr, min(a.top_k, n_sort), a.top_k);
   if (threadIdx.x == 0) {
     uint32_t ok = s_timeout ? 0u : 1u, n = 0;
     const uint32_t *st = bx_status(mine, a.world);

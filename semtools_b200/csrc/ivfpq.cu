@@ -285,18 +285,7 @@ ivf_probe_lut_kernel(const float *coarse, uint32_t nlist, uint32_t nprobe, const
   if (threadIdx.x < STB_D) sq[threadIdx.x] = q[threadIdx.x];
   __syncthreads();
   if (threadIdx.x == 0) { float s = 0.f; for (int i = 0; i < STB_D; ++i) s += sq[i] * sq[i]; s_inv = s > 0.f ? rsqrtf(s) : 0.f; }
-  for (uint32_t kk = 2; kk <= npow; kk <<= 1)
-    for (uint32_t j = kk >> 1; j > 0; j >>= 1) {
-      for (uint32_t i = threadIdx.x; i < npow; i += blockDim.x) {
-        const uint32_t ixj = i ^ j;
-        if (ixj > i) {
-          const uint64_t x = skeys[i], y = skeys[ixj];
-          const bool up = ((i & kk) == 0);
-          if ((x > y) == up) { skeys[i] = y; skeys[ixj] = x; }
-        }
-      }
-      __syncthreads();
-    }
+  stb_cta_sort_keys_strided(skeys, npow);
   // probe[0..nprobe) = list ids (best first); probe[nprobe_max .. ] = prefix of list lengths
   if (threadIdx.x == 0) {
     uint32_t acc = 0;
@@ -458,18 +447,7 @@ ivf_coarse_probe_kernel(const Probe2Args a) {
   if (threadIdx.x < STB_D) sq[threadIdx.x] = a.q[threadIdx.x];
   __syncthreads();
   if (threadIdx.x == 0) { float s = 0.f; for (int i = 0; i < STB_D; ++i) s += sq[i] * sq[i]; s_inv = s > 0.f ? rsqrtf(s) : 0.f; }
-  for (uint32_t kk = 2; kk <= npow; kk <<= 1)
-    for (uint32_t j = kk >> 1; j > 0; j >>= 1) {
-      for (uint32_t i = threadIdx.x; i < npow; i += blockDim.x) {
-        const uint32_t ixj = i ^ j;
-        if (ixj > i) {
-          const uint64_t x = p2_keys[i], y = p2_keys[ixj];
-          const bool up = ((i & kk) == 0);
-          if ((x > y) == up) { p2_keys[i] = y; p2_keys[ixj] = x; }
-        }
-      }
-      __syncthreads();
-    }
+  stb_cta_sort_keys_strided(p2_keys, npow);
   // list sizes in parallel (one thread per probed list), then a serial prefix over shared memory:
   // a single thread chasing 2 x nprobe dependent global loads cost ~20 us of this kernel's 62
   __shared__ uint32_t s_sz[1024];
@@ -503,21 +481,6 @@ struct Adc2Args {
   const float4 *rows; uint64_t row_base; const float *q; uint32_t top_k, rerank;
   stb_hit *out_hits; uint32_t *out_status;     // status: [0] hits, [1] codes scanned
 };
-
-__device__ __forceinline__ void adc2_sort_keys(uint64_t *k, uint32_t n, uint32_t tid, uint32_t nthreads) {
-  for (uint32_t kk = 2; kk <= n; kk <<= 1)
-    for (uint32_t j = kk >> 1; j > 0; j >>= 1) {
-      for (uint32_t i = tid; i < n; i += nthreads) {
-        const uint32_t ixj = i ^ j;
-        if (ixj > i) {
-          const uint64_t x = k[i], y = k[ixj];
-          const bool up = ((i & kk) == 0);
-          if ((x > y) == up) { k[i] = y; k[ixj] = x; }
-        }
-      }
-      __syncthreads();
-    }
-}
 
 __global__ void __launch_bounds__(ADC2_THREADS, 1)
 ivf_adc_finish_kernel(const Adc2Args a) {
@@ -567,7 +530,7 @@ ivf_adc_finish_kernel(const Adc2Args a) {
     s_keys[warp_in * 64 + e * 32 + lane] = ok ? stb_make_key(top.ls[e], top.lr[e]) : STB_KEY_INVALID;
   }
   __syncthreads();
-  adc2_sort_keys(s_keys, (ADC2_THREADS / 32) * 64, tid, ADC2_THREADS);
+  stb_cta_sort_keys_strided(s_keys, (ADC2_THREADS / 32) * 64);
   for (uint32_t i = tid; i < ADC2_KEEP; i += ADC2_THREADS) a.keys2[(size_t)blockIdx.x * ADC2_KEEP + i] = s_keys[i];
   __threadfence();
   __syncthreads();
@@ -587,12 +550,8 @@ ivf_adc_finish_kernel(const Adc2Args a) {
   for (uint32_t i = tid; i < STB_D; i += ADC2_THREADS) sqd[i] = (double)a.q[i];
   if (tid == 0) s_pass = 0;
   __syncthreads();
-  adc2_sort_keys(fk, n_sort, tid, ADC2_THREADS);
-  if (tid == 0) {
-    double q2 = 0.0;
-    for (int i = 0; i < STB_D; ++i) q2 = fma(sqd[i], sqd[i], q2);
-    s_q2 = q2;
-  }
+  stb_cta_sort_keys_strided(fk, n_sort);
+  if (tid == 0) s_q2 = stb_canon_q2(sqd);
   __syncthreads();
   const uint32_t r = min(min(a.rerank, (uint32_t)ADC2_RERANK_CAP), n_all);
   uint32_t n2 = 32;
@@ -607,51 +566,17 @@ ivf_adc_finish_kernel(const Adc2Args a) {
     const uint64_t key = (c < r) ? fk[c] : STB_KEY_INVALID;
     if (key != STB_KEY_INVALID) {
       const uint64_t row = a.order[stb_key_row(key)];
-      const float4 *rp = a.rows + row * STB_ROW_F4;
-      double ab = 0.0, r2 = 0.0;
-#pragma unroll 8
-      for (int i = 0; i < STB_ROW_F4; ++i) {
-        const float4 v = __ldg(rp + i);
-        const double vx = (double)v.x, vy = (double)v.y, vz = (double)v.z, vw = (double)v.w;
-        ab = fma(sqd[4 * i + 0], vx, ab); r2 = fma(vx, vx, r2);
-        ab = fma(sqd[4 * i + 1], vy, ab); r2 = fma(vy, vy, r2);
-        ab = fma(sqd[4 * i + 2], vz, ab); r2 = fma(vz, vz, r2);
-        ab = fma(sqd[4 * i + 3], vw, ab); r2 = fma(vw, vw, r2);
-      }
-      double dist;
-      if (q2 == 0.0 && r2 == 0.0) dist = 0.0;
-      else if (ab == 0.0) dist = 1.0;
-      else {
-        const double t = 1.0 - ab / (sqrt(q2) * sqrt(r2));
-        dist = t > 0.0 ? t : 0.0;
-      }
-      if (dist < 100.0) { d = dist; grow = a.row_base + row; atomicAdd(&s_pass, 1); }
+      double ab, r2;
+      stb_canon_dot<true>(sqd, a.rows + row * STB_ROW_F4, ab, r2);
+      const double dist = stb_canon_dist(ab, q2, r2);
+      if (dist < STB_DEFAULT_MAX_DIST) { d = dist; grow = a.row_base + row; atomicAdd(&s_pass, 1); }
     }
     sd[c] = d; sr[c] = grow;
   }
   __syncthreads();
-  for (uint32_t kk = 2; kk <= n2; kk <<= 1)
-    for (uint32_t j = kk >> 1; j > 0; j >>= 1) {
-      for (uint32_t i = tid; i < n2; i += ADC2_THREADS) {
-        const uint32_t ixj = i ^ j;
-        if (ixj > i) {
-          const bool up = ((i & kk) == 0);
-          const bool gt = stb_hit_less(sd[ixj], sr[ixj], sd[i], sr[i]);
-          if (gt == up) {
-            const double td = sd[i]; const uint64_t tr = sr[i];
-            sd[i] = sd[ixj]; sr[i] = sr[ixj]; sd[ixj] = td; sr[ixj] = tr;
-          }
-        }
-      }
-      __syncthreads();
-    }
+  stb_cta_sort_hits(sd, sr, n2);
   const uint32_t n_out = min((uint32_t)s_pass, a.top_k);
-  for (uint32_t i = tid; i < a.top_k; i += ADC2_THREADS) {          // unused tail: (+inf, UINT64_MAX), mergeable as-is
-    stb_hit h;
-    h.distance = (i < n_out) ? sd[i] : CUDART_INF;
-    h.row = (i < n_out) ? sr[i] : 0xffffffffffffffffull;
-    a.out_hits[i] = h;
-  }
+  stb_write_hits(a.out_hits, sd, sr, n_out, a.top_k);
   if (tid == 0) { a.out_status[0] = n_out; a.out_status[1] = total; *a.ticket = 0; }
 }
 
@@ -906,7 +831,7 @@ int stb_ivfpq_search(stb_ivfpq *x, const float *q, uint32_t nprobe, uint32_t top
     STB_CUDA(cudaMalloc(&ctx->collect_hits, e_pad * sizeof(stb_hit)));
     ctx->collect_hits_cap = e_pad;
   }
-  if ((rc = stb_launch_exact(ctx, x->corpus->rows, x->corpus->row_base, ctx->q_dev, x->cand_rows, nv, 100.0,
+  if ((rc = stb_launch_exact(ctx, x->corpus->rows, x->corpus->row_base, ctx->q_dev, x->cand_rows, nv, STB_DEFAULT_MAX_DIST,
                              ctx->collect_hits, e_pad, ctx->collect_count + 1)) != STB_OK) return rc;
   if ((rc = stb_launch_sort_hits(ctx, ctx->collect_hits, e_pad)) != STB_OK) return rc;
   unsigned long long pass = 0;

@@ -1095,18 +1095,12 @@ stb_scan_topk_kernel(const TopkArgs args) {
 
   // ---- exact re-rank of the best KF in canonical arithmetic --------------------------
   // Rows are staged through shared memory (coalesced, one DRAM latency), then one
-  // thread per candidate accumulates (ab, q2, r2) with f64 FMAs in index order:
-  // f32 x f32 products are exact in f64, so this equals orc_cosine_f32 bit for bit.
+  // thread per candidate accumulates (ab, r2) with stb_canon_dot and scores it with stb_canon_dist.
   for (int i = threadIdx.x; i < STB_D; i += blockDim.x) sqd[i] = (double)__ldg(args.scan.q + i);
   if (threadIdx.x < 2) s_nv[threadIdx.x] = 0;
   if (threadIdx.x < KF) { s_d[threadIdx.x] = CUDART_INF; s_r[threadIdx.x] = 0xffffffffffffffffull; }
   __syncthreads();
-  if (threadIdx.x == 5 * 32) {                       // an otherwise idle warp: ||q||^2 once
-    double q2 = 0.0;
-#pragma unroll 8
-    for (int i = 0; i < STB_D; ++i) q2 = fma(sqd[i], sqd[i], q2);
-    s_q2 = q2;
-  }
+  if (threadIdx.x == 5 * 32) s_q2 = stb_canon_q2(sqd);   // an otherwise idle warp: ||q||^2 once
   // Candidates are sorted by approximate score (or upper bound) best-first and re-scored 32 at a
   // time.  After the first 32 the k-th best EXACT cosine c_k among them is known; a later
   // candidate whose score + eps is below c_k cannot enter the top-k, and neither can anything
@@ -1143,18 +1137,8 @@ stb_scan_topk_kernel(const TopkArgs args) {
       const int cl = (threadIdx.x >> 5) * 8 + lane;          // candidate inside the chunk
       const int ci = chunk * 32 + cl;
       if (skeys[ci] != STB_KEY_INVALID) {
-        const float4 *rp = reinterpret_cast<const float4 *>(srows + cl * STB_RR_STRIDE);
-        double ab = 0.0, r2 = 0.0;
-#pragma unroll 8
-        for (int i = 0; i < STB_ROW_F4; ++i) {
-          const float4 v = rp[i];
-          const double vx = (double)v.x, vy = (double)v.y, vz = (double)v.z, vw = (double)v.w;
-          // oracle order (orc_cosine_f32(q,row)): index order, one rounding per step
-          ab = fma(sqd[4 * i + 0], vx, ab); r2 = fma(vx, vx, r2);
-          ab = fma(sqd[4 * i + 1], vy, ab); r2 = fma(vy, vy, r2);
-          ab = fma(sqd[4 * i + 2], vz, ab); r2 = fma(vz, vz, r2);
-          ab = fma(sqd[4 * i + 3], vw, ab); r2 = fma(vw, vw, r2);
-        }
+        double ab, r2;
+        stb_canon_dot<false>(sqd, reinterpret_cast<const float4 *>(srows + cl * STB_RR_STRIDE), ab, r2);
         s_d[ci] = ab;          // finalised below once ||q||^2 is known
         s_r2[ci] = r2;
       }
@@ -1166,11 +1150,8 @@ stb_scan_topk_kernel(const TopkArgs args) {
         const uint64_t key = skeys[lane];
         double dist = CUDART_INF;
         if (key != STB_KEY_INVALID) {
-          const double ab = s_d[lane], r2 = s_r2[lane], q2 = s_q2;
-          if (q2 == 0.0 && r2 == 0.0) dist = 0.0;
-          else if (ab == 0.0) dist = 1.0;
-          else { const double t = 1.0 - ab / (sqrt(q2) * sqrt(r2)); dist = t > 0.0 ? t : 0.0; }
-          if (!(dist < 100.0)) dist = CUDART_INF;
+          dist = stb_canon_dist(s_d[lane], s_q2, s_r2[lane]);
+          if (!(dist < STB_DEFAULT_MAX_DIST)) dist = CUDART_INF;
         }
         int rank = 0;
 #pragma unroll
@@ -1191,15 +1172,8 @@ stb_scan_topk_kernel(const TopkArgs args) {
     uint64_t grow = 0xffffffffffffffffull;
     if (key != STB_KEY_INVALID) atomicAdd(&s_nv[0], 1);     // valid candidates (re-scored or provably outside the top-k)
     if (key != STB_KEY_INVALID && (int)threadIdx.x < 32 * s_done) {
-      const double ab = s_d[threadIdx.x], r2 = s_r2[threadIdx.x], q2 = s_q2;
-      double dist;
-      if (q2 == 0.0 && r2 == 0.0) dist = 0.0;
-      else if (ab == 0.0) dist = 1.0;
-      else {
-        double t = 1.0 - ab / (sqrt(q2) * sqrt(r2));
-        dist = t > 0.0 ? t : 0.0;
-      }
-      if (dist < 100.0) {                         // max_distance.unwrap_or(100.0), strict
+      const double dist = stb_canon_dist(s_d[threadIdx.x], s_q2, s_r2[threadIdx.x]);
+      if (dist < STB_DEFAULT_MAX_DIST) {
         d = dist;
         grow = args.row_base + (uint64_t)stb_key_row(key);
         atomicAdd(&s_nv[1], 1);                   // passing
@@ -1209,23 +1183,7 @@ stb_scan_topk_kernel(const TopkArgs args) {
     s_r[threadIdx.x] = grow;
   }
   __syncthreads();
-  // bitonic sort of the KF (distance,row) pairs
-  for (int k = 2; k <= KF; k <<= 1) {
-    for (int jj = k >> 1; jj > 0; jj >>= 1) {
-      int i = threadIdx.x;
-      if (i < KF) {
-        int ixj = i ^ jj;
-        if (ixj > i) {
-          double da = s_d[i], db = s_d[ixj];
-          uint64_t ra = s_r[i], rb = s_r[ixj];
-          bool up = ((i & k) == 0);
-          bool gt = stb_hit_less(db, rb, da, ra);
-          if (gt == up) { s_d[i] = db; s_r[i] = rb; s_d[ixj] = da; s_r[ixj] = ra; }
-        }
-      }
-      __syncthreads();
-    }
-  }
+  stb_cta_sort_hits(s_d, s_r, KF);
   STB_T_MAX(5);                      // exact re-rank + hit sort done
   const int n_valid = s_nv[0], n_pass = s_nv[1];
   const uint32_t k = args.top_k;
@@ -1238,12 +1196,7 @@ stb_scan_topk_kernel(const TopkArgs args) {
     complete = (n_out == k) && ((1.0 - (double)s_drop - kScoreEps) > s_d[k - 1]);
   }
   if (args.xchg.world <= 1) {
-    for (uint32_t i = threadIdx.x; i < k; i += blockDim.x) {
-      stb_hit h;
-      h.distance = (i < n_out) ? s_d[i] : CUDART_INF;
-      h.row = (i < n_out) ? s_r[i] : 0xffffffffffffffffull;
-      args.out_hits[i] = h;
-    }
+    stb_write_hits(args.out_hits, s_d, s_r, n_out, k);
     if (threadIdx.x == 0) {
       args.out_status[0] = n_out;
       args.out_status[1] = complete ? 1u : 0u;
@@ -1257,13 +1210,7 @@ stb_scan_topk_kernel(const TopkArgs args) {
   const StbXchgArgs &X = args.xchg;
   const int world = (int)X.world, me = (int)X.rank;
   const size_t lane_off = (size_t)X.slot * world + me;
-  for (int idx = threadIdx.x; idx < world * (int)k; idx += blockDim.x) {
-    const int p = idx / (int)k, i = idx % (int)k;
-    stb_hit h;
-    h.distance = ((uint32_t)i < n_out) ? s_d[i] : CUDART_INF;
-    h.row = ((uint32_t)i < n_out) ? s_r[i] : 0xffffffffffffffffull;
-    stb_x_hits(X, p)[lane_off * X.max_k + i] = h;
-  }
+  for (int p = 0; p < world; ++p) stb_write_hits(stb_x_hits(X, p) + lane_off * X.max_k, s_d, s_r, n_out, k);
   if (threadIdx.x < world) stb_x_status(X, threadIdx.x)[lane_off] = (complete ? 1u : 0u) | (n_out << 8);
   __threadfence_system();
   __syncthreads();
@@ -1297,28 +1244,8 @@ stb_scan_topk_kernel(const TopkArgs args) {
     md[i] = d; mr[i] = r;
   }
   __syncthreads();
-  for (int kk = 2; kk <= n_sort; kk <<= 1) {
-    for (int jj = kk >> 1; jj > 0; jj >>= 1) {
-      for (int i = threadIdx.x; i < n_sort; i += blockDim.x) {
-        int ixj = i ^ jj;
-        if (ixj > i) {
-          bool up = ((i & kk) == 0);
-          bool gt = stb_hit_less(md[ixj], mr[ixj], md[i], mr[i]);
-          if (gt == up) {
-            double td = md[i]; uint64_t tr = mr[i];
-            md[i] = md[ixj]; mr[i] = mr[ixj]; md[ixj] = td; mr[ixj] = tr;
-          }
-        }
-      }
-      __syncthreads();
-    }
-  }
-  for (uint32_t i = threadIdx.x; i < k; i += blockDim.x) {
-    stb_hit h;
-    h.distance = md[i];
-    h.row = mr[i];
-    args.out_hits[i] = h;
-  }
+  stb_cta_sort_hits(md, mr, (uint32_t)n_sort);
+  stb_write_hits(args.out_hits, md, mr, k, k);     // n_sort >= world * k: no padding
   if (threadIdx.x == 0) {
     uint32_t all_complete = s_timeout ? 0u : 1u, total = 0u;
     const uint32_t *st = stb_x_status(X, me) + (size_t)X.slot * world;
@@ -1620,8 +1547,11 @@ __global__ void stb_exact_kernel(const float4 *rows, uint64_t row_base, const fl
                                  const uint32_t *row_ids, uint64_t m, double limit,
                                  stb_hit *hits, uint64_t m_padded,
                                  unsigned long long *pass_count) {
-  __shared__ __align__(16) float sq[STB_D];
-  for (int i = threadIdx.x; i < STB_D; i += blockDim.x) sq[i] = __ldg(q + i);
+  __shared__ double sqd[STB_D];
+  __shared__ double s_q2;
+  for (int i = threadIdx.x; i < STB_D; i += blockDim.x) sqd[i] = (double)__ldg(q + i);
+  __syncthreads();
+  if (threadIdx.x == 0) s_q2 = stb_canon_q2(sqd);
   __syncthreads();
   uint64_t idx = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= m_padded) return;
@@ -1630,25 +1560,9 @@ __global__ void stb_exact_kernel(const float4 *rows, uint64_t row_base, const fl
   h.row = 0xffffffffffffffffull;
   if (idx < m) {
     uint32_t row = row_ids[idx];
-    const float4 *rp = rows + (size_t)row * STB_ROW_F4;
-    const float4 *qp = reinterpret_cast<const float4 *>(sq);
-    double ab = 0.0, q2 = 0.0, r2 = 0.0;
-#pragma unroll 4
-    for (int i = 0; i < STB_ROW_F4; ++i) {
-      float4 v = __ldg(rp + i);
-      float4 w = qp[i];
-      ab = fma((double)w.x, (double)v.x, ab); q2 = fma((double)w.x, (double)w.x, q2); r2 = fma((double)v.x, (double)v.x, r2);
-      ab = fma((double)w.y, (double)v.y, ab); q2 = fma((double)w.y, (double)w.y, q2); r2 = fma((double)v.y, (double)v.y, r2);
-      ab = fma((double)w.z, (double)v.z, ab); q2 = fma((double)w.z, (double)w.z, q2); r2 = fma((double)v.z, (double)v.z, r2);
-      ab = fma((double)w.w, (double)v.w, ab); q2 = fma((double)w.w, (double)w.w, q2); r2 = fma((double)v.w, (double)v.w, r2);
-    }
-    double dist;
-    if (q2 == 0.0 && r2 == 0.0) dist = 0.0;
-    else if (ab == 0.0) dist = 1.0;
-    else {
-      double t = 1.0 - ab / (sqrt(q2) * sqrt(r2));
-      dist = t > 0.0 ? t : 0.0;
-    }
+    double ab, r2;
+    stb_canon_dot<true>(sqd, rows + (size_t)row * STB_ROW_F4, ab, r2);
+    const double dist = stb_canon_dist(ab, s_q2, r2);
     if (dist < limit) {
       h.distance = dist;
       h.row = row_base + (uint64_t)row;
