@@ -271,7 +271,19 @@ int stb_search_batch_xchg_dev(stb_ctx *ctx, const stb_corpus *corpus, const floa
  * product quantiser on the residual, ADC lookup-table scan of the nprobe best lists,
  * exact re-rank of the `rerank` best candidates.  Returned distances are exact canonical
  * distances; only the candidate set is approximate.  The index refers to the corpus it
- * was built on (rows [0, n) at build time) and must be destroyed before it. */
+ * was built on (rows [0, n) at build time) and must be destroyed before it.
+ * Forced rows: rows with a non-finite component or an fp32 squared norm outside [1e-30, 1e30]
+ * (K1's forced candidates) are kept out of training and of the inverted lists; every search
+ * re-ranks them exactly besides the ADC candidates.  More than 1024 such rows: the build fails
+ * with STB_ERR_STATE.  With nprobe = nlist and rerank >= the codes scanned (v2: <= 1024 codes;
+ * v1: <= 4096), every row is re-ranked and the hits equal stb_search's.
+ * stb_ivfpq_search: nprobe is clamped to [1, min(nlist, 1024)], rerank to [top_k, 4096];
+ * top_k > 4096 is STB_ERR_ARG.  *out_scanned = codes scanned (forced rows not counted).  It runs the
+ * fused search (v2, stb_ivfpq_search_dev's) when rerank <= 1024 and top_k <= 1024, else the
+ * multi-launch search (v1; also with STB_IVFPQ_V1=1).  v2's funnel: 32-code chunks dealt over 32
+ * CTAs then 16 warps, 64 best per warp, 64 best per CTA, then the `rerank` best of those 2048; it
+ * returns the `rerank` best ADC scores exactly when no warp and no CTA holds more than 64 of them.
+ * v1: 64 best per warp over enough warps to hold min(rerank, codes scanned) candidates. */
 typedef struct stb_ivfpq stb_ivfpq;
 int stb_ivfpq_build(stb_ctx *ctx, const stb_corpus *corpus, uint32_t nlist, uint32_t train_rows,
                     uint32_t iters, stb_ivfpq **out);
@@ -283,7 +295,7 @@ int stb_ivfpq_search(stb_ivfpq *index, const float *q, uint32_t nprobe, uint32_t
 /* Asynchronous device-resident form (query, hits and status stay in HBM, nothing synchronises): the
  * sharded index is one of these per rank, an all-gather of the k hits and stb_hits_merge_dev.
  * out_hits_dev: top_k entries (unused tail +inf / UINT64_MAX); out_status_dev[0] = hits, [1] = codes
- * scanned.  rerank is capped at 1024. */
+ * scanned.  top_k must be 1..1024; rerank is capped at 1024. */
 int stb_ivfpq_search_dev(stb_ivfpq *index, const float *q_dev, uint32_t nprobe, uint32_t top_k,
                          uint32_t rerank, stb_hit *out_hits_dev, uint32_t *out_status_dev);
 
@@ -355,6 +367,12 @@ int stb_debug_q4_refined(stb_ctx *ctx, int reset, uint64_t *refined);
  * NULL) the per-32-row maxima [ceil(nq/128)][ceil(n/256)*8][128]. */
 int stb_debug_batch_gemm(stb_ctx *ctx, const float *q, uint32_t nq, const float *rows,
                          uint64_t n, float *out_full, float *out_submax);
+/* Test hook for K5: synchronous copies of a built index into host buffers; a NULL pointer skips
+ * that array.  centroids [nlist][256] f32, codebooks [32][256][8] f32, list_off [nlist+1],
+ * order [m] (local row of each code), codes [m][32] u8, forced [n - m] (local rows outside the
+ * lists, ascending), where m = list_off[nlist]. */
+int stb_debug_ivfpq_export(const stb_ivfpq *index, float *centroids, float *codebooks,
+                           uint32_t *list_off, uint32_t *order, uint8_t *codes, uint32_t *forced);
 /* Build parameters of K2 (host-only): element type of the shadow the tensor-core pass runs on
  * (0 = bf16, 1 = fp16) and the bound |approximate - exact cosine| <= eps its selection uses. */
 int stb_debug_batch_params(int *shadow_is_f16, double *eps);

@@ -28,6 +28,7 @@ SYMBOLS = [
     "stb_xchg_connect", "stb_xchg_connect_local", "stb_search_topk_xchg", "stb_search_xchg", "stb_search_many", "stb_xchg_create_batch", "stb_search_batch_xchg_dev", "stb_ivfpq_build",
     "stb_ivfpq_destroy", "stb_ivfpq_stats", "stb_ivfpq_search", "stb_ivfpq_search_dev", "stb_hits_merge_dev", "stb_hits_merge_batch_dev", "stb_hits_merge", "stb_fnv1a64", "stb_line_id", "stb_line_ids",
     "stb_ctx_counters", "stb_debug_ticket_check", "stb_debug_timestamps", "stb_debug_q4_refined", "stb_debug_batch_gemm", "stb_debug_batch_params",
+    "stb_debug_ivfpq_export",
 ]
 
 
@@ -116,6 +117,7 @@ def lib() -> C.CDLL:
     L.stb_debug_q4_refined.argtypes = [vp, i32, C.POINTER(u64)]
     L.stb_debug_batch_gemm.argtypes = [vp, vp, u32, vp, u64, vp, vp]
     L.stb_debug_batch_params.argtypes = [C.POINTER(C.c_int), C.POINTER(C.c_double)]
+    L.stb_debug_ivfpq_export.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     for name in SYMBOLS:
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("stb_version", "stb_device_count"):
@@ -400,6 +402,22 @@ class IvfPq:
                                       C.byref(scanned)))
         return out[: n.value], int(scanned.value)
 
+    def export(self):
+        """stb_debug_ivfpq_export: the built index as numpy arrays (centroids, codebooks, list_off,
+        order, codes, forced); m = list_off[-1] rows are in the lists, the others in `forced`."""
+        nlist, n = self.stats()["nlist"], self.stats()["rows"]
+        list_off = np.zeros(nlist + 1, dtype=np.uint32)
+        _check(lib().stb_debug_ivfpq_export(self._h, None, None, _np_ptr(list_off), None, None, None))
+        m = int(list_off[-1])
+        centroids = np.zeros((nlist, STB_DIM), dtype=np.float32)
+        codebooks = np.zeros((32, 256, 8), dtype=np.float32)
+        order = np.zeros(max(m, 1), dtype=np.uint32)
+        codes = np.zeros((max(m, 1), 32), dtype=np.uint8)
+        forced = np.zeros(max(n - m, 1), dtype=np.uint32)
+        _check(lib().stb_debug_ivfpq_export(self._h, _np_ptr(centroids), _np_ptr(codebooks), _np_ptr(list_off),
+                                            _np_ptr(order), _np_ptr(codes), _np_ptr(forced)))
+        return {"centroids": centroids, "codebooks": codebooks, "list_off": list_off, "order": order[:m],
+                "codes": codes[:m], "forced": forced[: n - m]}
 
     def search_dev(self, q_dev: int, nprobe: int, top_k: int, rerank: int, out_hits_dev: int, out_status_dev: int):
         """stb_ivfpq_search_dev: asynchronous, everything stays in HBM."""

@@ -15,6 +15,12 @@
 // Query: coarse scores q^.c_j (nlist*1 KiB read), top-nprobe lists, LUT[s][code] = q^_s .
 // cb[s][code] (32 KiB), ADC score = q^.c_list + sum_s LUT[s][code_s] over the probed
 // lists' codes ((nprobe/nlist)*n*32 bytes), running top-R, exact re-rank of R rows.
+//
+// Forced rows: a row with a non-finite component or an fp32 ||x||^2 outside [1e-30, 1e30] (the
+// rows K1 forces into its candidates) has no usable direction, so its PQ code says nothing about
+// its cosine.  Such rows are kept out of the inverted lists and out of training; the build records
+// them in a side list (at most IVF_FORCED_CAP, usually empty) that every search re-ranks exactly
+// in addition to the ADC candidates.
 #include <math_constants.h>
 
 #include <algorithm>
@@ -25,18 +31,23 @@
 #define PQ_M 32
 #define PQ_DSUB 8
 #define PQ_KSUB 256
+#define IVF_FORCED_CAP 1024        // forced rows per index; more -> the build fails with STB_ERR_STATE
+#define IVF_HOST_TOPK_MAX 4096     // stb_ivfpq_search: top_k and rerank cap of the multi-launch search
+#define IVF_NO_LIST 0xffffffffu    // assign[] of a forced row
 
 struct stb_ivfpq {
   stb_ctx *ctx;
   const stb_corpus *corpus;
   uint32_t nlist;
-  uint64_t n;                 // rows indexed
+  uint64_t n;                 // rows indexed (listed + forced)
   float *centroids;           // [nlist][256]
   float *codebooks;           // [32][256][8]
-  uint8_t *codes;             // [n][32], grouped by list
-  uint32_t *order;            // [n] local row of code i
-  uint32_t *list_off;         // [nlist+1] (device)
+  uint8_t *codes;             // [n_listed][32], grouped by list
+  uint32_t *order;            // [n_listed] local row of code i
+  uint32_t *list_off;         // [nlist+1] (device); list_off[nlist] = n_listed = n - n_forced
   std::vector<uint32_t> list_off_h;
+  uint32_t *forced;           // [n_forced] local rows outside the lists, ascending
+  uint32_t n_forced;
   // query scratch
   float *coarse;              // [nlist]
   float *lut;                 // [32][256]
@@ -114,17 +125,41 @@ ivf_assign_kernel(const float *__restrict__ X, uint64_t n, const float *__restri
 }
 
 // ---------------------------------------------------------------- k-means updates -----
-// sums[c] += x^ (normalised row), counts[c] += 1   (warp per row)
+// K1's forced-candidate rule on the fp32 ||x||^2 (NaN and +inf included: a non-finite component
+// makes ss NaN or +inf).
+__device__ __forceinline__ bool ivf_forced(float ss) { return !(ss >= 1e-30f && ss <= 1e30f); }
+
+// fp32 ||x||^2 of a row held as 8 floats per lane of a full warp
+__device__ __forceinline__ float ivf_warp_ss(float4 v0, float4 v1) {
+  float ss = v0.x * v0.x + v0.y * v0.y + v0.z * v0.z + v0.w * v0.w + v1.x * v1.x + v1.y * v1.y + v1.z * v1.z + v1.w * v1.w;
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, off);
+  return ss;
+}
+
+// Loads into (v0, v1) the first row r, r+1, ... (mod n, at most 32 tries) that is not forced and
+// leaves its index in r; zeros and false if all of them are forced.  Seeds of centroids and codebook
+// entries come from here, so no seed is non-finite.
+__device__ __forceinline__ bool ivf_load_seed_row(const float4 *X, uint64_t n, uint64_t stride, uint64_t &r, float4 &v0,
+                                                  float4 &v1) {
+  const int lane = threadIdx.x & 31;
+  for (int t = 0; t < 32; ++t, r = (r + 1) % n) {
+    v0 = __ldg(X + r * stride * STB_ROW_F4 + 2 * lane); v1 = __ldg(X + r * stride * STB_ROW_F4 + 2 * lane + 1);
+    if (!ivf_forced(ivf_warp_ss(v0, v1))) return true;
+  }
+  v0 = v1 = make_float4(0.f, 0.f, 0.f, 0.f);
+  return false;
+}
+
+// sums[c] += x^ (normalised row), counts[c] += 1   (warp per row; forced rows are skipped)
 __global__ void ivf_accumulate_kernel(const float4 *__restrict__ X, uint64_t n, uint64_t stride,
                                       const uint32_t *__restrict__ assign, float *sums, uint32_t *counts) {
   const int lane = threadIdx.x & 31;
   const uint64_t i = (uint64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
   if (i >= n) return;
   const float4 v0 = __ldg(X + i * stride * STB_ROW_F4 + 2 * lane), v1 = __ldg(X + i * stride * STB_ROW_F4 + 2 * lane + 1);
-  float ss = v0.x * v0.x + v0.y * v0.y + v0.z * v0.z + v0.w * v0.w + v1.x * v1.x + v1.y * v1.y + v1.z * v1.z + v1.w * v1.w;
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, off);
-  if (!(ss > 0.f) || !(ss < CUDART_INF_F)) return;
+  const float ss = ivf_warp_ss(v0, v1);
+  if (ivf_forced(ss)) return;
   const float inv = rsqrtf(ss);
   float *dst = sums + (size_t)assign[i] * STB_D + 8 * lane;
   atomicAdd(dst + 0, v0.x * inv); atomicAdd(dst + 1, v0.y * inv); atomicAdd(dst + 2, v0.z * inv); atomicAdd(dst + 3, v0.w * inv);
@@ -132,7 +167,7 @@ __global__ void ivf_accumulate_kernel(const float4 *__restrict__ X, uint64_t n, 
   if (lane == 0) atomicAdd(counts + assign[i], 1u);
 }
 
-// centroid = normalise(sum); empty cluster -> re-seeded from a sample row
+// centroid = normalise(sum); empty cluster -> re-seeded from a sample row that is not forced
 __global__ void ivf_finish_centroids_kernel(float *C, const float *sums, const uint32_t *counts, uint32_t nlist,
                                             const float4 *X, uint64_t n, uint64_t stride, uint32_t iter) {
   const int lane = threadIdx.x & 31;
@@ -143,12 +178,10 @@ __global__ void ivf_finish_centroids_kernel(float *C, const float *sums, const u
     v0 = *reinterpret_cast<const float4 *>(sums + (size_t)c * STB_D + 8 * lane);
     v1 = *reinterpret_cast<const float4 *>(sums + (size_t)c * STB_D + 8 * lane + 4);
   } else {
-    const uint64_t r = ((uint64_t)c * 2654435761ull + (uint64_t)iter * 40503ull) % n;
-    v0 = __ldg(X + r * stride * STB_ROW_F4 + 2 * lane); v1 = __ldg(X + r * stride * STB_ROW_F4 + 2 * lane + 1);
+    uint64_t r = ((uint64_t)c * 2654435761ull + (uint64_t)iter * 40503ull) % n;
+    ivf_load_seed_row(X, n, stride, r, v0, v1);
   }
-  float ss = v0.x * v0.x + v0.y * v0.y + v0.z * v0.z + v0.w * v0.w + v1.x * v1.x + v1.y * v1.y + v1.z * v1.z + v1.w * v1.w;
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, off);
+  const float ss = ivf_warp_ss(v0, v1);
   const float inv = ss > 0.f ? rsqrtf(ss) : 0.f;
   float *dst = C + (size_t)c * STB_D + 8 * lane;
   dst[0] = v0.x * inv; dst[1] = v0.y * inv; dst[2] = v0.z * inv; dst[3] = v0.w * inv;
@@ -157,7 +190,8 @@ __global__ void ivf_finish_centroids_kernel(float *C, const float *sums, const u
 
 // ------------------------------------------------------------------ PQ train / encode --
 // Lane s of a warp owns sub-space s (8 dims) of the residual x^ - c(x) of one row.
-// mode 0: accumulate into the code's sums/counts (k-means step);  mode 1: write the code.
+// mode 0: accumulate into the code's sums/counts (k-means step; forced rows are skipped);
+// mode 1: write the code (a forced row's code is never read: the row stays out of the lists).
 // The 256 KB of codebooks do not fit in shared memory: a launch handles sub-spaces
 // [s0, s0+8) (64 KB), 4 rows per warp step (lane = row_in_group*8 + sub-space).
 struct PqArgs {
@@ -206,6 +240,7 @@ pq_step_kernel(const PqArgs a) {
     }
     if (!valid) continue;
     if (a.mode == 0) {
+      if (ivf_forced(ss)) continue;
       float *dst = a.sums + ((size_t)s * PQ_KSUB + bc) * PQ_DSUB;
 #pragma unroll
       for (int d = 0; d < 8; ++d) atomicAdd(dst + d, r[d]);
@@ -224,32 +259,45 @@ __global__ void pq_finish_codebooks_kernel(float *cb, const float *sums, const u
   for (int d = 0; d < 8; ++d) cb[(size_t)i * 8 + d] = sums[(size_t)i * 8 + d] / (float)c;
 }
 
-// seed codebooks from residuals of the first 256 sample rows
+// seed codebooks from residuals of 256 sample rows that are not forced (a zero entry if none is found)
 __global__ void pq_seed_kernel(float *cb, const float4 *X, uint64_t n, uint64_t stride, const uint32_t *assign, const float *C) {
   const int code = blockIdx.x, lane = threadIdx.x;          // 256 blocks x 32 lanes (lane = sub-space)
-  const uint64_t i = ((uint64_t)code * 7919u) % n;
-  const float4 *xr = X + i * stride * STB_ROW_F4;
-  const float4 x0 = __ldg(xr + lane * 2), x1 = __ldg(xr + lane * 2 + 1);
-  float ss = x0.x * x0.x + x0.y * x0.y + x0.z * x0.z + x0.w * x0.w + x1.x * x1.x + x1.y * x1.y + x1.z * x1.z + x1.w * x1.w;
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, off);
-  const float inv = ss > 0.f ? rsqrtf(ss) : 0.f;
+  uint64_t i = ((uint64_t)code * 7919u) % n;
+  float4 x0, x1;
+  float *dst = cb + ((size_t)lane * PQ_KSUB + code) * PQ_DSUB;
+  if (!ivf_load_seed_row(X, n, stride, i, x0, x1)) {
+    for (int d = 0; d < 8; ++d) dst[d] = 0.f;
+    return;
+  }
+  const float inv = rsqrtf(ivf_warp_ss(x0, x1));
   const float4 *cr = reinterpret_cast<const float4 *>(C + (size_t)assign[i] * STB_D);
   const float4 c0 = __ldg(cr + lane * 2), c1 = __ldg(cr + lane * 2 + 1);
-  float *dst = cb + ((size_t)lane * PQ_KSUB + code) * PQ_DSUB;
   dst[0] = x0.x * inv - c0.x; dst[1] = x0.y * inv - c0.y; dst[2] = x0.z * inv - c0.z; dst[3] = x0.w * inv - c0.w;
   dst[4] = x1.x * inv - c1.x; dst[5] = x1.y * inv - c1.y; dst[6] = x1.z * inv - c1.z; dst[7] = x1.w * inv - c1.w;
 }
 
 // ------------------------------------------------------------------ inverted lists ----
+// forced rows (warp per row): assign[i] = IVF_NO_LIST, local row appended to forced[] (count in
+// *n_forced; entries past `cap` are counted, not written)
+__global__ void ivf_flag_forced_kernel(const float4 *__restrict__ X, uint64_t n, uint32_t *assign, uint32_t *forced,
+                                       uint32_t cap, uint32_t *n_forced) {
+  const int lane = threadIdx.x & 31;
+  const uint64_t i = (uint64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (i >= n) return;
+  const float4 v0 = __ldg(X + i * STB_ROW_F4 + 2 * lane), v1 = __ldg(X + i * STB_ROW_F4 + 2 * lane + 1);
+  if (!ivf_forced(ivf_warp_ss(v0, v1)) || lane != 0) return;
+  assign[i] = IVF_NO_LIST;
+  const uint32_t k = atomicAdd(n_forced, 1u);
+  if (k < cap) forced[k] = (uint32_t)i;
+}
 __global__ void ivf_hist_kernel(const uint32_t *assign, uint64_t n, uint32_t *hist) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) atomicAdd(hist + assign[i], 1u);
+  if (i < n && assign[i] != IVF_NO_LIST) atomicAdd(hist + assign[i], 1u);
 }
 __global__ void ivf_scatter_kernel(const uint32_t *assign, uint64_t n, uint32_t *cursor, const uint8_t *codes_row,
                                    uint8_t *codes, uint32_t *order) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
+  if (i >= n || assign[i] == IVF_NO_LIST) return;
   const uint32_t pos = atomicAdd(cursor + assign[i], 1u);
   order[pos] = (uint32_t)i;
   const uint4 *src = reinterpret_cast<const uint4 *>(codes_row + i * PQ_M);
@@ -400,9 +448,12 @@ __global__ void ivf_pick_rows_kernel(const stb_hit *cand, uint32_t r, const uint
 //                            them, writes the probe list + prefix sums and the ADC table.
 //   ivf_adc_finish_kernel    ADC scan (32-row chunks dealt round-robin over CTAs first, then
 //                            warps, so a tight cluster's contiguous codes spread over every
-//                            CTA); each CTA keeps its ADC2_KEEP best; the LAST CTA sorts the
-//                            <= 8192 survivors, re-scores the best `rerank` rows exactly
-//                            (canonical f64, as K1) and writes the top-k hits.
+//                            CTA); each warp keeps its 64 best, each CTA its ADC2_KEEP best; the
+//                            LAST CTA sorts the 32 x 64 = 2048 survivors, re-scores the best
+//                            `rerank` rows and the forced rows exactly (canonical f64, as K1) and
+//                            writes the top-k hits.
+// The funnel returns the `rerank` best ADC scores exactly when no warp and no CTA of the deal holds
+// more than 64 of them (every code is re-ranked when the probed lists hold <= 2048 codes).
 // Default since round 2 (validated on hardware); STB_IVFPQ_V1=1 selects the multi-launch search above.
 #define ADC2_THREADS 512
 #define ADC2_MAX_CTAS 32
@@ -479,6 +530,7 @@ struct Adc2Args {
   const float *coarse; const float *lut; const uint32_t *order;
   uint64_t *keys2; unsigned int *ticket;
   const float4 *rows; uint64_t row_base; const float *q; uint32_t top_k, rerank;
+  const uint32_t *forced; uint32_t n_forced;   // re-ranked in addition to the ADC candidates
   stb_hit *out_hits; uint32_t *out_status;     // status: [0] hits, [1] codes scanned
 };
 
@@ -542,7 +594,7 @@ ivf_adc_finish_kernel(const Adc2Args a) {
   if (!s_last) return;
   __threadfence();
   // ---- last CTA: global selection + exact re-rank
-  uint64_t *fk = reinterpret_cast<uint64_t *>(dyn);       // up to 8192 keys = 64 KiB
+  uint64_t *fk = reinterpret_cast<uint64_t *>(dyn);       // up to 2048 keys = 16 KiB
   const uint32_t n_all = n_ctas * ADC2_KEEP;
   uint32_t n_sort = 64;
   while (n_sort < n_all) n_sort <<= 1;
@@ -555,17 +607,23 @@ ivf_adc_finish_kernel(const Adc2Args a) {
   __syncthreads();
   const uint32_t r = min(min(a.rerank, (uint32_t)ADC2_RERANK_CAP), n_all);
   uint32_t n2 = 32;
-  while (n2 < r) n2 <<= 1;
-  // keys 0..r) live in dyn[0, 8 KiB); the (distance,row) pairs go to dyn[16 KiB, 32 KiB)
+  while (n2 < r + a.n_forced) n2 <<= 1;
+  // keys 0..r) live in dyn[0, 8 KiB); the (distance,row) pairs of the r candidates and the forced
+  // rows (<= 1024 + IVF_FORCED_CAP) go to dyn[16 KiB, 48 KiB)
   double *sd = reinterpret_cast<double *>(dyn + 16384);
-  uint64_t *sr = reinterpret_cast<uint64_t *>(dyn + 16384 + 8 * ADC2_RERANK_CAP);
+  uint64_t *sr = reinterpret_cast<uint64_t *>(dyn + 16384 + 8 * (ADC2_RERANK_CAP + IVF_FORCED_CAP));
   const double q2 = s_q2;
   for (uint32_t c = tid; c < n2; c += ADC2_THREADS) {
     double d = CUDART_INF;
     uint64_t grow = 0xffffffffffffffffull;
-    const uint64_t key = (c < r) ? fk[c] : STB_KEY_INVALID;
-    if (key != STB_KEY_INVALID) {
-      const uint64_t row = a.order[stb_key_row(key)];
+    uint64_t row = 0xffffffffffffffffull;
+    if (c < r) {
+      const uint64_t key = fk[c];
+      if (key != STB_KEY_INVALID) row = a.order[stb_key_row(key)];
+    } else if (c < r + a.n_forced) {
+      row = a.forced[c - r];
+    }
+    if (row != 0xffffffffffffffffull) {
       double ab, r2;
       stb_canon_dot<true>(sqd, a.rows + row * STB_ROW_F4, ab, r2);
       const double dist = stb_canon_dist(ab, q2, r2);
@@ -587,7 +645,7 @@ int stb_ivfpq_destroy(stb_ivfpq *x) {
   if (!x) return STB_OK;
   cudaFree(x->centroids); cudaFree(x->codebooks); cudaFree(x->codes); cudaFree(x->order); cudaFree(x->list_off);
   cudaFree(x->coarse); cudaFree(x->lut); cudaFree(x->probe); cudaFree(x->cand); cudaFree(x->cand_rows);
-  cudaFree(x->keys2); cudaFree(x->tickets);
+  cudaFree(x->keys2); cudaFree(x->tickets); cudaFree(x->forced);
   cudaGetLastError();
   delete x;
   return STB_OK;
@@ -617,7 +675,7 @@ int stb_ivfpq_build(stb_ctx *ctx, const stb_corpus *corpus, uint32_t nlist, uint
   x->ctx = ctx; x->corpus = corpus; x->nlist = nlist; x->n = n;
   x->centroids = nullptr; x->codebooks = nullptr; x->codes = nullptr; x->order = nullptr; x->list_off = nullptr;
   x->coarse = nullptr; x->lut = nullptr; x->probe = nullptr; x->cand = nullptr; x->cand_cap = 0; x->cand_rows = nullptr;
-  x->keys2 = nullptr; x->tickets = nullptr;
+  x->keys2 = nullptr; x->tickets = nullptr; x->forced = nullptr; x->n_forced = 0;
   cudaStream_t st = ctx->stream;
   // training sample: every `stride`-th row
   uint64_t ns = std::min<uint64_t>(n, std::max<uint32_t>(train_rows, nlist * 32u));
@@ -630,7 +688,7 @@ int stb_ivfpq_build(stb_ctx *ctx, const stb_corpus *corpus, uint32_t nlist, uint
   IVF_CUDA(cudaMalloc(&x->centroids, (size_t)nlist * STB_D * 4));
   IVF_CUDA(cudaMalloc(&x->codebooks, (size_t)PQ_M * PQ_KSUB * PQ_DSUB * 4));
   IVF_CUDA(cudaMalloc(&sums, (size_t)nlist * STB_D * 4));
-  IVF_CUDA(cudaMalloc(&counts, (size_t)nlist * 4));
+  IVF_CUDA(cudaMalloc(&counts, (size_t)(nlist + 1) * 4));
   IVF_CUDA(cudaMalloc(&pq_sums, (size_t)PQ_M * PQ_KSUB * PQ_DSUB * 4));
   IVF_CUDA(cudaMalloc(&pq_counts, (size_t)PQ_M * PQ_KSUB * 4));
   IVF_CUDA(cudaMalloc(&assign, n * 4));
@@ -679,11 +737,31 @@ int stb_ivfpq_build(stb_ctx *ctx, const stb_corpus *corpus, uint32_t nlist, uint
     pa.s0 = s0; pa.mode = 1;
     pq_step_kernel<<<ctx->sm_count * 2, 256, 8 * PQ_KSUB * PQ_DSUB * 4, st>>>(pa);
   }
-  IVF_CUDA(cudaMemsetAsync(counts, 0, (size_t)nlist * 4, st));
+  // forced rows leave the lists (assign = IVF_NO_LIST) for the side list; counts[nlist] is their count
+  IVF_CUDA(cudaMalloc(&x->forced, IVF_FORCED_CAP * 4));
+  IVF_CUDA(cudaMemsetAsync(counts, 0, (size_t)(nlist + 1) * 4, st));
+  ivf_flag_forced_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(X4, n, assign, x->forced, IVF_FORCED_CAP, counts + nlist);
   ivf_hist_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(assign, n, counts);
-  std::vector<uint32_t> hist(nlist);
-  IVF_CUDA(cudaMemcpyAsync(hist.data(), counts, (size_t)nlist * 4, cudaMemcpyDeviceToHost, st));
+  std::vector<uint32_t> hist(nlist + 1);
+  IVF_CUDA(cudaMemcpyAsync(hist.data(), counts, (size_t)(nlist + 1) * 4, cudaMemcpyDeviceToHost, st));
   IVF_CUDA(cudaStreamSynchronize(st));
+  if (hist[nlist] > IVF_FORCED_CAP) {
+    stb_set_error("ivfpq_build: %u rows are non-finite or have an fp32 squared norm outside [1e-30, 1e30] (at most %u)",
+                  hist[nlist], (unsigned)IVF_FORCED_CAP);
+    cudaFree(sums); cudaFree(counts); cudaFree(pq_sums); cudaFree(pq_counts); cudaFree(assign); cudaFree(cursor);
+    cudaFree(codes_row); cudaFree(sample);
+    stb_ivfpq_destroy(x);
+    return STB_ERR_STATE;
+  }
+  x->n_forced = hist[nlist];
+  {  // ascending, so the side list does not depend on the order the atomics ran in
+    std::vector<uint32_t> f(x->n_forced);
+    IVF_CUDA(cudaMemcpyAsync(f.data(), x->forced, (size_t)x->n_forced * 4, cudaMemcpyDeviceToHost, st));
+    IVF_CUDA(cudaStreamSynchronize(st));
+    std::sort(f.begin(), f.end());
+    IVF_CUDA(cudaMemcpyAsync(x->forced, f.data(), (size_t)x->n_forced * 4, cudaMemcpyHostToDevice, st));
+    IVF_CUDA(cudaStreamSynchronize(st));
+  }
   x->list_off_h.assign(nlist + 1, 0);
   for (uint32_t l = 0; l < nlist; ++l) x->list_off_h[l + 1] = x->list_off_h[l] + hist[l];
   IVF_CUDA(cudaMemcpyAsync(x->list_off, x->list_off_h.data(), (size_t)(nlist + 1) * 4, cudaMemcpyHostToDevice, st));
@@ -693,7 +771,7 @@ int stb_ivfpq_build(stb_ctx *ctx, const stb_corpus *corpus, uint32_t nlist, uint
   IVF_CUDA(cudaMalloc(&x->coarse, (size_t)nlist * 4));
   IVF_CUDA(cudaMalloc(&x->lut, (size_t)PQ_M * PQ_KSUB * 4));
   IVF_CUDA(cudaMalloc(&x->probe, (size_t)(2 * 1024 + 1) * 4));
-  IVF_CUDA(cudaMalloc(&x->cand_rows, 4096 * 4 + 16));
+  IVF_CUDA(cudaMalloc(&x->cand_rows, (IVF_HOST_TOPK_MAX + IVF_FORCED_CAP) * 4 + 16));   // + the valid-row counter
   IVF_CUDA(cudaMalloc(&x->keys2, (size_t)ADC2_MAX_CTAS * ADC2_KEEP * 8));
   IVF_CUDA(cudaMalloc(&x->tickets, 2 * sizeof(unsigned int)));
   IVF_CUDA(cudaMemsetAsync(x->tickets, 0, 2 * sizeof(unsigned int), ctx->stream));
@@ -738,7 +816,8 @@ static int ivf_fused_launch(stb_ivfpq *x, const float *q_dev, uint32_t nprobe, u
   aa.codes = x->codes; aa.list_off = x->list_off; aa.probe = x->probe; aa.nprobe = nprobe; aa.coarse = x->coarse;
   aa.lut = x->lut; aa.order = x->order; aa.keys2 = x->keys2; aa.ticket = x->tickets + 1;
   aa.rows = reinterpret_cast<const float4 *>(x->corpus->rows); aa.row_base = x->corpus->row_base; aa.q = q_dev;
-  aa.top_k = top_k; aa.rerank = rerank; aa.out_hits = out_hits_dev; aa.out_status = out_status_dev;
+  aa.top_k = top_k; aa.rerank = rerank; aa.forced = x->forced; aa.n_forced = x->n_forced;
+  aa.out_hits = out_hits_dev; aa.out_status = out_status_dev;
   ivf_adc_finish_kernel<<<ADC2_MAX_CTAS, ADC2_THREADS, ADC2_SMEM, st>>>(aa);
   STB_CUDA(cudaGetLastError());
   ctx->kernel_launches += 2;
@@ -764,8 +843,9 @@ int stb_ivfpq_search(stb_ivfpq *x, const float *q, uint32_t nprobe, uint32_t top
   if (cudaSetDevice(ctx->device) != cudaSuccess) { stb_set_error("cudaSetDevice failed"); return STB_ERR_CUDA; }
   *out_n = 0;
   if (top_k == 0) return STB_OK;
+  if (top_k > IVF_HOST_TOPK_MAX) { stb_set_error("ivfpq_search: top_k must be <= %u", (unsigned)IVF_HOST_TOPK_MAX); return STB_ERR_ARG; }
   nprobe = std::max(1u, std::min(std::min(nprobe, x->nlist), 1024u));
-  rerank = std::max(top_k, std::min(rerank, 4096u));
+  rerank = std::max(top_k, std::min(rerank, (uint32_t)IVF_HOST_TOPK_MAX));
   cudaStream_t st = ctx->stream;
   memcpy(ctx->q_pin, q, STB_D * sizeof(float));
   STB_CUDA(cudaMemcpyAsync(ctx->q_dev, ctx->q_pin, STB_D * sizeof(float), cudaMemcpyHostToDevice, st));
@@ -788,40 +868,52 @@ int stb_ivfpq_search(stb_ivfpq *x, const float *q, uint32_t nprobe, uint32_t top
   STB_ATTR_ONCE(ctx, STB_ATTR_IVF_PROBE,
                 cudaFuncSetAttribute(ivf_probe_lut_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 8));
   ivf_probe_lut_kernel<<<1, 1024, npow * 8, st>>>(x->coarse, x->nlist, nprobe, x->list_off, x->codebooks, ctx->q_dev, x->probe, x->lut);
+  ctx->kernel_launches += 2;
   uint32_t total = 0;
   STB_CUDA(cudaMemcpyAsync(&total, x->probe + 2 * nprobe, 4, cudaMemcpyDeviceToHost, st));
   STB_CUDA(cudaStreamSynchronize(st));
   if (out_scanned) *out_scanned = total;
-  if (total == 0) return STB_OK;
-  // warps: enough to spread every list over many warps and fill the GPU, at most 512
-  uint32_t ctas = std::max<uint32_t>(1, std::min<uint32_t>((total + 2047) / 2048, 64));
-  uint64_t m = (uint64_t)ctas * 8 * 64, m_pad = 1024;
-  while (m_pad < m) m_pad <<= 1;
-  if (m_pad > x->cand_cap) {
-    cudaFree(x->cand); x->cand = nullptr; x->cand_cap = 0;
-    STB_CUDA(cudaMalloc(&x->cand, m_pad * sizeof(stb_hit)));
-    x->cand_cap = m_pad;
-  }
-  if (m_pad > m) {   // padding entries: +inf
-    std::vector<stb_hit> pad(m_pad - m);
-    for (auto &h : pad) { h.distance = INFINITY; h.row = 0xffffffffffffffffull; }
-    STB_CUDA(cudaMemcpyAsync(x->cand + m, pad.data(), pad.size() * sizeof(stb_hit), cudaMemcpyHostToDevice, st));
-    STB_CUDA(cudaStreamSynchronize(st));
-  }
-  AdcArgs a;
-  a.codes = x->codes; a.list_off = x->list_off; a.probe = x->probe; a.nprobe = nprobe; a.coarse = x->coarse; a.lut = x->lut;
-  a.cand = x->cand;
-  ivf_adc_kernel<<<ctas, 256, 0, st>>>(a);
-  STB_CUDA(cudaGetLastError());
   int rc;
-  if ((rc = stb_launch_sort_hits(ctx, x->cand, m_pad)) != STB_OK) return rc;
-  const uint32_t r = (uint32_t)std::min<uint64_t>(rerank, m);
-  uint32_t *n_valid = x->cand_rows + 4096;
-  STB_CUDA(cudaMemsetAsync(n_valid, 0, 4, st));
-  ivf_pick_rows_kernel<<<(r + 255) / 256, 256, 0, st>>>(x->cand, r, x->order, x->cand_rows, n_valid);
   uint32_t nv = 0;
-  STB_CUDA(cudaMemcpyAsync(&nv, n_valid, 4, cudaMemcpyDeviceToHost, st));
-  STB_CUDA(cudaStreamSynchronize(st));
+  if (total > 0) {
+    // warps: enough to spread every list over many warps and fill the GPU, at most 512, and enough
+    // that the warps' 64-entry lists hold min(rerank, total) candidates.  When total <= rerank no
+    // warp sees more than 64 codes, so every scanned code is re-ranked.
+    const uint32_t want = std::min(total, rerank);
+    const uint32_t ctas = std::max<uint32_t>(1, std::min<uint32_t>(std::max((total + 2047) / 2048, (want + 511) / 512), 64));
+    uint64_t m = (uint64_t)ctas * 8 * 64, m_pad = 1024;
+    while (m_pad < m) m_pad <<= 1;
+    if (m_pad > x->cand_cap) {
+      cudaFree(x->cand); x->cand = nullptr; x->cand_cap = 0;
+      STB_CUDA(cudaMalloc(&x->cand, m_pad * sizeof(stb_hit)));
+      x->cand_cap = m_pad;
+    }
+    if (m_pad > m) {   // padding entries: +inf
+      std::vector<stb_hit> pad(m_pad - m);
+      for (auto &h : pad) { h.distance = INFINITY; h.row = 0xffffffffffffffffull; }
+      STB_CUDA(cudaMemcpyAsync(x->cand + m, pad.data(), pad.size() * sizeof(stb_hit), cudaMemcpyHostToDevice, st));
+      STB_CUDA(cudaStreamSynchronize(st));
+    }
+    AdcArgs a;
+    a.codes = x->codes; a.list_off = x->list_off; a.probe = x->probe; a.nprobe = nprobe; a.coarse = x->coarse; a.lut = x->lut;
+    a.cand = x->cand;
+    ivf_adc_kernel<<<ctas, 256, 0, st>>>(a);
+    STB_CUDA(cudaGetLastError());
+    if ((rc = stb_launch_sort_hits(ctx, x->cand, m_pad)) != STB_OK) return rc;
+    // r <= rerank <= IVF_HOST_TOPK_MAX entries of cand_rows; the valid ones come first (sorted by -score)
+    const uint32_t r = (uint32_t)std::min<uint64_t>(rerank, m);
+    uint32_t *n_valid = x->cand_rows + IVF_HOST_TOPK_MAX + IVF_FORCED_CAP;
+    STB_CUDA(cudaMemsetAsync(n_valid, 0, 4, st));
+    ivf_pick_rows_kernel<<<(r + 255) / 256, 256, 0, st>>>(x->cand, r, x->order, x->cand_rows, n_valid);
+    STB_CUDA(cudaMemcpyAsync(&nv, n_valid, 4, cudaMemcpyDeviceToHost, st));
+    STB_CUDA(cudaStreamSynchronize(st));
+    ctx->kernel_launches += 2;
+  }
+  // the forced rows follow the ADC candidates
+  if (x->n_forced) {
+    STB_CUDA(cudaMemcpyAsync(x->cand_rows + nv, x->forced, (size_t)x->n_forced * 4, cudaMemcpyDeviceToDevice, st));
+    nv += x->n_forced;
+  }
   if (nv == 0) return STB_OK;
   // exact canonical distances of the nv candidate rows, sorted by (distance,row)
   uint64_t e_pad = 1024;
@@ -843,7 +935,21 @@ int stb_ivfpq_search(stb_ivfpq *x, const float *q, uint32_t nprobe, uint32_t top
     STB_CUDA(cudaStreamSynchronize(st));
   }
   *out_n = n_out;
-  ctx->kernel_launches += 6;
+  return STB_OK;
+}
+
+int stb_debug_ivfpq_export(const stb_ivfpq *x, float *centroids, float *codebooks, uint32_t *list_off, uint32_t *order,
+                           uint8_t *codes, uint32_t *forced) {
+  if (!x) { stb_set_error("ivfpq_export: null index"); return STB_ERR_ARG; }
+  if (cudaSetDevice(x->ctx->device) != cudaSuccess) { stb_set_error("cudaSetDevice failed"); return STB_ERR_CUDA; }
+  const uint64_t listed = x->list_off_h[x->nlist];
+  STB_CUDA(cudaStreamSynchronize(x->ctx->stream));
+  if (centroids) STB_CUDA(cudaMemcpy(centroids, x->centroids, (size_t)x->nlist * STB_D * 4, cudaMemcpyDeviceToHost));
+  if (codebooks) STB_CUDA(cudaMemcpy(codebooks, x->codebooks, (size_t)PQ_M * PQ_KSUB * PQ_DSUB * 4, cudaMemcpyDeviceToHost));
+  if (list_off) memcpy(list_off, x->list_off_h.data(), (size_t)(x->nlist + 1) * 4);
+  if (order && listed) STB_CUDA(cudaMemcpy(order, x->order, listed * 4, cudaMemcpyDeviceToHost));
+  if (codes && listed) STB_CUDA(cudaMemcpy(codes, x->codes, listed * PQ_M, cudaMemcpyDeviceToHost));
+  if (forced && x->n_forced) STB_CUDA(cudaMemcpy(forced, x->forced, (size_t)x->n_forced * 4, cudaMemcpyDeviceToHost));
   return STB_OK;
 }
 

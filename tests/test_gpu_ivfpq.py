@@ -79,7 +79,7 @@ def test_v2_fused_search_matches_v1_candidates_and_exact_distances(ctx):
                 assert h["distance"] == oracle.cosine(q, rows[int(h["row"]) - 7_000_000])
             exact = c.search(q, top_k=10)
             recalls.append(len(set(got["row"].tolist()) & set(exact["row"].tolist())) / 10.0)
-            # the per-warp top-64 / per-CTA top-256 reductions are lossless for the best 512 here,
+            # the per-warp top-64 / per-CTA top-64 reductions are lossless for the best 512 here,
             # so both versions re-rank the same candidates -> identical hits
             assert got["row"].tolist() == v1[i][0]["row"].tolist()
         assert np.mean(recalls) >= 0.9
