@@ -199,20 +199,26 @@ int stb_search_topk_dev(stb_ctx *ctx, const stb_corpus *corpus,
 /* ---- K2: batched queries on the tensor cores ------------------------------------------
  * Q independent top-k searches (the semantics of Q calls of search_documents,
  * src/search/mod.rs:77-120, without max_distance) in one pass over the corpus: an
- * L2-normalised bf16 copy of the corpus (built lazily, 512 B/row, rebuilt after the
- * corpus changes; stb_corpus_prepare_batch builds it ahead of time) is multiplied with
- * the query tile on the wgmma tensor cores, the 32 most promising 32-row sub-tiles per
- * query are re-scored exactly (canonical f64 distance on the f32 rows) and the result is
- * accepted only if the bf16 error bound proves no other row can enter the top-k;
- * unproven queries are answered by the single-query path (stb_search).  Results are
- * therefore identical to stb_search.
+ * L2-normalised 16-bit copy of the corpus (fp16 by default, bf16 with -DSTB_SHADOW_F16=0;
+ * built lazily, 512 B/row, extended after appends; stb_corpus_prepare_batch builds it ahead
+ * of time) is multiplied with the query tile on the wgmma tensor cores.  Pipeline v2 (top_k <= 64
+ * when the sampled threshold fits, see DESIGN §4) emits every row whose approximate score reaches a
+ * per-query threshold and re-scores those exactly; pipeline v1 (larger top_k, small corpora,
+ * STB_BATCH_V1=1) re-scores the 32 most promising 32-row sub-tiles per query.  Re-scores use the
+ * canonical f64 distance on the f32 rows, and a result is accepted only if the 16-bit error bound
+ * proves no other row can enter the top-k; unproven queries are answered by the single-query path
+ * (stb_search).  Results are therefore identical to stb_search.
  *   q         nq x 256 f32 (host);  out_hits nq x top_k (unused tail: +inf / UINT64_MAX)
  *   out_n     nq counts */
 int stb_corpus_prepare_batch(stb_corpus *corpus);
 int stb_search_batch(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t nq,
                      uint32_t top_k, stb_hit *out_hits, uint32_t *out_n);
 /* Asynchronous device-resident form: out_status_dev[2*i] = hits of query i,
- * [2*i+1] = 1 iff proven exact (0: re-run query i through stb_search). */
+ * [2*i+1] = 1 iff proven exact (0: re-run query i through stb_search).  A query that cannot be
+ * normalised in fp32 (a NaN or infinite component, or a non-zero fp32 squared norm outside
+ * [1e-30, 1e30]) is never proven; the other queries of the batch are unaffected.  A zero query is
+ * valid but every row ties with it, so it is proven only on corpora of at most top_k rows.
+ * Corpus rows that cannot be normalised make the call fail with STB_ERR_STATE. */
 int stb_search_batch_dev(stb_ctx *ctx, const stb_corpus *corpus, const float *q_dev,
                          uint32_t nq, uint32_t top_k, stb_hit *out_hits_dev,
                          uint32_t *out_status_dev);
@@ -254,7 +260,8 @@ int stb_search_topk_xchg(stb_ctx *ctx, const stb_corpus *corpus, const float *q_
  * stb_search_batch_xchg_dev = stb_search_batch_dev on the local shard, then a push kernel (this rank's
  * nq x k hits into every peer's slot over NVLink, release-stored sequence flag) and a merge kernel (waits
  * for every peer's flag, merges each query's world x k hits by (distance,row)): two launches, no NCCL.
- *   out_status_dev[2q] = hits of query q, [2q+1] = 1 iff every rank proved its part (0: re-run query q
+ *   out_status_dev[2q] = hits of query q, [2q+1] = 1 iff every rank proved its part, so a query that
+ *   cannot be normalised is unproven on every rank (0: re-run query q
  *   through stb_search_xchg / stb_search_many on every rank; 2: a peer never arrived -- see above:
  *   treat the exchange as dead, the flags of this batch are not the same on every rank).
  * All ranks must issue the same sequence of calls. */
@@ -373,6 +380,12 @@ int stb_debug_batch_gemm(stb_ctx *ctx, const float *q, uint32_t nq, const float 
  * lists, ascending), where m = list_off[nlist]. */
 int stb_debug_ivfpq_export(const stb_ivfpq *index, float *centroids, float *codebooks,
                            uint32_t *list_off, uint32_t *order, uint8_t *codes, uint32_t *forced);
+/* Test hook for K2: describes the most recent stb_search_batch_dev on ctx (synchronises the stream).
+ * info = {route (1 = v1, 2 = v2, 0 = none yet), nq, n_sample, stride, n_seg, seg_cap}; the last four are
+ * v2's sampled tiles (0, stride, 2*stride, ...), emitting grid and per-(query, CTA) key capacity, and 0
+ * after v1.  After v2, thr (may be NULL) receives the nq emission thresholds and cand_cnt (may be NULL)
+ * the raw emission counts [nq][n_seg]; a count above seg_cap marks an overflowed segment. */
+int stb_debug_batch_last(stb_ctx *ctx, uint32_t info[6], float *thr, uint32_t *cand_cnt);
 /* Build parameters of K2 (host-only): element type of the shadow the tensor-core pass runs on
  * (0 = bf16, 1 = fp16) and the bound |approximate - exact cosine| <= eps its selection uses. */
 int stb_debug_batch_params(int *shadow_is_f16, double *eps);

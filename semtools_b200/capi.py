@@ -28,6 +28,7 @@ SYMBOLS = [
     "stb_xchg_connect", "stb_xchg_connect_local", "stb_search_topk_xchg", "stb_search_xchg", "stb_search_many", "stb_xchg_create_batch", "stb_search_batch_xchg_dev", "stb_ivfpq_build",
     "stb_ivfpq_destroy", "stb_ivfpq_stats", "stb_ivfpq_search", "stb_ivfpq_search_dev", "stb_hits_merge_dev", "stb_hits_merge_batch_dev", "stb_hits_merge", "stb_fnv1a64", "stb_line_id", "stb_line_ids",
     "stb_ctx_counters", "stb_debug_ticket_check", "stb_debug_timestamps", "stb_debug_q4_refined", "stb_debug_batch_gemm", "stb_debug_batch_params",
+    "stb_debug_batch_last",
     "stb_debug_ivfpq_export",
 ]
 
@@ -117,6 +118,7 @@ def lib() -> C.CDLL:
     L.stb_debug_q4_refined.argtypes = [vp, i32, C.POINTER(u64)]
     L.stb_debug_batch_gemm.argtypes = [vp, vp, u32, vp, u64, vp, vp]
     L.stb_debug_batch_params.argtypes = [C.POINTER(C.c_int), C.POINTER(C.c_double)]
+    L.stb_debug_batch_last.argtypes = [vp, vp, vp, vp]
     L.stb_debug_ivfpq_export.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     for name in SYMBOLS:
         fn = getattr(L, name)
@@ -204,6 +206,20 @@ class Context:
         a, b = u64(0), u64(0)
         _check(lib().stb_debug_ticket_check(self._h, C.byref(a), C.byref(b)))
         return int(a.value), int(b.value)
+
+    def batch_last(self):
+        """stb_debug_batch_last: the most recent K2 device call on this context.  Returns a dict with
+        route (1 = v1, 2 = v2), nq, n_sample, stride, n_seg, seg_cap and, after v2, thr [nq] (f32) and
+        cand_cnt [nq][n_seg] (raw counts; > seg_cap marks an overflowed segment)."""
+        info = np.zeros(6, dtype=np.uint32)
+        _check(lib().stb_debug_batch_last(self._h, _np_ptr(info), None, None))
+        out = dict(zip(("route", "nq", "n_sample", "stride", "n_seg", "seg_cap"), (int(v) for v in info)))
+        if out["route"] == 2:
+            thr = np.zeros(max(out["nq"], 1), dtype=np.float32)
+            cnt = np.zeros((max(out["nq"], 1), max(out["n_seg"], 1)), dtype=np.uint32)
+            _check(lib().stb_debug_batch_last(self._h, _np_ptr(info), _np_ptr(thr), _np_ptr(cnt)))
+            out["thr"], out["cand_cnt"] = thr[: out["nq"]], cnt[: out["nq"]]
+        return out
 
     # -- K4 ------------------------------------------------------------------
     def hits_merge(self, lists: np.ndarray, top_k: int) -> np.ndarray:
@@ -348,7 +364,7 @@ class Corpus:
                 for i, name in enumerate(("f32", "h16", "q8"))}
 
     def prepare_batch(self):
-        """stb_corpus_prepare_batch: build the bf16 tensor-core shadow now."""
+        """stb_corpus_prepare_batch: build the 16-bit tensor-core shadow now."""
         _check(lib().stb_corpus_prepare_batch(self._h))
 
     def search_batch(self, queries, top_k: int = 10):

@@ -149,7 +149,7 @@ int stb_ctx_destroy(stb_ctx *c) {
   cudaFree(c->collect_hits); cudaFree(c->ranges_dev); cudaFree(c->err_flag);
   cudaFree(c->tickets); cudaFree(c->q4_thr); cudaFree(c->q4_refined);
   cudaFree(c->dbg_dev); cudaFree(c->hist_dev); cudaFree(c->bq_tiles); cudaFree(c->b_submax); cudaFree(c->b_tilemax); cudaFree(c->b_cand);
-  cudaFree(c->b_thr); cudaFree(c->b_cnt); cudaFree(c->b_keys);
+  cudaFree(c->b_thr); cudaFree(c->b_cnt); cudaFree(c->b_keys); cudaFree(c->b_qbad);
   cudaFree(c->bq_dev); cudaFree(c->bh_dev); cudaFree(c->bs_dev); cudaFree(c->embed_off_dev); cudaFree(c->embed_ids_dev); cudaFree(c->embed_out_dev);
   if (c->q_pin) cudaFreeHost(c->q_pin);
   if (c->hits_pin) cudaFreeHost(c->hits_pin);
@@ -1031,10 +1031,15 @@ int stb_search_batch_dev(stb_ctx *ctx, const stb_corpus *corpus_c, const float *
     n_sample = std::min<uint32_t>(std::min<uint32_t>(n_full, 8192u), (n_full / 64 + sm - 1) / sm * sm);
   }
   const bool v2_fits = n_sample >= top_k && expected_emitted(n_sample) <= 2048;
+  // one flag per query, written by the query shadow build: a query that cannot be normalised in fp32
+  // has a zero (or NaN) shadow whose scores bound nothing, and both finish kernels report it unproven
+  if ((rc = dev_reserve(&ctx->b_qbad, &ctx->b_qbad_cap, (size_t)q_pad)) != STB_OK) return rc;
   if (!force_v1 && top_k <= 64 && v2_fits) {
     constexpr uint32_t kSegCap = 64;                      // per (query, CTA): ~5 expected at 10M rows / 132 CTAs
     const uint32_t n_seg = stb_batch_emit_grid(ctx, n_tiles);
     const uint32_t stride = n_full / n_sample;
+    const uint32_t last[6] = {2u, nq, n_sample, stride, n_seg, kSegCap};
+    memcpy(ctx->b_last, last, sizeof(last));
     if ((rc = dev_reserve(&ctx->bq_tiles, &ctx->bq_tiles_cap, (size_t)q_pad * 512)) != STB_OK) return rc;
     if ((rc = dev_reserve(&ctx->b_tilemax, &ctx->b_tilemax_cap, (size_t)n_sample * q_pad)) != STB_OK) return rc;
     if ((rc = dev_reserve(&ctx->b_thr, &ctx->b_thr_cap, (size_t)q_pad)) != STB_OK) return rc;
@@ -1042,15 +1047,17 @@ int stb_search_batch_dev(stb_ctx *ctx, const stb_corpus *corpus_c, const float *
     if ((rc = dev_reserve(&ctx->b_keys, &ctx->b_keys_cap, (size_t)q_pad * n_seg * kSegCap)) != STB_OK) return rc;
     STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
     STB_CUDA(cudaMemsetAsync(ctx->b_cnt, 0, (size_t)q_pad * n_seg * sizeof(uint32_t), ctx->stream));
-    if ((rc = stb_launch_shadow_build(ctx, q_dev, nq, 128, ctx->bq_tiles, ctx->err_flag)) != STB_OK) return rc;
+    if ((rc = stb_launch_shadow_build(ctx, q_dev, nq, 128, ctx->bq_tiles, ctx->err_flag, 0, ctx->b_qbad)) != STB_OK) return rc;
     if ((rc = stb_launch_batch_gemm_strided(ctx, ctx->bq_tiles, m_tiles, corpus->shadow, n_sample, stride, nullptr,
                                             ctx->b_tilemax, nullptr)) != STB_OK) return rc;
     if ((rc = stb_launch_batch_thresh(ctx, ctx->b_tilemax, n_sample, nq, q_pad, top_k, ctx->b_thr)) != STB_OK) return rc;
     if ((rc = stb_launch_batch_gemm_emit(ctx, ctx->bq_tiles, m_tiles, corpus->shadow, n_tiles, corpus->n, ctx->b_thr,
                                          ctx->b_cnt, ctx->b_keys, kSegCap)) != STB_OK) return rc;
     return stb_launch_batch_finish2(ctx, ctx->b_keys, ctx->b_cnt, n_seg, kSegCap, nq, top_k, corpus->rows, corpus->n,
-                                    corpus->row_base, q_dev, out_hits_dev, out_status_dev);
+                                    corpus->row_base, q_dev, ctx->b_qbad, out_hits_dev, out_status_dev);
   }
+  const uint32_t last[6] = {1u, nq, 0u, 0u, 0u, 0u};
+  memcpy(ctx->b_last, last, sizeof(last));
   // selection slices: enough CTAs (m_tiles x n_slices) to hide the latency of the streaming
   // read; the finish kernel merges n_slices x 32 <= 4096 candidate tiles per query
   uint32_t n_slices = std::max<uint32_t>(1, std::min<uint32_t>(128, 1536 / m_tiles));
@@ -1061,13 +1068,13 @@ int stb_search_batch_dev(stb_ctx *ctx, const stb_corpus *corpus_c, const float *
   if ((rc = dev_reserve(&ctx->b_cand, &ctx->b_cand_cap, (size_t)q_pad * n_slices * 32)) != STB_OK) return rc;
   // query tiles: padding queries beyond nq are written as zeros by the shadow builder
   STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
-  if ((rc = stb_launch_shadow_build(ctx, q_dev, nq, 128, ctx->bq_tiles, ctx->err_flag)) != STB_OK) return rc;
+  if ((rc = stb_launch_shadow_build(ctx, q_dev, nq, 128, ctx->bq_tiles, ctx->err_flag, 0, ctx->b_qbad)) != STB_OK) return rc;
   if ((rc = stb_launch_batch_gemm(ctx, ctx->bq_tiles, m_tiles, corpus->shadow, n_tiles, ctx->b_submax, ctx->b_tilemax, nullptr)) != STB_OK) return rc;
   // two-level selection: the best tiles by tile maximum (1/8 of the data), refined to
   // sub-tiles inside the finish kernel
   if ((rc = stb_launch_batch_select(ctx, ctx->b_tilemax, n_tiles, q_pad, n_slices, ctx->b_cand)) != STB_OK) return rc;
   return stb_launch_batch_finish(ctx, ctx->b_cand, n_slices, n_sub, nq, top_k, corpus->rows, corpus->n,
-                                 corpus->row_base, q_dev, out_hits_dev, out_status_dev, ctx->b_submax, q_pad);
+                                 corpus->row_base, q_dev, ctx->b_qbad, out_hits_dev, out_status_dev, ctx->b_submax, q_pad);
 }
 
 int stb_search_batch(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t nq, uint32_t top_k,
@@ -1089,13 +1096,11 @@ int stb_search_batch(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uin
     if (rc == STB_ERR_STATE) { tensor_ok = false; }        // un-normalisable rows: K1 handles them
     else if (rc != STB_OK) return rc;
     else {
-      int qbad = 0;
-      STB_CUDA(cudaMemcpyAsync(&qbad, ctx->err_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+      // a query that could not be normalised comes back unproven (status[2q+1] = 0) like any other
       STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
       STB_CUDA(cudaMemcpyAsync(out_hits, ctx->bh_dev, (size_t)nq * top_k * sizeof(stb_hit), cudaMemcpyDeviceToHost, ctx->stream));
       STB_CUDA(cudaMemcpyAsync(status.data(), ctx->bs_dev, (size_t)nq * 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
       STB_CUDA(cudaStreamSynchronize(ctx->stream));
-      if (qbad) std::fill(status.begin(), status.end(), 0u);   // a query could not be normalised: trust none
     }
   }
   // queries the tensor path could not prove (or could not run): exact single-query path
@@ -1138,6 +1143,20 @@ int stb_search_batch_xchg_dev(stb_ctx *ctx, const stb_corpus *corpus, const floa
   a.ticket = x->batch_ticket;
   for (uint32_t r = 0; r < x->world; ++r) a.slot[r] = x->peers[r] + x->batch_off + (size_t)(a.seq & 1) * x->batch_slot_bytes;
   return stb_launch_batch_xchg(ctx, a, ctx->bh_dev, ctx->bs_dev, out_hits_dev, out_status_dev);
+}
+
+int stb_debug_batch_last(stb_ctx *ctx, uint32_t info[6], float *thr, uint32_t *cand_cnt) {
+  int rc = ctx_use(ctx);
+  if (rc) return rc;
+  if (!info) { stb_set_error("debug_batch_last: null info"); return STB_ERR_ARG; }
+  STB_CUDA(cudaStreamSynchronize(ctx->stream));
+  memcpy(info, ctx->b_last, sizeof(ctx->b_last));
+  const uint32_t nq = ctx->b_last[1], n_seg = ctx->b_last[4];
+  if (ctx->b_last[0] == 2u && nq) {
+    if (thr) STB_CUDA(cudaMemcpy(thr, ctx->b_thr, (size_t)nq * sizeof(float), cudaMemcpyDeviceToHost));
+    if (cand_cnt) STB_CUDA(cudaMemcpy(cand_cnt, ctx->b_cnt, (size_t)nq * n_seg * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  }
+  return STB_OK;
 }
 
 int stb_debug_batch_params(int *shadow_is_f16, double *eps) {

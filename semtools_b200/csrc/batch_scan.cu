@@ -25,7 +25,7 @@
 //                               completeness proof: every unselected row has approximate
 //                               cosine <= m* (the smallest selected sub-tile maximum),
 //                               hence exact cosine <= m* + EPS2 (bf16 rounding bound).
-// Tensor-bound: 2*Q*N*256 FLOP per batch; HBM traffic N*512 B (bf16 shadow) once.
+// Tensor-bound: 2*Q*N*256 FLOP per batch; HBM traffic N*512 B (16-bit shadow) once.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <math_constants.h>
@@ -43,8 +43,8 @@
 #define STB_A_RING 6
 #define STB_SUB 32                // rows per sub-tile
 #define STB_BATCH_KSEL 32         // sub-tiles kept per query
-// Shadow element type.  bf16 (default, the configuration validated on hardware) or fp16
-// (-DSTB_SHADOW_F16=1; same wgmma rate).  For L2-normalised rows every element is
+// Shadow element type.  fp16 (default, STB_SHADOW_F16=1 in common.cuh) or bf16
+// (-DSTB_SHADOW_F16=0; same wgmma rate).  For L2-normalised rows every element is
 // <= 1, so fp16's range suffices and its 10-bit mantissa shrinks the selection margin ~4x:
 //   bf16: 8 significand bits -> unit roundoff u = 2^-8; both operands rounded:
 //         |approx - exact cosine| <= (2u+u^2) = 0.00783, + f32 accumulation + rsqrt  < 0.0079
@@ -160,7 +160,7 @@ __device__ __forceinline__ uint64_t wg_desc_sw128(uint32_t smem_addr) {
 template <int TILE>
 __global__ void __launch_bounds__(256)
 stb_shadow_build_kernel(const float4 *__restrict__ rows, uint64_t first_row, uint64_t n_rows, uint64_t n_padded,
-                        uint8_t *__restrict__ out, int *bad_flag) {
+                        uint8_t *__restrict__ out, int *bad_flag, uint32_t *row_bad) {
   const int lane = threadIdx.x & 31;
   const uint64_t row = first_row + (uint64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
   if (row >= n_padded) return;
@@ -174,15 +174,20 @@ stb_shadow_build_kernel(const float4 *__restrict__ rows, uint64_t first_row, uin
 #pragma unroll
   for (int off = 16; off > 0; off >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, off);
   float inv = 0.f;
+  bool bad = false;
   if (ss != 0.f) {
-    if (!(ss >= 1e-30f && ss <= 1e30f)) { if (lane == 0) atomicExch(bad_flag, 1); }   // NaN/inf/extreme
+    if (!(ss >= 1e-30f && ss <= 1e30f)) bad = true;   // NaN/inf/extreme
     else inv = rsqrtf(ss);
   } else {
     // fp32 underflow of a tiny non-zero row: cannot be normalised here -> batch path unusable
     bool nz = (v0.x != 0.f) | (v0.y != 0.f) | (v0.z != 0.f) | (v0.w != 0.f) | (v1.x != 0.f) | (v1.y != 0.f) |
               (v1.z != 0.f) | (v1.w != 0.f);
-    if (__any_sync(0xffffffffu, nz) && lane == 0) atomicExch(bad_flag, 1);
+    bad = __any_sync(0xffffffffu, nz);
   }
+  if (bad && lane == 0) atomicExch(bad_flag, 1);
+  // per-row record (query tiles): a row that cannot be normalised is scaled by 0 (NaN where a component is
+  // NaN or infinite), so its approximate scores bound nothing; the finish kernels mark it unproven
+  if (row_bad && lane == 0) row_bad[row] = bad ? 1u : 0u;
 #if STB_SHADOW_F16
   __half2 p0 = __floats2half2_rn(v0.x * inv, v0.y * inv);
   __half2 p1 = __floats2half2_rn(v0.z * inv, v0.w * inv);
@@ -419,15 +424,15 @@ void stb_batch_build_params(int *shadow_is_f16, double *eps) {
 
 // ------------------------------------------------------- host-side: shadow + GEMM ------
 int stb_launch_shadow_build(stb_ctx *ctx, const float *rows_dev, uint64_t n_rows, int tile, uint8_t *out,
-                            int *bad_flag_dev, uint64_t first_row) {
+                            int *bad_flag_dev, uint64_t first_row, uint32_t *row_bad_dev) {
   // rows [first_row, n_rows) plus the zero padding of the last tile; first_row must be tile-aligned
   const uint64_t n_padded = (n_rows + tile - 1) / tile * tile;
   if (n_padded == 0 || first_row >= n_padded) return STB_OK;
   const unsigned blocks = (unsigned)((n_padded - first_row + 7) / 8);
   if (tile == STB_B_TILE)
-    stb_shadow_build_kernel<STB_B_TILE><<<blocks, 256, 0, ctx->stream>>>(reinterpret_cast<const float4 *>(rows_dev), first_row, n_rows, n_padded, out, bad_flag_dev);
+    stb_shadow_build_kernel<STB_B_TILE><<<blocks, 256, 0, ctx->stream>>>(reinterpret_cast<const float4 *>(rows_dev), first_row, n_rows, n_padded, out, bad_flag_dev, row_bad_dev);
   else
-    stb_shadow_build_kernel<STB_A_TILE><<<blocks, 256, 0, ctx->stream>>>(reinterpret_cast<const float4 *>(rows_dev), first_row, n_rows, n_padded, out, bad_flag_dev);
+    stb_shadow_build_kernel<STB_A_TILE><<<blocks, 256, 0, ctx->stream>>>(reinterpret_cast<const float4 *>(rows_dev), first_row, n_rows, n_padded, out, bad_flag_dev, row_bad_dev);
   STB_CUDA(cudaGetLastError());
   ctx->kernel_launches++;
   return STB_OK;
@@ -534,6 +539,7 @@ struct FinishArgs {
   const float4 *rows;       // corpus f32 rows (local)
   uint64_t n_rows, row_base;
   const float *queries;     // [nq][256] f32 (device)
+  const uint32_t *q_bad;    // [nq] 1: the query could not be normalised (never proven)
   stb_hit *out_hits;        // [nq][top_k]
   uint32_t *out_status;     // [nq][2]: hits, complete
 };
@@ -621,6 +627,7 @@ stb_batch_finish_kernel(const FinishArgs a) {
       const float m_star = stb_key_score(skeys[STB_BATCH_KSEL - 1]);
       complete = (n_out == k) && ((1.0 - (double)m_star - STB_BATCH_EPS) > sd[k - 1]);
     }
+    if (a.q_bad[q]) complete = false;       // unnormalisable query: its scores bound nothing
     a.out_status[2 * q] = n_out;
     a.out_status[2 * q + 1] = complete ? 1u : 0u;
   }
@@ -639,13 +646,13 @@ int stb_launch_batch_select(stb_ctx *ctx, const float *submax, uint32_t n_sub, u
 
 int stb_launch_batch_finish(stb_ctx *ctx, const uint64_t *cand, uint32_t n_slices, uint32_t n_sub,
                             uint32_t nq, uint32_t top_k, const float *rows, uint64_t n_rows,
-                            uint64_t row_base, const float *queries_dev, stb_hit *out_hits,
+                            uint64_t row_base, const float *queries_dev, const uint32_t *q_bad, stb_hit *out_hits,
                             uint32_t *out_status, const float *submax, uint32_t q_pad) {
   FinishArgs a;
   a.cand = cand; a.n_slices = n_slices; a.n_sub = n_sub; a.nq = nq; a.top_k = top_k;
   a.submax = submax; a.q_pad = q_pad;
   a.rows = reinterpret_cast<const float4 *>(rows); a.n_rows = n_rows; a.row_base = row_base;
-  a.queries = queries_dev; a.out_hits = out_hits; a.out_status = out_status;
+  a.queries = queries_dev; a.q_bad = q_bad; a.out_hits = out_hits; a.out_status = out_status;
   stb_batch_finish_kernel<<<nq, 256, 0, ctx->stream>>>(a);
   STB_CUDA(cudaGetLastError());
   ctx->kernel_launches++;
@@ -770,6 +777,7 @@ struct Finish2Args {
   const float4 *rows;
   uint64_t n_rows, row_base;
   const float *queries;        // [nq][256]
+  const uint32_t *q_bad;       // [nq] 1: the query could not be normalised (never proven)
   stb_hit *out_hits;           // [nq][top_k]
   uint32_t *out_status;        // [nq][2]: hits, complete
 };
@@ -891,7 +899,7 @@ stb_batch_finish2_kernel(const Finish2Args a) {
   stb_cta_sort_hits(sd, sr, n2);
   const uint32_t n_out = min((uint32_t)s_pass, k);
   stb_write_hits(a.out_hits + (size_t)q * k, sd, sr, n_out, k);
-  if (tid == 0) { a.out_status[2 * q] = n_out; a.out_status[2 * q + 1] = 1u; }
+  if (tid == 0) { a.out_status[2 * q] = n_out; a.out_status[2 * q + 1] = a.q_bad[q] ? 0u : 1u; }
 }
 
 int stb_launch_batch_thresh(stb_ctx *ctx, const float *tilemax, uint32_t n_sample, uint32_t nq, uint32_t q_pad,
@@ -912,12 +920,13 @@ uint32_t stb_batch_emit_grid(const stb_ctx *ctx, uint32_t n_tiles) {
 
 int stb_launch_batch_finish2(stb_ctx *ctx, const uint64_t *cand_keys, const uint32_t *cand_cnt, uint32_t n_seg,
                              uint32_t seg_cap, uint32_t nq, uint32_t top_k, const float *rows, uint64_t n_rows,
-                             uint64_t row_base, const float *queries_dev, stb_hit *out_hits, uint32_t *out_status) {
+                             uint64_t row_base, const float *queries_dev, const uint32_t *q_bad, stb_hit *out_hits,
+                             uint32_t *out_status) {
   if (top_k > STB_F2_RESCORE || n_seg > 256 || n_seg == 0) { stb_set_error("batch_finish2: bad shape"); return STB_ERR_ARG; }
   Finish2Args a;
   a.cand_keys = cand_keys; a.cand_cnt = cand_cnt; a.n_seg = n_seg; a.seg_cap = seg_cap; a.nq = nq; a.top_k = top_k;
   a.rows = reinterpret_cast<const float4 *>(rows); a.n_rows = n_rows; a.row_base = row_base;
-  a.queries = queries_dev; a.out_hits = out_hits; a.out_status = out_status;
+  a.queries = queries_dev; a.q_bad = q_bad; a.out_hits = out_hits; a.out_status = out_status;
   constexpr size_t smem = STB_F2_KEYS * sizeof(uint64_t) + 32 * STB_F2_STRIDE * sizeof(float);
   STB_ATTR_ONCE(ctx, STB_ATTR_FINISH2, cudaFuncSetAttribute(stb_batch_finish2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   stb_batch_finish2_kernel<<<nq, 256, smem, ctx->stream>>>(a);

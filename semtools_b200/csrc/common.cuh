@@ -116,6 +116,9 @@ struct stb_ctx {
   float *b_thr; size_t b_thr_cap;             // v2: [q_pad] emission thresholds
   uint32_t *b_cnt; size_t b_cnt_cap;          // v2: [q_pad] emitted-candidate counters
   uint64_t *b_keys; size_t b_keys_cap;        // v2: [q_pad][cand_cap] emitted keys
+  uint32_t *b_qbad; size_t b_qbad_cap;        // [q_pad] 1: query could not be normalised
+  // the last stb_search_batch_dev: route (1 = v1, 2 = v2), nq, n_sample, stride, n_seg, seg_cap
+  uint32_t b_last[6];
   float *bq_dev; size_t bq_dev_cap;           // host-call staging: queries
   stb_hit *bh_dev; size_t bh_dev_cap;         // host-call staging: hits
   uint32_t *bs_dev; size_t bs_dev_cap;        // host-call staging: status
@@ -277,7 +280,8 @@ int stb_launch_embed(stb_ctx *ctx, const stb_table *t, const uint64_t *offsets_d
 
 // ---- batch_scan.cu (K2) ------------------------------------------------------------------
 int stb_launch_shadow_build(stb_ctx *ctx, const float *rows_dev, uint64_t n_rows, int tile,
-                            uint8_t *out, int *bad_flag_dev, uint64_t first_row = 0);
+                            uint8_t *out, int *bad_flag_dev, uint64_t first_row = 0,
+                            uint32_t *row_bad_dev = nullptr);
 int stb_launch_batch_gemm(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_tiles,
                           const uint8_t *b_tiles, uint32_t n_tiles, float *submax,
                           float *tilemax, float *full_out);
@@ -296,14 +300,14 @@ uint32_t stb_batch_emit_grid(const stb_ctx *ctx, uint32_t n_tiles);
 int stb_launch_batch_finish2(stb_ctx *ctx, const uint64_t *cand_keys, const uint32_t *cand_cnt, uint32_t n_seg,
                              uint32_t seg_cap, uint32_t nq, uint32_t top_k, const float *rows,
                              uint64_t n_rows, uint64_t row_base, const float *queries_dev,
-                             stb_hit *out_hits, uint32_t *out_status);
+                             const uint32_t *q_bad, stb_hit *out_hits, uint32_t *out_status);
 void stb_batch_build_params(int *shadow_is_f16, double *eps);
 int stb_launch_batch_select(stb_ctx *ctx, const float *submax, uint32_t n_sub, uint32_t q_pad,
                             uint32_t n_slices, uint64_t *cand);
 int stb_launch_batch_finish(stb_ctx *ctx, const uint64_t *cand, uint32_t n_slices, uint32_t n_sub,
                             uint32_t nq, uint32_t top_k, const float *rows, uint64_t n_rows,
-                            uint64_t row_base, const float *queries_dev, stb_hit *out_hits,
-                            uint32_t *out_status, const float *submax, uint32_t q_pad);
+                            uint64_t row_base, const float *queries_dev, const uint32_t *q_bad,
+                            stb_hit *out_hits, uint32_t *out_status, const float *submax, uint32_t q_pad);
 
 // ---- device helpers ---------------------------------------------------------------
 // The distance limit of a search without max_distance: max_distance.unwrap_or(100.0), strict.

@@ -1,33 +1,39 @@
 """CPU model of the K2 pipeline-v2 selection rule (semtools_b200/csrc/batch_scan.cu, "Pipeline
-v2"): with a = bf16 approximate score and c = exact cosine, |a - c| <= EPS, the rows with
+v2"): with a = 16-bit (fp16 by default, or bf16) approximate score and c = exact cosine, |a - c| <= EPS, the rows with
 a >= S_k - 2 EPS (S_k = k-th largest sampled COMPLETE-tile maximum) contain the oracle's top-k,
 and so do the rows with a >= A_k - 2 EPS (A_k = k-th largest approximate score).  This checks
 the arithmetic claim on data with ties, duplicates, exact hits (c >= 1 clamps), zero rows and a
-ragged last tile; the kernels themselves are checked on the GPU (tests/test_gpu_batch.py)."""
+ragged last tile; the kernels themselves are checked on the GPU (tests/test_gpu_batch.py and
+tests/test_gpu_batch_contract.py)."""
 import numpy as np
 import pytest
 
 import oracle
 from conftest import unit_rows
 
-EPS = 0.0080          # STB_BATCH_EPS of the default (bf16) build; the fp16 option is modelled below
 TILE = 256
 
 
-def bf16(x):
+def to16(x, dtype="bfloat16"):
     torch = pytest.importorskip("torch")
-    return torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32)).to(torch.bfloat16).to(torch.float32).numpy()
+    return torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32)).to(getattr(torch, dtype)).to(torch.float32).numpy()
 
 
-def approx_scores(rows, queries):
+def bf16(x):
+    return to16(x, "bfloat16")
+
+
+def approx_scores(rows, queries, dtype="bfloat16"):
     norm = np.linalg.norm(rows.astype(np.float64), axis=1, keepdims=True)
-    rn = bf16(np.divide(rows, norm, out=np.zeros_like(rows), where=norm > 0).astype(np.float32))
-    qn = bf16((queries / np.linalg.norm(queries.astype(np.float64), axis=1, keepdims=True)).astype(np.float32))
+    rn = to16(np.divide(rows, norm, out=np.zeros_like(rows), where=norm > 0).astype(np.float32), dtype)
+    qn = to16((queries / np.linalg.norm(queries.astype(np.float64), axis=1, keepdims=True)).astype(np.float32), dtype)
     return qn @ rn.T                                            # f32 accumulation, like the wgmma accumulators
 
 
+# STB_BATCH_EPS of the two shadow types: fp16 (the default build) and bf16 (-DSTB_SHADOW_F16=0)
+@pytest.mark.parametrize("dtype,EPS", [("bfloat16", 0.0080), ("float16", 0.0012)])
 @pytest.mark.parametrize("n,k,n_sample", [(20_000, 10, 37), (20_000, 1, 78), (20_001, 64, 78), (5_000, 3, 5), (300, 5, 1)])
-def test_threshold_rule_keeps_the_exact_topk(n, k, n_sample):
+def test_threshold_rule_keeps_the_exact_topk(n, k, n_sample, dtype, EPS):
     rng = np.random.default_rng(n + k)
     rows = (unit_rows(rng, n) * rng.uniform(0.25, 4.0, (n, 1))).astype(np.float32)
     queries = unit_rows(rng, 12)
@@ -36,7 +42,7 @@ def test_threshold_rule_keeps_the_exact_topk(n, k, n_sample):
     queries[0] = rows[7] / np.linalg.norm(rows[7])                               # exact hit: c ~ 1
     dense = rng.choice(n, 200, replace=False)
     rows[dense] = (queries[1] + 0.01 * unit_rows(rng, 200)).astype(np.float32)   # 200 near-ties at the top
-    a = approx_scores(rows, queries)
+    a = approx_scores(rows, queries, dtype)
     n_full = n // TILE
     stride = max(n_full // n_sample, 1)
     for qi, q in enumerate(queries):

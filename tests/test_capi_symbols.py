@@ -34,7 +34,7 @@ def test_host_only_entry_points():
     import oracle
     for p, n in [("/test/doc1.txt", 0), ("a/ü.md", 7), ("x", -1)]:
         assert capi.line_id(p, n) == oracle.line_id(p, n)
-    f16, eps = capi.batch_params()                      # default build: bf16 shadow, EPS 0.0080
+    f16, eps = capi.batch_params()                      # default build: fp16 shadow, EPS 0.0012
     assert (f16, eps) in ((False, 0.0080), (True, 0.0012))
 
 
