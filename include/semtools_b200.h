@@ -305,6 +305,31 @@ int stb_ivfpq_search(stb_ivfpq *index, const float *q, uint32_t nprobe, uint32_t
  * scanned.  top_k must be 1..1024; rerank is capped at 1024. */
 int stb_ivfpq_search_dev(stb_ivfpq *index, const float *q_dev, uint32_t nprobe, uint32_t top_k,
                          uint32_t rerank, stb_hit *out_hits_dev, uint32_t *out_status_dev);
+/* Batched search: nq queries (q / q_dev: nq x 256 f32) in one pass over the GPU.
+ * out_hits: nq x top_k, entry i*top_k.. belongs to query i, unused tail (+inf, UINT64_MAX).
+ * Host form: out_n[i] = hits of query i, out_scanned[i] (may be NULL) = codes scanned for it; any nq,
+ * in chunks of 4096 queries with one synchronisation each; top_k == 0 sets every count to 0.
+ * Device form: asynchronous on the context's stream, never synchronises; out_status_dev[2i] = hits,
+ * [2i+1] = codes scanned; nq <= 4096 (more is STB_ERR_ARG).  Both: nq == 0 is a no-op; top_k must be
+ * 1..1024 (else STB_ERR_ARG); nprobe is clamped to [1, min(nlist, 1024)], rerank to [top_k, 1024].
+ * Scratch grows on demand (cudaFree/cudaMalloc, which synchronise, on the first call at a larger nq),
+ * belongs to the index and is separate from the single-query search's.
+ * Each query's answer is independent of the others in the batch and of the chunking:
+ *  - coarse scores, probe list (nprobe best by coarse score desc, list id asc) and LUT are bit-identical
+ *    to stb_ivfpq_search_dev's for that query, bad queries (zero, NaN / inf components, huge or tiny
+ *    scales) included;
+ *  - ADC score = coarse[list] + LUT[0][c0] + ... + LUT[31][c31], summed in that order in fp32;
+ *  - candidates: exactly the `rerank` best scanned codes by (ADC score desc, code position asc); a code
+ *    whose score is NaN or -inf is none.  Each of the 64 scan warps of a query keeps its 64 best codes;
+ *    when one of them dropped a code that would have been a candidate, the query is answered by an exact
+ *    slower route (a radix select over all its codes), never approximately;
+ *  - hits: the candidates' rows and the forced rows re-ranked with the canonical distance, as above.
+ * So with nprobe = nlist and rerank >= the codes scanned the hits equal stb_search's, and whenever v2's
+ * funnel returns the `rerank` best ADC scores the hits equal stb_ivfpq_search_dev's. */
+int stb_ivfpq_search_batch(stb_ivfpq *index, const float *q, uint32_t nq, uint32_t nprobe, uint32_t top_k,
+                           uint32_t rerank, stb_hit *out_hits, uint32_t *out_n, uint64_t *out_scanned);
+int stb_ivfpq_search_batch_dev(stb_ivfpq *index, const float *q_dev, uint32_t nq, uint32_t nprobe,
+                               uint32_t top_k, uint32_t rerank, stb_hit *out_hits_dev, uint32_t *out_status_dev);
 
 /* Host-buffer form of the fused multi-GPU search (the call a sharded host makes per query):
  * pinned H2D of the query, ONE kernel (scan + NVLink exchange + merge), D2H of the merged
@@ -380,6 +405,13 @@ int stb_debug_batch_gemm(stb_ctx *ctx, const float *q, uint32_t nq, const float 
  * lists, ascending), where m = list_off[nlist]. */
 int stb_debug_ivfpq_export(const stb_ivfpq *index, float *centroids, float *codebooks,
                            uint32_t *list_off, uint32_t *order, uint8_t *codes, uint32_t *forced);
+/* Test hook for K5: describes the most recent batched search on the index (either form; the last
+ * chunk of a chunked host call), synchronising the stream.  info = {nq, nprobe, top_k, rerank} after
+ * clamping; for query i, coarse receives [nlist] scores, probe [nprobe] list ids in probe order and
+ * lut [32][256].  Any pointer may be NULL.  STB_ERR_STATE before any batched search, STB_ERR_ARG for
+ * i >= nq. */
+int stb_debug_ivfpq_batch_last(const stb_ivfpq *index, uint32_t i, uint32_t info[4], float *coarse,
+                               uint32_t *probe, float *lut);
 /* Test hook for K2: describes the most recent stb_search_batch_dev on ctx (synchronises the stream).
  * info = {route (1 = v1, 2 = v2, 0 = none yet), nq, n_sample, stride, n_seg, seg_cap}; the last four are
  * v2's sampled tiles (0, stride, 2*stride, ...), emitting grid and per-(query, CTA) key capacity, and 0

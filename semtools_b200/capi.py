@@ -30,6 +30,7 @@ SYMBOLS = [
     "stb_ctx_counters", "stb_debug_ticket_check", "stb_debug_timestamps", "stb_debug_q4_refined", "stb_debug_batch_gemm", "stb_debug_batch_params",
     "stb_debug_batch_last",
     "stb_debug_ivfpq_export",
+    "stb_ivfpq_search_batch", "stb_ivfpq_search_batch_dev", "stb_debug_ivfpq_batch_last",
 ]
 
 
@@ -120,6 +121,9 @@ def lib() -> C.CDLL:
     L.stb_debug_batch_params.argtypes = [C.POINTER(C.c_int), C.POINTER(C.c_double)]
     L.stb_debug_batch_last.argtypes = [vp, vp, vp, vp]
     L.stb_debug_ivfpq_export.argtypes = [vp, vp, vp, vp, vp, vp, vp]
+    L.stb_ivfpq_search_batch.argtypes = [vp, vp, u32, u32, u32, u32, vp, vp, vp]
+    L.stb_ivfpq_search_batch_dev.argtypes = [vp, vp, u32, u32, u32, u32, vp, vp]
+    L.stb_debug_ivfpq_batch_last.argtypes = [vp, u32, vp, vp, vp, vp]
     for name in SYMBOLS:
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("stb_version", "stb_device_count"):
@@ -438,6 +442,36 @@ class IvfPq:
     def search_dev(self, q_dev: int, nprobe: int, top_k: int, rerank: int, out_hits_dev: int, out_status_dev: int):
         """stb_ivfpq_search_dev: asynchronous, everything stays in HBM."""
         _check(lib().stb_ivfpq_search_dev(self._h, vp(q_dev), nprobe, top_k, rerank, vp(out_hits_dev), vp(out_status_dev)))
+
+    def search_batch(self, queries, nprobe: int = 64, top_k: int = 10, rerank: int = 256):
+        """stb_ivfpq_search_batch: (hits [nq, top_k] of HIT_DTYPE, padded with (+inf, UINT64_MAX);
+        n [nq] hit counts; scanned [nq] codes scanned)."""
+        queries = np.ascontiguousarray(queries, dtype=np.float32).reshape(-1, STB_DIM)
+        nq = queries.shape[0]
+        out = np.zeros((nq, top_k), dtype=HIT_DTYPE)
+        n = np.zeros(nq, dtype=np.uint32)
+        scanned = np.zeros(nq, dtype=np.uint64)
+        _check(lib().stb_ivfpq_search_batch(self._h, _np_ptr(queries), nq, nprobe, top_k, rerank,
+                                            _np_ptr(out) if out.size else None, _np_ptr(n), _np_ptr(scanned)))
+        return out, n, scanned
+
+    def search_batch_dev(self, q_dev: int, nq: int, nprobe: int, top_k: int, rerank: int, out_hits_dev: int,
+                         out_status_dev: int):
+        """stb_ivfpq_search_batch_dev: asynchronous; hits [nq][top_k], status [nq][2] = (hits, codes scanned)."""
+        _check(lib().stb_ivfpq_search_batch_dev(self._h, vp(q_dev), nq, nprobe, top_k, rerank, vp(out_hits_dev),
+                                                vp(out_status_dev)))
+
+    def batch_last(self, i: int):
+        """stb_debug_ivfpq_batch_last: the last batched search's clamped {nq, nprobe, top_k, rerank} and
+        query i's coarse scores [nlist], probe list [nprobe] and LUT [32][256]."""
+        info = np.zeros(4, dtype=np.uint32)
+        _check(lib().stb_debug_ivfpq_batch_last(self._h, i, _np_ptr(info), None, None, None))
+        coarse = np.zeros(self.stats()["nlist"], dtype=np.float32)
+        probe = np.zeros(max(int(info[1]), 1), dtype=np.uint32)
+        lut = np.zeros((32, 256), dtype=np.float32)
+        _check(lib().stb_debug_ivfpq_batch_last(self._h, i, None, _np_ptr(coarse), _np_ptr(probe), _np_ptr(lut)))
+        return {"nq": int(info[0]), "nprobe": int(info[1]), "top_k": int(info[2]), "rerank": int(info[3]),
+                "coarse": coarse, "probe": probe[: int(info[1])], "lut": lut}
 
 
 class Exchange:

@@ -35,6 +35,18 @@
 #define IVF_HOST_TOPK_MAX 4096     // stb_ivfpq_search: top_k and rerank cap of the multi-launch search
 #define IVF_NO_LIST 0xffffffffu    // assign[] of a forced row
 
+// batched search (see "batched search" below)
+#define IVFB_MAX_NQ 4096           // queries per stb_ivfpq_search_batch_dev call (the host form chunks)
+#define IVFB_QTILE 16              // queries per CTA of the coarse kernel
+#define IVFB_SCAN_CTAS 8           // scan CTAs per query
+#define IVFB_SCAN_THREADS 256
+#define IVFB_WARPS (IVFB_SCAN_CTAS * IVFB_SCAN_THREADS / 32)   // 64 scan warps per query
+#define IVFB_WARP_KEEP 64          // best keys a scan warp keeps (2 per lane)
+#define IVFB_KEPT (IVFB_WARPS * IVFB_WARP_KEEP)                // 4096 kept keys per query
+#define IVFB_FIN_THREADS 512
+#define IVFB_FIN_SMEM 65536
+#define IVFB_RERANK_CAP 1024
+
 struct stb_ivfpq {
   stb_ctx *ctx;
   const stb_corpus *corpus;
@@ -58,6 +70,18 @@ struct stb_ivfpq {
   // fused search (v2)
   uint64_t *keys2;            // [ADC2_MAX_CTAS][ADC2_KEEP] per-CTA best candidates (score desc, code position)
   unsigned int *tickets;      // [2] last-CTA tickets of the two fused kernels (kernels re-zero them)
+  // batched search scratch (its own buffers: a batch and a single query enqueued back to back do not
+  // share any), sized for b_cap queries, grown on demand
+  uint32_t b_cap;
+  float *b_q;                 // [b_cap][256] queries of the host form
+  float *b_coarse;            // [b_cap][nlist]
+  uint32_t *b_probe;          // [b_cap][2 * 1024 + 1]: nprobe list ids, then the prefix of their lengths
+  float *b_lut;               // [b_cap][32][256]
+  uint64_t *b_kept;           // [b_cap][IVFB_KEPT] each warp's best keys
+  uint64_t *b_drop;           // [b_cap][IVFB_WARPS] the best key each warp dropped
+  stb_hit *b_hits;            // [b_cap][1024] hits of the host form
+  uint32_t *b_status;         // [b_cap][2]
+  uint32_t last_info[4];      // {nq, nprobe, top_k, rerank} of the last batch launch (nq = 0: none yet)
 };
 
 // ------------------------------------------------------------------ assignment GEMM ---
@@ -305,6 +329,55 @@ __global__ void ivf_scatter_kernel(const uint32_t *assign, uint64_t n, uint32_t 
   dst[0] = src[0]; dst[1] = src[1];
 }
 
+// ------------------------------------------------------------------ query arithmetic --
+// Every query kernel, single and batched, computes the coarse scores, the LUT and the ADC scores
+// with these helpers, so a query's values are the same bits whichever path computes them.
+
+// c . q and q . q of a centroid and a query held as 8 floats per lane of a full warp (lane L holds
+// dims 8L..8L+7), each reduced over the warp by an xor butterfly; every lane ends with both sums.
+__device__ __forceinline__ void ivf_coarse_dot(float4 a0, float4 a1, float4 b0, float4 b1, float &d, float &qq) {
+  d = a0.x * b0.x + a0.y * b0.y + a0.z * b0.z + a0.w * b0.w + a1.x * b1.x + a1.y * b1.y + a1.z * b1.z + a1.w * b1.w;
+  qq = b0.x * b0.x + b0.y * b0.y + b0.z * b0.z + b0.w * b0.w + b1.x * b1.x + b1.y * b1.y + b1.z * b1.z + b1.w * b1.w;
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) { d += __shfl_xor_sync(0xffffffffu, d, off); qq += __shfl_xor_sync(0xffffffffu, qq, off); }
+}
+// coarse score q^ . c from ivf_coarse_dot's sums (0 for a query whose q . q is not positive)
+__device__ __forceinline__ float ivf_coarse_score(float d, float qq) { return qq > 0.f ? d * rsqrtf(qq) : 0.f; }
+
+// 1 / ||q|| of the query in shared memory: serial fp32 sum in index order (one thread)
+__device__ __forceinline__ float ivf_query_inv(const float *sq) {
+  float s = 0.f;
+  for (int i = 0; i < STB_D; ++i) s += sq[i] * sq[i];
+  return s > 0.f ? rsqrtf(s) : 0.f;
+}
+
+// LUT entry i = (sub-space s = i / 256, code i % 256): FMA chain of q^_s . cb[s][code]
+__device__ __forceinline__ float ivf_lut_entry(const float *sq, float inv, const float *cb, int i) {
+  const int sub = i / PQ_KSUB;
+  const float *e = cb + (size_t)i * PQ_DSUB;
+  float d = 0.f;
+#pragma unroll
+  for (int t = 0; t < 8; ++t) d = fmaf(sq[sub * 8 + t] * inv, e[t], d);
+  return d;
+}
+
+
+// ADC score of a code (its 32 bytes in c0, c1): s (its list's coarse score) + LUT[0][c0] + ... +
+// LUT[31][c31], in that order.  Only fp32 additions in a fixed order, so the bits are those of any
+// such sum (numpy reproduces them).  ivf_adc_kernel and ivf_adc_finish_kernel spell the same sum out
+// inline: routed through this helper, the compiler assigns their registers differently.
+__device__ __forceinline__ float ivf_adc_sum(const float *s_lut, uint4 c0, uint4 c1, float s) {
+  const uint32_t w[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    s += s_lut[(4 * i + 0) * PQ_KSUB + (w[i] & 0xff)];
+    s += s_lut[(4 * i + 1) * PQ_KSUB + ((w[i] >> 8) & 0xff)];
+    s += s_lut[(4 * i + 2) * PQ_KSUB + ((w[i] >> 16) & 0xff)];
+    s += s_lut[(4 * i + 3) * PQ_KSUB + (w[i] >> 24)];
+  }
+  return s;
+}
+
 // ------------------------------------------------------------------ query kernels -----
 // coarse[j] = q^ . c_j   (warp per centroid)
 __global__ void ivf_coarse_kernel(const float *C, uint32_t nlist, const float *q, float *coarse) {
@@ -313,11 +386,9 @@ __global__ void ivf_coarse_kernel(const float *C, uint32_t nlist, const float *q
   if (c >= nlist) return;
   const float4 *cr = reinterpret_cast<const float4 *>(C + (size_t)c * STB_D), *q4 = reinterpret_cast<const float4 *>(q);
   const float4 a0 = __ldg(cr + 2 * lane), a1 = __ldg(cr + 2 * lane + 1), b0 = __ldg(q4 + 2 * lane), b1 = __ldg(q4 + 2 * lane + 1);
-  float d = a0.x * b0.x + a0.y * b0.y + a0.z * b0.z + a0.w * b0.w + a1.x * b1.x + a1.y * b1.y + a1.z * b1.z + a1.w * b1.w;
-  float qq = b0.x * b0.x + b0.y * b0.y + b0.z * b0.z + b0.w * b0.w + b1.x * b1.x + b1.y * b1.y + b1.z * b1.z + b1.w * b1.w;
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) { d += __shfl_xor_sync(0xffffffffu, d, off); qq += __shfl_xor_sync(0xffffffffu, qq, off); }
-  if (lane == 0) coarse[c] = qq > 0.f ? d * rsqrtf(qq) : 0.f;
+  float d, qq;
+  ivf_coarse_dot(a0, a1, b0, b1, d, qq);
+  if (lane == 0) coarse[c] = ivf_coarse_score(d, qq);
 }
 
 // one CTA: top-nprobe lists (bitonic sort of <= 8192 keys), prefix of their lengths, LUT
@@ -332,7 +403,7 @@ ivf_probe_lut_kernel(const float *coarse, uint32_t nlist, uint32_t nprobe, const
     skeys[i] = (i < nlist) ? stb_make_key(coarse[i], i) : STB_KEY_INVALID;
   if (threadIdx.x < STB_D) sq[threadIdx.x] = q[threadIdx.x];
   __syncthreads();
-  if (threadIdx.x == 0) { float s = 0.f; for (int i = 0; i < STB_D; ++i) s += sq[i] * sq[i]; s_inv = s > 0.f ? rsqrtf(s) : 0.f; }
+  if (threadIdx.x == 0) s_inv = ivf_query_inv(sq);
   stb_cta_sort_keys_strided(skeys, npow);
   // probe[0..nprobe) = list ids (best first); probe[nprobe_max .. ] = prefix of list lengths
   if (threadIdx.x == 0) {
@@ -346,14 +417,7 @@ ivf_probe_lut_kernel(const float *coarse, uint32_t nlist, uint32_t nprobe, const
     probe[2 * nprobe] = acc;
   }
   const float inv = s_inv;
-  for (int i = threadIdx.x; i < PQ_M * PQ_KSUB; i += blockDim.x) {
-    const int s = i / PQ_KSUB;
-    const float *e = cb + (size_t)i * PQ_DSUB;
-    float d = 0.f;
-#pragma unroll
-    for (int t = 0; t < 8; ++t) d = fmaf(sq[s * 8 + t] * inv, e[t], d);
-    lut[i] = d;
-  }
+  for (int i = threadIdx.x; i < PQ_M * PQ_KSUB; i += blockDim.x) lut[i] = ivf_lut_entry(sq, inv, cb, i);
 }
 
 // ADC scan over the probed lists: lane = one code (32 bytes); score = coarse[list] + sum LUT.
@@ -477,11 +541,9 @@ ivf_coarse_probe_kernel(const Probe2Args a) {
   if (c < a.nlist) {
     const float4 *cr = reinterpret_cast<const float4 *>(a.C + (size_t)c * STB_D), *q4 = reinterpret_cast<const float4 *>(a.q);
     const float4 a0 = __ldg(cr + 2 * lane), a1 = __ldg(cr + 2 * lane + 1), b0 = __ldg(q4 + 2 * lane), b1 = __ldg(q4 + 2 * lane + 1);
-    float d = a0.x * b0.x + a0.y * b0.y + a0.z * b0.z + a0.w * b0.w + a1.x * b1.x + a1.y * b1.y + a1.z * b1.z + a1.w * b1.w;
-    float qq = b0.x * b0.x + b0.y * b0.y + b0.z * b0.z + b0.w * b0.w + b1.x * b1.x + b1.y * b1.y + b1.z * b1.z + b1.w * b1.w;
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) { d += __shfl_xor_sync(0xffffffffu, d, off); qq += __shfl_xor_sync(0xffffffffu, qq, off); }
-    if (lane == 0) { a.coarse[c] = qq > 0.f ? d * rsqrtf(qq) : 0.f; __threadfence(); }
+    float d, qq;
+    ivf_coarse_dot(a0, a1, b0, b1, d, qq);
+    if (lane == 0) { a.coarse[c] = ivf_coarse_score(d, qq); __threadfence(); }
   }
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -497,7 +559,7 @@ ivf_coarse_probe_kernel(const Probe2Args a) {
     p2_keys[i] = (i < a.nlist) ? stb_make_key(__ldcg(a.coarse + i), i) : STB_KEY_INVALID;
   if (threadIdx.x < STB_D) sq[threadIdx.x] = a.q[threadIdx.x];
   __syncthreads();
-  if (threadIdx.x == 0) { float s = 0.f; for (int i = 0; i < STB_D; ++i) s += sq[i] * sq[i]; s_inv = s > 0.f ? rsqrtf(s) : 0.f; }
+  if (threadIdx.x == 0) s_inv = ivf_query_inv(sq);
   stb_cta_sort_keys_strided(p2_keys, npow);
   // list sizes in parallel (one thread per probed list), then a serial prefix over shared memory:
   // a single thread chasing 2 x nprobe dependent global loads cost ~20 us of this kernel's 62
@@ -515,14 +577,7 @@ ivf_coarse_probe_kernel(const Probe2Args a) {
     *a.ticket = 0;                                   // ready for the next query (stream-ordered)
   }
   const float inv = s_inv;
-  for (int i = threadIdx.x; i < PQ_M * PQ_KSUB; i += blockDim.x) {
-    const int sub = i / PQ_KSUB;
-    const float *e = a.cb + (size_t)i * PQ_DSUB;
-    float d = 0.f;
-#pragma unroll
-    for (int t = 0; t < 8; ++t) d = fmaf(sq[sub * 8 + t] * inv, e[t], d);
-    a.lut[i] = d;
-  }
+  for (int i = threadIdx.x; i < PQ_M * PQ_KSUB; i += blockDim.x) a.lut[i] = ivf_lut_entry(sq, inv, a.cb, i);
 }
 
 struct Adc2Args {
@@ -638,6 +693,288 @@ ivf_adc_finish_kernel(const Adc2Args a) {
   if (tid == 0) { a.out_status[0] = n_out; a.out_status[1] = total; *a.ticket = 0; }
 }
 
+// ------------------------------------------------------------------ batched search ------
+// nq queries in four launches, each query computed as the single path computes it and selected exactly:
+//   ivfb_coarse_kernel     coarse scores [nq][nlist]: a warp per centroid reduces it against a tile of
+//                          IVFB_QTILE queries staged in shared memory (ivf_coarse_dot, the single
+//                          path's lane split and butterfly, so the same bits).
+//   ivfb_probe_lut_kernel  a CTA per query: sort of the coarse keys, probe list + prefix of the list
+//                          lengths, LUT [32][256] (ivf_query_inv, ivf_lut_entry).
+//   ivfb_scan_kernel       grid (IVFB_SCAN_CTAS, nq): 32-code chunk g of a query's probed codes goes
+//                          to CTA g % 8, warp (g / 8) % 8 (a cluster's codes spread over all 64
+//                          warps); each warp keeps its IVFB_WARP_KEEP best keys (stb_make_key: ADC
+//                          score desc, code position asc) exactly and records the best key it dropped.
+//                          Every query reads its own codes: nq x (codes scanned x 32 B).
+//   ivfb_finish_kernel     a CTA per query: T = the rerank-th best of the 4096 kept keys.  When no warp
+//                          dropped a key better than T, the kept keys hold the `rerank` best codes;
+//                          otherwise the query takes the exact slow route: an MSB-first radix select of
+//                          the rerank-th best key over all its codes (8 passes of 8 bits, scores
+//                          recomputed), then one pass that emits every key at or above it.  The
+//                          candidates' rows and the forced rows are re-ranked with the canonical
+//                          distance as on every K5 path.
+// A code whose ADC score is NaN or -inf (a query with a non-finite component) is no candidate, as on
+// the single path.
+
+__global__ void __launch_bounds__(1024)
+ivfb_coarse_kernel(const float *C, uint32_t nlist, const float *qs, uint32_t nq, float *coarse) {
+  __shared__ float4 sq[IVFB_QTILE][STB_ROW_F4];
+  const int lane = threadIdx.x & 31;
+  const uint32_t q0 = blockIdx.y * IVFB_QTILE, nt = min((uint32_t)IVFB_QTILE, nq - q0);
+  const float4 *q4 = reinterpret_cast<const float4 *>(qs) + (size_t)q0 * STB_ROW_F4;
+  for (uint32_t i = threadIdx.x; i < nt * STB_ROW_F4; i += blockDim.x) sq[i / STB_ROW_F4][i % STB_ROW_F4] = __ldg(q4 + i);
+  __syncthreads();
+  const uint32_t c = blockIdx.x * 32 + (threadIdx.x >> 5);
+  if (c >= nlist) return;
+  const float4 *cr = reinterpret_cast<const float4 *>(C + (size_t)c * STB_D);
+  const float4 a0 = __ldg(cr + 2 * lane), a1 = __ldg(cr + 2 * lane + 1);
+  for (uint32_t j = 0; j < nt; ++j) {
+    float d, qq;
+    ivf_coarse_dot(a0, a1, sq[j][2 * lane], sq[j][2 * lane + 1], d, qq);
+    if (lane == 0) coarse[(size_t)(q0 + j) * nlist + c] = ivf_coarse_score(d, qq);
+  }
+}
+
+__global__ void __launch_bounds__(1024)
+ivfb_probe_lut_kernel(const float *coarse, uint32_t nlist, uint32_t nprobe, const uint32_t *list_off, const float *cb,
+                      const float *qs, uint32_t *probe, float *lut) {
+  extern __shared__ uint64_t pb_keys[];   // npow2 keys
+  __shared__ float sq[STB_D];
+  __shared__ float s_inv;
+  __shared__ uint32_t s_sz[1024];
+  const uint32_t q = blockIdx.x;
+  const float *cq = coarse + (size_t)q * nlist;
+  uint32_t *pr = probe + (size_t)q * (2 * nprobe + 1);
+  uint32_t npow = 1; while (npow < nlist) npow <<= 1;
+  for (uint32_t i = threadIdx.x; i < npow; i += blockDim.x) pb_keys[i] = (i < nlist) ? stb_make_key(cq[i], i) : STB_KEY_INVALID;
+  if (threadIdx.x < STB_D) sq[threadIdx.x] = qs[(size_t)q * STB_D + threadIdx.x];
+  __syncthreads();
+  if (threadIdx.x == 0) s_inv = ivf_query_inv(sq);
+  stb_cta_sort_keys_strided(pb_keys, npow);
+  if (threadIdx.x < nprobe) {
+    const uint32_t l = stb_key_row(pb_keys[threadIdx.x]);
+    pr[threadIdx.x] = l;
+    s_sz[threadIdx.x] = __ldg(list_off + l + 1) - __ldg(list_off + l);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint32_t acc = 0;
+    for (uint32_t p = 0; p < nprobe; ++p) { pr[nprobe + p] = acc; acc += s_sz[p]; }
+    pr[2 * nprobe] = acc;
+  }
+  const float inv = s_inv;
+  float *lq = lut + (size_t)q * PQ_M * PQ_KSUB;
+  for (int i = threadIdx.x; i < PQ_M * PQ_KSUB; i += blockDim.x) lq[i] = ivf_lut_entry(sq, inv, cb, i);
+}
+
+// The IVFB_WARP_KEEP best keys a warp has seen (2 per lane, exact: keys are distinct), and the best
+// (smallest) key it has dropped.  Smaller key = better; STB_KEY_INVALID fills empty slots.
+struct IvfbTop {
+  uint64_t k[2], thr, drop;   // thr: the worst kept key (warp-uniform)
+  int lane;
+  // keep < 64: slots keep..63 hold key 0, which no code has (its score would be a NaN) and which is
+  // never evicted, so the warp keeps `keep` codes
+  __device__ __forceinline__ void init(uint32_t keep) {
+    lane = threadIdx.x & 31;
+    k[0] = (uint32_t)lane < keep ? STB_KEY_INVALID : 0ull;
+    k[1] = (uint32_t)(32 + lane) < keep ? STB_KEY_INVALID : 0ull;
+    thr = drop = STB_KEY_INVALID;
+  }
+  __device__ __forceinline__ void insert(uint64_t ck) {   // warp-uniform ck < thr: replaces the worst kept key
+    const uint64_t m = k[0] > k[1] ? k[0] : k[1];
+    const unsigned owners = __ballot_sync(0xffffffffu, m == thr);
+    if (lane == __ffs(owners) - 1) { if (k[0] == m) k[0] = ck; else k[1] = ck; }
+    drop = min(drop, thr);
+    uint64_t t = k[0] > k[1] ? k[0] : k[1];
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) t = max(t, __shfl_xor_sync(0xffffffffu, t, off));
+    thr = t;
+  }
+  __device__ __forceinline__ void push(uint64_t key) {
+    unsigned mask = __ballot_sync(0xffffffffu, key < thr);
+    if (!(key < thr)) drop = min(drop, key);
+    while (mask) {
+      const int src = __ffs(mask) - 1;
+      mask &= mask - 1;
+      const uint64_t ck = __shfl_sync(0xffffffffu, key, src);
+      if (ck < thr) insert(ck); else drop = min(drop, ck);
+    }
+  }
+};
+
+// key of probed code v of a query (STB_KEY_INVALID past the end and for a NaN or -inf score); pref,
+// start and pc: per probed list the prefix of lengths, list_off of the list and its coarse score
+__device__ __forceinline__ uint64_t ivfb_code_key(uint64_t v, uint32_t total, uint32_t nprobe, const uint32_t *pref,
+                                                  const uint32_t *start, const float *pc, const float *s_lut,
+                                                  const uint8_t *codes) {
+  if (v >= total) return STB_KEY_INVALID;
+  uint32_t lo = 0, hi = nprobe;      // probe p with pref[p] <= v < pref[p+1]
+  while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (pref[mid] <= v) lo = mid; else hi = mid; }
+  const uint32_t pos = start[lo] + (uint32_t)(v - pref[lo]);
+  const uint4 *cp = reinterpret_cast<const uint4 *>(codes + (size_t)pos * PQ_M);
+  const float s = ivf_adc_sum(s_lut, __ldg(cp), __ldg(cp + 1), pc[lo]);
+  return s > -CUDART_INF_F ? stb_make_key(s, pos) : STB_KEY_INVALID;
+}
+
+struct IvfbArgs {
+  const float *C; uint32_t nlist, nq, nprobe, top_k, rerank, keep;
+  const uint32_t *list_off; const float *cb; const uint8_t *codes; const uint32_t *order;
+  const float *qs; float *coarse; uint32_t *probe; float *lut; uint64_t *kept, *drop;
+  const float4 *rows; uint64_t row_base; const uint32_t *forced; uint32_t n_forced;
+  stb_hit *out_hits; uint32_t *out_status;   // [nq][top_k], [nq][2] = {hits, codes scanned}
+};
+
+__global__ void __launch_bounds__(IVFB_SCAN_THREADS)
+ivfb_scan_kernel(const IvfbArgs a) {
+  __shared__ float s_lut[PQ_M * PQ_KSUB];      // 32 KiB
+  __shared__ uint32_t s_pref[1024], s_start[1024];
+  __shared__ float s_pc[1024];
+  const uint32_t q = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t *pr = a.probe + (size_t)q * (2 * a.nprobe + 1);
+  const float *lq = a.lut + (size_t)q * PQ_M * PQ_KSUB;
+  for (uint32_t i = tid; i < PQ_M * PQ_KSUB; i += IVFB_SCAN_THREADS) s_lut[i] = lq[i];
+  for (uint32_t p = tid; p < a.nprobe; p += IVFB_SCAN_THREADS) {
+    const uint32_t l = pr[p];
+    s_pref[p] = pr[a.nprobe + p]; s_start[p] = __ldg(a.list_off + l); s_pc[p] = a.coarse[(size_t)q * a.nlist + l];
+  }
+  __syncthreads();
+  const uint32_t total = pr[2 * a.nprobe];
+  IvfbTop top;
+  top.init(a.keep);
+  // chunk g (32 consecutive codes) -> CTA g % IVFB_SCAN_CTAS, warp (g / IVFB_SCAN_CTAS) % 8
+  for (uint64_t g = blockIdx.x + (uint64_t)IVFB_SCAN_CTAS * warp; g * 32 < total; g += IVFB_WARPS)
+    top.push(ivfb_code_key(g * 32 + lane, total, a.nprobe, s_pref, s_start, s_pc, s_lut, a.codes));
+  uint64_t d = top.drop;
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) d = min(d, __shfl_xor_sync(0xffffffffu, d, off));
+  const uint32_t w = blockIdx.x * (IVFB_SCAN_THREADS / 32) + warp;   // warp of the query, 0..63
+  uint64_t *kq = a.kept + (size_t)q * IVFB_KEPT + w * IVFB_WARP_KEEP;
+  kq[lane] = top.k[0] ? top.k[0] : STB_KEY_INVALID; kq[32 + lane] = top.k[1] ? top.k[1] : STB_KEY_INVALID;
+  if (lane == 0) a.drop[(size_t)q * IVFB_WARPS + w] = d;
+}
+
+__global__ void __launch_bounds__(IVFB_FIN_THREADS)
+ivfb_finish_kernel(const IvfbArgs a) {
+  extern __shared__ __align__(16) uint8_t dyn[];                     // IVFB_FIN_SMEM
+  uint64_t *keys = reinterpret_cast<uint64_t *>(dyn);               // [0, 32 KiB): kept keys, then candidates
+  __shared__ double sqd[STB_D];
+  __shared__ double s_q2;
+  __shared__ int s_pass;
+  __shared__ unsigned s_slow, s_nc, s_need;
+  __shared__ uint32_t s_hist[256];
+  __shared__ unsigned long long s_prefix;
+  const uint32_t q = blockIdx.x, tid = threadIdx.x;
+  const uint32_t *pr = a.probe + (size_t)q * (2 * a.nprobe + 1);
+  const uint32_t total = pr[2 * a.nprobe];
+  const uint32_t r = a.rerank;
+  for (uint32_t i = tid; i < IVFB_KEPT; i += IVFB_FIN_THREADS) keys[i] = a.kept[(size_t)q * IVFB_KEPT + i];
+  for (uint32_t i = tid; i < STB_D; i += IVFB_FIN_THREADS) sqd[i] = (double)a.qs[(size_t)q * STB_D + i];
+  if (tid == 0) { s_pass = 0; s_slow = 0; }
+  __syncthreads();
+  stb_cta_sort_keys_strided(keys, IVFB_KEPT);
+  // every key a warp dropped is >= its recorded drop; the kept keys hold the r best iff each is > T
+  const uint64_t T = keys[r - 1];
+  if (tid < IVFB_WARPS) {
+    const uint64_t d = a.drop[(size_t)q * IVFB_WARPS + tid];
+    if (d != STB_KEY_INVALID && d < T) s_slow = 1;
+  }
+  if (tid == 0) s_q2 = stb_canon_q2(sqd);
+  __syncthreads();
+  uint32_t nc = r;                                                   // candidates: keys[0, nc)
+  if (s_slow) {
+    // exact slow route: radix select of the r-th best key over every probed code
+    float *s_lut = reinterpret_cast<float *>(dyn + 32768);          // [32 KiB, 64 KiB)
+    const float *lq = a.lut + (size_t)q * PQ_M * PQ_KSUB;
+    for (uint32_t i = tid; i < PQ_M * PQ_KSUB; i += IVFB_FIN_THREADS) s_lut[i] = lq[i];
+    uint32_t *s_pref = reinterpret_cast<uint32_t *>(dyn);           // [0, 12 KiB) during the selection
+    uint32_t *s_start = s_pref + 1024;
+    float *s_pc = reinterpret_cast<float *>(s_pref + 2048);
+    for (uint32_t p = tid; p < a.nprobe; p += IVFB_FIN_THREADS) {
+      const uint32_t l = pr[p];
+      s_pref[p] = pr[a.nprobe + p]; s_start[p] = __ldg(a.list_off + l); s_pc[p] = a.coarse[(size_t)q * a.nlist + l];
+    }
+    if (tid == 0) { s_prefix = 0; s_need = r; }
+    for (int pass = 0; pass < 8; ++pass) {
+      const int shift = 56 - 8 * pass;
+      const uint64_t hi_mask = pass == 0 ? 0ull : (~0ull << (shift + 8));
+      for (uint32_t i = tid; i < 256; i += IVFB_FIN_THREADS) s_hist[i] = 0;
+      __syncthreads();
+      const uint64_t prefix = s_prefix;
+      for (uint64_t v = tid; v < total; v += IVFB_FIN_THREADS) {
+        const uint64_t key = ivfb_code_key(v, total, a.nprobe, s_pref, s_start, s_pc, s_lut, a.codes);
+        if (key != STB_KEY_INVALID && (key & hi_mask) == prefix) atomicAdd(&s_hist[(key >> shift) & 255], 1u);
+      }
+      __syncthreads();
+      if (tid == 0) {
+        uint32_t need = s_need;
+        if (pass == 0) {                                             // fewer valid codes than r: take them all
+          uint32_t valid = 0;
+          for (int b = 0; b < 256; ++b) valid += s_hist[b];
+          need = min(need, valid);
+        }
+        if (need > 0) {
+          uint32_t cum = 0, b = 0;
+          while (cum + s_hist[b] < need) cum += s_hist[b++];
+          s_prefix = prefix | ((uint64_t)b << shift);
+          need -= cum;
+        } else {
+          s_prefix = 0;                                              // nothing valid: the emit pass takes nothing
+        }
+        s_need = need;
+      }
+      __syncthreads();
+    }
+    const uint64_t thr = s_prefix;
+    const bool none = s_need == 0;
+    if (tid == 0) s_nc = 0;
+    __syncthreads();
+    uint64_t *cand = reinterpret_cast<uint64_t *>(dyn + 16384);     // [16 KiB, 24 KiB): r <= 1024 keys
+    if (!none)
+      for (uint64_t v = tid; v < total; v += IVFB_FIN_THREADS) {
+        const uint64_t key = ivfb_code_key(v, total, a.nprobe, s_pref, s_start, s_pc, s_lut, a.codes);
+        if (key <= thr) cand[atomicAdd(&s_nc, 1u)] = key;           // exactly min(r, valid) keys
+      }
+    __syncthreads();
+    nc = s_nc;
+    for (uint32_t i = tid; i < nc; i += IVFB_FIN_THREADS) keys[i] = cand[i];
+    __syncthreads();
+  }
+  // re-rank: the candidates' rows and the forced rows, canonical distance, (distance, row) order
+  uint32_t n2 = 32;
+  while (n2 < nc + a.n_forced) n2 <<= 1;
+  double *sd = reinterpret_cast<double *>(dyn + 16384);             // [16 KiB, 32 KiB)
+  uint64_t *sr = reinterpret_cast<uint64_t *>(dyn + 32768);         // [32 KiB, 48 KiB)
+  uint64_t *rows_c = reinterpret_cast<uint64_t *>(dyn + 49152);     // [48 KiB, 64 KiB): local row of entry c
+  for (uint32_t c = tid; c < n2; c += IVFB_FIN_THREADS) {
+    uint64_t row = 0xffffffffffffffffull;
+    if (c < nc) {
+      const uint64_t key = keys[c];
+      if (key != STB_KEY_INVALID) row = a.order[stb_key_row(key)];
+    } else if (c < nc + a.n_forced) {
+      row = a.forced[c - nc];
+    }
+    rows_c[c] = row;
+  }
+  __syncthreads();                                                   // keys are read before sd overwrites them
+  const double q2 = s_q2;
+  for (uint32_t c = tid; c < n2; c += IVFB_FIN_THREADS) {
+    double d = CUDART_INF;
+    uint64_t grow = 0xffffffffffffffffull;
+    const uint64_t row = rows_c[c];
+    if (row != 0xffffffffffffffffull) {
+      double ab, r2;
+      stb_canon_dot<true>(sqd, a.rows + row * STB_ROW_F4, ab, r2);
+      const double dist = stb_canon_dist(ab, q2, r2);
+      if (dist < STB_DEFAULT_MAX_DIST) { d = dist; grow = a.row_base + row; atomicAdd(&s_pass, 1); }
+    }
+    sd[c] = d; sr[c] = grow;
+  }
+  __syncthreads();
+  stb_cta_sort_hits(sd, sr, n2);
+  const uint32_t n_out = min((uint32_t)s_pass, a.top_k);
+  stb_write_hits(a.out_hits + (size_t)q * a.top_k, sd, sr, n_out, a.top_k);
+  if (tid == 0) { a.out_status[2 * q] = n_out; a.out_status[2 * q + 1] = total; }
+}
+
 // ------------------------------------------------------------------ host side ---------
 extern "C" {
 
@@ -646,6 +983,8 @@ int stb_ivfpq_destroy(stb_ivfpq *x) {
   cudaFree(x->centroids); cudaFree(x->codebooks); cudaFree(x->codes); cudaFree(x->order); cudaFree(x->list_off);
   cudaFree(x->coarse); cudaFree(x->lut); cudaFree(x->probe); cudaFree(x->cand); cudaFree(x->cand_rows);
   cudaFree(x->keys2); cudaFree(x->tickets); cudaFree(x->forced);
+  cudaFree(x->b_q); cudaFree(x->b_coarse); cudaFree(x->b_probe); cudaFree(x->b_lut); cudaFree(x->b_kept);
+  cudaFree(x->b_drop); cudaFree(x->b_hits); cudaFree(x->b_status);
   cudaGetLastError();
   delete x;
   return STB_OK;
@@ -676,6 +1015,9 @@ int stb_ivfpq_build(stb_ctx *ctx, const stb_corpus *corpus, uint32_t nlist, uint
   x->centroids = nullptr; x->codebooks = nullptr; x->codes = nullptr; x->order = nullptr; x->list_off = nullptr;
   x->coarse = nullptr; x->lut = nullptr; x->probe = nullptr; x->cand = nullptr; x->cand_cap = 0; x->cand_rows = nullptr;
   x->keys2 = nullptr; x->tickets = nullptr; x->forced = nullptr; x->n_forced = 0;
+  x->b_cap = 0; x->b_q = nullptr; x->b_coarse = nullptr; x->b_probe = nullptr; x->b_lut = nullptr; x->b_kept = nullptr;
+  x->b_drop = nullptr; x->b_hits = nullptr; x->b_status = nullptr;
+  for (int i = 0; i < 4; ++i) x->last_info[i] = 0;
   cudaStream_t st = ctx->stream;
   // training sample: every `stride`-th row
   uint64_t ns = std::min<uint64_t>(n, std::max<uint32_t>(train_rows, nlist * 32u));
@@ -836,6 +1178,117 @@ int stb_ivfpq_search_dev(stb_ivfpq *x, const float *q_dev, uint32_t nprobe, uint
   return ivf_fused_launch(x, q_dev, nprobe, top_k, rerank, out_hits_dev, out_status_dev);
 }
 
+// ---- batched search ----
+// grows the batch scratch to hold nq (<= IVFB_MAX_NQ) queries; cudaFree synchronises, so a batch still
+// in flight finishes before its buffers go
+static int ivfb_reserve(stb_ivfpq *x, uint32_t nq) {
+  if (nq <= x->b_cap) return STB_OK;
+  const uint32_t cap = std::min<uint32_t>(IVFB_MAX_NQ, (nq + 63) / 64 * 64);
+  cudaFree(x->b_q); cudaFree(x->b_coarse); cudaFree(x->b_probe); cudaFree(x->b_lut); cudaFree(x->b_kept);
+  cudaFree(x->b_drop); cudaFree(x->b_hits); cudaFree(x->b_status);
+  x->b_q = nullptr; x->b_coarse = nullptr; x->b_probe = nullptr; x->b_lut = nullptr; x->b_kept = nullptr;
+  x->b_drop = nullptr; x->b_hits = nullptr; x->b_status = nullptr;
+  x->b_cap = 0;
+  STB_CUDA(cudaMalloc(&x->b_q, (size_t)cap * STB_D * 4));
+  STB_CUDA(cudaMalloc(&x->b_coarse, (size_t)cap * x->nlist * 4));
+  STB_CUDA(cudaMalloc(&x->b_probe, (size_t)cap * (2 * 1024 + 1) * 4));
+  STB_CUDA(cudaMalloc(&x->b_lut, (size_t)cap * PQ_M * PQ_KSUB * 4));
+  STB_CUDA(cudaMalloc(&x->b_kept, (size_t)cap * IVFB_KEPT * 8));
+  STB_CUDA(cudaMalloc(&x->b_drop, (size_t)cap * IVFB_WARPS * 8));
+  STB_CUDA(cudaMalloc(&x->b_hits, (size_t)cap * 1024 * sizeof(stb_hit)));
+  STB_CUDA(cudaMalloc(&x->b_status, (size_t)cap * 2 * 4));
+  x->b_cap = cap;
+  return STB_OK;
+}
+
+// four launches for 1 <= nq <= IVFB_MAX_NQ queries (arguments already clamped); asynchronous
+static int ivfb_launch(stb_ivfpq *x, const float *q_dev, uint32_t nq, uint32_t nprobe, uint32_t top_k, uint32_t rerank,
+                       stb_hit *out_hits_dev, uint32_t *out_status_dev) {
+  stb_ctx *ctx = x->ctx;
+  cudaStream_t st = ctx->stream;
+  int rc = ivfb_reserve(x, nq);
+  if (rc != STB_OK) return rc;
+  uint32_t npow2 = 1; while (npow2 < x->nlist) npow2 <<= 1;
+  if (!(ctx->func_attr_mask & (1u << STB_ATTR_IVF_BATCH))) {
+    STB_CUDA(cudaFuncSetAttribute(ivfb_probe_lut_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 8));
+    STB_CUDA(cudaFuncSetAttribute(ivfb_finish_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, IVFB_FIN_SMEM));
+    ctx->func_attr_mask |= 1u << STB_ATTR_IVF_BATCH;
+  }
+  IvfbArgs a;
+  // STB_IVFPQ_BATCH_KEEP=k (1..64): each scan warp keeps only k codes (tests drive the exact slow route)
+  const char *keep_env = getenv("STB_IVFPQ_BATCH_KEEP");
+  a.keep = keep_env ? std::max(1, std::min(atoi(keep_env), IVFB_WARP_KEEP)) : IVFB_WARP_KEEP;
+  a.C = x->centroids; a.nlist = x->nlist; a.nq = nq; a.nprobe = nprobe; a.top_k = top_k; a.rerank = rerank;
+  a.list_off = x->list_off; a.cb = x->codebooks; a.codes = x->codes; a.order = x->order;
+  a.qs = q_dev; a.coarse = x->b_coarse; a.probe = x->b_probe; a.lut = x->b_lut; a.kept = x->b_kept; a.drop = x->b_drop;
+  a.rows = reinterpret_cast<const float4 *>(x->corpus->rows); a.row_base = x->corpus->row_base;
+  a.forced = x->forced; a.n_forced = x->n_forced; a.out_hits = out_hits_dev; a.out_status = out_status_dev;
+  ivfb_coarse_kernel<<<dim3((x->nlist + 31) / 32, (nq + IVFB_QTILE - 1) / IVFB_QTILE), 1024, 0, st>>>(x->centroids, x->nlist, q_dev,
+                                                                                                   nq, x->b_coarse);
+  STB_CUDA(cudaGetLastError());
+  ivfb_probe_lut_kernel<<<nq, 1024, npow2 * 8, st>>>(x->b_coarse, x->nlist, nprobe, x->list_off, x->codebooks, q_dev,
+                                                     x->b_probe, x->b_lut);
+  STB_CUDA(cudaGetLastError());
+  ivfb_scan_kernel<<<dim3(IVFB_SCAN_CTAS, nq), IVFB_SCAN_THREADS, 0, st>>>(a);
+  STB_CUDA(cudaGetLastError());
+  ivfb_finish_kernel<<<nq, IVFB_FIN_THREADS, IVFB_FIN_SMEM, st>>>(a);
+  STB_CUDA(cudaGetLastError());
+  ctx->kernel_launches += 4;
+  x->last_info[0] = nq; x->last_info[1] = nprobe; x->last_info[2] = top_k; x->last_info[3] = rerank;
+  return STB_OK;
+}
+
+static void ivfb_clamp(const stb_ivfpq *x, uint32_t top_k, uint32_t &nprobe, uint32_t &rerank) {
+  nprobe = std::max(1u, std::min(std::min(nprobe, x->nlist), 1024u));
+  rerank = std::max(top_k, std::min(rerank, (uint32_t)IVFB_RERANK_CAP));
+}
+
+int stb_ivfpq_search_batch_dev(stb_ivfpq *x, const float *q_dev, uint32_t nq, uint32_t nprobe, uint32_t top_k,
+                               uint32_t rerank, stb_hit *out_hits_dev, uint32_t *out_status_dev) {
+  if (!x) { stb_set_error("ivfpq_search_batch_dev: null index"); return STB_ERR_ARG; }
+  if (nq == 0) return STB_OK;
+  if (!q_dev || !out_hits_dev || !out_status_dev) { stb_set_error("ivfpq_search_batch_dev: null argument"); return STB_ERR_ARG; }
+  if (top_k == 0 || top_k > 1024) { stb_set_error("ivfpq_search_batch_dev: top_k must be 1..1024"); return STB_ERR_ARG; }
+  if (nq > IVFB_MAX_NQ) { stb_set_error("ivfpq_search_batch_dev: nq must be <= %u", (unsigned)IVFB_MAX_NQ); return STB_ERR_ARG; }
+  if (cudaSetDevice(x->ctx->device) != cudaSuccess) { stb_set_error("cudaSetDevice failed"); return STB_ERR_CUDA; }
+  ivfb_clamp(x, top_k, nprobe, rerank);
+  return ivfb_launch(x, q_dev, nq, nprobe, top_k, rerank, out_hits_dev, out_status_dev);
+}
+
+int stb_ivfpq_search_batch(stb_ivfpq *x, const float *q, uint32_t nq, uint32_t nprobe, uint32_t top_k, uint32_t rerank,
+                           stb_hit *out_hits, uint32_t *out_n, uint64_t *out_scanned) {
+  if (!x) { stb_set_error("ivfpq_search_batch: null index"); return STB_ERR_ARG; }
+  if (nq == 0) return STB_OK;
+  if (!q || !out_n || (top_k && !out_hits)) { stb_set_error("ivfpq_search_batch: null argument"); return STB_ERR_ARG; }
+  if (top_k > 1024) { stb_set_error("ivfpq_search_batch: top_k must be <= 1024"); return STB_ERR_ARG; }
+  if (top_k == 0) {
+    for (uint32_t i = 0; i < nq; ++i) { out_n[i] = 0; if (out_scanned) out_scanned[i] = 0; }
+    return STB_OK;
+  }
+  stb_ctx *ctx = x->ctx;
+  if (cudaSetDevice(ctx->device) != cudaSuccess) { stb_set_error("cudaSetDevice failed"); return STB_ERR_CUDA; }
+  ivfb_clamp(x, top_k, nprobe, rerank);
+  cudaStream_t st = ctx->stream;
+  std::vector<uint32_t> status;
+  for (uint32_t q0 = 0; q0 < nq; q0 += IVFB_MAX_NQ) {   // one synchronisation per chunk
+    const uint32_t m = std::min<uint32_t>(IVFB_MAX_NQ, nq - q0);
+    int rc = ivfb_reserve(x, m);
+    if (rc != STB_OK) return rc;
+    STB_CUDA(cudaMemcpyAsync(x->b_q, q + (size_t)q0 * STB_D, (size_t)m * STB_D * 4, cudaMemcpyHostToDevice, st));
+    if ((rc = ivfb_launch(x, x->b_q, m, nprobe, top_k, rerank, x->b_hits, x->b_status)) != STB_OK) return rc;
+    status.resize(2 * (size_t)m);
+    STB_CUDA(cudaMemcpyAsync(out_hits + (size_t)q0 * top_k, x->b_hits, (size_t)m * top_k * sizeof(stb_hit),
+                             cudaMemcpyDeviceToHost, st));
+    STB_CUDA(cudaMemcpyAsync(status.data(), x->b_status, (size_t)m * 2 * 4, cudaMemcpyDeviceToHost, st));
+    STB_CUDA(cudaStreamSynchronize(st));
+    for (uint32_t i = 0; i < m; ++i) {
+      out_n[q0 + i] = status[2 * i];
+      if (out_scanned) out_scanned[q0 + i] = status[2 * i + 1];
+    }
+  }
+  return STB_OK;
+}
+
 int stb_ivfpq_search(stb_ivfpq *x, const float *q, uint32_t nprobe, uint32_t top_k, uint32_t rerank,
                      stb_hit *out_hits, uint32_t *out_n, uint64_t *out_scanned) {
   if (!x || !q || !out_hits || !out_n) { stb_set_error("ivfpq_search: null argument"); return STB_ERR_ARG; }
@@ -950,6 +1403,21 @@ int stb_debug_ivfpq_export(const stb_ivfpq *x, float *centroids, float *codebook
   if (order && listed) STB_CUDA(cudaMemcpy(order, x->order, listed * 4, cudaMemcpyDeviceToHost));
   if (codes && listed) STB_CUDA(cudaMemcpy(codes, x->codes, listed * PQ_M, cudaMemcpyDeviceToHost));
   if (forced && x->n_forced) STB_CUDA(cudaMemcpy(forced, x->forced, (size_t)x->n_forced * 4, cudaMemcpyDeviceToHost));
+  return STB_OK;
+}
+
+int stb_debug_ivfpq_batch_last(const stb_ivfpq *x, uint32_t i, uint32_t info[4], float *coarse, uint32_t *probe,
+                               float *lut) {
+  if (!x) { stb_set_error("ivfpq_batch_last: null index"); return STB_ERR_ARG; }
+  if (x->last_info[0] == 0) { stb_set_error("ivfpq_batch_last: no batched search yet"); return STB_ERR_STATE; }
+  if (i >= x->last_info[0]) { stb_set_error("ivfpq_batch_last: query %u of %u", i, x->last_info[0]); return STB_ERR_ARG; }
+  if (cudaSetDevice(x->ctx->device) != cudaSuccess) { stb_set_error("cudaSetDevice failed"); return STB_ERR_CUDA; }
+  STB_CUDA(cudaStreamSynchronize(x->ctx->stream));
+  const uint32_t nprobe = x->last_info[1];
+  if (info) for (int k = 0; k < 4; ++k) info[k] = x->last_info[k];
+  if (coarse) STB_CUDA(cudaMemcpy(coarse, x->b_coarse + (size_t)i * x->nlist, (size_t)x->nlist * 4, cudaMemcpyDeviceToHost));
+  if (probe) STB_CUDA(cudaMemcpy(probe, x->b_probe + (size_t)i * (2 * nprobe + 1), (size_t)nprobe * 4, cudaMemcpyDeviceToHost));
+  if (lut) STB_CUDA(cudaMemcpy(lut, x->b_lut + (size_t)i * PQ_M * PQ_KSUB, (size_t)PQ_M * PQ_KSUB * 4, cudaMemcpyDeviceToHost));
   return STB_OK;
 }
 
