@@ -277,8 +277,10 @@ int stb_search_batch_xchg_dev(stb_ctx *ctx, const stb_corpus *corpus, const floa
  * measured by recall against stb_search: coarse spherical k-means (nlist lists), 32 x 8-bit
  * product quantiser on the residual, ADC lookup-table scan of the nprobe best lists,
  * exact re-rank of the `rerank` best candidates.  Returned distances are exact canonical
- * distances; only the candidate set is approximate.  The index refers to the corpus it
- * was built on (rows [0, n) at build time) and must be destroyed before it.
+ * distances; only the candidate set is approximate.  The index covers rows [0, rows) of its
+ * corpus (stb_ivfpq_stats): the rows present at the build and those stb_ivfpq_extend has added
+ * since; rows appended after that are not searched until the next extend.  It must be destroyed
+ * before its corpus.
  * Forced rows: rows with a non-finite component or an fp32 squared norm outside [1e-30, 1e30]
  * (K1's forced candidates) are kept out of training and of the inverted lists; every search
  * re-ranks them exactly besides the ADC candidates.  More than 1024 such rows: the build fails
@@ -295,6 +297,18 @@ typedef struct stb_ivfpq stb_ivfpq;
 int stb_ivfpq_build(stb_ctx *ctx, const stb_corpus *corpus, uint32_t nlist, uint32_t train_rows,
                     uint32_t iters, stb_ivfpq **out);
 int stb_ivfpq_destroy(stb_ivfpq *index);
+/* Index the rows appended to the index's corpus since the build or the last extend:
+ * rows [indexed, corpus rows).  Centroids and codebooks are not retrained.
+ * *out_added (may be NULL) = rows added, 0 when there were none.
+ * Synchronous: searches enqueued before the call see the old index, later ones the new.
+ * On any error the index is unchanged and still usable.
+ * STB_ERR_STATE: the corpus was cleared since the index last read it,
+ * or the forced rows would exceed 1024.
+ * Each new row gets the list and code the build would give it; within a list the new rows follow the
+ * old entries in ascending row order (a built index's lists are in ascending row order too), so two
+ * extends give the lists one extend of both parts gives.  Cost: the new rows' assignment and encoding
+ * plus one copy of the lists (36 B per row); extra memory while it runs: that copy and 48 B per new row. */
+int stb_ivfpq_extend(stb_ivfpq *index, uint64_t *out_added);
 int stb_ivfpq_stats(const stb_ivfpq *index, uint64_t *rows, uint32_t *nlist, uint32_t *max_list,
                     uint64_t *index_bytes);
 int stb_ivfpq_search(stb_ivfpq *index, const float *q, uint32_t nprobe, uint32_t top_k,

@@ -26,7 +26,7 @@ SYMBOLS = [
     "stb_search_topk_dev", "stb_corpus_prepare", "stb_corpus_tier_stats", "stb_corpus_prepare_batch", "stb_search_batch", "stb_search_batch_dev",
     "stb_xchg_create", "stb_xchg_destroy", "stb_xchg_local_handle",
     "stb_xchg_connect", "stb_xchg_connect_local", "stb_search_topk_xchg", "stb_search_xchg", "stb_search_many", "stb_xchg_create_batch", "stb_search_batch_xchg_dev", "stb_ivfpq_build",
-    "stb_ivfpq_destroy", "stb_ivfpq_stats", "stb_ivfpq_search", "stb_ivfpq_search_dev", "stb_hits_merge_dev", "stb_hits_merge_batch_dev", "stb_hits_merge", "stb_fnv1a64", "stb_line_id", "stb_line_ids",
+    "stb_ivfpq_destroy", "stb_ivfpq_extend", "stb_ivfpq_stats", "stb_ivfpq_search", "stb_ivfpq_search_dev", "stb_hits_merge_dev", "stb_hits_merge_batch_dev", "stb_hits_merge", "stb_fnv1a64", "stb_line_id", "stb_line_ids",
     "stb_ctx_counters", "stb_debug_ticket_check", "stb_debug_timestamps", "stb_debug_q4_refined", "stb_debug_batch_gemm", "stb_debug_batch_params",
     "stb_debug_batch_last",
     "stb_debug_ivfpq_export",
@@ -102,6 +102,7 @@ def lib() -> C.CDLL:
     L.stb_search_batch_xchg_dev.argtypes = [vp, vp, vp, u32, u32, vp, vp, vp]
     L.stb_ivfpq_build.argtypes = [vp, vp, u32, u32, u32, C.POINTER(vp)]
     L.stb_ivfpq_destroy.argtypes = [vp]
+    L.stb_ivfpq_extend.argtypes = [vp, C.POINTER(u64)]
     L.stb_ivfpq_stats.argtypes = [vp, C.POINTER(u64), C.POINTER(u32), C.POINTER(u32), C.POINTER(u64)]
     L.stb_ivfpq_search.argtypes = [vp, vp, u32, u32, u32, vp, C.POINTER(u32), C.POINTER(u64)]
     L.stb_ivfpq_search_dev.argtypes = [vp, vp, u32, u32, u32, vp, vp]
@@ -407,6 +408,13 @@ class IvfPq:
             self._h = None
 
     __del__ = close
+
+    def extend(self) -> int:
+        """stb_ivfpq_extend: index the rows appended to the corpus since the build or the last extend
+        (same quantisers); returns how many were added."""
+        added = u64(0)
+        _check(lib().stb_ivfpq_extend(self._h, C.byref(added)))
+        return int(added.value)
 
     def stats(self):
         rows, nbytes, nlist, mx = u64(0), u64(0), u32(0), u32(0)

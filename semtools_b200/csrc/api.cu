@@ -328,9 +328,9 @@ int stb_corpus_destroy(stb_corpus *c) {
 
 // The reduced-width copies (K2 shadow, K1 tiers) cover a PREFIX of the rows: an append leaves the
 // prefix valid and the next query / prepare only converts the new rows (q8_rows / shadow_rows < n);
-// anything else (clear) drops them.
+// anything else (clear) drops them and starts a new epoch.
 static void corpus_changed(stb_corpus *c, bool appended_only = false) {
-  if (!appended_only) { c->shadow_rows = 0; c->q8_rows = 0; }
+  if (!appended_only) { c->shadow_rows = 0; c->q8_rows = 0; ++c->epoch; }
   c->searches_since_change = 0;
   memset(c->tier_tries, 0, sizeof(c->tier_tries));
   memset(c->tier_proven, 0, sizeof(c->tier_proven));

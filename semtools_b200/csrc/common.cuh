@@ -190,6 +190,7 @@ struct stb_corpus {
   uint64_t n;
   uint64_t capacity;
   uint64_t row_base;
+  uint64_t epoch;            // bumped by every change that is not an append (an IVF-PQ index refuses to extend over it)
   // K2: L2-normalised bf16 copy in wgmma tile layout (built lazily, rebuilt when n changes)
   uint8_t *shadow;
   uint64_t shadow_rows;      // rows covered by `shadow` (== n when valid)

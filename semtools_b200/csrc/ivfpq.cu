@@ -11,7 +11,8 @@
 // Index (per shard, all in HBM):
 //   centroids  [nlist][256] f32, unit norm (spherical k-means on L2-normalised rows)
 //   codebooks  [32][256][8]  f32: product quantiser of the residual x^ - c(x), 8 dims/byte
-//   codes      [n][32] u8 sorted by list, order[n] = local row of each code, list_off[nlist+1]
+//   codes      [n][32] u8 grouped by list, order[n] = local row of each code, list_off[nlist+1]
+//              (within a list, ascending row order: see "adding rows")
 // Query: coarse scores q^.c_j (nlist*1 KiB read), top-nprobe lists, LUT[s][code] = q^_s .
 // cb[s][code] (32 KiB), ADC score = q^.c_list + sum_s LUT[s][code_s] over the probed
 // lists' codes ((nprobe/nlist)*n*32 bytes), running top-R, exact re-rank of R rows.
@@ -24,6 +25,7 @@
 #include <math_constants.h>
 
 #include <algorithm>
+#include <cub/device/device_radix_sort.cuh>
 #include <vector>
 
 #include "common.cuh"
@@ -31,7 +33,7 @@
 #define PQ_M 32
 #define PQ_DSUB 8
 #define PQ_KSUB 256
-#define IVF_FORCED_CAP 1024        // forced rows per index; more -> the build fails with STB_ERR_STATE
+#define IVF_FORCED_CAP 1024        // forced rows per index; more -> the build or extend fails with STB_ERR_STATE
 #define IVF_HOST_TOPK_MAX 4096     // stb_ivfpq_search: top_k and rerank cap of the multi-launch search
 #define IVF_NO_LIST 0xffffffffu    // assign[] of a forced row
 
@@ -50,8 +52,9 @@
 struct stb_ivfpq {
   stb_ctx *ctx;
   const stb_corpus *corpus;
+  uint64_t corpus_epoch;      // corpus->epoch when the index was built: extend refuses another
   uint32_t nlist;
-  uint64_t n;                 // rows indexed (listed + forced)
+  uint64_t n;                 // rows indexed (listed + forced): rows [0, n) of the corpus
   float *centroids;           // [nlist][256]
   float *codebooks;           // [32][256][8]
   uint8_t *codes;             // [n_listed][32], grouped by list
@@ -301,32 +304,76 @@ __global__ void pq_seed_kernel(float *cb, const float4 *X, uint64_t n, uint64_t 
 }
 
 // ------------------------------------------------------------------ inverted lists ----
-// forced rows (warp per row): assign[i] = IVF_NO_LIST, local row appended to forced[] (count in
-// *n_forced; entries past `cap` are counted, not written)
-__global__ void ivf_flag_forced_kernel(const float4 *__restrict__ X, uint64_t n, uint32_t *assign, uint32_t *forced,
-                                       uint32_t cap, uint32_t *n_forced) {
+// Adding rows [first, first + m) (the build's add phase over [0, n), and every stb_ivfpq_extend) is one
+// routine, ivf_add_rows:
+//   ivf_assign_kernel, pq_step_kernel mode 1   list and code of each new row (each row's arithmetic is
+//                                              independent of its place in the launch: an appended copy of
+//                                              an indexed row gets that row's list and code bit for bit)
+//   ivf_flag_forced_kernel                     forced rows: assign = IVF_NO_LIST, counted
+//   ivf_hist_kernel                            new rows per list; the sort's values 0..m-1
+//   cub::DeviceRadixSort::SortPairs            stable bucketing: keys = list id (the low bits that separate
+//                                              0..nlist-1 from IVF_NO_LIST), values = row - first.  An LSD radix
+//                                              sort is stable, so each list's new rows stay ascending and the
+//                                              forced rows come last, ascending; no atomic decides a position.
+//   ivf_merge_kernel                           the new codes / order: list l = its old entries in their old
+//                                              order, then its new rows ascending; the forced rows join the side
+//                                              list (ascending: new rows are larger than old ones).
+// So within a list the entries are in ascending row order, and two extends (A, then B) give the lists one
+// extend of A u B gives.  CUB rather than a hand-written counting scatter: it is stable by construction,
+// takes 2 passes for nlist <= 8192 (14 key bits) and ships header-only with the toolkit.
+
+// forced rows (warp per row): assign[i] = IVF_NO_LIST, counted in *n_forced
+__global__ void ivf_flag_forced_kernel(const float4 *__restrict__ X, uint64_t n, uint32_t *assign, uint32_t *n_forced) {
   const int lane = threadIdx.x & 31;
   const uint64_t i = (uint64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
   if (i >= n) return;
   const float4 v0 = __ldg(X + i * STB_ROW_F4 + 2 * lane), v1 = __ldg(X + i * STB_ROW_F4 + 2 * lane + 1);
   if (!ivf_forced(ivf_warp_ss(v0, v1)) || lane != 0) return;
   assign[i] = IVF_NO_LIST;
-  const uint32_t k = atomicAdd(n_forced, 1u);
-  if (k < cap) forced[k] = (uint32_t)i;
+  atomicAdd(n_forced, 1u);
 }
-__global__ void ivf_hist_kernel(const uint32_t *assign, uint64_t n, uint32_t *hist) {
+// hist[l] = new rows of list l (forced rows not counted); idx[i] = i
+__global__ void ivf_hist_kernel(const uint32_t *assign, uint64_t n, uint32_t *hist, uint32_t *idx) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n && assign[i] != IVF_NO_LIST) atomicAdd(hist + assign[i], 1u);
+  if (i >= n) return;
+  idx[i] = (uint32_t)i;
+  if (assign[i] != IVF_NO_LIST) atomicAdd(hist + assign[i], 1u);
 }
-__global__ void ivf_scatter_kernel(const uint32_t *assign, uint64_t n, uint32_t *cursor, const uint8_t *codes_row,
-                                   uint8_t *codes, uint32_t *order) {
-  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n || assign[i] == IVF_NO_LIST) return;
-  const uint32_t pos = atomicAdd(cursor + assign[i], 1u);
-  order[pos] = (uint32_t)i;
-  const uint4 *src = reinterpret_cast<const uint4 *>(codes_row + i * PQ_M);
-  uint4 *dst = reinterpret_cast<uint4 *>(codes + (size_t)pos * PQ_M);
-  dst[0] = src[0]; dst[1] = src[1];
+
+// Thread per entry of the new index.  Position o < n_out lies in list l (new_off[l] <= o < new_off[l+1]):
+// while o - new_off[l] is inside the old list it copies old entry old_off[l] + (o - new_off[l]), past it
+// the new row sorted[j], j = o - old_off[l+1] (the r-th new row of list l sits at sorted position
+// new_off[l] - old_off[l] + r).  Positions n_out.. copy the sorted forced rows (j = o - n_old) to forced_out.
+struct MergeArgs {
+  const uint8_t *old_codes; const uint32_t *old_order, *old_off, *new_off; uint32_t nlist;
+  const uint8_t *codes_row; const uint32_t *sorted; uint64_t first;   // new codes in row order, sorted row offsets
+  uint32_t n_old, n_out, n_forced_new;                                // listed entries before / after; new forced
+  uint8_t *codes; uint32_t *order; uint32_t *forced_out;
+};
+__global__ void __launch_bounds__(256)
+ivf_merge_kernel(const MergeArgs a) {
+  const uint64_t o = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= a.n_out) {
+    if (o < (uint64_t)a.n_out + a.n_forced_new) a.forced_out[o - a.n_out] = (uint32_t)(a.first + a.sorted[o - a.n_old]);
+    return;
+  }
+  uint32_t lo = 0, hi = a.nlist;      // the list l with new_off[l] <= o < new_off[l+1]
+  while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (__ldg(a.new_off + mid) <= o) lo = mid; else hi = mid; }
+  const uint32_t within = (uint32_t)o - __ldg(a.new_off + lo), ob = __ldg(a.old_off + lo), oe = __ldg(a.old_off + lo + 1);
+  const uint4 *src;
+  uint32_t row;
+  if (within < oe - ob) {
+    src = reinterpret_cast<const uint4 *>(a.old_codes + (size_t)(ob + within) * PQ_M);
+    row = __ldg(a.old_order + ob + within);
+  } else {
+    const uint32_t i = __ldg(a.sorted + ((uint32_t)o - oe));
+    src = reinterpret_cast<const uint4 *>(a.codes_row + (size_t)i * PQ_M);
+    row = (uint32_t)(a.first + i);
+  }
+  uint4 *dst = reinterpret_cast<uint4 *>(a.codes + o * PQ_M);
+  const uint4 c0 = __ldg(src), c1 = __ldg(src + 1);
+  dst[0] = c0; dst[1] = c1;
+  a.order[o] = row;
 }
 
 // ------------------------------------------------------------------ query arithmetic --
@@ -976,6 +1023,103 @@ ivfb_finish_kernel(const IvfbArgs a) {
 }
 
 // ------------------------------------------------------------------ host side ---------
+// Device buffers of one ivf_add_rows call: freed when it returns (after a stream synchronise, so no kernel
+// still reads them) unless adopted by the index.
+struct IvfScratch {
+  cudaStream_t st;
+  std::vector<void *> p;
+  template <class T> cudaError_t alloc(T **ptr, size_t bytes) {
+    *ptr = nullptr;
+    const cudaError_t e = cudaMalloc(reinterpret_cast<void **>(ptr), bytes);
+    if (e == cudaSuccess) p.push_back(*ptr);
+    return e;
+  }
+  void adopt(const void *q) { p.erase(std::find(p.begin(), p.end(), q)); }
+  ~IvfScratch() {
+    cudaStreamSynchronize(st);
+    for (void *q : p) cudaFree(q);
+    cudaGetLastError();
+  }
+};
+
+// Indexes rows [first, first + m) of x's corpus (see "inverted lists"): on success x holds the extended
+// lists and n = first + m; on any error x is unchanged and usable.  Every buffer is allocated before the
+// one synchronisation that reads the counts, and the old arrays are freed only after the merge finished.
+// Peak extra memory: the new codes + order (36 B per listed row, old and new) and 48 B per new row (list
+// ids and sort values, double-buffered, and the row-order codes) plus CUB's small temporary storage.
+static int ivf_add_rows(stb_ivfpq *x, uint64_t first, uint64_t m, const char *who) {
+  stb_ctx *ctx = x->ctx;
+  cudaStream_t st = ctx->stream;
+  const uint32_t nlist = x->nlist;
+  const uint64_t n_old = x->list_off_h[nlist];
+  const int key_bits = 32 - __builtin_clz(nlist);          // 2^key_bits - 1 >= nlist: IVF_NO_LIST sorts last
+  IvfScratch t{st, {}};
+  uint32_t *assign, *assign_alt, *idx, *idx_alt, *counts, *new_off_d, *order;
+  uint8_t *codes_row, *codes;
+  void *sort_tmp;
+  size_t sort_bytes = 0;
+  {
+    cub::DoubleBuffer<uint32_t> kb(nullptr, nullptr), vb(nullptr, nullptr);
+    STB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, kb, vb, (uint32_t)m, 0, key_bits, st));
+  }
+  STB_CUDA(t.alloc(&assign, m * 4));
+  STB_CUDA(t.alloc(&assign_alt, m * 4));
+  STB_CUDA(t.alloc(&idx, m * 4));
+  STB_CUDA(t.alloc(&idx_alt, m * 4));
+  STB_CUDA(t.alloc(&codes_row, m * PQ_M));
+  STB_CUDA(t.alloc(&counts, (size_t)(nlist + 1) * 4));
+  STB_CUDA(t.alloc(&sort_tmp, std::max<size_t>(sort_bytes, 16)));
+  STB_CUDA(t.alloc(&codes, (n_old + m) * PQ_M));
+  STB_CUDA(t.alloc(&order, (n_old + m) * 4));
+  STB_CUDA(t.alloc(&new_off_d, (size_t)(nlist + 1) * 4));
+  // list and code of every new row: the build's kernels on the rows from `first` on
+  const float4 *X4 = reinterpret_cast<const float4 *>(x->corpus->rows) + first * STB_ROW_F4;
+  ivf_assign_kernel<<<(unsigned)((m + 63) / 64), 256, 0, st>>>(x->corpus->rows + first * STB_D, m, x->centroids, nlist, assign);
+  STB_CUDA(cudaFuncSetAttribute(pq_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * PQ_KSUB * PQ_DSUB * 4));
+  PqArgs pa;
+  pa.X = X4; pa.n = m; pa.stride = 1; pa.assign = assign; pa.C = x->centroids; pa.cb = x->codebooks;
+  pa.sums = nullptr; pa.counts = nullptr; pa.codes_out = codes_row; pa.mode = 1;
+  for (int s0 = 0; s0 < PQ_M; s0 += 8) {
+    pa.s0 = s0;
+    pq_step_kernel<<<ctx->sm_count * 2, 256, 8 * PQ_KSUB * PQ_DSUB * 4, st>>>(pa);
+  }
+  // forced rows leave the lists; counts[nlist] is their count
+  STB_CUDA(cudaMemsetAsync(counts, 0, (size_t)(nlist + 1) * 4, st));
+  ivf_flag_forced_kernel<<<(unsigned)((m + 7) / 8), 256, 0, st>>>(X4, m, assign, counts + nlist);
+  ivf_hist_kernel<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(assign, m, counts, idx);
+  cub::DoubleBuffer<uint32_t> kb(assign, assign_alt), vb(idx, idx_alt);
+  STB_CUDA(cub::DeviceRadixSort::SortPairs(sort_tmp, sort_bytes, kb, vb, (uint32_t)m, 0, key_bits, st));
+  STB_CUDA(cudaGetLastError());
+  std::vector<uint32_t> hist(nlist + 1);
+  STB_CUDA(cudaMemcpyAsync(hist.data(), counts, (size_t)(nlist + 1) * 4, cudaMemcpyDeviceToHost, st));
+  STB_CUDA(cudaStreamSynchronize(st));
+  const uint32_t nf_new = hist[nlist];
+  if ((uint64_t)x->n_forced + nf_new > IVF_FORCED_CAP) {
+    stb_set_error("%s: %u rows are non-finite or have an fp32 squared norm outside [1e-30, 1e30] (at most %u)", who,
+                  x->n_forced + nf_new, (unsigned)IVF_FORCED_CAP);
+    return STB_ERR_STATE;
+  }
+  std::vector<uint32_t> new_off(nlist + 1, 0);
+  for (uint32_t l = 0; l < nlist; ++l) new_off[l + 1] = new_off[l] + (x->list_off_h[l + 1] - x->list_off_h[l]) + hist[l];
+  STB_CUDA(cudaMemcpyAsync(new_off_d, new_off.data(), (size_t)(nlist + 1) * 4, cudaMemcpyHostToDevice, st));
+  MergeArgs ma;
+  ma.old_codes = x->codes; ma.old_order = x->order; ma.old_off = x->list_off; ma.new_off = new_off_d; ma.nlist = nlist;
+  ma.codes_row = codes_row; ma.sorted = vb.Current(); ma.first = first;
+  ma.n_old = (uint32_t)n_old; ma.n_out = new_off[nlist]; ma.n_forced_new = nf_new;
+  ma.codes = codes; ma.order = order; ma.forced_out = x->forced + x->n_forced;   // past the entries searches read
+  ivf_merge_kernel<<<(unsigned)(((uint64_t)ma.n_out + nf_new + 255) / 256), 256, 0, st>>>(ma);
+  STB_CUDA(cudaGetLastError());
+  STB_CUDA(cudaStreamSynchronize(st));                     // searches enqueued before this call are done too
+  ctx->kernel_launches += 9;                               // assign, 4 x encode, flag, hist, sort (as one), merge
+  t.adopt(codes); t.adopt(order); t.adopt(new_off_d);
+  cudaFree(x->codes); cudaFree(x->order); cudaFree(x->list_off);
+  x->codes = codes; x->order = order; x->list_off = new_off_d;
+  x->list_off_h.swap(new_off);
+  x->n_forced += nf_new;
+  x->n = first + m;
+  return STB_OK;
+}
+
 extern "C" {
 
 int stb_ivfpq_destroy(stb_ivfpq *x) {
@@ -1011,7 +1155,7 @@ int stb_ivfpq_build(stb_ctx *ctx, const stb_corpus *corpus, uint32_t nlist, uint
   if (iters < 1) iters = 8;
   stb_ivfpq *x = new (std::nothrow) stb_ivfpq();
   if (!x) { stb_set_error("out of host memory"); return STB_ERR_NOMEM; }
-  x->ctx = ctx; x->corpus = corpus; x->nlist = nlist; x->n = n;
+  x->ctx = ctx; x->corpus = corpus; x->corpus_epoch = corpus->epoch; x->nlist = nlist; x->n = 0;
   x->centroids = nullptr; x->codebooks = nullptr; x->codes = nullptr; x->order = nullptr; x->list_off = nullptr;
   x->coarse = nullptr; x->lut = nullptr; x->probe = nullptr; x->cand = nullptr; x->cand_cap = 0; x->cand_rows = nullptr;
   x->keys2 = nullptr; x->tickets = nullptr; x->forced = nullptr; x->n_forced = 0;
@@ -1025,15 +1169,14 @@ int stb_ivfpq_build(stb_ctx *ctx, const stb_corpus *corpus, uint32_t nlist, uint
   ns = std::min<uint64_t>(ns, (n + stride - 1) / stride);
   const float4 *X4 = reinterpret_cast<const float4 *>(corpus->rows);
   float *sums = nullptr, *pq_sums = nullptr;
-  uint32_t *counts = nullptr, *pq_counts = nullptr, *assign = nullptr, *cursor = nullptr;
-  uint8_t *codes_row = nullptr;
+  uint32_t *counts = nullptr, *pq_counts = nullptr, *assign = nullptr;
   IVF_CUDA(cudaMalloc(&x->centroids, (size_t)nlist * STB_D * 4));
   IVF_CUDA(cudaMalloc(&x->codebooks, (size_t)PQ_M * PQ_KSUB * PQ_DSUB * 4));
   IVF_CUDA(cudaMalloc(&sums, (size_t)nlist * STB_D * 4));
   IVF_CUDA(cudaMalloc(&counts, (size_t)(nlist + 1) * 4));
   IVF_CUDA(cudaMalloc(&pq_sums, (size_t)PQ_M * PQ_KSUB * PQ_DSUB * 4));
   IVF_CUDA(cudaMalloc(&pq_counts, (size_t)PQ_M * PQ_KSUB * 4));
-  IVF_CUDA(cudaMalloc(&assign, n * 4));
+  IVF_CUDA(cudaMalloc(&assign, ns * 4));
   // ---- coarse k-means on the sample (strided view of the corpus: stride in rows) --------
   // initial centroids: evenly spaced sample rows, normalised
   IVF_CUDA(cudaMemsetAsync(counts, 0, (size_t)nlist * 4, st));
@@ -1067,48 +1210,16 @@ int stb_ivfpq_build(stb_ctx *ctx, const stb_corpus *corpus, uint32_t nlist, uint
     pq_finish_codebooks_kernel<<<(PQ_M * PQ_KSUB + 255) / 256, 256, 0, st>>>(x->codebooks, pq_sums, pq_counts);
   }
   IVF_CUDA(cudaGetLastError());
-  // ---- add: assign + encode every row, then group by list --------------------------------------
-  IVF_CUDA(cudaMalloc(&codes_row, n * PQ_M));
-  IVF_CUDA(cudaMalloc(&x->codes, n * PQ_M));
-  IVF_CUDA(cudaMalloc(&x->order, n * 4));
-  IVF_CUDA(cudaMalloc(&x->list_off, (size_t)(nlist + 1) * 4));
-  IVF_CUDA(cudaMalloc(&cursor, (size_t)nlist * 4));
-  ivf_assign_kernel<<<(unsigned)((n + 63) / 64), 256, 0, st>>>(corpus->rows, n, x->centroids, nlist, assign);
-  pa.X = X4; pa.n = n; pa.stride = 1; pa.codes_out = codes_row;
-  for (int s0 = 0; s0 < PQ_M; s0 += 8) {
-    pa.s0 = s0; pa.mode = 1;
-    pq_step_kernel<<<ctx->sm_count * 2, 256, 8 * PQ_KSUB * PQ_DSUB * 4, st>>>(pa);
-  }
-  // forced rows leave the lists (assign = IVF_NO_LIST) for the side list; counts[nlist] is their count
-  IVF_CUDA(cudaMalloc(&x->forced, IVF_FORCED_CAP * 4));
-  IVF_CUDA(cudaMemsetAsync(counts, 0, (size_t)(nlist + 1) * 4, st));
-  ivf_flag_forced_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(X4, n, assign, x->forced, IVF_FORCED_CAP, counts + nlist);
-  ivf_hist_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(assign, n, counts);
-  std::vector<uint32_t> hist(nlist + 1);
-  IVF_CUDA(cudaMemcpyAsync(hist.data(), counts, (size_t)(nlist + 1) * 4, cudaMemcpyDeviceToHost, st));
+  // training buffers go before the add phase allocates its own
   IVF_CUDA(cudaStreamSynchronize(st));
-  if (hist[nlist] > IVF_FORCED_CAP) {
-    stb_set_error("ivfpq_build: %u rows are non-finite or have an fp32 squared norm outside [1e-30, 1e30] (at most %u)",
-                  hist[nlist], (unsigned)IVF_FORCED_CAP);
-    cudaFree(sums); cudaFree(counts); cudaFree(pq_sums); cudaFree(pq_counts); cudaFree(assign); cudaFree(cursor);
-    cudaFree(codes_row); cudaFree(sample);
-    stb_ivfpq_destroy(x);
-    return STB_ERR_STATE;
-  }
-  x->n_forced = hist[nlist];
-  {  // ascending, so the side list does not depend on the order the atomics ran in
-    std::vector<uint32_t> f(x->n_forced);
-    IVF_CUDA(cudaMemcpyAsync(f.data(), x->forced, (size_t)x->n_forced * 4, cudaMemcpyDeviceToHost, st));
-    IVF_CUDA(cudaStreamSynchronize(st));
-    std::sort(f.begin(), f.end());
-    IVF_CUDA(cudaMemcpyAsync(x->forced, f.data(), (size_t)x->n_forced * 4, cudaMemcpyHostToDevice, st));
-    IVF_CUDA(cudaStreamSynchronize(st));
-  }
+  cudaFree(sums); cudaFree(counts); cudaFree(pq_sums); cudaFree(pq_counts); cudaFree(assign); cudaFree(sample);
+  // ---- add: rows [0, n) into empty lists, as stb_ivfpq_extend adds its rows ----------------------
+  IVF_CUDA(cudaMalloc(&x->forced, IVF_FORCED_CAP * 4));
+  IVF_CUDA(cudaMalloc(&x->list_off, (size_t)(nlist + 1) * 4));
+  IVF_CUDA(cudaMemsetAsync(x->list_off, 0, (size_t)(nlist + 1) * 4, st));
   x->list_off_h.assign(nlist + 1, 0);
-  for (uint32_t l = 0; l < nlist; ++l) x->list_off_h[l + 1] = x->list_off_h[l] + hist[l];
-  IVF_CUDA(cudaMemcpyAsync(x->list_off, x->list_off_h.data(), (size_t)(nlist + 1) * 4, cudaMemcpyHostToDevice, st));
-  IVF_CUDA(cudaMemcpyAsync(cursor, x->list_off_h.data(), (size_t)nlist * 4, cudaMemcpyHostToDevice, st));
-  ivf_scatter_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(assign, n, cursor, codes_row, x->codes, x->order);
+  int rc = ivf_add_rows(x, 0, n, "ivfpq_build");
+  if (rc != STB_OK) { stb_ivfpq_destroy(x); return rc; }
   // query scratch
   IVF_CUDA(cudaMalloc(&x->coarse, (size_t)nlist * 4));
   IVF_CUDA(cudaMalloc(&x->lut, (size_t)PQ_M * PQ_KSUB * 4));
@@ -1119,9 +1230,7 @@ int stb_ivfpq_build(stb_ctx *ctx, const stb_corpus *corpus, uint32_t nlist, uint
   IVF_CUDA(cudaMemsetAsync(x->tickets, 0, 2 * sizeof(unsigned int), ctx->stream));
   IVF_CUDA(cudaGetLastError());
   IVF_CUDA(cudaStreamSynchronize(st));
-  cudaFree(sums); cudaFree(counts); cudaFree(pq_sums); cudaFree(pq_counts); cudaFree(assign); cudaFree(cursor);
-  cudaFree(codes_row); cudaFree(sample);
-  ctx->kernel_launches += 8 + iters * 12;
+  ctx->kernel_launches += 3 + iters * 8;                   // training (the add phase counts its own)
   *out = x;
   return STB_OK;
 }
@@ -1133,6 +1242,25 @@ int stb_ivfpq_stats(const stb_ivfpq *x, uint64_t *rows, uint32_t *nlist, uint32_
   if (max_list) { uint32_t m = 0; for (uint32_t l = 0; l < x->nlist; ++l) m = std::max(m, x->list_off_h[l + 1] - x->list_off_h[l]); *max_list = m; }
   if (bytes) *bytes = x->n * (PQ_M + 4) + (uint64_t)x->nlist * 1024 + PQ_M * PQ_KSUB * PQ_DSUB * 4;
   return STB_OK;
+}
+
+// Indexes the rows appended to the corpus since the build or the last extend, with the build's quantisers
+// (ivf_add_rows).  A corpus that started a new epoch (cleared) no longer holds the rows the index refers to.
+int stb_ivfpq_extend(stb_ivfpq *x, uint64_t *out_added) {
+  if (out_added) *out_added = 0;
+  if (!x) { stb_set_error("ivfpq_extend: null index"); return STB_ERR_ARG; }
+  if (cudaSetDevice(x->ctx->device) != cudaSuccess) { stb_set_error("cudaSetDevice failed"); return STB_ERR_CUDA; }
+  const stb_corpus *c = x->corpus;
+  if (c->epoch != x->corpus_epoch || c->n < x->n) {
+    stb_set_error("ivfpq_extend: the corpus was cleared since the index was built (%llu rows, the index holds %llu)",
+                  (unsigned long long)c->n, (unsigned long long)x->n);
+    return STB_ERR_STATE;
+  }
+  const uint64_t m = c->n - x->n;
+  if (m == 0) return STB_OK;
+  const int rc = ivf_add_rows(x, x->n, m, "ivfpq_extend");
+  if (rc == STB_OK && out_added) *out_added = m;
+  return rc;
 }
 
 // Approximate top-k: probe `nprobe` lists, keep the `rerank` best ADC scores, re-score those
