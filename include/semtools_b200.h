@@ -408,6 +408,11 @@ int stb_debug_timestamps(stb_ctx *ctx, int reset, uint64_t out[8]);
  * top-k launches since the last reset (reset != 0 zeroes the counter after reading it).
  * Synchronises the context's stream. */
 int stb_debug_q4_refined(stb_ctx *ctx, int reset, uint64_t *refined);
+/* The tile offsets at which K1's last n (<= 8) top-k launches on the context started their pass,
+ * oldest first; 0xffffffff for a launch that did not co-scan.  A series of stb_search_topk_dev
+ * calls on one corpus co-scans: each query after the first starts where its predecessor is
+ * reading.  Synchronises the context's stream. */
+int stb_debug_coscan_offsets(stb_ctx *ctx, uint32_t n, uint32_t *out);
 /* Test hook for K2: shadow build + wgmma GEMM on host inputs; out_full receives the
  * approximate cosine matrix [ceil(nq/128)*128][ceil(n/256)*256] (f32), out_submax (may be
  * NULL) the per-32-row maxima [ceil(nq/128)][ceil(n/256)*8][128]. */

@@ -116,12 +116,15 @@ int stb_ctx_create(int device, void *cuda_stream, stb_ctx **out) {
     if ((rc = dev_reserve(&c->q4_thr, &one, STB_TICKET_SLOTS * STB_Q4_WORDS)) != STB_OK) goto fail;
     one = 0;
     if ((rc = dev_reserve(&c->q4_refined, &one, 1)) != STB_OK) goto fail;
+    one = 0;
+    if ((rc = dev_reserve(&c->coscan_off, &one, STB_TICKET_SLOTS)) != STB_OK) goto fail;
   }
   if ((rc = dev_reserve(&c->hits_dev, &c->hits_cap, 1024)) != STB_OK) goto fail;
   if (cudaMemset(c->counters, 0, c->counters_cap * sizeof(unsigned int)) != cudaSuccess ||
       cudaMemset(c->tickets, 0, STB_TICKET_SLOTS * sizeof(unsigned long long)) != cudaSuccess ||
       cudaMemset(c->q4_thr, 0, STB_TICKET_SLOTS * STB_Q4_WORDS * sizeof(unsigned long long)) != cudaSuccess ||
       cudaMemset(c->q4_refined, 0, sizeof(unsigned long long)) != cudaSuccess ||
+      cudaMemset(c->coscan_off, 0, STB_TICKET_SLOTS * sizeof(unsigned long long)) != cudaSuccess ||
       cudaMemset(c->err_flag, 0, sizeof(int)) != cudaSuccess ||
       cudaMallocHost((void **)&c->q_pin, STB_D * sizeof(float)) != cudaSuccess ||
       cudaMallocHost((void **)&c->status_pin, 8 * sizeof(uint32_t)) != cudaSuccess ||
@@ -147,7 +150,7 @@ int stb_ctx_destroy(stb_ctx *c) {
   cudaFree(c->block_keys); cudaFree(c->counters); cudaFree(c->q_dev); cudaFree(c->hits_dev);
   cudaFree(c->status_dev); cudaFree(c->collect_rows); cudaFree(c->collect_count);
   cudaFree(c->collect_hits); cudaFree(c->ranges_dev); cudaFree(c->err_flag);
-  cudaFree(c->tickets); cudaFree(c->q4_thr); cudaFree(c->q4_refined);
+  cudaFree(c->tickets); cudaFree(c->q4_thr); cudaFree(c->q4_refined); cudaFree(c->coscan_off);
   cudaFree(c->dbg_dev); cudaFree(c->hist_dev); cudaFree(c->bq_tiles); cudaFree(c->b_submax); cudaFree(c->b_tilemax); cudaFree(c->b_cand);
   cudaFree(c->b_thr); cudaFree(c->b_cnt); cudaFree(c->b_keys); cudaFree(c->b_qbad);
   cudaFree(c->bq_dev); cudaFree(c->bh_dev); cudaFree(c->bs_dev); cudaFree(c->embed_off_dev); cudaFree(c->embed_ids_dev); cudaFree(c->embed_out_dev);
@@ -214,6 +217,25 @@ int stb_debug_q4_refined(stb_ctx *ctx, int reset, uint64_t *refined) {
   STB_CUDA(cudaMemcpy(&v, ctx->q4_refined, sizeof(v), cudaMemcpyDeviceToHost));
   if (reset) STB_CUDA(cudaMemset(ctx->q4_refined, 0, sizeof(v)));
   if (refined) *refined = v;
+  return STB_OK;
+}
+
+// The tile offsets K1's last n top-k launches on the ticket ring started their pass at, oldest first;
+// 0xffffffff for a launch that did not co-scan (or whose slot a later launch reused).  Synchronises.
+int stb_debug_coscan_offsets(stb_ctx *ctx, uint32_t n, uint32_t *out) {
+  int rc = ctx_use(ctx);
+  if (rc) return rc;
+  if (n > STB_TICKET_SLOTS || (n && !out)) { stb_set_error("coscan_offsets: n must be 0..%d", STB_TICKET_SLOTS); return STB_ERR_ARG; }
+  unsigned long long w[STB_TICKET_SLOTS];
+  STB_CUDA(cudaStreamSynchronize(ctx->stream));
+  STB_CUDA(cudaMemcpy(w, ctx->coscan_off, sizeof(w), cudaMemcpyDeviceToHost));
+  for (uint32_t i = 0; i < n; ++i) {
+    out[i] = 0xffffffffu;
+    if (ctx->topk_launches < n - i) continue;
+    const int slot = (int)((ctx->topk_launches - (n - i)) % STB_TICKET_SLOTS);
+    const uint32_t tag = ctx->coscan_tag[slot];
+    if (tag && (uint32_t)(w[slot] >> 32) == tag) out[i] = (uint32_t)w[slot];
+  }
   return STB_OK;
 }
 
@@ -456,9 +478,11 @@ static int stb_env_max_tier() {
   if (e[0] == 'h') return STB_TIER_H16;
   return STB_TIER_Q8;
 }
-// STB_SCAN_OVERLAP=1 (opt-in until timed on hardware): the asynchronous entry points (stb_search_topk_dev,
-// stb_search_topk_xchg, stb_search_many) use the overlapped launch mode (one CTA per SM, dependent released
-// at kernel start); default: they launch like the synchronous ones (full grid, dependent released after the scan).
+// The single-GPU asynchronous entry points (stb_search_topk_dev, stb_search_many without an exchange) always
+// use the overlapped launch mode and co-scan (scan_topk.cu: stb_coscan_offset): back-to-back queries share
+// each tile's HBM read.  STB_SCAN_OVERLAP=1 (opt-in until timed on a multi-GPU box) gives the sharded forms
+// (stb_search_topk_xchg, stb_search_many with an exchange) the overlapped mode, without the co-scan; by default
+// they launch like the synchronous entry points (full grid, dependent released after the scan).
 static bool stb_env_overlap() {
   const char *e = getenv("STB_SCAN_OVERLAP");
   return e && e[0] == '1';
@@ -744,7 +768,7 @@ int stb_search_topk_dev(stb_ctx *ctx, const stb_corpus *corpus, const float *q_d
   // builds one: stb_corpus_prepare does); status[1] says whether the result is proven, the
   // caller's fallback is unchanged
   return stb_launch_scan_topk(ctx, corpus, best_built_tier(corpus, top_k), q_dev, top_k, nullptr, 0, corpus->n,
-                              out_hits_dev, out_status_dev, nullptr, stb_env_overlap());
+                              out_hits_dev, out_status_dev, nullptr, true);
 }
 
 // ------------------------------------------------------------ peer-memory exchange ---
@@ -1290,7 +1314,7 @@ int stb_search_many(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint
     uint32_t *os = ctx->many_status_pin + 4 * (size_t)i;
     if (x) rc = search_topk_xchg_impl(ctx, corpus, ctx->bq_dev + (size_t)i * STB_D, top_k, x, oh, os, nq > 1 && stb_env_overlap());
     else rc = stb_launch_scan_topk(ctx, corpus, tier, ctx->bq_dev + (size_t)i * STB_D, top_k, nullptr, 0, corpus->n, oh, os, nullptr,
-                                   nq > 1 && stb_env_overlap());
+                                   nq > 1);
     if (rc != STB_OK) { cudaStreamSynchronize(ctx->stream); return rc; }
   }
   STB_CUDA(cudaStreamSynchronize(ctx->stream));

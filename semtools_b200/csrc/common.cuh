@@ -85,6 +85,19 @@ struct stb_ctx {
   unsigned long long ticket_next[8];   // per slot: its value when the next launch using it starts
   unsigned long long topk_launches;    // picks the slot
   bool ticket_ring;                    // set by the first overlapped launch; until then every launch uses slot 0
+  // K1 co-scan (scan_topk.cu: stb_coscan_offset): per ticket slot, the tile offset its last co-scan launch
+  // chose, as a tagged word (tag << 32 | offset, the tag is the launch count); the host's copy of the tags
+  // (0: the slot's last launch did not co-scan) and the last co-scan launch, which the next one may follow
+  unsigned long long *coscan_off;
+  uint32_t coscan_tag[8];
+  struct {
+    const void *corpus;                // null: no launch to follow
+    int src;
+    uint64_t n_virtual, tiles, t_bulk;
+    unsigned long long t_base;
+    int slot;
+    uint32_t tag;
+  } coscan_prev;
   // q8 tier prefilter (scan_topk.cu: stb_scan_q4): STB_TICKET_SLOTS x STB_Q4_WORDS tagged threshold words,
   // one slot per launch in turn; the launch count is the tag
   unsigned long long *q4_thr;
@@ -217,7 +230,9 @@ struct stb_corpus {
 // tier: STB_TIER_* -- which copy of `c` the streaming pass reads (must exist and be current).
 // overlapped: the launch is one of a pipelined series (asynchronous entry points): the grid is sized
 // for ONE CTA per SM and releases its dependent at its START, so the next query's scan co-runs with
-// this one instead of waiting for it to drain (scan_topk.cu: "overlapped launches").
+// this one instead of waiting for it to drain (scan_topk.cu: "overlapped launches").  Without an
+// exchange and ranges the overlapped launch also co-scans: it starts its pass where its predecessor
+// on the same corpus is reading, so the two scans share each tile's read through L2.
 int stb_launch_scan_topk(stb_ctx *ctx, const stb_corpus *c, int tier, const float *q_dev, uint32_t top_k,
                          const uint64_t *ranges_dev, uint32_t n_ranges,
                          uint64_t n_virtual, stb_hit *out_hits_dev,

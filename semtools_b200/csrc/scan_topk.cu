@@ -60,7 +60,7 @@ struct ScanArgs {
   unsigned long long t_base;     // its value when this launch starts (host-tracked)
   uint64_t t_bulk;               // tickets [0, t_bulk) cover STB_TICKET_TILES tiles each, later ones one tile
 };
-#define STB_TICKET_TILES 4
+#define STB_TICKET_TILES 4   // co-scan, 10M rows, q8: 4 and 2 tiles 0.434 ms/query, 1 tile 0.635 ms
 
 // ---- tile schedule + row map shared by the three scans -----------------------------------
 // RANGES == 0: whole shard, tiles are warp-strided (the grid streams one contiguous window).
@@ -77,8 +77,12 @@ struct ScanArgs {
 // K'=128) on every pipelined query.  With tickets a late CTA simply finds less work.
 // Every warp makes exactly one failing draw, so a launch advances the counter by
 // n_tickets + total_warps -- the host tracks the base of the next launch with that.
+// Co-scan (RANGES == 0 only): the tickets count virtual tiles v, and the warp scores tile (v + off) mod
+// n_tiles, so the pass starts at tile off and wraps around the end
+// (stb_coscan_offset).  Which warp scores which row does not change the
+// lists, the drop bounds or the proof, so any offset gives the same result.
 template <int RANGES, int WB, class Body>
-__device__ __forceinline__ void stb_for_each_tile(const ScanArgs &args, uint64_t n_tiles, Body &&body) {
+__device__ __forceinline__ void stb_for_each_tile(const ScanArgs &args, uint64_t n_tiles, const uint32_t *off, Body &&body) {
   if (args.tickets) {
     // The next ticket is drawn BEFORE the current one is processed, so the atomic's L2 round trip
     // (~1 us under load) overlaps a ticket's worth of loads instead of stalling the warp 4-6 times per
@@ -98,7 +102,17 @@ __device__ __forceinline__ void stb_for_each_tile(const ScanArgs &args, uint64_t
       const unsigned long long nxt = draw();
       const uint64_t t0 = first_tile(cur);
       const uint64_t t1 = cur < args.t_bulk ? t0 + STB_TICKET_TILES : t0 + 1;
-      for (uint64_t tile = t0; tile < t1; ++tile) body(tile, tile == t0);
+      if constexpr (RANGES == 0) {
+        // *off: a shared word, read per ticket so that it holds no register across the scoring
+        uint32_t tile = (uint32_t)t0 + *reinterpret_cast<const volatile uint32_t *>(off);   // off < n_tiles < 2^32
+        if (tile >= n_tiles) tile -= (uint32_t)n_tiles;
+        for (uint32_t left = (uint32_t)(t1 - t0); left; --left) {
+          body(tile, false);
+          if (++tile == n_tiles) tile = 0;
+        }
+      } else {
+        for (uint64_t tile = t0; tile < t1; ++tile) body(tile, tile == t0);
+      }
       cur = nxt;
     }
     return;
@@ -172,7 +186,7 @@ __device__ __forceinline__ StbQueryNorm stb_query_norm(const float4 (&q)[8]) {
 // Approximate-cosine scan over the f32 rows.  Calls sink(score, local_row) once per 4*U-row
 // tile with a warp-uniform control flow; lanes that do not represent a row pass -inf.
 template <int U, int RANGES, class Sink>
-__device__ __forceinline__ void stb_scan_rows(const ScanArgs &args, Sink &sink) {
+__device__ __forceinline__ void stb_scan_rows(const ScanArgs &args, Sink &sink, const uint32_t *off = nullptr) {
   const int lane = threadIdx.x & 31;
   const int g = lane >> 3;   // row group inside the warp
   const int j = lane & 7;    // 16-byte column slot inside the group
@@ -189,7 +203,7 @@ __device__ __forceinline__ void stb_scan_rows(const ScanArgs &args, Sink &sink) 
   const uint64_t n_tiles = (args.n_virtual + tile_rows - 1) / tile_rows;
   StbRowMap<RANGES> rmap;
   rmap.restart();
-  stb_for_each_tile<RANGES, 64 / (4 * U)>(args, n_tiles, [&](uint64_t tile, bool first) {
+  stb_for_each_tile<RANGES, 64 / (4 * U)>(args, n_tiles, off, [&](uint64_t tile, bool first) {
     if (first) rmap.restart();
     float4 a[U][8];
     uint32_t row[U];
@@ -266,7 +280,7 @@ __device__ __forceinline__ float2 stb_shadow_pair(uint32_t w) {
 }
 
 template <int U, int RANGES, class Sink>
-__device__ __forceinline__ void stb_scan_shadow(const ScanArgs &args, const uint8_t *shadow, Sink &sink) {
+__device__ __forceinline__ void stb_scan_shadow(const ScanArgs &args, const uint8_t *shadow, Sink &sink, const uint32_t *off = nullptr) {
   const int lane = threadIdx.x & 31;
   const int g = lane >> 3;   // row group inside the warp
   const int j = lane & 7;    // logical 16-byte chunk of every K-slab
@@ -283,7 +297,7 @@ __device__ __forceinline__ void stb_scan_shadow(const ScanArgs &args, const uint
   const uint64_t n_tiles = (args.n_virtual + tile_rows - 1) / tile_rows;
   StbRowMap<RANGES> rmap;
   rmap.restart();
-  stb_for_each_tile<RANGES, 64 / (4 * U)>(args, n_tiles, [&](uint64_t tile, bool first) {
+  stb_for_each_tile<RANGES, 64 / (4 * U)>(args, n_tiles, off, [&](uint64_t tile, bool first) {
     if (first) rmap.restart();
     uint4 a[U][4];
     uint32_t row[U];
@@ -436,7 +450,7 @@ __device__ __forceinline__ void stb_q8_dots(const uint32_t *qhi, const uint32_t 
 }
 
 template <int U, int RANGES, class Sink>
-__device__ __forceinline__ void stb_scan_q8(const ScanArgs &args, const uint8_t *q8, const float *q8_scale, Sink &sink) {
+__device__ __forceinline__ void stb_scan_q8(const ScanArgs &args, const uint8_t *q8, const float *q8_scale, Sink &sink, const uint32_t *off = nullptr) {
   const int lane = threadIdx.x & 31;
   const int g = lane >> 3;   // row group inside the warp
   const int j = lane & 7;
@@ -446,7 +460,7 @@ __device__ __forceinline__ void stb_scan_q8(const ScanArgs &args, const uint8_t 
   const uint64_t n_tiles = (args.n_virtual + tile_rows - 1) / tile_rows;
   StbRowMap<RANGES> rmap;
   rmap.restart();
-  stb_for_each_tile<RANGES, 2>(args, n_tiles, [&](uint64_t tile, bool first) {
+  stb_for_each_tile<RANGES, 2>(args, n_tiles, off, [&](uint64_t tile, bool first) {
     if (first) rmap.restart();
     float sc_row[U];
     int dot[U];
@@ -513,7 +527,7 @@ struct StbQ4Args {
 
 template <int U, int RANGES, class Sink>
 __device__ __forceinline__ void stb_scan_q4(const ScanArgs &args, const uint8_t *q8, const float *q8_scale, const StbQ4Args &q4a,
-                                            uint32_t *wq, uint32_t *pw, Sink &sink) {
+                                            uint32_t *wq, uint32_t *pw, Sink &sink, const uint32_t *off = nullptr) {
   static_assert(U % 8 == 0 && STB_Q8_MAX_K <= 32, "each lane owns U / 8 rows of a tile; one lane per threshold word");
   constexpr int P = U / 8;
   const int lane = threadIdx.x & 31;
@@ -596,7 +610,7 @@ __device__ __forceinline__ void stb_scan_q4(const ScanArgs &args, const uint8_t 
   const uint64_t n_tiles = (args.n_virtual + tile_rows - 1) / tile_rows;
   StbRowMap<RANGES> rmap;
   rmap.restart();
-  stb_for_each_tile<RANGES, (64 / (4 * U) > 1 ? 64 / (4 * U) : 1)>(args, n_tiles, [&](uint64_t tile, bool first) {
+  stb_for_each_tile<RANGES, (64 / (4 * U) > 1 ? 64 / (4 * U) : 1)>(args, n_tiles, off, [&](uint64_t tile, bool first) {
     if (first) rmap.restart();
     // lane w < k: threshold word w as the other warps left it; issued with the tile's loads, folded in below
     const unsigned long long tw = lane < kw ? __ldcg(q4a.thr + lane) : 0ull;
@@ -866,8 +880,46 @@ __device__ __forceinline__ void stb_cta_sort_keys(uint64_t *keys, int n) {
   else stb_cta_sort_keys_t<4>(keys, n);
 }
 
+// Co-scan: a launch that co-runs with its predecessor on the same corpus starts its pass where the
+// predecessor is reading, so the second read of each tile is an L2 hit.  The first CTA to arrive fixes
+// the offset in this launch's tagged word (tag << 32 | offset, never cleared, like the q4 threshold
+// words); the others take its value.  The offset is a hint: a stale read of the predecessor's word or
+// counter (launch_dependents orders no memory) gives another valid offset and only costs sharing.
+// Nothing waits on the other grid.
+struct StbCoscanArgs {
+  unsigned long long *word;               // null: no co-scan, offset 0
+  uint32_t tag;
+  uint32_t pred_tag;                      // 0: no predecessor to follow (offset 0)
+  const unsigned long long *pred_word;    // the predecessor's offset word ...
+  const unsigned long long *pred_tickets; // ... its ticket counter, the counter's value at its start ...
+  unsigned long long pred_t_base;
+  uint64_t pred_t_bulk;                   // ... and its bulk ticket count (same tile count as this launch)
+};
+
+__device__ __forceinline__ uint32_t stb_coscan_offset(const StbCoscanArgs &c, uint64_t n_tiles) {
+  unsigned long long cur = __ldcg(c.word);
+  while ((uint32_t)(cur >> 32) != c.tag) {
+    uint64_t off = 0;
+    if (c.pred_tag) {
+      const unsigned long long pw = __ldcg(c.pred_word);
+      const uint64_t p_off = (uint32_t)(pw >> 32) == c.pred_tag ? (uint32_t)pw % n_tiles : 0;
+      // the predecessor's frontier: the first tile of its next undrawn ticket (stb_for_each_tile)
+      const unsigned long long drawn = __ldcg(c.pred_tickets) - c.pred_t_base;
+      uint64_t front = n_tiles;
+      if (drawn < n_tiles)
+        front = drawn < c.pred_t_bulk ? drawn * STB_TICKET_TILES : c.pred_t_bulk * STB_TICKET_TILES + (drawn - c.pred_t_bulk);
+      off = (p_off + (front < n_tiles ? front : 0)) % n_tiles;
+    }
+    const unsigned long long mine = ((unsigned long long)c.tag << 32) | off;
+    const unsigned long long prev = atomicCAS(c.word, cur, mine);
+    cur = prev == cur ? mine : prev;
+  }
+  return (uint32_t)cur % n_tiles;
+}
+
 struct TopkArgs {
   ScanArgs scan;
+  StbCoscanArgs co;
   uint64_t row_base;
   uint64_t *keys;            // sorted best-KP lists of every tree level
   unsigned int *counters;    // one arrival ticket per tree group, all levels
@@ -960,6 +1012,13 @@ stb_scan_topk_kernel(const TopkArgs args) {
   __shared__ int s_nv[2];
 
   STB_T_MIN(0);                      // first CTA starts
+  // co-scan: the tile this launch's pass starts at, fixed before the dependent is released so that
+  // the dependent's first CTA can read it
+  __shared__ uint32_t s_off;          // (stb_for_each_tile reads it with RANGES == 0 only)
+  if constexpr (RANGES == 0) {
+    if (threadIdx.x == 0) s_off = args.co.word ? stb_coscan_offset(args.co, (args.scan.n_virtual + 4 * U - 1) / (4 * U)) : 0u;
+    __syncthreads();
+  }
   // Overlapped launches (asynchronous entry points): the grid is sized for one CTA per SM and lets the
   // NEXT query's grid in right away, so two scans share the SMs and the ~10 us in which a draining
   // grid leaves HBM idle (CTA merge before exit, launch, ramp-up) are covered by the other scan.
@@ -972,9 +1031,9 @@ stb_scan_topk_kernel(const TopkArgs args) {
     // (per warp: STB_Q4_QUEUE queued rows + 256 query words)
     static_assert(STB_SCAN_WARPS * (STB_Q4_QUEUE + 256) <= 32 * STB_RR_STRIDE, "q4 scratch");
     uint32_t *scratch = reinterpret_cast<uint32_t *>(srows) + (threadIdx.x >> 5) * (STB_Q4_QUEUE + 256);
-    stb_scan_q4<U, RANGES>(args.scan, args.q8, args.q8_scale, args.q4, scratch, scratch + STB_Q4_QUEUE, sink);
-  } else if constexpr (SRC == 1) stb_scan_shadow<U, RANGES>(args.scan, args.shadow, sink);
-  else stb_scan_rows<U, RANGES>(args.scan, sink);
+    stb_scan_q4<U, RANGES>(args.scan, args.q8, args.q8_scale, args.q4, scratch, scratch + STB_Q4_QUEUE, sink, &s_off);
+  } else if constexpr (SRC == 1) stb_scan_shadow<U, RANGES>(args.scan, args.shadow, sink, &s_off);
+  else stb_scan_rows<U, RANGES>(args.scan, sink, &s_off);
   STB_T_MAX(1);                      // last CTA leaves the scan loop
   // Programmatic dependent launch: the scan above reads only the corpus and the query,
   // so the NEXT query's kernel may start streaming as soon as every CTA of this one has
@@ -1284,8 +1343,9 @@ static int stb_scan_ctas_per_sm_override() {
   return v;
 }
 
+// coscan: the corpus an overlapped launch may co-scan (null: never; stb_launch_scan_topk)
 template <int E, int RANGES, int SRC = 0, int EF = E>
-static int stb_launch_topk_t(stb_ctx *ctx, const TopkArgs &a_in, bool overlapped) {
+static int stb_launch_topk_t(stb_ctx *ctx, const TopkArgs &a_in, bool overlapped, const void *coscan) {
   constexpr int kU = SRC == 2 ? STB_Q4_SCAN_U : (SRC == 1 ? STB_SHADOW_SCAN_U : STB_SCAN_U);
   auto kern = stb_scan_topk_kernel<E, kU, RANGES, SRC, EF>;
   int occ = 0;
@@ -1323,7 +1383,27 @@ static int stb_launch_topk_t(stb_ctx *ctx, const TopkArgs &a_in, bool overlapped
     a.scan.tickets = ctx->tickets + slot;
     a.scan.t_base = ctx->ticket_next[slot];
     ctx->ticket_next[slot] += n_tickets + warps_total;
+    // co-scan: follow the last launch if it was one too, on the same corpus copy and rows (hence the
+    // same tiles); any other launch in between -- synchronous, sharded, ranged -- ends the series
+    const uint32_t tag = (uint32_t)ctx->topk_launches;   // the launch count, 0 only after a wrap: no co-scan then
+    const bool co = overlapped && coscan && RANGES == 0 && ctx->ticket_ring && tag != 0;
+    if (ctx->ticket_ring) ctx->coscan_tag[slot] = co ? tag : 0u;
+    if (co) {
+      auto &p = ctx->coscan_prev;
+      a.co.word = ctx->coscan_off + slot;
+      a.co.tag = tag;
+      if (p.corpus == coscan && p.src == SRC && p.n_virtual == a.scan.n_virtual && p.tiles == tiles) {
+        a.co.pred_tag = p.tag;
+        a.co.pred_word = ctx->coscan_off + p.slot;
+        a.co.pred_tickets = ctx->tickets + p.slot;
+        a.co.pred_t_base = p.t_base;
+        a.co.pred_t_bulk = p.t_bulk;
+      }
+      p.corpus = coscan; p.src = SRC; p.n_virtual = a.scan.n_virtual; p.tiles = tiles;
+      p.slot = slot; p.t_base = a.scan.t_base; p.t_bulk = a.scan.t_bulk; p.tag = tag;
+    }
   }
+  if (!a.co.word) ctx->coscan_prev.corpus = nullptr;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3((unsigned)grid);
@@ -1342,21 +1422,21 @@ static int stb_launch_topk_t(stb_ctx *ctx, const TopkArgs &a_in, bool overlapped
 }
 
 template <int RANGES>
-static int stb_launch_topk_r(stb_ctx *ctx, const TopkArgs &a, int tier, uint32_t top_k, bool ov) {
+static int stb_launch_topk_r(stb_ctx *ctx, const TopkArgs &a, int tier, uint32_t top_k, bool ov, const void *co) {
   const int e = stb_pick_e(top_k);
   // q8: 32-key lists below the root, 128 candidates re-ranked at the root (see stb_scan_q8)
-  if (tier == STB_TIER_Q8) return stb_launch_topk_t<1, RANGES, 2, 4>(ctx, a, ov);
+  if (tier == STB_TIER_Q8) return stb_launch_topk_t<1, RANGES, 2, 4>(ctx, a, ov, co);
   if (tier == STB_TIER_H16) {
     switch (e) {
-      case 1: return stb_launch_topk_t<1, RANGES, 1>(ctx, a, ov);
-      case 2: return stb_launch_topk_t<2, RANGES, 1>(ctx, a, ov);
-      default: return stb_launch_topk_t<4, RANGES, 1>(ctx, a, ov);
+      case 1: return stb_launch_topk_t<1, RANGES, 1>(ctx, a, ov, co);
+      case 2: return stb_launch_topk_t<2, RANGES, 1>(ctx, a, ov, co);
+      default: return stb_launch_topk_t<4, RANGES, 1>(ctx, a, ov, co);
     }
   }
   switch (e) {
-    case 1: return stb_launch_topk_t<1, RANGES, 0>(ctx, a, ov);
-    case 2: return stb_launch_topk_t<2, RANGES, 0>(ctx, a, ov);
-    default: return stb_launch_topk_t<4, RANGES, 0>(ctx, a, ov);
+    case 1: return stb_launch_topk_t<1, RANGES, 0>(ctx, a, ov, co);
+    case 2: return stb_launch_topk_t<2, RANGES, 0>(ctx, a, ov, co);
+    default: return stb_launch_topk_t<4, RANGES, 0>(ctx, a, ov, co);
   }
 }
 
@@ -1372,6 +1452,7 @@ int stb_launch_scan_topk(stb_ctx *ctx, const stb_corpus *c, int tier, const floa
   a.scan.rbegin = ranges_dev ? ranges_dev + (n_ranges + 1) : nullptr;
   a.scan.n_ranges = n_ranges;
   a.scan.tickets = nullptr; a.scan.t_base = 0; a.scan.t_bulk = 0;
+  memset(&a.co, 0, sizeof(a.co));
   a.row_base = c->row_base;
   a.keys = ctx->block_keys;
   a.counters = ctx->counters;
@@ -1400,7 +1481,9 @@ int stb_launch_scan_topk(stb_ctx *ctx, const stb_corpus *c, int tier, const floa
     a.q4.refined = ctx->q4_refined;
   }
   if (tier == STB_TIER_H16 && !c->shadow) { stb_set_error("scan_topk: h16 tier unavailable"); return STB_ERR_STATE; }
-  return n_ranges > 0 ? stb_launch_topk_r<1>(ctx, a, tier, top_k, overlapped) : stb_launch_topk_r<0>(ctx, a, tier, top_k, overlapped);
+  // the co-scan is the single-GPU form of the overlapped mode: a sharded launch keeps the plain tile order
+  const void *co = xchg ? nullptr : static_cast<const void *>(c);
+  return n_ranges > 0 ? stb_launch_topk_r<1>(ctx, a, tier, top_k, overlapped, co) : stb_launch_topk_r<0>(ctx, a, tier, top_k, overlapped, co);
 }
 
 // ------------------------------------------------------------------ collect path ---
