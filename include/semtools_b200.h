@@ -344,6 +344,45 @@ int stb_ivfpq_search_batch(stb_ivfpq *index, const float *q, uint32_t nq, uint32
                            uint32_t rerank, stb_hit *out_hits, uint32_t *out_n, uint64_t *out_scanned);
 int stb_ivfpq_search_batch_dev(stb_ivfpq *index, const float *q_dev, uint32_t nq, uint32_t nprobe,
                                uint32_t top_k, uint32_t rerank, stb_hit *out_hits_dev, uint32_t *out_status_dev);
+/* Filtered batched search: the query of Store::search_line_embeddings (src/workspace/store.rs:481-546)
+ * on the index -- only rows of a subset, an optional distance cap, top_k always caps
+ * (STB_MODE_STORE_QUERY semantics).  Shapes and argument rules are stb_ivfpq_search_batch's host form:
+ * nq == 0 is a no-op; top_k == 0 sets every count to 0; top_k > 1024 is STB_ERR_ARG; nprobe is clamped
+ * to [1, min(nlist, 1024)], rerank to [top_k, 1024]; any nq, in chunks of 4096 with one synchronisation
+ * each; the scratch belongs to the index and grows on demand.
+ *  - Filter: row_ranges holds n_ranges half-open [begin, end) pairs of GLOBAL rows, ascending and disjoint
+ *    as in stb_search (otherwise STB_ERR_RANGE before any launch, nothing written), clipped to the indexed
+ *    rows [row_base, row_base + rows) of stb_ivfpq_stats: rows appended but not yet extended into the index
+ *    are never returned.  row_ranges == NULL: every indexed row is eligible.  Non-NULL with n_ranges == 0:
+ *    the empty subset, every count 0 (store.rs:489).  n_ranges > 0 with NULL: STB_ERR_ARG.
+ *  - Eligible: a listed code whose row (row_base + order[i]) lies in a range; a forced row under the same rule.
+ *  - Probe list: the lists in the unfiltered order (coarse score desc, list id asc), skipping every list
+ *    with no eligible code; the first min(nprobe, E) of them are probed, E = lists with an eligible code.
+ *    Coarse scores and LUT are bit-identical to stb_ivfpq_search_batch's for that query.
+ *  - Candidates: exactly the `rerank` best eligible probed codes by (ADC score desc, code position asc);
+ *    a code whose score is NaN or -inf is none; a scan warp that overflows takes the batch's exact slow route.
+ *  - Hits: the candidates' rows and the eligible forced rows, canonical distance; a hit needs
+ *    distance < max_distance (strict; min(max_distance, 100) as stb_search) when has_max, else < 100;
+ *    ordered by (distance, row); at most top_k.
+ *  - Counts: out_n[i] = hits of query i; out_scanned[i] (may be NULL) = eligible codes in its probed lists.
+ *    out_hits: nq x top_k as stb_ivfpq_search_batch's, unused entries (+inf, UINT64_MAX).
+ * Cost per call, shared by its queries: a bitmap of the eligible rows (ceil(rows / 32) words) and one
+ * read of order[] (4 B per listed row) that counts each list's eligible codes.
+ * What follows:
+ *  - nprobe = nlist and rerank >= the eligible codes: the hits equal stb_search(..., has_max, max_distance,
+ *    STB_MODE_STORE_QUERY, row_ranges, n_ranges, ...) bit for bit;
+ *  - a query that normalises in fp32 (finite components, fp32 squared norm in [1e-30, 1e30]), no threshold,
+ *    nprobe >= top_k: min(top_k, eligible indexed rows) hits, as many as the exact scan (the canonical
+ *    distance is never NaN nor above 2, so every re-ranked row is a hit, and each probed list holds an
+ *    eligible code);
+ *  - row_ranges == NULL, no threshold and no empty list among the nprobe best: the hits equal
+ *    stb_ivfpq_search_batch's.
+ * stb_debug_ivfpq_batch_last describes a filtered call too: info[1] is the clamped nprobe, probe[] the lists
+ * actually probed followed by 0xffffffff. */
+int stb_ivfpq_search_filtered(stb_ivfpq *index, const float *q, uint32_t nq, uint32_t nprobe, uint32_t top_k,
+                              uint32_t rerank, int has_max, double max_distance,
+                              const uint64_t *row_ranges, uint32_t n_ranges,
+                              stb_hit *out_hits, uint32_t *out_n, uint64_t *out_scanned);
 
 /* Host-buffer form of the fused multi-GPU search (the call a sharded host makes per query):
  * pinned H2D of the query, ONE kernel (scan + NVLink exchange + merge), D2H of the merged

@@ -31,6 +31,7 @@ SYMBOLS = [
     "stb_debug_batch_last",
     "stb_debug_ivfpq_export",
     "stb_ivfpq_search_batch", "stb_ivfpq_search_batch_dev", "stb_debug_ivfpq_batch_last",
+    "stb_ivfpq_search_filtered",
 ]
 
 
@@ -126,6 +127,7 @@ def lib() -> C.CDLL:
     L.stb_ivfpq_search_batch.argtypes = [vp, vp, u32, u32, u32, u32, vp, vp, vp]
     L.stb_ivfpq_search_batch_dev.argtypes = [vp, vp, u32, u32, u32, u32, vp, vp]
     L.stb_debug_ivfpq_batch_last.argtypes = [vp, u32, vp, vp, vp, vp]
+    L.stb_ivfpq_search_filtered.argtypes = [vp, vp, u32, u32, u32, u32, i32, f64, vp, u32, vp, vp, vp]
     for name in SYMBOLS:
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("stb_version", "stb_device_count"):
@@ -468,6 +470,29 @@ class IvfPq:
         scanned = np.zeros(nq, dtype=np.uint64)
         _check(lib().stb_ivfpq_search_batch(self._h, _np_ptr(queries), nq, nprobe, top_k, rerank,
                                             _np_ptr(out) if out.size else None, _np_ptr(n), _np_ptr(scanned)))
+        return out, n, scanned
+
+    def search_filtered(self, queries, row_ranges=None, max_distance: float | None = None, nprobe: int = 64,
+                        top_k: int = 10, rerank: int = 256):
+        """stb_ivfpq_search_filtered: search_batch restricted to the rows of row_ranges ((n, 2) global
+        [begin, end) pairs as Corpus.search takes them; None = every indexed row, empty = no row), with an
+        optional distance cap.  Returns (hits [nq, top_k] padded with (+inf, UINT64_MAX), n [nq] hit counts,
+        scanned [nq] eligible codes scanned)."""
+        queries = np.ascontiguousarray(queries, dtype=np.float32).reshape(-1, STB_DIM)
+        nq = queries.shape[0]
+        rr, n_rr = None, 0
+        if row_ranges is not None:
+            rr = np.ascontiguousarray(row_ranges, dtype=np.uint64).reshape(-1, 2)
+            n_rr = rr.shape[0]
+            if n_rr == 0:
+                rr = np.zeros((1, 2), dtype=np.uint64)   # non-null pointer, zero ranges
+        out = np.zeros((nq, top_k), dtype=HIT_DTYPE)
+        n = np.zeros(nq, dtype=np.uint32)
+        scanned = np.zeros(nq, dtype=np.uint64)
+        _check(lib().stb_ivfpq_search_filtered(self._h, _np_ptr(queries), nq, nprobe, top_k, rerank,
+                                               int(max_distance is not None), float(max_distance or 0.0),
+                                               _np_ptr(rr), n_rr, _np_ptr(out) if out.size else None, _np_ptr(n),
+                                               _np_ptr(scanned)))
         return out, n, scanned
 
     def search_batch_dev(self, q_dev: int, nq: int, nprobe: int, top_k: int, rerank: int, out_hits_dev: int,

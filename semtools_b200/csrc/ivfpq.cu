@@ -78,13 +78,21 @@ struct stb_ivfpq {
   uint32_t b_cap;
   float *b_q;                 // [b_cap][256] queries of the host form
   float *b_coarse;            // [b_cap][nlist]
-  uint32_t *b_probe;          // [b_cap][2 * 1024 + 1]: nprobe list ids, then the prefix of their lengths
+  uint32_t *b_probe;          // [b_cap][2 * 1024 + 2]: nprobe list ids, the prefix of their lengths (filtered:
+                              // and the eligible codes), IVFB_PROBE_STRIDE apart
   float *b_lut;               // [b_cap][32][256]
   uint64_t *b_kept;           // [b_cap][IVFB_KEPT] each warp's best keys
   uint64_t *b_drop;           // [b_cap][IVFB_WARPS] the best key each warp dropped
   stb_hit *b_hits;            // [b_cap][1024] hits of the host form
   uint32_t *b_status;         // [b_cap][2]
   uint32_t last_info[4];      // {nq, nprobe, top_k, rerank} of the last batch launch (nq = 0: none yet)
+  bool last_filtered;         // the last batch launch was a filtered search's
+  // filtered search scratch (the eligibility pass), grown on demand
+  uint32_t *f_bitmap;         // [f_words] eligible local rows; f_words >= ceil(n / 32)
+  uint64_t f_words;
+  uint32_t *f_elig;           // [nlist] eligible codes per list
+  uint32_t *f_ranges;         // [f_ranges_cap][2] clipped local ranges
+  uint32_t f_ranges_cap;
 };
 
 // ------------------------------------------------------------------ assignment GEMM ---
@@ -781,26 +789,71 @@ ivfb_coarse_kernel(const float *C, uint32_t nlist, const float *qs, uint32_t nq,
   }
 }
 
+// Per query: probe[0, nprobe) list ids, probe[nprobe, 2 nprobe] the prefix of their lengths (the last entry
+// is the number of probed codes).  FILTER adds probe[2 nprobe + 1] = the eligible codes of the probed lists.
+#define IVFB_PROBE_STRIDE(nprobe, FILTER) (2 * (nprobe) + 1 + (FILTER ? 1 : 0))
+
+// FILTER: only lists with elig[l] > 0 are taken, in the same (coarse score desc, list id asc) order; the
+// slots past the min(nprobe, E) lists taken hold IVF_NO_LIST and the total as their prefix, so a search
+// of the prefix never lands on them.
+template <bool FILTER>
 __global__ void __launch_bounds__(1024)
 ivfb_probe_lut_kernel(const float *coarse, uint32_t nlist, uint32_t nprobe, const uint32_t *list_off, const float *cb,
-                      const float *qs, uint32_t *probe, float *lut) {
+                      const float *qs, uint32_t *probe, float *lut, const uint32_t *elig) {
   extern __shared__ uint64_t pb_keys[];   // npow2 keys
   __shared__ float sq[STB_D];
   __shared__ float s_inv;
   __shared__ uint32_t s_sz[1024];
   const uint32_t q = blockIdx.x;
   const float *cq = coarse + (size_t)q * nlist;
-  uint32_t *pr = probe + (size_t)q * (2 * nprobe + 1);
+  uint32_t *pr = probe + (size_t)q * IVFB_PROBE_STRIDE(nprobe, FILTER);
   uint32_t npow = 1; while (npow < nlist) npow <<= 1;
   for (uint32_t i = threadIdx.x; i < npow; i += blockDim.x) pb_keys[i] = (i < nlist) ? stb_make_key(cq[i], i) : STB_KEY_INVALID;
   if (threadIdx.x < STB_D) sq[threadIdx.x] = qs[(size_t)q * STB_D + threadIdx.x];
   __syncthreads();
   if (threadIdx.x == 0) s_inv = ivf_query_inv(sq);
   stb_cta_sort_keys_strided(pb_keys, npow);
-  if (threadIdx.x < nprobe) {
-    const uint32_t l = stb_key_row(pb_keys[threadIdx.x]);
-    pr[threadIdx.x] = l;
-    s_sz[threadIdx.x] = __ldg(list_off + l + 1) - __ldg(list_off + l);
+  if (!FILTER) {
+    if (threadIdx.x < nprobe) {
+      const uint32_t l = stb_key_row(pb_keys[threadIdx.x]);
+      pr[threadIdx.x] = l;
+      s_sz[threadIdx.x] = __ldg(list_off + l + 1) - __ldg(list_off + l);
+    }
+  } else {
+    // compaction of the sorted lists with an eligible code, 1024 sorted positions per step, until nprobe
+    // are taken; s_el[p] = eligible codes of probe slot p
+    __shared__ uint32_t s_el[1024], s_wcnt[32], s_taken;
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (threadIdx.x == 0) s_taken = 0;
+    __syncthreads();
+    for (uint32_t base = 0; base < nlist; base += blockDim.x) {
+      const uint32_t taken = s_taken;
+      if (taken >= nprobe) break;                                   // uniform: read after a barrier
+      const uint32_t i = base + threadIdx.x;
+      const uint32_t l = i < nlist ? stb_key_row(pb_keys[i]) : 0;
+      const uint32_t e = i < nlist ? __ldg(elig + l) : 0;
+      const unsigned bal = __ballot_sync(0xffffffffu, e > 0);
+      if (lane == 0) s_wcnt[warp] = __popc(bal);
+      __syncthreads();
+      uint32_t rank = taken + __popc(bal & ((1u << lane) - 1));
+      for (uint32_t w = 0; w < warp; ++w) rank += s_wcnt[w];
+      if (e > 0 && rank < nprobe) {
+        pr[rank] = l;
+        s_sz[rank] = __ldg(list_off + l + 1) - __ldg(list_off + l);
+        s_el[rank] = e;
+      }
+      __syncthreads();
+      if (threadIdx.x == 0) { uint32_t t = 0; for (uint32_t w = 0; w < blockDim.x / 32; ++w) t += s_wcnt[w]; s_taken = taken + t; }
+      __syncthreads();
+    }
+    const uint32_t used = min(s_taken, nprobe);
+    for (uint32_t p = used + threadIdx.x; p < nprobe; p += blockDim.x) { pr[p] = IVF_NO_LIST; s_sz[p] = 0; s_el[p] = 0; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      uint32_t el = 0;
+      for (uint32_t p = 0; p < used; ++p) el += s_el[p];
+      pr[2 * nprobe + 1] = el;
+    }
   }
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -849,14 +902,21 @@ struct IvfbTop {
 };
 
 // key of probed code v of a query (STB_KEY_INVALID past the end and for a NaN or -inf score); pref,
-// start and pc: per probed list the prefix of lengths, list_off of the list and its coarse score
+// start and pc: per probed list the prefix of lengths, list_off of the list and its coarse score.
+// FILTER with a bitmap: a code whose row (order[pos]) is not eligible is STB_KEY_INVALID too, decided
+// before its 32 bytes are read.
+template <bool FILTER>
 __device__ __forceinline__ uint64_t ivfb_code_key(uint64_t v, uint32_t total, uint32_t nprobe, const uint32_t *pref,
                                                   const uint32_t *start, const float *pc, const float *s_lut,
-                                                  const uint8_t *codes) {
+                                                  const uint8_t *codes, const uint32_t *order, const uint32_t *bitmap) {
   if (v >= total) return STB_KEY_INVALID;
   uint32_t lo = 0, hi = nprobe;      // probe p with pref[p] <= v < pref[p+1]
   while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (pref[mid] <= v) lo = mid; else hi = mid; }
   const uint32_t pos = start[lo] + (uint32_t)(v - pref[lo]);
+  if (FILTER && bitmap) {
+    const uint32_t row = __ldg(order + pos);
+    if (!((__ldg(bitmap + (row >> 5)) >> (row & 31)) & 1u)) return STB_KEY_INVALID;
+  }
   const uint4 *cp = reinterpret_cast<const uint4 *>(codes + (size_t)pos * PQ_M);
   const float s = ivf_adc_sum(s_lut, __ldg(cp), __ldg(cp + 1), pc[lo]);
   return s > -CUDART_INF_F ? stb_make_key(s, pos) : STB_KEY_INVALID;
@@ -868,19 +928,24 @@ struct IvfbArgs {
   const float *qs; float *coarse; uint32_t *probe; float *lut; uint64_t *kept, *drop;
   const float4 *rows; uint64_t row_base; const uint32_t *forced; uint32_t n_forced;
   stb_hit *out_hits; uint32_t *out_status;   // [nq][top_k], [nq][2] = {hits, codes scanned}
+  // filtered search only (the FILTER instantiations read them)
+  const uint32_t *bitmap;                    // eligible local rows, 1 bit each; NULL: every row
+  double max_dist;                           // a hit needs distance < max_dist
 };
 
+template <bool FILTER>
 __global__ void __launch_bounds__(IVFB_SCAN_THREADS)
 ivfb_scan_kernel(const IvfbArgs a) {
   __shared__ float s_lut[PQ_M * PQ_KSUB];      // 32 KiB
   __shared__ uint32_t s_pref[1024], s_start[1024];
   __shared__ float s_pc[1024];
   const uint32_t q = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const uint32_t *pr = a.probe + (size_t)q * (2 * a.nprobe + 1);
+  const uint32_t *pr = a.probe + (size_t)q * IVFB_PROBE_STRIDE(a.nprobe, FILTER);
   const float *lq = a.lut + (size_t)q * PQ_M * PQ_KSUB;
   for (uint32_t i = tid; i < PQ_M * PQ_KSUB; i += IVFB_SCAN_THREADS) s_lut[i] = lq[i];
   for (uint32_t p = tid; p < a.nprobe; p += IVFB_SCAN_THREADS) {
     const uint32_t l = pr[p];
+    if (FILTER && l == IVF_NO_LIST) { s_pref[p] = pr[a.nprobe + p]; s_start[p] = 0; s_pc[p] = 0.f; continue; }
     s_pref[p] = pr[a.nprobe + p]; s_start[p] = __ldg(a.list_off + l); s_pc[p] = a.coarse[(size_t)q * a.nlist + l];
   }
   __syncthreads();
@@ -889,7 +954,7 @@ ivfb_scan_kernel(const IvfbArgs a) {
   top.init(a.keep);
   // chunk g (32 consecutive codes) -> CTA g % IVFB_SCAN_CTAS, warp (g / IVFB_SCAN_CTAS) % 8
   for (uint64_t g = blockIdx.x + (uint64_t)IVFB_SCAN_CTAS * warp; g * 32 < total; g += IVFB_WARPS)
-    top.push(ivfb_code_key(g * 32 + lane, total, a.nprobe, s_pref, s_start, s_pc, s_lut, a.codes));
+    top.push(ivfb_code_key<FILTER>(g * 32 + lane, total, a.nprobe, s_pref, s_start, s_pc, s_lut, a.codes, a.order, a.bitmap));
   uint64_t d = top.drop;
 #pragma unroll
   for (int off = 16; off > 0; off >>= 1) d = min(d, __shfl_xor_sync(0xffffffffu, d, off));
@@ -899,6 +964,10 @@ ivfb_scan_kernel(const IvfbArgs a) {
   if (lane == 0) a.drop[(size_t)q * IVFB_WARPS + w] = d;
 }
 
+// FILTER: the slow route skips the IVF_NO_LIST slots and reads eligibility through ivfb_code_key, only
+// the eligible forced rows are re-ranked, a hit needs distance < a.max_dist, and the codes reported
+// scanned are the probed lists' eligible codes.
+template <bool FILTER>
 __global__ void __launch_bounds__(IVFB_FIN_THREADS)
 ivfb_finish_kernel(const IvfbArgs a) {
   extern __shared__ __align__(16) uint8_t dyn[];                     // IVFB_FIN_SMEM
@@ -910,7 +979,7 @@ ivfb_finish_kernel(const IvfbArgs a) {
   __shared__ uint32_t s_hist[256];
   __shared__ unsigned long long s_prefix;
   const uint32_t q = blockIdx.x, tid = threadIdx.x;
-  const uint32_t *pr = a.probe + (size_t)q * (2 * a.nprobe + 1);
+  const uint32_t *pr = a.probe + (size_t)q * IVFB_PROBE_STRIDE(a.nprobe, FILTER);
   const uint32_t total = pr[2 * a.nprobe];
   const uint32_t r = a.rerank;
   for (uint32_t i = tid; i < IVFB_KEPT; i += IVFB_FIN_THREADS) keys[i] = a.kept[(size_t)q * IVFB_KEPT + i];
@@ -937,6 +1006,7 @@ ivfb_finish_kernel(const IvfbArgs a) {
     float *s_pc = reinterpret_cast<float *>(s_pref + 2048);
     for (uint32_t p = tid; p < a.nprobe; p += IVFB_FIN_THREADS) {
       const uint32_t l = pr[p];
+      if (FILTER && l == IVF_NO_LIST) { s_pref[p] = pr[a.nprobe + p]; s_start[p] = 0; s_pc[p] = 0.f; continue; }
       s_pref[p] = pr[a.nprobe + p]; s_start[p] = __ldg(a.list_off + l); s_pc[p] = a.coarse[(size_t)q * a.nlist + l];
     }
     if (tid == 0) { s_prefix = 0; s_need = r; }
@@ -947,7 +1017,7 @@ ivfb_finish_kernel(const IvfbArgs a) {
       __syncthreads();
       const uint64_t prefix = s_prefix;
       for (uint64_t v = tid; v < total; v += IVFB_FIN_THREADS) {
-        const uint64_t key = ivfb_code_key(v, total, a.nprobe, s_pref, s_start, s_pc, s_lut, a.codes);
+        const uint64_t key = ivfb_code_key<FILTER>(v, total, a.nprobe, s_pref, s_start, s_pc, s_lut, a.codes, a.order, a.bitmap);
         if (key != STB_KEY_INVALID && (key & hi_mask) == prefix) atomicAdd(&s_hist[(key >> shift) & 255], 1u);
       }
       __syncthreads();
@@ -977,7 +1047,7 @@ ivfb_finish_kernel(const IvfbArgs a) {
     uint64_t *cand = reinterpret_cast<uint64_t *>(dyn + 16384);     // [16 KiB, 24 KiB): r <= 1024 keys
     if (!none)
       for (uint64_t v = tid; v < total; v += IVFB_FIN_THREADS) {
-        const uint64_t key = ivfb_code_key(v, total, a.nprobe, s_pref, s_start, s_pc, s_lut, a.codes);
+        const uint64_t key = ivfb_code_key<FILTER>(v, total, a.nprobe, s_pref, s_start, s_pc, s_lut, a.codes, a.order, a.bitmap);
         if (key <= thr) cand[atomicAdd(&s_nc, 1u)] = key;           // exactly min(r, valid) keys
       }
     __syncthreads();
@@ -998,11 +1068,13 @@ ivfb_finish_kernel(const IvfbArgs a) {
       if (key != STB_KEY_INVALID) row = a.order[stb_key_row(key)];
     } else if (c < nc + a.n_forced) {
       row = a.forced[c - nc];
+      if (FILTER && a.bitmap && !((__ldg(a.bitmap + (row >> 5)) >> (row & 31)) & 1u)) row = 0xffffffffffffffffull;
     }
     rows_c[c] = row;
   }
   __syncthreads();                                                   // keys are read before sd overwrites them
   const double q2 = s_q2;
+  const double limit = FILTER ? a.max_dist : STB_DEFAULT_MAX_DIST;
   for (uint32_t c = tid; c < n2; c += IVFB_FIN_THREADS) {
     double d = CUDART_INF;
     uint64_t grow = 0xffffffffffffffffull;
@@ -1011,7 +1083,7 @@ ivfb_finish_kernel(const IvfbArgs a) {
       double ab, r2;
       stb_canon_dot<true>(sqd, a.rows + row * STB_ROW_F4, ab, r2);
       const double dist = stb_canon_dist(ab, q2, r2);
-      if (dist < STB_DEFAULT_MAX_DIST) { d = dist; grow = a.row_base + row; atomicAdd(&s_pass, 1); }
+      if (dist < limit) { d = dist; grow = a.row_base + row; atomicAdd(&s_pass, 1); }
     }
     sd[c] = d; sr[c] = grow;
   }
@@ -1019,7 +1091,47 @@ ivfb_finish_kernel(const IvfbArgs a) {
   stb_cta_sort_hits(sd, sr, n2);
   const uint32_t n_out = min((uint32_t)s_pass, a.top_k);
   stb_write_hits(a.out_hits + (size_t)q * a.top_k, sd, sr, n_out, a.top_k);
-  if (tid == 0) { a.out_status[2 * q] = n_out; a.out_status[2 * q + 1] = total; }
+  if (tid == 0) { a.out_status[2 * q] = n_out; a.out_status[2 * q + 1] = FILTER ? pr[2 * a.nprobe + 1] : total; }
+}
+
+// ------------------------------------------------------------------ filtered search ------
+// The eligibility pass of stb_ivfpq_search_filtered, once per call (every query of the call shares it):
+//   ivff_bitmap_kernel  bit r of the bitmap = local row r lies in one of the clipped ranges (thread per
+//                       32-row word: a binary search for the first range ending past the word, then the
+//                       at most 32 non-empty ranges that touch it)
+//   ivff_elig_kernel    elig[l] = eligible codes of list l (warp per list, order[] read once: 4 B per
+//                       listed row); without a bitmap elig[l] is the list's length
+// The batched kernels' FILTER instantiations then probe only lists with elig > 0 and drop every code
+// and forced row whose bit is clear.
+__global__ void ivff_bitmap_kernel(const uint32_t *ranges, uint32_t n_ranges, uint32_t n_words, uint32_t *bitmap) {
+  const uint32_t w = blockIdx.x * blockDim.x + threadIdx.x;   // ranges: [begin, end) local pairs, ascending
+  if (w >= n_words) return;
+  const uint64_t w0 = (uint64_t)w * 32, w1 = w0 + 32;
+  uint32_t lo = 0, hi = n_ranges;                              // first range with end > w0
+  while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (ranges[2 * mid + 1] <= w0) lo = mid + 1; else hi = mid; }
+  uint32_t bits = 0;
+  for (uint32_t i = lo; i < n_ranges && ranges[2 * i] < w1; ++i) {
+    const uint32_t b = (uint32_t)(max((uint64_t)ranges[2 * i], w0) - w0);
+    const uint32_t e = (uint32_t)(min((uint64_t)ranges[2 * i + 1], w1) - w0);   // 0 <= b < e <= 32
+    bits |= (e - b == 32 ? 0xffffffffu : ((1u << (e - b)) - 1u)) << b;
+  }
+  bitmap[w] = bits;
+}
+
+__global__ void ivff_elig_kernel(const uint32_t *list_off, const uint32_t *order, uint32_t nlist, const uint32_t *bitmap,
+                                 uint32_t *elig) {
+  const uint32_t lane = threadIdx.x & 31, l = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (l >= nlist) return;
+  const uint32_t b = __ldg(list_off + l), e = __ldg(list_off + l + 1);
+  if (!bitmap) { if (lane == 0) elig[l] = e - b; return; }
+  uint32_t cnt = 0;
+  for (uint32_t i = b + lane; i < e; i += 32) {
+    const uint32_t row = __ldg(order + i);
+    cnt += (__ldg(bitmap + (row >> 5)) >> (row & 31)) & 1u;
+  }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, off);
+  if (lane == 0) elig[l] = cnt;
 }
 
 // ------------------------------------------------------------------ host side ---------
@@ -1129,6 +1241,7 @@ int stb_ivfpq_destroy(stb_ivfpq *x) {
   cudaFree(x->keys2); cudaFree(x->tickets); cudaFree(x->forced);
   cudaFree(x->b_q); cudaFree(x->b_coarse); cudaFree(x->b_probe); cudaFree(x->b_lut); cudaFree(x->b_kept);
   cudaFree(x->b_drop); cudaFree(x->b_hits); cudaFree(x->b_status);
+  cudaFree(x->f_bitmap); cudaFree(x->f_elig); cudaFree(x->f_ranges);
   cudaGetLastError();
   delete x;
   return STB_OK;
@@ -1162,6 +1275,8 @@ int stb_ivfpq_build(stb_ctx *ctx, const stb_corpus *corpus, uint32_t nlist, uint
   x->b_cap = 0; x->b_q = nullptr; x->b_coarse = nullptr; x->b_probe = nullptr; x->b_lut = nullptr; x->b_kept = nullptr;
   x->b_drop = nullptr; x->b_hits = nullptr; x->b_status = nullptr;
   for (int i = 0; i < 4; ++i) x->last_info[i] = 0;
+  x->last_filtered = false;
+  x->f_bitmap = nullptr; x->f_words = 0; x->f_elig = nullptr; x->f_ranges = nullptr; x->f_ranges_cap = 0;
   cudaStream_t st = ctx->stream;
   // training sample: every `stride`-th row
   uint64_t ns = std::min<uint64_t>(n, std::max<uint32_t>(train_rows, nlist * 32u));
@@ -1319,7 +1434,7 @@ static int ivfb_reserve(stb_ivfpq *x, uint32_t nq) {
   x->b_cap = 0;
   STB_CUDA(cudaMalloc(&x->b_q, (size_t)cap * STB_D * 4));
   STB_CUDA(cudaMalloc(&x->b_coarse, (size_t)cap * x->nlist * 4));
-  STB_CUDA(cudaMalloc(&x->b_probe, (size_t)cap * (2 * 1024 + 1) * 4));
+  STB_CUDA(cudaMalloc(&x->b_probe, (size_t)cap * IVFB_PROBE_STRIDE(1024, true) * 4));
   STB_CUDA(cudaMalloc(&x->b_lut, (size_t)cap * PQ_M * PQ_KSUB * 4));
   STB_CUDA(cudaMalloc(&x->b_kept, (size_t)cap * IVFB_KEPT * 8));
   STB_CUDA(cudaMalloc(&x->b_drop, (size_t)cap * IVFB_WARPS * 8));
@@ -1329,17 +1444,27 @@ static int ivfb_reserve(stb_ivfpq *x, uint32_t nq) {
   return STB_OK;
 }
 
-// four launches for 1 <= nq <= IVFB_MAX_NQ queries (arguments already clamped); asynchronous
+// The filter of a filtered launch: the eligibility pass's outputs and the distance limit.
+struct IvfbFilter {
+  const uint32_t *bitmap;     // NULL: every indexed row is eligible
+  const uint32_t *elig;       // [nlist]
+  double max_dist;
+};
+
+// four launches for 1 <= nq <= IVFB_MAX_NQ queries (arguments already clamped); asynchronous.
+// f != NULL: the filtered search's instantiations of the probe, scan and finish kernels.
 static int ivfb_launch(stb_ivfpq *x, const float *q_dev, uint32_t nq, uint32_t nprobe, uint32_t top_k, uint32_t rerank,
-                       stb_hit *out_hits_dev, uint32_t *out_status_dev) {
+                       stb_hit *out_hits_dev, uint32_t *out_status_dev, const IvfbFilter *f = nullptr) {
   stb_ctx *ctx = x->ctx;
   cudaStream_t st = ctx->stream;
   int rc = ivfb_reserve(x, nq);
   if (rc != STB_OK) return rc;
   uint32_t npow2 = 1; while (npow2 < x->nlist) npow2 <<= 1;
   if (!(ctx->func_attr_mask & (1u << STB_ATTR_IVF_BATCH))) {
-    STB_CUDA(cudaFuncSetAttribute(ivfb_probe_lut_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 8));
-    STB_CUDA(cudaFuncSetAttribute(ivfb_finish_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, IVFB_FIN_SMEM));
+    STB_CUDA(cudaFuncSetAttribute(ivfb_probe_lut_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 8));
+    STB_CUDA(cudaFuncSetAttribute(ivfb_finish_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, IVFB_FIN_SMEM));
+    STB_CUDA(cudaFuncSetAttribute(ivfb_probe_lut_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 8));
+    STB_CUDA(cudaFuncSetAttribute(ivfb_finish_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, IVFB_FIN_SMEM));
     ctx->func_attr_mask |= 1u << STB_ATTR_IVF_BATCH;
   }
   IvfbArgs a;
@@ -1351,18 +1476,29 @@ static int ivfb_launch(stb_ivfpq *x, const float *q_dev, uint32_t nq, uint32_t n
   a.qs = q_dev; a.coarse = x->b_coarse; a.probe = x->b_probe; a.lut = x->b_lut; a.kept = x->b_kept; a.drop = x->b_drop;
   a.rows = reinterpret_cast<const float4 *>(x->corpus->rows); a.row_base = x->corpus->row_base;
   a.forced = x->forced; a.n_forced = x->n_forced; a.out_hits = out_hits_dev; a.out_status = out_status_dev;
+  a.bitmap = f ? f->bitmap : nullptr; a.max_dist = f ? f->max_dist : STB_DEFAULT_MAX_DIST;
   ivfb_coarse_kernel<<<dim3((x->nlist + 31) / 32, (nq + IVFB_QTILE - 1) / IVFB_QTILE), 1024, 0, st>>>(x->centroids, x->nlist, q_dev,
                                                                                                    nq, x->b_coarse);
   STB_CUDA(cudaGetLastError());
-  ivfb_probe_lut_kernel<<<nq, 1024, npow2 * 8, st>>>(x->b_coarse, x->nlist, nprobe, x->list_off, x->codebooks, q_dev,
-                                                     x->b_probe, x->b_lut);
-  STB_CUDA(cudaGetLastError());
-  ivfb_scan_kernel<<<dim3(IVFB_SCAN_CTAS, nq), IVFB_SCAN_THREADS, 0, st>>>(a);
-  STB_CUDA(cudaGetLastError());
-  ivfb_finish_kernel<<<nq, IVFB_FIN_THREADS, IVFB_FIN_SMEM, st>>>(a);
+  if (!f) {
+    ivfb_probe_lut_kernel<false><<<nq, 1024, npow2 * 8, st>>>(x->b_coarse, x->nlist, nprobe, x->list_off, x->codebooks, q_dev,
+                                                              x->b_probe, x->b_lut, nullptr);
+    STB_CUDA(cudaGetLastError());
+    ivfb_scan_kernel<false><<<dim3(IVFB_SCAN_CTAS, nq), IVFB_SCAN_THREADS, 0, st>>>(a);
+    STB_CUDA(cudaGetLastError());
+    ivfb_finish_kernel<false><<<nq, IVFB_FIN_THREADS, IVFB_FIN_SMEM, st>>>(a);
+  } else {
+    ivfb_probe_lut_kernel<true><<<nq, 1024, npow2 * 8, st>>>(x->b_coarse, x->nlist, nprobe, x->list_off, x->codebooks, q_dev,
+                                                             x->b_probe, x->b_lut, f->elig);
+    STB_CUDA(cudaGetLastError());
+    ivfb_scan_kernel<true><<<dim3(IVFB_SCAN_CTAS, nq), IVFB_SCAN_THREADS, 0, st>>>(a);
+    STB_CUDA(cudaGetLastError());
+    ivfb_finish_kernel<true><<<nq, IVFB_FIN_THREADS, IVFB_FIN_SMEM, st>>>(a);
+  }
   STB_CUDA(cudaGetLastError());
   ctx->kernel_launches += 4;
   x->last_info[0] = nq; x->last_info[1] = nprobe; x->last_info[2] = top_k; x->last_info[3] = rerank;
+  x->last_filtered = f != nullptr;
   return STB_OK;
 }
 
@@ -1383,27 +1519,18 @@ int stb_ivfpq_search_batch_dev(stb_ivfpq *x, const float *q_dev, uint32_t nq, ui
   return ivfb_launch(x, q_dev, nq, nprobe, top_k, rerank, out_hits_dev, out_status_dev);
 }
 
-int stb_ivfpq_search_batch(stb_ivfpq *x, const float *q, uint32_t nq, uint32_t nprobe, uint32_t top_k, uint32_t rerank,
-                           stb_hit *out_hits, uint32_t *out_n, uint64_t *out_scanned) {
-  if (!x) { stb_set_error("ivfpq_search_batch: null index"); return STB_ERR_ARG; }
-  if (nq == 0) return STB_OK;
-  if (!q || !out_n || (top_k && !out_hits)) { stb_set_error("ivfpq_search_batch: null argument"); return STB_ERR_ARG; }
-  if (top_k > 1024) { stb_set_error("ivfpq_search_batch: top_k must be <= 1024"); return STB_ERR_ARG; }
-  if (top_k == 0) {
-    for (uint32_t i = 0; i < nq; ++i) { out_n[i] = 0; if (out_scanned) out_scanned[i] = 0; }
-    return STB_OK;
-  }
-  stb_ctx *ctx = x->ctx;
-  if (cudaSetDevice(ctx->device) != cudaSuccess) { stb_set_error("cudaSetDevice failed"); return STB_ERR_CUDA; }
-  ivfb_clamp(x, top_k, nprobe, rerank);
-  cudaStream_t st = ctx->stream;
+// The host forms' chunk loop (arguments checked and clamped, top_k >= 1): chunks of IVFB_MAX_NQ queries,
+// one synchronisation each.
+static int ivfb_host_chunks(stb_ivfpq *x, const float *q, uint32_t nq, uint32_t nprobe, uint32_t top_k, uint32_t rerank,
+                            stb_hit *out_hits, uint32_t *out_n, uint64_t *out_scanned, const IvfbFilter *f) {
+  cudaStream_t st = x->ctx->stream;
   std::vector<uint32_t> status;
   for (uint32_t q0 = 0; q0 < nq; q0 += IVFB_MAX_NQ) {   // one synchronisation per chunk
     const uint32_t m = std::min<uint32_t>(IVFB_MAX_NQ, nq - q0);
     int rc = ivfb_reserve(x, m);
     if (rc != STB_OK) return rc;
     STB_CUDA(cudaMemcpyAsync(x->b_q, q + (size_t)q0 * STB_D, (size_t)m * STB_D * 4, cudaMemcpyHostToDevice, st));
-    if ((rc = ivfb_launch(x, x->b_q, m, nprobe, top_k, rerank, x->b_hits, x->b_status)) != STB_OK) return rc;
+    if ((rc = ivfb_launch(x, x->b_q, m, nprobe, top_k, rerank, x->b_hits, x->b_status, f)) != STB_OK) return rc;
     status.resize(2 * (size_t)m);
     STB_CUDA(cudaMemcpyAsync(out_hits + (size_t)q0 * top_k, x->b_hits, (size_t)m * top_k * sizeof(stb_hit),
                              cudaMemcpyDeviceToHost, st));
@@ -1415,6 +1542,90 @@ int stb_ivfpq_search_batch(stb_ivfpq *x, const float *q, uint32_t nq, uint32_t n
     }
   }
   return STB_OK;
+}
+
+int stb_ivfpq_search_batch(stb_ivfpq *x, const float *q, uint32_t nq, uint32_t nprobe, uint32_t top_k, uint32_t rerank,
+                           stb_hit *out_hits, uint32_t *out_n, uint64_t *out_scanned) {
+  if (!x) { stb_set_error("ivfpq_search_batch: null index"); return STB_ERR_ARG; }
+  if (nq == 0) return STB_OK;
+  if (!q || !out_n || (top_k && !out_hits)) { stb_set_error("ivfpq_search_batch: null argument"); return STB_ERR_ARG; }
+  if (top_k > 1024) { stb_set_error("ivfpq_search_batch: top_k must be <= 1024"); return STB_ERR_ARG; }
+  if (top_k == 0) {
+    for (uint32_t i = 0; i < nq; ++i) { out_n[i] = 0; if (out_scanned) out_scanned[i] = 0; }
+    return STB_OK;
+  }
+  if (cudaSetDevice(x->ctx->device) != cudaSuccess) { stb_set_error("cudaSetDevice failed"); return STB_ERR_CUDA; }
+  ivfb_clamp(x, top_k, nprobe, rerank);
+  return ivfb_host_chunks(x, q, nq, nprobe, top_k, rerank, out_hits, out_n, out_scanned, nullptr);
+}
+
+int stb_ivfpq_search_filtered(stb_ivfpq *x, const float *q, uint32_t nq, uint32_t nprobe, uint32_t top_k, uint32_t rerank,
+                              int has_max, double max_distance, const uint64_t *row_ranges, uint32_t n_ranges,
+                              stb_hit *out_hits, uint32_t *out_n, uint64_t *out_scanned) {
+  if (!x) { stb_set_error("ivfpq_search_filtered: null index"); return STB_ERR_ARG; }
+  if (nq == 0) return STB_OK;
+  if (!q || !out_n || (top_k && !out_hits)) { stb_set_error("ivfpq_search_filtered: null argument"); return STB_ERR_ARG; }
+  if (n_ranges && !row_ranges) { stb_set_error("ivfpq_search_filtered: row_ranges is null"); return STB_ERR_ARG; }
+  if (top_k > 1024) { stb_set_error("ivfpq_search_filtered: top_k must be <= 1024"); return STB_ERR_ARG; }
+  // global ranges -> local [begin, end) pairs clipped to the indexed rows [row_base, row_base + n)
+  std::vector<uint32_t> loc;
+  if (row_ranges) {
+    const uint64_t lo = x->corpus->row_base, hi = lo + x->n;
+    uint64_t prev_end = 0;
+    loc.reserve(2 * (size_t)n_ranges);
+    for (uint32_t i = 0; i < n_ranges; ++i) {
+      uint64_t b = row_ranges[2 * i], e = row_ranges[2 * i + 1];
+      if (e < b || (i > 0 && b < prev_end)) {
+        stb_set_error("ivfpq_search_filtered: row_ranges must be ascending, disjoint, half-open");
+        return STB_ERR_RANGE;
+      }
+      prev_end = e;
+      b = std::max(b, lo); e = std::min(e, hi);
+      if (b >= e) continue;
+      loc.push_back((uint32_t)(b - lo)); loc.push_back((uint32_t)(e - lo));
+    }
+  }
+  if (top_k == 0 || (row_ranges && loc.empty())) {             // nothing can be returned: no launch
+    for (uint32_t i = 0; i < nq; ++i) { out_n[i] = 0; if (out_scanned) out_scanned[i] = 0; }
+    for (uint64_t i = 0; i < (uint64_t)nq * top_k; ++i) { out_hits[i].distance = INFINITY; out_hits[i].row = UINT64_MAX; }
+    return STB_OK;
+  }
+  stb_ctx *ctx = x->ctx;
+  if (cudaSetDevice(ctx->device) != cudaSuccess) { stb_set_error("cudaSetDevice failed"); return STB_ERR_CUDA; }
+  ivfb_clamp(x, top_k, nprobe, rerank);
+  cudaStream_t st = ctx->stream;
+  // eligibility pass: bitmap of the eligible rows, eligible codes per list
+  if (!x->f_elig) STB_CUDA(cudaMalloc(&x->f_elig, (size_t)x->nlist * 4));
+  const uint32_t *bitmap = nullptr;
+  if (row_ranges) {
+    const uint64_t words = (x->n + 31) / 32;
+    if (words > x->f_words) {
+      cudaFree(x->f_bitmap); x->f_bitmap = nullptr; x->f_words = 0;
+      STB_CUDA(cudaMalloc(&x->f_bitmap, words * 4));
+      x->f_words = words;
+    }
+    const uint32_t nr = (uint32_t)(loc.size() / 2);
+    if (nr > x->f_ranges_cap) {
+      const uint32_t cap = std::max<uint32_t>(nr, 1024);
+      cudaFree(x->f_ranges); x->f_ranges = nullptr; x->f_ranges_cap = 0;
+      STB_CUDA(cudaMalloc(&x->f_ranges, (size_t)cap * 2 * 4));
+      x->f_ranges_cap = cap;
+    }
+    STB_CUDA(cudaMemcpyAsync(x->f_ranges, loc.data(), loc.size() * 4, cudaMemcpyHostToDevice, st));
+    ivff_bitmap_kernel<<<(unsigned)((words + 255) / 256), 256, 0, st>>>(x->f_ranges, nr, (uint32_t)words, x->f_bitmap);
+    STB_CUDA(cudaGetLastError());
+    bitmap = x->f_bitmap;
+    ctx->kernel_launches += 1;
+  }
+  ivff_elig_kernel<<<(x->nlist + 7) / 8, 256, 0, st>>>(x->list_off, x->order, x->nlist, bitmap, x->f_elig);
+  STB_CUDA(cudaGetLastError());
+  ctx->kernel_launches += 1;
+  IvfbFilter f;
+  f.bitmap = bitmap; f.elig = x->f_elig;
+  f.max_dist = has_max ? std::min(max_distance, STB_DEFAULT_MAX_DIST) : STB_DEFAULT_MAX_DIST;   // as stb_search
+  const int rc = ivfb_host_chunks(x, q, nq, nprobe, top_k, rerank, out_hits, out_n, out_scanned, &f);
+  STB_CUDA(cudaStreamSynchronize(st));                         // `loc` is read by the copy above
+  return rc;
 }
 
 int stb_ivfpq_search(stb_ivfpq *x, const float *q, uint32_t nprobe, uint32_t top_k, uint32_t rerank,
@@ -1544,7 +1755,8 @@ int stb_debug_ivfpq_batch_last(const stb_ivfpq *x, uint32_t i, uint32_t info[4],
   const uint32_t nprobe = x->last_info[1];
   if (info) for (int k = 0; k < 4; ++k) info[k] = x->last_info[k];
   if (coarse) STB_CUDA(cudaMemcpy(coarse, x->b_coarse + (size_t)i * x->nlist, (size_t)x->nlist * 4, cudaMemcpyDeviceToHost));
-  if (probe) STB_CUDA(cudaMemcpy(probe, x->b_probe + (size_t)i * (2 * nprobe + 1), (size_t)nprobe * 4, cudaMemcpyDeviceToHost));
+  const size_t stride = x->last_filtered ? IVFB_PROBE_STRIDE(nprobe, true) : IVFB_PROBE_STRIDE(nprobe, false);
+  if (probe) STB_CUDA(cudaMemcpy(probe, x->b_probe + (size_t)i * stride, (size_t)nprobe * 4, cudaMemcpyDeviceToHost));
   if (lut) STB_CUDA(cudaMemcpy(lut, x->b_lut + (size_t)i * PQ_M * PQ_KSUB, (size_t)PQ_M * PQ_KSUB * 4, cudaMemcpyDeviceToHost));
   return STB_OK;
 }
