@@ -112,6 +112,36 @@ int stb_corpus_data_dev(const stb_corpus *corpus, float **rows_dev);
 /* copy rows [first, first+n) back to the host (tests, store write-back). */
 int stb_corpus_read(const stb_corpus *corpus, uint64_t first, uint64_t n,
                     float *rows);
+/* Replace and delete rows in HBM (a long-lived host that changes or drops a document's lines without
+ * clearing and re-uploading the corpus; the reference's upsert by id and delete by path filter,
+ * src/workspace/store.rs:298-357,402-434).
+ * stb_corpus_update: idx holds n GLOBAL row ids (row_base + local), strictly ascending, each below
+ *   row_base + rows; rows is n x 256 f32 (host).  Row idx[i] becomes rows[i].
+ * stb_corpus_remove: ranges holds n_ranges half-open [begin, end) pairs of GLOBAL rows, ascending and
+ *   disjoint as in stb_search, each non-empty and inside the corpus.  The rows after a removed range
+ *   move down; their order is kept.
+ * Both are synchronous on the context's stream, like stb_corpus_append:
+ *  - Validation first: a refused call writes nothing, the rows and the candidate copies stay byte for
+ *    byte as they were.  Unsorted, duplicate or out-of-range idx, and unsorted, overlapping, empty or
+ *    out-of-range ranges: STB_ERR_RANGE.  A NULL pointer with n > 0 (n_ranges > 0): STB_ERR_ARG.
+ *    n == 0 and n_ranges == 0 do nothing.
+ *  - STB_ERR_STATE while an IVF-PQ index built on this corpus is alive (stb_ivfpq_build .. destroy): the
+ *    index refers to rows by position and re-ranks from the rows.
+ *  - The candidate copies (q8 tier, 16-bit shadow) that exist stay built: each keeps covering a prefix of
+ *    the rows (all of them unless rows were appended and not yet converted), and that prefix is byte for
+ *    byte what stb_corpus_prepare writes on a fresh corpus holding the same rows, the zero padding of the
+ *    shadow's last tile included.  A copy marked unusable before the call (a row that cannot be normalised
+ *    in fp32) is dropped, so the next prepare or lazy build decides anew; otherwise a written row that
+ *    cannot be normalised marks the copy unusable, as a build does.
+ *  - Both start a new epoch (stb_ivfpq_extend refuses the corpus as after stb_corpus_clear), reset the
+ *    per-tier bookkeeping of stb_corpus_tier_stats, and end a co-scan series: the next asynchronous top-k
+ *    query starts its pass at tile 0.  The allocation never shrinks.
+ *  - Work already enqueued on the stream (e.g. stb_search_topk_dev) finishes on the old rows first.
+ * Cost: update moves ~4 KiB of HBM traffic per row plus its 1 KiB upload; remove ~5 KiB per row behind the
+ * first removed row.  Extra device memory: a staging buffer of at most 262144 rows (256 MiB), kept by the
+ * context, never a second copy of the corpus. */
+int stb_corpus_update(stb_corpus *corpus, const uint64_t *idx, const float *rows, uint64_t n);
+int stb_corpus_remove(stb_corpus *corpus, const uint64_t *ranges, uint32_t n_ranges);
 
 /* ---- K3: gather + mean-pool + L2-normalise -------------------------------------
  * Replaces model.encode_with_args(&lines, Some(2048), 16384)
@@ -280,7 +310,7 @@ int stb_search_batch_xchg_dev(stb_ctx *ctx, const stb_corpus *corpus, const floa
  * distances; only the candidate set is approximate.  The index covers rows [0, rows) of its
  * corpus (stb_ivfpq_stats): the rows present at the build and those stb_ivfpq_extend has added
  * since; rows appended after that are not searched until the next extend.  It must be destroyed
- * before its corpus.
+ * before its corpus; while it is alive stb_corpus_update and stb_corpus_remove refuse the corpus.
  * Forced rows: rows with a non-finite component or an fp32 squared norm outside [1e-30, 1e30]
  * (K1's forced candidates) are kept out of training and of the inverted lists; every search
  * re-ranks them exactly besides the ADC candidates.  More than 1024 such rows: the build fails
@@ -452,6 +482,18 @@ int stb_debug_q4_refined(stb_ctx *ctx, int reset, uint64_t *refined);
  * calls on one corpus co-scans: each query after the first starts where its predecessor is
  * reading.  Synchronises the context's stream. */
 int stb_debug_coscan_offsets(stb_ctx *ctx, uint32_t n, uint32_t *out);
+/* Test hook for the candidate copies: copies entries [first, first+n) of one copy to `out` and sets
+ * *covered (may be NULL) to the rows the copy covers (0: not built).  which = STB_COPY_Q8_CODES (256 B per
+ * row), _Q8_SCALES (f32 per row), _Q8_PLANE (nibble plane, 128 B per row), _Q8_SR ({s, rho}, 2 x f32 per
+ * row): entries are rows < covered; STB_COPY_H16_TILES: entries are whole 256-row tiles of the 16-bit shadow
+ * (131072 B each), tiles < ceil(covered / 256).  Beyond that: STB_ERR_RANGE.  Synchronises the stream. */
+#define STB_COPY_Q8_CODES 0
+#define STB_COPY_Q8_SCALES 1
+#define STB_COPY_Q8_PLANE 2
+#define STB_COPY_Q8_SR 3
+#define STB_COPY_H16_TILES 4
+int stb_debug_corpus_copy(const stb_corpus *corpus, int which, uint64_t first, uint64_t n, void *out,
+                          uint64_t *covered);
 /* Test hook for K2: shadow build + wgmma GEMM on host inputs; out_full receives the
  * approximate cosine matrix [ceil(nq/128)*128][ceil(n/256)*256] (f32), out_submax (may be
  * NULL) the per-32-row maxima [ceil(nq/128)][ceil(n/256)*8][128]. */

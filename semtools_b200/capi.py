@@ -15,20 +15,21 @@ STB_DIM = 256
 STB_OK, STB_ERR_ARG, STB_ERR_CUDA, STB_ERR_NOMEM = 0, -1, -2, -3
 STB_ERR_RANGE, STB_ERR_CAPACITY, STB_ERR_STATE = -4, -5, -6
 STB_MODE_SEARCH_DOCUMENTS, STB_MODE_STORE_QUERY = 0, 1
+STB_COPY_Q8_CODES, STB_COPY_Q8_SCALES, STB_COPY_Q8_PLANE, STB_COPY_Q8_SR, STB_COPY_H16_TILES = 0, 1, 2, 3, 4
 
 # every symbol include/semtools_b200.h declares (tests check the .so exports all)
 SYMBOLS = [
     "stb_version", "stb_last_error", "stb_device_count", "stb_ctx_create", "stb_ctx_destroy",
     "stb_ctx_sync", "stb_ctx_stream", "stb_table_load", "stb_table_destroy", "stb_corpus_create",
     "stb_corpus_destroy", "stb_corpus_append", "stb_corpus_append_dev", "stb_corpus_clear",
-    "stb_corpus_rows", "stb_corpus_data_dev", "stb_corpus_read", "stb_embed", "stb_embed_dev",
+    "stb_corpus_rows", "stb_corpus_data_dev", "stb_corpus_read", "stb_corpus_update", "stb_corpus_remove", "stb_embed", "stb_embed_dev",
     "stb_embed_status", "stb_search",
     "stb_search_topk_dev", "stb_corpus_prepare", "stb_corpus_tier_stats", "stb_corpus_prepare_batch", "stb_search_batch", "stb_search_batch_dev",
     "stb_xchg_create", "stb_xchg_destroy", "stb_xchg_local_handle",
     "stb_xchg_connect", "stb_xchg_connect_local", "stb_search_topk_xchg", "stb_search_xchg", "stb_search_many", "stb_xchg_create_batch", "stb_search_batch_xchg_dev", "stb_ivfpq_build",
     "stb_ivfpq_destroy", "stb_ivfpq_extend", "stb_ivfpq_stats", "stb_ivfpq_search", "stb_ivfpq_search_dev", "stb_hits_merge_dev", "stb_hits_merge_batch_dev", "stb_hits_merge", "stb_fnv1a64", "stb_line_id", "stb_line_ids",
     "stb_ctx_counters", "stb_debug_ticket_check", "stb_debug_timestamps", "stb_debug_q4_refined", "stb_debug_coscan_offsets", "stb_debug_batch_gemm", "stb_debug_batch_params",
-    "stb_debug_batch_last",
+    "stb_debug_batch_last", "stb_debug_corpus_copy",
     "stb_debug_ivfpq_export",
     "stb_ivfpq_search_batch", "stb_ivfpq_search_batch_dev", "stb_debug_ivfpq_batch_last",
     "stb_ivfpq_search_filtered",
@@ -81,6 +82,9 @@ def lib() -> C.CDLL:
     L.stb_corpus_rows.argtypes = [vp, C.POINTER(u64)]
     L.stb_corpus_data_dev.argtypes = [vp, C.POINTER(vp)]
     L.stb_corpus_read.argtypes = [vp, u64, u64, vp]
+    L.stb_corpus_update.argtypes = [vp, vp, vp, u64]
+    L.stb_corpus_remove.argtypes = [vp, vp, u32]
+    L.stb_debug_corpus_copy.argtypes = [vp, i32, u64, u64, vp, C.POINTER(u64)]
     L.stb_embed.argtypes = [vp, vp, vp, vp, u64, vp, vp]
     L.stb_embed_dev.argtypes = [vp, vp, vp, vp, u64, vp]
     L.stb_embed_status.argtypes = [vp]
@@ -321,6 +325,39 @@ class Corpus:
         out = np.empty((n, STB_DIM), dtype=np.float32)
         _check(lib().stb_corpus_read(self._h, first, n, _np_ptr(out)))
         return out
+
+    def update(self, idx, rows):
+        """stb_corpus_update: rows[i] replaces global row idx[i] (idx strictly ascending); the candidate
+        copies that exist are re-encoded at those rows and stay built."""
+        idx = np.ascontiguousarray(idx, dtype=np.uint64).reshape(-1)
+        rows = np.ascontiguousarray(rows, dtype=np.float32).reshape(-1, STB_DIM)
+        if rows.shape[0] != idx.size:
+            raise StbError(STB_ERR_ARG, f"{idx.size} row ids for {rows.shape[0]} rows")
+        if idx.size:
+            _check(lib().stb_corpus_update(self._h, _np_ptr(idx), _np_ptr(rows), idx.size))
+
+    def remove(self, ranges):
+        """stb_corpus_remove: delete the global rows of (n, 2) half-open [begin, end) ranges (ascending,
+        disjoint, non-empty); later rows move down in order, the candidate copies follow them."""
+        rr = np.ascontiguousarray(ranges, dtype=np.uint64).reshape(-1, 2)
+        if rr.shape[0]:
+            _check(lib().stb_corpus_remove(self._h, _np_ptr(rr), rr.shape[0]))
+
+    def debug_copy(self, which: int, first: int = 0, n: int | None = None):
+        """stb_debug_corpus_copy: (entries [first, first+n) of one candidate copy, rows the copy covers).
+        which: STB_COPY_Q8_CODES / _Q8_SCALES / _Q8_PLANE / _Q8_SR (entries are rows) or STB_COPY_H16_TILES
+        (entries are 256-row tiles of 131072 bytes); n=None: every covered entry from `first` on."""
+        covered = u64(0)
+        _check(lib().stb_debug_corpus_copy(self._h, which, 0, 0, None, C.byref(covered)))
+        cov = int(covered.value)
+        units = (cov + 255) // 256 if which == STB_COPY_H16_TILES else cov
+        n = units - first if n is None else n
+        shape, dtype = {STB_COPY_Q8_CODES: ((n, 256), np.int8), STB_COPY_Q8_SCALES: ((n,), np.float32),
+                        STB_COPY_Q8_PLANE: ((n, 128), np.uint8), STB_COPY_Q8_SR: ((n, 2), np.float32),
+                        STB_COPY_H16_TILES: ((n, 131072), np.uint8)}[which]
+        out = np.zeros(shape, dtype=dtype)
+        _check(lib().stb_debug_corpus_copy(self._h, which, first, n, _np_ptr(out) if n else None, C.byref(covered)))
+        return out, cov
 
     # -- K1 + K4 -------------------------------------------------------------
     def search(self, q, top_k: int = 3, max_distance: float | None = None,

@@ -58,6 +58,16 @@ static int dev_reserve(T **p, size_t *cap, size_t need, size_t floor_cap = 0) {
   return STB_OK;
 }
 
+bool stb_ranges_ordered(const uint64_t *ranges, uint32_t n) {
+  uint64_t prev_end = 0;
+  for (uint32_t i = 0; i < n; ++i) {
+    const uint64_t b = ranges[2 * i], e = ranges[2 * i + 1];
+    if (e < b || (i > 0 && b < prev_end)) return false;
+    prev_end = e;
+  }
+  return true;
+}
+
 extern "C" {
 
 int stb_version(void) { return 100; }
@@ -154,6 +164,7 @@ int stb_ctx_destroy(stb_ctx *c) {
   cudaFree(c->dbg_dev); cudaFree(c->hist_dev); cudaFree(c->bq_tiles); cudaFree(c->b_submax); cudaFree(c->b_tilemax); cudaFree(c->b_cand);
   cudaFree(c->b_thr); cudaFree(c->b_cnt); cudaFree(c->b_keys); cudaFree(c->b_qbad);
   cudaFree(c->bq_dev); cudaFree(c->bh_dev); cudaFree(c->bs_dev); cudaFree(c->embed_off_dev); cudaFree(c->embed_ids_dev); cudaFree(c->embed_out_dev);
+  cudaFree(c->mut_stage); cudaFree(c->mut_idx); cudaFree(c->mut_flags);
   if (c->q_pin) cudaFreeHost(c->q_pin);
   if (c->hits_pin) cudaFreeHost(c->hits_pin);
   if (c->status_pin) cudaFreeHost(c->status_pin);
@@ -350,9 +361,14 @@ int stb_corpus_destroy(stb_corpus *c) {
 
 // The reduced-width copies (K2 shadow, K1 tiers) cover a PREFIX of the rows: an append leaves the
 // prefix valid and the next query / prepare only converts the new rows (q8_rows / shadow_rows < n);
-// anything else (clear) drops them and starts a new epoch.
-static void corpus_changed(stb_corpus *c, bool appended_only = false) {
-  if (!appended_only) { c->shadow_rows = 0; c->q8_rows = 0; ++c->epoch; }
+// an update or a removal re-encodes the copies at the rows it writes, so they stay built; a clear drops
+// them.  Anything but an append starts a new epoch; an update or a removal also ends a co-scan series on
+// the corpus (the next asynchronous top-k query starts at tile 0).
+enum CorpusChange { CORPUS_APPEND, CORPUS_ROWS_REWRITTEN, CORPUS_CLEAR };
+static void corpus_changed(stb_corpus *c, CorpusChange kind) {
+  if (kind == CORPUS_CLEAR) { c->shadow_rows = 0; c->q8_rows = 0; }
+  if (kind != CORPUS_APPEND) ++c->epoch;
+  if (kind == CORPUS_ROWS_REWRITTEN && c->ctx->coscan_prev.corpus == c) c->ctx->coscan_prev.corpus = nullptr;
   c->searches_since_change = 0;
   memset(c->tier_tries, 0, sizeof(c->tier_tries));
   memset(c->tier_proven, 0, sizeof(c->tier_proven));
@@ -368,7 +384,7 @@ static int corpus_append_impl(stb_corpus *c, const float *rows, uint64_t n, cuda
   STB_CUDA(cudaMemcpyAsync(c->rows + c->n * STB_D, rows, n * STB_D * sizeof(float), kind, c->ctx->stream));
   STB_CUDA(cudaStreamSynchronize(c->ctx->stream));
   c->n += n;
-  corpus_changed(c, true);
+  corpus_changed(c, CORPUS_APPEND);
   return STB_OK;
 }
 
@@ -382,7 +398,7 @@ int stb_corpus_clear(stb_corpus *c) {
   if (!c) { stb_set_error("null corpus"); return STB_ERR_ARG; }
   if (!ctx_alive(c->ctx)) { stb_set_error("context was destroyed"); return STB_ERR_STATE; }
   c->n = 0;
-  corpus_changed(c);
+  corpus_changed(c, CORPUS_CLEAR);
   return STB_OK;
 }
 int stb_corpus_rows(const stb_corpus *c, uint64_t *n) {
@@ -440,7 +456,7 @@ int stb_embed(stb_ctx *ctx, const stb_table *table, const uint64_t *offsets, con
   if (out) STB_CUDA(cudaMemcpyAsync(out, dst, n_lines * STB_D * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
   STB_CUDA(cudaStreamSynchronize(ctx->stream));
   if (flag) { stb_set_error("embed: a token id maps outside the %llu-row table", (unsigned long long)table->V); return STB_ERR_RANGE; }
-  if (append_to) { append_to->n += n_lines; corpus_changed(append_to, true); }
+  if (append_to) { append_to->n += n_lines; corpus_changed(append_to, CORPUS_APPEND); }
   return STB_OK;
 }
 
@@ -564,14 +580,13 @@ int stb_search(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t 
   uint32_t n_loc = 0;
   uint64_t n_virtual = corpus->n;
   if (row_ranges) {
+    if (!stb_ranges_ordered(row_ranges, n_ranges)) { stb_set_error("search: row_ranges must be ascending, disjoint, half-open"); return STB_ERR_RANGE; }
     std::vector<uint64_t> vstart, rbegin;
     vstart.reserve(n_ranges + 1); rbegin.reserve(n_ranges);
-    uint64_t acc = 0, prev_end = 0;
+    uint64_t acc = 0;
     const uint64_t lo = corpus->row_base, hi = corpus->row_base + corpus->n;
     for (uint32_t i = 0; i < n_ranges; ++i) {
       uint64_t b = row_ranges[2 * i], e = row_ranges[2 * i + 1];
-      if (e < b || (i > 0 && b < prev_end)) { stb_set_error("search: row_ranges must be ascending, disjoint, half-open"); return STB_ERR_RANGE; }
-      prev_end = e;
       b = std::max(b, lo); e = std::min(e, hi);
       if (b >= e) continue;
       vstart.push_back(acc); rbegin.push_back(b - lo);
@@ -1011,6 +1026,176 @@ int stb_corpus_tier_stats(const stb_corpus *corpus, uint32_t tries[3], uint32_t 
     built_rows[STB_TIER_H16] = (corpus->shadow && !corpus->shadow_bad) ? corpus->shadow_rows : 0;   // < n after an append: a valid prefix
     built_rows[STB_TIER_Q8] = (corpus->q8 && !corpus->q8_bad) ? corpus->q8_rows : 0;
   }
+  return STB_OK;
+}
+
+// ------------------------------------------------------------- in-place mutations ---
+// stb_corpus_update / stb_corpus_remove (kernels: corpus_update.cu).  Validation comes first: a refused
+// call writes nothing.  A copy already marked bad is dropped (its flag is recomputed by the next build);
+// the others stay built and are re-encoded at every row the call writes inside their prefix.
+static int corpus_mutation_check(stb_corpus *c, const char *what) {
+  if (c->ivfpq_live) {
+    stb_set_error("%s: %u IVF-PQ index(es) on this corpus refer to its rows; destroy them first", what, c->ivfpq_live);
+    return STB_ERR_STATE;
+  }
+  return STB_OK;
+}
+
+static void corpus_drop_bad_copies(stb_corpus *c) {
+  if (c->q8_bad) { c->q8_rows = 0; c->q8_bad = 0; }
+  if (c->shadow_bad) { c->shadow_rows = 0; c->shadow_bad = 0; }
+}
+
+static StbCorpusWriteArgs corpus_write_args(stb_corpus *c, uint64_t q8_rows, uint64_t shadow_rows) {
+  StbCorpusWriteArgs a;
+  memset(&a, 0, sizeof(a));
+  a.rows = reinterpret_cast<float4 *>(c->rows);
+  a.stage = reinterpret_cast<const float4 *>(c->ctx->mut_stage);
+  a.q8 = c->q8; a.q8_scale = c->q8_scale; a.q4 = c->q4; a.q4_sr = c->q4_sr;
+  a.q8_rows = c->q8 ? q8_rows : 0;
+  a.shadow = c->shadow;
+  a.shadow_rows = c->shadow ? shadow_rows : 0;
+  a.flags = c->ctx->mut_flags;
+  return a;
+}
+
+// reads the bad-row flags the call's kernels raised (synchronises) and books the change
+static int corpus_mutation_finish(stb_corpus *c) {
+  stb_ctx *ctx = c->ctx;
+  int flags[2] = {0, 0};
+  STB_CUDA(cudaMemcpyAsync(flags, ctx->mut_flags, sizeof(flags), cudaMemcpyDeviceToHost, ctx->stream));
+  STB_CUDA(cudaStreamSynchronize(ctx->stream));
+  if (flags[0]) c->q8_bad = 1;
+  if (flags[1]) c->shadow_bad = 1;
+  corpus_changed(c, CORPUS_ROWS_REWRITTEN);
+  return STB_OK;
+}
+
+int stb_corpus_update(stb_corpus *c, const uint64_t *idx, const float *rows, uint64_t n) {
+  if (!c) { stb_set_error("null corpus"); return STB_ERR_ARG; }
+  int rc = ctx_use(c->ctx);
+  if (rc) return rc;
+  if (n == 0) return STB_OK;
+  if (!idx || !rows) { stb_set_error("corpus_update: null argument"); return STB_ERR_ARG; }
+  if ((rc = corpus_mutation_check(c, "corpus_update")) != STB_OK) return rc;
+  for (uint64_t i = 0; i < n; ++i) {
+    if (idx[i] < c->row_base || idx[i] - c->row_base >= c->n || (i > 0 && idx[i] <= idx[i - 1])) {
+      stb_set_error("corpus_update: idx[%llu] = %llu is out of order or outside rows [%llu, %llu)", (unsigned long long)i,
+                    (unsigned long long)idx[i], (unsigned long long)c->row_base, (unsigned long long)(c->row_base + c->n));
+      return STB_ERR_RANGE;
+    }
+  }
+  stb_ctx *ctx = c->ctx;
+  const uint64_t chunk = std::min<uint64_t>(n, STB_MUT_CHUNK_ROWS);
+  if ((rc = dev_reserve(&ctx->mut_stage, &ctx->mut_stage_cap, chunk * STB_D)) != STB_OK) return rc;
+  if ((rc = dev_reserve(&ctx->mut_idx, &ctx->mut_idx_cap, chunk)) != STB_OK) return rc;
+  if ((rc = dev_reserve(&ctx->mut_flags, &ctx->mut_flags_cap, 2)) != STB_OK) return rc;
+  corpus_drop_bad_copies(c);
+  STB_CUDA(cudaMemsetAsync(ctx->mut_flags, 0, 2 * sizeof(int), ctx->stream));
+  StbCorpusWriteArgs a = corpus_write_args(c, c->q8_rows, c->shadow_rows);
+  a.idx = ctx->mut_idx;
+  std::vector<uint64_t> local(chunk);
+  for (uint64_t i0 = 0; i0 < n; i0 += chunk) {
+    a.m = std::min(chunk, n - i0);
+    for (uint64_t i = 0; i < a.m; ++i) local[i] = idx[i0 + i] - c->row_base;
+    // the previous chunk's kernel reads the staging buffers: stream order keeps these copies behind it
+    STB_CUDA(cudaMemcpyAsync(ctx->mut_idx, local.data(), a.m * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->stream));
+    STB_CUDA(cudaMemcpyAsync(ctx->mut_stage, rows + i0 * STB_D, a.m * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    if ((rc = stb_launch_corpus_write(ctx, a)) != STB_OK) return rc;
+    if (i0 + chunk < n) STB_CUDA(cudaStreamSynchronize(ctx->stream));   // `local` is refilled next
+  }
+  return corpus_mutation_finish(c);
+}
+
+int stb_corpus_remove(stb_corpus *c, const uint64_t *ranges, uint32_t n_ranges) {
+  if (!c) { stb_set_error("null corpus"); return STB_ERR_ARG; }
+  int rc = ctx_use(c->ctx);
+  if (rc) return rc;
+  if (n_ranges == 0) return STB_OK;
+  if (!ranges) { stb_set_error("corpus_remove: ranges is null"); return STB_ERR_ARG; }
+  if ((rc = corpus_mutation_check(c, "corpus_remove")) != STB_OK) return rc;
+  if (!stb_ranges_ordered(ranges, n_ranges)) { stb_set_error("corpus_remove: ranges must be ascending, disjoint, half-open"); return STB_ERR_RANGE; }
+  const uint64_t lo = c->row_base, hi = c->row_base + c->n;
+  for (uint32_t i = 0; i < n_ranges; ++i)
+    if (!(ranges[2 * i] < ranges[2 * i + 1]) || ranges[2 * i] < lo || ranges[2 * i + 1] > hi) {
+      stb_set_error("corpus_remove: range %u [%llu, %llu) is empty or outside rows [%llu, %llu)", i, (unsigned long long)ranges[2 * i],
+                    (unsigned long long)ranges[2 * i + 1], (unsigned long long)lo, (unsigned long long)hi);
+      return STB_ERR_RANGE;
+    }
+  stb_ctx *ctx = c->ctx;
+  // kept segments behind the first removed row, as {destination, source} local rows; removed rows inside the
+  // prefix each copy covers (a copy marked bad is dropped below: it covers none)
+  std::vector<uint64_t> seg;
+  const uint64_t q8_had = c->q8_bad ? 0 : c->q8_rows, shadow_had = c->shadow_bad ? 0 : c->shadow_rows;
+  uint64_t removed = 0, removed_q8 = 0, removed_shadow = 0;
+  const uint64_t first = ranges[0] - lo;
+  uint64_t dst = first;
+  for (uint32_t i = 0; i < n_ranges; ++i) {
+    const uint64_t b = ranges[2 * i] - lo, e = ranges[2 * i + 1] - lo;
+    const uint64_t next = (i + 1 < n_ranges) ? ranges[2 * i + 2] - lo : c->n;
+    removed += e - b;
+    if (q8_had > b) removed_q8 += std::min(e, q8_had) - b;
+    if (shadow_had > b) removed_shadow += std::min(e, shadow_had) - b;
+    if (next > e) { seg.push_back(dst); seg.push_back(e); dst += next - e; }
+  }
+  const uint64_t moved = dst - first;
+  const uint64_t q8_rows = q8_had - removed_q8, shadow_rows = shadow_had - removed_shadow;
+  if ((rc = dev_reserve(&ctx->mut_flags, &ctx->mut_flags_cap, 2)) != STB_OK) return rc;
+  if (moved) {
+    const uint64_t chunk = std::min<uint64_t>(moved, STB_MUT_CHUNK_ROWS);
+    if ((rc = dev_reserve(&ctx->mut_stage, &ctx->mut_stage_cap, chunk * STB_D)) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->mut_idx, &ctx->mut_idx_cap, seg.size())) != STB_OK) return rc;
+  }
+  corpus_drop_bad_copies(c);
+  STB_CUDA(cudaMemsetAsync(ctx->mut_flags, 0, 2 * sizeof(int), ctx->stream));
+  if (moved) {
+    // Chunks in output order.  The sources of a chunk lie at or beyond its own output rows, so the gather
+    // reads rows no earlier chunk has overwritten, and it completes before the commit writes.
+    STB_CUDA(cudaMemcpyAsync(ctx->mut_idx, seg.data(), seg.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->stream));
+    const uint32_t n_seg = (uint32_t)(seg.size() / 2);
+    StbCorpusWriteArgs a = corpus_write_args(c, q8_rows, shadow_rows);
+    for (uint64_t d0 = first; d0 < first + moved; d0 += STB_MUT_CHUNK_ROWS) {
+      a.first = d0;
+      a.m = std::min<uint64_t>(STB_MUT_CHUNK_ROWS, first + moved - d0);
+      if ((rc = stb_launch_corpus_gather(ctx, c->rows, ctx->mut_idx, n_seg, a.first, a.m, ctx->mut_stage)) != STB_OK) return rc;
+      if ((rc = stb_launch_corpus_write(ctx, a)) != STB_OK) return rc;
+    }
+    STB_CUDA(cudaStreamSynchronize(ctx->stream));   // `seg` dies at scope end
+  }
+  // the shadow's last covered tile ends in zero padding, as a build of `shadow_rows` rows leaves it
+  if (c->shadow && shadow_rows % 256 &&
+      (rc = stb_launch_shadow_build(ctx, c->rows, shadow_rows, 256, c->shadow, ctx->mut_flags + 1, shadow_rows)) != STB_OK) return rc;
+  c->n -= removed;
+  c->q8_rows = q8_rows;
+  c->shadow_rows = shadow_rows;
+  return corpus_mutation_finish(c);
+}
+
+int stb_debug_corpus_copy(const stb_corpus *c, int which, uint64_t first, uint64_t n, void *out, uint64_t *covered) {
+  if (!c || (n && !out)) { stb_set_error("debug_corpus_copy: null argument"); return STB_ERR_ARG; }
+  int rc = ctx_use(c->ctx);
+  if (rc) return rc;
+  const void *src = nullptr;
+  size_t unit = 0;
+  uint64_t rows = c->q8 ? c->q8_rows : 0, units = rows;
+  switch (which) {
+    case STB_COPY_Q8_CODES: src = c->q8; unit = 256; break;
+    case STB_COPY_Q8_SCALES: src = c->q8_scale; unit = sizeof(float); break;
+    case STB_COPY_Q8_PLANE: src = c->q4; unit = 128; break;
+    case STB_COPY_Q8_SR: src = c->q4_sr; unit = sizeof(float2); break;
+    case STB_COPY_H16_TILES:
+      src = c->shadow; unit = 131072; rows = c->shadow ? c->shadow_rows : 0; units = (rows + 255) / 256; break;
+    default: stb_set_error("debug_corpus_copy: unknown copy %d", which); return STB_ERR_ARG;
+  }
+  if (covered) *covered = rows;
+  if (first > units || n > units - first) {
+    stb_set_error("debug_corpus_copy: [%llu, +%llu) outside the %llu the copy covers", (unsigned long long)first,
+                  (unsigned long long)n, (unsigned long long)units);
+    return STB_ERR_RANGE;
+  }
+  if (n == 0) return STB_OK;
+  STB_CUDA(cudaMemcpyAsync(out, (const uint8_t *)src + first * unit, n * unit, cudaMemcpyDeviceToHost, c->ctx->stream));
+  STB_CUDA(cudaStreamSynchronize(c->ctx->stream));
   return STB_OK;
 }
 

@@ -33,6 +33,7 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "row_encode.cuh"
 
 #define STB_B_TILE 256            // corpus rows per tile  (MMA N)
 #define STB_A_TILE 128            // queries per tile      (MMA M, two m64 warpgroups)
@@ -154,9 +155,8 @@ __device__ __forceinline__ uint64_t wg_desc_sw128(uint32_t smem_addr) {
 }
 
 // --------------------------------------------------------------- 1. shadow builder ---
-// One warp per row; lane l owns k = 8l..8l+7 = one 16-byte bf16 chunk (slab l/8, chunk
-// l%8).  Tile layout: tile t -> 4 slabs -> [TILE rows x 128 B], 8-row x 128-B atoms with
-// the 16-byte chunk index XOR-ed by (row % 8)  (the hardware 128B swizzle).
+// One warp per row; lane l owns k = 8l..8l+7 = one 16-byte chunk (row_encode.cuh: stb_shadow_pack_row,
+// stb_shadow_offset).  Rows [n_rows, n_padded) are the zero padding of the last tile.
 template <int TILE>
 __global__ void __launch_bounds__(256)
 stb_shadow_build_kernel(const float4 *__restrict__ rows, uint64_t first_row, uint64_t n_rows, uint64_t n_padded,
@@ -169,45 +169,10 @@ stb_shadow_build_kernel(const float4 *__restrict__ rows, uint64_t first_row, uin
     v0 = __ldg(rows + row * STB_ROW_F4 + 2 * lane);
     v1 = __ldg(rows + row * STB_ROW_F4 + 2 * lane + 1);
   }
-  float ss = v0.x * v0.x + v0.y * v0.y + v0.z * v0.z + v0.w * v0.w + v1.x * v1.x + v1.y * v1.y +
-             v1.z * v1.z + v1.w * v1.w;
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, off);
-  float inv = 0.f;
-  bool bad = false;
-  if (ss != 0.f) {
-    if (!(ss >= 1e-30f && ss <= 1e30f)) bad = true;   // NaN/inf/extreme
-    else inv = rsqrtf(ss);
-  } else {
-    // fp32 underflow of a tiny non-zero row: cannot be normalised here -> batch path unusable
-    bool nz = (v0.x != 0.f) | (v0.y != 0.f) | (v0.z != 0.f) | (v0.w != 0.f) | (v1.x != 0.f) | (v1.y != 0.f) |
-              (v1.z != 0.f) | (v1.w != 0.f);
-    bad = __any_sync(0xffffffffu, nz);
-  }
-  if (bad && lane == 0) atomicExch(bad_flag, 1);
-  // per-row record (query tiles): a row that cannot be normalised is scaled by 0 (NaN where a component is
-  // NaN or infinite), so its approximate scores bound nothing; the finish kernels mark it unproven
-  if (row_bad && lane == 0) row_bad[row] = bad ? 1u : 0u;
-#if STB_SHADOW_F16
-  __half2 p0 = __floats2half2_rn(v0.x * inv, v0.y * inv);
-  __half2 p1 = __floats2half2_rn(v0.z * inv, v0.w * inv);
-  __half2 p2 = __floats2half2_rn(v1.x * inv, v1.y * inv);
-  __half2 p3 = __floats2half2_rn(v1.z * inv, v1.w * inv);
-#else
-  __nv_bfloat162 p0 = __floats2bfloat162_rn(v0.x * inv, v0.y * inv);
-  __nv_bfloat162 p1 = __floats2bfloat162_rn(v0.z * inv, v0.w * inv);
-  __nv_bfloat162 p2 = __floats2bfloat162_rn(v1.x * inv, v1.y * inv);
-  __nv_bfloat162 p3 = __floats2bfloat162_rn(v1.z * inv, v1.w * inv);
-#endif
-  uint4 pk;
-  pk.x = *reinterpret_cast<uint32_t *>(&p0); pk.y = *reinterpret_cast<uint32_t *>(&p1);
-  pk.z = *reinterpret_cast<uint32_t *>(&p2); pk.w = *reinterpret_cast<uint32_t *>(&p3);
-  const uint64_t tile = row / TILE;
-  const uint32_t r = (uint32_t)(row % TILE);
-  const uint32_t slab = lane >> 3, chunk = lane & 7;
-  const size_t off = tile * (size_t)(TILE * 512) + (size_t)slab * (TILE * 128) + (size_t)(r >> 3) * 1024 +
-                     (size_t)(r & 7) * 128 + (size_t)((chunk ^ (r & 7)) * 16);
-  *reinterpret_cast<uint4 *>(out + off) = pk;
+  // per-row record (query tiles): a row that cannot be normalised bounds nothing; the finish kernels mark
+  // it unproven
+  const uint4 pk = stb_shadow_pack_row(v0, v1, lane, row, bad_flag, row_bad);
+  *reinterpret_cast<uint4 *>(out + stb_shadow_offset<TILE>(row, lane)) = pk;
 }
 
 // ------------------------------------------------------------------- 2. wgmma GEMM ---

@@ -141,6 +141,11 @@ struct stb_ctx {
   size_t embed_ids_cap;
   float *embed_out_dev;     // K3 output when not appending to a corpus
   size_t embed_out_cap;
+  // in-place corpus mutations (stb_corpus_update / _remove): row staging (<= STB_MUT_CHUNK_ROWS rows),
+  // row ids or kept-segment table, and the q8 / shadow bad-row flags
+  float *mut_stage; size_t mut_stage_cap;
+  uint64_t *mut_idx; size_t mut_idx_cap;
+  int *mut_flags; size_t mut_flags_cap;
   // --- pinned host staging ---
   float *q_pin;
   stb_hit *hits_pin;
@@ -221,7 +226,29 @@ struct stb_corpus {
   // results on this corpus (index = STB_TIER_*)
   uint32_t tier_tries[3], tier_proven[3];
   uint32_t searches_since_change;   // lazy builds wait for the second query on an unchanged corpus
+  uint32_t ivfpq_live;       // IVF-PQ indexes built on this corpus and not yet destroyed: update / remove refuse
 };
+
+// Row ranges as stb_search takes them: n half-open [begin, end) pairs, ascending and disjoint (api.cu).
+bool stb_ranges_ordered(const uint64_t *ranges, uint32_t n);
+
+// ---- corpus_update.cu -----------------------------------------------------------------------
+#define STB_MUT_CHUNK_ROWS 262144   // staging rows of an update / removal chunk: 256 MiB of f32 at most
+struct StbCorpusWriteArgs {
+  float4 *rows;
+  const float4 *stage;        // m staged rows
+  const uint64_t *idx;        // local destination of staged row i, or null: first + i
+  uint64_t first, m;
+  uint8_t *q8; float *q8_scale; uint8_t *q4; float2 *q4_sr;
+  uint64_t q8_rows;           // rows the q8 copy covers (0: none)
+  uint8_t *shadow;
+  uint64_t shadow_rows;       // rows the 16-bit shadow covers (0: none)
+  int *flags;                 // [0] a written q8 row cannot be normalised, [1] the same for the shadow
+};
+int stb_launch_corpus_write(stb_ctx *ctx, const StbCorpusWriteArgs &a);
+// staging row i <- the row that lands at local row first + i once the removed rows are gone
+int stb_launch_corpus_gather(stb_ctx *ctx, const float *rows, const uint64_t *seg_dev, uint32_t n_seg, uint64_t first,
+                             uint64_t m, float *stage);
 
 // ---- scan_topk.cu -------------------------------------------------------------
 // Fast path: one kernel = scan + per-warp running top-K' + CTA/tree merge +

@@ -1236,6 +1236,7 @@ extern "C" {
 
 int stb_ivfpq_destroy(stb_ivfpq *x) {
   if (!x) return STB_OK;
+  const_cast<stb_corpus *>(x->corpus)->ivfpq_live--;
   cudaFree(x->centroids); cudaFree(x->codebooks); cudaFree(x->codes); cudaFree(x->order); cudaFree(x->list_off);
   cudaFree(x->coarse); cudaFree(x->lut); cudaFree(x->probe); cudaFree(x->cand); cudaFree(x->cand_rows);
   cudaFree(x->keys2); cudaFree(x->tickets); cudaFree(x->forced);
@@ -1269,6 +1270,9 @@ int stb_ivfpq_build(stb_ctx *ctx, const stb_corpus *corpus, uint32_t nlist, uint
   stb_ivfpq *x = new (std::nothrow) stb_ivfpq();
   if (!x) { stb_set_error("out of host memory"); return STB_ERR_NOMEM; }
   x->ctx = ctx; x->corpus = corpus; x->corpus_epoch = corpus->epoch; x->nlist = nlist; x->n = 0;
+  // counted from here: every failure below ends in stb_ivfpq_destroy, which takes the count back, so only a
+  // built index holds it (stb_corpus_update / stb_corpus_remove refuse while it does)
+  const_cast<stb_corpus *>(corpus)->ivfpq_live++;
   x->centroids = nullptr; x->codebooks = nullptr; x->codes = nullptr; x->order = nullptr; x->list_off = nullptr;
   x->coarse = nullptr; x->lut = nullptr; x->probe = nullptr; x->cand = nullptr; x->cand_cap = 0; x->cand_rows = nullptr;
   x->keys2 = nullptr; x->tickets = nullptr; x->forced = nullptr; x->n_forced = 0;
@@ -1570,16 +1574,14 @@ int stb_ivfpq_search_filtered(stb_ivfpq *x, const float *q, uint32_t nq, uint32_
   // global ranges -> local [begin, end) pairs clipped to the indexed rows [row_base, row_base + n)
   std::vector<uint32_t> loc;
   if (row_ranges) {
+    if (!stb_ranges_ordered(row_ranges, n_ranges)) {
+      stb_set_error("ivfpq_search_filtered: row_ranges must be ascending, disjoint, half-open");
+      return STB_ERR_RANGE;
+    }
     const uint64_t lo = x->corpus->row_base, hi = lo + x->n;
-    uint64_t prev_end = 0;
     loc.reserve(2 * (size_t)n_ranges);
     for (uint32_t i = 0; i < n_ranges; ++i) {
       uint64_t b = row_ranges[2 * i], e = row_ranges[2 * i + 1];
-      if (e < b || (i > 0 && b < prev_end)) {
-        stb_set_error("ivfpq_search_filtered: row_ranges must be ascending, disjoint, half-open");
-        return STB_ERR_RANGE;
-      }
-      prev_end = e;
       b = std::max(b, lo); e = std::min(e, hi);
       if (b >= e) continue;
       loc.push_back((uint32_t)(b - lo)); loc.push_back((uint32_t)(e - lo));

@@ -26,6 +26,7 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "row_encode.cuh"
 
 #ifndef STB_SCAN_U
 #define STB_SCAN_U 2   // rows per 8-lane group per iteration (loads in flight = 8*U float4)
@@ -706,10 +707,8 @@ __device__ __forceinline__ void stb_scan_q4(const ScanArgs &args, const uint8_t 
   if (lane == 0 && refined) atomicAdd(q4a.refined, (unsigned long long)refined);
 }
 
-// q8 builder: one warp per row; lane l owns elements 8l .. 8l+7.  Rows whose fp32 squared norm
-// is not a normal number set *bad_flag (the tier is then refused for this corpus, like the
-// 16-bit shadow); true zero rows get scale 0 and all-zero codes (score = the query's slack).
-// The same pass writes the nibble plane and {s, rho} of the top-k scan's prefilter (stb_scan_q4).
+// q8 builder: one warp per row (row_encode.cuh: stb_q8_encode_row).  The same pass writes the nibble
+// plane and {s, rho} of the top-k scan's prefilter (stb_scan_q4).
 __global__ void __launch_bounds__(256)
 stb_q8_build_kernel(const float4 *__restrict__ rows, uint64_t first_row, uint64_t n_rows, uint8_t *__restrict__ out,
                     float *__restrict__ scale, uint8_t *__restrict__ plane, float2 *__restrict__ sr, int *bad_flag) {
@@ -718,55 +717,7 @@ stb_q8_build_kernel(const float4 *__restrict__ rows, uint64_t first_row, uint64_
   if (row >= n_rows) return;
   const float4 v0 = __ldg(rows + row * STB_ROW_F4 + 2 * lane);
   const float4 v1 = __ldg(rows + row * STB_ROW_F4 + 2 * lane + 1);
-  float ss = v0.x * v0.x + v0.y * v0.y + v0.z * v0.z + v0.w * v0.w + v1.x * v1.x + v1.y * v1.y + v1.z * v1.z + v1.w * v1.w;
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, off);
-  float inv = 0.f;
-  if (ss != 0.f) {
-    if (!(ss >= 1e-30f && ss <= 1e30f)) { if (lane == 0) atomicExch(bad_flag, 1); }   // NaN/inf/extreme
-    else inv = rsqrtf(ss);
-  } else {
-    const bool nz = (v0.x != 0.f) | (v0.y != 0.f) | (v0.z != 0.f) | (v0.w != 0.f) | (v1.x != 0.f) | (v1.y != 0.f) |
-                    (v1.z != 0.f) | (v1.w != 0.f);
-    if (__any_sync(0xffffffffu, nz) && lane == 0) atomicExch(bad_flag, 1);             // underflowed tiny row
-  }
-  const float x[8] = {v0.x * inv, v0.y * inv, v0.z * inv, v0.w * inv, v1.x * inv, v1.y * inv, v1.z * inv, v1.w * inv};
-  float am = 0.f;
-#pragma unroll
-  for (int e = 0; e < 8; ++e) am = fmaxf(am, fabsf(x[e]));
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) am = fmaxf(am, __shfl_xor_sync(0xffffffffu, am, off));
-  const float s = am * (1.0f / 127.0f);
-  const float inv_s = am > 0.f ? 127.0f / am : 0.f;
-  uint32_t w0 = 0, w1 = 0, n0 = 0, n1 = 0;
-  float r2 = 0.f;
-#pragma unroll
-  for (int e = 0; e < 4; ++e) {
-    const int c0 = max(-127, min(127, __float2int_rn(x[e] * inv_s)));
-    const int c1 = max(-127, min(127, __float2int_rn(x[4 + e] * inv_s)));
-    w0 |= (uint32_t)(c0 & 255) << (8 * e);
-    w1 |= (uint32_t)(c1 & 255) << (8 * e);
-    const int h0 = (c0 + 128) >> 4, h1 = (c1 + 128) >> 4;      // h + 8 in [0, 15]
-    n0 |= (uint32_t)h0 << (8 * e);
-    n1 |= (uint32_t)h1 << (8 * e);
-    // x^ - s (16 h + 7.5) with h = h0 - 8: the centre 16 h0 - 120.5 = (32 h0 - 241) / 2 is exact in fp32
-    const float d0 = x[e] - s * (0.5f * (float)(32 * h0 - 241));
-    const float d1 = x[4 + e] - s * (0.5f * (float)(32 * h1 - 241));
-    r2 = fmaf(d0, d0, fmaf(d1, d1, r2));
-  }
-  *reinterpret_cast<uint2 *>(out + row * 256 + (size_t)lane * 8) = make_uint2(w0, w1);
-  // plane: lane 4m + t holds components 32m + 8t .. +7; t < 2 are the low nibbles of bytes 16m + 8t ..,
-  // t >= 2 the high nibbles of the same bytes (from lane + 2)
-  const uint32_t p0 = __shfl_down_sync(0xffffffffu, n0, 2), p1 = __shfl_down_sync(0xffffffffu, n1, 2);
-  if ((lane & 2) == 0)
-    *reinterpret_cast<uint2 *>(plane + row * 128 + (size_t)(lane >> 2) * 16 + (size_t)(lane & 1) * 8) = make_uint2(n0 | (p0 << 4), n1 | (p1 << 4));
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) r2 += __shfl_xor_sync(0xffffffffu, r2, off);
-  if (lane == 0) {
-    scale[row] = s;
-    // rounded up: 1e-4 relative covers the fp32 evaluation of the 256 differences and their sum
-    sr[row] = make_float2(s, sqrtf(r2) * 1.0001f + 1e-6f);
-  }
+  stb_q8_encode_row(v0, v1, lane, row, out, scale, plane, sr, bad_flag);
 }
 
 int stb_launch_q8_build(stb_ctx *ctx, const float *rows_dev, uint64_t first_row, uint64_t n_rows, uint8_t *out,

@@ -408,6 +408,7 @@ class Store:
 
     def _apply_upsert_lines(self, line_embeddings) -> None:
         new_rows, new_emb = [], []
+        patched = {}                                                  # uploaded row -> its last vector of the batch
         for le in line_embeddings:
             emb = np.asarray(le.embedding, dtype=np.float32)
             if emb.shape != (LINE_EMBEDDING_SIZE,):
@@ -423,7 +424,8 @@ class Store:
                 self._emb[row] = emb                                  # upsert replaces by id
                 self._rows[row] = (pi, le.line_number)
                 self._dirty_rows.add(row)
-                self._corpus = None                                   # GPU mirror: re-upload (in-place change)
+                if row < self._corpus_n:
+                    patched[row] = emb
             elif row is not None:                                     # replaced inside this same batch
                 new_emb[row - len(self._emb)] = emb
             else:
@@ -433,7 +435,18 @@ class Store:
         if new_emb:
             self._emb = np.concatenate([self._emb, np.stack(new_emb)]) if len(self._emb) else np.stack(new_emb)
             self._rows = np.concatenate([self._rows, np.asarray(new_rows, dtype=np.int32).reshape(-1, 2)])
-        # appended rows reach the GPU mirror lazily
+        # the GPU mirror takes in-place patches of its rows now; appended rows reach it lazily
+        if patched and self._corpus is not None:
+            idx = np.fromiter(sorted(patched), dtype=np.uint64, count=len(patched))
+            self._mirror(lambda c: c.update(idx, np.stack([patched[int(r)] for r in idx])))
+
+    def _mirror(self, change) -> None:
+        """Apply one change to the GPU mirror; if the call fails the mirror is dropped and the next query
+        uploads the rows again."""
+        try:
+            change(self._corpus)
+        except capi.StbError:
+            self._corpus = None
 
     # -- store.rs:235-296: only metadata of the CURRENT embedding version is deleted
     def delete_document_metadata(self, paths) -> None:
@@ -454,11 +467,16 @@ class Store:
             kill = {self._path_idx[p] for p in paths if p in self._path_idx}
             if kill:
                 keep = ~np.isin(self._rows[:, 0], list(kill))
+                if self._corpus is not None:                          # the mirror drops the same rows in place
+                    gone = (~keep[: self._corpus_n]).astype(np.int8)
+                    ranges = np.flatnonzero(np.diff(np.concatenate([[0], gone, [0]]))).reshape(-1, 2).astype(np.uint64)
+                    if len(ranges):
+                        self._mirror(lambda c: c.remove(ranges))
+                        self._corpus_n -= int(gone.sum())
                 self._rows = self._rows[keep]
                 self._emb = np.ascontiguousarray(self._emb[keep])
                 ids = capi.line_ids(self._paths, self._rows) if len(self._rows) else []
                 self._id_row = {int(v): r for r, v in enumerate(ids)}
-                self._corpus = None
                 self._rewrite = True                                  # rows moved: a new generation of row files
         self._mutate(apply)
 
