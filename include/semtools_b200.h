@@ -310,7 +310,8 @@ int stb_search_batch_xchg_dev(stb_ctx *ctx, const stb_corpus *corpus, const floa
  * distances; only the candidate set is approximate.  The index covers rows [0, rows) of its
  * corpus (stb_ivfpq_stats): the rows present at the build and those stb_ivfpq_extend has added
  * since; rows appended after that are not searched until the next extend.  It must be destroyed
- * before its corpus; while it is alive stb_corpus_update and stb_corpus_remove refuse the corpus.
+ * before its corpus; while it is alive stb_corpus_update and stb_corpus_remove refuse the corpus
+ * (stb_ivfpq_update and stb_ivfpq_remove change the corpus and the index together).
  * Forced rows: rows with a non-finite component or an fp32 squared norm outside [1e-30, 1e30]
  * (K1's forced candidates) are kept out of training and of the inverted lists; every search
  * re-ranks them exactly besides the ADC candidates.  More than 1024 such rows: the build fails
@@ -339,6 +340,39 @@ int stb_ivfpq_destroy(stb_ivfpq *index);
  * extends give the lists one extend of both parts gives.  Cost: the new rows' assignment and encoding
  * plus one copy of the lists (36 B per row); extra memory while it runs: that copy and 48 B per new row. */
 int stb_ivfpq_extend(stb_ivfpq *index, uint64_t *out_added);
+/* Replace and delete rows of the index's corpus and keep the index current, without retraining.
+ * stb_ivfpq_update / stb_ivfpq_remove apply stb_corpus_update / stb_corpus_remove to the index's corpus:
+ * the arguments, their validation, the error codes, the chunking, the maintained q8 and 16-bit copies, the
+ * new epoch, the reset of the tier statistics and the end of a co-scan series are exactly those calls'.
+ * Instead of refusing a corpus with a live index they refuse (STB_ERR_STATE, nothing written):
+ *  - another live index on the same corpus;
+ *  - a corpus cleared since the index last read it (as stb_ivfpq_extend);
+ *  - a call that would leave more than 1024 forced rows.
+ * After success:
+ *  - Centroids and codebooks are the same bits: nothing is retrained.
+ *  - A removed indexed row leaves its list or the forced list; every entry behind it is renumbered (row
+ *    minus the removed rows below it).  stb_ivfpq_stats' rows drops by the removed rows that were indexed.
+ *  - A replaced indexed row gets the list and code the build would give its new value (a copy of another
+ *    indexed row: that row's list and code, bit for bit); it may move between a list and the forced list.
+ *  - Every list and the forced list stay in ascending row order.  The index is therefore a function of the
+ *    quantisers and the current rows: what the build's add phase with the same quantisers makes of rows
+ *    [0, indexed).  Any sequence of extend, update and remove calls that reaches the same rows reaches the
+ *    same index.
+ *  - Rows appended but not yet extended stay outside the index: updating them changes only the corpus,
+ *    removing them shortens that tail, and the next stb_ivfpq_extend indexes exactly the rows after the
+ *    indexed prefix.
+ *  - The index records the corpus's new epoch: extend and the searches keep working.
+ * Atomicity: on STB_ERR_ARG, STB_ERR_RANGE, STB_ERR_STATE or STB_ERR_NOMEM the corpus (rows and copies) and
+ * the index are byte for byte unchanged and the index stays usable.  Every buffer the index needs is
+ * allocated, and the replaced rows are encoded and the forced rows counted, before the corpus is written.
+ * The new rows are encoded from the corpus's staging buffer: an update of at most 262144 rows is uploaded
+ * once, a larger one twice (once to encode and count, once to write).
+ * Synchronous: searches enqueued before the call see the old rows and index, later ones the new.
+ * Cost, besides the corpus call's: the assignment and encoding of the replaced indexed rows and one pass
+ * over the lists (read and write, 36 B per entry).  Extra device memory while it runs: one copy of the lists,
+ * 48 B per replaced row, a bitmap of the indexed rows and 8 B per listed entry. */
+int stb_ivfpq_update(stb_ivfpq *index, const uint64_t *idx, const float *rows, uint64_t n);
+int stb_ivfpq_remove(stb_ivfpq *index, const uint64_t *ranges, uint32_t n_ranges);
 int stb_ivfpq_stats(const stb_ivfpq *index, uint64_t *rows, uint32_t *nlist, uint32_t *max_list,
                     uint64_t *index_bytes);
 int stb_ivfpq_search(stb_ivfpq *index, const float *q, uint32_t nprobe, uint32_t top_k,

@@ -32,7 +32,7 @@ SYMBOLS = [
     "stb_debug_batch_last", "stb_debug_corpus_copy",
     "stb_debug_ivfpq_export",
     "stb_ivfpq_search_batch", "stb_ivfpq_search_batch_dev", "stb_debug_ivfpq_batch_last",
-    "stb_ivfpq_search_filtered",
+    "stb_ivfpq_search_filtered", "stb_ivfpq_update", "stb_ivfpq_remove",
 ]
 
 
@@ -108,6 +108,8 @@ def lib() -> C.CDLL:
     L.stb_ivfpq_build.argtypes = [vp, vp, u32, u32, u32, C.POINTER(vp)]
     L.stb_ivfpq_destroy.argtypes = [vp]
     L.stb_ivfpq_extend.argtypes = [vp, C.POINTER(u64)]
+    L.stb_ivfpq_update.argtypes = [vp, vp, vp, u64]
+    L.stb_ivfpq_remove.argtypes = [vp, vp, u32]
     L.stb_ivfpq_stats.argtypes = [vp, C.POINTER(u64), C.POINTER(u32), C.POINTER(u32), C.POINTER(u64)]
     L.stb_ivfpq_search.argtypes = [vp, vp, u32, u32, u32, vp, C.POINTER(u32), C.POINTER(u64)]
     L.stb_ivfpq_search_dev.argtypes = [vp, vp, u32, u32, u32, vp, vp]
@@ -461,6 +463,23 @@ class IvfPq:
         added = u64(0)
         _check(lib().stb_ivfpq_extend(self._h, C.byref(added)))
         return int(added.value)
+
+    def update(self, idx, rows):
+        """stb_ivfpq_update: Corpus.update on the index's corpus, and the replaced indexed rows get the list
+        and code of their new value (same quantisers)."""
+        idx = np.ascontiguousarray(idx, dtype=np.uint64).reshape(-1)
+        rows = np.ascontiguousarray(rows, dtype=np.float32).reshape(-1, STB_DIM)
+        if rows.shape[0] != idx.size:
+            raise StbError(STB_ERR_ARG, f"{idx.size} row ids for {rows.shape[0]} rows")
+        if idx.size:
+            _check(lib().stb_ivfpq_update(self._h, _np_ptr(idx), _np_ptr(rows), idx.size))
+
+    def remove(self, ranges):
+        """stb_ivfpq_remove: Corpus.remove on the index's corpus; the removed rows leave the index and the
+        entries behind them are renumbered."""
+        rr = np.ascontiguousarray(ranges, dtype=np.uint64).reshape(-1, 2)
+        if rr.shape[0]:
+            _check(lib().stb_ivfpq_remove(self._h, _np_ptr(rr), rr.shape[0]))
 
     def stats(self):
         rows, nbytes, nlist, mx = u64(0), u64(0), u32(0), u32(0)

@@ -1071,16 +1071,19 @@ static int corpus_mutation_finish(stb_corpus *c) {
   return STB_OK;
 }
 
-int stb_corpus_update(stb_corpus *c, const uint64_t *idx, const float *rows, uint64_t n) {
+}  // extern "C"
+
+int stb_corpus_update_impl(stb_corpus *c, const uint64_t *idx, const float *rows, uint64_t n, const char *what,
+                           StbCorpusHook *hook) {
   if (!c) { stb_set_error("null corpus"); return STB_ERR_ARG; }
   int rc = ctx_use(c->ctx);
   if (rc) return rc;
   if (n == 0) return STB_OK;
-  if (!idx || !rows) { stb_set_error("corpus_update: null argument"); return STB_ERR_ARG; }
-  if ((rc = corpus_mutation_check(c, "corpus_update")) != STB_OK) return rc;
+  if (!idx || !rows) { stb_set_error("%s: null argument", what); return STB_ERR_ARG; }
+  if ((rc = hook ? hook->check() : corpus_mutation_check(c, what)) != STB_OK) return rc;
   for (uint64_t i = 0; i < n; ++i) {
     if (idx[i] < c->row_base || idx[i] - c->row_base >= c->n || (i > 0 && idx[i] <= idx[i - 1])) {
-      stb_set_error("corpus_update: idx[%llu] = %llu is out of order or outside rows [%llu, %llu)", (unsigned long long)i,
+      stb_set_error("%s: idx[%llu] = %llu is out of order or outside rows [%llu, %llu)", what, (unsigned long long)i,
                     (unsigned long long)idx[i], (unsigned long long)c->row_base, (unsigned long long)(c->row_base + c->n));
       return STB_ERR_RANGE;
     }
@@ -1090,6 +1093,18 @@ int stb_corpus_update(stb_corpus *c, const uint64_t *idx, const float *rows, uin
   if ((rc = dev_reserve(&ctx->mut_stage, &ctx->mut_stage_cap, chunk * STB_D)) != STB_OK) return rc;
   if ((rc = dev_reserve(&ctx->mut_idx, &ctx->mut_idx_cap, chunk)) != STB_OK) return rc;
   if ((rc = dev_reserve(&ctx->mut_flags, &ctx->mut_flags_cap, 2)) != STB_OK) return rc;
+  if (hook) {
+    // the hook sees its rows in the staging buffer before anything is written; an update of one chunk stays
+    // staged for the write below, a larger one is uploaded again
+    if ((rc = hook->begin()) != STB_OK) return rc;
+    for (uint64_t i0 = 0; i0 < hook->staged_rows; i0 += chunk) {
+      const uint64_t m = std::min(chunk, n - i0);
+      STB_CUDA(cudaMemcpyAsync(ctx->mut_stage, rows + i0 * STB_D, m * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+      if ((rc = hook->staged(ctx->mut_stage, i0, m)) != STB_OK) return rc;
+    }
+    if ((rc = hook->ready()) != STB_OK) return rc;
+  }
+  const bool staged = hook && hook->staged_rows && n <= chunk;
   corpus_drop_bad_copies(c);
   STB_CUDA(cudaMemsetAsync(ctx->mut_flags, 0, 2 * sizeof(int), ctx->stream));
   StbCorpusWriteArgs a = corpus_write_args(c, c->q8_rows, c->shadow_rows);
@@ -1100,25 +1115,34 @@ int stb_corpus_update(stb_corpus *c, const uint64_t *idx, const float *rows, uin
     for (uint64_t i = 0; i < a.m; ++i) local[i] = idx[i0 + i] - c->row_base;
     // the previous chunk's kernel reads the staging buffers: stream order keeps these copies behind it
     STB_CUDA(cudaMemcpyAsync(ctx->mut_idx, local.data(), a.m * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->stream));
-    STB_CUDA(cudaMemcpyAsync(ctx->mut_stage, rows + i0 * STB_D, a.m * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    if (!staged)
+      STB_CUDA(cudaMemcpyAsync(ctx->mut_stage, rows + i0 * STB_D, a.m * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
     if ((rc = stb_launch_corpus_write(ctx, a)) != STB_OK) return rc;
     if (i0 + chunk < n) STB_CUDA(cudaStreamSynchronize(ctx->stream));   // `local` is refilled next
   }
   return corpus_mutation_finish(c);
 }
 
-int stb_corpus_remove(stb_corpus *c, const uint64_t *ranges, uint32_t n_ranges) {
+extern "C" {
+
+int stb_corpus_update(stb_corpus *c, const uint64_t *idx, const float *rows, uint64_t n) {
+  return stb_corpus_update_impl(c, idx, rows, n, "corpus_update", nullptr);
+}
+
+}  // extern "C"
+
+int stb_corpus_remove_impl(stb_corpus *c, const uint64_t *ranges, uint32_t n_ranges, const char *what, StbCorpusHook *hook) {
   if (!c) { stb_set_error("null corpus"); return STB_ERR_ARG; }
   int rc = ctx_use(c->ctx);
   if (rc) return rc;
   if (n_ranges == 0) return STB_OK;
-  if (!ranges) { stb_set_error("corpus_remove: ranges is null"); return STB_ERR_ARG; }
-  if ((rc = corpus_mutation_check(c, "corpus_remove")) != STB_OK) return rc;
-  if (!stb_ranges_ordered(ranges, n_ranges)) { stb_set_error("corpus_remove: ranges must be ascending, disjoint, half-open"); return STB_ERR_RANGE; }
+  if (!ranges) { stb_set_error("%s: ranges is null", what); return STB_ERR_ARG; }
+  if ((rc = hook ? hook->check() : corpus_mutation_check(c, what)) != STB_OK) return rc;
+  if (!stb_ranges_ordered(ranges, n_ranges)) { stb_set_error("%s: ranges must be ascending, disjoint, half-open", what); return STB_ERR_RANGE; }
   const uint64_t lo = c->row_base, hi = c->row_base + c->n;
   for (uint32_t i = 0; i < n_ranges; ++i)
     if (!(ranges[2 * i] < ranges[2 * i + 1]) || ranges[2 * i] < lo || ranges[2 * i + 1] > hi) {
-      stb_set_error("corpus_remove: range %u [%llu, %llu) is empty or outside rows [%llu, %llu)", i, (unsigned long long)ranges[2 * i],
+      stb_set_error("%s: range %u [%llu, %llu) is empty or outside rows [%llu, %llu)", what, i, (unsigned long long)ranges[2 * i],
                     (unsigned long long)ranges[2 * i + 1], (unsigned long long)lo, (unsigned long long)hi);
       return STB_ERR_RANGE;
     }
@@ -1146,6 +1170,7 @@ int stb_corpus_remove(stb_corpus *c, const uint64_t *ranges, uint32_t n_ranges) 
     if ((rc = dev_reserve(&ctx->mut_stage, &ctx->mut_stage_cap, chunk * STB_D)) != STB_OK) return rc;
     if ((rc = dev_reserve(&ctx->mut_idx, &ctx->mut_idx_cap, seg.size())) != STB_OK) return rc;
   }
+  if (hook && ((rc = hook->begin()) != STB_OK || (rc = hook->ready()) != STB_OK)) return rc;
   corpus_drop_bad_copies(c);
   STB_CUDA(cudaMemsetAsync(ctx->mut_flags, 0, 2 * sizeof(int), ctx->stream));
   if (moved) {
@@ -1169,6 +1194,12 @@ int stb_corpus_remove(stb_corpus *c, const uint64_t *ranges, uint32_t n_ranges) 
   c->q8_rows = q8_rows;
   c->shadow_rows = shadow_rows;
   return corpus_mutation_finish(c);
+}
+
+extern "C" {
+
+int stb_corpus_remove(stb_corpus *c, const uint64_t *ranges, uint32_t n_ranges) {
+  return stb_corpus_remove_impl(c, ranges, n_ranges, "corpus_remove", nullptr);
 }
 
 int stb_debug_corpus_copy(const stb_corpus *c, int which, uint64_t first, uint64_t n, void *out, uint64_t *covered) {

@@ -232,6 +232,28 @@ struct stb_corpus {
 // Row ranges as stb_search takes them: n half-open [begin, end) pairs, ascending and disjoint (api.cu).
 bool stb_ranges_ordered(const uint64_t *ranges, uint32_t n);
 
+// stb_corpus_update / stb_corpus_remove without their refusal of live IVF-PQ indexes (api.cu).  With a
+// hook, an index that follows the change (stb_ivfpq_update / stb_ivfpq_remove) acts at the points where it
+// must, all before the first row is written:
+//   check()   in place of that refusal, after the null-argument checks;
+//   begin()   once the arguments are validated and the corpus's staging buffers are reserved;
+//   staged()  update only: rows [i0, i0 + m) of the call, uploaded to the staging buffer, for every chunk
+//             that holds one of the call's first `staged_rows` rows (set by begin());
+//   ready()   last chance to refuse.
+// A non-zero return ends the call with that status and nothing written.
+struct StbCorpusHook {
+  uint64_t staged_rows = 0;
+  virtual int check() = 0;
+  virtual int begin() { return STB_OK; }
+  virtual int staged(const float *stage_dev, uint64_t i0, uint64_t m) { (void)stage_dev; (void)i0; (void)m; return STB_OK; }
+  virtual int ready() { return STB_OK; }
+  virtual ~StbCorpusHook() {}
+};
+int stb_corpus_update_impl(stb_corpus *c, const uint64_t *idx, const float *rows, uint64_t n, const char *what,
+                           StbCorpusHook *hook);
+int stb_corpus_remove_impl(stb_corpus *c, const uint64_t *ranges, uint32_t n_ranges, const char *what,
+                           StbCorpusHook *hook);
+
 // ---- corpus_update.cu -----------------------------------------------------------------------
 #define STB_MUT_CHUNK_ROWS 262144   // staging rows of an update / removal chunk: 256 MiB of f32 at most
 struct StbCorpusWriteArgs {

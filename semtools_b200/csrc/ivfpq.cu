@@ -312,23 +312,31 @@ __global__ void pq_seed_kernel(float *cb, const float4 *X, uint64_t n, uint64_t 
 }
 
 // ------------------------------------------------------------------ inverted lists ----
-// Adding rows [first, first + m) (the build's add phase over [0, n), and every stb_ivfpq_extend) is one
-// routine, ivf_add_rows:
+// Every change of the lists -- the build's add phase over [0, n), stb_ivfpq_extend, stb_ivfpq_update and
+// stb_ivfpq_remove -- is one edit (IvfEdit, host side below): some old entries leave, the others are
+// renumbered, and m new entries join their lists.
 //   ivf_assign_kernel, pq_step_kernel mode 1   list and code of each new row (each row's arithmetic is
-//                                              independent of its place in the launch: an appended copy of
-//                                              an indexed row gets that row's list and code bit for bit)
+//                                              independent of its place in the launch and of where the row
+//                                              is read from: a copy of an indexed row gets that row's list
+//                                              and code bit for bit)
 //   ivf_flag_forced_kernel                     forced rows: assign = IVF_NO_LIST, counted
 //   ivf_hist_kernel                            new rows per list; the sort's values 0..m-1
 //   cub::DeviceRadixSort::SortPairs            stable bucketing: keys = list id (the low bits that separate
-//                                              0..nlist-1 from IVF_NO_LIST), values = row - first.  An LSD radix
-//                                              sort is stable, so each list's new rows stay ascending and the
+//                                              0..nlist-1 from IVF_NO_LIST), values = new entry i.  An LSD radix
+//                                              sort is stable, so each list's new entries stay ascending and the
 //                                              forced rows come last, ascending; no atomic decides a position.
-//   ivf_merge_kernel                           the new codes / order: list l = its old entries in their old
-//                                              order, then its new rows ascending; the forced rows join the side
-//                                              list (ascending: new rows are larger than old ones).
-// So within a list the entries are in ascending row order, and two extends (A, then B) give the lists one
-// extend of A u B gives.  CUB rather than a hand-written counting scatter: it is stable by construction,
-// takes 2 passes for nlist <= 8192 (14 key bits) and ships header-only with the toolkit.
+// An edit that drops entries (update, remove) describes the old indexed rows that stay as kept segments
+// {[begin, end), dst}: row r of segment k becomes dst_k + r - begin_k (dst_k = begin_k for an update).
+//   ivff_bitmap_kernel                         kept-row bitmap from the segments
+//   ivff_elig_kernel                           kept entries per list
+//   ivf_compact_kernel                         surviving entries of each list, in list order, renumbered
+//   ivf_merge_kernel                           the new codes / order: list l = a merge by row of its survivors
+//                                              (every old entry for extend and build) and its new entries.
+// The forced side list (at most IVF_FORCED_CAP rows) is filtered, renumbered and merged on the host.
+// So every list and the forced list are in ascending row order, and the index is a function of the
+// quantisers and the rows: any sequence of edits reaching the same rows gives the same arrays.  CUB rather
+// than a hand-written counting scatter: it is stable by construction, takes 2 passes for nlist <= 8192
+// (14 key bits) and ships header-only with the toolkit.
 
 // forced rows (warp per row): assign[i] = IVF_NO_LIST, counted in *n_forced
 __global__ void ivf_flag_forced_kernel(const float4 *__restrict__ X, uint64_t n, uint32_t *assign, uint32_t *n_forced) {
@@ -348,35 +356,81 @@ __global__ void ivf_hist_kernel(const uint32_t *assign, uint64_t n, uint32_t *hi
   if (assign[i] != IVF_NO_LIST) atomicAdd(hist + assign[i], 1u);
 }
 
-// Thread per entry of the new index.  Position o < n_out lies in list l (new_off[l] <= o < new_off[l+1]):
-// while o - new_off[l] is inside the old list it copies old entry old_off[l] + (o - new_off[l]), past it
-// the new row sorted[j], j = o - old_off[l+1] (the r-th new row of list l sits at sorted position
-// new_off[l] - old_off[l] + r).  Positions n_out.. copy the sorted forced rows (j = o - n_old) to forced_out.
+// Survivors of an edit that drops entries (warp per list, one pass over the list in order): entry i of
+// list l whose row is set in `bitmap` goes to position surv_off[l] + (survivors of l before it), with
+// surv_pos = i and surv_row = its renumbered row (binary search of the kept segment holding it).
+__global__ void ivf_compact_kernel(const uint32_t *__restrict__ list_off, const uint32_t *__restrict__ order, uint32_t nlist,
+                                   const uint32_t *__restrict__ bitmap, const uint32_t *__restrict__ kept,
+                                   const uint32_t *__restrict__ kept_dst, uint32_t n_kept,
+                                   const uint32_t *__restrict__ surv_off, uint32_t *surv_pos, uint32_t *surv_row) {
+  const uint32_t lane = threadIdx.x & 31, l = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (l >= nlist) return;
+  const uint32_t b = __ldg(list_off + l), e = __ldg(list_off + l + 1);
+  uint32_t out = __ldg(surv_off + l);
+  for (uint32_t i0 = b; i0 < e; i0 += 32) {
+    const uint32_t i = i0 + lane;
+    uint32_t row = 0;
+    bool keep = false;
+    if (i < e) { row = __ldg(order + i); keep = (__ldg(bitmap + (row >> 5)) >> (row & 31)) & 1u; }
+    const unsigned bal = __ballot_sync(0xffffffffu, keep);
+    if (keep) {
+      uint32_t lo = 0, hi = n_kept;   // the last segment with begin <= row (it holds the row: its bit is set)
+      while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (__ldg(kept + 2 * mid) <= row) lo = mid; else hi = mid; }
+      const uint32_t p = out + __popc(bal & ((1u << lane) - 1u));
+      surv_pos[p] = i;
+      surv_row[p] = __ldg(kept_dst + lo) + (row - __ldg(kept + 2 * lo));
+    }
+    out += __popc(bal);
+  }
+}
+
+// Thread per entry of the new lists.  Position o < n_out lies in list l (new_off[l] <= o < new_off[l+1]).
+// List l merges its ns survivors (positions surv_off[l].. of the survivor arrays; without them, the old
+// list itself) with its nn new entries (sorted positions new_off[l] - surv_off[l] ..), both ascending by row
+// and disjoint.  A merge-path binary search finds i = survivors among the list's first `within` outputs;
+// output `within` is then the smaller of survivor i and new entry within - i.  For an extend every new row
+// is larger than every old one: i = min(within, ns), i.e. the old entries, then the new rows.
 struct MergeArgs {
-  const uint8_t *old_codes; const uint32_t *old_order, *old_off, *new_off; uint32_t nlist;
-  const uint8_t *codes_row; const uint32_t *sorted; uint64_t first;   // new codes in row order, sorted row offsets
-  uint32_t n_old, n_out, n_forced_new;                                // listed entries before / after; new forced
-  uint8_t *codes; uint32_t *order; uint32_t *forced_out;
+  const uint8_t *old_codes; const uint32_t *old_order;
+  const uint32_t *surv_off, *new_off; uint32_t nlist;
+  const uint32_t *surv_pos, *surv_row;        // survivors (null: every old entry, unrenumbered; surv_off = old offsets)
+  const uint8_t *codes_row; const uint32_t *sorted; const uint32_t *new_rows; uint64_t first;   // new entry i: code
+                                              // codes_row[i], row new_rows[i] (null: first + i)
+  uint32_t n_out;
+  uint8_t *codes; uint32_t *order;
 };
+__device__ __forceinline__ uint32_t ivf_surv_row(const MergeArgs &a, uint32_t s) {
+  return a.surv_row ? __ldg(a.surv_row + s) : __ldg(a.old_order + s);
+}
+__device__ __forceinline__ uint32_t ivf_new_row(const MergeArgs &a, uint32_t i) {
+  return a.new_rows ? __ldg(a.new_rows + i) : (uint32_t)(a.first + i);
+}
 __global__ void __launch_bounds__(256)
 ivf_merge_kernel(const MergeArgs a) {
   const uint64_t o = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (o >= a.n_out) {
-    if (o < (uint64_t)a.n_out + a.n_forced_new) a.forced_out[o - a.n_out] = (uint32_t)(a.first + a.sorted[o - a.n_old]);
-    return;
-  }
+  if (o >= a.n_out) return;
   uint32_t lo = 0, hi = a.nlist;      // the list l with new_off[l] <= o < new_off[l+1]
   while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (__ldg(a.new_off + mid) <= o) lo = mid; else hi = mid; }
-  const uint32_t within = (uint32_t)o - __ldg(a.new_off + lo), ob = __ldg(a.old_off + lo), oe = __ldg(a.old_off + lo + 1);
+  const uint32_t nb0 = __ldg(a.new_off + lo), within = (uint32_t)o - nb0;
+  const uint32_t sb = __ldg(a.surv_off + lo), ns = __ldg(a.surv_off + lo + 1) - sb;
+  const uint32_t nb = nb0 - sb, nn = __ldg(a.new_off + lo + 1) - nb0 - ns;
+  uint32_t i = within > nn ? within - nn : 0, ie = min(within, ns);
+  while (i < ie) {
+    const uint32_t mid = (i + ie) >> 1;
+    if (ivf_surv_row(a, sb + mid) < ivf_new_row(a, __ldg(a.sorted + nb + within - mid - 1))) i = mid + 1; else ie = mid;
+  }
+  const uint32_t j = within - i;
   const uint4 *src;
   uint32_t row;
-  if (within < oe - ob) {
-    src = reinterpret_cast<const uint4 *>(a.old_codes + (size_t)(ob + within) * PQ_M);
-    row = __ldg(a.old_order + ob + within);
+  uint32_t nj = 0, nrow = 0;
+  if (j < nn) { nj = __ldg(a.sorted + nb + j); nrow = ivf_new_row(a, nj); }
+  if (i < ns && (j >= nn || ivf_surv_row(a, sb + i) < nrow)) {
+    const uint32_t pos = a.surv_pos ? __ldg(a.surv_pos + sb + i) : sb + i;
+    src = reinterpret_cast<const uint4 *>(a.old_codes + (size_t)pos * PQ_M);
+    row = ivf_surv_row(a, sb + i);
   } else {
-    const uint32_t i = __ldg(a.sorted + ((uint32_t)o - oe));
-    src = reinterpret_cast<const uint4 *>(a.codes_row + (size_t)i * PQ_M);
-    row = (uint32_t)(a.first + i);
+    src = reinterpret_cast<const uint4 *>(a.codes_row + (size_t)nj * PQ_M);
+    row = nrow;
   }
   uint4 *dst = reinterpret_cast<uint4 *>(a.codes + o * PQ_M);
   const uint4 c0 = __ldg(src), c1 = __ldg(src + 1);
@@ -1135,16 +1189,21 @@ __global__ void ivff_elig_kernel(const uint32_t *list_off, const uint32_t *order
 }
 
 // ------------------------------------------------------------------ host side ---------
-// Device buffers of one ivf_add_rows call: freed when it returns (after a stream synchronise, so no kernel
-// still reads them) unless adopted by the index.
+// Device buffers of one edit of the lists: freed with it (after a stream synchronise, so no kernel still
+// reads them) unless adopted by the index.  A failed allocation is STB_ERR_NOMEM.
 struct IvfScratch {
   cudaStream_t st;
   std::vector<void *> p;
-  template <class T> cudaError_t alloc(T **ptr, size_t bytes) {
+  template <class T> int alloc(T **ptr, size_t bytes) {
     *ptr = nullptr;
-    const cudaError_t e = cudaMalloc(reinterpret_cast<void **>(ptr), bytes);
-    if (e == cudaSuccess) p.push_back(*ptr);
-    return e;
+    const cudaError_t e = cudaMalloc(reinterpret_cast<void **>(ptr), std::max<size_t>(bytes, 16));
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      stb_set_error("ivfpq: cudaMalloc(%zu bytes) failed: %s", bytes, cudaGetErrorString(e));
+      return STB_ERR_NOMEM;
+    }
+    p.push_back(*ptr);
+    return STB_OK;
   }
   void adopt(const void *q) { p.erase(std::find(p.begin(), p.end(), q)); }
   ~IvfScratch() {
@@ -1153,83 +1212,214 @@ struct IvfScratch {
     cudaGetLastError();
   }
 };
+#define IVF_TRY(call)                      \
+  do {                                     \
+    const int _rc = (call);                \
+    if (_rc != STB_OK) return _rc;         \
+  } while (0)
 
-// Indexes rows [first, first + m) of x's corpus (see "inverted lists"): on success x holds the extended
-// lists and n = first + m; on any error x is unchanged and usable.  Every buffer is allocated before the
-// one synchronisation that reads the counts, and the old arrays are freed only after the merge finished.
-// Peak extra memory: the new codes + order (36 B per listed row, old and new) and 48 B per new row (list
-// ids and sort values, double-buffered, and the row-order codes) plus CUB's small temporary storage.
-static int ivf_add_rows(stb_ivfpq *x, uint64_t first, uint64_t m, const char *who) {
-  stb_ctx *ctx = x->ctx;
-  cudaStream_t st = ctx->stream;
-  const uint32_t nlist = x->nlist;
-  const uint64_t n_old = x->list_off_h[nlist];
-  const int key_bits = 32 - __builtin_clz(nlist);          // 2^key_bits - 1 >= nlist: IVF_NO_LIST sorts last
-  IvfScratch t{st, {}};
-  uint32_t *assign, *assign_alt, *idx, *idx_alt, *counts, *new_off_d, *order;
-  uint8_t *codes_row, *codes;
-  void *sort_tmp;
+// One edit of the lists (see "inverted lists").  The caller fills in what changes; then
+//   ivf_edit_alloc    allocates every buffer the edit needs,
+//   ivf_edit_encode   computes the list and code of new entries [i0, i0 + mc) from rows anywhere on the device,
+//   ivf_edit_plan     writes the new arrays beside the old ones; an edit that would leave more than
+//                     IVF_FORCED_CAP forced rows is refused (STB_ERR_STATE),
+//   ivf_edit_swap     installs them.
+// Until the swap the index is untouched and searchable, so a caller can still back out.  Peak extra memory:
+// the new codes + order (36 B per listed row, old and new), 48 B per new entry (list ids and sort values,
+// double-buffered, the codes in entry order, their rows) and, when entries leave, a bitmap of the indexed
+// rows, the kept segments and 8 B per old listed entry (survivor positions and rows).
+struct IvfEdit {
+  IvfScratch t;
+  uint64_t m = 0, first = 0;          // new entries: rows first + i (build, extend), or rows_h[i] (update)
+  std::vector<uint32_t> rows_h;       //   local rows, ascending
+  bool keep_all = true;               // no old entry leaves and none is renumbered (build, extend)
+  std::vector<uint32_t> kept, kept_dst;   // otherwise the kept segments: [begin, end) pairs and their dst
+  uint32_t n_kept = 0;
+  uint64_t n_after = 0;               // indexed rows after the edit
+  int key_bits = 0;
   size_t sort_bytes = 0;
-  {
-    cub::DoubleBuffer<uint32_t> kb(nullptr, nullptr), vb(nullptr, nullptr);
-    STB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, kb, vb, (uint32_t)m, 0, key_bits, st));
+  uint32_t *assign = nullptr, *assign_alt = nullptr, *vals = nullptr, *vals_alt = nullptr, *counts = nullptr;
+  uint32_t *new_rows = nullptr, *kept_d = nullptr, *bitmap = nullptr, *elig = nullptr, *surv_pos = nullptr;
+  uint32_t *surv_row = nullptr, *surv_off_d = nullptr, *new_off_d = nullptr, *order = nullptr, *forced = nullptr;
+  uint8_t *codes_row = nullptr, *codes = nullptr;
+  void *sort_tmp = nullptr;
+  std::vector<uint32_t> new_off, forced_h;
+  explicit IvfEdit(cudaStream_t st) : t{st, {}} {}
+  IvfEdit(const IvfEdit &) = delete;
+  IvfEdit &operator=(const IvfEdit &) = delete;
+  // kept segment {[b, e), dst}; segments come in ascending order
+  void keep(uint32_t b, uint32_t e, uint32_t dst) {
+    kept.push_back(b); kept.push_back(e); kept_dst.push_back(dst);
+    ++n_kept;
   }
-  STB_CUDA(t.alloc(&assign, m * 4));
-  STB_CUDA(t.alloc(&assign_alt, m * 4));
-  STB_CUDA(t.alloc(&idx, m * 4));
-  STB_CUDA(t.alloc(&idx_alt, m * 4));
-  STB_CUDA(t.alloc(&codes_row, m * PQ_M));
-  STB_CUDA(t.alloc(&counts, (size_t)(nlist + 1) * 4));
-  STB_CUDA(t.alloc(&sort_tmp, std::max<size_t>(sort_bytes, 16)));
-  STB_CUDA(t.alloc(&codes, (n_old + m) * PQ_M));
-  STB_CUDA(t.alloc(&order, (n_old + m) * 4));
-  STB_CUDA(t.alloc(&new_off_d, (size_t)(nlist + 1) * 4));
-  // list and code of every new row: the build's kernels on the rows from `first` on
-  const float4 *X4 = reinterpret_cast<const float4 *>(x->corpus->rows) + first * STB_ROW_F4;
-  ivf_assign_kernel<<<(unsigned)((m + 63) / 64), 256, 0, st>>>(x->corpus->rows + first * STB_D, m, x->centroids, nlist, assign);
+};
+
+static int ivf_edit_alloc(stb_ivfpq *x, IvfEdit &e) {
+  const uint32_t nlist = x->nlist;
+  const uint64_t m = e.m, n_old = x->list_off_h[nlist];
+  cudaStream_t st = e.t.st;
+  e.key_bits = 32 - __builtin_clz(nlist);          // 2^key_bits - 1 >= nlist: IVF_NO_LIST sorts last
+  if (m) {
+    cub::DoubleBuffer<uint32_t> kb(nullptr, nullptr), vb(nullptr, nullptr);
+    STB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, e.sort_bytes, kb, vb, (uint32_t)m, 0, e.key_bits, st));
+  }
+  IVF_TRY(e.t.alloc(&e.assign, m * 4));
+  IVF_TRY(e.t.alloc(&e.assign_alt, m * 4));
+  IVF_TRY(e.t.alloc(&e.vals, m * 4));
+  IVF_TRY(e.t.alloc(&e.vals_alt, m * 4));
+  IVF_TRY(e.t.alloc(&e.codes_row, m * PQ_M));
+  IVF_TRY(e.t.alloc(&e.counts, (size_t)(nlist + 1) * 4));
+  IVF_TRY(e.t.alloc(&e.sort_tmp, e.sort_bytes));
+  IVF_TRY(e.t.alloc(&e.codes, (n_old + m) * PQ_M));
+  IVF_TRY(e.t.alloc(&e.order, (n_old + m) * 4));
+  IVF_TRY(e.t.alloc(&e.new_off_d, (size_t)(nlist + 1) * 4));
+  IVF_TRY(e.t.alloc(&e.forced, IVF_FORCED_CAP * 4));
+  if (!e.rows_h.empty()) IVF_TRY(e.t.alloc(&e.new_rows, m * 4));
+  if (!e.keep_all) {
+    IVF_TRY(e.t.alloc(&e.kept_d, (size_t)e.n_kept * 3 * 4));   // pairs, then dst
+    IVF_TRY(e.t.alloc(&e.bitmap, (x->n + 31) / 32 * 4));
+    IVF_TRY(e.t.alloc(&e.elig, (size_t)nlist * 4));
+    IVF_TRY(e.t.alloc(&e.surv_pos, n_old * 4));
+    IVF_TRY(e.t.alloc(&e.surv_row, n_old * 4));
+    IVF_TRY(e.t.alloc(&e.surv_off_d, (size_t)(nlist + 1) * 4));
+  }
+  STB_CUDA(cudaMemsetAsync(e.counts, 0, (size_t)(nlist + 1) * 4, st));
+  return STB_OK;
+}
+
+// list, code and forced flag of new entries [i0, i0 + mc), rows X[0 .. mc)
+static int ivf_edit_encode(stb_ivfpq *x, IvfEdit &e, const float *X, uint64_t i0, uint64_t mc) {
+  if (mc == 0) return STB_OK;
+  stb_ctx *ctx = x->ctx;
+  cudaStream_t st = e.t.st;
+  const float4 *X4 = reinterpret_cast<const float4 *>(X);
+  ivf_assign_kernel<<<(unsigned)((mc + 63) / 64), 256, 0, st>>>(X, mc, x->centroids, x->nlist, e.assign + i0);
   STB_CUDA(cudaFuncSetAttribute(pq_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * PQ_KSUB * PQ_DSUB * 4));
   PqArgs pa;
-  pa.X = X4; pa.n = m; pa.stride = 1; pa.assign = assign; pa.C = x->centroids; pa.cb = x->codebooks;
-  pa.sums = nullptr; pa.counts = nullptr; pa.codes_out = codes_row; pa.mode = 1;
+  pa.X = X4; pa.n = mc; pa.stride = 1; pa.assign = e.assign + i0; pa.C = x->centroids; pa.cb = x->codebooks;
+  pa.sums = nullptr; pa.counts = nullptr; pa.codes_out = e.codes_row + i0 * PQ_M; pa.mode = 1;
   for (int s0 = 0; s0 < PQ_M; s0 += 8) {
     pa.s0 = s0;
     pq_step_kernel<<<ctx->sm_count * 2, 256, 8 * PQ_KSUB * PQ_DSUB * 4, st>>>(pa);
   }
   // forced rows leave the lists; counts[nlist] is their count
-  STB_CUDA(cudaMemsetAsync(counts, 0, (size_t)(nlist + 1) * 4, st));
-  ivf_flag_forced_kernel<<<(unsigned)((m + 7) / 8), 256, 0, st>>>(X4, m, assign, counts + nlist);
-  ivf_hist_kernel<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(assign, m, counts, idx);
-  cub::DoubleBuffer<uint32_t> kb(assign, assign_alt), vb(idx, idx_alt);
-  STB_CUDA(cub::DeviceRadixSort::SortPairs(sort_tmp, sort_bytes, kb, vb, (uint32_t)m, 0, key_bits, st));
+  ivf_flag_forced_kernel<<<(unsigned)((mc + 7) / 8), 256, 0, st>>>(X4, mc, e.assign + i0, e.counts + x->nlist);
   STB_CUDA(cudaGetLastError());
-  std::vector<uint32_t> hist(nlist + 1);
-  STB_CUDA(cudaMemcpyAsync(hist.data(), counts, (size_t)(nlist + 1) * 4, cudaMemcpyDeviceToHost, st));
+  ctx->kernel_launches += 6;                               // assign, 4 x encode, flag
+  return STB_OK;
+}
+
+// renumbered row of an old indexed row, or false if it leaves (host form of ivf_compact_kernel's search)
+static bool ivf_edit_renumber(const IvfEdit &e, uint32_t row, uint32_t &out) {
+  if (e.keep_all) { out = row; return true; }
+  uint32_t lo = 0, hi = e.n_kept;                          // first segment with begin > row
+  while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (e.kept[2 * mid] <= row) lo = mid + 1; else hi = mid; }
+  if (lo == 0 || row >= e.kept[2 * (lo - 1) + 1]) return false;
+  out = e.kept_dst[lo - 1] + (row - e.kept[2 * (lo - 1)]);
+  return true;
+}
+
+static int ivf_edit_plan(stb_ivfpq *x, IvfEdit &e, const char *who) {
+  stb_ctx *ctx = x->ctx;
+  cudaStream_t st = e.t.st;
+  const uint32_t nlist = x->nlist;
+  const uint64_t m = e.m;
+  cub::DoubleBuffer<uint32_t> kb(e.assign, e.assign_alt), vb(e.vals, e.vals_alt);
+  if (m) {
+    ivf_hist_kernel<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(e.assign, m, e.counts, e.vals);
+    STB_CUDA(cub::DeviceRadixSort::SortPairs(e.sort_tmp, e.sort_bytes, kb, vb, (uint32_t)m, 0, e.key_bits, st));
+    if (!e.rows_h.empty())
+      STB_CUDA(cudaMemcpyAsync(e.new_rows, e.rows_h.data(), m * 4, cudaMemcpyHostToDevice, st));
+    ctx->kernel_launches += 2;                             // hist, sort (as one)
+  }
+  std::vector<uint32_t> hist(nlist + 1), surv(nlist, 0);
+  if (!e.keep_all) {
+    const uint64_t words = (x->n + 31) / 32;
+    if (e.n_kept) {
+      STB_CUDA(cudaMemcpyAsync(e.kept_d, e.kept.data(), (size_t)e.n_kept * 8, cudaMemcpyHostToDevice, st));
+      STB_CUDA(cudaMemcpyAsync(e.kept_d + 2 * e.n_kept, e.kept_dst.data(), (size_t)e.n_kept * 4, cudaMemcpyHostToDevice, st));
+    }
+    if (words) ivff_bitmap_kernel<<<(unsigned)((words + 255) / 256), 256, 0, st>>>(e.kept_d, e.n_kept, (uint32_t)words, e.bitmap);
+    ivff_elig_kernel<<<(nlist + 7) / 8, 256, 0, st>>>(x->list_off, x->order, nlist, e.bitmap, e.elig);
+    STB_CUDA(cudaMemcpyAsync(surv.data(), e.elig, (size_t)nlist * 4, cudaMemcpyDeviceToHost, st));
+    ctx->kernel_launches += 2;
+  } else {
+    for (uint32_t l = 0; l < nlist; ++l) surv[l] = x->list_off_h[l + 1] - x->list_off_h[l];
+  }
+  STB_CUDA(cudaMemcpyAsync(hist.data(), e.counts, (size_t)(nlist + 1) * 4, cudaMemcpyDeviceToHost, st));
+  STB_CUDA(cudaGetLastError());
   STB_CUDA(cudaStreamSynchronize(st));
+  // the forced side list: old forced rows that stay (renumbered), merged with the new ones (the sort's tail)
   const uint32_t nf_new = hist[nlist];
-  if ((uint64_t)x->n_forced + nf_new > IVF_FORCED_CAP) {
-    stb_set_error("%s: %u rows are non-finite or have an fp32 squared norm outside [1e-30, 1e30] (at most %u)", who,
-                  x->n_forced + nf_new, (unsigned)IVF_FORCED_CAP);
+  std::vector<uint32_t> old_f(x->n_forced), tail(nf_new);
+  if (x->n_forced) STB_CUDA(cudaMemcpyAsync(old_f.data(), x->forced, (size_t)x->n_forced * 4, cudaMemcpyDeviceToHost, st));
+  if (nf_new) STB_CUDA(cudaMemcpyAsync(tail.data(), vb.Current() + (m - nf_new), (size_t)nf_new * 4, cudaMemcpyDeviceToHost, st));
+  STB_CUDA(cudaStreamSynchronize(st));
+  std::vector<uint32_t> kept_f;
+  for (uint32_t r : old_f) { uint32_t nr; if (ivf_edit_renumber(e, r, nr)) kept_f.push_back(nr); }
+  for (uint32_t &v : tail) v = e.rows_h.empty() ? (uint32_t)(e.first + v) : e.rows_h[v];
+  e.forced_h.resize(kept_f.size() + tail.size());
+  std::merge(kept_f.begin(), kept_f.end(), tail.begin(), tail.end(), e.forced_h.begin());
+  if (e.forced_h.size() > IVF_FORCED_CAP) {
+    stb_set_error("%s: %zu rows are non-finite or have an fp32 squared norm outside [1e-30, 1e30] (at most %u)", who,
+                  e.forced_h.size(), (unsigned)IVF_FORCED_CAP);
     return STB_ERR_STATE;
   }
-  std::vector<uint32_t> new_off(nlist + 1, 0);
-  for (uint32_t l = 0; l < nlist; ++l) new_off[l + 1] = new_off[l] + (x->list_off_h[l + 1] - x->list_off_h[l]) + hist[l];
-  STB_CUDA(cudaMemcpyAsync(new_off_d, new_off.data(), (size_t)(nlist + 1) * 4, cudaMemcpyHostToDevice, st));
+  std::vector<uint32_t> surv_off(nlist + 1, 0);
+  e.new_off.assign(nlist + 1, 0);
+  for (uint32_t l = 0; l < nlist; ++l) {
+    surv_off[l + 1] = surv_off[l] + surv[l];
+    e.new_off[l + 1] = e.new_off[l] + surv[l] + hist[l];
+  }
+  const uint32_t n_out = e.new_off[nlist];
+  STB_CUDA(cudaMemcpyAsync(e.new_off_d, e.new_off.data(), (size_t)(nlist + 1) * 4, cudaMemcpyHostToDevice, st));
+  if (!e.forced_h.empty())
+    STB_CUDA(cudaMemcpyAsync(e.forced, e.forced_h.data(), e.forced_h.size() * 4, cudaMemcpyHostToDevice, st));
   MergeArgs ma;
-  ma.old_codes = x->codes; ma.old_order = x->order; ma.old_off = x->list_off; ma.new_off = new_off_d; ma.nlist = nlist;
-  ma.codes_row = codes_row; ma.sorted = vb.Current(); ma.first = first;
-  ma.n_old = (uint32_t)n_old; ma.n_out = new_off[nlist]; ma.n_forced_new = nf_new;
-  ma.codes = codes; ma.order = order; ma.forced_out = x->forced + x->n_forced;   // past the entries searches read
-  ivf_merge_kernel<<<(unsigned)(((uint64_t)ma.n_out + nf_new + 255) / 256), 256, 0, st>>>(ma);
+  ma.old_codes = x->codes; ma.old_order = x->order; ma.new_off = e.new_off_d; ma.nlist = nlist;
+  ma.surv_off = x->list_off; ma.surv_pos = nullptr; ma.surv_row = nullptr;
+  if (!e.keep_all) {
+    STB_CUDA(cudaMemcpyAsync(e.surv_off_d, surv_off.data(), (size_t)(nlist + 1) * 4, cudaMemcpyHostToDevice, st));
+    ivf_compact_kernel<<<(nlist + 7) / 8, 256, 0, st>>>(x->list_off, x->order, nlist, e.bitmap, e.kept_d,
+                                                         e.kept_d + 2 * e.n_kept, e.n_kept, e.surv_off_d, e.surv_pos,
+                                                         e.surv_row);
+    ma.surv_off = e.surv_off_d; ma.surv_pos = e.surv_pos; ma.surv_row = e.surv_row;
+    ctx->kernel_launches += 1;
+  }
+  ma.codes_row = e.codes_row; ma.sorted = vb.Current(); ma.new_rows = e.new_rows; ma.first = e.first;
+  ma.n_out = n_out; ma.codes = e.codes; ma.order = e.order;
+  if (n_out) {
+    ivf_merge_kernel<<<(unsigned)(((uint64_t)n_out + 255) / 256), 256, 0, st>>>(ma);
+    ctx->kernel_launches += 1;
+  }
   STB_CUDA(cudaGetLastError());
-  STB_CUDA(cudaStreamSynchronize(st));                     // searches enqueued before this call are done too
-  ctx->kernel_launches += 9;                               // assign, 4 x encode, flag, hist, sort (as one), merge
-  t.adopt(codes); t.adopt(order); t.adopt(new_off_d);
-  cudaFree(x->codes); cudaFree(x->order); cudaFree(x->list_off);
-  x->codes = codes; x->order = order; x->list_off = new_off_d;
-  x->list_off_h.swap(new_off);
-  x->n_forced += nf_new;
-  x->n = first + m;
+  // the host vectors the copies above read die with the caller: the copies must be done
+  STB_CUDA(cudaStreamSynchronize(st));
   return STB_OK;
+}
+
+// Installs a planned edit.  Searches enqueued before it have finished (the stream is synchronised), so the
+// old arrays can go.
+static int ivf_edit_swap(stb_ivfpq *x, IvfEdit &e) {
+  STB_CUDA(cudaStreamSynchronize(e.t.st));
+  e.t.adopt(e.codes); e.t.adopt(e.order); e.t.adopt(e.new_off_d); e.t.adopt(e.forced);
+  cudaFree(x->codes); cudaFree(x->order); cudaFree(x->list_off); cudaFree(x->forced);
+  x->codes = e.codes; x->order = e.order; x->list_off = e.new_off_d; x->forced = e.forced;
+  x->list_off_h.swap(e.new_off);
+  x->n_forced = (uint32_t)e.forced_h.size();
+  x->n = e.n_after;
+  return STB_OK;
+}
+
+// Indexes rows [first, first + m) of x's corpus (the build's add phase and stb_ivfpq_extend): on success x
+// holds the extended lists and n = first + m; on any error x is unchanged and usable.
+static int ivf_add_rows(stb_ivfpq *x, uint64_t first, uint64_t m, const char *who) {
+  IvfEdit e(x->ctx->stream);
+  e.m = m; e.first = first; e.n_after = first + m;
+  IVF_TRY(ivf_edit_alloc(x, e));
+  IVF_TRY(ivf_edit_encode(x, e, x->corpus->rows + first * STB_D, 0, m));
+  IVF_TRY(ivf_edit_plan(x, e, who));
+  return ivf_edit_swap(x, e);
 }
 
 extern "C" {
@@ -1333,7 +1523,6 @@ int stb_ivfpq_build(stb_ctx *ctx, const stb_corpus *corpus, uint32_t nlist, uint
   IVF_CUDA(cudaStreamSynchronize(st));
   cudaFree(sums); cudaFree(counts); cudaFree(pq_sums); cudaFree(pq_counts); cudaFree(assign); cudaFree(sample);
   // ---- add: rows [0, n) into empty lists, as stb_ivfpq_extend adds its rows ----------------------
-  IVF_CUDA(cudaMalloc(&x->forced, IVF_FORCED_CAP * 4));
   IVF_CUDA(cudaMalloc(&x->list_off, (size_t)(nlist + 1) * 4));
   IVF_CUDA(cudaMemsetAsync(x->list_off, 0, (size_t)(nlist + 1) * 4, st));
   x->list_off_h.assign(nlist + 1, 0);
@@ -1380,6 +1569,113 @@ int stb_ivfpq_extend(stb_ivfpq *x, uint64_t *out_added) {
   const int rc = ivf_add_rows(x, x->n, m, "ivfpq_extend");
   if (rc == STB_OK && out_added) *out_added = m;
   return rc;
+}
+
+}  // extern "C"
+
+// ---- stb_ivfpq_update / stb_ivfpq_remove: the corpus call (api.cu) with the index's edit hooked in ----
+// The refusals of another live index and of a corpus in another epoch replace the corpus's refusal of live
+// indexes; the edit is planned (every buffer allocated, the forced rows counted) before the corpus writes
+// anything and installed once the corpus call has succeeded.
+struct IvfHook : StbCorpusHook {
+  stb_ivfpq *x;
+  const char *who;
+  IvfEdit e;
+  bool checked = false;               // the corpus call got past its argument checks
+  bool edit = false;                  // some indexed row changes
+  IvfHook(stb_ivfpq *x_, const char *who_) : x(x_), who(who_), e(x_->ctx->stream) {}
+  int check() override {
+    const stb_corpus *c = x->corpus;
+    if (c->ivfpq_live > 1) {
+      stb_set_error("%s: %u IVF-PQ indexes on this corpus refer to its rows; destroy the others first", who, c->ivfpq_live);
+      return STB_ERR_STATE;
+    }
+    if (c->epoch != x->corpus_epoch || c->n < x->n) {
+      stb_set_error("%s: the corpus was cleared since the index was built (%llu rows, the index holds %llu)", who,
+                    (unsigned long long)c->n, (unsigned long long)x->n);
+      return STB_ERR_STATE;
+    }
+    checked = true;
+    return STB_OK;
+  }
+  // after the corpus call: install the edit, follow the corpus into its new epoch
+  int finish(int rc) {
+    if (rc != STB_OK || !checked) return rc;
+    if (edit) IVF_TRY(ivf_edit_swap(x, e));
+    x->corpus_epoch = x->corpus->epoch;
+    return STB_OK;
+  }
+};
+
+// Update: the replaced indexed rows leave their lists (or the forced list) and come back as new entries with
+// the list and code of their new value, encoded from the staging buffer.  Nothing is renumbered.
+struct IvfUpdateHook : IvfHook {
+  const uint64_t *idx;
+  uint64_t n;
+  IvfUpdateHook(stb_ivfpq *x_, const uint64_t *idx_, uint64_t n_) : IvfHook(x_, "ivfpq_update"), idx(idx_), n(n_) {}
+  int begin() override {
+    const uint64_t base = x->corpus->row_base;
+    uint64_t m = 0;                   // idx is validated: ascending, so the indexed rows come first
+    while (m < n && idx[m] - base < x->n) ++m;
+    if (m == 0) return STB_OK;
+    edit = true;
+    staged_rows = m;
+    e.m = m; e.n_after = x->n; e.keep_all = false;
+    e.rows_h.resize(m);
+    uint32_t b = 0;
+    for (uint64_t i = 0; i < m; ++i) {
+      const uint32_t r = (uint32_t)(idx[i] - base);
+      if (r > b) e.keep(b, r, b);
+      b = r + 1;
+      e.rows_h[i] = r;
+    }
+    if (x->n > b) e.keep(b, (uint32_t)x->n, b);
+    return ivf_edit_alloc(x, e);
+  }
+  int staged(const float *stage, uint64_t i0, uint64_t m) override {
+    if (i0 >= e.m) return STB_OK;
+    return ivf_edit_encode(x, e, stage, i0, std::min(m, e.m - i0));
+  }
+  int ready() override { return edit ? ivf_edit_plan(x, e, who) : STB_OK; }
+};
+
+// Remove: the removed indexed rows leave; every entry behind them moves down by the removed rows below it.
+struct IvfRemoveHook : IvfHook {
+  const uint64_t *ranges;
+  uint32_t n_ranges;
+  IvfRemoveHook(stb_ivfpq *x_, const uint64_t *r, uint32_t nr) : IvfHook(x_, "ivfpq_remove"), ranges(r), n_ranges(nr) {}
+  int begin() override {
+    const uint64_t base = x->corpus->row_base;
+    uint64_t b = 0, dst = 0;          // ranges are validated: ascending, disjoint, inside the corpus
+    for (uint32_t i = 0; i < n_ranges; ++i) {
+      const uint64_t rb = std::min(ranges[2 * i] - base, x->n), re = std::min(ranges[2 * i + 1] - base, x->n);
+      if (rb == re) break;            // past the indexed rows
+      if (rb > b) { e.keep((uint32_t)b, (uint32_t)rb, (uint32_t)dst); dst += rb - b; }
+      b = re;
+    }
+    if (b == 0 && e.n_kept == 0) return STB_OK;   // no indexed row is removed
+    if (x->n > b) { e.keep((uint32_t)b, (uint32_t)x->n, (uint32_t)dst); dst += x->n - b; }
+    edit = true;
+    e.keep_all = false; e.n_after = dst;
+    IVF_TRY(ivf_edit_alloc(x, e));
+    return ivf_edit_plan(x, e, who);
+  }
+};
+
+extern "C" {
+
+// Replaces rows of the index's corpus (stb_corpus_update) and re-indexes the replaced indexed rows.
+int stb_ivfpq_update(stb_ivfpq *x, const uint64_t *idx, const float *rows, uint64_t n) {
+  if (!x) { stb_set_error("ivfpq_update: null index"); return STB_ERR_ARG; }
+  IvfUpdateHook h(x, idx, n);
+  return h.finish(stb_corpus_update_impl(const_cast<stb_corpus *>(x->corpus), idx, rows, n, "ivfpq_update", &h));
+}
+
+// Deletes rows of the index's corpus (stb_corpus_remove) and drops and renumbers the index's entries to match.
+int stb_ivfpq_remove(stb_ivfpq *x, const uint64_t *ranges, uint32_t n_ranges) {
+  if (!x) { stb_set_error("ivfpq_remove: null index"); return STB_ERR_ARG; }
+  IvfRemoveHook h(x, ranges, n_ranges);
+  return h.finish(stb_corpus_remove_impl(const_cast<stb_corpus *>(x->corpus), ranges, n_ranges, "ivfpq_remove", &h));
 }
 
 // Approximate top-k: probe `nprobe` lists, keep the `rerank` best ADC scores, re-score those
