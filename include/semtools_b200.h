@@ -150,20 +150,27 @@ int stb_corpus_remove(stb_corpus *corpus, const uint64_t *ranges, uint32_t n_ran
  * stays on the host: the caller passes the token ids of each line as a CSR batch
  * (offsets[n_lines+1], ids[offsets[n_lines]]), already unk-dropped and truncated
  * (2048 ids per corpus line, 512 for the query).  Output row i is bit-identical
- * to pool_ids(ids of line i) of model2vec-rs 0.1.3.
+ * to pool_ids(ids of line i) of model2vec-rs 0.1.3, subnormals included (no
+ * flush-to-zero).  One exception: a component that is NaN is NaN exactly where
+ * pool_ids gives NaN, but its payload is the canonical quiet NaN 0x7fffffff, not
+ * the payload a CPU may propagate from a NaN in the table or the weights.
  * `out` (host, n_lines x 256) and `append_to` may each be NULL; with `append_to`
  * the rows are written straight into the corpus in HBM and never visit the host.
  * A token whose table row is out of range fails the call with STB_ERR_RANGE
- * (upstream panics) and appends nothing. */
+ * (upstream panics) and appends nothing.  The call reports its own tokens only
+ * through its return value, never through the stb_embed_dev flag below. */
 int stb_embed(stb_ctx *ctx, const stb_table *table, const uint64_t *offsets,
               const uint32_t *ids, uint64_t n_lines, float *out,
               stb_corpus *append_to);
 
 /* Asynchronous device-resident form of stb_embed: CSR and output already in HBM
  * (out_dev: n_lines x 256 f32, e.g. a slice of stb_corpus_data_dev), nothing
- * synchronises.  A token outside the table sets a sticky flag instead of failing;
+ * synchronises.  A token outside the table sets a sticky per-context flag instead
+ * of failing (its line is pooled as if the token were row 0);
  * stb_embed_status() synchronises the stream, returns STB_ERR_RANGE if the flag was
- * set since the last call, and clears it. */
+ * set since the last call, and clears it.  Only stb_embed_dev sets the flag and
+ * only stb_embed_status clears it: no other call on the context (searches, copy
+ * builds, stb_embed) reads or writes it. */
 int stb_embed_dev(stb_ctx *ctx, const stb_table *table, const uint64_t *offsets_dev,
                   const uint32_t *ids_dev, uint64_t n_lines, float *out_dev);
 int stb_embed_status(stb_ctx *ctx);
@@ -471,15 +478,20 @@ int stb_search_many(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint
 /* ---- K4: merge per-shard hit lists -----------------------------------------------
  * The final sort_by + take of src/search/mod.rs:107-119 applied across row
  * shards: `lists_dev` holds n_lists x per_list hits (e.g. the all-gathered
- * per-GPU top-k; padding entries have distance = +inf); writes the top_k best by
- * (distance, row) to out_dev.  Asynchronous on the context's stream. */
+ * per-GPU top-k; padding entries are (+inf, UINT64_MAX)); writes the top_k best by
+ * (distance, row) to out_dev.  An entry whose row is UINT64_MAX or whose distance
+ * is NaN is padding and dropped wherever it sits; +inf on a real row is kept.
+ * -0.0 and +0.0 tie (then ordered by row) and keep their bits.  out_dev gets
+ * exactly top_k entries, the tail padded with (+inf, UINT64_MAX).
+ * n_lists*per_list <= 4096.  Asynchronous on the context's stream. */
 int stb_hits_merge_dev(stb_ctx *ctx, const stb_hit *lists_dev, uint32_t n_lists,
                        uint32_t per_list, uint32_t top_k, stb_hit *out_dev);
 /* Batched form for sharded K2: lists_dev[n_lists][nq][per_list] (e.g. the all-gathered
  * per-rank results of stb_search_batch_dev) -> out_dev[nq][top_k]; n_lists*per_list <= 2048. */
 int stb_hits_merge_batch_dev(stb_ctx *ctx, const stb_hit *lists_dev, uint32_t n_lists,
                              uint32_t nq, uint32_t per_list, uint32_t top_k, stb_hit *out_dev);
-/* Host-buffer convenience wrapper (copies in, merges on the GPU, copies out). */
+/* Host-buffer convenience wrapper (copies in, merges on the GPU, copies out): out
+ * gets the *out_n <= top_k valid hits, without the padding tail. */
 int stb_hits_merge(stb_ctx *ctx, const stb_hit *lists, uint32_t n_lists,
                    uint32_t per_list, uint32_t top_k, stb_hit *out,
                    uint32_t *out_n);

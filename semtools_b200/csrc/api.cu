@@ -117,6 +117,8 @@ int stb_ctx_create(int device, void *cuda_stream, stb_ctx **out) {
     one = 0;
     if ((rc = dev_reserve(&c->err_flag, &one, 1)) != STB_OK) goto fail;
     one = 0;
+    if ((rc = dev_reserve(&c->embed_flag, &one, 1)) != STB_OK) goto fail;
+    one = 0;
     if ((rc = dev_reserve(&c->dbg_dev, &one, 8)) != STB_OK) goto fail;
     one = 0;
     if ((rc = dev_reserve(&c->hist_dev, &one, 4096)) != STB_OK) goto fail;
@@ -136,6 +138,7 @@ int stb_ctx_create(int device, void *cuda_stream, stb_ctx **out) {
       cudaMemset(c->q4_refined, 0, sizeof(unsigned long long)) != cudaSuccess ||
       cudaMemset(c->coscan_off, 0, STB_TICKET_SLOTS * sizeof(unsigned long long)) != cudaSuccess ||
       cudaMemset(c->err_flag, 0, sizeof(int)) != cudaSuccess ||
+      cudaMemset(c->embed_flag, 0, sizeof(int)) != cudaSuccess ||
       cudaMallocHost((void **)&c->q_pin, STB_D * sizeof(float)) != cudaSuccess ||
       cudaMallocHost((void **)&c->status_pin, 8 * sizeof(uint32_t)) != cudaSuccess ||
       cudaMallocHost((void **)&c->hits_pin, 1024 * sizeof(stb_hit)) != cudaSuccess) {
@@ -159,7 +162,7 @@ int stb_ctx_destroy(stb_ctx *c) {
   cudaStreamSynchronize(c->stream);
   cudaFree(c->block_keys); cudaFree(c->counters); cudaFree(c->q_dev); cudaFree(c->hits_dev);
   cudaFree(c->status_dev); cudaFree(c->collect_rows); cudaFree(c->collect_count);
-  cudaFree(c->collect_hits); cudaFree(c->ranges_dev); cudaFree(c->err_flag);
+  cudaFree(c->collect_hits); cudaFree(c->ranges_dev); cudaFree(c->err_flag); cudaFree(c->embed_flag);
   cudaFree(c->tickets); cudaFree(c->q4_thr); cudaFree(c->q4_refined); cudaFree(c->coscan_off);
   cudaFree(c->dbg_dev); cudaFree(c->hist_dev); cudaFree(c->bq_tiles); cudaFree(c->b_submax); cudaFree(c->b_tilemax); cudaFree(c->b_cand);
   cudaFree(c->b_thr); cudaFree(c->b_cnt); cudaFree(c->b_keys); cudaFree(c->b_qbad);
@@ -449,10 +452,13 @@ int stb_embed(stb_ctx *ctx, const stb_table *table, const uint64_t *offsets, con
   }
   STB_CUDA(cudaMemcpyAsync(ctx->embed_off_dev, offsets, (n_lines + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->stream));
   if (total) STB_CUDA(cudaMemcpyAsync(ctx->embed_ids_dev, ids, total * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+  // the call's own tokens are reported through its return value: the scratch flag, never the sticky
+  // stb_embed_dev flag, and it is zeroed again after reading like every other synchronous user
   STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
   if ((rc = stb_launch_embed(ctx, table, ctx->embed_off_dev, ctx->embed_ids_dev, n_lines, dst, ctx->err_flag)) != STB_OK) return rc;
   int flag = 0;
   STB_CUDA(cudaMemcpyAsync(&flag, ctx->err_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
   if (out) STB_CUDA(cudaMemcpyAsync(out, dst, n_lines * STB_D * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
   STB_CUDA(cudaStreamSynchronize(ctx->stream));
   if (flag) { stb_set_error("embed: a token id maps outside the %llu-row table", (unsigned long long)table->V); return STB_ERR_RANGE; }
@@ -467,15 +473,15 @@ int stb_embed_dev(stb_ctx *ctx, const stb_table *table, const uint64_t *offsets_
   if (!table || table->ctx != ctx) { stb_set_error("embed_dev: bad table"); return STB_ERR_ARG; }
   if (n_lines == 0) return STB_OK;
   if (!offsets_dev || !ids_dev || !out_dev) { stb_set_error("embed_dev: null device pointer"); return STB_ERR_ARG; }
-  return stb_launch_embed(ctx, table, offsets_dev, ids_dev, n_lines, out_dev, ctx->err_flag);
+  return stb_launch_embed(ctx, table, offsets_dev, ids_dev, n_lines, out_dev, ctx->embed_flag);
 }
 
 int stb_embed_status(stb_ctx *ctx) {
   int rc = ctx_use(ctx);
   if (rc) return rc;
   int flag = 0;
-  STB_CUDA(cudaMemcpyAsync(&flag, ctx->err_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
+  STB_CUDA(cudaMemcpyAsync(&flag, ctx->embed_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  STB_CUDA(cudaMemsetAsync(ctx->embed_flag, 0, sizeof(int), ctx->stream));
   STB_CUDA(cudaStreamSynchronize(ctx->stream));
   if (flag) { stb_set_error("embed: a token id maps outside the table"); return STB_ERR_RANGE; }
   return STB_OK;

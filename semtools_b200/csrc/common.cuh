@@ -114,7 +114,7 @@ struct stb_ctx {
   size_t collect_hits_cap;
   uint64_t *ranges_dev;     // [3 * n] : begin(local), end(local), vstart
   size_t ranges_cap;
-  int *err_flag;            // device int for K3 range errors
+  int *err_flag;            // device int: scratch flag of the copy builders, stb_embed and K2's query shadow; zeroed before each use
   unsigned int *hist_dev;       // 4096-bin score histogram (large-k path)
   unsigned long long *dbg_dev;  // 8 u64 phase timestamps (STB_TAIL_TIMING builds; else unused)
   // cudaFuncSetAttribute is per DEVICE: remembered per context, never in function statics
@@ -157,6 +157,8 @@ struct stb_ctx {
   // --- counters ---
   uint64_t kernel_launches;
   uint64_t fallback_searches;
+  // --- K3 ---
+  int *embed_flag;          // device int: K3's sticky range flag; set only by stb_embed_dev, cleared only by stb_embed_status
 };
 
 #define STB_TICKET_SLOTS 8
