@@ -27,8 +27,8 @@
  * Environment switches (read per call; results are identical whatever their
  * value -- they select how candidates are found, never how the returned
  * distances are computed): STB_SCAN_TIER=f32|h16|q8 (narrowest candidate copy K1
- * may read, default q8), STB_DIRECT_OUT=0, STB_BATCH_V1=1, STB_IVFPQ_V1=1
- * (INTEGRATION.md, 5b).
+ * may read, default q8), STB_BATCH_V1=1, STB_IVFPQ_V1=1, STB_IVFPQ_BATCH_KEEP=k,
+ * STB_SCAN_OVERLAP=1 (INTEGRATION.md, 5b).
  */
 #ifndef SEMTOOLS_B200_H
 #define SEMTOOLS_B200_H
@@ -514,11 +514,6 @@ int stb_ctx_counters(const stb_ctx *ctx, uint64_t *kernel_launches,
 /* Consistency check of K1's dynamic tile schedule (synchronises): the device-side ticket counter
  * must equal the value the host booked over all launches so far; STB_ERR_STATE otherwise. */
 int stb_debug_ticket_check(stb_ctx *ctx, uint64_t *device_value, uint64_t *host_value);
-/* Tuning aid: phase timestamps (ns, %globaltimer) of the last K1 launch; only filled by
- * libraries built with -DSTB_TAIL_TIMING.  reset=1 arms, reset=0 reads 8 values:
- * [0] first CTA start, [1] last scan end, [2] last CTA merge end, [3] final ticket,
- * [4] select done, [5] re-rank done. */
-int stb_debug_timestamps(stb_ctx *ctx, int reset, uint64_t out[8]);
 /* Rows the q8 tier's top-k prefilter passed on to the int8 codes, summed over the
  * top-k launches since the last reset (reset != 0 zeroes the counter after reading it).
  * Synchronises the context's stream. */

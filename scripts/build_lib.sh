@@ -1,7 +1,7 @@
 #!/usr/bin/env bash
 # Builds libsemtools_b200.so for sm_90a (cross-compiles without a GPU).
-# STB_NVCC_EXTRA adds compiler flags (e.g. -DSTB_SHADOW_F16=1), STB_LIB_OUT redirects the output
-# (variants go to semtools_b200/lib/variants/, git-ignored; load them with STB_LIB_PATH).
+# STB_NVCC_EXTRA adds compiler flags (e.g. -DSTB_SHADOW_F16=0), STB_LIB_OUT redirects the output
+# (load such a library with STB_LIB_PATH).
 set -euo pipefail
 cd "$(dirname "$0")/.."
 mkdir -p semtools_b200/lib

@@ -25,7 +25,7 @@ e0.record(s); c.prepare(2); e1.record(s); torch.cuda.synchronize(); h16_ms = e0.
 nq = 32
 q = torch.randn((nq, 256), generator=g, device=dev); q /= q.norm(dim=1, keepdim=True)
 qh = q.cpu().numpy()
-out = {"rows": rows, "k": k, "build_ms": {"q8": q8_ms, "h16": h16_ms}, "ctas_per_sm": os.environ.get("STB_SCAN_CTAS_PER_SM", "default")}
+out = {"rows": rows, "k": k, "build_ms": {"q8": q8_ms, "h16": h16_ms}}
 ref = None
 BYTES = {"f32": 1024, "h16": 512, "q8": 260}
 for tier in ("f32", "h16", "q8"):

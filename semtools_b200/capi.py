@@ -28,7 +28,7 @@ SYMBOLS = [
     "stb_xchg_create", "stb_xchg_destroy", "stb_xchg_local_handle",
     "stb_xchg_connect", "stb_xchg_connect_local", "stb_search_topk_xchg", "stb_search_xchg", "stb_search_many", "stb_xchg_create_batch", "stb_search_batch_xchg_dev", "stb_ivfpq_build",
     "stb_ivfpq_destroy", "stb_ivfpq_extend", "stb_ivfpq_stats", "stb_ivfpq_search", "stb_ivfpq_search_dev", "stb_hits_merge_dev", "stb_hits_merge_batch_dev", "stb_hits_merge", "stb_fnv1a64", "stb_line_id", "stb_line_ids",
-    "stb_ctx_counters", "stb_debug_ticket_check", "stb_debug_timestamps", "stb_debug_q4_refined", "stb_debug_coscan_offsets", "stb_debug_batch_gemm", "stb_debug_batch_params",
+    "stb_ctx_counters", "stb_debug_ticket_check", "stb_debug_q4_refined", "stb_debug_coscan_offsets", "stb_debug_batch_gemm", "stb_debug_batch_params",
     "stb_debug_batch_last", "stb_debug_corpus_copy",
     "stb_debug_ivfpq_export",
     "stb_ivfpq_search_batch", "stb_ivfpq_search_batch_dev", "stb_debug_ivfpq_batch_last",
@@ -122,7 +122,6 @@ def lib() -> C.CDLL:
     L.stb_line_ids.argtypes = [vp, vp, u32, vp, u64, vp]
     L.stb_line_id.restype = u64
     L.stb_ctx_counters.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
-    L.stb_debug_timestamps.argtypes = [vp, i32, vp]
     L.stb_debug_ticket_check.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
     L.stb_debug_q4_refined.argtypes = [vp, i32, C.POINTER(u64)]
     L.stb_debug_coscan_offsets.argtypes = [vp, u32, vp]

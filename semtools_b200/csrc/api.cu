@@ -5,8 +5,6 @@
 #include <stdarg.h>
 #include <stdlib.h>
 
-#include <chrono>
-
 #include <algorithm>
 #include <mutex>
 #include <new>
@@ -119,8 +117,6 @@ int stb_ctx_create(int device, void *cuda_stream, stb_ctx **out) {
     one = 0;
     if ((rc = dev_reserve(&c->embed_flag, &one, 1)) != STB_OK) goto fail;
     one = 0;
-    if ((rc = dev_reserve(&c->dbg_dev, &one, 8)) != STB_OK) goto fail;
-    one = 0;
     if ((rc = dev_reserve(&c->hist_dev, &one, 4096)) != STB_OK) goto fail;
     one = 0;
     if ((rc = dev_reserve(&c->tickets, &one, STB_TICKET_SLOTS)) != STB_OK) goto fail;
@@ -164,7 +160,7 @@ int stb_ctx_destroy(stb_ctx *c) {
   cudaFree(c->status_dev); cudaFree(c->collect_rows); cudaFree(c->collect_count);
   cudaFree(c->collect_hits); cudaFree(c->ranges_dev); cudaFree(c->err_flag); cudaFree(c->embed_flag);
   cudaFree(c->tickets); cudaFree(c->q4_thr); cudaFree(c->q4_refined); cudaFree(c->coscan_off);
-  cudaFree(c->dbg_dev); cudaFree(c->hist_dev); cudaFree(c->bq_tiles); cudaFree(c->b_submax); cudaFree(c->b_tilemax); cudaFree(c->b_cand);
+  cudaFree(c->hist_dev); cudaFree(c->bq_tiles); cudaFree(c->b_submax); cudaFree(c->b_tilemax); cudaFree(c->b_cand);
   cudaFree(c->b_thr); cudaFree(c->b_cnt); cudaFree(c->b_keys); cudaFree(c->b_qbad);
   cudaFree(c->bq_dev); cudaFree(c->bh_dev); cudaFree(c->bs_dev); cudaFree(c->embed_off_dev); cudaFree(c->embed_ids_dev); cudaFree(c->embed_out_dev);
   cudaFree(c->mut_stage); cudaFree(c->mut_idx); cudaFree(c->mut_flags);
@@ -187,21 +183,6 @@ int stb_ctx_sync(stb_ctx *ctx) {
 }
 
 void *stb_ctx_stream(stb_ctx *ctx) { return ctx ? (void *)ctx->stream : nullptr; }
-
-// Tuning aid (STB_TAIL_TIMING builds): reset=1 arms the timestamps, reset=0 reads them.
-int stb_debug_timestamps(stb_ctx *ctx, int reset, uint64_t out[8]) {
-  int rc = ctx_use(ctx);
-  if (rc) return rc;
-  if (reset) {
-    unsigned long long init[8] = {~0ull, 0, 0, 0, 0, 0, 0, 0};
-    STB_CUDA(cudaMemcpyAsync(ctx->dbg_dev, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
-    STB_CUDA(cudaStreamSynchronize(ctx->stream));
-  } else {
-    STB_CUDA(cudaMemcpyAsync(out, ctx->dbg_dev, 8 * sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    STB_CUDA(cudaStreamSynchronize(ctx->stream));
-  }
-  return STB_OK;
-}
 
 // K1's tile tickets: every top-k launch must advance the device counter by exactly what the host
 // booked for it (n_tickets + total_warps); a mismatch would make later launches skip or repeat
@@ -509,14 +490,41 @@ static bool stb_env_overlap() {
   const char *e = getenv("STB_SCAN_OVERLAP");
   return e && e[0] == '1';
 }
-static bool stb_env_direct_out() {
-  const char *e = getenv("STB_DIRECT_OUT");
-  return !(e && e[0] == '0');
+
+// What a K1 entry point may do to a reduced-width candidate copy that does not cover every row yet:
+// build it from nothing (or rebuild one marked bad), and convert the rows appended behind a valid prefix.
+struct K1CopyPolicy {
+  bool build, extend;
+};
+static const K1CopyPolicy kBuiltOnly = {false, false};
+
+// The one rule for K1's candidate copies: sets *ready when the scan may read tier `tier` of c now.  It
+// applies the STB_SCAN_TIER cap, the q8 tier's k-limit (top_k: k of the top-k scan; 0 for the collect
+// and histogram passes, which have none) and the copy's state, building or extending the copy as the
+// policy allows.  Rows that cannot be normalised in fp32 make a copy unusable (the builder's
+// STB_ERR_STATE), which is not an error of the search.  f32 is always ready.
+static int k1_copy_ready(stb_ctx *ctx, stb_corpus *c, int tier, uint32_t top_k, K1CopyPolicy policy, bool *ready) {
+  *ready = tier == STB_TIER_F32;
+  if (*ready || tier > stb_env_max_tier() || (tier == STB_TIER_Q8 && top_k > STB_Q8_MAX_K)) return STB_OK;
+  const bool q8 = tier == STB_TIER_Q8;
+  const bool have = q8 ? c->q8 != nullptr : c->shadow != nullptr;
+  const uint64_t rows = q8 ? c->q8_rows : c->shadow_rows;
+  const bool bad = q8 ? c->q8_bad : c->shadow_bad;
+  if (have && rows == c->n) { *ready = !bad; return STB_OK; }
+  if (!policy.build && !(policy.extend && have && rows > 0 && !bad)) return STB_OK;
+  const int rc = q8 ? corpus_ensure_q8(ctx, c) : corpus_ensure_shadow(ctx, c);
+  *ready = rc == STB_OK;
+  return rc == STB_ERR_STATE ? STB_OK : rc;
 }
-static int best_built_tier(const stb_corpus *c, uint32_t top_k) {
-  const int max_tier = stb_env_max_tier();
-  if (max_tier >= STB_TIER_Q8 && top_k <= STB_Q8_MAX_K && c->q8 && c->q8_rows == c->n && !c->q8_bad) return STB_TIER_Q8;
-  if (max_tier >= STB_TIER_H16 && c->shadow && c->shadow_rows == c->n && !c->shadow_bad) return STB_TIER_H16;
+
+// The narrowest copy that is fully built and usable: the asynchronous entry points never build one
+// (stb_corpus_prepare does).
+static int best_built_tier(stb_ctx *ctx, const stb_corpus *c, uint32_t top_k) {
+  for (int tier = STB_TIER_Q8; tier > STB_TIER_F32; --tier) {
+    bool ready = false;
+    k1_copy_ready(ctx, const_cast<stb_corpus *>(c), tier, top_k, kBuiltOnly, &ready);   // builds nothing: cannot fail
+    if (ready) return tier;
+  }
   return STB_TIER_F32;
 }
 
@@ -586,18 +594,13 @@ int stb_search(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t 
   uint32_t n_loc = 0;
   uint64_t n_virtual = corpus->n;
   if (row_ranges) {
-    if (!stb_ranges_ordered(row_ranges, n_ranges)) { stb_set_error("search: row_ranges must be ascending, disjoint, half-open"); return STB_ERR_RANGE; }
     std::vector<uint64_t> vstart, rbegin;
     vstart.reserve(n_ranges + 1); rbegin.reserve(n_ranges);
     uint64_t acc = 0;
-    const uint64_t lo = corpus->row_base, hi = corpus->row_base + corpus->n;
-    for (uint32_t i = 0; i < n_ranges; ++i) {
-      uint64_t b = row_ranges[2 * i], e = row_ranges[2 * i + 1];
-      b = std::max(b, lo); e = std::min(e, hi);
-      if (b >= e) continue;
-      vstart.push_back(acc); rbegin.push_back(b - lo);
-      acc += e - b;
-    }
+    if ((rc = stb_clip_ranges("search", row_ranges, n_ranges, corpus->row_base, corpus->n, [&](uint64_t b, uint64_t e) {
+           vstart.push_back(acc); rbegin.push_back(b);
+           acc += e - b;
+         })) != STB_OK) return rc;
     if (acc == 0) return STB_OK;
     vstart.push_back(acc);
     n_loc = (uint32_t)rbegin.size();
@@ -613,52 +616,39 @@ int stb_search(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t 
   memcpy(ctx->q_pin, q, STB_D * sizeof(float));
   STB_CUDA(cudaMemcpyAsync(ctx->q_dev, ctx->q_pin, STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
 
+  // The reduced-width candidate copies are used when they exist (stb_corpus_prepare) and built lazily
+  // from the second search since the corpus last changed, on >= 32768 rows: a one-shot CLI query must
+  // not pay a full extra pass to save half of one.  A copy that covers a prefix (rows were appended
+  // since) is extended right away: converting the new rows costs far less than scanning everything at
+  // 1 KiB/row.
+  stb_corpus *cm = const_cast<stb_corpus *>(corpus);
+  const K1CopyPolicy lazy = {cm->searches_since_change >= 1 && cm->n >= 32768, true};
+  cm->searches_since_change++;
+
   uint64_t total = 0;
   const stb_hit *src_dev = nullptr;   // sorted device hits to copy out (collect path)
   if (!threshold_all && top_k <= stb_scan_topk_max_k()) {
     // ---- fast path: one kernel, k*16+16 bytes back -----------------------------
     // The kernel's last CTA stores the k hits + status straight into the pinned host buffers
     // (UVA: cudaMallocHost memory is device-accessible), which takes the two D2H copies off the
-    // stream; kernel completion makes the stores visible to the host.  STB_DIRECT_OUT=0 restores
-    // the device buffers + two cudaMemcpyAsync.
-    const bool direct = stb_env_direct_out();
+    // stream; kernel completion makes the stores visible to the host.
     auto run_fast = [&](int tier) -> int {
       int r;
-      if (direct) {
-        if ((r = stb_launch_scan_topk(ctx, corpus, tier, ctx->q_dev, top_k, ranges_dev, n_loc, n_virtual, ctx->hits_pin,
-                                      ctx->status_pin)) != STB_OK) return r;
-      } else {
-        if ((r = stb_launch_scan_topk(ctx, corpus, tier, ctx->q_dev, top_k, ranges_dev, n_loc, n_virtual, ctx->hits_dev,
-                                      ctx->status_dev)) != STB_OK) return r;
-        STB_CUDA(cudaMemcpyAsync(ctx->status_pin, ctx->status_dev, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-        STB_CUDA(cudaMemcpyAsync(ctx->hits_pin, ctx->hits_dev, top_k * sizeof(stb_hit), cudaMemcpyDeviceToHost, ctx->stream));
-      }
+      if ((r = stb_launch_scan_topk(ctx, corpus, tier, ctx->q_dev, top_k, ranges_dev, n_loc, n_virtual, ctx->hits_pin,
+                                    ctx->status_pin)) != STB_OK) return r;
       STB_CUDA(cudaStreamSynchronize(ctx->stream));
       return STB_OK;
     };
     // Tier ladder: q8 (260 B/row) -> h16 (512 B/row) -> f32 (1 KiB/row).  Every tier ends in the
     // same exact f64 re-rank and proves its own result; one that cannot is retried one tier up, so
-    // the answer is the oracle's whichever tier produced it.  Reduced-width copies are used when
-    // they exist (stb_corpus_prepare) and built lazily from the second query on an unchanged
-    // corpus of >= 32768 rows (a one-shot CLI query must not pay a full extra pass to save half
-    // of one); a tier that keeps failing its proofs on this corpus is dropped.
-    stb_corpus *cm = const_cast<stb_corpus *>(corpus);
-    const int max_tier = stb_env_max_tier();
-    const bool lazy_ok = cm->searches_since_change >= 1 && cm->n >= 32768;
-    cm->searches_since_change++;
+    // the answer is the oracle's whichever tier produced it.  A tier that keeps failing its proofs
+    // on this corpus is dropped.
     bool proven = false;
     for (int tier = STB_TIER_Q8; tier >= STB_TIER_H16 && !proven; --tier) {
-      if (tier > max_tier) continue;
-      if (tier == STB_TIER_Q8 && top_k > STB_Q8_MAX_K) continue;
       if (cm->tier_tries[tier] >= 8 && 2 * cm->tier_proven[tier] < cm->tier_tries[tier]) continue;
-      const bool built = (tier == STB_TIER_Q8) ? (cm->q8 && cm->q8_rows == cm->n) : (cm->shadow && cm->shadow_rows == cm->n);
-      // a copy that covers a prefix (rows were appended since) is extended right away: converting the
-      // new rows costs far less than scanning everything at 1 KiB/row
-      const bool extendable = (tier == STB_TIER_Q8) ? (cm->q8 && cm->q8_rows > 0 && !cm->q8_bad) : (cm->shadow && cm->shadow_rows > 0 && !cm->shadow_bad);
-      if (!built && !lazy_ok && !extendable) continue;
-      const int src = (tier == STB_TIER_Q8) ? corpus_ensure_q8(ctx, cm) : corpus_ensure_shadow(ctx, cm);
-      if (src == STB_ERR_STATE) continue;                  // rows that cannot be normalised in fp32
-      if (src != STB_OK) return src;
+      bool ready = false;
+      if ((rc = k1_copy_ready(ctx, cm, tier, top_k, lazy, &ready)) != STB_OK) return rc;
+      if (!ready) continue;
       if ((rc = run_fast(tier)) != STB_OK) return rc;
       proven = ctx->status_pin[1] != 0;
       cm->tier_tries[tier]++;
@@ -695,20 +685,8 @@ int stb_search(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t 
     // When the int8 copy exists (or may be built: same lazy rule as the top-k tiers) the streaming
     // passes read it instead of the f32 rows: its scores are upper bounds u >= c - 2e-5 of the exact
     // cosine, so "u >= floor" collects a superset of "c >= floor" at a quarter of the bytes.
-    stb_corpus *cm = const_cast<stb_corpus *>(corpus);
-    const bool lazy_ok = cm->searches_since_change >= 1 && cm->n >= 32768;
-    cm->searches_since_change++;
-    bool use_q8 = stb_env_max_tier() >= STB_TIER_Q8;
-    if (use_q8) {
-      const bool built = cm->q8 && cm->q8_rows == cm->n;
-      const bool extendable = cm->q8 && cm->q8_rows > 0 && !cm->q8_bad;
-      if (!built && !lazy_ok && !extendable) use_q8 = false;
-      else {
-        const int src = corpus_ensure_q8(ctx, cm);
-        if (src == STB_ERR_STATE) use_q8 = false;
-        else if (src != STB_OK) return src;
-      }
-    }
+    bool use_q8 = false;
+    if ((rc = k1_copy_ready(ctx, cm, STB_TIER_Q8, 0, lazy, &use_q8)) != STB_OK) return rc;
     float floor_cos = -INFINITY;
     double limit = STB_DEFAULT_MAX_DIST;
     uint64_t n_pass = 0;
@@ -785,10 +763,9 @@ int stb_search_topk_dev(stb_ctx *ctx, const stb_corpus *corpus, const float *q_d
   if (corpus->ctx != ctx) { stb_set_error("search_topk_dev: corpus belongs to another context"); return STB_ERR_ARG; }
   if (top_k == 0 || top_k > stb_scan_topk_max_k()) { stb_set_error("search_topk_dev: top_k must be 1..%u", stb_scan_topk_max_k()); return STB_ERR_ARG; }
   if (corpus->n == 0) { stb_set_error("search_topk_dev: empty corpus"); return STB_ERR_STATE; }
-  // candidates from the narrowest copy that already exists (this asynchronous entry point never
-  // builds one: stb_corpus_prepare does); status[1] says whether the result is proven, the
-  // caller's fallback is unchanged
-  return stb_launch_scan_topk(ctx, corpus, best_built_tier(corpus, top_k), q_dev, top_k, nullptr, 0, corpus->n,
+  // candidates from the narrowest copy that already exists; status[1] says whether the result is
+  // proven, the caller's fallback is unchanged
+  return stb_launch_scan_topk(ctx, corpus, best_built_tier(ctx, corpus, top_k), q_dev, top_k, nullptr, 0, corpus->n,
                               out_hits_dev, out_status_dev, nullptr, true);
 }
 
@@ -922,7 +899,7 @@ static int search_topk_xchg_impl(stb_ctx *ctx, const stb_corpus *corpus, const f
   a.world = x->world; a.rank = x->rank; a.max_k = x->max_k;
   a.seq = ++x->seq;
   a.slot = (uint32_t)(a.seq % STB_XCHG_SLOTS);
-  return stb_launch_scan_topk(ctx, corpus, best_built_tier(corpus, top_k), q_dev, top_k, nullptr, 0, corpus->n,
+  return stb_launch_scan_topk(ctx, corpus, best_built_tier(ctx, corpus, top_k), q_dev, top_k, nullptr, 0, corpus->n,
                               out_hits_dev, out_status_dev, &a, overlapped);
 }
 
@@ -1452,26 +1429,11 @@ int stb_search_xchg(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint
   int rc = ctx_use(ctx);
   if (rc) return rc;
   if (!q || !out_hits || !out_n || !out_complete) { stb_set_error("search_xchg: null argument"); return STB_ERR_ARG; }
-  static const bool prof = getenv("STB_XCHG_PROFILE") != nullptr;
-  static double t_enq = 0, t_sync = 0; static long n_calls = 0;
-  auto t0 = std::chrono::steady_clock::now();
   memcpy(ctx->q_pin, q, STB_D * sizeof(float));
   STB_CUDA(cudaMemcpyAsync(ctx->q_dev, ctx->q_pin, STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-  if (stb_env_direct_out()) {        // the merge CTA stores the hits + status straight into pinned host memory
-    if ((rc = search_topk_xchg_impl(ctx, corpus, ctx->q_dev, top_k, x, ctx->hits_pin, ctx->status_pin, false)) != STB_OK) return rc;
-  } else {
-    if ((rc = search_topk_xchg_impl(ctx, corpus, ctx->q_dev, top_k, x, ctx->hits_dev, ctx->status_dev, false)) != STB_OK) return rc;
-    STB_CUDA(cudaMemcpyAsync(ctx->status_pin, ctx->status_dev, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    STB_CUDA(cudaMemcpyAsync(ctx->hits_pin, ctx->hits_dev, top_k * sizeof(stb_hit), cudaMemcpyDeviceToHost, ctx->stream));
-  }
-  auto t1 = std::chrono::steady_clock::now();
+  // the merge CTA stores the hits + status straight into pinned host memory
+  if ((rc = search_topk_xchg_impl(ctx, corpus, ctx->q_dev, top_k, x, ctx->hits_pin, ctx->status_pin, false)) != STB_OK) return rc;
   STB_CUDA(cudaStreamSynchronize(ctx->stream));
-  if (prof) {
-    auto t2 = std::chrono::steady_clock::now();
-    t_enq += std::chrono::duration<double, std::micro>(t1 - t0).count();
-    t_sync += std::chrono::duration<double, std::micro>(t2 - t1).count();
-    if (++n_calls % 50 == 0) fprintf(stderr, "[stb_search_xchg rank %u] calls %ld  enqueue %.1f us  sync %.1f us (avg)\n", x->rank, n_calls, t_enq / n_calls, t_sync / n_calls);
-  }
   const uint32_t n = std::min<uint32_t>(ctx->status_pin[0], top_k);
   memcpy(out_hits, ctx->hits_pin, n * sizeof(stb_hit));
   *out_n = n;
@@ -1508,12 +1470,11 @@ int stb_search_many(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint
     }
     return STB_OK;
   }
-  // many queries amortise the reduced-width copy: build it now (same size rule as the lazy build)
-  stb_corpus *cm = const_cast<stb_corpus *>(corpus);
-  if (nq >= 2 && cm->n >= 32768 && stb_env_max_tier() >= STB_TIER_Q8 && top_k <= STB_Q8_MAX_K && !(cm->q8 && cm->q8_rows == cm->n)) {
-    rc = corpus_ensure_q8(ctx, cm);
-    if (rc != STB_OK && rc != STB_ERR_STATE) return rc;
-  }
+  // many queries amortise the int8 copy: build or extend it now (same size rule as the lazy build);
+  // otherwise the launches read the narrowest copy already built
+  const bool eager = nq >= 2 && corpus->n >= 32768;
+  bool q8_ready = false;
+  if ((rc = k1_copy_ready(ctx, const_cast<stb_corpus *>(corpus), STB_TIER_Q8, top_k, {eager, eager}, &q8_ready)) != STB_OK) return rc;
   if ((rc = dev_reserve(&ctx->bq_dev, &ctx->bq_dev_cap, (size_t)nq * STB_D)) != STB_OK) return rc;
   if ((rc = ensure_hits_pin(ctx, (size_t)nq * top_k)) != STB_OK) return rc;
   if ((size_t)nq * STB_D > ctx->many_q_pin_cap) {
@@ -1530,7 +1491,7 @@ int stb_search_many(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint
   }
   memcpy(ctx->many_q_pin, q, (size_t)nq * STB_D * sizeof(float));
   STB_CUDA(cudaMemcpyAsync(ctx->bq_dev, ctx->many_q_pin, (size_t)nq * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-  const int tier = best_built_tier(corpus, top_k);
+  const int tier = q8_ready ? STB_TIER_Q8 : best_built_tier(ctx, corpus, top_k);
   for (uint32_t i = 0; i < nq; ++i) {
     stb_hit *oh = ctx->hits_pin + (size_t)i * top_k;
     uint32_t *os = ctx->many_status_pin + 4 * (size_t)i;

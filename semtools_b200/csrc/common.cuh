@@ -12,12 +12,8 @@
 
 #define STB_D 256           // floats per row
 #define STB_ROW_F4 64       // float4 per row
-#ifndef STB_SCAN_THREADS
 #define STB_SCAN_THREADS 256
-#endif
-#ifndef STB_SCAN_MINB
 #define STB_SCAN_MINB 2     // CTAs per SM the scan kernels are register-budgeted for
-#endif
 #define STB_SCAN_WARPS (STB_SCAN_THREADS / 32)
 #define STB_SORT_CAP 1024   // keys one CTA sorts in shared memory
 // Rigorous bound (with ~4x slack) on |approx cosine - exact cosine| for the fp32
@@ -116,7 +112,6 @@ struct stb_ctx {
   size_t ranges_cap;
   int *err_flag;            // device int: scratch flag of the copy builders, stb_embed and K2's query shadow; zeroed before each use
   unsigned int *hist_dev;       // 4096-bin score histogram (large-k path)
-  unsigned long long *dbg_dev;  // 8 u64 phase timestamps (STB_TAIL_TIMING builds; else unused)
   // cudaFuncSetAttribute is per DEVICE: remembered per context, never in function statics
   // (one process may hold contexts on several GPUs)
   uint32_t func_attr_mask;
@@ -233,6 +228,21 @@ struct stb_corpus {
 
 // Row ranges as stb_search takes them: n half-open [begin, end) pairs, ascending and disjoint (api.cu).
 bool stb_ranges_ordered(const uint64_t *ranges, uint32_t n);
+
+// Validates such ranges (global rows) and clips them to a shard's rows [row_base, row_base + n_rows):
+// emit(begin, end) receives each non-empty piece in local rows, in order.  STB_ERR_RANGE, with `what`
+// leading the message, when the ranges are not ascending and disjoint.
+template <class Emit>
+int stb_clip_ranges(const char *what, const uint64_t *ranges, uint32_t n, uint64_t row_base, uint64_t n_rows, Emit &&emit) {
+  if (!stb_ranges_ordered(ranges, n)) { stb_set_error("%s: row_ranges must be ascending, disjoint, half-open", what); return STB_ERR_RANGE; }
+  const uint64_t hi = row_base + n_rows;
+  for (uint32_t i = 0; i < n; ++i) {
+    const uint64_t b = ranges[2 * i] > row_base ? ranges[2 * i] : row_base;
+    const uint64_t e = ranges[2 * i + 1] < hi ? ranges[2 * i + 1] : hi;
+    if (b < e) emit(b - row_base, e - row_base);
+  }
+  return STB_OK;
+}
 
 // stb_corpus_update / stb_corpus_remove without their refusal of live IVF-PQ indexes (api.cu).  With a
 // hook, an index that follows the change (stb_ivfpq_update / stb_ivfpq_remove) acts at the points where it

@@ -18,12 +18,8 @@
 
 #define STB_EMBED_THREADS 256
 #define STB_EMBED_WARPS (STB_EMBED_THREADS / 32)
-#ifndef STB_EMBED_DEPTH
 #define STB_EMBED_DEPTH 4     // tokens (2 x 512-byte warp loads each) in flight per warp
-#endif
-#ifndef STB_EMBED_MINB
 #define STB_EMBED_MINB 3      // CTAs per SM the register budget is sized for
-#endif
 
 struct EmbedArgs {
   const float4 *E;

@@ -1870,18 +1870,10 @@ int stb_ivfpq_search_filtered(stb_ivfpq *x, const float *q, uint32_t nq, uint32_
   // global ranges -> local [begin, end) pairs clipped to the indexed rows [row_base, row_base + n)
   std::vector<uint32_t> loc;
   if (row_ranges) {
-    if (!stb_ranges_ordered(row_ranges, n_ranges)) {
-      stb_set_error("ivfpq_search_filtered: row_ranges must be ascending, disjoint, half-open");
-      return STB_ERR_RANGE;
-    }
-    const uint64_t lo = x->corpus->row_base, hi = lo + x->n;
     loc.reserve(2 * (size_t)n_ranges);
-    for (uint32_t i = 0; i < n_ranges; ++i) {
-      uint64_t b = row_ranges[2 * i], e = row_ranges[2 * i + 1];
-      b = std::max(b, lo); e = std::min(e, hi);
-      if (b >= e) continue;
-      loc.push_back((uint32_t)(b - lo)); loc.push_back((uint32_t)(e - lo));
-    }
+    const int rc = stb_clip_ranges("ivfpq_search_filtered", row_ranges, n_ranges, x->corpus->row_base, x->n,
+                                   [&](uint64_t b, uint64_t e) { loc.push_back((uint32_t)b); loc.push_back((uint32_t)e); });
+    if (rc != STB_OK) return rc;
   }
   if (top_k == 0 || (row_ranges && loc.empty())) {             // nothing can be returned: no launch
     for (uint32_t i = 0; i < nq; ++i) { out_n[i] = 0; if (out_scanned) out_scanned[i] = 0; }

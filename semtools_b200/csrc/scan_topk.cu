@@ -28,25 +28,15 @@
 #include "common.cuh"
 #include "row_encode.cuh"
 
-#ifndef STB_SCAN_U
 #define STB_SCAN_U 2   // rows per 8-lane group per iteration (loads in flight = 8*U float4)
-#endif
-#ifndef STB_SCAN_LD
-#define STB_SCAN_LD 0  // 0: ld.global.nc.L1::no_allocate  1: __ldcs  2: __ldg
-#endif
 
+// streamed once: read through the non-coherent path without allocating in L1
 __device__ __forceinline__ float4 stb_ld_stream(const float4 *p) {
-#if STB_SCAN_LD == 0
   float4 r;
   asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%4];"
                : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w)
                : "l"(p));
   return r;
-#elif STB_SCAN_LD == 1
-  return __ldcs(p);
-#else
-  return __ldg(p);
-#endif
 }
 
 struct ScanArgs {
@@ -56,7 +46,8 @@ struct ScanArgs {
   const uint64_t *vstart;    // [n_ranges+1] virtual prefix (ranges mode)
   const uint64_t *rbegin;    // [n_ranges]   local first row of each range
   uint32_t n_ranges;
-  // dynamic tile schedule (top-k kernel; null = static warp-strided schedule):
+  // dynamic tile schedule, always used by the top-k kernel; null in the collect and histogram
+  // kernels, which keep the static warp-strided schedule:
   unsigned long long *tickets;   // monotonic counter shared by every launch of the context
   unsigned long long t_base;     // its value when this launch starts (host-tracked)
   uint64_t t_bulk;               // tickets [0, t_bulk) cover STB_TICKET_TILES tiles each, later ones one tile
@@ -878,26 +869,12 @@ struct TopkArgs {
   uint32_t *out_status;
   uint32_t top_k;
   StbXchgArgs xchg;          // world == 0: no cross-GPU exchange
-  unsigned long long *dbg;   // STB_TAIL_TIMING builds only: phase timestamps (ns)
-  const uint8_t *shadow;     // SRC == 1: 16-bit normalised corpus shadow (UMMA tile layout)
+  const uint8_t *shadow;    // SRC == 1: 16-bit normalised corpus shadow (UMMA tile layout)
   uint32_t early_trigger;    // overlapped launch: release the dependent launch at kernel start
   const uint8_t *q8;         // SRC == 2: int8 codes [n][256] ...
   const float *q8_scale;     //           ... and per-row scales [n]
   StbQ4Args q4;              //           ... and the prefilter's copy, threshold words, debug counter
 };
-
-__device__ __forceinline__ unsigned long long stb_globaltimer() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
-#ifdef STB_TAIL_TIMING
-#define STB_T_MIN(i) do { if (threadIdx.x == 0 && args.dbg) atomicMin(args.dbg + (i), stb_globaltimer()); } while (0)
-#define STB_T_MAX(i) do { if (threadIdx.x == 0 && args.dbg) atomicMax(args.dbg + (i), stb_globaltimer()); } while (0)
-#else
-#define STB_T_MIN(i) do { } while (0)
-#define STB_T_MAX(i) do { } while (0)
-#endif
 
 // ---- peer-memory exchange (fused K1 -> all-gather -> K4) ------------------------------
 // Every rank owns one exchange buffer (cudaMalloc, mapped into all peers through CUDA
@@ -962,7 +939,6 @@ stb_scan_topk_kernel(const TopkArgs args) {
   __shared__ uint64_t s_r[KF];
   __shared__ int s_nv[2];
 
-  STB_T_MIN(0);                      // first CTA starts
   // co-scan: the tile this launch's pass starts at, fixed before the dependent is released so that
   // the dependent's first CTA can read it
   __shared__ uint32_t s_off;          // (stb_for_each_tile reads it with RANGES == 0 only)
@@ -985,7 +961,6 @@ stb_scan_topk_kernel(const TopkArgs args) {
     stb_scan_q4<U, RANGES>(args.scan, args.q8, args.q8_scale, args.q4, scratch, scratch + STB_Q4_QUEUE, sink, &s_off);
   } else if constexpr (SRC == 1) stb_scan_shadow<U, RANGES>(args.scan, args.shadow, sink, &s_off);
   else stb_scan_rows<U, RANGES>(args.scan, sink, &s_off);
-  STB_T_MAX(1);                      // last CTA leaves the scan loop
   // Programmatic dependent launch: the scan above reads only the corpus and the query,
   // so the NEXT query's kernel may start streaming as soon as every CTA of this one has
   // left its scan loop; this kernel's merge / re-rank tail then overlaps with it.
@@ -1024,7 +999,6 @@ stb_scan_topk_kernel(const TopkArgs args) {
     bound = (s_T > kOrdNegInf) ? s_T : 0u;
     if (c > keep) bound = max(bound, stb_f2ord(stb_key_score(skeys[keep - 1])));
   }
-  STB_T_MAX(2);                      // last CTA-level merge done
 
   // Everything below writes scratch shared with the PREVIOUS launch on this stream
   // (keys, tickets, exchange slots): wait until that grid has completed and flushed.
@@ -1100,8 +1074,6 @@ stb_scan_topk_kernel(const TopkArgs args) {
       my_id = group;
     }
   }
-  STB_T_MAX(3);                      // survivor holds the global best KF
-  STB_T_MAX(4);
 
   // ---- exact re-rank of the best KF in canonical arithmetic --------------------------
   // Rows are staged through shared memory (coalesced, one DRAM latency), then one
@@ -1194,7 +1166,6 @@ stb_scan_topk_kernel(const TopkArgs args) {
   }
   __syncthreads();
   stb_cta_sort_hits(s_d, s_r, KF);
-  STB_T_MAX(5);                      // exact re-rank + hit sort done
   const int n_valid = s_nv[0], n_pass = s_nv[1];
   const uint32_t k = args.top_k;
   const uint32_t n_out = min((uint32_t)n_pass, k);
@@ -1282,31 +1253,18 @@ static int stb_pick_e(uint32_t top_k) {
 #define STB_SHADOW_SCAN_U 4     // 4 rows x 4 LDG.128 per lane in flight = the f32 path's 2 x 8
 #define STB_Q8_SCAN_U 8         // 8 rows x 2 LDG.128
 
-// STB_SCAN_CTAS_PER_SM (tuning aid): resident CTAs per SM the top-k grid is sized for
-// (default: what the occupancy calculator allows, 2 with the 128-register budget).
-// STB_SCAN_TICKETS=0 (tuning aid): static warp-strided tile partition instead of tickets.
-static bool stb_scan_tickets_enabled() {
-  static const bool v = [] { const char *e = getenv("STB_SCAN_TICKETS"); return !(e && e[0] == '0'); }();
-  return v;
-}
-static int stb_scan_ctas_per_sm_override() {
-  static const int v = [] { const char *e = getenv("STB_SCAN_CTAS_PER_SM"); return e ? atoi(e) : 0; }();
-  return v;
-}
-
 // coscan: the corpus an overlapped launch may co-scan (null: never; stb_launch_scan_topk)
 template <int E, int RANGES, int SRC = 0, int EF = E>
 static int stb_launch_topk_t(stb_ctx *ctx, const TopkArgs &a_in, bool overlapped, const void *coscan) {
   constexpr int kU = SRC == 2 ? STB_Q4_SCAN_U : (SRC == 1 ? STB_SHADOW_SCAN_U : STB_SCAN_U);
   auto kern = stb_scan_topk_kernel<E, kU, RANGES, SRC, EF>;
+  // resident CTAs per SM the grid is sized for: what the occupancy calculator allows (2 with the
+  // 128-register budget)
   int occ = 0;
   STB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, STB_SCAN_THREADS, 0));
   if (occ < 1) occ = 1;
-  const int ovr = stb_scan_ctas_per_sm_override();
-  if (ovr >= 1 && ovr < occ) occ = ovr;
   TopkArgs a = a_in;
-  const bool use_tickets = stb_scan_tickets_enabled();
-  overlapped = overlapped && use_tickets && occ >= 2;
+  overlapped = overlapped && occ >= 2;
   if (overlapped) occ = 1;                 // two consecutive grids co-reside, one CTA per SM each
   a.early_trigger = overlapped ? 1u : 0u;
   const uint64_t tiles = (a.scan.n_virtual + 4 * kU - 1) / (4 * kU);
@@ -1322,37 +1280,35 @@ static int stb_launch_topk_t(stb_ctx *ctx, const TopkArgs &a_in, bool overlapped
   // tile tickets (stb_for_each_tile): bulk tickets of STB_TICKET_TILES tiles, then the last ~2 tiles
   // per warp one by one.  The launch advances the counter by n_tickets + total_warps exactly.
   const uint64_t warps_total = grid * STB_SCAN_WARPS;
-  if (use_tickets) {
-    const uint64_t single = std::min<uint64_t>(tiles, 2 * warps_total);
-    a.scan.t_bulk = (tiles - single) / STB_TICKET_TILES;
-    const uint64_t n_tickets = a.scan.t_bulk + (tiles - a.scan.t_bulk * STB_TICKET_TILES);
-    // one counter serves back-to-back launches (a grid starts drawing only after its predecessor's scan, the
-    // validated default); the ring is needed -- and used -- from the first overlapped launch on, when two
-    // consecutive scans co-run (at most ~3 grids are ever in flight)
-    if (overlapped) ctx->ticket_ring = true;
-    const int slot = ctx->ticket_ring ? (int)(ctx->topk_launches++ % STB_TICKET_SLOTS) : 0;
-    a.scan.tickets = ctx->tickets + slot;
-    a.scan.t_base = ctx->ticket_next[slot];
-    ctx->ticket_next[slot] += n_tickets + warps_total;
-    // co-scan: follow the last launch if it was one too, on the same corpus copy and rows (hence the
-    // same tiles); any other launch in between -- synchronous, sharded, ranged -- ends the series
-    const uint32_t tag = (uint32_t)ctx->topk_launches;   // the launch count, 0 only after a wrap: no co-scan then
-    const bool co = overlapped && coscan && RANGES == 0 && ctx->ticket_ring && tag != 0;
-    if (ctx->ticket_ring) ctx->coscan_tag[slot] = co ? tag : 0u;
-    if (co) {
-      auto &p = ctx->coscan_prev;
-      a.co.word = ctx->coscan_off + slot;
-      a.co.tag = tag;
-      if (p.corpus == coscan && p.src == SRC && p.n_virtual == a.scan.n_virtual && p.tiles == tiles) {
-        a.co.pred_tag = p.tag;
-        a.co.pred_word = ctx->coscan_off + p.slot;
-        a.co.pred_tickets = ctx->tickets + p.slot;
-        a.co.pred_t_base = p.t_base;
-        a.co.pred_t_bulk = p.t_bulk;
-      }
-      p.corpus = coscan; p.src = SRC; p.n_virtual = a.scan.n_virtual; p.tiles = tiles;
-      p.slot = slot; p.t_base = a.scan.t_base; p.t_bulk = a.scan.t_bulk; p.tag = tag;
+  const uint64_t single = std::min<uint64_t>(tiles, 2 * warps_total);
+  a.scan.t_bulk = (tiles - single) / STB_TICKET_TILES;
+  const uint64_t n_tickets = a.scan.t_bulk + (tiles - a.scan.t_bulk * STB_TICKET_TILES);
+  // one counter serves back-to-back launches (a grid starts drawing only after its predecessor's scan, the
+  // validated default); the ring is needed -- and used -- from the first overlapped launch on, when two
+  // consecutive scans co-run (at most ~3 grids are ever in flight)
+  if (overlapped) ctx->ticket_ring = true;
+  const int slot = ctx->ticket_ring ? (int)(ctx->topk_launches++ % STB_TICKET_SLOTS) : 0;
+  a.scan.tickets = ctx->tickets + slot;
+  a.scan.t_base = ctx->ticket_next[slot];
+  ctx->ticket_next[slot] += n_tickets + warps_total;
+  // co-scan: follow the last launch if it was one too, on the same corpus copy and rows (hence the
+  // same tiles); any other launch in between -- synchronous, sharded, ranged -- ends the series
+  const uint32_t tag = (uint32_t)ctx->topk_launches;   // the launch count, 0 only after a wrap: no co-scan then
+  const bool co = overlapped && coscan && RANGES == 0 && ctx->ticket_ring && tag != 0;
+  if (ctx->ticket_ring) ctx->coscan_tag[slot] = co ? tag : 0u;
+  if (co) {
+    auto &p = ctx->coscan_prev;
+    a.co.word = ctx->coscan_off + slot;
+    a.co.tag = tag;
+    if (p.corpus == coscan && p.src == SRC && p.n_virtual == a.scan.n_virtual && p.tiles == tiles) {
+      a.co.pred_tag = p.tag;
+      a.co.pred_word = ctx->coscan_off + p.slot;
+      a.co.pred_tickets = ctx->tickets + p.slot;
+      a.co.pred_t_base = p.t_base;
+      a.co.pred_t_bulk = p.t_bulk;
     }
+    p.corpus = coscan; p.src = SRC; p.n_virtual = a.scan.n_virtual; p.tiles = tiles;
+    p.slot = slot; p.t_base = a.scan.t_base; p.t_bulk = a.scan.t_bulk; p.tag = tag;
   }
   if (!a.co.word) ctx->coscan_prev.corpus = nullptr;
   cudaLaunchConfig_t cfg;
@@ -1411,7 +1367,6 @@ int stb_launch_scan_topk(stb_ctx *ctx, const stb_corpus *c, int tier, const floa
   a.out_status = out_status_dev;
   a.top_k = top_k;
   if (xchg) a.xchg = *xchg; else memset(&a.xchg, 0, sizeof(a.xchg));
-  a.dbg = ctx->dbg_dev;
   a.early_trigger = 0;
   a.shadow = c->shadow;
   a.q8 = c->q8;

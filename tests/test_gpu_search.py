@@ -456,9 +456,9 @@ def test_large_k_histogram_path(ctx, n, k):
     assert got["row"].tolist() == [int(x) for x in r2]
 
 
-def test_direct_host_output_switch_gives_identical_hits(ctx, monkeypatch):
-    """Default: the scan kernel stores hits + status straight into pinned host memory;
-    STB_DIRECT_OUT=0 goes through device buffers + two D2H copies.  Same hits either way."""
+def test_hits_stored_straight_into_pinned_host_memory_match_the_oracle(ctx):
+    """stb_search's scan kernel stores hits + status straight into pinned host memory (no D2H copy);
+    what the host reads there is the oracle's answer, ties and the widest register list included."""
     rng = np.random.default_rng(321)
     rows = unit_rows(rng, 50_000)
     rows[777] = rows[5]
@@ -466,11 +466,7 @@ def test_direct_host_output_switch_gives_identical_hits(ctx, monkeypatch):
     c.append(rows)
     for k in (1, 10, 96):
         for qi in (5, 100, 49_999):
-            monkeypatch.setenv("STB_DIRECT_OUT", "0")
-            want = c.search(rows[qi], top_k=k)
-            monkeypatch.delenv("STB_DIRECT_OUT", raising=False)
             got = c.search(rows[qi], top_k=k)
-            assert np.array_equal(got, want)
             r, d = oracle.search_rows(rows, rows[qi], top_k=k)
             assert got["row"].tolist() == [int(x) for x in r] and np.array_equal(got["distance"], d)
 
@@ -598,12 +594,105 @@ def test_lazy_tier_build_waits_for_the_second_query(ctx, monkeypatch):
     assert small.tier_stats()["q8"]["built_rows"] == 0                  # below 32768 rows: never lazily
 
 
+def test_threshold_and_large_k_build_only_the_int8_copy_lazily(ctx, monkeypatch):
+    """Threshold mode and top_k beyond the register lists follow the lazy rule of the top-k tiers for
+    the int8 copy alone: built on the second search since a change, extended on the first search after
+    an append; the 16-bit shadow is never built and no tier counts a try."""
+    monkeypatch.delenv("STB_SCAN_TIER", raising=False)
+    rng = np.random.default_rng(77)
+    rows = unit_rows(rng, 40_000)
+    q = unit_rows(rng, 1)[0]
+    c = make_corpus(ctx, rows)
+    r, d = oracle.search_rows(rows, q, top_k=3, max_distance=0.9)
+    check(c.search(q, top_k=3, max_distance=0.9), r, d)
+    assert c.tier_stats()["q8"]["built_rows"] == 0                      # first search: f32 rows only
+    check(c.search(q, top_k=3, max_distance=0.9), r, d)
+    st = c.tier_stats()
+    assert st["q8"]["built_rows"] == 40_000 and st["h16"]["built_rows"] == 0, st
+    c.append(rows[:10])
+    rows2 = np.concatenate([rows, rows[:10]])
+    r, d = oracle.search_rows(rows2, q, top_k=200)
+    check(c.search(q, top_k=200), r, d)
+    st = c.tier_stats()
+    assert st["q8"]["built_rows"] == 40_010 and st["h16"]["built_rows"] == 0, st
+    assert all(v["tries"] == 0 for v in st.values()), st
+
+
+def test_search_many_builds_the_int8_copy_only_for_several_queries(ctx, monkeypatch):
+    """stb_search_many builds or extends the int8 copy when it holds >= 2 queries (>= 32768 rows); one
+    query reads the copies already built, whatever its history, and counts no tier."""
+    monkeypatch.delenv("STB_SCAN_TIER", raising=False)
+    rng = np.random.default_rng(616)
+    rows = unit_rows(rng, 40_000)
+    qs = unit_rows(rng, 2)
+    c = make_corpus(ctx, rows)
+    for _ in range(3):
+        got = c.search_many(qs[:1], top_k=10)
+        r, d = oracle.search_rows(rows, qs[0], top_k=10)
+        check(got[0], r, d)
+    st = c.tier_stats()
+    assert st["q8"]["built_rows"] == 0 and st["h16"]["built_rows"] == 0, st
+    assert all(v["tries"] == 0 for v in st.values()), st
+    c.search_many(qs, top_k=10)
+    assert c.tier_stats()["q8"]["built_rows"] == 40_000
+    c.append(rows[:10])
+    rows2 = np.concatenate([rows, rows[:10]])
+    got = c.search_many(qs[:1], top_k=10)
+    r, d = oracle.search_rows(rows2, qs[0], top_k=10)
+    check(got[0], r, d)
+    assert c.tier_stats()["q8"]["built_rows"] == 40_000                 # one query: the prefix is not extended
+    got = c.search_many(qs, top_k=10)
+    for i in range(2):
+        r, d = oracle.search_rows(rows2, qs[i], top_k=10)
+        check(got[i], r, d)
+    assert c.tier_stats()["q8"]["built_rows"] == 40_010
+
+
+def test_device_entry_point_reads_only_fully_built_copies(ctx, monkeypatch):
+    """stb_search_topk_dev never builds or extends a copy: it reads the narrowest one that covers every
+    row and that STB_SCAN_TIER allows, which status[3] >> 16 reports (0 f32, 1 h16, 2 q8)."""
+    torch = pytest.importorskip("torch")
+    monkeypatch.delenv("STB_SCAN_TIER", raising=False)
+    rng = np.random.default_rng(4040)
+    rows = unit_rows(rng, 40_000)
+    q = unit_rows(rng, 1)[0]
+    c = make_corpus(ctx, rows)
+    dev = torch.device("cuda:0")
+    q_dev = torch.from_numpy(q).to(dev)
+    hits = torch.zeros((10, 2), dtype=torch.float64, device=dev)
+    status = torch.zeros(4, dtype=torch.int32, device=dev)
+
+    def tier_read(rows_now):
+        torch.cuda.synchronize()
+        c.search_topk_dev(q_dev.data_ptr(), 10, hits.data_ptr(), status.data_ptr())
+        ctx.sync()
+        st = status.cpu().numpy()
+        assert st[1] == 1, st
+        r, d = oracle.search_rows(rows_now, q, top_k=10)
+        check(np.ascontiguousarray(hits.cpu().numpy()).view(capi.HIT_DTYPE).reshape(-1)[: st[0]], r, d)
+        return int(st[3]) >> 16
+
+    assert [tier_read(rows) for _ in range(3)] == [0, 0, 0]            # nothing built: never builds one
+    assert c.tier_stats()["q8"]["built_rows"] == 0
+    c.prepare()
+    assert tier_read(rows) == 2
+    c.append(rows[:10])
+    rows2 = np.concatenate([rows, rows[:10]])
+    assert tier_read(rows2) == 0                                         # a prefix is not extended ...
+    st = c.tier_stats()
+    assert st["q8"]["built_rows"] == 40_000 and st["h16"]["built_rows"] == 40_000, st
+    c.prepare()                                                          # ... until something else does
+    assert tier_read(rows2) == 2
+    monkeypatch.setenv("STB_SCAN_TIER", "h16")
+    assert tier_read(rows2) == 1
+    assert all(v["tries"] == 0 for v in c.tier_stats().values())
+
+
 @pytest.mark.parametrize("tier", ["f32", "h16", "q8"])
 def test_ticket_schedule_stays_consistent_and_order_independent(ctx, monkeypatch, tier):
     """The dynamic tile tickets must (a) leave the device counter exactly where the host booked it
-    after launches of many shapes, including back-to-back PDL launches, and (b) give the same hits
-    as the static partition (STB_SCAN_TICKETS is read once per process, so (b) is covered by the
-    oracle comparison here and by every other test in this file)."""
+    after launches of many shapes, including back-to-back PDL launches, and (b) give the oracle's
+    hits whichever warp draws which tile (the co-scan starts each pass at a different tile)."""
     torch = pytest.importorskip("torch")
     rng = np.random.default_rng(2024)
     monkeypatch.setenv("STB_SCAN_TIER", tier)
