@@ -27,8 +27,7 @@
  * Environment switches (read per call; results are identical whatever their
  * value -- they select how candidates are found, never how the returned
  * distances are computed): STB_SCAN_TIER=f32|h16|q8 (narrowest candidate copy K1
- * may read, default q8), STB_BATCH_V1=1, STB_IVFPQ_V1=1, STB_IVFPQ_BATCH_KEEP=k,
- * STB_SCAN_OVERLAP=1 (INTEGRATION.md, 5b).
+ * may read, default q8), STB_IVFPQ_BATCH_KEEP=k (INTEGRATION.md, 5b).
  */
 #ifndef SEMTOOLS_B200_H
 #define SEMTOOLS_B200_H
@@ -240,8 +239,8 @@ int stb_search_topk_dev(stb_ctx *ctx, const stb_corpus *corpus,
  * built lazily, 512 B/row, extended after appends; stb_corpus_prepare_batch builds it ahead
  * of time) is multiplied with the query tile on the wgmma tensor cores.  Pipeline v2 (top_k <= 64
  * when the sampled threshold fits, see DESIGN §4) emits every row whose approximate score reaches a
- * per-query threshold and re-scores those exactly; pipeline v1 (larger top_k, small corpora,
- * STB_BATCH_V1=1) re-scores the 32 most promising 32-row sub-tiles per query.  Re-scores use the
+ * per-query threshold and re-scores those exactly; pipeline v1 (top_k > 64, or wherever v2 does not
+ * fit) re-scores the 32 most promising 32-row sub-tiles per query.  Re-scores use the
  * canonical f64 distance on the f32 rows, and a result is accepted only if the 16-bit error bound
  * proves no other row can enter the top-k; unproven queries are answered by the single-query path
  * (stb_search).  Results are therefore identical to stb_search.
@@ -326,8 +325,8 @@ int stb_search_batch_xchg_dev(stb_ctx *ctx, const stb_corpus *corpus, const floa
  * v1: <= 4096), every row is re-ranked and the hits equal stb_search's.
  * stb_ivfpq_search: nprobe is clamped to [1, min(nlist, 1024)], rerank to [top_k, 4096];
  * top_k > 4096 is STB_ERR_ARG.  *out_scanned = codes scanned (forced rows not counted).  It runs the
- * fused search (v2, stb_ivfpq_search_dev's) when rerank <= 1024 and top_k <= 1024, else the
- * multi-launch search (v1; also with STB_IVFPQ_V1=1).  v2's funnel: 32-code chunks dealt over 32
+ * fused search (v2, stb_ivfpq_search_dev's) when rerank <= 1024 and top_k <= 1024, and the
+ * multi-launch search (v1) when rerank or top_k exceeds 1024.  v2's funnel: 32-code chunks dealt over 32
  * CTAs then 16 warps, 64 best per warp, 64 best per CTA, then the `rerank` best of those 2048; it
  * returns the `rerank` best ADC scores exactly when no warp and no CTA holds more than 64 of them.
  * v1: 64 best per warp over enough warps to hold min(rerank, codes scanned) candidates. */

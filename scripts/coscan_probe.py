@@ -3,7 +3,6 @@
 Each mode runs in a subprocess of its own, because the library path is fixed when it is first loaded:
   full     the parent commit (--parent-root: a checkout with its library built, loaded through
            STB_LIB_PATH with that checkout's bindings): full grid, one query per pass
-  overlap  the parent commit with STB_SCAN_OVERLAP=1: overlapped grids, every query from tile 0
   coscan   this build: overlapped grids, each query starting where its predecessor reads
   NAME     --extra NAME=PATH: another build of this tree (e.g. another ticket size), co-scan
 The modes alternate over --rounds rounds.  Each subprocess builds the headline corpus (--rows) and
@@ -74,7 +73,7 @@ def worker(a):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--parent-root", default=None, help="a built checkout of the parent commit (modes full, overlap)")
+    ap.add_argument("--parent-root", default=None, help="a built checkout of the parent commit (mode full)")
     ap.add_argument("--extra", action="append", default=[], help="NAME=PATH: another co-scan build to time")
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--rows", type=int, default=10_000_000)
@@ -96,18 +95,17 @@ def main():
     modes = []
     if a.parent_root:
         plib = os.path.join(a.parent_root, "semtools_b200", "lib", "libsemtools_b200.so")
-        modes += [("full", a.parent_root, plib, {}), ("overlap", a.parent_root, plib, {"STB_SCAN_OVERLAP": "1"})]
-    modes.append(("coscan", ROOT, own, {}))
+        modes.append(("full", a.parent_root, plib))
+    modes.append(("coscan", ROOT, own))
     for e in a.extra:
         name, path = e.split("=", 1)
-        modes.append((name, ROOT, path, {}))
+        modes.append((name, ROOT, path))
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                           capture_output=True, text=True).stdout.strip()
     results = []
     for r in range(a.rounds):
-        for name, root, lib, env in modes:
-            e = {k: v for k, v in os.environ.items() if k not in ("STB_SCAN_OVERLAP", "STB_SCAN_TIER")}
-            e.update(env)
+        for name, root, lib in modes:
+            e = {k: v for k, v in os.environ.items() if k != "STB_SCAN_TIER"}
             e["STB_LIB_PATH"] = os.path.abspath(lib)
             cmd = [sys.executable, os.path.abspath(__file__), "--worker", "--mode", name, "--rows", str(a.rows),
                    "--rows2", str(a.rows2), "--tiers", a.tiers, "--topk", str(a.topk), "--queries", str(a.queries),

@@ -352,7 +352,7 @@ enum CorpusChange { CORPUS_APPEND, CORPUS_ROWS_REWRITTEN, CORPUS_CLEAR };
 static void corpus_changed(stb_corpus *c, CorpusChange kind) {
   if (kind == CORPUS_CLEAR) { c->shadow_rows = 0; c->q8_rows = 0; }
   if (kind != CORPUS_APPEND) ++c->epoch;
-  if (kind == CORPUS_ROWS_REWRITTEN && c->ctx->coscan_prev.corpus == c) c->ctx->coscan_prev.corpus = nullptr;
+  if (kind == CORPUS_ROWS_REWRITTEN && c->ctx->coscan_prev.rows == c->rows) c->ctx->coscan_prev.rows = nullptr;
   c->searches_since_change = 0;
   memset(c->tier_tries, 0, sizeof(c->tier_tries));
   memset(c->tier_proven, 0, sizeof(c->tier_proven));
@@ -483,13 +483,8 @@ static int stb_env_max_tier() {
 }
 // The single-GPU asynchronous entry points (stb_search_topk_dev, stb_search_many without an exchange) always
 // use the overlapped launch mode and co-scan (scan_topk.cu: stb_coscan_offset): back-to-back queries share
-// each tile's HBM read.  STB_SCAN_OVERLAP=1 (opt-in until timed on a multi-GPU box) gives the sharded forms
-// (stb_search_topk_xchg, stb_search_many with an exchange) the overlapped mode, without the co-scan; by default
-// they launch like the synchronous entry points (full grid, dependent released after the scan).
-static bool stb_env_overlap() {
-  const char *e = getenv("STB_SCAN_OVERLAP");
-  return e && e[0] == '1';
-}
+// each tile's HBM read.  The sharded forms (stb_search_topk_xchg, stb_search_many with an exchange) launch
+// like the synchronous entry points (full grid, dependent released after the scan).
 
 // What a K1 entry point may do to a reduced-width candidate copy that does not cover every row yet:
 // build it from nothing (or rebuild one marked bad), and convert the rows appended behind a valid prefix.
@@ -884,8 +879,8 @@ int stb_xchg_connect_local(stb_xchg *x, stb_xchg *const *peers) {
   return STB_OK;
 }
 
-static int search_topk_xchg_impl(stb_ctx *ctx, const stb_corpus *corpus, const float *q_dev, uint32_t top_k,
-                                 stb_xchg *x, stb_hit *out_hits_dev, uint32_t *out_status_dev, bool overlapped) {
+int stb_search_topk_xchg(stb_ctx *ctx, const stb_corpus *corpus, const float *q_dev, uint32_t top_k,
+                         stb_xchg *x, stb_hit *out_hits_dev, uint32_t *out_status_dev) {
   int rc = ctx_use(ctx);
   if (rc) return rc;
   if (!corpus || !q_dev || !x || !out_hits_dev || !out_status_dev) { stb_set_error("search_topk_xchg: null argument"); return STB_ERR_ARG; }
@@ -900,12 +895,7 @@ static int search_topk_xchg_impl(stb_ctx *ctx, const stb_corpus *corpus, const f
   a.seq = ++x->seq;
   a.slot = (uint32_t)(a.seq % STB_XCHG_SLOTS);
   return stb_launch_scan_topk(ctx, corpus, best_built_tier(ctx, corpus, top_k), q_dev, top_k, nullptr, 0, corpus->n,
-                              out_hits_dev, out_status_dev, &a, overlapped);
-}
-
-int stb_search_topk_xchg(stb_ctx *ctx, const stb_corpus *corpus, const float *q_dev, uint32_t top_k,
-                         stb_xchg *x, stb_hit *out_hits_dev, uint32_t *out_status_dev) {
-  return search_topk_xchg_impl(ctx, corpus, q_dev, top_k, x, out_hits_dev, out_status_dev, stb_env_overlap());
+                              out_hits_dev, out_status_dev, &a);
 }
 
 // ----------------------------------------------------------------- K2 batched search ---
@@ -1235,10 +1225,8 @@ int stb_search_batch_dev(stb_ctx *ctx, const stb_corpus *corpus_c, const float *
   const uint32_t m_tiles = (nq + 127) / 128, q_pad = m_tiles * 128;
   const uint32_t n_tiles = (uint32_t)((corpus->n + 255) / 256), n_sub = n_tiles * 8;
   // Pipeline v2 (default): sampled threshold -> candidate-emitting wgmma epilogue -> exact finish
-  // (batch_scan.cu).  Proves every query for any top_k <= 64 unless a capacity overflows.
-  // STB_BATCH_V1=1 forces the round-1 maxima/select/finish pipeline (also used when v2 does not fit).
-  const char *v1_env = getenv("STB_BATCH_V1");            // read per call so one process can compare both
-  const bool force_v1 = v1_env != nullptr && v1_env[0] == '1';
+  // (batch_scan.cu).  Proves every query for any top_k <= 64 unless a capacity overflows.  The round-1
+  // maxima/select/finish pipeline (v1) runs for top_k > 64 and wherever v2 does not fit.
   // v2 sampling: ~4 COMPLETE tiles per SM, strided over the shard (a padding row must never stand
   // in for a real one).  Expected candidates per query ~ top_k * n_full / n_sample * e^(2 EPS x / sigma^2)
   // (x = top score, sigma = 1/16 for the benchmark's rows: factor ~1.2 with the fp16 shadow's
@@ -1257,7 +1245,7 @@ int stb_search_batch_dev(stb_ctx *ctx, const stb_corpus *corpus_c, const float *
   // one flag per query, written by the query shadow build: a query that cannot be normalised in fp32
   // has a zero (or NaN) shadow whose scores bound nothing, and both finish kernels report it unproven
   if ((rc = dev_reserve(&ctx->b_qbad, &ctx->b_qbad_cap, (size_t)q_pad)) != STB_OK) return rc;
-  if (!force_v1 && top_k <= 64 && v2_fits) {
+  if (top_k <= 64 && v2_fits) {
     constexpr uint32_t kSegCap = 64;                      // per (query, CTA): ~5 expected at 10M rows / 132 CTAs
     const uint32_t n_seg = stb_batch_emit_grid(ctx, n_tiles);
     const uint32_t stride = n_full / n_sample;
@@ -1432,7 +1420,7 @@ int stb_search_xchg(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint
   memcpy(ctx->q_pin, q, STB_D * sizeof(float));
   STB_CUDA(cudaMemcpyAsync(ctx->q_dev, ctx->q_pin, STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
   // the merge CTA stores the hits + status straight into pinned host memory
-  if ((rc = search_topk_xchg_impl(ctx, corpus, ctx->q_dev, top_k, x, ctx->hits_pin, ctx->status_pin, false)) != STB_OK) return rc;
+  if ((rc = stb_search_topk_xchg(ctx, corpus, ctx->q_dev, top_k, x, ctx->hits_pin, ctx->status_pin)) != STB_OK) return rc;
   STB_CUDA(cudaStreamSynchronize(ctx->stream));
   const uint32_t n = std::min<uint32_t>(ctx->status_pin[0], top_k);
   memcpy(out_hits, ctx->hits_pin, n * sizeof(stb_hit));
@@ -1495,7 +1483,7 @@ int stb_search_many(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint
   for (uint32_t i = 0; i < nq; ++i) {
     stb_hit *oh = ctx->hits_pin + (size_t)i * top_k;
     uint32_t *os = ctx->many_status_pin + 4 * (size_t)i;
-    if (x) rc = search_topk_xchg_impl(ctx, corpus, ctx->bq_dev + (size_t)i * STB_D, top_k, x, oh, os, nq > 1 && stb_env_overlap());
+    if (x) rc = stb_search_topk_xchg(ctx, corpus, ctx->bq_dev + (size_t)i * STB_D, top_k, x, oh, os);
     else rc = stb_launch_scan_topk(ctx, corpus, tier, ctx->bq_dev + (size_t)i * STB_D, top_k, nullptr, 0, corpus->n, oh, os, nullptr,
                                    nq > 1);
     if (rc != STB_OK) { cudaStreamSynchronize(ctx->stream); return rc; }

@@ -625,7 +625,7 @@ int stb_launch_batch_finish(stb_ctx *ctx, const uint64_t *cand, uint32_t n_slice
 }
 
 // =========================================================================================
-// Pipeline v2 (default since round 2; STB_BATCH_V1=1 selects the maxima/select/finish pipeline above):
+// Pipeline v2 (top_k <= 64 where it fits; the maxima/select/finish pipeline above serves the rest):
 //   sampling GEMM (maxima epilogue over ~4*SMs strided COMPLETE tiles) -> per-query threshold
 //   -> full GEMM whose epilogue emits the rows reaching the threshold -> exact finish.
 // Why the candidate set is sufficient, for ANY k (a = approximate score, c = exact cosine,

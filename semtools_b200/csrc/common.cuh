@@ -87,7 +87,7 @@ struct stb_ctx {
   unsigned long long *coscan_off;
   uint32_t coscan_tag[8];
   struct {
-    const void *corpus;                // null: no launch to follow
+    const void *rows;                  // the scanned corpus's f32 rows; null: no launch to follow
     int src;
     uint64_t n_virtual, tiles, t_bulk;
     unsigned long long t_base;
@@ -289,11 +289,11 @@ int stb_launch_corpus_gather(stb_ctx *ctx, const float *rows, const uint64_t *se
 // exact f64 re-rank + completeness check.  q_dev: 256 f32 on device.
 // n_ranges > 0: ranges_dev holds local [begin,end,vstart] triples.
 // tier: STB_TIER_* -- which copy of `c` the streaming pass reads (must exist and be current).
-// overlapped: the launch is one of a pipelined series (asynchronous entry points): the grid is sized
-// for ONE CTA per SM and releases its dependent at its START, so the next query's scan co-runs with
-// this one instead of waiting for it to drain (scan_topk.cu: "overlapped launches").  Without an
-// exchange and ranges the overlapped launch also co-scans: it starts its pass where its predecessor
-// on the same corpus is reading, so the two scans share each tile's read through L2.
+// overlapped: the launch is one of a pipelined single-GPU series (stb_search_topk_dev, stb_search_many
+// without an exchange) and takes no exchange or ranges: the grid is sized for ONE CTA per SM and
+// releases its dependent at its START, so the next query's scan co-runs with this one instead of
+// waiting for it to drain (scan_topk.cu: "overlapped launches").  It co-scans: it starts its pass where
+// its predecessor on the same corpus is reading, so the two scans share each tile's read through L2.
 int stb_launch_scan_topk(stb_ctx *ctx, const stb_corpus *c, int tier, const float *q_dev, uint32_t top_k,
                          const uint64_t *ranges_dev, uint32_t n_ranges,
                          uint64_t n_virtual, stb_hit *out_hits_dev,

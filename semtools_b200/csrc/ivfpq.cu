@@ -627,7 +627,7 @@ __global__ void ivf_pick_rows_kernel(const stb_hit *cand, uint32_t r, const uint
 //                            writes the top-k hits.
 // The funnel returns the `rerank` best ADC scores exactly when no warp and no CTA of the deal holds
 // more than 64 of them (every code is re-ranked when the probed lists hold <= 2048 codes).
-// Default since round 2 (validated on hardware); STB_IVFPQ_V1=1 selects the multi-launch search above.
+// stb_ivfpq_search runs it iff rerank <= ADC2_RERANK_CAP and top_k <= 1024, else the multi-launch search above.
 #define ADC2_THREADS 512
 #define ADC2_MAX_CTAS 32
 #define ADC2_KEEP 64        // per CTA; chunks are dealt round-robin over the 32 CTAs, so each sees a uniform sample: ~16 of the best 512 land in one CTA
@@ -1931,8 +1931,7 @@ int stb_ivfpq_search(stb_ivfpq *x, const float *q, uint32_t nprobe, uint32_t top
   cudaStream_t st = ctx->stream;
   memcpy(ctx->q_pin, q, STB_D * sizeof(float));
   STB_CUDA(cudaMemcpyAsync(ctx->q_dev, ctx->q_pin, STB_D * sizeof(float), cudaMemcpyHostToDevice, st));
-  const char *v1_env = getenv("STB_IVFPQ_V1");            // STB_IVFPQ_V1=1: the round-1 multi-launch search
-  if (!(v1_env && v1_env[0] == '1') && rerank <= ADC2_RERANK_CAP && top_k <= 1024) {
+  if (rerank <= ADC2_RERANK_CAP && top_k <= 1024) {
     // fused search: two launches, one synchronisation
     int frc = ivf_fused_launch(x, ctx->q_dev, nprobe, top_k, rerank, ctx->hits_dev, ctx->status_dev);
     if (frc != STB_OK) return frc;

@@ -1253,9 +1253,9 @@ static int stb_pick_e(uint32_t top_k) {
 #define STB_SHADOW_SCAN_U 4     // 4 rows x 4 LDG.128 per lane in flight = the f32 path's 2 x 8
 #define STB_Q8_SCAN_U 8         // 8 rows x 2 LDG.128
 
-// coscan: the corpus an overlapped launch may co-scan (null: never; stb_launch_scan_topk)
+// overlapped: a co-scan launch (no exchange, no ranges; stb_launch_scan_topk)
 template <int E, int RANGES, int SRC = 0, int EF = E>
-static int stb_launch_topk_t(stb_ctx *ctx, const TopkArgs &a_in, bool overlapped, const void *coscan) {
+static int stb_launch_topk_t(stb_ctx *ctx, const TopkArgs &a_in, bool overlapped) {
   constexpr int kU = SRC == 2 ? STB_Q4_SCAN_U : (SRC == 1 ? STB_SHADOW_SCAN_U : STB_SCAN_U);
   auto kern = stb_scan_topk_kernel<E, kU, RANGES, SRC, EF>;
   // resident CTAs per SM the grid is sized for: what the occupancy calculator allows (2 with the
@@ -1294,23 +1294,23 @@ static int stb_launch_topk_t(stb_ctx *ctx, const TopkArgs &a_in, bool overlapped
   // co-scan: follow the last launch if it was one too, on the same corpus copy and rows (hence the
   // same tiles); any other launch in between -- synchronous, sharded, ranged -- ends the series
   const uint32_t tag = (uint32_t)ctx->topk_launches;   // the launch count, 0 only after a wrap: no co-scan then
-  const bool co = overlapped && coscan && RANGES == 0 && ctx->ticket_ring && tag != 0;
+  const bool co = overlapped && tag != 0;
   if (ctx->ticket_ring) ctx->coscan_tag[slot] = co ? tag : 0u;
   if (co) {
     auto &p = ctx->coscan_prev;
     a.co.word = ctx->coscan_off + slot;
     a.co.tag = tag;
-    if (p.corpus == coscan && p.src == SRC && p.n_virtual == a.scan.n_virtual && p.tiles == tiles) {
+    if (p.rows == a.scan.rows && p.src == SRC && p.n_virtual == a.scan.n_virtual && p.tiles == tiles) {
       a.co.pred_tag = p.tag;
       a.co.pred_word = ctx->coscan_off + p.slot;
       a.co.pred_tickets = ctx->tickets + p.slot;
       a.co.pred_t_base = p.t_base;
       a.co.pred_t_bulk = p.t_bulk;
     }
-    p.corpus = coscan; p.src = SRC; p.n_virtual = a.scan.n_virtual; p.tiles = tiles;
+    p.rows = a.scan.rows; p.src = SRC; p.n_virtual = a.scan.n_virtual; p.tiles = tiles;
     p.slot = slot; p.t_base = a.scan.t_base; p.t_bulk = a.scan.t_bulk; p.tag = tag;
   }
-  if (!a.co.word) ctx->coscan_prev.corpus = nullptr;
+  if (!a.co.word) ctx->coscan_prev.rows = nullptr;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3((unsigned)grid);
@@ -1329,21 +1329,21 @@ static int stb_launch_topk_t(stb_ctx *ctx, const TopkArgs &a_in, bool overlapped
 }
 
 template <int RANGES>
-static int stb_launch_topk_r(stb_ctx *ctx, const TopkArgs &a, int tier, uint32_t top_k, bool ov, const void *co) {
+static int stb_launch_topk_r(stb_ctx *ctx, const TopkArgs &a, int tier, uint32_t top_k, bool ov) {
   const int e = stb_pick_e(top_k);
   // q8: 32-key lists below the root, 128 candidates re-ranked at the root (see stb_scan_q8)
-  if (tier == STB_TIER_Q8) return stb_launch_topk_t<1, RANGES, 2, 4>(ctx, a, ov, co);
+  if (tier == STB_TIER_Q8) return stb_launch_topk_t<1, RANGES, 2, 4>(ctx, a, ov);
   if (tier == STB_TIER_H16) {
     switch (e) {
-      case 1: return stb_launch_topk_t<1, RANGES, 1>(ctx, a, ov, co);
-      case 2: return stb_launch_topk_t<2, RANGES, 1>(ctx, a, ov, co);
-      default: return stb_launch_topk_t<4, RANGES, 1>(ctx, a, ov, co);
+      case 1: return stb_launch_topk_t<1, RANGES, 1>(ctx, a, ov);
+      case 2: return stb_launch_topk_t<2, RANGES, 1>(ctx, a, ov);
+      default: return stb_launch_topk_t<4, RANGES, 1>(ctx, a, ov);
     }
   }
   switch (e) {
-    case 1: return stb_launch_topk_t<1, RANGES, 0>(ctx, a, ov, co);
-    case 2: return stb_launch_topk_t<2, RANGES, 0>(ctx, a, ov, co);
-    default: return stb_launch_topk_t<4, RANGES, 0>(ctx, a, ov, co);
+    case 1: return stb_launch_topk_t<1, RANGES, 0>(ctx, a, ov);
+    case 2: return stb_launch_topk_t<2, RANGES, 0>(ctx, a, ov);
+    default: return stb_launch_topk_t<4, RANGES, 0>(ctx, a, ov);
   }
 }
 
@@ -1351,6 +1351,7 @@ int stb_launch_scan_topk(stb_ctx *ctx, const stb_corpus *c, int tier, const floa
                          const uint64_t *ranges_dev, uint32_t n_ranges,
                          uint64_t n_virtual, stb_hit *out_hits_dev,
                          uint32_t *out_status_dev, const StbXchgArgs *xchg, bool overlapped) {
+  if (overlapped && (xchg || n_ranges)) { stb_set_error("scan_topk: an overlapped launch takes no exchange or ranges"); return STB_ERR_ARG; }
   TopkArgs a;
   a.scan.rows = reinterpret_cast<const float4 *>(c->rows);
   a.scan.n_virtual = n_virtual;
@@ -1387,9 +1388,7 @@ int stb_launch_scan_topk(stb_ctx *ctx, const stb_corpus *c, int tier, const floa
     a.q4.refined = ctx->q4_refined;
   }
   if (tier == STB_TIER_H16 && !c->shadow) { stb_set_error("scan_topk: h16 tier unavailable"); return STB_ERR_STATE; }
-  // the co-scan is the single-GPU form of the overlapped mode: a sharded launch keeps the plain tile order
-  const void *co = xchg ? nullptr : static_cast<const void *>(c);
-  return n_ranges > 0 ? stb_launch_topk_r<1>(ctx, a, tier, top_k, overlapped, co) : stb_launch_topk_r<0>(ctx, a, tier, top_k, overlapped, co);
+  return n_ranges > 0 ? stb_launch_topk_r<1>(ctx, a, tier, top_k, overlapped) : stb_launch_topk_r<0>(ctx, a, tier, top_k, overlapped);
 }
 
 // ------------------------------------------------------------------ collect path ---

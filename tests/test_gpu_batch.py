@@ -12,26 +12,12 @@ from semtools_b200 import capi
 
 pytestmark = pytest.mark.gpu
 
-# ------------------------------------------------------------------------------------------
-# Pipeline v2 (sampled threshold -> emitting epilogue -> exact finish) is the default since
-# round 2; STB_BATCH_V1=1 forces the round-1 maxima/select/finish pipeline.  Both run here.
-import os
 
-
-@pytest.fixture(params=["v2", "v1"])
-def batch_pipeline(request, monkeypatch):
-    if request.param == "v1":
-        monkeypatch.setenv("STB_BATCH_V1", "1")
-    else:
-        monkeypatch.delenv("STB_BATCH_V1", raising=False)
-    return request.param
-
-
-@pytest.fixture
-def batch_v2(monkeypatch):
-    monkeypatch.delenv("STB_BATCH_V1", raising=False)
-
-
+def expected_route(n, k):
+    """Pipeline v2 (sampled threshold -> emitting epilogue -> exact finish) for k <= 64 on a corpus of at
+    least k complete tiles; v1 (maxima/select/finish) otherwise.  These shapes stay far below the shard size
+    at which v2's sample overflows (test_gpu_batch_contract.route_rule)."""
+    return 2 if k <= 64 and n // 256 >= k else 1
 
 
 def bf16_round(x):
@@ -76,8 +62,10 @@ def check_batch(res, rows, queries, k):
         assert np.array_equal(res[i]["distance"], d), i
 
 
-@pytest.mark.parametrize("nq,n,k", [(1, 40, 3), (5, 1000, 10), (130, 70_000, 10), (300, 20_000, 1), (64, 50_000, 40)])
-def test_search_batch_matches_oracle(ctx, batch_pipeline, nq, n, k):
+@pytest.mark.parametrize("nq,n,k", [(1, 40, 3), (5, 1000, 10), (130, 70_000, 10), (300, 20_000, 1), (64, 50_000, 40),
+                                    (130, 70_000, 80), (64, 50_000, 96), (20, 20_000, 200), (300, 2_000, 16),
+                                    (40, 9_000, 64)])
+def test_search_batch_matches_oracle(ctx, nq, n, k):
     rng = np.random.default_rng(nq + n + k)
     rows = unit_rows(rng, n)
     queries = unit_rows(rng, nq)
@@ -85,6 +73,7 @@ def test_search_batch_matches_oracle(ctx, batch_pipeline, nq, n, k):
     c.append(rows)
     before = ctx.counters()["fallback_searches"]
     res = c.search_batch(queries, top_k=k)
+    assert ctx.batch_last()["route"] == expected_route(n, k)
     check_batch(res, rows, queries, k)
     if n >= 20_000 and k <= 16:
         # 32 sub-tiles are re-scored per query, enough to PROVE top-k for k <= ~16 for nearly every
@@ -94,7 +83,9 @@ def test_search_batch_matches_oracle(ctx, batch_pipeline, nq, n, k):
         assert ctx.counters()["fallback_searches"] - before <= max(2, nq // 8)
 
 
-def test_search_batch_ties_zero_rows_and_unprovable_queries(ctx, batch_pipeline):
+@pytest.mark.parametrize("route", ["v2", "v1"])
+def test_search_batch_ties_zero_rows_and_unprovable_queries(ctx, route):
+    k = 10 if route == "v2" else 80                            # v1: k > 64
     rng = np.random.default_rng(42)
     rows = unit_rows(rng, 30_000)
     rows[rng.integers(0, 30_000, 20)] = rows[rng.integers(0, 30_000, 20)]      # duplicates
@@ -107,8 +98,9 @@ def test_search_batch_ties_zero_rows_and_unprovable_queries(ctx, batch_pipeline)
     c = capi.Corpus(ctx, 30_000)
     c.append(rows)
     before = ctx.counters()["fallback_searches"]
-    res = c.search_batch(queries, top_k=10)
-    check_batch(res, rows, queries, 10)
+    res = c.search_batch(queries, top_k=k)
+    assert ctx.batch_last()["route"] == expected_route(30_000, k)
+    check_batch(res, rows, queries, k)
     assert ctx.counters()["fallback_searches"] >= before + 2     # queries 1 and 2 cannot be proven
 
 
@@ -144,17 +136,19 @@ def test_search_batch_sharded_row_base_and_rebuild_after_append(ctx):
         assert np.array_equal(res[i]["distance"], d)
 
 
-def test_sharded_batch_search_merges_to_the_unsharded_answer(ctx, batch_pipeline):
+@pytest.mark.parametrize("route", ["v2", "v1"])
+def test_sharded_batch_search_merges_to_the_unsharded_answer(ctx, route):
     """Sharded K2: per-shard stb_search_batch_dev + stb_hits_merge_batch_dev (what ranks do
     after all-gathering their nq x k hits) == oracle over the whole corpus."""
     torch = pytest.importorskip("torch")
     rng = np.random.default_rng(77)
-    n, nq, k = 60_000, 70, 10
+    n = 60_000 if route == "v2" else 6_000                     # v1: shards of fewer than k complete tiles
+    nq, k = 70, 10
     rows = unit_rows(rng, n)
-    rows[59_999] = rows[5]                      # cross-shard exact tie
+    rows[n - 1] = rows[5]                       # cross-shard exact tie
     queries = unit_rows(rng, nq)
     queries[0] = rows[5]
-    bounds = [0, 20_000, 45_000, n]
+    bounds = [0, n // 3, n * 3 // 4, n]
     dev = torch.device("cuda:0")
     q_dev = torch.from_numpy(queries).to(dev)
     world = len(bounds) - 1
@@ -168,6 +162,7 @@ def test_sharded_batch_search_merges_to_the_unsharded_answer(ctx, batch_pipeline
         c.append(rows[bounds[r]:bounds[r + 1]])
         shards.append(c)
         c.search_batch_dev(q_dev.data_ptr(), nq, k, lists[r].data_ptr(), status[r].data_ptr())
+        assert ctx.batch_last()["route"] == expected_route(bounds[r + 1] - bounds[r], k)
     ctx.hits_merge_batch_dev(lists.data_ptr(), world, nq, k, k, out.data_ptr())
     ctx.sync()
     proven = (status[:, :, 1] == 1).all(dim=0).cpu().numpy()      # per query: every shard proved its part
@@ -180,12 +175,12 @@ def test_sharded_batch_search_merges_to_the_unsharded_answer(ctx, batch_pipeline
         assert got[i]["row"].tolist() == [int(x) for x in r], i
         assert np.array_equal(got[i]["distance"], d), i
     if proven[0]:
-        assert got[0]["row"][:2].tolist() == [5, 59_999]
+        assert got[0]["row"][:2].tolist() == [5, n - 1]
 
 
 @pytest.mark.parametrize("nq,n,k", [(1, 40, 3), (5, 1000, 10), (130, 70_000, 10), (300, 20_001, 1), (64, 50_000, 40),
                                     (3, 255, 5), (9, 256, 64), (20, 200_000, 10)])
-def test_v2_search_batch_matches_oracle_without_fallback(ctx, batch_v2, nq, n, k):
+def test_v2_search_batch_matches_oracle_without_fallback(ctx, nq, n, k):
     rng = np.random.default_rng(nq + n + k)
     rows = unit_rows(rng, n)
     queries = unit_rows(rng, nq)
@@ -197,10 +192,10 @@ def test_v2_search_batch_matches_oracle_without_fallback(ctx, batch_v2, nq, n, k
     assert ctx.counters()["fallback_searches"] == before        # v2 proves every k <= 64 unless a capacity overflows
     # v2 samples complete tiles: a corpus of fewer than k of them, (1,40,3), (5,1000,10), (3,255,5) and
     # (9,256,64), is answered by v1, which proves these small shapes too
-    assert ctx.batch_last()["route"] == (2 if n // 256 >= k else 1)
+    assert ctx.batch_last()["route"] == expected_route(n, k)
 
 
-def test_v2_ties_zero_rows_dense_neighbourhoods(ctx, batch_v2):
+def test_v2_ties_zero_rows_dense_neighbourhoods(ctx):
     rng = np.random.default_rng(42)
     rows = unit_rows(rng, 30_000)
     rows[rng.integers(0, 30_000, 20)] = rows[rng.integers(0, 30_000, 20)]

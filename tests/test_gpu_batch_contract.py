@@ -60,20 +60,7 @@ def sm_count():
     return torch.cuda.get_device_properties(0).multi_processor_count
 
 
-@pytest.fixture
-def route_env(monkeypatch):
-    """set_v1(True) forces pipeline v1 (STB_BATCH_V1=1, read per call); the default is unset."""
-    monkeypatch.delenv("STB_BATCH_V1", raising=False)
-
-    def set_v1(on):
-        if on:
-            monkeypatch.setenv("STB_BATCH_V1", "1")
-        else:
-            monkeypatch.delenv("STB_BATCH_V1", raising=False)
-    return set_v1
-
-
-def route_rule(n, k, sm, force_v1=False):
+def route_rule(n, k, sm):
     """api.cu stb_search_batch_dev: which pipeline runs, and v2's sampling and emission grid."""
     f16, _ = capi.batch_params()
     n_full = n // TILE
@@ -85,7 +72,7 @@ def route_rule(n, k, sm, force_v1=False):
     if expected_emitted(n_sample) > 2048:
         n_sample = min(min(n_full, 8192), (n_full // 64 + sm - 1) // sm * sm)
     v2_fits = n_sample >= k and expected_emitted(n_sample) <= 2048
-    if not force_v1 and k <= MAX_K and v2_fits:
+    if k <= MAX_K and v2_fits:
         n_tiles = -(-n // TILE)
         return {"route": 2, "n_sample": n_sample, "stride": n_full // n_sample, "n_seg": min(n_tiles, sm),
                 "seg_cap": SEG_CAP}
@@ -222,7 +209,7 @@ def corpus_of(kind, rng, n):
 @pytest.mark.parametrize("kind,n,nq,k", [("random", 70_000, 130, 10), ("duplicated", 120_000, 64, 5),
                                          ("clustered", 280_000, 40, 16), ("random", 140_001, 257, 1),
                                          ("clustered", 51_200, 20, 64)])
-def test_v2_stage_contracts(ctx, route_env, sm_count, kind, n, nq, k):
+def test_v2_stage_contracts(ctx, sm_count, kind, n, nq, k):
     rng = np.random.default_rng(n + nq + k)
     rows = corpus_of(kind, rng, n)
     queries = unit_rows(rng, nq)
@@ -284,7 +271,7 @@ def anchored_corpus(rng, q, n_tiles, n_seg, special_tiles):
 
 
 @pytest.mark.parametrize("n_keys", [64, 65])
-def test_segment_capacity(ctx, route_env, sm_count, n_keys):
+def test_segment_capacity(ctx, sm_count, n_keys):
     rng = np.random.default_rng(640 + n_keys)
     q = unit_rows(rng, 1)[0]
     n_tiles = 2 * sm_count + 10
@@ -299,7 +286,7 @@ def test_segment_capacity(ctx, route_env, sm_count, n_keys):
 
 
 @pytest.mark.parametrize("first,second", [(40, 24), (40, 40)])
-def test_segment_cursor_across_tiles_of_one_cta(ctx, route_env, sm_count, first, second):
+def test_segment_cursor_across_tiles_of_one_cta(ctx, sm_count, first, second):
     rng = np.random.default_rng(first * 100 + second)
     q = unit_rows(rng, 1)[0]
     n_tiles = 2 * sm_count + 10
@@ -316,7 +303,7 @@ def test_segment_cursor_across_tiles_of_one_cta(ctx, route_env, sm_count, first,
 
 
 @pytest.mark.parametrize("total", [4096, 4097])
-def test_total_key_capacity(ctx, route_env, sm_count, total):
+def test_total_key_capacity(ctx, sm_count, total):
     """k = 1: one row at cos 0.9 in sampled tile 0 sets the threshold, an exact copy of q in an unsampled tile
     is the answer (the only narrowed key), and total - 2 rows at cos 0.8995 fill the segments <= 40 each."""
     rng = np.random.default_rng(total)
@@ -347,7 +334,7 @@ def test_total_key_capacity(ctx, route_env, sm_count, total):
 
 
 @pytest.mark.parametrize("narrowed", [1024, 1025])
-def test_rescore_capacity(ctx, route_env, sm_count, narrowed):
+def test_rescore_capacity(ctx, sm_count, narrowed):
     """k = 1: an exact copy of q and narrowed - 1 copies of a row at cos 0.9995, all within 2 EPS of the top."""
     rng = np.random.default_rng(narrowed)
     q = unit_rows(rng, 1)[0]
@@ -361,7 +348,7 @@ def test_rescore_capacity(ctx, route_env, sm_count, narrowed):
     assert proven == (narrowed <= F2_RESCORE)
 
 
-def test_narrowing_band_uses_two_eps(ctx, route_env, sm_count):
+def test_narrowing_band_uses_two_eps(ctx, sm_count):
     """About 1100 rows whose scores sit between A_k - 2 EPS and A_k - EPS: the 2 EPS cut narrows them all
     (over the re-score cap: unproven); a 1 EPS cut would keep none and prove the query."""
     _, eps = capi.batch_params()
@@ -382,13 +369,12 @@ def test_narrowing_band_uses_two_eps(ctx, route_env, sm_count):
 # ------------------------------------------------------------------ c. routes x shapes ---
 V2_SHAPES = [(1, 70_000, 10), (127, 20_001, 1), (128, 64 * TILE, 64), (129, 2 * TILE + 255, 2),
              (257, 140 * TILE + 1, 63), (2049, 40 * TILE + 255, 2), (5, 3 * TILE, 3), (129, 300 * TILE + 128, 64)]
-V1_SHAPES = [(9, 63 * TILE + 200, 64, False), (128, 30_000, 65, False), (257, 20_000, 97, False),
-             (3, 5000, 1024, False), (2049, 20 * TILE + 1, 65, False), (1, 255, 1, False), (5, 1000, 10, False),
-             (129, 50_000, 10, True), (1, 64 * TILE + 255, 64, True), (130, 140 * TILE + 255, 1, True)]
+V1_SHAPES = [(9, 63 * TILE + 200, 64), (128, 30_000, 65), (257, 20_000, 97), (3, 5000, 1024), (2049, 20 * TILE + 1, 65),
+             (1, 255, 1), (5, 1000, 10), (129, 50_000, 80), (1, 16 * TILE + 255, 17), (130, 140 * TILE + 255, 96)]
 
 
 @pytest.mark.parametrize("nq,n,k", V2_SHAPES)
-def test_v2_route_and_shapes(ctx, route_env, sm_count, nq, n, k):
+def test_v2_route_and_shapes(ctx, sm_count, nq, n, k):
     rng = np.random.default_rng(nq * 3 + n + k)
     rows = unit_rows(rng, n)
     queries = unit_rows(rng, nq)
@@ -400,16 +386,15 @@ def test_v2_route_and_shapes(ctx, route_env, sm_count, nq, n, k):
     check_v2_call(ctx, rows, queries, k, got, st, info, rng=rng, require_all_proven=True)
 
 
-@pytest.mark.parametrize("nq,n,k,force", V1_SHAPES)
-def test_v1_route_and_shapes(ctx, route_env, sm_count, nq, n, k, force):
-    route_env(force)
+@pytest.mark.parametrize("nq,n,k", V1_SHAPES)
+def test_v1_route_and_shapes(ctx, sm_count, nq, n, k):
     rng = np.random.default_rng(nq * 5 + n + k)
     rows = unit_rows(rng, n)
     queries = unit_rows(rng, nq)
     queries[0] = rows[n - 1]
     c = new_corpus(ctx, rows)
     got, st, info = run_dev(ctx, c, queries, k)
-    assert route_rule(n, k, sm_count, force_v1=force)["route"] == 1
+    assert route_rule(n, k, sm_count)["route"] == 1
     assert info["route"] == 1 and info["nq"] == nq, info
     assert np.all(st[:, 0] <= min(k, n))
     for i in sample_ids(nq, rng):
@@ -424,7 +409,7 @@ def test_v1_route_and_shapes(ctx, route_env, sm_count, nq, n, k, force):
         assert host[j]["row"].tolist() == [int(x) for x in r] and np.array_equal(host[j]["distance"], d), i
 
 
-def test_route_boundary_n_full_equals_k(ctx, route_env, sm_count):
+def test_route_boundary_n_full_equals_k(ctx, sm_count):
     """n_full == k samples every tile (v2); n_full == k - 1 falls to v1."""
     rng = np.random.default_rng(7)
     for k, n_full, route in [(16, 16, 2), (17, 16, 1), (64, 64, 2), (65, 64, 1), (64, 63, 1)]:
@@ -482,11 +467,12 @@ def with_bad_queries(rng, rows, n_good):
     return np.ascontiguousarray(np.stack(queries), dtype=np.float32), kinds
 
 
-@pytest.mark.parametrize("route,k", [("v2", 10), ("v1", 10), ("v1", 97)])
-def test_bad_queries_are_never_proven_wrong(ctx, route_env, sm_count, route, k):
-    route_env(route == "v1")
-    rng = np.random.default_rng(k + len(route))
-    n = 70_000
+@pytest.mark.parametrize("n,k", [(70_000, 10), (2_000, 10), (70_000, 97)])
+def test_bad_queries_are_never_proven_wrong(ctx, sm_count, n, k):
+    """Pipeline v2, then v1 twice: on a corpus of fewer than k complete tiles, and for k > 64."""
+    route = "v2" if route_rule(n, k, sm_count)["route"] == 2 else "v1"
+    assert route == ("v1" if n // TILE < k or k > MAX_K else "v2")
+    rng = np.random.default_rng(n + k)
     rows = unit_rows(rng, n)
     queries, kinds = with_bad_queries(rng, rows, 40)
     bad = unnormalisable(queries)
@@ -513,7 +499,7 @@ def test_bad_queries_are_never_proven_wrong(ctx, route_env, sm_count, route, k):
         assert np.array_equal(host[i]["distance"], d), (kinds[i], i)
 
 
-def test_bad_queries_in_the_sharded_exchange(route_env):
+def test_bad_queries_in_the_sharded_exchange():
     torch = pytest.importorskip("torch")
     from semtools_b200.sharded import shard_bounds
     world, k = 2, 10
@@ -588,9 +574,10 @@ def test_bad_queries_through_k1_topk_dev(ctx):
 
 
 # ------------------------------------------------------------------ e. data edges ---
-@pytest.mark.parametrize("route", ["v2", "v1"])
-def test_data_edges(ctx, route_env, sm_count, route):
-    route_env(route == "v1")
+@pytest.mark.parametrize("k", [8, 72])
+def test_data_edges(ctx, sm_count, k):
+    """k = 8 runs pipeline v2, k = 72 (> 64) pipeline v1."""
+    route = "v2" if k <= MAX_K else "v1"
     rng = np.random.default_rng(55)
     n_tiles = sm_count + 20
     n = n_tiles * TILE - 37                                   # ragged last tile
@@ -608,24 +595,24 @@ def test_data_edges(ctx, route_env, sm_count, route):
     queries[7] = rows[n - 2] * np.float32(3.0)
     row_base = 5_000_000_000
     c = new_corpus(ctx, rows, row_base=row_base)
-    got, st, info = run_dev(ctx, c, queries, 8)
-    assert info["route"] == (2 if route == "v2" else 1)
+    got, st, info = run_dev(ctx, c, queries, k)
+    assert info["route"] == route_rule(n, k, sm_count)["route"] == (2 if route == "v2" else 1)
     if route == "v2":
-        check_v2_call(ctx, rows, queries, 8, got, st, info, row_base=row_base, require_all_proven=False)
+        check_v2_call(ctx, rows, queries, k, got, st, info, row_base=row_base, require_all_proven=False)
     for i in range(len(queries)):
         if st[i, 1]:
-            check_query(got[i], st[i], rows, queries[i], 8, row_base=row_base, where=f"query {i}")
+            check_query(got[i], st[i], rows, queries[i], k, row_base=row_base, where=f"query {i}")
     if st[0, 1]:
         assert got[0]["row"][:2].tolist() == [row_base + 255, row_base + 256]
     if st[5, 1]:
         assert got[5]["row"][:4].tolist() == [row_base + r for r in (10, 2000, 9000, n - 2)]
-    host = c.search_batch(queries, top_k=8)
+    host = c.search_batch(queries, top_k=k)
     for i in range(len(queries)):
-        r, d = oracle.search_rows(rows, queries[i], top_k=8)
+        r, d = oracle.search_rows(rows, queries[i], top_k=k)
         assert host[i]["row"].tolist() == [int(x) + row_base for x in r] and np.array_equal(host[i]["distance"], d), i
 
 
-def test_append_extends_a_ragged_shadow(ctx, route_env, sm_count):
+def test_append_extends_a_ragged_shadow(ctx, sm_count):
     rng = np.random.default_rng(66)
     rows = unit_rows(rng, 60 * TILE + 300)
     queries = unit_rows(rng, 20)
@@ -676,18 +663,12 @@ def test_gemm_error_bound_on_adversarial_rows(ctx):
     assert worst <= eps, f"worst |a - c| = {worst:.6f}, margin {eps - worst:.6f} of EPS {eps}"
 
 
-# ------------------------------------------------------------------ g. the big-sample threshold kernel ---
-def test_big_sample_threshold_kernel(ctx, route_env, sm_count):
-    """n_sample > 608 takes stb_batch_thresh_big_kernel: about 8.7M rows on 132 SMs, k = 16."""
+# ------------------------------------------------------------------ g. shards of millions of rows ---
+def random_device_corpus(ctx, n, seed):
+    """n random unit rows generated on the device (too many to scan on the host): (rows, corpus)."""
     torch = pytest.importorskip("torch")
-    k = 16
-    n_full = next(f for f in range(33_000, 200_000) if route_rule(f * TILE, k, sm_count)["route"] == 2
-                  and route_rule(f * TILE, k, sm_count)["n_sample"] > MAX_SAMPLE)
-    n = n_full * TILE + 100
-    exp = route_rule(n, k, sm_count)
-    assert exp["n_sample"] > MAX_SAMPLE
     dev = torch.device("cuda:0")
-    g = torch.Generator(device=dev).manual_seed(8)
+    g = torch.Generator(device=dev).manual_seed(seed)
     R = torch.empty((n, 256), dtype=torch.float32, device=dev)
     for lo in range(0, n, 1 << 20):
         hi = min(n, lo + (1 << 20))
@@ -696,6 +677,31 @@ def test_big_sample_threshold_kernel(ctx, route_env, sm_count):
     c = capi.Corpus(ctx, n)
     torch.cuda.synchronize()
     c.append_dev(R.data_ptr(), n)
+    return R, c
+
+
+def exact_topk(R, q, k):
+    """oracle.search_rows over device rows R: an f32 shortlist (error ~1e-6 on unit rows), ranked by
+    oracle.distances -> (rows, distances)."""
+    torch = pytest.importorskip("torch")
+    cos = R @ torch.from_numpy(q).to(R.device)
+    kth = torch.topk(cos, k).values[-1]
+    short = torch.nonzero(cos >= kth - 1e-4).flatten().cpu().numpy()
+    d = oracle.distances(R[torch.from_numpy(short).to(R.device)].cpu().numpy(), q)
+    order = np.lexsort((short, d))[:k]
+    return short[order], d[order]
+
+
+def test_big_sample_threshold_kernel(ctx, sm_count):
+    """n_sample > 608 takes stb_batch_thresh_big_kernel: about 8.7M rows on 132 SMs, k = 16."""
+    torch = pytest.importorskip("torch")
+    k = 16
+    n_full = next(f for f in range(33_000, 200_000) if route_rule(f * TILE, k, sm_count)["route"] == 2
+                  and route_rule(f * TILE, k, sm_count)["n_sample"] > MAX_SAMPLE)
+    n = n_full * TILE + 100
+    exp = route_rule(n, k, sm_count)
+    assert exp["n_sample"] > MAX_SAMPLE
+    R, c = random_device_corpus(ctx, n, 8)
     rng = np.random.default_rng(8)
     queries = unit_rows(rng, 8)
     queries[0] = c.read(n - 5, 1)[0]
@@ -710,23 +716,45 @@ def test_big_sample_threshold_kernel(ctx, route_env, sm_count):
     thr = (s_k.astype(np.float32) - np.float32(2.0) * np.float32(eps)).astype(np.float32)
     assert np.array_equal(info["thr"].view(np.uint32), thr.view(np.uint32))
     assert st[:, 1].all()
-    qt = torch.from_numpy(queries).to(dev)
-    cos = (R @ qt.T).T                                        # f32: error ~1e-6 on unit rows
     for i in range(len(queries)):
-        kth = torch.topk(cos[i], k).values[-1]
-        short = torch.nonzero(cos[i] >= kth - 1e-4).flatten().cpu().numpy()
-        rows_s = R[torch.from_numpy(short).to(dev)].cpu().numpy()
-        d = oracle.distances(rows_s, queries[i])
-        order = np.lexsort((short, d))[:k]
-        assert got[i]["row"].tolist() == short[order].tolist(), i
-        assert np.array_equal(got[i]["distance"], d[order]), i
+        r, d = exact_topk(R, queries[i], k)
+        assert got[i]["row"].tolist() == r.tolist(), i
+        assert np.array_equal(got[i]["distance"], d), i
     c.close()
-    del R, cos
+    del R
+    torch.cuda.empty_cache()
+
+
+def test_v1_route_when_the_second_sample_overflows(ctx, sm_count):
+    """17 <= k <= 64 on a shard so large that even the 1/64 sample expects more than 2048 keys per query
+    runs v1: k = 64 from about 2.2M rows on 132 SMs."""
+    torch = pytest.importorskip("torch")
+    k = 64
+    n_full = next(f for f in range(k, 200_000) if route_rule(f * TILE, k, sm_count)["route"] == 1)
+    n = n_full * TILE + 100
+    assert route_rule(n, k, sm_count)["route"] == 1
+    R, c = random_device_corpus(ctx, n, 9)
+    rng = np.random.default_rng(9)
+    queries = unit_rows(rng, 6)
+    queries[0] = c.read(n - 5, 1)[0]
+    got, st, info = run_dev(ctx, c, queries, k)
+    assert info["route"] == 1 and info["nq"] == len(queries), info
+    assert np.all(st[:, 0] <= k)
+    exact = [exact_topk(R, q, k) for q in queries]
+    for i, (r, d) in enumerate(exact):
+        if st[i, 1]:
+            assert got[i]["row"].tolist() == r.tolist() and np.array_equal(got[i]["distance"], d), i
+    host = c.search_batch(queries, top_k=k)
+    assert ctx.batch_last()["route"] == 1
+    for i, (r, d) in enumerate(exact):
+        assert host[i]["row"].tolist() == r.tolist() and np.array_equal(host[i]["distance"], d), i
+    c.close()
+    del R
     torch.cuda.empty_cache()
 
 
 # ------------------------------------------------------------------ h. scratch reuse ---
-def test_scratch_reuse_across_shapes(ctx, route_env, sm_count):
+def test_scratch_reuse_across_shapes(ctx, sm_count):
     """Alternate corpora of different tile counts and (nq, k) pairs on one context: stale counts, keys or
     thresholds from the previous call would show."""
     rng = np.random.default_rng(1234)

@@ -51,13 +51,9 @@ def test_ivfpq_recall_and_exact_distances(ctx):
     idx.close()
 
 
-# ------------------------------------------------------------------------------------------
-# Fused search (v2: two launches, one sync) is the default since round 2; STB_IVFPQ_V1=1 selects
-# the round-1 multi-launch search, which this test uses as the comparator.
-import os
-
-
 def test_v2_fused_search_matches_v1_candidates_and_exact_distances(ctx):
+    """The fused search (rerank <= 1024) against the batched search, which has the same coarse scores,
+    probe lists and LUT and selects its candidates exactly (stb_ivfpq_search_batch)."""
     rng = np.random.default_rng(6)
     n = 200_000
     centers = make_centers(rng)
@@ -66,22 +62,20 @@ def test_v2_fused_search_matches_v1_candidates_and_exact_distances(ctx):
     c.append(rows)
     idx = capi.IvfPq(c, nlist=256, train_rows=65536, iters=6)
     queries = clustered(rng, centers, 30)
-    os.environ["STB_IVFPQ_V1"] = "1"
-    v1 = [idx.search(q, nprobe=32, top_k=10, rerank=512) for q in queries]
-    os.environ.pop("STB_IVFPQ_V1", None)
+    batch, batch_n, batch_scanned = idx.search_batch(queries, nprobe=32, top_k=10, rerank=512)
     try:
         recalls = []
         for i, q in enumerate(queries):
             got, n_scan = idx.search(q, nprobe=32, top_k=10, rerank=512)
-            assert n_scan == v1[i][1]                              # same probe lists
+            assert n_scan == batch_scanned[i]                      # same probe lists
             assert len(got) == 10 and np.all(np.diff(got["distance"]) >= 0)
             for h in got[:3]:
                 assert h["distance"] == oracle.cosine(q, rows[int(h["row"]) - 7_000_000])
             exact = c.search(q, top_k=10)
             recalls.append(len(set(got["row"].tolist()) & set(exact["row"].tolist())) / 10.0)
             # the per-warp top-64 / per-CTA top-64 reductions are lossless for the best 512 here,
-            # so both versions re-rank the same candidates -> identical hits
-            assert got["row"].tolist() == v1[i][0]["row"].tolist()
+            # so both searches re-rank the same candidates -> identical hits
+            assert np.array_equal(got, batch[i][: batch_n[i]]), i
         assert np.mean(recalls) >= 0.9
         # probing every list: exact answer (rerank capped at 1024 in v2)
         got, n_scan = idx.search(queries[0], nprobe=256, top_k=10, rerank=1024)
@@ -93,7 +87,6 @@ def test_v2_fused_search_matches_v1_candidates_and_exact_distances(ctx):
         got, _ = idx.search(np.zeros(256, np.float32), nprobe=4, top_k=5, rerank=64)
         assert len(got) == 5 and np.all(got["distance"] == 1.0)
     finally:
-        os.environ.pop("STB_IVFPQ_V1", None)
         idx.close()
 
 

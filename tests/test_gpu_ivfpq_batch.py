@@ -36,6 +36,7 @@ SCAN_WARPS_PER_CTA = _define("IVFB_SCAN_THREADS") // 32
 WARP_KEEP = _define("IVFB_WARP_KEEP")
 MAX_NQ = _define("IVFB_MAX_NQ")
 RERANK_CAP = _define("IVFB_RERANK_CAP")
+FUSED_CAP = _define("ADC2_RERANK_CAP")      # stb_ivfpq_search: the fused search up to this rerank and top_k
 INVALID = np.uint64(0xFFFFFFFFFFFFFFFF)
 U64MAX = np.iinfo(np.uint64).max
 
@@ -98,6 +99,20 @@ def bad_queries(rng):
     ninf = q.copy(); ninf[200] = -np.inf
     return [np.zeros(256, np.float32), nan, pinf, ninf, (q * np.float32(1e-20)).astype(np.float32),
             (q * np.float32(1e20)).astype(np.float32)]
+
+
+def search_on_route(ctx, idx, q, nprobe, top_k, rerank):
+    """idx.search, checking from the context's launch count the route that rerank (in [top_k, 4096]) and top_k
+    select: the fused search (2 launches) when both are <= FUSED_CAP, else the multi-launch search (more, as
+    soon as a probed list holds a code)."""
+    before = ctx.counters()["kernel_launches"]
+    got, n_scan = idx.search(q, nprobe=nprobe, top_k=top_k, rerank=rerank)
+    launches = ctx.counters()["kernel_launches"] - before
+    if rerank <= FUSED_CAP and top_k <= FUSED_CAP:
+        assert launches == 2, (rerank, top_k, launches)
+    else:
+        assert n_scan > 0 and launches > 2, (rerank, top_k, n_scan, launches)
+    return got, n_scan
 
 
 def build(ctx, rows, nlist, row_base=0, iters=4, extra=0):

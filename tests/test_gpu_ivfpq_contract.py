@@ -9,11 +9,17 @@ The GPU computes in fp32; each check carries a bound derived from the kernel's a
   rsqrtf is within 2 ulp, i.e. a relative 2^-22 (CUDA C Programming Guide, single-precision functions).
 """
 
+import os
+import sys
+
 import numpy as np
 import pytest
 
 import oracle
 from semtools_b200 import capi
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from test_gpu_ivfpq_batch import FUSED_CAP, search_on_route  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -145,27 +151,25 @@ def test_index_invariants(ctx, nlist, n):
 
 # ---------------------------------------------------------------------- exhaustive search is exact ---
 # nprobe = nlist and rerank >= n: every row is re-ranked, so the answer is the oracle's, bit for bit.
-# v2 (fused) re-ranks every code when the probed lists hold <= 1024; v1 runs for rerank > 1024 by itself
-# and for small n under STB_IVFPQ_V1=1.
+# v2 (fused) re-ranks every code when the probed lists hold <= 1024; v1 (multi-launch) runs for rerank > 1024,
+# which the v1 cases ask for at every n.
 @pytest.mark.parametrize("version,n", [("v2", 256), ("v2", 300), ("v2", 1000), ("v2", 1024),
                                        ("v1", 256), ("v1", 1000), ("v1", 1025), ("v1", 2000), ("v1", 4096)])
-def test_exhaustive_search_is_exact(ctx, monkeypatch, version, n):
+def test_exhaustive_search_is_exact(ctx, version, n):
     rng = np.random.default_rng(n + (7 if version == "v1" else 0))
     rows, p = edge_corpus(rng, n)
     base = 3 << 32
     c, idx = build(ctx, rows, nlist=3, row_base=base)
     n_forced = int(forced_ref(rows).sum())
-    if version == "v1" and n <= 1024:
-        monkeypatch.setenv("STB_IVFPQ_V1", "1")
+    rerank_min = FUSED_CAP + 1 if version == "v1" else 0
     try:
         for name, q in edge_queries(rng, rows, p).items():
             for k in sorted({1, 10, 1024, n}):
-                got, n_scan = idx.search(q, nprobe=3, top_k=k, rerank=max(n, k))
+                got, n_scan = search_on_route(ctx, idx, q, 3, k, max(n, k, rerank_min))
                 assert n_scan == n - n_forced
                 assert len(got) == min(k, n), (name, k)
                 assert_exact(got, rows, q, k, base)
     finally:
-        monkeypatch.delenv("STB_IVFPQ_V1", raising=False)
         idx.close(); c.close()
 
 

@@ -20,9 +20,10 @@ import oracle
 from semtools_b200 import capi
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from test_gpu_ivfpq_batch import (F64_SLOP, INV_REL, RERANK_CAP, U, WARP_KEEP, adc_keys, assert_hits,  # noqa: E402
-                                  bad_queries, check_batch, clustered, edge_corpus, edge_queries, forced_ref,
-                                  gamma, make_centers, predict, scan_routes, v2_precondition)
+from test_gpu_ivfpq_batch import (F64_SLOP, FUSED_CAP, INV_REL, RERANK_CAP, U, WARP_KEEP, adc_keys,  # noqa: E402
+                                  assert_hits, bad_queries, check_batch, clustered, edge_corpus, edge_queries,
+                                  forced_ref, gamma, make_centers, predict, scan_routes, search_on_route,
+                                  v2_precondition)
 
 pytestmark = pytest.mark.gpu
 
@@ -167,7 +168,7 @@ def test_appended_copies_get_their_originals_bits_and_fresh_rows_the_build_s_rul
 
 # ------------------------------------------------------------------------- exhaustive search is exact ---
 @pytest.mark.parametrize("n,n0", [(1000, 400), (3000, 1200)])
-def test_exhaustive_search_over_an_extended_index_is_exact(ctx, monkeypatch, n, n0):
+def test_exhaustive_search_over_an_extended_index_is_exact(ctx, n, n0):
     """Edge rows (NaN / +-inf, zero, 1e-25, 1e22, duplicates) on both sides of the build, two extends,
     nlist 3, row_base >= 2^32: with every list probed and every code re-ranked, each search path returns
     the oracle's answer over all n rows."""
@@ -192,9 +193,9 @@ def test_exhaustive_search_over_an_extended_index_is_exact(ctx, monkeypatch, n, 
             want_rows, want_d = oracle.search_rows(rows, q, k)
             return [int(r) + base for r in want_rows], np.asarray(want_d, np.float64)
 
-        def single(k):
+        def single(k, rerank_min=0):
             for q in Q:
-                got, n_scan = idx.search(q, nprobe=3, top_k=k, rerank=max(n, k))
+                got, n_scan = search_on_route(ctx, idx, q, 3, k, max(n, k, rerank_min))
                 assert n_scan == n_listed
                 want_rows, want_d = oracle_hits(q, k)
                 assert got["row"].tolist() == want_rows
@@ -206,12 +207,8 @@ def test_exhaustive_search_over_an_extended_index_is_exact(ctx, monkeypatch, n, 
             return
         for k in ks:
             single(k)                                           # fused v2
-        monkeypatch.setenv("STB_IVFPQ_V1", "1")
-        try:
-            for k in ks:
-                single(k)                                       # v1
-        finally:
-            monkeypatch.delenv("STB_IVFPQ_V1")
+        for k in ks:
+            single(k, FUSED_CAP + 1)                            # v1
         dev = torch.device("cuda:0")
         q_dev = torch.from_numpy(np.ascontiguousarray(Q)).to(dev)
         for k in (1, 10, 1024):

@@ -21,8 +21,8 @@ from semtools_b200 import capi
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from test_gpu_corpus_update import CHUNK, bits, check, scattered_ranges, snapshot  # noqa: E402
-from test_gpu_ivfpq_batch import (RERANK_CAP, assert_hits, check_batch, clustered, edge_corpus,  # noqa: E402
-                                  edge_queries, forced_ref, make_centers)
+from test_gpu_ivfpq_batch import (FUSED_CAP, RERANK_CAP, assert_hits, check_batch, clustered, edge_corpus,  # noqa: E402
+                                  edge_queries, forced_ref, make_centers, search_on_route)
 from test_gpu_ivfpq_extend import check_assignment_and_codes, list_and_code, same_export  # noqa: E402
 from test_gpu_ivfpq_filter import assert_store_query  # noqa: E402
 
@@ -247,7 +247,7 @@ def test_same_rows_give_the_same_index(ctx):
 
 # ------------------------------------------------------------------------------------------- search ---
 @pytest.mark.parametrize("n,n0", [(1200, 700)])
-def test_exhaustive_search_after_a_mixed_sequence_is_exact(ctx, monkeypatch, n, n0):
+def test_exhaustive_search_after_a_mixed_sequence_is_exact(ctx, n, n0):
     torch = pytest.importorskip("torch")
     rng = np.random.default_rng(705)
     rows, p = edge_corpus(rng, n)
@@ -277,15 +277,12 @@ def test_exhaustive_search_after_a_mixed_sequence_is_exact(ctx, monkeypatch, n, 
             return [int(x) + base for x in r], np.asarray(d, np.float64)
 
         for k in (1, 10, 1024):
-            for v1 in (False, True):
-                if v1:
-                    monkeypatch.setenv("STB_IVFPQ_V1", "1")
+            for rerank_min in (0, FUSED_CAP + 1):                  # fused v2, then v1
                 for q in Q:
-                    got, n_scan = idx.search(q, nprobe=3, top_k=k, rerank=max(n_listed, k))
+                    got, n_scan = search_on_route(ctx, idx, q, 3, k, max(n_listed, k, rerank_min))
                     wr, wd = want(q, k)
                     assert n_scan == n_listed and got["row"].tolist() == wr
                     assert np.array_equal(got["distance"].view(np.uint64), wd.view(np.uint64))
-                monkeypatch.delenv("STB_IVFPQ_V1", raising=False)
             dev = torch.device("cuda:0")
             q_dev = torch.from_numpy(np.ascontiguousarray(Q)).to(dev)
             hits = torch.zeros((len(Q), k, 2), dtype=torch.float64, device=dev)
