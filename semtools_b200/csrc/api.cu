@@ -12,6 +12,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "row_encode.cuh"
 
 static thread_local char g_err[512] = "";
 
@@ -945,7 +946,7 @@ static int corpus_ensure_q8(stb_ctx *ctx, stb_corpus *c) {
     const uint64_t cap = std::max<uint64_t>(c->n, c->capacity);
     cudaError_t e = cudaMalloc((void **)&np, cap * 256ull);
     if (e == cudaSuccess) e = cudaMalloc((void **)&ns, cap * sizeof(float));
-    if (e == cudaSuccess) e = cudaMalloc((void **)&pp, cap * 128ull);
+    if (e == cudaSuccess) e = cudaMalloc((void **)&pp, stb_q4_plane_bytes(cap));
     if (e == cudaSuccess) e = cudaMalloc((void **)&sp, cap * sizeof(float2));
     if (e != cudaSuccess) {
       cudaGetLastError(); cudaFree(np); cudaFree(ns); cudaFree(pp);
@@ -955,7 +956,7 @@ static int corpus_ensure_q8(stb_ctx *ctx, stb_corpus *c) {
     if (c->q8 && first) {
       STB_CUDA(cudaMemcpyAsync(np, c->q8, first * 256ull, cudaMemcpyDeviceToDevice, ctx->stream));
       STB_CUDA(cudaMemcpyAsync(ns, c->q8_scale, first * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
-      STB_CUDA(cudaMemcpyAsync(pp, c->q4, first * 128ull, cudaMemcpyDeviceToDevice, ctx->stream));
+      STB_CUDA(cudaMemcpyAsync(pp, c->q4, stb_q4_plane_bytes(first), cudaMemcpyDeviceToDevice, ctx->stream));   // whole tiles
       STB_CUDA(cudaMemcpyAsync(sp, c->q4_sr, first * sizeof(float2), cudaMemcpyDeviceToDevice, ctx->stream));
       STB_CUDA(cudaStreamSynchronize(ctx->stream));
     } else first = 0;
@@ -1198,6 +1199,18 @@ int stb_debug_corpus_copy(const stb_corpus *c, int which, uint64_t first, uint64
     return STB_ERR_RANGE;
   }
   if (n == 0) return STB_OK;
+  if (which == STB_COPY_Q8_PLANE) {   // the tiles that hold the rows, gathered back into row order
+    const uint64_t t0 = first / STB_Q4_TILE_ROWS;
+    const size_t off = stb_q4_plane_bytes(t0 * STB_Q4_TILE_ROWS), bytes = stb_q4_plane_bytes(first + n) - off;
+    uint8_t *tiles = (uint8_t *)malloc(bytes);
+    if (!tiles) { stb_set_error("debug_corpus_copy: cannot allocate %llu bytes", (unsigned long long)bytes); return STB_ERR_NOMEM; }
+    cudaError_t e = cudaMemcpyAsync(tiles, (const uint8_t *)src + off, bytes, cudaMemcpyDeviceToHost, c->ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->ctx->stream);
+    if (e == cudaSuccess) stb_q4_plane_gather(tiles, first, n, (uint8_t *)out);
+    free(tiles);
+    STB_CUDA(e);
+    return STB_OK;
+  }
   STB_CUDA(cudaMemcpyAsync(out, (const uint8_t *)src + first * unit, n * unit, cudaMemcpyDeviceToHost, c->ctx->stream));
   STB_CUDA(cudaStreamSynchronize(c->ctx->stream));
   return STB_OK;

@@ -7,7 +7,26 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
+#include <cstring>
+
 #include "common.cuh"
+
+// Nibble plane layout: 32-row tiles of 4096 B.  Chunk m (m < 8, 16 B: components 32m .. 32m+31) of row r
+// sits at (r / 32) * 4096 + m * 512 + (r % 32) * 16, so one lane per row reading chunk m of a tile makes
+// one 512-byte contiguous warp load (stb_scan_q4).  A plane of n rows takes ceil(n / 32) whole tiles.
+#define STB_Q4_TILE_ROWS 32
+__host__ __device__ __forceinline__ size_t stb_q4_plane_offset(uint64_t row, int m) {
+  return (size_t)(row >> 5) * 4096 + (size_t)m * 512 + (size_t)((uint32_t)row & 31u) * 16;
+}
+__host__ __device__ __forceinline__ size_t stb_q4_plane_bytes(uint64_t rows) { return (size_t)((rows + 31) >> 5) * 4096; }
+
+// rows [first, first + n) in row order (128 B each) from `tiles`, a copy of the plane's tiles from tile
+// first / 32 on (stb_debug_corpus_copy)
+inline void stb_q4_plane_gather(const uint8_t *tiles, uint64_t first, uint64_t n, uint8_t *out) {
+  const size_t base = stb_q4_plane_offset(first & ~(uint64_t)31, 0);
+  for (uint64_t i = 0; i < n; ++i)
+    for (int m = 0; m < 8; ++m) memcpy(out + i * 128 + m * 16, tiles + (stb_q4_plane_offset(first + i, m) - base), 16);
+}
 
 // q8 tier entry of one row: int8 codes, scale, nibble plane and {s, rho} (scan_topk.cu: stb_scan_q8,
 // stb_scan_q4).  Rows whose fp32 squared norm is not a normal number set *bad_flag (the tier is then
@@ -52,11 +71,11 @@ __device__ __forceinline__ void stb_q8_encode_row(float4 v0, float4 v1, int lane
     r2 = fmaf(d0, d0, fmaf(d1, d1, r2));
   }
   *reinterpret_cast<uint2 *>(out + row * 256 + (size_t)lane * 8) = make_uint2(w0, w1);
-  // plane: lane 4m + t holds components 32m + 8t .. +7; t < 2 are the low nibbles of bytes 16m + 8t ..,
+  // plane: lane 4m + t holds components 32m + 8t .. +7; t < 2 are the low nibbles of bytes 8t .. of chunk m,
   // t >= 2 the high nibbles of the same bytes (from lane + 2)
   const uint32_t p0 = __shfl_down_sync(0xffffffffu, n0, 2), p1 = __shfl_down_sync(0xffffffffu, n1, 2);
   if ((lane & 2) == 0)
-    *reinterpret_cast<uint2 *>(plane + row * 128 + (size_t)(lane >> 2) * 16 + (size_t)(lane & 1) * 8) = make_uint2(n0 | (p0 << 4), n1 | (p1 << 4));
+    *reinterpret_cast<uint2 *>(plane + stb_q4_plane_offset(row, lane >> 2) + (size_t)(lane & 1) * 8) = make_uint2(n0 | (p0 << 4), n1 | (p1 << 4));
 #pragma unroll
   for (int off = 16; off > 0; off >>= 1) r2 += __shfl_xor_sync(0xffffffffu, r2, off);
   if (lane == 0) {

@@ -484,10 +484,11 @@ __device__ __forceinline__ void stb_scan_q8(const ScanArgs &args, const uint8_t 
 // ---- the q8 tier's top-k scan: a 4-bit prefilter in front of the int8 codes --------------------
 // Beside the int8 codes the builder keeps a nibble plane, h_i = code_i >> 4 in [-8, 7] stored as
 // h_i + 8, two per byte (128 B/row), and per row {s, rho} with rho >= ||x^ - s (16 h + 7.5)||_2
-// (16 h + 7.5 is the midpoint of the 16 codes a nibble stands for).  Byte 16m + r of the plane
+// (16 h + 7.5 is the midpoint of the 16 codes a nibble stands for).  Byte r of a row's chunk m
 // (m < 8, r < 16) holds component 32m + r in its low nibble and 32m + 16 + r in its high nibble,
-// so lane j of a row's 8-lane group reads one 16-byte chunk, and w & 0x0F0F0F0F and
-// (w >> 4) & 0x0F0F0F0F each line up with one query word.  With the query quantised exactly as
+// so w & 0x0F0F0F0F and w & 0xF0F0F0F0 (16x the high nibbles) each line up with one query word;
+// the chunks of 32 consecutive rows are stored together (row_encode.cuh: stb_q4_plane_offset) and
+// one lane scores one row.  With the query quantised exactly as
 // in stb_scan_q8 (q~ = q16 / S, |q^_i - q~_i| <= 0.6 / S):
 //     c  <=  q^ . x~ + rho  <=  s (16 q~ . h + 7.5 sum q~) + rho + (0.6 / S) ||x~||_1
 //     ||x~||_1 <= 16 ||x~||_2 <= 16 (1 + rho) <= 32.3        (rho <= 128 s <= 1.01)
@@ -505,11 +506,11 @@ __device__ __forceinline__ void stb_scan_q8(const ScanArgs &args, const uint8_t 
 // identifies the launch: a later launch that shares the slot writes larger words, a word with
 // another tag reads as "no bound", so slots are never cleared and overlapped launches need no
 // ordering between them.  Warps re-read the words once per tile.
-#define STB_Q4_SCAN_U 8         // 8 rows x 1 LDG.128 per lane in flight (4 KiB per warp)
-#define STB_Q4_SPARE (32 * (STB_Q4_SCAN_U / 8 + 1))   // queued rows per warp: < 32 left over + one tile's worth ...
+#define STB_Q4_SCAN_U 8         // 32-row tiles (4 * U): one row x 8 LDG.128 per lane in flight (4 KiB per warp)
+#define STB_Q4_SPARE 64         // queued rows per warp: < 32 left over + one tile's worth ...
 #define STB_Q4_QUEUE (STB_Q4_SPARE + 4)                 // ... + a spare slot for lanes with nothing to store (16-B aligned)
 struct StbQ4Args {
-  const uint8_t *plane;          // [n][128] nibbles
+  const uint8_t *plane;          // nibbles, 128 B per row in 32-row tiles (stb_q4_plane_offset)
   const float2 *sr;              // [n] {s, rho}
   unsigned long long *thr;       // the k threshold words of this launch
   uint32_t tag;                  // this launch's tag (never 0)
@@ -517,19 +518,25 @@ struct StbQ4Args {
   unsigned long long *refined;   // debug counter: rows refined from the int8 codes
 };
 
+// c + sum of the four products of a's unsigned bytes with b's signed bytes
+__device__ __forceinline__ int stb_dp4a_us(uint32_t a, uint32_t b, int c) {
+  int d;
+  asm("dp4a.u32.s32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
+  return d;
+}
+
 template <int U, int RANGES, class Sink>
 __device__ __forceinline__ void stb_scan_q4(const ScanArgs &args, const uint8_t *q8, const float *q8_scale, const StbQ4Args &q4a,
                                             uint32_t *wq, uint32_t *pw, Sink &sink, const uint32_t *off = nullptr) {
-  static_assert(U % 8 == 0 && STB_Q8_MAX_K <= 32, "each lane owns U / 8 rows of a tile; one lane per threshold word");
-  constexpr int P = U / 8;
+  static_assert(4 * U == STB_Q4_TILE_ROWS && STB_Q8_MAX_K <= 32, "one plane tile per warp tile, one row per lane; one lane per threshold word");
   const int lane = threadIdx.x & 31;
-  const int g = lane >> 3;   // row group inside the warp
-  const int j = lane & 7;    // this lane reads plane bytes [16j, 16j+16): components 32j .. 32j+31
+  const int g = lane >> 3;   // refine: row group inside the warp
+  const int j = lane & 7;    // refine: int8 code bytes [16j, 16j+16) and [128+16j, ...)
   const StbQ8Query Q = stb_q8_query(args.q, j);
-  // query words in shared memory (registers go to the loads in flight).  Plane chunk of lane j: word i
-  // (components 32j + 4i .. +3; i < 4 pairs with the low nibbles of chunk word i, else with the high
-  // nibbles of word i - 4) as hi / lo byte words at pw[(i * 8 + j) * 2 + {0, 1}]; the int8 codes' words
-  // (StbQ8Query) at pw[128 + 16 j + {0..7: hi, 8..15: lo}]
+  // query words in shared memory, read by every lane at once.  Chunk m, word k (components 32m + 4k .. +3
+  // pair with its low nibbles, 32m + 16 + 4k .. +3 with its high nibbles): {low hi, low lo, high hi, high lo}
+  // byte words at pw[(4m + k) * 4 + {0..3}]; the int8 codes' words (StbQ8Query) of refine lane j at
+  // pw[128 + 16 j + {0..7: hi, 8..15: lo}]
   int sumq = 0;
   {
     const float4 *qv = reinterpret_cast<const float4 *>(args.q);
@@ -539,7 +546,7 @@ __device__ __forceinline__ void stb_scan_q4(const ScanArgs &args, const uint8_t 
       uint32_t hw, lw;
       stb_q16_words(__ldg(qv + 8 * j + i), Q.qs, Q.unusable, hw, lw, l1, sumq);
       if (g == 0) {
-        *reinterpret_cast<uint2 *>(pw + (i * 8 + j) * 2) = make_uint2(hw, lw);
+        *reinterpret_cast<uint2 *>(pw + (4 * j + (i & 3)) * 4 + (i < 4 ? 0 : 2)) = make_uint2(hw, lw);
         pw[128 + 16 * j + i] = Q.qhi[i];
         pw[128 + 16 * j + 8 + i] = Q.qlo[i];
       }
@@ -600,93 +607,59 @@ __device__ __forceinline__ void stb_scan_q4(const ScanArgs &args, const uint8_t 
 
   constexpr uint64_t tile_rows = 4 * U;
   const uint64_t n_tiles = (args.n_virtual + tile_rows - 1) / tile_rows;
+  const uint32_t n_rows = (uint32_t)args.n_virtual;
   StbRowMap<RANGES> rmap;
   rmap.restart();
-  stb_for_each_tile<RANGES, (64 / (4 * U) > 1 ? 64 / (4 * U) : 1)>(args, n_tiles, off, [&](uint64_t tile, bool first) {
+  stb_for_each_tile<RANGES, 2>(args, n_tiles, off, [&](uint64_t tile, bool first) {
     if (first) rmap.restart();
     // lane w < k: threshold word w as the other warps left it; issued with the tile's loads, folded in below
     const unsigned long long tw = lane < kw ? __ldcg(q4a.thr + lane) : 0ull;
-    uint4 a[U];
-    uint32_t row[U];
-    bool valid[U];
+    // lane l owns virtual row 32 tile + l (< 2^32: a shard holds at most 2^32 - 2 rows); past the end it
+    // reads the last row and is not queued
+    const uint32_t v = (uint32_t)tile * (uint32_t)tile_rows + (uint32_t)lane;
+    const bool valid = v < n_rows;
+    const uint32_t row = rmap.map(args, valid ? v : n_rows - 1);
+    const uint8_t *p = q4a.plane + stb_q4_plane_offset(row, 0);
+    uint4 a[8];
 #pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const uint64_t v = tile * tile_rows + (uint64_t)(u * 4 + g);
-      valid[u] = v < args.n_virtual;
-      const uint64_t vc = valid[u] ? v : (args.n_virtual - 1);
-      row[u] = rmap.map(args, vc);
-      const float4 t = stb_ld_stream(reinterpret_cast<const float4 *>(q4a.plane + (size_t)row[u] * 128 + (size_t)j * 16));
-      a[u] = make_uint4(__float_as_uint(t.x), __float_as_uint(t.y), __float_as_uint(t.z), __float_as_uint(t.w));
+    for (int m = 0; m < 8; ++m) {
+      const float4 t = stb_ld_stream(reinterpret_cast<const float4 *>(p + m * 512));
+      a[m] = make_uint4(__float_as_uint(t.x), __float_as_uint(t.y), __float_as_uint(t.z), __float_as_uint(t.w));
     }
-    // lane j of group g owns rows u = 8p + j: their {s, rho} (the warp's 32 owned rows of one p are consecutive)
-    uint32_t my_row[P];
-    bool my_valid[P];
-    float2 sr[P];
+    const float2 sr = __ldg(q4a.sr + row);
+    // low nibbles x {hi, lo} query bytes, 16 x high nibbles x {hi, lo}: exact in int32
+    int lh = 0, ll = 0, hh = 0, hl = 0;
 #pragma unroll
-    for (int p = 0; p < P; ++p) {
-      my_row[p] = row[8 * p];
-      my_valid[p] = valid[8 * p];
+    for (int m = 0; m < 8; ++m) {
 #pragma unroll
-      for (int u = 1; u < 8; ++u)
-        if (j == u) { my_row[p] = row[8 * p + u]; my_valid[p] = valid[8 * p + u]; }
-      sr[p] = __ldg(q4a.sr + my_row[p]);
-    }
-    int dot[U];
-#pragma unroll
-    for (int u = 0; u < U; ++u) { dot[u] = 0; }
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const uint2 ql = *reinterpret_cast<const uint2 *>(pw + (k * 8 + j) * 2);         // with the low nibbles
-      const uint2 qh = *reinterpret_cast<const uint2 *>(pw + ((4 + k) * 8 + j) * 2);   // with the high nibbles
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        const uint32_t w = k == 0 ? a[u].x : (k == 1 ? a[u].y : (k == 2 ? a[u].z : a[u].w));
-        const int lo = (int)(w & 0x0F0F0F0Fu), hi = (int)((w >> 4) & 0x0F0F0F0Fu);
-        int dh = __dp4a(lo, (int)ql.x, 0), dl = __dp4a(lo, (int)ql.y, 0);
-        dh = __dp4a(hi, (int)qh.x, dh);
-        dl = __dp4a(hi, (int)qh.y, dl);
-        dot[u] += dh * 256 + dl;
+      for (int k = 0; k < 4; ++k) {
+        const uint4 qw = *reinterpret_cast<const uint4 *>(pw + (4 * m + k) * 4);
+        const uint32_t w = k == 0 ? a[m].x : (k == 1 ? a[m].y : (k == 2 ? a[m].z : a[m].w));
+        const uint32_t lo = w & 0x0F0F0F0Fu, hi = w & 0xF0F0F0F0u;
+        lh = __dp4a((int)lo, (int)qw.x, lh);
+        ll = __dp4a((int)lo, (int)qw.y, ll);
+        hh = stb_dp4a_us(hi, qw.z, hh);
+        hl = stb_dp4a_us(hi, qw.w, hl);
       }
     }
     if (lane < kw && (uint32_t)(tw >> 32) == q4a.tag) tcache = max(tcache, (unsigned)tw);
     {
-      unsigned tmin = lane < kw ? tcache : 0xffffffffu;
-#pragma unroll
-      for (int off = 16; off > 0; off >>= 1) tmin = min(tmin, __shfl_xor_sync(0xffffffffu, tmin, off));
+      const unsigned tmin = __reduce_min_sync(0xffffffffu, lane < kw ? tcache : 0xffffffffu);
       T = tmin ? stb_ord2f(tmin) : -CUDART_INF_F;
     }
-#pragma unroll
-    for (int p = 0; p < P; ++p) {
-      // reduce-scatter over the 8-lane group (7 shuffles for 8 rows): lane j ends with row 8p + j
-      const int *x = dot + 8 * p;
-      int y4[4], y2[2];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int send = (j & 4) ? x[i] : x[i + 4], keep = (j & 4) ? x[i + 4] : x[i];
-        y4[i] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
-      }
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const int send = (j & 2) ? y4[i] : y4[i + 2], keep = (j & 2) ? y4[i + 2] : y4[i];
-        y2[i] = keep + __shfl_xor_sync(0xffffffffu, send, 2);
-      }
-      const int send = (j & 1) ? y2[0] : y2[1], keep = (j & 1) ? y2[1] : y2[0];
-      const int D = keep + __shfl_xor_sync(0xffffffffu, send, 1) - 8 * sumq;   // q16 . h
-      const float u4 = fmaf(sr[p].x, fmaf((float)D, A, B), sr[p].y + e_q4);
-      const bool want = my_valid[p] && (Q.unusable || !(u4 + (float)STB_Q4_SKIP_EPS < T));
-      const unsigned m = __ballot_sync(0xffffffffu, want);
-      wq[want ? qn + __popc(m & ((1u << lane) - 1u)) : STB_Q4_SPARE] = my_row[p];
-      qn += __popc(m);
-    }
-    while (qn >= 32) {
+    const int D = (lh + (hh >> 4)) * 256 + (ll + (hl >> 4)) - 8 * sumq;   // q16 . h (hh, hl: multiples of 16)
+    const float u4 = fmaf(sr.x, fmaf((float)D, A, B), sr.y + e_q4);
+    // an unusable query publishes no bound (refine), so T stays -inf and every valid row is queued
+    const bool want = valid && !(u4 + (float)STB_Q4_SKIP_EPS < T);
+    const unsigned mk = __ballot_sync(0xffffffffu, want);
+    wq[want ? qn + __popc(mk & ((1u << lane) - 1u)) : STB_Q4_SPARE] = row;
+    qn += __popc(mk);
+    if (qn >= 32) {                  // qn < 64: one batch at most
       __syncwarp();
       refine();
-      uint32_t rest[P];
-#pragma unroll
-      for (int p = 0; p < P; ++p) rest[p] = (32 * (p + 1) + lane < qn) ? wq[32 * (p + 1) + lane] : 0u;
+      const uint32_t rest = (32 + lane < qn) ? wq[32 + lane] : 0u;
       __syncwarp();
-#pragma unroll
-      for (int p = 0; p < P; ++p) wq[(32 * (p + 1) + lane < qn) ? 32 * p + lane : STB_Q4_SPARE] = rest[p];
+      wq[(32 + lane < qn) ? lane : STB_Q4_SPARE] = rest;
       qn -= 32;
     }
   });
