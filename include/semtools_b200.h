@@ -258,6 +258,20 @@ int stb_search_batch(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uin
 int stb_search_batch_dev(stb_ctx *ctx, const stb_corpus *corpus, const float *q_dev,
                          uint32_t nq, uint32_t top_k, stb_hit *out_hits_dev,
                          uint32_t *out_status_dev);
+/* The workspace query (Store::search_line_embeddings, src/workspace/store.rs:481-546) for a batch:
+ * for every query i, out_hits[i*top_k ..] and out_n[i] equal, bit for bit, what
+ *   stb_search(ctx, corpus, q_i, top_k, has_max, max_distance, STB_MODE_STORE_QUERY, row_ranges, n_ranges, ...)
+ * returns (unused tail: +inf / UINT64_MAX).  row_ranges are GLOBAL rows as stb_search takes them and are
+ * clipped to the shard; NULL = every row; non-NULL with n_ranges == 0 = the empty subset (every count 0).
+ * Ranges stb_search refuses are refused with the same status before anything is written.  Any top_k.
+ * Pipeline v2 runs on the eligible rows only (its sample over the 256-row tiles that hold an eligible row,
+ * ineligible scores masked out of both epilogues) when top_k <= 64 and the plan fits; K1 (stb_search)
+ * answers every query it leaves unproven, and all queries otherwise.  Pipeline v1 is never used here.
+ * The distance cap (strict; a NaN cap passes nothing) is applied to the sorted hits on the host. */
+int stb_search_batch_filtered(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t nq,
+                              uint32_t top_k, int has_max, double max_distance,
+                              const uint64_t *row_ranges, uint32_t n_ranges,
+                              stb_hit *out_hits, uint32_t *out_n);
 
 /* ---- fused multi-GPU search: K1 -> exchange over NVLink peer memory -> K4 -------------
  * One process (or thread) per GPU, one stb_xchg per rank.  Each rank allocates an
@@ -552,11 +566,14 @@ int stb_debug_ivfpq_export(const stb_ivfpq *index, float *centroids, float *code
  * i >= nq. */
 int stb_debug_ivfpq_batch_last(const stb_ivfpq *index, uint32_t i, uint32_t info[4], float *coarse,
                                uint32_t *probe, float *lut);
-/* Test hook for K2: describes the most recent stb_search_batch_dev on ctx (synchronises the stream).
- * info = {route (1 = v1, 2 = v2, 0 = none yet), nq, n_sample, stride, n_seg, seg_cap}; the last four are
- * v2's sampled tiles (0, stride, 2*stride, ...), emitting grid and per-(query, CTA) key capacity, and 0
- * after v1.  After v2, thr (may be NULL) receives the nq emission thresholds and cand_cnt (may be NULL)
- * the raw emission counts [nq][n_seg]; a count above seg_cap marks an overflowed segment. */
+/* Test hook for K2: describes the most recent stb_search_batch_dev or stb_search_batch_filtered on ctx
+ * (synchronises the stream).  info = {route, nq, n_sample, stride, n_seg, seg_cap}; route 1 = v1, 2 = v2,
+ * 3 = filtered v2, 4 = a filtered call that launched nothing on the tensor cores (K1 answered it, or nothing
+ * could be returned), 0 = none yet.  The last four are v2's sampled tiles (0, stride, 2*stride, ...; after
+ * route 3 they count listed tiles, the tiles holding an eligible row, in ascending order), emitting grid and
+ * per-(query, CTA) key capacity, and 0 after routes 1 and 4.  After routes 2 and 3, thr (may be NULL)
+ * receives the nq emission thresholds and cand_cnt (may be NULL) the raw emission counts [nq][n_seg]; a count
+ * above seg_cap marks an overflowed segment. */
 int stb_debug_batch_last(stb_ctx *ctx, uint32_t info[6], float *thr, uint32_t *cand_cnt);
 /* Build parameters of K2 (host-only): element type of the shadow the tensor-core pass runs on
  * (0 = bf16, 1 = fp16) and the bound |approximate - exact cosine| <= eps its selection uses. */

@@ -163,6 +163,7 @@ int stb_ctx_destroy(stb_ctx *c) {
   cudaFree(c->tickets); cudaFree(c->q4_thr); cudaFree(c->q4_refined); cudaFree(c->coscan_off);
   cudaFree(c->hist_dev); cudaFree(c->bq_tiles); cudaFree(c->b_submax); cudaFree(c->b_tilemax); cudaFree(c->b_cand);
   cudaFree(c->b_thr); cudaFree(c->b_cnt); cudaFree(c->b_keys); cudaFree(c->b_qbad);
+  cudaFree(c->b_franges); cudaFree(c->b_ftiles); cudaFree(c->b_fbits);
   cudaFree(c->bq_dev); cudaFree(c->bh_dev); cudaFree(c->bs_dev); cudaFree(c->embed_off_dev); cudaFree(c->embed_ids_dev); cudaFree(c->embed_out_dev);
   cudaFree(c->mut_stage); cudaFree(c->mut_idx); cudaFree(c->mut_flags);
   if (c->q_pin) cudaFreeHost(c->q_pin);
@@ -539,6 +540,15 @@ static int ensure_hits_pin(stb_ctx *ctx, size_t need) {
   return STB_OK;
 }
 
+// The distance cap of a top-k result sorted by (distance, row): how many leading hits have distance <
+// max_distance (strict; a NaN cap passes none).  Where top_k always caps (store-query mode, the top-k fast
+// path) the capped result is this prefix of the uncapped one.
+static uint64_t capped_hits(const stb_hit *hits, uint64_t n, int has_max, double max_distance) {
+  uint64_t i = 0;
+  while (i < n && !(has_max && !(hits[i].distance < max_distance))) ++i;
+  return i;
+}
+
 // Exact path for any input: collect rows whose approximate cosine >= cos_floor,
 // score them canonically, keep distance < limit, sort by (distance,row).
 // On return ctx->collect_hits holds the sorted hits and *n_pass their count.
@@ -657,12 +667,8 @@ int stb_search(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t 
     }
     const uint32_t n_hits = ctx->status_pin[0];
     if (ctx->status_pin[1]) {
-      uint64_t n = 0;
-      for (uint32_t i = 0; i < n_hits; ++i) {
-        if (has_max && !(ctx->hits_pin[i].distance < max_distance)) break;   // strict, sorted ascending
-        if (n < cap) out_hits[n] = ctx->hits_pin[i];
-        ++n;
-      }
+      const uint64_t n = capped_hits(ctx->hits_pin, n_hits, has_max, max_distance);
+      if (n && cap) memcpy(out_hits, ctx->hits_pin, std::min(n, cap) * sizeof(stb_hit));
       *out_n = n;
       if (n > cap) { stb_set_error("search: %llu hits, capacity %llu", (unsigned long long)n, (unsigned long long)cap); return STB_ERR_CAPACITY; }
       return STB_OK;
@@ -1224,6 +1230,76 @@ int stb_corpus_prepare_batch(stb_corpus *corpus) {
   return corpus_ensure_shadow(corpus->ctx, corpus);
 }
 
+}  // extern "C"
+
+// Pipeline v2's sample size and fit rule over the n_cover tiles it may sample: the COMPLETE tiles of the
+// shard (a padding row must never stand in for a real one), or, filtered, the listed tiles (tiles holding an
+// eligible row; the sampling epilogue takes their maxima over eligible rows only).
+//   ~4 tiles per SM, strided over the n_cover.  Expected candidates per query ~ top_k * n_cover / n_sample *
+//   e^(2 EPS x / sigma^2) (x = top score, sigma = 1/16 for the benchmark's rows: factor ~1.2 with the fp16
+//   shadow's EPS = 0.0012, ~3.8 with bf16's 0.0080).  Shards so large that this exceeds half of the finish
+//   kernel's 4096-key capacity sample 1/64 of the tiles instead (threshold kernel: CTA-per-query variant,
+//   <= 8192 tiles); beyond that v2 does not fit.
+struct BatchV2Plan {
+  uint32_t n_sample, stride;
+  bool fits;
+};
+static BatchV2Plan batch_v2_plan(const stb_ctx *ctx, uint32_t n_cover, uint32_t top_k) {
+  uint32_t n_sample = std::min<uint32_t>(n_cover, std::min<uint32_t>(4u * (uint32_t)ctx->sm_count, 608u));
+  const uint32_t margin_factor = STB_SHADOW_F16 ? 2u : 4u;
+  auto expected_emitted = [&](uint32_t ns) { return ns ? (uint64_t)top_k * margin_factor * ((n_cover + ns - 1) / ns) : 0; };
+  if (expected_emitted(n_sample) > 2048) {
+    const uint32_t sm = (uint32_t)ctx->sm_count;
+    n_sample = std::min<uint32_t>(std::min<uint32_t>(n_cover, 8192u), (n_cover / 64 + sm - 1) / sm * sm);
+  }
+  const bool fits = top_k <= 64 && n_sample >= top_k && expected_emitted(n_sample) <= 2048;
+  return {n_sample, fits ? n_cover / n_sample : 0u, fits};
+}
+
+// Pipeline v2 (batch_scan.cu): sampled threshold -> candidate-emitting wgmma epilogue -> exact finish.
+// Unfiltered (tile_ids == NULL) it samples and emits over the shadow tiles 0 .. n_cover-1 (the sample over
+// complete tiles only); filtered over the n_cover listed tiles tile_ids[] with the eligible-row bitmap.
+static int batch_v2_run(stb_ctx *ctx, const stb_corpus *corpus, const float *q_dev, uint32_t nq, uint32_t top_k,
+                        uint32_t n_cover, BatchV2Plan p, const uint32_t *tile_ids, const uint32_t *bitmap,
+                        stb_hit *out_hits_dev, uint32_t *out_status_dev) {
+  int rc;
+  const uint32_t m_tiles = (nq + 127) / 128, q_pad = m_tiles * 128;
+  const uint32_t n_tiles = (uint32_t)((corpus->n + 255) / 256);
+  const uint32_t n_emit = tile_ids ? n_cover : n_tiles;
+  constexpr uint32_t kSegCap = 64;                      // per (query, CTA): ~5 expected at 10M rows / 132 CTAs
+  const uint32_t n_seg = stb_batch_emit_grid(ctx, n_emit);
+  const uint32_t last[6] = {tile_ids ? 3u : 2u, nq, p.n_sample, p.stride, n_seg, kSegCap};
+  memcpy(ctx->b_last, last, sizeof(last));
+  if ((rc = dev_reserve(&ctx->b_qbad, &ctx->b_qbad_cap, (size_t)q_pad)) != STB_OK) return rc;
+  if ((rc = dev_reserve(&ctx->bq_tiles, &ctx->bq_tiles_cap, (size_t)q_pad * 512)) != STB_OK) return rc;
+  if ((rc = dev_reserve(&ctx->b_tilemax, &ctx->b_tilemax_cap, (size_t)p.n_sample * q_pad)) != STB_OK) return rc;
+  if ((rc = dev_reserve(&ctx->b_thr, &ctx->b_thr_cap, (size_t)q_pad)) != STB_OK) return rc;
+  if ((rc = dev_reserve(&ctx->b_cnt, &ctx->b_cnt_cap, (size_t)q_pad * n_seg)) != STB_OK) return rc;
+  if ((rc = dev_reserve(&ctx->b_keys, &ctx->b_keys_cap, (size_t)q_pad * n_seg * kSegCap)) != STB_OK) return rc;
+  STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
+  STB_CUDA(cudaMemsetAsync(ctx->b_cnt, 0, (size_t)q_pad * n_seg * sizeof(uint32_t), ctx->stream));
+  if ((rc = stb_launch_shadow_build(ctx, q_dev, nq, 128, ctx->bq_tiles, ctx->err_flag, 0, ctx->b_qbad)) != STB_OK) return rc;
+  if (tile_ids)
+    rc = stb_launch_batch_gemm_sample_filtered(ctx, ctx->bq_tiles, m_tiles, corpus->shadow, tile_ids, bitmap, p.n_sample,
+                                               p.stride, ctx->b_tilemax);
+  else
+    rc = stb_launch_batch_gemm_strided(ctx, ctx->bq_tiles, m_tiles, corpus->shadow, p.n_sample, p.stride, nullptr,
+                                       ctx->b_tilemax, nullptr);
+  if (rc != STB_OK) return rc;
+  if ((rc = stb_launch_batch_thresh(ctx, ctx->b_tilemax, p.n_sample, nq, q_pad, top_k, ctx->b_thr)) != STB_OK) return rc;
+  if (tile_ids)
+    rc = stb_launch_batch_gemm_emit_filtered(ctx, ctx->bq_tiles, m_tiles, corpus->shadow, tile_ids, bitmap, n_cover,
+                                             corpus->n, ctx->b_thr, ctx->b_cnt, ctx->b_keys, kSegCap);
+  else
+    rc = stb_launch_batch_gemm_emit(ctx, ctx->bq_tiles, m_tiles, corpus->shadow, n_tiles, corpus->n, ctx->b_thr,
+                                    ctx->b_cnt, ctx->b_keys, kSegCap);
+  if (rc != STB_OK) return rc;
+  return stb_launch_batch_finish2(ctx, ctx->b_keys, ctx->b_cnt, n_seg, kSegCap, nq, top_k, corpus->rows, corpus->n,
+                                  corpus->row_base, q_dev, ctx->b_qbad, out_hits_dev, out_status_dev);
+}
+
+extern "C" {
+
 int stb_search_batch_dev(stb_ctx *ctx, const stb_corpus *corpus_c, const float *q_dev, uint32_t nq,
                          uint32_t top_k, stb_hit *out_hits_dev, uint32_t *out_status_dev) {
   int rc = ctx_use(ctx);
@@ -1237,49 +1313,14 @@ int stb_search_batch_dev(stb_ctx *ctx, const stb_corpus *corpus_c, const float *
   if ((rc = corpus_ensure_shadow(ctx, corpus)) != STB_OK) return rc;
   const uint32_t m_tiles = (nq + 127) / 128, q_pad = m_tiles * 128;
   const uint32_t n_tiles = (uint32_t)((corpus->n + 255) / 256), n_sub = n_tiles * 8;
-  // Pipeline v2 (default): sampled threshold -> candidate-emitting wgmma epilogue -> exact finish
-  // (batch_scan.cu).  Proves every query for any top_k <= 64 unless a capacity overflows.  The round-1
-  // maxima/select/finish pipeline (v1) runs for top_k > 64 and wherever v2 does not fit.
-  // v2 sampling: ~4 COMPLETE tiles per SM, strided over the shard (a padding row must never stand
-  // in for a real one).  Expected candidates per query ~ top_k * n_full / n_sample * e^(2 EPS x / sigma^2)
-  // (x = top score, sigma = 1/16 for the benchmark's rows: factor ~1.2 with the fp16 shadow's
-  // EPS = 0.0012, ~3.8 with bf16's 0.0080).  Shards so large that this exceeds half of the finish
-  // kernel's 4096-key capacity sample 1/64 of the tiles instead (threshold kernel: CTA-per-query
-  // variant, <= 8192 tiles); beyond that, v1.
+  // Pipeline v2 (default, batch_v2_run).  Proves every query for any top_k <= 64 unless a capacity
+  // overflows.  The round-1 maxima/select/finish pipeline (v1) runs for top_k > 64 and wherever v2 does not fit.
   const uint32_t n_full = (uint32_t)(corpus->n / 256);
-  uint32_t n_sample = std::min<uint32_t>(n_full, std::min<uint32_t>(4u * (uint32_t)ctx->sm_count, 608u));
-  const uint32_t margin_factor = STB_SHADOW_F16 ? 2u : 4u;
-  auto expected_emitted = [&](uint32_t ns) { return ns ? (uint64_t)top_k * margin_factor * ((n_full + ns - 1) / ns) : 0; };
-  if (expected_emitted(n_sample) > 2048) {
-    const uint32_t sm = (uint32_t)ctx->sm_count;
-    n_sample = std::min<uint32_t>(std::min<uint32_t>(n_full, 8192u), (n_full / 64 + sm - 1) / sm * sm);
-  }
-  const bool v2_fits = n_sample >= top_k && expected_emitted(n_sample) <= 2048;
+  const BatchV2Plan plan = batch_v2_plan(ctx, n_full, top_k);
+  if (plan.fits) return batch_v2_run(ctx, corpus, q_dev, nq, top_k, n_full, plan, nullptr, nullptr, out_hits_dev, out_status_dev);
   // one flag per query, written by the query shadow build: a query that cannot be normalised in fp32
   // has a zero (or NaN) shadow whose scores bound nothing, and both finish kernels report it unproven
   if ((rc = dev_reserve(&ctx->b_qbad, &ctx->b_qbad_cap, (size_t)q_pad)) != STB_OK) return rc;
-  if (top_k <= 64 && v2_fits) {
-    constexpr uint32_t kSegCap = 64;                      // per (query, CTA): ~5 expected at 10M rows / 132 CTAs
-    const uint32_t n_seg = stb_batch_emit_grid(ctx, n_tiles);
-    const uint32_t stride = n_full / n_sample;
-    const uint32_t last[6] = {2u, nq, n_sample, stride, n_seg, kSegCap};
-    memcpy(ctx->b_last, last, sizeof(last));
-    if ((rc = dev_reserve(&ctx->bq_tiles, &ctx->bq_tiles_cap, (size_t)q_pad * 512)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->b_tilemax, &ctx->b_tilemax_cap, (size_t)n_sample * q_pad)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->b_thr, &ctx->b_thr_cap, (size_t)q_pad)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->b_cnt, &ctx->b_cnt_cap, (size_t)q_pad * n_seg)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->b_keys, &ctx->b_keys_cap, (size_t)q_pad * n_seg * kSegCap)) != STB_OK) return rc;
-    STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
-    STB_CUDA(cudaMemsetAsync(ctx->b_cnt, 0, (size_t)q_pad * n_seg * sizeof(uint32_t), ctx->stream));
-    if ((rc = stb_launch_shadow_build(ctx, q_dev, nq, 128, ctx->bq_tiles, ctx->err_flag, 0, ctx->b_qbad)) != STB_OK) return rc;
-    if ((rc = stb_launch_batch_gemm_strided(ctx, ctx->bq_tiles, m_tiles, corpus->shadow, n_sample, stride, nullptr,
-                                            ctx->b_tilemax, nullptr)) != STB_OK) return rc;
-    if ((rc = stb_launch_batch_thresh(ctx, ctx->b_tilemax, n_sample, nq, q_pad, top_k, ctx->b_thr)) != STB_OK) return rc;
-    if ((rc = stb_launch_batch_gemm_emit(ctx, ctx->bq_tiles, m_tiles, corpus->shadow, n_tiles, corpus->n, ctx->b_thr,
-                                         ctx->b_cnt, ctx->b_keys, kSegCap)) != STB_OK) return rc;
-    return stb_launch_batch_finish2(ctx, ctx->b_keys, ctx->b_cnt, n_seg, kSegCap, nq, top_k, corpus->rows, corpus->n,
-                                    corpus->row_base, q_dev, ctx->b_qbad, out_hits_dev, out_status_dev);
-  }
   const uint32_t last[6] = {1u, nq, 0u, 0u, 0u, 0u};
   memcpy(ctx->b_last, last, sizeof(last));
   // selection slices: enough CTAs (m_tiles x n_slices) to hide the latency of the streaming
@@ -1341,6 +1382,91 @@ int stb_search_batch(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uin
   return STB_OK;
 }
 
+// The store query (stb_search in STB_MODE_STORE_QUERY) for a batch.  The eligible rows' bitmap and the listed
+// tiles both come from one list of clipped ranges; filtered v2 runs when its plan fits over the listed tiles,
+// and K1 answers every query it leaves unproven (or all of them, route 4).  The cap is applied on the host:
+// store-query hits are a prefix of the uncapped top-k.
+int stb_search_batch_filtered(stb_ctx *ctx, const stb_corpus *corpus_c, const float *q, uint32_t nq, uint32_t top_k,
+                              int has_max, double max_distance, const uint64_t *row_ranges, uint32_t n_ranges,
+                              stb_hit *out_hits, uint32_t *out_n) {
+  int rc = ctx_use(ctx);
+  if (rc) return rc;
+  stb_corpus *corpus = const_cast<stb_corpus *>(corpus_c);
+  if (!corpus) { stb_set_error("search_batch_filtered: null corpus"); return STB_ERR_ARG; }
+  if (corpus->ctx != ctx) { stb_set_error("search_batch_filtered: corpus belongs to another context"); return STB_ERR_ARG; }
+  if (n_ranges && !row_ranges) { stb_set_error("search_batch_filtered: row_ranges is null"); return STB_ERR_ARG; }
+  if (nq == 0) return STB_OK;
+  if (!q || !out_n || (top_k && !out_hits)) { stb_set_error("search_batch_filtered: null argument"); return STB_ERR_ARG; }
+  auto pad = [&](uint32_t i, uint64_t n) {               // the unused tail, as the kernels pad it
+    for (uint64_t j = n; j < top_k; ++j) { out_hits[(size_t)i * top_k + j].distance = INFINITY; out_hits[(size_t)i * top_k + j].row = 0xffffffffffffffffull; }
+  };
+  // stb_search's early outs come before it reads the ranges (store.rs:489-491: top_k 0, the empty subset)
+  std::vector<uint32_t> loc;                             // clipped local [begin, end) pairs
+  if (top_k && !(row_ranges && n_ranges == 0) && corpus->n) {
+    if (row_ranges) {
+      loc.reserve(2 * (size_t)n_ranges);
+      if ((rc = stb_clip_ranges("search_batch_filtered", row_ranges, n_ranges, corpus->row_base, corpus->n,
+                                [&](uint64_t b, uint64_t e) { loc.push_back((uint32_t)b); loc.push_back((uint32_t)e); })) != STB_OK)
+        return rc;                                       // refused before anything is written
+    } else {
+      loc = {0u, (uint32_t)corpus->n};
+    }
+  }
+  const uint32_t none[6] = {4u, nq, 0u, 0u, 0u, 0u};
+  memcpy(ctx->b_last, none, sizeof(none));
+  if (loc.empty()) {
+    for (uint32_t i = 0; i < nq; ++i) { out_n[i] = 0; pad(i, 0); }
+    return STB_OK;
+  }
+  // listed tiles: the shadow tiles a clipped range touches (ascending, disjoint ranges -> ascending tiles)
+  std::vector<uint32_t> tiles;
+  for (size_t r = 0; r < loc.size(); r += 2)
+    for (uint32_t t = loc[r] / 256; t <= (loc[r + 1] - 1) / 256; ++t)
+      if (tiles.empty() || tiles.back() < t) tiles.push_back(t);
+  const uint32_t n_listed = (uint32_t)tiles.size();
+  const BatchV2Plan plan = batch_v2_plan(ctx, n_listed, top_k);
+  bool tensor_ok = plan.fits;
+  if (tensor_ok) {
+    rc = corpus_ensure_shadow(ctx, corpus);
+    if (rc == STB_ERR_STATE) tensor_ok = false;          // un-normalisable rows: K1 handles them
+    else if (rc != STB_OK) return rc;
+  }
+  std::vector<uint32_t> status((size_t)nq * 2, 0);
+  if (tensor_ok) {
+    const uint64_t n_words = (corpus->n + 255) / 256 * 8;
+    if ((rc = dev_reserve(&ctx->bq_dev, &ctx->bq_dev_cap, (size_t)nq * STB_D)) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->bh_dev, &ctx->bh_dev_cap, (size_t)nq * top_k)) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->bs_dev, &ctx->bs_dev_cap, (size_t)nq * 2)) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->b_franges, &ctx->b_franges_cap, loc.size(), 2048)) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->b_ftiles, &ctx->b_ftiles_cap, tiles.size(), 1024)) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->b_fbits, &ctx->b_fbits_cap, (size_t)n_words)) != STB_OK) return rc;
+    STB_CUDA(cudaMemcpyAsync(ctx->bq_dev, q, (size_t)nq * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    STB_CUDA(cudaMemcpyAsync(ctx->b_franges, loc.data(), loc.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+    STB_CUDA(cudaMemcpyAsync(ctx->b_ftiles, tiles.data(), tiles.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+    if ((rc = stb_launch_row_bitmap(ctx, ctx->b_franges, (uint32_t)(loc.size() / 2), n_words, ctx->b_fbits)) != STB_OK) return rc;
+    if ((rc = batch_v2_run(ctx, corpus, ctx->bq_dev, nq, top_k, n_listed, plan, ctx->b_ftiles, ctx->b_fbits, ctx->bh_dev,
+                           ctx->bs_dev)) != STB_OK) return rc;
+    STB_CUDA(cudaMemcpyAsync(out_hits, ctx->bh_dev, (size_t)nq * top_k * sizeof(stb_hit), cudaMemcpyDeviceToHost, ctx->stream));
+    STB_CUDA(cudaMemcpyAsync(status.data(), ctx->bs_dev, (size_t)nq * 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    STB_CUDA(cudaStreamSynchronize(ctx->stream));        // `loc` and `tiles` are read by the copies above
+  }
+  for (uint32_t i = 0; i < nq; ++i) {
+    stb_hit *oh = out_hits + (size_t)i * top_k;
+    uint64_t n = 0;
+    if (tensor_ok && status[2 * i + 1]) {
+      n = capped_hits(oh, status[2 * i], has_max, max_distance);
+    } else {
+      ctx->fallback_searches++;
+      rc = stb_search(ctx, corpus, q + (size_t)i * STB_D, top_k, has_max, max_distance, STB_MODE_STORE_QUERY, row_ranges,
+                      n_ranges, oh, top_k, &n);
+      if (rc != STB_OK) return rc;
+    }
+    out_n[i] = (uint32_t)n;
+    pad(i, n);
+  }
+  return STB_OK;
+}
+
 // Sharded K2: every rank answers the nq queries on its shard (stb_search_batch_dev), then ONE exchange over
 // NVLink peer memory -- each rank stores its nq x k hits + per-query proof flags into every peer's batch slot
 // (push kernel), waits for all peers' sequence flags and merges per query (merge kernel).  Two launches, no
@@ -1376,7 +1502,7 @@ int stb_debug_batch_last(stb_ctx *ctx, uint32_t info[6], float *thr, uint32_t *c
   STB_CUDA(cudaStreamSynchronize(ctx->stream));
   memcpy(info, ctx->b_last, sizeof(ctx->b_last));
   const uint32_t nq = ctx->b_last[1], n_seg = ctx->b_last[4];
-  if (ctx->b_last[0] == 2u && nq) {
+  if ((ctx->b_last[0] == 2u || ctx->b_last[0] == 3u) && nq) {
     if (thr) STB_CUDA(cudaMemcpy(thr, ctx->b_thr, (size_t)nq * sizeof(float), cudaMemcpyDeviceToHost));
     if (cand_cnt) STB_CUDA(cudaMemcpy(cand_cnt, ctx->b_cnt, (size_t)nq * n_seg * sizeof(uint32_t), cudaMemcpyDeviceToHost));
   }

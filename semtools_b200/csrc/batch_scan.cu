@@ -193,6 +193,9 @@ struct GemmArgs {
   uint64_t *cand_keys;        // [q_pad][grid][cand_cap] keys (score desc, local row)
   uint32_t cand_cap;          // per-segment capacity
   uint64_t n_rows;            // real corpus rows (padding rows of the last tile are never emitted)
+  // FILTER (stb_search_batch_filtered): tile t of the launch is shadow tile tile_ids[t * tile_stride]
+  const uint32_t *tile_ids;   // listed tiles: the shadow tiles holding an eligible row, ascending
+  const uint32_t *bitmap;     // eligible local rows, 1 bit each: 8 words per shadow tile
 };
 
 // warpgroup 0: bulk-copy producer (one thread); warpgroups 1 and 2: wgmma + epilogue, each on
@@ -203,7 +206,10 @@ struct GemmArgs {
 
 // EPI 0: per-sub-tile / per-tile maxima (pipeline v1, and the sampling pass of v2).
 // EPI 1: emit every (query,row) whose approximate score reaches the query's threshold.
-template <int EPI>
+// FILTER: the CTAs walk the listed tiles (args.tile_ids) and only eligible rows count (args.bitmap): EPI 0
+// takes each tile maximum over its eligible rows, EPI 1 emits eligible rows only.  The tile's 8 bitmap words
+// arrive with its first corpus slab, double-buffered behind the mbarriers.
+template <int EPI, bool FILTER>
 __global__ void __launch_bounds__(STB_GEMM_THREADS, 1)
 stb_batch_gemm_kernel(const GemmArgs args) {
   extern __shared__ uint8_t smem_raw[];
@@ -214,6 +220,10 @@ stb_batch_gemm_kernel(const GemmArgs args) {
   uint64_t *bars = reinterpret_cast<uint64_t *>(sA + STB_A_RING * STB_A_SLAB_BYTES);
   uint64_t *b_full = bars + 0, *b_empty = bars + STB_N_SLABS;      // one pair per K-slab
   uint64_t *a_full = bars + 2 * STB_N_SLABS, *a_empty = a_full + STB_A_RING;
+  // FILTER: [2][8] bitmap words, slot it & 1 = the tile of iteration it (the 256 bytes behind the ring hold
+  // the 20 barriers, then these 64 bytes)
+  [[maybe_unused]] uint32_t *s_mask = reinterpret_cast<uint32_t *>(bars + 24);
+  static_assert(24 * 8 + 2 * 8 * 4 <= 256, "mask words must fit behind the barriers");
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
@@ -234,11 +244,28 @@ stb_batch_gemm_kernel(const GemmArgs args) {
         const uint64_t t = blockIdx.x + (uint64_t)it * gridDim.x;
         // corpus tile, slab by slab: slab s of the previous tile is released as soon as the
         // last query tile's MMAs on it retire, so the refill overlaps the remaining slabs
-        const uint8_t *src = args.b_tiles + t * args.tile_stride * (size_t)(STB_N_SLABS * STB_B_SLAB_BYTES);
-        for (int s = 0; s < STB_N_SLABS; ++s) {
-          mbar_wait(b_empty + s, (it & 1) ^ 1);
-          mbar_expect_tx(b_full + s, STB_B_SLAB_BYTES);
-          bulk_g2s(sB + s * STB_B_SLAB_BYTES, src + (size_t)s * STB_B_SLAB_BYTES, STB_B_SLAB_BYTES, b_full + s);
+        if constexpr (FILTER) {
+          const uint64_t tile = __ldg(args.tile_ids + t * args.tile_stride);
+          const uint8_t *src = args.b_tiles + tile * (size_t)(STB_N_SLABS * STB_B_SLAB_BYTES);
+          for (int s = 0; s < STB_N_SLABS; ++s) {
+            mbar_wait(b_empty + s, (it & 1) ^ 1);
+            if (s == 0) {
+              // the mask slot of iteration it - 2 is free: every consumer warp released slab 0 of the tile
+              // of it - 1, which it does only after the epilogues of the tile of it - 2
+              mbar_expect_tx(b_full, STB_B_SLAB_BYTES + 32);
+              bulk_g2s(s_mask + (it & 1) * 8, args.bitmap + tile * 8, 32, b_full);
+            } else {
+              mbar_expect_tx(b_full + s, STB_B_SLAB_BYTES);
+            }
+            bulk_g2s(sB + s * STB_B_SLAB_BYTES, src + (size_t)s * STB_B_SLAB_BYTES, STB_B_SLAB_BYTES, b_full + s);
+          }
+        } else {
+          const uint8_t *src = args.b_tiles + t * args.tile_stride * (size_t)(STB_N_SLABS * STB_B_SLAB_BYTES);
+          for (int s = 0; s < STB_N_SLABS; ++s) {
+            mbar_wait(b_empty + s, (it & 1) ^ 1);
+            mbar_expect_tx(b_full + s, STB_B_SLAB_BYTES);
+            bulk_g2s(sB + s * STB_B_SLAB_BYTES, src + (size_t)s * STB_B_SLAB_BYTES, STB_B_SLAB_BYTES, b_full + s);
+          }
         }
         for (uint32_t m = 0; m < args.m_tiles; ++m) {
           for (int s = 0; s < STB_N_SLABS; ++s, ++a_cnt) {
@@ -269,6 +296,8 @@ stb_batch_gemm_kernel(const GemmArgs args) {
   uint32_t a_cnt = 0;
   for (uint32_t it = 0; it < my_tiles; ++it) {
     const uint64_t t = blockIdx.x + (uint64_t)it * gridDim.x;
+    [[maybe_unused]] uint64_t tile_row0 = 0;                 // FILTER: first row of the shadow tile
+    if constexpr (FILTER) tile_row0 = (uint64_t)__ldg(args.tile_ids + t * args.tile_stride) * STB_B_TILE;
     for (uint32_t m = 0; m < args.m_tiles; ++m, a_cnt += STB_N_SLABS) {
       const uint32_t q0 = m * STB_A_TILE + qrow;
       [[maybe_unused]] float thr[2];
@@ -314,12 +343,26 @@ stb_batch_gemm_kernel(const GemmArgs args) {
         float tmx[2] = {-CUDART_INF_F, -CUDART_INF_F};
 #pragma unroll
         for (int c = 0; c < STB_B_TILE / STB_SUB; ++c) {
+          [[maybe_unused]] uint32_t mw = 0;
+          if constexpr (FILTER) mw = s_mask[(it & 1) * 8 + c];
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            float mx = d[16 * c + 2 * h];
+            float mx;
+            if constexpr (FILTER) {
+              // an ineligible row's score is -inf here (a select, no branch): the maximum is an eligible
+              // row's score, which the threshold's sufficiency argument needs
+              mx = -CUDART_INF_F;
 #pragma unroll
-            for (int ii = 0; ii < 4; ++ii)
-              mx = fmaxf(mx, fmaxf(d[16 * c + 4 * ii + 2 * h], d[16 * c + 4 * ii + 2 * h + 1]));
+              for (int ii = 0; ii < 4; ++ii)
+#pragma unroll
+                for (int e = 0; e < 2; ++e)
+                  mx = fmaxf(mx, ((mw >> (ii * 8 + quad * 2 + e)) & 1u) ? d[16 * c + 4 * ii + 2 * h + e] : -CUDART_INF_F);
+            } else {
+              mx = d[16 * c + 2 * h];
+#pragma unroll
+              for (int ii = 0; ii < 4; ++ii)
+                mx = fmaxf(mx, fmaxf(d[16 * c + 4 * ii + 2 * h], d[16 * c + 4 * ii + 2 * h + 1]));
+            }
             mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
             mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
             tmx[h] = fmaxf(tmx[h], mx);
@@ -347,7 +390,14 @@ stb_batch_gemm_kernel(const GemmArgs args) {
         // no atomics, and keys land in ascending row order within a 32-row sub-tile.
 #pragma unroll
         for (int c = 0; c < STB_B_TILE / STB_SUB; ++c) {
-          const uint64_t row0 = t * STB_B_TILE + (uint64_t)c * STB_SUB;
+          uint64_t row0;
+          [[maybe_unused]] uint32_t mw = 0;
+          if constexpr (FILTER) {
+            row0 = tile_row0 + (uint64_t)c * STB_SUB;
+            mw = s_mask[(it & 1) * 8 + c];
+          } else {
+            row0 = t * STB_B_TILE + (uint64_t)c * STB_SUB;
+          }
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             // Branch-free on purpose: an accumulator read on a divergent path makes the compiler
@@ -361,6 +411,7 @@ stb_batch_gemm_kernel(const GemmArgs args) {
             hit |= __shfl_xor_sync(0xffffffffu, hit, 1);
             hit |= __shfl_xor_sync(0xffffffffu, hit, 2);
             if (row0 + 32 > args.n_rows) hit &= (row0 < args.n_rows) ? ((1u << (uint32_t)(args.n_rows - row0)) - 1u) : 0u;   // padding rows
+            if constexpr (FILTER) hit &= mw;                                                                                    // ineligible rows
             uint64_t *seg = args.cand_keys + ((size_t)(q0 + 8 * h) * gridDim.x + blockIdx.x) * args.cand_cap;
 #pragma unroll
             for (int ii = 0; ii < 4; ++ii)
@@ -403,13 +454,14 @@ int stb_launch_shadow_build(stb_ctx *ctx, const float *rows_dev, uint64_t n_rows
   return STB_OK;
 }
 
-template <int EPI>
+template <int EPI, bool FILTER = false>
 static int launch_gemm(stb_ctx *ctx, const GemmArgs &a) {
-  STB_ATTR_ONCE(ctx, EPI == 0 ? STB_ATTR_GEMM0 : STB_ATTR_GEMM1,
-                cudaFuncSetAttribute(stb_batch_gemm_kernel<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, STB_GEMM_SMEM));
+  const int attr = FILTER ? (EPI == 0 ? STB_ATTR_GEMM0F : STB_ATTR_GEMM1F) : (EPI == 0 ? STB_ATTR_GEMM0 : STB_ATTR_GEMM1);
+  STB_ATTR_ONCE(ctx, attr,
+                cudaFuncSetAttribute(stb_batch_gemm_kernel<EPI, FILTER>, cudaFuncAttributeMaxDynamicSharedMemorySize, STB_GEMM_SMEM));
   unsigned grid = (unsigned)std::min<uint32_t>(a.n_tiles, (uint32_t)ctx->sm_count);
   if (grid == 0) return STB_OK;
-  stb_batch_gemm_kernel<EPI><<<grid, STB_GEMM_THREADS, STB_GEMM_SMEM, ctx->stream>>>(a);
+  stb_batch_gemm_kernel<EPI, FILTER><<<grid, STB_GEMM_THREADS, STB_GEMM_SMEM, ctx->stream>>>(a);
   STB_CUDA(cudaGetLastError());
   ctx->kernel_launches++;
   return STB_OK;
@@ -437,6 +489,28 @@ int stb_launch_batch_gemm_emit(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_
   a.a_tiles = a_tiles; a.b_tiles = b_tiles; a.m_tiles = m_tiles; a.n_tiles = n_tiles; a.tile_stride = 1;
   a.thr = thr; a.cand_cnt = cand_cnt; a.cand_keys = cand_keys; a.cand_cap = cand_cap; a.n_rows = n_rows;
   return launch_gemm<1>(ctx, a);
+}
+
+// Pipeline v2 on the eligible rows only (stb_search_batch_filtered): the sampling pass over the listed tiles
+// 0, stride, 2*stride, ... (n_sample of them), tile maxima over eligible rows ...
+int stb_launch_batch_gemm_sample_filtered(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_tiles, const uint8_t *b_tiles,
+                                          const uint32_t *tile_ids, const uint32_t *bitmap, uint32_t n_sample,
+                                          uint32_t tile_stride, float *tilemax) {
+  GemmArgs a{};
+  a.a_tiles = a_tiles; a.b_tiles = b_tiles; a.m_tiles = m_tiles; a.n_tiles = n_sample; a.tile_stride = tile_stride;
+  a.tilemax = tilemax; a.tile_ids = tile_ids; a.bitmap = bitmap;
+  return launch_gemm<0, true>(ctx, a);
+}
+
+// ... and the candidate-emitting pass over all n_listed listed tiles, eligible rows only
+int stb_launch_batch_gemm_emit_filtered(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_tiles, const uint8_t *b_tiles,
+                                        const uint32_t *tile_ids, const uint32_t *bitmap, uint32_t n_listed, uint64_t n_rows,
+                                        const float *thr, uint32_t *cand_cnt, uint64_t *cand_keys, uint32_t cand_cap) {
+  GemmArgs a{};
+  a.a_tiles = a_tiles; a.b_tiles = b_tiles; a.m_tiles = m_tiles; a.n_tiles = n_listed; a.tile_stride = 1;
+  a.thr = thr; a.cand_cnt = cand_cnt; a.cand_keys = cand_keys; a.cand_cap = cand_cap; a.n_rows = n_rows;
+  a.tile_ids = tile_ids; a.bitmap = bitmap;
+  return launch_gemm<1, true>(ctx, a);
 }
 
 
@@ -638,6 +712,10 @@ int stb_launch_batch_finish(stb_ctx *ctx, const uint64_t *cand, uint32_t n_slice
 //   The same argument with "sample" = all rows narrows the emitted set to a >= A_k - 2 EPS
 //   (A_k = k-th largest emitted score = k-th largest score overall) before the exact re-score.
 //   No further proof obligation: the result is complete unless a capacity overflowed.
+// Filtered (FILTER GEMMs): "rows" are the eligible rows.  The sample is taken over listed tiles (each holds an
+//   eligible row) with ineligible scores masked to -inf, so each sampled maximum is an eligible row's score and
+//   S_k bounds the eligible k-th cosine; an unmasked ineligible row could lift S_k above it, and the eligible
+//   top-k would then go unemitted while the finish still reports the query proven.
 // =========================================================================================
 #define STB_V2_MAX_SAMPLE 608          // 19 values per lane in the threshold kernel
 #define STB_V2_MAX_K 64                // threshold kernel extracts k maxima serially

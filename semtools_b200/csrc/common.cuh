@@ -125,7 +125,13 @@ struct stb_ctx {
   uint32_t *b_cnt; size_t b_cnt_cap;          // v2: [q_pad] emitted-candidate counters
   uint64_t *b_keys; size_t b_keys_cap;        // v2: [q_pad][cand_cap] emitted keys
   uint32_t *b_qbad; size_t b_qbad_cap;        // [q_pad] 1: query could not be normalised
-  // the last stb_search_batch_dev: route (1 = v1, 2 = v2), nq, n_sample, stride, n_seg, seg_cap
+  // stb_search_batch_filtered: the clipped ranges (local [begin, end) u32 pairs), the listed tiles and the
+  // eligible-row bitmap (8 words per shadow tile), all built from the same clipped ranges
+  uint32_t *b_franges; size_t b_franges_cap;
+  uint32_t *b_ftiles; size_t b_ftiles_cap;
+  uint32_t *b_fbits; size_t b_fbits_cap;
+  // the last K2 call: route (1 = v1, 2 = v2, 3 = filtered v2, 4 = filtered, nothing on the tensor cores), nq,
+  // n_sample, stride, n_seg, seg_cap
   uint32_t b_last[6];
   float *bq_dev; size_t bq_dev_cap;           // host-call staging: queries
   stb_hit *bh_dev; size_t bh_dev_cap;         // host-call staging: hits
@@ -342,7 +348,7 @@ int stb_launch_batch_xchg(stb_ctx *ctx, const StbBatchXchgArgs &a, const stb_hit
 
 // opt-in to > 48 KiB dynamic shared memory (or another function attribute) once per context
 enum { STB_ATTR_GEMM0 = 0, STB_ATTR_GEMM1, STB_ATTR_MERGE, STB_ATTR_IVF_PROBE, STB_ATTR_IVF_V2, STB_ATTR_FINISH2,
-       STB_ATTR_IVF_BATCH };
+       STB_ATTR_IVF_BATCH, STB_ATTR_GEMM0F, STB_ATTR_GEMM1F };
 #define STB_ATTR_ONCE(ctx, bit, call)                         \
   do {                                                        \
     if (!((ctx)->func_attr_mask & (1u << (bit)))) {           \
@@ -370,6 +376,16 @@ int stb_launch_batch_gemm_emit(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_
                                const uint8_t *b_tiles, uint32_t n_tiles, uint64_t n_rows,
                                const float *thr, uint32_t *cand_cnt, uint64_t *cand_keys,
                                uint32_t cand_cap);
+// the same two passes over the listed tiles tile_ids[0, n_listed), eligible rows (bitmap) only
+int stb_launch_batch_gemm_sample_filtered(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_tiles,
+                                          const uint8_t *b_tiles, const uint32_t *tile_ids,
+                                          const uint32_t *bitmap, uint32_t n_sample, uint32_t tile_stride,
+                                          float *tilemax);
+int stb_launch_batch_gemm_emit_filtered(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_tiles,
+                                        const uint8_t *b_tiles, const uint32_t *tile_ids,
+                                        const uint32_t *bitmap, uint32_t n_listed, uint64_t n_rows,
+                                        const float *thr, uint32_t *cand_cnt, uint64_t *cand_keys,
+                                        uint32_t cand_cap);
 int stb_launch_batch_thresh(stb_ctx *ctx, const float *tilemax, uint32_t n_sample, uint32_t nq,
                             uint32_t q_pad, uint32_t top_k, float *thr);
 // candidates live in per-(query, CTA) segments: keys [q_pad][n_seg][seg_cap], counts [q_pad][n_seg];
@@ -386,6 +402,12 @@ int stb_launch_batch_finish(stb_ctx *ctx, const uint64_t *cand, uint32_t n_slice
                             uint32_t nq, uint32_t top_k, const float *rows, uint64_t n_rows,
                             uint64_t row_base, const float *queries_dev, const uint32_t *q_bad,
                             stb_hit *out_hits, uint32_t *out_status, const float *submax, uint32_t q_pad);
+
+// ---- ivfpq.cu: the eligibility bitmap of a path filter ----------------------------
+// bitmap[w] bit j = local row 32w + j lies in one of the n_ranges local [begin, end) u32 pairs of ranges_dev
+// (ascending, disjoint), for w < n_words
+int stb_launch_row_bitmap(stb_ctx *ctx, const uint32_t *ranges_dev, uint32_t n_ranges, uint64_t n_words,
+                          uint32_t *bitmap);
 
 // ---- device helpers ---------------------------------------------------------------
 // The distance limit of a search without max_distance: max_distance.unwrap_or(100.0), strict.

@@ -1152,7 +1152,8 @@ ivfb_finish_kernel(const IvfbArgs a) {
 // The eligibility pass of stb_ivfpq_search_filtered, once per call (every query of the call shares it):
 //   ivff_bitmap_kernel  bit r of the bitmap = local row r lies in one of the clipped ranges (thread per
 //                       32-row word: a binary search for the first range ending past the word, then the
-//                       at most 32 non-empty ranges that touch it)
+//                       at most 32 non-empty ranges that touch it); stb_launch_row_bitmap, which
+//                       stb_search_batch_filtered uses too
 //   ivff_elig_kernel    elig[l] = eligible codes of list l (warp per list, order[] read once: 4 B per
 //                       listed row); without a bitmap elig[l] is the list's length
 // The batched kernels' FILTER instantiations then probe only lists with elig > 0 and drop every code
@@ -1170,6 +1171,14 @@ __global__ void ivff_bitmap_kernel(const uint32_t *ranges, uint32_t n_ranges, ui
     bits |= (e - b == 32 ? 0xffffffffu : ((1u << (e - b)) - 1u)) << b;
   }
   bitmap[w] = bits;
+}
+
+int stb_launch_row_bitmap(stb_ctx *ctx, const uint32_t *ranges_dev, uint32_t n_ranges, uint64_t n_words, uint32_t *bitmap) {
+  if (n_words == 0) return STB_OK;
+  ivff_bitmap_kernel<<<(unsigned)((n_words + 255) / 256), 256, 0, ctx->stream>>>(ranges_dev, n_ranges, (uint32_t)n_words, bitmap);
+  STB_CUDA(cudaGetLastError());
+  ctx->kernel_launches += 1;
+  return STB_OK;
 }
 
 __global__ void ivff_elig_kernel(const uint32_t *list_off, const uint32_t *order, uint32_t nlist, const uint32_t *bitmap,
@@ -1902,10 +1911,9 @@ int stb_ivfpq_search_filtered(stb_ivfpq *x, const float *q, uint32_t nq, uint32_
       x->f_ranges_cap = cap;
     }
     STB_CUDA(cudaMemcpyAsync(x->f_ranges, loc.data(), loc.size() * 4, cudaMemcpyHostToDevice, st));
-    ivff_bitmap_kernel<<<(unsigned)((words + 255) / 256), 256, 0, st>>>(x->f_ranges, nr, (uint32_t)words, x->f_bitmap);
-    STB_CUDA(cudaGetLastError());
+    const int rc = stb_launch_row_bitmap(ctx, x->f_ranges, nr, words, x->f_bitmap);
+    if (rc != STB_OK) return rc;
     bitmap = x->f_bitmap;
-    ctx->kernel_launches += 1;
   }
   ivff_elig_kernel<<<(x->nlist + 7) / 8, 256, 0, st>>>(x->list_off, x->order, x->nlist, bitmap, x->f_elig);
   STB_CUDA(cudaGetLastError());

@@ -532,6 +532,22 @@ class Store:
             return []
         hits = self._gpu_corpus().search(query_vec, top_k, max_distance, capi.STB_MODE_STORE_QUERY,
                                          row_ranges=ranges)
+        return self._ranked(hits)
+
+    def search_line_embeddings_batch(self, query_vecs, subset_paths, top_k: int, max_distance=None) -> list:
+        """search_line_embeddings for many queries at once (stb_search_batch_filtered, one path filter for the
+        batch): element i is what search_line_embeddings(query_vecs[i], subset_paths, top_k, max_distance)
+        returns."""
+        query_vecs = np.ascontiguousarray(query_vecs, dtype=np.float32).reshape(-1, capi.STB_DIM)
+        if len(subset_paths) == 0 or top_k == 0:                     # :489-491
+            return [[] for _ in range(len(query_vecs))]
+        ranges = self._ranges_for(subset_paths)
+        if len(ranges) == 0:
+            return [[] for _ in range(len(query_vecs))]
+        res = self._gpu_corpus().search_batch_filtered(query_vecs, ranges, top_k, max_distance)
+        return [self._ranked(hits) for hits in res]
+
+    def _ranked(self, hits) -> list:
         out = []
         for h in hits:
             pi, ln = self._rows[int(h["row"])]
