@@ -272,6 +272,25 @@ int stb_search_batch_filtered(stb_ctx *ctx, const stb_corpus *corpus, const floa
                               uint32_t top_k, int has_max, double max_distance,
                               const uint64_t *row_ranges, uint32_t n_ranges,
                               stb_hit *out_hits, uint32_t *out_n);
+/* Threshold mode of search_documents (src/search/mod.rs:88-89,115-116) for a batch: for every query i,
+ * out_hits[out_offsets[i] .. out_offsets[i+1]) equals, bit for bit, the hits of
+ *   stb_search(ctx, corpus, q_i, 0, 1, max_distance, STB_MODE_SEARCH_DOCUMENTS, NULL, 0, ...)
+ * (every row with canonical distance < max_distance, ordered by (distance, row), global rows).
+ *   q            nq x 256 f32 (host)
+ *   out_offsets  nq + 1 entries, out_offsets[0] = 0; the hits of all queries are concatenated in query order
+ *   out_hits     cap entries (may be NULL when cap == 0).  If out_offsets[nq] > cap the first cap hits of the
+ *                concatenation are filled, every offset is still written and the call returns STB_ERR_CAPACITY.
+ * nq == 0 does nothing.  NULL q or out_offsets, or a corpus of another context: STB_ERR_ARG.  An empty corpus,
+ * and a max_distance that is NaN or <= 0, give every count 0 without a launch; +inf passes every row.  No top_k
+ * (threshold mode drops the cap) and no row ranges.
+ * Route (DESIGN §4, K2 item 6): the emitting wgmma pass with a per-query threshold derived from max_distance
+ * (DESIGN §5) into 64 keys per (query, CTA); queries with an overflowed segment get one more pass into exactly
+ * sized segments, as long as that pass's keys stay within STB_BATCH_THRESHOLD_RETRY_KEYS (128 MiB of keys);
+ * then the exact canonical re-score.  stb_search answers the rest: queries that cannot be normalised, the zero
+ * query, queries beyond the budget, and every query when the corpus holds rows that cannot be normalised. */
+#define STB_BATCH_THRESHOLD_RETRY_KEYS (1ull << 24)
+int stb_search_batch_threshold(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t nq,
+                               double max_distance, stb_hit *out_hits, uint64_t cap, uint64_t *out_offsets);
 
 /* ---- fused multi-GPU search: K1 -> exchange over NVLink peer memory -> K4 -------------
  * One process (or thread) per GPU, one stb_xchg per rank.  Each rank allocates an
@@ -566,14 +585,17 @@ int stb_debug_ivfpq_export(const stb_ivfpq *index, float *centroids, float *code
  * i >= nq. */
 int stb_debug_ivfpq_batch_last(const stb_ivfpq *index, uint32_t i, uint32_t info[4], float *coarse,
                                uint32_t *probe, float *lut);
-/* Test hook for K2: describes the most recent stb_search_batch_dev or stb_search_batch_filtered on ctx
- * (synchronises the stream).  info = {route, nq, n_sample, stride, n_seg, seg_cap}; route 1 = v1, 2 = v2,
- * 3 = filtered v2, 4 = a filtered call that launched nothing on the tensor cores (K1 answered it, or nothing
- * could be returned), 0 = none yet.  The last four are v2's sampled tiles (0, stride, 2*stride, ...; after
- * route 3 they count listed tiles, the tiles holding an eligible row, in ascending order), emitting grid and
- * per-(query, CTA) key capacity, and 0 after routes 1 and 4.  After routes 2 and 3, thr (may be NULL)
- * receives the nq emission thresholds and cand_cnt (may be NULL) the raw emission counts [nq][n_seg]; a count
- * above seg_cap marks an overflowed segment. */
+/* Test hook for K2: describes the most recent stb_search_batch_dev, stb_search_batch_filtered or
+ * stb_search_batch_threshold on ctx (synchronises the stream).  info = {route, nq, a, b, n_seg, seg_cap}; route
+ * 1 = v1, 2 = v2, 3 = filtered v2, 4 = a filtered call that launched nothing on the tensor cores (K1 answered it,
+ * or nothing could be returned), 5 = threshold mode, 0 = none yet.  Slots 2-3 (a, b):
+ *   routes 1-4: n_sample, stride -- v2's sampled tiles (0, stride, 2*stride, ...; after route 3 they count listed
+ *               tiles, the tiles holding an eligible row, in ascending order); 0 after routes 1 and 4;
+ *   route 5:    the queries re-emitted by the second tensor pass, and the queries stb_search answered.
+ * n_seg and seg_cap are the emitting grid and the first pass's per-(query, CTA) key capacity, 0 after routes 1
+ * and 4 and after a route 5 call that launched nothing.  After routes 2, 3 and a route 5 call that ran the
+ * tensor pass, thr (may be NULL) receives the nq emission thresholds and cand_cnt (may be NULL) the raw
+ * first-pass emission counts [nq][n_seg]; a count above seg_cap marks an overflowed segment. */
 int stb_debug_batch_last(stb_ctx *ctx, uint32_t info[6], float *thr, uint32_t *cand_cnt);
 /* Build parameters of K2 (host-only): element type of the shadow the tensor-core pass runs on
  * (0 = bf16, 1 = fp16) and the bound |approximate - exact cosine| <= eps its selection uses. */

@@ -12,4 +12,4 @@ $NVCC -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 \
   semtools_b200/csrc/api.cu semtools_b200/csrc/scan_topk.cu \
   semtools_b200/csrc/hits_merge.cu semtools_b200/csrc/embed_pool.cu \
   semtools_b200/csrc/batch_scan.cu semtools_b200/csrc/ivfpq.cu \
-  semtools_b200/csrc/corpus_update.cu "$@"
+  semtools_b200/csrc/corpus_update.cu semtools_b200/csrc/batch_threshold.cu "$@"

@@ -25,7 +25,7 @@ SYMBOLS = [
     "stb_corpus_rows", "stb_corpus_data_dev", "stb_corpus_read", "stb_corpus_update", "stb_corpus_remove", "stb_embed", "stb_embed_dev",
     "stb_embed_status", "stb_search",
     "stb_search_topk_dev", "stb_corpus_prepare", "stb_corpus_tier_stats", "stb_corpus_prepare_batch", "stb_search_batch", "stb_search_batch_dev",
-    "stb_search_batch_filtered",
+    "stb_search_batch_filtered", "stb_search_batch_threshold",
     "stb_xchg_create", "stb_xchg_destroy", "stb_xchg_local_handle",
     "stb_xchg_connect", "stb_xchg_connect_local", "stb_search_topk_xchg", "stb_search_xchg", "stb_search_many", "stb_xchg_create_batch", "stb_search_batch_xchg_dev", "stb_ivfpq_build",
     "stb_ivfpq_destroy", "stb_ivfpq_extend", "stb_ivfpq_stats", "stb_ivfpq_search", "stb_ivfpq_search_dev", "stb_hits_merge_dev", "stb_hits_merge_batch_dev", "stb_hits_merge", "stb_fnv1a64", "stb_line_id", "stb_line_ids",
@@ -97,6 +97,7 @@ def lib() -> C.CDLL:
     L.stb_search_batch.argtypes = [vp, vp, vp, u32, u32, vp, vp]
     L.stb_search_batch_dev.argtypes = [vp, vp, vp, u32, u32, vp, vp]
     L.stb_search_batch_filtered.argtypes = [vp, vp, vp, u32, u32, i32, f64, vp, u32, vp, vp]
+    L.stb_search_batch_threshold.argtypes = [vp, vp, vp, u32, f64, vp, u64, vp]
     L.stb_xchg_create.argtypes = [vp, u32, u32, u32, C.POINTER(vp)]
     L.stb_xchg_destroy.argtypes = [vp]
     L.stb_xchg_local_handle.argtypes = [vp, vp]
@@ -230,13 +231,15 @@ class Context:
 
     def batch_last(self):
         """stb_debug_batch_last: the most recent K2 device call on this context.  Returns a dict with
-        route (1 = v1, 2 = v2, 3 = filtered v2, 4 = filtered without the tensor cores), nq, n_sample, stride,
-        n_seg, seg_cap and, after v2 (filtered or not), thr [nq] (f32) and cand_cnt [nq][n_seg] (raw counts;
-        > seg_cap marks an overflowed segment)."""
+        route (1 = v1, 2 = v2, 3 = filtered v2, 4 = filtered without the tensor cores, 5 = threshold mode), nq,
+        n_sample, stride (routes 1-4) or retried, k1 (route 5: queries re-emitted by the second tensor pass /
+        answered by stb_search), n_seg, seg_cap and, after v2 (filtered or not) and a route 5 call that ran the
+        tensor pass, thr [nq] (f32) and cand_cnt [nq][n_seg] (raw counts; > seg_cap marks an overflowed segment)."""
         info = np.zeros(6, dtype=np.uint32)
         _check(lib().stb_debug_batch_last(self._h, _np_ptr(info), None, None))
-        out = dict(zip(("route", "nq", "n_sample", "stride", "n_seg", "seg_cap"), (int(v) for v in info)))
-        if out["route"] in (2, 3):
+        names = ("retried", "k1") if info[0] == 5 else ("n_sample", "stride")
+        out = dict(zip(("route", "nq") + names + ("n_seg", "seg_cap"), (int(v) for v in info)))
+        if out["route"] in (2, 3) or (out["route"] == 5 and out["n_seg"]):
             thr = np.zeros(max(out["nq"], 1), dtype=np.float32)
             cnt = np.zeros((max(out["nq"], 1), max(out["n_seg"], 1)), dtype=np.uint32)
             _check(lib().stb_debug_batch_last(self._h, _np_ptr(info), _np_ptr(thr), _np_ptr(cnt)))
@@ -453,6 +456,26 @@ class Corpus:
                                                int(max_distance is not None), float(max_distance or 0.0),
                                                _np_ptr(rr), n_rr, _np_ptr(out), _np_ptr(cnt)))
         return [out[i, : cnt[i]] for i in range(nq)]
+
+    def search_batch_threshold(self, queries, max_distance: float, cap: int | None = None):
+        """stb_search_batch_threshold: for each query, what search(q, 0, max_distance) returns in threshold mode
+        (every row with distance < max_distance).  Starts from a modest capacity and retries once with the
+        reported total.  Returns a list of HIT_DTYPE arrays, one per query."""
+        queries = np.ascontiguousarray(queries, dtype=np.float32)
+        if queries.ndim != 2 or queries.shape[1] != STB_DIM:
+            raise StbError(STB_ERR_ARG, f"queries must be (nq,{STB_DIM}) f32")
+        nq = queries.shape[0]
+        if cap is None:
+            cap = max(nq, 1) * 64
+        offsets = np.zeros(nq + 1, dtype=np.uint64)
+        while True:
+            out = np.zeros(max(cap, 1), dtype=HIT_DTYPE)
+            rc = _check(lib().stb_search_batch_threshold(self.ctx._h, self._h, _np_ptr(queries), nq, float(max_distance),
+                                                         _np_ptr(out), cap, _np_ptr(offsets)), allow_capacity=True)
+            if rc == STB_ERR_CAPACITY:
+                cap = int(offsets[nq])
+                continue
+            return [out[int(offsets[i]): int(offsets[i + 1])] for i in range(nq)]
 
     def search_batch_dev(self, q_dev: int, nq: int, top_k: int, out_hits_dev: int, out_status_dev: int):
         """stb_search_batch_dev: asynchronous, everything stays in HBM."""

@@ -6,6 +6,8 @@
 #include <stdlib.h>
 
 #include <algorithm>
+#include <cmath>
+#include <memory>
 #include <mutex>
 #include <new>
 #include <unordered_set>
@@ -164,6 +166,9 @@ int stb_ctx_destroy(stb_ctx *c) {
   cudaFree(c->hist_dev); cudaFree(c->bq_tiles); cudaFree(c->b_submax); cudaFree(c->b_tilemax); cudaFree(c->b_cand);
   cudaFree(c->b_thr); cudaFree(c->b_cnt); cudaFree(c->b_keys); cudaFree(c->b_qbad);
   cudaFree(c->b_franges); cudaFree(c->b_ftiles); cudaFree(c->b_fbits);
+  cudaFree(c->t_dst); cudaFree(c->t_segoff); cudaFree(c->t_cur); cudaFree(c->t_rq); cudaFree(c->t_rthr);
+  cudaFree(c->t_buf); cudaFree(c->t_off); cudaFree(c->t_slot); cudaFree(c->t_out_at); cudaFree(c->t_hits);
+  cudaFree(c->t_sort_tmp);
   cudaFree(c->bq_dev); cudaFree(c->bh_dev); cudaFree(c->bs_dev); cudaFree(c->embed_off_dev); cudaFree(c->embed_ids_dev); cudaFree(c->embed_out_dev);
   cudaFree(c->mut_stage); cudaFree(c->mut_idx); cudaFree(c->mut_flags);
   if (c->q_pin) cudaFreeHost(c->q_pin);
@@ -1467,6 +1472,222 @@ int stb_search_batch_filtered(stb_ctx *ctx, const stb_corpus *corpus_c, const fl
   return STB_OK;
 }
 
+}  // extern "C"
+
+// ---- threshold mode for a batch (stb_search_batch_threshold, route 5) ---------------------------------------
+// delta: |canonical f64 distance - (1 - exact cosine)| of any pair of f32 vectors the shadow can normalise is
+// below ~1e-13 (256-term f64 FMA chains, two square roots, one division; DESIGN §5); 1e-12 leaves 10x slack.
+#define STB_THR_DELTA 1.0e-12
+#define STB_THR_SEG_CAP 64u        // first pass: keys per (query, CTA), as pipeline v2
+#define STB_THR_CHUNK 4096u        // queries per pipeline run (keeps every candidate count within int)
+
+// The emission threshold of the queries the tensor cores answer: ((1 - M) - EPS) - delta in f64, rounded toward
+// -inf to f32.  Every row with canonical d < M has exact cosine c > 1 - M - delta and score a >= c - EPS.
+static float thr_emission_value(double max_distance) {
+  double eps = 0.0;
+  stb_batch_build_params(nullptr, &eps);
+  const double x = ((1.0 - max_distance) - eps) - STB_THR_DELTA;
+  float f = (float)x;
+  if ((double)f > x) f = std::nextafter(f, -INFINITY);
+  return f;
+}
+
+// One chunk of queries q[0, n) (global indices c0 ..) on the tensor cores.  On return slot_query[s] / pass[s]
+// are the chunk-local query and hit count of every answered slot, k1 lists the queries K1 must answer, and the
+// sorted hits of slot s sit at ctx->t_buf (distance bits at [0, K), rows at [K, 2K)) from (*off)[s].
+struct ThrChunk {
+  std::vector<uint32_t> slot_query, pass, k1;
+  std::vector<int> off;
+  uint32_t retried = 0;
+};
+static int thr_chunk_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, uint32_t c0, uint32_t n, double max_distance,
+                         float t, ThrChunk *out) {
+  int rc;
+  const uint32_t m_tiles = (n + 127) / 128, q_pad = m_tiles * 128;
+  const uint32_t n_tiles = (uint32_t)((corpus->n + 255) / 256);
+  const uint32_t n_seg = stb_batch_emit_grid(ctx, n_tiles);
+  float *thr = ctx->b_thr + c0;
+  uint32_t *cnt = ctx->b_cnt + (size_t)c0 * n_seg;
+  if ((rc = dev_reserve(&ctx->bq_dev, &ctx->bq_dev_cap, (size_t)n * STB_D)) != STB_OK) return rc;
+  if ((rc = dev_reserve(&ctx->b_qbad, &ctx->b_qbad_cap, (size_t)q_pad)) != STB_OK) return rc;
+  if ((rc = dev_reserve(&ctx->bq_tiles, &ctx->bq_tiles_cap, (size_t)q_pad * 512)) != STB_OK) return rc;
+  if ((rc = dev_reserve(&ctx->b_keys, &ctx->b_keys_cap, (size_t)q_pad * n_seg * STB_THR_SEG_CAP)) != STB_OK) return rc;
+  STB_CUDA(cudaMemcpyAsync(ctx->bq_dev, q, (size_t)n * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+  STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
+  STB_CUDA(cudaMemsetAsync(cnt, 0, (size_t)q_pad * n_seg * sizeof(uint32_t), ctx->stream));
+  if ((rc = stb_launch_shadow_build(ctx, ctx->bq_dev, n, 128, ctx->bq_tiles, ctx->err_flag, 0, ctx->b_qbad)) != STB_OK) return rc;
+  if ((rc = stb_launch_batch_thr_dist(ctx, ctx->bq_dev, ctx->b_qbad, n, q_pad, t, thr)) != STB_OK) return rc;
+  if ((rc = stb_launch_batch_gemm_emit(ctx, ctx->bq_tiles, m_tiles, corpus->shadow, n_tiles, corpus->n, thr, cnt,
+                                       ctx->b_keys, STB_THR_SEG_CAP)) != STB_OK) return rc;
+  std::vector<uint32_t> hcnt((size_t)n * n_seg);
+  std::vector<float> hthr(n);
+  STB_CUDA(cudaMemcpyAsync(hcnt.data(), cnt, hcnt.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  STB_CUDA(cudaMemcpyAsync(hthr.data(), thr, n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+  STB_CUDA(cudaStreamSynchronize(ctx->stream));
+
+  // Route: a query excluded by its threshold goes to K1; one whose segments all fit is answered from the first
+  // pass; one with an overflowed segment is re-emitted while the re-emission's keys stay within the budget, and
+  // goes to K1 beyond it.  Slots: the first-pass queries in query order, then the re-emitted ones.
+  std::vector<uint32_t> direct, retry;
+  std::vector<uint64_t> totals(n, 0);
+  uint64_t retry_keys = 0;
+  for (uint32_t i = 0; i < n; ++i) {
+    if (hthr[i] == INFINITY) { out->k1.push_back(i); continue; }
+    bool over = false;
+    for (uint32_t s = 0; s < n_seg; ++s) {
+      const uint32_t c = hcnt[(size_t)i * n_seg + s];
+      totals[i] += c;
+      over |= c > STB_THR_SEG_CAP;
+    }
+    if (!over) direct.push_back(i);
+    else if (retry_keys + totals[i] <= STB_BATCH_THRESHOLD_RETRY_KEYS) { retry.push_back(i); retry_keys += totals[i]; }
+    else out->k1.push_back(i);
+  }
+  out->retried = (uint32_t)retry.size();
+  const uint32_t n_direct = (uint32_t)direct.size(), n_retry = out->retried, n_slots = n_direct + n_retry;
+  out->slot_query = direct;
+  out->slot_query.insert(out->slot_query.end(), retry.begin(), retry.end());
+  out->pass.assign(n_slots, 0);
+  out->off.assign(n_slots + 1, 0);
+  if (n_slots == 0) return STB_OK;
+  // key layout: slot s owns [off[s], off[s+1]); a first-pass segment lands at dst, a re-emitted one at segoff
+  const uint32_t r_tiles = (n_retry + 127) / 128, r_pad = r_tiles * 128;
+  std::vector<uint64_t> dst((size_t)n * n_seg, ~0ull), segoff((size_t)r_pad * n_seg + 1, 0);
+  uint64_t at = 0;
+  for (uint32_t s = 0; s < n_slots; ++s) {
+    const uint32_t i = out->slot_query[s];
+    out->off[s] = (int)at;
+    for (uint32_t g = 0; g < n_seg; ++g) {
+      if (s < n_direct) dst[(size_t)i * n_seg + g] = at;
+      else segoff[(size_t)(s - n_direct) * n_seg + g] = at;
+      at += hcnt[(size_t)i * n_seg + g];
+    }
+  }
+  out->off[n_slots] = (int)at;
+  for (size_t j = (size_t)n_retry * n_seg; j < segoff.size(); ++j) segoff[j] = at;   // padding slots: empty
+  const int K = (int)at;
+  if ((rc = dev_reserve(&ctx->t_buf, &ctx->t_buf_cap, std::max<size_t>(4 * (size_t)K, 1))) != STB_OK) return rc;
+  if ((rc = dev_reserve(&ctx->t_off, &ctx->t_off_cap, (size_t)n_slots + 1)) != STB_OK) return rc;
+  if ((rc = dev_reserve(&ctx->t_slot, &ctx->t_slot_cap, 2 * (size_t)n_slots)) != STB_OK) return rc;
+  if ((rc = dev_reserve(&ctx->t_dst, &ctx->t_dst_cap, dst.size())) != STB_OK) return rc;
+  size_t sort_bytes = 0;
+  if ((rc = stb_batch_thr_sort_bytes(ctx, K, n_slots, ctx->t_off, &sort_bytes)) != STB_OK) return rc;
+  if ((rc = dev_reserve(&ctx->t_sort_tmp, &ctx->t_sort_tmp_cap, sort_bytes)) != STB_OK) return rc;
+  uint64_t *A = ctx->t_buf, *B = A + K, *C = B + K, *D = C + K;
+  STB_CUDA(cudaMemcpyAsync(ctx->t_off, out->off.data(), out->off.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+  STB_CUDA(cudaMemcpyAsync(ctx->t_slot, out->slot_query.data(), n_slots * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+  STB_CUDA(cudaMemcpyAsync(ctx->t_dst, dst.data(), dst.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->stream));
+  if ((rc = stb_launch_batch_thr_compact(ctx, ctx->b_keys, cnt, ctx->t_dst, (uint64_t)n * n_seg, STB_THR_SEG_CAP, A)) != STB_OK) return rc;
+  if (n_retry) {
+    // one more pass over the re-emitted queries' shadow tiles (rebuilt from their f32 rows: the same bits), into
+    // segments sized by the first pass's exact counts
+    if ((rc = dev_reserve(&ctx->t_segoff, &ctx->t_segoff_cap, segoff.size())) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->t_cur, &ctx->t_cur_cap, (size_t)r_pad * n_seg)) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->t_rq, &ctx->t_rq_cap, (size_t)n_retry * STB_D)) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->t_rthr, &ctx->t_rthr_cap, (size_t)r_pad)) != STB_OK) return rc;
+    STB_CUDA(cudaMemcpyAsync(ctx->t_segoff, segoff.data(), segoff.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->stream));
+    STB_CUDA(cudaMemsetAsync(ctx->t_cur, 0, (size_t)r_pad * n_seg * sizeof(uint32_t), ctx->stream));
+    STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
+    if ((rc = stb_launch_batch_thr_gather(ctx, ctx->bq_dev, thr, ctx->t_slot + n_direct, n_retry, r_pad, ctx->t_rq,
+                                          ctx->t_rthr)) != STB_OK) return rc;
+    if ((rc = stb_launch_shadow_build(ctx, ctx->t_rq, n_retry, 128, ctx->bq_tiles, ctx->err_flag)) != STB_OK) return rc;
+    if ((rc = stb_launch_batch_gemm_emit_sized(ctx, ctx->bq_tiles, r_tiles, corpus->shadow, n_tiles, corpus->n, ctx->t_rthr,
+                                               ctx->t_cur, A, ctx->t_segoff)) != STB_OK) return rc;
+  }
+  // exact finish: rows ascending -> canonical re-score, d < M -> stable sort by distance = (distance, row) order
+  if ((rc = stb_batch_thr_sort_rows(ctx, ctx->t_sort_tmp, sort_bytes, K, n_slots, ctx->t_off, A, B)) != STB_OK) return rc;
+  if ((rc = stb_launch_batch_thr_rescore(ctx, B, ctx->t_off, ctx->t_slot, n_slots, ctx->bq_dev, corpus->rows,
+                                         corpus->row_base, max_distance, C, D, ctx->t_slot + n_slots)) != STB_OK) return rc;
+  if ((rc = stb_batch_thr_sort_dist(ctx, ctx->t_sort_tmp, sort_bytes, K, n_slots, ctx->t_off, C, A, D, B)) != STB_OK) return rc;
+  STB_CUDA(cudaMemcpyAsync(out->pass.data(), ctx->t_slot + n_slots, n_slots * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  STB_CUDA(cudaStreamSynchronize(ctx->stream));
+  return STB_OK;
+}
+
+extern "C" {
+
+// Threshold mode of search_documents for a batch (route 5).  Chunks of STB_THR_CHUNK queries run the tensor-core
+// pipeline (thr_chunk_run); K1 (stb_search) answers the queries it leaves, and each chunk's hits are laid out
+// once all its counts are known: a chunk's output is one contiguous stretch of the concatenation.
+int stb_search_batch_threshold(stb_ctx *ctx, const stb_corpus *corpus_c, const float *q, uint32_t nq, double max_distance,
+                               stb_hit *out_hits, uint64_t cap, uint64_t *out_offsets) {
+  int rc = ctx_use(ctx);
+  if (rc) return rc;
+  stb_corpus *corpus = const_cast<stb_corpus *>(corpus_c);
+  if (!corpus) { stb_set_error("search_batch_threshold: null corpus"); return STB_ERR_ARG; }
+  if (corpus->ctx != ctx) { stb_set_error("search_batch_threshold: corpus belongs to another context"); return STB_ERR_ARG; }
+  if (nq == 0) return STB_OK;
+  if (!q || !out_offsets || (cap && !out_hits)) { stb_set_error("search_batch_threshold: null argument"); return STB_ERR_ARG; }
+  uint32_t last[6] = {5u, nq, 0u, 0u, 0u, 0u};
+  memcpy(ctx->b_last, last, sizeof(last));
+  for (uint32_t i = 0; i <= nq; ++i) out_offsets[i] = 0;
+  if (corpus->n == 0 || !(max_distance > 0.0)) return STB_OK;      // NaN or <= 0: no distance is below it
+  rc = corpus_ensure_shadow(ctx, corpus);
+  const bool tensor_ok = rc == STB_OK;
+  if (rc != STB_OK && rc != STB_ERR_STATE) return rc;                // STB_ERR_STATE: rows K2 cannot normalise, all K1
+  const uint32_t n_seg = tensor_ok ? stb_batch_emit_grid(ctx, (uint32_t)((corpus->n + 255) / 256)) : 0u;
+  const size_t nq_pad = ((size_t)nq + 127) / 128 * 128;
+  if (tensor_ok) {
+    if ((rc = dev_reserve(&ctx->b_thr, &ctx->b_thr_cap, nq_pad)) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->b_cnt, &ctx->b_cnt_cap, nq_pad * n_seg)) != STB_OK) return rc;
+  }
+  const float t = thr_emission_value(max_distance);
+  std::unique_ptr<stb_hit[]> k1_buf;                                 // one K1 result: at most every row
+  uint32_t retried = 0, k1_total = 0;
+  for (uint32_t c0 = 0; c0 < nq; c0 += STB_THR_CHUNK) {
+    const uint32_t n = std::min(STB_THR_CHUNK, nq - c0);
+    ThrChunk ch;
+    if (tensor_ok) {
+      if ((rc = thr_chunk_run(ctx, corpus, q + (size_t)c0 * STB_D, c0, n, max_distance, t, &ch)) != STB_OK) return rc;
+    } else {
+      for (uint32_t i = 0; i < n; ++i) ch.k1.push_back(i);
+    }
+    retried += ch.retried;
+    k1_total += (uint32_t)ch.k1.size();
+    std::vector<uint64_t> count(n, 0);
+    for (size_t s = 0; s < ch.slot_query.size(); ++s) count[ch.slot_query[s]] = ch.pass[s];
+    std::vector<std::vector<stb_hit>> k1_hits(ch.k1.size());
+    for (size_t j = 0; j < ch.k1.size(); ++j) {
+      if (!k1_buf) k1_buf.reset(new (std::nothrow) stb_hit[corpus->n]);
+      if (!k1_buf) { stb_set_error("search_batch_threshold: host allocation failed"); return STB_ERR_NOMEM; }
+      ctx->fallback_searches++;
+      uint64_t m = 0;
+      if ((rc = stb_search(ctx, corpus, q + (size_t)(c0 + ch.k1[j]) * STB_D, 0, 1, max_distance, STB_MODE_SEARCH_DOCUMENTS,
+                           nullptr, 0, k1_buf.get(), corpus->n, &m)) != STB_OK) return rc;
+      k1_hits[j].assign(k1_buf.get(), k1_buf.get() + m);
+      count[ch.k1[j]] = m;
+    }
+    for (uint32_t i = 0; i < n; ++i) out_offsets[c0 + i + 1] = out_offsets[c0 + i] + count[i];
+    const uint64_t base = out_offsets[c0], total = out_offsets[c0 + n] - base;
+    const uint64_t n_copy = base < cap ? std::min(total, cap - base) : 0;
+    if (n_copy && !ch.slot_query.empty()) {
+      // the tensor-answered queries' hits at their place in this chunk's stretch (K1's are filled in below)
+      const uint32_t n_slots = (uint32_t)ch.slot_query.size();
+      const int K = ch.off[n_slots];
+      std::vector<uint64_t> out_at(n_slots);
+      for (uint32_t s = 0; s < n_slots; ++s) out_at[s] = out_offsets[c0 + ch.slot_query[s]] - base;
+      if ((rc = dev_reserve(&ctx->t_out_at, &ctx->t_out_at_cap, (size_t)n_slots)) != STB_OK) return rc;
+      if ((rc = dev_reserve(&ctx->t_hits, &ctx->t_hits_cap, std::max<size_t>(total, 1))) != STB_OK) return rc;
+      STB_CUDA(cudaMemcpyAsync(ctx->t_out_at, out_at.data(), n_slots * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->stream));
+      if ((rc = stb_launch_batch_thr_write(ctx, ctx->t_buf, ctx->t_buf + K, ctx->t_off, ctx->t_slot + n_slots, n_slots,
+                                           ctx->t_out_at, ctx->t_hits)) != STB_OK) return rc;
+      STB_CUDA(cudaMemcpyAsync(out_hits + base, ctx->t_hits, n_copy * sizeof(stb_hit), cudaMemcpyDeviceToHost, ctx->stream));
+      STB_CUDA(cudaStreamSynchronize(ctx->stream));
+    }
+    for (size_t j = 0; j < ch.k1.size(); ++j) {
+      const uint64_t o = out_offsets[c0 + ch.k1[j]];
+      if (o < cap) memcpy(out_hits + o, k1_hits[j].data(), std::min<uint64_t>(k1_hits[j].size(), cap - o) * sizeof(stb_hit));
+    }
+  }
+  const uint32_t done[6] = {5u, nq, retried, k1_total, n_seg, tensor_ok ? STB_THR_SEG_CAP : 0u};
+  memcpy(ctx->b_last, done, sizeof(done));
+  if (out_offsets[nq] > cap) {
+    stb_set_error("search_batch_threshold: %llu hits, capacity %llu", (unsigned long long)out_offsets[nq], (unsigned long long)cap);
+    return STB_ERR_CAPACITY;
+  }
+  return STB_OK;
+}
+
 // Sharded K2: every rank answers the nq queries on its shard (stb_search_batch_dev), then ONE exchange over
 // NVLink peer memory -- each rank stores its nq x k hits + per-query proof flags into every peer's batch slot
 // (push kernel), waits for all peers' sequence flags and merges per query (merge kernel).  Two launches, no
@@ -1502,7 +1723,7 @@ int stb_debug_batch_last(stb_ctx *ctx, uint32_t info[6], float *thr, uint32_t *c
   STB_CUDA(cudaStreamSynchronize(ctx->stream));
   memcpy(info, ctx->b_last, sizeof(ctx->b_last));
   const uint32_t nq = ctx->b_last[1], n_seg = ctx->b_last[4];
-  if ((ctx->b_last[0] == 2u || ctx->b_last[0] == 3u) && nq) {
+  if ((ctx->b_last[0] == 2u || ctx->b_last[0] == 3u || (ctx->b_last[0] == 5u && n_seg)) && nq) {
     if (thr) STB_CUDA(cudaMemcpy(thr, ctx->b_thr, (size_t)nq * sizeof(float), cudaMemcpyDeviceToHost));
     if (cand_cnt) STB_CUDA(cudaMemcpy(cand_cnt, ctx->b_cnt, (size_t)nq * n_seg * sizeof(uint32_t), cudaMemcpyDeviceToHost));
   }

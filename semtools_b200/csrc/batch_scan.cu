@@ -196,6 +196,9 @@ struct GemmArgs {
   // FILTER (stb_search_batch_filtered): tile t of the launch is shadow tile tile_ids[t * tile_stride]
   const uint32_t *tile_ids;   // listed tiles: the shadow tiles holding an eligible row, ascending
   const uint32_t *bitmap;     // eligible local rows, 1 bit each: 8 words per shadow tile
+  // EPI == 2 (stb_search_batch_threshold's re-emission): segment (q, CTA) is cand_keys[seg_off[q * grid + CTA],
+  // seg_off[q * grid + CTA + 1]), sized by the first pass's exact counts; cand_cnt holds the cursors
+  const uint64_t *seg_off;    // [q_pad * grid + 1]
 };
 
 // warpgroup 0: bulk-copy producer (one thread); warpgroups 1 and 2: wgmma + epilogue, each on
@@ -206,6 +209,7 @@ struct GemmArgs {
 
 // EPI 0: per-sub-tile / per-tile maxima (pipeline v1, and the sampling pass of v2).
 // EPI 1: emit every (query,row) whose approximate score reaches the query's threshold.
+// EPI 2: the same emission into exactly sized segments at args.seg_off (unfiltered only).
 // FILTER: the CTAs walk the listed tiles (args.tile_ids) and only eligible rows count (args.bitmap): EPI 0
 // takes each tile maximum over its eligible rows, EPI 1 emits eligible rows only.  The tile's 8 bitmap words
 // arrive with its first corpus slab, double-buffered behind the mbarriers.
@@ -302,12 +306,19 @@ stb_batch_gemm_kernel(const GemmArgs args) {
       const uint32_t q0 = m * STB_A_TILE + qrow;
       [[maybe_unused]] float thr[2];
       [[maybe_unused]] uint32_t cnt[2], cnt0[2];
-      if constexpr (EPI == 1) {       // epilogue state, fetched while the MMAs run
+      [[maybe_unused]] uint64_t seg_base[2];
+      [[maybe_unused]] uint32_t seg_len[2];
+      if constexpr (EPI >= 1) {       // epilogue state, fetched while the MMAs run
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           thr[h] = __ldg(args.thr + q0 + 8 * h);
           cnt0[h] = args.cand_cnt[(size_t)(q0 + 8 * h) * gridDim.x + blockIdx.x];
           cnt[h] = cnt0[h];
+          if constexpr (EPI == 2) {
+            const uint64_t *so = args.seg_off + (size_t)(q0 + 8 * h) * gridDim.x + blockIdx.x;
+            seg_base[h] = __ldg(so);
+            seg_len[h] = (uint32_t)(__ldg(so + 1) - seg_base[h]);
+          }
         }
       }
       wg_reg_fence(d);
@@ -412,7 +423,15 @@ stb_batch_gemm_kernel(const GemmArgs args) {
             hit |= __shfl_xor_sync(0xffffffffu, hit, 2);
             if (row0 + 32 > args.n_rows) hit &= (row0 < args.n_rows) ? ((1u << (uint32_t)(args.n_rows - row0)) - 1u) : 0u;   // padding rows
             if constexpr (FILTER) hit &= mw;                                                                                    // ineligible rows
-            uint64_t *seg = args.cand_keys + ((size_t)(q0 + 8 * h) * gridDim.x + blockIdx.x) * args.cand_cap;
+            uint64_t *seg;
+            uint32_t seg_cap;
+            if constexpr (EPI == 2) {
+              seg = args.cand_keys + seg_base[h];
+              seg_cap = seg_len[h];
+            } else {
+              seg = args.cand_keys + ((size_t)(q0 + 8 * h) * gridDim.x + blockIdx.x) * args.cand_cap;
+              seg_cap = args.cand_cap;
+            }
 #pragma unroll
             for (int ii = 0; ii < 4; ++ii)
 #pragma unroll
@@ -420,7 +439,7 @@ stb_batch_gemm_kernel(const GemmArgs args) {
                 const uint32_t b = ii * 8 + quad * 2 + e;
                 const uint32_t pos = cnt[h] + __popc(hit & ((1u << b) - 1u));
                 const uint64_t key = stb_make_key(d[16 * c + 4 * ii + 2 * h + e], (uint32_t)(row0 + b));
-                if (((hit >> b) & 1u) && pos < args.cand_cap) seg[pos] = key;
+                if (((hit >> b) & 1u) && pos < seg_cap) seg[pos] = key;
               }
             cnt[h] += __popc(hit);                       // > cand_cap = overflow marker
           }
@@ -456,7 +475,8 @@ int stb_launch_shadow_build(stb_ctx *ctx, const float *rows_dev, uint64_t n_rows
 
 template <int EPI, bool FILTER = false>
 static int launch_gemm(stb_ctx *ctx, const GemmArgs &a) {
-  const int attr = FILTER ? (EPI == 0 ? STB_ATTR_GEMM0F : STB_ATTR_GEMM1F) : (EPI == 0 ? STB_ATTR_GEMM0 : STB_ATTR_GEMM1);
+  const int attr = FILTER ? (EPI == 0 ? STB_ATTR_GEMM0F : STB_ATTR_GEMM1F)
+                          : (EPI == 0 ? STB_ATTR_GEMM0 : (EPI == 1 ? STB_ATTR_GEMM1 : STB_ATTR_GEMM2));
   STB_ATTR_ONCE(ctx, attr,
                 cudaFuncSetAttribute(stb_batch_gemm_kernel<EPI, FILTER>, cudaFuncAttributeMaxDynamicSharedMemorySize, STB_GEMM_SMEM));
   unsigned grid = (unsigned)std::min<uint32_t>(a.n_tiles, (uint32_t)ctx->sm_count);
@@ -511,6 +531,17 @@ int stb_launch_batch_gemm_emit_filtered(stb_ctx *ctx, const uint8_t *a_tiles, ui
   a.thr = thr; a.cand_cnt = cand_cnt; a.cand_keys = cand_keys; a.cand_cap = cand_cap; a.n_rows = n_rows;
   a.tile_ids = tile_ids; a.bitmap = bitmap;
   return launch_gemm<1, true>(ctx, a);
+}
+
+// Threshold mode's re-emission: the candidate-emitting pass over all tiles into the exactly sized segments
+// seg_off[] of cand_keys; cursors [q_pad][grid] zeroed by the caller
+int stb_launch_batch_gemm_emit_sized(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_tiles, const uint8_t *b_tiles,
+                                     uint32_t n_tiles, uint64_t n_rows, const float *thr, uint32_t *cursors,
+                                     uint64_t *cand_keys, const uint64_t *seg_off) {
+  GemmArgs a{};
+  a.a_tiles = a_tiles; a.b_tiles = b_tiles; a.m_tiles = m_tiles; a.n_tiles = n_tiles; a.tile_stride = 1;
+  a.thr = thr; a.cand_cnt = cursors; a.cand_keys = cand_keys; a.n_rows = n_rows; a.seg_off = seg_off;
+  return launch_gemm<2>(ctx, a);
 }
 
 
@@ -977,3 +1008,4 @@ int stb_launch_batch_finish2(stb_ctx *ctx, const uint64_t *cand_keys, const uint
   ctx->kernel_launches++;
   return STB_OK;
 }
+

@@ -130,8 +130,24 @@ struct stb_ctx {
   uint32_t *b_franges; size_t b_franges_cap;
   uint32_t *b_ftiles; size_t b_ftiles_cap;
   uint32_t *b_fbits; size_t b_fbits_cap;
-  // the last K2 call: route (1 = v1, 2 = v2, 3 = filtered v2, 4 = filtered, nothing on the tensor cores), nq,
-  // n_sample, stride, n_seg, seg_cap
+  // stb_search_batch_threshold (per chunk of queries): per-(query, segment) destinations of the first pass's
+  // keys, the re-emission's segment offsets, cursors, queries and thresholds, the compact candidates and their
+  // sort buffers (4 x u64 per candidate), per-slot offsets / query / pass count / output position, the hits
+  // in output order and the sorts' scratch
+  uint64_t *t_dst; size_t t_dst_cap;
+  uint64_t *t_segoff; size_t t_segoff_cap;
+  uint32_t *t_cur; size_t t_cur_cap;
+  float *t_rq; size_t t_rq_cap;
+  float *t_rthr; size_t t_rthr_cap;
+  uint64_t *t_buf; size_t t_buf_cap;
+  int *t_off; size_t t_off_cap;
+  uint32_t *t_slot; size_t t_slot_cap;       // [2][slots]: query of each slot, then its pass count
+  uint64_t *t_out_at; size_t t_out_at_cap;
+  stb_hit *t_hits; size_t t_hits_cap;
+  uint8_t *t_sort_tmp; size_t t_sort_tmp_cap;
+  // the last K2 call: route (1 = v1, 2 = v2, 3 = filtered v2, 4 = filtered, nothing on the tensor cores,
+  // 5 = threshold mode), nq, then n_sample, stride (routes 1-4) or retried queries, K1 queries (route 5), n_seg,
+  // seg_cap
   uint32_t b_last[6];
   float *bq_dev; size_t bq_dev_cap;           // host-call staging: queries
   stb_hit *bh_dev; size_t bh_dev_cap;         // host-call staging: hits
@@ -348,7 +364,7 @@ int stb_launch_batch_xchg(stb_ctx *ctx, const StbBatchXchgArgs &a, const stb_hit
 
 // opt-in to > 48 KiB dynamic shared memory (or another function attribute) once per context
 enum { STB_ATTR_GEMM0 = 0, STB_ATTR_GEMM1, STB_ATTR_MERGE, STB_ATTR_IVF_PROBE, STB_ATTR_IVF_V2, STB_ATTR_FINISH2,
-       STB_ATTR_IVF_BATCH, STB_ATTR_GEMM0F, STB_ATTR_GEMM1F };
+       STB_ATTR_IVF_BATCH, STB_ATTR_GEMM0F, STB_ATTR_GEMM1F, STB_ATTR_GEMM2 };
 #define STB_ATTR_ONCE(ctx, bit, call)                         \
   do {                                                        \
     if (!((ctx)->func_attr_mask & (1u << (bit)))) {           \
@@ -396,6 +412,37 @@ int stb_launch_batch_finish2(stb_ctx *ctx, const uint64_t *cand_keys, const uint
                              uint64_t n_rows, uint64_t row_base, const float *queries_dev,
                              const uint32_t *q_bad, stb_hit *out_hits, uint32_t *out_status);
 void stb_batch_build_params(int *shadow_is_f16, double *eps);
+// threshold mode's re-emission: the emitting pass into exactly sized segments cand_keys[seg_off[i], seg_off[i+1])
+// (i = query * grid + CTA), cursors [q_pad][grid] zeroed
+int stb_launch_batch_gemm_emit_sized(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_tiles,
+                                     const uint8_t *b_tiles, uint32_t n_tiles, uint64_t n_rows,
+                                     const float *thr, uint32_t *cursors, uint64_t *cand_keys,
+                                     const uint64_t *seg_off);
+
+// ---- batch_threshold.cu (K2 threshold mode) -------------------------------------------------------
+// thr[i] = t for the queries i < nq that are non-zero and normalisable, +inf for the others and the padding
+int stb_launch_batch_thr_dist(stb_ctx *ctx, const float *q_dev, const uint32_t *q_bad, uint32_t nq, uint32_t q_pad,
+                              float t, float *thr);
+// segment i of the first pass (cnt[i] keys at keys + i * seg_cap) -> out[dst[i] ..]; dst[i] = ~0: skipped
+int stb_launch_batch_thr_compact(stb_ctx *ctx, const uint64_t *keys, const uint32_t *cnt, const uint64_t *dst,
+                                 uint64_t n_pairs, uint32_t seg_cap, uint64_t *out);
+// slot r < n: query src[idx[r]] and thr_src[idx[r]]; slots [n, r_pad): thr +inf
+int stb_launch_batch_thr_gather(stb_ctx *ctx, const float *src, const float *thr_src, const uint32_t *idx, uint32_t n,
+                                uint32_t r_pad, float *dst, float *thr_dst);
+// slot s: keys [off[s], off[s+1]) re-scored against query qidx[s]: (distance bits, global row), or (+inf, ~0)
+// when not d < limit; pass[s] = rows kept
+int stb_launch_batch_thr_rescore(stb_ctx *ctx, const uint64_t *keys, const int *off, const uint32_t *qidx,
+                                 uint32_t n_slots, const float *queries_dev, const float *rows, uint64_t row_base,
+                                 double limit, uint64_t *dist_bits, uint64_t *grow, uint32_t *pass);
+// slot s: its first pass[s] sorted pairs -> out[dst[s] ..]
+int stb_launch_batch_thr_write(stb_ctx *ctx, const uint64_t *dist_bits, const uint64_t *grow, const int *off,
+                               const uint32_t *pass, uint32_t n_slots, const uint64_t *dst, stb_hit *out);
+// segmented sorts over the slots: keys by row (low 32 bits); (distance bits, row) pairs stably by distance
+int stb_batch_thr_sort_bytes(stb_ctx *ctx, int n_items, uint32_t n_slots, const int *off, size_t *bytes);
+int stb_batch_thr_sort_rows(stb_ctx *ctx, void *tmp, size_t tmp_bytes, int n_items, uint32_t n_slots, const int *off,
+                            const uint64_t *keys_in, uint64_t *keys_out);
+int stb_batch_thr_sort_dist(stb_ctx *ctx, void *tmp, size_t tmp_bytes, int n_items, uint32_t n_slots, const int *off,
+                            const uint64_t *dist_bits, uint64_t *dist_out, const uint64_t *grow, uint64_t *grow_out);
 int stb_launch_batch_select(stb_ctx *ctx, const float *submax, uint32_t n_sub, uint32_t q_pad,
                             uint32_t n_slices, uint64_t *cand);
 int stb_launch_batch_finish(stb_ctx *ctx, const uint64_t *cand, uint32_t n_slices, uint32_t n_sub,

@@ -107,6 +107,10 @@ class Searcher:
     def search_documents(self, query_embedding, config: SearchConfig):
         hits = self.corpus.search(query_embedding, config.top_k, config.max_distance,
                                   capi.STB_MODE_SEARCH_DOCUMENTS)
+        return self._results(hits, config)
+
+    def _results(self, hits, config: SearchConfig):
+        """SearchResults with their context windows (:88-119) for hits ordered by (distance, row)."""
         out = []
         for h in hits:
             doc, idx = self._locate(int(h["row"]))
@@ -115,6 +119,15 @@ class Searcher:
             out.append(SearchResult(doc.filename, doc.lines[start:end], start, end, idx,
                                     float(h["distance"])))
         return out
+
+    # -- search_documents for a batch of queries: element i equals search_documents(query_embeddings[i], config)
+    def search_documents_batch(self, query_embeddings, config: SearchConfig):
+        q = np.ascontiguousarray(query_embeddings, dtype=np.float32).reshape(-1, capi.STB_DIM)
+        if config.max_distance is None:
+            hits = self.corpus.search_batch(q, config.top_k)
+        else:
+            hits = self.corpus.search_batch_threshold(q, config.max_distance)
+        return [self._results(h, config) for h in hits]
 
     # -- Store::search_line_embeddings (src/workspace/store.rs:481-546)
     def search_line_embeddings(self, query_vec, subset_paths, top_k: int, max_distance=None):
