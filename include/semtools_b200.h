@@ -101,6 +101,53 @@ int stb_table_destroy(stb_table *table);
  * (non-zero when this context holds one row-shard of a larger corpus). */
 int stb_corpus_create(stb_ctx *ctx, uint32_t D, uint64_t capacity_rows,
                       uint64_t row_base, stb_corpus **out);
+/* A corpus larger than HBM: its f32 rows live in page-locked, device-mapped host memory that the library
+ * allocates and owns, and only the q8 copy (396 B per row) lives in HBM, so one 80 GB card holds ~190M rows
+ * instead of ~50M.  It returns an ordinary stb_corpus handle; the hits of every search are bit for bit those
+ * of a device corpus holding the same rows, because every route ends in the same canonical re-rank, which
+ * reads the candidate rows over the host link.  Only the route differs.
+ *  - The q8 copy is always current.  Creation allocates the host rows and the q8 copy for capacity_rows;
+ *    STB_ERR_NOMEM if either fails, and nothing is created.  stb_corpus_append, stb_corpus_append_dev,
+ *    stb_embed with append_to, stb_corpus_update and stb_corpus_remove encode the rows they add or write into
+ *    the q8 copy from HBM in the same call: there is no lazy build.  Its bytes are those stb_corpus_prepare
+ *    (STB_PREPARE_Q8) writes on a device corpus holding the same rows; a row that cannot be normalised marks it
+ *    unusable as on a device corpus (stb_corpus_tier_stats: built_rows[q8] = 0), and searches then use the f32
+ *    passes.  An update or removal on a corpus whose copy is unusable re-encodes the whole copy from the rows.
+ *  - Appending.  stb_corpus_append uploads each row once, into the context's staging buffer (chunks of at most
+ *    262144 rows, 256 MiB of HBM, the buffer stb_corpus_update uses); one kernel writes the chunk to the host
+ *    rows and encodes its q8 entries.  stb_corpus_append_dev does the same from the caller's device rows, and
+ *    stb_embed with append_to lets K3 write chunks of lines into the staging buffer.  A call that fails appends
+ *    nothing.  Growing past the capacity allocates new host rows and a new q8 copy and then frees the old ones:
+ *    while it runs the corpus holds two host buffers (1 KiB per row each).
+ *  - stb_corpus_update / stb_corpus_remove: arguments, validation, atomicity, epochs, the tier statistics and
+ *    the end of a co-scan series are the device corpus's.  The kernels write the host rows in place through the
+ *    mapped pointer; neither holds a second copy of the rows.  Their cost is the host link's: an update moves
+ *    each written row up once and down once (~2 KiB per row); a removal reads and writes every row behind the
+ *    first removed one over the link (~2 KiB per moved row).  Measured on an H100 80GB HBM3 at 700 W with 10M
+ *    rows: an update of 10000 rows 2.9 ms (device corpus 2.1 ms); a removal of 10000 rows at the middle, which
+ *    moves 5M rows, 673 ms (device corpus 9.3 ms).
+ *  - stb_search never streams the f32 rows while an HBM copy can answer: top_k <= 16 without a threshold takes
+ *    the q8 top-k scan; a result it cannot prove, and any top_k <= 96, next takes the 16-bit top-k scan if the
+ *    shadow exists (stb_corpus_prepare(STB_PREPARE_H16) or K2 built it; it is never built lazily here), and
+ *    otherwise the q8 histogram -> q8 collect -> proof route that top_k > 96 and threshold mode take.  The f32
+ *    passes, which stream the rows over the host link, run only when that route cannot prove its result or the
+ *    q8 copy is unusable; stb_ctx_counters' fallback count counts those searches, and stb_corpus_tier_stats
+ *    shows no f32 top-k scan.
+ *  - stb_search_topk_dev and stb_search_many (without an exchange) read the q8 copy (top_k <= 16) or the
+ *    16-bit shadow if it is built; otherwise they return STB_ERR_STATE and launch nothing.
+ *  - K2 (stb_search_batch, _dev, _filtered, _threshold) works as on a device corpus: the shadow (512 B per row
+ *    of HBM; STB_ERR_NOMEM when it does not fit) is built from the host rows through the staging buffer, and
+ *    the re-scores and the K1 fallback read the host rows.
+ *  - Refused with STB_ERR_STATE, nothing changed: stb_corpus_data_dev (there is no device matrix to hand to a
+ *    zero-copy producer), stb_ivfpq_build, and the exchange forms (stb_search_topk_xchg, stb_search_xchg,
+ *    stb_search_batch_xchg_dev, stb_search_many with an exchange).  These are scope limits of this release,
+ *    not technical ones.
+ *  - stb_corpus_read, _clear, _rows, _prepare and destroy work as on a device corpus; the corpus may outlive
+ *    its context.
+ * Cost of the K1 re-rank over the host link, on an H100 80GB HBM3 at 700 W with 10M rows: not visible at
+ * top_k = 10 (1754 vs 1753 q/s through stb_search, within noise), so the kernels read the mapped rows as they
+ * are.  The collect routes re-rank more rows: top_k = 50 500 vs 546 q/s, threshold 814 vs 838 q/s. */
+int stb_corpus_create_host(stb_ctx *ctx, uint32_t D, uint64_t capacity_rows, uint64_t row_base, stb_corpus **out);
 int stb_corpus_destroy(stb_corpus *corpus);
 int stb_corpus_append(stb_corpus *corpus, const float *rows, uint64_t n);
 int stb_corpus_append_dev(stb_corpus *corpus, const float *rows_dev, uint64_t n);

@@ -20,7 +20,7 @@ STB_COPY_Q8_CODES, STB_COPY_Q8_SCALES, STB_COPY_Q8_PLANE, STB_COPY_Q8_SR, STB_CO
 # every symbol include/semtools_b200.h declares (tests check the .so exports all)
 SYMBOLS = [
     "stb_version", "stb_last_error", "stb_device_count", "stb_ctx_create", "stb_ctx_destroy",
-    "stb_ctx_sync", "stb_ctx_stream", "stb_table_load", "stb_table_destroy", "stb_corpus_create",
+    "stb_ctx_sync", "stb_ctx_stream", "stb_table_load", "stb_table_destroy", "stb_corpus_create", "stb_corpus_create_host",
     "stb_corpus_destroy", "stb_corpus_append", "stb_corpus_append_dev", "stb_corpus_clear",
     "stb_corpus_rows", "stb_corpus_data_dev", "stb_corpus_read", "stb_corpus_update", "stb_corpus_remove", "stb_embed", "stb_embed_dev",
     "stb_embed_status", "stb_search",
@@ -76,6 +76,7 @@ def lib() -> C.CDLL:
     L.stb_table_load.argtypes = [vp, vp, u64, u32, vp, u64, vp, u64, i32, C.POINTER(vp)]
     L.stb_table_destroy.argtypes = [vp]
     L.stb_corpus_create.argtypes = [vp, u32, u64, u64, C.POINTER(vp)]
+    L.stb_corpus_create_host.argtypes = [vp, u32, u64, u64, C.POINTER(vp)]
     L.stb_corpus_destroy.argtypes = [vp]
     L.stb_corpus_append.argtypes = [vp, vp, u64]
     L.stb_corpus_append_dev.argtypes = [vp, vp, u64]
@@ -288,12 +289,23 @@ class Table:
 
 class Corpus:
     """stb_corpus: contiguous N x 256 f32 line-vector matrix in HBM."""
+    host_rows = False
 
     def __init__(self, ctx: Context, capacity_rows: int = 1024, row_base: int = 0):
         self.ctx = ctx
         self.row_base = row_base
         self._h = vp()
         _check(lib().stb_corpus_create(ctx._h, STB_DIM, capacity_rows, row_base, C.byref(self._h)))
+
+    @classmethod
+    def in_host_memory(cls, ctx: Context, capacity_rows: int = 1024, row_base: int = 0) -> "Corpus":
+        """stb_corpus_create_host: the f32 rows in page-locked host memory, only the q8 copy in HBM (a corpus
+        larger than the card's memory; the same hits as a device corpus, see the header for the routes)."""
+        self = cls.__new__(cls)
+        self.ctx, self.row_base, self.host_rows = ctx, row_base, True
+        self._h = vp()
+        _check(lib().stb_corpus_create_host(ctx._h, STB_DIM, capacity_rows, row_base, C.byref(self._h)))
+        return self
 
     def close(self):
         if getattr(self, "_h", None) is not None and self._h and _lib is not None:

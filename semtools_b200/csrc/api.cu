@@ -298,10 +298,65 @@ int stb_table_destroy(stb_table *t) {
 }
 
 // -------------------------------------------------------------------- corpus ---
+// q8 copy of `cap` rows (int8 codes + scales, 260 B/row, and the top-k prefilter's nibble plane + {s, rho},
+// 136 B/row) with the first `keep` rows of the current one; nothing changes when an allocation fails.
+static int q8_realloc(stb_corpus *c, uint64_t cap, uint64_t keep) {
+  stb_ctx *ctx = c->ctx;
+  uint8_t *np = nullptr, *pp = nullptr;
+  float *ns = nullptr;
+  float2 *sp = nullptr;
+  cudaError_t e = cudaMalloc((void **)&np, cap * 256ull);
+  if (e == cudaSuccess) e = cudaMalloc((void **)&ns, cap * sizeof(float));
+  if (e == cudaSuccess) e = cudaMalloc((void **)&pp, stb_q4_plane_bytes(cap));
+  if (e == cudaSuccess) e = cudaMalloc((void **)&sp, cap * sizeof(float2));
+  if (e != cudaSuccess) {
+    cudaGetLastError(); cudaFree(np); cudaFree(ns); cudaFree(pp);
+    stb_set_error("q8 tier: cannot allocate %llu MiB", (unsigned long long)(cap * 396 >> 20));
+    return STB_ERR_NOMEM;
+  }
+  if (c->q8 && keep) {
+    STB_CUDA(cudaMemcpyAsync(np, c->q8, keep * 256ull, cudaMemcpyDeviceToDevice, ctx->stream));
+    STB_CUDA(cudaMemcpyAsync(ns, c->q8_scale, keep * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
+    STB_CUDA(cudaMemcpyAsync(pp, c->q4, stb_q4_plane_bytes(keep), cudaMemcpyDeviceToDevice, ctx->stream));   // whole tiles
+    STB_CUDA(cudaMemcpyAsync(sp, c->q4_sr, keep * sizeof(float2), cudaMemcpyDeviceToDevice, ctx->stream));
+    STB_CUDA(cudaStreamSynchronize(ctx->stream));
+  }
+  cudaFree(c->q8); cudaFree(c->q8_scale); cudaFree(c->q4); cudaFree(c->q4_sr);
+  c->q8 = np; c->q8_scale = ns; c->q4 = pp; c->q4_sr = sp; c->q8_cap_rows = cap;
+  return STB_OK;
+}
+
+// A host-rows corpus grows both halves together: new pinned rows and a new q8 copy, then the old ones are
+// copied and freed (so growing briefly holds two host buffers).  A failed allocation changes nothing.
+static int host_corpus_reserve(stb_corpus *c, uint64_t ncap) {
+  stb_ctx *ctx = c->ctx;
+  float *hp = nullptr, *dp = nullptr;
+  cudaError_t e = cudaHostAlloc((void **)&hp, ncap * STB_D * sizeof(float), cudaHostAllocMapped | cudaHostAllocPortable);
+  if (e == cudaSuccess) e = cudaHostGetDevicePointer((void **)&dp, hp, 0);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    if (hp) cudaFreeHost(hp);
+    stb_set_error("corpus: cannot allocate %llu rows of page-locked host memory: %s", (unsigned long long)ncap, cudaGetErrorString(e));
+    return STB_ERR_NOMEM;
+  }
+  int rc = q8_realloc(c, ncap, c->n);
+  if (rc != STB_OK) { cudaFreeHost(hp); return rc; }
+  STB_CUDA(cudaStreamSynchronize(ctx->stream));   // kernels write the rows (update, remove)
+  if (c->rows_host) {
+    memcpy(hp, c->rows_host, c->n * STB_D * sizeof(float));
+    cudaFreeHost(c->rows_host);
+  }
+  c->rows_host = hp;
+  c->rows = dp;
+  c->capacity = ncap;
+  return STB_OK;
+}
+
 static int corpus_reserve(stb_corpus *c, uint64_t need) {
   if (need <= c->capacity && c->rows) return STB_OK;
   if (need > 0xfffffffeull) { stb_set_error("corpus shard exceeds 2^32-2 rows; shard it"); return STB_ERR_ARG; }
   uint64_t ncap = std::max<uint64_t>(std::max<uint64_t>(need, 1024), c->capacity + c->capacity / 2);
+  if (c->host_rows) return host_corpus_reserve(c, ncap);
   float *np = nullptr;
   cudaError_t e = cudaMalloc((void **)&np, ncap * STB_D * sizeof(float));
   if (e != cudaSuccess) {
@@ -335,6 +390,22 @@ int stb_corpus_create(stb_ctx *ctx, uint32_t D, uint64_t capacity_rows, uint64_t
   return STB_OK;
 }
 
+int stb_corpus_create_host(stb_ctx *ctx, uint32_t D, uint64_t capacity_rows, uint64_t row_base, stb_corpus **out) {
+  int rc = ctx_use(ctx);
+  if (rc) return rc;
+  if (!out) { stb_set_error("out is null"); return STB_ERR_ARG; }
+  if (D != STB_D) { stb_set_error("corpus_create_host: D=%u, only %u supported", D, STB_D); return STB_ERR_ARG; }
+  if (capacity_rows > 0xfffffffeull) { stb_set_error("corpus shard exceeds 2^32-2 rows; shard it"); return STB_ERR_ARG; }
+  stb_corpus *c = new (std::nothrow) stb_corpus();
+  if (!c) { stb_set_error("out of host memory"); return STB_ERR_NOMEM; }
+  memset(c, 0, sizeof(*c));
+  c->ctx = ctx; c->row_base = row_base; c->host_rows = 1;
+  rc = host_corpus_reserve(c, std::max<uint64_t>(capacity_rows, 1));
+  if (rc) { delete c; return rc; }
+  *out = c;
+  return STB_OK;
+}
+
 int stb_corpus_destroy(stb_corpus *c) {
   if (!c) return STB_OK;
   if (c->ctx && ctx_alive(c->ctx)) { cudaSetDevice(c->ctx->device); cudaStreamSynchronize(c->ctx->stream); }
@@ -344,7 +415,8 @@ int stb_corpus_destroy(stb_corpus *c) {
   cudaFree(c->q8_scale);
   cudaFree(c->q4);
   cudaFree(c->q4_sr);
-  cudaFree(c->rows);
+  if (c->host_rows) cudaFreeHost(c->rows_host);
+  else cudaFree(c->rows);
   cudaGetLastError();
   delete c;
   return STB_OK;
@@ -357,12 +429,45 @@ int stb_corpus_destroy(stb_corpus *c) {
 // the corpus (the next asynchronous top-k query starts at tile 0).
 enum CorpusChange { CORPUS_APPEND, CORPUS_ROWS_REWRITTEN, CORPUS_CLEAR };
 static void corpus_changed(stb_corpus *c, CorpusChange kind) {
-  if (kind == CORPUS_CLEAR) { c->shadow_rows = 0; c->q8_rows = 0; }
+  if (kind == CORPUS_CLEAR) { c->shadow_rows = 0; c->q8_rows = 0; c->shadow_bad = 0; c->q8_bad = 0; }
   if (kind != CORPUS_APPEND) ++c->epoch;
   if (kind == CORPUS_ROWS_REWRITTEN && c->ctx->coscan_prev.rows == c->rows) c->ctx->coscan_prev.rows = nullptr;
   c->searches_since_change = 0;
   memset(c->tier_tries, 0, sizeof(c->tier_tries));
   memset(c->tier_proven, 0, sizeof(c->tier_proven));
+}
+
+static StbCorpusWriteArgs corpus_write_args(stb_corpus *c, uint64_t q8_rows, uint64_t shadow_rows);
+
+// Appending to a host-rows corpus: staged rows [0, m) become rows first .. first + m - 1.  The commit kernel of the
+// in-place mutations writes them to the host rows and encodes their q8 entries from HBM in the same pass; the
+// 16-bit shadow stays the prefix it was.  The caller books the rows (host_append_finish) once every chunk is in.
+static int host_append_chunk(stb_corpus *c, const float *stage_dev, uint64_t first, uint64_t m) {
+  StbCorpusWriteArgs a = corpus_write_args(c, first + m, 0);
+  a.stage = reinterpret_cast<const float4 *>(stage_dev);
+  a.first = first;
+  a.m = m;
+  return stb_launch_corpus_write(c->ctx, a);
+}
+static int host_append_begin(stb_corpus *c, uint64_t n, uint64_t stage_rows) {
+  stb_ctx *ctx = c->ctx;
+  int rc;
+  if ((rc = corpus_reserve(c, c->n + n)) != STB_OK) return rc;
+  if (stage_rows && (rc = dev_reserve(&ctx->mut_stage, &ctx->mut_stage_cap, stage_rows * STB_D)) != STB_OK) return rc;
+  if ((rc = dev_reserve(&ctx->mut_flags, &ctx->mut_flags_cap, 2)) != STB_OK) return rc;
+  STB_CUDA(cudaMemsetAsync(ctx->mut_flags, 0, 2 * sizeof(int), ctx->stream));
+  return STB_OK;
+}
+// synchronises; a row of the call that cannot be normalised marks the q8 copy unusable, as a build does
+static int host_append_finish(stb_corpus *c, uint64_t n) {
+  int flags[2] = {0, 0};
+  STB_CUDA(cudaMemcpyAsync(flags, c->ctx->mut_flags, sizeof(flags), cudaMemcpyDeviceToHost, c->ctx->stream));
+  STB_CUDA(cudaStreamSynchronize(c->ctx->stream));
+  c->n += n;
+  c->q8_rows = c->n;
+  if (flags[0]) c->q8_bad = 1;
+  corpus_changed(c, CORPUS_APPEND);
+  return STB_OK;
 }
 
 static int corpus_append_impl(stb_corpus *c, const float *rows, uint64_t n, cudaMemcpyKind kind) {
@@ -371,6 +476,22 @@ static int corpus_append_impl(stb_corpus *c, const float *rows, uint64_t n, cuda
   if (rc) return rc;
   if (n == 0) return STB_OK;
   if (!rows) { stb_set_error("corpus_append: rows is null"); return STB_ERR_ARG; }
+  if (c->host_rows) {
+    // host rows: each row goes up once (through the staging buffer unless it is in HBM already)
+    const bool up = kind == cudaMemcpyHostToDevice;
+    const uint64_t chunk = std::min<uint64_t>(n, STB_MUT_CHUNK_ROWS);
+    if ((rc = host_append_begin(c, n, up ? chunk : 0)) != STB_OK) return rc;
+    for (uint64_t i0 = 0; i0 < n; i0 += chunk) {
+      const uint64_t m = std::min(chunk, n - i0);
+      const float *src = rows + i0 * STB_D;
+      if (up) {   // stream order keeps the copy behind the previous chunk's kernel
+        STB_CUDA(cudaMemcpyAsync(c->ctx->mut_stage, src, m * STB_D * sizeof(float), cudaMemcpyHostToDevice, c->ctx->stream));
+        src = c->ctx->mut_stage;
+      }
+      if ((rc = host_append_chunk(c, src, c->n + i0, m)) != STB_OK) return rc;
+    }
+    return host_append_finish(c, n);
+  }
   if ((rc = corpus_reserve(c, c->n + n)) != STB_OK) return rc;
   STB_CUDA(cudaMemcpyAsync(c->rows + c->n * STB_D, rows, n * STB_D * sizeof(float), kind, c->ctx->stream));
   STB_CUDA(cudaStreamSynchronize(c->ctx->stream));
@@ -399,6 +520,7 @@ int stb_corpus_rows(const stb_corpus *c, uint64_t *n) {
 }
 int stb_corpus_data_dev(const stb_corpus *c, float **rows_dev) {
   if (!c || !rows_dev) { stb_set_error("null argument"); return STB_ERR_ARG; }
+  if (c->host_rows) { stb_set_error("corpus_data_dev: the rows of this corpus are in host memory; there is no device matrix"); return STB_ERR_STATE; }
   *rows_dev = c->rows;
   return STB_OK;
 }
@@ -409,6 +531,11 @@ int stb_corpus_read(const stb_corpus *c, uint64_t first, uint64_t n, float *rows
   if (first > c->n || n > c->n - first) { stb_set_error("corpus_read: rows [%llu,+%llu) outside corpus of %llu",
       (unsigned long long)first, (unsigned long long)n, (unsigned long long)c->n); return STB_ERR_RANGE; }
   if (n == 0) return STB_OK;
+  if (c->host_rows) {   // after the kernels that write rows
+    STB_CUDA(cudaStreamSynchronize(c->ctx->stream));
+    memcpy(rows, c->rows_host + first * STB_D, n * STB_D * sizeof(float));
+    return STB_OK;
+  }
   STB_CUDA(cudaMemcpyAsync(rows, c->rows + first * STB_D, n * STB_D * sizeof(float), cudaMemcpyDeviceToHost, c->ctx->stream));
   STB_CUDA(cudaStreamSynchronize(c->ctx->stream));
   return STB_OK;
@@ -430,6 +557,27 @@ int stb_embed(stb_ctx *ctx, const stb_table *table, const uint64_t *offsets, con
   if (total && !ids) { stb_set_error("embed: ids is null"); return STB_ERR_ARG; }
   if ((rc = dev_reserve(&ctx->embed_off_dev, &ctx->embed_off_cap, n_lines + 1, 4096)) != STB_OK) return rc;
   if ((rc = dev_reserve(&ctx->embed_ids_dev, &ctx->embed_ids_cap, std::max<uint64_t>(total, 1), 65536)) != STB_OK) return rc;
+  if (append_to && append_to->host_rows) {
+    // K3 writes chunks of lines into the staging buffer; each chunk is committed to the host rows and its q8
+    // entries from there.  The rows are booked only if no token was out of range.
+    const uint64_t chunk = std::min<uint64_t>(n_lines, STB_MUT_CHUNK_ROWS);
+    if ((rc = host_append_begin(append_to, n_lines, chunk)) != STB_OK) return rc;
+    STB_CUDA(cudaMemcpyAsync(ctx->embed_off_dev, offsets, (n_lines + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->stream));
+    if (total) STB_CUDA(cudaMemcpyAsync(ctx->embed_ids_dev, ids, total * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+    STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
+    for (uint64_t l0 = 0; l0 < n_lines; l0 += chunk) {
+      const uint64_t m = std::min(chunk, n_lines - l0);
+      if ((rc = stb_launch_embed(ctx, table, ctx->embed_off_dev + l0, ctx->embed_ids_dev, m, ctx->mut_stage, ctx->err_flag)) != STB_OK) return rc;
+      if (out) STB_CUDA(cudaMemcpyAsync(out + l0 * STB_D, ctx->mut_stage, m * STB_D * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+      if ((rc = host_append_chunk(append_to, ctx->mut_stage, append_to->n + l0, m)) != STB_OK) return rc;
+    }
+    int flag = 0;
+    STB_CUDA(cudaMemcpyAsync(&flag, ctx->err_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
+    STB_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (flag) { stb_set_error("embed: a token id maps outside the %llu-row table", (unsigned long long)table->V); return STB_ERR_RANGE; }
+    return host_append_finish(append_to, n_lines);
+  }
   float *dst = nullptr;
   if (append_to) {
     if ((rc = corpus_reserve(append_to, append_to->n + n_lines)) != STB_OK) return rc;
@@ -528,6 +676,22 @@ static int best_built_tier(stb_ctx *ctx, const stb_corpus *c, uint32_t top_k) {
     if (ready) return tier;
   }
   return STB_TIER_F32;
+}
+
+// The asynchronous top-k forms on a host-rows corpus read an HBM copy or launch nothing: an f32 top-k scan
+// would stream the whole matrix over the host link.
+static int host_rows_tier_check(const stb_corpus *c, int tier, const char *what) {
+  if (c->host_rows && tier == STB_TIER_F32) {
+    stb_set_error("%s: the rows of this corpus are in host memory and no HBM copy serves this top_k "
+                  "(q8: top_k <= %d; 16-bit shadow: stb_corpus_prepare); use stb_search", what, STB_Q8_MAX_K);
+    return STB_ERR_STATE;
+  }
+  return STB_OK;
+}
+// Deliberate scope limit: host-rows corpora are not sharded over an exchange.
+static int host_rows_refuse(const stb_corpus *c, const char *what) {
+  if (c && c->host_rows) { stb_set_error("%s: not available on a corpus whose rows are in host memory", what); return STB_ERR_STATE; }
+  return STB_OK;
 }
 
 static int ensure_hits_pin(stb_ctx *ctx, size_t need) {
@@ -632,12 +796,17 @@ int stb_search(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t 
   // not pay a full extra pass to save half of one.  A copy that covers a prefix (rows were appended
   // since) is extended right away: converting the new rows costs far less than scanning everything at
   // 1 KiB/row.
+  // A host-rows corpus builds nothing lazily: its q8 copy is always current, and its shadow is read when
+  // stb_corpus_prepare or K2 built it.  No pass streams its f32 rows while an HBM copy can answer: a top-k
+  // query no copy proves goes to the q8 histogram / collect route below, not to the f32 top-k scan.
   stb_corpus *cm = const_cast<stb_corpus *>(corpus);
-  const K1CopyPolicy lazy = {cm->searches_since_change >= 1 && cm->n >= 32768, true};
+  const bool host = cm->host_rows != 0;
+  const K1CopyPolicy lazy = {!host && cm->searches_since_change >= 1 && cm->n >= 32768, true};
   cm->searches_since_change++;
 
   uint64_t total = 0;
   const stb_hit *src_dev = nullptr;   // sorted device hits to copy out (collect path)
+  bool answered = false;
   if (!threshold_all && top_k <= stb_scan_topk_max_k()) {
     // ---- fast path: one kernel, k*16+16 bytes back -----------------------------
     // The kernel's last CTA stores the k hits + status straight into the pinned host buffers
@@ -665,30 +834,35 @@ int stb_search(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t 
       cm->tier_tries[tier]++;
       if (proven) cm->tier_proven[tier]++;
     }
-    if (!proven) {
+    if (!proven && !host) {
       if ((rc = run_fast(STB_TIER_F32)) != STB_OK) return rc;
       cm->tier_tries[STB_TIER_F32]++;
       if (ctx->status_pin[1]) cm->tier_proven[STB_TIER_F32]++;
     }
-    const uint32_t n_hits = ctx->status_pin[0];
-    if (ctx->status_pin[1]) {
-      const uint64_t n = capped_hits(ctx->hits_pin, n_hits, has_max, max_distance);
-      if (n && cap) memcpy(out_hits, ctx->hits_pin, std::min(n, cap) * sizeof(stb_hit));
-      *out_n = n;
-      if (n > cap) { stb_set_error("search: %llu hits, capacity %llu", (unsigned long long)n, (unsigned long long)cap); return STB_ERR_CAPACITY; }
-      return STB_OK;
+    if (proven || !host) {
+      const uint32_t n_hits = ctx->status_pin[0];
+      if (ctx->status_pin[1]) {
+        const uint64_t n = capped_hits(ctx->hits_pin, n_hits, has_max, max_distance);
+        if (n && cap) memcpy(out_hits, ctx->hits_pin, std::min(n, cap) * sizeof(stb_hit));
+        *out_n = n;
+        if (n > cap) { stb_set_error("search: %llu hits, capacity %llu", (unsigned long long)n, (unsigned long long)cap); return STB_ERR_CAPACITY; }
+        return STB_OK;
+      }
+      // ---- candidate margin not provable: exact collect pass --------------------
+      ctx->fallback_searches++;
+      float floor_cos = -INFINITY;
+      if (n_hits == top_k) floor_cos = (float)(1.0 - ctx->hits_pin[top_k - 1].distance - 2.0 * STB_SCORE_EPS);
+      uint64_t n_pass = 0;
+      if ((rc = collect_exact_sorted(ctx, corpus, floor_cos, has_max ? std::min(max_distance, STB_DEFAULT_MAX_DIST) : STB_DEFAULT_MAX_DIST,
+                                     ranges_dev, n_loc, n_virtual, &n_pass)) != STB_OK) return rc;
+      total = std::min<uint64_t>(n_pass, top_k);
+      src_dev = ctx->collect_hits;
+      answered = true;
     }
-    // ---- candidate margin not provable: exact collect pass --------------------
-    ctx->fallback_searches++;
-    float floor_cos = -INFINITY;
-    if (n_hits == top_k) floor_cos = (float)(1.0 - ctx->hits_pin[top_k - 1].distance - 2.0 * STB_SCORE_EPS);
-    uint64_t n_pass = 0;
-    if ((rc = collect_exact_sorted(ctx, corpus, floor_cos, has_max ? std::min(max_distance, STB_DEFAULT_MAX_DIST) : STB_DEFAULT_MAX_DIST,
-                                   ranges_dev, n_loc, n_virtual, &n_pass)) != STB_OK) return rc;
-    total = std::min<uint64_t>(n_pass, top_k);
-    src_dev = ctx->collect_hits;
-  } else {
-    // ---- threshold mode / top_k beyond the register lists: collect -> exact -> sort --------------
+  }
+  if (!answered) {
+    // ---- threshold mode / top_k beyond the register lists (on host rows: any top-k no copy proved) -------
+    // collect -> exact -> sort
     // When the int8 copy exists (or may be built: same lazy rule as the top-k tiers) the streaming
     // passes read it instead of the f32 rows: its scores are upper bounds u >= c - 2e-5 of the exact
     // cosine, so "u >= floor" collects a superset of "c >= floor" at a quarter of the bytes.
@@ -772,8 +946,9 @@ int stb_search_topk_dev(stb_ctx *ctx, const stb_corpus *corpus, const float *q_d
   if (corpus->n == 0) { stb_set_error("search_topk_dev: empty corpus"); return STB_ERR_STATE; }
   // candidates from the narrowest copy that already exists; status[1] says whether the result is
   // proven, the caller's fallback is unchanged
-  return stb_launch_scan_topk(ctx, corpus, best_built_tier(ctx, corpus, top_k), q_dev, top_k, nullptr, 0, corpus->n,
-                              out_hits_dev, out_status_dev, nullptr, true);
+  const int tier = best_built_tier(ctx, corpus, top_k);
+  if ((rc = host_rows_tier_check(corpus, tier, "search_topk_dev")) != STB_OK) return rc;
+  return stb_launch_scan_topk(ctx, corpus, tier, q_dev, top_k, nullptr, 0, corpus->n, out_hits_dev, out_status_dev, nullptr, true);
 }
 
 // ------------------------------------------------------------ peer-memory exchange ---
@@ -897,6 +1072,7 @@ int stb_search_topk_xchg(stb_ctx *ctx, const stb_corpus *corpus, const float *q_
   if (rc) return rc;
   if (!corpus || !q_dev || !x || !out_hits_dev || !out_status_dev) { stb_set_error("search_topk_xchg: null argument"); return STB_ERR_ARG; }
   if (corpus->ctx != ctx || x->ctx != ctx) { stb_set_error("search_topk_xchg: handles belong to another context"); return STB_ERR_ARG; }
+  if ((rc = host_rows_refuse(corpus, "search_topk_xchg")) != STB_OK) return rc;
   if (!x->connected) { stb_set_error("search_topk_xchg: exchange not connected"); return STB_ERR_STATE; }
   if (x->dead) { stb_set_error("search_topk_xchg: this exchange saw a peer time-out; destroy it on every rank"); return STB_ERR_STATE; }
   if (top_k == 0 || top_k > x->max_k) { stb_set_error("search_topk_xchg: top_k must be 1..%u", x->max_k); return STB_ERR_ARG; }
@@ -911,6 +1087,25 @@ int stb_search_topk_xchg(stb_ctx *ctx, const stb_corpus *corpus, const float *q_
 }
 
 // ----------------------------------------------------------------- K2 batched search ---
+// Rows [first, n) of a host-rows corpus for a copy builder: uploaded into the context's staging buffer in chunks
+// of at most STB_MUT_CHUNK_ROWS rows (a multiple of the shadow's 256-row tile), fn(stage, r0, r1) per chunk.
+}  // extern "C"
+template <class F>
+static int host_rows_staged(stb_corpus *c, uint64_t first, F &&fn) {
+  stb_ctx *ctx = c->ctx;
+  if (first >= c->n) return STB_OK;
+  const uint64_t chunk = std::min<uint64_t>(c->n - first, STB_MUT_CHUNK_ROWS);
+  int rc;
+  if ((rc = dev_reserve(&ctx->mut_stage, &ctx->mut_stage_cap, chunk * STB_D)) != STB_OK) return rc;
+  for (uint64_t r0 = first; r0 < c->n; r0 += chunk) {
+    const uint64_t m = std::min(chunk, c->n - r0);
+    STB_CUDA(cudaMemcpyAsync(ctx->mut_stage, c->rows_host + r0 * STB_D, m * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    if ((rc = fn(ctx->mut_stage, r0, r0 + m)) != STB_OK) return rc;
+  }
+  return STB_OK;
+}
+extern "C" {
+
 static int corpus_ensure_shadow(stb_ctx *ctx, stb_corpus *c) {
   if (c->shadow && c->shadow_rows == c->n) {
     if (c->shadow_bad) { stb_set_error("search_batch: corpus holds rows whose norm is not a normal fp32 number; use stb_search"); return STB_ERR_STATE; }
@@ -932,7 +1127,13 @@ static int corpus_ensure_shadow(stb_ctx *ctx, stb_corpus *c) {
   }
   int rc;
   STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
-  if ((rc = stb_launch_shadow_build(ctx, c->rows, c->n, 256, c->shadow, ctx->err_flag, first)) != STB_OK) return rc;
+  if (c->host_rows)
+    rc = host_rows_staged(c, first, [&](const float *stage, uint64_t r0, uint64_t r1) {
+      return stb_launch_shadow_build(ctx, stage, r1, 256, c->shadow, ctx->err_flag, r0, nullptr, r0);
+    });
+  else
+    rc = stb_launch_shadow_build(ctx, c->rows, c->n, 256, c->shadow, ctx->err_flag, first);
+  if (rc != STB_OK) return rc;
   int flag = 0;
   STB_CUDA(cudaMemcpyAsync(&flag, ctx->err_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
@@ -949,34 +1150,19 @@ static int corpus_ensure_q8(stb_ctx *ctx, stb_corpus *c) {
     return STB_OK;
   }
   uint64_t first = (c->q8 && c->q8_rows < c->n && !c->q8_bad) ? c->q8_rows : 0;      // valid prefix: convert only the new rows
-  if (c->n > c->q8_cap_rows || !c->q8) {
-    // int8 codes + scales (260 B/row) and the top-k prefilter's nibble plane + {s, rho} (136 B/row)
-    uint8_t *np = nullptr, *pp = nullptr;
-    float *ns = nullptr;
-    float2 *sp = nullptr;
-    const uint64_t cap = std::max<uint64_t>(c->n, c->capacity);
-    cudaError_t e = cudaMalloc((void **)&np, cap * 256ull);
-    if (e == cudaSuccess) e = cudaMalloc((void **)&ns, cap * sizeof(float));
-    if (e == cudaSuccess) e = cudaMalloc((void **)&pp, stb_q4_plane_bytes(cap));
-    if (e == cudaSuccess) e = cudaMalloc((void **)&sp, cap * sizeof(float2));
-    if (e != cudaSuccess) {
-      cudaGetLastError(); cudaFree(np); cudaFree(ns); cudaFree(pp);
-      stb_set_error("q8 tier: cannot allocate %llu MiB", (unsigned long long)(cap * 396 >> 20));
-      return STB_ERR_NOMEM;
-    }
-    if (c->q8 && first) {
-      STB_CUDA(cudaMemcpyAsync(np, c->q8, first * 256ull, cudaMemcpyDeviceToDevice, ctx->stream));
-      STB_CUDA(cudaMemcpyAsync(ns, c->q8_scale, first * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
-      STB_CUDA(cudaMemcpyAsync(pp, c->q4, stb_q4_plane_bytes(first), cudaMemcpyDeviceToDevice, ctx->stream));   // whole tiles
-      STB_CUDA(cudaMemcpyAsync(sp, c->q4_sr, first * sizeof(float2), cudaMemcpyDeviceToDevice, ctx->stream));
-      STB_CUDA(cudaStreamSynchronize(ctx->stream));
-    } else first = 0;
-    cudaFree(c->q8); cudaFree(c->q8_scale); cudaFree(c->q4); cudaFree(c->q4_sr);
-    c->q8 = np; c->q8_scale = ns; c->q4 = pp; c->q4_sr = sp; c->q8_cap_rows = cap;
-  }
   int rc;
+  if (c->n > c->q8_cap_rows || !c->q8) {
+    if ((rc = q8_realloc(c, std::max<uint64_t>(c->n, c->capacity), first)) != STB_OK) return rc;
+  }
   STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
-  if ((rc = stb_launch_q8_build(ctx, c->rows, first, c->n, c->q8, c->q8_scale, c->q4, c->q4_sr, ctx->err_flag)) != STB_OK) return rc;
+  // a host-rows corpus gets here only to re-encode a copy a mutation dropped as unusable
+  if (c->host_rows)
+    rc = host_rows_staged(c, first, [&](const float *stage, uint64_t r0, uint64_t r1) {
+      return stb_launch_q8_build(ctx, stage, r0, r1, c->q8, c->q8_scale, c->q4, c->q4_sr, ctx->err_flag, r0);
+    });
+  else
+    rc = stb_launch_q8_build(ctx, c->rows, first, c->n, c->q8, c->q8_scale, c->q4, c->q4_sr, ctx->err_flag);
+  if (rc != STB_OK) return rc;
   int flag = 0;
   STB_CUDA(cudaMemcpyAsync(&flag, ctx->err_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
@@ -1053,6 +1239,11 @@ static int corpus_mutation_finish(stb_corpus *c) {
   if (flags[0]) c->q8_bad = 1;
   if (flags[1]) c->shadow_bad = 1;
   corpus_changed(c, CORPUS_ROWS_REWRITTEN);
+  // a host-rows corpus keeps its q8 copy current: one dropped as unusable is re-encoded from the rows now
+  if (c->host_rows && c->q8_rows < c->n) {
+    const int rc = corpus_ensure_q8(ctx, c);
+    if (rc != STB_OK && rc != STB_ERR_STATE) return rc;
+  }
   return STB_OK;
 }
 
@@ -1700,6 +1891,7 @@ int stb_search_batch_xchg_dev(stb_ctx *ctx, const stb_corpus *corpus, const floa
   if (rc) return rc;
   if (!corpus || !q_dev || !x || !out_hits_dev || !out_status_dev) { stb_set_error("search_batch_xchg_dev: null argument"); return STB_ERR_ARG; }
   if (corpus->ctx != ctx || x->ctx != ctx) { stb_set_error("search_batch_xchg_dev: handles belong to another context"); return STB_ERR_ARG; }
+  if ((rc = host_rows_refuse(corpus, "search_batch_xchg_dev")) != STB_OK) return rc;
   if (!x->connected) { stb_set_error("search_batch_xchg_dev: exchange not connected"); return STB_ERR_STATE; }
   if (x->dead) { stb_set_error("search_batch_xchg_dev: this exchange saw a peer time-out; destroy it on every rank"); return STB_ERR_STATE; }
   if (nq == 0) return STB_OK;
@@ -1777,6 +1969,7 @@ int stb_search_xchg(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint
   int rc = ctx_use(ctx);
   if (rc) return rc;
   if (!q || !out_hits || !out_n || !out_complete) { stb_set_error("search_xchg: null argument"); return STB_ERR_ARG; }
+  if ((rc = host_rows_refuse(corpus, "search_xchg")) != STB_OK) return rc;
   memcpy(ctx->q_pin, q, STB_D * sizeof(float));
   STB_CUDA(cudaMemcpyAsync(ctx->q_dev, ctx->q_pin, STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
   // the merge CTA stores the hits + status straight into pinned host memory
@@ -1801,6 +1994,7 @@ int stb_search_many(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint
   if (rc) return rc;
   if (!corpus || !q || !out_hits || !out_n) { stb_set_error("search_many: null argument"); return STB_ERR_ARG; }
   if (corpus->ctx != ctx || (x && x->ctx != ctx)) { stb_set_error("search_many: handles belong to another context"); return STB_ERR_ARG; }
+  if (x && (rc = host_rows_refuse(corpus, "search_many with an exchange")) != STB_OK) return rc;
   if (nq == 0) return STB_OK;
   for (uint32_t i = 0; i < nq; ++i) { out_n[i] = 0; if (out_complete) out_complete[i] = 1; }
   if (top_k == 0 || corpus->n == 0) {
@@ -1823,6 +2017,8 @@ int stb_search_many(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint
   const bool eager = nq >= 2 && corpus->n >= 32768;
   bool q8_ready = false;
   if ((rc = k1_copy_ready(ctx, const_cast<stb_corpus *>(corpus), STB_TIER_Q8, top_k, {eager, eager}, &q8_ready)) != STB_OK) return rc;
+  const int tier = q8_ready ? STB_TIER_Q8 : best_built_tier(ctx, corpus, top_k);
+  if ((rc = host_rows_tier_check(corpus, tier, "search_many")) != STB_OK) return rc;
   if ((rc = dev_reserve(&ctx->bq_dev, &ctx->bq_dev_cap, (size_t)nq * STB_D)) != STB_OK) return rc;
   if ((rc = ensure_hits_pin(ctx, (size_t)nq * top_k)) != STB_OK) return rc;
   if ((size_t)nq * STB_D > ctx->many_q_pin_cap) {
@@ -1839,7 +2035,6 @@ int stb_search_many(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint
   }
   memcpy(ctx->many_q_pin, q, (size_t)nq * STB_D * sizeof(float));
   STB_CUDA(cudaMemcpyAsync(ctx->bq_dev, ctx->many_q_pin, (size_t)nq * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-  const int tier = q8_ready ? STB_TIER_Q8 : best_built_tier(ctx, corpus, top_k);
   for (uint32_t i = 0; i < nq; ++i) {
     stb_hit *oh = ctx->hits_pin + (size_t)i * top_k;
     uint32_t *os = ctx->many_status_pin + 4 * (size_t)i;

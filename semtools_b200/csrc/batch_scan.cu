@@ -160,14 +160,14 @@ __device__ __forceinline__ uint64_t wg_desc_sw128(uint32_t smem_addr) {
 template <int TILE>
 __global__ void __launch_bounds__(256)
 stb_shadow_build_kernel(const float4 *__restrict__ rows, uint64_t first_row, uint64_t n_rows, uint64_t n_padded,
-                        uint8_t *__restrict__ out, int *bad_flag, uint32_t *row_bad) {
+                        uint8_t *__restrict__ out, int *bad_flag, uint32_t *row_bad, uint64_t rows_first) {
   const int lane = threadIdx.x & 31;
   const uint64_t row = first_row + (uint64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
   if (row >= n_padded) return;
   float4 v0 = make_float4(0.f, 0.f, 0.f, 0.f), v1 = v0;
   if (row < n_rows) {
-    v0 = __ldg(rows + row * STB_ROW_F4 + 2 * lane);
-    v1 = __ldg(rows + row * STB_ROW_F4 + 2 * lane + 1);
+    v0 = __ldg(rows + (row - rows_first) * STB_ROW_F4 + 2 * lane);
+    v1 = __ldg(rows + (row - rows_first) * STB_ROW_F4 + 2 * lane + 1);
   }
   // per-row record (query tiles): a row that cannot be normalised bounds nothing; the finish kernels mark
   // it unproven
@@ -459,15 +459,15 @@ void stb_batch_build_params(int *shadow_is_f16, double *eps) {
 
 // ------------------------------------------------------- host-side: shadow + GEMM ------
 int stb_launch_shadow_build(stb_ctx *ctx, const float *rows_dev, uint64_t n_rows, int tile, uint8_t *out,
-                            int *bad_flag_dev, uint64_t first_row, uint32_t *row_bad_dev) {
+                            int *bad_flag_dev, uint64_t first_row, uint32_t *row_bad_dev, uint64_t rows_first) {
   // rows [first_row, n_rows) plus the zero padding of the last tile; first_row must be tile-aligned
   const uint64_t n_padded = (n_rows + tile - 1) / tile * tile;
   if (n_padded == 0 || first_row >= n_padded) return STB_OK;
   const unsigned blocks = (unsigned)((n_padded - first_row + 7) / 8);
   if (tile == STB_B_TILE)
-    stb_shadow_build_kernel<STB_B_TILE><<<blocks, 256, 0, ctx->stream>>>(reinterpret_cast<const float4 *>(rows_dev), first_row, n_rows, n_padded, out, bad_flag_dev, row_bad_dev);
+    stb_shadow_build_kernel<STB_B_TILE><<<blocks, 256, 0, ctx->stream>>>(reinterpret_cast<const float4 *>(rows_dev), first_row, n_rows, n_padded, out, bad_flag_dev, row_bad_dev, rows_first);
   else
-    stb_shadow_build_kernel<STB_A_TILE><<<blocks, 256, 0, ctx->stream>>>(reinterpret_cast<const float4 *>(rows_dev), first_row, n_rows, n_padded, out, bad_flag_dev, row_bad_dev);
+    stb_shadow_build_kernel<STB_A_TILE><<<blocks, 256, 0, ctx->stream>>>(reinterpret_cast<const float4 *>(rows_dev), first_row, n_rows, n_padded, out, bad_flag_dev, row_bad_dev, rows_first);
   STB_CUDA(cudaGetLastError());
   ctx->kernel_launches++;
   return STB_OK;

@@ -223,7 +223,11 @@ struct stb_table {
 
 struct stb_corpus {
   stb_ctx *ctx;
-  float *rows;         // capacity x 256
+  float *rows;         // capacity x 256; on a host-rows corpus the device address of rows_host
+  // stb_corpus_create_host: the rows live in page-locked, device-mapped host memory (kernels read them over
+  // the host link through `rows`) and the q8 copy is kept current by every call that writes rows
+  float *rows_host;    // null on a device corpus
+  int host_rows;
   uint64_t n;
   uint64_t capacity;
   uint64_t row_base;
@@ -321,8 +325,9 @@ int stb_launch_scan_topk(stb_ctx *ctx, const stb_corpus *c, int tier, const floa
                          uint64_t n_virtual, stb_hit *out_hits_dev,
                          uint32_t *out_status_dev, const StbXchgArgs *xchg = nullptr, bool overlapped = false);
 // int8 codes + scales, nibble plane + {s, rho} of rows [first_row, n_rows) (q8 tier)
+// rows_first: the row rows_dev[0] holds (a staged chunk of a host-rows corpus), 0 for a whole matrix
 int stb_launch_q8_build(stb_ctx *ctx, const float *rows_dev, uint64_t first_row, uint64_t n_rows, uint8_t *out,
-                        float *scale, uint8_t *plane, float2 *sr, int *bad_flag_dev);
+                        float *scale, uint8_t *plane, float2 *sr, int *bad_flag_dev, uint64_t rows_first = 0);
 // Largest top_k the fast path serves.
 uint32_t stb_scan_topk_max_k(void);
 // Collect path: every row whose approximate cosine >= cos_floor (or that cannot be
@@ -379,9 +384,10 @@ int stb_launch_embed(stb_ctx *ctx, const stb_table *t, const uint64_t *offsets_d
                      int *err_flag_dev);
 
 // ---- batch_scan.cu (K2) ------------------------------------------------------------------
+// rows_first: the row rows_dev[0] holds, as stb_launch_q8_build
 int stb_launch_shadow_build(stb_ctx *ctx, const float *rows_dev, uint64_t n_rows, int tile,
                             uint8_t *out, int *bad_flag_dev, uint64_t first_row = 0,
-                            uint32_t *row_bad_dev = nullptr);
+                            uint32_t *row_bad_dev = nullptr, uint64_t rows_first = 0);
 int stb_launch_batch_gemm(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_tiles,
                           const uint8_t *b_tiles, uint32_t n_tiles, float *submax,
                           float *tilemax, float *full_out);

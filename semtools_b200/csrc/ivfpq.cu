@@ -1462,6 +1462,7 @@ int stb_ivfpq_build(stb_ctx *ctx, const stb_corpus *corpus, uint32_t nlist, uint
                     stb_ivfpq **out) {
   if (!ctx || !corpus || !out) { stb_set_error("ivfpq_build: null argument"); return STB_ERR_ARG; }
   if (corpus->ctx != ctx) { stb_set_error("ivfpq_build: corpus belongs to another context"); return STB_ERR_ARG; }
+  if (corpus->host_rows) { stb_set_error("ivfpq_build: not available on a corpus whose rows are in host memory"); return STB_ERR_STATE; }
   if (cudaSetDevice(ctx->device) != cudaSuccess) { stb_set_error("cudaSetDevice failed"); return STB_ERR_CUDA; }
   const uint64_t n = corpus->n;
   if (nlist < 1 || nlist > 8192 || n < nlist || n < 256) { stb_set_error("ivfpq_build: need 1 <= nlist <= 8192 <= rows and rows >= 256"); return STB_ERR_ARG; }

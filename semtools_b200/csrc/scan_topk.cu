@@ -675,21 +675,22 @@ __device__ __forceinline__ void stb_scan_q4(const ScanArgs &args, const uint8_t 
 // plane and {s, rho} of the top-k scan's prefilter (stb_scan_q4).
 __global__ void __launch_bounds__(256)
 stb_q8_build_kernel(const float4 *__restrict__ rows, uint64_t first_row, uint64_t n_rows, uint8_t *__restrict__ out,
-                    float *__restrict__ scale, uint8_t *__restrict__ plane, float2 *__restrict__ sr, int *bad_flag) {
+                    float *__restrict__ scale, uint8_t *__restrict__ plane, float2 *__restrict__ sr, int *bad_flag,
+                    uint64_t rows_first) {
   const int lane = threadIdx.x & 31;
   const uint64_t row = first_row + (uint64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
   if (row >= n_rows) return;
-  const float4 v0 = __ldg(rows + row * STB_ROW_F4 + 2 * lane);
-  const float4 v1 = __ldg(rows + row * STB_ROW_F4 + 2 * lane + 1);
+  const float4 v0 = __ldg(rows + (row - rows_first) * STB_ROW_F4 + 2 * lane);
+  const float4 v1 = __ldg(rows + (row - rows_first) * STB_ROW_F4 + 2 * lane + 1);
   stb_q8_encode_row(v0, v1, lane, row, out, scale, plane, sr, bad_flag);
 }
 
 int stb_launch_q8_build(stb_ctx *ctx, const float *rows_dev, uint64_t first_row, uint64_t n_rows, uint8_t *out,
-                        float *scale, uint8_t *plane, float2 *sr, int *bad_flag_dev) {
+                        float *scale, uint8_t *plane, float2 *sr, int *bad_flag_dev, uint64_t rows_first) {
   if (first_row >= n_rows) return STB_OK;
   const unsigned blocks = (unsigned)((n_rows - first_row + 7) / 8);
   stb_q8_build_kernel<<<blocks, 256, 0, ctx->stream>>>(reinterpret_cast<const float4 *>(rows_dev), first_row, n_rows, out, scale,
-                                                       plane, sr, bad_flag_dev);
+                                                       plane, sr, bad_flag_dev, rows_first);
   STB_CUDA(cudaGetLastError());
   ctx->kernel_launches++;
   return STB_OK;
@@ -1444,17 +1445,19 @@ int stb_launch_scan_collect(stb_ctx *ctx, const stb_corpus *c, int tier,
 
 // ------------------------------------------------------------ histogram pass (large k) ---
 // For top_k beyond the register lists: one scan builds a 4096-bin histogram of the
-// approximate cosine (bin b covers cos in (1-(b+1)/2048, 1-b/2048]; forced candidates fall
-// in bin 0), the host picks the bin that contains the k-th best, and the collect pass
-// gathers everything at or above that bin's lower edge (minus the score error bound).
+// approximate cosine (bin b covers cos in (1-(b+1)/2048, 1-b/2048]), the host picks the bin that
+// contains the k-th best, and the collect pass gathers everything at or above that bin's lower edge
+// (minus the score error bound).  Forced candidates (score +inf: rows that cannot be scored safely) are
+// not counted: the collect pass takes them whatever the floor, so the k-th bin is the k-th best of the
+// scored rows -- counting them would put the floor above a row of the exact top-k.
 #define STB_HIST_BINS 4096
 struct HistSink {
   unsigned int *hist;   // shared-memory histogram of this CTA
   template <int ROWS>
   __device__ __forceinline__ void consume(float s, uint32_t) {
-    if (s > -CUDART_INF_F) {
+    if (s > -CUDART_INF_F && s < CUDART_INF_F) {
       float b = floorf((1.0f - s) * (STB_HIST_BINS / 2.0f));
-      int bin = b < 0.f ? 0 : (b > (float)(STB_HIST_BINS - 1) ? STB_HIST_BINS - 1 : (int)b);   // +inf -> 0, NaN cannot occur
+      int bin = b < 0.f ? 0 : (b > (float)(STB_HIST_BINS - 1) ? STB_HIST_BINS - 1 : (int)b);   // NaN cannot occur
       atomicAdd(hist + bin, 1u);
     }
   }

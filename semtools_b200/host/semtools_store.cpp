@@ -435,6 +435,22 @@ std::vector<uint64_t> Store::ranges_for(const std::vector<std::string> &subset_p
   return ranges;
 }
 
+int upload_mirror(stb_ctx *ctx, const float *rows, uint64_t n, stb_corpus **out, CorpusCreateFn create) {
+  *out = nullptr;
+  stb_corpus *c = nullptr;
+  int rc = create(ctx, STB_DIM, n, 0, &c);
+  if (rc == STB_OK) rc = stb_corpus_append(c, rows, n);
+  if (rc == STB_OK) { *out = c; return STB_OK; }
+  stb_corpus_destroy(c);
+  if (rc != STB_ERR_NOMEM) return rc;
+  c = nullptr;
+  rc = stb_corpus_create_host(ctx, STB_DIM, n, 0, &c);
+  if (rc == STB_OK) rc = stb_corpus_append(c, rows, n);
+  if (rc == STB_OK) *out = c;
+  else stb_corpus_destroy(c);
+  return rc;
+}
+
 std::vector<RankedLine> Store::search_line_embeddings(const std::vector<float> &query, const std::vector<std::string> &subset_paths,
                                                       size_t top_k, std::optional<float> max_distance, int device) {
   std::vector<RankedLine> out;
@@ -444,8 +460,7 @@ std::vector<RankedLine> Store::search_line_embeddings(const std::vector<float> &
   stb_ctx *ctx = nullptr; stb_corpus *corpus = nullptr;
   auto chk = [&](int rc) { if (rc < 0) { std::string m = stb_last_error(); stb_corpus_destroy(corpus); stb_ctx_destroy(ctx); throw StbError(rc, m); } };
   chk(stb_ctx_create(device, nullptr, &ctx));
-  chk(stb_corpus_create(ctx, STB_DIM, rows_.size() / 2, 0, &corpus));
-  chk(stb_corpus_append(corpus, emb_.data(), rows_.size() / 2));
+  chk(upload_mirror(ctx, emb_.data(), rows_.size() / 2, &corpus));
   std::vector<stb_hit> hits(top_k);
   uint64_t n = 0;
   chk(stb_search(ctx, corpus, query.data(), (uint32_t)top_k, max_distance ? 1 : 0, max_distance ? (double)*max_distance : 0.0,

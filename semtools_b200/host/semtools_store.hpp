@@ -21,6 +21,13 @@ namespace semtools {
 constexpr uint32_t CURRENT_EMBEDDING_VERSION = 2;      // store.rs:34
 constexpr size_t LINE_EMBEDDING_SIZE = 256;            // store.rs:37
 
+// The one rule for where a store's GPU mirror lives: in HBM, unless creating or uploading it there fails with
+// STB_ERR_NOMEM; then its rows stay in host memory and only their q8 copy goes to HBM (stb_corpus_create_host).
+// The hits are the same either way.  `create` is the device attempt (a test passes one that fails).  Returns the
+// stb status; *out is the mirror holding the n rows, or null.
+using CorpusCreateFn = int (*)(stb_ctx *, uint32_t, uint64_t, uint64_t, stb_corpus **);
+int upload_mirror(stb_ctx *ctx, const float *rows, uint64_t n, stb_corpus **out, CorpusCreateFn create = stb_corpus_create);
+
 struct WorkspaceConfig {                               // mod.rs:8-25
   std::string name = "default";
   std::string root_dir;

@@ -506,8 +506,20 @@ class Store:
     def _gpu_corpus(self) -> capi.Corpus:
         if self.ctx is None:
             self.ctx = capi.Context(0)                               # no GPU -> StbError, never a CPU scan
+        try:
+            return self._upload_mirror(capi.Corpus)
+        except capi.StbError as e:
+            # The one rule for where the mirror lives: in HBM, unless creating or uploading it there fails with
+            # STB_ERR_NOMEM; then its rows stay in host memory and only their q8 copy goes to HBM.  The hits are
+            # the same either way.
+            if e.status != capi.STB_ERR_NOMEM or (self._corpus is not None and self._corpus.host_rows):
+                raise
+            self._corpus = None
+            return self._upload_mirror(capi.Corpus.in_host_memory)
+
+    def _upload_mirror(self, make) -> capi.Corpus:
         if self._corpus is None:
-            self._corpus = capi.Corpus(self.ctx, max(len(self._emb), 1))
+            self._corpus = make(self.ctx, max(len(self._emb), 1))
             self._corpus_n = 0
         while self._corpus_n < len(self._emb):                        # only rows not uploaded yet, 256 MiB at a time
             hi = min(len(self._emb), self._corpus_n + 262144)
