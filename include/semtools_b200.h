@@ -614,6 +614,24 @@ int stb_debug_coscan_offsets(stb_ctx *ctx, uint32_t n, uint32_t *out);
 #define STB_COPY_H16_TILES 4
 int stb_debug_corpus_copy(const stb_corpus *corpus, int which, uint64_t first, uint64_t n, void *out,
                           uint64_t *covered);
+/* Test hooks for K1's per-row score contracts (DESIGN.md section 5).  Both run the production scan code on
+ * query q (256 f32, host) over the corpus's rows or over row_ranges (global [begin, end) pairs, as
+ * stb_search takes them; NULL with n_ranges = 0: every row), ignore STB_SCAN_TIER and synchronise the stream.
+ * Outputs are per LOCAL row, cap >= the corpus's rows; a row outside the ranges keeps score NaN and count 0.
+ * stb_debug_scan_scores: tier 0 / 1 / 2 picks the pass (f32 rows / 16-bit shadow / int8 codes, the order of
+ *   stb_corpus_tier_stats); scores[row] is the score the pass gave the row and seen[row] how many times it was scored.
+ *   hist (may be NULL; f32 and q8 only) receives the 4096-bin histogram of the large-k route's pass.
+ * stb_debug_q4_scan: the q8 tier's prefiltered top-k scan for top_k (1..16) with threshold words of its own;
+ *   per row its 4-bit bound u4 and the threshold T it was tested against, refined[row] = times it was scored
+ *   from the int8 codes and, for such rows, that score u8 and the lower bound l8 it published; words receives
+ *   the top_k final threshold words (tag 1 in the high half).  pin != 0 holds T at -inf: every row is refined.
+ * STB_ERR_ARG: a null pointer or cap too small; STB_ERR_STATE: the tier's copy is not built or unusable. */
+int stb_debug_scan_scores(stb_ctx *ctx, const stb_corpus *corpus, int tier, const float *q,
+                          const uint64_t *row_ranges, uint32_t n_ranges, uint64_t cap, float *scores,
+                          uint32_t *seen, uint32_t *hist);
+int stb_debug_q4_scan(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t top_k,
+                      const uint64_t *row_ranges, uint32_t n_ranges, int pin, uint64_t cap, float *u4,
+                      float *t, uint32_t *refined, float *u8, float *l8, uint64_t *words);
 /* Test hook for K2: shadow build + wgmma GEMM on host inputs; out_full receives the
  * approximate cosine matrix [ceil(nq/128)*128][ceil(n/256)*256] (f32), out_submax (may be
  * NULL) the per-32-row maxima [ceil(nq/128)][ceil(n/256)*8][128]. */

@@ -30,7 +30,7 @@ SYMBOLS = [
     "stb_xchg_connect", "stb_xchg_connect_local", "stb_search_topk_xchg", "stb_search_xchg", "stb_search_many", "stb_xchg_create_batch", "stb_search_batch_xchg_dev", "stb_ivfpq_build",
     "stb_ivfpq_destroy", "stb_ivfpq_extend", "stb_ivfpq_stats", "stb_ivfpq_search", "stb_ivfpq_search_dev", "stb_hits_merge_dev", "stb_hits_merge_batch_dev", "stb_hits_merge", "stb_fnv1a64", "stb_line_id", "stb_line_ids",
     "stb_ctx_counters", "stb_debug_ticket_check", "stb_debug_q4_refined", "stb_debug_coscan_offsets", "stb_debug_batch_gemm", "stb_debug_batch_params",
-    "stb_debug_batch_last", "stb_debug_corpus_copy",
+    "stb_debug_batch_last", "stb_debug_corpus_copy", "stb_debug_scan_scores", "stb_debug_q4_scan",
     "stb_debug_ivfpq_export",
     "stb_ivfpq_search_batch", "stb_ivfpq_search_batch_dev", "stb_debug_ivfpq_batch_last",
     "stb_ivfpq_search_filtered", "stb_ivfpq_update", "stb_ivfpq_remove",
@@ -87,6 +87,8 @@ def lib() -> C.CDLL:
     L.stb_corpus_update.argtypes = [vp, vp, vp, u64]
     L.stb_corpus_remove.argtypes = [vp, vp, u32]
     L.stb_debug_corpus_copy.argtypes = [vp, i32, u64, u64, vp, C.POINTER(u64)]
+    L.stb_debug_scan_scores.argtypes = [vp, vp, i32, vp, vp, u32, u64, vp, vp, vp]
+    L.stb_debug_q4_scan.argtypes = [vp, vp, vp, u32, vp, u32, i32, u64, vp, vp, vp, vp, vp, vp]
     L.stb_embed.argtypes = [vp, vp, vp, vp, u64, vp, vp]
     L.stb_embed_dev.argtypes = [vp, vp, vp, vp, u64, vp]
     L.stb_embed_status.argtypes = [vp]
@@ -377,6 +379,43 @@ class Corpus:
         out = np.zeros(shape, dtype=dtype)
         _check(lib().stb_debug_corpus_copy(self._h, which, first, n, _np_ptr(out) if n else None, C.byref(covered)))
         return out, cov
+
+    @staticmethod
+    def _debug_args(q, row_ranges):
+        q = np.ascontiguousarray(q, dtype=np.float32)
+        if q.size != STB_DIM:
+            raise StbError(STB_ERR_ARG, f"query must have {STB_DIM} floats")
+        if row_ranges is None:
+            return q, None, 0
+        rr = np.ascontiguousarray(row_ranges, dtype=np.uint64).reshape(-1, 2)
+        return q, (rr if rr.shape[0] else np.zeros((1, 2), dtype=np.uint64)), rr.shape[0]
+
+    def debug_scan_scores(self, q, tier: str = "f32", row_ranges=None, hist: bool = False):
+        """stb_debug_scan_scores: (score [n] f32, times scored [n] u32, 4096-bin histogram or None) of one K1
+        pass, tier "f32" | "h16" | "q8", per local row; rows outside row_ranges keep NaN and 0."""
+        q, rr, n_rr = self._debug_args(q, row_ranges)
+        n = len(self)
+        scores, seen = np.zeros(max(n, 1), np.float32), np.zeros(max(n, 1), np.uint32)
+        h = np.zeros(4096, np.uint32) if hist else None
+        _check(lib().stb_debug_scan_scores(self.ctx._h, self._h, ("f32", "h16", "q8").index(tier), _np_ptr(q), _np_ptr(rr), n_rr,
+                                           n, _np_ptr(scores), _np_ptr(seen), _np_ptr(h)))
+        return scores[:n], seen[:n], h
+
+    def debug_q4_scan(self, q, top_k: int, row_ranges=None, pin: bool = True):
+        """stb_debug_q4_scan: the q8 tier's prefiltered top-k scan, per local row.  Returns a dict of numpy
+        arrays: u4, t (the threshold the row was tested against), refined (times scored from the int8 codes), u8,
+        l8 (refined rows; NaN elsewhere), and words [top_k] u64 (the final threshold words)."""
+        q, rr, n_rr = self._debug_args(q, row_ranges)
+        n = len(self)
+        out = {k: np.zeros(max(n, 1), np.float32) for k in ("u4", "t", "u8", "l8")}
+        out["refined"] = np.zeros(max(n, 1), np.uint32)
+        words = np.zeros(max(top_k, 1), np.uint64)
+        _check(lib().stb_debug_q4_scan(self.ctx._h, self._h, _np_ptr(q), top_k, _np_ptr(rr), n_rr, int(pin), n,
+                                       _np_ptr(out["u4"]), _np_ptr(out["t"]), _np_ptr(out["refined"]), _np_ptr(out["u8"]),
+                                       _np_ptr(out["l8"]), _np_ptr(words)))
+        out = {k: v[:n] for k, v in out.items()}
+        out["words"] = words[:top_k]
+        return out
 
     # -- K1 + K4 -------------------------------------------------------------
     def search(self, q, top_k: int = 3, max_distance: float | None = None,

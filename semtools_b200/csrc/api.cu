@@ -718,6 +718,36 @@ static uint64_t capped_hits(const stb_hit *hits, uint64_t n, int has_max, double
   return i;
 }
 
+// ---- row ranges: global -> local, clipped to this shard, uploaded as the K1 passes read them (ScanArgs: the
+// virtual prefix of every range, then its first local row).  Without ranges the pass reads every row; *n_virtual
+// = 0: no row of the corpus lies in the ranges.
+static int k1_upload_ranges(stb_ctx *ctx, const stb_corpus *c, const char *what, const uint64_t *row_ranges, uint32_t n_ranges,
+                            const uint64_t **ranges_dev, uint32_t *n_loc, uint64_t *n_virtual) {
+  *ranges_dev = nullptr;
+  *n_loc = 0;
+  *n_virtual = c->n;
+  if (!row_ranges) return STB_OK;
+  std::vector<uint64_t> vstart, rbegin;
+  vstart.reserve(n_ranges + 1); rbegin.reserve(n_ranges);
+  uint64_t acc = 0;
+  int rc;
+  if ((rc = stb_clip_ranges(what, row_ranges, n_ranges, c->row_base, c->n, [&](uint64_t b, uint64_t e) {
+         vstart.push_back(acc); rbegin.push_back(b);
+         acc += e - b;
+       })) != STB_OK) return rc;
+  *n_virtual = acc;
+  if (acc == 0) return STB_OK;
+  vstart.push_back(acc);
+  *n_loc = (uint32_t)rbegin.size();
+  std::vector<uint64_t> packed(vstart);
+  packed.insert(packed.end(), rbegin.begin(), rbegin.end());
+  if ((rc = dev_reserve(&ctx->ranges_dev, &ctx->ranges_cap, packed.size(), 4096)) != STB_OK) return rc;
+  STB_CUDA(cudaMemcpyAsync(ctx->ranges_dev, packed.data(), packed.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->stream));
+  STB_CUDA(cudaStreamSynchronize(ctx->stream));   // `packed` dies at scope end
+  *ranges_dev = ctx->ranges_dev;
+  return STB_OK;
+}
+
 // Exact path for any input: collect rows whose approximate cosine >= cos_floor,
 // score them canonically, keep distance < limit, sort by (distance,row).
 // On return ctx->collect_hits holds the sorted hits and *n_pass their count.
@@ -764,29 +794,11 @@ int stb_search(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t 
   if (mode == STB_MODE_STORE_QUERY && row_ranges && n_ranges == 0) return STB_OK;  // empty subset, store.rs:489
   if (corpus->n == 0) return STB_OK;
 
-  // ---- row ranges: global -> local, clipped to this shard ----------------------
   const uint64_t *ranges_dev = nullptr;
   uint32_t n_loc = 0;
-  uint64_t n_virtual = corpus->n;
-  if (row_ranges) {
-    std::vector<uint64_t> vstart, rbegin;
-    vstart.reserve(n_ranges + 1); rbegin.reserve(n_ranges);
-    uint64_t acc = 0;
-    if ((rc = stb_clip_ranges("search", row_ranges, n_ranges, corpus->row_base, corpus->n, [&](uint64_t b, uint64_t e) {
-           vstart.push_back(acc); rbegin.push_back(b);
-           acc += e - b;
-         })) != STB_OK) return rc;
-    if (acc == 0) return STB_OK;
-    vstart.push_back(acc);
-    n_loc = (uint32_t)rbegin.size();
-    n_virtual = acc;
-    std::vector<uint64_t> packed(vstart);
-    packed.insert(packed.end(), rbegin.begin(), rbegin.end());
-    if ((rc = dev_reserve(&ctx->ranges_dev, &ctx->ranges_cap, packed.size(), 4096)) != STB_OK) return rc;
-    STB_CUDA(cudaMemcpyAsync(ctx->ranges_dev, packed.data(), packed.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->stream));
-    STB_CUDA(cudaStreamSynchronize(ctx->stream));   // `packed` dies at scope end
-    ranges_dev = ctx->ranges_dev;
-  }
+  uint64_t n_virtual = 0;
+  if ((rc = k1_upload_ranges(ctx, corpus, "search", row_ranges, n_ranges, &ranges_dev, &n_loc, &n_virtual)) != STB_OK) return rc;
+  if (n_virtual == 0) return STB_OK;
 
   memcpy(ctx->q_pin, q, STB_D * sizeof(float));
   STB_CUDA(cudaMemcpyAsync(ctx->q_dev, ctx->q_pin, STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
@@ -1961,6 +1973,113 @@ int stb_debug_batch_gemm(stb_ctx *ctx, const float *q, uint32_t nq, const float 
   if (e == cudaSuccess && rc == STB_OK) e = cudaStreamSynchronize(ctx->stream);
   cudaFree(dq); cudaFree(dr); cudaFree(da); cudaFree(db); cudaFree(dfull); cudaFree(dsub); cudaFree(dtile); cudaFree(dbad);
   if (e != cudaSuccess) { stb_set_error("debug_batch_gemm: %s", cudaGetErrorString(e)); cudaGetLastError(); return STB_ERR_CUDA; }
+  return rc;
+}
+
+// ------------------------------------------------------------------- K1 debug hooks ---
+// The scan passes' per-row scores, for tests that check each pass's contract row by row (DESIGN.md section 5).
+static bool k1_copy_usable(const stb_corpus *c, int tier) {
+  if (tier == STB_TIER_Q8) return c->q8 && c->q4 && c->q8_rows == c->n && !c->q8_bad;
+  if (tier == STB_TIER_H16) return c->shadow && c->shadow_rows == c->n && !c->shadow_bad;
+  return true;
+}
+
+// Query and ranges staged like stb_search's; per-row device outputs: `floats` arrays of n f32 (NaN-filled) and one of
+// n u32 (zeroed), in one allocation that the caller frees.
+static int k1_debug_stage(stb_ctx *ctx, const stb_corpus *c, const char *what, const float *q, const uint64_t *row_ranges,
+                          uint32_t n_ranges, int floats, float **f_dev, unsigned int **u_dev, const uint64_t **ranges_dev,
+                          uint32_t *n_loc, uint64_t *n_virtual) {
+  int rc;
+  if ((rc = k1_upload_ranges(ctx, c, what, row_ranges, n_ranges, ranges_dev, n_loc, n_virtual)) != STB_OK) return rc;
+  memcpy(ctx->q_pin, q, STB_D * sizeof(float));
+  STB_CUDA(cudaMemcpyAsync(ctx->q_dev, ctx->q_pin, STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+  const size_t n = c->n;
+  void *p = nullptr;
+  if (cudaMalloc(&p, n * sizeof(float) * (floats + 1)) != cudaSuccess) {
+    cudaGetLastError();
+    stb_set_error("%s: cannot allocate the per-row outputs", what);
+    return STB_ERR_NOMEM;
+  }
+  *f_dev = (float *)p;
+  *u_dev = (unsigned int *)(*f_dev + n * floats);
+  STB_CUDA(cudaMemsetAsync(*f_dev, 0xff, n * sizeof(float) * floats, ctx->stream));
+  STB_CUDA(cudaMemsetAsync(*u_dev, 0, n * sizeof(unsigned int), ctx->stream));
+  return STB_OK;
+}
+
+int stb_debug_scan_scores(stb_ctx *ctx, const stb_corpus *corpus, int tier, const float *q, const uint64_t *row_ranges,
+                          uint32_t n_ranges, uint64_t cap, float *scores, uint32_t *seen, uint32_t *hist) {
+  int rc = ctx_use(ctx);
+  if (rc) return rc;
+  if (!corpus || !q || !scores || !seen || (n_ranges && !row_ranges)) { stb_set_error("debug_scan_scores: null argument"); return STB_ERR_ARG; }
+  if (corpus->ctx != ctx) { stb_set_error("debug_scan_scores: corpus belongs to another context"); return STB_ERR_ARG; }
+  if (tier < STB_TIER_F32 || tier > STB_TIER_Q8) { stb_set_error("debug_scan_scores: unknown tier %d", tier); return STB_ERR_ARG; }
+  if (hist && tier == STB_TIER_H16) { stb_set_error("debug_scan_scores: no histogram pass reads the 16-bit shadow"); return STB_ERR_ARG; }
+  if (cap < corpus->n) { stb_set_error("debug_scan_scores: outputs hold %llu rows, the corpus %llu", (unsigned long long)cap, (unsigned long long)corpus->n); return STB_ERR_ARG; }
+  if (!k1_copy_usable(corpus, tier)) { stb_set_error("debug_scan_scores: tier %d copy not built or unusable", tier); return STB_ERR_STATE; }
+  if (hist) memset(hist, 0, 4096 * sizeof(uint32_t));
+  if (corpus->n == 0) return STB_OK;
+  float *d_score = nullptr;
+  unsigned int *d_seen = nullptr;
+  const uint64_t *ranges_dev = nullptr;
+  uint32_t n_loc = 0;
+  uint64_t n_virtual = 0;
+  if ((rc = k1_debug_stage(ctx, corpus, "debug_scan_scores", q, row_ranges, n_ranges, 1, &d_score, &d_seen, &ranges_dev, &n_loc,
+                           &n_virtual)) == STB_OK && n_virtual) {
+    rc = stb_launch_debug_scan(ctx, corpus, tier, ctx->q_dev, ranges_dev, n_loc, n_virtual, d_score, d_seen);
+    if (rc == STB_OK && hist) rc = stb_launch_scan_hist(ctx, corpus, tier, ctx->q_dev, ranges_dev, n_loc, n_virtual, ctx->hist_dev);
+  }
+  cudaError_t e = cudaSuccess;
+  if (rc == STB_OK) e = cudaMemcpyAsync(scores, d_score, corpus->n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream);
+  if (rc == STB_OK && e == cudaSuccess) e = cudaMemcpyAsync(seen, d_seen, corpus->n * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream);
+  if (rc == STB_OK && e == cudaSuccess && hist && n_virtual)
+    e = cudaMemcpyAsync(hist, ctx->hist_dev, 4096 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+  cudaFree(d_score);
+  if (rc == STB_OK && e != cudaSuccess) { stb_set_error("debug_scan_scores: %s", cudaGetErrorString(e)); cudaGetLastError(); return STB_ERR_CUDA; }
+  return rc;
+}
+
+int stb_debug_q4_scan(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t top_k, const uint64_t *row_ranges,
+                      uint32_t n_ranges, int pin, uint64_t cap, float *u4, float *t, uint32_t *refined, float *u8, float *l8,
+                      uint64_t *words) {
+  int rc = ctx_use(ctx);
+  if (rc) return rc;
+  if (!corpus || !q || !u4 || !t || !refined || !u8 || !l8 || !words || (n_ranges && !row_ranges)) {
+    stb_set_error("debug_q4_scan: null argument");
+    return STB_ERR_ARG;
+  }
+  if (corpus->ctx != ctx) { stb_set_error("debug_q4_scan: corpus belongs to another context"); return STB_ERR_ARG; }
+  if (top_k < 1 || top_k > STB_Q8_MAX_K) { stb_set_error("debug_q4_scan: top_k must be 1..%d", STB_Q8_MAX_K); return STB_ERR_ARG; }
+  if (cap < corpus->n) { stb_set_error("debug_q4_scan: outputs hold %llu rows, the corpus %llu", (unsigned long long)cap, (unsigned long long)corpus->n); return STB_ERR_ARG; }
+  if (!k1_copy_usable(corpus, STB_TIER_Q8)) { stb_set_error("debug_q4_scan: q8 copy not built or unusable"); return STB_ERR_STATE; }
+  memset(words, 0, top_k * sizeof(uint64_t));
+  if (corpus->n == 0) return STB_OK;
+  const size_t n = corpus->n;
+  float *d_f = nullptr;
+  unsigned int *d_seen = nullptr;
+  unsigned long long *d_words = nullptr;
+  const uint64_t *ranges_dev = nullptr;
+  uint32_t n_loc = 0;
+  uint64_t n_virtual = 0;
+  rc = k1_debug_stage(ctx, corpus, "debug_q4_scan", q, row_ranges, n_ranges, 4, &d_f, &d_seen, &ranges_dev, &n_loc, &n_virtual);
+  cudaError_t e = cudaSuccess;
+  if (rc == STB_OK) {
+    e = cudaMalloc(&d_words, (STB_Q4_WORDS + 1) * sizeof(unsigned long long));   // the words, then the refined counter
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_words, 0, (STB_Q4_WORDS + 1) * sizeof(unsigned long long), ctx->stream);
+  }
+  if (rc == STB_OK && e == cudaSuccess && n_virtual)
+    rc = stb_launch_debug_q4(ctx, corpus, ctx->q_dev, top_k, ranges_dev, n_loc, n_virtual, d_words, d_words + STB_Q4_WORDS, pin,
+                             d_f, d_f + n, d_f + 2 * n, d_f + 3 * n, d_seen);
+  float *outs[4] = {u4, t, l8, u8};
+  for (int i = 0; i < 4 && rc == STB_OK && e == cudaSuccess; ++i)
+    e = cudaMemcpyAsync(outs[i], d_f + i * n, n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream);
+  if (rc == STB_OK && e == cudaSuccess) e = cudaMemcpyAsync(refined, d_seen, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream);
+  if (rc == STB_OK && e == cudaSuccess) e = cudaMemcpyAsync(words, d_words, top_k * sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+  cudaFree(d_f);
+  cudaFree(d_words);
+  if (rc == STB_OK && e != cudaSuccess) { stb_set_error("debug_q4_scan: %s", cudaGetErrorString(e)); cudaGetLastError(); return STB_ERR_CUDA; }
   return rc;
 }
 

@@ -341,6 +341,15 @@ int stb_launch_scan_collect(stb_ctx *ctx, const stb_corpus *c, int tier,
 // (bin b: cos in (1-(b+1)/2048, 1-b/2048]).  hist_dev: 4096 u32 on device.
 int stb_launch_scan_hist(stb_ctx *ctx, const stb_corpus *c, int tier, const float *q_dev, const uint64_t *ranges_dev,
                          uint32_t n_ranges, uint64_t n_virtual, unsigned int *hist_dev);
+// Test hooks (stb_debug_scan_scores, stb_debug_q4_scan): the f32 / h16 / q8 pass, or the q8 tier's prefiltered
+// top-k scan, with a sink that stores each scanned local row's score into score[row] and counts it in seen[row].
+// The q4 form also stores u4 and T per row and l8 per refined row (pin != 0: T held at -inf); words: top_k
+// threshold words (zeroed; tag 1), refined: a zeroed counter.
+int stb_launch_debug_scan(stb_ctx *ctx, const stb_corpus *c, int tier, const float *q_dev, const uint64_t *ranges_dev,
+                          uint32_t n_ranges, uint64_t n_virtual, float *score, unsigned int *seen);
+int stb_launch_debug_q4(stb_ctx *ctx, const stb_corpus *c, const float *q_dev, uint32_t top_k, const uint64_t *ranges_dev,
+                        uint32_t n_ranges, uint64_t n_virtual, unsigned long long *words, unsigned long long *refined,
+                        int pin, float *u4, float *t, float *l8, float *u8, unsigned int *seen);
 // Exact canonical distances of m collected rows -> hits (invalid/failing rows get
 // distance=+inf,row=UINT64_MAX); counts passing rows into pass_count.
 int stb_launch_exact(stb_ctx *ctx, const float *rows, uint64_t row_base,

@@ -525,9 +525,17 @@ __device__ __forceinline__ int stb_dp4a_us(uint32_t a, uint32_t b, int c) {
   return d;
 }
 
-template <int U, int RANGES, class Sink>
+// Test hook (stb_debug_q4_scan, DUMP = 1): per local row, the u4 and the T it was tested against, and for refined
+// rows the l8 before stb_f2ord; pin != 0 holds T at -inf, so every row is refined.
+struct StbQ4Dump {
+  float *u4, *t, *l8;
+  int pin;
+};
+
+template <int U, int RANGES, int DUMP = 0, class Sink>
 __device__ __forceinline__ void stb_scan_q4(const ScanArgs &args, const uint8_t *q8, const float *q8_scale, const StbQ4Args &q4a,
-                                            uint32_t *wq, uint32_t *pw, Sink &sink, const uint32_t *off = nullptr) {
+                                            uint32_t *wq, uint32_t *pw, Sink &sink, const uint32_t *off = nullptr,
+                                            const StbQ4Dump *dump = nullptr) {
   static_assert(4 * U == STB_Q4_TILE_ROWS && STB_Q8_MAX_K <= 32, "one plane tile per warp tile, one row per lane; one lane per threshold word");
   const int lane = threadIdx.x & 31;
   const int g = lane >> 3;   // refine: row group inside the warp
@@ -599,7 +607,11 @@ __device__ __forceinline__ void stb_scan_q4(const ScanArgs &args, const uint8_t 
     if (Q.unusable) return;
     // publish the lower bounds that beat the published value of their word (rare after the first tickets);
     // the warp learns its own contributions with the next read
-    const unsigned o8 = stb_f2ord(fmaf(sc, fmaf((float)d, Q.inv_S, -Q.h_l1), -Q.e_q) - (float)STB_Q8_SCAN_EPS);
+    const float l8 = fmaf(sc, fmaf((float)d, Q.inv_S, -Q.h_l1), -Q.e_q) - (float)STB_Q8_SCAN_EPS;
+    if constexpr (DUMP) {
+      if (v) dump->l8[r] = l8;
+    }
+    const unsigned o8 = stb_f2ord(l8);
     const int w = (int)(r % (uint32_t)kw);
     const unsigned known = __shfl_sync(0xffffffffu, tcache, w);   // every lane takes part in the shuffle
     if (v && o8 > known) atomicMax(q4a.thr + w, ((unsigned long long)q4a.tag << 32) | o8);
@@ -649,6 +661,10 @@ __device__ __forceinline__ void stb_scan_q4(const ScanArgs &args, const uint8_t 
     }
     const int D = (lh + (hh >> 4)) * 256 + (ll + (hl >> 4)) - 8 * sumq;   // q16 . h (hh, hl: multiples of 16)
     const float u4 = fmaf(sr.x, fmaf((float)D, A, B), sr.y + e_q4);
+    if constexpr (DUMP) {
+      if (dump->pin) T = -CUDART_INF_F;
+      if (valid) { dump->u4[row] = u4; dump->t[row] = T; }
+    }
     // an unusable query publishes no bound (refine), so T stays -inf and every valid row is queued
     const bool want = valid && !(u4 + (float)STB_Q4_SKIP_EPS < T);
     const unsigned mk = __ballot_sync(0xffffffffu, want);
@@ -1501,6 +1517,104 @@ int stb_launch_scan_hist(stb_ctx *ctx, const stb_corpus *c, int tier, const floa
     stb_scan_hist_kernel<STB_SCAN_U, true><<<(unsigned)grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, hist_dev, nullptr, nullptr);
   else
     stb_scan_hist_kernel<STB_SCAN_U, false><<<(unsigned)grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, hist_dev, nullptr, nullptr);
+  STB_CUDA(cudaGetLastError());
+  ctx->kernel_launches++;
+  return STB_OK;
+}
+
+// ------------------------------------------------------------------- test hooks ---
+// stb_debug_scan_scores / stb_debug_q4_scan (api.cu): the production passes with a sink that records, per local
+// row, the score the pass handed it and how many times.  Static warp-strided schedule, like the histogram pass.
+struct DumpSink {
+  float *score;
+  unsigned int *seen;
+  template <int ROWS>
+  __device__ __forceinline__ void consume(float s, uint32_t r) {
+    if (s != -CUDART_INF_F) {   // -inf marks lanes that carry no row; a NaN score is recorded
+      score[r] = s;
+      atomicAdd(seen + r, 1u);
+    }
+  }
+};
+
+template <int U, bool RANGES, int SRC>
+__global__ void __launch_bounds__(STB_SCAN_THREADS, STB_SCAN_MINB)
+stb_debug_scan_kernel(const ScanArgs scan, const uint8_t *shadow, const uint8_t *q8, const float *q8_scale, DumpSink sink) {
+  if constexpr (SRC == 2) stb_scan_q8<U, RANGES>(scan, q8, q8_scale, sink);
+  else if constexpr (SRC == 1) stb_scan_shadow<U, RANGES>(scan, shadow, sink);
+  else stb_scan_rows<U, RANGES>(scan, sink);
+}
+
+static ScanArgs stb_debug_scan_args(const stb_corpus *c, const float *q_dev, const uint64_t *ranges_dev, uint32_t n_ranges,
+                                    uint64_t n_virtual) {
+  ScanArgs a;
+  a.rows = reinterpret_cast<const float4 *>(c->rows);
+  a.n_virtual = n_virtual;
+  a.q = q_dev;
+  a.vstart = ranges_dev;
+  a.rbegin = ranges_dev ? ranges_dev + (n_ranges + 1) : nullptr;
+  a.n_ranges = n_ranges;
+  a.tickets = nullptr; a.t_base = 0; a.t_bulk = 0;
+  return a;
+}
+
+static unsigned stb_debug_grid(const stb_ctx *ctx, uint64_t n_virtual, int u) {
+  const uint64_t tiles = (n_virtual + 4 * u - 1) / (4 * u);
+  const uint64_t want = (tiles + STB_SCAN_WARPS - 1) / STB_SCAN_WARPS;
+  const uint64_t grid = (uint64_t)ctx->sm_count * STB_SCAN_MINB;
+  return (unsigned)(want < grid ? (want < 1 ? 1 : want) : grid);
+}
+
+int stb_launch_debug_scan(stb_ctx *ctx, const stb_corpus *c, int tier, const float *q_dev, const uint64_t *ranges_dev,
+                          uint32_t n_ranges, uint64_t n_virtual, float *score, unsigned int *seen) {
+  const ScanArgs a = stb_debug_scan_args(c, q_dev, ranges_dev, n_ranges, n_virtual);
+  const DumpSink sink{score, seen};
+  const bool r = n_ranges > 0;
+  if (tier == STB_TIER_Q8) {
+    const unsigned grid = stb_debug_grid(ctx, n_virtual, STB_Q8_SCAN_U);
+    if (r) stb_debug_scan_kernel<STB_Q8_SCAN_U, true, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, nullptr, c->q8, c->q8_scale, sink);
+    else stb_debug_scan_kernel<STB_Q8_SCAN_U, false, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, nullptr, c->q8, c->q8_scale, sink);
+  } else if (tier == STB_TIER_H16) {
+    const unsigned grid = stb_debug_grid(ctx, n_virtual, STB_SHADOW_SCAN_U);
+    if (r) stb_debug_scan_kernel<STB_SHADOW_SCAN_U, true, 1><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, c->shadow, nullptr, nullptr, sink);
+    else stb_debug_scan_kernel<STB_SHADOW_SCAN_U, false, 1><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, c->shadow, nullptr, nullptr, sink);
+  } else {
+    const unsigned grid = stb_debug_grid(ctx, n_virtual, STB_SCAN_U);
+    if (r) stb_debug_scan_kernel<STB_SCAN_U, true, 0><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, nullptr, nullptr, nullptr, sink);
+    else stb_debug_scan_kernel<STB_SCAN_U, false, 0><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, nullptr, nullptr, nullptr, sink);
+  }
+  STB_CUDA(cudaGetLastError());
+  ctx->kernel_launches++;
+  return STB_OK;
+}
+
+// stb_scan_q4 with DUMP = 1; its queues live in static shared memory (the top-k kernel lends them its re-rank area)
+template <bool RANGES>
+__global__ void __launch_bounds__(STB_SCAN_THREADS, STB_SCAN_MINB)
+stb_debug_q4_kernel(const ScanArgs scan, const uint8_t *q8, const float *q8_scale, const StbQ4Args q4a, DumpSink sink,
+                    const StbQ4Dump dump) {
+  __shared__ __align__(16) uint32_t s_scratch[STB_SCAN_WARPS * (STB_Q4_QUEUE + 256)];
+  uint32_t *scratch = s_scratch + (threadIdx.x >> 5) * (STB_Q4_QUEUE + 256);
+  DumpSink s = sink;
+  stb_scan_q4<STB_Q4_SCAN_U, RANGES, 1>(scan, q8, q8_scale, q4a, scratch, scratch + STB_Q4_QUEUE, s, nullptr, &dump);
+}
+
+int stb_launch_debug_q4(stb_ctx *ctx, const stb_corpus *c, const float *q_dev, uint32_t top_k, const uint64_t *ranges_dev,
+                        uint32_t n_ranges, uint64_t n_virtual, unsigned long long *words, unsigned long long *refined,
+                        int pin, float *u4, float *t, float *l8, float *u8, unsigned int *seen) {
+  const ScanArgs a = stb_debug_scan_args(c, q_dev, ranges_dev, n_ranges, n_virtual);
+  StbQ4Args q4a;
+  q4a.plane = c->q4;
+  q4a.sr = c->q4_sr;
+  q4a.thr = words;
+  q4a.tag = 1u;
+  q4a.top_k = top_k;
+  q4a.refined = refined;
+  const DumpSink sink{u8, seen};
+  const StbQ4Dump dump{u4, t, l8, pin};
+  const unsigned grid = stb_debug_grid(ctx, n_virtual, STB_Q4_SCAN_U);
+  if (n_ranges > 0) stb_debug_q4_kernel<true><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, c->q8, c->q8_scale, q4a, sink, dump);
+  else stb_debug_q4_kernel<false><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, c->q8, c->q8_scale, q4a, sink, dump);
   STB_CUDA(cudaGetLastError());
   ctx->kernel_launches++;
   return STB_OK;
