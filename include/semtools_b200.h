@@ -319,6 +319,32 @@ int stb_search_batch_filtered(stb_ctx *ctx, const stb_corpus *corpus, const floa
                               uint32_t top_k, int has_max, double max_distance,
                               const uint64_t *row_ranges, uint32_t n_ranges,
                               stb_hit *out_hits, uint32_t *out_n);
+/* The workspace query for a batch in which every query names its own subset (an agent host's tool calls, a
+ * server over one workspace): for every query i, out_hits[i*top_k ..] and out_n[i] equal, bit for bit, what
+ *   stb_search(ctx, corpus, q_i, top_k, has_max, max_distance, STB_MODE_STORE_QUERY,
+ *              row_ranges + 2*range_offsets[i], range_offsets[i+1] - range_offsets[i], ...)
+ * returns (unused tail: +inf / UINT64_MAX).
+ *   range_offsets  nq + 1 entries, range_offsets[0] = 0, non-decreasing: query i's ranges are
+ *                  row_ranges[2*range_offsets[i] .. 2*range_offsets[i+1]), GLOBAL [begin, end) pairs clipped to the
+ *                  shard.  A query with zero ranges has the empty subset and 0 hits; there is no NULL meaning "every
+ *                  row" (pass the shard's own range for that).
+ * Refused before anything is written: range_offsets[0] != 0, decreasing offsets, or row_ranges == NULL with
+ * range_offsets[nq] > 0 (STB_ERR_ARG); a query's ranges that stb_search refuses (the same status).  nq == 0 is a
+ * no-op; top_k == 0 sets every count to 0.  Host-rows corpora are served as stb_search_batch_filtered serves them.
+ * Queries whose clipped ranges are identical form one group.  One group for the whole batch is exactly
+ * stb_search_batch_filtered on it (route 3 or 4).  Otherwise (route 6) every group whose v2 plan fits over its
+ * listed tiles (top_k <= 64) runs on the tensor cores, each in whole 64-query halves of the query tiles, with
+ * one sampling pass and one emitting pass for all of them; K1 (stb_search, with the query's own ranges)
+ * answers the other groups and every query the tensor passes leave unproven.  Extra device memory, in context
+ * scratch that grows on demand: one eligible-row bitmap per tensor group (N/8 bytes each, whose 8-word slices
+ * are the mask slots a work item names; 64 bytes of mask words reach shared memory per item), the two passes'
+ * work lists (16 bytes per (corpus tile, query tile) item, 4 per listed tile and per CTA), the queries in slot
+ * order (1 KiB per slot, 64 slots per half), and the per-group sample, laid out [query tile][largest
+ * n_sample][128 queries]. */
+int stb_search_batch_subsets(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t nq,
+                             uint32_t top_k, int has_max, double max_distance,
+                             const uint64_t *range_offsets, const uint64_t *row_ranges,
+                             stb_hit *out_hits, uint32_t *out_n);
 /* Threshold mode of search_documents (src/search/mod.rs:88-89,115-116) for a batch: for every query i,
  * out_hits[out_offsets[i] .. out_offsets[i+1]) equals, bit for bit, the hits of
  *   stb_search(ctx, corpus, q_i, 0, 1, max_distance, STB_MODE_SEARCH_DOCUMENTS, NULL, 0, ...)
@@ -650,13 +676,17 @@ int stb_debug_ivfpq_export(const stb_ivfpq *index, float *centroids, float *code
  * i >= nq. */
 int stb_debug_ivfpq_batch_last(const stb_ivfpq *index, uint32_t i, uint32_t info[4], float *coarse,
                                uint32_t *probe, float *lut);
-/* Test hook for K2: describes the most recent stb_search_batch_dev, stb_search_batch_filtered or
- * stb_search_batch_threshold on ctx (synchronises the stream).  info = {route, nq, a, b, n_seg, seg_cap}; route
- * 1 = v1, 2 = v2, 3 = filtered v2, 4 = a filtered call that launched nothing on the tensor cores (K1 answered it,
- * or nothing could be returned), 5 = threshold mode, 0 = none yet.  Slots 2-3 (a, b):
+/* Test hook for K2: describes the most recent stb_search_batch_dev, stb_search_batch_filtered,
+ * stb_search_batch_subsets or stb_search_batch_threshold on ctx (synchronises the stream).  info = {route, nq, a,
+ * b, n_seg, seg_cap}; route 1 = v1, 2 = v2, 3 = filtered v2, 4 = a filtered call that launched nothing on the
+ * tensor cores (K1 answered it, or nothing could be returned), 5 = threshold mode, 6 = one filter per query
+ * group, 0 = none yet.  Slots 2-3 (a, b):
  *   routes 1-4: n_sample, stride -- v2's sampled tiles (0, stride, 2*stride, ...; after route 3 they count listed
  *               tiles, the tiles holding an eligible row, in ascending order); 0 after routes 1 and 4;
- *   route 5:    the queries re-emitted by the second tensor pass, and the queries stb_search answered.
+ *   route 5:    the queries re-emitted by the second tensor pass, and the queries stb_search answered;
+ *   route 6:    the groups that ran on the tensor cores, and the queries stb_search answered.  After a route 6
+ *               call that ran the tensor passes, thr and cand_cnt are in caller query order; a query those
+ *               passes did not take has threshold +inf and zero counts.
  * n_seg and seg_cap are the emitting grid and the first pass's per-(query, CTA) key capacity, 0 after routes 1
  * and 4 and after a route 5 call that launched nothing.  After routes 2, 3 and a route 5 call that ran the
  * tensor pass, thr (may be NULL) receives the nq emission thresholds and cand_cnt (may be NULL) the raw

@@ -25,7 +25,7 @@ SYMBOLS = [
     "stb_corpus_rows", "stb_corpus_data_dev", "stb_corpus_read", "stb_corpus_update", "stb_corpus_remove", "stb_embed", "stb_embed_dev",
     "stb_embed_status", "stb_search",
     "stb_search_topk_dev", "stb_corpus_prepare", "stb_corpus_tier_stats", "stb_corpus_prepare_batch", "stb_search_batch", "stb_search_batch_dev",
-    "stb_search_batch_filtered", "stb_search_batch_threshold",
+    "stb_search_batch_filtered", "stb_search_batch_subsets", "stb_search_batch_threshold",
     "stb_xchg_create", "stb_xchg_destroy", "stb_xchg_local_handle",
     "stb_xchg_connect", "stb_xchg_connect_local", "stb_search_topk_xchg", "stb_search_xchg", "stb_search_many", "stb_xchg_create_batch", "stb_search_batch_xchg_dev", "stb_ivfpq_build",
     "stb_ivfpq_destroy", "stb_ivfpq_extend", "stb_ivfpq_stats", "stb_ivfpq_search", "stb_ivfpq_search_dev", "stb_hits_merge_dev", "stb_hits_merge_batch_dev", "stb_hits_merge", "stb_fnv1a64", "stb_line_id", "stb_line_ids",
@@ -100,6 +100,7 @@ def lib() -> C.CDLL:
     L.stb_search_batch.argtypes = [vp, vp, vp, u32, u32, vp, vp]
     L.stb_search_batch_dev.argtypes = [vp, vp, vp, u32, u32, vp, vp]
     L.stb_search_batch_filtered.argtypes = [vp, vp, vp, u32, u32, i32, f64, vp, u32, vp, vp]
+    L.stb_search_batch_subsets.argtypes = [vp, vp, vp, u32, u32, i32, f64, vp, vp, vp, vp]
     L.stb_search_batch_threshold.argtypes = [vp, vp, vp, u32, f64, vp, u64, vp]
     L.stb_xchg_create.argtypes = [vp, u32, u32, u32, C.POINTER(vp)]
     L.stb_xchg_destroy.argtypes = [vp]
@@ -234,15 +235,17 @@ class Context:
 
     def batch_last(self):
         """stb_debug_batch_last: the most recent K2 device call on this context.  Returns a dict with
-        route (1 = v1, 2 = v2, 3 = filtered v2, 4 = filtered without the tensor cores, 5 = threshold mode), nq,
-        n_sample, stride (routes 1-4) or retried, k1 (route 5: queries re-emitted by the second tensor pass /
-        answered by stb_search), n_seg, seg_cap and, after v2 (filtered or not) and a route 5 call that ran the
-        tensor pass, thr [nq] (f32) and cand_cnt [nq][n_seg] (raw counts; > seg_cap marks an overflowed segment)."""
+        route (1 = v1, 2 = v2, 3 = filtered v2, 4 = filtered without the tensor cores, 5 = threshold mode, 6 = one
+        filter per query group), nq, n_sample, stride (routes 1-4) or retried, k1 (route 5: queries re-emitted by the
+        second tensor pass / answered by stb_search) or groups, k1 (route 6: groups on the tensor cores / queries
+        answered by stb_search), n_seg, seg_cap and, after v2 (filtered or not) and a route 5 or 6 call that ran the
+        tensor passes, thr [nq] (f32) and cand_cnt [nq][n_seg] (raw counts; > seg_cap marks an overflowed segment;
+        route 6: caller order, +inf and zeros for a query the tensor passes did not take)."""
         info = np.zeros(6, dtype=np.uint32)
         _check(lib().stb_debug_batch_last(self._h, _np_ptr(info), None, None))
-        names = ("retried", "k1") if info[0] == 5 else ("n_sample", "stride")
+        names = {5: ("retried", "k1"), 6: ("groups", "k1")}.get(int(info[0]), ("n_sample", "stride"))
         out = dict(zip(("route", "nq") + names + ("n_seg", "seg_cap"), (int(v) for v in info)))
-        if out["route"] in (2, 3) or (out["route"] == 5 and out["n_seg"]):
+        if out["route"] in (2, 3) or (out["route"] in (5, 6) and out["n_seg"]):
             thr = np.zeros(max(out["nq"], 1), dtype=np.float32)
             cnt = np.zeros((max(out["nq"], 1), max(out["n_seg"], 1)), dtype=np.uint32)
             _check(lib().stb_debug_batch_last(self._h, _np_ptr(info), _np_ptr(thr), _np_ptr(cnt)))
@@ -506,6 +509,29 @@ class Corpus:
         _check(lib().stb_search_batch_filtered(self.ctx._h, self._h, _np_ptr(queries), nq, top_k,
                                                int(max_distance is not None), float(max_distance or 0.0),
                                                _np_ptr(rr), n_rr, _np_ptr(out), _np_ptr(cnt)))
+        return [out[i, : cnt[i]] for i in range(nq)]
+
+    def search_batch_subsets(self, queries, ranges_per_query, top_k: int = 10, max_distance: float | None = None):
+        """stb_search_batch_subsets: for each query i, what search(queries[i], top_k, max_distance,
+        STB_MODE_STORE_QUERY, ranges_per_query[i]) returns (each an (n, 2) array of global [begin, end) pairs;
+        n = 0 is the empty subset).  Returns a list of HIT_DTYPE arrays, one per query."""
+        queries = np.ascontiguousarray(queries, dtype=np.float32)
+        if queries.ndim != 2 or queries.shape[1] != STB_DIM:
+            raise StbError(STB_ERR_ARG, f"queries must be (nq,{STB_DIM}) f32")
+        nq = queries.shape[0]
+        if len(ranges_per_query) != nq:
+            raise StbError(STB_ERR_ARG, f"{len(ranges_per_query)} range lists for {nq} queries")
+        parts = [np.asarray(r, dtype=np.uint64).reshape(-1, 2) for r in ranges_per_query]
+        offsets = np.zeros(nq + 1, dtype=np.uint64)
+        offsets[1:] = np.cumsum([len(p) for p in parts]) if nq else []
+        rr = np.ascontiguousarray(np.concatenate(parts) if parts else np.zeros((0, 2), np.uint64), dtype=np.uint64)
+        if len(rr) == 0:
+            rr = np.zeros((1, 2), dtype=np.uint64)
+        out = np.zeros((nq, max(top_k, 1)), dtype=HIT_DTYPE)
+        cnt = np.zeros(max(nq, 1), dtype=np.uint32)
+        _check(lib().stb_search_batch_subsets(self.ctx._h, self._h, _np_ptr(queries), nq, top_k,
+                                              int(max_distance is not None), float(max_distance or 0.0),
+                                              _np_ptr(offsets), _np_ptr(rr), _np_ptr(out), _np_ptr(cnt)))
         return [out[i, : cnt[i]] for i in range(nq)]
 
     def search_batch_threshold(self, queries, max_distance: float, cap: int | None = None):

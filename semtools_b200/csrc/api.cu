@@ -7,9 +7,11 @@
 
 #include <algorithm>
 #include <cmath>
+#include <map>
 #include <memory>
 #include <mutex>
 #include <new>
+#include <unordered_map>
 #include <unordered_set>
 #include <vector>
 
@@ -166,6 +168,7 @@ int stb_ctx_destroy(stb_ctx *c) {
   cudaFree(c->hist_dev); cudaFree(c->bq_tiles); cudaFree(c->b_submax); cudaFree(c->b_tilemax); cudaFree(c->b_cand);
   cudaFree(c->b_thr); cudaFree(c->b_cnt); cudaFree(c->b_keys); cudaFree(c->b_qbad);
   cudaFree(c->b_franges); cudaFree(c->b_ftiles); cudaFree(c->b_fbits);
+  cudaFree(c->s_work); cudaFree(c->s_qslots); cudaFree(c->s_qbad); free(c->s_map);
   cudaFree(c->t_dst); cudaFree(c->t_segoff); cudaFree(c->t_cur); cudaFree(c->t_rq); cudaFree(c->t_rthr);
   cudaFree(c->t_buf); cudaFree(c->t_off); cudaFree(c->t_slot); cudaFree(c->t_out_at); cudaFree(c->t_hits);
   cudaFree(c->t_sort_tmp);
@@ -1677,6 +1680,285 @@ int stb_search_batch_filtered(stb_ctx *ctx, const stb_corpus *corpus_c, const fl
 
 }  // extern "C"
 
+// ---- one filter per query for a batch (stb_search_batch_subsets, route 6) -----------------------------------
+// The work list of one pass: for every corpus tile some tensor group covers (ascending), the query tiles that
+// meet it, each with the mask slot of both 64-query halves (zero_slot: the half's group does not cover the
+// tile) and, sampling, the half's column of its group's sample.  A group's halves are consecutive, so walking
+// groups in order yields every tile's query tiles in ascending order, and at most two halves share one.
+struct SubsetsWork {
+  std::vector<uint32_t> tiles, item_off, cta_tiles;
+  std::vector<uint4> items;
+};
+static void subsets_work(const std::vector<std::vector<uint32_t>> &tiles_of, const std::vector<uint32_t> &half0,
+                         const std::vector<uint32_t> &n_halves, uint32_t n_tiles, bool sample, uint32_t zero_slot,
+                         uint32_t grid_cap, SubsetsWork *w) {
+  const uint32_t T = (uint32_t)tiles_of.size();
+  std::vector<uint32_t> off(n_tiles + 1, 0);
+  for (uint32_t g = 0; g < T; ++g)
+    for (uint32_t t : tiles_of[g]) off[t + 1]++;
+  for (uint32_t t = 0; t < n_tiles; ++t) off[t + 1] += off[t];
+  std::vector<uint32_t> grp(off[n_tiles]), col(off[n_tiles]), at(off.begin(), off.end() - 1);
+  for (uint32_t g = 0; g < T; ++g)
+    for (uint32_t j = 0; j < (uint32_t)tiles_of[g].size(); ++j) {
+      const uint32_t p = at[tiles_of[g][j]]++;
+      grp[p] = g;
+      col[p] = sample ? j : 0xffffu;
+    }
+  w->tiles.clear(); w->items.clear();
+  w->item_off.assign(1, 0);
+  for (uint32_t t = 0; t < n_tiles; ++t) {
+    if (off[t] == off[t + 1]) continue;
+    w->tiles.push_back(t);
+    const size_t first = w->items.size();
+    for (uint32_t p = off[t]; p < off[t + 1]; ++p) {
+      const uint32_t g = grp[p];
+      for (uint32_t H = half0[g]; H < half0[g] + n_halves[g]; ++H) {
+        if (w->items.size() == first || w->items.back().x != H / 2)
+          w->items.push_back(make_uint4(H / 2, zero_slot, zero_slot, 0xffffffffu));
+        uint4 &it = w->items.back();
+        const uint32_t slot = g * n_tiles + t;
+        if (H & 1) { it.z = slot; it.w = (it.w & 0xffffu) | (col[p] << 16); }
+        else { it.y = slot; it.w = (it.w & 0xffff0000u) | col[p]; }
+      }
+    }
+    w->item_off.push_back((uint32_t)w->items.size());
+  }
+  // CTAs take consecutive corpus tiles of equal work, a tile costing its items plus 2: reading the 128 KiB tile
+  // at an SM's share of HBM bandwidth takes about as long as two items' MMAs
+  const uint32_t n_union = (uint32_t)w->tiles.size();
+  const uint32_t grid = std::min(n_union, grid_cap);
+  const uint64_t total = (uint64_t)w->items.size() + 2ull * n_union;
+  w->cta_tiles.assign(1, 0);
+  uint64_t acc = 0;
+  for (uint32_t u = 0; u < n_union; ++u) {
+    while (w->cta_tiles.size() < grid && acc >= total * w->cta_tiles.size() / grid) w->cta_tiles.push_back(u);
+    acc += w->item_off[u + 1] - w->item_off[u] + 2;
+  }
+  while (w->cta_tiles.size() <= grid) w->cta_tiles.push_back(n_union);
+}
+
+extern "C" {
+
+// The store query for a batch in which every query names its own subset (route 6).  Queries whose clipped
+// ranges are identical form one group; one group for the whole batch is stb_search_batch_filtered's call.
+// Otherwise every group whose v2 plan fits runs on the tensor cores, each occupying whole 64-query halves of
+// the query slots: one sampling pass over the union of the groups' sampled tiles, the per-slot threshold, one
+// emitting pass over the union of their listed tiles, finish2 over the groups' queries in compact order.  K1
+// answers the other groups and every query the tensor passes leave unproven.
+int stb_search_batch_subsets(stb_ctx *ctx, const stb_corpus *corpus_c, const float *q, uint32_t nq, uint32_t top_k,
+                             int has_max, double max_distance, const uint64_t *range_offsets, const uint64_t *row_ranges,
+                             stb_hit *out_hits, uint32_t *out_n) {
+  int rc = ctx_use(ctx);
+  if (rc) return rc;
+  stb_corpus *corpus = const_cast<stb_corpus *>(corpus_c);
+  if (!corpus) { stb_set_error("search_batch_subsets: null corpus"); return STB_ERR_ARG; }
+  if (corpus->ctx != ctx) { stb_set_error("search_batch_subsets: corpus belongs to another context"); return STB_ERR_ARG; }
+  if (nq == 0) return STB_OK;
+  if (!range_offsets || !q || !out_n || (top_k && !out_hits)) { stb_set_error("search_batch_subsets: null argument"); return STB_ERR_ARG; }
+  if (range_offsets[0] != 0) { stb_set_error("search_batch_subsets: range_offsets[0] must be 0"); return STB_ERR_ARG; }
+  for (uint32_t i = 0; i < nq; ++i)
+    if (range_offsets[i + 1] < range_offsets[i] || range_offsets[i + 1] - range_offsets[i] > UINT32_MAX) {
+      stb_set_error("search_batch_subsets: range_offsets decrease (or exceed 2^32 - 1 ranges) at query %u", i);
+      return STB_ERR_ARG;
+    }
+  if (range_offsets[nq] && !row_ranges) { stb_set_error("search_batch_subsets: row_ranges is null"); return STB_ERR_ARG; }
+  auto n_of = [&](uint32_t i) { return (uint32_t)(range_offsets[i + 1] - range_offsets[i]); };
+  auto ranges_of = [&](uint32_t i) { return row_ranges + 2 * range_offsets[i]; };
+  auto pad = [&](uint32_t i, uint64_t n) {
+    for (uint64_t j = n; j < top_k; ++j) { out_hits[(size_t)i * top_k + j].distance = INFINITY; out_hits[(size_t)i * top_k + j].row = 0xffffffffffffffffull; }
+  };
+  // clip every query's ranges as stb_search would (its refusals come before anything is written); a query with
+  // no clipped range has 0 hits (store.rs:489-491, or no row of this shard), the others are grouped
+  constexpr uint32_t kNone = 0xffffffffu;
+  std::map<std::vector<uint32_t>, uint32_t> ids;
+  std::vector<const std::vector<uint32_t> *> lists;       // group -> clipped local [begin, end) pairs
+  std::vector<uint32_t> group(nq, kNone);
+  if (top_k && corpus->n) {
+    std::vector<uint32_t> loc;
+    // a range list given again (byte for byte) has the first one's status and group: each distinct list is
+    // validated and clipped once (queries: those that clipped it, by a fingerprint of count and end points)
+    std::unordered_map<uint64_t, std::vector<uint32_t>> clipped;
+    for (uint32_t i = 0; i < nq; ++i) {
+      const uint32_t n = n_of(i);
+      if (n == 0) continue;
+      const uint64_t *r = ranges_of(i);
+      const uint64_t fp = (uint64_t)n * 0x9e3779b97f4a7c15ull ^ r[0] ^ (r[2 * (size_t)n - 1] << 1) ^ (r[n] << 2);
+      std::vector<uint32_t> &same = clipped[fp];
+      auto j = std::find_if(same.begin(), same.end(), [&](uint32_t j) {
+        return n_of(j) == n && memcmp(ranges_of(j), r, 2 * (size_t)n * sizeof(uint64_t)) == 0;
+      });
+      if (j != same.end()) { group[i] = group[*j]; continue; }
+      same.push_back(i);
+      loc.clear();
+      if ((rc = stb_clip_ranges("search_batch_subsets", ranges_of(i), n_of(i), corpus->row_base, corpus->n,
+                                [&](uint64_t b, uint64_t e) { loc.push_back((uint32_t)b); loc.push_back((uint32_t)e); })) != STB_OK)
+        return rc;
+      if (loc.empty()) continue;
+      auto it = ids.find(loc);                             // a new key is copied only once
+      if (it == ids.end()) {
+        it = ids.emplace(loc, (uint32_t)lists.size()).first;
+        lists.push_back(&it->first);
+      }
+      group[i] = it->second;
+    }
+  }
+  const uint32_t G = (uint32_t)lists.size();
+  if (G == 1 && std::find(group.begin(), group.end(), kNone) == group.end())
+    return stb_search_batch_filtered(ctx, corpus, q, nq, top_k, has_max, max_distance, ranges_of(0), n_of(0), out_hits, out_n);
+  uint32_t last[6] = {6u, nq, 0u, 0u, 0u, 0u};
+  memcpy(ctx->b_last, last, sizeof(last));
+  // the plan of every group; groups whose plan fits run on the tensor cores (tensor group tg = tensor[g])
+  const uint32_t n_tiles = (uint32_t)((corpus->n + 255) / 256);
+  std::vector<std::vector<uint32_t>> listed(G);
+  std::vector<BatchV2Plan> plan(G);
+  std::vector<uint32_t> tensor(G, kNone), tgroups;
+  for (uint32_t g = 0; g < G; ++g) {
+    const std::vector<uint32_t> &loc = *lists[g];
+    for (size_t r = 0; r < loc.size(); r += 2)
+      for (uint32_t t = loc[r] / 256; t <= (loc[r + 1] - 1) / 256; ++t)
+        if (listed[g].empty() || listed[g].back() < t) listed[g].push_back(t);
+    plan[g] = batch_v2_plan(ctx, (uint32_t)listed[g].size(), top_k);
+    if (plan[g].fits) tgroups.push_back(g);
+  }
+  if ((uint64_t)tgroups.size() * n_tiles >= UINT32_MAX) tgroups.clear();   // mask slots are 32-bit
+  if (!tgroups.empty()) {
+    rc = corpus_ensure_shadow(ctx, corpus);
+    if (rc == STB_ERR_STATE) tgroups.clear();              // un-normalisable rows: K1 answers every query
+    else if (rc != STB_OK) return rc;
+  }
+  const uint32_t T = (uint32_t)tgroups.size();
+  for (uint32_t tg = 0; tg < T; ++tg) tensor[tgroups[tg]] = tg;
+  // query slots: tensor group tg owns halves [half0[tg], half0[tg] + n_halves[tg]), its queries in caller order;
+  // row r of the compact order is query qrow[r]
+  std::vector<uint32_t> members(T, 0), half0(T), n_halves(T), row_of(nq, kNone), slot_of(nq, kNone), qrow;
+  for (uint32_t i = 0; i < nq; ++i)
+    if (group[i] != kNone && tensor[group[i]] != kNone) members[tensor[group[i]]]++;
+  uint32_t halves = 0;
+  for (uint32_t tg = 0; tg < T; ++tg) { half0[tg] = halves; n_halves[tg] = (members[tg] + 63) / 64; halves += n_halves[tg]; }
+  const uint32_t m_tiles = (halves + 1) / 2, q_pad = m_tiles * 128;
+  std::vector<uint32_t> slot_row(q_pad, kNone), fill(T, 0);
+  for (uint32_t i = 0; i < nq; ++i) {
+    if (group[i] == kNone || tensor[group[i]] == kNone) continue;
+    const uint32_t tg = tensor[group[i]], j = fill[tg]++;
+    slot_of[i] = half0[tg] * 64 + j;
+    row_of[i] = (uint32_t)qrow.size();
+    slot_row[slot_of[i]] = row_of[i];
+    qrow.push_back(i);
+  }
+  const uint32_t nt = (uint32_t)qrow.size();
+  std::vector<uint32_t> status((size_t)nt * 2, 0);
+  std::vector<stb_hit> hits((size_t)nt * top_k);
+  const uint32_t kSegCap = 64;                               // as batch_v2_run
+  uint32_t n_seg = 0;
+  if (T) {
+    std::vector<std::vector<uint32_t>> sampled(T), tiles_of(T);
+    uint32_t n_cols = 0;
+    for (uint32_t tg = 0; tg < T; ++tg) {
+      const uint32_t g = tgroups[tg];
+      for (uint32_t j = 0; j < plan[g].n_sample; ++j) sampled[tg].push_back(listed[g][(size_t)j * plan[g].stride]);
+      n_cols = std::max(n_cols, plan[g].n_sample);
+      tiles_of[tg] = std::move(listed[g]);
+    }
+    const uint32_t zero_slot = T * n_tiles;
+    SubsetsWork ws, we;
+    subsets_work(sampled, half0, n_halves, n_tiles, true, zero_slot, (uint32_t)ctx->sm_count, &ws);
+    subsets_work(tiles_of, half0, n_halves, n_tiles, false, zero_slot, (uint32_t)ctx->sm_count, &we);
+    n_seg = stb_batch_emit_grid(ctx, (uint32_t)we.tiles.size());
+    // one upload: items (16-byte aligned at the front), then the u32 arrays
+    std::vector<uint32_t> up;
+    auto put = [&](const void *p, size_t words) { const size_t o = up.size(); up.resize(o + words); memcpy(up.data() + o, p, words * 4); return o; };
+    const size_t o_is = put(ws.items.data(), 4 * ws.items.size()), o_ie = put(we.items.data(), 4 * we.items.size());
+    const size_t o_ts = put(ws.tiles.data(), ws.tiles.size()), o_os = put(ws.item_off.data(), ws.item_off.size());
+    const size_t o_cs = put(ws.cta_tiles.data(), ws.cta_tiles.size());
+    const size_t o_te = put(we.tiles.data(), we.tiles.size()), o_oe = put(we.item_off.data(), we.item_off.size());
+    const size_t o_ce = put(we.cta_tiles.data(), we.cta_tiles.size()), o_sr = put(slot_row.data(), slot_row.size());
+    // every tensor group's clipped ranges, back to back, for its bitmap
+    std::vector<uint32_t> rr, rr_off(T + 1, 0);
+    for (uint32_t tg = 0; tg < T; ++tg) {
+      const std::vector<uint32_t> &loc = *lists[tgroups[tg]];
+      rr.insert(rr.end(), loc.begin(), loc.end());
+      rr_off[tg + 1] = (uint32_t)rr.size();
+    }
+    const uint64_t n_words = (uint64_t)n_tiles * 8;
+    if ((rc = dev_reserve(&ctx->s_work, &ctx->s_work_cap, up.size())) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->b_franges, &ctx->b_franges_cap, rr.size(), 2048)) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->b_fbits, &ctx->b_fbits_cap, (size_t)(T * n_words + 8))) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->bq_dev, &ctx->bq_dev_cap, (size_t)nt * STB_D)) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->s_qslots, &ctx->s_qslots_cap, (size_t)q_pad * STB_D)) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->s_qbad, &ctx->s_qbad_cap, (size_t)nt)) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->b_qbad, &ctx->b_qbad_cap, (size_t)q_pad)) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->bq_tiles, &ctx->bq_tiles_cap, (size_t)q_pad * 512)) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->b_tilemax, &ctx->b_tilemax_cap, (size_t)n_cols * q_pad)) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->b_thr, &ctx->b_thr_cap, (size_t)q_pad)) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->b_cnt, &ctx->b_cnt_cap, (size_t)nt * n_seg)) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->b_keys, &ctx->b_keys_cap, (size_t)nt * n_seg * kSegCap)) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->bh_dev, &ctx->bh_dev_cap, (size_t)nt * top_k)) != STB_OK) return rc;
+    if ((rc = dev_reserve(&ctx->bs_dev, &ctx->bs_dev_cap, (size_t)nt * 2)) != STB_OK) return rc;
+    std::vector<float> qc((size_t)nt * STB_D);
+    for (uint32_t r = 0; r < nt; ++r) memcpy(qc.data() + (size_t)r * STB_D, q + (size_t)qrow[r] * STB_D, STB_D * sizeof(float));
+    STB_CUDA(cudaMemcpyAsync(ctx->s_work, up.data(), up.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+    STB_CUDA(cudaMemcpyAsync(ctx->b_franges, rr.data(), rr.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+    STB_CUDA(cudaMemcpyAsync(ctx->bq_dev, qc.data(), qc.size() * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    STB_CUDA(cudaMemsetAsync(ctx->b_fbits + T * n_words, 0, 8 * sizeof(uint32_t), ctx->stream));   // the zero slot
+    STB_CUDA(cudaMemsetAsync(ctx->b_cnt, 0, (size_t)nt * n_seg * sizeof(uint32_t), ctx->stream));
+    STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
+    for (uint32_t tg = 0; tg < T; ++tg)
+      if ((rc = stb_launch_row_bitmap(ctx, ctx->b_franges + rr_off[tg], (rr_off[tg + 1] - rr_off[tg]) / 2, n_words,
+                                      ctx->b_fbits + tg * n_words)) != STB_OK) return rc;
+    const uint32_t *W = ctx->s_work;
+    const uint32_t *d_slot_row = W + o_sr;
+    if ((rc = stb_launch_batch_slots_gather(ctx, ctx->bq_dev, d_slot_row, q_pad, ctx->s_qslots)) != STB_OK) return rc;
+    if ((rc = stb_launch_shadow_build(ctx, ctx->s_qslots, q_pad, 128, ctx->bq_tiles, ctx->err_flag, 0, ctx->b_qbad)) != STB_OK) return rc;
+    if ((rc = stb_launch_batch_slots_prep(ctx, d_slot_row, ctx->b_qbad, q_pad, ctx->s_qbad, ctx->b_tilemax,
+                                          (uint64_t)n_cols * q_pad)) != STB_OK) return rc;
+    if ((rc = stb_launch_batch_gemm_sample_work(ctx, ctx->bq_tiles, corpus->shadow, W + o_ts, (uint32_t)ws.tiles.size(), W + o_cs,
+                                                W + o_os, reinterpret_cast<const uint4 *>(W + o_is), ctx->b_fbits, n_cols,
+                                                ctx->b_tilemax)) != STB_OK) return rc;
+    if ((rc = stb_launch_batch_thresh(ctx, ctx->b_tilemax, n_cols, q_pad, q_pad, top_k, ctx->b_thr)) != STB_OK) return rc;
+    if ((rc = stb_launch_batch_gemm_emit_work(ctx, ctx->bq_tiles, corpus->shadow, W + o_te, (uint32_t)we.tiles.size(), W + o_ce,
+                                              W + o_oe, reinterpret_cast<const uint4 *>(W + o_ie), ctx->b_fbits, d_slot_row,
+                                              corpus->n, ctx->b_thr, ctx->b_cnt, ctx->b_keys, kSegCap)) != STB_OK) return rc;
+    if ((rc = stb_launch_batch_finish2(ctx, ctx->b_keys, ctx->b_cnt, n_seg, kSegCap, nt, top_k, corpus->rows, corpus->n,
+                                       corpus->row_base, ctx->bq_dev, ctx->s_qbad, ctx->bh_dev, ctx->bs_dev)) != STB_OK) return rc;
+    STB_CUDA(cudaMemcpyAsync(hits.data(), ctx->bh_dev, hits.size() * sizeof(stb_hit), cudaMemcpyDeviceToHost, ctx->stream));
+    STB_CUDA(cudaMemcpyAsync(status.data(), ctx->bs_dev, status.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    STB_CUDA(cudaStreamSynchronize(ctx->stream));           // the host arrays above are read by the copies
+  }
+  // each caller query's slot and compact row, for stb_debug_batch_last
+  if (ctx->s_map_cap < 2 * (size_t)nq) {
+    uint32_t *m = (uint32_t *)realloc(ctx->s_map, 2 * (size_t)nq * sizeof(uint32_t));
+    if (!m) { stb_set_error("search_batch_subsets: host allocation failed"); return STB_ERR_NOMEM; }
+    ctx->s_map = m;
+    ctx->s_map_cap = 2 * (size_t)nq;
+  }
+  memcpy(ctx->s_map, slot_of.data(), nq * sizeof(uint32_t));
+  memcpy(ctx->s_map + nq, row_of.data(), nq * sizeof(uint32_t));
+  uint32_t k1 = 0;
+  for (uint32_t i = 0; i < nq; ++i) {
+    stb_hit *oh = out_hits + (size_t)i * top_k;
+    uint64_t n = 0;
+    const uint32_t r = row_of[i];
+    if (group[i] == kNone) {
+      n = 0;
+    } else if (r != kNone && status[2 * (size_t)r + 1]) {
+      memcpy(oh, hits.data() + (size_t)r * top_k, (size_t)top_k * sizeof(stb_hit));
+      n = capped_hits(oh, status[2 * (size_t)r], has_max, max_distance);
+    } else {
+      ctx->fallback_searches++;
+      k1++;
+      if ((rc = stb_search(ctx, corpus, q + (size_t)i * STB_D, top_k, has_max, max_distance, STB_MODE_STORE_QUERY,
+                           ranges_of(i), n_of(i), oh, top_k, &n)) != STB_OK) return rc;
+    }
+    out_n[i] = (uint32_t)n;
+    pad(i, n);
+  }
+  const uint32_t done[6] = {6u, nq, T, k1, n_seg, T ? kSegCap : 0u};
+  memcpy(ctx->b_last, done, sizeof(done));
+  return STB_OK;
+}
+
+}  // extern "C"
+
 // ---- threshold mode for a batch (stb_search_batch_threshold, route 5) ---------------------------------------
 // delta: |canonical f64 distance - (1 - exact cosine)| of any pair of f32 vectors the shadow can normalise is
 // below ~1e-13 (256-term f64 FMA chains, two square roots, one division; DESIGN §5); 1e-12 leaves 10x slack.
@@ -1927,6 +2209,24 @@ int stb_debug_batch_last(stb_ctx *ctx, uint32_t info[6], float *thr, uint32_t *c
   STB_CUDA(cudaStreamSynchronize(ctx->stream));
   memcpy(info, ctx->b_last, sizeof(ctx->b_last));
   const uint32_t nq = ctx->b_last[1], n_seg = ctx->b_last[4];
+  if (ctx->b_last[0] == 6u && n_seg && nq) {
+    // slot-indexed thresholds, compact-row counts -> caller order (+inf, 0: a query the tensor passes did not take)
+    const uint32_t *slot = ctx->s_map, *row = ctx->s_map + nq;
+    uint32_t n_slots = 0, n_rows = 0;
+    for (uint32_t i = 0; i < nq; ++i) {
+      if (slot[i] != 0xffffffffu) n_slots = std::max(n_slots, slot[i] + 1);
+      if (row[i] != 0xffffffffu) n_rows = std::max(n_rows, row[i] + 1);
+    }
+    std::vector<float> t(n_slots);
+    std::vector<uint32_t> c((size_t)n_rows * n_seg);
+    STB_CUDA(cudaMemcpy(t.data(), ctx->b_thr, t.size() * sizeof(float), cudaMemcpyDeviceToHost));
+    STB_CUDA(cudaMemcpy(c.data(), ctx->b_cnt, c.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    for (uint32_t i = 0; i < nq; ++i) {
+      if (thr) thr[i] = slot[i] == 0xffffffffu ? INFINITY : t[slot[i]];
+      for (uint32_t s = 0; cand_cnt && s < n_seg; ++s) cand_cnt[(size_t)i * n_seg + s] = row[i] == 0xffffffffu ? 0u : c[(size_t)row[i] * n_seg + s];
+    }
+    return STB_OK;
+  }
   if ((ctx->b_last[0] == 2u || ctx->b_last[0] == 3u || (ctx->b_last[0] == 5u && n_seg)) && nq) {
     if (thr) STB_CUDA(cudaMemcpy(thr, ctx->b_thr, (size_t)nq * sizeof(float), cudaMemcpyDeviceToHost));
     if (cand_cnt) STB_CUDA(cudaMemcpy(cand_cnt, ctx->b_cnt, (size_t)nq * n_seg * sizeof(uint32_t), cudaMemcpyDeviceToHost));

@@ -183,9 +183,18 @@ struct GemmArgs {
   uint32_t n_tiles;           // ceil(N / 256)
   // maxima are stored [query tile][sub-tile or tile][128 queries]: the selection pass streams
   // them contiguously
-  float *submax;              // [m_tiles][n_tiles * 8][128]  per-32-row maxima
-  float *tilemax;             // [m_tiles][n_tiles][128]      per-256-row maxima
-  float *full_out;            // debug: full score matrix [m_tiles*128][n_tiles*256] or null
+  union {
+    float *submax;            // [m_tiles][n_tiles * 8][128]  per-32-row maxima
+    const uint4 *items;       // STB_GEMM_WORK (below)
+  };
+  union {
+    float *tilemax;           // [m_tiles][n_tiles][128]      per-256-row maxima (STB_GEMM_WORK: [m_tiles][tile_stride][128])
+    const uint32_t *slot_row; // STB_GEMM_WORK, EPI 1 (below)
+  };
+  union {
+    float *full_out;          // debug: full score matrix [m_tiles*128][n_tiles*256] or null
+    const uint32_t *item_off; // STB_GEMM_WORK (below)
+  };
   uint32_t tile_stride;       // corpus tile t of this launch is shadow tile t * tile_stride (sampling pass)
   // EPI == 1 (candidate-emitting epilogue, pipeline v2):
   const float *thr;           // [q_pad] per-query score threshold (+inf for padding queries)
@@ -198,22 +207,213 @@ struct GemmArgs {
   const uint32_t *bitmap;     // eligible local rows, 1 bit each: 8 words per shadow tile
   // EPI == 2 (stb_search_batch_threshold's re-emission): segment (q, CTA) is cand_keys[seg_off[q * grid + CTA],
   // seg_off[q * grid + CTA + 1]), sized by the first pass's exact counts; cand_cnt holds the cursors
-  const uint64_t *seg_off;    // [q_pad * grid + 1]
+  union {
+    const uint64_t *seg_off;  // [q_pad * grid + 1]
+    const uint32_t *cta_tiles;  // STB_GEMM_WORK (below)
+  };
+  // STB_GEMM_WORK (stb_search_batch_subsets; the unions keep the layout the other modes compile against): CTA b
+  // walks the corpus tiles u in [cta_tiles[b], cta_tiles[b + 1]) (shadow tile tile_ids[u]); tile u's work items
+  // are items[item_off[u], item_off[u + 1]), each {query tile, mask slot of half 0, mask slot of half 1, sample
+  // columns}: a mask slot is 8 bitmap words at bitmap + 8 * slot; the sample columns (EPI 0: low / high 16
+  // bits, 0xffff: none) index tilemax [m_tiles][tile_stride][128].  EPI 1 writes query slot s's keys and count
+  // at row slot_row[s] (~0: a padding slot, which never emits).
 };
+
+// Filter modes of the GEMM: every tile, the listed tiles of one filter, or a work list of (query tile, masks)
+// per corpus tile, one filter per 64-query half
+#define STB_GEMM_ALL 0
+#define STB_GEMM_LISTED 1
+#define STB_GEMM_WORK 2
 
 // warpgroup 0: bulk-copy producer (one thread); warpgroups 1 and 2: wgmma + epilogue, each on
 // 64 of the 128 queries of a query tile (m64n256 accumulators, 128 f32 registers per thread)
 #define STB_GEMM_THREADS 384
 #define STB_GEMM_CONSUMER_WARPS 8
 #define STB_GEMM_SMEM (STB_N_SLABS * STB_B_SLAB_BYTES + STB_A_RING * STB_A_SLAB_BYTES + 1024 + 256)
+// STB_GEMM_WORK: three 64-byte mask buffers behind the barriers instead of two 32-byte ones
+#define STB_GEMM_SMEM_WORK (STB_GEMM_SMEM + 128)
+static_assert(STB_GEMM_SMEM_WORK <= 227 * 1024, "GEMM shared memory");
+
+// FILTER == STB_GEMM_WORK (EPI 0 or 1), the body of stb_batch_gemm_kernel below on its shared memory and
+// initialised barriers: the same pipeline and epilogues per 64-query half, over each corpus tile's work items
+// (GemmArgs) instead of every query tile.  Kept apart from the kernel body so the other modes compile as they
+// did.  An item's 2 x 8 mask words arrive with its first query slab; item i of a CTA uses mask buffer i % 3:
+// item i + 3's slab 0 reuses the ring slot of item i + 1's slab 2, which every consumer warp releases only
+// after the epilogue of item i.
+template <int EPI>
+__device__ __forceinline__ void stb_batch_gemm_work(const GemmArgs &args, uint8_t *sB, uint8_t *sA, uint64_t *bars) {
+  uint64_t *b_full = bars + 0, *b_empty = bars + STB_N_SLABS;
+  uint64_t *a_full = bars + 2 * STB_N_SLABS, *a_empty = a_full + STB_A_RING;
+  uint32_t *s_mask = reinterpret_cast<uint32_t *>(bars + 24);       // [3][2][8]
+  static_assert(24 * 8 + 3 * 16 * 4 <= 256 + (STB_GEMM_SMEM_WORK - STB_GEMM_SMEM), "work-item mask words must fit");
+  static_assert(STB_A_RING == 6 && STB_N_SLABS == 4, "the mask buffer rule (item % 3) assumes this ring");
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t t0 = __ldg(args.cta_tiles + blockIdx.x), t1 = __ldg(args.cta_tiles + blockIdx.x + 1);
+
+  if (warp < 4) {
+    // ===== bulk-copy producer (one thread) =====
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
+      uint32_t a_cnt = 0;
+      for (uint32_t u = t0, it = 0; u < t1; ++u, ++it) {
+        const uint8_t *src = args.b_tiles + (uint64_t)__ldg(args.tile_ids + u) * (size_t)(STB_N_SLABS * STB_B_SLAB_BYTES);
+        for (int s = 0; s < STB_N_SLABS; ++s) {
+          mbar_wait(b_empty + s, (it & 1) ^ 1);
+          mbar_expect_tx(b_full + s, STB_B_SLAB_BYTES);
+          bulk_g2s(sB + s * STB_B_SLAB_BYTES, src + (size_t)s * STB_B_SLAB_BYTES, STB_B_SLAB_BYTES, b_full + s);
+        }
+        const uint32_t w1 = __ldg(args.item_off + u + 1);
+        for (uint32_t w = __ldg(args.item_off + u); w < w1; ++w) {
+          const uint4 item = __ldg(args.items + w);
+          for (int s = 0; s < STB_N_SLABS; ++s, ++a_cnt) {
+            const uint32_t slot = a_cnt % STB_A_RING;
+            mbar_wait(a_empty + slot, ((a_cnt / STB_A_RING) & 1) ^ 1);
+            if (s == 0) {
+              uint32_t *mk = s_mask + ((a_cnt / STB_N_SLABS) % 3) * 16;
+              mbar_expect_tx(a_full + slot, STB_A_SLAB_BYTES + 64);
+              bulk_g2s(mk, args.bitmap + (size_t)item.y * 8, 32, a_full + slot);
+              bulk_g2s(mk + 8, args.bitmap + (size_t)item.z * 8, 32, a_full + slot);
+            } else {
+              mbar_expect_tx(a_full + slot, STB_A_SLAB_BYTES);
+            }
+            bulk_g2s(sA + slot * STB_A_SLAB_BYTES, args.a_tiles + ((size_t)item.x * STB_N_SLABS + s) * STB_A_SLAB_BYTES,
+                     STB_A_SLAB_BYTES, a_full + slot);
+          }
+        }
+      }
+    }
+    return;
+  }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  // ===== consumers (accumulator layout as in stb_batch_gemm_kernel) =====
+  const uint32_t half = (uint32_t)(warp >> 2) - 1u;
+  const uint32_t qrow = half * 64 + (warp & 3) * 16 + (lane >> 2);
+  const uint32_t quad = lane & 3;
+  float d[128];
+#pragma unroll
+  for (int i = 0; i < 128; ++i) d[i] = 0.f;
+  uint32_t a_cnt = 0;
+  for (uint32_t u = t0, it = 0; u < t1; ++u, ++it) {
+    const uint64_t tile_row0 = (uint64_t)__ldg(args.tile_ids + u) * STB_B_TILE;
+    const uint32_t w0 = __ldg(args.item_off + u), w1 = __ldg(args.item_off + u + 1);
+    for (uint32_t w = w0; w < w1; ++w, a_cnt += STB_N_SLABS) {
+      const uint4 item = __ldg(args.items + w);
+      const uint32_t m = item.x;
+      const uint32_t *mask = s_mask + ((a_cnt / STB_N_SLABS) % 3) * 16 + half * 8;   // this half's filter
+      const uint32_t q0 = m * STB_A_TILE + qrow;
+      [[maybe_unused]] float thr[2];
+      [[maybe_unused]] uint32_t cnt[2], cnt0[2], qout[2];
+      if constexpr (EPI == 1) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          // a padding slot never emits and owns no segment
+          const uint32_t r = __ldg(args.slot_row + q0 + 8 * h);
+          thr[h] = (r == 0xffffffffu) ? CUDART_INF_F : __ldg(args.thr + q0 + 8 * h);
+          qout[h] = (r == 0xffffffffu) ? 0u : r;
+          cnt0[h] = args.cand_cnt[(size_t)qout[h] * gridDim.x + blockIdx.x];
+          cnt[h] = cnt0[h];
+        }
+      }
+      wg_reg_fence(d);
+#pragma unroll
+      for (int s = 0; s < STB_N_SLABS; ++s) {
+        const uint32_t slot = (a_cnt + s) % STB_A_RING;
+        if (w == w0) mbar_wait(b_full + s, it & 1);
+        mbar_wait(a_full + slot, ((a_cnt + s) / STB_A_RING) & 1);
+        wg_fence();
+        const uint32_t a_addr = smem_u32(sA + slot * STB_A_SLAB_BYTES + half * (64 * 128));
+        const uint32_t b_addr = smem_u32(sB + s * STB_B_SLAB_BYTES);
+#pragma unroll
+        for (int k = 0; k < STB_SLAB_K / 16; ++k)
+          wg_mma_m64n256k16(d, wg_desc_sw128(a_addr + k * 32), wg_desc_sw128(b_addr + k * 32), (uint32_t)((s | k) != 0));
+        wg_commit();
+        if (s > 0) {
+          wg_wait<1>();
+          if (lane == 0) {
+            mbar_arrive(a_empty + (a_cnt + s - 1) % STB_A_RING);
+            if (w + 1 == w1) mbar_arrive(b_empty + s - 1);
+          }
+        }
+      }
+      wg_wait<0>();
+      wg_reg_fence(d);
+      if (lane == 0) {
+        mbar_arrive(a_empty + (a_cnt + STB_N_SLABS - 1) % STB_A_RING);
+        if (w + 1 == w1) mbar_arrive(b_empty + STB_N_SLABS - 1);
+      }
+
+      if constexpr (EPI == 0) {
+        // tile maximum over this half's eligible rows (ineligible scores -inf, as FILTER == STB_GEMM_LISTED),
+        // stored at the half's column of its group's sample (0xffff: the tile is not in that sample)
+        float tmx[2] = {-CUDART_INF_F, -CUDART_INF_F};
+#pragma unroll
+        for (int c = 0; c < STB_B_TILE / STB_SUB; ++c) {
+          const uint32_t mw = mask[c];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float mx = -CUDART_INF_F;
+#pragma unroll
+            for (int ii = 0; ii < 4; ++ii)
+#pragma unroll
+              for (int e = 0; e < 2; ++e)
+                mx = fmaxf(mx, ((mw >> (ii * 8 + quad * 2 + e)) & 1u) ? d[16 * c + 4 * ii + 2 * h + e] : -CUDART_INF_F);
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            tmx[h] = fmaxf(tmx[h], mx);
+          }
+        }
+        const uint32_t col = half ? (item.w >> 16) : (item.w & 0xffffu);
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          if (quad == (uint32_t)(2 + h) && col != 0xffffu)
+            args.tilemax[((size_t)m * args.tile_stride + col) * STB_A_TILE + qrow + 8 * h] = tmx[h];
+      } else {
+        // emission as stb_batch_gemm_kernel's EPI 1, into the segments of row qout
+#pragma unroll
+        for (int c = 0; c < STB_B_TILE / STB_SUB; ++c) {
+          const uint64_t row0 = tile_row0 + (uint64_t)c * STB_SUB;
+          const uint32_t mw = mask[c];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            uint32_t hit = 0u;
+#pragma unroll
+            for (int ii = 0; ii < 4; ++ii)
+#pragma unroll
+              for (int e = 0; e < 2; ++e)
+                hit |= (d[16 * c + 4 * ii + 2 * h + e] >= thr[h] ? 1u : 0u) << (ii * 8 + quad * 2 + e);
+            hit |= __shfl_xor_sync(0xffffffffu, hit, 1);
+            hit |= __shfl_xor_sync(0xffffffffu, hit, 2);
+            if (row0 + 32 > args.n_rows) hit &= (row0 < args.n_rows) ? ((1u << (uint32_t)(args.n_rows - row0)) - 1u) : 0u;
+            hit &= mw;
+            uint64_t *seg = args.cand_keys + ((size_t)qout[h] * gridDim.x + blockIdx.x) * args.cand_cap;
+#pragma unroll
+            for (int ii = 0; ii < 4; ++ii)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const uint32_t b = ii * 8 + quad * 2 + e;
+                const uint32_t pos = cnt[h] + __popc(hit & ((1u << b) - 1u));
+                const uint64_t key = stb_make_key(d[16 * c + 4 * ii + 2 * h + e], (uint32_t)(row0 + b));
+                if (((hit >> b) & 1u) && pos < args.cand_cap) seg[pos] = key;
+              }
+            cnt[h] += __popc(hit);
+          }
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          if (quad == 0 && cnt[h] != cnt0[h]) args.cand_cnt[(size_t)qout[h] * gridDim.x + blockIdx.x] = cnt[h];
+      }
+    }
+  }
+}
 
 // EPI 0: per-sub-tile / per-tile maxima (pipeline v1, and the sampling pass of v2).
 // EPI 1: emit every (query,row) whose approximate score reaches the query's threshold.
 // EPI 2: the same emission into exactly sized segments at args.seg_off (unfiltered only).
-// FILTER: the CTAs walk the listed tiles (args.tile_ids) and only eligible rows count (args.bitmap): EPI 0
-// takes each tile maximum over its eligible rows, EPI 1 emits eligible rows only.  The tile's 8 bitmap words
-// arrive with its first corpus slab, double-buffered behind the mbarriers.
-template <int EPI, bool FILTER>
+// FILTER == STB_GEMM_LISTED: the CTAs walk the listed tiles (args.tile_ids) and only eligible rows count
+// (args.bitmap): EPI 0 takes each tile maximum over its eligible rows, EPI 1 emits eligible rows only.  The
+// tile's 8 bitmap words arrive with its first corpus slab, double-buffered behind the mbarriers.
+// FILTER == STB_GEMM_WORK: stb_batch_gemm_work above.
+template <int EPI, int FILTER>
 __global__ void __launch_bounds__(STB_GEMM_THREADS, 1)
 stb_batch_gemm_kernel(const GemmArgs args) {
   extern __shared__ uint8_t smem_raw[];
@@ -236,6 +436,11 @@ stb_batch_gemm_kernel(const GemmArgs args) {
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
+  if constexpr (FILTER == STB_GEMM_WORK) {
+    static_assert(EPI == 0 || EPI == 1, "work lists serve v2's two passes");
+    stb_batch_gemm_work<EPI>(args, sB, sA, bars);
+    return;
+  }
 
   const uint32_t my_tiles = (args.n_tiles > blockIdx.x) ? (args.n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
 
@@ -248,7 +453,7 @@ stb_batch_gemm_kernel(const GemmArgs args) {
         const uint64_t t = blockIdx.x + (uint64_t)it * gridDim.x;
         // corpus tile, slab by slab: slab s of the previous tile is released as soon as the
         // last query tile's MMAs on it retire, so the refill overlaps the remaining slabs
-        if constexpr (FILTER) {
+        if constexpr (FILTER == STB_GEMM_LISTED) {
           const uint64_t tile = __ldg(args.tile_ids + t * args.tile_stride);
           const uint8_t *src = args.b_tiles + tile * (size_t)(STB_N_SLABS * STB_B_SLAB_BYTES);
           for (int s = 0; s < STB_N_SLABS; ++s) {
@@ -301,7 +506,7 @@ stb_batch_gemm_kernel(const GemmArgs args) {
   for (uint32_t it = 0; it < my_tiles; ++it) {
     const uint64_t t = blockIdx.x + (uint64_t)it * gridDim.x;
     [[maybe_unused]] uint64_t tile_row0 = 0;                 // FILTER: first row of the shadow tile
-    if constexpr (FILTER) tile_row0 = (uint64_t)__ldg(args.tile_ids + t * args.tile_stride) * STB_B_TILE;
+    if constexpr (FILTER == STB_GEMM_LISTED) tile_row0 = (uint64_t)__ldg(args.tile_ids + t * args.tile_stride) * STB_B_TILE;
     for (uint32_t m = 0; m < args.m_tiles; ++m, a_cnt += STB_N_SLABS) {
       const uint32_t q0 = m * STB_A_TILE + qrow;
       [[maybe_unused]] float thr[2];
@@ -355,11 +560,11 @@ stb_batch_gemm_kernel(const GemmArgs args) {
 #pragma unroll
         for (int c = 0; c < STB_B_TILE / STB_SUB; ++c) {
           [[maybe_unused]] uint32_t mw = 0;
-          if constexpr (FILTER) mw = s_mask[(it & 1) * 8 + c];
+          if constexpr (FILTER == STB_GEMM_LISTED) mw = s_mask[(it & 1) * 8 + c];
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             float mx;
-            if constexpr (FILTER) {
+            if constexpr (FILTER == STB_GEMM_LISTED) {
               // an ineligible row's score is -inf here (a select, no branch): the maximum is an eligible
               // row's score, which the threshold's sufficiency argument needs
               mx = -CUDART_INF_F;
@@ -403,7 +608,7 @@ stb_batch_gemm_kernel(const GemmArgs args) {
         for (int c = 0; c < STB_B_TILE / STB_SUB; ++c) {
           uint64_t row0;
           [[maybe_unused]] uint32_t mw = 0;
-          if constexpr (FILTER) {
+          if constexpr (FILTER == STB_GEMM_LISTED) {
             row0 = tile_row0 + (uint64_t)c * STB_SUB;
             mw = s_mask[(it & 1) * 8 + c];
           } else {
@@ -422,7 +627,7 @@ stb_batch_gemm_kernel(const GemmArgs args) {
             hit |= __shfl_xor_sync(0xffffffffu, hit, 1);
             hit |= __shfl_xor_sync(0xffffffffu, hit, 2);
             if (row0 + 32 > args.n_rows) hit &= (row0 < args.n_rows) ? ((1u << (uint32_t)(args.n_rows - row0)) - 1u) : 0u;   // padding rows
-            if constexpr (FILTER) hit &= mw;                                                                                    // ineligible rows
+            if constexpr (FILTER == STB_GEMM_LISTED) hit &= mw;                                                                                    // ineligible rows
             uint64_t *seg;
             uint32_t seg_cap;
             if constexpr (EPI == 2) {
@@ -473,15 +678,18 @@ int stb_launch_shadow_build(stb_ctx *ctx, const float *rows_dev, uint64_t n_rows
   return STB_OK;
 }
 
-template <int EPI, bool FILTER = false>
+template <int EPI, int FILTER = STB_GEMM_ALL>
 static int launch_gemm(stb_ctx *ctx, const GemmArgs &a) {
-  const int attr = FILTER ? (EPI == 0 ? STB_ATTR_GEMM0F : STB_ATTR_GEMM1F)
-                          : (EPI == 0 ? STB_ATTR_GEMM0 : (EPI == 1 ? STB_ATTR_GEMM1 : STB_ATTR_GEMM2));
+  const int attr = FILTER == STB_GEMM_WORK ? (EPI == 0 ? STB_ATTR_GEMM0W : STB_ATTR_GEMM1W)
+                   : FILTER == STB_GEMM_LISTED ? (EPI == 0 ? STB_ATTR_GEMM0F : STB_ATTR_GEMM1F)
+                   : (EPI == 0 ? STB_ATTR_GEMM0 : (EPI == 1 ? STB_ATTR_GEMM1 : STB_ATTR_GEMM2));
+  const int smem = FILTER == STB_GEMM_WORK ? STB_GEMM_SMEM_WORK : STB_GEMM_SMEM;
   STB_ATTR_ONCE(ctx, attr,
-                cudaFuncSetAttribute(stb_batch_gemm_kernel<EPI, FILTER>, cudaFuncAttributeMaxDynamicSharedMemorySize, STB_GEMM_SMEM));
+                cudaFuncSetAttribute(stb_batch_gemm_kernel<EPI, FILTER>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  // STB_GEMM_WORK: the same grid as the caller's cta_tiles (stb_batch_emit_grid)
   unsigned grid = (unsigned)std::min<uint32_t>(a.n_tiles, (uint32_t)ctx->sm_count);
   if (grid == 0) return STB_OK;
-  stb_batch_gemm_kernel<EPI, FILTER><<<grid, STB_GEMM_THREADS, STB_GEMM_SMEM, ctx->stream>>>(a);
+  stb_batch_gemm_kernel<EPI, FILTER><<<grid, STB_GEMM_THREADS, smem, ctx->stream>>>(a);
   STB_CUDA(cudaGetLastError());
   ctx->kernel_launches++;
   return STB_OK;
@@ -519,7 +727,7 @@ int stb_launch_batch_gemm_sample_filtered(stb_ctx *ctx, const uint8_t *a_tiles, 
   GemmArgs a{};
   a.a_tiles = a_tiles; a.b_tiles = b_tiles; a.m_tiles = m_tiles; a.n_tiles = n_sample; a.tile_stride = tile_stride;
   a.tilemax = tilemax; a.tile_ids = tile_ids; a.bitmap = bitmap;
-  return launch_gemm<0, true>(ctx, a);
+  return launch_gemm<0, STB_GEMM_LISTED>(ctx, a);
 }
 
 // ... and the candidate-emitting pass over all n_listed listed tiles, eligible rows only
@@ -530,7 +738,75 @@ int stb_launch_batch_gemm_emit_filtered(stb_ctx *ctx, const uint8_t *a_tiles, ui
   a.a_tiles = a_tiles; a.b_tiles = b_tiles; a.m_tiles = m_tiles; a.n_tiles = n_listed; a.tile_stride = 1;
   a.thr = thr; a.cand_cnt = cand_cnt; a.cand_keys = cand_keys; a.cand_cap = cand_cap; a.n_rows = n_rows;
   a.tile_ids = tile_ids; a.bitmap = bitmap;
-  return launch_gemm<1, true>(ctx, a);
+  return launch_gemm<1, STB_GEMM_LISTED>(ctx, a);
+}
+
+// Pipeline v2 with one filter per 64-query half (stb_search_batch_subsets): the sampling pass and the emitting
+// pass over corpus tiles tile_ids[0, n_tiles), each with its work items (GemmArgs, STB_GEMM_WORK); masks are
+// 8-word slots of `bitmap`.  The sampling pass writes tilemax [m_tiles][tm_cols][128] at each half's sample
+// column; the emitting pass writes slot s's keys and count at row slot_row[s].
+int stb_launch_batch_gemm_sample_work(stb_ctx *ctx, const uint8_t *a_tiles, const uint8_t *b_tiles, const uint32_t *tile_ids,
+                                      uint32_t n_tiles, const uint32_t *cta_tiles, const uint32_t *item_off, const uint4 *items,
+                                      const uint32_t *bitmap, uint32_t tm_cols, float *tilemax) {
+  GemmArgs a{};
+  a.a_tiles = a_tiles; a.b_tiles = b_tiles; a.tile_ids = tile_ids; a.n_tiles = n_tiles; a.cta_tiles = cta_tiles;
+  a.item_off = item_off; a.items = items; a.bitmap = bitmap; a.tile_stride = tm_cols; a.tilemax = tilemax;
+  return launch_gemm<0, STB_GEMM_WORK>(ctx, a);
+}
+
+int stb_launch_batch_gemm_emit_work(stb_ctx *ctx, const uint8_t *a_tiles, const uint8_t *b_tiles, const uint32_t *tile_ids,
+                                    uint32_t n_tiles, const uint32_t *cta_tiles, const uint32_t *item_off, const uint4 *items,
+                                    const uint32_t *bitmap, const uint32_t *slot_row, uint64_t n_rows, const float *thr,
+                                    uint32_t *cand_cnt, uint64_t *cand_keys, uint32_t cand_cap) {
+  GemmArgs a{};
+  a.a_tiles = a_tiles; a.b_tiles = b_tiles; a.tile_ids = tile_ids; a.n_tiles = n_tiles; a.cta_tiles = cta_tiles;
+  a.item_off = item_off; a.items = items; a.bitmap = bitmap; a.slot_row = slot_row; a.n_rows = n_rows;
+  a.thr = thr; a.cand_cnt = cand_cnt; a.cand_keys = cand_keys; a.cand_cap = cand_cap;
+  return launch_gemm<1, STB_GEMM_WORK>(ctx, a);
+}
+
+// stb_search_batch_subsets's query slots: slot s holds the f32 query row slot_row[s] of `rows` (zeros for a
+// padding slot, ~0) ...
+__global__ void stb_batch_slots_gather_kernel(const float4 *__restrict__ rows, const uint32_t *__restrict__ slot_row,
+                                              uint32_t n_slots, float4 *__restrict__ out) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;       // one float4 each
+  if (i >= (uint64_t)n_slots * STB_ROW_F4) return;
+  const uint32_t r = __ldg(slot_row + i / STB_ROW_F4);
+  out[i] = (r == 0xffffffffu) ? make_float4(0.f, 0.f, 0.f, 0.f) : __ldg(rows + (uint64_t)r * STB_ROW_F4 + i % STB_ROW_F4);
+}
+
+// ... and, once the slots' shadow is built: row_bad[slot_row[s]] = slot_bad[s], and every tilemax entry -inf,
+// so the columns past a group's own sample never rank above its sampled maxima
+__global__ void stb_batch_slots_prep_kernel(const uint32_t *__restrict__ slot_row, const uint32_t *__restrict__ slot_bad,
+                                            uint32_t n_slots, uint32_t *__restrict__ row_bad, float *__restrict__ tilemax,
+                                            uint64_t n_tilemax) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n_slots) {
+    const uint32_t r = slot_row[i];
+    if (r != 0xffffffffu) row_bad[r] = slot_bad[i];
+  }
+  if (i < n_tilemax) tilemax[i] = -CUDART_INF_F;
+}
+
+int stb_launch_batch_slots_gather(stb_ctx *ctx, const float *rows, const uint32_t *slot_row, uint32_t n_slots, float *out) {
+  const uint64_t n = (uint64_t)n_slots * STB_ROW_F4;
+  if (n == 0) return STB_OK;
+  stb_batch_slots_gather_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(
+      reinterpret_cast<const float4 *>(rows), slot_row, n_slots, reinterpret_cast<float4 *>(out));
+  STB_CUDA(cudaGetLastError());
+  ctx->kernel_launches++;
+  return STB_OK;
+}
+
+int stb_launch_batch_slots_prep(stb_ctx *ctx, const uint32_t *slot_row, const uint32_t *slot_bad, uint32_t n_slots,
+                                uint32_t *row_bad, float *tilemax, uint64_t n_tilemax) {
+  const uint64_t n = std::max<uint64_t>(n_slots, n_tilemax);
+  if (n == 0) return STB_OK;
+  stb_batch_slots_prep_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(slot_row, slot_bad, n_slots, row_bad,
+                                                                                     tilemax, n_tilemax);
+  STB_CUDA(cudaGetLastError());
+  ctx->kernel_launches++;
+  return STB_OK;
 }
 
 // Threshold mode's re-emission: the candidate-emitting pass over all tiles into the exactly sized segments

@@ -130,6 +130,13 @@ struct stb_ctx {
   uint32_t *b_franges; size_t b_franges_cap;
   uint32_t *b_ftiles; size_t b_ftiles_cap;
   uint32_t *b_fbits; size_t b_fbits_cap;
+  // stb_search_batch_subsets (route 6; b_franges / b_fbits hold every tensor group's ranges / bitmap): both
+  // passes' work lists and the slots' rows in one upload, the queries in slot order, the bad flags per
+  // compact row, and (host, malloc) each caller query's slot and compact row for stb_debug_batch_last
+  uint32_t *s_work; size_t s_work_cap;
+  float *s_qslots; size_t s_qslots_cap;
+  uint32_t *s_qbad; size_t s_qbad_cap;
+  uint32_t *s_map; size_t s_map_cap;
   // stb_search_batch_threshold (per chunk of queries): per-(query, segment) destinations of the first pass's
   // keys, the re-emission's segment offsets, cursors, queries and thresholds, the compact candidates and their
   // sort buffers (4 x u64 per candidate), per-slot offsets / query / pass count / output position, the hits
@@ -146,8 +153,8 @@ struct stb_ctx {
   stb_hit *t_hits; size_t t_hits_cap;
   uint8_t *t_sort_tmp; size_t t_sort_tmp_cap;
   // the last K2 call: route (1 = v1, 2 = v2, 3 = filtered v2, 4 = filtered, nothing on the tensor cores,
-  // 5 = threshold mode), nq, then n_sample, stride (routes 1-4) or retried queries, K1 queries (route 5), n_seg,
-  // seg_cap
+  // 5 = threshold mode, 6 = one filter per query), nq, then n_sample, stride (routes 1-4) or retried queries, K1
+  // queries (route 5) or tensor groups, K1 queries (route 6), n_seg, seg_cap
   uint32_t b_last[6];
   float *bq_dev; size_t bq_dev_cap;           // host-call staging: queries
   stb_hit *bh_dev; size_t bh_dev_cap;         // host-call staging: hits
@@ -378,7 +385,7 @@ int stb_launch_batch_xchg(stb_ctx *ctx, const StbBatchXchgArgs &a, const stb_hit
 
 // opt-in to > 48 KiB dynamic shared memory (or another function attribute) once per context
 enum { STB_ATTR_GEMM0 = 0, STB_ATTR_GEMM1, STB_ATTR_MERGE, STB_ATTR_IVF_PROBE, STB_ATTR_IVF_V2, STB_ATTR_FINISH2,
-       STB_ATTR_IVF_BATCH, STB_ATTR_GEMM0F, STB_ATTR_GEMM1F, STB_ATTR_GEMM2 };
+       STB_ATTR_IVF_BATCH, STB_ATTR_GEMM0F, STB_ATTR_GEMM1F, STB_ATTR_GEMM2, STB_ATTR_GEMM0W, STB_ATTR_GEMM1W };
 #define STB_ATTR_ONCE(ctx, bit, call)                         \
   do {                                                        \
     if (!((ctx)->func_attr_mask & (1u << (bit)))) {           \
@@ -417,6 +424,21 @@ int stb_launch_batch_gemm_emit_filtered(stb_ctx *ctx, const uint8_t *a_tiles, ui
                                         const uint32_t *bitmap, uint32_t n_listed, uint64_t n_rows,
                                         const float *thr, uint32_t *cand_cnt, uint64_t *cand_keys,
                                         uint32_t cand_cap);
+// the same two passes with one filter per 64-query half, over per-corpus-tile work items (batch_scan.cu, GemmArgs)
+int stb_launch_batch_gemm_sample_work(stb_ctx *ctx, const uint8_t *a_tiles, const uint8_t *b_tiles,
+                                      const uint32_t *tile_ids, uint32_t n_tiles, const uint32_t *cta_tiles,
+                                      const uint32_t *item_off, const uint4 *items, const uint32_t *bitmap,
+                                      uint32_t tm_cols, float *tilemax);
+int stb_launch_batch_gemm_emit_work(stb_ctx *ctx, const uint8_t *a_tiles, const uint8_t *b_tiles,
+                                    const uint32_t *tile_ids, uint32_t n_tiles, const uint32_t *cta_tiles,
+                                    const uint32_t *item_off, const uint4 *items, const uint32_t *bitmap,
+                                    const uint32_t *slot_row, uint64_t n_rows, const float *thr, uint32_t *cand_cnt,
+                                    uint64_t *cand_keys, uint32_t cand_cap);
+// the query slots of those passes: f32 rows gathered into slot order, then the per-row bad flags scattered
+// back and the sampled maxima preset to -inf
+int stb_launch_batch_slots_gather(stb_ctx *ctx, const float *rows, const uint32_t *slot_row, uint32_t n_slots, float *out);
+int stb_launch_batch_slots_prep(stb_ctx *ctx, const uint32_t *slot_row, const uint32_t *slot_bad, uint32_t n_slots,
+                                uint32_t *row_bad, float *tilemax, uint64_t n_tilemax);
 int stb_launch_batch_thresh(stb_ctx *ctx, const float *tilemax, uint32_t n_sample, uint32_t nq,
                             uint32_t q_pad, uint32_t top_k, float *thr);
 // candidates live in per-(query, CTA) segments: keys [q_pad][n_seg][seg_cap], counts [q_pad][n_seg];

@@ -559,6 +559,21 @@ class Store:
         res = self._gpu_corpus().search_batch_filtered(query_vecs, ranges, top_k, max_distance)
         return [self._ranked(hits) for hits in res]
 
+    def search_line_embeddings_many(self, query_vecs, subsets, top_k: int, max_distance=None) -> list:
+        """search_line_embeddings for many queries, each with its own subset paths (stb_search_batch_subsets):
+        element i is what search_line_embeddings(query_vecs[i], subsets[i], top_k, max_distance) returns."""
+        query_vecs = np.ascontiguousarray(query_vecs, dtype=np.float32).reshape(-1, capi.STB_DIM)
+        if len(subsets) != len(query_vecs):
+            raise ValueError(f"{len(subsets)} subsets for {len(query_vecs)} queries")
+        if top_k == 0 or len(query_vecs) == 0:                       # :489-491
+            return [[] for _ in range(len(query_vecs))]
+        # an empty subset, or one naming no stored path, has no ranges: 0 hits
+        ranges = [self._ranges_for(paths) if len(paths) else np.zeros((0, 2), np.uint64) for paths in subsets]
+        if not any(len(r) for r in ranges):
+            return [[] for _ in range(len(query_vecs))]
+        res = self._gpu_corpus().search_batch_subsets(query_vecs, ranges, top_k, max_distance)
+        return [self._ranked(hits) for hits in res]
+
     def _ranked(self, hits) -> list:
         out = []
         for h in hits:
