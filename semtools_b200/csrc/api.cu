@@ -44,23 +44,6 @@ static int ctx_use(const stb_ctx *ctx) {
   return STB_OK;
 }
 
-template <class T>
-static int dev_reserve(T **p, size_t *cap, size_t need, size_t floor_cap = 0) {
-  if (need <= *cap && *p) return STB_OK;
-  size_t ncap = std::max(std::max(need, floor_cap), *cap + *cap / 2);
-  T *np = nullptr;
-  cudaError_t e = cudaMalloc((void **)&np, ncap * sizeof(T));
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    stb_set_error("cudaMalloc(%zu bytes) failed: %s", ncap * sizeof(T), cudaGetErrorString(e));
-    return STB_ERR_NOMEM;
-  }
-  if (*p) cudaFree(*p);
-  *p = np;
-  *cap = ncap;
-  return STB_OK;
-}
-
 bool stb_ranges_ordered(const uint64_t *ranges, uint32_t n) {
   uint64_t prev_end = 0;
   for (uint32_t i = 0; i < n; ++i) {
@@ -97,7 +80,6 @@ int stb_ctx_create(int device, void *cuda_stream, stb_ctx **out) {
   }
   stb_ctx *c = new (std::nothrow) stb_ctx();
   if (!c) { stb_set_error("out of host memory"); return STB_ERR_NOMEM; }
-  memset(c, 0, sizeof(*c));
   c->device = device;
   c->sm_count = prop.multiProcessorCount;
   if (cuda_stream) { c->stream = (cudaStream_t)cuda_stream; c->own_stream = false; }
@@ -108,46 +90,34 @@ int stb_ctx_create(int device, void *cuda_stream, stb_ctx **out) {
   }
   int rc = STB_OK;
   const size_t max_grid = (size_t)c->sm_count * 8;
-  if ((rc = dev_reserve(&c->block_keys, &c->block_keys_cap, 2 * max_grid * 129 + STB_SORT_CAP)) != STB_OK) goto fail;
-  if ((rc = dev_reserve(&c->counters, &c->counters_cap, max_grid + 64)) != STB_OK) goto fail;
-  {
-    size_t one = 0;
-    if ((rc = dev_reserve(&c->q_dev, &one, STB_D)) != STB_OK) goto fail;
-    one = 0;
-    if ((rc = dev_reserve(&c->status_dev, &one, 8)) != STB_OK) goto fail;
-    one = 0;
-    if ((rc = dev_reserve(&c->collect_count, &one, 2)) != STB_OK) goto fail;
-    one = 0;
-    if ((rc = dev_reserve(&c->err_flag, &one, 1)) != STB_OK) goto fail;
-    one = 0;
-    if ((rc = dev_reserve(&c->embed_flag, &one, 1)) != STB_OK) goto fail;
-    one = 0;
-    if ((rc = dev_reserve(&c->hist_dev, &one, 4096)) != STB_OK) goto fail;
-    one = 0;
-    if ((rc = dev_reserve(&c->tickets, &one, STB_TICKET_SLOTS)) != STB_OK) goto fail;
-    one = 0;
-    if ((rc = dev_reserve(&c->q4_thr, &one, STB_TICKET_SLOTS * STB_Q4_WORDS)) != STB_OK) goto fail;
-    one = 0;
-    if ((rc = dev_reserve(&c->q4_refined, &one, 1)) != STB_OK) goto fail;
-    one = 0;
-    if ((rc = dev_reserve(&c->coscan_off, &one, STB_TICKET_SLOTS)) != STB_OK) goto fail;
-  }
-  if ((rc = dev_reserve(&c->hits_dev, &c->hits_cap, 1024)) != STB_OK) goto fail;
-  if (cudaMemset(c->counters, 0, c->counters_cap * sizeof(unsigned int)) != cudaSuccess ||
+  if ((rc = c->block_keys.alloc(2 * max_grid * 129 + STB_SORT_CAP)) != STB_OK ||
+      (rc = c->counters.alloc(max_grid + 64)) != STB_OK ||
+      (rc = c->q_dev.alloc(STB_D)) != STB_OK ||
+      (rc = c->status_dev.alloc(8)) != STB_OK ||
+      (rc = c->collect_count.alloc(2)) != STB_OK ||
+      (rc = c->err_flag.alloc(1)) != STB_OK ||
+      (rc = c->embed_flag.alloc(1)) != STB_OK ||
+      (rc = c->hist_dev.alloc(4096)) != STB_OK ||
+      (rc = c->tickets.alloc(STB_TICKET_SLOTS)) != STB_OK ||
+      (rc = c->q4_thr.alloc(STB_TICKET_SLOTS * STB_Q4_WORDS)) != STB_OK ||
+      (rc = c->q4_refined.alloc(1)) != STB_OK ||
+      (rc = c->coscan_off.alloc(STB_TICKET_SLOTS)) != STB_OK ||
+      (rc = c->hits_dev.alloc(1024)) != STB_OK ||
+      (rc = c->q_pin.alloc(STB_D)) != STB_OK ||
+      (rc = c->status_pin.alloc(8)) != STB_OK ||
+      (rc = c->hits_pin.alloc(1024)) != STB_OK)
+    goto fail;
+  if (cudaMemset(c->counters, 0, c->counters.cap * sizeof(unsigned int)) != cudaSuccess ||
       cudaMemset(c->tickets, 0, STB_TICKET_SLOTS * sizeof(unsigned long long)) != cudaSuccess ||
       cudaMemset(c->q4_thr, 0, STB_TICKET_SLOTS * STB_Q4_WORDS * sizeof(unsigned long long)) != cudaSuccess ||
       cudaMemset(c->q4_refined, 0, sizeof(unsigned long long)) != cudaSuccess ||
       cudaMemset(c->coscan_off, 0, STB_TICKET_SLOTS * sizeof(unsigned long long)) != cudaSuccess ||
       cudaMemset(c->err_flag, 0, sizeof(int)) != cudaSuccess ||
-      cudaMemset(c->embed_flag, 0, sizeof(int)) != cudaSuccess ||
-      cudaMallocHost((void **)&c->q_pin, STB_D * sizeof(float)) != cudaSuccess ||
-      cudaMallocHost((void **)&c->status_pin, 8 * sizeof(uint32_t)) != cudaSuccess ||
-      cudaMallocHost((void **)&c->hits_pin, 1024 * sizeof(stb_hit)) != cudaSuccess) {
+      cudaMemset(c->embed_flag, 0, sizeof(int)) != cudaSuccess) {
     stb_set_error("context staging allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
     rc = STB_ERR_NOMEM;
     goto fail;
   }
-  c->hits_pin_cap = 1024;
   { std::lock_guard<std::mutex> lk(g_ctx_mu); g_ctx_live.insert(c); }
   *out = c;
   return STB_OK;
@@ -161,27 +131,10 @@ int stb_ctx_destroy(stb_ctx *c) {
   { std::lock_guard<std::mutex> lk(g_ctx_mu); g_ctx_live.erase(c); }
   cudaSetDevice(c->device);
   cudaStreamSynchronize(c->stream);
-  cudaFree(c->block_keys); cudaFree(c->counters); cudaFree(c->q_dev); cudaFree(c->hits_dev);
-  cudaFree(c->status_dev); cudaFree(c->collect_rows); cudaFree(c->collect_count);
-  cudaFree(c->collect_hits); cudaFree(c->ranges_dev); cudaFree(c->err_flag); cudaFree(c->embed_flag);
-  cudaFree(c->tickets); cudaFree(c->q4_thr); cudaFree(c->q4_refined); cudaFree(c->coscan_off);
-  cudaFree(c->hist_dev); cudaFree(c->bq_tiles); cudaFree(c->b_submax); cudaFree(c->b_tilemax); cudaFree(c->b_cand);
-  cudaFree(c->b_thr); cudaFree(c->b_cnt); cudaFree(c->b_keys); cudaFree(c->b_qbad);
-  cudaFree(c->b_franges); cudaFree(c->b_ftiles); cudaFree(c->b_fbits);
-  cudaFree(c->s_work); cudaFree(c->s_qslots); cudaFree(c->s_qbad); free(c->s_map);
-  cudaFree(c->t_dst); cudaFree(c->t_segoff); cudaFree(c->t_cur); cudaFree(c->t_rq); cudaFree(c->t_rthr);
-  cudaFree(c->t_buf); cudaFree(c->t_off); cudaFree(c->t_slot); cudaFree(c->t_out_at); cudaFree(c->t_hits);
-  cudaFree(c->t_sort_tmp);
-  cudaFree(c->bq_dev); cudaFree(c->bh_dev); cudaFree(c->bs_dev); cudaFree(c->embed_off_dev); cudaFree(c->embed_ids_dev); cudaFree(c->embed_out_dev);
-  cudaFree(c->mut_stage); cudaFree(c->mut_idx); cudaFree(c->mut_flags);
-  if (c->q_pin) cudaFreeHost(c->q_pin);
-  if (c->hits_pin) cudaFreeHost(c->hits_pin);
-  if (c->status_pin) cudaFreeHost(c->status_pin);
-  if (c->many_q_pin) cudaFreeHost(c->many_q_pin);
-  if (c->many_status_pin) cudaFreeHost(c->many_status_pin);
-  if (c->own_stream && c->stream) cudaStreamDestroy(c->stream);
+  const cudaStream_t own = c->own_stream ? c->stream : nullptr;
+  delete c;   // the buffers go with it
+  if (own) cudaStreamDestroy(own);
   cudaGetLastError();
-  delete c;
   return STB_OK;
 }
 
@@ -262,20 +215,15 @@ int stb_table_load(stb_ctx *ctx, const float *E, uint64_t V, uint32_t D, const f
   if (V > 0xffffffffull) { stb_set_error("table_load: V exceeds 2^32 rows"); return STB_ERR_ARG; }
   stb_table *t = new (std::nothrow) stb_table();
   if (!t) { stb_set_error("out of host memory"); return STB_ERR_NOMEM; }
-  memset(t, 0, sizeof(*t));
   t->ctx = ctx; t->V = V; t->normalize = normalize ? 1 : 0;
   t->n_weights = weights ? n_weights : 0;
   t->n_mapping = mapping ? n_mapping : 0;
-  cudaError_t e = cudaMalloc((void **)&t->E, V * STB_D * sizeof(float));
-  if (e == cudaSuccess && t->n_weights) e = cudaMalloc((void **)&t->weights, t->n_weights * sizeof(float));
-  if (e == cudaSuccess && t->n_mapping) e = cudaMalloc((void **)&t->mapping, t->n_mapping * sizeof(uint32_t));
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    stb_set_error("table_load: device allocation failed: %s", cudaGetErrorString(e));
+  if ((rc = t->E.alloc(V * STB_D)) != STB_OK || (t->n_weights && (rc = t->weights.alloc(t->n_weights)) != STB_OK) ||
+      (t->n_mapping && (rc = t->mapping.alloc(t->n_mapping)) != STB_OK)) {
     stb_table_destroy(t);
-    return STB_ERR_NOMEM;
+    return rc;
   }
-  e = cudaMemcpyAsync(t->E, E, V * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream);
+  cudaError_t e = cudaMemcpyAsync(t->E, E, V * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream);
   if (e == cudaSuccess && t->n_weights)
     e = cudaMemcpyAsync(t->weights, weights, t->n_weights * sizeof(float), cudaMemcpyHostToDevice, ctx->stream);
   if (e == cudaSuccess && t->n_mapping)
@@ -294,38 +242,39 @@ int stb_table_destroy(stb_table *t) {
   if (!t) return STB_OK;
   if (t->ctx && ctx_alive(t->ctx)) { cudaSetDevice(t->ctx->device); cudaStreamSynchronize(t->ctx->stream); }
   else cudaDeviceSynchronize();
-  cudaFree(t->E); cudaFree(t->weights); cudaFree(t->mapping);
   cudaGetLastError();
   delete t;
   return STB_OK;
 }
 
 // -------------------------------------------------------------------- corpus ---
+// A grown corpus copy gets the first `bytes` of the old one: copied on the stream and waited for, also when the
+// copy fails, so either buffer may be freed on return.
+static int copy_prefix(stb_ctx *ctx, void *dst, const void *src, size_t bytes) {
+  cudaError_t e = bytes ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, ctx->stream) : cudaSuccess;
+  const cudaError_t se = cudaStreamSynchronize(ctx->stream);
+  if (e == cudaSuccess) e = se;
+  if (e != cudaSuccess) { stb_set_error("corpus grow copy: %s", cudaGetErrorString(e)); return STB_ERR_CUDA; }
+  return STB_OK;
+}
+
 // q8 copy of `cap` rows (int8 codes + scales, 260 B/row, and the top-k prefilter's nibble plane + {s, rho},
 // 136 B/row) with the first `keep` rows of the current one; nothing changes when an allocation fails.
 static int q8_realloc(stb_corpus *c, uint64_t cap, uint64_t keep) {
-  stb_ctx *ctx = c->ctx;
-  uint8_t *np = nullptr, *pp = nullptr;
-  float *ns = nullptr;
-  float2 *sp = nullptr;
-  cudaError_t e = cudaMalloc((void **)&np, cap * 256ull);
-  if (e == cudaSuccess) e = cudaMalloc((void **)&ns, cap * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc((void **)&pp, stb_q4_plane_bytes(cap));
-  if (e == cudaSuccess) e = cudaMalloc((void **)&sp, cap * sizeof(float2));
-  if (e != cudaSuccess) {
-    cudaGetLastError(); cudaFree(np); cudaFree(ns); cudaFree(pp);
-    stb_set_error("q8 tier: cannot allocate %llu MiB", (unsigned long long)(cap * 396 >> 20));
-    return STB_ERR_NOMEM;
-  }
-  if (c->q8 && keep) {
-    STB_CUDA(cudaMemcpyAsync(np, c->q8, keep * 256ull, cudaMemcpyDeviceToDevice, ctx->stream));
-    STB_CUDA(cudaMemcpyAsync(ns, c->q8_scale, keep * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
-    STB_CUDA(cudaMemcpyAsync(pp, c->q4, stb_q4_plane_bytes(keep), cudaMemcpyDeviceToDevice, ctx->stream));   // whole tiles
-    STB_CUDA(cudaMemcpyAsync(sp, c->q4_sr, keep * sizeof(float2), cudaMemcpyDeviceToDevice, ctx->stream));
-    STB_CUDA(cudaStreamSynchronize(ctx->stream));
-  }
-  cudaFree(c->q8); cudaFree(c->q8_scale); cudaFree(c->q4); cudaFree(c->q4_sr);
-  c->q8 = np; c->q8_scale = ns; c->q4 = pp; c->q4_sr = sp; c->q8_cap_rows = cap;
+  StbBuf<uint8_t> q8, q4;
+  StbBuf<float> scale;
+  StbBuf<float2> sr;
+  int rc;
+  if ((rc = q8.alloc(cap * 256ull)) != STB_OK || (rc = scale.alloc(cap)) != STB_OK ||
+      (rc = q4.alloc(stb_q4_plane_bytes(cap))) != STB_OK || (rc = sr.alloc(cap)) != STB_OK)
+    return rc;
+  if (c->q8 && keep &&
+      ((rc = copy_prefix(c->ctx, q8, c->q8, keep * 256ull)) != STB_OK ||
+       (rc = copy_prefix(c->ctx, scale, c->q8_scale, keep * sizeof(float))) != STB_OK ||
+       (rc = copy_prefix(c->ctx, q4, c->q4, stb_q4_plane_bytes(keep))) != STB_OK ||   // whole tiles
+       (rc = copy_prefix(c->ctx, sr, c->q4_sr, keep * sizeof(float2))) != STB_OK))
+    return rc;
+  c->q8 = std::move(q8); c->q8_scale = std::move(scale); c->q4 = std::move(q4); c->q4_sr = std::move(sr);
   return STB_OK;
 }
 
@@ -360,20 +309,12 @@ static int corpus_reserve(stb_corpus *c, uint64_t need) {
   if (need > 0xfffffffeull) { stb_set_error("corpus shard exceeds 2^32-2 rows; shard it"); return STB_ERR_ARG; }
   uint64_t ncap = std::max<uint64_t>(std::max<uint64_t>(need, 1024), c->capacity + c->capacity / 2);
   if (c->host_rows) return host_corpus_reserve(c, ncap);
-  float *np = nullptr;
-  cudaError_t e = cudaMalloc((void **)&np, ncap * STB_D * sizeof(float));
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    stb_set_error("corpus: cudaMalloc(%llu rows) failed: %s", (unsigned long long)ncap, cudaGetErrorString(e));
-    return STB_ERR_NOMEM;
-  }
-  if (c->rows && c->n) {
-    e = cudaMemcpyAsync(np, c->rows, c->n * STB_D * sizeof(float), cudaMemcpyDeviceToDevice, c->ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->ctx->stream);
-    if (e != cudaSuccess) { cudaFree(np); stb_set_error("corpus grow copy: %s", cudaGetErrorString(e)); return STB_ERR_CUDA; }
-  }
-  if (c->rows) cudaFree(c->rows);
-  c->rows = np;
+  StbBuf<float> grown;
+  int rc;
+  if ((rc = grown.alloc(ncap * STB_D)) != STB_OK) return rc;
+  if (c->rows && c->n && (rc = copy_prefix(c->ctx, grown, c->rows, c->n * STB_D * sizeof(float))) != STB_OK) return rc;
+  c->dev_rows = std::move(grown);
+  c->rows = c->dev_rows;
   c->capacity = ncap;
   return STB_OK;
 }
@@ -385,7 +326,6 @@ int stb_corpus_create(stb_ctx *ctx, uint32_t D, uint64_t capacity_rows, uint64_t
   if (D != STB_D) { stb_set_error("corpus_create: D=%u, only %u supported", D, STB_D); return STB_ERR_ARG; }
   stb_corpus *c = new (std::nothrow) stb_corpus();
   if (!c) { stb_set_error("out of host memory"); return STB_ERR_NOMEM; }
-  memset(c, 0, sizeof(*c));
   c->ctx = ctx; c->row_base = row_base;
   rc = corpus_reserve(c, std::max<uint64_t>(capacity_rows, 1));
   if (rc) { delete c; return rc; }
@@ -401,7 +341,6 @@ int stb_corpus_create_host(stb_ctx *ctx, uint32_t D, uint64_t capacity_rows, uin
   if (capacity_rows > 0xfffffffeull) { stb_set_error("corpus shard exceeds 2^32-2 rows; shard it"); return STB_ERR_ARG; }
   stb_corpus *c = new (std::nothrow) stb_corpus();
   if (!c) { stb_set_error("out of host memory"); return STB_ERR_NOMEM; }
-  memset(c, 0, sizeof(*c));
   c->ctx = ctx; c->row_base = row_base; c->host_rows = 1;
   rc = host_corpus_reserve(c, std::max<uint64_t>(capacity_rows, 1));
   if (rc) { delete c; return rc; }
@@ -413,13 +352,7 @@ int stb_corpus_destroy(stb_corpus *c) {
   if (!c) return STB_OK;
   if (c->ctx && ctx_alive(c->ctx)) { cudaSetDevice(c->ctx->device); cudaStreamSynchronize(c->ctx->stream); }
   else cudaDeviceSynchronize();
-  cudaFree(c->shadow);
-  cudaFree(c->q8);
-  cudaFree(c->q8_scale);
-  cudaFree(c->q4);
-  cudaFree(c->q4_sr);
   if (c->host_rows) cudaFreeHost(c->rows_host);
-  else cudaFree(c->rows);
   cudaGetLastError();
   delete c;
   return STB_OK;
@@ -456,8 +389,8 @@ static int host_append_begin(stb_corpus *c, uint64_t n, uint64_t stage_rows) {
   stb_ctx *ctx = c->ctx;
   int rc;
   if ((rc = corpus_reserve(c, c->n + n)) != STB_OK) return rc;
-  if (stage_rows && (rc = dev_reserve(&ctx->mut_stage, &ctx->mut_stage_cap, stage_rows * STB_D)) != STB_OK) return rc;
-  if ((rc = dev_reserve(&ctx->mut_flags, &ctx->mut_flags_cap, 2)) != STB_OK) return rc;
+  if (stage_rows && (rc = ctx->mut_stage.reserve(stage_rows * STB_D)) != STB_OK) return rc;
+  if ((rc = ctx->mut_flags.reserve(2)) != STB_OK) return rc;
   STB_CUDA(cudaMemsetAsync(ctx->mut_flags, 0, 2 * sizeof(int), ctx->stream));
   return STB_OK;
 }
@@ -558,8 +491,8 @@ int stb_embed(stb_ctx *ctx, const stb_table *table, const uint64_t *offsets, con
   for (uint64_t i = 0; i < n_lines; ++i)
     if (offsets[i + 1] < offsets[i]) { stb_set_error("embed: offsets not monotone at line %llu", (unsigned long long)i); return STB_ERR_ARG; }
   if (total && !ids) { stb_set_error("embed: ids is null"); return STB_ERR_ARG; }
-  if ((rc = dev_reserve(&ctx->embed_off_dev, &ctx->embed_off_cap, n_lines + 1, 4096)) != STB_OK) return rc;
-  if ((rc = dev_reserve(&ctx->embed_ids_dev, &ctx->embed_ids_cap, std::max<uint64_t>(total, 1), 65536)) != STB_OK) return rc;
+  if ((rc = ctx->embed_off_dev.reserve(n_lines + 1, 4096)) != STB_OK) return rc;
+  if ((rc = ctx->embed_ids_dev.reserve(std::max<uint64_t>(total, 1), 65536)) != STB_OK) return rc;
   if (append_to && append_to->host_rows) {
     // K3 writes chunks of lines into the staging buffer; each chunk is committed to the host rows and its q8
     // entries from there.  The rows are booked only if no token was out of range.
@@ -586,7 +519,7 @@ int stb_embed(stb_ctx *ctx, const stb_table *table, const uint64_t *offsets, con
     if ((rc = corpus_reserve(append_to, append_to->n + n_lines)) != STB_OK) return rc;
     dst = append_to->rows + append_to->n * STB_D;
   } else {
-    if ((rc = dev_reserve(&ctx->embed_out_dev, &ctx->embed_out_cap, n_lines * STB_D, 4096 * STB_D)) != STB_OK) return rc;
+    if ((rc = ctx->embed_out_dev.reserve(n_lines * STB_D, 4096 * STB_D)) != STB_OK) return rc;
     dst = ctx->embed_out_dev;
   }
   STB_CUDA(cudaMemcpyAsync(ctx->embed_off_dev, offsets, (n_lines + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->stream));
@@ -697,21 +630,6 @@ static int host_rows_refuse(const stb_corpus *c, const char *what) {
   return STB_OK;
 }
 
-static int ensure_hits_pin(stb_ctx *ctx, size_t need) {
-  if (need <= ctx->hits_pin_cap) return STB_OK;
-  stb_hit *np = nullptr;
-  size_t ncap = std::max(need, ctx->hits_pin_cap * 2);
-  if (cudaMallocHost((void **)&np, ncap * sizeof(stb_hit)) != cudaSuccess) {
-    cudaGetLastError();
-    stb_set_error("pinned staging allocation failed");
-    return STB_ERR_NOMEM;
-  }
-  cudaFreeHost(ctx->hits_pin);
-  ctx->hits_pin = np;
-  ctx->hits_pin_cap = ncap;
-  return STB_OK;
-}
-
 // The distance cap of a top-k result sorted by (distance, row): how many leading hits have distance <
 // max_distance (strict; a NaN cap passes none).  Where top_k always caps (store-query mode, the top-k fast
 // path) the capped result is this prefix of the uncapped one.
@@ -744,7 +662,7 @@ static int k1_upload_ranges(stb_ctx *ctx, const stb_corpus *c, const char *what,
   *n_loc = (uint32_t)rbegin.size();
   std::vector<uint64_t> packed(vstart);
   packed.insert(packed.end(), rbegin.begin(), rbegin.end());
-  if ((rc = dev_reserve(&ctx->ranges_dev, &ctx->ranges_cap, packed.size(), 4096)) != STB_OK) return rc;
+  if ((rc = ctx->ranges_dev.reserve(packed.size(), 4096)) != STB_OK) return rc;
   STB_CUDA(cudaMemcpyAsync(ctx->ranges_dev, packed.data(), packed.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->stream));
   STB_CUDA(cudaStreamSynchronize(ctx->stream));   // `packed` dies at scope end
   *ranges_dev = ctx->ranges_dev;
@@ -759,18 +677,18 @@ static int collect_exact_sorted(stb_ctx *ctx, const stb_corpus *c, float cos_flo
                                 uint64_t *n_pass, int tier = STB_TIER_F32) {
   int rc;
   unsigned long long count = 0;
-  if ((rc = dev_reserve(&ctx->collect_rows, &ctx->collect_cap, 1, 1u << 20)) != STB_OK) return rc;
+  if ((rc = ctx->collect_rows.reserve(1, 1u << 20)) != STB_OK) return rc;
   for (int attempt = 0; attempt < 3; ++attempt) {
     if ((rc = stb_launch_scan_collect(ctx, c, tier, ctx->q_dev, cos_floor, ranges_dev, n_ranges, n_virtual)) != STB_OK) return rc;
     STB_CUDA(cudaMemcpyAsync(&count, ctx->collect_count, sizeof(count), cudaMemcpyDeviceToHost, ctx->stream));
     STB_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (count <= ctx->collect_cap) break;
-    if ((rc = dev_reserve(&ctx->collect_rows, &ctx->collect_cap, (size_t)count)) != STB_OK) return rc;
+    if (count <= ctx->collect_rows.cap) break;
+    if ((rc = ctx->collect_rows.reserve((size_t)count)) != STB_OK) return rc;
   }
-  if (count > ctx->collect_cap) { stb_set_error("collect buffer could not be sized"); return STB_ERR_STATE; }
+  if (count > ctx->collect_rows.cap) { stb_set_error("collect buffer could not be sized"); return STB_ERR_STATE; }
   uint64_t m = count, m_padded = 1024;
   while (m_padded < m) m_padded <<= 1;
-  if ((rc = dev_reserve(&ctx->collect_hits, &ctx->collect_hits_cap, (size_t)m_padded)) != STB_OK) return rc;
+  if ((rc = ctx->collect_hits.reserve((size_t)m_padded)) != STB_OK) return rc;
   if ((rc = stb_launch_exact(ctx, c->rows, c->row_base, ctx->q_dev, ctx->collect_rows, m, limit,
                              ctx->collect_hits, m_padded, ctx->collect_count + 1)) != STB_OK) return rc;
   if ((rc = stb_launch_sort_hits(ctx, ctx->collect_hits, m_padded)) != STB_OK) return rc;
@@ -985,20 +903,19 @@ static int xchg_create_impl(stb_ctx *ctx, uint32_t world, uint32_t rank, uint32_
   if (max_nq > 65536 || (uint64_t)world * max_k > 2048) { stb_set_error("xchg_create: batch area too large (max_nq <= 65536, world * max_k <= 2048)"); return STB_ERR_ARG; }
   stb_xchg *x = new (std::nothrow) stb_xchg();
   if (!x) { stb_set_error("out of host memory"); return STB_ERR_NOMEM; }
-  memset(x, 0, sizeof(*x));
   x->ctx = ctx; x->world = world; x->rank = rank; x->max_k = max_k; x->max_nq = max_nq;
   x->batch_off = (xchg_bytes(world, max_k) + 255) & ~(size_t)255;
   x->batch_slot_bytes = max_nq ? xchg_batch_slot_bytes(world, max_nq, max_k) : 0;
   x->bytes = x->batch_off + 2 * x->batch_slot_bytes;
-  // plain cudaMalloc memory: required for cudaIpcGetMemHandle
-  cudaError_t e = cudaMalloc((void **)&x->local, x->bytes);
-  if (e == cudaSuccess) e = cudaMemset(x->local, 0, x->bytes);
-  if (e == cudaSuccess) e = cudaMalloc((void **)&x->batch_ticket, sizeof(unsigned int));
+  // plain device memory: required for cudaIpcGetMemHandle
+  if ((rc = x->local.alloc(x->bytes)) != STB_OK || (rc = x->batch_ticket.alloc(1)) != STB_OK) { delete x; return rc; }
+  cudaError_t e = cudaMemset(x->local, 0, x->bytes);
   if (e == cudaSuccess) e = cudaMemset(x->batch_ticket, 0, sizeof(unsigned int));
   // cudaMemset on device memory may return before it ran (legacy default stream, which a non-blocking
   // stream does not order against): the zeroed flags must be in place before any peer can store to them
-  if (e == cudaSuccess) e = cudaDeviceSynchronize();
-  if (e != cudaSuccess) { cudaGetLastError(); cudaFree(x->local); stb_set_error("xchg_create: %s", cudaGetErrorString(e)); delete x; return STB_ERR_NOMEM; }
+  const cudaError_t se = cudaDeviceSynchronize();
+  if (e == cudaSuccess) e = se;
+  if (e != cudaSuccess) { cudaGetLastError(); stb_set_error("xchg_create: %s", cudaGetErrorString(e)); delete x; return STB_ERR_NOMEM; }
   x->peers[rank] = x->local;
   x->connected = (world == 1);
   *out = x;
@@ -1019,8 +936,6 @@ int stb_xchg_destroy(stb_xchg *x) {
   else cudaDeviceSynchronize();
   for (uint32_t r = 0; r < x->world; ++r)
     if (x->ipc_opened[r] && x->peers[r]) cudaIpcCloseMemHandle(x->peers[r]);
-  cudaFree(x->batch_ticket);
-  cudaFree(x->local);
   cudaGetLastError();
   delete x;
   return STB_OK;
@@ -1111,7 +1026,7 @@ static int host_rows_staged(stb_corpus *c, uint64_t first, F &&fn) {
   if (first >= c->n) return STB_OK;
   const uint64_t chunk = std::min<uint64_t>(c->n - first, STB_MUT_CHUNK_ROWS);
   int rc;
-  if ((rc = dev_reserve(&ctx->mut_stage, &ctx->mut_stage_cap, chunk * STB_D)) != STB_OK) return rc;
+  if ((rc = ctx->mut_stage.reserve(chunk * STB_D)) != STB_OK) return rc;
   for (uint64_t r0 = first; r0 < c->n; r0 += chunk) {
     const uint64_t m = std::min(chunk, c->n - r0);
     STB_CUDA(cudaMemcpyAsync(ctx->mut_stage, c->rows_host + r0 * STB_D, m * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
@@ -1128,19 +1043,14 @@ static int corpus_ensure_shadow(stb_ctx *ctx, stb_corpus *c) {
   }
   const uint64_t tiles = (c->n + 255) / 256;
   uint64_t first = (c->shadow && c->shadow_rows < c->n && !c->shadow_bad) ? (c->shadow_rows / 256) * 256 : 0;   // valid prefix, whole tiles
-  if (tiles > c->shadow_cap_tiles || !c->shadow) {
-    uint8_t *np = nullptr;
-    const uint64_t cap_tiles = std::max<uint64_t>(tiles, (c->capacity + 255) / 256);
-    cudaError_t e = cudaMalloc((void **)&np, cap_tiles * 131072ull);
-    if (e != cudaSuccess) { cudaGetLastError(); stb_set_error("search_batch: cannot allocate the %llu MiB 16-bit shadow", (unsigned long long)(cap_tiles >> 3)); return STB_ERR_NOMEM; }
-    if (c->shadow && first) STB_CUDA(cudaMemcpyAsync(np, c->shadow, (first / 256) * 131072ull, cudaMemcpyDeviceToDevice, ctx->stream));
-    else first = 0;
-    STB_CUDA(cudaStreamSynchronize(ctx->stream));
-    cudaFree(c->shadow);
-    c->shadow = np;
-    c->shadow_cap_tiles = cap_tiles;
-  }
   int rc;
+  if (tiles * 131072ull > c->shadow.cap || !c->shadow) {
+    StbBuf<uint8_t> grown;
+    if ((rc = grown.alloc(std::max<uint64_t>(tiles, (c->capacity + 255) / 256) * 131072ull)) != STB_OK ||
+        (rc = copy_prefix(ctx, grown, c->shadow, (first / 256) * 131072ull)) != STB_OK)
+      return rc;
+    c->shadow = std::move(grown);
+  }
   STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
   if (c->host_rows)
     rc = host_rows_staged(c, first, [&](const float *stage, uint64_t r0, uint64_t r1) {
@@ -1166,7 +1076,7 @@ static int corpus_ensure_q8(stb_ctx *ctx, stb_corpus *c) {
   }
   uint64_t first = (c->q8 && c->q8_rows < c->n && !c->q8_bad) ? c->q8_rows : 0;      // valid prefix: convert only the new rows
   int rc;
-  if (c->n > c->q8_cap_rows || !c->q8) {
+  if (c->n > c->q8_scale.cap || !c->q8) {
     if ((rc = q8_realloc(c, std::max<uint64_t>(c->n, c->capacity), first)) != STB_OK) return rc;
   }
   STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
@@ -1236,7 +1146,7 @@ static StbCorpusWriteArgs corpus_write_args(stb_corpus *c, uint64_t q8_rows, uin
   StbCorpusWriteArgs a;
   memset(&a, 0, sizeof(a));
   a.rows = reinterpret_cast<float4 *>(c->rows);
-  a.stage = reinterpret_cast<const float4 *>(c->ctx->mut_stage);
+  a.stage = reinterpret_cast<const float4 *>(c->ctx->mut_stage.p);
   a.q8 = c->q8; a.q8_scale = c->q8_scale; a.q4 = c->q4; a.q4_sr = c->q4_sr;
   a.q8_rows = c->q8 ? q8_rows : 0;
   a.shadow = c->shadow;
@@ -1281,9 +1191,9 @@ int stb_corpus_update_impl(stb_corpus *c, const uint64_t *idx, const float *rows
   }
   stb_ctx *ctx = c->ctx;
   const uint64_t chunk = std::min<uint64_t>(n, STB_MUT_CHUNK_ROWS);
-  if ((rc = dev_reserve(&ctx->mut_stage, &ctx->mut_stage_cap, chunk * STB_D)) != STB_OK) return rc;
-  if ((rc = dev_reserve(&ctx->mut_idx, &ctx->mut_idx_cap, chunk)) != STB_OK) return rc;
-  if ((rc = dev_reserve(&ctx->mut_flags, &ctx->mut_flags_cap, 2)) != STB_OK) return rc;
+  if ((rc = ctx->mut_stage.reserve(chunk * STB_D)) != STB_OK) return rc;
+  if ((rc = ctx->mut_idx.reserve(chunk)) != STB_OK) return rc;
+  if ((rc = ctx->mut_flags.reserve(2)) != STB_OK) return rc;
   if (hook) {
     // the hook sees its rows in the staging buffer before anything is written; an update of one chunk stays
     // staged for the write below, a larger one is uploaded again
@@ -1355,11 +1265,11 @@ int stb_corpus_remove_impl(stb_corpus *c, const uint64_t *ranges, uint32_t n_ran
   }
   const uint64_t moved = dst - first;
   const uint64_t q8_rows = q8_had - removed_q8, shadow_rows = shadow_had - removed_shadow;
-  if ((rc = dev_reserve(&ctx->mut_flags, &ctx->mut_flags_cap, 2)) != STB_OK) return rc;
+  if ((rc = ctx->mut_flags.reserve(2)) != STB_OK) return rc;
   if (moved) {
     const uint64_t chunk = std::min<uint64_t>(moved, STB_MUT_CHUNK_ROWS);
-    if ((rc = dev_reserve(&ctx->mut_stage, &ctx->mut_stage_cap, chunk * STB_D)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->mut_idx, &ctx->mut_idx_cap, seg.size())) != STB_OK) return rc;
+    if ((rc = ctx->mut_stage.reserve(chunk * STB_D)) != STB_OK) return rc;
+    if ((rc = ctx->mut_idx.reserve(seg.size())) != STB_OK) return rc;
   }
   if (hook && ((rc = hook->begin()) != STB_OK || (rc = hook->ready()) != STB_OK)) return rc;
   corpus_drop_bad_copies(c);
@@ -1481,12 +1391,12 @@ static int batch_v2_run(stb_ctx *ctx, const stb_corpus *corpus, const float *q_d
   const uint32_t n_seg = stb_batch_emit_grid(ctx, n_emit);
   const uint32_t last[6] = {tile_ids ? 3u : 2u, nq, p.n_sample, p.stride, n_seg, kSegCap};
   memcpy(ctx->b_last, last, sizeof(last));
-  if ((rc = dev_reserve(&ctx->b_qbad, &ctx->b_qbad_cap, (size_t)q_pad)) != STB_OK) return rc;
-  if ((rc = dev_reserve(&ctx->bq_tiles, &ctx->bq_tiles_cap, (size_t)q_pad * 512)) != STB_OK) return rc;
-  if ((rc = dev_reserve(&ctx->b_tilemax, &ctx->b_tilemax_cap, (size_t)p.n_sample * q_pad)) != STB_OK) return rc;
-  if ((rc = dev_reserve(&ctx->b_thr, &ctx->b_thr_cap, (size_t)q_pad)) != STB_OK) return rc;
-  if ((rc = dev_reserve(&ctx->b_cnt, &ctx->b_cnt_cap, (size_t)q_pad * n_seg)) != STB_OK) return rc;
-  if ((rc = dev_reserve(&ctx->b_keys, &ctx->b_keys_cap, (size_t)q_pad * n_seg * kSegCap)) != STB_OK) return rc;
+  if ((rc = ctx->b_qbad.reserve((size_t)q_pad)) != STB_OK) return rc;
+  if ((rc = ctx->bq_tiles.reserve((size_t)q_pad * 512)) != STB_OK) return rc;
+  if ((rc = ctx->b_tilemax.reserve((size_t)p.n_sample * q_pad)) != STB_OK) return rc;
+  if ((rc = ctx->b_thr.reserve((size_t)q_pad)) != STB_OK) return rc;
+  if ((rc = ctx->b_cnt.reserve((size_t)q_pad * n_seg)) != STB_OK) return rc;
+  if ((rc = ctx->b_keys.reserve((size_t)q_pad * n_seg * kSegCap)) != STB_OK) return rc;
   STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
   STB_CUDA(cudaMemsetAsync(ctx->b_cnt, 0, (size_t)q_pad * n_seg * sizeof(uint32_t), ctx->stream));
   if ((rc = stb_launch_shadow_build(ctx, q_dev, nq, 128, ctx->bq_tiles, ctx->err_flag, 0, ctx->b_qbad)) != STB_OK) return rc;
@@ -1531,17 +1441,17 @@ int stb_search_batch_dev(stb_ctx *ctx, const stb_corpus *corpus_c, const float *
   if (plan.fits) return batch_v2_run(ctx, corpus, q_dev, nq, top_k, n_full, plan, nullptr, nullptr, out_hits_dev, out_status_dev);
   // one flag per query, written by the query shadow build: a query that cannot be normalised in fp32
   // has a zero (or NaN) shadow whose scores bound nothing, and both finish kernels report it unproven
-  if ((rc = dev_reserve(&ctx->b_qbad, &ctx->b_qbad_cap, (size_t)q_pad)) != STB_OK) return rc;
+  if ((rc = ctx->b_qbad.reserve((size_t)q_pad)) != STB_OK) return rc;
   const uint32_t last[6] = {1u, nq, 0u, 0u, 0u, 0u};
   memcpy(ctx->b_last, last, sizeof(last));
   // selection slices: enough CTAs (m_tiles x n_slices) to hide the latency of the streaming
   // read; the finish kernel merges n_slices x 32 <= 4096 candidate tiles per query
   uint32_t n_slices = std::max<uint32_t>(1, std::min<uint32_t>(128, 1536 / m_tiles));
   n_slices = std::min<uint32_t>(n_slices, std::max<uint32_t>(1, n_tiles / 48));
-  if ((rc = dev_reserve(&ctx->bq_tiles, &ctx->bq_tiles_cap, (size_t)q_pad * 512)) != STB_OK) return rc;
-  if ((rc = dev_reserve(&ctx->b_submax, &ctx->b_submax_cap, (size_t)n_sub * q_pad)) != STB_OK) return rc;
-  if ((rc = dev_reserve(&ctx->b_tilemax, &ctx->b_tilemax_cap, (size_t)n_tiles * q_pad)) != STB_OK) return rc;
-  if ((rc = dev_reserve(&ctx->b_cand, &ctx->b_cand_cap, (size_t)q_pad * n_slices * 32)) != STB_OK) return rc;
+  if ((rc = ctx->bq_tiles.reserve((size_t)q_pad * 512)) != STB_OK) return rc;
+  if ((rc = ctx->b_submax.reserve((size_t)n_sub * q_pad)) != STB_OK) return rc;
+  if ((rc = ctx->b_tilemax.reserve((size_t)n_tiles * q_pad)) != STB_OK) return rc;
+  if ((rc = ctx->b_cand.reserve((size_t)q_pad * n_slices * 32)) != STB_OK) return rc;
   // query tiles: padding queries beyond nq are written as zeros by the shadow builder
   STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
   if ((rc = stb_launch_shadow_build(ctx, q_dev, nq, 128, ctx->bq_tiles, ctx->err_flag, 0, ctx->b_qbad)) != STB_OK) return rc;
@@ -1564,9 +1474,9 @@ int stb_search_batch(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uin
   bool tensor_ok = top_k <= 1024;
   std::vector<uint32_t> status((size_t)nq * 2, 0);
   if (tensor_ok) {
-    if ((rc = dev_reserve(&ctx->bq_dev, &ctx->bq_dev_cap, (size_t)nq * STB_D)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->bh_dev, &ctx->bh_dev_cap, (size_t)nq * top_k)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->bs_dev, &ctx->bs_dev_cap, (size_t)nq * 2)) != STB_OK) return rc;
+    if ((rc = ctx->bq_dev.reserve((size_t)nq * STB_D)) != STB_OK) return rc;
+    if ((rc = ctx->bh_dev.reserve((size_t)nq * top_k)) != STB_OK) return rc;
+    if ((rc = ctx->bs_dev.reserve((size_t)nq * 2)) != STB_OK) return rc;
     STB_CUDA(cudaMemcpyAsync(ctx->bq_dev, q, (size_t)nq * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
     rc = stb_search_batch_dev(ctx, corpus, ctx->bq_dev, nq, top_k, ctx->bh_dev, ctx->bs_dev);
     if (rc == STB_ERR_STATE) { tensor_ok = false; }        // un-normalisable rows: K1 handles them
@@ -1645,12 +1555,12 @@ int stb_search_batch_filtered(stb_ctx *ctx, const stb_corpus *corpus_c, const fl
   std::vector<uint32_t> status((size_t)nq * 2, 0);
   if (tensor_ok) {
     const uint64_t n_words = (corpus->n + 255) / 256 * 8;
-    if ((rc = dev_reserve(&ctx->bq_dev, &ctx->bq_dev_cap, (size_t)nq * STB_D)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->bh_dev, &ctx->bh_dev_cap, (size_t)nq * top_k)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->bs_dev, &ctx->bs_dev_cap, (size_t)nq * 2)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->b_franges, &ctx->b_franges_cap, loc.size(), 2048)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->b_ftiles, &ctx->b_ftiles_cap, tiles.size(), 1024)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->b_fbits, &ctx->b_fbits_cap, (size_t)n_words)) != STB_OK) return rc;
+    if ((rc = ctx->bq_dev.reserve((size_t)nq * STB_D)) != STB_OK) return rc;
+    if ((rc = ctx->bh_dev.reserve((size_t)nq * top_k)) != STB_OK) return rc;
+    if ((rc = ctx->bs_dev.reserve((size_t)nq * 2)) != STB_OK) return rc;
+    if ((rc = ctx->b_franges.reserve(loc.size(), 2048)) != STB_OK) return rc;
+    if ((rc = ctx->b_ftiles.reserve(tiles.size(), 1024)) != STB_OK) return rc;
+    if ((rc = ctx->b_fbits.reserve((size_t)n_words)) != STB_OK) return rc;
     STB_CUDA(cudaMemcpyAsync(ctx->bq_dev, q, (size_t)nq * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
     STB_CUDA(cudaMemcpyAsync(ctx->b_franges, loc.data(), loc.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
     STB_CUDA(cudaMemcpyAsync(ctx->b_ftiles, tiles.data(), tiles.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
@@ -1880,20 +1790,20 @@ int stb_search_batch_subsets(stb_ctx *ctx, const stb_corpus *corpus_c, const flo
       rr_off[tg + 1] = (uint32_t)rr.size();
     }
     const uint64_t n_words = (uint64_t)n_tiles * 8;
-    if ((rc = dev_reserve(&ctx->s_work, &ctx->s_work_cap, up.size())) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->b_franges, &ctx->b_franges_cap, rr.size(), 2048)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->b_fbits, &ctx->b_fbits_cap, (size_t)(T * n_words + 8))) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->bq_dev, &ctx->bq_dev_cap, (size_t)nt * STB_D)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->s_qslots, &ctx->s_qslots_cap, (size_t)q_pad * STB_D)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->s_qbad, &ctx->s_qbad_cap, (size_t)nt)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->b_qbad, &ctx->b_qbad_cap, (size_t)q_pad)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->bq_tiles, &ctx->bq_tiles_cap, (size_t)q_pad * 512)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->b_tilemax, &ctx->b_tilemax_cap, (size_t)n_cols * q_pad)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->b_thr, &ctx->b_thr_cap, (size_t)q_pad)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->b_cnt, &ctx->b_cnt_cap, (size_t)nt * n_seg)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->b_keys, &ctx->b_keys_cap, (size_t)nt * n_seg * kSegCap)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->bh_dev, &ctx->bh_dev_cap, (size_t)nt * top_k)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->bs_dev, &ctx->bs_dev_cap, (size_t)nt * 2)) != STB_OK) return rc;
+    if ((rc = ctx->s_work.reserve(up.size())) != STB_OK) return rc;
+    if ((rc = ctx->b_franges.reserve(rr.size(), 2048)) != STB_OK) return rc;
+    if ((rc = ctx->b_fbits.reserve((size_t)(T * n_words + 8))) != STB_OK) return rc;
+    if ((rc = ctx->bq_dev.reserve((size_t)nt * STB_D)) != STB_OK) return rc;
+    if ((rc = ctx->s_qslots.reserve((size_t)q_pad * STB_D)) != STB_OK) return rc;
+    if ((rc = ctx->s_qbad.reserve((size_t)nt)) != STB_OK) return rc;
+    if ((rc = ctx->b_qbad.reserve((size_t)q_pad)) != STB_OK) return rc;
+    if ((rc = ctx->bq_tiles.reserve((size_t)q_pad * 512)) != STB_OK) return rc;
+    if ((rc = ctx->b_tilemax.reserve((size_t)n_cols * q_pad)) != STB_OK) return rc;
+    if ((rc = ctx->b_thr.reserve((size_t)q_pad)) != STB_OK) return rc;
+    if ((rc = ctx->b_cnt.reserve((size_t)nt * n_seg)) != STB_OK) return rc;
+    if ((rc = ctx->b_keys.reserve((size_t)nt * n_seg * kSegCap)) != STB_OK) return rc;
+    if ((rc = ctx->bh_dev.reserve((size_t)nt * top_k)) != STB_OK) return rc;
+    if ((rc = ctx->bs_dev.reserve((size_t)nt * 2)) != STB_OK) return rc;
     std::vector<float> qc((size_t)nt * STB_D);
     for (uint32_t r = 0; r < nt; ++r) memcpy(qc.data() + (size_t)r * STB_D, q + (size_t)qrow[r] * STB_D, STB_D * sizeof(float));
     STB_CUDA(cudaMemcpyAsync(ctx->s_work, up.data(), up.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
@@ -1925,14 +1835,8 @@ int stb_search_batch_subsets(stb_ctx *ctx, const stb_corpus *corpus_c, const flo
     STB_CUDA(cudaStreamSynchronize(ctx->stream));           // the host arrays above are read by the copies
   }
   // each caller query's slot and compact row, for stb_debug_batch_last
-  if (ctx->s_map_cap < 2 * (size_t)nq) {
-    uint32_t *m = (uint32_t *)realloc(ctx->s_map, 2 * (size_t)nq * sizeof(uint32_t));
-    if (!m) { stb_set_error("search_batch_subsets: host allocation failed"); return STB_ERR_NOMEM; }
-    ctx->s_map = m;
-    ctx->s_map_cap = 2 * (size_t)nq;
-  }
-  memcpy(ctx->s_map, slot_of.data(), nq * sizeof(uint32_t));
-  memcpy(ctx->s_map + nq, row_of.data(), nq * sizeof(uint32_t));
+  ctx->s_map.assign(slot_of.begin(), slot_of.begin() + nq);
+  ctx->s_map.insert(ctx->s_map.end(), row_of.begin(), row_of.begin() + nq);
   uint32_t k1 = 0;
   for (uint32_t i = 0; i < nq; ++i) {
     stb_hit *oh = out_hits + (size_t)i * top_k;
@@ -1993,10 +1897,10 @@ static int thr_chunk_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, uint3
   const uint32_t n_seg = stb_batch_emit_grid(ctx, n_tiles);
   float *thr = ctx->b_thr + c0;
   uint32_t *cnt = ctx->b_cnt + (size_t)c0 * n_seg;
-  if ((rc = dev_reserve(&ctx->bq_dev, &ctx->bq_dev_cap, (size_t)n * STB_D)) != STB_OK) return rc;
-  if ((rc = dev_reserve(&ctx->b_qbad, &ctx->b_qbad_cap, (size_t)q_pad)) != STB_OK) return rc;
-  if ((rc = dev_reserve(&ctx->bq_tiles, &ctx->bq_tiles_cap, (size_t)q_pad * 512)) != STB_OK) return rc;
-  if ((rc = dev_reserve(&ctx->b_keys, &ctx->b_keys_cap, (size_t)q_pad * n_seg * STB_THR_SEG_CAP)) != STB_OK) return rc;
+  if ((rc = ctx->bq_dev.reserve((size_t)n * STB_D)) != STB_OK) return rc;
+  if ((rc = ctx->b_qbad.reserve((size_t)q_pad)) != STB_OK) return rc;
+  if ((rc = ctx->bq_tiles.reserve((size_t)q_pad * 512)) != STB_OK) return rc;
+  if ((rc = ctx->b_keys.reserve((size_t)q_pad * n_seg * STB_THR_SEG_CAP)) != STB_OK) return rc;
   STB_CUDA(cudaMemcpyAsync(ctx->bq_dev, q, (size_t)n * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
   STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
   STB_CUDA(cudaMemsetAsync(cnt, 0, (size_t)q_pad * n_seg * sizeof(uint32_t), ctx->stream));
@@ -2051,13 +1955,13 @@ static int thr_chunk_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, uint3
   out->off[n_slots] = (int)at;
   for (size_t j = (size_t)n_retry * n_seg; j < segoff.size(); ++j) segoff[j] = at;   // padding slots: empty
   const int K = (int)at;
-  if ((rc = dev_reserve(&ctx->t_buf, &ctx->t_buf_cap, std::max<size_t>(4 * (size_t)K, 1))) != STB_OK) return rc;
-  if ((rc = dev_reserve(&ctx->t_off, &ctx->t_off_cap, (size_t)n_slots + 1)) != STB_OK) return rc;
-  if ((rc = dev_reserve(&ctx->t_slot, &ctx->t_slot_cap, 2 * (size_t)n_slots)) != STB_OK) return rc;
-  if ((rc = dev_reserve(&ctx->t_dst, &ctx->t_dst_cap, dst.size())) != STB_OK) return rc;
+  if ((rc = ctx->t_buf.reserve(std::max<size_t>(4 * (size_t)K, 1))) != STB_OK) return rc;
+  if ((rc = ctx->t_off.reserve((size_t)n_slots + 1)) != STB_OK) return rc;
+  if ((rc = ctx->t_slot.reserve(2 * (size_t)n_slots)) != STB_OK) return rc;
+  if ((rc = ctx->t_dst.reserve(dst.size())) != STB_OK) return rc;
   size_t sort_bytes = 0;
   if ((rc = stb_batch_thr_sort_bytes(ctx, K, n_slots, ctx->t_off, &sort_bytes)) != STB_OK) return rc;
-  if ((rc = dev_reserve(&ctx->t_sort_tmp, &ctx->t_sort_tmp_cap, sort_bytes)) != STB_OK) return rc;
+  if ((rc = ctx->t_sort_tmp.reserve(sort_bytes)) != STB_OK) return rc;
   uint64_t *A = ctx->t_buf, *B = A + K, *C = B + K, *D = C + K;
   STB_CUDA(cudaMemcpyAsync(ctx->t_off, out->off.data(), out->off.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
   STB_CUDA(cudaMemcpyAsync(ctx->t_slot, out->slot_query.data(), n_slots * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
@@ -2066,10 +1970,10 @@ static int thr_chunk_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, uint3
   if (n_retry) {
     // one more pass over the re-emitted queries' shadow tiles (rebuilt from their f32 rows: the same bits), into
     // segments sized by the first pass's exact counts
-    if ((rc = dev_reserve(&ctx->t_segoff, &ctx->t_segoff_cap, segoff.size())) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->t_cur, &ctx->t_cur_cap, (size_t)r_pad * n_seg)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->t_rq, &ctx->t_rq_cap, (size_t)n_retry * STB_D)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->t_rthr, &ctx->t_rthr_cap, (size_t)r_pad)) != STB_OK) return rc;
+    if ((rc = ctx->t_segoff.reserve(segoff.size())) != STB_OK) return rc;
+    if ((rc = ctx->t_cur.reserve((size_t)r_pad * n_seg)) != STB_OK) return rc;
+    if ((rc = ctx->t_rq.reserve((size_t)n_retry * STB_D)) != STB_OK) return rc;
+    if ((rc = ctx->t_rthr.reserve((size_t)r_pad)) != STB_OK) return rc;
     STB_CUDA(cudaMemcpyAsync(ctx->t_segoff, segoff.data(), segoff.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->stream));
     STB_CUDA(cudaMemsetAsync(ctx->t_cur, 0, (size_t)r_pad * n_seg * sizeof(uint32_t), ctx->stream));
     STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
@@ -2113,8 +2017,8 @@ int stb_search_batch_threshold(stb_ctx *ctx, const stb_corpus *corpus_c, const f
   const uint32_t n_seg = tensor_ok ? stb_batch_emit_grid(ctx, (uint32_t)((corpus->n + 255) / 256)) : 0u;
   const size_t nq_pad = ((size_t)nq + 127) / 128 * 128;
   if (tensor_ok) {
-    if ((rc = dev_reserve(&ctx->b_thr, &ctx->b_thr_cap, nq_pad)) != STB_OK) return rc;
-    if ((rc = dev_reserve(&ctx->b_cnt, &ctx->b_cnt_cap, nq_pad * n_seg)) != STB_OK) return rc;
+    if ((rc = ctx->b_thr.reserve(nq_pad)) != STB_OK) return rc;
+    if ((rc = ctx->b_cnt.reserve(nq_pad * n_seg)) != STB_OK) return rc;
   }
   const float t = thr_emission_value(max_distance);
   std::unique_ptr<stb_hit[]> k1_buf;                                 // one K1 result: at most every row
@@ -2151,8 +2055,8 @@ int stb_search_batch_threshold(stb_ctx *ctx, const stb_corpus *corpus_c, const f
       const int K = ch.off[n_slots];
       std::vector<uint64_t> out_at(n_slots);
       for (uint32_t s = 0; s < n_slots; ++s) out_at[s] = out_offsets[c0 + ch.slot_query[s]] - base;
-      if ((rc = dev_reserve(&ctx->t_out_at, &ctx->t_out_at_cap, (size_t)n_slots)) != STB_OK) return rc;
-      if ((rc = dev_reserve(&ctx->t_hits, &ctx->t_hits_cap, std::max<size_t>(total, 1))) != STB_OK) return rc;
+      if ((rc = ctx->t_out_at.reserve((size_t)n_slots)) != STB_OK) return rc;
+      if ((rc = ctx->t_hits.reserve(std::max<size_t>(total, 1))) != STB_OK) return rc;
       STB_CUDA(cudaMemcpyAsync(ctx->t_out_at, out_at.data(), n_slots * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->stream));
       if ((rc = stb_launch_batch_thr_write(ctx, ctx->t_buf, ctx->t_buf + K, ctx->t_off, ctx->t_slot + n_slots, n_slots,
                                            ctx->t_out_at, ctx->t_hits)) != STB_OK) return rc;
@@ -2190,8 +2094,8 @@ int stb_search_batch_xchg_dev(stb_ctx *ctx, const stb_corpus *corpus, const floa
   if (x->dead) { stb_set_error("search_batch_xchg_dev: this exchange saw a peer time-out; destroy it on every rank"); return STB_ERR_STATE; }
   if (nq == 0) return STB_OK;
   if (x->max_nq == 0 || nq > x->max_nq || top_k == 0 || top_k > x->max_k) { stb_set_error("search_batch_xchg_dev: needs stb_xchg_create_batch with max_nq >= %u, max_k >= %u", nq, top_k); return STB_ERR_ARG; }
-  if ((rc = dev_reserve(&ctx->bh_dev, &ctx->bh_dev_cap, (size_t)nq * top_k)) != STB_OK) return rc;
-  if ((rc = dev_reserve(&ctx->bs_dev, &ctx->bs_dev_cap, (size_t)nq * 2)) != STB_OK) return rc;
+  if ((rc = ctx->bh_dev.reserve((size_t)nq * top_k)) != STB_OK) return rc;
+  if ((rc = ctx->bs_dev.reserve((size_t)nq * 2)) != STB_OK) return rc;
   if ((rc = stb_search_batch_dev(ctx, corpus, q_dev, nq, top_k, ctx->bh_dev, ctx->bs_dev)) != STB_OK) return rc;
   StbBatchXchgArgs a;
   memset(&a, 0, sizeof(a));
@@ -2211,7 +2115,7 @@ int stb_debug_batch_last(stb_ctx *ctx, uint32_t info[6], float *thr, uint32_t *c
   const uint32_t nq = ctx->b_last[1], n_seg = ctx->b_last[4];
   if (ctx->b_last[0] == 6u && n_seg && nq) {
     // slot-indexed thresholds, compact-row counts -> caller order (+inf, 0: a query the tensor passes did not take)
-    const uint32_t *slot = ctx->s_map, *row = ctx->s_map + nq;
+    const uint32_t *slot = ctx->s_map.data(), *row = slot + nq;
     uint32_t n_slots = 0, n_rows = 0;
     for (uint32_t i = 0; i < nq; ++i) {
       if (slot[i] != 0xffffffffu) n_slots = std::max(n_slots, slot[i] + 1);
@@ -2250,28 +2154,23 @@ int stb_debug_batch_gemm(stb_ctx *ctx, const float *q, uint32_t nq, const float 
   const uint32_t m_tiles = (nq + 127) / 128;
   const uint32_t n_tiles = (uint32_t)((n + 255) / 256);
   const size_t q_pad = (size_t)m_tiles * 128, n_pad = (size_t)n_tiles * 256;
-  float *dq = nullptr, *dr = nullptr, *dfull = nullptr, *dsub = nullptr, *dtile = nullptr;
-  uint8_t *da = nullptr, *db = nullptr;
-  int *dbad = nullptr;
-  cudaError_t e = cudaMalloc(&dq, (size_t)nq * 1024);
-  if (e == cudaSuccess) e = cudaMalloc(&dr, n * 1024);
-  if (e == cudaSuccess) e = cudaMalloc(&da, q_pad * 512);
-  if (e == cudaSuccess) e = cudaMalloc(&db, n_pad * 512);
-  if (e == cudaSuccess) e = cudaMalloc(&dfull, q_pad * n_pad * 4);
-  if (e == cudaSuccess) e = cudaMalloc(&dsub, (size_t)n_tiles * 8 * q_pad * 4);
-  if (e == cudaSuccess) e = cudaMalloc(&dtile, (size_t)n_tiles * q_pad * 4);
-  if (e == cudaSuccess) e = cudaMalloc(&dbad, 4);
-  if (e == cudaSuccess) e = cudaMemsetAsync(dbad, 0, 4, ctx->stream);
+  StbBuf<float> dq, dr, dfull, dsub, dtile;
+  StbBuf<uint8_t> da, db;
+  StbBuf<int> dbad;
+  if ((rc = dq.alloc((size_t)nq * STB_D)) != STB_OK || (rc = dr.alloc(n * STB_D)) != STB_OK ||
+      (rc = da.alloc(q_pad * 512)) != STB_OK || (rc = db.alloc(n_pad * 512)) != STB_OK ||
+      (rc = dfull.alloc(q_pad * n_pad)) != STB_OK || (rc = dsub.alloc((size_t)n_tiles * 8 * q_pad)) != STB_OK ||
+      (rc = dtile.alloc((size_t)n_tiles * q_pad)) != STB_OK || (rc = dbad.alloc(1)) != STB_OK)
+    return rc;
+  cudaError_t e = cudaMemsetAsync(dbad, 0, 4, ctx->stream);
   if (e == cudaSuccess) e = cudaMemcpyAsync(dq, q, (size_t)nq * 1024, cudaMemcpyHostToDevice, ctx->stream);
   if (e == cudaSuccess) e = cudaMemcpyAsync(dr, rows, n * 1024, cudaMemcpyHostToDevice, ctx->stream);
-  rc = STB_OK;
   if (e == cudaSuccess) rc = stb_launch_shadow_build(ctx, dq, nq, 128, da, dbad);
   if (e == cudaSuccess && rc == STB_OK) rc = stb_launch_shadow_build(ctx, dr, n, 256, db, dbad);
   if (e == cudaSuccess && rc == STB_OK) rc = stb_launch_batch_gemm(ctx, da, m_tiles, db, n_tiles, dsub, dtile, dfull);
   if (e == cudaSuccess && rc == STB_OK) e = cudaMemcpyAsync(out_full, dfull, q_pad * n_pad * 4, cudaMemcpyDeviceToHost, ctx->stream);
   if (e == cudaSuccess && rc == STB_OK && out_submax) e = cudaMemcpyAsync(out_submax, dsub, (size_t)n_tiles * 8 * q_pad * 4, cudaMemcpyDeviceToHost, ctx->stream);
   if (e == cudaSuccess && rc == STB_OK) e = cudaStreamSynchronize(ctx->stream);
-  cudaFree(dq); cudaFree(dr); cudaFree(da); cudaFree(db); cudaFree(dfull); cudaFree(dsub); cudaFree(dtile); cudaFree(dbad);
   if (e != cudaSuccess) { stb_set_error("debug_batch_gemm: %s", cudaGetErrorString(e)); cudaGetLastError(); return STB_ERR_CUDA; }
   return rc;
 }
@@ -2285,24 +2184,18 @@ static bool k1_copy_usable(const stb_corpus *c, int tier) {
 }
 
 // Query and ranges staged like stb_search's; per-row device outputs: `floats` arrays of n f32 (NaN-filled) and one of
-// n u32 (zeroed), in one allocation that the caller frees.
+// n u32 (zeroed), in the one buffer f_dev.
 static int k1_debug_stage(stb_ctx *ctx, const stb_corpus *c, const char *what, const float *q, const uint64_t *row_ranges,
-                          uint32_t n_ranges, int floats, float **f_dev, unsigned int **u_dev, const uint64_t **ranges_dev,
+                          uint32_t n_ranges, int floats, StbBuf<float> &f_dev, unsigned int **u_dev, const uint64_t **ranges_dev,
                           uint32_t *n_loc, uint64_t *n_virtual) {
   int rc;
   if ((rc = k1_upload_ranges(ctx, c, what, row_ranges, n_ranges, ranges_dev, n_loc, n_virtual)) != STB_OK) return rc;
   memcpy(ctx->q_pin, q, STB_D * sizeof(float));
   STB_CUDA(cudaMemcpyAsync(ctx->q_dev, ctx->q_pin, STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
   const size_t n = c->n;
-  void *p = nullptr;
-  if (cudaMalloc(&p, n * sizeof(float) * (floats + 1)) != cudaSuccess) {
-    cudaGetLastError();
-    stb_set_error("%s: cannot allocate the per-row outputs", what);
-    return STB_ERR_NOMEM;
-  }
-  *f_dev = (float *)p;
-  *u_dev = (unsigned int *)(*f_dev + n * floats);
-  STB_CUDA(cudaMemsetAsync(*f_dev, 0xff, n * sizeof(float) * floats, ctx->stream));
+  if ((rc = f_dev.alloc(n * (floats + 1))) != STB_OK) return rc;
+  *u_dev = (unsigned int *)(f_dev + n * floats);
+  STB_CUDA(cudaMemsetAsync(f_dev, 0xff, n * sizeof(float) * floats, ctx->stream));
   STB_CUDA(cudaMemsetAsync(*u_dev, 0, n * sizeof(unsigned int), ctx->stream));
   return STB_OK;
 }
@@ -2319,12 +2212,12 @@ int stb_debug_scan_scores(stb_ctx *ctx, const stb_corpus *corpus, int tier, cons
   if (!k1_copy_usable(corpus, tier)) { stb_set_error("debug_scan_scores: tier %d copy not built or unusable", tier); return STB_ERR_STATE; }
   if (hist) memset(hist, 0, 4096 * sizeof(uint32_t));
   if (corpus->n == 0) return STB_OK;
-  float *d_score = nullptr;
+  StbBuf<float> d_score;
   unsigned int *d_seen = nullptr;
   const uint64_t *ranges_dev = nullptr;
   uint32_t n_loc = 0;
   uint64_t n_virtual = 0;
-  if ((rc = k1_debug_stage(ctx, corpus, "debug_scan_scores", q, row_ranges, n_ranges, 1, &d_score, &d_seen, &ranges_dev, &n_loc,
+  if ((rc = k1_debug_stage(ctx, corpus, "debug_scan_scores", q, row_ranges, n_ranges, 1, d_score, &d_seen, &ranges_dev, &n_loc,
                            &n_virtual)) == STB_OK && n_virtual) {
     rc = stb_launch_debug_scan(ctx, corpus, tier, ctx->q_dev, ranges_dev, n_loc, n_virtual, d_score, d_seen);
     if (rc == STB_OK && hist) rc = stb_launch_scan_hist(ctx, corpus, tier, ctx->q_dev, ranges_dev, n_loc, n_virtual, ctx->hist_dev);
@@ -2335,7 +2228,6 @@ int stb_debug_scan_scores(stb_ctx *ctx, const stb_corpus *corpus, int tier, cons
   if (rc == STB_OK && e == cudaSuccess && hist && n_virtual)
     e = cudaMemcpyAsync(hist, ctx->hist_dev, 4096 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-  cudaFree(d_score);
   if (rc == STB_OK && e != cudaSuccess) { stb_set_error("debug_scan_scores: %s", cudaGetErrorString(e)); cudaGetLastError(); return STB_ERR_CUDA; }
   return rc;
 }
@@ -2356,18 +2248,16 @@ int stb_debug_q4_scan(stb_ctx *ctx, const stb_corpus *corpus, const float *q, ui
   memset(words, 0, top_k * sizeof(uint64_t));
   if (corpus->n == 0) return STB_OK;
   const size_t n = corpus->n;
-  float *d_f = nullptr;
+  StbBuf<float> d_f;
   unsigned int *d_seen = nullptr;
-  unsigned long long *d_words = nullptr;
+  StbBuf<unsigned long long> d_words;
   const uint64_t *ranges_dev = nullptr;
   uint32_t n_loc = 0;
   uint64_t n_virtual = 0;
-  rc = k1_debug_stage(ctx, corpus, "debug_q4_scan", q, row_ranges, n_ranges, 4, &d_f, &d_seen, &ranges_dev, &n_loc, &n_virtual);
+  rc = k1_debug_stage(ctx, corpus, "debug_q4_scan", q, row_ranges, n_ranges, 4, d_f, &d_seen, &ranges_dev, &n_loc, &n_virtual);
   cudaError_t e = cudaSuccess;
-  if (rc == STB_OK) {
-    e = cudaMalloc(&d_words, (STB_Q4_WORDS + 1) * sizeof(unsigned long long));   // the words, then the refined counter
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_words, 0, (STB_Q4_WORDS + 1) * sizeof(unsigned long long), ctx->stream);
-  }
+  if (rc == STB_OK && (rc = d_words.alloc(STB_Q4_WORDS + 1)) == STB_OK)   // the words, then the refined counter
+    e = cudaMemsetAsync(d_words, 0, (STB_Q4_WORDS + 1) * sizeof(unsigned long long), ctx->stream);
   if (rc == STB_OK && e == cudaSuccess && n_virtual)
     rc = stb_launch_debug_q4(ctx, corpus, ctx->q_dev, top_k, ranges_dev, n_loc, n_virtual, d_words, d_words + STB_Q4_WORDS, pin,
                              d_f, d_f + n, d_f + 2 * n, d_f + 3 * n, d_seen);
@@ -2377,8 +2267,6 @@ int stb_debug_q4_scan(stb_ctx *ctx, const stb_corpus *corpus, const float *q, ui
   if (rc == STB_OK && e == cudaSuccess) e = cudaMemcpyAsync(refined, d_seen, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream);
   if (rc == STB_OK && e == cudaSuccess) e = cudaMemcpyAsync(words, d_words, top_k * sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-  cudaFree(d_f);
-  cudaFree(d_words);
   if (rc == STB_OK && e != cudaSuccess) { stb_set_error("debug_q4_scan: %s", cudaGetErrorString(e)); cudaGetLastError(); return STB_ERR_CUDA; }
   return rc;
 }
@@ -2438,19 +2326,11 @@ int stb_search_many(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint
   if ((rc = k1_copy_ready(ctx, const_cast<stb_corpus *>(corpus), STB_TIER_Q8, top_k, {eager, eager}, &q8_ready)) != STB_OK) return rc;
   const int tier = q8_ready ? STB_TIER_Q8 : best_built_tier(ctx, corpus, top_k);
   if ((rc = host_rows_tier_check(corpus, tier, "search_many")) != STB_OK) return rc;
-  if ((rc = dev_reserve(&ctx->bq_dev, &ctx->bq_dev_cap, (size_t)nq * STB_D)) != STB_OK) return rc;
-  if ((rc = ensure_hits_pin(ctx, (size_t)nq * top_k)) != STB_OK) return rc;
-  if ((size_t)nq * STB_D > ctx->many_q_pin_cap) {
-    float *np = nullptr; uint32_t *ns = nullptr;
+  if ((rc = ctx->bq_dev.reserve((size_t)nq * STB_D)) != STB_OK) return rc;
+  if ((rc = ctx->hits_pin.reserve((size_t)nq * top_k, 2 * ctx->hits_pin.cap)) != STB_OK) return rc;
+  if ((size_t)nq * STB_D > ctx->many_q_pin.cap || (size_t)nq * 4 > ctx->many_status_pin.cap) {
     const size_t cap = std::max<size_t>((size_t)nq, 64);
-    if (cudaMallocHost((void **)&np, cap * STB_D * sizeof(float)) != cudaSuccess ||
-        cudaMallocHost((void **)&ns, cap * 4 * sizeof(uint32_t)) != cudaSuccess) {
-      cudaGetLastError(); if (np) cudaFreeHost(np);
-      stb_set_error("search_many: pinned staging allocation failed"); return STB_ERR_NOMEM;
-    }
-    if (ctx->many_q_pin) cudaFreeHost(ctx->many_q_pin);
-    if (ctx->many_status_pin) cudaFreeHost(ctx->many_status_pin);
-    ctx->many_q_pin = np; ctx->many_status_pin = ns; ctx->many_q_pin_cap = cap * STB_D;
+    if ((rc = ctx->many_q_pin.alloc(cap * STB_D)) != STB_OK || (rc = ctx->many_status_pin.alloc(cap * 4)) != STB_OK) return rc;
   }
   memcpy(ctx->many_q_pin, q, (size_t)nq * STB_D * sizeof(float));
   STB_CUDA(cudaMemcpyAsync(ctx->bq_dev, ctx->many_q_pin, (size_t)nq * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
@@ -2509,8 +2389,8 @@ int stb_hits_merge(stb_ctx *ctx, const stb_hit *lists, uint32_t n_lists, uint32_
   *out_n = 0;
   if (top_k == 0) return STB_OK;
   const size_t total = (size_t)n_lists * per_list;
-  if ((rc = dev_reserve(&ctx->hits_dev, &ctx->hits_cap, total + top_k)) != STB_OK) return rc;
-  if ((rc = ensure_hits_pin(ctx, std::max<size_t>(total, top_k))) != STB_OK) return rc;
+  if ((rc = ctx->hits_dev.reserve(total + top_k)) != STB_OK) return rc;
+  if ((rc = ctx->hits_pin.reserve(std::max<size_t>(total, top_k), 2 * ctx->hits_pin.cap)) != STB_OK) return rc;
   memcpy(ctx->hits_pin, lists, total * sizeof(stb_hit));
   STB_CUDA(cudaMemcpyAsync(ctx->hits_dev, ctx->hits_pin, total * sizeof(stb_hit), cudaMemcpyHostToDevice, ctx->stream));
   if ((rc = stb_launch_hits_merge(ctx, ctx->hits_dev, n_lists, per_list, top_k, ctx->hits_dev + total)) != STB_OK) return rc;

@@ -8,6 +8,8 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <vector>
+
 #include "../../include/semtools_b200.h"
 
 #define STB_D 256           // floats per row
@@ -64,27 +66,82 @@ void stb_set_error(const char *fmt, ...);
     }                                                                              \
   } while (0)
 
+// The one owner of every device (cudaMalloc) and page-locked host (cudaMallocHost) buffer of the library: cap
+// elements of T at p, freed by the destructor.  It converts to T *, so launches, copies and indexing read it as
+// the pointer.  alloc(n) frees what it holds, then allocates exactly n elements.  reserve(need, floor) keeps
+// the buffer if it holds need elements, else allocates max(need, floor, 1.5 cap) and only then frees the old
+// one.  Neither keeps the contents.  A failed allocation returns STB_ERR_NOMEM with the byte count in the
+// error message and leaves the buffer as it was (after alloc's free: empty).  Freeing an old buffer that a
+// kernel may still read is the caller's to order (stream synchronise).
+template <class T, bool PINNED = false>
+struct StbBuf {
+  T *p = nullptr;
+  size_t cap = 0;
+  StbBuf() = default;
+  StbBuf(const StbBuf &) = delete;
+  StbBuf &operator=(const StbBuf &) = delete;
+  StbBuf(StbBuf &&o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  StbBuf &operator=(StbBuf &&o) noexcept {
+    if (this != &o) { release(); p = o.p; cap = o.cap; o.p = nullptr; o.cap = 0; }
+    return *this;
+  }
+  ~StbBuf() { release(); }
+  operator T *() const { return p; }
+  int alloc(size_t n) {
+    release();
+    return take(n);
+  }
+  int reserve(size_t need, size_t floor = 0) {
+    if (need <= cap && p) return STB_OK;
+    size_t n = need > floor ? need : floor;
+    if (cap + cap / 2 > n) n = cap + cap / 2;
+    return take(n);
+  }
+
+ private:
+  int take(size_t n) {
+    void *np = nullptr;
+    const cudaError_t e = PINNED ? cudaMallocHost(&np, n * sizeof(T)) : cudaMalloc(&np, n * sizeof(T));
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      stb_set_error("%s(%zu bytes) failed: %s", PINNED ? "cudaMallocHost" : "cudaMalloc", n * sizeof(T), cudaGetErrorString(e));
+      return STB_ERR_NOMEM;
+    }
+    release();
+    p = static_cast<T *>(np);
+    cap = n;
+    return STB_OK;
+  }
+  void release() {
+    if (p) {
+      if (PINNED) cudaFreeHost(p); else cudaFree(p);
+      cudaGetLastError();
+    }
+    p = nullptr;
+    cap = 0;
+  }
+};
+template <class T> using StbPinned = StbBuf<T, true>;
+
 struct stb_ctx {
   int device;
   int sm_count;
   cudaStream_t stream;
   bool own_stream;
   // --- scan scratch (device) ---
-  uint64_t *block_keys;     // candidate keys of every tree level
-  size_t block_keys_cap;    // in keys
-  unsigned int *counters;   // tree arrival counters (zeroed; kernels re-zero)
-  size_t counters_cap;
+  StbBuf<uint64_t> block_keys;     // candidate keys of every tree level
+  StbBuf<unsigned int> counters;   // tree arrival counters (zeroed; kernels re-zero)
   // K1 tile-ticket counters (monotonic; scan_topk.cu: stb_for_each_tile).  A ring of STB_TICKET_SLOTS
   // counters, one per launch in turn: with the overlapped launch mode two consecutive scans run
   // concurrently and must not draw from the same counter.
-  unsigned long long *tickets;
+  StbBuf<unsigned long long> tickets;
   unsigned long long ticket_next[8];   // per slot: its value when the next launch using it starts
   unsigned long long topk_launches;    // picks the slot
   bool ticket_ring;                    // set by the first overlapped launch; until then every launch uses slot 0
   // K1 co-scan (scan_topk.cu: stb_coscan_offset): per ticket slot, the tile offset its last co-scan launch
   // chose, as a tagged word (tag << 32 | offset, the tag is the launch count); the host's copy of the tags
   // (0: the slot's last launch did not co-scan) and the last co-scan launch, which the next one may follow
-  unsigned long long *coscan_off;
+  StbBuf<unsigned long long> coscan_off;
   uint32_t coscan_tag[8];
   struct {
     const void *rows;                  // the scanned corpus's f32 rows; null: no launch to follow
@@ -96,93 +153,84 @@ struct stb_ctx {
   } coscan_prev;
   // q8 tier prefilter (scan_topk.cu: stb_scan_q4): STB_TICKET_SLOTS x STB_Q4_WORDS tagged threshold words,
   // one slot per launch in turn; the launch count is the tag
-  unsigned long long *q4_thr;
+  StbBuf<unsigned long long> q4_thr;
   unsigned long long q4_launches;
-  unsigned long long *q4_refined;      // rows the prefilter passed on to the int8 codes (stb_debug_q4_refined)
-  float *q_dev;             // 256 f32 staging for host queries
-  stb_hit *hits_dev;        // result hits (top-k path)
-  size_t hits_cap;
-  uint32_t *status_dev;     // [0]=n hits, [1]=complete flag, [2..] debug
-  uint32_t *collect_rows;   // threshold/fallback compaction: local row ids
-  size_t collect_cap;
-  unsigned long long *collect_count;
-  stb_hit *collect_hits;    // exact hits of collected rows (sorted in place)
-  size_t collect_hits_cap;
-  uint64_t *ranges_dev;     // [3 * n] : begin(local), end(local), vstart
-  size_t ranges_cap;
-  int *err_flag;            // device int: scratch flag of the copy builders, stb_embed and K2's query shadow; zeroed before each use
-  unsigned int *hist_dev;       // 4096-bin score histogram (large-k path)
+  StbBuf<unsigned long long> q4_refined;   // rows the prefilter passed on to the int8 codes (stb_debug_q4_refined)
+  StbBuf<float> q_dev;             // 256 f32 staging for host queries
+  StbBuf<stb_hit> hits_dev;        // result hits (top-k path)
+  StbBuf<uint32_t> status_dev;     // [0]=n hits, [1]=complete flag, [2..] debug
+  StbBuf<uint32_t> collect_rows;   // threshold/fallback compaction: local row ids
+  StbBuf<unsigned long long> collect_count;
+  StbBuf<stb_hit> collect_hits;    // exact hits of collected rows (sorted in place)
+  StbBuf<uint64_t> ranges_dev;     // [3 * n] : begin(local), end(local), vstart
+  StbBuf<int> err_flag;            // device int: scratch flag of the copy builders, stb_embed and K2's query shadow; zeroed before each use
+  StbBuf<unsigned int> hist_dev;   // 4096-bin score histogram (large-k path)
   // cudaFuncSetAttribute is per DEVICE: remembered per context, never in function statics
   // (one process may hold contexts on several GPUs)
   uint32_t func_attr_mask;
   size_t finish2_smem_set;
   // --- K2 scratch ---
-  uint8_t *bq_tiles; size_t bq_tiles_cap;     // query shadow tiles
-  float *b_submax; size_t b_submax_cap;       // [n_sub][q_pad]
-  float *b_tilemax; size_t b_tilemax_cap;     // [n_tiles][q_pad]
-  uint64_t *b_cand; size_t b_cand_cap;        // [q_pad][slices][32]
-  float *b_thr; size_t b_thr_cap;             // v2: [q_pad] emission thresholds
-  uint32_t *b_cnt; size_t b_cnt_cap;          // v2: [q_pad] emitted-candidate counters
-  uint64_t *b_keys; size_t b_keys_cap;        // v2: [q_pad][cand_cap] emitted keys
-  uint32_t *b_qbad; size_t b_qbad_cap;        // [q_pad] 1: query could not be normalised
+  StbBuf<uint8_t> bq_tiles;     // query shadow tiles
+  StbBuf<float> b_submax;       // [n_sub][q_pad]
+  StbBuf<float> b_tilemax;     // [n_tiles][q_pad]
+  StbBuf<uint64_t> b_cand;        // [q_pad][slices][32]
+  StbBuf<float> b_thr;             // v2: [q_pad] emission thresholds
+  StbBuf<uint32_t> b_cnt;          // v2: [q_pad] emitted-candidate counters
+  StbBuf<uint64_t> b_keys;        // v2: [q_pad][cand_cap] emitted keys
+  StbBuf<uint32_t> b_qbad;        // [q_pad] 1: query could not be normalised
   // stb_search_batch_filtered: the clipped ranges (local [begin, end) u32 pairs), the listed tiles and the
   // eligible-row bitmap (8 words per shadow tile), all built from the same clipped ranges
-  uint32_t *b_franges; size_t b_franges_cap;
-  uint32_t *b_ftiles; size_t b_ftiles_cap;
-  uint32_t *b_fbits; size_t b_fbits_cap;
+  StbBuf<uint32_t> b_franges;
+  StbBuf<uint32_t> b_ftiles;
+  StbBuf<uint32_t> b_fbits;
   // stb_search_batch_subsets (route 6; b_franges / b_fbits hold every tensor group's ranges / bitmap): both
   // passes' work lists and the slots' rows in one upload, the queries in slot order, the bad flags per
   // compact row, and (host, malloc) each caller query's slot and compact row for stb_debug_batch_last
-  uint32_t *s_work; size_t s_work_cap;
-  float *s_qslots; size_t s_qslots_cap;
-  uint32_t *s_qbad; size_t s_qbad_cap;
-  uint32_t *s_map; size_t s_map_cap;
+  StbBuf<uint32_t> s_work;
+  StbBuf<float> s_qslots;
+  StbBuf<uint32_t> s_qbad;
+  std::vector<uint32_t> s_map;
   // stb_search_batch_threshold (per chunk of queries): per-(query, segment) destinations of the first pass's
   // keys, the re-emission's segment offsets, cursors, queries and thresholds, the compact candidates and their
   // sort buffers (4 x u64 per candidate), per-slot offsets / query / pass count / output position, the hits
   // in output order and the sorts' scratch
-  uint64_t *t_dst; size_t t_dst_cap;
-  uint64_t *t_segoff; size_t t_segoff_cap;
-  uint32_t *t_cur; size_t t_cur_cap;
-  float *t_rq; size_t t_rq_cap;
-  float *t_rthr; size_t t_rthr_cap;
-  uint64_t *t_buf; size_t t_buf_cap;
-  int *t_off; size_t t_off_cap;
-  uint32_t *t_slot; size_t t_slot_cap;       // [2][slots]: query of each slot, then its pass count
-  uint64_t *t_out_at; size_t t_out_at_cap;
-  stb_hit *t_hits; size_t t_hits_cap;
-  uint8_t *t_sort_tmp; size_t t_sort_tmp_cap;
+  StbBuf<uint64_t> t_dst;
+  StbBuf<uint64_t> t_segoff;
+  StbBuf<uint32_t> t_cur;
+  StbBuf<float> t_rq;
+  StbBuf<float> t_rthr;
+  StbBuf<uint64_t> t_buf;
+  StbBuf<int> t_off;
+  StbBuf<uint32_t> t_slot;       // [2][slots]: query of each slot, then its pass count
+  StbBuf<uint64_t> t_out_at;
+  StbBuf<stb_hit> t_hits;
+  StbBuf<uint8_t> t_sort_tmp;
   // the last K2 call: route (1 = v1, 2 = v2, 3 = filtered v2, 4 = filtered, nothing on the tensor cores,
   // 5 = threshold mode, 6 = one filter per query), nq, then n_sample, stride (routes 1-4) or retried queries, K1
   // queries (route 5) or tensor groups, K1 queries (route 6), n_seg, seg_cap
   uint32_t b_last[6];
-  float *bq_dev; size_t bq_dev_cap;           // host-call staging: queries
-  stb_hit *bh_dev; size_t bh_dev_cap;         // host-call staging: hits
-  uint32_t *bs_dev; size_t bs_dev_cap;        // host-call staging: status
-  uint64_t *embed_off_dev;  // K3 staging: CSR offsets
-  size_t embed_off_cap;
-  uint32_t *embed_ids_dev;  // K3 staging: token ids
-  size_t embed_ids_cap;
-  float *embed_out_dev;     // K3 output when not appending to a corpus
-  size_t embed_out_cap;
+  StbBuf<float> bq_dev;           // host-call staging: queries
+  StbBuf<stb_hit> bh_dev;         // host-call staging: hits
+  StbBuf<uint32_t> bs_dev;        // host-call staging: status
+  StbBuf<uint64_t> embed_off_dev;  // K3 staging: CSR offsets
+  StbBuf<uint32_t> embed_ids_dev;  // K3 staging: token ids
+  StbBuf<float> embed_out_dev;     // K3 output when not appending to a corpus
   // in-place corpus mutations (stb_corpus_update / _remove): row staging (<= STB_MUT_CHUNK_ROWS rows),
   // row ids or kept-segment table, and the q8 / shadow bad-row flags
-  float *mut_stage; size_t mut_stage_cap;
-  uint64_t *mut_idx; size_t mut_idx_cap;
-  int *mut_flags; size_t mut_flags_cap;
+  StbBuf<float> mut_stage;
+  StbBuf<uint64_t> mut_idx;
+  StbBuf<int> mut_flags;
   // --- pinned host staging ---
-  float *q_pin;
-  stb_hit *hits_pin;
-  size_t hits_pin_cap;
-  uint32_t *status_pin;
-  float *many_q_pin;          // stb_search_many: queries / per-query status (kernels write the latter directly)
-  uint32_t *many_status_pin;
-  size_t many_q_pin_cap;      // in floats
+  StbPinned<float> q_pin;
+  StbPinned<stb_hit> hits_pin;
+  StbPinned<uint32_t> status_pin;
+  StbPinned<float> many_q_pin;          // stb_search_many: queries / per-query status (kernels write the latter directly)
+  StbPinned<uint32_t> many_status_pin;
   // --- counters ---
   uint64_t kernel_launches;
   uint64_t fallback_searches;
   // --- K3 ---
-  int *embed_flag;          // device int: K3's sticky range flag; set only by stb_embed_dev, cleared only by stb_embed_status
+  StbBuf<int> embed_flag;          // device int: K3's sticky range flag; set only by stb_embed_dev, cleared only by stb_embed_status
 };
 
 #define STB_TICKET_SLOTS 8
@@ -202,7 +250,7 @@ struct StbXchgArgs {
 struct stb_xchg {
   stb_ctx *ctx;
   uint32_t world, rank, max_k;
-  unsigned char *local;                      // this rank's buffer (cudaMalloc)
+  StbBuf<unsigned char> local;               // this rank's buffer (plain device memory, which IPC requires)
   size_t bytes;
   unsigned char *peers[STB_XCHG_MAX_WORLD];  // peers[rank] == local
   bool ipc_opened[STB_XCHG_MAX_WORLD];
@@ -213,24 +261,25 @@ struct stb_xchg {
   uint32_t max_nq;
   size_t batch_off, batch_slot_bytes;
   unsigned long long batch_seq;
-  unsigned int *batch_ticket;                // device: arrival counter of the push kernel
+  StbBuf<unsigned int> batch_ticket;         // device: arrival counter of the push kernel
   bool dead;                                 // a synchronous call saw a peer time-out: every later call is refused
 };
 
 struct stb_table {
   stb_ctx *ctx;
-  float *E;            // V x 256
+  StbBuf<float> E;            // V x 256
   uint64_t V;
-  float *weights;      // or nullptr
+  StbBuf<float> weights;      // or empty
   uint64_t n_weights;
-  uint32_t *mapping;   // or nullptr
+  StbBuf<uint32_t> mapping;   // or empty
   uint64_t n_mapping;
   int normalize;
 };
 
 struct stb_corpus {
   stb_ctx *ctx;
-  float *rows;         // capacity x 256; on a host-rows corpus the device address of rows_host
+  float *rows;         // capacity x 256: dev_rows, or on a host-rows corpus the device address of rows_host
+  StbBuf<float> dev_rows;   // a device corpus's rows
   // stb_corpus_create_host: the rows live in page-locked, device-mapped host memory (kernels read them over
   // the host link through `rows`) and the q8 copy is kept current by every call that writes rows
   float *rows_host;    // null on a device corpus
@@ -240,17 +289,16 @@ struct stb_corpus {
   uint64_t row_base;
   uint64_t epoch;            // bumped by every change that is not an append (an IVF-PQ index refuses to extend over it)
   // K2: L2-normalised bf16 copy in wgmma tile layout (built lazily, rebuilt when n changes)
-  uint8_t *shadow;
+  StbBuf<uint8_t> shadow;    // whole 256-row tiles of 128 KiB
   uint64_t shadow_rows;      // rows covered by `shadow` (== n when valid)
-  uint64_t shadow_cap_tiles;
   int shadow_bad;            // 1: some row cannot be normalised in fp32 -> tensor path refused
   // K1 tier q8: int8 codes [capacity][256] + per-row scale, built lazily / by stb_corpus_prepare
-  uint8_t *q8;
-  float *q8_scale;
-  uint8_t *q4;               // ... its nibble plane [capacity][128] and per-row {s, rho} (top-k prefilter)
-  float2 *q4_sr;
+  // (q8_scale.cap: the rows all four hold)
+  StbBuf<uint8_t> q8;
+  StbBuf<float> q8_scale;
+  StbBuf<uint8_t> q4;        // ... its nibble plane [capacity][128] and per-row {s, rho} (top-k prefilter)
+  StbBuf<float2> q4_sr;
   uint64_t q8_rows;          // rows covered (== n when valid; also the plane's)
-  uint64_t q8_cap_rows;
   int q8_bad;
   // per-tier bookkeeping: a reduced-width tier is skipped once it proves fewer than half of its
   // results on this corpus (index = STB_TIER_*)

@@ -129,7 +129,7 @@ int stb_launch_embed(stb_ctx *ctx, const stb_table *t, const uint64_t *offsets_d
                      int *err_flag_dev) {
   if (n_lines == 0) return STB_OK;
   EmbedArgs a;
-  a.E = reinterpret_cast<const float4 *>(t->E);
+  a.E = reinterpret_cast<const float4 *>(t->E.p);
   a.V = t->V;
   a.weights = t->weights;
   a.n_weights = t->n_weights;

@@ -55,44 +55,41 @@ struct stb_ivfpq {
   uint64_t corpus_epoch;      // corpus->epoch when the index was built: extend refuses another
   uint32_t nlist;
   uint64_t n;                 // rows indexed (listed + forced): rows [0, n) of the corpus
-  float *centroids;           // [nlist][256]
-  float *codebooks;           // [32][256][8]
-  uint8_t *codes;             // [n_listed][32], grouped by list
-  uint32_t *order;            // [n_listed] local row of code i
-  uint32_t *list_off;         // [nlist+1] (device); list_off[nlist] = n_listed = n - n_forced
+  StbBuf<float> centroids;           // [nlist][256]
+  StbBuf<float> codebooks;           // [32][256][8]
+  StbBuf<uint8_t> codes;             // [n_listed][32], grouped by list
+  StbBuf<uint32_t> order;            // [n_listed] local row of code i
+  StbBuf<uint32_t> list_off;         // [nlist+1] (device); list_off[nlist] = n_listed = n - n_forced
   std::vector<uint32_t> list_off_h;
-  uint32_t *forced;           // [n_forced] local rows outside the lists, ascending
+  StbBuf<uint32_t> forced;           // [n_forced] local rows outside the lists, ascending
   uint32_t n_forced;
   // query scratch
-  float *coarse;              // [nlist]
-  float *lut;                 // [32][256]
-  uint32_t *probe;            // [nprobe_max] list ids, [nprobe_max+1] prefix of lengths
-  stb_hit *cand;              // candidate (-score,pos) hits, padded
-  size_t cand_cap;
-  uint32_t *cand_rows;        // local rows of the R best candidates
+  StbBuf<float> coarse;              // [nlist]
+  StbBuf<float> lut;                 // [32][256]
+  StbBuf<uint32_t> probe;            // [nprobe_max] list ids, [nprobe_max+1] prefix of lengths
+  StbBuf<stb_hit> cand;              // candidate (-score,pos) hits, padded
+  StbBuf<uint32_t> cand_rows;        // local rows of the R best candidates
   // fused search (v2)
-  uint64_t *keys2;            // [ADC2_MAX_CTAS][ADC2_KEEP] per-CTA best candidates (score desc, code position)
-  unsigned int *tickets;      // [2] last-CTA tickets of the two fused kernels (kernels re-zero them)
+  StbBuf<uint64_t> keys2;            // [ADC2_MAX_CTAS][ADC2_KEEP] per-CTA best candidates (score desc, code position)
+  StbBuf<unsigned int> tickets;      // [2] last-CTA tickets of the two fused kernels (kernels re-zero them)
   // batched search scratch (its own buffers: a batch and a single query enqueued back to back do not
   // share any), sized for b_cap queries, grown on demand
   uint32_t b_cap;
-  float *b_q;                 // [b_cap][256] queries of the host form
-  float *b_coarse;            // [b_cap][nlist]
-  uint32_t *b_probe;          // [b_cap][2 * 1024 + 2]: nprobe list ids, the prefix of their lengths (filtered:
-                              // and the eligible codes), IVFB_PROBE_STRIDE apart
-  float *b_lut;               // [b_cap][32][256]
-  uint64_t *b_kept;           // [b_cap][IVFB_KEPT] each warp's best keys
-  uint64_t *b_drop;           // [b_cap][IVFB_WARPS] the best key each warp dropped
-  stb_hit *b_hits;            // [b_cap][1024] hits of the host form
-  uint32_t *b_status;         // [b_cap][2]
+  StbBuf<float> b_q;                 // [b_cap][256] queries of the host form
+  StbBuf<float> b_coarse;            // [b_cap][nlist]
+  StbBuf<uint32_t> b_probe;          // [b_cap][2 * 1024 + 2]: nprobe list ids, the prefix of their lengths (filtered:
+                                     // and the eligible codes), IVFB_PROBE_STRIDE apart
+  StbBuf<float> b_lut;               // [b_cap][32][256]
+  StbBuf<uint64_t> b_kept;           // [b_cap][IVFB_KEPT] each warp's best keys
+  StbBuf<uint64_t> b_drop;           // [b_cap][IVFB_WARPS] the best key each warp dropped
+  StbBuf<stb_hit> b_hits;            // [b_cap][1024] hits of the host form
+  StbBuf<uint32_t> b_status;         // [b_cap][2]
   uint32_t last_info[4];      // {nq, nprobe, top_k, rerank} of the last batch launch (nq = 0: none yet)
   bool last_filtered;         // the last batch launch was a filtered search's
   // filtered search scratch (the eligibility pass), grown on demand
-  uint32_t *f_bitmap;         // [f_words] eligible local rows; f_words >= ceil(n / 32)
-  uint64_t f_words;
-  uint32_t *f_elig;           // [nlist] eligible codes per list
-  uint32_t *f_ranges;         // [f_ranges_cap][2] clipped local ranges
-  uint32_t f_ranges_cap;
+  StbBuf<uint32_t> f_bitmap;         // eligible local rows; cap >= ceil(n / 32) words
+  StbBuf<uint32_t> f_elig;           // [nlist] eligible codes per list
+  StbBuf<uint32_t> f_ranges;         // clipped local ranges, [begin, end) pairs
 };
 
 // ------------------------------------------------------------------ assignment GEMM ---
@@ -1198,29 +1195,6 @@ __global__ void ivff_elig_kernel(const uint32_t *list_off, const uint32_t *order
 }
 
 // ------------------------------------------------------------------ host side ---------
-// Device buffers of one edit of the lists: freed with it (after a stream synchronise, so no kernel still
-// reads them) unless adopted by the index.  A failed allocation is STB_ERR_NOMEM.
-struct IvfScratch {
-  cudaStream_t st;
-  std::vector<void *> p;
-  template <class T> int alloc(T **ptr, size_t bytes) {
-    *ptr = nullptr;
-    const cudaError_t e = cudaMalloc(reinterpret_cast<void **>(ptr), std::max<size_t>(bytes, 16));
-    if (e != cudaSuccess) {
-      cudaGetLastError();
-      stb_set_error("ivfpq: cudaMalloc(%zu bytes) failed: %s", bytes, cudaGetErrorString(e));
-      return STB_ERR_NOMEM;
-    }
-    p.push_back(*ptr);
-    return STB_OK;
-  }
-  void adopt(const void *q) { p.erase(std::find(p.begin(), p.end(), q)); }
-  ~IvfScratch() {
-    cudaStreamSynchronize(st);
-    for (void *q : p) cudaFree(q);
-    cudaGetLastError();
-  }
-};
 #define IVF_TRY(call)                      \
   do {                                     \
     const int _rc = (call);                \
@@ -1238,7 +1212,7 @@ struct IvfScratch {
 // double-buffered, the codes in entry order, their rows) and, when entries leave, a bitmap of the indexed
 // rows, the kept segments and 8 B per old listed entry (survivor positions and rows).
 struct IvfEdit {
-  IvfScratch t;
+  cudaStream_t st;
   uint64_t m = 0, first = 0;          // new entries: rows first + i (build, extend), or rows_h[i] (update)
   std::vector<uint32_t> rows_h;       //   local rows, ascending
   bool keep_all = true;               // no old entry leaves and none is renumbered (build, extend)
@@ -1247,15 +1221,13 @@ struct IvfEdit {
   uint64_t n_after = 0;               // indexed rows after the edit
   int key_bits = 0;
   size_t sort_bytes = 0;
-  uint32_t *assign = nullptr, *assign_alt = nullptr, *vals = nullptr, *vals_alt = nullptr, *counts = nullptr;
-  uint32_t *new_rows = nullptr, *kept_d = nullptr, *bitmap = nullptr, *elig = nullptr, *surv_pos = nullptr;
-  uint32_t *surv_row = nullptr, *surv_off_d = nullptr, *new_off_d = nullptr, *order = nullptr, *forced = nullptr;
-  uint8_t *codes_row = nullptr, *codes = nullptr;
-  void *sort_tmp = nullptr;
+  // device buffers (at least 16 bytes each): the ones the swap does not move into the index go with the edit
+  StbBuf<uint32_t> assign, assign_alt, vals, vals_alt, counts, new_rows, kept_d, bitmap, elig, surv_pos, surv_row,
+      surv_off_d, new_off_d, order, forced;
+  StbBuf<uint8_t> codes_row, codes, sort_tmp;
   std::vector<uint32_t> new_off, forced_h;
-  explicit IvfEdit(cudaStream_t st) : t{st, {}} {}
-  IvfEdit(const IvfEdit &) = delete;
-  IvfEdit &operator=(const IvfEdit &) = delete;
+  explicit IvfEdit(cudaStream_t st_) : st(st_) {}
+  ~IvfEdit() { cudaStreamSynchronize(st); }   // no kernel still reads a buffer when it is freed
   // kept segment {[b, e), dst}; segments come in ascending order
   void keep(uint32_t b, uint32_t e, uint32_t dst) {
     kept.push_back(b); kept.push_back(e); kept_dst.push_back(dst);
@@ -1263,34 +1235,39 @@ struct IvfEdit {
   }
 };
 
+template <class T>
+static int ivf_edit_buf(StbBuf<T> &b, size_t bytes) {
+  return b.alloc((std::max<size_t>(bytes, 16) + sizeof(T) - 1) / sizeof(T));
+}
+
 static int ivf_edit_alloc(stb_ivfpq *x, IvfEdit &e) {
   const uint32_t nlist = x->nlist;
   const uint64_t m = e.m, n_old = x->list_off_h[nlist];
-  cudaStream_t st = e.t.st;
+  cudaStream_t st = e.st;
   e.key_bits = 32 - __builtin_clz(nlist);          // 2^key_bits - 1 >= nlist: IVF_NO_LIST sorts last
   if (m) {
     cub::DoubleBuffer<uint32_t> kb(nullptr, nullptr), vb(nullptr, nullptr);
     STB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, e.sort_bytes, kb, vb, (uint32_t)m, 0, e.key_bits, st));
   }
-  IVF_TRY(e.t.alloc(&e.assign, m * 4));
-  IVF_TRY(e.t.alloc(&e.assign_alt, m * 4));
-  IVF_TRY(e.t.alloc(&e.vals, m * 4));
-  IVF_TRY(e.t.alloc(&e.vals_alt, m * 4));
-  IVF_TRY(e.t.alloc(&e.codes_row, m * PQ_M));
-  IVF_TRY(e.t.alloc(&e.counts, (size_t)(nlist + 1) * 4));
-  IVF_TRY(e.t.alloc(&e.sort_tmp, e.sort_bytes));
-  IVF_TRY(e.t.alloc(&e.codes, (n_old + m) * PQ_M));
-  IVF_TRY(e.t.alloc(&e.order, (n_old + m) * 4));
-  IVF_TRY(e.t.alloc(&e.new_off_d, (size_t)(nlist + 1) * 4));
-  IVF_TRY(e.t.alloc(&e.forced, IVF_FORCED_CAP * 4));
-  if (!e.rows_h.empty()) IVF_TRY(e.t.alloc(&e.new_rows, m * 4));
+  IVF_TRY(ivf_edit_buf(e.assign, m * 4));
+  IVF_TRY(ivf_edit_buf(e.assign_alt, m * 4));
+  IVF_TRY(ivf_edit_buf(e.vals, m * 4));
+  IVF_TRY(ivf_edit_buf(e.vals_alt, m * 4));
+  IVF_TRY(ivf_edit_buf(e.codes_row, m * PQ_M));
+  IVF_TRY(ivf_edit_buf(e.counts, (size_t)(nlist + 1) * 4));
+  IVF_TRY(ivf_edit_buf(e.sort_tmp, e.sort_bytes));
+  IVF_TRY(ivf_edit_buf(e.codes, (n_old + m) * PQ_M));
+  IVF_TRY(ivf_edit_buf(e.order, (n_old + m) * 4));
+  IVF_TRY(ivf_edit_buf(e.new_off_d, (size_t)(nlist + 1) * 4));
+  IVF_TRY(ivf_edit_buf(e.forced, IVF_FORCED_CAP * 4));
+  if (!e.rows_h.empty()) IVF_TRY(ivf_edit_buf(e.new_rows, m * 4));
   if (!e.keep_all) {
-    IVF_TRY(e.t.alloc(&e.kept_d, (size_t)e.n_kept * 3 * 4));   // pairs, then dst
-    IVF_TRY(e.t.alloc(&e.bitmap, (x->n + 31) / 32 * 4));
-    IVF_TRY(e.t.alloc(&e.elig, (size_t)nlist * 4));
-    IVF_TRY(e.t.alloc(&e.surv_pos, n_old * 4));
-    IVF_TRY(e.t.alloc(&e.surv_row, n_old * 4));
-    IVF_TRY(e.t.alloc(&e.surv_off_d, (size_t)(nlist + 1) * 4));
+    IVF_TRY(ivf_edit_buf(e.kept_d, (size_t)e.n_kept * 3 * 4));   // pairs, then dst
+    IVF_TRY(ivf_edit_buf(e.bitmap, (x->n + 31) / 32 * 4));
+    IVF_TRY(ivf_edit_buf(e.elig, (size_t)nlist * 4));
+    IVF_TRY(ivf_edit_buf(e.surv_pos, n_old * 4));
+    IVF_TRY(ivf_edit_buf(e.surv_row, n_old * 4));
+    IVF_TRY(ivf_edit_buf(e.surv_off_d, (size_t)(nlist + 1) * 4));
   }
   STB_CUDA(cudaMemsetAsync(e.counts, 0, (size_t)(nlist + 1) * 4, st));
   return STB_OK;
@@ -1300,7 +1277,7 @@ static int ivf_edit_alloc(stb_ivfpq *x, IvfEdit &e) {
 static int ivf_edit_encode(stb_ivfpq *x, IvfEdit &e, const float *X, uint64_t i0, uint64_t mc) {
   if (mc == 0) return STB_OK;
   stb_ctx *ctx = x->ctx;
-  cudaStream_t st = e.t.st;
+  cudaStream_t st = e.st;
   const float4 *X4 = reinterpret_cast<const float4 *>(X);
   ivf_assign_kernel<<<(unsigned)((mc + 63) / 64), 256, 0, st>>>(X, mc, x->centroids, x->nlist, e.assign + i0);
   STB_CUDA(cudaFuncSetAttribute(pq_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * PQ_KSUB * PQ_DSUB * 4));
@@ -1330,7 +1307,7 @@ static bool ivf_edit_renumber(const IvfEdit &e, uint32_t row, uint32_t &out) {
 
 static int ivf_edit_plan(stb_ivfpq *x, IvfEdit &e, const char *who) {
   stb_ctx *ctx = x->ctx;
-  cudaStream_t st = e.t.st;
+  cudaStream_t st = e.st;
   const uint32_t nlist = x->nlist;
   const uint64_t m = e.m;
   cub::DoubleBuffer<uint32_t> kb(e.assign, e.assign_alt), vb(e.vals, e.vals_alt);
@@ -1410,10 +1387,9 @@ static int ivf_edit_plan(stb_ivfpq *x, IvfEdit &e, const char *who) {
 // Installs a planned edit.  Searches enqueued before it have finished (the stream is synchronised), so the
 // old arrays can go.
 static int ivf_edit_swap(stb_ivfpq *x, IvfEdit &e) {
-  STB_CUDA(cudaStreamSynchronize(e.t.st));
-  e.t.adopt(e.codes); e.t.adopt(e.order); e.t.adopt(e.new_off_d); e.t.adopt(e.forced);
-  cudaFree(x->codes); cudaFree(x->order); cudaFree(x->list_off); cudaFree(x->forced);
-  x->codes = e.codes; x->order = e.order; x->list_off = e.new_off_d; x->forced = e.forced;
+  STB_CUDA(cudaStreamSynchronize(e.st));
+  x->codes = std::move(e.codes); x->order = std::move(e.order); x->list_off = std::move(e.new_off_d);
+  x->forced = std::move(e.forced);
   x->list_off_h.swap(e.new_off);
   x->n_forced = (uint32_t)e.forced_h.size();
   x->n = e.n_after;
@@ -1436,26 +1412,31 @@ extern "C" {
 int stb_ivfpq_destroy(stb_ivfpq *x) {
   if (!x) return STB_OK;
   const_cast<stb_corpus *>(x->corpus)->ivfpq_live--;
-  cudaFree(x->centroids); cudaFree(x->codebooks); cudaFree(x->codes); cudaFree(x->order); cudaFree(x->list_off);
-  cudaFree(x->coarse); cudaFree(x->lut); cudaFree(x->probe); cudaFree(x->cand); cudaFree(x->cand_rows);
-  cudaFree(x->keys2); cudaFree(x->tickets); cudaFree(x->forced);
-  cudaFree(x->b_q); cudaFree(x->b_coarse); cudaFree(x->b_probe); cudaFree(x->b_lut); cudaFree(x->b_kept);
-  cudaFree(x->b_drop); cudaFree(x->b_hits); cudaFree(x->b_status);
-  cudaFree(x->f_bitmap); cudaFree(x->f_elig); cudaFree(x->f_ranges);
-  cudaGetLastError();
   delete x;
   return STB_OK;
 }
 
+// stb_ivfpq_build's failure exits: the stream is synchronised, so no kernel still reads a buffer the index or the
+// training temporaries free on the way out
+#define IVF_FAIL(rc)                                                                    \
+  do {                                                                                  \
+    cudaStreamSynchronize(st);                                                          \
+    cudaGetLastError();                                                                 \
+    stb_ivfpq_destroy(x);                                                               \
+    return (rc);                                                                        \
+  } while (0)
 #define IVF_CUDA(call)                                                                  \
   do {                                                                                  \
     cudaError_t _e = (call);                                                            \
     if (_e != cudaSuccess) {                                                            \
       stb_set_error("%s:%d: %s -> %s", __FILE__, __LINE__, #call, cudaGetErrorString(_e)); \
-      cudaGetLastError();                                                               \
-      stb_ivfpq_destroy(x);                                                             \
-      return STB_ERR_CUDA;                                                              \
+      IVF_FAIL(STB_ERR_CUDA);                                                           \
     }                                                                                   \
+  } while (0)
+#define IVF_ALLOC(buf, n)                                                               \
+  do {                                                                                  \
+    const int _rc = (buf).alloc(n);                                                     \
+    if (_rc != STB_OK) IVF_FAIL(_rc);                                                   \
   } while (0)
 
 int stb_ivfpq_build(stb_ctx *ctx, const stb_corpus *corpus, uint32_t nlist, uint32_t train_rows, uint32_t iters,
@@ -1473,38 +1454,30 @@ int stb_ivfpq_build(stb_ctx *ctx, const stb_corpus *corpus, uint32_t nlist, uint
   // counted from here: every failure below ends in stb_ivfpq_destroy, which takes the count back, so only a
   // built index holds it (stb_corpus_update / stb_corpus_remove refuse while it does)
   const_cast<stb_corpus *>(corpus)->ivfpq_live++;
-  x->centroids = nullptr; x->codebooks = nullptr; x->codes = nullptr; x->order = nullptr; x->list_off = nullptr;
-  x->coarse = nullptr; x->lut = nullptr; x->probe = nullptr; x->cand = nullptr; x->cand_cap = 0; x->cand_rows = nullptr;
-  x->keys2 = nullptr; x->tickets = nullptr; x->forced = nullptr; x->n_forced = 0;
-  x->b_cap = 0; x->b_q = nullptr; x->b_coarse = nullptr; x->b_probe = nullptr; x->b_lut = nullptr; x->b_kept = nullptr;
-  x->b_drop = nullptr; x->b_hits = nullptr; x->b_status = nullptr;
-  for (int i = 0; i < 4; ++i) x->last_info[i] = 0;
-  x->last_filtered = false;
-  x->f_bitmap = nullptr; x->f_words = 0; x->f_elig = nullptr; x->f_ranges = nullptr; x->f_ranges_cap = 0;
   cudaStream_t st = ctx->stream;
   // training sample: every `stride`-th row
   uint64_t ns = std::min<uint64_t>(n, std::max<uint32_t>(train_rows, nlist * 32u));
   const uint64_t stride = std::max<uint64_t>(1, n / ns);
   ns = std::min<uint64_t>(ns, (n + stride - 1) / stride);
   const float4 *X4 = reinterpret_cast<const float4 *>(corpus->rows);
-  float *sums = nullptr, *pq_sums = nullptr;
-  uint32_t *counts = nullptr, *pq_counts = nullptr, *assign = nullptr;
-  IVF_CUDA(cudaMalloc(&x->centroids, (size_t)nlist * STB_D * 4));
-  IVF_CUDA(cudaMalloc(&x->codebooks, (size_t)PQ_M * PQ_KSUB * PQ_DSUB * 4));
-  IVF_CUDA(cudaMalloc(&sums, (size_t)nlist * STB_D * 4));
-  IVF_CUDA(cudaMalloc(&counts, (size_t)(nlist + 1) * 4));
-  IVF_CUDA(cudaMalloc(&pq_sums, (size_t)PQ_M * PQ_KSUB * PQ_DSUB * 4));
-  IVF_CUDA(cudaMalloc(&pq_counts, (size_t)PQ_M * PQ_KSUB * 4));
-  IVF_CUDA(cudaMalloc(&assign, ns * 4));
+  // training temporaries: freed on every way out, and before the add phase allocates its own
+  StbBuf<float> sums, pq_sums, sample;
+  StbBuf<uint32_t> counts, pq_counts, assign;
+  IVF_ALLOC(x->centroids, (size_t)nlist * STB_D);
+  IVF_ALLOC(x->codebooks, (size_t)PQ_M * PQ_KSUB * PQ_DSUB);
+  IVF_ALLOC(sums, (size_t)nlist * STB_D);
+  IVF_ALLOC(counts, (size_t)nlist + 1);
+  IVF_ALLOC(pq_sums, (size_t)PQ_M * PQ_KSUB * PQ_DSUB);
+  IVF_ALLOC(pq_counts, (size_t)PQ_M * PQ_KSUB);
+  IVF_ALLOC(assign, ns);
   // ---- coarse k-means on the sample (strided view of the corpus: stride in rows) --------
   // initial centroids: evenly spaced sample rows, normalised
   IVF_CUDA(cudaMemsetAsync(counts, 0, (size_t)nlist * 4, st));
   ivf_finish_centroids_kernel<<<(nlist + 7) / 8, 256, 0, st>>>(x->centroids, sums, counts, nlist, X4, ns, stride, 0);
   // the strided sample is gathered into a dense buffer so the GEMM kernel sees contiguous rows
-  float *sample = nullptr;
-  IVF_CUDA(cudaMalloc(&sample, ns * STB_D * 4));
+  IVF_ALLOC(sample, ns * STB_D);
   IVF_CUDA(cudaMemcpy2DAsync(sample, STB_D * 4, corpus->rows, stride * STB_D * 4, STB_D * 4, ns, cudaMemcpyDeviceToDevice, st));
-  const float4 *S4 = reinterpret_cast<const float4 *>(sample);
+  const float4 *S4 = reinterpret_cast<const float4 *>(sample.p);
   for (uint32_t it = 0; it < iters; ++it) {
     ivf_assign_kernel<<<(unsigned)((ns + 63) / 64), 256, 0, st>>>(sample, ns, x->centroids, nlist, assign);
     IVF_CUDA(cudaMemsetAsync(sums, 0, (size_t)nlist * STB_D * 4, st));
@@ -1531,20 +1504,20 @@ int stb_ivfpq_build(stb_ctx *ctx, const stb_corpus *corpus, uint32_t nlist, uint
   IVF_CUDA(cudaGetLastError());
   // training buffers go before the add phase allocates its own
   IVF_CUDA(cudaStreamSynchronize(st));
-  cudaFree(sums); cudaFree(counts); cudaFree(pq_sums); cudaFree(pq_counts); cudaFree(assign); cudaFree(sample);
+  sums = {}; counts = {}; pq_sums = {}; pq_counts = {}; assign = {}; sample = {};
   // ---- add: rows [0, n) into empty lists, as stb_ivfpq_extend adds its rows ----------------------
-  IVF_CUDA(cudaMalloc(&x->list_off, (size_t)(nlist + 1) * 4));
+  IVF_ALLOC(x->list_off, (size_t)nlist + 1);
   IVF_CUDA(cudaMemsetAsync(x->list_off, 0, (size_t)(nlist + 1) * 4, st));
   x->list_off_h.assign(nlist + 1, 0);
   int rc = ivf_add_rows(x, 0, n, "ivfpq_build");
-  if (rc != STB_OK) { stb_ivfpq_destroy(x); return rc; }
+  if (rc != STB_OK) IVF_FAIL(rc);
   // query scratch
-  IVF_CUDA(cudaMalloc(&x->coarse, (size_t)nlist * 4));
-  IVF_CUDA(cudaMalloc(&x->lut, (size_t)PQ_M * PQ_KSUB * 4));
-  IVF_CUDA(cudaMalloc(&x->probe, (size_t)(2 * 1024 + 1) * 4));
-  IVF_CUDA(cudaMalloc(&x->cand_rows, (IVF_HOST_TOPK_MAX + IVF_FORCED_CAP) * 4 + 16));   // + the valid-row counter
-  IVF_CUDA(cudaMalloc(&x->keys2, (size_t)ADC2_MAX_CTAS * ADC2_KEEP * 8));
-  IVF_CUDA(cudaMalloc(&x->tickets, 2 * sizeof(unsigned int)));
+  IVF_ALLOC(x->coarse, nlist);
+  IVF_ALLOC(x->lut, (size_t)PQ_M * PQ_KSUB);
+  IVF_ALLOC(x->probe, 2 * 1024 + 1);
+  IVF_ALLOC(x->cand_rows, IVF_HOST_TOPK_MAX + IVF_FORCED_CAP + 4);   // + the valid-row counter
+  IVF_ALLOC(x->keys2, (size_t)ADC2_MAX_CTAS * ADC2_KEEP);
+  IVF_ALLOC(x->tickets, 2);
   IVF_CUDA(cudaMemsetAsync(x->tickets, 0, 2 * sizeof(unsigned int), ctx->stream));
   IVF_CUDA(cudaGetLastError());
   IVF_CUDA(cudaStreamSynchronize(st));
@@ -1732,25 +1705,21 @@ int stb_ivfpq_search_dev(stb_ivfpq *x, const float *q_dev, uint32_t nprobe, uint
 }
 
 // ---- batched search ----
-// grows the batch scratch to hold nq (<= IVFB_MAX_NQ) queries; cudaFree synchronises, so a batch still
-// in flight finishes before its buffers go
+// grows the batch scratch to hold nq (<= IVFB_MAX_NQ) queries, sized exactly: all eight buffers go before any is
+// allocated again.  cudaFree synchronises, so a batch still in flight finishes before its buffers go.
 static int ivfb_reserve(stb_ivfpq *x, uint32_t nq) {
   if (nq <= x->b_cap) return STB_OK;
-  const uint32_t cap = std::min<uint32_t>(IVFB_MAX_NQ, (nq + 63) / 64 * 64);
-  cudaFree(x->b_q); cudaFree(x->b_coarse); cudaFree(x->b_probe); cudaFree(x->b_lut); cudaFree(x->b_kept);
-  cudaFree(x->b_drop); cudaFree(x->b_hits); cudaFree(x->b_status);
-  x->b_q = nullptr; x->b_coarse = nullptr; x->b_probe = nullptr; x->b_lut = nullptr; x->b_kept = nullptr;
-  x->b_drop = nullptr; x->b_hits = nullptr; x->b_status = nullptr;
+  const size_t cap = std::min<uint32_t>(IVFB_MAX_NQ, (nq + 63) / 64 * 64);
   x->b_cap = 0;
-  STB_CUDA(cudaMalloc(&x->b_q, (size_t)cap * STB_D * 4));
-  STB_CUDA(cudaMalloc(&x->b_coarse, (size_t)cap * x->nlist * 4));
-  STB_CUDA(cudaMalloc(&x->b_probe, (size_t)cap * IVFB_PROBE_STRIDE(1024, true) * 4));
-  STB_CUDA(cudaMalloc(&x->b_lut, (size_t)cap * PQ_M * PQ_KSUB * 4));
-  STB_CUDA(cudaMalloc(&x->b_kept, (size_t)cap * IVFB_KEPT * 8));
-  STB_CUDA(cudaMalloc(&x->b_drop, (size_t)cap * IVFB_WARPS * 8));
-  STB_CUDA(cudaMalloc(&x->b_hits, (size_t)cap * 1024 * sizeof(stb_hit)));
-  STB_CUDA(cudaMalloc(&x->b_status, (size_t)cap * 2 * 4));
-  x->b_cap = cap;
+  x->b_q = {}; x->b_coarse = {}; x->b_probe = {}; x->b_lut = {}; x->b_kept = {}; x->b_drop = {}; x->b_hits = {}; x->b_status = {};
+  int rc;
+  if ((rc = x->b_q.alloc(cap * STB_D)) != STB_OK || (rc = x->b_coarse.alloc(cap * x->nlist)) != STB_OK ||
+      (rc = x->b_probe.alloc(cap * IVFB_PROBE_STRIDE(1024, true))) != STB_OK ||
+      (rc = x->b_lut.alloc(cap * PQ_M * PQ_KSUB)) != STB_OK || (rc = x->b_kept.alloc(cap * IVFB_KEPT)) != STB_OK ||
+      (rc = x->b_drop.alloc(cap * IVFB_WARPS)) != STB_OK || (rc = x->b_hits.alloc(cap * 1024)) != STB_OK ||
+      (rc = x->b_status.alloc(cap * 2)) != STB_OK)
+    return rc;
+  x->b_cap = (uint32_t)cap;
   return STB_OK;
 }
 
@@ -1895,25 +1864,15 @@ int stb_ivfpq_search_filtered(stb_ivfpq *x, const float *q, uint32_t nq, uint32_
   ivfb_clamp(x, top_k, nprobe, rerank);
   cudaStream_t st = ctx->stream;
   // eligibility pass: bitmap of the eligible rows, eligible codes per list
-  if (!x->f_elig) STB_CUDA(cudaMalloc(&x->f_elig, (size_t)x->nlist * 4));
+  int rc;
+  if ((rc = x->f_elig.reserve(x->nlist)) != STB_OK) return rc;
   const uint32_t *bitmap = nullptr;
   if (row_ranges) {
     const uint64_t words = (x->n + 31) / 32;
-    if (words > x->f_words) {
-      cudaFree(x->f_bitmap); x->f_bitmap = nullptr; x->f_words = 0;
-      STB_CUDA(cudaMalloc(&x->f_bitmap, words * 4));
-      x->f_words = words;
-    }
     const uint32_t nr = (uint32_t)(loc.size() / 2);
-    if (nr > x->f_ranges_cap) {
-      const uint32_t cap = std::max<uint32_t>(nr, 1024);
-      cudaFree(x->f_ranges); x->f_ranges = nullptr; x->f_ranges_cap = 0;
-      STB_CUDA(cudaMalloc(&x->f_ranges, (size_t)cap * 2 * 4));
-      x->f_ranges_cap = cap;
-    }
+    if ((rc = x->f_bitmap.reserve(words)) != STB_OK || (rc = x->f_ranges.reserve(loc.size(), 2048)) != STB_OK) return rc;
     STB_CUDA(cudaMemcpyAsync(x->f_ranges, loc.data(), loc.size() * 4, cudaMemcpyHostToDevice, st));
-    const int rc = stb_launch_row_bitmap(ctx, x->f_ranges, nr, words, x->f_bitmap);
-    if (rc != STB_OK) return rc;
+    if ((rc = stb_launch_row_bitmap(ctx, x->f_ranges, nr, words, x->f_bitmap)) != STB_OK) return rc;
     bitmap = x->f_bitmap;
   }
   ivff_elig_kernel<<<(x->nlist + 7) / 8, 256, 0, st>>>(x->list_off, x->order, x->nlist, bitmap, x->f_elig);
@@ -1922,7 +1881,7 @@ int stb_ivfpq_search_filtered(stb_ivfpq *x, const float *q, uint32_t nq, uint32_
   IvfbFilter f;
   f.bitmap = bitmap; f.elig = x->f_elig;
   f.max_dist = has_max ? std::min(max_distance, STB_DEFAULT_MAX_DIST) : STB_DEFAULT_MAX_DIST;   // as stb_search
-  const int rc = ivfb_host_chunks(x, q, nq, nprobe, top_k, rerank, out_hits, out_n, out_scanned, &f);
+  rc = ivfb_host_chunks(x, q, nq, nprobe, top_k, rerank, out_hits, out_n, out_scanned, &f);
   STB_CUDA(cudaStreamSynchronize(st));                         // `loc` is read by the copy above
   return rc;
 }
@@ -1973,11 +1932,7 @@ int stb_ivfpq_search(stb_ivfpq *x, const float *q, uint32_t nprobe, uint32_t top
     const uint32_t ctas = std::max<uint32_t>(1, std::min<uint32_t>(std::max((total + 2047) / 2048, (want + 511) / 512), 64));
     uint64_t m = (uint64_t)ctas * 8 * 64, m_pad = 1024;
     while (m_pad < m) m_pad <<= 1;
-    if (m_pad > x->cand_cap) {
-      cudaFree(x->cand); x->cand = nullptr; x->cand_cap = 0;
-      STB_CUDA(cudaMalloc(&x->cand, m_pad * sizeof(stb_hit)));
-      x->cand_cap = m_pad;
-    }
+    if ((rc = x->cand.reserve(m_pad)) != STB_OK) return rc;
     if (m_pad > m) {   // padding entries: +inf
       std::vector<stb_hit> pad(m_pad - m);
       for (auto &h : pad) { h.distance = INFINITY; h.row = 0xffffffffffffffffull; }
@@ -2008,11 +1963,7 @@ int stb_ivfpq_search(stb_ivfpq *x, const float *q, uint32_t nprobe, uint32_t top
   // exact canonical distances of the nv candidate rows, sorted by (distance,row)
   uint64_t e_pad = 1024;
   while (e_pad < nv) e_pad <<= 1;
-  if ((size_t)e_pad > ctx->collect_hits_cap) {
-    cudaFree(ctx->collect_hits); ctx->collect_hits = nullptr; ctx->collect_hits_cap = 0;
-    STB_CUDA(cudaMalloc(&ctx->collect_hits, e_pad * sizeof(stb_hit)));
-    ctx->collect_hits_cap = e_pad;
-  }
+  if ((rc = ctx->collect_hits.reserve(e_pad)) != STB_OK) return rc;
   if ((rc = stb_launch_exact(ctx, x->corpus->rows, x->corpus->row_base, ctx->q_dev, x->cand_rows, nv, STB_DEFAULT_MAX_DIST,
                              ctx->collect_hits, e_pad, ctx->collect_count + 1)) != STB_OK) return rc;
   if ((rc = stb_launch_sort_hits(ctx, ctx->collect_hits, e_pad)) != STB_OK) return rc;

@@ -1263,7 +1263,7 @@ static int stb_launch_topk_t(stb_ctx *ctx, const TopkArgs &a_in, bool overlapped
   if (want < grid) grid = want < 1 ? 1 : want;
   // scratch: lists (KP keys + bound) for all tree levels (< 2 * grid lists), counters (< grid groups)
   size_t need_keys = (size_t)2 * grid * (32 * E + 1) + STB_SORT_CAP;
-  if (need_keys > ctx->block_keys_cap || grid + 8 > ctx->counters_cap) {
+  if (need_keys > ctx->block_keys.cap || grid + 8 > ctx->counters.cap) {
     stb_set_error("scan scratch too small (grid=%llu)", (unsigned long long)grid);
     return STB_ERR_STATE;
   }
@@ -1439,7 +1439,7 @@ int stb_launch_scan_collect(stb_ctx *ctx, const stb_corpus *c, int tier,
   a.cos_floor = cos_floor;
   a.out = ctx->collect_rows;
   a.count = ctx->collect_count;
-  a.cap = ctx->collect_cap;
+  a.cap = ctx->collect_rows.cap;
   STB_CUDA(cudaMemsetAsync(ctx->collect_count, 0, sizeof(unsigned long long), ctx->stream));
   const int u = tier == STB_TIER_Q8 ? STB_Q8_SCAN_U : STB_SCAN_U;
   uint64_t tiles = (n_virtual + 4 * u - 1) / (4 * u);
