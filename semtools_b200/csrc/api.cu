@@ -639,9 +639,9 @@ static uint64_t capped_hits(const stb_hit *hits, uint64_t n, int has_max, double
   return i;
 }
 
-// ---- row ranges: global -> local, clipped to this shard, uploaded as the K1 passes read them (ScanArgs: the
-// virtual prefix of every range, then its first local row).  Without ranges the pass reads every row; *n_virtual
-// = 0: no row of the corpus lies in the ranges.
+// ---- row ranges: global -> local, clipped to this shard, uploaded as the K1 passes read them: vstart[m + 1] (the
+// virtual prefix of every range, then the total), then rbegin[m] (its first local row); the only decoder is
+// stb_scan_args (scan_topk.cu).  Without ranges the pass reads every row; *n_virtual = 0: no row lies in them.
 static int k1_upload_ranges(stb_ctx *ctx, const stb_corpus *c, const char *what, const uint64_t *row_ranges, uint32_t n_ranges,
                             const uint64_t **ranges_dev, uint32_t *n_loc, uint64_t *n_virtual) {
   *ranges_dev = nullptr;
@@ -1353,6 +1353,20 @@ int stb_corpus_prepare_batch(stb_corpus *corpus) {
 
 }  // extern "C"
 
+// ---- K2 host calls -------------------------------------------------------------------------------------------
+// The record of the last K2 call, which stb_debug_batch_last returns: route, nq, two route words (routes 1-4:
+// n_sample, stride; 5: retried queries, K1 queries; 6: tensor groups, K1 queries), n_seg, seg_cap.
+enum K2Route : uint32_t { kRouteV1 = 1, kRouteV2 = 2, kRouteFiltered = 3, kRouteFilteredK1 = 4, kRouteThreshold = 5,
+                          kRouteSubsets = 6 };
+static void k2_record(stb_ctx *ctx, K2Route route, uint32_t nq, uint32_t a = 0, uint32_t b = 0, uint32_t n_seg = 0,
+                      uint32_t seg_cap = 0) {
+  const uint32_t words[6] = {route, nq, a, b, n_seg, seg_cap};
+  memcpy(ctx->b_last, words, sizeof(words));
+}
+
+// Keys per (query, CTA) segment of the emitting pass of v2 and route 6: ~5 expected at 10M rows / 132 CTAs.
+static constexpr uint32_t kSegCap = 64;
+
 // Pipeline v2's sample size and fit rule over the n_cover tiles it may sample: the COMPLETE tiles of the
 // shard (a padding row must never stand in for a real one), or, filtered, the listed tiles (tiles holding an
 // eligible row; the sampling epilogue takes their maxima over eligible rows only).
@@ -1387,10 +1401,8 @@ static int batch_v2_run(stb_ctx *ctx, const stb_corpus *corpus, const float *q_d
   const uint32_t m_tiles = (nq + 127) / 128, q_pad = m_tiles * 128;
   const uint32_t n_tiles = (uint32_t)((corpus->n + 255) / 256);
   const uint32_t n_emit = tile_ids ? n_cover : n_tiles;
-  constexpr uint32_t kSegCap = 64;                      // per (query, CTA): ~5 expected at 10M rows / 132 CTAs
   const uint32_t n_seg = stb_batch_emit_grid(ctx, n_emit);
-  const uint32_t last[6] = {tile_ids ? 3u : 2u, nq, p.n_sample, p.stride, n_seg, kSegCap};
-  memcpy(ctx->b_last, last, sizeof(last));
+  k2_record(ctx, tile_ids ? kRouteFiltered : kRouteV2, nq, p.n_sample, p.stride, n_seg, kSegCap);
   if ((rc = ctx->b_qbad.reserve((size_t)q_pad)) != STB_OK) return rc;
   if ((rc = ctx->bq_tiles.reserve((size_t)q_pad * 512)) != STB_OK) return rc;
   if ((rc = ctx->b_tilemax.reserve((size_t)p.n_sample * q_pad)) != STB_OK) return rc;
@@ -1419,6 +1431,101 @@ static int batch_v2_run(stb_ctx *ctx, const stb_corpus *corpus, const float *q_d
                                   corpus->row_base, q_dev, ctx->b_qbad, out_hits_dev, out_status_dev);
 }
 
+// The listed tiles of clipped local [begin, end) pairs: the shadow tiles a range touches (ascending, disjoint
+// ranges -> ascending tiles).
+static std::vector<uint32_t> listed_tiles(const std::vector<uint32_t> &loc) {
+  std::vector<uint32_t> tiles;
+  for (size_t r = 0; r < loc.size(); r += 2)
+    for (uint32_t t = loc[r] / 256; t <= (loc[r + 1] - 1) / 256; ++t)
+      if (tiles.empty() || tiles.back() < t) tiles.push_back(t);
+  return tiles;
+}
+
+// How a K2 host call answers query i once its tensor passes are done (k2_complete).
+struct K2Answer {
+  enum Kind { kEmpty, kProven, kK1 } kind;
+  const stb_hit *hits;       // kProven: the proven result, `n` hits (it may already be the output row)
+  uint64_t n;
+  const uint64_t *ranges;    // kK1: the query's ranges, as stb_search takes them
+  uint32_t n_ranges;
+};
+
+// Completes a K2 host call: query i gets 0 hits, its proven tensor result capped at max_distance, or K1's answer
+// (stb_search in `mode`, counted in fallback_searches), as answer(i) says; every row is then padded to top_k.
+// *n_k1 (if given): the queries K1 answered.
+template <class Answer>
+static int k2_complete(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t nq, uint32_t top_k, int has_max,
+                       double max_distance, int mode, Answer &&answer, stb_hit *out_hits, uint32_t *out_n,
+                       uint32_t *n_k1 = nullptr) {
+  uint32_t k1 = 0;
+  for (uint32_t i = 0; i < nq; ++i) {
+    stb_hit *oh = out_hits + (size_t)i * top_k;
+    const K2Answer a = answer(i);
+    uint64_t n = 0;
+    if (a.kind == K2Answer::kProven) {
+      if (a.hits != oh) memcpy(oh, a.hits, (size_t)top_k * sizeof(stb_hit));
+      n = capped_hits(oh, a.n, has_max, max_distance);
+    } else if (a.kind == K2Answer::kK1) {
+      ctx->fallback_searches++;
+      k1++;
+      const int rc = stb_search(ctx, corpus, q + (size_t)i * STB_D, top_k, has_max, max_distance, mode, a.ranges, a.n_ranges,
+                                oh, top_k, &n);
+      if (rc != STB_OK) return rc;
+    }
+    out_n[i] = (uint32_t)n;
+    stb_pad_hits(oh, n, top_k);
+  }
+  if (n_k1) *n_k1 = k1;
+  return STB_OK;
+}
+
+// The store query (stb_search in STB_MODE_STORE_QUERY) for a batch, over `loc`: the caller's row_ranges clipped
+// to local [begin, end) pairs (K1 answers with the former).  The eligible rows' bitmap and the listed tiles both
+// come from `loc`; filtered v2 runs when its plan fits over the listed tiles, and K1 answers every query it leaves
+// unproven (or all of them, route 4).  The cap is applied on the host: store-query hits are a prefix of the
+// uncapped top-k.
+static int batch_filtered_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, uint32_t nq, uint32_t top_k, int has_max,
+                              double max_distance, const std::vector<uint32_t> &loc, const uint64_t *row_ranges,
+                              uint32_t n_ranges, stb_hit *out_hits, uint32_t *out_n) {
+  int rc;
+  k2_record(ctx, kRouteFilteredK1, nq);
+  if (loc.empty())
+    return k2_complete(ctx, corpus, q, nq, top_k, has_max, max_distance, STB_MODE_STORE_QUERY,
+                       [](uint32_t) { return K2Answer{K2Answer::kEmpty}; }, out_hits, out_n);
+  const std::vector<uint32_t> tiles = listed_tiles(loc);
+  const uint32_t n_listed = (uint32_t)tiles.size();
+  const BatchV2Plan plan = batch_v2_plan(ctx, n_listed, top_k);
+  bool tensor_ok = plan.fits;
+  if (tensor_ok) {
+    rc = corpus_ensure_shadow(ctx, corpus);
+    if (rc == STB_ERR_STATE) tensor_ok = false;          // un-normalisable rows: K1 handles them
+    else if (rc != STB_OK) return rc;
+  }
+  std::vector<uint32_t> status((size_t)nq * 2, 0);
+  if (tensor_ok) {
+    const uint64_t n_words = (corpus->n + 255) / 256 * 8;
+    if ((rc = ctx->bq_dev.reserve((size_t)nq * STB_D)) != STB_OK) return rc;
+    if ((rc = ctx->bh_dev.reserve((size_t)nq * top_k)) != STB_OK) return rc;
+    if ((rc = ctx->bs_dev.reserve((size_t)nq * 2)) != STB_OK) return rc;
+    if ((rc = ctx->b_franges.reserve(loc.size(), 2048)) != STB_OK) return rc;
+    if ((rc = ctx->b_ftiles.reserve(tiles.size(), 1024)) != STB_OK) return rc;
+    if ((rc = ctx->b_fbits.reserve((size_t)n_words)) != STB_OK) return rc;
+    STB_CUDA(cudaMemcpyAsync(ctx->bq_dev, q, (size_t)nq * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    STB_CUDA(cudaMemcpyAsync(ctx->b_franges, loc.data(), loc.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+    STB_CUDA(cudaMemcpyAsync(ctx->b_ftiles, tiles.data(), tiles.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+    if ((rc = stb_launch_row_bitmap(ctx, ctx->b_franges, (uint32_t)(loc.size() / 2), n_words, ctx->b_fbits)) != STB_OK) return rc;
+    if ((rc = batch_v2_run(ctx, corpus, ctx->bq_dev, nq, top_k, n_listed, plan, ctx->b_ftiles, ctx->b_fbits, ctx->bh_dev,
+                           ctx->bs_dev)) != STB_OK) return rc;
+    STB_CUDA(cudaMemcpyAsync(out_hits, ctx->bh_dev, (size_t)nq * top_k * sizeof(stb_hit), cudaMemcpyDeviceToHost, ctx->stream));
+    STB_CUDA(cudaMemcpyAsync(status.data(), ctx->bs_dev, (size_t)nq * 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    STB_CUDA(cudaStreamSynchronize(ctx->stream));        // `loc` and `tiles` are read by the copies above
+  }
+  return k2_complete(ctx, corpus, q, nq, top_k, has_max, max_distance, STB_MODE_STORE_QUERY, [&](uint32_t i) -> K2Answer {
+    if (tensor_ok && status[2 * i + 1]) return {K2Answer::kProven, out_hits + (size_t)i * top_k, status[2 * i]};
+    return {K2Answer::kK1, nullptr, 0, row_ranges, n_ranges};
+  }, out_hits, out_n);
+}
+
 extern "C" {
 
 int stb_search_batch_dev(stb_ctx *ctx, const stb_corpus *corpus_c, const float *q_dev, uint32_t nq,
@@ -1442,8 +1549,7 @@ int stb_search_batch_dev(stb_ctx *ctx, const stb_corpus *corpus_c, const float *
   // one flag per query, written by the query shadow build: a query that cannot be normalised in fp32
   // has a zero (or NaN) shadow whose scores bound nothing, and both finish kernels report it unproven
   if ((rc = ctx->b_qbad.reserve((size_t)q_pad)) != STB_OK) return rc;
-  const uint32_t last[6] = {1u, nq, 0u, 0u, 0u, 0u};
-  memcpy(ctx->b_last, last, sizeof(last));
+  k2_record(ctx, kRouteV1, nq);
   // selection slices: enough CTAs (m_tiles x n_slices) to hide the latency of the streaming
   // read; the finish kernel merges n_slices x 32 <= 4096 candidate tiles per query
   uint32_t n_slices = std::max<uint32_t>(1, std::min<uint32_t>(128, 1536 / m_tiles));
@@ -1490,23 +1596,12 @@ int stb_search_batch(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uin
     }
   }
   // queries the tensor path could not prove (or could not run): exact single-query path
-  for (uint32_t i = 0; i < nq; ++i) {
-    if (tensor_ok && status[2 * i + 1]) { out_n[i] = status[2 * i]; continue; }
-    ctx->fallback_searches++;
-    uint64_t n = 0;
-    rc = stb_search(ctx, corpus, q + (size_t)i * STB_D, top_k, 0, 0.0, STB_MODE_SEARCH_DOCUMENTS, nullptr, 0,
-                    out_hits + (size_t)i * top_k, top_k, &n);
-    if (rc != STB_OK) return rc;
-    out_n[i] = (uint32_t)n;
-    for (uint64_t j = n; j < top_k; ++j) { out_hits[(size_t)i * top_k + j].distance = INFINITY; out_hits[(size_t)i * top_k + j].row = 0xffffffffffffffffull; }
-  }
-  return STB_OK;
+  return k2_complete(ctx, corpus, q, nq, top_k, 0, 0.0, STB_MODE_SEARCH_DOCUMENTS, [&](uint32_t i) -> K2Answer {
+    if (tensor_ok && status[2 * i + 1]) return {K2Answer::kProven, out_hits + (size_t)i * top_k, status[2 * i]};
+    return {K2Answer::kK1};
+  }, out_hits, out_n);
 }
 
-// The store query (stb_search in STB_MODE_STORE_QUERY) for a batch.  The eligible rows' bitmap and the listed
-// tiles both come from one list of clipped ranges; filtered v2 runs when its plan fits over the listed tiles,
-// and K1 answers every query it leaves unproven (or all of them, route 4).  The cap is applied on the host:
-// store-query hits are a prefix of the uncapped top-k.
 int stb_search_batch_filtered(stb_ctx *ctx, const stb_corpus *corpus_c, const float *q, uint32_t nq, uint32_t top_k,
                               int has_max, double max_distance, const uint64_t *row_ranges, uint32_t n_ranges,
                               stb_hit *out_hits, uint32_t *out_n) {
@@ -1518,74 +1613,14 @@ int stb_search_batch_filtered(stb_ctx *ctx, const stb_corpus *corpus_c, const fl
   if (n_ranges && !row_ranges) { stb_set_error("search_batch_filtered: row_ranges is null"); return STB_ERR_ARG; }
   if (nq == 0) return STB_OK;
   if (!q || !out_n || (top_k && !out_hits)) { stb_set_error("search_batch_filtered: null argument"); return STB_ERR_ARG; }
-  auto pad = [&](uint32_t i, uint64_t n) {               // the unused tail, as the kernels pad it
-    for (uint64_t j = n; j < top_k; ++j) { out_hits[(size_t)i * top_k + j].distance = INFINITY; out_hits[(size_t)i * top_k + j].row = 0xffffffffffffffffull; }
-  };
   // stb_search's early outs come before it reads the ranges (store.rs:489-491: top_k 0, the empty subset)
   std::vector<uint32_t> loc;                             // clipped local [begin, end) pairs
   if (top_k && !(row_ranges && n_ranges == 0) && corpus->n) {
-    if (row_ranges) {
-      loc.reserve(2 * (size_t)n_ranges);
-      if ((rc = stb_clip_ranges("search_batch_filtered", row_ranges, n_ranges, corpus->row_base, corpus->n,
-                                [&](uint64_t b, uint64_t e) { loc.push_back((uint32_t)b); loc.push_back((uint32_t)e); })) != STB_OK)
-        return rc;                                       // refused before anything is written
-    } else {
-      loc = {0u, (uint32_t)corpus->n};
-    }
+    if (!row_ranges) loc = {0u, (uint32_t)corpus->n};
+    else if ((rc = stb_clip_ranges_u32("search_batch_filtered", row_ranges, n_ranges, corpus->row_base, corpus->n, &loc)) != STB_OK)
+      return rc;                                         // refused before anything is written
   }
-  const uint32_t none[6] = {4u, nq, 0u, 0u, 0u, 0u};
-  memcpy(ctx->b_last, none, sizeof(none));
-  if (loc.empty()) {
-    for (uint32_t i = 0; i < nq; ++i) { out_n[i] = 0; pad(i, 0); }
-    return STB_OK;
-  }
-  // listed tiles: the shadow tiles a clipped range touches (ascending, disjoint ranges -> ascending tiles)
-  std::vector<uint32_t> tiles;
-  for (size_t r = 0; r < loc.size(); r += 2)
-    for (uint32_t t = loc[r] / 256; t <= (loc[r + 1] - 1) / 256; ++t)
-      if (tiles.empty() || tiles.back() < t) tiles.push_back(t);
-  const uint32_t n_listed = (uint32_t)tiles.size();
-  const BatchV2Plan plan = batch_v2_plan(ctx, n_listed, top_k);
-  bool tensor_ok = plan.fits;
-  if (tensor_ok) {
-    rc = corpus_ensure_shadow(ctx, corpus);
-    if (rc == STB_ERR_STATE) tensor_ok = false;          // un-normalisable rows: K1 handles them
-    else if (rc != STB_OK) return rc;
-  }
-  std::vector<uint32_t> status((size_t)nq * 2, 0);
-  if (tensor_ok) {
-    const uint64_t n_words = (corpus->n + 255) / 256 * 8;
-    if ((rc = ctx->bq_dev.reserve((size_t)nq * STB_D)) != STB_OK) return rc;
-    if ((rc = ctx->bh_dev.reserve((size_t)nq * top_k)) != STB_OK) return rc;
-    if ((rc = ctx->bs_dev.reserve((size_t)nq * 2)) != STB_OK) return rc;
-    if ((rc = ctx->b_franges.reserve(loc.size(), 2048)) != STB_OK) return rc;
-    if ((rc = ctx->b_ftiles.reserve(tiles.size(), 1024)) != STB_OK) return rc;
-    if ((rc = ctx->b_fbits.reserve((size_t)n_words)) != STB_OK) return rc;
-    STB_CUDA(cudaMemcpyAsync(ctx->bq_dev, q, (size_t)nq * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-    STB_CUDA(cudaMemcpyAsync(ctx->b_franges, loc.data(), loc.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-    STB_CUDA(cudaMemcpyAsync(ctx->b_ftiles, tiles.data(), tiles.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-    if ((rc = stb_launch_row_bitmap(ctx, ctx->b_franges, (uint32_t)(loc.size() / 2), n_words, ctx->b_fbits)) != STB_OK) return rc;
-    if ((rc = batch_v2_run(ctx, corpus, ctx->bq_dev, nq, top_k, n_listed, plan, ctx->b_ftiles, ctx->b_fbits, ctx->bh_dev,
-                           ctx->bs_dev)) != STB_OK) return rc;
-    STB_CUDA(cudaMemcpyAsync(out_hits, ctx->bh_dev, (size_t)nq * top_k * sizeof(stb_hit), cudaMemcpyDeviceToHost, ctx->stream));
-    STB_CUDA(cudaMemcpyAsync(status.data(), ctx->bs_dev, (size_t)nq * 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    STB_CUDA(cudaStreamSynchronize(ctx->stream));        // `loc` and `tiles` are read by the copies above
-  }
-  for (uint32_t i = 0; i < nq; ++i) {
-    stb_hit *oh = out_hits + (size_t)i * top_k;
-    uint64_t n = 0;
-    if (tensor_ok && status[2 * i + 1]) {
-      n = capped_hits(oh, status[2 * i], has_max, max_distance);
-    } else {
-      ctx->fallback_searches++;
-      rc = stb_search(ctx, corpus, q + (size_t)i * STB_D, top_k, has_max, max_distance, STB_MODE_STORE_QUERY, row_ranges,
-                      n_ranges, oh, top_k, &n);
-      if (rc != STB_OK) return rc;
-    }
-    out_n[i] = (uint32_t)n;
-    pad(i, n);
-  }
-  return STB_OK;
+  return batch_filtered_run(ctx, corpus, q, nq, top_k, has_max, max_distance, loc, row_ranges, n_ranges, out_hits, out_n);
 }
 
 }  // extern "C"
@@ -1674,9 +1709,6 @@ int stb_search_batch_subsets(stb_ctx *ctx, const stb_corpus *corpus_c, const flo
   if (range_offsets[nq] && !row_ranges) { stb_set_error("search_batch_subsets: row_ranges is null"); return STB_ERR_ARG; }
   auto n_of = [&](uint32_t i) { return (uint32_t)(range_offsets[i + 1] - range_offsets[i]); };
   auto ranges_of = [&](uint32_t i) { return row_ranges + 2 * range_offsets[i]; };
-  auto pad = [&](uint32_t i, uint64_t n) {
-    for (uint64_t j = n; j < top_k; ++j) { out_hits[(size_t)i * top_k + j].distance = INFINITY; out_hits[(size_t)i * top_k + j].row = 0xffffffffffffffffull; }
-  };
   // clip every query's ranges as stb_search would (its refusals come before anything is written); a query with
   // no clipped range has 0 hits (store.rs:489-491, or no row of this shard), the others are grouped
   constexpr uint32_t kNone = 0xffffffffu;
@@ -1700,8 +1732,7 @@ int stb_search_batch_subsets(stb_ctx *ctx, const stb_corpus *corpus_c, const flo
       if (j != same.end()) { group[i] = group[*j]; continue; }
       same.push_back(i);
       loc.clear();
-      if ((rc = stb_clip_ranges("search_batch_subsets", ranges_of(i), n_of(i), corpus->row_base, corpus->n,
-                                [&](uint64_t b, uint64_t e) { loc.push_back((uint32_t)b); loc.push_back((uint32_t)e); })) != STB_OK)
+      if ((rc = stb_clip_ranges_u32("search_batch_subsets", ranges_of(i), n_of(i), corpus->row_base, corpus->n, &loc)) != STB_OK)
         return rc;
       if (loc.empty()) continue;
       auto it = ids.find(loc);                             // a new key is copied only once
@@ -1714,19 +1745,15 @@ int stb_search_batch_subsets(stb_ctx *ctx, const stb_corpus *corpus_c, const flo
   }
   const uint32_t G = (uint32_t)lists.size();
   if (G == 1 && std::find(group.begin(), group.end(), kNone) == group.end())
-    return stb_search_batch_filtered(ctx, corpus, q, nq, top_k, has_max, max_distance, ranges_of(0), n_of(0), out_hits, out_n);
-  uint32_t last[6] = {6u, nq, 0u, 0u, 0u, 0u};
-  memcpy(ctx->b_last, last, sizeof(last));
+    return batch_filtered_run(ctx, corpus, q, nq, top_k, has_max, max_distance, *lists[0], ranges_of(0), n_of(0), out_hits, out_n);
+  k2_record(ctx, kRouteSubsets, nq);
   // the plan of every group; groups whose plan fits run on the tensor cores (tensor group tg = tensor[g])
   const uint32_t n_tiles = (uint32_t)((corpus->n + 255) / 256);
   std::vector<std::vector<uint32_t>> listed(G);
   std::vector<BatchV2Plan> plan(G);
   std::vector<uint32_t> tensor(G, kNone), tgroups;
   for (uint32_t g = 0; g < G; ++g) {
-    const std::vector<uint32_t> &loc = *lists[g];
-    for (size_t r = 0; r < loc.size(); r += 2)
-      for (uint32_t t = loc[r] / 256; t <= (loc[r + 1] - 1) / 256; ++t)
-        if (listed[g].empty() || listed[g].back() < t) listed[g].push_back(t);
+    listed[g] = listed_tiles(*lists[g]);
     plan[g] = batch_v2_plan(ctx, (uint32_t)listed[g].size(), top_k);
     if (plan[g].fits) tgroups.push_back(g);
   }
@@ -1758,7 +1785,6 @@ int stb_search_batch_subsets(stb_ctx *ctx, const stb_corpus *corpus_c, const flo
   const uint32_t nt = (uint32_t)qrow.size();
   std::vector<uint32_t> status((size_t)nt * 2, 0);
   std::vector<stb_hit> hits((size_t)nt * top_k);
-  const uint32_t kSegCap = 64;                               // as batch_v2_run
   uint32_t n_seg = 0;
   if (T) {
     std::vector<std::vector<uint32_t>> sampled(T), tiles_of(T);
@@ -1837,27 +1863,14 @@ int stb_search_batch_subsets(stb_ctx *ctx, const stb_corpus *corpus_c, const flo
   // each caller query's slot and compact row, for stb_debug_batch_last
   ctx->s_map.assign(slot_of.begin(), slot_of.begin() + nq);
   ctx->s_map.insert(ctx->s_map.end(), row_of.begin(), row_of.begin() + nq);
-  uint32_t k1 = 0;
-  for (uint32_t i = 0; i < nq; ++i) {
-    stb_hit *oh = out_hits + (size_t)i * top_k;
-    uint64_t n = 0;
-    const uint32_t r = row_of[i];
-    if (group[i] == kNone) {
-      n = 0;
-    } else if (r != kNone && status[2 * (size_t)r + 1]) {
-      memcpy(oh, hits.data() + (size_t)r * top_k, (size_t)top_k * sizeof(stb_hit));
-      n = capped_hits(oh, status[2 * (size_t)r], has_max, max_distance);
-    } else {
-      ctx->fallback_searches++;
-      k1++;
-      if ((rc = stb_search(ctx, corpus, q + (size_t)i * STB_D, top_k, has_max, max_distance, STB_MODE_STORE_QUERY,
-                           ranges_of(i), n_of(i), oh, top_k, &n)) != STB_OK) return rc;
-    }
-    out_n[i] = (uint32_t)n;
-    pad(i, n);
-  }
-  const uint32_t done[6] = {6u, nq, T, k1, n_seg, T ? kSegCap : 0u};
-  memcpy(ctx->b_last, done, sizeof(done));
+  uint32_t k1;
+  if ((rc = k2_complete(ctx, corpus, q, nq, top_k, has_max, max_distance, STB_MODE_STORE_QUERY, [&](uint32_t i) -> K2Answer {
+         const uint32_t r = row_of[i];
+         if (group[i] == kNone) return {K2Answer::kEmpty};
+         if (r != kNone && status[2 * (size_t)r + 1]) return {K2Answer::kProven, hits.data() + (size_t)r * top_k, status[2 * (size_t)r]};
+         return {K2Answer::kK1, nullptr, 0, ranges_of(i), n_of(i)};
+       }, out_hits, out_n, &k1)) != STB_OK) return rc;
+  k2_record(ctx, kRouteSubsets, nq, T, k1, n_seg, T ? kSegCap : 0u);
   return STB_OK;
 }
 
@@ -1868,6 +1881,7 @@ int stb_search_batch_subsets(stb_ctx *ctx, const stb_corpus *corpus_c, const flo
 // below ~1e-13 (256-term f64 FMA chains, two square roots, one division; DESIGN §5); 1e-12 leaves 10x slack.
 #define STB_THR_DELTA 1.0e-12
 #define STB_THR_SEG_CAP 64u        // first pass: keys per (query, CTA), as pipeline v2
+static_assert(STB_THR_SEG_CAP == kSegCap, "route 5's first pass uses pipeline v2's segment capacity");
 #define STB_THR_CHUNK 4096u        // queries per pipeline run (keeps every candidate count within int)
 
 // The emission threshold of the queries the tensor cores answer: ((1 - M) - EPS) - delta in f64, rounded toward
@@ -2007,8 +2021,7 @@ int stb_search_batch_threshold(stb_ctx *ctx, const stb_corpus *corpus_c, const f
   if (corpus->ctx != ctx) { stb_set_error("search_batch_threshold: corpus belongs to another context"); return STB_ERR_ARG; }
   if (nq == 0) return STB_OK;
   if (!q || !out_offsets || (cap && !out_hits)) { stb_set_error("search_batch_threshold: null argument"); return STB_ERR_ARG; }
-  uint32_t last[6] = {5u, nq, 0u, 0u, 0u, 0u};
-  memcpy(ctx->b_last, last, sizeof(last));
+  k2_record(ctx, kRouteThreshold, nq);
   for (uint32_t i = 0; i <= nq; ++i) out_offsets[i] = 0;
   if (corpus->n == 0 || !(max_distance > 0.0)) return STB_OK;      // NaN or <= 0: no distance is below it
   rc = corpus_ensure_shadow(ctx, corpus);
@@ -2068,8 +2081,7 @@ int stb_search_batch_threshold(stb_ctx *ctx, const stb_corpus *corpus_c, const f
       if (o < cap) memcpy(out_hits + o, k1_hits[j].data(), std::min<uint64_t>(k1_hits[j].size(), cap - o) * sizeof(stb_hit));
     }
   }
-  const uint32_t done[6] = {5u, nq, retried, k1_total, n_seg, tensor_ok ? STB_THR_SEG_CAP : 0u};
-  memcpy(ctx->b_last, done, sizeof(done));
+  k2_record(ctx, kRouteThreshold, nq, retried, k1_total, n_seg, tensor_ok ? STB_THR_SEG_CAP : 0u);
   if (out_offsets[nq] > cap) {
     stb_set_error("search_batch_threshold: %llu hits, capacity %llu", (unsigned long long)out_offsets[nq], (unsigned long long)cap);
     return STB_ERR_CAPACITY;
@@ -2112,8 +2124,8 @@ int stb_debug_batch_last(stb_ctx *ctx, uint32_t info[6], float *thr, uint32_t *c
   if (!info) { stb_set_error("debug_batch_last: null info"); return STB_ERR_ARG; }
   STB_CUDA(cudaStreamSynchronize(ctx->stream));
   memcpy(info, ctx->b_last, sizeof(ctx->b_last));
-  const uint32_t nq = ctx->b_last[1], n_seg = ctx->b_last[4];
-  if (ctx->b_last[0] == 6u && n_seg && nq) {
+  const uint32_t route = ctx->b_last[0], nq = ctx->b_last[1], n_seg = ctx->b_last[4];
+  if (route == kRouteSubsets && n_seg && nq) {
     // slot-indexed thresholds, compact-row counts -> caller order (+inf, 0: a query the tensor passes did not take)
     const uint32_t *slot = ctx->s_map.data(), *row = slot + nq;
     uint32_t n_slots = 0, n_rows = 0;
@@ -2131,7 +2143,7 @@ int stb_debug_batch_last(stb_ctx *ctx, uint32_t info[6], float *thr, uint32_t *c
     }
     return STB_OK;
   }
-  if ((ctx->b_last[0] == 2u || ctx->b_last[0] == 3u || (ctx->b_last[0] == 5u && n_seg)) && nq) {
+  if ((route == kRouteV2 || route == kRouteFiltered || (route == kRouteThreshold && n_seg)) && nq) {
     if (thr) STB_CUDA(cudaMemcpy(thr, ctx->b_thr, (size_t)nq * sizeof(float), cudaMemcpyDeviceToHost));
     if (cand_cnt) STB_CUDA(cudaMemcpy(cand_cnt, ctx->b_cnt, (size_t)nq * n_seg * sizeof(uint32_t), cudaMemcpyDeviceToHost));
   }

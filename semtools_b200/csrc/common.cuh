@@ -205,10 +205,7 @@ struct stb_ctx {
   StbBuf<uint64_t> t_out_at;
   StbBuf<stb_hit> t_hits;
   StbBuf<uint8_t> t_sort_tmp;
-  // the last K2 call: route (1 = v1, 2 = v2, 3 = filtered v2, 4 = filtered, nothing on the tensor cores,
-  // 5 = threshold mode, 6 = one filter per query), nq, then n_sample, stride (routes 1-4) or retried queries, K1
-  // queries (route 5) or tensor groups, K1 queries (route 6), n_seg, seg_cap
-  uint32_t b_last[6];
+  uint32_t b_last[6];             // the last K2 call's route record (api.cu: k2_record)
   StbBuf<float> bq_dev;           // host-call staging: queries
   StbBuf<stb_hit> bh_dev;         // host-call staging: hits
   StbBuf<uint32_t> bs_dev;        // host-call staging: status
@@ -323,6 +320,19 @@ int stb_clip_ranges(const char *what, const uint64_t *ranges, uint32_t n, uint64
     if (b < e) emit(b - row_base, e - row_base);
   }
   return STB_OK;
+}
+
+// stb_clip_ranges appending each local piece to *loc as a [begin, end) u32 pair (a shard holds < 2^32 rows).
+inline int stb_clip_ranges_u32(const char *what, const uint64_t *ranges, uint32_t n, uint64_t row_base, uint64_t n_rows,
+                               std::vector<uint32_t> *loc) {
+  loc->reserve(loc->size() + 2 * (size_t)n);
+  return stb_clip_ranges(what, ranges, n, row_base, n_rows,
+                         [&](uint64_t b, uint64_t e) { loc->push_back((uint32_t)b); loc->push_back((uint32_t)e); });
+}
+
+// hits[n, k) = (+inf, UINT64_MAX): the unused tail of a top-k result, as the kernels pad it.
+inline void stb_pad_hits(stb_hit *hits, uint64_t n, uint64_t k) {
+  for (uint64_t j = n; j < k; ++j) { hits[j].distance = INFINITY; hits[j].row = UINT64_MAX; }
 }
 
 // stb_corpus_update / stb_corpus_remove without their refusal of live IVF-PQ indexes (api.cu).  With a

@@ -1849,14 +1849,12 @@ int stb_ivfpq_search_filtered(stb_ivfpq *x, const float *q, uint32_t nq, uint32_
   // global ranges -> local [begin, end) pairs clipped to the indexed rows [row_base, row_base + n)
   std::vector<uint32_t> loc;
   if (row_ranges) {
-    loc.reserve(2 * (size_t)n_ranges);
-    const int rc = stb_clip_ranges("ivfpq_search_filtered", row_ranges, n_ranges, x->corpus->row_base, x->n,
-                                   [&](uint64_t b, uint64_t e) { loc.push_back((uint32_t)b); loc.push_back((uint32_t)e); });
+    const int rc = stb_clip_ranges_u32("ivfpq_search_filtered", row_ranges, n_ranges, x->corpus->row_base, x->n, &loc);
     if (rc != STB_OK) return rc;
   }
   if (top_k == 0 || (row_ranges && loc.empty())) {             // nothing can be returned: no launch
     for (uint32_t i = 0; i < nq; ++i) { out_n[i] = 0; if (out_scanned) out_scanned[i] = 0; }
-    for (uint64_t i = 0; i < (uint64_t)nq * top_k; ++i) { out_hits[i].distance = INFINITY; out_hits[i].row = UINT64_MAX; }
+    stb_pad_hits(out_hits, 0, (uint64_t)nq * top_k);
     return STB_OK;
   }
   stb_ctx *ctx = x->ctx;
@@ -1935,7 +1933,7 @@ int stb_ivfpq_search(stb_ivfpq *x, const float *q, uint32_t nprobe, uint32_t top
     if ((rc = x->cand.reserve(m_pad)) != STB_OK) return rc;
     if (m_pad > m) {   // padding entries: +inf
       std::vector<stb_hit> pad(m_pad - m);
-      for (auto &h : pad) { h.distance = INFINITY; h.row = 0xffffffffffffffffull; }
+      stb_pad_hits(pad.data(), 0, pad.size());
       STB_CUDA(cudaMemcpyAsync(x->cand + m, pad.data(), pad.size() * sizeof(stb_hit), cudaMemcpyHostToDevice, st));
       STB_CUDA(cudaStreamSynchronize(st));
     }

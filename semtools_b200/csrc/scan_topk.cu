@@ -54,6 +54,30 @@ struct ScanArgs {
 };
 #define STB_TICKET_TILES 4   // co-scan, 10M rows, q8: 4 and 2 tiles 0.434 ms/query, 1 tile 0.635 ms
 
+// A pass's ScanArgs over ranges_dev as k1_upload_ranges (api.cu) packs them: vstart[n_ranges + 1], then
+// rbegin[n_ranges]; the only decoder of that layout.  No tickets: the top-k launch sets its own.
+static ScanArgs stb_scan_args(const stb_corpus *c, const float *q_dev, const uint64_t *ranges_dev, uint32_t n_ranges,
+                              uint64_t n_virtual) {
+  ScanArgs a;
+  a.rows = reinterpret_cast<const float4 *>(c->rows);
+  a.n_virtual = n_virtual;
+  a.q = q_dev;
+  a.vstart = ranges_dev;
+  a.rbegin = ranges_dev ? ranges_dev + (n_ranges + 1) : nullptr;
+  a.n_ranges = n_ranges;
+  a.tickets = nullptr; a.t_base = 0; a.t_bulk = 0;
+  return a;
+}
+
+// Grid of the static warp-strided schedule over n_virtual rows, 4 * u rows per tile: one tile per warp, at most
+// STB_SCAN_MINB CTAs per SM.
+static unsigned stb_scan_grid(const stb_ctx *ctx, uint64_t n_virtual, int u) {
+  const uint64_t tiles = (n_virtual + 4 * u - 1) / (4 * u);
+  const uint64_t want = (tiles + STB_SCAN_WARPS - 1) / STB_SCAN_WARPS;
+  const uint64_t grid = (uint64_t)ctx->sm_count * STB_SCAN_MINB;
+  return (unsigned)(want < grid ? (want < 1 ? 1 : want) : grid);
+}
+
 // ---- tile schedule + row map shared by the three scans -----------------------------------
 // RANGES == 0: whole shard, tiles are warp-strided (the grid streams one contiguous window).
 // RANGES == 1: row ranges (workspace path filter).  Blocks of WB consecutive tiles are
@@ -1343,13 +1367,7 @@ int stb_launch_scan_topk(stb_ctx *ctx, const stb_corpus *c, int tier, const floa
                          uint32_t *out_status_dev, const StbXchgArgs *xchg, bool overlapped) {
   if (overlapped && (xchg || n_ranges)) { stb_set_error("scan_topk: an overlapped launch takes no exchange or ranges"); return STB_ERR_ARG; }
   TopkArgs a;
-  a.scan.rows = reinterpret_cast<const float4 *>(c->rows);
-  a.scan.n_virtual = n_virtual;
-  a.scan.q = q_dev;
-  a.scan.vstart = ranges_dev;
-  a.scan.rbegin = ranges_dev ? ranges_dev + (n_ranges + 1) : nullptr;
-  a.scan.n_ranges = n_ranges;
-  a.scan.tickets = nullptr; a.scan.t_base = 0; a.scan.t_bulk = 0;
+  a.scan = stb_scan_args(c, q_dev, ranges_dev, n_ranges, n_virtual);
   memset(&a.co, 0, sizeof(a.co));
   a.row_base = c->row_base;
   a.keys = ctx->block_keys;
@@ -1428,32 +1446,22 @@ int stb_launch_scan_collect(stb_ctx *ctx, const stb_corpus *c, int tier,
                             const uint64_t *ranges_dev, uint32_t n_ranges,
                             uint64_t n_virtual) {
   CollectArgs a;
-  a.scan.rows = reinterpret_cast<const float4 *>(c->rows);
+  a.scan = stb_scan_args(c, q_dev, ranges_dev, n_ranges, n_virtual);
   a.q8 = c->q8; a.q8_scale = c->q8_scale;
-  a.scan.n_virtual = n_virtual;
-  a.scan.q = q_dev;
-  a.scan.vstart = ranges_dev;
-  a.scan.rbegin = ranges_dev ? ranges_dev + (n_ranges + 1) : nullptr;
-  a.scan.n_ranges = n_ranges;
-  a.scan.tickets = nullptr; a.scan.t_base = 0; a.scan.t_bulk = 0;
   a.cos_floor = cos_floor;
   a.out = ctx->collect_rows;
   a.count = ctx->collect_count;
   a.cap = ctx->collect_rows.cap;
   STB_CUDA(cudaMemsetAsync(ctx->collect_count, 0, sizeof(unsigned long long), ctx->stream));
-  const int u = tier == STB_TIER_Q8 ? STB_Q8_SCAN_U : STB_SCAN_U;
-  uint64_t tiles = (n_virtual + 4 * u - 1) / (4 * u);
-  uint64_t want = (tiles + STB_SCAN_WARPS - 1) / STB_SCAN_WARPS;
-  uint64_t grid = (uint64_t)ctx->sm_count * STB_SCAN_MINB;
-  if (want < grid) grid = want < 1 ? 1 : want;
+  const unsigned grid = stb_scan_grid(ctx, n_virtual, tier == STB_TIER_Q8 ? STB_Q8_SCAN_U : STB_SCAN_U);
   if (tier == STB_TIER_Q8) {
     if (!c->q8) { stb_set_error("scan_collect: q8 tier unavailable"); return STB_ERR_STATE; }
-    if (n_ranges > 0) stb_scan_collect_kernel<STB_Q8_SCAN_U, true, 2><<<(unsigned)grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a);
-    else stb_scan_collect_kernel<STB_Q8_SCAN_U, false, 2><<<(unsigned)grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a);
+    if (n_ranges > 0) stb_scan_collect_kernel<STB_Q8_SCAN_U, true, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a);
+    else stb_scan_collect_kernel<STB_Q8_SCAN_U, false, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a);
   } else if (n_ranges > 0)
-    stb_scan_collect_kernel<STB_SCAN_U, true><<<(unsigned)grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a);
+    stb_scan_collect_kernel<STB_SCAN_U, true><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a);
   else
-    stb_scan_collect_kernel<STB_SCAN_U, false><<<(unsigned)grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a);
+    stb_scan_collect_kernel<STB_SCAN_U, false><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a);
   STB_CUDA(cudaGetLastError());
   ctx->kernel_launches++;
   return STB_OK;
@@ -1495,28 +1503,17 @@ stb_scan_hist_kernel(const ScanArgs scan, unsigned int *global_hist, const uint8
 
 int stb_launch_scan_hist(stb_ctx *ctx, const stb_corpus *c, int tier, const float *q_dev, const uint64_t *ranges_dev,
                          uint32_t n_ranges, uint64_t n_virtual, unsigned int *hist_dev) {
-  ScanArgs a;
-  a.rows = reinterpret_cast<const float4 *>(c->rows);
-  a.n_virtual = n_virtual;
-  a.q = q_dev;
-  a.vstart = ranges_dev;
-  a.rbegin = ranges_dev ? ranges_dev + (n_ranges + 1) : nullptr;
-  a.n_ranges = n_ranges;
-  a.tickets = nullptr; a.t_base = 0; a.t_bulk = 0;
+  const ScanArgs a = stb_scan_args(c, q_dev, ranges_dev, n_ranges, n_virtual);
   STB_CUDA(cudaMemsetAsync(hist_dev, 0, STB_HIST_BINS * sizeof(unsigned int), ctx->stream));
-  const int u = tier == STB_TIER_Q8 ? STB_Q8_SCAN_U : STB_SCAN_U;
-  uint64_t tiles = (n_virtual + 4 * u - 1) / (4 * u);
-  uint64_t want = (tiles + STB_SCAN_WARPS - 1) / STB_SCAN_WARPS;
-  uint64_t grid = (uint64_t)ctx->sm_count * STB_SCAN_MINB;
-  if (want < grid) grid = want < 1 ? 1 : want;
+  const unsigned grid = stb_scan_grid(ctx, n_virtual, tier == STB_TIER_Q8 ? STB_Q8_SCAN_U : STB_SCAN_U);
   if (tier == STB_TIER_Q8) {
     if (!c->q8) { stb_set_error("scan_hist: q8 tier unavailable"); return STB_ERR_STATE; }
-    if (n_ranges > 0) stb_scan_hist_kernel<STB_Q8_SCAN_U, true, 2><<<(unsigned)grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, hist_dev, c->q8, c->q8_scale);
-    else stb_scan_hist_kernel<STB_Q8_SCAN_U, false, 2><<<(unsigned)grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, hist_dev, c->q8, c->q8_scale);
+    if (n_ranges > 0) stb_scan_hist_kernel<STB_Q8_SCAN_U, true, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, hist_dev, c->q8, c->q8_scale);
+    else stb_scan_hist_kernel<STB_Q8_SCAN_U, false, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, hist_dev, c->q8, c->q8_scale);
   } else if (n_ranges > 0)
-    stb_scan_hist_kernel<STB_SCAN_U, true><<<(unsigned)grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, hist_dev, nullptr, nullptr);
+    stb_scan_hist_kernel<STB_SCAN_U, true><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, hist_dev, nullptr, nullptr);
   else
-    stb_scan_hist_kernel<STB_SCAN_U, false><<<(unsigned)grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, hist_dev, nullptr, nullptr);
+    stb_scan_hist_kernel<STB_SCAN_U, false><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, hist_dev, nullptr, nullptr);
   STB_CUDA(cudaGetLastError());
   ctx->kernel_launches++;
   return STB_OK;
@@ -1545,41 +1542,21 @@ stb_debug_scan_kernel(const ScanArgs scan, const uint8_t *shadow, const uint8_t 
   else stb_scan_rows<U, RANGES>(scan, sink);
 }
 
-static ScanArgs stb_debug_scan_args(const stb_corpus *c, const float *q_dev, const uint64_t *ranges_dev, uint32_t n_ranges,
-                                    uint64_t n_virtual) {
-  ScanArgs a;
-  a.rows = reinterpret_cast<const float4 *>(c->rows);
-  a.n_virtual = n_virtual;
-  a.q = q_dev;
-  a.vstart = ranges_dev;
-  a.rbegin = ranges_dev ? ranges_dev + (n_ranges + 1) : nullptr;
-  a.n_ranges = n_ranges;
-  a.tickets = nullptr; a.t_base = 0; a.t_bulk = 0;
-  return a;
-}
-
-static unsigned stb_debug_grid(const stb_ctx *ctx, uint64_t n_virtual, int u) {
-  const uint64_t tiles = (n_virtual + 4 * u - 1) / (4 * u);
-  const uint64_t want = (tiles + STB_SCAN_WARPS - 1) / STB_SCAN_WARPS;
-  const uint64_t grid = (uint64_t)ctx->sm_count * STB_SCAN_MINB;
-  return (unsigned)(want < grid ? (want < 1 ? 1 : want) : grid);
-}
-
 int stb_launch_debug_scan(stb_ctx *ctx, const stb_corpus *c, int tier, const float *q_dev, const uint64_t *ranges_dev,
                           uint32_t n_ranges, uint64_t n_virtual, float *score, unsigned int *seen) {
-  const ScanArgs a = stb_debug_scan_args(c, q_dev, ranges_dev, n_ranges, n_virtual);
+  const ScanArgs a = stb_scan_args(c, q_dev, ranges_dev, n_ranges, n_virtual);
   const DumpSink sink{score, seen};
   const bool r = n_ranges > 0;
   if (tier == STB_TIER_Q8) {
-    const unsigned grid = stb_debug_grid(ctx, n_virtual, STB_Q8_SCAN_U);
+    const unsigned grid = stb_scan_grid(ctx, n_virtual, STB_Q8_SCAN_U);
     if (r) stb_debug_scan_kernel<STB_Q8_SCAN_U, true, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, nullptr, c->q8, c->q8_scale, sink);
     else stb_debug_scan_kernel<STB_Q8_SCAN_U, false, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, nullptr, c->q8, c->q8_scale, sink);
   } else if (tier == STB_TIER_H16) {
-    const unsigned grid = stb_debug_grid(ctx, n_virtual, STB_SHADOW_SCAN_U);
+    const unsigned grid = stb_scan_grid(ctx, n_virtual, STB_SHADOW_SCAN_U);
     if (r) stb_debug_scan_kernel<STB_SHADOW_SCAN_U, true, 1><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, c->shadow, nullptr, nullptr, sink);
     else stb_debug_scan_kernel<STB_SHADOW_SCAN_U, false, 1><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, c->shadow, nullptr, nullptr, sink);
   } else {
-    const unsigned grid = stb_debug_grid(ctx, n_virtual, STB_SCAN_U);
+    const unsigned grid = stb_scan_grid(ctx, n_virtual, STB_SCAN_U);
     if (r) stb_debug_scan_kernel<STB_SCAN_U, true, 0><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, nullptr, nullptr, nullptr, sink);
     else stb_debug_scan_kernel<STB_SCAN_U, false, 0><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, nullptr, nullptr, nullptr, sink);
   }
@@ -1602,7 +1579,7 @@ stb_debug_q4_kernel(const ScanArgs scan, const uint8_t *q8, const float *q8_scal
 int stb_launch_debug_q4(stb_ctx *ctx, const stb_corpus *c, const float *q_dev, uint32_t top_k, const uint64_t *ranges_dev,
                         uint32_t n_ranges, uint64_t n_virtual, unsigned long long *words, unsigned long long *refined,
                         int pin, float *u4, float *t, float *l8, float *u8, unsigned int *seen) {
-  const ScanArgs a = stb_debug_scan_args(c, q_dev, ranges_dev, n_ranges, n_virtual);
+  const ScanArgs a = stb_scan_args(c, q_dev, ranges_dev, n_ranges, n_virtual);
   StbQ4Args q4a;
   q4a.plane = c->q4;
   q4a.sr = c->q4_sr;
@@ -1612,7 +1589,7 @@ int stb_launch_debug_q4(stb_ctx *ctx, const stb_corpus *c, const float *q_dev, u
   q4a.refined = refined;
   const DumpSink sink{u8, seen};
   const StbQ4Dump dump{u4, t, l8, pin};
-  const unsigned grid = stb_debug_grid(ctx, n_virtual, STB_Q4_SCAN_U);
+  const unsigned grid = stb_scan_grid(ctx, n_virtual, STB_Q4_SCAN_U);
   if (n_ranges > 0) stb_debug_q4_kernel<true><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, c->q8, c->q8_scale, q4a, sink, dump);
   else stb_debug_q4_kernel<false><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, c->q8, c->q8_scale, q4a, sink, dump);
   STB_CUDA(cudaGetLastError());
