@@ -362,6 +362,9 @@ int stb_search_batch_subsets(stb_ctx *ctx, const stb_corpus *corpus, const float
  * then the exact canonical re-score.  stb_search answers the rest: queries that cannot be normalised, the zero
  * query, queries beyond the budget, and every query when the corpus holds rows that cannot be normalised. */
 #define STB_BATCH_THRESHOLD_RETRY_KEYS (1ull << 24)
+/* Eligibility scratch of one stb_ivfpq_search_subsets launch (256 MiB): each distinct subset of a launch takes
+ * ceil(rows / 32) + nlist words, and a launch holds as many subsets as fit (at least one). */
+#define STB_IVFPQ_SUBSET_SCRATCH (1ull << 28)
 int stb_search_batch_threshold(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t nq,
                                double max_distance, stb_hit *out_hits, uint64_t cap, uint64_t *out_offsets);
 
@@ -559,6 +562,36 @@ int stb_ivfpq_search_filtered(stb_ivfpq *index, const float *q, uint32_t nq, uin
                               uint32_t rerank, int has_max, double max_distance,
                               const uint64_t *row_ranges, uint32_t n_ranges,
                               stb_hit *out_hits, uint32_t *out_n, uint64_t *out_scanned);
+/* Filtered batched search over many subsets in one call: a batch of store queries (a server's or an agent
+ * host's) that name different folders, each distinct subset passed once.
+ *  - Subsets: subset_offsets has n_subsets + 1 entries, subset_offsets[0] = 0, never decreasing; subset s is
+ *    row_ranges[2*subset_offsets[s] .. 2*subset_offsets[s+1]), GLOBAL [begin, end) pairs as stb_search takes
+ *    them, clipped to the indexed rows as stb_ivfpq_search_filtered clips them.  A subset with no ranges, or
+ *    none left after clipping, is the empty subset.
+ *  - Queries: q is nq x 256 f32 (host); query i searches subset subset_of[i] (< n_subsets).
+ *  - Contract: for every query i, out_hits[i*top_k ..], out_n[i] and out_scanned[i] equal, bit for bit, what
+ *      stb_ivfpq_search_filtered(index, q_i, 1, nprobe, top_k, rerank, has_max, max_distance,
+ *                                <ranges of subset subset_of[i]>, <their count>, ...)
+ *    returns (a batched query's answer depends neither on the other queries nor on the launches).
+ *  - Argument rules are stb_ivfpq_search_filtered's: nq == 0 is a no-op; top_k == 0 sets every count to 0;
+ *    top_k > 1024 is STB_ERR_ARG; nprobe is clamped to [1, min(nlist, 1024)], rerank to [top_k, 1024];
+ *    out_scanned may be NULL.  A query of an empty subset gets 0 hits and 0 scanned and takes no part in
+ *    any launch.
+ *  - Refusals, all before anything is written or launched: STB_ERR_ARG for a NULL pointer that is needed
+ *    (row_ranges may be NULL when subset_offsets[n_subsets] == 0), subset_offsets[0] != 0, decreasing
+ *    offsets, a subset of more than 2^32 - 1 ranges, or subset_of[i] >= n_subsets; STB_ERR_RANGE when any
+ *    subset holds ranges stb_search refuses -- every subset is validated, also those no query names.
+ *  - Launches: the queries in caller order, at most 4096 per launch and no more distinct subsets than
+ *    STB_IVFPQ_SUBSET_SCRATCH holds (each takes an eligible-row bitmap of ceil(rows / 32) words and nlist
+ *    counts; a launch holds at least one query).  Each launch: one bitmap launch and one count launch for
+ *    all its subsets, the four batched kernels, one synchronisation.  The scratch belongs to the index and
+ *    grows on demand.
+ * stb_debug_ivfpq_batch_last describes the call's last launch: slot j is the j-th query of that launch
+ * (in caller order, queries of empty subsets skipped). */
+int stb_ivfpq_search_subsets(stb_ivfpq *index, const float *q, uint32_t nq, uint32_t nprobe, uint32_t top_k,
+                             uint32_t rerank, int has_max, double max_distance,
+                             uint32_t n_subsets, const uint64_t *subset_offsets, const uint64_t *row_ranges,
+                             const uint32_t *subset_of, stb_hit *out_hits, uint32_t *out_n, uint64_t *out_scanned);
 
 /* Host-buffer form of the fused multi-GPU search (the call a sharded host makes per query):
  * pinned H2D of the query, ONE kernel (scan + NVLink exchange + merge), D2H of the merged

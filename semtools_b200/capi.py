@@ -33,7 +33,7 @@ SYMBOLS = [
     "stb_debug_batch_last", "stb_debug_corpus_copy", "stb_debug_scan_scores", "stb_debug_q4_scan",
     "stb_debug_ivfpq_export",
     "stb_ivfpq_search_batch", "stb_ivfpq_search_batch_dev", "stb_debug_ivfpq_batch_last",
-    "stb_ivfpq_search_filtered", "stb_ivfpq_update", "stb_ivfpq_remove",
+    "stb_ivfpq_search_filtered", "stb_ivfpq_search_subsets", "stb_ivfpq_update", "stb_ivfpq_remove",
 ]
 
 
@@ -140,6 +140,7 @@ def lib() -> C.CDLL:
     L.stb_ivfpq_search_batch_dev.argtypes = [vp, vp, u32, u32, u32, u32, vp, vp]
     L.stb_debug_ivfpq_batch_last.argtypes = [vp, u32, vp, vp, vp, vp]
     L.stb_ivfpq_search_filtered.argtypes = [vp, vp, u32, u32, u32, u32, i32, f64, vp, u32, vp, vp, vp]
+    L.stb_ivfpq_search_subsets.argtypes = [vp, vp, u32, u32, u32, u32, i32, f64, u32, vp, vp, vp, vp, vp, vp]
     for name in SYMBOLS:
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("stb_version", "stb_device_count"):
@@ -672,6 +673,30 @@ class IvfPq:
                                                int(max_distance is not None), float(max_distance or 0.0),
                                                _np_ptr(rr), n_rr, _np_ptr(out) if out.size else None, _np_ptr(n),
                                                _np_ptr(scanned)))
+        return out, n, scanned
+
+    def search_subsets(self, queries, subsets, subset_of, max_distance: float | None = None, nprobe: int = 64,
+                       top_k: int = 10, rerank: int = 256):
+        """stb_ivfpq_search_subsets: search_filtered for a batch whose queries name different subsets.  subsets
+        is a list of (n, 2) global [begin, end) range arrays, each distinct subset given once (an empty array is
+        the empty subset); query i searches subsets[subset_of[i]].  Returns what search_filtered returns: (hits
+        [nq, top_k] padded with (+inf, UINT64_MAX), n [nq] hit counts, scanned [nq] eligible codes scanned)."""
+        queries = np.ascontiguousarray(queries, dtype=np.float32).reshape(-1, STB_DIM)
+        nq = queries.shape[0]
+        subset_of = np.ascontiguousarray(subset_of, dtype=np.uint32).reshape(-1)
+        if len(subset_of) != nq:
+            raise ValueError(f"subset_of has {len(subset_of)} entries for {nq} queries")
+        parts = [np.asarray(r, dtype=np.uint64).reshape(-1, 2) for r in subsets]
+        offsets = np.zeros(len(parts) + 1, dtype=np.uint64)
+        offsets[1:] = np.cumsum([len(r) for r in parts], dtype=np.uint64)
+        rr = np.ascontiguousarray(np.concatenate(parts) if parts else np.zeros((0, 2), np.uint64), dtype=np.uint64)
+        out = np.zeros((nq, top_k), dtype=HIT_DTYPE)
+        n = np.zeros(nq, dtype=np.uint32)
+        scanned = np.zeros(nq, dtype=np.uint64)
+        _check(lib().stb_ivfpq_search_subsets(self._h, _np_ptr(queries), nq, nprobe, top_k, rerank,
+                                              int(max_distance is not None), float(max_distance or 0.0), len(parts),
+                                              _np_ptr(offsets), _np_ptr(rr) if rr.size else None, _np_ptr(subset_of),
+                                              _np_ptr(out) if out.size else None, _np_ptr(n), _np_ptr(scanned)))
         return out, n, scanned
 
     def search_batch_dev(self, q_dev: int, nq: int, nprobe: int, top_k: int, rerank: int, out_hits_dev: int,

@@ -547,9 +547,11 @@ int stb_launch_batch_finish(stb_ctx *ctx, const uint64_t *cand, uint32_t n_slice
 
 // ---- ivfpq.cu: the eligibility bitmap of a path filter ----------------------------
 // bitmap[w] bit j = local row 32w + j lies in one of the n_ranges local [begin, end) u32 pairs of ranges_dev
-// (ascending, disjoint), for w < n_words
+// (ascending, disjoint), for w < n_words.  With set_off_dev (2 n_sets entries on the device), one launch
+// writes n_sets bitmaps: bitmap s at bitmap + s * n_words from the pairs [set_off_dev[2s], set_off_dev[2s+1])
+// of ranges_dev, and n_ranges is unused.
 int stb_launch_row_bitmap(stb_ctx *ctx, const uint32_t *ranges_dev, uint32_t n_ranges, uint64_t n_words,
-                          uint32_t *bitmap);
+                          uint32_t *bitmap, uint32_t n_sets = 1, const uint64_t *set_off_dev = nullptr);
 
 // ---- device helpers ---------------------------------------------------------------
 // The distance limit of a search without max_distance: max_distance.unwrap_or(100.0), strict.

@@ -90,6 +90,9 @@ struct stb_ivfpq {
   StbBuf<uint32_t> f_bitmap;         // eligible local rows; cap >= ceil(n / 32) words
   StbBuf<uint32_t> f_elig;           // [nlist] eligible codes per list
   StbBuf<uint32_t> f_ranges;         // clipped local ranges, [begin, end) pairs
+  // subsets search (f_bitmap and f_elig then hold one bitmap and one count array per subset of a launch)
+  StbBuf<uint64_t> f_set_off;        // [2 per subset of a launch]: its pairs [begin, end) in f_ranges
+  StbBuf<uint32_t> f_slot_set;       // [query slot]: its subset within the launch
 };
 
 // ------------------------------------------------------------------ assignment GEMM ---
@@ -846,11 +849,12 @@ ivfb_coarse_kernel(const float *C, uint32_t nlist, const float *qs, uint32_t nq,
 
 // FILTER: only lists with elig[l] > 0 are taken, in the same (coarse score desc, list id asc) order; the
 // slots past the min(nprobe, E) lists taken hold IVF_NO_LIST and the total as their prefix, so a search
-// of the prefix never lands on them.
+// of the prefix never lands on them.  Query slot q reads the counts of subset slot_set[q], elig +
+// slot_set[q] * nlist (slot_set NULL: subset 0).
 template <bool FILTER>
 __global__ void __launch_bounds__(1024)
 ivfb_probe_lut_kernel(const float *coarse, uint32_t nlist, uint32_t nprobe, const uint32_t *list_off, const float *cb,
-                      const float *qs, uint32_t *probe, float *lut, const uint32_t *elig) {
+                      const float *qs, uint32_t *probe, float *lut, const uint32_t *elig, const uint32_t *slot_set) {
   extern __shared__ uint64_t pb_keys[];   // npow2 keys
   __shared__ float sq[STB_D];
   __shared__ float s_inv;
@@ -875,6 +879,7 @@ ivfb_probe_lut_kernel(const float *coarse, uint32_t nlist, uint32_t nprobe, cons
     // are taken; s_el[p] = eligible codes of probe slot p
     __shared__ uint32_t s_el[1024], s_wcnt[32], s_taken;
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (slot_set) elig += (size_t)__ldg(slot_set + q) * nlist;
     if (threadIdx.x == 0) s_taken = 0;
     __syncthreads();
     for (uint32_t base = 0; base < nlist; base += blockDim.x) {
@@ -982,7 +987,15 @@ struct IvfbArgs {
   // filtered search only (the FILTER instantiations read them)
   const uint32_t *bitmap;                    // eligible local rows, 1 bit each; NULL: every row
   double max_dist;                           // a hit needs distance < max_dist
+  // query slot q reads the bitmap of subset slot_set[q], bitmap + slot_set[q] * bm_words (NULL: subset 0)
+  const uint32_t *slot_set;
+  uint64_t bm_words;
 };
+
+// the eligibility bitmap of query slot q in a FILTER instantiation
+__device__ __forceinline__ const uint32_t *ivfb_slot_bitmap(const IvfbArgs &a, uint32_t q) {
+  return a.bitmap && a.slot_set ? a.bitmap + (size_t)__ldg(a.slot_set + q) * a.bm_words : a.bitmap;
+}
 
 template <bool FILTER>
 __global__ void __launch_bounds__(IVFB_SCAN_THREADS)
@@ -992,6 +1005,7 @@ ivfb_scan_kernel(const IvfbArgs a) {
   __shared__ float s_pc[1024];
   const uint32_t q = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint32_t *pr = a.probe + (size_t)q * IVFB_PROBE_STRIDE(a.nprobe, FILTER);
+  const uint32_t *bitmap = FILTER ? ivfb_slot_bitmap(a, q) : a.bitmap;
   const float *lq = a.lut + (size_t)q * PQ_M * PQ_KSUB;
   for (uint32_t i = tid; i < PQ_M * PQ_KSUB; i += IVFB_SCAN_THREADS) s_lut[i] = lq[i];
   for (uint32_t p = tid; p < a.nprobe; p += IVFB_SCAN_THREADS) {
@@ -1005,7 +1019,7 @@ ivfb_scan_kernel(const IvfbArgs a) {
   top.init(a.keep);
   // chunk g (32 consecutive codes) -> CTA g % IVFB_SCAN_CTAS, warp (g / IVFB_SCAN_CTAS) % 8
   for (uint64_t g = blockIdx.x + (uint64_t)IVFB_SCAN_CTAS * warp; g * 32 < total; g += IVFB_WARPS)
-    top.push(ivfb_code_key<FILTER>(g * 32 + lane, total, a.nprobe, s_pref, s_start, s_pc, s_lut, a.codes, a.order, a.bitmap));
+    top.push(ivfb_code_key<FILTER>(g * 32 + lane, total, a.nprobe, s_pref, s_start, s_pc, s_lut, a.codes, a.order, bitmap));
   uint64_t d = top.drop;
 #pragma unroll
   for (int off = 16; off > 0; off >>= 1) d = min(d, __shfl_xor_sync(0xffffffffu, d, off));
@@ -1031,6 +1045,7 @@ ivfb_finish_kernel(const IvfbArgs a) {
   __shared__ unsigned long long s_prefix;
   const uint32_t q = blockIdx.x, tid = threadIdx.x;
   const uint32_t *pr = a.probe + (size_t)q * IVFB_PROBE_STRIDE(a.nprobe, FILTER);
+  const uint32_t *bitmap = FILTER ? ivfb_slot_bitmap(a, q) : a.bitmap;
   const uint32_t total = pr[2 * a.nprobe];
   const uint32_t r = a.rerank;
   for (uint32_t i = tid; i < IVFB_KEPT; i += IVFB_FIN_THREADS) keys[i] = a.kept[(size_t)q * IVFB_KEPT + i];
@@ -1068,7 +1083,7 @@ ivfb_finish_kernel(const IvfbArgs a) {
       __syncthreads();
       const uint64_t prefix = s_prefix;
       for (uint64_t v = tid; v < total; v += IVFB_FIN_THREADS) {
-        const uint64_t key = ivfb_code_key<FILTER>(v, total, a.nprobe, s_pref, s_start, s_pc, s_lut, a.codes, a.order, a.bitmap);
+        const uint64_t key = ivfb_code_key<FILTER>(v, total, a.nprobe, s_pref, s_start, s_pc, s_lut, a.codes, a.order, bitmap);
         if (key != STB_KEY_INVALID && (key & hi_mask) == prefix) atomicAdd(&s_hist[(key >> shift) & 255], 1u);
       }
       __syncthreads();
@@ -1098,7 +1113,7 @@ ivfb_finish_kernel(const IvfbArgs a) {
     uint64_t *cand = reinterpret_cast<uint64_t *>(dyn + 16384);     // [16 KiB, 24 KiB): r <= 1024 keys
     if (!none)
       for (uint64_t v = tid; v < total; v += IVFB_FIN_THREADS) {
-        const uint64_t key = ivfb_code_key<FILTER>(v, total, a.nprobe, s_pref, s_start, s_pc, s_lut, a.codes, a.order, a.bitmap);
+        const uint64_t key = ivfb_code_key<FILTER>(v, total, a.nprobe, s_pref, s_start, s_pc, s_lut, a.codes, a.order, bitmap);
         if (key <= thr) cand[atomicAdd(&s_nc, 1u)] = key;           // exactly min(r, valid) keys
       }
     __syncthreads();
@@ -1119,7 +1134,7 @@ ivfb_finish_kernel(const IvfbArgs a) {
       if (key != STB_KEY_INVALID) row = a.order[stb_key_row(key)];
     } else if (c < nc + a.n_forced) {
       row = a.forced[c - nc];
-      if (FILTER && a.bitmap && !((__ldg(a.bitmap + (row >> 5)) >> (row & 31)) & 1u)) row = 0xffffffffffffffffull;
+      if (FILTER && bitmap && !((__ldg(bitmap + (row >> 5)) >> (row & 31)) & 1u)) row = 0xffffffffffffffffull;
     }
     rows_c[c] = row;
   }
@@ -1146,18 +1161,27 @@ ivfb_finish_kernel(const IvfbArgs a) {
 }
 
 // ------------------------------------------------------------------ filtered search ------
-// The eligibility pass of stb_ivfpq_search_filtered, once per call (every query of the call shares it):
-//   ivff_bitmap_kernel  bit r of the bitmap = local row r lies in one of the clipped ranges (thread per
-//                       32-row word: a binary search for the first range ending past the word, then the
-//                       at most 32 non-empty ranges that touch it); stb_launch_row_bitmap, which
-//                       stb_search_batch_filtered uses too
-//   ivff_elig_kernel    elig[l] = eligible codes of list l (warp per list, order[] read once: 4 B per
-//                       listed row); without a bitmap elig[l] is the list's length
+// The eligibility pass of stb_ivfpq_search_filtered (one subset, shared by every query of the call) and of
+// stb_ivfpq_search_subsets (every distinct subset of a launch), two launches whatever the subset count;
+// grid row y = subset y, whose bitmap is bitmap + y * n_words and whose counts are elig + y * nlist:
+//   ivff_bitmap_kernel  bit r of the bitmap = local row r lies in one of the subset's clipped ranges (thread
+//                       per 32-row word: a binary search for the first range ending past the word, then the
+//                       at most 32 non-empty ranges that touch it); subset y's ranges are the pairs
+//                       [set_off[2y], set_off[2y+1]) (set_off NULL: one subset of n_ranges pairs);
+//                       stb_launch_row_bitmap, which stb_search_batch_filtered uses too
+//   ivff_elig_kernel    elig[l] = eligible codes of list l (warp per list and subset, order[] read once per
+//                       subset: 4 B per listed row); without a bitmap elig[l] is the list's length
 // The batched kernels' FILTER instantiations then probe only lists with elig > 0 and drop every code
 // and forced row whose bit is clear.
-__global__ void ivff_bitmap_kernel(const uint32_t *ranges, uint32_t n_ranges, uint32_t n_words, uint32_t *bitmap) {
+__global__ void ivff_bitmap_kernel(const uint32_t *ranges, uint32_t n_ranges, uint32_t n_words, uint32_t *bitmap,
+                                   const uint64_t *set_off) {
   const uint32_t w = blockIdx.x * blockDim.x + threadIdx.x;   // ranges: [begin, end) local pairs, ascending
   if (w >= n_words) return;
+  if (set_off) {
+    ranges += 2 * set_off[2 * blockIdx.y];
+    n_ranges = (uint32_t)(set_off[2 * blockIdx.y + 1] - set_off[2 * blockIdx.y]);
+    bitmap += (size_t)blockIdx.y * n_words;
+  }
   const uint64_t w0 = (uint64_t)w * 32, w1 = w0 + 32;
   uint32_t lo = 0, hi = n_ranges;                              // first range with end > w0
   while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (ranges[2 * mid + 1] <= w0) lo = mid + 1; else hi = mid; }
@@ -1170,20 +1194,24 @@ __global__ void ivff_bitmap_kernel(const uint32_t *ranges, uint32_t n_ranges, ui
   bitmap[w] = bits;
 }
 
-int stb_launch_row_bitmap(stb_ctx *ctx, const uint32_t *ranges_dev, uint32_t n_ranges, uint64_t n_words, uint32_t *bitmap) {
-  if (n_words == 0) return STB_OK;
-  ivff_bitmap_kernel<<<(unsigned)((n_words + 255) / 256), 256, 0, ctx->stream>>>(ranges_dev, n_ranges, (uint32_t)n_words, bitmap);
+int stb_launch_row_bitmap(stb_ctx *ctx, const uint32_t *ranges_dev, uint32_t n_ranges, uint64_t n_words, uint32_t *bitmap,
+                          uint32_t n_sets, const uint64_t *set_off_dev) {
+  if (n_words == 0 || n_sets == 0) return STB_OK;
+  ivff_bitmap_kernel<<<dim3((unsigned)((n_words + 255) / 256), n_sets), 256, 0, ctx->stream>>>(ranges_dev, n_ranges,
+                                                                                             (uint32_t)n_words, bitmap, set_off_dev);
   STB_CUDA(cudaGetLastError());
   ctx->kernel_launches += 1;
   return STB_OK;
 }
 
 __global__ void ivff_elig_kernel(const uint32_t *list_off, const uint32_t *order, uint32_t nlist, const uint32_t *bitmap,
-                                 uint32_t *elig) {
+                                 uint64_t bm_words, uint32_t *elig) {
   const uint32_t lane = threadIdx.x & 31, l = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (l >= nlist) return;
+  elig += (size_t)blockIdx.y * nlist;
   const uint32_t b = __ldg(list_off + l), e = __ldg(list_off + l + 1);
   if (!bitmap) { if (lane == 0) elig[l] = e - b; return; }
+  bitmap += (size_t)blockIdx.y * bm_words;
   uint32_t cnt = 0;
   for (uint32_t i = b + lane; i < e; i += 32) {
     const uint32_t row = __ldg(order + i);
@@ -1325,8 +1353,9 @@ static int ivf_edit_plan(stb_ivfpq *x, IvfEdit &e, const char *who) {
       STB_CUDA(cudaMemcpyAsync(e.kept_d, e.kept.data(), (size_t)e.n_kept * 8, cudaMemcpyHostToDevice, st));
       STB_CUDA(cudaMemcpyAsync(e.kept_d + 2 * e.n_kept, e.kept_dst.data(), (size_t)e.n_kept * 4, cudaMemcpyHostToDevice, st));
     }
-    if (words) ivff_bitmap_kernel<<<(unsigned)((words + 255) / 256), 256, 0, st>>>(e.kept_d, e.n_kept, (uint32_t)words, e.bitmap);
-    ivff_elig_kernel<<<(nlist + 7) / 8, 256, 0, st>>>(x->list_off, x->order, nlist, e.bitmap, e.elig);
+    if (words) ivff_bitmap_kernel<<<(unsigned)((words + 255) / 256), 256, 0, st>>>(e.kept_d, e.n_kept, (uint32_t)words, e.bitmap,
+                                                                                   nullptr);
+    ivff_elig_kernel<<<(nlist + 7) / 8, 256, 0, st>>>(x->list_off, x->order, nlist, e.bitmap, 0, e.elig);
     STB_CUDA(cudaMemcpyAsync(surv.data(), e.elig, (size_t)nlist * 4, cudaMemcpyDeviceToHost, st));
     ctx->kernel_launches += 2;
   } else {
@@ -1726,8 +1755,10 @@ static int ivfb_reserve(stb_ivfpq *x, uint32_t nq) {
 // The filter of a filtered launch: the eligibility pass's outputs and the distance limit.
 struct IvfbFilter {
   const uint32_t *bitmap;     // NULL: every indexed row is eligible
-  const uint32_t *elig;       // [nlist]
+  const uint32_t *elig;       // [nlist] per subset
   double max_dist;
+  const uint32_t *slot_set;   // [nq] subset of each query slot (device); NULL: one subset
+  uint64_t bm_words;          // bitmap words per subset
 };
 
 // four launches for 1 <= nq <= IVFB_MAX_NQ queries (arguments already clamped); asynchronous.
@@ -1756,19 +1787,20 @@ static int ivfb_launch(stb_ivfpq *x, const float *q_dev, uint32_t nq, uint32_t n
   a.rows = reinterpret_cast<const float4 *>(x->corpus->rows); a.row_base = x->corpus->row_base;
   a.forced = x->forced; a.n_forced = x->n_forced; a.out_hits = out_hits_dev; a.out_status = out_status_dev;
   a.bitmap = f ? f->bitmap : nullptr; a.max_dist = f ? f->max_dist : STB_DEFAULT_MAX_DIST;
+  a.slot_set = f ? f->slot_set : nullptr; a.bm_words = f ? f->bm_words : 0;
   ivfb_coarse_kernel<<<dim3((x->nlist + 31) / 32, (nq + IVFB_QTILE - 1) / IVFB_QTILE), 1024, 0, st>>>(x->centroids, x->nlist, q_dev,
                                                                                                    nq, x->b_coarse);
   STB_CUDA(cudaGetLastError());
   if (!f) {
     ivfb_probe_lut_kernel<false><<<nq, 1024, npow2 * 8, st>>>(x->b_coarse, x->nlist, nprobe, x->list_off, x->codebooks, q_dev,
-                                                              x->b_probe, x->b_lut, nullptr);
+                                                              x->b_probe, x->b_lut, nullptr, nullptr);
     STB_CUDA(cudaGetLastError());
     ivfb_scan_kernel<false><<<dim3(IVFB_SCAN_CTAS, nq), IVFB_SCAN_THREADS, 0, st>>>(a);
     STB_CUDA(cudaGetLastError());
     ivfb_finish_kernel<false><<<nq, IVFB_FIN_THREADS, IVFB_FIN_SMEM, st>>>(a);
   } else {
     ivfb_probe_lut_kernel<true><<<nq, 1024, npow2 * 8, st>>>(x->b_coarse, x->nlist, nprobe, x->list_off, x->codebooks, q_dev,
-                                                             x->b_probe, x->b_lut, f->elig);
+                                                             x->b_probe, x->b_lut, f->elig, f->slot_set);
     STB_CUDA(cudaGetLastError());
     ivfb_scan_kernel<true><<<dim3(IVFB_SCAN_CTAS, nq), IVFB_SCAN_THREADS, 0, st>>>(a);
     STB_CUDA(cudaGetLastError());
@@ -1873,15 +1905,121 @@ int stb_ivfpq_search_filtered(stb_ivfpq *x, const float *q, uint32_t nq, uint32_
     if ((rc = stb_launch_row_bitmap(ctx, x->f_ranges, nr, words, x->f_bitmap)) != STB_OK) return rc;
     bitmap = x->f_bitmap;
   }
-  ivff_elig_kernel<<<(x->nlist + 7) / 8, 256, 0, st>>>(x->list_off, x->order, x->nlist, bitmap, x->f_elig);
+  ivff_elig_kernel<<<(x->nlist + 7) / 8, 256, 0, st>>>(x->list_off, x->order, x->nlist, bitmap, 0, x->f_elig);
   STB_CUDA(cudaGetLastError());
   ctx->kernel_launches += 1;
   IvfbFilter f;
-  f.bitmap = bitmap; f.elig = x->f_elig;
+  f.bitmap = bitmap; f.elig = x->f_elig; f.slot_set = nullptr; f.bm_words = 0;
   f.max_dist = has_max ? std::min(max_distance, STB_DEFAULT_MAX_DIST) : STB_DEFAULT_MAX_DIST;   // as stb_search
   rc = ivfb_host_chunks(x, q, nq, nprobe, top_k, rerank, out_hits, out_n, out_scanned, &f);
   STB_CUDA(cudaStreamSynchronize(st));                         // `loc` is read by the copy above
   return rc;
+}
+
+int stb_ivfpq_search_subsets(stb_ivfpq *x, const float *q, uint32_t nq, uint32_t nprobe, uint32_t top_k, uint32_t rerank,
+                             int has_max, double max_distance, uint32_t n_subsets, const uint64_t *subset_offsets,
+                             const uint64_t *row_ranges, const uint32_t *subset_of, stb_hit *out_hits, uint32_t *out_n,
+                             uint64_t *out_scanned) {
+  static const char *who = "ivfpq_search_subsets";
+  if (!x) { stb_set_error("%s: null index", who); return STB_ERR_ARG; }
+  if (nq == 0) return STB_OK;
+  if (!q || !out_n || !subset_of || !subset_offsets || (top_k && !out_hits)) { stb_set_error("%s: null argument", who); return STB_ERR_ARG; }
+  if (top_k > 1024) { stb_set_error("%s: top_k must be <= 1024", who); return STB_ERR_ARG; }
+  if (subset_offsets[0] != 0) { stb_set_error("%s: subset_offsets[0] must be 0", who); return STB_ERR_ARG; }
+  for (uint32_t s = 0; s < n_subsets; ++s)
+    if (subset_offsets[s + 1] < subset_offsets[s] || subset_offsets[s + 1] - subset_offsets[s] > UINT32_MAX) {
+      stb_set_error("%s: subset_offsets must not decrease, by at most 2^32 - 1 ranges per subset (subset %u)", who, s);
+      return STB_ERR_ARG;
+    }
+  if (subset_offsets[n_subsets] && !row_ranges) { stb_set_error("%s: row_ranges is null", who); return STB_ERR_ARG; }
+  for (uint32_t i = 0; i < nq; ++i)
+    if (subset_of[i] >= n_subsets) { stb_set_error("%s: query %u names subset %u of %u", who, i, subset_of[i], n_subsets); return STB_ERR_ARG; }
+  // every subset, named or not, validated and clipped as stb_ivfpq_search_filtered does; the clipped local pairs
+  // lie back to back, subset s at pairs [loc_off[s], loc_off[s+1])
+  std::vector<uint32_t> loc;
+  std::vector<uint64_t> loc_off(n_subsets + 1, 0);
+  loc.reserve(2 * subset_offsets[n_subsets]);                  // one allocation: the clipping appends subset by subset
+  for (uint32_t s = 0; s < n_subsets; ++s) {
+    const int rc = stb_clip_ranges_u32(who, row_ranges + 2 * subset_offsets[s], (uint32_t)(subset_offsets[s + 1] - subset_offsets[s]),
+                                       x->corpus->row_base, x->n, &loc);
+    if (rc != STB_OK) return rc;
+    loc_off[s + 1] = loc.size() / 2;
+  }
+  if (top_k == 0) {
+    for (uint32_t i = 0; i < nq; ++i) { out_n[i] = 0; if (out_scanned) out_scanned[i] = 0; }
+    return STB_OK;
+  }
+  stb_ctx *ctx = x->ctx;
+  if (cudaSetDevice(ctx->device) != cudaSuccess) { stb_set_error("cudaSetDevice failed"); return STB_ERR_CUDA; }
+  ivfb_clamp(x, top_k, nprobe, rerank);
+  cudaStream_t st = ctx->stream;
+  int rc;
+  if (!loc.empty()) {
+    if ((rc = x->f_ranges.reserve(loc.size(), 2048)) != STB_OK) return rc;
+    STB_CUDA(cudaMemcpyAsync(x->f_ranges, loc.data(), loc.size() * 4, cudaMemcpyHostToDevice, st));
+  }
+  // launches: queries in caller order, at most IVFB_MAX_NQ, and as many distinct subsets as the scratch cap
+  // holds (at least one); a query of an empty subset is answered here and takes no part
+  const uint64_t words = (x->n + 31) / 32;
+  const uint64_t set_cap = std::max<uint64_t>(1, STB_IVFPQ_SUBSET_SCRATCH / ((words + x->nlist) * 4));
+  IvfbFilter f;
+  f.max_dist = has_max ? std::min(max_distance, STB_DEFAULT_MAX_DIST) : STB_DEFAULT_MAX_DIST;   // as stb_search
+  f.bm_words = words;
+  std::vector<uint32_t> local(n_subsets, UINT32_MAX), qrow, slot_set, status;
+  std::vector<uint64_t> set_off;                                 // per subset of the launch: [begin, end) pairs
+  std::vector<float> qc;
+  std::vector<stb_hit> hits;
+  for (uint32_t i = 0; i < nq;) {
+    qrow.clear(); slot_set.clear(); set_off.clear();
+    for (; i < nq && qrow.size() < IVFB_MAX_NQ; ++i) {
+      const uint32_t s = subset_of[i];
+      if (loc_off[s] == loc_off[s + 1]) {
+        out_n[i] = 0;
+        if (out_scanned) out_scanned[i] = 0;
+        stb_pad_hits(out_hits + (size_t)i * top_k, 0, top_k);
+        continue;
+      }
+      if (local[s] == UINT32_MAX) {
+        if (set_off.size() / 2 == set_cap) break;
+        local[s] = (uint32_t)(set_off.size() / 2);
+        set_off.push_back(loc_off[s]); set_off.push_back(loc_off[s + 1]);
+      }
+      qrow.push_back(i); slot_set.push_back(local[s]);
+    }
+    const uint32_t m = (uint32_t)qrow.size(), n_sets = (uint32_t)(set_off.size() / 2);
+    if (m == 0) break;
+    if ((rc = ivfb_reserve(x, m)) != STB_OK || (rc = x->f_bitmap.reserve((size_t)n_sets * words)) != STB_OK ||
+        (rc = x->f_elig.reserve((size_t)n_sets * x->nlist)) != STB_OK || (rc = x->f_set_off.reserve(set_off.size(), 512)) != STB_OK ||
+        (rc = x->f_slot_set.reserve(m, 512)) != STB_OK)
+      return rc;
+    qc.resize((size_t)m * STB_D);
+    for (uint32_t j = 0; j < m; ++j) memcpy(qc.data() + (size_t)j * STB_D, q + (size_t)qrow[j] * STB_D, STB_D * sizeof(float));
+    STB_CUDA(cudaMemcpyAsync(x->b_q, qc.data(), qc.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+    STB_CUDA(cudaMemcpyAsync(x->f_set_off, set_off.data(), set_off.size() * 8, cudaMemcpyHostToDevice, st));
+    STB_CUDA(cudaMemcpyAsync(x->f_slot_set, slot_set.data(), (size_t)m * 4, cudaMemcpyHostToDevice, st));
+    // the eligibility pass of every subset of the launch: one bitmap launch, one count launch
+    if ((rc = stb_launch_row_bitmap(ctx, x->f_ranges, 0, words, x->f_bitmap, n_sets, x->f_set_off)) != STB_OK) return rc;
+    ivff_elig_kernel<<<dim3((x->nlist + 7) / 8, n_sets), 256, 0, st>>>(x->list_off, x->order, x->nlist, x->f_bitmap, words,
+                                                                      x->f_elig);
+    STB_CUDA(cudaGetLastError());
+    ctx->kernel_launches += 1;
+    f.bitmap = x->f_bitmap; f.elig = x->f_elig; f.slot_set = x->f_slot_set;
+    if ((rc = ivfb_launch(x, x->b_q, m, nprobe, top_k, rerank, x->b_hits, x->b_status, &f)) != STB_OK) return rc;
+    hits.resize((size_t)m * top_k);
+    status.resize(2 * (size_t)m);
+    STB_CUDA(cudaMemcpyAsync(hits.data(), x->b_hits, hits.size() * sizeof(stb_hit), cudaMemcpyDeviceToHost, st));
+    STB_CUDA(cudaMemcpyAsync(status.data(), x->b_status, status.size() * 4, cudaMemcpyDeviceToHost, st));
+    STB_CUDA(cudaStreamSynchronize(st));                         // also ends the reads of loc, qc, set_off, slot_set
+    for (uint32_t j = 0; j < m; ++j) {
+      const uint32_t r = qrow[j];
+      memcpy(out_hits + (size_t)r * top_k, hits.data() + (size_t)j * top_k, top_k * sizeof(stb_hit));
+      out_n[r] = status[2 * j];
+      if (out_scanned) out_scanned[r] = status[2 * j + 1];
+    }
+    for (uint32_t j = 0; j < m; ++j) local[subset_of[qrow[j]]] = UINT32_MAX;
+  }
+  STB_CUDA(cudaStreamSynchronize(st));                           // `loc` is read by the copy above
+  return STB_OK;
 }
 
 int stb_ivfpq_search(stb_ivfpq *x, const float *q, uint32_t nprobe, uint32_t top_k, uint32_t rerank,
