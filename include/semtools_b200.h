@@ -291,6 +291,17 @@ int stb_search_topk_dev(stb_ctx *ctx, const stb_corpus *corpus,
  * canonical f64 distance on the f32 rows, and a result is accepted only if the 16-bit error bound
  * proves no other row can enter the top-k; unproven queries are answered by the single-query path
  * (stb_search).  Results are therefore identical to stb_search.
+ * Where the shadow cannot be allocated (a corpus too large for HBM to hold it beside the rows and the q8
+ * copy), both forms read the q8 copy instead (route 7, built or extended first; DESIGN §4): the queries are
+ * quantised to 16 bits as K1 quantises them, their two bytes are multiplied with the int8 codes on the int8
+ * tensor cores, and the threshold, emission, exact re-score and proof run on K1's upper and lower bounds.
+ * It returns what the shadow's routes would: the host form's hits and counts are bit for bit stb_search's,
+ * and a query the _dev form marks proven carries exactly stb_search's hits.  It runs when its sampled threshold
+ * fits: top_k <= 64 up to ~50M rows, top_k <= 32 up to ~100M, top_k <= 16 up to ~200M (in general
+ * ceil(ceil(n / 256) / 49152) <= floor(256 / top_k); stb_debug_batch_q8_plan).  Otherwise every query comes
+ * back unproven, and the host form answers it through stb_search.
+ * Zero and unnormalisable queries are never proven there.  If the q8 copy cannot be used either (it does not
+ * fit, or a row cannot be normalised), the call fails with the shadow's STB_ERR_NOMEM and writes nothing.
  *   q         nq x 256 f32 (host);  out_hits nq x top_k (unused tail: +inf / UINT64_MAX)
  *   out_n     nq counts */
 int stb_corpus_prepare_batch(stb_corpus *corpus);
@@ -696,6 +707,16 @@ int stb_debug_q4_scan(stb_ctx *ctx, const stb_corpus *corpus, const float *q, ui
  * NULL) the per-32-row maxima [ceil(nq/128)][ceil(n/256)*8][128]. */
 int stb_debug_batch_gemm(stb_ctx *ctx, const float *q, uint32_t nq, const float *rows,
                          uint64_t n, float *out_full, float *out_submax);
+/* Test hook for K2's route 7: stb_search_batch run on the q8 copy whatever the state of the 16-bit shadow
+ * (it builds no shadow and leaves an existing one untouched), with the same outputs and the same answer by
+ * stb_search for every query the route leaves unproven. */
+int stb_debug_batch_q8(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t nq, uint32_t top_k,
+                       stb_hit *out_hits, uint32_t *out_n);
+/* Test hook for K2's route 7: the query quantisation and the integer GEMM over the corpus's q8 copy (built or
+ * extended first).  q16 receives [nq][256] the 16-bit query components, dot [nq][n] the int32 products with
+ * the int8 codes, u and l [nq][n] the upper and lower bounds of the exact cosine computed from them. */
+int stb_debug_batch_q8_gemm(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t nq, int16_t *q16,
+                            int32_t *dot, float *u, float *l);
 /* Test hook for K5: synchronous copies of a built index into host buffers; a NULL pointer skips
  * that array.  centroids [nlist][256] f32, codebooks [32][256][8] f32, list_off [nlist+1],
  * order [m] (local row of each code), codes [m][32] u8, forced [n - m] (local rows outside the
@@ -713,21 +734,26 @@ int stb_debug_ivfpq_batch_last(const stb_ivfpq *index, uint32_t i, uint32_t info
  * stb_search_batch_subsets or stb_search_batch_threshold on ctx (synchronises the stream).  info = {route, nq, a,
  * b, n_seg, seg_cap}; route 1 = v1, 2 = v2, 3 = filtered v2, 4 = a filtered call that launched nothing on the
  * tensor cores (K1 answered it, or nothing could be returned), 5 = threshold mode, 6 = one filter per query
- * group, 0 = none yet.  Slots 2-3 (a, b):
- *   routes 1-4: n_sample, stride -- v2's sampled tiles (0, stride, 2*stride, ...; after route 3 they count listed
- *               tiles, the tiles holding an eligible row, in ascending order); 0 after routes 1 and 4;
+ * group, 7 = v2 on the q8 copy and the int8 tensor cores (the shadow did not fit, or stb_debug_batch_q8),
+ * 0 = none yet.  Slots 2-3 (a, b):
+ *   routes 1-4, 7: n_sample, stride -- v2's sampled tiles (0, stride, 2*stride, ...; after route 3 they count
+ *               listed tiles, the tiles holding an eligible row, in ascending order); 0 after routes 1 and 4
+ *               and after a route 7 call whose batch did not fit its plan (n_seg and seg_cap are 0 then too);
  *   route 5:    the queries re-emitted by the second tensor pass, and the queries stb_search answered;
  *   route 6:    the groups that ran on the tensor cores, and the queries stb_search answered.  After a route 6
  *               call that ran the tensor passes, thr and cand_cnt are in caller query order; a query those
  *               passes did not take has threshold +inf and zero counts.
  * n_seg and seg_cap are the emitting grid and the first pass's per-(query, CTA) key capacity, 0 after routes 1
- * and 4 and after a route 5 call that launched nothing.  After routes 2, 3 and a route 5 call that ran the
+ * and 4 and after a route 5 call that launched nothing.  After routes 2, 3 and a route 5 or 7 call that ran the
  * tensor pass, thr (may be NULL) receives the nq emission thresholds and cand_cnt (may be NULL) the raw
  * first-pass emission counts [nq][n_seg]; a count above seg_cap marks an overflowed segment. */
 int stb_debug_batch_last(stb_ctx *ctx, uint32_t info[6], float *thr, uint32_t *cand_cnt);
 /* Build parameters of K2 (host-only): element type of the shadow the tensor-core pass runs on
  * (0 = bf16, 1 = fp16) and the bound |approximate - exact cosine| <= eps its selection uses. */
 int stb_debug_batch_params(int *shadow_is_f16, double *eps);
+/* Route 7's plan (host-only): for a card with sm_count SMs, a corpus of n_rows rows and top_k, plan = {sampled
+ * tiles, sample stride, 1 if the batch runs on the route (0: stb_search answers every query)}. */
+int stb_debug_batch_q8_plan(uint32_t sm_count, uint64_t n_rows, uint32_t top_k, uint32_t plan[3]);
 
 #ifdef __cplusplus
 }

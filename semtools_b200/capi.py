@@ -30,7 +30,7 @@ SYMBOLS = [
     "stb_xchg_connect", "stb_xchg_connect_local", "stb_search_topk_xchg", "stb_search_xchg", "stb_search_many", "stb_xchg_create_batch", "stb_search_batch_xchg_dev", "stb_ivfpq_build",
     "stb_ivfpq_destroy", "stb_ivfpq_extend", "stb_ivfpq_stats", "stb_ivfpq_search", "stb_ivfpq_search_dev", "stb_hits_merge_dev", "stb_hits_merge_batch_dev", "stb_hits_merge", "stb_fnv1a64", "stb_line_id", "stb_line_ids",
     "stb_ctx_counters", "stb_debug_ticket_check", "stb_debug_q4_refined", "stb_debug_coscan_offsets", "stb_debug_batch_gemm", "stb_debug_batch_params",
-    "stb_debug_batch_last", "stb_debug_corpus_copy", "stb_debug_scan_scores", "stb_debug_q4_scan",
+    "stb_debug_batch_last", "stb_debug_batch_q8", "stb_debug_batch_q8_gemm", "stb_debug_batch_q8_plan", "stb_debug_corpus_copy", "stb_debug_scan_scores", "stb_debug_q4_scan",
     "stb_debug_ivfpq_export",
     "stb_ivfpq_search_batch", "stb_ivfpq_search_batch_dev", "stb_debug_ivfpq_batch_last",
     "stb_ivfpq_search_filtered", "stb_ivfpq_search_subsets", "stb_ivfpq_update", "stb_ivfpq_remove",
@@ -135,6 +135,9 @@ def lib() -> C.CDLL:
     L.stb_debug_batch_gemm.argtypes = [vp, vp, u32, vp, u64, vp, vp]
     L.stb_debug_batch_params.argtypes = [C.POINTER(C.c_int), C.POINTER(C.c_double)]
     L.stb_debug_batch_last.argtypes = [vp, vp, vp, vp]
+    L.stb_debug_batch_q8.argtypes = [vp, vp, vp, u32, u32, vp, vp]
+    L.stb_debug_batch_q8_gemm.argtypes = [vp, vp, vp, u32, vp, vp, vp, vp]
+    L.stb_debug_batch_q8_plan.argtypes = [u32, u64, u32, vp]
     L.stb_debug_ivfpq_export.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     L.stb_ivfpq_search_batch.argtypes = [vp, vp, u32, u32, u32, u32, vp, vp, vp]
     L.stb_ivfpq_search_batch_dev.argtypes = [vp, vp, u32, u32, u32, u32, vp, vp]
@@ -168,6 +171,14 @@ def batch_params():
     f16, eps = C.c_int(0), C.c_double(0.0)
     _check(lib().stb_debug_batch_params(C.byref(f16), C.byref(eps)))
     return bool(f16.value), float(eps.value)
+
+
+def batch_q8_plan(sm_count: int, n_rows: int, top_k: int):
+    """(n_sample, stride, fits) of K2 route 7's plan for a card with sm_count SMs (stb_debug_batch_q8_plan;
+    host-only)."""
+    out = np.zeros(3, dtype=np.uint32)
+    _check(lib().stb_debug_batch_q8_plan(sm_count, n_rows, top_k, _np_ptr(out)))
+    return int(out[0]), int(out[1]), bool(out[2])
 
 
 def fnv1a64(data: bytes) -> int:
@@ -237,16 +248,16 @@ class Context:
     def batch_last(self):
         """stb_debug_batch_last: the most recent K2 device call on this context.  Returns a dict with
         route (1 = v1, 2 = v2, 3 = filtered v2, 4 = filtered without the tensor cores, 5 = threshold mode, 6 = one
-        filter per query group), nq, n_sample, stride (routes 1-4) or retried, k1 (route 5: queries re-emitted by the
+        filter per query group, 7 = v2 on the q8 copy), nq, n_sample, stride (routes 1-4, 7) or retried, k1 (route 5: queries re-emitted by the
         second tensor pass / answered by stb_search) or groups, k1 (route 6: groups on the tensor cores / queries
-        answered by stb_search), n_seg, seg_cap and, after v2 (filtered or not) and a route 5 or 6 call that ran the
+        answered by stb_search), n_seg, seg_cap and, after v2 (filtered or not) and a route 5, 6 or 7 call that ran the
         tensor passes, thr [nq] (f32) and cand_cnt [nq][n_seg] (raw counts; > seg_cap marks an overflowed segment;
         route 6: caller order, +inf and zeros for a query the tensor passes did not take)."""
         info = np.zeros(6, dtype=np.uint32)
         _check(lib().stb_debug_batch_last(self._h, _np_ptr(info), None, None))
         names = {5: ("retried", "k1"), 6: ("groups", "k1")}.get(int(info[0]), ("n_sample", "stride"))
         out = dict(zip(("route", "nq") + names + ("n_seg", "seg_cap"), (int(v) for v in info)))
-        if out["route"] in (2, 3) or (out["route"] in (5, 6) and out["n_seg"]):
+        if out["route"] in (2, 3) or (out["route"] in (5, 6, 7) and out["n_seg"]):
             thr = np.zeros(max(out["nq"], 1), dtype=np.float32)
             cnt = np.zeros((max(out["nq"], 1), max(out["n_seg"], 1)), dtype=np.uint32)
             _check(lib().stb_debug_batch_last(self._h, _np_ptr(info), _np_ptr(thr), _np_ptr(cnt)))
@@ -490,6 +501,31 @@ class Corpus:
         cnt = np.zeros(max(nq, 1), dtype=np.uint32)
         _check(lib().stb_search_batch(self.ctx._h, self._h, _np_ptr(queries), nq, top_k, _np_ptr(out), _np_ptr(cnt)))
         return [out[i, : cnt[i]] for i in range(nq)]
+
+    def debug_batch_q8(self, queries, top_k: int = 10):
+        """stb_debug_batch_q8: search_batch on route 7 (the q8 copy on the int8 tensor cores) whatever the state of
+        the 16-bit shadow.  Returns a list of HIT_DTYPE arrays, one per query."""
+        queries = np.ascontiguousarray(queries, dtype=np.float32)
+        if queries.ndim != 2 or queries.shape[1] != STB_DIM:
+            raise StbError(STB_ERR_ARG, f"queries must be (nq,{STB_DIM}) f32")
+        nq = queries.shape[0]
+        out = np.zeros((nq, max(top_k, 1)), dtype=HIT_DTYPE)
+        cnt = np.zeros(max(nq, 1), dtype=np.uint32)
+        _check(lib().stb_debug_batch_q8(self.ctx._h, self._h, _np_ptr(queries), nq, top_k, _np_ptr(out), _np_ptr(cnt)))
+        return [out[i, : cnt[i]] for i in range(nq)]
+
+    def debug_batch_q8_gemm(self, queries):
+        """stb_debug_batch_q8_gemm: route 7's query quantisation and integer GEMM.  Returns (q16 [nq, 256] int16,
+        dot [nq, n] int32, u [nq, n] f32, l [nq, n] f32)."""
+        queries = np.ascontiguousarray(queries, dtype=np.float32).reshape(-1, STB_DIM)
+        nq, n = queries.shape[0], len(self)
+        q16 = np.zeros((nq, STB_DIM), dtype=np.int16)
+        dot = np.zeros((nq, n), dtype=np.int32)
+        u = np.zeros((nq, n), dtype=np.float32)
+        l = np.zeros((nq, n), dtype=np.float32)
+        _check(lib().stb_debug_batch_q8_gemm(self.ctx._h, self._h, _np_ptr(queries), nq, _np_ptr(q16), _np_ptr(dot),
+                                             _np_ptr(u), _np_ptr(l)))
+        return q16, dot, u, l
 
     def search_batch_filtered(self, queries, row_ranges=None, top_k: int = 10, max_distance: float | None = None):
         """stb_search_batch_filtered: for each query, what search(q, top_k, max_distance, STB_MODE_STORE_QUERY,

@@ -11,6 +11,7 @@
 #include <memory>
 #include <mutex>
 #include <new>
+#include <string>
 #include <unordered_map>
 #include <unordered_set>
 #include <vector>
@@ -1354,10 +1355,10 @@ int stb_corpus_prepare_batch(stb_corpus *corpus) {
 }  // extern "C"
 
 // ---- K2 host calls -------------------------------------------------------------------------------------------
-// The record of the last K2 call, which stb_debug_batch_last returns: route, nq, two route words (routes 1-4:
-// n_sample, stride; 5: retried queries, K1 queries; 6: tensor groups, K1 queries), n_seg, seg_cap.
+// The record of the last K2 call, which stb_debug_batch_last returns: route, nq, two route words (routes 1-4
+// and 7: n_sample, stride; 5: retried queries, K1 queries; 6: tensor groups, K1 queries), n_seg, seg_cap.
 enum K2Route : uint32_t { kRouteV1 = 1, kRouteV2 = 2, kRouteFiltered = 3, kRouteFilteredK1 = 4, kRouteThreshold = 5,
-                          kRouteSubsets = 6 };
+                          kRouteSubsets = 6, kRouteQ8 = 7 };
 static void k2_record(stb_ctx *ctx, K2Route route, uint32_t nq, uint32_t a = 0, uint32_t b = 0, uint32_t n_seg = 0,
                       uint32_t seg_cap = 0) {
   const uint32_t words[6] = {route, nq, a, b, n_seg, seg_cap};
@@ -1429,6 +1430,71 @@ static int batch_v2_run(stb_ctx *ctx, const stb_corpus *corpus, const float *q_d
   if (rc != STB_OK) return rc;
   return stb_launch_batch_finish2(ctx, ctx->b_keys, ctx->b_cnt, n_seg, kSegCap, nq, top_k, corpus->rows, corpus->n,
                                   corpus->row_base, q_dev, ctx->b_qbad, out_hits_dev, out_status_dev);
+}
+
+// Route 7's sample size and fit rule (v2's, batch_scan.cu: "Route 7", with the q8 bounds in place of the shadow's
+// EPS).  A row's bounds are u, l = a +- w with w = s h_l1 + e_q (~0.011 on the benchmark's rows: s ~ 0.21 / 127,
+// h_l1 ~ ||q^||_1 / 2 ~ 6.4), and the threshold sits w below the sampled k-th cosine, so the emitted rows are those
+// with a >= S - 2w instead of v2's a >= S - 2 EPS: ~e^(2 w x / sigma^2) ~ 7.2 times the top_k * n_cover / n_sample
+// rows that reach the sampled k-th score (x ~ 0.35, sigma = 1/16), taken as 8.  The sample is ~4 tiles per SM,
+// or as many as keep that estimate within half of the finish's 4096-key capacity (a multiple of the SM count,
+// at most kQ8MaxSample: the threshold kernel's CTA-per-query variant holds that many maxima in 192 KiB of shared
+// memory); any tile may be sampled, since rows past n are masked out of the maxima.  So a batch fits while
+// ceil(n_tiles / 49152) <= floor(256 / top_k), top_k <= 64: every top_k up to ~50M rows, top_k <= 32 up to
+// ~100M, top_k <= 16 up to ~200M (tests/test_batch_q8_plan.py).  Batches that do not fit are answered by K1.
+static constexpr uint32_t kQ8MaxSample = 49152;
+static BatchV2Plan batch_q8_plan(uint32_t sm, uint32_t n_cover, uint32_t top_k) {
+  if (top_k == 0 || top_k > 64 || n_cover == 0 || sm == 0) return {0, 0, false};
+  const uint32_t per_sample = 2048u / (8u * top_k);            // tiles one sampled tile may stand for (>= 4)
+  uint32_t n_sample = std::max<uint32_t>(std::min<uint32_t>(4u * sm, 608u), (n_cover + per_sample - 1) / per_sample);
+  if (n_sample > 608u) n_sample = std::min<uint32_t>((n_sample + sm - 1) / sm * sm, kQ8MaxSample);
+  n_sample = std::min(n_sample, n_cover);
+  const bool fits = n_sample >= top_k && (n_cover + n_sample - 1) / n_sample <= per_sample;
+  return {n_sample, fits ? n_cover / n_sample : 0u, fits};
+}
+
+// Route 7 (batch_scan.cu): q8 query tiles -> sampled threshold on the lower bounds -> upper-bound-emitting int8
+// wgmma epilogue -> the finish with the q8 proof.  Builds or extends the q8 copy first (its status is returned
+// if it cannot be used).  A batch that does not fit the plan comes back with every query unproven.
+static int batch_q8_run(stb_ctx *ctx, stb_corpus *corpus, const float *q_dev, uint32_t nq, uint32_t top_k,
+                        stb_hit *out_hits_dev, uint32_t *out_status_dev) {
+  int rc;
+  if ((rc = corpus_ensure_q8(ctx, corpus)) != STB_OK) return rc;
+  const uint32_t m_tiles = (nq + 127) / 128, q_pad = m_tiles * 128;
+  const uint32_t n_tiles = (uint32_t)((corpus->n + 255) / 256);
+  const BatchV2Plan p = batch_q8_plan((uint32_t)ctx->sm_count, n_tiles, top_k);
+  const uint32_t n_seg = stb_batch_emit_grid(ctx, n_tiles);
+  if (!p.fits) {
+    std::vector<stb_hit> pad((size_t)nq * top_k);
+    stb_pad_hits(pad.data(), 0, pad.size());
+    STB_CUDA(cudaMemcpyAsync(out_hits_dev, pad.data(), pad.size() * sizeof(stb_hit), cudaMemcpyHostToDevice, ctx->stream));
+    STB_CUDA(cudaMemsetAsync(out_status_dev, 0, (size_t)nq * 2 * sizeof(uint32_t), ctx->stream));
+    STB_CUDA(cudaStreamSynchronize(ctx->stream));       // `pad` is read by the copy
+    k2_record(ctx, kRouteQ8, nq);
+    return STB_OK;
+  }
+  // every buffer first: a call refused for lack of memory leaves the record as it was
+  if ((rc = ctx->b_qbad.reserve((size_t)q_pad)) != STB_OK) return rc;
+  if ((rc = ctx->b_q8c.reserve((size_t)q_pad)) != STB_OK) return rc;
+  if ((rc = ctx->bq_tiles.reserve((size_t)q_pad * 512)) != STB_OK) return rc;
+  if ((rc = ctx->b_tilemax.reserve((size_t)p.n_sample * q_pad)) != STB_OK) return rc;
+  if ((rc = ctx->b_thr.reserve((size_t)q_pad)) != STB_OK) return rc;
+  if ((rc = ctx->b_cnt.reserve((size_t)q_pad * n_seg)) != STB_OK) return rc;
+  if ((rc = ctx->b_keys.reserve((size_t)q_pad * n_seg * kSegCap)) != STB_OK) return rc;
+  k2_record(ctx, kRouteQ8, nq, p.n_sample, p.stride, n_seg, kSegCap);
+  STB_CUDA(cudaMemsetAsync(ctx->b_cnt, 0, (size_t)q_pad * n_seg * sizeof(uint32_t), ctx->stream));
+  if ((rc = stb_launch_q8_query_tiles(ctx, q_dev, nq, q_pad, ctx->bq_tiles, ctx->b_q8c, ctx->b_qbad, nullptr)) != STB_OK ||
+      (rc = stb_launch_batch_q8_gemm_sample(ctx, ctx->bq_tiles, ctx->b_q8c, m_tiles, corpus->q8, corpus->q8_scale, corpus->n,
+                                            p.n_sample, p.stride, ctx->b_tilemax)) != STB_OK ||
+      // an unusable query (zero, or not normalisable) emits nothing and comes back unproven
+      (rc = stb_launch_batch_thresh(ctx, ctx->b_tilemax, p.n_sample, nq, q_pad, top_k, ctx->b_thr, (float)STB_Q8_SCAN_EPS,
+                                    ctx->b_qbad)) != STB_OK ||
+      (rc = stb_launch_batch_q8_gemm_emit(ctx, ctx->bq_tiles, ctx->b_q8c, m_tiles, corpus->q8, corpus->q8_scale, corpus->n,
+                                          ctx->b_thr, ctx->b_cnt, ctx->b_keys, kSegCap)) != STB_OK)
+    return rc;
+  return stb_launch_batch_finish2(ctx, ctx->b_keys, ctx->b_cnt, n_seg, kSegCap, nq, top_k, corpus->rows, corpus->n,
+                                  corpus->row_base, q_dev, ctx->b_qbad, out_hits_dev, out_status_dev, corpus->q8_scale,
+                                  ctx->b_q8c, ctx->b_thr);
 }
 
 // The listed tiles of clipped local [begin, end) pairs: the shadow tiles a range touches (ascending, disjoint
@@ -1528,8 +1594,11 @@ static int batch_filtered_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, 
 
 extern "C" {
 
-int stb_search_batch_dev(stb_ctx *ctx, const stb_corpus *corpus_c, const float *q_dev, uint32_t nq,
-                         uint32_t top_k, stb_hit *out_hits_dev, uint32_t *out_status_dev) {
+}  // extern "C"
+
+// stb_search_batch_dev; q8_route: route 7 whatever the shadow's state (stb_debug_batch_q8)
+static int batch_dev_impl(stb_ctx *ctx, const stb_corpus *corpus_c, const float *q_dev, uint32_t nq, uint32_t top_k,
+                          stb_hit *out_hits_dev, uint32_t *out_status_dev, bool q8_route) {
   int rc = ctx_use(ctx);
   if (rc) return rc;
   stb_corpus *corpus = const_cast<stb_corpus *>(corpus_c);
@@ -1538,7 +1607,16 @@ int stb_search_batch_dev(stb_ctx *ctx, const stb_corpus *corpus_c, const float *
   if (nq == 0) return STB_OK;
   if (top_k == 0 || top_k > 1024) { stb_set_error("search_batch_dev: top_k must be 1..1024"); return STB_ERR_ARG; }
   if (corpus->n == 0) { stb_set_error("search_batch_dev: empty corpus"); return STB_ERR_STATE; }
-  if ((rc = corpus_ensure_shadow(ctx, corpus)) != STB_OK) return rc;
+  if (q8_route) return batch_q8_run(ctx, corpus, q_dev, nq, top_k, out_hits_dev, out_status_dev);
+  if ((rc = corpus_ensure_shadow(ctx, corpus)) != STB_OK) {
+    if (rc != STB_ERR_NOMEM) return rc;
+    // the shadow does not fit in HBM: route 7 reads the q8 copy instead.  If that copy cannot be used either, the
+    // call is refused as before, with the shadow's status and message and nothing written
+    std::string shadow_err = stb_last_error();
+    const int q8_rc = batch_q8_run(ctx, corpus, q_dev, nq, top_k, out_hits_dev, out_status_dev);
+    if (q8_rc == STB_ERR_NOMEM || q8_rc == STB_ERR_STATE) { stb_set_error("%s", shadow_err.c_str()); return rc; }
+    return q8_rc;
+  }
   const uint32_t m_tiles = (nq + 127) / 128, q_pad = m_tiles * 128;
   const uint32_t n_tiles = (uint32_t)((corpus->n + 255) / 256), n_sub = n_tiles * 8;
   // Pipeline v2 (default, batch_v2_run).  Proves every query for any top_k <= 64 unless a capacity
@@ -1569,8 +1647,9 @@ int stb_search_batch_dev(stb_ctx *ctx, const stb_corpus *corpus_c, const float *
                                  corpus->row_base, q_dev, ctx->b_qbad, out_hits_dev, out_status_dev, ctx->b_submax, q_pad);
 }
 
-int stb_search_batch(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t nq, uint32_t top_k,
-                     stb_hit *out_hits, uint32_t *out_n) {
+// stb_search_batch on batch_dev_impl's route choice
+static int batch_host_impl(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t nq, uint32_t top_k,
+                           stb_hit *out_hits, uint32_t *out_n, bool q8_route) {
   int rc = ctx_use(ctx);
   if (rc) return rc;
   if (!corpus || !q || !out_hits || !out_n) { stb_set_error("search_batch: null argument"); return STB_ERR_ARG; }
@@ -1584,7 +1663,7 @@ int stb_search_batch(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uin
     if ((rc = ctx->bh_dev.reserve((size_t)nq * top_k)) != STB_OK) return rc;
     if ((rc = ctx->bs_dev.reserve((size_t)nq * 2)) != STB_OK) return rc;
     STB_CUDA(cudaMemcpyAsync(ctx->bq_dev, q, (size_t)nq * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-    rc = stb_search_batch_dev(ctx, corpus, ctx->bq_dev, nq, top_k, ctx->bh_dev, ctx->bs_dev);
+    rc = batch_dev_impl(ctx, corpus, ctx->bq_dev, nq, top_k, ctx->bh_dev, ctx->bs_dev, q8_route);
     if (rc == STB_ERR_STATE) { tensor_ok = false; }        // un-normalisable rows: K1 handles them
     else if (rc != STB_OK) return rc;
     else {
@@ -1600,6 +1679,23 @@ int stb_search_batch(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uin
     if (tensor_ok && status[2 * i + 1]) return {K2Answer::kProven, out_hits + (size_t)i * top_k, status[2 * i]};
     return {K2Answer::kK1};
   }, out_hits, out_n);
+}
+
+extern "C" {
+
+int stb_search_batch_dev(stb_ctx *ctx, const stb_corpus *corpus, const float *q_dev, uint32_t nq,
+                         uint32_t top_k, stb_hit *out_hits_dev, uint32_t *out_status_dev) {
+  return batch_dev_impl(ctx, corpus, q_dev, nq, top_k, out_hits_dev, out_status_dev, false);
+}
+
+int stb_search_batch(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t nq, uint32_t top_k,
+                     stb_hit *out_hits, uint32_t *out_n) {
+  return batch_host_impl(ctx, corpus, q, nq, top_k, out_hits, out_n, false);
+}
+
+int stb_debug_batch_q8(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t nq, uint32_t top_k,
+                       stb_hit *out_hits, uint32_t *out_n) {
+  return batch_host_impl(ctx, corpus, q, nq, top_k, out_hits, out_n, true);
 }
 
 int stb_search_batch_filtered(stb_ctx *ctx, const stb_corpus *corpus_c, const float *q, uint32_t nq, uint32_t top_k,
@@ -2143,10 +2239,17 @@ int stb_debug_batch_last(stb_ctx *ctx, uint32_t info[6], float *thr, uint32_t *c
     }
     return STB_OK;
   }
-  if ((route == kRouteV2 || route == kRouteFiltered || (route == kRouteThreshold && n_seg)) && nq) {
+  if ((route == kRouteV2 || route == kRouteFiltered || ((route == kRouteThreshold || route == kRouteQ8) && n_seg)) && nq) {
     if (thr) STB_CUDA(cudaMemcpy(thr, ctx->b_thr, (size_t)nq * sizeof(float), cudaMemcpyDeviceToHost));
     if (cand_cnt) STB_CUDA(cudaMemcpy(cand_cnt, ctx->b_cnt, (size_t)nq * n_seg * sizeof(uint32_t), cudaMemcpyDeviceToHost));
   }
+  return STB_OK;
+}
+
+int stb_debug_batch_q8_plan(uint32_t sm_count, uint64_t n_rows, uint32_t top_k, uint32_t plan[3]) {
+  if (!plan || n_rows > 0xffffffffull * 256) { stb_set_error("debug_batch_q8_plan: bad argument"); return STB_ERR_ARG; }
+  const BatchV2Plan p = batch_q8_plan(sm_count, (uint32_t)((n_rows + 255) / 256), top_k);
+  plan[0] = p.n_sample; plan[1] = p.stride; plan[2] = p.fits ? 1u : 0u;
   return STB_OK;
 }
 
@@ -2185,6 +2288,40 @@ int stb_debug_batch_gemm(stb_ctx *ctx, const float *q, uint32_t nq, const float 
   if (e == cudaSuccess && rc == STB_OK) e = cudaStreamSynchronize(ctx->stream);
   if (e != cudaSuccess) { stb_set_error("debug_batch_gemm: %s", cudaGetErrorString(e)); cudaGetLastError(); return STB_ERR_CUDA; }
   return rc;
+}
+
+// Route 7's query tiles and integer GEMM over a corpus's q8 copy (built or extended first): per query its q16
+// [nq][256], and per (query, row) the int32 dot and the bounds u, l [nq][n].
+int stb_debug_batch_q8_gemm(stb_ctx *ctx, const stb_corpus *corpus_c, const float *q, uint32_t nq, int16_t *q16,
+                            int32_t *dot, float *u, float *l) {
+  int rc = ctx_use(ctx);
+  if (rc) return rc;
+  stb_corpus *corpus = const_cast<stb_corpus *>(corpus_c);
+  if (!corpus || !q || !q16 || !dot || !u || !l || nq == 0 || corpus->n == 0) { stb_set_error("debug_batch_q8_gemm: bad argument"); return STB_ERR_ARG; }
+  if (corpus->ctx != ctx) { stb_set_error("debug_batch_q8_gemm: corpus belongs to another context"); return STB_ERR_ARG; }
+  if ((rc = corpus_ensure_q8(ctx, corpus)) != STB_OK) return rc;
+  const uint32_t m_tiles = (nq + 127) / 128;
+  const size_t q_pad = (size_t)m_tiles * 128, n = corpus->n, n_pad = (n + 255) / 256 * 256;
+  StbBuf<float> dq, du, dl;
+  StbBuf<uint8_t> da;
+  StbBuf<float4> dc;
+  StbBuf<uint32_t> dbad;
+  StbBuf<int16_t> d16;
+  StbBuf<int32_t> ddot;
+  if ((rc = dq.alloc((size_t)nq * STB_D)) != STB_OK || (rc = da.alloc(q_pad * 512)) != STB_OK || (rc = dc.alloc(q_pad)) != STB_OK ||
+      (rc = dbad.alloc(q_pad)) != STB_OK || (rc = d16.alloc((size_t)nq * STB_D)) != STB_OK ||
+      (rc = ddot.alloc(q_pad * n_pad)) != STB_OK || (rc = du.alloc(q_pad * n_pad)) != STB_OK || (rc = dl.alloc(q_pad * n_pad)) != STB_OK)
+    return rc;
+  STB_CUDA(cudaMemcpyAsync(dq, q, (size_t)nq * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+  if ((rc = stb_launch_q8_query_tiles(ctx, dq, nq, (uint32_t)q_pad, da, dc, dbad, d16)) != STB_OK ||
+      (rc = stb_launch_batch_q8_gemm_debug(ctx, da, dc, m_tiles, corpus->q8, corpus->q8_scale, n, ddot, du, dl)) != STB_OK)
+    return rc;
+  STB_CUDA(cudaMemcpyAsync(q16, d16, (size_t)nq * STB_D * sizeof(int16_t), cudaMemcpyDeviceToHost, ctx->stream));
+  STB_CUDA(cudaMemcpy2DAsync(dot, n * 4, ddot, n_pad * 4, n * 4, nq, cudaMemcpyDeviceToHost, ctx->stream));
+  STB_CUDA(cudaMemcpy2DAsync(u, n * 4, du, n_pad * 4, n * 4, nq, cudaMemcpyDeviceToHost, ctx->stream));
+  STB_CUDA(cudaMemcpy2DAsync(l, n * 4, dl, n_pad * 4, n * 4, nq, cudaMemcpyDeviceToHost, ctx->stream));
+  STB_CUDA(cudaStreamSynchronize(ctx->stream));
+  return STB_OK;
 }
 
 // ------------------------------------------------------------------- K1 debug hooks ---

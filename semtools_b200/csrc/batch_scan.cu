@@ -26,6 +26,7 @@
 //                               cosine <= m* (the smallest selected sub-tile maximum),
 //                               hence exact cosine <= m* + EPS2 (bf16 rounding bound).
 // Tensor-bound: 2*Q*N*256 FLOP per batch; HBM traffic N*512 B (16-bit shadow) once.
+#include <cudaTypedefs.h>   // CUtensorMap, PFN_cuTensorMapEncodeTiled (route 7); no libcuda link
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <math_constants.h>
@@ -34,6 +35,7 @@
 
 #include "common.cuh"
 #include "row_encode.cuh"
+#include "q8_query.cuh"
 
 #define STB_B_TILE 256            // corpus rows per tile  (MMA N)
 #define STB_A_TILE 128            // queries per tile      (MMA M, two m64 warpgroups)
@@ -1031,6 +1033,8 @@ struct ThreshArgs {
   const float *tilemax;     // [m_tiles][n_sample][128]
   uint32_t n_sample, nq, q_pad, top_k;
   float *thr;               // [q_pad]
+  float slack;              // thr = k-th largest sampled maximum - slack
+  const uint32_t *q_skip;   // [nq] or null: 1 = the query emits nothing (thr +inf)
 };
 
 // one warp per query: lane l holds sampled tile maxima l, l+32, ...; k rounds of warp-max
@@ -1068,12 +1072,13 @@ stb_batch_thresh_kernel(const ThreshArgs a) {
     }
   }
   // fewer than k sampled tiles (or k too large): -inf = emit everything (tiny corpora fit the cap)
-  if (lane == 0) a.thr[q] = (kth == -CUDART_INF_F) ? -CUDART_INF_F : kth - 2.0f * (float)STB_BATCH_EPS;
+  if (lane == 0) a.thr[q] = (a.q_skip && a.q_skip[q]) ? CUDART_INF_F : (kth == -CUDART_INF_F) ? -CUDART_INF_F : kth - a.slack;
 }
 
 // Same result for samples beyond 608 tiles (large shards): CTA per query, the sampled maxima
-// staged in shared memory, k rounds of block-max extraction.
-#define STB_V2_BIG_SAMPLE 8192
+// staged in shared memory, k rounds of block-max extraction.  Up to 49152 maxima (192 KiB): v2's plans stay
+// within 8192 (32 KiB, the default limit); route 7's plan samples up to the full capacity on the largest corpora.
+#define STB_V2_BIG_SAMPLE 49152
 __global__ void __launch_bounds__(256)
 stb_batch_thresh_big_kernel(const ThreshArgs a) {
   extern __shared__ float tb_vals[];          // n_sample floats
@@ -1116,7 +1121,7 @@ stb_batch_thresh_big_kernel(const ThreshArgs a) {
   }
   if (tid == 0) {
     const float kth = (a.top_k <= a.n_sample && a.top_k <= STB_V2_MAX_K) ? s_kth : -CUDART_INF_F;
-    a.thr[q] = (kth == -CUDART_INF_F) ? -CUDART_INF_F : kth - 2.0f * (float)STB_BATCH_EPS;
+    a.thr[q] = (a.q_skip && a.q_skip[q]) ? CUDART_INF_F : (kth == -CUDART_INF_F) ? -CUDART_INF_F : kth - a.slack;
   }
 }
 
@@ -1130,6 +1135,11 @@ struct Finish2Args {
   const uint32_t *q_bad;       // [nq] 1: the query could not be normalised (never proven)
   stb_hit *out_hits;           // [nq][top_k]
   uint32_t *out_status;        // [nq][2]: hits, complete
+  // route 7 (null on the shadow's routes): the keys hold q8 upper bounds u (stb_batch_q8_gemm_kernel); the q8
+  // scales, the queries' {1/S, h_l1, e_q, S} and the emission thresholds the proof is checked against
+  const float *q8_scale;
+  const float4 *q8_qc;
+  const float *thr;
 };
 
 #define STB_F2_KEYS 4096         // emitted candidates one query may bring (sum over its segments)
@@ -1152,6 +1162,7 @@ stb_batch_finish2_kernel(const Finish2Args a) {
   __shared__ uint32_t s_off[256 + 1];
   __shared__ int s_pass, s_over;
   __shared__ unsigned s_m2;
+  __shared__ unsigned s_sel[3];
   const uint32_t q = blockIdx.x;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint32_t k = a.top_k;
@@ -1160,7 +1171,7 @@ stb_batch_finish2_kernel(const Finish2Args a) {
     if (tid == 0) { a.out_status[2 * q] = 0; a.out_status[2 * q + 1] = 0; }
   };
   // 1. segment counts -> offsets (n_seg <= 256: one thread per segment, warp scans + 8-entry fix-up)
-  if (tid == 0) { s_pass = 0; s_over = 0; s_m2 = 0; }
+  if (tid == 0) { s_pass = 0; s_over = 0; s_m2 = 0; s_sel[0] = s_sel[1] = s_sel[2] = 0; }
   __syncthreads();
   uint32_t c = 0;
   if ((uint32_t)tid < a.n_seg) {
@@ -1201,7 +1212,36 @@ stb_batch_finish2_kernel(const Finish2Args a) {
   else stb_cta_sort_keys_t<16>(skeys, n_sort);
   // 3. narrow to a >= A_k - 2 EPS (everything when fewer than k rows were emitted)
   float cut = -CUDART_INF_F;
-  if (m_all >= k) cut = stb_key_score(skeys[k - 1]) - 2.0f * (float)STB_BATCH_EPS;
+  if (a.q8_scale) {
+    // route 7: the keys are upper bounds u >= c - 1e-5.  l = u - 2 (s h_l1 + e_q) - 2 STB_Q8_SCAN_EPS is a lower bound
+    // of c (the q8 bounds' two error terms, plus the fp32 evaluation of u and of this difference), so the k
+    // emitted rows with the largest l have c >= L_k, and a row with u < L_k - STB_Q8_SCAN_EPS has c < L_k: it
+    // can neither be a result nor tie with one.  Those rows are dropped before any f32 row is read.  L_k: the
+    // largest T with #{l >= T} >= k, bit by bit on the ordered l (staged where the rows go later)
+    if (m_all >= k) {
+      uint32_t *lo = reinterpret_cast<uint32_t *>(srows);
+      const float4 qc = __ldg(a.q8_qc + q);
+      for (uint32_t i = tid; i < m_all; i += 256) {
+        const float w = fmaf(__ldg(a.q8_scale + stb_key_row(skeys[i])), qc.y, qc.z);
+        lo[i] = stb_f2ord(stb_key_score(skeys[i]) - 2.0f * w - 2.0f * (float)STB_Q8_SCAN_EPS);
+      }
+      __syncthreads();
+      uint32_t T = 0;
+      for (int bit = 31; bit >= 0; --bit) {
+        const uint32_t cand = T | (1u << bit);
+        uint32_t n_ge = 0;
+        for (uint32_t i = tid; i < m_all; i += 256) n_ge += lo[i] >= cand ? 1u : 0u;
+        n_ge = __reduce_add_sync(0xffffffffu, n_ge);
+        if (lane == 0 && n_ge) atomicAdd(&s_sel[bit % 3], n_ge);
+        __syncthreads();
+        if (s_sel[bit % 3] >= k) T = cand;
+        if (tid == 0) s_sel[(bit + 1) % 3] = 0;     // the counter of round bit - 2, last read before this round's barrier
+      }
+      cut = stb_ord2f(T) - (float)STB_Q8_SCAN_EPS;
+    }
+  } else if (m_all >= k) {
+    cut = stb_key_score(skeys[k - 1]) - 2.0f * (float)STB_BATCH_EPS;
+  }
   for (uint32_t i = tid; i < m_all; i += 256)
     if (stb_key_score(skeys[i]) >= cut) atomicMax(&s_m2, i + 1);
   if (tid == 5 * 32) s_q2 = stb_canon_q2(sqd);
@@ -1249,16 +1289,33 @@ stb_batch_finish2_kernel(const Finish2Args a) {
   stb_cta_sort_hits(sd, sr, n2);
   const uint32_t n_out = min((uint32_t)s_pass, k);
   stb_write_hits(a.out_hits + (size_t)q * k, sd, sr, n_out, k);
-  if (tid == 0) { a.out_status[2 * q] = n_out; a.out_status[2 * q + 1] = a.q_bad[q] ? 0u : 1u; }
+  if (tid == 0) {
+    bool complete = !a.q_bad[q];
+    if (a.q8_scale) {
+      // route 7: a row that was not emitted has u < thr, hence c <= u + 1e-5 < thr + 1e-5; the query is proven if
+      // the k-th re-scored distance beats every such row strictly (the margin also covers the f64 distance's
+      // rounding).  thr is finite here: the plan samples at least k tiles, each holding a real row
+      complete = complete && n_out == k && sd[k - 1] < 1.0 - (double)a.thr[q] - STB_Q8_SCAN_EPS;
+    }
+    a.out_status[2 * q] = n_out;
+    a.out_status[2 * q + 1] = complete ? 1u : 0u;
+  }
 }
 
 int stb_launch_batch_thresh(stb_ctx *ctx, const float *tilemax, uint32_t n_sample, uint32_t nq, uint32_t q_pad,
-                            uint32_t top_k, float *thr) {
+                            uint32_t top_k, float *thr, float slack, const uint32_t *q_skip) {
   if (n_sample > STB_V2_BIG_SAMPLE) { stb_set_error("batch_thresh: sample too large"); return STB_ERR_ARG; }
   ThreshArgs a;
   a.tilemax = tilemax; a.n_sample = n_sample; a.nq = nq; a.q_pad = q_pad; a.top_k = top_k; a.thr = thr;
+  a.slack = slack < 0.f ? 2.0f * (float)STB_BATCH_EPS : slack; a.q_skip = q_skip;
   if (n_sample <= STB_V2_MAX_SAMPLE) stb_batch_thresh_kernel<<<(q_pad + 7) / 8, 256, 0, ctx->stream>>>(a);
-  else stb_batch_thresh_big_kernel<<<q_pad, 256, (size_t)n_sample * sizeof(float), ctx->stream>>>(a);
+  else {
+    const size_t smem = (size_t)n_sample * sizeof(float);
+    if (smem > 48 * 1024)
+      STB_ATTR_ONCE(ctx, STB_ATTR_THRESH_BIG, cudaFuncSetAttribute(stb_batch_thresh_big_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                                   STB_V2_BIG_SAMPLE * (int)sizeof(float)));
+    stb_batch_thresh_big_kernel<<<q_pad, 256, smem, ctx->stream>>>(a);
+  }
   STB_CUDA(cudaGetLastError());
   ctx->kernel_launches++;
   return STB_OK;
@@ -1271,12 +1328,13 @@ uint32_t stb_batch_emit_grid(const stb_ctx *ctx, uint32_t n_tiles) {
 int stb_launch_batch_finish2(stb_ctx *ctx, const uint64_t *cand_keys, const uint32_t *cand_cnt, uint32_t n_seg,
                              uint32_t seg_cap, uint32_t nq, uint32_t top_k, const float *rows, uint64_t n_rows,
                              uint64_t row_base, const float *queries_dev, const uint32_t *q_bad, stb_hit *out_hits,
-                             uint32_t *out_status) {
+                             uint32_t *out_status, const float *q8_scale, const float4 *q8_qc, const float *thr) {
   if (top_k > STB_F2_RESCORE || n_seg > 256 || n_seg == 0) { stb_set_error("batch_finish2: bad shape"); return STB_ERR_ARG; }
   Finish2Args a;
   a.cand_keys = cand_keys; a.cand_cnt = cand_cnt; a.n_seg = n_seg; a.seg_cap = seg_cap; a.nq = nq; a.top_k = top_k;
   a.rows = reinterpret_cast<const float4 *>(rows); a.n_rows = n_rows; a.row_base = row_base;
   a.queries = queries_dev; a.q_bad = q_bad; a.out_hits = out_hits; a.out_status = out_status;
+  a.q8_scale = q8_scale; a.q8_qc = q8_qc; a.thr = thr;
   constexpr size_t smem = STB_F2_KEYS * sizeof(uint64_t) + 32 * STB_F2_STRIDE * sizeof(float);
   STB_ATTR_ONCE(ctx, STB_ATTR_FINISH2, cudaFuncSetAttribute(stb_batch_finish2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   stb_batch_finish2_kernel<<<nq, 256, smem, ctx->stream>>>(a);
@@ -1285,3 +1343,425 @@ int stb_launch_batch_finish2(stb_ctx *ctx, const uint64_t *cand_keys, const uint
   return STB_OK;
 }
 
+// =========================================================================================
+// Route 7: pipeline v2 on the q8 copy and the int8 tensor cores, for corpora whose 16-bit shadow does not fit
+// in HBM.  Every row already has int8 codes x8 and a scale s there (K1's q8 tier, 260 B per row); the query is
+// quantised exactly as K1 quantises it (q8_query.cuh: q16 = rint(q^ S) = 256 hi + lo, two signed bytes).  Per
+// (query, row) the GEMM computes K1's integer dot = 256 (hi . x8) + lo . x8 (exact in int32) and from it K1's
+// bounds, bit for bit (scan_topk.cu: stb_scan_q8, stb_scan_q4):
+//     u = s (dot / S + h_l1) + e_q  >=  c - 1e-5        l = s (dot / S - h_l1) - e_q - 2e-5  <=  c - 1e-5
+// Sufficiency, as v2's with the two bounds in place of the one symmetric EPS: S_k = k-th largest sampled tile
+// maximum of l; each is a real row's l (rows past n are masked), so k distinct rows have c >= S_k and C_k >= S_k.
+// A row of the exact top-k has c >= min(C_k, 1) >= S_k (l < 1), so u >= S_k - 1e-5: emitting u >= thr = S_k -
+// STB_Q8_SCAN_EPS loses none.  The finish (stb_batch_finish2_kernel with the q8 arguments) drops emitted rows
+// that cannot win, re-scores the rest exactly and proves the query only if the k-th distance beats thr + eps.
+// =========================================================================================
+
+#define STB_Q8_B_SLAB_BYTES (STB_B_TILE * 128)            // 128 code bytes of 256 rows: 32 KiB
+#define STB_Q8_GEMM_SMEM (2 * STB_Q8_B_SLAB_BYTES + STB_A_RING * STB_A_SLAB_BYTES + 2 * STB_B_TILE * 4 + 256 + 1024)
+static_assert(STB_Q8_GEMM_SMEM <= 227 * 1024, "q8 GEMM shared memory");
+
+// 1. Query tiles.  One warp per query slot (all four lane groups compute the same query, as stb_q8_query's
+// reductions require); lane j < 8 writes its 16-byte chunk j of each of the tile's four K-slabs: hi bytes of
+// components 0-127, hi 128-255, lo 0-127, lo 128-255, each [128 queries x 128 B] in the 128-byte swizzle.
+// Padding slots (>= nq) are zero and flagged.
+__global__ void __launch_bounds__(256)
+stb_q8_query_tiles_kernel(const float *__restrict__ q, uint32_t nq, uint32_t q_pad, uint8_t *__restrict__ tiles,
+                          float4 *__restrict__ qc, uint32_t *__restrict__ q_bad, int16_t *__restrict__ q16) {
+  const int lane = threadIdx.x & 31, j = lane & 7;
+  const uint32_t qi = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (qi >= q_pad) return;                                  // warp-uniform
+  uint32_t hi[8] = {0, 0, 0, 0, 0, 0, 0, 0}, lo[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  float4 c = make_float4(0.f, 0.f, 0.f, 0.f);
+  bool bad = true;
+  if (qi < nq) {
+    const StbQ8Query Q = stb_q8_query(q + (size_t)qi * STB_D, j);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { hi[i] = Q.qhi[i]; lo[i] = Q.qlo[i]; }
+    c = make_float4(Q.inv_S, Q.h_l1, Q.e_q, Q.S);
+    bad = Q.unusable;
+  }
+  if (lane < 8) {
+    const uint32_t r = qi % STB_A_TILE;
+    uint8_t *t = tiles + (size_t)(qi / STB_A_TILE) * (4 * STB_A_SLAB_BYTES) + (r >> 3) * 1024 + (r & 7) * 128 +
+                 ((j ^ (r & 7)) * 16);
+    *reinterpret_cast<uint4 *>(t) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+    *reinterpret_cast<uint4 *>(t + STB_A_SLAB_BYTES) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
+    *reinterpret_cast<uint4 *>(t + 2 * STB_A_SLAB_BYTES) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+    *reinterpret_cast<uint4 *>(t + 3 * STB_A_SLAB_BYTES) = make_uint4(lo[4], lo[5], lo[6], lo[7]);
+    if (q16 && qi < nq) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int k = (i < 4 ? 16 * j + 4 * i : 128 + 16 * j + 4 * (i - 4)) + e;
+          q16[(size_t)qi * STB_D + k] = (int16_t)(256 * (int)(int8_t)(hi[i] >> (8 * e)) + (int)(int8_t)(lo[i] >> (8 * e)));
+        }
+    }
+  }
+  if (lane == 0) { qc[qi] = c; q_bad[qi] = bad ? 1u : 0u; }
+}
+
+int stb_launch_q8_query_tiles(stb_ctx *ctx, const float *q_dev, uint32_t nq, uint32_t q_pad, uint8_t *tiles, float4 *qc,
+                              uint32_t *q_bad, int16_t *q16) {
+  if (q_pad == 0) return STB_OK;
+  stb_q8_query_tiles_kernel<<<(q_pad + 7) / 8, 256, 0, ctx->stream>>>(q_dev, nq, q_pad, tiles, qc, q_bad, q16);
+  STB_CUDA(cudaGetLastError());
+  ctx->kernel_launches++;
+  return STB_OK;
+}
+
+// 2. The GEMM.  Corpus tile = 256 rows: two K-slabs of codes (bytes 0-127 and 128-255 of each row, 32 KiB each)
+// loaded with the tensor maps below, which apply the 128-byte swizzle on the way in (the q8 copy stays row-major
+// for K1 and zero-fills rows past n), and the tile's 256 scales (1 KiB) with slab 0, double-buffered by tile
+// parity: the producer refills buffer (it + 1) & 1 only after every consumer warp released slab 0 of tile it,
+// which it does after the epilogues of tile it - 1.  Query tiles stream through the 6-slab ring of
+// stb_batch_gemm_kernel.  Per (query tile, corpus tile) a consumer warpgroup runs the hi slabs (K = 256, 8
+// wgmma m64n256k32 s8), waits, multiplies its s32 accumulators by 256 and accumulates the lo slabs on top.
+__device__ __forceinline__ void wg_reg_fence_s32(int32_t (&d)[128]) {
+#pragma unroll
+  for (int i = 0; i < 128; ++i) asm volatile("" : "+r"(d[i])::"memory");
+}
+__device__ __forceinline__ void wg_mma_m64n256k32_s8(int32_t (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k32.s32.s8.s8 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p;\n\t}"
+      :
+        "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+        "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+        "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+        "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+        "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+        "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+        "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+        "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]),
+        "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]),
+        "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79]),
+        "+r"(d[80]), "+r"(d[81]), "+r"(d[82]), "+r"(d[83]), "+r"(d[84]), "+r"(d[85]), "+r"(d[86]), "+r"(d[87]),
+        "+r"(d[88]), "+r"(d[89]), "+r"(d[90]), "+r"(d[91]), "+r"(d[92]), "+r"(d[93]), "+r"(d[94]), "+r"(d[95]),
+        "+r"(d[96]), "+r"(d[97]), "+r"(d[98]), "+r"(d[99]), "+r"(d[100]), "+r"(d[101]), "+r"(d[102]), "+r"(d[103]),
+        "+r"(d[104]), "+r"(d[105]), "+r"(d[106]), "+r"(d[107]), "+r"(d[108]), "+r"(d[109]), "+r"(d[110]), "+r"(d[111]),
+        "+r"(d[112]), "+r"(d[113]), "+r"(d[114]), "+r"(d[115]), "+r"(d[116]), "+r"(d[117]), "+r"(d[118]), "+r"(d[119]),
+        "+r"(d[120]), "+r"(d[121]), "+r"(d[122]), "+r"(d[123]), "+r"(d[124]), "+r"(d[125]), "+r"(d[126]), "+r"(d[127])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+__device__ __forceinline__ void tma_load_2d(void *dst_smem, const CUtensorMap *map, int x, int y, uint64_t *bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
+          smem_u32(dst_smem)),
+      "l"(reinterpret_cast<uint64_t>(map)), "r"(x), "r"(y), "r"(smem_u32(bar))
+      : "memory");
+}
+__device__ __forceinline__ void tma_load_1d(void *dst_smem, const CUtensorMap *map, int x, uint64_t *bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.1d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2}], [%3];" ::"r"(
+          smem_u32(dst_smem)),
+      "l"(reinterpret_cast<uint64_t>(map)), "r"(x), "r"(smem_u32(bar))
+      : "memory");
+}
+
+struct Q8GemmArgs {
+  const uint8_t *a_tiles;     // m_tiles x 4 slabs x 16 KiB (stb_q8_query_tiles_kernel)
+  const float4 *qc;           // [q_pad] {1/S, h_l1, e_q, S}
+  uint32_t m_tiles;
+  uint32_t n_tiles;           // corpus tiles of this launch: tile t is corpus tile t * tile_stride
+  uint32_t tile_stride;
+  uint64_t n_rows;            // rows past n (the zero-filled tail of the last tile) never count
+  float *tilemax;             // EPI 0: [m_tiles][n_tiles][128] maximum of l per tile
+  const float *thr;           // EPI 1: [q_pad] emission thresholds on u ...
+  uint32_t *cand_cnt;         //        [q_pad][grid] counts (> cand_cap: overflow marker)
+  uint64_t *cand_keys;        //        [q_pad][grid][cand_cap] keys (u desc, local row)
+  uint32_t cand_cap;
+  int32_t *dot_out;           // EPI 2: [m_tiles * 128][n_tiles * 256] dot, u and l
+  float *u_out, *l_out;
+};
+
+// EPI 0: sampling (tile maxima of l); EPI 1: emit every row whose u reaches the query's threshold; EPI 2: debug
+template <int EPI>
+__global__ void __launch_bounds__(STB_GEMM_THREADS, 1)
+stb_batch_q8_gemm_kernel(const __grid_constant__ CUtensorMap codes_map, const __grid_constant__ CUtensorMap scale_map,
+                         const Q8GemmArgs args) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint8_t *sB = smem;                                          // 2 code slabs
+  uint8_t *sA = smem + 2 * STB_Q8_B_SLAB_BYTES;                // query ring
+  float *s_scale = reinterpret_cast<float *>(sA + STB_A_RING * STB_A_SLAB_BYTES);   // [2][256]
+  uint64_t *bars = reinterpret_cast<uint64_t *>(s_scale + 2 * STB_B_TILE);
+  uint64_t *b_full = bars + 0, *b_empty = bars + 2;
+  uint64_t *a_full = bars + 4, *a_empty = a_full + STB_A_RING;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < 2; ++i) { mbar_init(b_full + i, 1); mbar_init(b_empty + i, STB_GEMM_CONSUMER_WARPS); }
+    for (int i = 0; i < STB_A_RING; ++i) { mbar_init(a_full + i, 1); mbar_init(a_empty + i, STB_GEMM_CONSUMER_WARPS); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  const uint32_t my_tiles = (args.n_tiles > blockIdx.x) ? (args.n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+
+  if (warp < 4) {
+    // ===== producer (one thread) =====
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
+      uint32_t a_cnt = 0;
+      for (uint32_t it = 0; it < my_tiles; ++it) {
+        const int row0 = (int)((blockIdx.x + (uint64_t)it * gridDim.x) * args.tile_stride * STB_B_TILE);
+        for (int s = 0; s < 2; ++s) {
+          mbar_wait(b_empty + s, (it & 1) ^ 1);
+          if (s == 0) {
+            mbar_expect_tx(b_full, STB_Q8_B_SLAB_BYTES + STB_B_TILE * 4);
+            tma_load_1d(s_scale + (it & 1) * STB_B_TILE, &scale_map, row0, b_full);
+          } else {
+            mbar_expect_tx(b_full + s, STB_Q8_B_SLAB_BYTES);
+          }
+          tma_load_2d(sB + s * STB_Q8_B_SLAB_BYTES, &codes_map, s * 128, row0, b_full + s);
+        }
+        for (uint32_t m = 0; m < args.m_tiles; ++m) {
+          for (int s = 0; s < 4; ++s, ++a_cnt) {
+            const uint32_t slot = a_cnt % STB_A_RING;
+            mbar_wait(a_empty + slot, ((a_cnt / STB_A_RING) & 1) ^ 1);
+            mbar_expect_tx(a_full + slot, STB_A_SLAB_BYTES);
+            bulk_g2s(sA + slot * STB_A_SLAB_BYTES, args.a_tiles + ((size_t)m * 4 + s) * STB_A_SLAB_BYTES, STB_A_SLAB_BYTES,
+                     a_full + slot);
+          }
+        }
+      }
+    }
+    return;
+  }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  // ===== consumers (accumulator layout as in stb_batch_gemm_kernel) =====
+  const uint32_t half = (uint32_t)(warp >> 2) - 1u;
+  const uint32_t qrow = half * 64 + (warp & 3) * 16 + (lane >> 2);
+  const uint32_t quad = lane & 3;
+  int32_t d[128];
+#pragma unroll
+  for (int i = 0; i < 128; ++i) d[i] = 0;
+  uint32_t a_cnt = 0;
+  for (uint32_t it = 0; it < my_tiles; ++it) {
+    const uint64_t t = blockIdx.x + (uint64_t)it * gridDim.x;
+    const uint64_t row0 = t * args.tile_stride * STB_B_TILE;
+    const float *sc = s_scale + (it & 1) * STB_B_TILE;
+    for (uint32_t m = 0; m < args.m_tiles; ++m, a_cnt += 4) {
+      const uint32_t q0 = m * STB_A_TILE + qrow;
+      float4 qc[2];
+      [[maybe_unused]] float thr[2];
+      [[maybe_unused]] uint32_t cnt[2], cnt0[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        qc[h] = __ldg(args.qc + q0 + 8 * h);
+        if constexpr (EPI == 1) {
+          thr[h] = __ldg(args.thr + q0 + 8 * h);
+          cnt0[h] = args.cand_cnt[(size_t)(q0 + 8 * h) * gridDim.x + blockIdx.x];
+          cnt[h] = cnt0[h];
+        }
+      }
+      wg_reg_fence_s32(d);
+#pragma unroll
+      for (int s = 0; s < 4; ++s) {
+        const uint32_t slot = (a_cnt + s) % STB_A_RING;
+        if (m == 0 && s < 2) mbar_wait(b_full + s, it & 1);
+        mbar_wait(a_full + slot, ((a_cnt + s) / STB_A_RING) & 1);
+        if (s == 2) {
+          // the hi products are complete: dot = 256 hi.x8 + lo.x8 (|256 hi.x8| <= 256 * 127 * 127 * 256 < 2^31)
+          wg_wait<0>();
+          wg_reg_fence_s32(d);
+#pragma unroll
+          for (int i = 0; i < 128; ++i) d[i] *= 256;
+          wg_reg_fence_s32(d);
+        }
+        wg_fence();
+        const uint32_t a_addr = smem_u32(sA + slot * STB_A_SLAB_BYTES + half * (64 * 128));
+        const uint32_t b_addr = smem_u32(sB + (s & 1) * STB_Q8_B_SLAB_BYTES);
+#pragma unroll
+        for (int k = 0; k < 4; ++k)   // K by 32 bytes inside the swizzle atom
+          wg_mma_m64n256k32_s8(d, wg_desc_sw128(a_addr + k * 32), wg_desc_sw128(b_addr + k * 32), (uint32_t)((s | k) != 0));
+        wg_commit();
+        if (s > 0) {
+          wg_wait<1>();
+          if (lane == 0) {
+            mbar_arrive(a_empty + (a_cnt + s - 1) % STB_A_RING);
+            if (m + 1 == args.m_tiles && s == 3) mbar_arrive(b_empty);    // slab 0's lo pass has retired
+          }
+        }
+      }
+      wg_wait<0>();
+      wg_reg_fence_s32(d);
+      if (lane == 0) {
+        mbar_arrive(a_empty + (a_cnt + 3) % STB_A_RING);
+        if (m + 1 == args.m_tiles) mbar_arrive(b_empty + 1);
+      }
+
+      // d[16c + 4ii + 2h + e]: query qrow + 8h, tile column 32c + 8ii + 2quad + e
+      if constexpr (EPI == 0) {
+        const uint32_t n_real = args.n_rows > row0 + STB_B_TILE ? STB_B_TILE : (uint32_t)(args.n_rows > row0 ? args.n_rows - row0 : 0);
+        float tmx[2] = {-CUDART_INF_F, -CUDART_INF_F};
+#pragma unroll
+        for (int c = 0; c < STB_B_TILE / STB_SUB; ++c)
+#pragma unroll
+          for (int ii = 0; ii < 4; ++ii) {
+            const uint32_t col = c * STB_SUB + ii * 8 + quad * 2;
+            const float2 s2 = *reinterpret_cast<const float2 *>(sc + col);
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const bool real = col + e < n_real;
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const float l = fmaf(e ? s2.y : s2.x, fmaf((float)d[16 * c + 4 * ii + 2 * h + e], qc[h].x, -qc[h].y), -qc[h].z) -
+                                (float)STB_Q8_SCAN_EPS;
+                tmx[h] = fmaxf(tmx[h], real ? l : -CUDART_INF_F);
+              }
+            }
+          }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          tmx[h] = fmaxf(tmx[h], __shfl_xor_sync(0xffffffffu, tmx[h], 1));
+          tmx[h] = fmaxf(tmx[h], __shfl_xor_sync(0xffffffffu, tmx[h], 2));
+          if (quad == (uint32_t)h) args.tilemax[((size_t)m * args.n_tiles + t) * STB_A_TILE + qrow + 8 * h] = tmx[h];
+        }
+      } else if constexpr (EPI == 1) {
+        // as stb_batch_gemm_kernel's EPI 1: a private segment per (query, CTA), branch-free hit masks
+#pragma unroll
+        for (int c = 0; c < STB_B_TILE / STB_SUB; ++c) {
+          const uint64_t r0 = row0 + (uint64_t)c * STB_SUB;
+          float u[4][2][2];
+#pragma unroll
+          for (int ii = 0; ii < 4; ++ii) {
+            const float2 s2 = *reinterpret_cast<const float2 *>(sc + c * STB_SUB + ii * 8 + quad * 2);
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int e = 0; e < 2; ++e)
+                u[ii][h][e] = fmaf(e ? s2.y : s2.x, fmaf((float)d[16 * c + 4 * ii + 2 * h + e], qc[h].x, qc[h].y), qc[h].z);
+          }
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            uint32_t hit = 0u;
+#pragma unroll
+            for (int ii = 0; ii < 4; ++ii)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) hit |= (u[ii][h][e] >= thr[h] ? 1u : 0u) << (ii * 8 + quad * 2 + e);
+            hit |= __shfl_xor_sync(0xffffffffu, hit, 1);
+            hit |= __shfl_xor_sync(0xffffffffu, hit, 2);
+            if (r0 + 32 > args.n_rows) hit &= (r0 < args.n_rows) ? ((1u << (uint32_t)(args.n_rows - r0)) - 1u) : 0u;
+            uint64_t *seg = args.cand_keys + ((size_t)(q0 + 8 * h) * gridDim.x + blockIdx.x) * args.cand_cap;
+#pragma unroll
+            for (int ii = 0; ii < 4; ++ii)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const uint32_t b = ii * 8 + quad * 2 + e;
+                const uint32_t pos = cnt[h] + __popc(hit & ((1u << b) - 1u));
+                if (((hit >> b) & 1u) && pos < args.cand_cap) seg[pos] = stb_make_key(u[ii][h][e], (uint32_t)(r0 + b));
+              }
+            cnt[h] += __popc(hit);
+          }
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          if (quad == 0 && cnt[h] != cnt0[h]) args.cand_cnt[(size_t)(q0 + 8 * h) * gridDim.x + blockIdx.x] = cnt[h];
+      } else {
+        const size_t ld = (size_t)args.n_tiles * STB_B_TILE;
+#pragma unroll
+        for (int c = 0; c < STB_B_TILE / STB_SUB; ++c)
+#pragma unroll
+          for (int ii = 0; ii < 4; ++ii) {
+            const uint32_t col = c * STB_SUB + ii * 8 + quad * 2;
+            const float2 s2 = *reinterpret_cast<const float2 *>(sc + col);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const size_t o = (size_t)(q0 + 8 * h) * ld + row0 + col;
+              const int32_t d0 = d[16 * c + 4 * ii + 2 * h], d1 = d[16 * c + 4 * ii + 2 * h + 1];
+              *reinterpret_cast<int2 *>(args.dot_out + o) = make_int2(d0, d1);
+              *reinterpret_cast<float2 *>(args.u_out + o) =
+                  make_float2(fmaf(s2.x, fmaf((float)d0, qc[h].x, qc[h].y), qc[h].z), fmaf(s2.y, fmaf((float)d1, qc[h].x, qc[h].y), qc[h].z));
+              *reinterpret_cast<float2 *>(args.l_out + o) =
+                  make_float2(fmaf(s2.x, fmaf((float)d0, qc[h].x, -qc[h].y), -qc[h].z) - (float)STB_Q8_SCAN_EPS,
+                              fmaf(s2.y, fmaf((float)d1, qc[h].x, -qc[h].y), -qc[h].z) - (float)STB_Q8_SCAN_EPS);
+            }
+          }
+      }
+    }
+  }
+}
+
+// The q8 copy's tensor maps, encoded per launch (a map holds the buffer's address, which moves when the copy
+// grows): codes as [n_rows][256] u8 in [256 rows][128 B] boxes with the 128-byte swizzle, scales as [n_rows] f32
+// in 256-entry boxes.  Rows past n_rows read as zeros.  The driver's encoder is taken through the runtime, so the
+// library does not link libcuda.
+static int q8_tensor_maps(const uint8_t *codes, const float *scales, uint64_t n_rows, CUtensorMap *codes_map,
+                          CUtensorMap *scale_map) {
+  // looked up once per process (thread-safe initialisation of the local static); null if unavailable
+  static const PFN_cuTensorMapEncodeTiled_v12000 encode = []() -> PFN_cuTensorMapEncodeTiled_v12000 {
+    void *fn = nullptr;
+    cudaDriverEntryPointQueryResult qr;
+    const cudaError_t e = cudaGetDriverEntryPointByVersion("cuTensorMapEncodeTiled", &fn, 12000, cudaEnableDefault, &qr);
+    if (e != cudaSuccess) cudaGetLastError();
+    return (e == cudaSuccess && qr == cudaDriverEntryPointSuccess) ? reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fn) : nullptr;
+  }();
+  if (!encode) { stb_set_error("q8 GEMM: cuTensorMapEncodeTiled unavailable"); return STB_ERR_CUDA; }
+  const cuuint64_t cdim[2] = {256, n_rows}, cstride[1] = {256};
+  const cuuint32_t cbox[2] = {128, STB_B_TILE}, one[2] = {1, 1};
+  CUresult r = encode(codes_map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<uint8_t *>(codes), cdim, cstride, cbox, one,
+                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { stb_set_error("q8 GEMM: code tensor map (error %d)", (int)r); return STB_ERR_CUDA; }
+  const cuuint64_t sdim[1] = {n_rows}, sstride[1] = {4};
+  const cuuint32_t sbox[1] = {STB_B_TILE};
+  r = encode(scale_map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 1, const_cast<float *>(scales), sdim, sstride, sbox, one,
+             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { stb_set_error("q8 GEMM: scale tensor map (error %d)", (int)r); return STB_ERR_CUDA; }
+  return STB_OK;
+}
+
+template <int EPI>
+static int launch_q8_gemm(stb_ctx *ctx, const uint8_t *codes, const float *scales, const Q8GemmArgs &a) {
+  if (a.n_rows == 0 || a.n_rows > 0x7fffff00ull) { stb_set_error("q8 GEMM: %llu rows", (unsigned long long)a.n_rows); return STB_ERR_ARG; }
+  CUtensorMap cm, sm;
+  int rc = q8_tensor_maps(codes, scales, a.n_rows, &cm, &sm);
+  if (rc != STB_OK) return rc;
+  STB_ATTR_ONCE(ctx, EPI == 0 ? STB_ATTR_Q8GEMM0 : (EPI == 1 ? STB_ATTR_Q8GEMM1 : STB_ATTR_Q8GEMM2),
+                cudaFuncSetAttribute(stb_batch_q8_gemm_kernel<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, STB_Q8_GEMM_SMEM));
+  const unsigned grid = (unsigned)std::min<uint32_t>(a.n_tiles, (uint32_t)ctx->sm_count);   // = stb_batch_emit_grid
+  if (grid == 0) return STB_OK;
+  stb_batch_q8_gemm_kernel<EPI><<<grid, STB_GEMM_THREADS, STB_Q8_GEMM_SMEM, ctx->stream>>>(cm, sm, a);
+  STB_CUDA(cudaGetLastError());
+  ctx->kernel_launches++;
+  return STB_OK;
+}
+
+int stb_launch_batch_q8_gemm_sample(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
+                                    const uint8_t *codes, const float *scales, uint64_t n_rows, uint32_t n_sample,
+                                    uint32_t tile_stride, float *tilemax) {
+  Q8GemmArgs a{};
+  a.a_tiles = a_tiles; a.qc = qc; a.m_tiles = m_tiles; a.n_tiles = n_sample; a.tile_stride = tile_stride;
+  a.n_rows = n_rows; a.tilemax = tilemax;
+  return launch_q8_gemm<0>(ctx, codes, scales, a);
+}
+
+int stb_launch_batch_q8_gemm_emit(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
+                                  const uint8_t *codes, const float *scales, uint64_t n_rows, const float *thr,
+                                  uint32_t *cand_cnt, uint64_t *cand_keys, uint32_t cand_cap) {
+  Q8GemmArgs a{};
+  a.a_tiles = a_tiles; a.qc = qc; a.m_tiles = m_tiles; a.n_tiles = (uint32_t)((n_rows + STB_B_TILE - 1) / STB_B_TILE);
+  a.tile_stride = 1; a.n_rows = n_rows; a.thr = thr; a.cand_cnt = cand_cnt; a.cand_keys = cand_keys; a.cand_cap = cand_cap;
+  return launch_q8_gemm<1>(ctx, codes, scales, a);
+}
+
+int stb_launch_batch_q8_gemm_debug(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
+                                   const uint8_t *codes, const float *scales, uint64_t n_rows, int32_t *dot, float *u,
+                                   float *l) {
+  Q8GemmArgs a{};
+  a.a_tiles = a_tiles; a.qc = qc; a.m_tiles = m_tiles; a.n_tiles = (uint32_t)((n_rows + STB_B_TILE - 1) / STB_B_TILE);
+  a.tile_stride = 1; a.n_rows = n_rows; a.dot_out = dot; a.u_out = u; a.l_out = l;
+  return launch_q8_gemm<2>(ctx, codes, scales, a);
+}

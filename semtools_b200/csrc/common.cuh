@@ -178,6 +178,7 @@ struct stb_ctx {
   StbBuf<uint32_t> b_cnt;          // v2: [q_pad] emitted-candidate counters
   StbBuf<uint64_t> b_keys;        // v2: [q_pad][cand_cap] emitted keys
   StbBuf<uint32_t> b_qbad;        // [q_pad] 1: query could not be normalised
+  StbBuf<float4> b_q8c;          // route 7: [q_pad] {1/S, h_l1, e_q, S} of each query's q16
   // stb_search_batch_filtered: the clipped ranges (local [begin, end) u32 pairs), the listed tiles and the
   // eligible-row bitmap (8 words per shadow tile), all built from the same clipped ranges
   StbBuf<uint32_t> b_franges;
@@ -443,7 +444,8 @@ int stb_launch_batch_xchg(stb_ctx *ctx, const StbBatchXchgArgs &a, const stb_hit
 
 // opt-in to > 48 KiB dynamic shared memory (or another function attribute) once per context
 enum { STB_ATTR_GEMM0 = 0, STB_ATTR_GEMM1, STB_ATTR_MERGE, STB_ATTR_IVF_PROBE, STB_ATTR_IVF_V2, STB_ATTR_FINISH2,
-       STB_ATTR_IVF_BATCH, STB_ATTR_GEMM0F, STB_ATTR_GEMM1F, STB_ATTR_GEMM2, STB_ATTR_GEMM0W, STB_ATTR_GEMM1W };
+       STB_ATTR_IVF_BATCH, STB_ATTR_GEMM0F, STB_ATTR_GEMM1F, STB_ATTR_GEMM2, STB_ATTR_GEMM0W, STB_ATTR_GEMM1W,
+       STB_ATTR_Q8GEMM0, STB_ATTR_Q8GEMM1, STB_ATTR_Q8GEMM2, STB_ATTR_THRESH_BIG };
 #define STB_ATTR_ONCE(ctx, bit, call)                         \
   do {                                                        \
     if (!((ctx)->func_attr_mask & (1u << (bit)))) {           \
@@ -497,15 +499,36 @@ int stb_launch_batch_gemm_emit_work(stb_ctx *ctx, const uint8_t *a_tiles, const 
 int stb_launch_batch_slots_gather(stb_ctx *ctx, const float *rows, const uint32_t *slot_row, uint32_t n_slots, float *out);
 int stb_launch_batch_slots_prep(stb_ctx *ctx, const uint32_t *slot_row, const uint32_t *slot_bad, uint32_t n_slots,
                                 uint32_t *row_bad, float *tilemax, uint64_t n_tilemax);
+// thr[q] = k-th largest of query q's n_sample sampled maxima - slack (negative: the shadow's 2 STB_BATCH_EPS), -inf
+// when fewer than k were sampled, +inf for padding queries and where q_skip (may be null) is set
 int stb_launch_batch_thresh(stb_ctx *ctx, const float *tilemax, uint32_t n_sample, uint32_t nq,
-                            uint32_t q_pad, uint32_t top_k, float *thr);
+                            uint32_t q_pad, uint32_t top_k, float *thr, float slack = -1.0f,
+                            const uint32_t *q_skip = nullptr);
 // candidates live in per-(query, CTA) segments: keys [q_pad][n_seg][seg_cap], counts [q_pad][n_seg];
 // n_seg = stb_batch_emit_grid() = the grid the emitting GEMM runs with
 uint32_t stb_batch_emit_grid(const stb_ctx *ctx, uint32_t n_tiles);
 int stb_launch_batch_finish2(stb_ctx *ctx, const uint64_t *cand_keys, const uint32_t *cand_cnt, uint32_t n_seg,
                              uint32_t seg_cap, uint32_t nq, uint32_t top_k, const float *rows,
                              uint64_t n_rows, uint64_t row_base, const float *queries_dev,
-                             const uint32_t *q_bad, stb_hit *out_hits, uint32_t *out_status);
+                             const uint32_t *q_bad, stb_hit *out_hits, uint32_t *out_status,
+                             const float *q8_scale = nullptr, const float4 *q8_qc = nullptr,
+                             const float *thr = nullptr);
+// Route 7 (the q8 copy on the int8 tensor cores, batch_scan.cu): the query tiles -- hi / lo bytes of q16 in the
+// wgmma layout, m_tiles x 64 KiB -- with per-query {1/S, h_l1, e_q, S} and unusable flags (q16: [nq][256] or null);
+// the sampling pass (tile maxima of the lower bound l over tiles 0, stride, ... (n_sample of them)); the emitting
+// pass (every row whose upper bound u reaches thr, into the segments as stb_launch_batch_gemm_emit); and the
+// debug pass (dot, u and l of every (query, row) into [m_tiles * 128][ceil(n_rows / 256) * 256] matrices)
+int stb_launch_q8_query_tiles(stb_ctx *ctx, const float *q_dev, uint32_t nq, uint32_t q_pad, uint8_t *tiles,
+                              float4 *qc, uint32_t *q_bad, int16_t *q16);
+int stb_launch_batch_q8_gemm_sample(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
+                                    const uint8_t *codes, const float *scales, uint64_t n_rows, uint32_t n_sample,
+                                    uint32_t tile_stride, float *tilemax);
+int stb_launch_batch_q8_gemm_emit(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
+                                  const uint8_t *codes, const float *scales, uint64_t n_rows, const float *thr,
+                                  uint32_t *cand_cnt, uint64_t *cand_keys, uint32_t cand_cap);
+int stb_launch_batch_q8_gemm_debug(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
+                                   const uint8_t *codes, const float *scales, uint64_t n_rows, int32_t *dot, float *u,
+                                   float *l);
 void stb_batch_build_params(int *shadow_is_f16, double *eps);
 // threshold mode's re-emission: the emitting pass into exactly sized segments cand_keys[seg_off[i], seg_off[i+1])
 // (i = query * grid + CTA), cursors [q_pad][grid] zeroed
