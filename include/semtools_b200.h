@@ -325,6 +325,12 @@ int stb_search_batch_dev(stb_ctx *ctx, const stb_corpus *corpus, const float *q_
  * Pipeline v2 runs on the eligible rows only (its sample over the 256-row tiles that hold an eligible row,
  * ineligible scores masked out of both epilogues) when top_k <= 64 and the plan fits; K1 (stb_search)
  * answers every query it leaves unproven, and all queries otherwise.  Pipeline v1 is never used here.
+ * Where the 16-bit shadow does not fit in HBM, the same passes run on the q8 copy and the int8 tensor cores
+ * (route 8, as stb_search_batch's route 7, over the listed tiles) when top_k <= 64 and the q8 plan fits, whether or
+ * not v2's does.  The shadow is built only where v2's plan fits; where only the q8 plan fits, the call asks whether
+ * the shadow could be allocated with a trial allocation, released at once.  K1 answers
+ * the rest, and every query when the q8 copy cannot be used either.  The shadow's STB_ERR_NOMEM is never returned;
+ * a failure to reserve scratch is (STB_ERR_NOMEM, before anything is written).
  * The distance cap (strict; a NaN cap passes nothing) is applied to the sorted hits on the host. */
 int stb_search_batch_filtered(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t nq,
                               uint32_t top_k, int has_max, double max_distance,
@@ -351,7 +357,11 @@ int stb_search_batch_filtered(stb_ctx *ctx, const stb_corpus *corpus, const floa
  * are the mask slots a work item names; 64 bytes of mask words reach shared memory per item), the two passes'
  * work lists (16 bytes per (corpus tile, query tile) item, 4 per listed tile and per CTA), the queries in slot
  * order (1 KiB per slot, 64 slots per half), and the per-group sample, laid out [query tile][largest
- * n_sample][128 queries]. */
+ * n_sample][128 queries].
+ * Where the 16-bit shadow does not fit in HBM and a group fits either plan (the shadow is asked for as in
+ * stb_search_batch_filtered), route 9 runs instead: each group whose q8 plan fits runs route 8's passes
+ * (stb_search_batch_filtered) on its own queries, one group after another; K1 answers the rest, and every query
+ * when the q8 copy cannot be used either.  The shadow's STB_ERR_NOMEM is never returned. */
 int stb_search_batch_subsets(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t nq,
                              uint32_t top_k, int has_max, double max_distance,
                              const uint64_t *range_offsets, const uint64_t *row_ranges,
@@ -371,7 +381,11 @@ int stb_search_batch_subsets(stb_ctx *ctx, const stb_corpus *corpus, const float
  * (DESIGN §5) into 64 keys per (query, CTA); queries with an overflowed segment get one more pass into exactly
  * sized segments, as long as that pass's keys stay within STB_BATCH_THRESHOLD_RETRY_KEYS (128 MiB of keys);
  * then the exact canonical re-score.  stb_search answers the rest: queries that cannot be normalised, the zero
- * query, queries beyond the budget, and every query when the corpus holds rows that cannot be normalised. */
+ * query, queries beyond the budget, and every query when the corpus holds rows that cannot be normalised.
+ * Where the 16-bit shadow does not fit in HBM (route 10), the same two passes run on the q8 copy and the int8
+ * tensor cores, with thr = RD_f32(((1 - M) - 2e-5) - 1e-12) on K1's upper bounds; their band is wider, so more
+ * queries need the second pass or pass the budget and go to stb_search.  If the q8 copy cannot be used either,
+ * stb_search answers every query; the shadow's STB_ERR_NOMEM is never returned. */
 #define STB_BATCH_THRESHOLD_RETRY_KEYS (1ull << 24)
 /* Eligibility scratch of one stb_ivfpq_search_subsets launch (256 MiB): each distinct subset of a launch takes
  * ceil(rows / 32) + nlist words, and a launch holds as many subsets as fit (at least one). */
@@ -712,6 +726,10 @@ int stb_debug_batch_gemm(stb_ctx *ctx, const float *q, uint32_t nq, const float 
  * stb_search for every query the route leaves unproven. */
 int stb_debug_batch_q8(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t nq, uint32_t top_k,
                        stb_hit *out_hits, uint32_t *out_n);
+/* Test hook for K2's q8 routes: while on != 0, every K2 search call on ctx (stb_search_batch, its _dev form and the
+ * filtered, subsets and threshold calls) behaves as if the 16-bit shadow did not fit in HBM, so it takes its q8
+ * route (7, 8, 9 or 10).  It builds no shadow and leaves a built shadow's bytes as they are.  Off by default. */
+int stb_debug_batch_no_shadow(stb_ctx *ctx, int on);
 /* Test hook for K2's route 7: the query quantisation and the integer GEMM over the corpus's q8 copy (built or
  * extended first).  q16 receives [nq][256] the 16-bit query components, dot [nq][n] the int32 products with
  * the int8 codes, u and l [nq][n] the upper and lower bounds of the exact cosine computed from them. */
@@ -735,7 +753,7 @@ int stb_debug_ivfpq_batch_last(const stb_ivfpq *index, uint32_t i, uint32_t info
  * b, n_seg, seg_cap}; route 1 = v1, 2 = v2, 3 = filtered v2, 4 = a filtered call that launched nothing on the
  * tensor cores (K1 answered it, or nothing could be returned), 5 = threshold mode, 6 = one filter per query
  * group, 7 = v2 on the q8 copy and the int8 tensor cores (the shadow did not fit, or stb_debug_batch_q8),
- * 0 = none yet.  Slots 2-3 (a, b):
+ * 8-10 = below, 0 = none yet.  Slots 2-3 (a, b):
  *   routes 1-4, 7: n_sample, stride -- v2's sampled tiles (0, stride, 2*stride, ...; after route 3 they count
  *               listed tiles, the tiles holding an eligible row, in ascending order); 0 after routes 1 and 4
  *               and after a route 7 call whose batch did not fit its plan (n_seg and seg_cap are 0 then too);
@@ -743,8 +761,16 @@ int stb_debug_ivfpq_batch_last(const stb_ivfpq *index, uint32_t i, uint32_t info
  *   route 6:    the groups that ran on the tensor cores, and the queries stb_search answered.  After a route 6
  *               call that ran the tensor passes, thr and cand_cnt are in caller query order; a query those
  *               passes did not take has threshold +inf and zero counts.
+ *   routes 8-10: routes 3, 6 and 5 on the q8 copy (the shadow did not fit, or stb_debug_batch_no_shadow), with
+ *               the words of those routes; route 9 reports n_seg = seg_cap = 0.  A filtered call that launched
+ *               nothing on the tensor cores records route 4 whatever the reason: neither plan fits, the shadow fits
+ *               but its plan does not, its rows cannot be normalised, or the shadow does not fit and then the q8
+ *               plan does not fit or the q8 copy cannot be used.  A subsets call whose shadow does not fit records
+ *               route 9, with 0 groups when none ran on the tensor cores; a threshold call whose shadow does not
+ *               fit records route 10, with n_seg = 0 and every query answered by stb_search when the q8 copy
+ *               cannot be used.
  * n_seg and seg_cap are the emitting grid and the first pass's per-(query, CTA) key capacity, 0 after routes 1
- * and 4 and after a route 5 call that launched nothing.  After routes 2, 3 and a route 5 or 7 call that ran the
+ * and 4 and after a route 5 or 10 call that launched nothing.  After routes 2, 3 and a route 5, 7, 8 or 10 call that ran the
  * tensor pass, thr (may be NULL) receives the nq emission thresholds and cand_cnt (may be NULL) the raw
  * first-pass emission counts [nq][n_seg]; a count above seg_cap marks an overflowed segment. */
 int stb_debug_batch_last(stb_ctx *ctx, uint32_t info[6], float *thr, uint32_t *cand_cnt);

@@ -3,6 +3,7 @@ point, same names, same argument meaning.  Raises StbError on any negative
 status; never substitutes a CPU computation."""
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import os
 
@@ -30,7 +31,7 @@ SYMBOLS = [
     "stb_xchg_connect", "stb_xchg_connect_local", "stb_search_topk_xchg", "stb_search_xchg", "stb_search_many", "stb_xchg_create_batch", "stb_search_batch_xchg_dev", "stb_ivfpq_build",
     "stb_ivfpq_destroy", "stb_ivfpq_extend", "stb_ivfpq_stats", "stb_ivfpq_search", "stb_ivfpq_search_dev", "stb_hits_merge_dev", "stb_hits_merge_batch_dev", "stb_hits_merge", "stb_fnv1a64", "stb_line_id", "stb_line_ids",
     "stb_ctx_counters", "stb_debug_ticket_check", "stb_debug_q4_refined", "stb_debug_coscan_offsets", "stb_debug_batch_gemm", "stb_debug_batch_params",
-    "stb_debug_batch_last", "stb_debug_batch_q8", "stb_debug_batch_q8_gemm", "stb_debug_batch_q8_plan", "stb_debug_corpus_copy", "stb_debug_scan_scores", "stb_debug_q4_scan",
+    "stb_debug_batch_last", "stb_debug_batch_q8", "stb_debug_batch_no_shadow", "stb_debug_batch_q8_gemm", "stb_debug_batch_q8_plan", "stb_debug_corpus_copy", "stb_debug_scan_scores", "stb_debug_q4_scan",
     "stb_debug_ivfpq_export",
     "stb_ivfpq_search_batch", "stb_ivfpq_search_batch_dev", "stb_debug_ivfpq_batch_last",
     "stb_ivfpq_search_filtered", "stb_ivfpq_search_subsets", "stb_ivfpq_update", "stb_ivfpq_remove",
@@ -136,6 +137,7 @@ def lib() -> C.CDLL:
     L.stb_debug_batch_params.argtypes = [C.POINTER(C.c_int), C.POINTER(C.c_double)]
     L.stb_debug_batch_last.argtypes = [vp, vp, vp, vp]
     L.stb_debug_batch_q8.argtypes = [vp, vp, vp, u32, u32, vp, vp]
+    L.stb_debug_batch_no_shadow.argtypes = [vp, i32]
     L.stb_debug_batch_q8_gemm.argtypes = [vp, vp, vp, u32, vp, vp, vp, vp]
     L.stb_debug_batch_q8_plan.argtypes = [u32, u64, u32, vp]
     L.stb_debug_ivfpq_export.argtypes = [vp, vp, vp, vp, vp, vp, vp]
@@ -248,21 +250,34 @@ class Context:
     def batch_last(self):
         """stb_debug_batch_last: the most recent K2 device call on this context.  Returns a dict with
         route (1 = v1, 2 = v2, 3 = filtered v2, 4 = filtered without the tensor cores, 5 = threshold mode, 6 = one
-        filter per query group, 7 = v2 on the q8 copy), nq, n_sample, stride (routes 1-4, 7) or retried, k1 (route 5: queries re-emitted by the
-        second tensor pass / answered by stb_search) or groups, k1 (route 6: groups on the tensor cores / queries
-        answered by stb_search), n_seg, seg_cap and, after v2 (filtered or not) and a route 5, 6 or 7 call that ran the
-        tensor passes, thr [nq] (f32) and cand_cnt [nq][n_seg] (raw counts; > seg_cap marks an overflowed segment;
-        route 6: caller order, +inf and zeros for a query the tensor passes did not take)."""
+        filter per query group, 7 = v2 on the q8 copy, 8 = filtered v2 on the q8 copy, 9 = one filter per query group
+        on the q8 copy, 10 = threshold mode on the q8 copy), nq, n_sample, stride (routes 1-4, 7, 8) or retried, k1
+        (routes 5, 10: queries re-emitted by the second tensor pass / answered by stb_search) or groups, k1 (routes 6,
+        9: groups on the tensor cores / queries answered by stb_search), n_seg, seg_cap and, after v2 (filtered or
+        not) and a route 5, 6, 7, 8 or 10 call that ran the tensor passes, thr [nq] (f32) and cand_cnt [nq][n_seg]
+        (raw counts; > seg_cap marks an overflowed segment; route 6: caller order, +inf and zeros for a query the
+        tensor passes did not take)."""
         info = np.zeros(6, dtype=np.uint32)
         _check(lib().stb_debug_batch_last(self._h, _np_ptr(info), None, None))
-        names = {5: ("retried", "k1"), 6: ("groups", "k1")}.get(int(info[0]), ("n_sample", "stride"))
+        names = {5: ("retried", "k1"), 6: ("groups", "k1"), 9: ("groups", "k1"), 10: ("retried", "k1")}.get(
+            int(info[0]), ("n_sample", "stride"))
         out = dict(zip(("route", "nq") + names + ("n_seg", "seg_cap"), (int(v) for v in info)))
-        if out["route"] in (2, 3) or (out["route"] in (5, 6, 7) and out["n_seg"]):
+        if out["route"] in (2, 3) or (out["route"] in (5, 6, 7, 8, 10) and out["n_seg"]):
             thr = np.zeros(max(out["nq"], 1), dtype=np.float32)
             cnt = np.zeros((max(out["nq"], 1), max(out["n_seg"], 1)), dtype=np.uint32)
             _check(lib().stb_debug_batch_last(self._h, _np_ptr(info), _np_ptr(thr), _np_ptr(cnt)))
             out["thr"], out["cand_cnt"] = thr[: out["nq"]], cnt[: out["nq"]]
         return out
+
+    @contextlib.contextmanager
+    def batch_no_shadow(self):
+        """stb_debug_batch_no_shadow: within the block, every K2 search on this context behaves as if the 16-bit
+        shadow did not fit in HBM and takes its q8 route (7-10); no shadow is built or changed."""
+        _check(lib().stb_debug_batch_no_shadow(self._h, 1))
+        try:
+            yield self
+        finally:
+            _check(lib().stb_debug_batch_no_shadow(self._h, 0))
 
     # -- K4 ------------------------------------------------------------------
     def hits_merge(self, lists: np.ndarray, top_k: int) -> np.ndarray:

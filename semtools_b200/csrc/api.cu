@@ -1037,17 +1037,23 @@ static int host_rows_staged(stb_corpus *c, uint64_t first, F &&fn) {
 }
 extern "C" {
 
+// The bytes corpus_ensure_shadow allocates to cover every row (0: the shadow it holds already has room)
+static uint64_t shadow_grow_bytes(const stb_corpus *c) {
+  const uint64_t tiles = (c->n + 255) / 256;
+  if (c->shadow && tiles * 131072ull <= c->shadow.cap) return 0;
+  return std::max<uint64_t>(tiles, (c->capacity + 255) / 256) * 131072ull;
+}
+
 static int corpus_ensure_shadow(stb_ctx *ctx, stb_corpus *c) {
   if (c->shadow && c->shadow_rows == c->n) {
     if (c->shadow_bad) { stb_set_error("search_batch: corpus holds rows whose norm is not a normal fp32 number; use stb_search"); return STB_ERR_STATE; }
     return STB_OK;
   }
-  const uint64_t tiles = (c->n + 255) / 256;
   uint64_t first = (c->shadow && c->shadow_rows < c->n && !c->shadow_bad) ? (c->shadow_rows / 256) * 256 : 0;   // valid prefix, whole tiles
   int rc;
-  if (tiles * 131072ull > c->shadow.cap || !c->shadow) {
+  if (const uint64_t bytes = shadow_grow_bytes(c)) {
     StbBuf<uint8_t> grown;
-    if ((rc = grown.alloc(std::max<uint64_t>(tiles, (c->capacity + 255) / 256) * 131072ull)) != STB_OK ||
+    if ((rc = grown.alloc(bytes)) != STB_OK ||
         (rc = copy_prefix(ctx, grown, c->shadow, (first / 256) * 131072ull)) != STB_OK)
       return rc;
     c->shadow = std::move(grown);
@@ -1355,14 +1361,39 @@ int stb_corpus_prepare_batch(stb_corpus *corpus) {
 }  // extern "C"
 
 // ---- K2 host calls -------------------------------------------------------------------------------------------
-// The record of the last K2 call, which stb_debug_batch_last returns: route, nq, two route words (routes 1-4
-// and 7: n_sample, stride; 5: retried queries, K1 queries; 6: tensor groups, K1 queries), n_seg, seg_cap.
+// The record of the last K2 call, which stb_debug_batch_last returns: route, nq, two route words (routes 1-4,
+// 7 and 8: n_sample, stride; 5 and 10: retried queries, K1 queries; 6 and 9: tensor groups, K1 queries), n_seg,
+// seg_cap.  Routes 7-10 are 2, 3, 6 and 5 on the q8 copy, for corpora whose shadow does not fit.
 enum K2Route : uint32_t { kRouteV1 = 1, kRouteV2 = 2, kRouteFiltered = 3, kRouteFilteredK1 = 4, kRouteThreshold = 5,
-                          kRouteSubsets = 6, kRouteQ8 = 7 };
+                          kRouteSubsets = 6, kRouteQ8 = 7, kRouteFilteredQ8 = 8, kRouteSubsetsQ8 = 9,
+                          kRouteThresholdQ8 = 10 };
 static void k2_record(stb_ctx *ctx, K2Route route, uint32_t nq, uint32_t a = 0, uint32_t b = 0, uint32_t n_seg = 0,
                       uint32_t seg_cap = 0) {
   const uint32_t words[6] = {route, nq, a, b, n_seg, seg_cap};
   memcpy(ctx->b_last, words, sizeof(words));
+}
+
+// The shadow as every K2 search call sees it.  batch_shadow is corpus_ensure_shadow, for a call that then reads the
+// shadow.  batch_shadow_fits is for a call whose shadow plan does not fit but whose q8 plan does: it would not read
+// the shadow, so none is built; it asks only whether corpus_ensure_shadow could allocate it (STB_ERR_NOMEM if not),
+// with a trial allocation of the same size, released at once.  STB_ERR_NOMEM is the trigger of the q8 routes.
+// While stb_debug_batch_no_shadow is on, both return STB_ERR_NOMEM without building or touching the shadow.
+static int batch_no_shadow_hook(const stb_ctx *ctx) {
+  if (!ctx->b_no_shadow) return STB_OK;
+  stb_set_error("search_batch: the 16-bit shadow is off on this context (stb_debug_batch_no_shadow)");
+  return STB_ERR_NOMEM;
+}
+static int batch_shadow(stb_ctx *ctx, stb_corpus *c) {
+  const int rc = batch_no_shadow_hook(ctx);
+  return rc != STB_OK ? rc : corpus_ensure_shadow(ctx, c);
+}
+static int batch_shadow_fits(stb_ctx *ctx, const stb_corpus *c) {
+  const int rc = batch_no_shadow_hook(ctx);
+  if (rc != STB_OK) return rc;
+  const uint64_t bytes = shadow_grow_bytes(c);
+  if (bytes == 0) return STB_OK;
+  StbBuf<uint8_t> trial;
+  return trial.alloc(bytes);
 }
 
 // Keys per (query, CTA) segment of the emitting pass of v2 and route 6: ~5 expected at 10M rows / 132 CTAs.
@@ -1453,17 +1484,59 @@ static BatchV2Plan batch_q8_plan(uint32_t sm, uint32_t n_cover, uint32_t top_k) 
   return {n_sample, fits ? n_cover / n_sample : 0u, fits};
 }
 
-// Route 7 (batch_scan.cu): q8 query tiles -> sampled threshold on the lower bounds -> upper-bound-emitting int8
-// wgmma epilogue -> the finish with the q8 proof.  Builds or extends the q8 copy first (its status is returned
-// if it cannot be used).  A batch that does not fit the plan comes back with every query unproven.
+// The tensor passes of routes 7 and 8 (batch_scan.cu) on a built q8 copy: q8 query tiles -> sampled threshold on
+// the lower bounds -> upper-bound-emitting int8 wgmma epilogue -> the finish with the q8 proof.  Unfiltered
+// (tile_ids == NULL, route 7) over the corpus tiles 0 .. n_cover-1; filtered (route 8) over the n_cover listed
+// tiles tile_ids[] with the eligible-row bitmap.  p must fit.
+static int batch_q8_passes(stb_ctx *ctx, stb_corpus *corpus, const float *q_dev, uint32_t nq, uint32_t top_k,
+                           uint32_t n_cover, BatchV2Plan p, const uint32_t *tile_ids, const uint32_t *bitmap,
+                           stb_hit *out_hits_dev, uint32_t *out_status_dev) {
+  int rc;
+  const uint32_t m_tiles = (nq + 127) / 128, q_pad = m_tiles * 128;
+  const uint32_t n_seg = stb_batch_emit_grid(ctx, n_cover);
+  // every buffer first: a call refused for lack of memory leaves the record as it was
+  if ((rc = ctx->b_qbad.reserve((size_t)q_pad)) != STB_OK) return rc;
+  if ((rc = ctx->b_q8c.reserve((size_t)q_pad)) != STB_OK) return rc;
+  if ((rc = ctx->bq_tiles.reserve((size_t)q_pad * 512)) != STB_OK) return rc;
+  if ((rc = ctx->b_tilemax.reserve((size_t)p.n_sample * q_pad)) != STB_OK) return rc;
+  if ((rc = ctx->b_thr.reserve((size_t)q_pad)) != STB_OK) return rc;
+  if ((rc = ctx->b_cnt.reserve((size_t)q_pad * n_seg)) != STB_OK) return rc;
+  if ((rc = ctx->b_keys.reserve((size_t)q_pad * n_seg * kSegCap)) != STB_OK) return rc;
+  k2_record(ctx, tile_ids ? kRouteFilteredQ8 : kRouteQ8, nq, p.n_sample, p.stride, n_seg, kSegCap);
+  STB_CUDA(cudaMemsetAsync(ctx->b_cnt, 0, (size_t)q_pad * n_seg * sizeof(uint32_t), ctx->stream));
+  if ((rc = stb_launch_q8_query_tiles(ctx, q_dev, nq, q_pad, ctx->bq_tiles, ctx->b_q8c, ctx->b_qbad, nullptr)) != STB_OK)
+    return rc;
+  if (tile_ids)
+    rc = stb_launch_batch_q8_gemm_sample_filtered(ctx, ctx->bq_tiles, ctx->b_q8c, m_tiles, corpus->q8, corpus->q8_scale,
+                                                  corpus->n, tile_ids, bitmap, p.n_sample, p.stride, ctx->b_tilemax);
+  else
+    rc = stb_launch_batch_q8_gemm_sample(ctx, ctx->bq_tiles, ctx->b_q8c, m_tiles, corpus->q8, corpus->q8_scale, corpus->n,
+                                         p.n_sample, p.stride, ctx->b_tilemax);
+  if (rc != STB_OK) return rc;
+  // an unusable query (zero, or not normalisable) emits nothing and comes back unproven
+  if ((rc = stb_launch_batch_thresh(ctx, ctx->b_tilemax, p.n_sample, nq, q_pad, top_k, ctx->b_thr, (float)STB_Q8_SCAN_EPS,
+                                    ctx->b_qbad)) != STB_OK) return rc;
+  if (tile_ids)
+    rc = stb_launch_batch_q8_gemm_emit_filtered(ctx, ctx->bq_tiles, ctx->b_q8c, m_tiles, corpus->q8, corpus->q8_scale,
+                                                corpus->n, tile_ids, bitmap, n_cover, ctx->b_thr, ctx->b_cnt, ctx->b_keys,
+                                                kSegCap);
+  else
+    rc = stb_launch_batch_q8_gemm_emit(ctx, ctx->bq_tiles, ctx->b_q8c, m_tiles, corpus->q8, corpus->q8_scale, corpus->n,
+                                       ctx->b_thr, ctx->b_cnt, ctx->b_keys, kSegCap);
+  if (rc != STB_OK) return rc;
+  return stb_launch_batch_finish2(ctx, ctx->b_keys, ctx->b_cnt, n_seg, kSegCap, nq, top_k, corpus->rows, corpus->n,
+                                  corpus->row_base, q_dev, ctx->b_qbad, out_hits_dev, out_status_dev, corpus->q8_scale,
+                                  ctx->b_q8c, ctx->b_thr);
+}
+
+// Route 7: builds or extends the q8 copy first (its status is returned if it cannot be used), then runs
+// batch_q8_passes over every corpus tile.  A batch that does not fit the plan comes back with every query unproven.
 static int batch_q8_run(stb_ctx *ctx, stb_corpus *corpus, const float *q_dev, uint32_t nq, uint32_t top_k,
                         stb_hit *out_hits_dev, uint32_t *out_status_dev) {
   int rc;
   if ((rc = corpus_ensure_q8(ctx, corpus)) != STB_OK) return rc;
-  const uint32_t m_tiles = (nq + 127) / 128, q_pad = m_tiles * 128;
   const uint32_t n_tiles = (uint32_t)((corpus->n + 255) / 256);
   const BatchV2Plan p = batch_q8_plan((uint32_t)ctx->sm_count, n_tiles, top_k);
-  const uint32_t n_seg = stb_batch_emit_grid(ctx, n_tiles);
   if (!p.fits) {
     std::vector<stb_hit> pad((size_t)nq * top_k);
     stb_pad_hits(pad.data(), 0, pad.size());
@@ -1473,28 +1546,7 @@ static int batch_q8_run(stb_ctx *ctx, stb_corpus *corpus, const float *q_dev, ui
     k2_record(ctx, kRouteQ8, nq);
     return STB_OK;
   }
-  // every buffer first: a call refused for lack of memory leaves the record as it was
-  if ((rc = ctx->b_qbad.reserve((size_t)q_pad)) != STB_OK) return rc;
-  if ((rc = ctx->b_q8c.reserve((size_t)q_pad)) != STB_OK) return rc;
-  if ((rc = ctx->bq_tiles.reserve((size_t)q_pad * 512)) != STB_OK) return rc;
-  if ((rc = ctx->b_tilemax.reserve((size_t)p.n_sample * q_pad)) != STB_OK) return rc;
-  if ((rc = ctx->b_thr.reserve((size_t)q_pad)) != STB_OK) return rc;
-  if ((rc = ctx->b_cnt.reserve((size_t)q_pad * n_seg)) != STB_OK) return rc;
-  if ((rc = ctx->b_keys.reserve((size_t)q_pad * n_seg * kSegCap)) != STB_OK) return rc;
-  k2_record(ctx, kRouteQ8, nq, p.n_sample, p.stride, n_seg, kSegCap);
-  STB_CUDA(cudaMemsetAsync(ctx->b_cnt, 0, (size_t)q_pad * n_seg * sizeof(uint32_t), ctx->stream));
-  if ((rc = stb_launch_q8_query_tiles(ctx, q_dev, nq, q_pad, ctx->bq_tiles, ctx->b_q8c, ctx->b_qbad, nullptr)) != STB_OK ||
-      (rc = stb_launch_batch_q8_gemm_sample(ctx, ctx->bq_tiles, ctx->b_q8c, m_tiles, corpus->q8, corpus->q8_scale, corpus->n,
-                                            p.n_sample, p.stride, ctx->b_tilemax)) != STB_OK ||
-      // an unusable query (zero, or not normalisable) emits nothing and comes back unproven
-      (rc = stb_launch_batch_thresh(ctx, ctx->b_tilemax, p.n_sample, nq, q_pad, top_k, ctx->b_thr, (float)STB_Q8_SCAN_EPS,
-                                    ctx->b_qbad)) != STB_OK ||
-      (rc = stb_launch_batch_q8_gemm_emit(ctx, ctx->bq_tiles, ctx->b_q8c, m_tiles, corpus->q8, corpus->q8_scale, corpus->n,
-                                          ctx->b_thr, ctx->b_cnt, ctx->b_keys, kSegCap)) != STB_OK)
-    return rc;
-  return stb_launch_batch_finish2(ctx, ctx->b_keys, ctx->b_cnt, n_seg, kSegCap, nq, top_k, corpus->rows, corpus->n,
-                                  corpus->row_base, q_dev, ctx->b_qbad, out_hits_dev, out_status_dev, corpus->q8_scale,
-                                  ctx->b_q8c, ctx->b_thr);
+  return batch_q8_passes(ctx, corpus, q_dev, nq, top_k, n_tiles, p, nullptr, nullptr, out_hits_dev, out_status_dev);
 }
 
 // The listed tiles of clipped local [begin, end) pairs: the shadow tiles a range touches (ascending, disjoint
@@ -1545,11 +1597,44 @@ static int k2_complete(stb_ctx *ctx, const stb_corpus *corpus, const float *q, u
   return STB_OK;
 }
 
+// The filtered tensor passes for nq host queries over `loc` (clipped local [begin, end) pairs) and its listed tiles:
+// filtered v2 on the shadow (route 3), or, q8, route 7's passes on the q8 copy over the listed tiles (route 8);
+// `plan` (v2's or the q8 plan, over the listed tiles) must fit.  Hits land in out_hits [nq][top_k], {hits, proven}
+// in status [nq][2].
+static int filtered_tensor_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, uint32_t nq, uint32_t top_k,
+                               const std::vector<uint32_t> &loc, const std::vector<uint32_t> &tiles, BatchV2Plan plan,
+                               bool q8, stb_hit *out_hits, uint32_t *status) {
+  int rc;
+  const uint64_t n_words = (corpus->n + 255) / 256 * 8;
+  if ((rc = ctx->bq_dev.reserve((size_t)nq * STB_D)) != STB_OK) return rc;
+  if ((rc = ctx->bh_dev.reserve((size_t)nq * top_k)) != STB_OK) return rc;
+  if ((rc = ctx->bs_dev.reserve((size_t)nq * 2)) != STB_OK) return rc;
+  if ((rc = ctx->b_franges.reserve(loc.size(), 2048)) != STB_OK) return rc;
+  if ((rc = ctx->b_ftiles.reserve(tiles.size(), 1024)) != STB_OK) return rc;
+  if ((rc = ctx->b_fbits.reserve((size_t)n_words)) != STB_OK) return rc;
+  STB_CUDA(cudaMemcpyAsync(ctx->bq_dev, q, (size_t)nq * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+  STB_CUDA(cudaMemcpyAsync(ctx->b_franges, loc.data(), loc.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+  STB_CUDA(cudaMemcpyAsync(ctx->b_ftiles, tiles.data(), tiles.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+  if ((rc = stb_launch_row_bitmap(ctx, ctx->b_franges, (uint32_t)(loc.size() / 2), n_words, ctx->b_fbits)) != STB_OK) return rc;
+  const uint32_t n_listed = (uint32_t)tiles.size();
+  if (q8)
+    rc = batch_q8_passes(ctx, corpus, ctx->bq_dev, nq, top_k, n_listed, plan, ctx->b_ftiles, ctx->b_fbits, ctx->bh_dev, ctx->bs_dev);
+  else
+    rc = batch_v2_run(ctx, corpus, ctx->bq_dev, nq, top_k, n_listed, plan, ctx->b_ftiles, ctx->b_fbits, ctx->bh_dev, ctx->bs_dev);
+  if (rc != STB_OK) return rc;
+  STB_CUDA(cudaMemcpyAsync(out_hits, ctx->bh_dev, (size_t)nq * top_k * sizeof(stb_hit), cudaMemcpyDeviceToHost, ctx->stream));
+  STB_CUDA(cudaMemcpyAsync(status, ctx->bs_dev, (size_t)nq * 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  STB_CUDA(cudaStreamSynchronize(ctx->stream));        // `loc` and `tiles` are read by the copies above
+  return STB_OK;
+}
+
 // The store query (stb_search in STB_MODE_STORE_QUERY) for a batch, over `loc`: the caller's row_ranges clipped
 // to local [begin, end) pairs (K1 answers with the former).  The eligible rows' bitmap and the listed tiles both
-// come from `loc`; filtered v2 runs when its plan fits over the listed tiles, and K1 answers every query it leaves
-// unproven (or all of them, route 4).  The cap is applied on the host: store-query hits are a prefix of the
-// uncapped top-k.
+// come from `loc`; filtered v2 runs when its plan fits over the listed tiles (route 3).  Where the shadow does not
+// fit, route 8 runs the same passes on the q8 copy when the q8 plan fits over the listed tiles, whether or not v2's
+// does (the shadow is asked for whenever either plan fits, and built only where v2's fits).  K1 answers every query
+// the tensor passes leave unproven, and all of them when nothing runs on the tensor cores (route 4).  The cap is
+// applied on the host: store-query hits are a prefix of the uncapped top-k.
 static int batch_filtered_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, uint32_t nq, uint32_t top_k, int has_max,
                               double max_distance, const std::vector<uint32_t> &loc, const uint64_t *row_ranges,
                               uint32_t n_ranges, stb_hit *out_hits, uint32_t *out_n) {
@@ -1560,32 +1645,21 @@ static int batch_filtered_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, 
                        [](uint32_t) { return K2Answer{K2Answer::kEmpty}; }, out_hits, out_n);
   const std::vector<uint32_t> tiles = listed_tiles(loc);
   const uint32_t n_listed = (uint32_t)tiles.size();
-  const BatchV2Plan plan = batch_v2_plan(ctx, n_listed, top_k);
-  bool tensor_ok = plan.fits;
-  if (tensor_ok) {
-    rc = corpus_ensure_shadow(ctx, corpus);
-    if (rc == STB_ERR_STATE) tensor_ok = false;          // un-normalisable rows: K1 handles them
-    else if (rc != STB_OK) return rc;
+  BatchV2Plan plan = batch_v2_plan(ctx, n_listed, top_k);
+  const BatchV2Plan q8_plan = batch_q8_plan((uint32_t)ctx->sm_count, n_listed, top_k);
+  bool tensor_ok = false, q8 = false;
+  if (plan.fits || q8_plan.fits) {
+    rc = plan.fits ? batch_shadow(ctx, corpus) : batch_shadow_fits(ctx, corpus);
+    if (rc == STB_OK) tensor_ok = plan.fits;              // the shadow fits but not its plan: K1 answers all, as before
+    else if (rc == STB_ERR_NOMEM) {
+      // the shadow does not fit: route 8, if its plan fits and the q8 copy can be used (else K1 answers all)
+      if (q8_plan.fits && (rc = corpus_ensure_q8(ctx, corpus)) == STB_OK) { tensor_ok = q8 = true; plan = q8_plan; }
+      else if (q8_plan.fits && rc != STB_ERR_NOMEM && rc != STB_ERR_STATE) return rc;
+    } else if (rc != STB_ERR_STATE) return rc;            // STB_ERR_STATE: un-normalisable rows, K1 handles them
   }
   std::vector<uint32_t> status((size_t)nq * 2, 0);
-  if (tensor_ok) {
-    const uint64_t n_words = (corpus->n + 255) / 256 * 8;
-    if ((rc = ctx->bq_dev.reserve((size_t)nq * STB_D)) != STB_OK) return rc;
-    if ((rc = ctx->bh_dev.reserve((size_t)nq * top_k)) != STB_OK) return rc;
-    if ((rc = ctx->bs_dev.reserve((size_t)nq * 2)) != STB_OK) return rc;
-    if ((rc = ctx->b_franges.reserve(loc.size(), 2048)) != STB_OK) return rc;
-    if ((rc = ctx->b_ftiles.reserve(tiles.size(), 1024)) != STB_OK) return rc;
-    if ((rc = ctx->b_fbits.reserve((size_t)n_words)) != STB_OK) return rc;
-    STB_CUDA(cudaMemcpyAsync(ctx->bq_dev, q, (size_t)nq * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-    STB_CUDA(cudaMemcpyAsync(ctx->b_franges, loc.data(), loc.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-    STB_CUDA(cudaMemcpyAsync(ctx->b_ftiles, tiles.data(), tiles.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-    if ((rc = stb_launch_row_bitmap(ctx, ctx->b_franges, (uint32_t)(loc.size() / 2), n_words, ctx->b_fbits)) != STB_OK) return rc;
-    if ((rc = batch_v2_run(ctx, corpus, ctx->bq_dev, nq, top_k, n_listed, plan, ctx->b_ftiles, ctx->b_fbits, ctx->bh_dev,
-                           ctx->bs_dev)) != STB_OK) return rc;
-    STB_CUDA(cudaMemcpyAsync(out_hits, ctx->bh_dev, (size_t)nq * top_k * sizeof(stb_hit), cudaMemcpyDeviceToHost, ctx->stream));
-    STB_CUDA(cudaMemcpyAsync(status.data(), ctx->bs_dev, (size_t)nq * 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    STB_CUDA(cudaStreamSynchronize(ctx->stream));        // `loc` and `tiles` are read by the copies above
-  }
+  if (tensor_ok && (rc = filtered_tensor_run(ctx, corpus, q, nq, top_k, loc, tiles, plan, q8, out_hits, status.data())) != STB_OK)
+    return rc;
   return k2_complete(ctx, corpus, q, nq, top_k, has_max, max_distance, STB_MODE_STORE_QUERY, [&](uint32_t i) -> K2Answer {
     if (tensor_ok && status[2 * i + 1]) return {K2Answer::kProven, out_hits + (size_t)i * top_k, status[2 * i]};
     return {K2Answer::kK1, nullptr, 0, row_ranges, n_ranges};
@@ -1608,7 +1682,7 @@ static int batch_dev_impl(stb_ctx *ctx, const stb_corpus *corpus_c, const float 
   if (top_k == 0 || top_k > 1024) { stb_set_error("search_batch_dev: top_k must be 1..1024"); return STB_ERR_ARG; }
   if (corpus->n == 0) { stb_set_error("search_batch_dev: empty corpus"); return STB_ERR_STATE; }
   if (q8_route) return batch_q8_run(ctx, corpus, q_dev, nq, top_k, out_hits_dev, out_status_dev);
-  if ((rc = corpus_ensure_shadow(ctx, corpus)) != STB_OK) {
+  if ((rc = batch_shadow(ctx, corpus)) != STB_OK) {
     if (rc != STB_ERR_NOMEM) return rc;
     // the shadow does not fit in HBM: route 7 reads the q8 copy instead.  If that copy cannot be used either, the
     // call is refused as before, with the shadow's status and message and nothing written
@@ -1778,6 +1852,66 @@ static void subsets_work(const std::vector<std::vector<uint32_t>> &tiles_of, con
   while (w->cta_tiles.size() <= grid) w->cta_tiles.push_back(n_union);
 }
 
+// Route 9: stb_search_batch_subsets where the shadow does not fit, with several groups (group[i]: query i's group
+// in `lists`, or kNone for a query with no clipped range; listed[g]: group g's listed tiles).  Each group whose q8
+// plan fits over its listed tiles runs route 8's passes on its own queries, one group after another; K1 answers the
+// other groups (all of them when the q8 copy cannot be used) and every query the passes leave unproven.
+static int subsets_q8_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, uint32_t nq, uint32_t top_k, int has_max,
+                          double max_distance, const std::vector<uint32_t> &group,
+                          const std::vector<const std::vector<uint32_t> *> &lists,
+                          const std::vector<std::vector<uint32_t>> &listed, const uint64_t *range_offsets,
+                          const uint64_t *row_ranges, stb_hit *out_hits, uint32_t *out_n) {
+  constexpr uint32_t kNone = 0xffffffffu;
+  int rc;
+  k2_record(ctx, kRouteSubsetsQ8, nq);
+  const uint32_t G = (uint32_t)lists.size();
+  std::vector<std::vector<uint32_t>> members(G);
+  for (uint32_t i = 0; i < nq; ++i)
+    if (group[i] != kNone) members[group[i]].push_back(i);
+  std::vector<BatchV2Plan> plan(G);
+  bool any = false;
+  for (uint32_t g = 0; g < G; ++g) {
+    plan[g] = batch_q8_plan((uint32_t)ctx->sm_count, (uint32_t)listed[g].size(), top_k);
+    any |= plan[g].fits;
+  }
+  if (any) {
+    rc = corpus_ensure_q8(ctx, corpus);
+    if (rc == STB_ERR_NOMEM || rc == STB_ERR_STATE) any = false;      // K1 answers every query
+    else if (rc != STB_OK) return rc;
+  }
+  // per caller query: the tensor result and {hits, proven}; the output is written only once every group has run,
+  // so a group refused for lack of scratch leaves it untouched
+  std::vector<uint32_t> status((size_t)nq * 2, 0), gstatus;
+  std::vector<stb_hit> hits(any ? (size_t)nq * top_k : 0), ghits;
+  std::vector<float> gq;
+  uint32_t n_tensor = 0;
+  for (uint32_t g = 0; any && g < G; ++g) {
+    if (!plan[g].fits) continue;
+    const std::vector<uint32_t> &mem = members[g];
+    const uint32_t m = (uint32_t)mem.size();
+    gq.resize((size_t)m * STB_D);
+    ghits.resize((size_t)m * top_k);
+    gstatus.assign((size_t)m * 2, 0);
+    for (uint32_t j = 0; j < m; ++j) memcpy(gq.data() + (size_t)j * STB_D, q + (size_t)mem[j] * STB_D, STB_D * sizeof(float));
+    if ((rc = filtered_tensor_run(ctx, corpus, gq.data(), m, top_k, *lists[g], listed[g], plan[g], true, ghits.data(),
+                                  gstatus.data())) != STB_OK) return rc;
+    for (uint32_t j = 0; j < m; ++j) {
+      memcpy(hits.data() + (size_t)mem[j] * top_k, ghits.data() + (size_t)j * top_k, (size_t)top_k * sizeof(stb_hit));
+      status[2 * (size_t)mem[j]] = gstatus[2 * j];
+      status[2 * (size_t)mem[j] + 1] = gstatus[2 * j + 1];
+    }
+    n_tensor++;
+  }
+  uint32_t k1;
+  if ((rc = k2_complete(ctx, corpus, q, nq, top_k, has_max, max_distance, STB_MODE_STORE_QUERY, [&](uint32_t i) -> K2Answer {
+         if (group[i] == kNone) return {K2Answer::kEmpty};
+         if (status[2 * (size_t)i + 1]) return {K2Answer::kProven, hits.data() + (size_t)i * top_k, status[2 * (size_t)i]};
+         return {K2Answer::kK1, nullptr, 0, row_ranges + 2 * range_offsets[i], (uint32_t)(range_offsets[i + 1] - range_offsets[i])};
+       }, out_hits, out_n, &k1)) != STB_OK) return rc;
+  k2_record(ctx, kRouteSubsetsQ8, nq, n_tensor, k1);
+  return STB_OK;
+}
+
 extern "C" {
 
 // The store query for a batch in which every query names its own subset (route 6).  Queries whose clipped
@@ -1785,7 +1919,8 @@ extern "C" {
 // Otherwise every group whose v2 plan fits runs on the tensor cores, each occupying whole 64-query halves of
 // the query slots: one sampling pass over the union of the groups' sampled tiles, the per-slot threshold, one
 // emitting pass over the union of their listed tiles, finish2 over the groups' queries in compact order.  K1
-// answers the other groups and every query the tensor passes leave unproven.
+// answers the other groups and every query the tensor passes leave unproven.  Where the shadow does not fit and a
+// group fits either plan, route 9 (subsets_q8_run) runs instead.
 int stb_search_batch_subsets(stb_ctx *ctx, const stb_corpus *corpus_c, const float *q, uint32_t nq, uint32_t top_k,
                              int has_max, double max_distance, const uint64_t *range_offsets, const uint64_t *row_ranges,
                              stb_hit *out_hits, uint32_t *out_n) {
@@ -1854,8 +1989,14 @@ int stb_search_batch_subsets(stb_ctx *ctx, const stb_corpus *corpus_c, const flo
     if (plan[g].fits) tgroups.push_back(g);
   }
   if ((uint64_t)tgroups.size() * n_tiles >= UINT32_MAX) tgroups.clear();   // mask slots are 32-bit
-  if (!tgroups.empty()) {
-    rc = corpus_ensure_shadow(ctx, corpus);
+  // the shadow is asked for whenever a group fits either plan, and built only where route 6 reads it
+  bool q8_fits = false;
+  for (uint32_t g = 0; g < G && !q8_fits; ++g) q8_fits = batch_q8_plan((uint32_t)ctx->sm_count, (uint32_t)listed[g].size(), top_k).fits;
+  if (!tgroups.empty() || q8_fits) {
+    rc = !tgroups.empty() ? batch_shadow(ctx, corpus) : batch_shadow_fits(ctx, corpus);
+    if (rc == STB_ERR_NOMEM)                               // the shadow does not fit: route 9
+      return subsets_q8_run(ctx, corpus, q, nq, top_k, has_max, max_distance, group, lists, listed, range_offsets,
+                            row_ranges, out_hits, out_n);
     if (rc == STB_ERR_STATE) tgroups.clear();              // un-normalisable rows: K1 answers every query
     else if (rc != STB_OK) return rc;
   }
@@ -1980,27 +2121,28 @@ int stb_search_batch_subsets(stb_ctx *ctx, const stb_corpus *corpus_c, const flo
 static_assert(STB_THR_SEG_CAP == kSegCap, "route 5's first pass uses pipeline v2's segment capacity");
 #define STB_THR_CHUNK 4096u        // queries per pipeline run (keeps every candidate count within int)
 
-// The emission threshold of the queries the tensor cores answer: ((1 - M) - EPS) - delta in f64, rounded toward
-// -inf to f32.  Every row with canonical d < M has exact cosine c > 1 - M - delta and score a >= c - EPS.
-static float thr_emission_value(double max_distance) {
-  double eps = 0.0;
-  stb_batch_build_params(nullptr, &eps);
+// The emission threshold of the queries the tensor cores answer: ((1 - M) - eps) - delta in f64, rounded toward
+// -inf to f32.  Every row with canonical d < M has exact cosine c > 1 - M - delta, so its score a >= c - EPS on
+// the shadow (eps = EPS), and its upper bound u >= c - 1e-5 on the q8 copy (eps = STB_Q8_SCAN_EPS, route 10).
+static float thr_emission_value(double max_distance, double eps) {
   const double x = ((1.0 - max_distance) - eps) - STB_THR_DELTA;
   float f = (float)x;
   if ((double)f > x) f = std::nextafter(f, -INFINITY);
   return f;
 }
 
-// One chunk of queries q[0, n) (global indices c0 ..) on the tensor cores.  On return slot_query[s] / pass[s]
-// are the chunk-local query and hit count of every answered slot, k1 lists the queries K1 must answer, and the
-// sorted hits of slot s sit at ctx->t_buf (distance bits at [0, K), rows at [K, 2K)) from (*off)[s].
+// One chunk of queries q[0, n) (global indices c0 ..) on the tensor cores: the shadow (route 5) or, q8, the q8
+// copy (route 10: the queries' q8 tiles and unusable flags, K1's upper bounds u as the emitted scores).  On return
+// slot_query[s] / pass[s] are the chunk-local query and hit count of every answered slot, k1 lists the queries K1
+// must answer, and the sorted hits of slot s sit at ctx->t_buf (distance bits at [0, K), rows at [K, 2K)) from
+// (*off)[s].
 struct ThrChunk {
   std::vector<uint32_t> slot_query, pass, k1;
   std::vector<int> off;
   uint32_t retried = 0;
 };
 static int thr_chunk_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, uint32_t c0, uint32_t n, double max_distance,
-                         float t, ThrChunk *out) {
+                         float t, bool q8, ThrChunk *out) {
   int rc;
   const uint32_t m_tiles = (n + 127) / 128, q_pad = m_tiles * 128;
   const uint32_t n_tiles = (uint32_t)((corpus->n + 255) / 256);
@@ -2011,13 +2153,22 @@ static int thr_chunk_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, uint3
   if ((rc = ctx->b_qbad.reserve((size_t)q_pad)) != STB_OK) return rc;
   if ((rc = ctx->bq_tiles.reserve((size_t)q_pad * 512)) != STB_OK) return rc;
   if ((rc = ctx->b_keys.reserve((size_t)q_pad * n_seg * STB_THR_SEG_CAP)) != STB_OK) return rc;
+  if (q8 && (rc = ctx->b_q8c.reserve((size_t)q_pad)) != STB_OK) return rc;
   STB_CUDA(cudaMemcpyAsync(ctx->bq_dev, q, (size_t)n * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
   STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
   STB_CUDA(cudaMemsetAsync(cnt, 0, (size_t)q_pad * n_seg * sizeof(uint32_t), ctx->stream));
-  if ((rc = stb_launch_shadow_build(ctx, ctx->bq_dev, n, 128, ctx->bq_tiles, ctx->err_flag, 0, ctx->b_qbad)) != STB_OK) return rc;
-  if ((rc = stb_launch_batch_thr_dist(ctx, ctx->bq_dev, ctx->b_qbad, n, q_pad, t, thr)) != STB_OK) return rc;
-  if ((rc = stb_launch_batch_gemm_emit(ctx, ctx->bq_tiles, m_tiles, corpus->shadow, n_tiles, corpus->n, thr, cnt,
-                                       ctx->b_keys, STB_THR_SEG_CAP)) != STB_OK) return rc;
+  if (q8) {
+    // the q8 flags mark the zero query and the unnormalisable ones: their threshold is +inf, K1 answers them
+    if ((rc = stb_launch_q8_query_tiles(ctx, ctx->bq_dev, n, q_pad, ctx->bq_tiles, ctx->b_q8c, ctx->b_qbad, nullptr)) != STB_OK ||
+        (rc = stb_launch_batch_thr_dist(ctx, ctx->bq_dev, ctx->b_qbad, n, q_pad, t, thr)) != STB_OK ||
+        (rc = stb_launch_batch_q8_gemm_emit(ctx, ctx->bq_tiles, ctx->b_q8c, m_tiles, corpus->q8, corpus->q8_scale, corpus->n,
+                                            thr, cnt, ctx->b_keys, STB_THR_SEG_CAP)) != STB_OK) return rc;
+  } else {
+    if ((rc = stb_launch_shadow_build(ctx, ctx->bq_dev, n, 128, ctx->bq_tiles, ctx->err_flag, 0, ctx->b_qbad)) != STB_OK) return rc;
+    if ((rc = stb_launch_batch_thr_dist(ctx, ctx->bq_dev, ctx->b_qbad, n, q_pad, t, thr)) != STB_OK) return rc;
+    if ((rc = stb_launch_batch_gemm_emit(ctx, ctx->bq_tiles, m_tiles, corpus->shadow, n_tiles, corpus->n, thr, cnt,
+                                         ctx->b_keys, STB_THR_SEG_CAP)) != STB_OK) return rc;
+  }
   std::vector<uint32_t> hcnt((size_t)n * n_seg);
   std::vector<float> hthr(n);
   STB_CUDA(cudaMemcpyAsync(hcnt.data(), cnt, hcnt.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -2078,8 +2229,8 @@ static int thr_chunk_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, uint3
   STB_CUDA(cudaMemcpyAsync(ctx->t_dst, dst.data(), dst.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->stream));
   if ((rc = stb_launch_batch_thr_compact(ctx, ctx->b_keys, cnt, ctx->t_dst, (uint64_t)n * n_seg, STB_THR_SEG_CAP, A)) != STB_OK) return rc;
   if (n_retry) {
-    // one more pass over the re-emitted queries' shadow tiles (rebuilt from their f32 rows: the same bits), into
-    // segments sized by the first pass's exact counts
+    // one more pass over the re-emitted queries' shadow (or q8) tiles, rebuilt from their f32 rows: the same bits,
+    // the same emitted rows; into segments sized by the first pass's exact counts
     if ((rc = ctx->t_segoff.reserve(segoff.size())) != STB_OK) return rc;
     if ((rc = ctx->t_cur.reserve((size_t)r_pad * n_seg)) != STB_OK) return rc;
     if ((rc = ctx->t_rq.reserve((size_t)n_retry * STB_D)) != STB_OK) return rc;
@@ -2089,9 +2240,16 @@ static int thr_chunk_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, uint3
     STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
     if ((rc = stb_launch_batch_thr_gather(ctx, ctx->bq_dev, thr, ctx->t_slot + n_direct, n_retry, r_pad, ctx->t_rq,
                                           ctx->t_rthr)) != STB_OK) return rc;
-    if ((rc = stb_launch_shadow_build(ctx, ctx->t_rq, n_retry, 128, ctx->bq_tiles, ctx->err_flag)) != STB_OK) return rc;
-    if ((rc = stb_launch_batch_gemm_emit_sized(ctx, ctx->bq_tiles, r_tiles, corpus->shadow, n_tiles, corpus->n, ctx->t_rthr,
-                                               ctx->t_cur, A, ctx->t_segoff)) != STB_OK) return rc;
+    if (q8) {
+      // b_q8c / b_qbad of the first pass are no longer read (r_pad <= q_pad)
+      if ((rc = stb_launch_q8_query_tiles(ctx, ctx->t_rq, n_retry, r_pad, ctx->bq_tiles, ctx->b_q8c, ctx->b_qbad, nullptr)) != STB_OK ||
+          (rc = stb_launch_batch_q8_gemm_emit_sized(ctx, ctx->bq_tiles, ctx->b_q8c, r_tiles, corpus->q8, corpus->q8_scale,
+                                                    corpus->n, ctx->t_rthr, ctx->t_cur, A, ctx->t_segoff)) != STB_OK) return rc;
+    } else {
+      if ((rc = stb_launch_shadow_build(ctx, ctx->t_rq, n_retry, 128, ctx->bq_tiles, ctx->err_flag)) != STB_OK) return rc;
+      if ((rc = stb_launch_batch_gemm_emit_sized(ctx, ctx->bq_tiles, r_tiles, corpus->shadow, n_tiles, corpus->n, ctx->t_rthr,
+                                                 ctx->t_cur, A, ctx->t_segoff)) != STB_OK) return rc;
+    }
   }
   // exact finish: rows ascending -> canonical re-score, d < M -> stable sort by distance = (distance, row) order
   if ((rc = stb_batch_thr_sort_rows(ctx, ctx->t_sort_tmp, sort_bytes, K, n_slots, ctx->t_off, A, B)) != STB_OK) return rc;
@@ -2105,9 +2263,10 @@ static int thr_chunk_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, uint3
 
 extern "C" {
 
-// Threshold mode of search_documents for a batch (route 5).  Chunks of STB_THR_CHUNK queries run the tensor-core
-// pipeline (thr_chunk_run); K1 (stb_search) answers the queries it leaves, and each chunk's hits are laid out
-// once all its counts are known: a chunk's output is one contiguous stretch of the concatenation.
+// Threshold mode of search_documents for a batch (route 5; route 10 on the q8 copy where the shadow does not fit).
+// Chunks of STB_THR_CHUNK queries run the tensor-core pipeline (thr_chunk_run); K1 (stb_search) answers the
+// queries it leaves (all of them when neither copy can be used), and each chunk's hits are laid out once all its
+// counts are known: a chunk's output is one contiguous stretch of the concatenation.
 int stb_search_batch_threshold(stb_ctx *ctx, const stb_corpus *corpus_c, const float *q, uint32_t nq, double max_distance,
                                stb_hit *out_hits, uint64_t cap, uint64_t *out_offsets) {
   int rc = ctx_use(ctx);
@@ -2120,23 +2279,30 @@ int stb_search_batch_threshold(stb_ctx *ctx, const stb_corpus *corpus_c, const f
   k2_record(ctx, kRouteThreshold, nq);
   for (uint32_t i = 0; i <= nq; ++i) out_offsets[i] = 0;
   if (corpus->n == 0 || !(max_distance > 0.0)) return STB_OK;      // NaN or <= 0: no distance is below it
-  rc = corpus_ensure_shadow(ctx, corpus);
+  rc = batch_shadow(ctx, corpus);
+  const bool q8 = rc == STB_ERR_NOMEM;                               // the shadow does not fit: route 10
+  const K2Route route = q8 ? kRouteThresholdQ8 : kRouteThreshold;
+  if (q8) rc = corpus_ensure_q8(ctx, corpus);
   const bool tensor_ok = rc == STB_OK;
-  if (rc != STB_OK && rc != STB_ERR_STATE) return rc;                // STB_ERR_STATE: rows K2 cannot normalise, all K1
+  // STB_ERR_STATE: rows K2 cannot normalise; route 10 also STB_ERR_NOMEM: the q8 copy does not fit.  All K1
+  if (rc != STB_OK && rc != STB_ERR_STATE && !(q8 && rc == STB_ERR_NOMEM)) return rc;
+  if (q8) k2_record(ctx, route, nq);
   const uint32_t n_seg = tensor_ok ? stb_batch_emit_grid(ctx, (uint32_t)((corpus->n + 255) / 256)) : 0u;
   const size_t nq_pad = ((size_t)nq + 127) / 128 * 128;
   if (tensor_ok) {
     if ((rc = ctx->b_thr.reserve(nq_pad)) != STB_OK) return rc;
     if ((rc = ctx->b_cnt.reserve(nq_pad * n_seg)) != STB_OK) return rc;
   }
-  const float t = thr_emission_value(max_distance);
+  double eps = STB_Q8_SCAN_EPS;
+  if (!q8) stb_batch_build_params(nullptr, &eps);
+  const float t = thr_emission_value(max_distance, eps);
   std::unique_ptr<stb_hit[]> k1_buf;                                 // one K1 result: at most every row
   uint32_t retried = 0, k1_total = 0;
   for (uint32_t c0 = 0; c0 < nq; c0 += STB_THR_CHUNK) {
     const uint32_t n = std::min(STB_THR_CHUNK, nq - c0);
     ThrChunk ch;
     if (tensor_ok) {
-      if ((rc = thr_chunk_run(ctx, corpus, q + (size_t)c0 * STB_D, c0, n, max_distance, t, &ch)) != STB_OK) return rc;
+      if ((rc = thr_chunk_run(ctx, corpus, q + (size_t)c0 * STB_D, c0, n, max_distance, t, q8, &ch)) != STB_OK) return rc;
     } else {
       for (uint32_t i = 0; i < n; ++i) ch.k1.push_back(i);
     }
@@ -2177,7 +2343,7 @@ int stb_search_batch_threshold(stb_ctx *ctx, const stb_corpus *corpus_c, const f
       if (o < cap) memcpy(out_hits + o, k1_hits[j].data(), std::min<uint64_t>(k1_hits[j].size(), cap - o) * sizeof(stb_hit));
     }
   }
-  k2_record(ctx, kRouteThreshold, nq, retried, k1_total, n_seg, tensor_ok ? STB_THR_SEG_CAP : 0u);
+  k2_record(ctx, route, nq, retried, k1_total, n_seg, tensor_ok ? STB_THR_SEG_CAP : 0u);
   if (out_offsets[nq] > cap) {
     stb_set_error("search_batch_threshold: %llu hits, capacity %llu", (unsigned long long)out_offsets[nq], (unsigned long long)cap);
     return STB_ERR_CAPACITY;
@@ -2239,10 +2405,18 @@ int stb_debug_batch_last(stb_ctx *ctx, uint32_t info[6], float *thr, uint32_t *c
     }
     return STB_OK;
   }
-  if ((route == kRouteV2 || route == kRouteFiltered || ((route == kRouteThreshold || route == kRouteQ8) && n_seg)) && nq) {
+  if ((route == kRouteV2 || route == kRouteFiltered ||
+       ((route == kRouteThreshold || route == kRouteQ8 || route == kRouteFilteredQ8 || route == kRouteThresholdQ8) && n_seg)) && nq) {
     if (thr) STB_CUDA(cudaMemcpy(thr, ctx->b_thr, (size_t)nq * sizeof(float), cudaMemcpyDeviceToHost));
     if (cand_cnt) STB_CUDA(cudaMemcpy(cand_cnt, ctx->b_cnt, (size_t)nq * n_seg * sizeof(uint32_t), cudaMemcpyDeviceToHost));
   }
+  return STB_OK;
+}
+
+int stb_debug_batch_no_shadow(stb_ctx *ctx, int on) {
+  int rc = ctx_use(ctx);
+  if (rc) return rc;
+  ctx->b_no_shadow = on ? 1 : 0;
   return STB_OK;
 }
 

@@ -1484,13 +1484,26 @@ struct Q8GemmArgs {
   uint32_t cand_cap;
   int32_t *dot_out;           // EPI 2: [m_tiles * 128][n_tiles * 256] dot, u and l
   float *u_out, *l_out;
+  // (appended, so the unfiltered EPI 0-2 kernels keep their parameter offsets)
+  // FILTER (route 8): tile t of the launch is corpus tile tile_ids[t * tile_stride], and only the eligible rows
+  // of `bitmap` (8 words per corpus tile, stb_launch_row_bitmap) count
+  const uint32_t *tile_ids;
+  const uint32_t *bitmap;
+  // EPI 3 (route 10's re-emission): segment (q, CTA) is cand_keys[seg_off[q * grid + CTA], seg_off[q * grid + CTA + 1]),
+  // sized by the first pass's exact counts; cand_cnt holds the cursors
+  const uint64_t *seg_off;
 };
 
-// EPI 0: sampling (tile maxima of l); EPI 1: emit every row whose u reaches the query's threshold; EPI 2: debug
-template <int EPI>
+// EPI 0: sampling (tile maxima of l); EPI 1: emit every row whose u reaches the query's threshold; EPI 2: debug;
+// EPI 3: EPI 1 into exactly sized segments (unfiltered only).
+// FILTER: the CTAs walk the listed tiles and only eligible rows count: EPI 0 takes each tile maximum of l over
+// its eligible rows (an ineligible row's l is -inf, DESIGN §5), EPI 1 emits eligible rows only.  The tile's 8
+// bitmap words arrive with its scales, double-buffered by tile parity like them.
+template <int EPI, bool FILTER>
 __global__ void __launch_bounds__(STB_GEMM_THREADS, 1)
 stb_batch_q8_gemm_kernel(const __grid_constant__ CUtensorMap codes_map, const __grid_constant__ CUtensorMap scale_map,
                          const Q8GemmArgs args) {
+  static_assert(!FILTER || EPI == 0 || EPI == 1, "route 8 runs the sampling and the emitting pass");
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t *sB = smem;                                          // 2 code slabs
@@ -1499,6 +1512,9 @@ stb_batch_q8_gemm_kernel(const __grid_constant__ CUtensorMap codes_map, const __
   uint64_t *bars = reinterpret_cast<uint64_t *>(s_scale + 2 * STB_B_TILE);
   uint64_t *b_full = bars + 0, *b_empty = bars + 2;
   uint64_t *a_full = bars + 4, *a_empty = a_full + STB_A_RING;
+  // FILTER: [2][8] bitmap words behind the 16 barriers, slot it & 1 = the tile of iteration it
+  [[maybe_unused]] uint32_t *s_mask = reinterpret_cast<uint32_t *>(bars + 4 + 2 * STB_A_RING);
+  static_assert((4 + 2 * STB_A_RING) * 8 + 2 * 8 * 4 <= 256, "mask words must fit behind the barriers");
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     for (int i = 0; i < 2; ++i) { mbar_init(b_full + i, 1); mbar_init(b_empty + i, STB_GEMM_CONSUMER_WARPS); }
@@ -1514,11 +1530,18 @@ stb_batch_q8_gemm_kernel(const __grid_constant__ CUtensorMap codes_map, const __
     if (threadIdx.x == 0) {
       uint32_t a_cnt = 0;
       for (uint32_t it = 0; it < my_tiles; ++it) {
-        const int row0 = (int)((blockIdx.x + (uint64_t)it * gridDim.x) * args.tile_stride * STB_B_TILE);
+        const uint64_t t = blockIdx.x + (uint64_t)it * gridDim.x;
+        const uint64_t tile = FILTER ? (uint64_t)__ldg(args.tile_ids + t * args.tile_stride) : t * args.tile_stride;
+        const int row0 = (int)(tile * STB_B_TILE);
         for (int s = 0; s < 2; ++s) {
           mbar_wait(b_empty + s, (it & 1) ^ 1);
           if (s == 0) {
-            mbar_expect_tx(b_full, STB_Q8_B_SLAB_BYTES + STB_B_TILE * 4);
+            if constexpr (FILTER) {
+              mbar_expect_tx(b_full, STB_Q8_B_SLAB_BYTES + STB_B_TILE * 4 + 32);
+              bulk_g2s(s_mask + (it & 1) * 8, args.bitmap + tile * 8, 32, b_full);
+            } else {
+              mbar_expect_tx(b_full, STB_Q8_B_SLAB_BYTES + STB_B_TILE * 4);
+            }
             tma_load_1d(s_scale + (it & 1) * STB_B_TILE, &scale_map, row0, b_full);
           } else {
             mbar_expect_tx(b_full + s, STB_Q8_B_SLAB_BYTES);
@@ -1549,20 +1572,29 @@ stb_batch_q8_gemm_kernel(const __grid_constant__ CUtensorMap codes_map, const __
   uint32_t a_cnt = 0;
   for (uint32_t it = 0; it < my_tiles; ++it) {
     const uint64_t t = blockIdx.x + (uint64_t)it * gridDim.x;
-    const uint64_t row0 = t * args.tile_stride * STB_B_TILE;
+    const uint64_t row0 = FILTER ? (uint64_t)__ldg(args.tile_ids + t * args.tile_stride) * STB_B_TILE
+                                 : t * args.tile_stride * STB_B_TILE;
     const float *sc = s_scale + (it & 1) * STB_B_TILE;
+    [[maybe_unused]] const uint32_t *mk = s_mask + (it & 1) * 8;
     for (uint32_t m = 0; m < args.m_tiles; ++m, a_cnt += 4) {
       const uint32_t q0 = m * STB_A_TILE + qrow;
       float4 qc[2];
       [[maybe_unused]] float thr[2];
       [[maybe_unused]] uint32_t cnt[2], cnt0[2];
+      [[maybe_unused]] uint64_t seg_base[2];
+      [[maybe_unused]] uint32_t seg_len[2];
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         qc[h] = __ldg(args.qc + q0 + 8 * h);
-        if constexpr (EPI == 1) {
+        if constexpr (EPI == 1 || EPI == 3) {
           thr[h] = __ldg(args.thr + q0 + 8 * h);
           cnt0[h] = args.cand_cnt[(size_t)(q0 + 8 * h) * gridDim.x + blockIdx.x];
           cnt[h] = cnt0[h];
+          if constexpr (EPI == 3) {
+            const uint64_t *so = args.seg_off + (size_t)(q0 + 8 * h) * gridDim.x + blockIdx.x;
+            seg_base[h] = __ldg(so);
+            seg_len[h] = (uint32_t)(__ldg(so + 1) - seg_base[h]);
+          }
         }
       }
       wg_reg_fence_s32(d);
@@ -1613,7 +1645,8 @@ stb_batch_q8_gemm_kernel(const __grid_constant__ CUtensorMap codes_map, const __
             const float2 s2 = *reinterpret_cast<const float2 *>(sc + col);
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-              const bool real = col + e < n_real;
+              // FILTER: the eligible rows (the bitmap holds no row past n)
+              const bool real = FILTER ? ((mk[c] >> (ii * 8 + quad * 2 + e)) & 1u) != 0u : col + e < n_real;
 #pragma unroll
               for (int h = 0; h < 2; ++h) {
                 const float l = fmaf(e ? s2.y : s2.x, fmaf((float)d[16 * c + 4 * ii + 2 * h + e], qc[h].x, -qc[h].y), -qc[h].z) -
@@ -1628,8 +1661,8 @@ stb_batch_q8_gemm_kernel(const __grid_constant__ CUtensorMap codes_map, const __
           tmx[h] = fmaxf(tmx[h], __shfl_xor_sync(0xffffffffu, tmx[h], 2));
           if (quad == (uint32_t)h) args.tilemax[((size_t)m * args.n_tiles + t) * STB_A_TILE + qrow + 8 * h] = tmx[h];
         }
-      } else if constexpr (EPI == 1) {
-        // as stb_batch_gemm_kernel's EPI 1: a private segment per (query, CTA), branch-free hit masks
+      } else if constexpr (EPI == 1 || EPI == 3) {
+        // as stb_batch_gemm_kernel's EPI 1 (EPI 3: its EPI 2): a private segment per (query, CTA), branch-free hit masks
 #pragma unroll
         for (int c = 0; c < STB_B_TILE / STB_SUB; ++c) {
           const uint64_t r0 = row0 + (uint64_t)c * STB_SUB;
@@ -1653,14 +1686,23 @@ stb_batch_q8_gemm_kernel(const __grid_constant__ CUtensorMap codes_map, const __
             hit |= __shfl_xor_sync(0xffffffffu, hit, 1);
             hit |= __shfl_xor_sync(0xffffffffu, hit, 2);
             if (r0 + 32 > args.n_rows) hit &= (r0 < args.n_rows) ? ((1u << (uint32_t)(args.n_rows - r0)) - 1u) : 0u;
-            uint64_t *seg = args.cand_keys + ((size_t)(q0 + 8 * h) * gridDim.x + blockIdx.x) * args.cand_cap;
+            if constexpr (FILTER) hit &= mk[c];                                    // ineligible rows
+            uint64_t *seg;
+            uint32_t seg_cap;
+            if constexpr (EPI == 3) {
+              seg = args.cand_keys + seg_base[h];
+              seg_cap = seg_len[h];
+            } else {
+              seg = args.cand_keys + ((size_t)(q0 + 8 * h) * gridDim.x + blockIdx.x) * args.cand_cap;
+              seg_cap = args.cand_cap;
+            }
 #pragma unroll
             for (int ii = 0; ii < 4; ++ii)
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
                 const uint32_t b = ii * 8 + quad * 2 + e;
                 const uint32_t pos = cnt[h] + __popc(hit & ((1u << b) - 1u));
-                if (((hit >> b) & 1u) && pos < args.cand_cap) seg[pos] = stb_make_key(u[ii][h][e], (uint32_t)(r0 + b));
+                if (((hit >> b) & 1u) && pos < seg_cap) seg[pos] = stb_make_key(u[ii][h][e], (uint32_t)(r0 + b));
               }
             cnt[h] += __popc(hit);
           }
@@ -1723,17 +1765,19 @@ static int q8_tensor_maps(const uint8_t *codes, const float *scales, uint64_t n_
   return STB_OK;
 }
 
-template <int EPI>
+template <int EPI, bool FILTER = false>
 static int launch_q8_gemm(stb_ctx *ctx, const uint8_t *codes, const float *scales, const Q8GemmArgs &a) {
   if (a.n_rows == 0 || a.n_rows > 0x7fffff00ull) { stb_set_error("q8 GEMM: %llu rows", (unsigned long long)a.n_rows); return STB_ERR_ARG; }
   CUtensorMap cm, sm;
   int rc = q8_tensor_maps(codes, scales, a.n_rows, &cm, &sm);
   if (rc != STB_OK) return rc;
-  STB_ATTR_ONCE(ctx, EPI == 0 ? STB_ATTR_Q8GEMM0 : (EPI == 1 ? STB_ATTR_Q8GEMM1 : STB_ATTR_Q8GEMM2),
-                cudaFuncSetAttribute(stb_batch_q8_gemm_kernel<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, STB_Q8_GEMM_SMEM));
+  const int attr = FILTER ? (EPI == 0 ? STB_ATTR_Q8GEMM0F : STB_ATTR_Q8GEMM1F)
+                          : (EPI == 0 ? STB_ATTR_Q8GEMM0 : EPI == 1 ? STB_ATTR_Q8GEMM1 : EPI == 2 ? STB_ATTR_Q8GEMM2 : STB_ATTR_Q8GEMM3);
+  STB_ATTR_ONCE(ctx, attr,
+                cudaFuncSetAttribute(stb_batch_q8_gemm_kernel<EPI, FILTER>, cudaFuncAttributeMaxDynamicSharedMemorySize, STB_Q8_GEMM_SMEM));
   const unsigned grid = (unsigned)std::min<uint32_t>(a.n_tiles, (uint32_t)ctx->sm_count);   // = stb_batch_emit_grid
   if (grid == 0) return STB_OK;
-  stb_batch_q8_gemm_kernel<EPI><<<grid, STB_GEMM_THREADS, STB_Q8_GEMM_SMEM, ctx->stream>>>(cm, sm, a);
+  stb_batch_q8_gemm_kernel<EPI, FILTER><<<grid, STB_GEMM_THREADS, STB_Q8_GEMM_SMEM, ctx->stream>>>(cm, sm, a);
   STB_CUDA(cudaGetLastError());
   ctx->kernel_launches++;
   return STB_OK;
@@ -1764,4 +1808,38 @@ int stb_launch_batch_q8_gemm_debug(stb_ctx *ctx, const uint8_t *a_tiles, const f
   a.a_tiles = a_tiles; a.qc = qc; a.m_tiles = m_tiles; a.n_tiles = (uint32_t)((n_rows + STB_B_TILE - 1) / STB_B_TILE);
   a.tile_stride = 1; a.n_rows = n_rows; a.dot_out = dot; a.u_out = u; a.l_out = l;
   return launch_q8_gemm<2>(ctx, codes, scales, a);
+}
+
+// Route 8: the sampling pass over the listed tiles 0, stride, 2*stride, ... (n_sample of them), tile maxima of l
+// over eligible rows ...
+int stb_launch_batch_q8_gemm_sample_filtered(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
+                                             const uint8_t *codes, const float *scales, uint64_t n_rows,
+                                             const uint32_t *tile_ids, const uint32_t *bitmap, uint32_t n_sample,
+                                             uint32_t tile_stride, float *tilemax) {
+  Q8GemmArgs a{};
+  a.a_tiles = a_tiles; a.qc = qc; a.m_tiles = m_tiles; a.n_tiles = n_sample; a.tile_stride = tile_stride;
+  a.n_rows = n_rows; a.tilemax = tilemax; a.tile_ids = tile_ids; a.bitmap = bitmap;
+  return launch_q8_gemm<0, true>(ctx, codes, scales, a);
+}
+
+// ... and the emitting pass over all n_listed listed tiles, eligible rows only
+int stb_launch_batch_q8_gemm_emit_filtered(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
+                                           const uint8_t *codes, const float *scales, uint64_t n_rows,
+                                           const uint32_t *tile_ids, const uint32_t *bitmap, uint32_t n_listed,
+                                           const float *thr, uint32_t *cand_cnt, uint64_t *cand_keys, uint32_t cand_cap) {
+  Q8GemmArgs a{};
+  a.a_tiles = a_tiles; a.qc = qc; a.m_tiles = m_tiles; a.n_tiles = n_listed; a.tile_stride = 1; a.n_rows = n_rows;
+  a.thr = thr; a.cand_cnt = cand_cnt; a.cand_keys = cand_keys; a.cand_cap = cand_cap; a.tile_ids = tile_ids; a.bitmap = bitmap;
+  return launch_q8_gemm<1, true>(ctx, codes, scales, a);
+}
+
+// Route 10's re-emission: the emitting pass over all tiles into the exactly sized segments seg_off[] of cand_keys;
+// cursors [q_pad][grid] zeroed by the caller
+int stb_launch_batch_q8_gemm_emit_sized(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
+                                        const uint8_t *codes, const float *scales, uint64_t n_rows, const float *thr,
+                                        uint32_t *cursors, uint64_t *cand_keys, const uint64_t *seg_off) {
+  Q8GemmArgs a{};
+  a.a_tiles = a_tiles; a.qc = qc; a.m_tiles = m_tiles; a.n_tiles = (uint32_t)((n_rows + STB_B_TILE - 1) / STB_B_TILE);
+  a.tile_stride = 1; a.n_rows = n_rows; a.thr = thr; a.cand_cnt = cursors; a.cand_keys = cand_keys; a.seg_off = seg_off;
+  return launch_q8_gemm<3>(ctx, codes, scales, a);
 }

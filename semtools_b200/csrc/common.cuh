@@ -207,6 +207,7 @@ struct stb_ctx {
   StbBuf<stb_hit> t_hits;
   StbBuf<uint8_t> t_sort_tmp;
   uint32_t b_last[6];             // the last K2 call's route record (api.cu: k2_record)
+  int b_no_shadow = 0;            // stb_debug_batch_no_shadow: K2 calls act as if the shadow did not fit
   StbBuf<float> bq_dev;           // host-call staging: queries
   StbBuf<stb_hit> bh_dev;         // host-call staging: hits
   StbBuf<uint32_t> bs_dev;        // host-call staging: status
@@ -445,7 +446,8 @@ int stb_launch_batch_xchg(stb_ctx *ctx, const StbBatchXchgArgs &a, const stb_hit
 // opt-in to > 48 KiB dynamic shared memory (or another function attribute) once per context
 enum { STB_ATTR_GEMM0 = 0, STB_ATTR_GEMM1, STB_ATTR_MERGE, STB_ATTR_IVF_PROBE, STB_ATTR_IVF_V2, STB_ATTR_FINISH2,
        STB_ATTR_IVF_BATCH, STB_ATTR_GEMM0F, STB_ATTR_GEMM1F, STB_ATTR_GEMM2, STB_ATTR_GEMM0W, STB_ATTR_GEMM1W,
-       STB_ATTR_Q8GEMM0, STB_ATTR_Q8GEMM1, STB_ATTR_Q8GEMM2, STB_ATTR_THRESH_BIG };
+       STB_ATTR_Q8GEMM0, STB_ATTR_Q8GEMM1, STB_ATTR_Q8GEMM2, STB_ATTR_THRESH_BIG,
+       STB_ATTR_Q8GEMM0F, STB_ATTR_Q8GEMM1F, STB_ATTR_Q8GEMM3 };
 #define STB_ATTR_ONCE(ctx, bit, call)                         \
   do {                                                        \
     if (!((ctx)->func_attr_mask & (1u << (bit)))) {           \
@@ -529,6 +531,20 @@ int stb_launch_batch_q8_gemm_emit(stb_ctx *ctx, const uint8_t *a_tiles, const fl
 int stb_launch_batch_q8_gemm_debug(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
                                    const uint8_t *codes, const float *scales, uint64_t n_rows, int32_t *dot, float *u,
                                    float *l);
+// Routes 8 and 10: route 7's two passes over the listed tiles tile_ids[0, n_listed), eligible rows (bitmap) only,
+// and its emitting pass into exactly sized segments cand_keys[seg_off[i], seg_off[i+1]) (i = query * grid + CTA,
+// cursors [q_pad][grid] zeroed), as stb_launch_batch_gemm_*_filtered and stb_launch_batch_gemm_emit_sized
+int stb_launch_batch_q8_gemm_sample_filtered(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
+                                             const uint8_t *codes, const float *scales, uint64_t n_rows,
+                                             const uint32_t *tile_ids, const uint32_t *bitmap, uint32_t n_sample,
+                                             uint32_t tile_stride, float *tilemax);
+int stb_launch_batch_q8_gemm_emit_filtered(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
+                                           const uint8_t *codes, const float *scales, uint64_t n_rows,
+                                           const uint32_t *tile_ids, const uint32_t *bitmap, uint32_t n_listed,
+                                           const float *thr, uint32_t *cand_cnt, uint64_t *cand_keys, uint32_t cand_cap);
+int stb_launch_batch_q8_gemm_emit_sized(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
+                                        const uint8_t *codes, const float *scales, uint64_t n_rows, const float *thr,
+                                        uint32_t *cursors, uint64_t *cand_keys, const uint64_t *seg_off);
 void stb_batch_build_params(int *shadow_is_f16, double *eps);
 // threshold mode's re-emission: the emitting pass into exactly sized segments cand_keys[seg_off[i], seg_off[i+1])
 // (i = query * grid + CTA), cursors [q_pad][grid] zeroed
