@@ -1363,7 +1363,7 @@ int stb_corpus_prepare_batch(stb_corpus *corpus) {
 // ---- K2 host calls -------------------------------------------------------------------------------------------
 // The record of the last K2 call, which stb_debug_batch_last returns: route, nq, two route words (routes 1-4,
 // 7 and 8: n_sample, stride; 5 and 10: retried queries, K1 queries; 6 and 9: tensor groups, K1 queries), n_seg,
-// seg_cap.  Routes 7-10 are 2, 3, 6 and 5 on the q8 copy, for corpora whose shadow does not fit.
+// seg_cap.  Routes 7-10 are the routes of a corpus whose shadow does not fit (k2_route).
 enum K2Route : uint32_t { kRouteV1 = 1, kRouteV2 = 2, kRouteFiltered = 3, kRouteFilteredK1 = 4, kRouteThreshold = 5,
                           kRouteSubsets = 6, kRouteQ8 = 7, kRouteFilteredQ8 = 8, kRouteSubsetsQ8 = 9,
                           kRouteThresholdQ8 = 10 };
@@ -1396,6 +1396,45 @@ static int batch_shadow_fits(stb_ctx *ctx, const stb_corpus *c) {
   return trial.alloc(bytes);
 }
 
+// The copy a K2 call reads: the 16-bit shadow, the q8 copy (where the shadow does not fit in HBM), or neither
+// (K1 answers).  k2_route(on_q8, route): the number of a pipeline's route where the q8 copy stands in for the
+// shadow: 2 -> 7, 3 -> 8, 6 -> 9, 5 -> 10.
+enum class K2Copy { kShadow, kQ8, kNone };
+static K2Route k2_route(bool on_q8, K2Route route) {
+  if (!on_q8) return route;
+  return route == kRouteV2 ? kRouteQ8 : route == kRouteFiltered ? kRouteFilteredQ8
+       : route == kRouteSubsets ? kRouteSubsetsQ8 : route == kRouteThreshold ? kRouteThresholdQ8 : route;
+}
+
+// Which copy a K2 call reads.  reads_shadow: the call's shadow plan fits (the shadow is built, batch_shadow);
+// q8_usable: its q8 plan fits.  With only the latter, the shadow is asked for with batch_shadow_fits; with neither,
+// nothing is asked (kNone, STB_OK).  A shadow that does not fit (STB_ERR_NOMEM) makes the call read the q8 copy,
+// built or extended here, if q8_usable and that copy can be used.  Hard errors are returned; otherwise *out says
+// which copy, whether the shadow was missing (which picks the route number) and, for kNone, why: STB_ERR_STATE
+// (rows K2 cannot normalise) or the shadow's STB_ERR_NOMEM, whose message is kept in shadow_err and is the last error.
+struct K2Choice {
+  K2Copy copy = K2Copy::kNone;
+  bool shadow_missing = false;
+  int status = STB_OK;
+  std::string shadow_err;
+};
+static int k2_choose_copy(stb_ctx *ctx, stb_corpus *corpus, bool reads_shadow, bool q8_usable, K2Choice *out) {
+  *out = K2Choice{};
+  if (!reads_shadow && !q8_usable) return STB_OK;
+  int rc = reads_shadow ? batch_shadow(ctx, corpus) : batch_shadow_fits(ctx, corpus);
+  if (rc == STB_OK && reads_shadow) out->copy = K2Copy::kShadow;
+  if (rc == STB_OK || rc == STB_ERR_STATE) { out->status = rc; return STB_OK; }
+  if (rc != STB_ERR_NOMEM) return rc;
+  out->shadow_missing = true;
+  out->status = rc;
+  out->shadow_err = stb_last_error();
+  if (!q8_usable) return STB_OK;
+  if ((rc = corpus_ensure_q8(ctx, corpus)) == STB_OK) { out->copy = K2Copy::kQ8; return STB_OK; }
+  if (rc != STB_ERR_NOMEM && rc != STB_ERR_STATE) return rc;
+  stb_set_error("%s", out->shadow_err.c_str());
+  return STB_OK;
+}
+
 // Keys per (query, CTA) segment of the emitting pass of v2 and route 6: ~5 expected at 10M rows / 132 CTAs.
 static constexpr uint32_t kSegCap = 64;
 
@@ -1423,46 +1462,6 @@ static BatchV2Plan batch_v2_plan(const stb_ctx *ctx, uint32_t n_cover, uint32_t 
   return {n_sample, fits ? n_cover / n_sample : 0u, fits};
 }
 
-// Pipeline v2 (batch_scan.cu): sampled threshold -> candidate-emitting wgmma epilogue -> exact finish.
-// Unfiltered (tile_ids == NULL) it samples and emits over the shadow tiles 0 .. n_cover-1 (the sample over
-// complete tiles only); filtered over the n_cover listed tiles tile_ids[] with the eligible-row bitmap.
-static int batch_v2_run(stb_ctx *ctx, const stb_corpus *corpus, const float *q_dev, uint32_t nq, uint32_t top_k,
-                        uint32_t n_cover, BatchV2Plan p, const uint32_t *tile_ids, const uint32_t *bitmap,
-                        stb_hit *out_hits_dev, uint32_t *out_status_dev) {
-  int rc;
-  const uint32_t m_tiles = (nq + 127) / 128, q_pad = m_tiles * 128;
-  const uint32_t n_tiles = (uint32_t)((corpus->n + 255) / 256);
-  const uint32_t n_emit = tile_ids ? n_cover : n_tiles;
-  const uint32_t n_seg = stb_batch_emit_grid(ctx, n_emit);
-  k2_record(ctx, tile_ids ? kRouteFiltered : kRouteV2, nq, p.n_sample, p.stride, n_seg, kSegCap);
-  if ((rc = ctx->b_qbad.reserve((size_t)q_pad)) != STB_OK) return rc;
-  if ((rc = ctx->bq_tiles.reserve((size_t)q_pad * 512)) != STB_OK) return rc;
-  if ((rc = ctx->b_tilemax.reserve((size_t)p.n_sample * q_pad)) != STB_OK) return rc;
-  if ((rc = ctx->b_thr.reserve((size_t)q_pad)) != STB_OK) return rc;
-  if ((rc = ctx->b_cnt.reserve((size_t)q_pad * n_seg)) != STB_OK) return rc;
-  if ((rc = ctx->b_keys.reserve((size_t)q_pad * n_seg * kSegCap)) != STB_OK) return rc;
-  STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
-  STB_CUDA(cudaMemsetAsync(ctx->b_cnt, 0, (size_t)q_pad * n_seg * sizeof(uint32_t), ctx->stream));
-  if ((rc = stb_launch_shadow_build(ctx, q_dev, nq, 128, ctx->bq_tiles, ctx->err_flag, 0, ctx->b_qbad)) != STB_OK) return rc;
-  if (tile_ids)
-    rc = stb_launch_batch_gemm_sample_filtered(ctx, ctx->bq_tiles, m_tiles, corpus->shadow, tile_ids, bitmap, p.n_sample,
-                                               p.stride, ctx->b_tilemax);
-  else
-    rc = stb_launch_batch_gemm_strided(ctx, ctx->bq_tiles, m_tiles, corpus->shadow, p.n_sample, p.stride, nullptr,
-                                       ctx->b_tilemax, nullptr);
-  if (rc != STB_OK) return rc;
-  if ((rc = stb_launch_batch_thresh(ctx, ctx->b_tilemax, p.n_sample, nq, q_pad, top_k, ctx->b_thr)) != STB_OK) return rc;
-  if (tile_ids)
-    rc = stb_launch_batch_gemm_emit_filtered(ctx, ctx->bq_tiles, m_tiles, corpus->shadow, tile_ids, bitmap, n_cover,
-                                             corpus->n, ctx->b_thr, ctx->b_cnt, ctx->b_keys, kSegCap);
-  else
-    rc = stb_launch_batch_gemm_emit(ctx, ctx->bq_tiles, m_tiles, corpus->shadow, n_tiles, corpus->n, ctx->b_thr,
-                                    ctx->b_cnt, ctx->b_keys, kSegCap);
-  if (rc != STB_OK) return rc;
-  return stb_launch_batch_finish2(ctx, ctx->b_keys, ctx->b_cnt, n_seg, kSegCap, nq, top_k, corpus->rows, corpus->n,
-                                  corpus->row_base, q_dev, ctx->b_qbad, out_hits_dev, out_status_dev);
-}
-
 // Route 7's sample size and fit rule (v2's, batch_scan.cu: "Route 7", with the q8 bounds in place of the shadow's
 // EPS).  A row's bounds are u, l = a +- w with w = s h_l1 + e_q (~0.011 on the benchmark's rows: s ~ 0.21 / 127,
 // h_l1 ~ ||q^||_1 / 2 ~ 6.4), and the threshold sits w below the sampled k-th cosine, so the emitted rows are those
@@ -1484,69 +1483,68 @@ static BatchV2Plan batch_q8_plan(uint32_t sm, uint32_t n_cover, uint32_t top_k) 
   return {n_sample, fits ? n_cover / n_sample : 0u, fits};
 }
 
-// The tensor passes of routes 7 and 8 (batch_scan.cu) on a built q8 copy: q8 query tiles -> sampled threshold on
-// the lower bounds -> upper-bound-emitting int8 wgmma epilogue -> the finish with the q8 proof.  Unfiltered
-// (tile_ids == NULL, route 7) over the corpus tiles 0 .. n_cover-1; filtered (route 8) over the n_cover listed
-// tiles tile_ids[] with the eligible-row bitmap.  p must fit.
-static int batch_q8_passes(stb_ctx *ctx, stb_corpus *corpus, const float *q_dev, uint32_t nq, uint32_t top_k,
-                           uint32_t n_cover, BatchV2Plan p, const uint32_t *tile_ids, const uint32_t *bitmap,
-                           stb_hit *out_hits_dev, uint32_t *out_status_dev) {
+// The plan of the top-k passes over n_cover tiles on `copy`
+static BatchV2Plan k2_plan(const stb_ctx *ctx, K2Copy copy, uint32_t n_cover, uint32_t top_k) {
+  return copy == K2Copy::kQ8 ? batch_q8_plan((uint32_t)ctx->sm_count, n_cover, top_k) : batch_v2_plan(ctx, n_cover, top_k);
+}
+
+// The query tiles of q_dev[0, nq) for a GEMM on `copy`, q_pad slots in ctx->bq_tiles with every query's unusable
+// flag in ctx->b_qbad: the shadow's, or the q8 copy's with the per-query constants in ctx->b_q8c
+static int k2_query_tiles(stb_ctx *ctx, K2Copy copy, const float *q_dev, uint32_t nq, uint32_t q_pad) {
+  if (copy == K2Copy::kQ8) return stb_launch_q8_query_tiles(ctx, q_dev, nq, q_pad, ctx->bq_tiles, ctx->b_q8c, ctx->b_qbad, nullptr);
+  STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
+  return stb_launch_shadow_build(ctx, q_dev, nq, 128, ctx->bq_tiles, ctx->err_flag, 0, ctx->b_qbad);
+}
+
+// GEMM pass p of the m_tiles query tiles in ctx->bq_tiles over the corpus's `copy`
+static int k2_gemm(stb_ctx *ctx, const stb_corpus *corpus, K2Copy copy, uint32_t m_tiles, StbGemmPass p) {
+  p.a_tiles = ctx->bq_tiles; p.m_tiles = m_tiles; p.n_rows = corpus->n;
+  return copy == K2Copy::kQ8 ? stb_launch_gemm_q8(ctx, p, corpus->q8, corpus->q8_scale, ctx->b_q8c)
+                             : stb_launch_gemm_shadow(ctx, p, corpus->shadow);
+}
+
+// The top-k passes of routes 2, 3, 7 and 8 (batch_scan.cu) on `copy`: query tiles -> sampled threshold ->
+// candidate-emitting GEMM -> exact finish (on the q8 copy: thresholds on the lower bounds, the upper bounds emitted,
+// the finish with the q8 proof).  Unfiltered (tile_ids == NULL) the sample covers the tiles 0 .. n_cover-1 and the
+// emission every tile; filtered, both cover the n_cover listed tiles tile_ids[] with the eligible-row bitmap.  p
+// (k2_plan over n_cover) must fit.  Every buffer comes first: a call refused for lack of memory leaves the record
+// as it was.
+static int k2_topk_run(stb_ctx *ctx, const stb_corpus *corpus, K2Copy copy, const float *q_dev, uint32_t nq,
+                       uint32_t top_k, uint32_t n_cover, BatchV2Plan p, const uint32_t *tile_ids, const uint32_t *bitmap,
+                       stb_hit *out_hits_dev, uint32_t *out_status_dev) {
   int rc;
+  const bool q8 = copy == K2Copy::kQ8;
   const uint32_t m_tiles = (nq + 127) / 128, q_pad = m_tiles * 128;
-  const uint32_t n_seg = stb_batch_emit_grid(ctx, n_cover);
-  // every buffer first: a call refused for lack of memory leaves the record as it was
+  const uint32_t n_emit = tile_ids ? n_cover : (uint32_t)((corpus->n + 255) / 256);
+  const uint32_t n_seg = stb_batch_emit_grid(ctx, n_emit);
   if ((rc = ctx->b_qbad.reserve((size_t)q_pad)) != STB_OK) return rc;
-  if ((rc = ctx->b_q8c.reserve((size_t)q_pad)) != STB_OK) return rc;
+  if (q8 && (rc = ctx->b_q8c.reserve((size_t)q_pad)) != STB_OK) return rc;
   if ((rc = ctx->bq_tiles.reserve((size_t)q_pad * 512)) != STB_OK) return rc;
   if ((rc = ctx->b_tilemax.reserve((size_t)p.n_sample * q_pad)) != STB_OK) return rc;
   if ((rc = ctx->b_thr.reserve((size_t)q_pad)) != STB_OK) return rc;
   if ((rc = ctx->b_cnt.reserve((size_t)q_pad * n_seg)) != STB_OK) return rc;
   if ((rc = ctx->b_keys.reserve((size_t)q_pad * n_seg * kSegCap)) != STB_OK) return rc;
-  k2_record(ctx, tile_ids ? kRouteFilteredQ8 : kRouteQ8, nq, p.n_sample, p.stride, n_seg, kSegCap);
+  k2_record(ctx, k2_route(q8, tile_ids ? kRouteFiltered : kRouteV2), nq, p.n_sample, p.stride, n_seg, kSegCap);
   STB_CUDA(cudaMemsetAsync(ctx->b_cnt, 0, (size_t)q_pad * n_seg * sizeof(uint32_t), ctx->stream));
-  if ((rc = stb_launch_q8_query_tiles(ctx, q_dev, nq, q_pad, ctx->bq_tiles, ctx->b_q8c, ctx->b_qbad, nullptr)) != STB_OK)
-    return rc;
-  if (tile_ids)
-    rc = stb_launch_batch_q8_gemm_sample_filtered(ctx, ctx->bq_tiles, ctx->b_q8c, m_tiles, corpus->q8, corpus->q8_scale,
-                                                  corpus->n, tile_ids, bitmap, p.n_sample, p.stride, ctx->b_tilemax);
-  else
-    rc = stb_launch_batch_q8_gemm_sample(ctx, ctx->bq_tiles, ctx->b_q8c, m_tiles, corpus->q8, corpus->q8_scale, corpus->n,
-                                         p.n_sample, p.stride, ctx->b_tilemax);
+  if ((rc = k2_query_tiles(ctx, copy, q_dev, nq, q_pad)) != STB_OK) return rc;
+  StbGemmPass pass;
+  pass.select = tile_ids ? STB_GEMM_LISTED : STB_GEMM_ALL;
+  pass.tile_ids = tile_ids; pass.bitmap = bitmap;
+  pass.n_tiles = p.n_sample; pass.tile_stride = p.stride; pass.tilemax = ctx->b_tilemax;
+  if ((rc = k2_gemm(ctx, corpus, copy, m_tiles, pass)) != STB_OK) return rc;
+  // the q8 copy's threshold sits STB_Q8_SCAN_EPS lower, and an unusable query (zero, or not normalisable) emits
+  // nothing and comes back unproven
+  rc = q8 ? stb_launch_batch_thresh(ctx, ctx->b_tilemax, p.n_sample, nq, q_pad, top_k, ctx->b_thr, (float)STB_Q8_SCAN_EPS, ctx->b_qbad)
+          : stb_launch_batch_thresh(ctx, ctx->b_tilemax, p.n_sample, nq, q_pad, top_k, ctx->b_thr);
   if (rc != STB_OK) return rc;
-  // an unusable query (zero, or not normalisable) emits nothing and comes back unproven
-  if ((rc = stb_launch_batch_thresh(ctx, ctx->b_tilemax, p.n_sample, nq, q_pad, top_k, ctx->b_thr, (float)STB_Q8_SCAN_EPS,
-                                    ctx->b_qbad)) != STB_OK) return rc;
-  if (tile_ids)
-    rc = stb_launch_batch_q8_gemm_emit_filtered(ctx, ctx->bq_tiles, ctx->b_q8c, m_tiles, corpus->q8, corpus->q8_scale,
-                                                corpus->n, tile_ids, bitmap, n_cover, ctx->b_thr, ctx->b_cnt, ctx->b_keys,
-                                                kSegCap);
-  else
-    rc = stb_launch_batch_q8_gemm_emit(ctx, ctx->bq_tiles, ctx->b_q8c, m_tiles, corpus->q8, corpus->q8_scale, corpus->n,
-                                       ctx->b_thr, ctx->b_cnt, ctx->b_keys, kSegCap);
-  if (rc != STB_OK) return rc;
+  pass.epi = STB_EPI_EMIT;
+  pass.n_tiles = n_emit; pass.tile_stride = 1; pass.tilemax = nullptr;
+  pass.thr = ctx->b_thr; pass.cand_cnt = ctx->b_cnt; pass.cand_keys = ctx->b_keys; pass.cand_cap = kSegCap;
+  if ((rc = k2_gemm(ctx, corpus, copy, m_tiles, pass)) != STB_OK) return rc;
   return stb_launch_batch_finish2(ctx, ctx->b_keys, ctx->b_cnt, n_seg, kSegCap, nq, top_k, corpus->rows, corpus->n,
-                                  corpus->row_base, q_dev, ctx->b_qbad, out_hits_dev, out_status_dev, corpus->q8_scale,
-                                  ctx->b_q8c, ctx->b_thr);
-}
-
-// Route 7: builds or extends the q8 copy first (its status is returned if it cannot be used), then runs
-// batch_q8_passes over every corpus tile.  A batch that does not fit the plan comes back with every query unproven.
-static int batch_q8_run(stb_ctx *ctx, stb_corpus *corpus, const float *q_dev, uint32_t nq, uint32_t top_k,
-                        stb_hit *out_hits_dev, uint32_t *out_status_dev) {
-  int rc;
-  if ((rc = corpus_ensure_q8(ctx, corpus)) != STB_OK) return rc;
-  const uint32_t n_tiles = (uint32_t)((corpus->n + 255) / 256);
-  const BatchV2Plan p = batch_q8_plan((uint32_t)ctx->sm_count, n_tiles, top_k);
-  if (!p.fits) {
-    std::vector<stb_hit> pad((size_t)nq * top_k);
-    stb_pad_hits(pad.data(), 0, pad.size());
-    STB_CUDA(cudaMemcpyAsync(out_hits_dev, pad.data(), pad.size() * sizeof(stb_hit), cudaMemcpyHostToDevice, ctx->stream));
-    STB_CUDA(cudaMemsetAsync(out_status_dev, 0, (size_t)nq * 2 * sizeof(uint32_t), ctx->stream));
-    STB_CUDA(cudaStreamSynchronize(ctx->stream));       // `pad` is read by the copy
-    k2_record(ctx, kRouteQ8, nq);
-    return STB_OK;
-  }
-  return batch_q8_passes(ctx, corpus, q_dev, nq, top_k, n_tiles, p, nullptr, nullptr, out_hits_dev, out_status_dev);
+                                  corpus->row_base, q_dev, ctx->b_qbad, out_hits_dev, out_status_dev,
+                                  q8 ? (const float *)corpus->q8_scale : nullptr, q8 ? (const float4 *)ctx->b_q8c : nullptr,
+                                  q8 ? (const float *)ctx->b_thr : nullptr);
 }
 
 // The listed tiles of clipped local [begin, end) pairs: the shadow tiles a range touches (ascending, disjoint
@@ -1597,13 +1595,12 @@ static int k2_complete(stb_ctx *ctx, const stb_corpus *corpus, const float *q, u
   return STB_OK;
 }
 
-// The filtered tensor passes for nq host queries over `loc` (clipped local [begin, end) pairs) and its listed tiles:
-// filtered v2 on the shadow (route 3), or, q8, route 7's passes on the q8 copy over the listed tiles (route 8);
-// `plan` (v2's or the q8 plan, over the listed tiles) must fit.  Hits land in out_hits [nq][top_k], {hits, proven}
-// in status [nq][2].
-static int filtered_tensor_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, uint32_t nq, uint32_t top_k,
-                               const std::vector<uint32_t> &loc, const std::vector<uint32_t> &tiles, BatchV2Plan plan,
-                               bool q8, stb_hit *out_hits, uint32_t *status) {
+// The filtered top-k passes for nq host queries over `loc` (clipped local [begin, end) pairs) and its listed tiles, on
+// `copy` (route 3 on the shadow, 8 on the q8 copy); k2_plan over the listed tiles must fit.  Hits land in
+// out_hits [nq][top_k], {hits, proven} in status [nq][2].
+static int filtered_tensor_run(stb_ctx *ctx, stb_corpus *corpus, K2Copy copy, const float *q, uint32_t nq, uint32_t top_k,
+                               const std::vector<uint32_t> &loc, const std::vector<uint32_t> &tiles, stb_hit *out_hits,
+                               uint32_t *status) {
   int rc;
   const uint64_t n_words = (corpus->n + 255) / 256 * 8;
   if ((rc = ctx->bq_dev.reserve((size_t)nq * STB_D)) != STB_OK) return rc;
@@ -1617,11 +1614,8 @@ static int filtered_tensor_run(stb_ctx *ctx, stb_corpus *corpus, const float *q,
   STB_CUDA(cudaMemcpyAsync(ctx->b_ftiles, tiles.data(), tiles.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
   if ((rc = stb_launch_row_bitmap(ctx, ctx->b_franges, (uint32_t)(loc.size() / 2), n_words, ctx->b_fbits)) != STB_OK) return rc;
   const uint32_t n_listed = (uint32_t)tiles.size();
-  if (q8)
-    rc = batch_q8_passes(ctx, corpus, ctx->bq_dev, nq, top_k, n_listed, plan, ctx->b_ftiles, ctx->b_fbits, ctx->bh_dev, ctx->bs_dev);
-  else
-    rc = batch_v2_run(ctx, corpus, ctx->bq_dev, nq, top_k, n_listed, plan, ctx->b_ftiles, ctx->b_fbits, ctx->bh_dev, ctx->bs_dev);
-  if (rc != STB_OK) return rc;
+  if ((rc = k2_topk_run(ctx, corpus, copy, ctx->bq_dev, nq, top_k, n_listed, k2_plan(ctx, copy, n_listed, top_k), ctx->b_ftiles,
+                        ctx->b_fbits, ctx->bh_dev, ctx->bs_dev)) != STB_OK) return rc;
   STB_CUDA(cudaMemcpyAsync(out_hits, ctx->bh_dev, (size_t)nq * top_k * sizeof(stb_hit), cudaMemcpyDeviceToHost, ctx->stream));
   STB_CUDA(cudaMemcpyAsync(status, ctx->bs_dev, (size_t)nq * 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
   STB_CUDA(cudaStreamSynchronize(ctx->stream));        // `loc` and `tiles` are read by the copies above
@@ -1630,11 +1624,10 @@ static int filtered_tensor_run(stb_ctx *ctx, stb_corpus *corpus, const float *q,
 
 // The store query (stb_search in STB_MODE_STORE_QUERY) for a batch, over `loc`: the caller's row_ranges clipped
 // to local [begin, end) pairs (K1 answers with the former).  The eligible rows' bitmap and the listed tiles both
-// come from `loc`; filtered v2 runs when its plan fits over the listed tiles (route 3).  Where the shadow does not
-// fit, route 8 runs the same passes on the q8 copy when the q8 plan fits over the listed tiles, whether or not v2's
-// does (the shadow is asked for whenever either plan fits, and built only where v2's fits).  K1 answers every query
-// the tensor passes leave unproven, and all of them when nothing runs on the tensor cores (route 4).  The cap is
-// applied on the host: store-query hits are a prefix of the uncapped top-k.
+// come from `loc`; the filtered top-k passes run on the copy k2_choose_copy picks from the two plans over the listed
+// tiles (route 3 on the shadow, 8 on the q8 copy).  K1 answers every query the tensor passes leave unproven, and
+// all of them when nothing runs on the tensor cores (route 4).  The cap is applied on the host: store-query hits
+// are a prefix of the uncapped top-k.
 static int batch_filtered_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, uint32_t nq, uint32_t top_k, int has_max,
                               double max_distance, const std::vector<uint32_t> &loc, const uint64_t *row_ranges,
                               uint32_t n_ranges, stb_hit *out_hits, uint32_t *out_n) {
@@ -1645,20 +1638,12 @@ static int batch_filtered_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, 
                        [](uint32_t) { return K2Answer{K2Answer::kEmpty}; }, out_hits, out_n);
   const std::vector<uint32_t> tiles = listed_tiles(loc);
   const uint32_t n_listed = (uint32_t)tiles.size();
-  BatchV2Plan plan = batch_v2_plan(ctx, n_listed, top_k);
-  const BatchV2Plan q8_plan = batch_q8_plan((uint32_t)ctx->sm_count, n_listed, top_k);
-  bool tensor_ok = false, q8 = false;
-  if (plan.fits || q8_plan.fits) {
-    rc = plan.fits ? batch_shadow(ctx, corpus) : batch_shadow_fits(ctx, corpus);
-    if (rc == STB_OK) tensor_ok = plan.fits;              // the shadow fits but not its plan: K1 answers all, as before
-    else if (rc == STB_ERR_NOMEM) {
-      // the shadow does not fit: route 8, if its plan fits and the q8 copy can be used (else K1 answers all)
-      if (q8_plan.fits && (rc = corpus_ensure_q8(ctx, corpus)) == STB_OK) { tensor_ok = q8 = true; plan = q8_plan; }
-      else if (q8_plan.fits && rc != STB_ERR_NOMEM && rc != STB_ERR_STATE) return rc;
-    } else if (rc != STB_ERR_STATE) return rc;            // STB_ERR_STATE: un-normalisable rows, K1 handles them
-  }
+  K2Choice ch;
+  if ((rc = k2_choose_copy(ctx, corpus, k2_plan(ctx, K2Copy::kShadow, n_listed, top_k).fits,
+                           k2_plan(ctx, K2Copy::kQ8, n_listed, top_k).fits, &ch)) != STB_OK) return rc;
+  const bool tensor_ok = ch.copy != K2Copy::kNone;
   std::vector<uint32_t> status((size_t)nq * 2, 0);
-  if (tensor_ok && (rc = filtered_tensor_run(ctx, corpus, q, nq, top_k, loc, tiles, plan, q8, out_hits, status.data())) != STB_OK)
+  if (tensor_ok && (rc = filtered_tensor_run(ctx, corpus, ch.copy, q, nq, top_k, loc, tiles, out_hits, status.data())) != STB_OK)
     return rc;
   return k2_complete(ctx, corpus, q, nq, top_k, has_max, max_distance, STB_MODE_STORE_QUERY, [&](uint32_t i) -> K2Answer {
     if (tensor_ok && status[2 * i + 1]) return {K2Answer::kProven, out_hits + (size_t)i * top_k, status[2 * i]};
@@ -1666,11 +1651,7 @@ static int batch_filtered_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, 
   }, out_hits, out_n);
 }
 
-extern "C" {
-
-}  // extern "C"
-
-// stb_search_batch_dev; q8_route: route 7 whatever the shadow's state (stb_debug_batch_q8)
+// stb_search_batch_dev; q8_route: the q8 copy whatever the shadow's state (stb_debug_batch_q8)
 static int batch_dev_impl(stb_ctx *ctx, const stb_corpus *corpus_c, const float *q_dev, uint32_t nq, uint32_t top_k,
                           stb_hit *out_hits_dev, uint32_t *out_status_dev, bool q8_route) {
   int rc = ctx_use(ctx);
@@ -1681,24 +1662,40 @@ static int batch_dev_impl(stb_ctx *ctx, const stb_corpus *corpus_c, const float 
   if (nq == 0) return STB_OK;
   if (top_k == 0 || top_k > 1024) { stb_set_error("search_batch_dev: top_k must be 1..1024"); return STB_ERR_ARG; }
   if (corpus->n == 0) { stb_set_error("search_batch_dev: empty corpus"); return STB_ERR_STATE; }
-  if (q8_route) return batch_q8_run(ctx, corpus, q_dev, nq, top_k, out_hits_dev, out_status_dev);
-  if ((rc = batch_shadow(ctx, corpus)) != STB_OK) {
-    if (rc != STB_ERR_NOMEM) return rc;
-    // the shadow does not fit in HBM: route 7 reads the q8 copy instead.  If that copy cannot be used either, the
-    // call is refused as before, with the shadow's status and message and nothing written
-    std::string shadow_err = stb_last_error();
-    const int q8_rc = batch_q8_run(ctx, corpus, q_dev, nq, top_k, out_hits_dev, out_status_dev);
-    if (q8_rc == STB_ERR_NOMEM || q8_rc == STB_ERR_STATE) { stb_set_error("%s", shadow_err.c_str()); return rc; }
-    return q8_rc;
+  K2Choice ch;
+  if (q8_route) {
+    if ((rc = corpus_ensure_q8(ctx, corpus)) != STB_OK) return rc;
+    ch.copy = K2Copy::kQ8;
+  } else if ((rc = k2_choose_copy(ctx, corpus, true, true, &ch)) != STB_OK) {
+    return rc;
   }
+  // neither copy can be used: refused with the status and message that say why, nothing written
+  if (ch.copy == K2Copy::kNone) return ch.status;
   const uint32_t m_tiles = (nq + 127) / 128, q_pad = m_tiles * 128;
   const uint32_t n_tiles = (uint32_t)((corpus->n + 255) / 256), n_sub = n_tiles * 8;
-  // Pipeline v2 (default, batch_v2_run).  Proves every query for any top_k <= 64 unless a capacity
-  // overflows.  The round-1 maxima/select/finish pipeline (v1) runs for top_k > 64 and wherever v2 does not fit.
-  const uint32_t n_full = (uint32_t)(corpus->n / 256);
-  const BatchV2Plan plan = batch_v2_plan(ctx, n_full, top_k);
-  if (plan.fits) return batch_v2_run(ctx, corpus, q_dev, nq, top_k, n_full, plan, nullptr, nullptr, out_hits_dev, out_status_dev);
-  // one flag per query, written by the query shadow build: a query that cannot be normalised in fp32
+  // The top-k passes (k2_topk_run) prove every query for any top_k <= 64 unless a capacity overflows.  Their sample
+  // covers the shadow's complete tiles (a padding row must never stand in for a real one), or any tile of the q8
+  // copy, whose maxima leave out the rows past n.
+  const uint32_t n_cover = ch.copy == K2Copy::kQ8 ? n_tiles : (uint32_t)(corpus->n / 256);
+  const BatchV2Plan plan = k2_plan(ctx, ch.copy, n_cover, top_k);
+  if (plan.fits) {
+    rc = k2_topk_run(ctx, corpus, ch.copy, q_dev, nq, top_k, n_cover, plan, nullptr, nullptr, out_hits_dev, out_status_dev);
+    // where the q8 copy stands in for the shadow, running out of memory there is the shadow's refusal
+    if (ch.shadow_missing && (rc == STB_ERR_NOMEM || rc == STB_ERR_STATE)) { stb_set_error("%s", ch.shadow_err.c_str()); return STB_ERR_NOMEM; }
+    return rc;
+  }
+  if (ch.copy == K2Copy::kQ8) {
+    // the q8 plan does not fit: every query comes back unproven
+    std::vector<stb_hit> pad((size_t)nq * top_k);
+    stb_pad_hits(pad.data(), 0, pad.size());
+    STB_CUDA(cudaMemcpyAsync(out_hits_dev, pad.data(), pad.size() * sizeof(stb_hit), cudaMemcpyHostToDevice, ctx->stream));
+    STB_CUDA(cudaMemsetAsync(out_status_dev, 0, (size_t)nq * 2 * sizeof(uint32_t), ctx->stream));
+    STB_CUDA(cudaStreamSynchronize(ctx->stream));       // `pad` is read by the copy
+    k2_record(ctx, kRouteQ8, nq);
+    return STB_OK;
+  }
+  // The round-1 maxima/select/finish pipeline (v1) runs on the shadow for top_k > 64 and wherever v2 does not fit.
+  // One flag per query, written by the query shadow build: a query that cannot be normalised in fp32
   // has a zero (or NaN) shadow whose scores bound nothing, and both finish kernels report it unproven
   if ((rc = ctx->b_qbad.reserve((size_t)q_pad)) != STB_OK) return rc;
   k2_record(ctx, kRouteV1, nq);
@@ -1711,9 +1708,10 @@ static int batch_dev_impl(stb_ctx *ctx, const stb_corpus *corpus_c, const float 
   if ((rc = ctx->b_tilemax.reserve((size_t)n_tiles * q_pad)) != STB_OK) return rc;
   if ((rc = ctx->b_cand.reserve((size_t)q_pad * n_slices * 32)) != STB_OK) return rc;
   // query tiles: padding queries beyond nq are written as zeros by the shadow builder
-  STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
-  if ((rc = stb_launch_shadow_build(ctx, q_dev, nq, 128, ctx->bq_tiles, ctx->err_flag, 0, ctx->b_qbad)) != STB_OK) return rc;
-  if ((rc = stb_launch_batch_gemm(ctx, ctx->bq_tiles, m_tiles, corpus->shadow, n_tiles, ctx->b_submax, ctx->b_tilemax, nullptr)) != STB_OK) return rc;
+  if ((rc = k2_query_tiles(ctx, K2Copy::kShadow, q_dev, nq, q_pad)) != STB_OK) return rc;
+  StbGemmPass maxima;
+  maxima.n_tiles = n_tiles; maxima.submax = ctx->b_submax; maxima.tilemax = ctx->b_tilemax;
+  if ((rc = k2_gemm(ctx, corpus, K2Copy::kShadow, m_tiles, maxima)) != STB_OK) return rc;
   // two-level selection: the best tiles by tile maximum (1/8 of the data), refined to
   // sub-tiles inside the finish kernel
   if ((rc = stb_launch_batch_select(ctx, ctx->b_tilemax, n_tiles, q_pad, n_slices, ctx->b_cand)) != STB_OK) return rc;
@@ -1853,32 +1851,22 @@ static void subsets_work(const std::vector<std::vector<uint32_t>> &tiles_of, con
 }
 
 // Route 9: stb_search_batch_subsets where the shadow does not fit, with several groups (group[i]: query i's group
-// in `lists`, or kNone for a query with no clipped range; listed[g]: group g's listed tiles).  Each group whose q8
-// plan fits over its listed tiles runs route 8's passes on its own queries, one group after another; K1 answers the
-// other groups (all of them when the q8 copy cannot be used) and every query the passes leave unproven.
-static int subsets_q8_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, uint32_t nq, uint32_t top_k, int has_max,
-                          double max_distance, const std::vector<uint32_t> &group,
+// in `lists`, or kNone for a query with no clipped range; listed[g]: group g's listed tiles).  On the q8 copy (copy
+// kQ8), each group whose q8 plan fits over its listed tiles runs the filtered top-k passes on its own queries, one
+// group after another; K1 answers the other groups (all of them with copy kNone) and every query the passes leave
+// unproven.
+static int subsets_q8_run(stb_ctx *ctx, stb_corpus *corpus, K2Copy copy, const float *q, uint32_t nq, uint32_t top_k,
+                          int has_max, double max_distance, const std::vector<uint32_t> &group,
                           const std::vector<const std::vector<uint32_t> *> &lists,
                           const std::vector<std::vector<uint32_t>> &listed, const uint64_t *range_offsets,
                           const uint64_t *row_ranges, stb_hit *out_hits, uint32_t *out_n) {
   constexpr uint32_t kNone = 0xffffffffu;
   int rc;
-  k2_record(ctx, kRouteSubsetsQ8, nq);
   const uint32_t G = (uint32_t)lists.size();
   std::vector<std::vector<uint32_t>> members(G);
   for (uint32_t i = 0; i < nq; ++i)
     if (group[i] != kNone) members[group[i]].push_back(i);
-  std::vector<BatchV2Plan> plan(G);
-  bool any = false;
-  for (uint32_t g = 0; g < G; ++g) {
-    plan[g] = batch_q8_plan((uint32_t)ctx->sm_count, (uint32_t)listed[g].size(), top_k);
-    any |= plan[g].fits;
-  }
-  if (any) {
-    rc = corpus_ensure_q8(ctx, corpus);
-    if (rc == STB_ERR_NOMEM || rc == STB_ERR_STATE) any = false;      // K1 answers every query
-    else if (rc != STB_OK) return rc;
-  }
+  const bool any = copy == K2Copy::kQ8;
   // per caller query: the tensor result and {hits, proven}; the output is written only once every group has run,
   // so a group refused for lack of scratch leaves it untouched
   std::vector<uint32_t> status((size_t)nq * 2, 0), gstatus;
@@ -1886,14 +1874,14 @@ static int subsets_q8_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, uint
   std::vector<float> gq;
   uint32_t n_tensor = 0;
   for (uint32_t g = 0; any && g < G; ++g) {
-    if (!plan[g].fits) continue;
+    if (!k2_plan(ctx, copy, (uint32_t)listed[g].size(), top_k).fits) continue;
     const std::vector<uint32_t> &mem = members[g];
     const uint32_t m = (uint32_t)mem.size();
     gq.resize((size_t)m * STB_D);
     ghits.resize((size_t)m * top_k);
     gstatus.assign((size_t)m * 2, 0);
     for (uint32_t j = 0; j < m; ++j) memcpy(gq.data() + (size_t)j * STB_D, q + (size_t)mem[j] * STB_D, STB_D * sizeof(float));
-    if ((rc = filtered_tensor_run(ctx, corpus, gq.data(), m, top_k, *lists[g], listed[g], plan[g], true, ghits.data(),
+    if ((rc = filtered_tensor_run(ctx, corpus, copy, gq.data(), m, top_k, *lists[g], listed[g], ghits.data(),
                                   gstatus.data())) != STB_OK) return rc;
     for (uint32_t j = 0; j < m; ++j) {
       memcpy(hits.data() + (size_t)mem[j] * top_k, ghits.data() + (size_t)j * top_k, (size_t)top_k * sizeof(stb_hit));
@@ -1919,8 +1907,8 @@ extern "C" {
 // Otherwise every group whose v2 plan fits runs on the tensor cores, each occupying whole 64-query halves of
 // the query slots: one sampling pass over the union of the groups' sampled tiles, the per-slot threshold, one
 // emitting pass over the union of their listed tiles, finish2 over the groups' queries in compact order.  K1
-// answers the other groups and every query the tensor passes leave unproven.  Where the shadow does not fit and a
-// group fits either plan, route 9 (subsets_q8_run) runs instead.
+// answers the other groups and every query the tensor passes leave unproven.  Where the shadow does not fit,
+// route 9 (subsets_q8_run) runs instead.
 int stb_search_batch_subsets(stb_ctx *ctx, const stb_corpus *corpus_c, const float *q, uint32_t nq, uint32_t top_k,
                              int has_max, double max_distance, const uint64_t *range_offsets, const uint64_t *row_ranges,
                              stb_hit *out_hits, uint32_t *out_n) {
@@ -1991,15 +1979,15 @@ int stb_search_batch_subsets(stb_ctx *ctx, const stb_corpus *corpus_c, const flo
   if ((uint64_t)tgroups.size() * n_tiles >= UINT32_MAX) tgroups.clear();   // mask slots are 32-bit
   // the shadow is asked for whenever a group fits either plan, and built only where route 6 reads it
   bool q8_fits = false;
-  for (uint32_t g = 0; g < G && !q8_fits; ++g) q8_fits = batch_q8_plan((uint32_t)ctx->sm_count, (uint32_t)listed[g].size(), top_k).fits;
-  if (!tgroups.empty() || q8_fits) {
-    rc = !tgroups.empty() ? batch_shadow(ctx, corpus) : batch_shadow_fits(ctx, corpus);
-    if (rc == STB_ERR_NOMEM)                               // the shadow does not fit: route 9
-      return subsets_q8_run(ctx, corpus, q, nq, top_k, has_max, max_distance, group, lists, listed, range_offsets,
-                            row_ranges, out_hits, out_n);
-    if (rc == STB_ERR_STATE) tgroups.clear();              // un-normalisable rows: K1 answers every query
-    else if (rc != STB_OK) return rc;
-  }
+  for (uint32_t g = 0; g < G && !q8_fits; ++g) q8_fits = k2_plan(ctx, K2Copy::kQ8, (uint32_t)listed[g].size(), top_k).fits;
+  K2Choice ch;
+  rc = k2_choose_copy(ctx, corpus, !tgroups.empty(), q8_fits, &ch);
+  if (ch.shadow_missing) k2_record(ctx, kRouteSubsetsQ8, nq);       // even if K1 answers every query
+  if (rc != STB_OK) return rc;
+  if (ch.shadow_missing)
+    return subsets_q8_run(ctx, corpus, ch.copy, q, nq, top_k, has_max, max_distance, group, lists, listed, range_offsets,
+                          row_ranges, out_hits, out_n);
+  if (ch.copy != K2Copy::kShadow) tgroups.clear();         // e.g. un-normalisable rows: K1 answers every query
   const uint32_t T = (uint32_t)tgroups.size();
   for (uint32_t tg = 0; tg < T; ++tg) tensor[tgroups[tg]] = tg;
   // query slots: tensor group tg owns halves [half0[tg], half0[tg] + n_halves[tg]), its queries in caller order;
@@ -2084,13 +2072,18 @@ int stb_search_batch_subsets(stb_ctx *ctx, const stb_corpus *corpus_c, const flo
     if ((rc = stb_launch_shadow_build(ctx, ctx->s_qslots, q_pad, 128, ctx->bq_tiles, ctx->err_flag, 0, ctx->b_qbad)) != STB_OK) return rc;
     if ((rc = stb_launch_batch_slots_prep(ctx, d_slot_row, ctx->b_qbad, q_pad, ctx->s_qbad, ctx->b_tilemax,
                                           (uint64_t)n_cols * q_pad)) != STB_OK) return rc;
-    if ((rc = stb_launch_batch_gemm_sample_work(ctx, ctx->bq_tiles, corpus->shadow, W + o_ts, (uint32_t)ws.tiles.size(), W + o_cs,
-                                                W + o_os, reinterpret_cast<const uint4 *>(W + o_is), ctx->b_fbits, n_cols,
-                                                ctx->b_tilemax)) != STB_OK) return rc;
+    StbGemmPass pass;
+    pass.select = STB_GEMM_WORK; pass.bitmap = ctx->b_fbits;
+    pass.tile_ids = W + o_ts; pass.n_tiles = (uint32_t)ws.tiles.size(); pass.cta_tiles = W + o_cs; pass.item_off = W + o_os;
+    pass.items = reinterpret_cast<const uint4 *>(W + o_is); pass.tile_stride = n_cols; pass.tilemax = ctx->b_tilemax;
+    if ((rc = k2_gemm(ctx, corpus, K2Copy::kShadow, m_tiles, pass)) != STB_OK) return rc;
     if ((rc = stb_launch_batch_thresh(ctx, ctx->b_tilemax, n_cols, q_pad, q_pad, top_k, ctx->b_thr)) != STB_OK) return rc;
-    if ((rc = stb_launch_batch_gemm_emit_work(ctx, ctx->bq_tiles, corpus->shadow, W + o_te, (uint32_t)we.tiles.size(), W + o_ce,
-                                              W + o_oe, reinterpret_cast<const uint4 *>(W + o_ie), ctx->b_fbits, d_slot_row,
-                                              corpus->n, ctx->b_thr, ctx->b_cnt, ctx->b_keys, kSegCap)) != STB_OK) return rc;
+    pass.epi = STB_EPI_EMIT;
+    pass.tile_ids = W + o_te; pass.n_tiles = (uint32_t)we.tiles.size(); pass.cta_tiles = W + o_ce; pass.item_off = W + o_oe;
+    pass.items = reinterpret_cast<const uint4 *>(W + o_ie); pass.tile_stride = 1; pass.tilemax = nullptr;
+    pass.slot_row = d_slot_row; pass.thr = ctx->b_thr; pass.cand_cnt = ctx->b_cnt; pass.cand_keys = ctx->b_keys;
+    pass.cand_cap = kSegCap;
+    if ((rc = k2_gemm(ctx, corpus, K2Copy::kShadow, m_tiles, pass)) != STB_OK) return rc;
     if ((rc = stb_launch_batch_finish2(ctx, ctx->b_keys, ctx->b_cnt, n_seg, kSegCap, nt, top_k, corpus->rows, corpus->n,
                                        corpus->row_base, ctx->bq_dev, ctx->s_qbad, ctx->bh_dev, ctx->bs_dev)) != STB_OK) return rc;
     STB_CUDA(cudaMemcpyAsync(hits.data(), ctx->bh_dev, hits.size() * sizeof(stb_hit), cudaMemcpyDeviceToHost, ctx->stream));
@@ -2131,7 +2124,7 @@ static float thr_emission_value(double max_distance, double eps) {
   return f;
 }
 
-// One chunk of queries q[0, n) (global indices c0 ..) on the tensor cores: the shadow (route 5) or, q8, the q8
+// One chunk of queries q[0, n) (global indices c0 ..) on the tensor cores, on `copy`: the shadow (route 5) or the q8
 // copy (route 10: the queries' q8 tiles and unusable flags, K1's upper bounds u as the emitted scores).  On return
 // slot_query[s] / pass[s] are the chunk-local query and hit count of every answered slot, k1 lists the queries K1
 // must answer, and the sorted hits of slot s sit at ctx->t_buf (distance bits at [0, K), rows at [K, 2K)) from
@@ -2142,7 +2135,7 @@ struct ThrChunk {
   uint32_t retried = 0;
 };
 static int thr_chunk_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, uint32_t c0, uint32_t n, double max_distance,
-                         float t, bool q8, ThrChunk *out) {
+                         float t, K2Copy copy, ThrChunk *out) {
   int rc;
   const uint32_t m_tiles = (n + 127) / 128, q_pad = m_tiles * 128;
   const uint32_t n_tiles = (uint32_t)((corpus->n + 255) / 256);
@@ -2153,22 +2146,17 @@ static int thr_chunk_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, uint3
   if ((rc = ctx->b_qbad.reserve((size_t)q_pad)) != STB_OK) return rc;
   if ((rc = ctx->bq_tiles.reserve((size_t)q_pad * 512)) != STB_OK) return rc;
   if ((rc = ctx->b_keys.reserve((size_t)q_pad * n_seg * STB_THR_SEG_CAP)) != STB_OK) return rc;
-  if (q8 && (rc = ctx->b_q8c.reserve((size_t)q_pad)) != STB_OK) return rc;
+  if (copy == K2Copy::kQ8 && (rc = ctx->b_q8c.reserve((size_t)q_pad)) != STB_OK) return rc;
   STB_CUDA(cudaMemcpyAsync(ctx->bq_dev, q, (size_t)n * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-  STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
   STB_CUDA(cudaMemsetAsync(cnt, 0, (size_t)q_pad * n_seg * sizeof(uint32_t), ctx->stream));
-  if (q8) {
-    // the q8 flags mark the zero query and the unnormalisable ones: their threshold is +inf, K1 answers them
-    if ((rc = stb_launch_q8_query_tiles(ctx, ctx->bq_dev, n, q_pad, ctx->bq_tiles, ctx->b_q8c, ctx->b_qbad, nullptr)) != STB_OK ||
-        (rc = stb_launch_batch_thr_dist(ctx, ctx->bq_dev, ctx->b_qbad, n, q_pad, t, thr)) != STB_OK ||
-        (rc = stb_launch_batch_q8_gemm_emit(ctx, ctx->bq_tiles, ctx->b_q8c, m_tiles, corpus->q8, corpus->q8_scale, corpus->n,
-                                            thr, cnt, ctx->b_keys, STB_THR_SEG_CAP)) != STB_OK) return rc;
-  } else {
-    if ((rc = stb_launch_shadow_build(ctx, ctx->bq_dev, n, 128, ctx->bq_tiles, ctx->err_flag, 0, ctx->b_qbad)) != STB_OK) return rc;
-    if ((rc = stb_launch_batch_thr_dist(ctx, ctx->bq_dev, ctx->b_qbad, n, q_pad, t, thr)) != STB_OK) return rc;
-    if ((rc = stb_launch_batch_gemm_emit(ctx, ctx->bq_tiles, m_tiles, corpus->shadow, n_tiles, corpus->n, thr, cnt,
-                                         ctx->b_keys, STB_THR_SEG_CAP)) != STB_OK) return rc;
-  }
+  // the unusable flags mark the queries that cannot be normalised (on the q8 copy, the zero query too): their
+  // threshold is +inf, K1 answers them
+  StbGemmPass emit;
+  emit.epi = STB_EPI_EMIT; emit.n_tiles = n_tiles; emit.thr = thr; emit.cand_cnt = cnt; emit.cand_keys = ctx->b_keys;
+  emit.cand_cap = STB_THR_SEG_CAP;
+  if ((rc = k2_query_tiles(ctx, copy, ctx->bq_dev, n, q_pad)) != STB_OK) return rc;
+  if ((rc = stb_launch_batch_thr_dist(ctx, ctx->bq_dev, ctx->b_qbad, n, q_pad, t, thr)) != STB_OK) return rc;
+  if ((rc = k2_gemm(ctx, corpus, copy, m_tiles, emit)) != STB_OK) return rc;
   std::vector<uint32_t> hcnt((size_t)n * n_seg);
   std::vector<float> hthr(n);
   STB_CUDA(cudaMemcpyAsync(hcnt.data(), cnt, hcnt.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -2229,27 +2217,21 @@ static int thr_chunk_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, uint3
   STB_CUDA(cudaMemcpyAsync(ctx->t_dst, dst.data(), dst.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->stream));
   if ((rc = stb_launch_batch_thr_compact(ctx, ctx->b_keys, cnt, ctx->t_dst, (uint64_t)n * n_seg, STB_THR_SEG_CAP, A)) != STB_OK) return rc;
   if (n_retry) {
-    // one more pass over the re-emitted queries' shadow (or q8) tiles, rebuilt from their f32 rows: the same bits,
-    // the same emitted rows; into segments sized by the first pass's exact counts
+    // one more pass over the re-emitted queries' tiles, rebuilt from their f32 rows: the same bits, the same emitted
+    // rows; into segments sized by the first pass's exact counts (the first pass's flags and q8 constants are no
+    // longer read, r_pad <= q_pad)
     if ((rc = ctx->t_segoff.reserve(segoff.size())) != STB_OK) return rc;
     if ((rc = ctx->t_cur.reserve((size_t)r_pad * n_seg)) != STB_OK) return rc;
     if ((rc = ctx->t_rq.reserve((size_t)n_retry * STB_D)) != STB_OK) return rc;
     if ((rc = ctx->t_rthr.reserve((size_t)r_pad)) != STB_OK) return rc;
     STB_CUDA(cudaMemcpyAsync(ctx->t_segoff, segoff.data(), segoff.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->stream));
     STB_CUDA(cudaMemsetAsync(ctx->t_cur, 0, (size_t)r_pad * n_seg * sizeof(uint32_t), ctx->stream));
-    STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
     if ((rc = stb_launch_batch_thr_gather(ctx, ctx->bq_dev, thr, ctx->t_slot + n_direct, n_retry, r_pad, ctx->t_rq,
                                           ctx->t_rthr)) != STB_OK) return rc;
-    if (q8) {
-      // b_q8c / b_qbad of the first pass are no longer read (r_pad <= q_pad)
-      if ((rc = stb_launch_q8_query_tiles(ctx, ctx->t_rq, n_retry, r_pad, ctx->bq_tiles, ctx->b_q8c, ctx->b_qbad, nullptr)) != STB_OK ||
-          (rc = stb_launch_batch_q8_gemm_emit_sized(ctx, ctx->bq_tiles, ctx->b_q8c, r_tiles, corpus->q8, corpus->q8_scale,
-                                                    corpus->n, ctx->t_rthr, ctx->t_cur, A, ctx->t_segoff)) != STB_OK) return rc;
-    } else {
-      if ((rc = stb_launch_shadow_build(ctx, ctx->t_rq, n_retry, 128, ctx->bq_tiles, ctx->err_flag)) != STB_OK) return rc;
-      if ((rc = stb_launch_batch_gemm_emit_sized(ctx, ctx->bq_tiles, r_tiles, corpus->shadow, n_tiles, corpus->n, ctx->t_rthr,
-                                                 ctx->t_cur, A, ctx->t_segoff)) != STB_OK) return rc;
-    }
+    emit.epi = STB_EPI_EMIT_SIZED; emit.thr = ctx->t_rthr; emit.cand_cnt = ctx->t_cur; emit.cand_keys = A;
+    emit.cand_cap = 0; emit.seg_off = ctx->t_segoff;
+    if ((rc = k2_query_tiles(ctx, copy, ctx->t_rq, n_retry, r_pad)) != STB_OK) return rc;
+    if ((rc = k2_gemm(ctx, corpus, copy, r_tiles, emit)) != STB_OK) return rc;
   }
   // exact finish: rows ascending -> canonical re-score, d < M -> stable sort by distance = (distance, row) order
   if ((rc = stb_batch_thr_sort_rows(ctx, ctx->t_sort_tmp, sort_bytes, K, n_slots, ctx->t_off, A, B)) != STB_OK) return rc;
@@ -2263,10 +2245,10 @@ static int thr_chunk_run(stb_ctx *ctx, stb_corpus *corpus, const float *q, uint3
 
 extern "C" {
 
-// Threshold mode of search_documents for a batch (route 5; route 10 on the q8 copy where the shadow does not fit).
-// Chunks of STB_THR_CHUNK queries run the tensor-core pipeline (thr_chunk_run); K1 (stb_search) answers the
-// queries it leaves (all of them when neither copy can be used), and each chunk's hits are laid out once all its
-// counts are known: a chunk's output is one contiguous stretch of the concatenation.
+// Threshold mode of search_documents for a batch (route 5; route 10 where the shadow does not fit).  Chunks of
+// STB_THR_CHUNK queries run the tensor-core pipeline (thr_chunk_run) on the copy k2_choose_copy picks; K1
+// (stb_search) answers the queries it leaves (all of them when neither copy can be used), and each chunk's hits are
+// laid out once all its counts are known: a chunk's output is one contiguous stretch of the concatenation.
 int stb_search_batch_threshold(stb_ctx *ctx, const stb_corpus *corpus_c, const float *q, uint32_t nq, double max_distance,
                                stb_hit *out_hits, uint64_t cap, uint64_t *out_offsets) {
   int rc = ctx_use(ctx);
@@ -2279,14 +2261,11 @@ int stb_search_batch_threshold(stb_ctx *ctx, const stb_corpus *corpus_c, const f
   k2_record(ctx, kRouteThreshold, nq);
   for (uint32_t i = 0; i <= nq; ++i) out_offsets[i] = 0;
   if (corpus->n == 0 || !(max_distance > 0.0)) return STB_OK;      // NaN or <= 0: no distance is below it
-  rc = batch_shadow(ctx, corpus);
-  const bool q8 = rc == STB_ERR_NOMEM;                               // the shadow does not fit: route 10
-  const K2Route route = q8 ? kRouteThresholdQ8 : kRouteThreshold;
-  if (q8) rc = corpus_ensure_q8(ctx, corpus);
-  const bool tensor_ok = rc == STB_OK;
-  // STB_ERR_STATE: rows K2 cannot normalise; route 10 also STB_ERR_NOMEM: the q8 copy does not fit.  All K1
-  if (rc != STB_OK && rc != STB_ERR_STATE && !(q8 && rc == STB_ERR_NOMEM)) return rc;
-  if (q8) k2_record(ctx, route, nq);
+  K2Choice choice;
+  if ((rc = k2_choose_copy(ctx, corpus, true, true, &choice)) != STB_OK) return rc;
+  const K2Route route = k2_route(choice.shadow_missing, kRouteThreshold);
+  if (choice.shadow_missing) k2_record(ctx, route, nq);             // route 10, even if K1 answers all
+  const bool tensor_ok = choice.copy != K2Copy::kNone;
   const uint32_t n_seg = tensor_ok ? stb_batch_emit_grid(ctx, (uint32_t)((corpus->n + 255) / 256)) : 0u;
   const size_t nq_pad = ((size_t)nq + 127) / 128 * 128;
   if (tensor_ok) {
@@ -2294,7 +2273,7 @@ int stb_search_batch_threshold(stb_ctx *ctx, const stb_corpus *corpus_c, const f
     if ((rc = ctx->b_cnt.reserve(nq_pad * n_seg)) != STB_OK) return rc;
   }
   double eps = STB_Q8_SCAN_EPS;
-  if (!q8) stb_batch_build_params(nullptr, &eps);
+  if (choice.copy == K2Copy::kShadow) stb_batch_build_params(nullptr, &eps);
   const float t = thr_emission_value(max_distance, eps);
   std::unique_ptr<stb_hit[]> k1_buf;                                 // one K1 result: at most every row
   uint32_t retried = 0, k1_total = 0;
@@ -2302,7 +2281,7 @@ int stb_search_batch_threshold(stb_ctx *ctx, const stb_corpus *corpus_c, const f
     const uint32_t n = std::min(STB_THR_CHUNK, nq - c0);
     ThrChunk ch;
     if (tensor_ok) {
-      if ((rc = thr_chunk_run(ctx, corpus, q + (size_t)c0 * STB_D, c0, n, max_distance, t, q8, &ch)) != STB_OK) return rc;
+      if ((rc = thr_chunk_run(ctx, corpus, q + (size_t)c0 * STB_D, c0, n, max_distance, t, choice.copy, &ch)) != STB_OK) return rc;
     } else {
       for (uint32_t i = 0; i < n; ++i) ch.k1.push_back(i);
     }
@@ -2456,7 +2435,9 @@ int stb_debug_batch_gemm(stb_ctx *ctx, const float *q, uint32_t nq, const float 
   if (e == cudaSuccess) e = cudaMemcpyAsync(dr, rows, n * 1024, cudaMemcpyHostToDevice, ctx->stream);
   if (e == cudaSuccess) rc = stb_launch_shadow_build(ctx, dq, nq, 128, da, dbad);
   if (e == cudaSuccess && rc == STB_OK) rc = stb_launch_shadow_build(ctx, dr, n, 256, db, dbad);
-  if (e == cudaSuccess && rc == STB_OK) rc = stb_launch_batch_gemm(ctx, da, m_tiles, db, n_tiles, dsub, dtile, dfull);
+  StbGemmPass p;
+  p.a_tiles = da; p.m_tiles = m_tiles; p.n_tiles = n_tiles; p.submax = dsub; p.tilemax = dtile; p.full_out = dfull;
+  if (e == cudaSuccess && rc == STB_OK) rc = stb_launch_gemm_shadow(ctx, p, db);
   if (e == cudaSuccess && rc == STB_OK) e = cudaMemcpyAsync(out_full, dfull, q_pad * n_pad * 4, cudaMemcpyDeviceToHost, ctx->stream);
   if (e == cudaSuccess && rc == STB_OK && out_submax) e = cudaMemcpyAsync(out_submax, dsub, (size_t)n_tiles * 8 * q_pad * 4, cudaMemcpyDeviceToHost, ctx->stream);
   if (e == cudaSuccess && rc == STB_OK) e = cudaStreamSynchronize(ctx->stream);
@@ -2464,7 +2445,7 @@ int stb_debug_batch_gemm(stb_ctx *ctx, const float *q, uint32_t nq, const float 
   return rc;
 }
 
-// Route 7's query tiles and integer GEMM over a corpus's q8 copy (built or extended first): per query its q16
+// The q8 copy's query tiles and integer GEMM over a corpus's q8 copy (built or extended first): per query its q16
 // [nq][256], and per (query, row) the int32 dot and the bounds u, l [nq][n].
 int stb_debug_batch_q8_gemm(stb_ctx *ctx, const stb_corpus *corpus_c, const float *q, uint32_t nq, int16_t *q16,
                             int32_t *dot, float *u, float *l) {
@@ -2486,9 +2467,12 @@ int stb_debug_batch_q8_gemm(stb_ctx *ctx, const stb_corpus *corpus_c, const floa
       (rc = dbad.alloc(q_pad)) != STB_OK || (rc = d16.alloc((size_t)nq * STB_D)) != STB_OK ||
       (rc = ddot.alloc(q_pad * n_pad)) != STB_OK || (rc = du.alloc(q_pad * n_pad)) != STB_OK || (rc = dl.alloc(q_pad * n_pad)) != STB_OK)
     return rc;
+  StbGemmPass p;
+  p.epi = STB_EPI_DEBUG; p.a_tiles = da; p.m_tiles = m_tiles; p.n_tiles = (uint32_t)(n_pad / 256); p.n_rows = n;
+  p.dot_out = ddot; p.u_out = du; p.l_out = dl;
   STB_CUDA(cudaMemcpyAsync(dq, q, (size_t)nq * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
   if ((rc = stb_launch_q8_query_tiles(ctx, dq, nq, (uint32_t)q_pad, da, dc, dbad, d16)) != STB_OK ||
-      (rc = stb_launch_batch_q8_gemm_debug(ctx, da, dc, m_tiles, corpus->q8, corpus->q8_scale, n, ddot, du, dl)) != STB_OK)
+      (rc = stb_launch_gemm_q8(ctx, p, corpus->q8, corpus->q8_scale, dc)) != STB_OK)
     return rc;
   STB_CUDA(cudaMemcpyAsync(q16, d16, (size_t)nq * STB_D * sizeof(int16_t), cudaMemcpyDeviceToHost, ctx->stream));
   STB_CUDA(cudaMemcpy2DAsync(dot, n * 4, ddot, n_pad * 4, n * 4, nq, cudaMemcpyDeviceToHost, ctx->stream));

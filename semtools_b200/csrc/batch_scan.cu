@@ -221,11 +221,8 @@ struct GemmArgs {
   // at row slot_row[s] (~0: a padding slot, which never emits).
 };
 
-// Filter modes of the GEMM: every tile, the listed tiles of one filter, or a work list of (query tile, masks)
-// per corpus tile, one filter per 64-query half
-#define STB_GEMM_ALL 0
-#define STB_GEMM_LISTED 1
-#define STB_GEMM_WORK 2
+// Filter modes of the GEMM (STB_GEMM_ALL, _LISTED, _WORK: common.cuh): every tile, the listed tiles of one filter,
+// or a work list of (query tile, masks) per corpus tile, one filter per 64-query half
 
 // warpgroup 0: bulk-copy producer (one thread); warpgroups 1 and 2: wgmma + epilogue, each on
 // 64 of the 128 queries of a query tile (m64n256 accumulators, 128 f32 registers per thread)
@@ -697,74 +694,30 @@ static int launch_gemm(stb_ctx *ctx, const GemmArgs &a) {
   return STB_OK;
 }
 
-int stb_launch_batch_gemm(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_tiles, const uint8_t *b_tiles,
-                          uint32_t n_tiles, float *submax, float *tilemax, float *full_out) {
-  return stb_launch_batch_gemm_strided(ctx, a_tiles, m_tiles, b_tiles, n_tiles, 1, submax, tilemax, full_out);
-}
-
-// maxima epilogue over the tiles 0, stride, 2*stride, ... (n_tiles of them); submax may be null
-int stb_launch_batch_gemm_strided(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_tiles, const uint8_t *b_tiles,
-                                  uint32_t n_tiles, uint32_t tile_stride, float *submax, float *tilemax, float *full_out) {
+// The pass on the shadow: GemmArgs's unions hold the work list's arrays in STB_GEMM_WORK
+int stb_launch_gemm_shadow(stb_ctx *ctx, const StbGemmPass &p, const uint8_t *shadow) {
   GemmArgs a{};
-  a.a_tiles = a_tiles; a.b_tiles = b_tiles; a.m_tiles = m_tiles; a.n_tiles = n_tiles;
-  a.submax = submax; a.tilemax = tilemax; a.full_out = full_out; a.tile_stride = tile_stride;
-  return launch_gemm<0>(ctx, a);
-}
-
-// candidate-emitting epilogue over all tiles
-int stb_launch_batch_gemm_emit(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_tiles, const uint8_t *b_tiles,
-                               uint32_t n_tiles, uint64_t n_rows, const float *thr, uint32_t *cand_cnt,
-                               uint64_t *cand_keys, uint32_t cand_cap) {
-  GemmArgs a{};
-  a.a_tiles = a_tiles; a.b_tiles = b_tiles; a.m_tiles = m_tiles; a.n_tiles = n_tiles; a.tile_stride = 1;
-  a.thr = thr; a.cand_cnt = cand_cnt; a.cand_keys = cand_keys; a.cand_cap = cand_cap; a.n_rows = n_rows;
-  return launch_gemm<1>(ctx, a);
-}
-
-// Pipeline v2 on the eligible rows only (stb_search_batch_filtered): the sampling pass over the listed tiles
-// 0, stride, 2*stride, ... (n_sample of them), tile maxima over eligible rows ...
-int stb_launch_batch_gemm_sample_filtered(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_tiles, const uint8_t *b_tiles,
-                                          const uint32_t *tile_ids, const uint32_t *bitmap, uint32_t n_sample,
-                                          uint32_t tile_stride, float *tilemax) {
-  GemmArgs a{};
-  a.a_tiles = a_tiles; a.b_tiles = b_tiles; a.m_tiles = m_tiles; a.n_tiles = n_sample; a.tile_stride = tile_stride;
-  a.tilemax = tilemax; a.tile_ids = tile_ids; a.bitmap = bitmap;
-  return launch_gemm<0, STB_GEMM_LISTED>(ctx, a);
-}
-
-// ... and the candidate-emitting pass over all n_listed listed tiles, eligible rows only
-int stb_launch_batch_gemm_emit_filtered(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_tiles, const uint8_t *b_tiles,
-                                        const uint32_t *tile_ids, const uint32_t *bitmap, uint32_t n_listed, uint64_t n_rows,
-                                        const float *thr, uint32_t *cand_cnt, uint64_t *cand_keys, uint32_t cand_cap) {
-  GemmArgs a{};
-  a.a_tiles = a_tiles; a.b_tiles = b_tiles; a.m_tiles = m_tiles; a.n_tiles = n_listed; a.tile_stride = 1;
-  a.thr = thr; a.cand_cnt = cand_cnt; a.cand_keys = cand_keys; a.cand_cap = cand_cap; a.n_rows = n_rows;
-  a.tile_ids = tile_ids; a.bitmap = bitmap;
-  return launch_gemm<1, STB_GEMM_LISTED>(ctx, a);
-}
-
-// Pipeline v2 with one filter per 64-query half (stb_search_batch_subsets): the sampling pass and the emitting
-// pass over corpus tiles tile_ids[0, n_tiles), each with its work items (GemmArgs, STB_GEMM_WORK); masks are
-// 8-word slots of `bitmap`.  The sampling pass writes tilemax [m_tiles][tm_cols][128] at each half's sample
-// column; the emitting pass writes slot s's keys and count at row slot_row[s].
-int stb_launch_batch_gemm_sample_work(stb_ctx *ctx, const uint8_t *a_tiles, const uint8_t *b_tiles, const uint32_t *tile_ids,
-                                      uint32_t n_tiles, const uint32_t *cta_tiles, const uint32_t *item_off, const uint4 *items,
-                                      const uint32_t *bitmap, uint32_t tm_cols, float *tilemax) {
-  GemmArgs a{};
-  a.a_tiles = a_tiles; a.b_tiles = b_tiles; a.tile_ids = tile_ids; a.n_tiles = n_tiles; a.cta_tiles = cta_tiles;
-  a.item_off = item_off; a.items = items; a.bitmap = bitmap; a.tile_stride = tm_cols; a.tilemax = tilemax;
-  return launch_gemm<0, STB_GEMM_WORK>(ctx, a);
-}
-
-int stb_launch_batch_gemm_emit_work(stb_ctx *ctx, const uint8_t *a_tiles, const uint8_t *b_tiles, const uint32_t *tile_ids,
-                                    uint32_t n_tiles, const uint32_t *cta_tiles, const uint32_t *item_off, const uint4 *items,
-                                    const uint32_t *bitmap, const uint32_t *slot_row, uint64_t n_rows, const float *thr,
-                                    uint32_t *cand_cnt, uint64_t *cand_keys, uint32_t cand_cap) {
-  GemmArgs a{};
-  a.a_tiles = a_tiles; a.b_tiles = b_tiles; a.tile_ids = tile_ids; a.n_tiles = n_tiles; a.cta_tiles = cta_tiles;
-  a.item_off = item_off; a.items = items; a.bitmap = bitmap; a.slot_row = slot_row; a.n_rows = n_rows;
-  a.thr = thr; a.cand_cnt = cand_cnt; a.cand_keys = cand_keys; a.cand_cap = cand_cap;
-  return launch_gemm<1, STB_GEMM_WORK>(ctx, a);
+  a.a_tiles = p.a_tiles; a.b_tiles = shadow; a.m_tiles = p.m_tiles; a.n_tiles = p.n_tiles; a.tile_stride = p.tile_stride;
+  a.thr = p.thr; a.cand_cnt = p.cand_cnt; a.cand_keys = p.cand_keys; a.cand_cap = p.cand_cap; a.n_rows = p.n_rows;
+  a.tile_ids = p.tile_ids; a.bitmap = p.bitmap;
+  if (p.select == STB_GEMM_WORK) {
+    a.items = p.items; a.item_off = p.item_off; a.cta_tiles = p.cta_tiles;
+    if (p.epi == STB_EPI_EMIT) a.slot_row = p.slot_row;
+    else a.tilemax = p.tilemax;
+  } else {
+    a.submax = p.submax; a.tilemax = p.tilemax; a.full_out = p.full_out; a.seg_off = p.seg_off;
+  }
+  switch (p.select * 4 + p.epi) {
+    case STB_GEMM_ALL * 4 + STB_EPI_SAMPLE: return launch_gemm<0>(ctx, a);
+    case STB_GEMM_ALL * 4 + STB_EPI_EMIT: return launch_gemm<1>(ctx, a);
+    case STB_GEMM_ALL * 4 + STB_EPI_EMIT_SIZED: return launch_gemm<2>(ctx, a);
+    case STB_GEMM_LISTED * 4 + STB_EPI_SAMPLE: return launch_gemm<0, STB_GEMM_LISTED>(ctx, a);
+    case STB_GEMM_LISTED * 4 + STB_EPI_EMIT: return launch_gemm<1, STB_GEMM_LISTED>(ctx, a);
+    case STB_GEMM_WORK * 4 + STB_EPI_SAMPLE: return launch_gemm<0, STB_GEMM_WORK>(ctx, a);
+    case STB_GEMM_WORK * 4 + STB_EPI_EMIT: return launch_gemm<1, STB_GEMM_WORK>(ctx, a);
+  }
+  stb_set_error("batch GEMM: no shadow kernel for epilogue %d over tile selection %d", p.epi, p.select);
+  return STB_ERR_ARG;
 }
 
 // stb_search_batch_subsets's query slots: slot s holds the f32 query row slot_row[s] of `rows` (zeros for a
@@ -809,17 +762,6 @@ int stb_launch_batch_slots_prep(stb_ctx *ctx, const uint32_t *slot_row, const ui
   STB_CUDA(cudaGetLastError());
   ctx->kernel_launches++;
   return STB_OK;
-}
-
-// Threshold mode's re-emission: the candidate-emitting pass over all tiles into the exactly sized segments
-// seg_off[] of cand_keys; cursors [q_pad][grid] zeroed by the caller
-int stb_launch_batch_gemm_emit_sized(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_tiles, const uint8_t *b_tiles,
-                                     uint32_t n_tiles, uint64_t n_rows, const float *thr, uint32_t *cursors,
-                                     uint64_t *cand_keys, const uint64_t *seg_off) {
-  GemmArgs a{};
-  a.a_tiles = a_tiles; a.b_tiles = b_tiles; a.m_tiles = m_tiles; a.n_tiles = n_tiles; a.tile_stride = 1;
-  a.thr = thr; a.cand_cnt = cursors; a.cand_keys = cand_keys; a.n_rows = n_rows; a.seg_off = seg_off;
-  return launch_gemm<2>(ctx, a);
 }
 
 
@@ -1783,63 +1725,20 @@ static int launch_q8_gemm(stb_ctx *ctx, const uint8_t *codes, const float *scale
   return STB_OK;
 }
 
-int stb_launch_batch_q8_gemm_sample(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
-                                    const uint8_t *codes, const float *scales, uint64_t n_rows, uint32_t n_sample,
-                                    uint32_t tile_stride, float *tilemax) {
+int stb_launch_gemm_q8(stb_ctx *ctx, const StbGemmPass &p, const uint8_t *codes, const float *scales, const float4 *qc) {
   Q8GemmArgs a{};
-  a.a_tiles = a_tiles; a.qc = qc; a.m_tiles = m_tiles; a.n_tiles = n_sample; a.tile_stride = tile_stride;
-  a.n_rows = n_rows; a.tilemax = tilemax;
-  return launch_q8_gemm<0>(ctx, codes, scales, a);
-}
-
-int stb_launch_batch_q8_gemm_emit(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
-                                  const uint8_t *codes, const float *scales, uint64_t n_rows, const float *thr,
-                                  uint32_t *cand_cnt, uint64_t *cand_keys, uint32_t cand_cap) {
-  Q8GemmArgs a{};
-  a.a_tiles = a_tiles; a.qc = qc; a.m_tiles = m_tiles; a.n_tiles = (uint32_t)((n_rows + STB_B_TILE - 1) / STB_B_TILE);
-  a.tile_stride = 1; a.n_rows = n_rows; a.thr = thr; a.cand_cnt = cand_cnt; a.cand_keys = cand_keys; a.cand_cap = cand_cap;
-  return launch_q8_gemm<1>(ctx, codes, scales, a);
-}
-
-int stb_launch_batch_q8_gemm_debug(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
-                                   const uint8_t *codes, const float *scales, uint64_t n_rows, int32_t *dot, float *u,
-                                   float *l) {
-  Q8GemmArgs a{};
-  a.a_tiles = a_tiles; a.qc = qc; a.m_tiles = m_tiles; a.n_tiles = (uint32_t)((n_rows + STB_B_TILE - 1) / STB_B_TILE);
-  a.tile_stride = 1; a.n_rows = n_rows; a.dot_out = dot; a.u_out = u; a.l_out = l;
-  return launch_q8_gemm<2>(ctx, codes, scales, a);
-}
-
-// Route 8: the sampling pass over the listed tiles 0, stride, 2*stride, ... (n_sample of them), tile maxima of l
-// over eligible rows ...
-int stb_launch_batch_q8_gemm_sample_filtered(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
-                                             const uint8_t *codes, const float *scales, uint64_t n_rows,
-                                             const uint32_t *tile_ids, const uint32_t *bitmap, uint32_t n_sample,
-                                             uint32_t tile_stride, float *tilemax) {
-  Q8GemmArgs a{};
-  a.a_tiles = a_tiles; a.qc = qc; a.m_tiles = m_tiles; a.n_tiles = n_sample; a.tile_stride = tile_stride;
-  a.n_rows = n_rows; a.tilemax = tilemax; a.tile_ids = tile_ids; a.bitmap = bitmap;
-  return launch_q8_gemm<0, true>(ctx, codes, scales, a);
-}
-
-// ... and the emitting pass over all n_listed listed tiles, eligible rows only
-int stb_launch_batch_q8_gemm_emit_filtered(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
-                                           const uint8_t *codes, const float *scales, uint64_t n_rows,
-                                           const uint32_t *tile_ids, const uint32_t *bitmap, uint32_t n_listed,
-                                           const float *thr, uint32_t *cand_cnt, uint64_t *cand_keys, uint32_t cand_cap) {
-  Q8GemmArgs a{};
-  a.a_tiles = a_tiles; a.qc = qc; a.m_tiles = m_tiles; a.n_tiles = n_listed; a.tile_stride = 1; a.n_rows = n_rows;
-  a.thr = thr; a.cand_cnt = cand_cnt; a.cand_keys = cand_keys; a.cand_cap = cand_cap; a.tile_ids = tile_ids; a.bitmap = bitmap;
-  return launch_q8_gemm<1, true>(ctx, codes, scales, a);
-}
-
-// Route 10's re-emission: the emitting pass over all tiles into the exactly sized segments seg_off[] of cand_keys;
-// cursors [q_pad][grid] zeroed by the caller
-int stb_launch_batch_q8_gemm_emit_sized(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
-                                        const uint8_t *codes, const float *scales, uint64_t n_rows, const float *thr,
-                                        uint32_t *cursors, uint64_t *cand_keys, const uint64_t *seg_off) {
-  Q8GemmArgs a{};
-  a.a_tiles = a_tiles; a.qc = qc; a.m_tiles = m_tiles; a.n_tiles = (uint32_t)((n_rows + STB_B_TILE - 1) / STB_B_TILE);
-  a.tile_stride = 1; a.n_rows = n_rows; a.thr = thr; a.cand_cnt = cursors; a.cand_keys = cand_keys; a.seg_off = seg_off;
-  return launch_q8_gemm<3>(ctx, codes, scales, a);
+  a.a_tiles = p.a_tiles; a.qc = qc; a.m_tiles = p.m_tiles; a.n_tiles = p.n_tiles; a.tile_stride = p.tile_stride;
+  a.n_rows = p.n_rows; a.tilemax = p.tilemax; a.thr = p.thr; a.cand_cnt = p.cand_cnt; a.cand_keys = p.cand_keys;
+  a.cand_cap = p.cand_cap; a.dot_out = p.dot_out; a.u_out = p.u_out; a.l_out = p.l_out; a.tile_ids = p.tile_ids;
+  a.bitmap = p.bitmap; a.seg_off = p.seg_off;
+  switch (p.select * 4 + p.epi) {
+    case STB_GEMM_ALL * 4 + STB_EPI_SAMPLE: return launch_q8_gemm<0>(ctx, codes, scales, a);
+    case STB_GEMM_ALL * 4 + STB_EPI_EMIT: return launch_q8_gemm<1>(ctx, codes, scales, a);
+    case STB_GEMM_ALL * 4 + STB_EPI_DEBUG: return launch_q8_gemm<2>(ctx, codes, scales, a);
+    case STB_GEMM_ALL * 4 + STB_EPI_EMIT_SIZED: return launch_q8_gemm<3>(ctx, codes, scales, a);
+    case STB_GEMM_LISTED * 4 + STB_EPI_SAMPLE: return launch_q8_gemm<0, true>(ctx, codes, scales, a);
+    case STB_GEMM_LISTED * 4 + STB_EPI_EMIT: return launch_q8_gemm<1, true>(ctx, codes, scales, a);
+  }
+  stb_set_error("batch GEMM: no q8 kernel for epilogue %d over tile selection %d", p.epi, p.select);
+  return STB_ERR_ARG;
 }

@@ -466,37 +466,45 @@ int stb_launch_embed(stb_ctx *ctx, const stb_table *t, const uint64_t *offsets_d
 int stb_launch_shadow_build(stb_ctx *ctx, const float *rows_dev, uint64_t n_rows, int tile,
                             uint8_t *out, int *bad_flag_dev, uint64_t first_row = 0,
                             uint32_t *row_bad_dev = nullptr, uint64_t rows_first = 0);
-int stb_launch_batch_gemm(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_tiles,
-                          const uint8_t *b_tiles, uint32_t n_tiles, float *submax,
-                          float *tilemax, float *full_out);
-int stb_launch_batch_gemm_strided(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_tiles,
-                                  const uint8_t *b_tiles, uint32_t n_tiles, uint32_t tile_stride,
-                                  float *submax, float *tilemax, float *full_out);
-int stb_launch_batch_gemm_emit(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_tiles,
-                               const uint8_t *b_tiles, uint32_t n_tiles, uint64_t n_rows,
-                               const float *thr, uint32_t *cand_cnt, uint64_t *cand_keys,
-                               uint32_t cand_cap);
-// the same two passes over the listed tiles tile_ids[0, n_listed), eligible rows (bitmap) only
-int stb_launch_batch_gemm_sample_filtered(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_tiles,
-                                          const uint8_t *b_tiles, const uint32_t *tile_ids,
-                                          const uint32_t *bitmap, uint32_t n_sample, uint32_t tile_stride,
-                                          float *tilemax);
-int stb_launch_batch_gemm_emit_filtered(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_tiles,
-                                        const uint8_t *b_tiles, const uint32_t *tile_ids,
-                                        const uint32_t *bitmap, uint32_t n_listed, uint64_t n_rows,
-                                        const float *thr, uint32_t *cand_cnt, uint64_t *cand_keys,
-                                        uint32_t cand_cap);
-// the same two passes with one filter per 64-query half, over per-corpus-tile work items (batch_scan.cu, GemmArgs)
-int stb_launch_batch_gemm_sample_work(stb_ctx *ctx, const uint8_t *a_tiles, const uint8_t *b_tiles,
-                                      const uint32_t *tile_ids, uint32_t n_tiles, const uint32_t *cta_tiles,
-                                      const uint32_t *item_off, const uint4 *items, const uint32_t *bitmap,
-                                      uint32_t tm_cols, float *tilemax);
-int stb_launch_batch_gemm_emit_work(stb_ctx *ctx, const uint8_t *a_tiles, const uint8_t *b_tiles,
-                                    const uint32_t *tile_ids, uint32_t n_tiles, const uint32_t *cta_tiles,
-                                    const uint32_t *item_off, const uint4 *items, const uint32_t *bitmap,
-                                    const uint32_t *slot_row, uint64_t n_rows, const float *thr, uint32_t *cand_cnt,
-                                    uint64_t *cand_keys, uint32_t cand_cap);
-// the query slots of those passes: f32 rows gathered into slot order, then the per-row bad flags scattered
+// One pass of K2's GEMM (batch_scan.cu) over either copy: the epilogue, the corpus tiles it covers, and what those
+// read and write.  Tile t of a pass is corpus tile t * tile_stride (STB_GEMM_ALL), listed tile tile_ids[t *
+// tile_stride] with the eligible rows of `bitmap` (STB_GEMM_LISTED), or, STB_GEMM_WORK (shadow only), the t-th
+// tile of a work list: per corpus tile tile_ids[u] its (query tile, mask slots, sample columns) items, one filter
+// per 64-query half (batch_scan.cu, GemmArgs).  Rows past n_rows never count.
+#define STB_GEMM_ALL 0
+#define STB_GEMM_LISTED 1
+#define STB_GEMM_WORK 2
+enum StbGemmEpi {
+  STB_EPI_SAMPLE,             // tile maxima into tilemax [m_tiles][n_tiles][128] (shadow: per-32-row submax and the
+                              // full score matrix full_out too, if given; q8: of the lower bound l)
+  STB_EPI_EMIT,               // every (query, row) whose score (q8: upper bound u) reaches thr[query], into the
+                              // per-(query, CTA) segments cand_keys [q_pad][grid][cand_cap], counts cand_cnt
+  STB_EPI_EMIT_SIZED,         // the same into exactly sized segments cand_keys[seg_off[i], seg_off[i+1]) (i = query *
+                              // grid + CTA), cand_cnt the zeroed cursors; STB_GEMM_ALL only
+  STB_EPI_DEBUG               // q8, STB_GEMM_ALL: dot, u and l of every (query, row), [m_tiles * 128][n_tiles * 256]
+};
+struct StbGemmPass {
+  int epi = STB_EPI_SAMPLE, select = STB_GEMM_ALL;
+  const uint8_t *a_tiles = nullptr;              // query tiles: m_tiles x 64 KiB
+  uint32_t m_tiles = 0, n_tiles = 0, tile_stride = 1;
+  uint64_t n_rows = 0;
+  const uint32_t *tile_ids = nullptr, *bitmap = nullptr;
+  const uint32_t *cta_tiles = nullptr, *item_off = nullptr, *slot_row = nullptr;   // STB_GEMM_WORK
+  const uint4 *items = nullptr;
+  float *tilemax = nullptr, *submax = nullptr, *full_out = nullptr;
+  const float *thr = nullptr;
+  uint32_t *cand_cnt = nullptr;
+  uint64_t *cand_keys = nullptr;
+  uint32_t cand_cap = 0;
+  const uint64_t *seg_off = nullptr;
+  int32_t *dot_out = nullptr;
+  float *u_out = nullptr, *l_out = nullptr;
+};
+// The pass on the corpus shadow, or on the q8 copy (codes, scales) with the query constants qc of
+// stb_launch_q8_query_tiles; a combination no kernel is built for is refused with STB_ERR_ARG
+int stb_launch_gemm_shadow(stb_ctx *ctx, const StbGemmPass &p, const uint8_t *shadow);
+int stb_launch_gemm_q8(stb_ctx *ctx, const StbGemmPass &p, const uint8_t *codes, const float *scales, const float4 *qc);
+// the query slots of the STB_GEMM_WORK passes: f32 rows gathered into slot order, then the per-row bad flags scattered
 // back and the sampled maxima preset to -inf
 int stb_launch_batch_slots_gather(stb_ctx *ctx, const float *rows, const uint32_t *slot_row, uint32_t n_slots, float *out);
 int stb_launch_batch_slots_prep(stb_ctx *ctx, const uint32_t *slot_row, const uint32_t *slot_bad, uint32_t n_slots,
@@ -515,43 +523,11 @@ int stb_launch_batch_finish2(stb_ctx *ctx, const uint64_t *cand_keys, const uint
                              const uint32_t *q_bad, stb_hit *out_hits, uint32_t *out_status,
                              const float *q8_scale = nullptr, const float4 *q8_qc = nullptr,
                              const float *thr = nullptr);
-// Route 7 (the q8 copy on the int8 tensor cores, batch_scan.cu): the query tiles -- hi / lo bytes of q16 in the
-// wgmma layout, m_tiles x 64 KiB -- with per-query {1/S, h_l1, e_q, S} and unusable flags (q16: [nq][256] or null);
-// the sampling pass (tile maxima of the lower bound l over tiles 0, stride, ... (n_sample of them)); the emitting
-// pass (every row whose upper bound u reaches thr, into the segments as stb_launch_batch_gemm_emit); and the
-// debug pass (dot, u and l of every (query, row) into [m_tiles * 128][ceil(n_rows / 256) * 256] matrices)
+// The q8 copy's query tiles (batch_scan.cu): hi / lo bytes of q16 in the wgmma layout, m_tiles x 64 KiB, with
+// per-query {1/S, h_l1, e_q, S} and unusable flags (q16: [nq][256] or null)
 int stb_launch_q8_query_tiles(stb_ctx *ctx, const float *q_dev, uint32_t nq, uint32_t q_pad, uint8_t *tiles,
                               float4 *qc, uint32_t *q_bad, int16_t *q16);
-int stb_launch_batch_q8_gemm_sample(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
-                                    const uint8_t *codes, const float *scales, uint64_t n_rows, uint32_t n_sample,
-                                    uint32_t tile_stride, float *tilemax);
-int stb_launch_batch_q8_gemm_emit(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
-                                  const uint8_t *codes, const float *scales, uint64_t n_rows, const float *thr,
-                                  uint32_t *cand_cnt, uint64_t *cand_keys, uint32_t cand_cap);
-int stb_launch_batch_q8_gemm_debug(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
-                                   const uint8_t *codes, const float *scales, uint64_t n_rows, int32_t *dot, float *u,
-                                   float *l);
-// Routes 8 and 10: route 7's two passes over the listed tiles tile_ids[0, n_listed), eligible rows (bitmap) only,
-// and its emitting pass into exactly sized segments cand_keys[seg_off[i], seg_off[i+1]) (i = query * grid + CTA,
-// cursors [q_pad][grid] zeroed), as stb_launch_batch_gemm_*_filtered and stb_launch_batch_gemm_emit_sized
-int stb_launch_batch_q8_gemm_sample_filtered(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
-                                             const uint8_t *codes, const float *scales, uint64_t n_rows,
-                                             const uint32_t *tile_ids, const uint32_t *bitmap, uint32_t n_sample,
-                                             uint32_t tile_stride, float *tilemax);
-int stb_launch_batch_q8_gemm_emit_filtered(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
-                                           const uint8_t *codes, const float *scales, uint64_t n_rows,
-                                           const uint32_t *tile_ids, const uint32_t *bitmap, uint32_t n_listed,
-                                           const float *thr, uint32_t *cand_cnt, uint64_t *cand_keys, uint32_t cand_cap);
-int stb_launch_batch_q8_gemm_emit_sized(stb_ctx *ctx, const uint8_t *a_tiles, const float4 *qc, uint32_t m_tiles,
-                                        const uint8_t *codes, const float *scales, uint64_t n_rows, const float *thr,
-                                        uint32_t *cursors, uint64_t *cand_keys, const uint64_t *seg_off);
 void stb_batch_build_params(int *shadow_is_f16, double *eps);
-// threshold mode's re-emission: the emitting pass into exactly sized segments cand_keys[seg_off[i], seg_off[i+1])
-// (i = query * grid + CTA), cursors [q_pad][grid] zeroed
-int stb_launch_batch_gemm_emit_sized(stb_ctx *ctx, const uint8_t *a_tiles, uint32_t m_tiles,
-                                     const uint8_t *b_tiles, uint32_t n_tiles, uint64_t n_rows,
-                                     const float *thr, uint32_t *cursors, uint64_t *cand_keys,
-                                     const uint64_t *seg_off);
 
 // ---- batch_threshold.cu (K2 threshold mode) -------------------------------------------------------
 // thr[i] = t for the queries i < nq that are non-zero and normalisable, +inf for the others and the padding
