@@ -54,6 +54,7 @@ typedef enum stb_status {
 typedef struct stb_ctx stb_ctx;       /* one CUDA device + stream + scratch        */
 typedef struct stb_table stb_table;   /* model2vec embedding table resident in HBM */
 typedef struct stb_corpus stb_corpus; /* row-major N x 256 f32 line-vector matrix  */
+typedef struct stb_tokenizer stb_tokenizer; /* tokenizer.json loaded; Unigram model in HBM */
 
 /* One search hit: (distance, global row) -- 16 bytes, the unit of the
  * cross-GPU top-k exchange.  `row` is the line's position in (document order,
@@ -220,6 +221,51 @@ int stb_embed(stb_ctx *ctx, const stb_table *table, const uint64_t *offsets,
 int stb_embed_dev(stb_ctx *ctx, const stb_table *table, const uint64_t *offsets_dev,
                   const uint32_t *ids_dev, uint64_t n_lines, float *out_dev);
 int stb_embed_status(stb_ctx *ctx);
+
+/* ---- K3 from text: the tokenizer on the GPU ----------------------------------------
+ * The same rows as stb_embed, from the lines' text instead of their token ids: the tokenisation half of
+ * encode_with_args (tokenizer.encode_batch_fast(add_special_tokens = false), the unk_token drop, truncation to
+ * max_length ids) moves into the library.
+ *
+ * stb_tokenizer_load takes the bytes of a tokenizer.json.  The library parses it with the C++ host's
+ * tokenizer (host/semtools_tokenizer.hpp, HfTokenizer): a shape that tokenizer refuses fails with
+ * STB_ERR_ARG and its message.  A loaded handle belongs to `ctx`; its Unigram model (byte trie, f64 scores,
+ * unk id) is resident in HBM.
+ *
+ * Which lines are tokenised on the GPU is decided by stb_tokenizer_gpu_lines alone (pure host code): taken[i]
+ * = 1 iff the tokenizer has the GPU shape -- a Unigram model with an unk_id, one Metaspace pre-tokenizer with
+ * split = true whose replacement is one non-ASCII character, normaliser steps among Lowercase, Precompiled,
+ * Replace(" {2,}" -> " "), Strip and Prepend (printable ASCII text) -- and line i
+ *   - is printable ASCII (0x20-0x7E) only,
+ *   - has only bytes that every Precompiled step leaves alone, as they are and lowercased,
+ *   - contains no added token's content, neither as given nor after normalisation,
+ *   - has no run of non-space bytes whose length, plus the replacement's bytes and the Prepend steps' bytes,
+ *     exceeds STB_TOKENIZER_PIECE_CAP (a Metaspace piece is the replacement plus such a run).
+ * Any other shape (WhitespaceSplit, Sequence pre-tokenizers, a string Replace, NFKC, ...) loads, and no line is taken.
+ *
+ * stb_embed_text: lines are text[text_offsets[i], text_offsets[i + 1]) (text_offsets[0] = 0), already cut
+ * by model2vec's truncate_str.  Taken lines are uploaded and tokenised on the GPU (normalise, Metaspace split,
+ * a Viterbi that follows the host's exactly: f64 scores, strict > on ties, unknown characters at
+ * min_score - 10, consecutive unknowns fused into one unk id); declined lines are tokenised on host threads by
+ * the same tokenizer.  The ids of both form one CSR in HBM, which the K3 kernel of stb_embed pools.  Rows,
+ * `out`, `append_to` and STB_ERR_RANGE are exactly stb_embed's on the ids encode_with_args would produce
+ * (a failed call appends nothing).  A line the host tokenizer refuses (e.g. NFKC on non-ASCII text) fails
+ * the call with STB_ERR_ARG before anything is written.  Large inputs are processed in chunks of
+ * context scratch that grows on demand.
+ *
+ * stb_debug_tokenize returns the CSR stb_embed_text would pool (ids_offsets[n_lines + 1] always; ids while
+ * they fit ids_cap, else STB_ERR_CAPACITY) and, if taken is not NULL, the rule's verdict. */
+#define STB_TOKENIZER_PIECE_CAP 256u
+int stb_tokenizer_load(stb_ctx *ctx, const uint8_t *json, uint64_t len, stb_tokenizer **out);
+int stb_tokenizer_destroy(stb_tokenizer *tok);
+int stb_tokenizer_gpu_lines(const stb_tokenizer *tok, const uint8_t *text, const uint64_t *text_offsets,
+                            uint64_t n_lines, uint8_t *taken);
+int stb_embed_text(stb_ctx *ctx, const stb_tokenizer *tok, const stb_table *table,
+                   const uint8_t *text, const uint64_t *text_offsets, uint64_t n_lines,
+                   uint32_t max_length, float *out, stb_corpus *append_to);
+int stb_debug_tokenize(stb_ctx *ctx, const stb_tokenizer *tok, const uint8_t *text,
+                       const uint64_t *text_offsets, uint64_t n_lines, uint32_t max_length,
+                       uint64_t *ids_offsets, uint32_t *ids, uint64_t ids_cap, uint8_t *taken);
 
 /* ---- K1 + K4: cosine scan, top-k / threshold, exact re-rank ---------------------
  * Replaces search_documents' scan/filter/sort/take (src/search/mod.rs:84-119,

@@ -35,7 +35,9 @@ SYMBOLS = [
     "stb_debug_ivfpq_export",
     "stb_ivfpq_search_batch", "stb_ivfpq_search_batch_dev", "stb_debug_ivfpq_batch_last",
     "stb_ivfpq_search_filtered", "stb_ivfpq_search_subsets", "stb_ivfpq_update", "stb_ivfpq_remove",
+    "stb_tokenizer_load", "stb_tokenizer_destroy", "stb_tokenizer_gpu_lines", "stb_embed_text", "stb_debug_tokenize",
 ]
+STB_TOKENIZER_PIECE_CAP = 256
 
 
 class StbHit(C.Structure):
@@ -146,6 +148,11 @@ def lib() -> C.CDLL:
     L.stb_debug_ivfpq_batch_last.argtypes = [vp, u32, vp, vp, vp, vp]
     L.stb_ivfpq_search_filtered.argtypes = [vp, vp, u32, u32, u32, u32, i32, f64, vp, u32, vp, vp, vp]
     L.stb_ivfpq_search_subsets.argtypes = [vp, vp, u32, u32, u32, u32, i32, f64, u32, vp, vp, vp, vp, vp, vp]
+    L.stb_tokenizer_load.argtypes = [vp, vp, u64, C.POINTER(vp)]
+    L.stb_tokenizer_destroy.argtypes = [vp]
+    L.stb_tokenizer_gpu_lines.argtypes = [vp, vp, vp, u64, vp]
+    L.stb_embed_text.argtypes = [vp, vp, vp, vp, vp, u64, u32, vp, vp]
+    L.stb_debug_tokenize.argtypes = [vp, vp, vp, vp, u64, u32, vp, vp, u64, vp]
     for name in SYMBOLS:
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("stb_version", "stb_device_count"):
@@ -317,6 +324,57 @@ class Table:
             self._h = None
 
     __del__ = close
+
+
+class Tokenizer:
+    """stb_tokenizer: a tokenizer.json loaded into the library (Unigram model resident in HBM)."""
+
+    def __init__(self, ctx: Context, json_bytes: bytes):
+        self.ctx = ctx
+        self._h = vp()
+        buf = np.frombuffer(json_bytes, dtype=np.uint8)
+        _check(lib().stb_tokenizer_load(ctx._h, _np_ptr(buf), buf.size, C.byref(self._h)))
+
+    def close(self):
+        if getattr(self, "_h", None) is not None and self._h and _lib is not None:
+            _lib.stb_tokenizer_destroy(self._h)
+            self._h = None
+
+    __del__ = close
+
+    def gpu_lines(self, lines) -> np.ndarray:
+        """stb_tokenizer_gpu_lines: 1 for each line the GPU tokenises (host-only)."""
+        text, offsets = pack_lines(lines)
+        taken = np.zeros(len(lines), dtype=np.uint8)
+        _check(lib().stb_tokenizer_gpu_lines(self._h, _np_ptr(text), _np_ptr(offsets), len(lines), _np_ptr(taken)))
+        return taken.astype(bool)
+
+    def debug_tokenize(self, lines, max_length: int):
+        """stb_debug_tokenize -> (offsets u64[n+1], ids u32, taken bool[n]): the CSR stb_embed_text pools."""
+        text, offsets = pack_lines(lines)
+        n = len(lines)
+        out_off = np.zeros(n + 1, dtype=np.uint64)
+        taken = np.zeros(max(n, 1), dtype=np.uint8)
+        cap = int(offsets[-1]) + 2 * n + 1                    # a line of k bytes has at most k + 1 ids
+        ids = np.zeros(cap, dtype=np.uint32)
+        rc = _check(lib().stb_debug_tokenize(self.ctx._h, self._h, _np_ptr(text), _np_ptr(offsets), n, max_length,
+                                             _np_ptr(out_off), _np_ptr(ids), cap, _np_ptr(taken)), allow_capacity=True)
+        if rc == STB_ERR_CAPACITY:
+            cap = int(out_off[-1])
+            ids = np.zeros(max(cap, 1), dtype=np.uint32)
+            _check(lib().stb_debug_tokenize(self.ctx._h, self._h, _np_ptr(text), _np_ptr(offsets), n, max_length,
+                                            _np_ptr(out_off), _np_ptr(ids), cap, _np_ptr(taken)))
+        return out_off, ids[: int(out_off[-1])].copy(), taken[:n].astype(bool)
+
+
+def pack_lines(lines):
+    """Lines (str or bytes) -> (UTF-8 text u8, offsets u64[n+1])."""
+    enc = [l.encode("utf-8") if isinstance(l, str) else bytes(l) for l in lines]
+    offsets = np.zeros(len(enc) + 1, dtype=np.uint64)
+    if enc:
+        offsets[1:] = np.cumsum([len(b) for b in enc])
+    text = np.frombuffer(b"".join(enc) or b"\0", dtype=np.uint8)
+    return text, offsets
 
 
 class Corpus:
@@ -846,4 +904,15 @@ def embed(ctx: Context, table: Table, offsets, ids, out: bool = True, append_to:
         ids = np.zeros(1, dtype=np.uint32)
     _check(lib().stb_embed(ctx._h, table._h, _np_ptr(offsets), _np_ptr(ids), n_lines, _np_ptr(res),
                            append_to._h if append_to is not None else None))
+    return res
+
+
+def embed_text(ctx: Context, tok: Tokenizer, table: Table, lines, max_length: int, out: bool = True,
+               append_to: Corpus | None = None):
+    """stb_embed_text: the rows of stb_embed from the lines' text (str or UTF-8 bytes), tokenised in the library."""
+    text, offsets = pack_lines(lines)
+    n_lines = len(lines)
+    res = np.empty((n_lines, STB_DIM), dtype=np.float32) if out else None
+    _check(lib().stb_embed_text(ctx._h, tok._h, table._h, _np_ptr(text), _np_ptr(offsets), n_lines, max_length,
+                                _np_ptr(res), append_to._h if append_to is not None else None))
     return res

@@ -160,8 +160,7 @@ def create_document_from_content(searcher: Searcher, filename: str, content: str
     if not lines:
         return None                                            # :57-59
     emb_lines = [l.lower() for l in lines] if ignore_case else lines
-    offsets, ids = model.tokenize(emb_lines, 2048)              # encode_with_args(.., Some(2048), 16384)
-    return searcher.add_document_tokens(filename, lines, model.table(), offsets, ids)
+    return searcher.add_document_lines(filename, lines, model, emb_lines)   # encode_with_args(.., Some(2048), 16384)
 
 
 def search_files(files, query: str, model, config: SearchConfig, ctx: capi.Context | None = None):
@@ -188,8 +187,7 @@ def search_cmd(query, files, n_lines, top_k, max_distance, ignore_case, json, wo
                 model.ctx = capi.Context(0)
             searcher = Searcher(model.ctx, capi.Corpus(model.ctx, 1024))
             emb = [l.lower() for l in lines] if ignore_case else lines
-            offsets, ids = model.tokenize(emb, 2048)
-            searcher.add_document_tokens("<stdin>", lines, model.table(), offsets, ids)
+            searcher.add_document_lines("<stdin>", lines, model, emb)
             results = searcher.search_documents(model.encode_single(query), cfg)
             out.write(to_string_pretty({"results": [search_result_to_json(r) for r in results]}) + "\n" if json
                       else format_search_results(results, stdout_is_tty))

@@ -45,6 +45,9 @@ static int ctx_use(const stb_ctx *ctx) {
   return STB_OK;
 }
 
+int stb_ctx_use(const stb_ctx *ctx) { return ctx_use(ctx); }
+bool stb_ctx_alive(const stb_ctx *ctx) { return ctx_alive(ctx); }
+
 bool stb_ranges_ordered(const uint64_t *ranges, uint32_t n) {
   uint64_t prev_end = 0;
   for (uint32_t i = 0; i < n; ++i) {
@@ -535,6 +538,48 @@ int stb_embed(stb_ctx *ctx, const stb_table *table, const uint64_t *offsets, con
   if (out) STB_CUDA(cudaMemcpyAsync(out, dst, n_lines * STB_D * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
   STB_CUDA(cudaStreamSynchronize(ctx->stream));
   if (flag) { stb_set_error("embed: a token id maps outside the %llu-row table", (unsigned long long)table->V); return STB_ERR_RANGE; }
+  if (append_to) { append_to->n += n_lines; corpus_changed(append_to, CORPUS_APPEND); }
+  return STB_OK;
+}
+
+// The rows of stb_embed from text: per chunk of lines, the GPU tokenizer (tokenize.cu) leaves the chunk's CSR in
+// embed_off_dev / embed_ids_dev and K3 pools it, into the corpus or the output staging; rows are booked at the end
+// only if no token was out of range, as stb_embed does.
+int stb_embed_text(stb_ctx *ctx, const stb_tokenizer *tok, const stb_table *table, const uint8_t *text,
+                   const uint64_t *text_offsets, uint64_t n_lines, uint32_t max_length, float *out, stb_corpus *append_to) {
+  int rc = ctx_use(ctx);
+  if (rc) return rc;
+  if (!tok || !table) { stb_set_error("embed_text: null tokenizer or table"); return STB_ERR_ARG; }
+  if (stb_tokenizer_ctx(tok) != ctx || table->ctx != ctx || (append_to && append_to->ctx != ctx)) {
+    stb_set_error("embed_text: handles belong to another context"); return STB_ERR_ARG;
+  }
+  if (n_lines == 0) return STB_OK;
+  StbTextHost h;
+  if ((rc = stb_text_host(tok, text, text_offsets, n_lines, max_length, h)) != STB_OK) return rc;
+  const bool host_rows = append_to && append_to->host_rows;
+  const uint64_t n0 = append_to ? append_to->n : 0;
+  if (host_rows) { if ((rc = host_append_begin(append_to, n_lines, std::min<uint64_t>(n_lines, STB_TEXT_CHUNK_LINES))) != STB_OK) return rc; }
+  else if (append_to) { if ((rc = corpus_reserve(append_to, n0 + n_lines)) != STB_OK) return rc; }
+  else if ((rc = ctx->embed_out_dev.reserve(std::min<uint64_t>(n_lines, STB_TEXT_CHUNK_LINES) * STB_D, 4096 * STB_D)) != STB_OK) return rc;
+  if ((rc = stb_tok_reserve(ctx, tok, h, text_offsets, max_length)) != STB_OK) return rc;
+  STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
+  STB_CUDA(cudaMemsetAsync(ctx->tok_flag, 0, sizeof(int), ctx->stream));
+  for (size_t c = 0; c + 1 < h.chunk_at.size(); ++c) {
+    const uint64_t l0 = h.chunk_at[c], m = h.chunk_at[c + 1] - l0;
+    if ((rc = stb_tok_chunk(ctx, tok, h, text, text_offsets, l0, m, max_length)) != STB_OK) return rc;
+    float *dst = host_rows ? ctx->mut_stage.p : append_to ? append_to->rows + (n0 + l0) * STB_D : ctx->embed_out_dev.p;
+    if ((rc = stb_launch_embed(ctx, table, ctx->embed_off_dev, ctx->embed_ids_dev, m, dst, ctx->err_flag)) != STB_OK) return rc;
+    if (out) STB_CUDA(cudaMemcpyAsync(out + l0 * STB_D, dst, m * STB_D * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+    if (host_rows && (rc = host_append_chunk(append_to, ctx->mut_stage, n0 + l0, m)) != STB_OK) return rc;
+  }
+  int flag[2] = {0, 0};
+  STB_CUDA(cudaMemcpyAsync(&flag[0], ctx->err_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  STB_CUDA(cudaMemcpyAsync(&flag[1], ctx->tok_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
+  STB_CUDA(cudaStreamSynchronize(ctx->stream));
+  if (flag[1]) { stb_set_error("embed_text: a GPU piece overflowed its bound (flag %d)", flag[1]); return STB_ERR_STATE; }
+  if (flag[0]) { stb_set_error("embed: a token id maps outside the %llu-row table", (unsigned long long)table->V); return STB_ERR_RANGE; }
+  if (host_rows) return host_append_finish(append_to, n_lines);
   if (append_to) { append_to->n += n_lines; corpus_changed(append_to, CORPUS_APPEND); }
   return STB_OK;
 }

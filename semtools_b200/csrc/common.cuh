@@ -214,6 +214,12 @@ struct stb_ctx {
   StbBuf<uint64_t> embed_off_dev;  // K3 staging: CSR offsets
   StbBuf<uint32_t> embed_ids_dev;  // K3 staging: token ids
   StbBuf<float> embed_out_dev;     // K3 output when not appending to a corpus
+  // GPU tokenizer (tokenize.cu), one chunk of stb_embed_text at a time: text and line offsets, the rule's verdict,
+  // the host-tokenised lines' ids, the normalised lines and their ids before compaction, per-line counts
+  StbBuf<uint8_t> tok_text, tok_taken, tok_norm;
+  StbBuf<uint64_t> tok_off, tok_hoff;
+  StbBuf<uint32_t> tok_hids, tok_nlen, tok_tmp, tok_cnt;
+  StbBuf<int> tok_flag;            // device int: a piece past the cap (never set when the rule holds)
   // in-place corpus mutations (stb_corpus_update / _remove): row staging (<= STB_MUT_CHUNK_ROWS rows),
   // row ids or kept-segment table, and the q8 / shadow bad-row flags
   StbBuf<float> mut_stage;
@@ -460,6 +466,32 @@ enum { STB_ATTR_GEMM0 = 0, STB_ATTR_GEMM1, STB_ATTR_MERGE, STB_ATTR_IVF_PROBE, S
 int stb_launch_embed(stb_ctx *ctx, const stb_table *t, const uint64_t *offsets_dev,
                      const uint32_t *ids_dev, uint64_t n_lines, float *out_dev,
                      int *err_flag_dev);
+
+// ---- api.cu ----------------------------------------------------------------------
+int stb_ctx_use(const stb_ctx *ctx);      // validates the handle and makes its device current
+bool stb_ctx_alive(const stb_ctx *ctx);
+
+// ---- tokenize.cu (GPU tokenizer of stb_embed_text) ------------------------------------
+#define STB_TEXT_CHUNK_LINES 65536                 // lines per chunk of stb_embed_text
+#define STB_TEXT_CHUNK_BYTES (16ull << 20)         // text bytes per chunk (a longer line is a chunk of its own)
+// The host half of a text call: the rule's verdict per line, the declined lines tokenised on host threads
+// (CSR over ALL lines, empty for a taken line; already unk-dropped and truncated), the chunk boundaries.
+struct StbTextHost {
+  std::vector<uint8_t> taken;
+  std::vector<uint64_t> hoff;
+  std::vector<uint32_t> hids;
+  std::vector<uint64_t> chunk_at;                  // first line of each chunk, then n_lines
+};
+// Checks the text CSR, applies the rule and runs the host half; STB_ERR_ARG if the host tokenizer refuses a line.
+int stb_text_host(const stb_tokenizer *tok, const uint8_t *text, const uint64_t *offsets, uint64_t n_lines,
+                  uint32_t max_length, StbTextHost &h);
+// Grows the tokenizer scratch and K3's CSR staging to the largest chunk of the call, before its first chunk.
+int stb_tok_reserve(stb_ctx *ctx, const stb_tokenizer *tok, const StbTextHost &h, const uint64_t *offsets, uint32_t max_length);
+// Tokenises lines [l0, l0 + m) (one chunk) into the K3 CSR ctx->embed_off_dev[m + 1] / ctx->embed_ids_dev, on the
+// stream; the pieces-past-the-cap flag goes to ctx->tok_flag (zeroed by the caller).
+const stb_ctx *stb_tokenizer_ctx(const stb_tokenizer *tok);
+int stb_tok_chunk(stb_ctx *ctx, const stb_tokenizer *tok, const StbTextHost &h, const uint8_t *text,
+                  const uint64_t *offsets, uint64_t l0, uint64_t m, uint32_t max_length);
 
 // ---- batch_scan.cu (K2) ------------------------------------------------------------------
 // rows_first: the row rows_dev[0] holds, as stb_launch_q8_build

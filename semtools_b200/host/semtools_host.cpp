@@ -234,6 +234,17 @@ std::vector<uint32_t> WordLevelTokenizer::encode(const std::string &text) const 
   return ids;
 }
 
+std::string_view truncate_chars(std::string_view line, size_t max_chars) {
+  if (!max_chars || line.size() <= max_chars) return line;        // bytes >= chars: only then can it be too long
+  size_t pos = 0, chars = 0;
+  while (pos < line.size() && chars < max_chars) {
+    const unsigned char c = (unsigned char)line[pos];
+    pos += c < 0x80 ? 1 : (c >> 5) == 6 ? 2 : (c >> 4) == 14 ? 3 : (c >> 3) == 30 ? 4 : 1;
+    ++chars;
+  }
+  return line.substr(0, std::min(pos, line.size()));
+}
+
 void tokenize_to_csr(const std::vector<std::string> &lines, const Tokenizer &tok, size_t max_len,
                      std::vector<uint64_t> &offsets, std::vector<uint32_t> &ids, unsigned threads) {
   const size_t n = lines.size();
@@ -246,19 +257,7 @@ void tokenize_to_csr(const std::vector<std::string> &lines, const Tokenizer &tok
     auto &out = part[t];
     const size_t max_chars = tok.median_token_length() ? max_len * tok.median_token_length() : 0;
     for (size_t i = lo; i < hi; ++i) {
-      // truncate_str(line, max_tokens, median_token_length): cut at max_tokens * median CHARACTERS first
-      const std::string *line = &lines[i];
-      std::string cut;
-      if (max_chars && line->size() > max_chars) {              // bytes >= chars: only then can it be too long
-        size_t pos = 0, chars = 0;
-        while (pos < line->size() && chars < max_chars) {
-          const unsigned char c = (unsigned char)(*line)[pos];
-          pos += c < 0x80 ? 1 : (c >> 5) == 6 ? 2 : (c >> 4) == 14 ? 3 : (c >> 3) == 30 ? 4 : 1;
-          ++chars;
-        }
-        if (pos < line->size()) { cut = line->substr(0, pos); line = &cut; }
-      }
-      auto v = tok.encode(*line);
+      auto v = tok.encode(std::string(truncate_chars(lines[i], max_chars)));
       if (v.size() > max_len) v.resize(max_len);               // truncate(max_length)
       offsets[i + 1] = v.size();                               // per-line count; prefix-summed below
       out.insert(out.end(), v.begin(), v.end());
@@ -282,6 +281,7 @@ Searcher::Searcher(int device) {
 }
 
 Searcher::~Searcher() {
+  stb_tokenizer_destroy(text_tok_);
   stb_corpus_destroy(corpus_);
   stb_table_destroy(table_);
   stb_ctx_destroy(ctx_);
@@ -292,6 +292,14 @@ void Searcher::load_table(const float *E, uint64_t V, bool normalize, const floa
   if (table_) { stb_table_destroy(table_); table_ = nullptr; }
   check(stb_table_load(ctx_, E, V, STB_DIM, n_weights ? weights : nullptr, n_weights, n_mapping ? mapping : nullptr, n_mapping,
                        normalize ? 1 : 0, &table_));
+}
+
+bool Searcher::load_text_tokenizer(const std::string &json) {
+  if (text_tok_) { stb_tokenizer_destroy(text_tok_); text_tok_ = nullptr; }
+  const int rc = stb_tokenizer_load(ctx_, reinterpret_cast<const uint8_t *>(json.data()), json.size(), &text_tok_);
+  if (rc == STB_ERR_ARG) { text_tok_ = nullptr; return false; }
+  check(rc);
+  return true;
 }
 
 // ---- model directory (safetensors) ---------------------------------------------------------------
@@ -391,9 +399,28 @@ static void to_csr(const std::vector<std::string> &lines, const Tokenizer &tok, 
 // (stb_embed: CSR H2D + kernel + optional D2H), so host tokenisation and the GPU overlap; the result is
 // identical to one big batch because lines are independent.  `out` (n x 256) and `append_to` may be null.
 static const size_t kEmbedBatchLines = 16384;
+// With the tokenizer loaded into the library (text_tok), each batch goes to stb_embed_text as text instead, cut by
+// truncate_str as tokenize_to_csr cuts it: the library tokenises it, so there is no producer thread to run.
 static void embed_batched(stb_ctx *ctx, stb_table *table, const std::vector<std::string> &lines, const Tokenizer &tok,
-                          float *out, stb_corpus *append_to) {
+                          float *out, stb_corpus *append_to, const stb_tokenizer *text_tok) {
   const size_t n = lines.size(), n_batches = (n + kEmbedBatchLines - 1) / kEmbedBatchLines;
+  if (text_tok) {
+    const size_t max_chars = tok.median_token_length() ? 2048 * tok.median_token_length() : 0;
+    std::string text;
+    std::vector<uint64_t> offsets;
+    for (size_t b = 0; b < n_batches; ++b) {
+      const size_t first = b * kEmbedBatchLines, count = std::min(kEmbedBatchLines, n - first);
+      text.clear();
+      offsets.assign(1, 0);
+      for (size_t i = first; i < first + count; ++i) {
+        text += truncate_chars(lines[i], max_chars);
+        offsets.push_back(text.size());
+      }
+      check(stb_embed_text(ctx, text_tok, table, reinterpret_cast<const uint8_t *>(text.data()), offsets.data(), count, 2048,
+                           out ? out + first * STB_DIM : nullptr, append_to));
+    }
+    return;
+  }
   struct Batch { std::vector<uint64_t> offsets; std::vector<uint32_t> ids; size_t first = 0, count = 0; };
   auto tokenise = [&](size_t b, Batch &dst) {
     dst.first = b * kEmbedBatchLines;
@@ -426,7 +453,7 @@ bool Searcher::add_document(const std::string &filename, const std::string &cont
   std::vector<std::string> emb_lines = lines;
   if (ignore_case) for (auto &l : emb_lines) l = to_lowercase(l);
   Document d{filename, std::move(lines), rows()};
-  embed_batched(ctx_, table_, emb_lines, tok, nullptr, corpus_);   // rows go straight into the corpus in HBM
+  embed_batched(ctx_, table_, emb_lines, tok, nullptr, corpus_, text_tok_);   // rows go straight into the corpus in HBM
   docs_.push_back(std::move(d));
   return true;
 }
@@ -437,7 +464,7 @@ std::vector<float> Searcher::embed_lines(const std::vector<std::string> &lines, 
   if (lines.empty()) return out;
   std::vector<std::string> emb_lines = lines;
   if (ignore_case) for (auto &l : emb_lines) l = to_lowercase(l);
-  embed_batched(ctx_, table_, emb_lines, tok, out.data(), nullptr);
+  embed_batched(ctx_, table_, emb_lines, tok, out.data(), nullptr, text_tok_);
   return out;
 }
 

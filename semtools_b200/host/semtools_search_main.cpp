@@ -264,7 +264,15 @@ static int real_main(int argc, char **argv) {
     const float *tab_E = model_dir.empty() ? reinterpret_cast<const float *>(raw.data()) : md.E.data();
     const uint64_t tab_V = model_dir.empty() ? raw.size() / (STB_DIM * sizeof(float)) : md.V;
     const bool tab_norm = model_dir.empty() ? true : md.normalize;
-    auto load = [&](Searcher &s) { s.load_table(tab_E, tab_V, tab_norm, md.weights.data(), md.weights.size(), md.mapping.data(), md.mapping.size()); };
+    std::string tok_text;                          // a tokenizer.json also goes to the library: lines are embedded from text
+    if (!tokenizer_json.empty()) {
+      std::ifstream tf(tokenizer_json, std::ios::binary);
+      tok_text.assign((std::istreambuf_iterator<char>(tf)), std::istreambuf_iterator<char>());
+    }
+    auto load = [&](Searcher &s) {
+      s.load_table(tab_E, tab_V, tab_norm, md.weights.data(), md.weights.size(), md.mapping.data(), md.mapping.size());
+      if (!tok_text.empty()) s.load_text_tokenizer(tok_text);
+    };
     // identity of this host's embedder, recorded in the store so its vectors are never mixed with another
     // host's / model's (ADVICE r1): a model directory gets the Python host's fingerprint string, the
     // synthetic forms (vocabulary file / bare tokenizer.json + raw table) their own

@@ -296,8 +296,15 @@ void HfTokenizer::add_pre(const Json &j) {
   throw std::runtime_error("tokenizer.json: pre_tokenizer \"" + t + "\" is not supported by the C++ host");
 }
 
-HfTokenizer::HfTokenizer(const std::string &path) {
-  const std::string text = slurp(path);
+HfTokenizer::HfTokenizer(const std::string &path) { load(slurp(path)); }
+
+std::unique_ptr<HfTokenizer> HfTokenizer::from_json(const std::string &json_text) {
+  std::unique_ptr<HfTokenizer> t(new HfTokenizer());
+  t->load(json_text);
+  return t;
+}
+
+void HfTokenizer::load(const std::string &text) {
   file_hash_ = stb_fnv1a64(reinterpret_cast<const uint8_t *>(text.data()), text.size());
   const Json j = Json::parse(text);
   if (const Json *n = j.get("normalizer")) add_norm(*n);
@@ -366,6 +373,57 @@ HfTokenizer::HfTokenizer(const std::string &path) {
   for (const auto &t : tokens_) lens.push_back(t.size());
   std::sort(lens.begin(), lens.end());
   median_len_ = std::max<size_t>(1, lens[lens.size() / 2]);
+}
+
+HfTokenizer::AsciiPlan HfTokenizer::ascii_plan() const {
+  AsciiPlan p, none;
+  if (pre_.size() != 1 || pre_[0].kind != P_METASPACE || !pre_[0].split || !has_unk_) return none;
+  const std::string &rep = pre_[0].replacement;
+  // one non-ASCII character: it cannot occur in a printable-ASCII line, so only spaces delimit pieces
+  if (rep.empty() || (unsigned char)rep[0] < 0x80 || utf8_len((unsigned char)rep[0]) != rep.size()) return none;
+  p.replacement = rep;
+  p.prepend_scheme = pre_[0].prepend;
+  bool lower = false;
+  for (const auto &st : norm_) lower = lower || st.kind == N_LOWER;
+  for (int c = 0x20; c < 0x7F; ++c) p.byte_ok[c] = true;
+  for (const auto &st : norm_) {
+    switch (st.kind) {
+      case N_LOWER: p.ops.push_back({OP_LOWER, true, true, ""}); break;
+      case N_REPLACE_MULTISPACE:
+        if (st.b != " ") return none;
+        p.ops.push_back({OP_MULTISPACE, true, true, ""}); break;
+      case N_STRIP:
+        p.ops.push_back({OP_STRIP, st.left, st.right, ""});
+        p.decline_leading_space = p.decline_leading_space || (st.left && p.prepend_scheme == PREPEND_FIRST);
+        break;
+      case N_PREPEND:
+        p.ops.push_back({OP_PREPEND, true, true, st.a});
+        p.grow += st.a.size(); break;
+      case N_PRECOMPILED: {
+        const Charsmap &m = maps_[st.map];
+        if (m.trie.empty()) break;                           // identity
+        for (int c = 0x20; c < 0x7F; ++c) {
+          const int l = (lower && c >= 'A' && c <= 'Z') ? c + 32 : c;
+          p.byte_ok[c] = p.byte_ok[c] && m.ascii_plain[c] && m.ascii_plain[l];
+        }
+        break;
+      }
+      default: return none;                                  // string Replace, the Unicode forms
+    }
+  }
+  for (const auto &op : p.ops)                               // Prepend text goes through the same checks as the line
+    for (unsigned char c : op.text)
+      if (c < 0x20 || c > 0x7E || !p.byte_ok[c]) return none;
+  for (const auto &a : added_raw_) p.added.push_back(a.content);
+  for (const auto &a : added_norm_) p.added.push_back(a.content);
+  p.added_normalized = !added_norm_.empty();
+  p.ok = true;
+  return p;
+}
+
+HfTokenizer::TrieView HfTokenizer::trie() const {
+  return {root_, first_child_.data(), child_byte_.data(), child_node_.data(), terminal_.data(), terminal_.size(), child_node_.size(),
+          scores_.data(), scores_.size(), min_score_ - 10.0, has_unk_, unk_id_, drop_unk_, drop_id_};
 }
 
 std::string HfTokenizer::normalize(const std::string &in) const {

@@ -25,6 +25,7 @@
 #pragma once
 
 #include <cstdint>
+#include <memory>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -37,6 +38,8 @@ namespace semtools {
 class HfTokenizer : public Tokenizer {
  public:
   explicit HfTokenizer(const std::string &tokenizer_json_path);
+  // the same from the bytes of a tokenizer.json (stb_tokenizer_load)
+  static std::unique_ptr<HfTokenizer> from_json(const std::string &json_text);
   // ids of one line as encode_with_args prepares them: the id of the model's `unk_token` removed -- when the
   // model section NAMES one (WordPiece / BPE style "unk_token": "<tok>"; model2vec-rs reads exactly that key,
   // [UPSTREAM-MEMORY]).  A Unigram section carries `unk_id` instead, so -- as in the Python host and in
@@ -54,7 +57,38 @@ class HfTokenizer : public Tokenizer {
   // fnv1a64 of the file: part of the store's model fingerprint
   uint64_t fingerprint() const { return file_hash_; }
 
+  // What the library's GPU tokenizer (stb_embed_text) restates: encode_raw's fast path -- a single Metaspace
+  // step with split = true -- on lines of printable ASCII, where every normaliser step is one of the ops below.
+  // ok = false: the shape has no GPU form and every line stays on the host.
+  enum AsciiOpKind { OP_LOWER = 0, OP_MULTISPACE, OP_STRIP, OP_PREPEND };
+  struct AsciiOp { int kind; bool left = true, right = true; std::string text; };
+  struct AsciiPlan {
+    bool ok = false;
+    std::vector<AsciiOp> ops;              // the normaliser on printable ASCII, in order (Precompiled steps are the identity there)
+    bool byte_ok[128] = {};                // printable bytes every Precompiled step leaves alone, as they are and lowercased
+    size_t grow = 0;                       // bytes the Prepend steps can add to a line
+    std::string replacement;               // Metaspace: one non-ASCII character
+    int prepend_scheme = 0;                // 0 always, 1 first, 2 never
+    std::vector<std::string> added;        // contents of every added token, normalised or not
+    bool added_normalized = false;         // some of them are matched in the normalised text
+    // a left Strip under prepend scheme "first": HF decides "first" by the original offset of the split, which a
+    // stripped leading space moves off 0, so a line that starts with a space is not taken
+    bool decline_leading_space = false;
+  };
+  AsciiPlan ascii_plan() const;
+  // The Unigram model as unigram() reads it: root_[256], first_child_[n_nodes + 1], child_byte_ / child_node_
+  // [n_edges], terminal_[n_nodes], scores_[vocab]
+  struct TrieView {
+    const uint32_t *root; const uint32_t *first_child; const uint8_t *child_byte; const uint32_t *child_node;
+    const int32_t *terminal; size_t n_nodes, n_edges;
+    const double *scores; size_t n_scores; double unk_score;   // min_score - 10
+    bool has_unk; uint32_t unk_id; bool drop_unk; uint32_t drop_id;
+  };
+  TrieView trie() const;
+
  private:
+  HfTokenizer() = default;
+  void load(const std::string &json_text);
   struct NormStep { int kind; std::string a, b; bool left = true, right = true; int map = -1; };
   // SentencePiece precompiled charsmap: darts-clone double array + NUL-separated replacement strings
   struct Charsmap {

@@ -31,6 +31,8 @@ class StaticModel:
         self.unk_token_id = unk_token_id
         self.ctx = ctx
         self._table = None
+        self._tokenizer_json = None                              # tokenizer.json bytes (from_pretrained)
+        self._text_tok = None
 
     # -- StaticModel::from_pretrained(path, token, normalize, subfolder) -----------------------
     @classmethod
@@ -70,7 +72,8 @@ class StaticModel:
             raise ValueError(f"embedding table must be V x {capi.STB_DIM}, got {emb.shape}")
         m = cls(tokenizer, emb, weights, mapping, normalize, median, unk_id, ctx)
         with open(tok_path, "rb") as f:
-            m._tokenizer_file_hash = capi.fnv1a64(f.read())     # the C++ host hashes the same bytes (load_model_dir)
+            m._tokenizer_json = f.read()
+        m._tokenizer_file_hash = capi.fnv1a64(m._tokenizer_json)     # the C++ host hashes the same bytes (load_model_dir)
         return m
 
     def fingerprint(self) -> str:
@@ -91,11 +94,14 @@ class StaticModel:
         """Keep the first max_tokens * median_token_length chars (char boundary safe)."""
         return text[: max_tokens * median_token_length]
 
+    def truncated(self, sentences, max_length):
+        return [self.truncate_str(s, max_length, self.median_token_length) if max_length is not None else s
+                for s in sentences]
+
     def tokenize(self, sentences, max_length):
         """-> (offsets u64[n+1], ids u32[...]) exactly as encode_with_args prepares them:
         char-truncate, encode_batch_fast(add_special_tokens=false), drop unk, truncate."""
-        texts = [self.truncate_str(s, max_length, self.median_token_length) if max_length is not None else s
-                 for s in sentences]
+        texts = self.truncated(sentences, max_length)
         encs = self.tokenizer.encode_batch(texts, add_special_tokens=False) if texts else []
         rows = []
         for e in encs:
@@ -119,15 +125,51 @@ class StaticModel:
             self._table = capi.Table(self.ctx, self.embeddings, self.weights, self.mapping, self.normalize)
         return self._table
 
+    def text_tokenizer(self) -> capi.Tokenizer | None:
+        """The model's tokenizer.json loaded into the library (stb_embed_text tokenises on the GPU), or None:
+        a model built in memory, or a tokenizer shape the library's tokenizer does not read."""
+        if self._text_tok is None and self._tokenizer_json is not None:
+            self.table()
+            try:
+                self._text_tok = capi.Tokenizer(self.ctx, self._tokenizer_json)
+            except capi.StbError as e:
+                if e.status != capi.STB_ERR_ARG:
+                    raise
+                self._text_tok = False
+        return self._text_tok or None
+
+    def _prepare(self, sentences, max_length):
+        """One batch, ready for the GPU: ("text", truncated lines) when the library's tokenizer takes every line
+        (stb_tokenizer_gpu_lines), else ("ids", CSR) from HF `tokenizers` -- the same ids either way."""
+        tok = self.text_tokenizer() if max_length is not None else None
+        if tok is not None:
+            texts = self.truncated(sentences, max_length)
+            if len(texts) and tok.gpu_lines(texts).all():
+                return "text", texts
+        return "ids", self.tokenize(sentences, max_length)
+
+    def _embed_prepared(self, item, max_length, append_to):
+        kind, data = item
+        table = self.table()
+        if kind == "text":
+            return capi.embed_text(self.ctx, self.text_tokenizer(), table, data, max_length, out=append_to is None,
+                                   append_to=append_to)
+        offsets, ids = data
+        return capi.embed(self.ctx, table, offsets, ids, out=append_to is None, append_to=append_to)
+
+    def embed_batch(self, sentences, max_length, append_to: capi.Corpus | None = None):
+        """encode_with_args for one batch, without the producer thread: rows, or None with append_to."""
+        return self._embed_prepared(self._prepare(sentences, max_length), max_length, append_to)
+
     # -- encode_with_args(&sentences, max_length, batch_size) -> Vec<Vec<f32>> -------------------------
     def encode_with_args(self, sentences, max_length=512, batch_size=1024, append_to: capi.Corpus | None = None):
-        """Batches are tokenised on a producer thread (HF tokenizers releases the GIL and is
-        itself multi-threaded) while the previous batch is pooled on the GPU: host
-        tokenisation, the remaining CPU cost of ingestion (SURVEY 8f-2), overlaps K3."""
+        """Batches are prepared on a producer thread while the previous batch is pooled on the GPU.  A batch
+        whose every line the library's tokenizer takes is tokenised on the GPU (stb_embed_text); any other is
+        tokenised by HF tokenizers (which releases the GIL and is itself multi-threaded), overlapping K3."""
         import queue
         import threading
         out = [] if append_to is None else None
-        table = self.table()
+        self.table()
         starts = list(range(0, len(sentences), batch_size))
         if not starts:
             return None if append_to is not None else np.zeros((0, capi.STB_DIM), dtype=np.float32)
@@ -136,7 +178,7 @@ class StaticModel:
         def producer():
             try:
                 for b in starts:
-                    q.put(self.tokenize(sentences[b:b + batch_size], max_length))
+                    q.put(self._prepare(sentences[b:b + batch_size], max_length))
             except BaseException as e:          # surface tokenizer failures on the consumer side
                 q.put(e)
 
@@ -146,8 +188,7 @@ class StaticModel:
             item = q.get()
             if isinstance(item, BaseException):
                 raise item
-            offsets, ids = item
-            res = capi.embed(self.ctx, table, offsets, ids, out=append_to is None, append_to=append_to)
+            res = self._embed_prepared(item, max_length, append_to)
             if out is not None:
                 out.append(res)
         t.join()

@@ -87,13 +87,13 @@ class Searcher:
         self._starts.append(doc.row_start)
         return doc
 
-    def add_document_tokens(self, filename: str, lines: list, table: capi.Table, offsets, ids):
-        """Same, with the embeddings produced by K3 straight into HBM
-        (encode_with_args(lines, Some(2048), 16384) at :69, tokenisation on host)."""
+    def add_document_lines(self, filename: str, lines: list, model, emb_lines: list):
+        """Same, with the model embedding emb_lines straight into HBM (encode_with_args(lines, Some(2048), 16384)
+        at :69; StaticModel.embed_batch picks the GPU tokenizer or HF tokenizers)."""
         if len(lines) == 0:
             return None
         doc = Document(filename, list(lines), len(self.corpus))
-        capi.embed(self.ctx, table, offsets, ids, out=False, append_to=self.corpus)
+        model.embed_batch(emb_lines, 2048, append_to=self.corpus)
         self.documents.append(doc)
         self._starts.append(doc.row_start)
         return doc
