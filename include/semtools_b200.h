@@ -732,6 +732,14 @@ int stb_debug_q4_refined(stb_ctx *ctx, int reset, uint64_t *refined);
  * calls on one corpus co-scans: each query after the first starts where its predecessor is
  * reading.  Synchronises the context's stream. */
 int stb_debug_coscan_offsets(stb_ctx *ctx, uint32_t n, uint32_t *out);
+/* Test hooks for K1's pairs: a q8 top-k query of an asynchronous series (stb_search_topk_dev, stb_search_many
+ * without an exchange) that follows a query on the same corpus joins its running scan, which scores both
+ * queries from one read of each plane tile.  stb_debug_pair_joins: for the last n top-k launches on the
+ * ticket ring, oldest first, the tile at which each joined its host; -1 for a launch that was not such a
+ * guest, -2 for a guest whose join was refused (it scanned alone).  Synchronises the context's stream.
+ * stb_debug_pair_floor: later joins wait until their host has drawn v_floor tile tickets (0: no wait). */
+int stb_debug_pair_joins(stb_ctx *ctx, uint32_t n, int64_t *out);
+int stb_debug_pair_floor(stb_ctx *ctx, uint64_t v_floor);
 /* Test hook for the candidate copies: copies entries [first, first+n) of one copy to `out` and sets
  * *covered (may be NULL) to the rows the copy covers (0: not built).  which = STB_COPY_Q8_CODES (256 B per
  * row), _Q8_SCALES (f32 per row), _Q8_PLANE (nibble plane, 128 B per row), _Q8_SR ({s, rho}, 2 x f32 per

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Per-kernel SASS mnemonic counts of the shipped library (a reader's view of tests/test_sass_contract.py),
-and the q8 top-k prefilter's tile body: instructions per 32-row tile and their opcode mix
+and the q8 top-k prefilter's tile bodies, the pair's included: instructions per 32-row tile and their opcode mix
     python scripts/sass_summary.py [lib.so]"""
 import collections, re, subprocess, sys
 lib = sys.argv[1] if len(sys.argv) > 1 else "semtools_b200/lib/libsemtools_b200.so"
@@ -34,34 +34,44 @@ for fn, c in cnt.items():
 print("\nTOTAL  " + ", ".join(f"{k}: {tot[k]}" for k in pat))
 
 
-def tile_body(ins):
-    """The prefilter's tile: from the head of the innermost loop around the first ballot (VOTE.ANY with a
-    register result: the refine-queue vote) to the first conditional branch after it (the queue-full test)."""
-    vote = next((i for i, (_, t) in enumerate(ins) if re.match(r"VOTE\.ANY R", t)), None)
-    if vote is None:
-        return None
+def tile_bodies(ins):
+    """The prefilter's tile bodies: from the head of the innermost loop around a ballot (VOTE.ANY with a register
+    result: the refine-queue vote) to the first conditional branch after it (the queue-full test).  A pair's host
+    has three: its own query's, the pair's (both queries' accumulators on one set of plane loads: two votes) and
+    the guest-only wrap's."""
     at = {a: i for i, (a, _) in enumerate(ins)}
-    head = None
-    for i, (a, t) in enumerate(ins):
-        m = re.match(r"(@!?U?P\w+ )?BRA (0x[0-9a-f]+)", t)
-        if m and i > vote and at.get(int(m.group(2), 16), i) <= vote:
-            h = at[int(m.group(2), 16)]
-            head = h if head is None or h > head else head
-    end = next((i for i in range(vote, len(ins)) if re.match(r"@!?P\w+ BRA ", ins[i][1])), None)
-    return None if head is None or end is None else ins[head:end + 1]
+    seen = set()
+    for vote, (_, t) in enumerate(ins):
+        if not re.match(r"VOTE\.ANY R", t):
+            continue
+        head = None
+        for i, (a, tt) in enumerate(ins):
+            m = re.match(r"(@!?U?P\w+ )?BRA (0x[0-9a-f]+)", tt)
+            if m and i > vote and at.get(int(m.group(2), 16), i) <= vote:
+                h = at[int(m.group(2), 16)]
+                head = h if head is None or h > head else head
+        end = next((i for i in range(vote, len(ins)) if re.match(r"@!?P\w+ BRA ", ins[i][1])), None)
+        if head is None or end is None or head in seen:
+            continue
+        seen.add(head)
+        yield ins[head:end + 1]
 
 
-print("\n# q8 top-k prefilter tile body (32 rows per warp)")
+print("\n# q8 top-k prefilter tile bodies (32 rows per warp)")
 for fn, ins in code.items():
-    if not re.search(r"stb_scan_topk_kernel<\d+, \d+, \d+, 2, \d+>", names.get(fn, "")):
+    if not re.search(r"stb_scan_topk_kernel_q8<\d+, \d+, \d+, \d+>", names.get(fn, "")):
         continue
-    body = tile_body(ins)
-    if body is None:
+    found = False
+    for body in tile_bodies(ins):
+        mix = collections.Counter()
+        for _, t in body:
+            op = re.sub(r"^@!?U?P\w+ ", "", t).split()[0]
+            mix["IDP.4A" if op.startswith("IDP.4A") else op.split(".")[0]] += 1
+        if mix["IDP.4A"] < 128 or mix["LOP3"] < 64:   # not a plane tile (lists, sorts, the int8 refine)
+            continue
+        found = True
+        kind = "pair (two queries)" if mix["IDP.4A"] >= 256 else "one query"
+        print(f"{names[fn]} [{kind}]: {len(body)} instructions ({len(body) / 32:.1f} per row)")
+        print("    " + ", ".join(f"{k}: {v}" for k, v in mix.most_common()))
+    if not found:
         print(names[fn], ": tile body not found")
-        continue
-    mix = collections.Counter()
-    for _, t in body:
-        op = re.sub(r"^@!?U?P\w+ ", "", t).split()[0]
-        mix["IDP.4A" if op.startswith("IDP.4A") else op.split(".")[0]] += 1
-    print(f"{names[fn]}: {len(body)} instructions ({len(body) / 32:.1f} per row)")
-    print("    " + ", ".join(f"{k}: {v}" for k, v in mix.most_common()))

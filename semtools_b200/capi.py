@@ -30,7 +30,7 @@ SYMBOLS = [
     "stb_xchg_create", "stb_xchg_destroy", "stb_xchg_local_handle",
     "stb_xchg_connect", "stb_xchg_connect_local", "stb_search_topk_xchg", "stb_search_xchg", "stb_search_many", "stb_xchg_create_batch", "stb_search_batch_xchg_dev", "stb_ivfpq_build",
     "stb_ivfpq_destroy", "stb_ivfpq_extend", "stb_ivfpq_stats", "stb_ivfpq_search", "stb_ivfpq_search_dev", "stb_hits_merge_dev", "stb_hits_merge_batch_dev", "stb_hits_merge", "stb_fnv1a64", "stb_line_id", "stb_line_ids",
-    "stb_ctx_counters", "stb_debug_ticket_check", "stb_debug_q4_refined", "stb_debug_coscan_offsets", "stb_debug_batch_gemm", "stb_debug_batch_params",
+    "stb_ctx_counters", "stb_debug_ticket_check", "stb_debug_q4_refined", "stb_debug_coscan_offsets", "stb_debug_pair_joins", "stb_debug_pair_floor", "stb_debug_batch_gemm", "stb_debug_batch_params",
     "stb_debug_batch_last", "stb_debug_batch_q8", "stb_debug_batch_no_shadow", "stb_debug_batch_q8_gemm", "stb_debug_batch_q8_plan", "stb_debug_corpus_copy", "stb_debug_scan_scores", "stb_debug_q4_scan",
     "stb_debug_ivfpq_export",
     "stb_ivfpq_search_batch", "stb_ivfpq_search_batch_dev", "stb_debug_ivfpq_batch_last",
@@ -135,6 +135,8 @@ def lib() -> C.CDLL:
     L.stb_debug_ticket_check.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
     L.stb_debug_q4_refined.argtypes = [vp, i32, C.POINTER(u64)]
     L.stb_debug_coscan_offsets.argtypes = [vp, u32, vp]
+    L.stb_debug_pair_joins.argtypes = [vp, u32, vp]
+    L.stb_debug_pair_floor.argtypes = [vp, u64]
     L.stb_debug_batch_gemm.argtypes = [vp, vp, u32, vp, u64, vp, vp]
     L.stb_debug_batch_params.argtypes = [C.POINTER(C.c_int), C.POINTER(C.c_double)]
     L.stb_debug_batch_last.argtypes = [vp, vp, vp, vp]
@@ -253,6 +255,17 @@ class Context:
         out = np.zeros(max(n, 1), dtype=np.uint32)
         _check(lib().stb_debug_coscan_offsets(self._h, n, _np_ptr(out)))
         return [None if v == 0xFFFFFFFF else int(v) for v in out[:n]]
+
+    def pair_joins(self, n: int = 8):
+        """stb_debug_pair_joins: join tile of each of the last n top-k launches, oldest first (None: not a
+        guest, "refused": a guest that scanned alone)."""
+        out = np.zeros(max(n, 1), dtype=np.int64)
+        _check(lib().stb_debug_pair_joins(self._h, n, _np_ptr(out)))
+        return [None if v == -1 else ("refused" if v == -2 else int(v)) for v in out[:n]]
+
+    def pair_floor(self, v_floor: int = 0):
+        """stb_debug_pair_floor: later joins wait until their host has drawn v_floor tile tickets."""
+        _check(lib().stb_debug_pair_floor(self._h, int(v_floor)))
 
     def batch_last(self):
         """stb_debug_batch_last: the most recent K2 device call on this context.  Returns a dict with

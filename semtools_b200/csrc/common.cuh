@@ -156,6 +156,20 @@ struct stb_ctx {
   StbBuf<unsigned long long> q4_thr;
   unsigned long long q4_launches;
   StbBuf<unsigned long long> q4_refined;   // rows the prefilter passed on to the int8 codes (stb_debug_q4_refined)
+  // K1 pairs (scan_topk.cu: "pairs"): one seat of STB_SEAT_WORDS device words per ticket slot; the host whose seat
+  // is open; per ticket slot, 1 + the host's slot if its launch was a guest (0: it was not), the guest's tag and
+  // t_bulk (stb_debug_pair_joins); the test hook's floor on the join ticket
+  StbBuf<unsigned long long> pair_seats;
+  struct {
+    const void *rows;
+    uint64_t n_virtual, n_tickets;
+    unsigned long long t_base;
+    int slot;
+    bool open;
+  } pair_host;
+  uint32_t pair_guest_of[8], pair_guest_tag[8];
+  uint64_t pair_t_bulk[8];
+  uint64_t pair_floor;
   StbBuf<float> q_dev;             // 256 f32 staging for host queries
   StbBuf<stb_hit> hits_dev;        // result hits (top-k path)
   StbBuf<uint32_t> status_dev;     // [0]=n hits, [1]=complete flag, [2..] debug
@@ -239,6 +253,16 @@ struct stb_ctx {
 };
 
 #define STB_TICKET_SLOTS 8
+#define STB_TICKET_TILES 4   // co-scan, 10M rows, q8: 4 and 2 tiles 0.434 ms/query, 1 tile 0.635 ms
+// K1 pairs (scan_topk.cu: "pairs"): the words of a seat.  (one seat per ticket slot, indexed by the host's slot; never cleared: the tags tell launches apart)
+#define STB_SEAT_Q 0                 // guest query (device pointer)
+#define STB_SEAT_HITS 1              // guest hits
+#define STB_SEAT_STATUS 2            // guest status
+#define STB_SEAT_THR 3               // guest threshold words
+#define STB_SEAT_INFO 4              // guest q4 tag << 32 | top_k
+#define STB_SEAT_DECIDED 5           // guest tag << 32 | (joined: 0x80000000 | join ticket v; refused: 0)
+#define STB_SEAT_WRAP 6              // host q4 tag << 32 | guest-only tickets drawn
+#define STB_SEAT_WORDS 8
 // Spin-wait bound of the peer-memory exchanges (SM cycles, ~15 s): long enough that ranks entering a sharded
 // search a few seconds apart (first-call allocations, a busy host) still meet; a peer that is really gone
 // costs one bound, the call reports it (status 0xfffffffe / 2) and the caller must stop using the exchange:

@@ -24,6 +24,7 @@
 #include <cuda_fp16.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "common.cuh"
 #include "row_encode.cuh"
@@ -53,7 +54,6 @@ struct ScanArgs {
   unsigned long long t_base;     // its value when this launch starts (host-tracked)
   uint64_t t_bulk;               // tickets [0, t_bulk) cover STB_TICKET_TILES tiles each, later ones one tile
 };
-#define STB_TICKET_TILES 4   // co-scan, 10M rows, q8: 4 and 2 tiles 0.434 ms/query, 1 tile 0.635 ms
 
 // A pass's ScanArgs over ranges_dev as k1_upload_ranges (api.cu) packs them: vstart[n_ranges + 1], then
 // rbegin[n_ranges]; the only decoder of that layout.  No tickets: the top-k launch sets its own.
@@ -478,22 +478,29 @@ struct StbQ4Dump {
   int pin;
 };
 
-template <int U, int RANGES, int DUMP = 0, class Sink>
-__device__ __forceinline__ void stb_scan_q4(const ScanArgs &args, const uint8_t *q8, const float *q8_scale, const StbQ4Args &q4a,
-                                            uint32_t *wq, uint32_t *pw, Sink &sink, const uint32_t *off = nullptr,
-                                            const StbQ4Dump *dump = nullptr) {
-  static_assert(4 * U == STB_Q4_TILE_ROWS && STB_Q8_MAX_K <= 32, "one plane tile per warp tile, one row per lane; one lane per threshold word");
-  const int lane = threadIdx.x & 31;
-  const int g = lane >> 3;   // refine: row group inside the warp
-  const int j = lane & 7;    // refine: int8 code bytes [16j, 16j+16) and [128+16j, ...)
-  const StbQ8Query Q = stb_q8_query(args.q, j);
+// One query as the prefilter sees it: its words in shared memory (layout: stb_scan_q4) and the constants of its
+// bounds.  The guest of a pair keeps a copy of the constants, its threshold words and k in shared memory.
+struct StbQ4Side {
+  float inv_S, h_l1, e_q;        // StbQ8Query
+  float A, B, e_q4;              // u4 = s (A D + B) + rho + e_q4
+  int sumq;                      // sum of the q16 components
+  int unusable;
+  unsigned long long *thr;       // threshold words, their tag and count
+  uint32_t tag;
+  int kw;
+};
+
+// Writes the warp's copy of the query words of q to pw (every lane of the warp calls it) and returns its constants.
+__device__ __forceinline__ StbQ4Side stb_q4_query(const float *q, uint32_t *pw, int lane) {
+  const int g = lane >> 3, j = lane & 7;
+  const StbQ8Query Q = stb_q8_query(q, j);
   // query words in shared memory, read by every lane at once.  Chunk m, word k (components 32m + 4k .. +3
   // pair with its low nibbles, 32m + 16 + 4k .. +3 with its high nibbles): {low hi, low lo, high hi, high lo}
   // byte words at pw[(4m + k) * 4 + {0..3}]; the int8 codes' words (StbQ8Query) of refine lane j at
   // pw[128 + 16 j + {0..7: hi, 8..15: lo}]
   int sumq = 0;
   {
-    const float4 *qv = reinterpret_cast<const float4 *>(args.q);
+    const float4 *qv = reinterpret_cast<const float4 *>(q);
     int l1 = 0;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -510,24 +517,76 @@ __device__ __forceinline__ void stb_scan_q4(const ScanArgs &args, const uint8_t 
   sumq += __shfl_xor_sync(0xffffffffu, sumq, 4);
   sumq += __shfl_xor_sync(0xffffffffu, sumq, 2);
   sumq += __shfl_xor_sync(0xffffffffu, sumq, 1);
-  const float A = 16.0f * Q.inv_S;
-  const float B = 7.5f * (float)sumq * Q.inv_S;
-  const float e_q4 = 19.4f * Q.inv_S;
+  StbQ4Side S;
+  S.inv_S = Q.inv_S; S.h_l1 = Q.h_l1; S.e_q = Q.e_q;
+  S.A = 16.0f * Q.inv_S;
+  S.B = 7.5f * (float)sumq * Q.inv_S;
+  S.e_q4 = 19.4f * Q.inv_S;
+  S.sumq = sumq;
+  S.unusable = Q.unusable ? 1 : 0;
+  S.thr = nullptr; S.tag = 0u; S.kw = 1;
+  return S;
+}
 
-  const int kw = (int)q4a.top_k;
+// ---- pairs: one read of each plane tile scores two back-to-back queries ----------------------------------
+// A q8 top-k launch of an overlapped series is a HOST or a GUEST (stb_launch_topk_t).  A guest is two launches:
+// stb_pair_join_kernel, which the host releases at its start, and its own scan kernel.  The join publishes
+// the guest's query in the host's seat and then adds STB_PAIR_JUMP to the host's ticket counter: the ticket v
+// the add returns is the join point.  Host draws at or above the jump are tickets >= v, and those below
+// n_tickets score their tiles for both queries; after the host's own tickets run out its warps draw tickets
+// [0, v) again from the seat's wrap word and score them for the guest alone.  So each tile is scored once for
+// each query, and the jump tells a draw that it follows the join with no window between the two.  The host
+// then runs the tail (CTA merge, tree merge, re-rank, proof, hits) once per query.  A join whose add finds
+// every ticket drawn refuses (the host's warps, whose failing draws may follow the jump, read the decision
+// from the seat: the join kernel writes it right after its add, and it is running); so does a query the q8
+// tier cannot use, without a jump.  A refused guest's scan kernel scans by itself.  The host books the jump on
+// its counter when the guest launches; a join without one adds it once the host has completed.
+__device__ __forceinline__ unsigned long long stb_ld_acquire_gpu(const unsigned long long *p) {
+  unsigned long long v;
+  asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+  return v;
+}
+
+// A join kernel starts when its host has drawn ~30k tiles (H100, 10M and 1M rows: median join tiles 29.4k and
+// 27.1k), so a pair reads (n + 30k) tiles for two queries.  Below ~60k tiles (1.9M rows) that saves too little
+// to pay for running the hosts one after the other, and the series co-scans instead (1M rows: 0.070 ms per
+// query paired, 0.053 co-scanning).
+#define STB_PAIR_MIN_TILES 60000
+#define STB_PAIR_JUMP (1ull << 31)   // > every ticket count (tiles < 2^27); a jumped ticket still fits 32 bits
+// seat words: common.cuh (STB_SEAT_*)
+#define STB_PAIR_SCRATCH (STB_Q4_QUEUE + 256 + 16)   // per warp: the guest's queue, words and StbQ4Side
+
+template <int U, int RANGES, int DUMP = 0, bool PAIR = false, class Sink>
+__device__ __forceinline__ bool stb_scan_q4(const ScanArgs &args, const uint8_t *q8, const float *q8_scale, const StbQ4Args &q4a,
+                                            uint32_t *wq, uint32_t *pw, Sink &sink, const uint32_t *off = nullptr,
+                                            const StbQ4Dump *dump = nullptr, unsigned long long *seat = nullptr,
+                                            uint32_t *gscr = nullptr, Sink *sink2 = nullptr) {
+  static_assert(4 * U == STB_Q4_TILE_ROWS && STB_Q8_MAX_K <= 32, "one plane tile per warp tile, one row per lane; one lane per threshold word");
+  static_assert(!PAIR || (RANGES == 0 && DUMP == 0), "pairs scan whole shards");
+  static_assert(sizeof(StbQ4Side) <= 16 * 4, "guest constants");
+  const int lane = threadIdx.x & 31;
+  const int g = lane >> 3;   // refine: row group inside the warp
+  const int j = lane & 7;    // refine: int8 code bytes [16j, 16j+16) and [128+16j, ...)
+  const StbQ4Side S1 = stb_q4_query(args.q, pw, lane);   // its threshold words, tag and k: q4a
   unsigned tcache = 0u;              // lane w < k: best ordered l8 of word w this warp knows (0: none)
-  float T = -CUDART_INF_F;
   int qn = 0;                        // queued rows (warp-uniform)
   unsigned refined = 0u;
+  // the guest (PAIR): queue, words and constants in gscr, list in *sink2
+  uint32_t *wq2 = gscr, *pw2 = gscr + STB_Q4_QUEUE;
+  StbQ4Side *side2 = reinterpret_cast<StbQ4Side *>(gscr + STB_Q4_QUEUE + 256);
+  unsigned tcache2 = 0u;
+  int qn2 = 0;
 
-  auto refine = [&]() {              // the first 32 queue slots (0xffffffff: empty; slot 0 is never empty)
+  // the first 32 queue slots of one query (0xffffffff: empty; slot 0 is never empty)
+  auto refine = [&](const uint32_t *q_wq, const uint32_t *q_pw, const StbQ4Side &S, unsigned long long *thr, uint32_t tag, int kw,
+                    auto &snk, unsigned tc) {
     uint32_t row[8];
     bool valid[8];
 #pragma unroll
     for (int u = 0; u < 8; ++u) {
-      row[u] = wq[u * 4 + g];
+      row[u] = q_wq[u * 4 + g];
       valid[u] = row[u] != 0xffffffffu;
-      if (!valid[u]) row[u] = wq[0];
+      if (!valid[u]) row[u] = q_wq[0];
     }
     int dot[8];
     float sc_row[8];
@@ -536,7 +595,7 @@ __device__ __forceinline__ void stb_scan_q4(const ScanArgs &args, const uint8_t 
       const uint32_t rh[4] = {row[4 * h], row[4 * h + 1], row[4 * h + 2], row[4 * h + 3]};
       int dh[4];
       float sh[4];
-      stb_q8_dots<4>(pw + 128 + 16 * j, pw + 128 + 16 * j + 8, q8, q8_scale, rh, j, dh, sh);
+      stb_q8_dots<4>(q_pw + 128 + 16 * j, q_pw + 128 + 16 * j + 8, q8, q8_scale, rh, j, dh, sh);
 #pragma unroll
       for (int u = 0; u < 4; ++u) { dot[4 * h + u] = dh[u]; sc_row[4 * h + u] = sh[u]; }
     }
@@ -547,20 +606,50 @@ __device__ __forceinline__ void stb_scan_q4(const ScanArgs &args, const uint8_t 
 #pragma unroll
     for (int u = 0; u < 8; ++u)
       if (j == u) { d = dot[u]; sc = sc_row[u]; r = row[u]; v = valid[u]; }
-    const float s = !v ? -CUDART_INF_F : (Q.unusable ? CUDART_INF_F : fmaf(sc, fmaf((float)d, Q.inv_S, Q.h_l1), Q.e_q));
+    const float s = !v ? -CUDART_INF_F : (S.unusable ? CUDART_INF_F : fmaf(sc, fmaf((float)d, S.inv_S, S.h_l1), S.e_q));
     refined += (unsigned)__popc(__ballot_sync(0xffffffffu, v));
-    sink.template consume<32>(s, r);
-    if (Q.unusable) return;
+    snk.template consume<32>(s, r);
+    if (S.unusable) return;
     // publish the lower bounds that beat the published value of their word (rare after the first tickets);
     // the warp learns its own contributions with the next read
-    const float l8 = fmaf(sc, fmaf((float)d, Q.inv_S, -Q.h_l1), -Q.e_q) - (float)STB_Q8_SCAN_EPS;
+    const float l8 = fmaf(sc, fmaf((float)d, S.inv_S, -S.h_l1), -S.e_q) - (float)STB_Q8_SCAN_EPS;
     if constexpr (DUMP) {
       if (v) dump->l8[r] = l8;
     }
     const unsigned o8 = stb_f2ord(l8);
     const int w = (int)(r % (uint32_t)kw);
-    const unsigned known = __shfl_sync(0xffffffffu, tcache, w);   // every lane takes part in the shuffle
-    if (v && o8 > known) atomicMax(q4a.thr + w, ((unsigned long long)q4a.tag << 32) | o8);
+    const unsigned known = __shfl_sync(0xffffffffu, tc, w);   // every lane takes part in the shuffle
+    if (v && o8 > known) atomicMax(thr + w, ((unsigned long long)tag << 32) | o8);
+  };
+
+  // one query's side of a tile: fold in its threshold words, test the row's bound, queue it, refine 32 queued rows
+  auto pass = [&](int lh, int ll, int hh, int hl, float2 sr, unsigned tw, const StbQ4Side &S, unsigned long long *thr,
+                  uint32_t tag, int kw, unsigned &tc, uint32_t *q_wq, const uint32_t *q_pw, int &q_n, auto &snk, bool valid, uint32_t row) {
+    if (lane < kw) tc = max(tc, tw);  // tw: the word's ordered l8 if it carries the query's tag, else 0
+    float T;
+    {
+      const unsigned tmin = __reduce_min_sync(0xffffffffu, lane < kw ? tc : 0xffffffffu);
+      T = tmin ? stb_ord2f(tmin) : -CUDART_INF_F;
+    }
+    const int D = (lh + (hh >> 4)) * 256 + (ll + (hl >> 4)) - 8 * S.sumq;   // q16 . h (hh, hl: multiples of 16)
+    const float u4 = fmaf(sr.x, fmaf((float)D, S.A, S.B), sr.y + S.e_q4);
+    if constexpr (DUMP) {
+      if (dump->pin) T = -CUDART_INF_F;
+      if (valid) { dump->u4[row] = u4; dump->t[row] = T; }
+    }
+    // an unusable query publishes no bound (refine), so T stays -inf and every valid row is queued
+    const bool want = valid && !(u4 + (float)STB_Q4_SKIP_EPS < T);
+    const unsigned mk = __ballot_sync(0xffffffffu, want);
+    q_wq[want ? q_n + __popc(mk & ((1u << lane) - 1u)) : STB_Q4_SPARE] = row;
+    q_n += __popc(mk);
+    if (q_n >= 32) {                 // q_n < 64: one batch at most
+      __syncwarp();
+      refine(q_wq, q_pw, S, thr, tag, kw, snk, tc);
+      const uint32_t rest = (32 + lane < q_n) ? q_wq[32 + lane] : 0u;
+      __syncwarp();
+      q_wq[(32 + lane < q_n) ? lane : STB_Q4_SPARE] = rest;
+      q_n -= 32;
+    }
   };
 
   constexpr uint64_t tile_rows = 4 * U;
@@ -568,10 +657,16 @@ __device__ __forceinline__ void stb_scan_q4(const ScanArgs &args, const uint8_t 
   const uint32_t n_rows = (uint32_t)args.n_virtual;
   StbRowMap<RANGES> rmap;
   rmap.restart();
-  stb_for_each_tile<RANGES, 2>(args, n_tiles, off, [&](uint64_t tile, bool first) {
+  // M & 1: score the tile for the launch's own query, M & 2: for the guest.  M == 3 is the pair's tile body: one
+  // set of plane loads feeds two sets of dp4a accumulators.
+  auto tile_body = [&](uint64_t tile, bool first, auto mode) {
+    constexpr int M = decltype(mode)::value;
     if (first) rmap.restart();
+    const StbQ4Side &S2 = *side2;      // read where used: shared memory, not registers
     // lane w < k: threshold word w as the other warps left it; issued with the tile's loads, folded in below
-    const unsigned long long tw = lane < kw ? __ldcg(q4a.thr + lane) : 0ull;
+    unsigned long long tw = 0ull, tw2 = 0ull;
+    if constexpr ((M & 1) != 0) tw = lane < (int)q4a.top_k ? __ldcg(q4a.thr + lane) : 0ull;
+    if constexpr ((M & 2) != 0) tw2 = lane < S2.kw ? __ldcg(S2.thr + lane) : 0ull;
     // lane l owns virtual row 32 tile + l (< 2^32: a shard holds at most 2^32 - 2 rows); past the end it
     // reads the last row and is not queued
     const uint32_t v = (uint32_t)tile * (uint32_t)tile_rows + (uint32_t)lane;
@@ -585,52 +680,140 @@ __device__ __forceinline__ void stb_scan_q4(const ScanArgs &args, const uint8_t 
       a[m] = make_uint4(__float_as_uint(t.x), __float_as_uint(t.y), __float_as_uint(t.z), __float_as_uint(t.w));
     }
     const float2 sr = __ldg(q4a.sr + row);
+    // the threshold words as one register each: 0 unless the word carries the query's tag
+    const unsigned tv = (uint32_t)(tw >> 32) == q4a.tag ? (unsigned)tw : 0u;
+    unsigned tv2 = 0u;
+    if constexpr ((M & 2) != 0) tv2 = (uint32_t)(tw2 >> 32) == S2.tag ? (unsigned)tw2 : 0u;
     // low nibbles x {hi, lo} query bytes, 16 x high nibbles x {hi, lo}: exact in int32
-    int lh = 0, ll = 0, hh = 0, hl = 0;
+    int lh = 0, ll = 0, hh = 0, hl = 0, lh2 = 0, ll2 = 0, hh2 = 0, hl2 = 0;
 #pragma unroll
     for (int m = 0; m < 8; ++m) {
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        const uint4 qw = *reinterpret_cast<const uint4 *>(pw + (4 * m + k) * 4);
         const uint32_t w = k == 0 ? a[m].x : (k == 1 ? a[m].y : (k == 2 ? a[m].z : a[m].w));
         const uint32_t lo = w & 0x0F0F0F0Fu, hi = w & 0xF0F0F0F0u;
-        lh = __dp4a((int)lo, (int)qw.x, lh);
-        ll = __dp4a((int)lo, (int)qw.y, ll);
-        hh = stb_dp4a_us(hi, qw.z, hh);
-        hl = stb_dp4a_us(hi, qw.w, hl);
+        if constexpr ((M & 1) != 0) {
+          const uint4 qw = *reinterpret_cast<const uint4 *>(pw + (4 * m + k) * 4);
+          lh = __dp4a((int)lo, (int)qw.x, lh);
+          ll = __dp4a((int)lo, (int)qw.y, ll);
+          hh = stb_dp4a_us(hi, qw.z, hh);
+          hl = stb_dp4a_us(hi, qw.w, hl);
+        }
+        if constexpr ((M & 2) != 0) {
+          const uint4 qw = *reinterpret_cast<const uint4 *>(pw2 + (4 * m + k) * 4);
+          lh2 = __dp4a((int)lo, (int)qw.x, lh2);
+          ll2 = __dp4a((int)lo, (int)qw.y, ll2);
+          hh2 = stb_dp4a_us(hi, qw.z, hh2);
+          hl2 = stb_dp4a_us(hi, qw.w, hl2);
+        }
       }
     }
-    if (lane < kw && (uint32_t)(tw >> 32) == q4a.tag) tcache = max(tcache, (unsigned)tw);
-    {
-      const unsigned tmin = __reduce_min_sync(0xffffffffu, lane < kw ? tcache : 0xffffffffu);
-      T = tmin ? stb_ord2f(tmin) : -CUDART_INF_F;
+    if constexpr ((M & 1) != 0) pass(lh, ll, hh, hl, sr, tv, S1, q4a.thr, q4a.tag, (int)q4a.top_k, tcache, wq, pw, qn, sink, valid, row);
+    if constexpr ((M & 2) != 0) pass(lh2, ll2, hh2, hl2, sr, tv2, S2, S2.thr, S2.tag, S2.kw, tcache2, wq2, pw2, qn2, *sink2, valid, row);
+  };
+
+  bool joined = false;               // warp-uniform; the same in every warp once the scan is over
+  bool paired = false;
+  if constexpr (PAIR) paired = seat != nullptr;
+  if (!paired) {
+    stb_for_each_tile<RANGES, 2>(args, n_tiles, off, [&](uint64_t tile, bool first) {
+      tile_body(tile, first, std::integral_constant<int, 1>());
+    });
+  } else if constexpr (PAIR) {
+    // the host of a pair: stb_for_each_tile's ticket loop, with the join read off every draw
+    auto draw = [&]() -> uint32_t {     // relative to the launch's start: < 2^32 with the jump
+      uint32_t t = 0;
+      if (lane == 0) t = (uint32_t)(atomicAdd(args.tickets, 1ull) - args.t_base);
+      return __shfl_sync(0xffffffffu, t, 0);
+    };
+    auto first_tile = [&](uint64_t t) -> uint64_t {
+      return t < args.t_bulk ? t * STB_TICKET_TILES : args.t_bulk * STB_TICKET_TILES + (t - args.t_bulk);
+    };
+    auto run_ticket = [&](uint64_t t, auto mode) {
+      const uint64_t t0 = first_tile(t);
+      const uint64_t t1 = t < args.t_bulk ? t0 + STB_TICKET_TILES : t0 + 1;
+      uint32_t tile = (uint32_t)t0 + *reinterpret_cast<const volatile uint32_t *>(off);   // off < n_tiles < 2^32
+      if (tile >= n_tiles) tile -= (uint32_t)n_tiles;
+      for (uint32_t left = (uint32_t)(t1 - t0); left; --left) {
+        tile_body(tile, false, mode);
+        if (++tile == n_tiles) tile = 0;
+      }
+    };
+    // host tickets until a draw carries the jump (or fails), then the pair's tickets
+    uint32_t cur = draw();
+    while (cur < STB_PAIR_JUMP && first_tile(cur) < n_tiles) {
+      const uint32_t nxt = draw();        // drawn before the ticket is scored (stb_for_each_tile)
+      run_ticket(cur, std::integral_constant<int, 1>());
+      cur = nxt;
     }
-    const int D = (lh + (hh >> 4)) * 256 + (ll + (hl >> 4)) - 8 * sumq;   // q16 . h (hh, hl: multiples of 16)
-    const float u4 = fmaf(sr.x, fmaf((float)D, A, B), sr.y + e_q4);
-    if constexpr (DUMP) {
-      if (dump->pin) T = -CUDART_INF_F;
-      if (valid) { dump->u4[row] = u4; dump->t[row] = T; }
-    }
-    // an unusable query publishes no bound (refine), so T stays -inf and every valid row is queued
-    const bool want = valid && !(u4 + (float)STB_Q4_SKIP_EPS < T);
-    const unsigned mk = __ballot_sync(0xffffffffu, want);
-    wq[want ? qn + __popc(mk & ((1u << lane) - 1u)) : STB_Q4_SPARE] = row;
-    qn += __popc(mk);
-    if (qn >= 32) {                  // qn < 64: one batch at most
+    joined = cur >= STB_PAIR_JUMP;
+    if (joined) {
+      // the first draw after the join: the seat holds what the join kernel wrote before its jump
+      __threadfence();
+      StbQ4Side S = stb_q4_query(reinterpret_cast<const float *>(__ldcg(seat + STB_SEAT_Q)), pw2, lane);
+      const unsigned long long info = __ldcg(seat + STB_SEAT_INFO);
+      S.thr = reinterpret_cast<unsigned long long *>(__ldcg(seat + STB_SEAT_THR));
+      S.tag = (uint32_t)(info >> 32);
+      S.kw = (int)(uint32_t)info;
+      if (lane == 0) *side2 = S;
       __syncwarp();
-      refine();
-      const uint32_t rest = (32 + lane < qn) ? wq[32 + lane] : 0u;
-      __syncwarp();
-      wq[(32 + lane < qn) ? lane : STB_Q4_SPARE] = rest;
-      qn -= 32;
+      cur -= (uint32_t)STB_PAIR_JUMP;
+      while (first_tile(cur) < n_tiles) {
+        const uint32_t nxt = draw() - (uint32_t)STB_PAIR_JUMP;
+        run_ticket(cur, std::integral_constant<int, 3>());
+        cur = nxt;
+      }
     }
-  });
+    if (joined) {
+      // the join kernel writes its decision right after its jump, and it is running: wait for the word.  A
+      // warp whose only draw after the jump failed cannot tell a late refusal from a join without it.
+      uint32_t d = 0;                    // 0x80000000 | v: joined at ticket v
+      if (lane == 0) {
+        const uint32_t gtag = side2->tag;
+        unsigned long long w;
+        do w = stb_ld_acquire_gpu(seat + STB_SEAT_DECIDED); while ((uint32_t)(w >> 32) != gtag);
+        d = (uint32_t)w;
+      }
+      d = __shfl_sync(0xffffffffu, d, 0);
+      joined = (d & 0x80000000u) != 0;
+      if (lane == 0) gscr[STB_PAIR_SCRATCH - 1] = d & 0x7fffffffu;   // v: in shared memory, the wrap's tile body needs the registers
+      __syncwarp();
+    }
+    if (joined) {
+      // the guest-only wrap: tickets [0, v), drawn from the seat's wrap word (tagged with this launch's q4 tag)
+      unsigned long long *wrap = seat + STB_SEAT_WRAP;
+      const volatile uint32_t *v = gscr + STB_PAIR_SCRATCH - 1;
+      for (;;) {
+        unsigned long long w = 0;
+        if (lane == 0) {
+          unsigned long long c = __ldcg(wrap);
+          while ((uint32_t)(c >> 32) != q4a.tag) {
+            const unsigned long long prev = atomicCAS(wrap, c, (unsigned long long)q4a.tag << 32);
+            c = prev == c ? (unsigned long long)q4a.tag << 32 : prev;
+          }
+          w = atomicAdd(wrap, 1ull) & 0xffffffffull;
+        }
+        w = __shfl_sync(0xffffffffu, w, 0);
+        if (w >= *v) break;
+        run_ticket(w, std::integral_constant<int, 2>());
+      }
+    }
+  }
   if (qn > 0) {                      // the rest, with the empty slots marked
     wq[lane >= qn ? lane : STB_Q4_SPARE] = 0xffffffffu;
     __syncwarp();
-    refine();
+    refine(wq, pw, S1, q4a.thr, q4a.tag, (int)q4a.top_k, sink, tcache);
+  }
+  if constexpr (PAIR) {
+    if (joined && qn2 > 0) {
+      const StbQ4Side &S2 = *side2;
+      wq2[lane >= qn2 ? lane : STB_Q4_SPARE] = 0xffffffffu;
+      __syncwarp();
+      refine(wq2, pw2, S2, S2.thr, S2.tag, S2.kw, *sink2, tcache2);
+    }
   }
   if (lane == 0 && refined) atomicAdd(q4a.refined, (unsigned long long)refined);
+  return joined;
 }
 
 // q8 builder: one warp per row (row_encode.cuh: stb_q8_encode_row).  The same pass writes the nibble
@@ -774,7 +957,8 @@ struct StbCoscanArgs {
   uint64_t pred_t_bulk;                   // ... and its bulk ticket count (same tile count as this launch)
 };
 
-__device__ __forceinline__ uint32_t stb_coscan_offset(const StbCoscanArgs &c, uint64_t n_tiles) {
+// join_front >= 0: a joined guest, whose pass starts at its join tile of the host's pass (the predecessor's).
+__device__ __forceinline__ uint32_t stb_coscan_offset(const StbCoscanArgs &c, uint64_t n_tiles, int64_t join_front = -1) {
   unsigned long long cur = __ldcg(c.word);
   while ((uint32_t)(cur >> 32) != c.tag) {
     uint64_t off = 0;
@@ -784,7 +968,8 @@ __device__ __forceinline__ uint32_t stb_coscan_offset(const StbCoscanArgs &c, ui
       // the predecessor's frontier: the first tile of its next undrawn ticket (stb_for_each_tile)
       const unsigned long long drawn = __ldcg(c.pred_tickets) - c.pred_t_base;
       uint64_t front = n_tiles;
-      if (drawn < n_tiles)
+      if (join_front >= 0) front = (uint64_t)join_front;
+      else if (drawn < n_tiles)
         front = drawn < c.pred_t_bulk ? drawn * STB_TICKET_TILES : c.pred_t_bulk * STB_TICKET_TILES + (drawn - c.pred_t_bulk);
       off = (p_off + (front < n_tiles ? front : 0)) % n_tiles;
     }
@@ -795,9 +980,21 @@ __device__ __forceinline__ uint32_t stb_coscan_offset(const StbCoscanArgs &c, ui
   return (uint32_t)cur % n_tiles;
 }
 
+// A pair (SRC == 2, RANGES == 0; see "pairs" above).  Host: its seat and the guest tail's tree-merge scratch.
+// Guest: the seat's decided word and the tag it waits for, and its own ticket counter's booked advance.
+struct StbPairArgs {
+  unsigned long long *seat;            // host; null: no guest can join
+  uint64_t *keys2;
+  unsigned int *counters2;
+  const unsigned long long *decided;   // guest; null: not a guest
+  uint32_t tag;
+  unsigned long long booked;
+};
+
 struct TopkArgs {
   ScanArgs scan;
   StbCoscanArgs co;
+  StbPairArgs pair;
   uint64_t row_base;
   uint64_t *keys;            // sorted best-KP lists of every tree level
   unsigned int *counters;    // one arrival ticket per tree group, all levels
@@ -849,6 +1046,57 @@ __device__ __forceinline__ int stb_pad_and_sort(uint64_t *skeys, int c, int min_
 
 #define STB_RR_STRIDE 260   // floats per staged row (1 KiB + 16 B pad: conflict-free LDS.128)
 
+// The join kernel of a guest (see "pairs" above): one warp beside the host's CTAs.  It decides, writes the seat's
+// decided word, releases the guest's scan kernel and completes only after the host has.
+struct StbPairJoinArgs {
+  unsigned long long *seat;        // the host's seat
+  unsigned long long *tickets;     // the host's ticket counter ...
+  unsigned long long t_base;       // ... its value at the host's start and the host's ticket count
+  uint64_t n_tickets;
+  uint64_t v_floor;                // test hook (stb_debug_pair_floor): join no earlier than ticket v_floor
+  const float *q;                  // the guest: query, outputs, k, threshold words and tags
+  stb_hit *hits;
+  uint32_t *status;
+  uint32_t top_k;
+  unsigned long long *thr;
+  uint32_t q4_tag, tag;
+};
+
+// A warp's registers come from one of the SM's four 16K-register sub-partitions.  Two q8 scan CTAs put four
+// warps of 120 registers on each (15,360), so the join's one warp must make do with the 1,024 left: 32 each.
+#define STB_PAIR_JOIN_REGS 32
+__global__ void __maxnreg__(STB_PAIR_JOIN_REGS) stb_pair_join_kernel(const StbPairJoinArgs a) {
+  const StbQ8Query Q = stb_q8_query(a.q, threadIdx.x & 7);
+  bool jumped = false;
+  if (threadIdx.x == 0) {
+    unsigned long long decided = (unsigned long long)a.tag << 32;   // refused
+    if (!Q.unusable) {
+      unsigned long long *s = a.seat;
+      s[STB_SEAT_Q] = reinterpret_cast<unsigned long long>(a.q);
+      s[STB_SEAT_HITS] = reinterpret_cast<unsigned long long>(a.hits);
+      s[STB_SEAT_STATUS] = reinterpret_cast<unsigned long long>(a.status);
+      s[STB_SEAT_THR] = reinterpret_cast<unsigned long long>(a.thr);
+      s[STB_SEAT_INFO] = ((unsigned long long)a.q4_tag << 32) | a.top_k;
+      if (a.v_floor) {                               // the host is running: it draws on or runs out
+        unsigned long long t;
+        do t = stb_ld_acquire_gpu(a.tickets) - a.t_base; while (t < a.v_floor && t < a.n_tickets);
+      }
+      __threadfence();                               // the seat before the jump
+      // an atomic add, not a CAS: the host's warps draw hundreds of tickets per microsecond
+      const unsigned long long t = atomicAdd(a.tickets, STB_PAIR_JUMP) - a.t_base;
+      jumped = true;
+      if (t < a.n_tickets) decided |= 0x80000000ull | t;   // joined at ticket t
+    }
+    a.seat[STB_SEAT_DECIDED] = decided;
+    __threadfence();
+  }
+  __syncwarp();
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  // complete after the host: the guest's scan kernel waits on this grid, the next launch on the guest's
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  if (threadIdx.x == 0 && !jumped) atomicAdd(a.tickets, STB_PAIR_JUMP);   // the jump the host booked, after its last draw
+}
+
 // E: 32*E candidates per warp / CTA / inner tree list.  EF: the ROOT of the merge tree (the CTA
 // itself when the grid is one CTA) keeps 32*EF >= 32*E candidates for the exact re-rank.
 // EF > E lets a tier with a wide error term (q8) re-rank 128 rows while every level below the
@@ -857,14 +1105,14 @@ __device__ __forceinline__ int stb_pad_and_sort(uint64_t *skeys, int c, int min_
 // key), the bounds are max-reduced up the tree, and the proof compares the k-th exact distance
 // with that bound instead of "the K'-th key of one uniform list".
 template <int E, int U, int RANGES, int SRC = 0, int EF = E>
-__global__ void __launch_bounds__(STB_SCAN_THREADS, STB_SCAN_MINB)
-stb_scan_topk_kernel(const TopkArgs args) {
+__device__ __forceinline__ void stb_scan_topk_body(const TopkArgs &args) {
   // SRC 0: scores from the f32 rows; SRC 1: from the 16-bit shadow (wider proof margin);
   // SRC 2: upper bounds of the exact cosine from the int8 copy (margin folded into the score)
   constexpr double kScoreEps = SRC == 1 ? STB_SHADOW_SCAN_EPS : (SRC == 2 ? STB_Q8_SCAN_EPS : STB_SCORE_EPS);
   constexpr int KP = 32 * E;          // list length below the root
   constexpr int KF = 32 * EF;         // candidates the root keeps
   constexpr int KPS = KP + 1;         // published list stride: KP keys + the node's drop bound
+  constexpr bool kPair = SRC == 2 && RANGES == 0;   // q8 whole-shard scans host and guest pairs
   static_assert(EF >= E && 8 * KP <= STB_SORT_CAP && KF <= STB_SORT_CAP / 2, "list sizes");
   __shared__ uint64_t skeys[STB_SORT_CAP];
   __shared__ unsigned int s_T, s_cnt, s_ticket, s_bound, s_nin;
@@ -874,27 +1122,60 @@ stb_scan_topk_kernel(const TopkArgs args) {
   __shared__ double s_d[KF], s_r2[KF], s_q2;
   __shared__ uint64_t s_r[KF];
   __shared__ int s_nv[2];
+  __shared__ double s_cthr;
+  __shared__ int s_done;
+  __shared__ unsigned int s_timeout;
 
   // co-scan: the tile this launch's pass starts at, fixed before the dependent is released so that
   // the dependent's first CTA can read it
   __shared__ uint32_t s_off;          // (stb_for_each_tile reads it with RANGES == 0 only)
   if constexpr (RANGES == 0) {
-    if (threadIdx.x == 0) s_off = args.co.word ? stb_coscan_offset(args.co, (args.scan.n_virtual + 4 * U - 1) / (4 * U)) : 0u;
+    __shared__ int s_guest_joined;
+    const uint64_t n_tiles = (args.scan.n_virtual + 4 * U - 1) / (4 * U);
+    if (threadIdx.x == 0) {
+      int64_t front = -1;
+      s_guest_joined = 0;
+      if (kPair && args.pair.decided) {
+        // a guest: the join kernel wrote the decided word before it released this grid
+        unsigned long long w;
+        do w = stb_ld_acquire_gpu(args.pair.decided); while ((uint32_t)(w >> 32) != args.pair.tag);
+        if (w & 0x80000000ull) {
+          s_guest_joined = 1;
+          const uint64_t v = (uint32_t)w & 0x7fffffffu, tb = args.scan.t_bulk;   // the host's tickets: same grid
+          front = (int64_t)(v < tb ? v * STB_TICKET_TILES : tb * STB_TICKET_TILES + (v - tb));
+        }
+      }
+      s_off = args.co.word ? stb_coscan_offset(args.co, n_tiles, front) : 0u;
+    }
     __syncthreads();
+    if (s_guest_joined) {
+      // the host scores this query: release the next launch; one CTA completes after the host (through the
+      // join kernel) and books this launch's tickets
+      asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+      if (blockIdx.x == 0) {
+        asm volatile("griddepcontrol.wait;" ::: "memory");
+        if (threadIdx.x == 0) atomicAdd(args.scan.tickets, args.pair.booked);
+      }
+      return;
+    }
   }
-  // Overlapped launches (asynchronous entry points): the grid is sized for one CTA per SM and lets the
-  // NEXT query's grid in right away, so two scans share the SMs and the ~10 us in which a draining
-  // grid leaves HBM idle (CTA merge before exit, launch, ramp-up) are covered by the other scan.
+  // Overlapped launches (asynchronous entry points): the grid lets the NEXT query's grid in right away, so
+  // the ~10 us in which a draining grid leaves HBM idle (CTA merge before exit, launch, ramp-up) are covered
+  // by the other scan, and a pair's join kernel runs while its host starts.
   // Tails stay ordered: everything after the scan sits behind griddepcontrol.wait.
   if (args.early_trigger) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  TopSink<E> sink;
+  TopSink<E> sink, sink2;
   sink.init();
+  bool joined = false;
   if constexpr (SRC == 2) {
     // the refine queues live in the re-rank staging area, which is first used after the CTA merge
-    // (per warp: STB_Q4_QUEUE queued rows + 256 query words)
-    static_assert(STB_SCAN_WARPS * (STB_Q4_QUEUE + 256) <= 32 * STB_RR_STRIDE, "q4 scratch");
+    // (per warp: STB_Q4_QUEUE queued rows + 256 query words; a host's guest: STB_PAIR_SCRATCH more)
+    static_assert(STB_SCAN_WARPS * (STB_Q4_QUEUE + 256 + STB_PAIR_SCRATCH) <= 32 * STB_RR_STRIDE, "q4 scratch");
     uint32_t *scratch = reinterpret_cast<uint32_t *>(srows) + (threadIdx.x >> 5) * (STB_Q4_QUEUE + 256);
-    stb_scan_q4<U, RANGES>(args.scan, args.q8, args.q8_scale, args.q4, scratch, scratch + STB_Q4_QUEUE, sink, &s_off);
+    uint32_t *gscr = reinterpret_cast<uint32_t *>(srows) + STB_SCAN_WARPS * (STB_Q4_QUEUE + 256) + (threadIdx.x >> 5) * STB_PAIR_SCRATCH;
+    sink2.init();
+    joined = stb_scan_q4<U, RANGES, 0, kPair>(args.scan, args.q8, args.q8_scale, args.q4, scratch, scratch + STB_Q4_QUEUE, sink, &s_off,
+                                              nullptr, args.pair.seat, gscr, &sink2);
   } else if constexpr (SRC == 1) stb_scan_shadow<U, RANGES>(args.scan, args.shadow, sink, &s_off);
   else stb_scan_rows<U, RANGES>(args.scan, sink, &s_off);
   // Programmatic dependent launch: the scan above reads only the corpus and the query,
@@ -902,280 +1183,316 @@ stb_scan_topk_kernel(const TopkArgs args) {
   // left its scan loop; this kernel's merge / re-rank tail then overlaps with it.
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
-  // ---- CTA merge ------------------------------------------------------------------
-  // T = max over warps of the warp list minimum is a lower bound of the CTA's KP-th
-  // best score (that warp alone holds KP keys >= its minimum), so only keys >= T can
-  // matter: compact those (typically ~KP..2KP of the 8*KP) and sort the small set.
-  // Drop bounds are ordered scores (stb_f2ord); 0 = "nothing dropped so far".
-  const int lane = threadIdx.x & 31;
-  const unsigned kOrdNegInf = 0x007fffffu;       // stb_f2ord(-inf): a list that never filled
-  if (threadIdx.x == 0) { s_T = 0u; s_cnt = 0u; }
-  __syncthreads();
-  if (lane == 0) atomicMax(&s_T, stb_f2ord(sink.thr));
-  __syncthreads();
-  {
-    const unsigned T = s_T;
-#pragma unroll
-    for (int e = 0; e < E; ++e) {
-      const bool take = sink.lr[e] != 0xffffffffu && stb_f2ord(sink.ls[e]) >= T;
-      const unsigned m = __ballot_sync(0xffffffffu, take);
-      unsigned base = 0u;
-      if (lane == 0 && m) base = atomicAdd(&s_cnt, (unsigned)__popc(m));   // <= 8*KP <= STB_SORT_CAP
-      base = __shfl_sync(0xffffffffu, base, 0);
-      if (take) skeys[base + __popc(m & ((1u << lane) - 1u))] = stb_make_key(sink.ls[e], sink.lr[e]);
-    }
-  }
-  __syncthreads();
-  unsigned bound;                                // uniform per CTA from here on
-  {
-    const int c = (int)s_cnt;
-    stb_pad_and_sort(skeys, c, KP);
-    const int keep = (gridDim.x == 1) ? KF : KP;
-    // warps dropped keys below their own minimum (<= T); the compaction dropped keys < T
-    bound = (s_T > kOrdNegInf) ? s_T : 0u;
-    if (c > keep) bound = max(bound, stb_f2ord(stb_key_score(skeys[keep - 1])));
-  }
+  // The tail of one query: CTA merge, tree merge over tkeys / tcnt, exact re-rank, proof and output.  A pair's
+  // host runs it for its own query, then for the guest's.
+  auto tail = [&](TopSink<E> &snk, const float *tq, uint32_t tk, stb_hit *th, uint32_t *ts, uint64_t *tkeys, unsigned int *tcnt,
+                  bool xchg) {
+    __syncthreads();
 
-  // Everything below writes scratch shared with the PREVIOUS launch on this stream
-  // (keys, tickets, exchange slots): wait until that grid has completed and flushed.
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-
-  // ---- tree merge across CTAs ------------------------------------------------------------
-  // Lists of KP sorted keys (+ their drop bound) are merged F = 1024/KP at a time by the last
-  // CTA to arrive in each group (atomic ticket + fences), level by level: 296 -> 10 -> 1 lists
-  // at E = 1.  Each merge is one register/shuffle bitonic sort of <= 1024 keys; the groups of a
-  // level run in parallel on different SMs.  Level l's lists live at key offset
-  // lvl_key_off*KPS, its tickets at counters[lvl_cnt_off + group].
-  {
-    constexpr int F = STB_SORT_CAP / KP;
-    uint32_t lists = gridDim.x, my_id = blockIdx.x, lvl_key_off = 0, lvl_cnt_off = 0;
-    while (lists > 1) {
-      uint64_t *lvl = args.keys + (size_t)lvl_key_off * KPS;
-      for (int i = threadIdx.x; i < KP; i += blockDim.x) lvl[(size_t)my_id * KPS + i] = skeys[i];
-      if (threadIdx.x == 0) lvl[(size_t)my_id * KPS + KP] = (uint64_t)bound;
-      __threadfence();
-      __syncthreads();
-      const uint32_t group = my_id / F, first = group * F;
-      const uint32_t n_in = min((uint32_t)F, lists - first);
-      if (threadIdx.x == 0) s_ticket = atomicAdd(args.counters + lvl_cnt_off + group, 1u);
-      __syncthreads();
-      if (s_ticket != n_in - 1) return;            // not the last of my group: done
-      __threadfence();
-      if (threadIdx.x == 0) args.counters[lvl_cnt_off + group] = 0u;   // re-arm for the next launch
-      const uint32_t groups = (lists + F - 1) / F;
-      const int keep = (groups == 1) ? KF : KP;     // the root keeps the re-rank set
-      {
-        // Pre-filter before sorting: every list is sorted best-first, so with
-        // r = ceil(keep / n_in) - 1 the worst of the lists' r-th keys is a lower bound of the
-        // group's keep-th best (n_in * (r+1) >= keep keys are at least that good).  Only keys at
-        // or above it can survive the merge -- typically ~100 of the 1024 -- and the sort
-        // shrinks from the 1024-key to the 256-key network.  r >= KP (fewer than `keep` keys
-        // in total): nothing can be filtered.
-        constexpr int PER = STB_SORT_CAP / STB_SCAN_THREADS;
-        uint64_t v[PER];
-        const uint32_t r = (keep + n_in - 1) / n_in - 1;
-        if (threadIdx.x == 0) { s_T64 = (r >= (uint32_t)KP) ? STB_KEY_INVALID : 0ull; s_cnt = 0u; s_bound = 0u; s_nin = 0u; }
-        __syncthreads();
-        unsigned my_valid = 0;
-#pragma unroll
-        for (int u = 0; u < PER; ++u) {
-          const int i = threadIdx.x + u * STB_SCAN_THREADS;
-          const uint32_t li = i / KP;
-          v[u] = (li < n_in) ? __ldcg(lvl + (size_t)(first + li) * KPS + (i % KP)) : STB_KEY_INVALID;
-          my_valid += (v[u] != STB_KEY_INVALID) ? 1u : 0u;
-          if (li < n_in && (uint32_t)(i % KP) == r) atomicMax(&s_T64, v[u]);   // INVALID (all ones) disables the filter
-        }
-        if (threadIdx.x < n_in) atomicMax(&s_bound, (unsigned)__ldcg(lvl + (size_t)(first + threadIdx.x) * KPS + KP));
-        my_valid = __reduce_add_sync(0xffffffffu, my_valid);
-        if (lane == 0 && my_valid) atomicAdd(&s_nin, my_valid);
-        __syncthreads();
-        const uint64_t T = s_T64;
-#pragma unroll
-        for (int u = 0; u < PER; ++u) {
-          const bool take = v[u] != STB_KEY_INVALID && v[u] <= T;
-          const unsigned m = __ballot_sync(0xffffffffu, take);
-          unsigned base = 0u;
-          if (lane == 0 && m) base = atomicAdd(&s_cnt, (unsigned)__popc(m));
-          base = __shfl_sync(0xffffffffu, base, 0);
-          if (take) skeys[base + __popc(m & ((1u << lane) - 1u))] = v[u];
-        }
-      }
-      __syncthreads();
-      stb_pad_and_sort(skeys, (int)s_cnt, KP);
-      bound = s_bound;
-      if ((int)s_nin > keep) bound = max(bound, stb_f2ord(stb_key_score(skeys[keep - 1])));
-      lvl_key_off += lists;
-      lvl_cnt_off += groups;
-      lists = groups;
-      my_id = group;
-    }
-  }
-
-  // ---- exact re-rank of the best KF in canonical arithmetic --------------------------
-  // Rows are staged through shared memory (coalesced, one DRAM latency), then one
-  // thread per candidate accumulates (ab, r2) with stb_canon_dot and scores it with stb_canon_dist.
-  for (int i = threadIdx.x; i < STB_D; i += blockDim.x) sqd[i] = (double)__ldg(args.scan.q + i);
-  if (threadIdx.x < 2) s_nv[threadIdx.x] = 0;
-  if (threadIdx.x < KF) { s_d[threadIdx.x] = CUDART_INF; s_r[threadIdx.x] = 0xffffffffffffffffull; }
-  __syncthreads();
-  if (threadIdx.x == 5 * 32) s_q2 = stb_canon_q2(sqd);   // an otherwise idle warp: ||q||^2 once
-  // Candidates are sorted by approximate score (or upper bound) best-first and re-scored 32 at a
-  // time.  After the first 32 the k-th best EXACT cosine c_k among them is known; a later
-  // candidate whose score + eps is below c_k cannot enter the top-k, and neither can anything
-  // after it -- with K' = 128 (q8) this usually ends the re-rank after one pass instead of four.
-  __shared__ double s_cthr;
-  __shared__ int s_done;
-  if (threadIdx.x == 0) { s_cthr = -CUDART_INF; s_done = 0; }
-  for (int chunk = 0; chunk < EF; ++chunk) {
-    if (chunk > 0) {
-      const uint64_t nk = skeys[chunk * 32];                            // uniform
-      if (nk == STB_KEY_INVALID || (double)stb_key_score(nk) + kScoreEps < s_cthr) break;
-    }
+    // ---- CTA merge ------------------------------------------------------------------
+    // T = max over warps of the warp list minimum is a lower bound of the CTA's KP-th
+    // best score (that warp alone holds KP keys >= its minimum), so only keys >= T can
+    // matter: compact those (typically ~KP..2KP of the 8*KP) and sort the small set.
+    // Drop bounds are ordered scores (stb_f2ord); 0 = "nothing dropped so far".
+    const int lane = threadIdx.x & 31;
+    const unsigned kOrdNegInf = 0x007fffffu;       // stb_f2ord(-inf): a list that never filled
+    if (threadIdx.x == 0) { s_T = 0u; s_cnt = 0u; }
+    __syncthreads();
+    if (lane == 0) atomicMax(&s_T, stb_f2ord(snk.thr));
+    __syncthreads();
     {
-      constexpr int PER = 32 * STB_ROW_F4 / STB_SCAN_THREADS;   // float4 per thread
-      float4 v[PER];
+      const unsigned T = s_T;
 #pragma unroll
-      for (int u = 0; u < PER; ++u) {
-        const int t = threadIdx.x + u * STB_SCAN_THREADS;
-        const uint64_t key = skeys[chunk * 32 + (t >> 6)];
-        v[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (key != STB_KEY_INVALID)
-          v[u] = __ldg(args.scan.rows + (size_t)stb_key_row(key) * STB_ROW_F4 + (t & 63));
-      }
-#pragma unroll
-      for (int u = 0; u < PER; ++u) {
-        const int t = threadIdx.x + u * STB_SCAN_THREADS;
-        *reinterpret_cast<float4 *>(srows + (t >> 6) * STB_RR_STRIDE + (t & 63) * 4) = v[u];
+      for (int e = 0; e < E; ++e) {
+        const bool take = snk.lr[e] != 0xffffffffu && stb_f2ord(snk.ls[e]) >= T;
+        const unsigned m = __ballot_sync(0xffffffffu, take);
+        unsigned base = 0u;
+        if (lane == 0 && m) base = atomicAdd(&s_cnt, (unsigned)__popc(m));   // <= 8*KP <= STB_SORT_CAP
+        base = __shfl_sync(0xffffffffu, base, 0);
+        if (take) skeys[base + __popc(m & ((1u << lane) - 1u))] = stb_make_key(snk.ls[e], snk.lr[e]);
       }
     }
     __syncthreads();
-    // 8 candidates per warp on 4 warps (one per SM sub-partition): the f64 chains are
-    // latency-bound, so spreading them quarters the issue time
-    if (threadIdx.x < 128 && lane < 8) {
-      const int cl = (threadIdx.x >> 5) * 8 + lane;          // candidate inside the chunk
-      const int ci = chunk * 32 + cl;
-      if (skeys[ci] != STB_KEY_INVALID) {
-        double ab, r2;
-        stb_canon_dot<false>(sqd, reinterpret_cast<const float4 *>(srows + cl * STB_RR_STRIDE), ab, r2);
-        s_d[ci] = ab;          // finalised below once ||q||^2 is known
-        s_r2[ci] = r2;
+    unsigned bound;                                // uniform per CTA from here on
+    {
+      const int c = (int)s_cnt;
+      stb_pad_and_sort(skeys, c, KP);
+      const int keep = (gridDim.x == 1) ? KF : KP;
+      // warps dropped keys below their own minimum (<= T); the compaction dropped keys < T
+      bound = (s_T > kOrdNegInf) ? s_T : 0u;
+      if (c > keep) bound = max(bound, stb_f2ord(stb_key_score(skeys[keep - 1])));
+    }
+
+    // Everything below writes scratch shared with the PREVIOUS launch on this stream
+    // (keys, tickets, exchange slots): wait until that grid has completed and flushed.
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+
+    // ---- tree merge across CTAs ------------------------------------------------------------
+    // Lists of KP sorted keys (+ their drop bound) are merged F = 1024/KP at a time by the last
+    // CTA to arrive in each group (atomic ticket + fences), level by level: 296 -> 10 -> 1 lists
+    // at E = 1.  Each merge is one register/shuffle bitonic sort of <= 1024 keys; the groups of a
+    // level run in parallel on different SMs.  Level l's lists live at key offset
+    // lvl_key_off*KPS, its tickets at counters[lvl_cnt_off + group].
+    {
+      constexpr int F = STB_SORT_CAP / KP;
+      uint32_t lists = gridDim.x, my_id = blockIdx.x, lvl_key_off = 0, lvl_cnt_off = 0;
+      while (lists > 1) {
+        uint64_t *lvl = tkeys + (size_t)lvl_key_off * KPS;
+        for (int i = threadIdx.x; i < KP; i += blockDim.x) lvl[(size_t)my_id * KPS + i] = skeys[i];
+        if (threadIdx.x == 0) lvl[(size_t)my_id * KPS + KP] = (uint64_t)bound;
+        __threadfence();
+        __syncthreads();
+        const uint32_t group = my_id / F, first = group * F;
+        const uint32_t n_in = min((uint32_t)F, lists - first);
+        if (threadIdx.x == 0) s_ticket = atomicAdd(tcnt + lvl_cnt_off + group, 1u);
+        __syncthreads();
+        if (s_ticket != n_in - 1) return;            // not the last of my group: done
+        __threadfence();
+        if (threadIdx.x == 0) tcnt[lvl_cnt_off + group] = 0u;   // re-arm for the next launch
+        const uint32_t groups = (lists + F - 1) / F;
+        const int keep = (groups == 1) ? KF : KP;     // the root keeps the re-rank set
+        {
+          // Pre-filter before sorting: every list is sorted best-first, so with
+          // r = ceil(keep / n_in) - 1 the worst of the lists' r-th keys is a lower bound of the
+          // group's keep-th best (n_in * (r+1) >= keep keys are at least that good).  Only keys at
+          // or above it can survive the merge -- typically ~100 of the 1024 -- and the sort
+          // shrinks from the 1024-key to the 256-key network.  r >= KP (fewer than `keep` keys
+          // in total): nothing can be filtered.
+          constexpr int PER = STB_SORT_CAP / STB_SCAN_THREADS;
+          uint64_t v[PER];
+          const uint32_t r = (keep + n_in - 1) / n_in - 1;
+          if (threadIdx.x == 0) { s_T64 = (r >= (uint32_t)KP) ? STB_KEY_INVALID : 0ull; s_cnt = 0u; s_bound = 0u; s_nin = 0u; }
+          __syncthreads();
+          unsigned my_valid = 0;
+#pragma unroll
+          for (int u = 0; u < PER; ++u) {
+            const int i = threadIdx.x + u * STB_SCAN_THREADS;
+            const uint32_t li = i / KP;
+            v[u] = (li < n_in) ? __ldcg(lvl + (size_t)(first + li) * KPS + (i % KP)) : STB_KEY_INVALID;
+            my_valid += (v[u] != STB_KEY_INVALID) ? 1u : 0u;
+            if (li < n_in && (uint32_t)(i % KP) == r) atomicMax(&s_T64, v[u]);   // INVALID (all ones) disables the filter
+          }
+          if (threadIdx.x < n_in) atomicMax(&s_bound, (unsigned)__ldcg(lvl + (size_t)(first + threadIdx.x) * KPS + KP));
+          my_valid = __reduce_add_sync(0xffffffffu, my_valid);
+          if (lane == 0 && my_valid) atomicAdd(&s_nin, my_valid);
+          __syncthreads();
+          const uint64_t T = s_T64;
+#pragma unroll
+          for (int u = 0; u < PER; ++u) {
+            const bool take = v[u] != STB_KEY_INVALID && v[u] <= T;
+            const unsigned m = __ballot_sync(0xffffffffu, take);
+            unsigned base = 0u;
+            if (lane == 0 && m) base = atomicAdd(&s_cnt, (unsigned)__popc(m));
+            base = __shfl_sync(0xffffffffu, base, 0);
+            if (take) skeys[base + __popc(m & ((1u << lane) - 1u))] = v[u];
+          }
+        }
+        __syncthreads();
+        stb_pad_and_sort(skeys, (int)s_cnt, KP);
+        bound = s_bound;
+        if ((int)s_nin > keep) bound = max(bound, stb_f2ord(stb_key_score(skeys[keep - 1])));
+        lvl_key_off += lists;
+        lvl_cnt_off += groups;
+        lists = groups;
+        my_id = group;
       }
     }
+
+    // ---- exact re-rank of the best KF in canonical arithmetic --------------------------
+    // Rows are staged through shared memory (coalesced, one DRAM latency), then one
+    // thread per candidate accumulates (ab, r2) with stb_canon_dot and scores it with stb_canon_dist.
+    for (int i = threadIdx.x; i < STB_D; i += blockDim.x) sqd[i] = (double)__ldg(tq + i);
+    if (threadIdx.x < 2) s_nv[threadIdx.x] = 0;
+    if (threadIdx.x < KF) { s_d[threadIdx.x] = CUDART_INF; s_r[threadIdx.x] = 0xffffffffffffffffull; }
     __syncthreads();
-    if (threadIdx.x == 0) s_done = chunk + 1;
-    if (chunk == 0 && EF > 1 && args.top_k <= 32) {
-      if (threadIdx.x < 32) {
-        const uint64_t key = skeys[lane];
-        double dist = CUDART_INF;
-        if (key != STB_KEY_INVALID) {
-          dist = stb_canon_dist(s_d[lane], s_q2, s_r2[lane]);
-          if (!(dist < STB_DEFAULT_MAX_DIST)) dist = CUDART_INF;
-        }
-        int rank = 0;
+    if (threadIdx.x == 5 * 32) s_q2 = stb_canon_q2(sqd);   // an otherwise idle warp: ||q||^2 once
+    // Candidates are sorted by approximate score (or upper bound) best-first and re-scored 32 at a
+    // time.  After the first 32 the k-th best EXACT cosine c_k among them is known; a later
+    // candidate whose score + eps is below c_k cannot enter the top-k, and neither can anything
+    // after it -- with K' = 128 (q8) this usually ends the re-rank after one pass instead of four.
+    if (threadIdx.x == 0) { s_cthr = -CUDART_INF; s_done = 0; }
+    for (int chunk = 0; chunk < EF; ++chunk) {
+      if (chunk > 0) {
+        const uint64_t nk = skeys[chunk * 32];                            // uniform
+        if (nk == STB_KEY_INVALID || (double)stb_key_score(nk) + kScoreEps < s_cthr) break;
+      }
+      {
+        constexpr int PER = 32 * STB_ROW_F4 / STB_SCAN_THREADS;   // float4 per thread
+        float4 v[PER];
 #pragma unroll
-        for (int jj = 0; jj < 32; ++jj) {
-          const double dj = __shfl_sync(0xffffffffu, dist, jj);
-          rank += (dj < dist || (dj == dist && jj < lane)) ? 1 : 0;
+        for (int u = 0; u < PER; ++u) {
+          const int t = threadIdx.x + u * STB_SCAN_THREADS;
+          const uint64_t key = skeys[chunk * 32 + (t >> 6)];
+          v[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (key != STB_KEY_INVALID)
+            v[u] = __ldg(args.scan.rows + (size_t)stb_key_row(key) * STB_ROW_F4 + (t & 63));
         }
-        const unsigned passing = __ballot_sync(0xffffffffu, dist < CUDART_INF);
-        if ((uint32_t)__popc(passing) >= args.top_k && rank == (int)args.top_k - 1) s_cthr = 1.0 - dist;
+#pragma unroll
+        for (int u = 0; u < PER; ++u) {
+          const int t = threadIdx.x + u * STB_SCAN_THREADS;
+          *reinterpret_cast<float4 *>(srows + (t >> 6) * STB_RR_STRIDE + (t & 63) * 4) = v[u];
+        }
       }
       __syncthreads();
-    }
-  }
-  __syncthreads();
-  if (threadIdx.x < KF) {
-    const uint64_t key = skeys[threadIdx.x];
-    double d = CUDART_INF;
-    uint64_t grow = 0xffffffffffffffffull;
-    if (key != STB_KEY_INVALID) atomicAdd(&s_nv[0], 1);     // valid candidates (re-scored or provably outside the top-k)
-    if (key != STB_KEY_INVALID && (int)threadIdx.x < 32 * s_done) {
-      const double dist = stb_canon_dist(s_d[threadIdx.x], s_q2, s_r2[threadIdx.x]);
-      if (dist < STB_DEFAULT_MAX_DIST) {
-        d = dist;
-        grow = args.row_base + (uint64_t)stb_key_row(key);
-        atomicAdd(&s_nv[1], 1);                   // passing
+      // 8 candidates per warp on 4 warps (one per SM sub-partition): the f64 chains are
+      // latency-bound, so spreading them quarters the issue time
+      if (threadIdx.x < 128 && lane < 8) {
+        const int cl = (threadIdx.x >> 5) * 8 + lane;          // candidate inside the chunk
+        const int ci = chunk * 32 + cl;
+        if (skeys[ci] != STB_KEY_INVALID) {
+          double ab, r2;
+          stb_canon_dot<false>(sqd, reinterpret_cast<const float4 *>(srows + cl * STB_RR_STRIDE), ab, r2);
+          s_d[ci] = ab;          // finalised below once ||q||^2 is known
+          s_r2[ci] = r2;
+        }
+      }
+      __syncthreads();
+      if (threadIdx.x == 0) s_done = chunk + 1;
+      if (chunk == 0 && EF > 1 && tk <= 32) {
+        if (threadIdx.x < 32) {
+          const uint64_t key = skeys[lane];
+          double dist = CUDART_INF;
+          if (key != STB_KEY_INVALID) {
+            dist = stb_canon_dist(s_d[lane], s_q2, s_r2[lane]);
+            if (!(dist < STB_DEFAULT_MAX_DIST)) dist = CUDART_INF;
+          }
+          int rank = 0;
+#pragma unroll
+          for (int jj = 0; jj < 32; ++jj) {
+            const double dj = __shfl_sync(0xffffffffu, dist, jj);
+            rank += (dj < dist || (dj == dist && jj < lane)) ? 1 : 0;
+          }
+          const unsigned passing = __ballot_sync(0xffffffffu, dist < CUDART_INF);
+          if ((uint32_t)__popc(passing) >= tk && rank == (int)tk - 1) s_cthr = 1.0 - dist;
+        }
+        __syncthreads();
       }
     }
-    s_d[threadIdx.x] = d;
-    s_r[threadIdx.x] = grow;
-  }
-  __syncthreads();
-  stb_cta_sort_hits(s_d, s_r, KF);
-  const int n_valid = s_nv[0], n_pass = s_nv[1];
-  const uint32_t k = args.top_k;
-  const uint32_t n_out = min((uint32_t)n_pass, k);
-  bool complete;
-  if (bound == 0u) complete = true;    // no node dropped a key: every scorable row is a candidate
-  else {
-    // every row that is not a candidate scored <= the best dropped score
-    const float s_drop = stb_ord2f(bound);
-    complete = (n_out == k) && ((1.0 - (double)s_drop - kScoreEps) > s_d[k - 1]);
-  }
-  if (args.xchg.world <= 1) {
-    stb_write_hits(args.out_hits, s_d, s_r, n_out, k);
-    if (threadIdx.x == 0) {
-      args.out_status[0] = n_out;
-      args.out_status[1] = complete ? 1u : 0u;
-      args.out_status[2] = (uint32_t)n_valid;
-      args.out_status[3] = (uint32_t)KF | ((uint32_t)SRC << 16);
+    __syncthreads();
+    if (threadIdx.x < KF) {
+      const uint64_t key = skeys[threadIdx.x];
+      double d = CUDART_INF;
+      uint64_t grow = 0xffffffffffffffffull;
+      if (key != STB_KEY_INVALID) atomicAdd(&s_nv[0], 1);     // valid candidates (re-scored or provably outside the top-k)
+      if (key != STB_KEY_INVALID && (int)threadIdx.x < 32 * s_done) {
+        const double dist = stb_canon_dist(s_d[threadIdx.x], s_q2, s_r2[threadIdx.x]);
+        if (dist < STB_DEFAULT_MAX_DIST) {
+          d = dist;
+          grow = args.row_base + (uint64_t)stb_key_row(key);
+          atomicAdd(&s_nv[1], 1);                   // passing
+        }
+      }
+      s_d[threadIdx.x] = d;
+      s_r[threadIdx.x] = grow;
     }
-    return;
-  }
+    __syncthreads();
+    stb_cta_sort_hits(s_d, s_r, KF);
+    const int n_valid = s_nv[0], n_pass = s_nv[1];
+    const uint32_t k = tk;
+    const uint32_t n_out = min((uint32_t)n_pass, k);
+    bool complete;
+    if (bound == 0u) complete = true;    // no node dropped a key: every scorable row is a candidate
+    else {
+      // every row that is not a candidate scored <= the best dropped score
+      const float s_drop = stb_ord2f(bound);
+      complete = (n_out == k) && ((1.0 - (double)s_drop - kScoreEps) > s_d[k - 1]);
+    }
+    if (!xchg || args.xchg.world <= 1) {
+      stb_write_hits(th, s_d, s_r, n_out, k);
+      if (threadIdx.x == 0) {
+        ts[0] = n_out;
+        ts[1] = complete ? 1u : 0u;
+        ts[2] = (uint32_t)n_valid;
+        ts[3] = (uint32_t)KF | ((uint32_t)SRC << 16);
+      }
+      return;
+    }
 
-  // ---- fused exchange over NVLink peer memory + global merge ---------------------------
-  const StbXchgArgs &X = args.xchg;
-  const int world = (int)X.world, me = (int)X.rank;
-  const size_t lane_off = (size_t)X.slot * world + me;
-  for (int p = 0; p < world; ++p) stb_write_hits(stb_x_hits(X, p) + lane_off * X.max_k, s_d, s_r, n_out, k);
-  if (threadIdx.x < world) stb_x_status(X, threadIdx.x)[lane_off] = (complete ? 1u : 0u) | (n_out << 8);
-  __threadfence_system();
-  __syncthreads();
-  if (threadIdx.x < world) stb_st_release_sys(stb_x_flags(X, threadIdx.x) + lane_off, X.seq);
-  __shared__ unsigned int s_timeout;
-  if (threadIdx.x == 0) s_timeout = 0u;
-  __syncthreads();
-  if (threadIdx.x < world) {
-    const unsigned long long *f = stb_x_flags(X, me) + (size_t)X.slot * world + threadIdx.x;
-    const long long t0 = clock64();
-    while (stb_ld_acquire_sys(f) != X.seq) {
-      if (clock64() - t0 > STB_XCHG_TIMEOUT_CYCLES) { s_timeout = 1u; break; }   // a peer is gone
+    // ---- fused exchange over NVLink peer memory + global merge ---------------------------
+    const StbXchgArgs &X = args.xchg;
+    const int world = (int)X.world, me = (int)X.rank;
+    const size_t lane_off = (size_t)X.slot * world + me;
+    for (int p = 0; p < world; ++p) stb_write_hits(stb_x_hits(X, p) + lane_off * X.max_k, s_d, s_r, n_out, k);
+    if (threadIdx.x < world) stb_x_status(X, threadIdx.x)[lane_off] = (complete ? 1u : 0u) | (n_out << 8);
+    __threadfence_system();
+    __syncthreads();
+    if (threadIdx.x < world) stb_st_release_sys(stb_x_flags(X, threadIdx.x) + lane_off, X.seq);
+    if (threadIdx.x == 0) s_timeout = 0u;
+    __syncthreads();
+    if (threadIdx.x < world) {
+      const unsigned long long *f = stb_x_flags(X, me) + (size_t)X.slot * world + threadIdx.x;
+      const long long t0 = clock64();
+      while (stb_ld_acquire_sys(f) != X.seq) {
+        if (clock64() - t0 > STB_XCHG_TIMEOUT_CYCLES) { s_timeout = 1u; break; }   // a peer is gone
+      }
+    }
+    __syncthreads();
+    // merge world x k hits by (distance,row); buffers alias the re-rank staging area
+    double *md = reinterpret_cast<double *>(srows);
+    uint64_t *mr = reinterpret_cast<uint64_t *>(srows) + 1024;
+    const int n_in = world * (int)k;
+    int n_sort = 2;
+    while (n_sort < n_in) n_sort <<= 1;
+    const stb_hit *lh = stb_x_hits(X, me) + (size_t)X.slot * world * X.max_k;
+    for (int i = threadIdx.x; i < n_sort; i += blockDim.x) {
+      double d = CUDART_INF;
+      uint64_t r = 0xffffffffffffffffull;
+      if (i < n_in) {
+        const stb_hit *src = lh + (size_t)(i / (int)k) * X.max_k + (i % (int)k);
+        d = __ldcv(&src->distance);
+        r = __ldcv(&src->row);
+      }
+      md[i] = d; mr[i] = r;
+    }
+    __syncthreads();
+    stb_cta_sort_hits(md, mr, (uint32_t)n_sort);
+    stb_write_hits(th, md, mr, k, k);     // n_sort >= world * k: no padding
+    if (threadIdx.x == 0) {
+      uint32_t all_complete = s_timeout ? 0u : 1u, total = 0u;
+      const uint32_t *st = stb_x_status(X, me) + (size_t)X.slot * world;
+      for (int p = 0; p < world; ++p) {
+        uint32_t v = __ldcv(st + p);
+        all_complete &= (v & 1u);
+        total += v >> 8;
+      }
+      ts[0] = min(total, k);
+      ts[1] = all_complete;
+      ts[2] = s_timeout ? 0xfffffffeu : (uint32_t)n_valid;
+      ts[3] = (uint32_t)KF | ((uint32_t)SRC << 16);
+    }
+  };
+  // every warp of a pair's host learns the join by its last (failing) draw at the latest: the CTA agrees.  The
+  // flag waits in shared memory while the host's tail runs.
+  __shared__ int s_pair_joined;
+  if constexpr (kPair) {
+    if (threadIdx.x == 0) s_pair_joined = 0;
+    __syncthreads();
+    if (joined && (threadIdx.x & 31) == 0) s_pair_joined = 1;
+  }
+  tail(sink, args.scan.q, args.top_k, args.out_hits, args.out_status, args.keys, args.counters, true);
+  if constexpr (kPair) {
+    if (s_pair_joined) {
+      const unsigned long long *s = args.pair.seat;
+      tail(sink2, reinterpret_cast<const float *>(__ldcg(s + STB_SEAT_Q)), (uint32_t)__ldcg(s + STB_SEAT_INFO),
+           reinterpret_cast<stb_hit *>(__ldcg(s + STB_SEAT_HITS)), reinterpret_cast<uint32_t *>(__ldcg(s + STB_SEAT_STATUS)),
+           args.pair.keys2, args.pair.counters2, false);
     }
   }
-  __syncthreads();
-  // merge world x k hits by (distance,row); buffers alias the re-rank staging area
-  double *md = reinterpret_cast<double *>(srows);
-  uint64_t *mr = reinterpret_cast<uint64_t *>(srows) + 1024;
-  const int n_in = world * (int)k;
-  int n_sort = 2;
-  while (n_sort < n_in) n_sort <<= 1;
-  const stb_hit *lh = stb_x_hits(X, me) + (size_t)X.slot * world * X.max_k;
-  for (int i = threadIdx.x; i < n_sort; i += blockDim.x) {
-    double d = CUDART_INF;
-    uint64_t r = 0xffffffffffffffffull;
-    if (i < n_in) {
-      const stb_hit *src = lh + (size_t)(i / (int)k) * X.max_k + (i % (int)k);
-      d = __ldcv(&src->distance);
-      r = __ldcv(&src->row);
-    }
-    md[i] = d; mr[i] = r;
-  }
-  __syncthreads();
-  stb_cta_sort_hits(md, mr, (uint32_t)n_sort);
-  stb_write_hits(args.out_hits, md, mr, k, k);     // n_sort >= world * k: no padding
-  if (threadIdx.x == 0) {
-    uint32_t all_complete = s_timeout ? 0u : 1u, total = 0u;
-    const uint32_t *st = stb_x_status(X, me) + (size_t)X.slot * world;
-    for (int p = 0; p < world; ++p) {
-      uint32_t v = __ldcv(st + p);
-      all_complete &= (v & 1u);
-      total += v >> 8;
-    }
-    args.out_status[0] = min(total, k);
-    args.out_status[1] = all_complete;
-    args.out_status[2] = s_timeout ? 0xfffffffeu : (uint32_t)n_valid;
-    args.out_status[3] = (uint32_t)KF | ((uint32_t)SRC << 16);
-  }
+}
+
+template <int E, int U, int RANGES, int SRC = 0, int EF = E>
+__global__ void __launch_bounds__(STB_SCAN_THREADS, STB_SCAN_MINB)
+stb_scan_topk_kernel(const TopkArgs args) {
+  stb_scan_topk_body<E, U, RANGES, SRC, EF>(args);
+}
+
+// The q8 tier: at most STB_Q8_SCAN_REGS registers, so that two CTAs leave an SM room for a pair's join kernel
+// (__maxnreg__ excludes __launch_bounds__; 256 x 120 x 2 <= 65536 keeps the 2 CTAs per SM).
+#define STB_Q8_SCAN_REGS 120
+template <int E, int U, int RANGES, int EF>
+__global__ void __maxnreg__(STB_Q8_SCAN_REGS)
+stb_scan_topk_kernel_q8(const TopkArgs args) {
+  stb_scan_topk_body<E, U, RANGES, 2, EF>(args);
 }
 
 uint32_t stb_scan_topk_max_k(void) { return 96; }
@@ -1193,19 +1510,29 @@ static int stb_pick_e(uint32_t top_k) {
 template <int E, int RANGES, int SRC = 0, int EF = E>
 static int stb_launch_topk_t(stb_ctx *ctx, const TopkArgs &a_in, bool overlapped) {
   constexpr int kU = SRC == 2 ? STB_Q4_SCAN_U : (SRC == 1 ? STB_SHADOW_SCAN_U : STB_SCAN_U);
-  auto kern = stb_scan_topk_kernel<E, kU, RANGES, SRC, EF>;
+  void (*kern)(const TopkArgs);
+  if constexpr (SRC == 2) kern = stb_scan_topk_kernel_q8<E, kU, RANGES, EF>;
+  else kern = stb_scan_topk_kernel<E, kU, RANGES, SRC, EF>;
   // resident CTAs per SM the grid is sized for: what the occupancy calculator allows (2 with the
   // 128-register budget)
   int occ = 0;
   STB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, STB_SCAN_THREADS, 0));
   if (occ < 1) occ = 1;
   TopkArgs a = a_in;
+  memset(&a.pair, 0, sizeof(a.pair));
   overlapped = overlapped && occ >= 2;
-  if (overlapped) occ = 1;                 // two consecutive grids co-reside, one CTA per SM each
-  a.early_trigger = overlapped ? 1u : 0u;
+  // q8 whole-shard launches of an overlapped series come in pairs (see "pairs"): a host fills the SMs, and
+  // the guest after it is scored by it.  Other overlapped launches: two consecutive grids co-reside, one CTA
+  // per SM each.
   const uint64_t tiles = (a.scan.n_virtual + 4 * kU - 1) / (4 * kU);
+  const bool pairable = SRC == 2 && RANGES == 0 && overlapped && a.xchg.world == 0 && tiles >= STB_PAIR_MIN_TILES;
+  if (overlapped && !pairable) occ = 1;
+  a.early_trigger = overlapped ? 1u : 0u;
   uint64_t want = (tiles + STB_SCAN_WARPS - 1) / STB_SCAN_WARPS;
   uint64_t grid = (uint64_t)ctx->sm_count * occ;
+  // a pair's host leaves two CTA slots to the pair before it, whose last tail CTA and guest CTA outlive its
+  // other CTAs: so the whole grid, and with it the next join kernel, starts while they finish
+  if (pairable && grid > 2) grid -= 2;
   if (want < grid) grid = want < 1 ? 1 : want;
   // scratch: lists (KP keys + bound) for all tree levels (< 2 * grid lists), counters (< grid groups)
   size_t need_keys = (size_t)2 * grid * (32 * E + 1) + STB_SORT_CAP;
@@ -1247,15 +1574,59 @@ static int stb_launch_topk_t(stb_ctx *ctx, const TopkArgs &a_in, bool overlapped
     p.slot = slot; p.t_base = a.scan.t_base; p.t_bulk = a.scan.t_bulk; p.tag = tag;
   }
   if (!a.co.word) ctx->coscan_prev.rows = nullptr;
+  // pairs: a pairable launch right after a host with an open seat on the same rows becomes its guest; any
+  // other launch closes the seat, and a pairable one opens its own
+  auto &ph = ctx->pair_host;
+  const bool guest = pairable && ph.open && ph.rows == a.scan.rows && ph.n_virtual == a.scan.n_virtual;
+  ph.open = false;
+  ctx->pair_guest_of[slot] = 0;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;   // PDL, see the kernel
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  if (guest) {
+    unsigned long long *seat = ctx->pair_seats + (size_t)ph.slot * STB_SEAT_WORDS;
+    StbPairJoinArgs j;
+    j.seat = seat;
+    j.tickets = ctx->tickets + ph.slot;
+    j.t_base = ph.t_base;
+    j.n_tickets = ph.n_tickets;
+    j.v_floor = ctx->pair_floor;
+    j.q = a.scan.q; j.hits = a.out_hits; j.status = a.out_status; j.top_k = a.top_k;
+    j.thr = a.q4.thr; j.q4_tag = a.q4.tag; j.tag = a.q4.tag;
+    a.pair.decided = seat + STB_SEAT_DECIDED;
+    a.pair.tag = a.q4.tag;
+    a.pair.booked = n_tickets + warps_total;
+    ctx->ticket_next[ph.slot] += STB_PAIR_JUMP;    // the join's jump (a refusing join adds it after the host)
+    ctx->pair_guest_of[slot] = (uint32_t)ph.slot + 1;
+    ctx->pair_guest_tag[slot] = a.q4.tag;
+    cudaLaunchConfig_t jc;
+    memset(&jc, 0, sizeof(jc));
+    jc.gridDim = dim3(1);
+    jc.blockDim = dim3(32);
+    jc.stream = ctx->stream;
+    jc.attrs = attr;
+    jc.numAttrs = 1;
+    STB_CUDA(cudaLaunchKernelEx(&jc, stb_pair_join_kernel, j));
+    ctx->kernel_launches++;
+  } else if (pairable) {
+    // the guest's tail merges its lists through the second half of the scratch
+    if (2 * need_keys > ctx->block_keys.cap || 2 * (grid + 8) > ctx->counters.cap) {
+      stb_set_error("scan scratch too small for a pair (grid=%llu)", (unsigned long long)grid);
+      return STB_ERR_STATE;
+    }
+    a.pair.seat = ctx->pair_seats + (size_t)slot * STB_SEAT_WORDS;
+    a.pair.keys2 = ctx->block_keys + need_keys;
+    a.pair.counters2 = ctx->counters + grid + 8;
+    ph.rows = a.scan.rows; ph.n_virtual = a.scan.n_virtual; ph.slot = slot;
+    ph.t_base = a.scan.t_base; ph.n_tickets = n_tickets; ph.open = true;
+  }
+  ctx->pair_t_bulk[slot] = a.scan.t_bulk;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3((unsigned)grid);
   cfg.blockDim = dim3(STB_SCAN_THREADS);
   cfg.dynamicSmemBytes = 0;
   cfg.stream = ctx->stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;   // PDL, see the kernel
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   STB_CUDA(cudaLaunchKernelEx(&cfg, kern, a));
@@ -1308,6 +1679,7 @@ int stb_launch_scan_topk(stb_ctx *ctx, const stb_corpus *c, int tier, const floa
     // a fresh tag per launch, slots in turn (stb_scan_q4); after 2^32 launches the words are cleared once
     if ((uint32_t)++ctx->q4_launches == 0) {
       STB_CUDA(cudaMemsetAsync(ctx->q4_thr, 0, STB_TICKET_SLOTS * STB_Q4_WORDS * sizeof(unsigned long long), ctx->stream));
+      STB_CUDA(cudaMemsetAsync(ctx->pair_seats, 0, STB_TICKET_SLOTS * STB_SEAT_WORDS * sizeof(unsigned long long), ctx->stream));
       ++ctx->q4_launches;
     }
     a.q4.plane = c->q4;
