@@ -734,8 +734,8 @@ int stb_debug_q4_refined(stb_ctx *ctx, int reset, uint64_t *refined);
 int stb_debug_coscan_offsets(stb_ctx *ctx, uint32_t n, uint32_t *out);
 /* Test hooks for K1's pairs: a q8 top-k query of an asynchronous series (stb_search_topk_dev, stb_search_many
  * without an exchange) that follows a query on the same corpus joins its running scan, which scores both
- * queries from one read of each plane tile.  stb_debug_pair_joins: for the last n top-k launches on the
- * ticket ring, oldest first, the tile at which each joined its host; -1 for a launch that was not such a
+ * queries from one read of each plane tile.  stb_debug_pair_joins: for the last n (<= 8) top-k launches on
+ * the context, oldest first, the tile at which each joined its host; -1 for a launch that was not such a
  * guest, -2 for a guest whose join was refused (it scanned alone).  Synchronises the context's stream.
  * stb_debug_pair_floor: later joins wait until their host has drawn v_floor tile tickets (0: no wait). */
 int stb_debug_pair_joins(stb_ctx *ctx, uint32_t n, int64_t *out);

@@ -102,22 +102,15 @@ int stb_ctx_create(int device, void *cuda_stream, stb_ctx **out) {
       (rc = c->err_flag.alloc(1)) != STB_OK ||
       (rc = c->embed_flag.alloc(1)) != STB_OK ||
       (rc = c->hist_dev.alloc(4096)) != STB_OK ||
-      (rc = c->tickets.alloc(STB_TICKET_SLOTS)) != STB_OK ||
-      (rc = c->q4_thr.alloc(STB_TICKET_SLOTS * STB_Q4_WORDS)) != STB_OK ||
+      (rc = c->series.init(c->stream)) != STB_OK ||
       (rc = c->q4_refined.alloc(1)) != STB_OK ||
-      (rc = c->coscan_off.alloc(STB_TICKET_SLOTS)) != STB_OK ||
-      (rc = c->pair_seats.alloc(STB_TICKET_SLOTS * STB_SEAT_WORDS)) != STB_OK ||
       (rc = c->hits_dev.alloc(1024)) != STB_OK ||
       (rc = c->q_pin.alloc(STB_D)) != STB_OK ||
       (rc = c->status_pin.alloc(8)) != STB_OK ||
       (rc = c->hits_pin.alloc(1024)) != STB_OK)
     goto fail;
   if (cudaMemset(c->counters, 0, c->counters.cap * sizeof(unsigned int)) != cudaSuccess ||
-      cudaMemset(c->tickets, 0, STB_TICKET_SLOTS * sizeof(unsigned long long)) != cudaSuccess ||
-      cudaMemset(c->q4_thr, 0, STB_TICKET_SLOTS * STB_Q4_WORDS * sizeof(unsigned long long)) != cudaSuccess ||
       cudaMemset(c->q4_refined, 0, sizeof(unsigned long long)) != cudaSuccess ||
-      cudaMemset(c->coscan_off, 0, STB_TICKET_SLOTS * sizeof(unsigned long long)) != cudaSuccess ||
-      cudaMemset(c->pair_seats, 0, STB_TICKET_SLOTS * STB_SEAT_WORDS * sizeof(unsigned long long)) != cudaSuccess ||
       cudaMemset(c->err_flag, 0, sizeof(int)) != cudaSuccess ||
       cudaMemset(c->embed_flag, 0, sizeof(int)) != cudaSuccess) {
     stb_set_error("context staging allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
@@ -153,24 +146,6 @@ int stb_ctx_sync(stb_ctx *ctx) {
 
 void *stb_ctx_stream(stb_ctx *ctx) { return ctx ? (void *)ctx->stream : nullptr; }
 
-// K1's tile tickets: every top-k launch must advance the device counter by exactly what the host
-// booked for it (n_tickets + total_warps); a mismatch would make later launches skip or repeat
-// tiles.  Synchronises; returns STB_ERR_STATE on a mismatch.
-int stb_debug_ticket_check(stb_ctx *ctx, uint64_t *device_value, uint64_t *host_value) {
-  int rc = ctx_use(ctx);
-  if (rc) return rc;
-  unsigned long long v[STB_TICKET_SLOTS];
-  STB_CUDA(cudaStreamSynchronize(ctx->stream));
-  STB_CUDA(cudaMemcpy(v, ctx->tickets, sizeof(v), cudaMemcpyDeviceToHost));
-  unsigned long long dsum = 0, hsum = 0;
-  int bad = -1;
-  for (int i = 0; i < STB_TICKET_SLOTS; ++i) { dsum += v[i]; hsum += ctx->ticket_next[i]; if (v[i] != ctx->ticket_next[i] && bad < 0) bad = i; }
-  if (device_value) *device_value = dsum;          // sums over the counter ring
-  if (host_value) *host_value = hsum;
-  if (bad >= 0) { stb_set_error("ticket counter %d is %llu, host expects %llu", bad, v[bad], ctx->ticket_next[bad]); return STB_ERR_STATE; }
-  return STB_OK;
-}
-
 // Rows the q8 tier's prefilter passed on to the int8 codes, summed over the top-k launches since the
 // last reset.  Synchronises.
 int stb_debug_q4_refined(stb_ctx *ctx, int reset, uint64_t *refined) {
@@ -181,57 +156,6 @@ int stb_debug_q4_refined(stb_ctx *ctx, int reset, uint64_t *refined) {
   STB_CUDA(cudaMemcpy(&v, ctx->q4_refined, sizeof(v), cudaMemcpyDeviceToHost));
   if (reset) STB_CUDA(cudaMemset(ctx->q4_refined, 0, sizeof(v)));
   if (refined) *refined = v;
-  return STB_OK;
-}
-
-// The tile offsets K1's last n top-k launches on the ticket ring started their pass at, oldest first;
-// 0xffffffff for a launch that did not co-scan (or whose slot a later launch reused).  Synchronises.
-int stb_debug_coscan_offsets(stb_ctx *ctx, uint32_t n, uint32_t *out) {
-  int rc = ctx_use(ctx);
-  if (rc) return rc;
-  if (n > STB_TICKET_SLOTS || (n && !out)) { stb_set_error("coscan_offsets: n must be 0..%d", STB_TICKET_SLOTS); return STB_ERR_ARG; }
-  unsigned long long w[STB_TICKET_SLOTS];
-  STB_CUDA(cudaStreamSynchronize(ctx->stream));
-  STB_CUDA(cudaMemcpy(w, ctx->coscan_off, sizeof(w), cudaMemcpyDeviceToHost));
-  for (uint32_t i = 0; i < n; ++i) {
-    out[i] = 0xffffffffu;
-    if (ctx->topk_launches < n - i) continue;
-    const int slot = (int)((ctx->topk_launches - (n - i)) % STB_TICKET_SLOTS);
-    const uint32_t tag = ctx->coscan_tag[slot];
-    if (tag && (uint32_t)(w[slot] >> 32) == tag) out[i] = (uint32_t)w[slot];
-  }
-  return STB_OK;
-}
-
-// Where K1's last n top-k launches on the ticket ring joined their host, oldest first: the join tile (the first
-// tile of the join ticket), -1 for a launch that was not a guest (or whose slot a later launch reused), -2 for a
-// guest whose join was refused.  Synchronises.
-int stb_debug_pair_joins(stb_ctx *ctx, uint32_t n, int64_t *out) {
-  int rc = ctx_use(ctx);
-  if (rc) return rc;
-  if (n > STB_TICKET_SLOTS || (n && !out)) { stb_set_error("pair_joins: n must be 0..%d", STB_TICKET_SLOTS); return STB_ERR_ARG; }
-  unsigned long long w[STB_TICKET_SLOTS * STB_SEAT_WORDS];
-  STB_CUDA(cudaStreamSynchronize(ctx->stream));
-  STB_CUDA(cudaMemcpy(w, ctx->pair_seats, sizeof(w), cudaMemcpyDeviceToHost));
-  for (uint32_t i = 0; i < n; ++i) {
-    out[i] = -1;
-    if (ctx->topk_launches < n - i) continue;
-    const int slot = (int)((ctx->topk_launches - (n - i)) % STB_TICKET_SLOTS);
-    if (!ctx->pair_guest_of[slot]) continue;
-    const unsigned long long d = w[(ctx->pair_guest_of[slot] - 1) * STB_SEAT_WORDS + STB_SEAT_DECIDED];
-    if ((uint32_t)(d >> 32) != ctx->pair_guest_tag[slot]) continue;                         // a later pair reused the seat
-    if (!(d & 0x80000000ull)) { out[i] = -2; continue; }
-    const uint64_t v = (uint32_t)d & 0x7fffffffu, tb = ctx->pair_t_bulk[slot];
-    out[i] = (int64_t)(v < tb ? v * STB_TICKET_TILES : tb * STB_TICKET_TILES + (v - tb));
-  }
-  return STB_OK;
-}
-
-// Test hook: a join waits until its host has drawn v_floor tickets (0: joins as early as it runs).
-int stb_debug_pair_floor(stb_ctx *ctx, uint64_t v_floor) {
-  int rc = ctx_use(ctx);
-  if (rc) return rc;
-  ctx->pair_floor = v_floor;
   return STB_OK;
 }
 
@@ -405,8 +329,7 @@ enum CorpusChange { CORPUS_APPEND, CORPUS_ROWS_REWRITTEN, CORPUS_CLEAR };
 static void corpus_changed(stb_corpus *c, CorpusChange kind) {
   if (kind == CORPUS_CLEAR) { c->shadow_rows = 0; c->q8_rows = 0; c->shadow_bad = 0; c->q8_bad = 0; }
   if (kind != CORPUS_APPEND) ++c->epoch;
-  if (kind == CORPUS_ROWS_REWRITTEN && c->ctx->coscan_prev.rows == c->rows) c->ctx->coscan_prev.rows = nullptr;
-  if (c->ctx->pair_host.rows == c->rows) c->ctx->pair_host.open = false;   // a guest after this starts its own pair
+  c->ctx->series.forget_rows(c->rows, kind == CORPUS_ROWS_REWRITTEN);
   c->searches_since_change = 0;
   memset(c->tier_tries, 0, sizeof(c->tier_tries));
   memset(c->tier_proven, 0, sizeof(c->tier_proven));

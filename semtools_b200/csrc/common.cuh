@@ -123,6 +123,70 @@ struct StbBuf {
 };
 template <class T> using StbPinned = StbBuf<T, true>;
 
+#define STB_TICKET_SLOTS 8
+#define STB_TICKET_TILES 4   // co-scan, 10M rows, q8: 4 and 2 tiles 0.434 ms/query, 1 tile 0.635 ms
+// K1 pairs (scan_topk.cu: "pairs"): the words of a seat.  (one seat per ticket slot, indexed by the host's slot; never cleared: the tags tell launches apart)
+#define STB_SEAT_Q 0                 // guest query (device pointer)
+#define STB_SEAT_HITS 1              // guest hits
+#define STB_SEAT_STATUS 2            // guest status
+#define STB_SEAT_THR 3               // guest threshold words
+#define STB_SEAT_INFO 4              // guest tag << 32 | top_k
+#define STB_SEAT_DECIDED 5           // guest tag << 32 | (joined: 0x80000000 | join ticket v; refused: 0)
+#define STB_SEAT_WRAP 6              // host tag << 32 | guest-only tickets drawn
+#define STB_SEAT_WORDS 8
+
+// K1's tile tickets (scan_topk.cu: stb_for_each_tile) for `tiles` tiles on `warps` warps: t_bulk tickets of
+// STB_TICKET_TILES tiles, then the last ~2 tiles per warp one by one.  A launch advances its counter by
+// n_tickets + warps.
+struct StbTicketPlan {
+  uint64_t t_bulk, n_tickets;
+};
+__host__ __device__ inline StbTicketPlan stb_ticket_plan(uint64_t tiles, uint64_t warps) {
+  const uint64_t single = tiles < 2 * warps ? tiles : 2 * warps;
+  const uint64_t t_bulk = (tiles - single) / STB_TICKET_TILES;
+  return {t_bulk, t_bulk + (tiles - t_bulk * STB_TICKET_TILES)};
+}
+// Ticket t covers tiles [stb_ticket_first_tile(t), stb_ticket_first_tile(t + 1)) of the launch's pass.
+__host__ __device__ __forceinline__ uint64_t stb_ticket_first_tile(uint64_t t, uint64_t t_bulk) {
+  return t < t_bulk ? t * STB_TICKET_TILES : t_bulk * STB_TICKET_TILES + (t - t_bulk);
+}
+
+// One K1 top-k launch as its slot of the series records it.
+struct StbSeriesLaunch {
+  uint32_t tag;                  // the low 32 bits of its launch number (0: no launch)
+  unsigned long long t_base;     // its ticket counter's value at its start
+  uint64_t t_bulk, n_tickets;    // its ticket plan
+  bool coscan;                   // it co-scanned: its co-scan word carries its tag
+  int host;                      // a guest: the slot of the host it joined; -1: not a guest
+  // what the next launch compares to follow it (co-scan) or take its seat: the corpus copy and shape it
+  // scanned (rows null: nothing to follow), and whether it is a pair host with an open seat
+  const void *rows;
+  int src;
+  uint64_t n_virtual, tiles;
+  bool seat_open;
+};
+
+// K1's series of top-k launches (DESIGN.md §4 item 2; only scan_topk.cu: stb_launch_topk_t writes it).  Launch n
+// (counted from 1) takes slot n % STB_TICKET_SLOTS -- its ticket counter, co-scan word, q4 threshold words and
+// seat -- and the tag (uint32_t)n, which every tagged word it writes carries.  Tag 0 is skipped: there the
+// series is reset once.
+struct StbScanSeries {
+  StbBuf<unsigned long long> tickets;      // [slot]: monotonic ticket counter
+  StbBuf<unsigned long long> coscan_off;   // [slot]: tag << 32 | the tile offset its launch chose (stb_coscan_offset)
+  StbBuf<unsigned long long> q4_thr;       // [slot][STB_Q4_WORDS]: tagged threshold words (stb_scan_q4)
+  StbBuf<unsigned long long> seats;        // [slot][STB_SEAT_WORDS]: the seat of a pair host ("pairs")
+  unsigned long long ticket_next[STB_TICKET_SLOTS];   // [slot]: the counter's value when its next launch starts
+  uint64_t launches;                       // the last launch's number
+  StbSeriesLaunch launch[STB_TICKET_SLOTS];
+  uint64_t pair_floor;                     // test hook (stb_debug_pair_floor): joins wait for this many host tickets
+
+  int init(cudaStream_t stream);           // allocates the device words, then reset()
+  int reset(cudaStream_t stream);          // zeroes every device word, ticket_next and the records
+  // The rows at `rows` changed: a launch after this takes no seat on the last launch if it scanned them, and
+  // after a rewrite of the rows does not follow it either.
+  void forget_rows(const void *rows, bool rewritten);
+};
+
 struct stb_ctx {
   int device;
   int sm_count;
@@ -131,45 +195,8 @@ struct stb_ctx {
   // --- scan scratch (device) ---
   StbBuf<uint64_t> block_keys;     // candidate keys of every tree level
   StbBuf<unsigned int> counters;   // tree arrival counters (zeroed; kernels re-zero)
-  // K1 tile-ticket counters (monotonic; scan_topk.cu: stb_for_each_tile).  A ring of STB_TICKET_SLOTS
-  // counters, one per launch in turn: with the overlapped launch mode two consecutive scans run
-  // concurrently and must not draw from the same counter.
-  StbBuf<unsigned long long> tickets;
-  unsigned long long ticket_next[8];   // per slot: its value when the next launch using it starts
-  unsigned long long topk_launches;    // picks the slot
-  bool ticket_ring;                    // set by the first overlapped launch; until then every launch uses slot 0
-  // K1 co-scan (scan_topk.cu: stb_coscan_offset): per ticket slot, the tile offset its last co-scan launch
-  // chose, as a tagged word (tag << 32 | offset, the tag is the launch count); the host's copy of the tags
-  // (0: the slot's last launch did not co-scan) and the last co-scan launch, which the next one may follow
-  StbBuf<unsigned long long> coscan_off;
-  uint32_t coscan_tag[8];
-  struct {
-    const void *rows;                  // the scanned corpus's f32 rows; null: no launch to follow
-    int src;
-    uint64_t n_virtual, tiles, t_bulk;
-    unsigned long long t_base;
-    int slot;
-    uint32_t tag;
-  } coscan_prev;
-  // q8 tier prefilter (scan_topk.cu: stb_scan_q4): STB_TICKET_SLOTS x STB_Q4_WORDS tagged threshold words,
-  // one slot per launch in turn; the launch count is the tag
-  StbBuf<unsigned long long> q4_thr;
-  unsigned long long q4_launches;
+  StbScanSeries series;            // K1's top-k launches: ticket counters, co-scan, q4 threshold words, pairs
   StbBuf<unsigned long long> q4_refined;   // rows the prefilter passed on to the int8 codes (stb_debug_q4_refined)
-  // K1 pairs (scan_topk.cu: "pairs"): one seat of STB_SEAT_WORDS device words per ticket slot; the host whose seat
-  // is open; per ticket slot, 1 + the host's slot if its launch was a guest (0: it was not), the guest's tag and
-  // t_bulk (stb_debug_pair_joins); the test hook's floor on the join ticket
-  StbBuf<unsigned long long> pair_seats;
-  struct {
-    const void *rows;
-    uint64_t n_virtual, n_tickets;
-    unsigned long long t_base;
-    int slot;
-    bool open;
-  } pair_host;
-  uint32_t pair_guest_of[8], pair_guest_tag[8];
-  uint64_t pair_t_bulk[8];
-  uint64_t pair_floor;
   StbBuf<float> q_dev;             // 256 f32 staging for host queries
   StbBuf<stb_hit> hits_dev;        // result hits (top-k path)
   StbBuf<uint32_t> status_dev;     // [0]=n hits, [1]=complete flag, [2..] debug
@@ -252,17 +279,6 @@ struct stb_ctx {
   StbBuf<int> embed_flag;          // device int: K3's sticky range flag; set only by stb_embed_dev, cleared only by stb_embed_status
 };
 
-#define STB_TICKET_SLOTS 8
-#define STB_TICKET_TILES 4   // co-scan, 10M rows, q8: 4 and 2 tiles 0.434 ms/query, 1 tile 0.635 ms
-// K1 pairs (scan_topk.cu: "pairs"): the words of a seat.  (one seat per ticket slot, indexed by the host's slot; never cleared: the tags tell launches apart)
-#define STB_SEAT_Q 0                 // guest query (device pointer)
-#define STB_SEAT_HITS 1              // guest hits
-#define STB_SEAT_STATUS 2            // guest status
-#define STB_SEAT_THR 3               // guest threshold words
-#define STB_SEAT_INFO 4              // guest q4 tag << 32 | top_k
-#define STB_SEAT_DECIDED 5           // guest tag << 32 | (joined: 0x80000000 | join ticket v; refused: 0)
-#define STB_SEAT_WRAP 6              // host q4 tag << 32 | guest-only tickets drawn
-#define STB_SEAT_WORDS 8
 // Spin-wait bound of the peer-memory exchanges (SM cycles, ~15 s): long enough that ranks entering a sharded
 // search a few seconds apart (first-call allocations, a busy host) still meet; a peer that is really gone
 // costs one bound, the call reports it (status 0xfffffffe / 2) and the caller must stop using the exchange:

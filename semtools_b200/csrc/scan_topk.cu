@@ -98,6 +98,24 @@ static unsigned stb_scan_grid(const stb_ctx *ctx, uint64_t n_virtual, int u) {
 // n_tiles, so the pass starts at tile off and wraps around the end
 // (stb_coscan_offset).  Which warp scores which row does not change the
 // lists, the drop bounds or the proof, so any offset gives the same result.
+// The tiles of ticket t in pass order: with RANGES == 0 shifted by the co-scan offset *off and wrapped at n_tiles.
+template <int RANGES, class Body>
+__device__ __forceinline__ void stb_ticket_walk(const ScanArgs &args, uint64_t t, uint64_t n_tiles, const uint32_t *off, Body &&body) {
+  const uint64_t t0 = stb_ticket_first_tile(t, args.t_bulk);
+  const uint64_t t1 = t < args.t_bulk ? t0 + STB_TICKET_TILES : t0 + 1;
+  if constexpr (RANGES == 0) {
+    // *off: a shared word, read per ticket so that it holds no register across the scoring
+    uint32_t tile = (uint32_t)t0 + *reinterpret_cast<const volatile uint32_t *>(off);   // off < n_tiles < 2^32
+    if (tile >= n_tiles) tile -= (uint32_t)n_tiles;
+    for (uint32_t left = (uint32_t)(t1 - t0); left; --left) {
+      body(tile, false);
+      if (++tile == n_tiles) tile = 0;
+    }
+  } else {
+    for (uint64_t tile = t0; tile < t1; ++tile) body(tile, tile == t0);
+  }
+}
+
 template <int RANGES, int WB, class Body>
 __device__ __forceinline__ void stb_for_each_tile(const ScanArgs &args, uint64_t n_tiles, const uint32_t *off, Body &&body) {
   if (args.tickets) {
@@ -111,25 +129,10 @@ __device__ __forceinline__ void stb_for_each_tile(const ScanArgs &args, uint64_t
       if (lane == 0) t = atomicAdd(args.tickets, 1ull);
       return __shfl_sync(0xffffffffu, t, 0) - args.t_base;
     };
-    auto first_tile = [&](unsigned long long t) -> uint64_t {
-      return t < args.t_bulk ? t * STB_TICKET_TILES : args.t_bulk * STB_TICKET_TILES + (t - args.t_bulk);
-    };
     unsigned long long cur = draw();
-    while (first_tile(cur) < n_tiles) {
+    while (stb_ticket_first_tile(cur, args.t_bulk) < n_tiles) {
       const unsigned long long nxt = draw();
-      const uint64_t t0 = first_tile(cur);
-      const uint64_t t1 = cur < args.t_bulk ? t0 + STB_TICKET_TILES : t0 + 1;
-      if constexpr (RANGES == 0) {
-        // *off: a shared word, read per ticket so that it holds no register across the scoring
-        uint32_t tile = (uint32_t)t0 + *reinterpret_cast<const volatile uint32_t *>(off);   // off < n_tiles < 2^32
-        if (tile >= n_tiles) tile -= (uint32_t)n_tiles;
-        for (uint32_t left = (uint32_t)(t1 - t0); left; --left) {
-          body(tile, false);
-          if (++tile == n_tiles) tile = 0;
-        }
-      } else {
-        for (uint64_t tile = t0; tile < t1; ++tile) body(tile, tile == t0);
-      }
+      stb_ticket_walk<RANGES>(args, cur, n_tiles, off, body);
       cur = nxt;
     }
     return;
@@ -726,22 +729,12 @@ __device__ __forceinline__ bool stb_scan_q4(const ScanArgs &args, const uint8_t 
       if (lane == 0) t = (uint32_t)(atomicAdd(args.tickets, 1ull) - args.t_base);
       return __shfl_sync(0xffffffffu, t, 0);
     };
-    auto first_tile = [&](uint64_t t) -> uint64_t {
-      return t < args.t_bulk ? t * STB_TICKET_TILES : args.t_bulk * STB_TICKET_TILES + (t - args.t_bulk);
-    };
     auto run_ticket = [&](uint64_t t, auto mode) {
-      const uint64_t t0 = first_tile(t);
-      const uint64_t t1 = t < args.t_bulk ? t0 + STB_TICKET_TILES : t0 + 1;
-      uint32_t tile = (uint32_t)t0 + *reinterpret_cast<const volatile uint32_t *>(off);   // off < n_tiles < 2^32
-      if (tile >= n_tiles) tile -= (uint32_t)n_tiles;
-      for (uint32_t left = (uint32_t)(t1 - t0); left; --left) {
-        tile_body(tile, false, mode);
-        if (++tile == n_tiles) tile = 0;
-      }
+      stb_ticket_walk<0>(args, t, n_tiles, off, [&](uint64_t tile, bool) { tile_body(tile, false, mode); });
     };
     // host tickets until a draw carries the jump (or fails), then the pair's tickets
     uint32_t cur = draw();
-    while (cur < STB_PAIR_JUMP && first_tile(cur) < n_tiles) {
+    while (cur < STB_PAIR_JUMP && stb_ticket_first_tile(cur, args.t_bulk) < n_tiles) {
       const uint32_t nxt = draw();        // drawn before the ticket is scored (stb_for_each_tile)
       run_ticket(cur, std::integral_constant<int, 1>());
       cur = nxt;
@@ -758,7 +751,7 @@ __device__ __forceinline__ bool stb_scan_q4(const ScanArgs &args, const uint8_t 
       if (lane == 0) *side2 = S;
       __syncwarp();
       cur -= (uint32_t)STB_PAIR_JUMP;
-      while (first_tile(cur) < n_tiles) {
+      while (stb_ticket_first_tile(cur, args.t_bulk) < n_tiles) {
         const uint32_t nxt = draw() - (uint32_t)STB_PAIR_JUMP;
         run_ticket(cur, std::integral_constant<int, 3>());
         cur = nxt;
@@ -780,7 +773,7 @@ __device__ __forceinline__ bool stb_scan_q4(const ScanArgs &args, const uint8_t 
       __syncwarp();
     }
     if (joined) {
-      // the guest-only wrap: tickets [0, v), drawn from the seat's wrap word (tagged with this launch's q4 tag)
+      // the guest-only wrap: tickets [0, v), drawn from the seat's wrap word (tagged with this launch's tag)
       unsigned long long *wrap = seat + STB_SEAT_WRAP;
       const volatile uint32_t *v = gscr + STB_PAIR_SCRATCH - 1;
       for (;;) {
@@ -969,8 +962,7 @@ __device__ __forceinline__ uint32_t stb_coscan_offset(const StbCoscanArgs &c, ui
       const unsigned long long drawn = __ldcg(c.pred_tickets) - c.pred_t_base;
       uint64_t front = n_tiles;
       if (join_front >= 0) front = (uint64_t)join_front;
-      else if (drawn < n_tiles)
-        front = drawn < c.pred_t_bulk ? drawn * STB_TICKET_TILES : c.pred_t_bulk * STB_TICKET_TILES + (drawn - c.pred_t_bulk);
+      else if (drawn < n_tiles) front = stb_ticket_first_tile(drawn, c.pred_t_bulk);
       off = (p_off + (front < n_tiles ? front : 0)) % n_tiles;
     }
     const unsigned long long mine = ((unsigned long long)c.tag << 32) | off;
@@ -1054,12 +1046,12 @@ struct StbPairJoinArgs {
   unsigned long long t_base;       // ... its value at the host's start and the host's ticket count
   uint64_t n_tickets;
   uint64_t v_floor;                // test hook (stb_debug_pair_floor): join no earlier than ticket v_floor
-  const float *q;                  // the guest: query, outputs, k, threshold words and tags
+  const float *q;                  // the guest: query, outputs, k, threshold words and tag
   stb_hit *hits;
   uint32_t *status;
   uint32_t top_k;
   unsigned long long *thr;
-  uint32_t q4_tag, tag;
+  uint32_t tag;
 };
 
 // A warp's registers come from one of the SM's four 16K-register sub-partitions.  Two q8 scan CTAs put four
@@ -1076,7 +1068,7 @@ __global__ void __maxnreg__(STB_PAIR_JOIN_REGS) stb_pair_join_kernel(const StbPa
       s[STB_SEAT_HITS] = reinterpret_cast<unsigned long long>(a.hits);
       s[STB_SEAT_STATUS] = reinterpret_cast<unsigned long long>(a.status);
       s[STB_SEAT_THR] = reinterpret_cast<unsigned long long>(a.thr);
-      s[STB_SEAT_INFO] = ((unsigned long long)a.q4_tag << 32) | a.top_k;
+      s[STB_SEAT_INFO] = ((unsigned long long)a.tag << 32) | a.top_k;
       if (a.v_floor) {                               // the host is running: it draws on or runs out
         unsigned long long t;
         do t = stb_ld_acquire_gpu(a.tickets) - a.t_base; while (t < a.v_floor && t < a.n_tickets);
@@ -1141,8 +1133,7 @@ __device__ __forceinline__ void stb_scan_topk_body(const TopkArgs &args) {
         do w = stb_ld_acquire_gpu(args.pair.decided); while ((uint32_t)(w >> 32) != args.pair.tag);
         if (w & 0x80000000ull) {
           s_guest_joined = 1;
-          const uint64_t v = (uint32_t)w & 0x7fffffffu, tb = args.scan.t_bulk;   // the host's tickets: same grid
-          front = (int64_t)(v < tb ? v * STB_TICKET_TILES : tb * STB_TICKET_TILES + (v - tb));
+          front = (int64_t)stb_ticket_first_tile((uint32_t)w & 0x7fffffffu, args.scan.t_bulk);   // the host's plan: same grid
         }
       }
       s_off = args.co.word ? stb_coscan_offset(args.co, n_tiles, front) : 0u;
@@ -1540,65 +1531,66 @@ static int stb_launch_topk_t(stb_ctx *ctx, const TopkArgs &a_in, bool overlapped
     stb_set_error("scan scratch too small (grid=%llu)", (unsigned long long)grid);
     return STB_ERR_STATE;
   }
-  // tile tickets (stb_for_each_tile): bulk tickets of STB_TICKET_TILES tiles, then the last ~2 tiles
-  // per warp one by one.  The launch advances the counter by n_tickets + total_warps exactly.
   const uint64_t warps_total = grid * STB_SCAN_WARPS;
-  const uint64_t single = std::min<uint64_t>(tiles, 2 * warps_total);
-  a.scan.t_bulk = (tiles - single) / STB_TICKET_TILES;
-  const uint64_t n_tickets = a.scan.t_bulk + (tiles - a.scan.t_bulk * STB_TICKET_TILES);
-  // one counter serves back-to-back launches (a grid starts drawing only after its predecessor's scan, the
-  // validated default); the ring is needed -- and used -- from the first overlapped launch on, when two
-  // consecutive scans co-run (at most ~3 grids are ever in flight)
-  if (overlapped) ctx->ticket_ring = true;
-  const int slot = ctx->ticket_ring ? (int)(ctx->topk_launches++ % STB_TICKET_SLOTS) : 0;
-  a.scan.tickets = ctx->tickets + slot;
-  a.scan.t_base = ctx->ticket_next[slot];
-  ctx->ticket_next[slot] += n_tickets + warps_total;
+  const StbTicketPlan plan = stb_ticket_plan(tiles, warps_total);
+  a.scan.t_bulk = plan.t_bulk;
+  // a pair host's guest merges its lists through the second half of the scratch
+  if (pairable && (2 * need_keys > ctx->block_keys.cap || 2 * (grid + 8) > ctx->counters.cap)) {
+    stb_set_error("scan scratch too small for a pair (grid=%llu)", (unsigned long long)grid);
+    return STB_ERR_STATE;
+  }
+  // the launch's number gives its slot and tag (StbScanSeries)
+  StbScanSeries &ser = ctx->series;
+  if ((uint32_t)++ser.launches == 0) {
+    const int rc = ser.reset(ctx->stream);
+    if (rc != STB_OK) return rc;
+    ++ser.launches;
+  }
+  const int slot = (int)(ser.launches % STB_TICKET_SLOTS), prev_slot = (int)((ser.launches - 1) % STB_TICKET_SLOTS);
+  const uint32_t tag = (uint32_t)ser.launches;
+  const StbSeriesLaunch &prev = ser.launch[prev_slot];
+  a.scan.tickets = ser.tickets + slot;
+  a.scan.t_base = ser.ticket_next[slot];
+  ser.ticket_next[slot] += plan.n_tickets + warps_total;
+  if constexpr (SRC == 2) {
+    a.q4.thr = ser.q4_thr + (size_t)slot * STB_Q4_WORDS;
+    a.q4.tag = tag;
+  }
   // co-scan: follow the last launch if it was one too, on the same corpus copy and rows (hence the
   // same tiles); any other launch in between -- synchronous, sharded, ranged -- ends the series
-  const uint32_t tag = (uint32_t)ctx->topk_launches;   // the launch count, 0 only after a wrap: no co-scan then
-  const bool co = overlapped && tag != 0;
-  if (ctx->ticket_ring) ctx->coscan_tag[slot] = co ? tag : 0u;
-  if (co) {
-    auto &p = ctx->coscan_prev;
-    a.co.word = ctx->coscan_off + slot;
+  if (overlapped) {
+    a.co.word = ser.coscan_off + slot;
     a.co.tag = tag;
-    if (p.rows == a.scan.rows && p.src == SRC && p.n_virtual == a.scan.n_virtual && p.tiles == tiles) {
-      a.co.pred_tag = p.tag;
-      a.co.pred_word = ctx->coscan_off + p.slot;
-      a.co.pred_tickets = ctx->tickets + p.slot;
-      a.co.pred_t_base = p.t_base;
-      a.co.pred_t_bulk = p.t_bulk;
+    if (prev.coscan && prev.rows == a.scan.rows && prev.src == SRC && prev.n_virtual == a.scan.n_virtual && prev.tiles == tiles) {
+      a.co.pred_tag = prev.tag;
+      a.co.pred_word = ser.coscan_off + prev_slot;
+      a.co.pred_tickets = ser.tickets + prev_slot;
+      a.co.pred_t_base = prev.t_base;
+      a.co.pred_t_bulk = prev.t_bulk;
     }
-    p.rows = a.scan.rows; p.src = SRC; p.n_virtual = a.scan.n_virtual; p.tiles = tiles;
-    p.slot = slot; p.t_base = a.scan.t_base; p.t_bulk = a.scan.t_bulk; p.tag = tag;
   }
-  if (!a.co.word) ctx->coscan_prev.rows = nullptr;
-  // pairs: a pairable launch right after a host with an open seat on the same rows becomes its guest; any
-  // other launch closes the seat, and a pairable one opens its own
-  auto &ph = ctx->pair_host;
-  const bool guest = pairable && ph.open && ph.rows == a.scan.rows && ph.n_virtual == a.scan.n_virtual;
-  ph.open = false;
-  ctx->pair_guest_of[slot] = 0;
+  // pairs: a pairable launch right after a host with an open seat on the same rows becomes its guest; a
+  // pairable launch that is not a guest opens its own seat
+  const bool guest = pairable && prev.seat_open && prev.rows == a.scan.rows && prev.n_virtual == a.scan.n_virtual;
+  ser.launch[slot] = StbSeriesLaunch{tag, a.scan.t_base, plan.t_bulk, plan.n_tickets, overlapped, guest ? prev_slot : -1,
+                                     a.scan.rows, SRC, a.scan.n_virtual, tiles, pairable && !guest};
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;   // PDL, see the kernel
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   if (guest) {
-    unsigned long long *seat = ctx->pair_seats + (size_t)ph.slot * STB_SEAT_WORDS;
+    unsigned long long *seat = ser.seats + (size_t)prev_slot * STB_SEAT_WORDS;
     StbPairJoinArgs j;
     j.seat = seat;
-    j.tickets = ctx->tickets + ph.slot;
-    j.t_base = ph.t_base;
-    j.n_tickets = ph.n_tickets;
-    j.v_floor = ctx->pair_floor;
+    j.tickets = ser.tickets + prev_slot;
+    j.t_base = prev.t_base;
+    j.n_tickets = prev.n_tickets;
+    j.v_floor = ser.pair_floor;
     j.q = a.scan.q; j.hits = a.out_hits; j.status = a.out_status; j.top_k = a.top_k;
-    j.thr = a.q4.thr; j.q4_tag = a.q4.tag; j.tag = a.q4.tag;
+    j.thr = a.q4.thr; j.tag = tag;
     a.pair.decided = seat + STB_SEAT_DECIDED;
-    a.pair.tag = a.q4.tag;
-    a.pair.booked = n_tickets + warps_total;
-    ctx->ticket_next[ph.slot] += STB_PAIR_JUMP;    // the join's jump (a refusing join adds it after the host)
-    ctx->pair_guest_of[slot] = (uint32_t)ph.slot + 1;
-    ctx->pair_guest_tag[slot] = a.q4.tag;
+    a.pair.tag = tag;
+    a.pair.booked = plan.n_tickets + warps_total;
+    ser.ticket_next[prev_slot] += STB_PAIR_JUMP;    // the join's jump (a refusing join adds it after the host)
     cudaLaunchConfig_t jc;
     memset(&jc, 0, sizeof(jc));
     jc.gridDim = dim3(1);
@@ -1609,18 +1601,10 @@ static int stb_launch_topk_t(stb_ctx *ctx, const TopkArgs &a_in, bool overlapped
     STB_CUDA(cudaLaunchKernelEx(&jc, stb_pair_join_kernel, j));
     ctx->kernel_launches++;
   } else if (pairable) {
-    // the guest's tail merges its lists through the second half of the scratch
-    if (2 * need_keys > ctx->block_keys.cap || 2 * (grid + 8) > ctx->counters.cap) {
-      stb_set_error("scan scratch too small for a pair (grid=%llu)", (unsigned long long)grid);
-      return STB_ERR_STATE;
-    }
-    a.pair.seat = ctx->pair_seats + (size_t)slot * STB_SEAT_WORDS;
+    a.pair.seat = ser.seats + (size_t)slot * STB_SEAT_WORDS;
     a.pair.keys2 = ctx->block_keys + need_keys;
     a.pair.counters2 = ctx->counters + grid + 8;
-    ph.rows = a.scan.rows; ph.n_virtual = a.scan.n_virtual; ph.slot = slot;
-    ph.t_base = a.scan.t_base; ph.n_tickets = n_tickets; ph.open = true;
   }
-  ctx->pair_t_bulk[slot] = a.scan.t_bulk;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3((unsigned)grid);
@@ -1676,21 +1660,111 @@ int stb_launch_scan_topk(stb_ctx *ctx, const stb_corpus *c, int tier, const floa
   memset(&a.q4, 0, sizeof(a.q4));
   if (tier == STB_TIER_Q8 && (top_k > STB_Q8_MAX_K || !c->q8 || !c->q4)) { stb_set_error("scan_topk: q8 tier unavailable"); return STB_ERR_STATE; }
   if (tier == STB_TIER_Q8) {
-    // a fresh tag per launch, slots in turn (stb_scan_q4); after 2^32 launches the words are cleared once
-    if ((uint32_t)++ctx->q4_launches == 0) {
-      STB_CUDA(cudaMemsetAsync(ctx->q4_thr, 0, STB_TICKET_SLOTS * STB_Q4_WORDS * sizeof(unsigned long long), ctx->stream));
-      STB_CUDA(cudaMemsetAsync(ctx->pair_seats, 0, STB_TICKET_SLOTS * STB_SEAT_WORDS * sizeof(unsigned long long), ctx->stream));
-      ++ctx->q4_launches;
-    }
-    a.q4.plane = c->q4;
+    a.q4.plane = c->q4;   // its threshold words and tag: the launch's slot of the series (stb_launch_topk_t)
     a.q4.sr = c->q4_sr;
-    a.q4.thr = ctx->q4_thr + (ctx->q4_launches % STB_TICKET_SLOTS) * STB_Q4_WORDS;
-    a.q4.tag = (uint32_t)ctx->q4_launches;
     a.q4.top_k = top_k > 0 ? top_k : 1;
     a.q4.refined = ctx->q4_refined;
   }
   if (tier == STB_TIER_H16 && !c->shadow) { stb_set_error("scan_topk: h16 tier unavailable"); return STB_ERR_STATE; }
   return n_ranges > 0 ? stb_launch_topk_r<1>(ctx, a, tier, top_k, overlapped) : stb_launch_topk_r<0>(ctx, a, tier, top_k, overlapped);
+}
+
+// ---- the series of top-k launches (StbScanSeries, common.cuh) ----------------------------------------------
+int StbScanSeries::init(cudaStream_t stream) {
+  int rc;
+  if ((rc = tickets.alloc(STB_TICKET_SLOTS)) != STB_OK || (rc = coscan_off.alloc(STB_TICKET_SLOTS)) != STB_OK ||
+      (rc = q4_thr.alloc(STB_TICKET_SLOTS * STB_Q4_WORDS)) != STB_OK || (rc = seats.alloc(STB_TICKET_SLOTS * STB_SEAT_WORDS)) != STB_OK)
+    return rc;
+  return reset(stream);
+}
+
+int StbScanSeries::reset(cudaStream_t stream) {
+  for (StbBuf<unsigned long long> *b : {&tickets, &coscan_off, &q4_thr, &seats})
+    STB_CUDA(cudaMemsetAsync(*b, 0, b->cap * sizeof(unsigned long long), stream));
+  memset(ticket_next, 0, sizeof(ticket_next));
+  memset(launch, 0, sizeof(launch));
+  return STB_OK;
+}
+
+void StbScanSeries::forget_rows(const void *rows, bool rewritten) {
+  StbSeriesLaunch &last = launch[launches % STB_TICKET_SLOTS];
+  if (last.rows != rows) return;
+  last.seat_open = false;                // a guest after this starts its own pair
+  if (rewritten) last.rows = nullptr;    // the next co-scan starts at tile 0
+}
+
+// The slot of the launch `back` launches before the last one (back < STB_TICKET_SLOTS), -1 if there was none.
+static int stb_series_recent(const StbScanSeries &s, uint32_t back) {
+  if (s.launches <= back) return -1;
+  const uint64_t n = s.launches - back;
+  const uint32_t tag = s.launch[n % STB_TICKET_SLOTS].tag;
+  return tag != 0 && tag == (uint32_t)n ? (int)(n % STB_TICKET_SLOTS) : -1;
+}
+
+// K1's tile tickets: every top-k launch must advance the device counter by exactly what the host
+// booked for it (n_tickets + total_warps); a mismatch would make later launches skip or repeat
+// tiles.  Synchronises; returns STB_ERR_STATE on a mismatch.
+int stb_debug_ticket_check(stb_ctx *ctx, uint64_t *device_value, uint64_t *host_value) {
+  int rc = stb_ctx_use(ctx);
+  if (rc) return rc;
+  const StbScanSeries &s = ctx->series;
+  unsigned long long v[STB_TICKET_SLOTS];
+  STB_CUDA(cudaStreamSynchronize(ctx->stream));
+  STB_CUDA(cudaMemcpy(v, s.tickets, sizeof(v), cudaMemcpyDeviceToHost));
+  unsigned long long dsum = 0, hsum = 0;
+  int bad = -1;
+  for (int i = 0; i < STB_TICKET_SLOTS; ++i) { dsum += v[i]; hsum += s.ticket_next[i]; if (v[i] != s.ticket_next[i] && bad < 0) bad = i; }
+  if (device_value) *device_value = dsum;          // sums over the slots
+  if (host_value) *host_value = hsum;
+  if (bad >= 0) { stb_set_error("ticket counter %d is %llu, host expects %llu", bad, v[bad], s.ticket_next[bad]); return STB_ERR_STATE; }
+  return STB_OK;
+}
+
+// The tile offsets K1's last n top-k launches started their pass at, oldest first; 0xffffffff for a launch
+// that did not co-scan.  Synchronises.
+int stb_debug_coscan_offsets(stb_ctx *ctx, uint32_t n, uint32_t *out) {
+  int rc = stb_ctx_use(ctx);
+  if (rc) return rc;
+  if (n > STB_TICKET_SLOTS || (n && !out)) { stb_set_error("coscan_offsets: n must be 0..%d", STB_TICKET_SLOTS); return STB_ERR_ARG; }
+  unsigned long long w[STB_TICKET_SLOTS];
+  STB_CUDA(cudaStreamSynchronize(ctx->stream));
+  STB_CUDA(cudaMemcpy(w, ctx->series.coscan_off, sizeof(w), cudaMemcpyDeviceToHost));
+  for (uint32_t i = 0; i < n; ++i) {
+    out[i] = 0xffffffffu;
+    const int k = stb_series_recent(ctx->series, n - 1 - i);
+    if (k >= 0 && ctx->series.launch[k].coscan && (uint32_t)(w[k] >> 32) == ctx->series.launch[k].tag) out[i] = (uint32_t)w[k];
+  }
+  return STB_OK;
+}
+
+// Where K1's last n top-k launches joined their host, oldest first: the join tile (the first tile of the join
+// ticket), -1 for a launch that was not a guest, -2 for a guest whose join was refused.  Synchronises.
+int stb_debug_pair_joins(stb_ctx *ctx, uint32_t n, int64_t *out) {
+  int rc = stb_ctx_use(ctx);
+  if (rc) return rc;
+  if (n > STB_TICKET_SLOTS || (n && !out)) { stb_set_error("pair_joins: n must be 0..%d", STB_TICKET_SLOTS); return STB_ERR_ARG; }
+  unsigned long long w[STB_TICKET_SLOTS * STB_SEAT_WORDS];
+  STB_CUDA(cudaStreamSynchronize(ctx->stream));
+  STB_CUDA(cudaMemcpy(w, ctx->series.seats, sizeof(w), cudaMemcpyDeviceToHost));
+  for (uint32_t i = 0; i < n; ++i) {
+    out[i] = -1;
+    const int k = stb_series_recent(ctx->series, n - 1 - i);
+    if (k < 0) continue;
+    const StbSeriesLaunch &r = ctx->series.launch[k];
+    if (r.host < 0) continue;
+    const unsigned long long d = w[r.host * STB_SEAT_WORDS + STB_SEAT_DECIDED];
+    if ((uint32_t)(d >> 32) != r.tag) continue;                         // a later pair reused the seat
+    out[i] = d & 0x80000000ull ? (int64_t)stb_ticket_first_tile((uint32_t)d & 0x7fffffffu, r.t_bulk) : -2;
+  }
+  return STB_OK;
+}
+
+// Test hook: a join waits until its host has drawn v_floor tickets (0: joins as early as it runs).
+int stb_debug_pair_floor(stb_ctx *ctx, uint64_t v_floor) {
+  int rc = stb_ctx_use(ctx);
+  if (rc) return rc;
+  ctx->series.pair_floor = v_floor;
+  return STB_OK;
 }
 
 // ------------------------------------------------------------------ collect path ---

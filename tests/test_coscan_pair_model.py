@@ -13,7 +13,7 @@ WARPS_PER_CTA = 8
 
 
 def plan(tiles, warps):
-    """stb_launch_topk_t: bulk tickets of TICKET_TILES tiles, then the last ~2 tiles per warp one by one."""
+    """stb_ticket_plan: bulk tickets of TICKET_TILES tiles, then the last ~2 tiles per warp one by one."""
     single = min(tiles, 2 * warps)
     t_bulk = (tiles - single) // TICKET_TILES
     n_tickets = t_bulk + (tiles - t_bulk * TICKET_TILES)
