@@ -655,8 +655,10 @@ int stb_ivfpq_search_filtered(stb_ivfpq *index, const float *q, uint32_t nq, uin
  *  - Launches: the queries in caller order, at most 4096 per launch and no more distinct subsets than
  *    STB_IVFPQ_SUBSET_SCRATCH holds (each takes an eligible-row bitmap of ceil(rows / 32) words and nlist
  *    counts; a launch holds at least one query).  Each launch: one bitmap launch and one count launch for
- *    all its subsets, the four batched kernels, one synchronisation.  The scratch belongs to the index and
- *    grows on demand.
+ *    all its subsets, the four batched kernels, one synchronisation.  The bitmap and count launches are
+ *    skipped when the previous launch of the same call named exactly the same subsets, in the same order of
+ *    first appearance: the scratch still holds their bitmaps and counts.  The scratch belongs to the index
+ *    and grows on demand.
  * stb_debug_ivfpq_batch_last describes the call's last launch: slot j is the j-th query of that launch
  * (in caller order, queries of empty subsets skipped). */
 int stb_ivfpq_search_subsets(stb_ivfpq *index, const float *q, uint32_t nq, uint32_t nprobe, uint32_t top_k,

@@ -490,7 +490,7 @@ int stb_launch_batch_xchg(stb_ctx *ctx, const StbBatchXchgArgs &a, const stb_hit
                           stb_hit *out_hits, uint32_t *out_status);
 
 // opt-in to > 48 KiB dynamic shared memory (or another function attribute) once per context
-enum { STB_ATTR_GEMM0 = 0, STB_ATTR_GEMM1, STB_ATTR_MERGE, STB_ATTR_IVF_PROBE, STB_ATTR_IVF_V2, STB_ATTR_FINISH2,
+enum { STB_ATTR_GEMM0 = 0, STB_ATTR_GEMM1, STB_ATTR_MERGE, STB_ATTR_IVF_V2, STB_ATTR_FINISH2,
        STB_ATTR_IVF_BATCH, STB_ATTR_GEMM0F, STB_ATTR_GEMM1F, STB_ATTR_GEMM2, STB_ATTR_GEMM0W, STB_ATTR_GEMM1W,
        STB_ATTR_Q8GEMM0, STB_ATTR_Q8GEMM1, STB_ATTR_Q8GEMM2, STB_ATTR_THRESH_BIG,
        STB_ATTR_Q8GEMM0F, STB_ATTR_Q8GEMM1F, STB_ATTR_Q8GEMM3 };

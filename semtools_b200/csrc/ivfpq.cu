@@ -488,47 +488,9 @@ __device__ __forceinline__ float ivf_adc_sum(const float *s_lut, uint4 c0, uint4
 }
 
 // ------------------------------------------------------------------ query kernels -----
-// coarse[j] = q^ . c_j   (warp per centroid)
-__global__ void ivf_coarse_kernel(const float *C, uint32_t nlist, const float *q, float *coarse) {
-  const int lane = threadIdx.x & 31;
-  const uint32_t c = blockIdx.x * 8 + (threadIdx.x >> 5);
-  if (c >= nlist) return;
-  const float4 *cr = reinterpret_cast<const float4 *>(C + (size_t)c * STB_D), *q4 = reinterpret_cast<const float4 *>(q);
-  const float4 a0 = __ldg(cr + 2 * lane), a1 = __ldg(cr + 2 * lane + 1), b0 = __ldg(q4 + 2 * lane), b1 = __ldg(q4 + 2 * lane + 1);
-  float d, qq;
-  ivf_coarse_dot(a0, a1, b0, b1, d, qq);
-  if (lane == 0) coarse[c] = ivf_coarse_score(d, qq);
-}
-
-// one CTA: top-nprobe lists (bitonic sort of <= 8192 keys), prefix of their lengths, LUT
-__global__ void __launch_bounds__(1024)
-ivf_probe_lut_kernel(const float *coarse, uint32_t nlist, uint32_t nprobe, const uint32_t *list_off, const float *cb,
-                     const float *q, uint32_t *probe, float *lut) {
-  extern __shared__ uint64_t skeys[];   // npow2 keys
-  __shared__ float sq[STB_D];
-  __shared__ float s_inv;
-  uint32_t npow = 1; while (npow < nlist) npow <<= 1;
-  for (uint32_t i = threadIdx.x; i < npow; i += blockDim.x)
-    skeys[i] = (i < nlist) ? stb_make_key(coarse[i], i) : STB_KEY_INVALID;
-  if (threadIdx.x < STB_D) sq[threadIdx.x] = q[threadIdx.x];
-  __syncthreads();
-  if (threadIdx.x == 0) s_inv = ivf_query_inv(sq);
-  stb_cta_sort_keys_strided(skeys, npow);
-  // probe[0..nprobe) = list ids (best first); probe[nprobe_max .. ] = prefix of list lengths
-  if (threadIdx.x == 0) {
-    uint32_t acc = 0;
-    for (uint32_t p = 0; p < nprobe; ++p) {
-      const uint32_t l = stb_key_row(skeys[p]);
-      probe[p] = l;
-      probe[nprobe + p] = acc;
-      acc += list_off[l + 1] - list_off[l];
-    }
-    probe[2 * nprobe] = acc;
-  }
-  const float inv = s_inv;
-  for (int i = threadIdx.x; i < PQ_M * PQ_KSUB; i += blockDim.x) lut[i] = ivf_lut_entry(sq, inv, cb, i);
-}
-
+// The multi-launch single search (v1) takes its coarse scores, probe list and LUT from the batched
+// search's probe stage at nq = 1 (ivfb_probe, below).
+//
 // ADC scan over the probed lists: lane = one code (32 bytes); score = coarse[list] + sum LUT.
 // Rows are dealt to warps 32 at a time round-robin (a list's -- i.e. a cluster's -- rows
 // spread over all warps); each warp keeps its 64 best in registers (same running top-K'
@@ -1161,9 +1123,9 @@ ivfb_finish_kernel(const IvfbArgs a) {
 }
 
 // ------------------------------------------------------------------ filtered search ------
-// The eligibility pass of stb_ivfpq_search_filtered (one subset, shared by every query of the call) and of
-// stb_ivfpq_search_subsets (every distinct subset of a launch), two launches whatever the subset count;
-// grid row y = subset y, whose bitmap is bitmap + y * n_words and whose counts are elig + y * nlist:
+// The eligibility pass of a filtered launch of the host batch search (ivfb_host_search: every distinct subset of
+// the launch), two launches whatever the subset count; grid row y = subset y, whose bitmap is
+// bitmap + y * n_words and whose counts are elig + y * nlist:
 //   ivff_bitmap_kernel  bit r of the bitmap = local row r lies in one of the subset's clipped ranges (thread
 //                       per 32-row word: a binary search for the first range ending past the word, then the
 //                       at most 32 non-empty ranges that touch it); subset y's ranges are the pairs
@@ -1721,6 +1683,19 @@ static int ivf_fused_launch(stb_ivfpq *x, const float *q_dev, uint32_t nprobe, u
   return STB_OK;
 }
 
+// The query entry points' argument rule: nprobe to [1, min(nlist, 1024)], rerank to [top_k, rerank_cap].
+static void ivf_clamp(const stb_ivfpq *x, uint32_t top_k, uint32_t rerank_cap, uint32_t &nprobe, uint32_t &rerank) {
+  nprobe = std::max(1u, std::min(std::min(nprobe, x->nlist), 1024u));
+  rerank = std::max(top_k, std::min(rerank, rerank_cap));
+}
+
+// Queries [i0, i0 + n) of a host form that nothing can answer: 0 hits, 0 codes scanned, hits padded.
+static void ivf_answer_none(stb_hit *out_hits, uint32_t *out_n, uint64_t *out_scanned, uint32_t i0, uint32_t n,
+                            uint32_t top_k) {
+  for (uint32_t i = i0; i < i0 + n; ++i) { out_n[i] = 0; if (out_scanned) out_scanned[i] = 0; }
+  if (top_k) stb_pad_hits(out_hits + (size_t)i0 * top_k, 0, (uint64_t)n * top_k);
+}
+
 // Asynchronous device-resident form (sharded use: per-rank probe -> all-gather of k hits -> stb_hits_merge_dev).
 // out_hits_dev receives top_k entries (unused tail: +inf / UINT64_MAX), out_status_dev[0] = hits, [1] = codes scanned.
 int stb_ivfpq_search_dev(stb_ivfpq *x, const float *q_dev, uint32_t nprobe, uint32_t top_k, uint32_t rerank,
@@ -1728,8 +1703,7 @@ int stb_ivfpq_search_dev(stb_ivfpq *x, const float *q_dev, uint32_t nprobe, uint
   if (!x || !q_dev || !out_hits_dev || !out_status_dev) { stb_set_error("ivfpq_search_dev: null argument"); return STB_ERR_ARG; }
   if (cudaSetDevice(x->ctx->device) != cudaSuccess) { stb_set_error("cudaSetDevice failed"); return STB_ERR_CUDA; }
   if (top_k == 0 || top_k > 1024) { stb_set_error("ivfpq_search_dev: top_k must be 1..1024"); return STB_ERR_ARG; }
-  nprobe = std::max(1u, std::min(std::min(nprobe, x->nlist), 1024u));
-  rerank = std::max(top_k, std::min(rerank, (uint32_t)ADC2_RERANK_CAP));
+  ivf_clamp(x, top_k, ADC2_RERANK_CAP, nprobe, rerank);
   return ivf_fused_launch(x, q_dev, nprobe, top_k, rerank, out_hits_dev, out_status_dev);
 }
 
@@ -1761,14 +1735,12 @@ struct IvfbFilter {
   uint64_t bm_words;          // bitmap words per subset
 };
 
-// four launches for 1 <= nq <= IVFB_MAX_NQ queries (arguments already clamped); asynchronous.
-// f != NULL: the filtered search's instantiations of the probe, scan and finish kernels.
-static int ivfb_launch(stb_ivfpq *x, const float *q_dev, uint32_t nq, uint32_t nprobe, uint32_t top_k, uint32_t rerank,
-                       stb_hit *out_hits_dev, uint32_t *out_status_dev, const IvfbFilter *f = nullptr) {
+// The probe stage of nq queries q_dev [nq][256] (two launches, asynchronous): coarse scores [nq][nlist], then per
+// query its probe list (IVFB_PROBE_STRIDE apart) and LUT [32][256].  f != NULL: the FILTER instantiation.
+static int ivfb_probe(stb_ivfpq *x, const float *q_dev, uint32_t nq, uint32_t nprobe, float *coarse, uint32_t *probe,
+                      float *lut, const IvfbFilter *f) {
   stb_ctx *ctx = x->ctx;
   cudaStream_t st = ctx->stream;
-  int rc = ivfb_reserve(x, nq);
-  if (rc != STB_OK) return rc;
   uint32_t npow2 = 1; while (npow2 < x->nlist) npow2 <<= 1;
   if (!(ctx->func_attr_mask & (1u << STB_ATTR_IVF_BATCH))) {
     STB_CUDA(cudaFuncSetAttribute(ivfb_probe_lut_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 8));
@@ -1777,6 +1749,28 @@ static int ivfb_launch(stb_ivfpq *x, const float *q_dev, uint32_t nq, uint32_t n
     STB_CUDA(cudaFuncSetAttribute(ivfb_finish_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, IVFB_FIN_SMEM));
     ctx->func_attr_mask |= 1u << STB_ATTR_IVF_BATCH;
   }
+  ivfb_coarse_kernel<<<dim3((x->nlist + 31) / 32, (nq + IVFB_QTILE - 1) / IVFB_QTILE), 1024, 0, st>>>(x->centroids, x->nlist, q_dev,
+                                                                                                   nq, coarse);
+  STB_CUDA(cudaGetLastError());
+  if (!f)
+    ivfb_probe_lut_kernel<false><<<nq, 1024, npow2 * 8, st>>>(coarse, x->nlist, nprobe, x->list_off, x->codebooks, q_dev, probe,
+                                                              lut, nullptr, nullptr);
+  else
+    ivfb_probe_lut_kernel<true><<<nq, 1024, npow2 * 8, st>>>(coarse, x->nlist, nprobe, x->list_off, x->codebooks, q_dev, probe,
+                                                             lut, f->elig, f->slot_set);
+  STB_CUDA(cudaGetLastError());
+  ctx->kernel_launches += 2;
+  return STB_OK;
+}
+
+// four launches for 1 <= nq <= IVFB_MAX_NQ queries (arguments already clamped); asynchronous.
+// f != NULL: the filtered search's instantiations of the probe, scan and finish kernels.
+static int ivfb_launch(stb_ivfpq *x, const float *q_dev, uint32_t nq, uint32_t nprobe, uint32_t top_k, uint32_t rerank,
+                       stb_hit *out_hits_dev, uint32_t *out_status_dev, const IvfbFilter *f = nullptr) {
+  stb_ctx *ctx = x->ctx;
+  cudaStream_t st = ctx->stream;
+  int rc = ivfb_reserve(x, nq);
+  if (rc != STB_OK) return rc;
   IvfbArgs a;
   // STB_IVFPQ_BATCH_KEEP=k (1..64): each scan warp keeps only k codes (tests drive the exact slow route)
   const char *keep_env = getenv("STB_IVFPQ_BATCH_KEEP");
@@ -1788,34 +1782,21 @@ static int ivfb_launch(stb_ivfpq *x, const float *q_dev, uint32_t nq, uint32_t n
   a.forced = x->forced; a.n_forced = x->n_forced; a.out_hits = out_hits_dev; a.out_status = out_status_dev;
   a.bitmap = f ? f->bitmap : nullptr; a.max_dist = f ? f->max_dist : STB_DEFAULT_MAX_DIST;
   a.slot_set = f ? f->slot_set : nullptr; a.bm_words = f ? f->bm_words : 0;
-  ivfb_coarse_kernel<<<dim3((x->nlist + 31) / 32, (nq + IVFB_QTILE - 1) / IVFB_QTILE), 1024, 0, st>>>(x->centroids, x->nlist, q_dev,
-                                                                                                   nq, x->b_coarse);
-  STB_CUDA(cudaGetLastError());
+  if ((rc = ivfb_probe(x, q_dev, nq, nprobe, x->b_coarse, x->b_probe, x->b_lut, f)) != STB_OK) return rc;
   if (!f) {
-    ivfb_probe_lut_kernel<false><<<nq, 1024, npow2 * 8, st>>>(x->b_coarse, x->nlist, nprobe, x->list_off, x->codebooks, q_dev,
-                                                              x->b_probe, x->b_lut, nullptr, nullptr);
-    STB_CUDA(cudaGetLastError());
     ivfb_scan_kernel<false><<<dim3(IVFB_SCAN_CTAS, nq), IVFB_SCAN_THREADS, 0, st>>>(a);
     STB_CUDA(cudaGetLastError());
     ivfb_finish_kernel<false><<<nq, IVFB_FIN_THREADS, IVFB_FIN_SMEM, st>>>(a);
   } else {
-    ivfb_probe_lut_kernel<true><<<nq, 1024, npow2 * 8, st>>>(x->b_coarse, x->nlist, nprobe, x->list_off, x->codebooks, q_dev,
-                                                             x->b_probe, x->b_lut, f->elig, f->slot_set);
-    STB_CUDA(cudaGetLastError());
     ivfb_scan_kernel<true><<<dim3(IVFB_SCAN_CTAS, nq), IVFB_SCAN_THREADS, 0, st>>>(a);
     STB_CUDA(cudaGetLastError());
     ivfb_finish_kernel<true><<<nq, IVFB_FIN_THREADS, IVFB_FIN_SMEM, st>>>(a);
   }
   STB_CUDA(cudaGetLastError());
-  ctx->kernel_launches += 4;
+  ctx->kernel_launches += 2;
   x->last_info[0] = nq; x->last_info[1] = nprobe; x->last_info[2] = top_k; x->last_info[3] = rerank;
   x->last_filtered = f != nullptr;
   return STB_OK;
-}
-
-static void ivfb_clamp(const stb_ivfpq *x, uint32_t top_k, uint32_t &nprobe, uint32_t &rerank) {
-  nprobe = std::max(1u, std::min(std::min(nprobe, x->nlist), 1024u));
-  rerank = std::max(top_k, std::min(rerank, (uint32_t)IVFB_RERANK_CAP));
 }
 
 int stb_ivfpq_search_batch_dev(stb_ivfpq *x, const float *q_dev, uint32_t nq, uint32_t nprobe, uint32_t top_k,
@@ -1826,32 +1807,116 @@ int stb_ivfpq_search_batch_dev(stb_ivfpq *x, const float *q_dev, uint32_t nq, ui
   if (top_k == 0 || top_k > 1024) { stb_set_error("ivfpq_search_batch_dev: top_k must be 1..1024"); return STB_ERR_ARG; }
   if (nq > IVFB_MAX_NQ) { stb_set_error("ivfpq_search_batch_dev: nq must be <= %u", (unsigned)IVFB_MAX_NQ); return STB_ERR_ARG; }
   if (cudaSetDevice(x->ctx->device) != cudaSuccess) { stb_set_error("cudaSetDevice failed"); return STB_ERR_CUDA; }
-  ivfb_clamp(x, top_k, nprobe, rerank);
+  ivf_clamp(x, top_k, IVFB_RERANK_CAP, nprobe, rerank);
   return ivfb_launch(x, q_dev, nq, nprobe, top_k, rerank, out_hits_dev, out_status_dev);
 }
 
-// The host forms' chunk loop (arguments checked and clamped, top_k >= 1): chunks of IVFB_MAX_NQ queries,
-// one synchronisation each.
-static int ivfb_host_chunks(stb_ivfpq *x, const float *q, uint32_t nq, uint32_t nprobe, uint32_t top_k, uint32_t rerank,
-                            stb_hit *out_hits, uint32_t *out_n, uint64_t *out_scanned, const IvfbFilter *f) {
-  cudaStream_t st = x->ctx->stream;
-  std::vector<uint32_t> status;
-  for (uint32_t q0 = 0; q0 < nq; q0 += IVFB_MAX_NQ) {   // one synchronisation per chunk
-    const uint32_t m = std::min<uint32_t>(IVFB_MAX_NQ, nq - q0);
-    int rc = ivfb_reserve(x, m);
-    if (rc != STB_OK) return rc;
-    STB_CUDA(cudaMemcpyAsync(x->b_q, q + (size_t)q0 * STB_D, (size_t)m * STB_D * 4, cudaMemcpyHostToDevice, st));
-    if ((rc = ivfb_launch(x, x->b_q, m, nprobe, top_k, rerank, x->b_hits, x->b_status, f)) != STB_OK) return rc;
+// The subsets of a host batch search.  filter false: no filter (the unfiltered instantiations).  Otherwise subset s
+// is the clipped local pairs [off[s], off[s+1]) of loc, back to back (off empty: one subset, every indexed row, with
+// no bitmap); query i searches subset subset_of[i] (NULL: subset 0); a hit needs distance < max_dist.
+struct IvfbSubsets {
+  bool filter = false;
+  double max_dist = STB_DEFAULT_MAX_DIST;
+  std::vector<uint32_t> loc;
+  std::vector<uint64_t> off;
+  const uint32_t *subset_of = nullptr;
+  IvfbSubsets() = default;
+  IvfbSubsets(int has_max, double max_distance)   // the distance limit as stb_search sets it
+      : filter(true), max_dist(has_max ? std::min(max_distance, STB_DEFAULT_MAX_DIST) : STB_DEFAULT_MAX_DIST) {}
+};
+
+// The host forms' one loop (arguments checked, subsets clipped).  Launches take the queries in caller order, at most
+// IVFB_MAX_NQ of them and as many distinct subsets as STB_IVFPQ_SUBSET_SCRATCH holds; a query of an empty subset is
+// answered here and takes no part.  Each launch: the eligibility pass of its subsets, the four batched kernels, one
+// synchronisation.  The pass is skipped when the previous launch of the call had the same subsets in the same slots,
+// whose bitmaps and counts the scratch still holds.  A launch of consecutive caller rows reads q and writes out_hits
+// in place; any other gathers its queries and scatters its hits.
+static int ivfb_host_search(stb_ivfpq *x, const float *q, uint32_t nq, uint32_t nprobe, uint32_t top_k, uint32_t rerank,
+                            const IvfbSubsets &s, stb_hit *out_hits, uint32_t *out_n, uint64_t *out_scanned) {
+  if (top_k == 0) { ivf_answer_none(out_hits, out_n, out_scanned, 0, nq, 0); return STB_OK; }
+  stb_ctx *ctx = x->ctx;
+  if (cudaSetDevice(ctx->device) != cudaSuccess) { stb_set_error("cudaSetDevice failed"); return STB_ERR_CUDA; }
+  ivf_clamp(x, top_k, IVFB_RERANK_CAP, nprobe, rerank);
+  cudaStream_t st = ctx->stream;
+  const bool bitmap = !s.off.empty();
+  const uint64_t words = (x->n + 31) / 32;
+  const uint64_t set_cap = std::max<uint64_t>(1, STB_IVFPQ_SUBSET_SCRATCH / ((words + x->nlist) * 4));
+  int rc;
+  if (!s.loc.empty()) {
+    if ((rc = x->f_ranges.reserve(s.loc.size(), 2048)) != STB_OK) return rc;
+    STB_CUDA(cudaMemcpyAsync(x->f_ranges, s.loc.data(), s.loc.size() * 4, cudaMemcpyHostToDevice, st));
+  }
+  IvfbFilter f;
+  f.max_dist = s.max_dist; f.bm_words = words;
+  std::vector<uint32_t> local(bitmap ? s.off.size() - 1 : 1, UINT32_MAX), qrow, slot_set, sets, prev_sets, status;
+  std::vector<uint64_t> set_off;                                 // per subset of the launch: [begin, end) pairs
+  std::vector<float> qc;
+  std::vector<stb_hit> hits;
+  for (uint32_t i = 0; i < nq;) {
+    qrow.clear(); slot_set.clear(); sets.clear();
+    for (; i < nq && qrow.size() < IVFB_MAX_NQ; ++i) {
+      const uint32_t si = s.subset_of ? s.subset_of[i] : 0;
+      if (bitmap && s.off[si] == s.off[si + 1]) { ivf_answer_none(out_hits, out_n, out_scanned, i, 1, top_k); continue; }
+      if (local[si] == UINT32_MAX) {
+        if (sets.size() == set_cap) break;
+        local[si] = (uint32_t)sets.size();
+        sets.push_back(si);
+      }
+      qrow.push_back(i); slot_set.push_back(local[si]);
+    }
+    const uint32_t m = (uint32_t)qrow.size(), n_sets = (uint32_t)sets.size();
+    if (m == 0) break;
+    for (uint32_t si : sets) local[si] = UINT32_MAX;
+    const bool run = qrow[m - 1] - qrow[0] == m - 1;            // consecutive caller rows
+    if ((rc = ivfb_reserve(x, m)) != STB_OK) return rc;
+    const float *qs = q + (size_t)qrow[0] * STB_D;
+    if (!run) {
+      qc.resize((size_t)m * STB_D);
+      for (uint32_t j = 0; j < m; ++j) memcpy(qc.data() + (size_t)j * STB_D, q + (size_t)qrow[j] * STB_D, STB_D * sizeof(float));
+      qs = qc.data();
+    }
+    STB_CUDA(cudaMemcpyAsync(x->b_q, qs, (size_t)m * STB_D * sizeof(float), cudaMemcpyHostToDevice, st));
+    if (s.filter && sets != prev_sets) {
+      // the eligibility pass of every subset of the launch: one bitmap launch, one count launch
+      if ((rc = x->f_elig.reserve((size_t)n_sets * x->nlist)) != STB_OK) return rc;
+      if (bitmap) {
+        set_off.clear();
+        for (uint32_t si : sets) { set_off.push_back(s.off[si]); set_off.push_back(s.off[si + 1]); }
+        if ((rc = x->f_bitmap.reserve((size_t)n_sets * words)) != STB_OK || (rc = x->f_set_off.reserve(set_off.size(), 512)) != STB_OK)
+          return rc;
+        STB_CUDA(cudaMemcpyAsync(x->f_set_off, set_off.data(), set_off.size() * 8, cudaMemcpyHostToDevice, st));
+        if ((rc = stb_launch_row_bitmap(ctx, x->f_ranges, 0, words, x->f_bitmap, n_sets, x->f_set_off)) != STB_OK) return rc;
+      }
+      ivff_elig_kernel<<<dim3((x->nlist + 7) / 8, n_sets), 256, 0, st>>>(x->list_off, x->order, x->nlist,
+                                                                        bitmap ? x->f_bitmap.p : nullptr, words, x->f_elig);
+      STB_CUDA(cudaGetLastError());
+      ctx->kernel_launches += 1;
+      prev_sets = sets;
+    }
+    if (s.filter) {
+      f.bitmap = bitmap ? x->f_bitmap.p : nullptr; f.elig = x->f_elig; f.slot_set = nullptr;
+      if (n_sets > 1) {                                          // one subset: every slot reads subset 0
+        if ((rc = x->f_slot_set.reserve(m, 512)) != STB_OK) return rc;
+        STB_CUDA(cudaMemcpyAsync(x->f_slot_set, slot_set.data(), (size_t)m * 4, cudaMemcpyHostToDevice, st));
+        f.slot_set = x->f_slot_set;
+      }
+    }
+    if ((rc = ivfb_launch(x, x->b_q, m, nprobe, top_k, rerank, x->b_hits, x->b_status, s.filter ? &f : nullptr)) != STB_OK)
+      return rc;
+    hits.resize(run ? 0 : (size_t)m * top_k);
     status.resize(2 * (size_t)m);
-    STB_CUDA(cudaMemcpyAsync(out_hits + (size_t)q0 * top_k, x->b_hits, (size_t)m * top_k * sizeof(stb_hit),
+    STB_CUDA(cudaMemcpyAsync(run ? out_hits + (size_t)qrow[0] * top_k : hits.data(), x->b_hits, (size_t)m * top_k * sizeof(stb_hit),
                              cudaMemcpyDeviceToHost, st));
-    STB_CUDA(cudaMemcpyAsync(status.data(), x->b_status, (size_t)m * 2 * 4, cudaMemcpyDeviceToHost, st));
-    STB_CUDA(cudaStreamSynchronize(st));
-    for (uint32_t i = 0; i < m; ++i) {
-      out_n[q0 + i] = status[2 * i];
-      if (out_scanned) out_scanned[q0 + i] = status[2 * i + 1];
+    STB_CUDA(cudaMemcpyAsync(status.data(), x->b_status, status.size() * 4, cudaMemcpyDeviceToHost, st));
+    STB_CUDA(cudaStreamSynchronize(st));                         // also ends the reads of qc, set_off, slot_set
+    for (uint32_t j = 0; j < m; ++j) {
+      const uint32_t r = qrow[j];
+      if (!run) memcpy(out_hits + (size_t)r * top_k, hits.data() + (size_t)j * top_k, top_k * sizeof(stb_hit));
+      out_n[r] = status[2 * j];
+      if (out_scanned) out_scanned[r] = status[2 * j + 1];
     }
   }
+  STB_CUDA(cudaStreamSynchronize(st));                           // `s.loc` is read by the copy above
   return STB_OK;
 }
 
@@ -1861,13 +1926,7 @@ int stb_ivfpq_search_batch(stb_ivfpq *x, const float *q, uint32_t nq, uint32_t n
   if (nq == 0) return STB_OK;
   if (!q || !out_n || (top_k && !out_hits)) { stb_set_error("ivfpq_search_batch: null argument"); return STB_ERR_ARG; }
   if (top_k > 1024) { stb_set_error("ivfpq_search_batch: top_k must be <= 1024"); return STB_ERR_ARG; }
-  if (top_k == 0) {
-    for (uint32_t i = 0; i < nq; ++i) { out_n[i] = 0; if (out_scanned) out_scanned[i] = 0; }
-    return STB_OK;
-  }
-  if (cudaSetDevice(x->ctx->device) != cudaSuccess) { stb_set_error("cudaSetDevice failed"); return STB_ERR_CUDA; }
-  ivfb_clamp(x, top_k, nprobe, rerank);
-  return ivfb_host_chunks(x, q, nq, nprobe, top_k, rerank, out_hits, out_n, out_scanned, nullptr);
+  return ivfb_host_search(x, q, nq, nprobe, top_k, rerank, IvfbSubsets(), out_hits, out_n, out_scanned);
 }
 
 int stb_ivfpq_search_filtered(stb_ivfpq *x, const float *q, uint32_t nq, uint32_t nprobe, uint32_t top_k, uint32_t rerank,
@@ -1878,42 +1937,14 @@ int stb_ivfpq_search_filtered(stb_ivfpq *x, const float *q, uint32_t nq, uint32_
   if (!q || !out_n || (top_k && !out_hits)) { stb_set_error("ivfpq_search_filtered: null argument"); return STB_ERR_ARG; }
   if (n_ranges && !row_ranges) { stb_set_error("ivfpq_search_filtered: row_ranges is null"); return STB_ERR_ARG; }
   if (top_k > 1024) { stb_set_error("ivfpq_search_filtered: top_k must be <= 1024"); return STB_ERR_ARG; }
-  // global ranges -> local [begin, end) pairs clipped to the indexed rows [row_base, row_base + n)
-  std::vector<uint32_t> loc;
+  // one subset: global ranges -> local [begin, end) pairs clipped to the indexed rows [row_base, row_base + n)
+  IvfbSubsets s(has_max, max_distance);
   if (row_ranges) {
-    const int rc = stb_clip_ranges_u32("ivfpq_search_filtered", row_ranges, n_ranges, x->corpus->row_base, x->n, &loc);
+    const int rc = stb_clip_ranges_u32("ivfpq_search_filtered", row_ranges, n_ranges, x->corpus->row_base, x->n, &s.loc);
     if (rc != STB_OK) return rc;
+    s.off = {0, s.loc.size() / 2};
   }
-  if (top_k == 0 || (row_ranges && loc.empty())) {             // nothing can be returned: no launch
-    for (uint32_t i = 0; i < nq; ++i) { out_n[i] = 0; if (out_scanned) out_scanned[i] = 0; }
-    stb_pad_hits(out_hits, 0, (uint64_t)nq * top_k);
-    return STB_OK;
-  }
-  stb_ctx *ctx = x->ctx;
-  if (cudaSetDevice(ctx->device) != cudaSuccess) { stb_set_error("cudaSetDevice failed"); return STB_ERR_CUDA; }
-  ivfb_clamp(x, top_k, nprobe, rerank);
-  cudaStream_t st = ctx->stream;
-  // eligibility pass: bitmap of the eligible rows, eligible codes per list
-  int rc;
-  if ((rc = x->f_elig.reserve(x->nlist)) != STB_OK) return rc;
-  const uint32_t *bitmap = nullptr;
-  if (row_ranges) {
-    const uint64_t words = (x->n + 31) / 32;
-    const uint32_t nr = (uint32_t)(loc.size() / 2);
-    if ((rc = x->f_bitmap.reserve(words)) != STB_OK || (rc = x->f_ranges.reserve(loc.size(), 2048)) != STB_OK) return rc;
-    STB_CUDA(cudaMemcpyAsync(x->f_ranges, loc.data(), loc.size() * 4, cudaMemcpyHostToDevice, st));
-    if ((rc = stb_launch_row_bitmap(ctx, x->f_ranges, nr, words, x->f_bitmap)) != STB_OK) return rc;
-    bitmap = x->f_bitmap;
-  }
-  ivff_elig_kernel<<<(x->nlist + 7) / 8, 256, 0, st>>>(x->list_off, x->order, x->nlist, bitmap, 0, x->f_elig);
-  STB_CUDA(cudaGetLastError());
-  ctx->kernel_launches += 1;
-  IvfbFilter f;
-  f.bitmap = bitmap; f.elig = x->f_elig; f.slot_set = nullptr; f.bm_words = 0;
-  f.max_dist = has_max ? std::min(max_distance, STB_DEFAULT_MAX_DIST) : STB_DEFAULT_MAX_DIST;   // as stb_search
-  rc = ivfb_host_chunks(x, q, nq, nprobe, top_k, rerank, out_hits, out_n, out_scanned, &f);
-  STB_CUDA(cudaStreamSynchronize(st));                         // `loc` is read by the copy above
-  return rc;
+  return ivfb_host_search(x, q, nq, nprobe, top_k, rerank, s, out_hits, out_n, out_scanned);
 }
 
 int stb_ivfpq_search_subsets(stb_ivfpq *x, const float *q, uint32_t nq, uint32_t nprobe, uint32_t top_k, uint32_t rerank,
@@ -1934,92 +1965,18 @@ int stb_ivfpq_search_subsets(stb_ivfpq *x, const float *q, uint32_t nq, uint32_t
   if (subset_offsets[n_subsets] && !row_ranges) { stb_set_error("%s: row_ranges is null", who); return STB_ERR_ARG; }
   for (uint32_t i = 0; i < nq; ++i)
     if (subset_of[i] >= n_subsets) { stb_set_error("%s: query %u names subset %u of %u", who, i, subset_of[i], n_subsets); return STB_ERR_ARG; }
-  // every subset, named or not, validated and clipped as stb_ivfpq_search_filtered does; the clipped local pairs
-  // lie back to back, subset s at pairs [loc_off[s], loc_off[s+1])
-  std::vector<uint32_t> loc;
-  std::vector<uint64_t> loc_off(n_subsets + 1, 0);
-  loc.reserve(2 * subset_offsets[n_subsets]);                  // one allocation: the clipping appends subset by subset
+  // every subset, named or not, validated and clipped as stb_ivfpq_search_filtered does
+  IvfbSubsets sub(has_max, max_distance);
+  sub.off.assign(n_subsets + 1, 0);
+  sub.loc.reserve(2 * subset_offsets[n_subsets]);              // one allocation: the clipping appends subset by subset
   for (uint32_t s = 0; s < n_subsets; ++s) {
     const int rc = stb_clip_ranges_u32(who, row_ranges + 2 * subset_offsets[s], (uint32_t)(subset_offsets[s + 1] - subset_offsets[s]),
-                                       x->corpus->row_base, x->n, &loc);
+                                       x->corpus->row_base, x->n, &sub.loc);
     if (rc != STB_OK) return rc;
-    loc_off[s + 1] = loc.size() / 2;
+    sub.off[s + 1] = sub.loc.size() / 2;
   }
-  if (top_k == 0) {
-    for (uint32_t i = 0; i < nq; ++i) { out_n[i] = 0; if (out_scanned) out_scanned[i] = 0; }
-    return STB_OK;
-  }
-  stb_ctx *ctx = x->ctx;
-  if (cudaSetDevice(ctx->device) != cudaSuccess) { stb_set_error("cudaSetDevice failed"); return STB_ERR_CUDA; }
-  ivfb_clamp(x, top_k, nprobe, rerank);
-  cudaStream_t st = ctx->stream;
-  int rc;
-  if (!loc.empty()) {
-    if ((rc = x->f_ranges.reserve(loc.size(), 2048)) != STB_OK) return rc;
-    STB_CUDA(cudaMemcpyAsync(x->f_ranges, loc.data(), loc.size() * 4, cudaMemcpyHostToDevice, st));
-  }
-  // launches: queries in caller order, at most IVFB_MAX_NQ, and as many distinct subsets as the scratch cap
-  // holds (at least one); a query of an empty subset is answered here and takes no part
-  const uint64_t words = (x->n + 31) / 32;
-  const uint64_t set_cap = std::max<uint64_t>(1, STB_IVFPQ_SUBSET_SCRATCH / ((words + x->nlist) * 4));
-  IvfbFilter f;
-  f.max_dist = has_max ? std::min(max_distance, STB_DEFAULT_MAX_DIST) : STB_DEFAULT_MAX_DIST;   // as stb_search
-  f.bm_words = words;
-  std::vector<uint32_t> local(n_subsets, UINT32_MAX), qrow, slot_set, status;
-  std::vector<uint64_t> set_off;                                 // per subset of the launch: [begin, end) pairs
-  std::vector<float> qc;
-  std::vector<stb_hit> hits;
-  for (uint32_t i = 0; i < nq;) {
-    qrow.clear(); slot_set.clear(); set_off.clear();
-    for (; i < nq && qrow.size() < IVFB_MAX_NQ; ++i) {
-      const uint32_t s = subset_of[i];
-      if (loc_off[s] == loc_off[s + 1]) {
-        out_n[i] = 0;
-        if (out_scanned) out_scanned[i] = 0;
-        stb_pad_hits(out_hits + (size_t)i * top_k, 0, top_k);
-        continue;
-      }
-      if (local[s] == UINT32_MAX) {
-        if (set_off.size() / 2 == set_cap) break;
-        local[s] = (uint32_t)(set_off.size() / 2);
-        set_off.push_back(loc_off[s]); set_off.push_back(loc_off[s + 1]);
-      }
-      qrow.push_back(i); slot_set.push_back(local[s]);
-    }
-    const uint32_t m = (uint32_t)qrow.size(), n_sets = (uint32_t)(set_off.size() / 2);
-    if (m == 0) break;
-    if ((rc = ivfb_reserve(x, m)) != STB_OK || (rc = x->f_bitmap.reserve((size_t)n_sets * words)) != STB_OK ||
-        (rc = x->f_elig.reserve((size_t)n_sets * x->nlist)) != STB_OK || (rc = x->f_set_off.reserve(set_off.size(), 512)) != STB_OK ||
-        (rc = x->f_slot_set.reserve(m, 512)) != STB_OK)
-      return rc;
-    qc.resize((size_t)m * STB_D);
-    for (uint32_t j = 0; j < m; ++j) memcpy(qc.data() + (size_t)j * STB_D, q + (size_t)qrow[j] * STB_D, STB_D * sizeof(float));
-    STB_CUDA(cudaMemcpyAsync(x->b_q, qc.data(), qc.size() * sizeof(float), cudaMemcpyHostToDevice, st));
-    STB_CUDA(cudaMemcpyAsync(x->f_set_off, set_off.data(), set_off.size() * 8, cudaMemcpyHostToDevice, st));
-    STB_CUDA(cudaMemcpyAsync(x->f_slot_set, slot_set.data(), (size_t)m * 4, cudaMemcpyHostToDevice, st));
-    // the eligibility pass of every subset of the launch: one bitmap launch, one count launch
-    if ((rc = stb_launch_row_bitmap(ctx, x->f_ranges, 0, words, x->f_bitmap, n_sets, x->f_set_off)) != STB_OK) return rc;
-    ivff_elig_kernel<<<dim3((x->nlist + 7) / 8, n_sets), 256, 0, st>>>(x->list_off, x->order, x->nlist, x->f_bitmap, words,
-                                                                      x->f_elig);
-    STB_CUDA(cudaGetLastError());
-    ctx->kernel_launches += 1;
-    f.bitmap = x->f_bitmap; f.elig = x->f_elig; f.slot_set = x->f_slot_set;
-    if ((rc = ivfb_launch(x, x->b_q, m, nprobe, top_k, rerank, x->b_hits, x->b_status, &f)) != STB_OK) return rc;
-    hits.resize((size_t)m * top_k);
-    status.resize(2 * (size_t)m);
-    STB_CUDA(cudaMemcpyAsync(hits.data(), x->b_hits, hits.size() * sizeof(stb_hit), cudaMemcpyDeviceToHost, st));
-    STB_CUDA(cudaMemcpyAsync(status.data(), x->b_status, status.size() * 4, cudaMemcpyDeviceToHost, st));
-    STB_CUDA(cudaStreamSynchronize(st));                         // also ends the reads of loc, qc, set_off, slot_set
-    for (uint32_t j = 0; j < m; ++j) {
-      const uint32_t r = qrow[j];
-      memcpy(out_hits + (size_t)r * top_k, hits.data() + (size_t)j * top_k, top_k * sizeof(stb_hit));
-      out_n[r] = status[2 * j];
-      if (out_scanned) out_scanned[r] = status[2 * j + 1];
-    }
-    for (uint32_t j = 0; j < m; ++j) local[subset_of[qrow[j]]] = UINT32_MAX;
-  }
-  STB_CUDA(cudaStreamSynchronize(st));                           // `loc` is read by the copy above
-  return STB_OK;
+  sub.subset_of = subset_of;
+  return ivfb_host_search(x, q, nq, nprobe, top_k, rerank, sub, out_hits, out_n, out_scanned);
 }
 
 int stb_ivfpq_search(stb_ivfpq *x, const float *q, uint32_t nprobe, uint32_t top_k, uint32_t rerank,
@@ -2030,8 +1987,7 @@ int stb_ivfpq_search(stb_ivfpq *x, const float *q, uint32_t nprobe, uint32_t top
   *out_n = 0;
   if (top_k == 0) return STB_OK;
   if (top_k > IVF_HOST_TOPK_MAX) { stb_set_error("ivfpq_search: top_k must be <= %u", (unsigned)IVF_HOST_TOPK_MAX); return STB_ERR_ARG; }
-  nprobe = std::max(1u, std::min(std::min(nprobe, x->nlist), 1024u));
-  rerank = std::max(top_k, std::min(rerank, (uint32_t)IVF_HOST_TOPK_MAX));
+  ivf_clamp(x, top_k, IVF_HOST_TOPK_MAX, nprobe, rerank);
   cudaStream_t st = ctx->stream;
   memcpy(ctx->q_pin, q, STB_D * sizeof(float));
   STB_CUDA(cudaMemcpyAsync(ctx->q_dev, ctx->q_pin, STB_D * sizeof(float), cudaMemcpyHostToDevice, st));
@@ -2048,17 +2004,12 @@ int stb_ivfpq_search(stb_ivfpq *x, const float *q, uint32_t nprobe, uint32_t top
     if (out_scanned) *out_scanned = ctx->status_pin[1];
     return STB_OK;
   }
-  ivf_coarse_kernel<<<(x->nlist + 7) / 8, 256, 0, st>>>(x->centroids, x->nlist, ctx->q_dev, x->coarse);
-  uint32_t npow = 1; while (npow < x->nlist) npow <<= 1;
-  STB_ATTR_ONCE(ctx, STB_ATTR_IVF_PROBE,
-                cudaFuncSetAttribute(ivf_probe_lut_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 8));
-  ivf_probe_lut_kernel<<<1, 1024, npow * 8, st>>>(x->coarse, x->nlist, nprobe, x->list_off, x->codebooks, ctx->q_dev, x->probe, x->lut);
-  ctx->kernel_launches += 2;
+  int rc;
+  if ((rc = ivfb_probe(x, ctx->q_dev, 1, nprobe, x->coarse, x->probe, x->lut, nullptr)) != STB_OK) return rc;
   uint32_t total = 0;
   STB_CUDA(cudaMemcpyAsync(&total, x->probe + 2 * nprobe, 4, cudaMemcpyDeviceToHost, st));
   STB_CUDA(cudaStreamSynchronize(st));
   if (out_scanned) *out_scanned = total;
-  int rc;
   uint32_t nv = 0;
   if (total > 0) {
     // warps: enough to spread every list over many warps and fill the GPU, at most 512, and enough

@@ -182,6 +182,37 @@ def test_more_than_one_launch_of_queries(ctx):
         idx.close(); c.close()
 
 
+@pytest.mark.parametrize("shape, launches", [
+    ("batch", 2 * 4),                        # two launches of the four batched kernels
+    ("filtered", 2 + 2 * 4),                 # one eligibility pass (bitmap, counts) per call
+    ("filtered_every_row", 1 + 4),           # no bitmap: the counts are the list lengths
+    ("subsets_different", 2 * (2 + 4)),      # each launch names another subset: a pass per launch
+    ("subsets_same", 2 + 2 * 4),             # the second launch names the first one's subset: its pass is reused
+])
+def test_kernel_launches_per_call(ctx, sub_index, shape, launches):
+    """The host forms share one loop: their launch counts, and the hits of a launch whose pass was skipped."""
+    rows, Q, c, idx, base, nlist, subsets = sub_index
+    QQ = np.ascontiguousarray(np.resize(Q, (MAX_NQ + 1, 256)))
+    kw = dict(nprobe=8, top_k=10, rerank=64)
+    before = ctx.counters()["kernel_launches"]
+    if shape == "batch":
+        idx.search_batch(QQ, **kw)
+    elif shape == "filtered":
+        idx.search_filtered(QQ, subsets[0], **kw)
+    elif shape == "filtered_every_row":
+        idx.search_filtered(Q, None, **kw)
+    else:
+        subset_of = np.zeros(len(QQ), np.uint32)
+        if shape == "subsets_different":
+            subset_of[MAX_NQ:] = 1
+        got = idx.search_subsets(QQ, subsets, subset_of, **kw)
+    assert ctx.counters()["kernel_launches"] - before == launches
+    if shape.startswith("subsets"):
+        for sl in (slice(0, MAX_NQ), slice(MAX_NQ, None)):
+            want = idx.search_filtered(QQ[sl], subsets[subset_of[sl][0]], **kw)
+            assert all(g[sl].tobytes() == w.tobytes() for g, w in zip(got, want)), sl
+
+
 def _check_last_launch(idx, Q, subsets, subset_of, last, kw):
     """batch_last describes the call's last launch: slot j = its j-th query, as the single filtered call has it."""
     info = [idx.batch_last(j) for j in (0, len(last) - 1)]
