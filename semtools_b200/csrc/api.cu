@@ -576,11 +576,6 @@ static int stb_env_max_tier() {
   if (e[0] == 'h') return STB_TIER_H16;
   return STB_TIER_Q8;
 }
-// The single-GPU asynchronous entry points (stb_search_topk_dev, stb_search_many without an exchange) always
-// use the overlapped launch mode and co-scan (scan_topk.cu: stb_coscan_offset): back-to-back queries share
-// each tile's HBM read.  The sharded forms (stb_search_topk_xchg, stb_search_many with an exchange) launch
-// like the synchronous entry points (full grid, dependent released after the scan).
-
 // What a K1 entry point may do to a reduced-width candidate copy that does not cover every row yet:
 // build it from nothing (or rebuild one marked bad), and convert the rows appended behind a valid prefix.
 struct K1CopyPolicy {
@@ -607,21 +602,21 @@ static int k1_copy_ready(stb_ctx *ctx, stb_corpus *c, int tier, uint32_t top_k, 
   return rc == STB_ERR_STATE ? STB_OK : rc;
 }
 
-// The narrowest copy that is fully built and usable: the asynchronous entry points never build one
-// (stb_corpus_prepare does).
-static int best_built_tier(stb_ctx *ctx, const stb_corpus *c, uint32_t top_k) {
-  for (int tier = STB_TIER_Q8; tier > STB_TIER_F32; --tier) {
+// The single-GPU asynchronous entry points (stb_search_topk_dev, stb_search_many without an exchange) always
+// use the overlapped launch mode and co-scan (scan_topk.cu: stb_coscan_offset): back-to-back queries share
+// each tile's HBM read.  The sharded forms (stb_search_topk_xchg, stb_search_many with an exchange) launch
+// like the synchronous entry points (full grid, dependent released after the scan).
+// All of them read the narrowest copy that is fully built and usable; `policy` may let the q8 copy be built or
+// extended first, and nothing else builds one (stb_corpus_prepare does).  On a host-rows corpus they read an HBM
+// copy or launch nothing: an f32 top-k scan would stream the whole matrix over the host link.
+static int k1_async_tier(stb_ctx *ctx, const stb_corpus *c, uint32_t top_k, K1CopyPolicy policy, const char *what, int *tier) {
+  for (*tier = STB_TIER_Q8; *tier > STB_TIER_F32; --*tier) {
     bool ready = false;
-    k1_copy_ready(ctx, const_cast<stb_corpus *>(c), tier, top_k, kBuiltOnly, &ready);   // builds nothing: cannot fail
-    if (ready) return tier;
+    const int rc = k1_copy_ready(ctx, const_cast<stb_corpus *>(c), *tier, top_k, *tier == STB_TIER_Q8 ? policy : kBuiltOnly, &ready);
+    if (rc != STB_OK) return rc;
+    if (ready) return STB_OK;
   }
-  return STB_TIER_F32;
-}
-
-// The asynchronous top-k forms on a host-rows corpus read an HBM copy or launch nothing: an f32 top-k scan
-// would stream the whole matrix over the host link.
-static int host_rows_tier_check(const stb_corpus *c, int tier, const char *what) {
-  if (c->host_rows && tier == STB_TIER_F32) {
+  if (c->host_rows) {
     stb_set_error("%s: the rows of this corpus are in host memory and no HBM copy serves this top_k "
                   "(q8: top_k <= %d; 16-bit shadow: stb_corpus_prepare); use stb_search", what, STB_Q8_MAX_K);
     return STB_ERR_STATE;
@@ -634,23 +629,43 @@ static int host_rows_refuse(const stb_corpus *c, const char *what) {
   return STB_OK;
 }
 
-// The distance cap of a top-k result sorted by (distance, row): how many leading hits have distance <
-// max_distance (strict; a NaN cap passes none).  Where top_k always caps (store-query mode, the top-k fast
-// path) the capped result is this prefix of the uncapped one.
+// The status words a K1 top-k scan stores beside its hits: [0] the hits (at most top_k), [1] non-zero when the
+// scan proved them, [2] STB_XCHG_STATUS_TIMEOUT when a peer of a sharded scan never arrived.
+struct K1Status {
+  uint32_t n;
+  bool proven, timeout;
+};
+static K1Status k1_status(const uint32_t *st, uint32_t top_k) {
+  return {std::min(st[0], top_k), st[1] != 0, st[2] == STB_XCHG_STATUS_TIMEOUT};
+}
+
+// The distance limit of a search's hits, strict (distance < limit): max_distance.unwrap_or(100.0), which a top-k
+// search also caps at STB_DEFAULT_MAX_DIST and threshold mode takes as given.  A NaN cap passes nothing: no
+// distance compares below it.
+static double k1_limit(bool threshold_all, int has_max, double max_distance) {
+  if (!has_max) return STB_DEFAULT_MAX_DIST;
+  return threshold_all || !(max_distance > STB_DEFAULT_MAX_DIST) ? max_distance : STB_DEFAULT_MAX_DIST;
+}
+
+// The collect floor for the rows at distance < d, from scores that may sit up to `margin` below the exact
+// cosine 1 - d.  A NaN d collects nothing.
+static float k1_floor(double d, double margin) { return d == d ? (float)(1.0 - d - margin) : INFINITY; }
+
+// The distance cap of a top-k result sorted by (distance, row): how many leading hits pass the top-k limit
+// (k1_limit).  Where top_k always caps (store-query mode, the top-k fast path) the capped result is this
+// prefix of the uncapped one.
 static uint64_t capped_hits(const stb_hit *hits, uint64_t n, int has_max, double max_distance) {
+  const double limit = k1_limit(false, has_max, max_distance);
   uint64_t i = 0;
-  while (i < n && !(has_max && !(hits[i].distance < max_distance))) ++i;
+  while (i < n && hits[i].distance < limit) ++i;
   return i;
 }
 
-// ---- row ranges: global -> local, clipped to this shard, uploaded as the K1 passes read them: vstart[m + 1] (the
-// virtual prefix of every range, then the total), then rbegin[m] (its first local row); the only decoder is
-// stb_scan_args (scan_topk.cu).  Without ranges the pass reads every row; *n_virtual = 0: no row lies in them.
+// ---- row ranges: global -> local, clipped to this shard and uploaded in the layout of StbRowRanges (common.cuh).
+// Without ranges the passes read every row; n_virtual = 0: no row lies in them.
 static int k1_upload_ranges(stb_ctx *ctx, const stb_corpus *c, const char *what, const uint64_t *row_ranges, uint32_t n_ranges,
-                            const uint64_t **ranges_dev, uint32_t *n_loc, uint64_t *n_virtual) {
-  *ranges_dev = nullptr;
-  *n_loc = 0;
-  *n_virtual = c->n;
+                            StbRowRanges *out) {
+  *out = {nullptr, 0, c->n};
   if (!row_ranges) return STB_OK;
   std::vector<uint64_t> vstart, rbegin;
   vstart.reserve(n_ranges + 1); rbegin.reserve(n_ranges);
@@ -660,30 +675,35 @@ static int k1_upload_ranges(stb_ctx *ctx, const stb_corpus *c, const char *what,
          vstart.push_back(acc); rbegin.push_back(b);
          acc += e - b;
        })) != STB_OK) return rc;
-  *n_virtual = acc;
+  out->n_virtual = acc;
   if (acc == 0) return STB_OK;
   vstart.push_back(acc);
-  *n_loc = (uint32_t)rbegin.size();
   std::vector<uint64_t> packed(vstart);
   packed.insert(packed.end(), rbegin.begin(), rbegin.end());
   if ((rc = ctx->ranges_dev.reserve(packed.size(), 4096)) != STB_OK) return rc;
   STB_CUDA(cudaMemcpyAsync(ctx->ranges_dev, packed.data(), packed.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->stream));
   STB_CUDA(cudaStreamSynchronize(ctx->stream));   // `packed` dies at scope end
-  *ranges_dev = ctx->ranges_dev;
+  *out = {ctx->ranges_dev, (uint32_t)rbegin.size(), acc};
+  return STB_OK;
+}
+
+// A host query into ctx->q_dev, through the pinned staging buffer.
+static int k1_stage_query(stb_ctx *ctx, const float *q) {
+  memcpy(ctx->q_pin, q, STB_D * sizeof(float));
+  STB_CUDA(cudaMemcpyAsync(ctx->q_dev, ctx->q_pin, STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
   return STB_OK;
 }
 
 // Exact path for any input: collect rows whose approximate cosine >= cos_floor,
 // score them canonically, keep distance < limit, sort by (distance,row).
 // On return ctx->collect_hits holds the sorted hits and *n_pass their count.
-static int collect_exact_sorted(stb_ctx *ctx, const stb_corpus *c, float cos_floor, double limit,
-                                const uint64_t *ranges_dev, uint32_t n_ranges, uint64_t n_virtual,
+static int collect_exact_sorted(stb_ctx *ctx, const stb_corpus *c, float cos_floor, double limit, const StbRowRanges &ranges,
                                 uint64_t *n_pass, int tier = STB_TIER_F32) {
   int rc;
   unsigned long long count = 0;
   if ((rc = ctx->collect_rows.reserve(1, 1u << 20)) != STB_OK) return rc;
   for (int attempt = 0; attempt < 3; ++attempt) {
-    if ((rc = stb_launch_scan_collect(ctx, c, tier, ctx->q_dev, cos_floor, ranges_dev, n_ranges, n_virtual)) != STB_OK) return rc;
+    if ((rc = stb_launch_scan_collect(ctx, c, tier, ctx->q_dev, cos_floor, ranges)) != STB_OK) return rc;
     STB_CUDA(cudaMemcpyAsync(&count, ctx->collect_count, sizeof(count), cudaMemcpyDeviceToHost, ctx->stream));
     STB_CUDA(cudaStreamSynchronize(ctx->stream));
     if (count <= ctx->collect_rows.cap) break;
@@ -703,6 +723,81 @@ static int collect_exact_sorted(stb_ctx *ctx, const stb_corpus *c, float cos_flo
   return STB_OK;
 }
 
+// The top-k tier ladder: q8 (260 B/row) -> h16 (512 B/row) -> f32 (1 KiB/row; not on a host-rows corpus).  Every
+// tier ends in the same exact f64 re-rank and proves its own result; one that cannot is retried one tier up, so
+// the answer is the oracle's whichever tier produced it.  A reduced-width tier that keeps failing its proofs on
+// this corpus is dropped.  Each scan's last CTA stores the k hits + status straight into the pinned host buffers
+// (UVA: cudaMallocHost memory is device-accessible), which takes the two D2H copies off the stream; kernel
+// completion makes the stores visible to the host.  *proven: the last scan proved its hits.
+static int k1_topk_ladder(stb_ctx *ctx, stb_corpus *c, const StbRowRanges &ranges, uint32_t top_k, K1CopyPolicy lazy,
+                          bool *proven) {
+  *proven = false;
+  const int last = c->host_rows ? STB_TIER_H16 : STB_TIER_F32;
+  for (int tier = STB_TIER_Q8; tier >= last && !*proven; --tier) {
+    if (tier != STB_TIER_F32 && c->tier_tries[tier] >= 8 && 2 * c->tier_proven[tier] < c->tier_tries[tier]) continue;
+    bool ready = false;
+    int rc;
+    if ((rc = k1_copy_ready(ctx, c, tier, top_k, lazy, &ready)) != STB_OK) return rc;
+    if (!ready) continue;
+    if ((rc = stb_launch_scan_topk(ctx, c, tier, ctx->q_dev, top_k, ranges, ctx->hits_pin, ctx->status_pin)) != STB_OK) return rc;
+    STB_CUDA(cudaStreamSynchronize(ctx->stream));
+    *proven = k1_status(ctx->status_pin, top_k).proven;
+    c->tier_tries[tier]++;
+    if (*proven) c->tier_proven[tier]++;
+  }
+  return STB_OK;
+}
+
+// The k-th-bin route (top_k beyond the register lists; on a host-rows corpus any top-k no copy proved): a histogram
+// pass finds the score bin of the k-th best row, then the collect pass takes only the rows at or above that bin
+// (a bin at the end: fewer than k rows, take all).  The q8 passes come first when the copy is usable.  Their
+// histogram is over UPPER BOUNDS, which sit up to ~0.02-0.04 above the exact cosines, so the floor is put 0.04
+// below the k-th best bound and the result is PROVEN afterwards: every row that was not collected has
+// c < floor + 2e-5; if the k-th exact distance found is below 1 - floor - 2e-5 nothing outside can enter or tie.
+// Otherwise (a fallback search) the f32 passes answer, with the floor 2 * STB_SCORE_EPS below the bin.
+static int k1_kth_bin_collect(stb_ctx *ctx, const stb_corpus *c, const StbRowRanges &ranges, uint32_t top_k, double limit,
+                              bool use_q8, uint64_t *n_pass) {
+  std::vector<unsigned int> hist(4096);
+  int rc;
+  for (const int tier : {STB_TIER_Q8, STB_TIER_F32}) {
+    const bool q8 = tier == STB_TIER_Q8;
+    if (q8 && !use_q8) continue;
+    if ((rc = stb_launch_scan_hist(ctx, c, tier, ctx->q_dev, ranges, ctx->hist_dev)) != STB_OK) return rc;
+    STB_CUDA(cudaMemcpyAsync(hist.data(), ctx->hist_dev, 4096 * sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
+    STB_CUDA(cudaStreamSynchronize(ctx->stream));
+    uint64_t cum = 0;
+    int b = 0;
+    for (; b < 4096; ++b) { cum += hist[b]; if (cum >= top_k) break; }
+    const float floor_cos = b < 4095 ? k1_floor((double)(b + 1) / 2048.0, q8 ? 0.04 : 2.0 * STB_SCORE_EPS) : -INFINITY;
+    if ((rc = collect_exact_sorted(ctx, c, floor_cos, limit, ranges, n_pass, tier)) != STB_OK) return rc;
+    if (!q8 || floor_cos == -INFINITY) return STB_OK;
+    if (*n_pass >= top_k) {
+      stb_hit kth;
+      STB_CUDA(cudaMemcpyAsync(&kth, ctx->collect_hits + (top_k - 1), sizeof(kth), cudaMemcpyDeviceToHost, ctx->stream));
+      STB_CUDA(cudaStreamSynchronize(ctx->stream));
+      if (kth.distance < 1.0 - (double)floor_cos - 2.0 * STB_Q8_SCAN_EPS) return STB_OK;
+    }
+    ctx->fallback_searches++;
+  }
+  return STB_OK;
+}
+
+// A search's n sorted hits to the caller: the first min(n, cap) from `src` (device memory, or pinned host memory
+// the kernel stored into), *out_n = n, and STB_ERR_CAPACITY when they do not all fit.
+static int k1_copy_out(stb_ctx *ctx, const stb_hit *src, bool on_device, uint64_t n, stb_hit *out_hits, uint64_t cap,
+                       uint64_t *out_n) {
+  const uint64_t m = std::min(n, cap);
+  *out_n = n;
+  if (m && on_device) {
+    STB_CUDA(cudaMemcpyAsync(out_hits, src, m * sizeof(stb_hit), cudaMemcpyDeviceToHost, ctx->stream));
+    STB_CUDA(cudaStreamSynchronize(ctx->stream));
+  } else if (m) {
+    memcpy(out_hits, src, m * sizeof(stb_hit));
+  }
+  if (n > cap) { stb_set_error("search: %llu hits, capacity %llu", (unsigned long long)n, (unsigned long long)cap); return STB_ERR_CAPACITY; }
+  return STB_OK;
+}
+
 int stb_search(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t top_k, int has_max,
                double max_distance, int mode, const uint64_t *row_ranges, uint32_t n_ranges,
                stb_hit *out_hits, uint64_t cap, uint64_t *out_n) {
@@ -719,14 +814,10 @@ int stb_search(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t 
   if (mode == STB_MODE_STORE_QUERY && row_ranges && n_ranges == 0) return STB_OK;  // empty subset, store.rs:489
   if (corpus->n == 0) return STB_OK;
 
-  const uint64_t *ranges_dev = nullptr;
-  uint32_t n_loc = 0;
-  uint64_t n_virtual = 0;
-  if ((rc = k1_upload_ranges(ctx, corpus, "search", row_ranges, n_ranges, &ranges_dev, &n_loc, &n_virtual)) != STB_OK) return rc;
-  if (n_virtual == 0) return STB_OK;
-
-  memcpy(ctx->q_pin, q, STB_D * sizeof(float));
-  STB_CUDA(cudaMemcpyAsync(ctx->q_dev, ctx->q_pin, STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+  StbRowRanges ranges;
+  if ((rc = k1_upload_ranges(ctx, corpus, "search", row_ranges, n_ranges, &ranges)) != STB_OK) return rc;
+  if (ranges.n_virtual == 0) return STB_OK;
+  if ((rc = k1_stage_query(ctx, q)) != STB_OK) return rc;
 
   // The reduced-width candidate copies are used when they exist (stb_corpus_prepare) and built lazily
   // from the second search since the corpus last changed, on >= 32768 rows: a one-shot CLI query must
@@ -735,142 +826,41 @@ int stb_search(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint32_t 
   // 1 KiB/row.
   // A host-rows corpus builds nothing lazily: its q8 copy is always current, and its shadow is read when
   // stb_corpus_prepare or K2 built it.  No pass streams its f32 rows while an HBM copy can answer: a top-k
-  // query no copy proves goes to the q8 histogram / collect route below, not to the f32 top-k scan.
+  // query no copy proves goes to the k-th-bin route below, not to the f32 top-k scan.
   stb_corpus *cm = const_cast<stb_corpus *>(corpus);
   const bool host = cm->host_rows != 0;
   const K1CopyPolicy lazy = {!host && cm->searches_since_change >= 1 && cm->n >= 32768, true};
   cm->searches_since_change++;
 
-  uint64_t total = 0;
-  const stb_hit *src_dev = nullptr;   // sorted device hits to copy out (collect path)
-  bool answered = false;
+  const double limit = k1_limit(threshold_all, has_max, max_distance);
   if (!threshold_all && top_k <= stb_scan_topk_max_k()) {
-    // ---- fast path: one kernel, k*16+16 bytes back -----------------------------
-    // The kernel's last CTA stores the k hits + status straight into the pinned host buffers
-    // (UVA: cudaMallocHost memory is device-accessible), which takes the two D2H copies off the
-    // stream; kernel completion makes the stores visible to the host.
-    auto run_fast = [&](int tier) -> int {
-      int r;
-      if ((r = stb_launch_scan_topk(ctx, corpus, tier, ctx->q_dev, top_k, ranges_dev, n_loc, n_virtual, ctx->hits_pin,
-                                    ctx->status_pin)) != STB_OK) return r;
-      STB_CUDA(cudaStreamSynchronize(ctx->stream));
-      return STB_OK;
-    };
-    // Tier ladder: q8 (260 B/row) -> h16 (512 B/row) -> f32 (1 KiB/row).  Every tier ends in the
-    // same exact f64 re-rank and proves its own result; one that cannot is retried one tier up, so
-    // the answer is the oracle's whichever tier produced it.  A tier that keeps failing its proofs
-    // on this corpus is dropped.
     bool proven = false;
-    for (int tier = STB_TIER_Q8; tier >= STB_TIER_H16 && !proven; --tier) {
-      if (cm->tier_tries[tier] >= 8 && 2 * cm->tier_proven[tier] < cm->tier_tries[tier]) continue;
-      bool ready = false;
-      if ((rc = k1_copy_ready(ctx, cm, tier, top_k, lazy, &ready)) != STB_OK) return rc;
-      if (!ready) continue;
-      if ((rc = run_fast(tier)) != STB_OK) return rc;
-      proven = ctx->status_pin[1] != 0;
-      cm->tier_tries[tier]++;
-      if (proven) cm->tier_proven[tier]++;
-    }
-    if (!proven && !host) {
-      if ((rc = run_fast(STB_TIER_F32)) != STB_OK) return rc;
-      cm->tier_tries[STB_TIER_F32]++;
-      if (ctx->status_pin[1]) cm->tier_proven[STB_TIER_F32]++;
-    }
-    if (proven || !host) {
-      const uint32_t n_hits = ctx->status_pin[0];
-      if (ctx->status_pin[1]) {
-        const uint64_t n = capped_hits(ctx->hits_pin, n_hits, has_max, max_distance);
-        if (n && cap) memcpy(out_hits, ctx->hits_pin, std::min(n, cap) * sizeof(stb_hit));
-        *out_n = n;
-        if (n > cap) { stb_set_error("search: %llu hits, capacity %llu", (unsigned long long)n, (unsigned long long)cap); return STB_ERR_CAPACITY; }
-        return STB_OK;
-      }
-      // ---- candidate margin not provable: exact collect pass --------------------
+    if ((rc = k1_topk_ladder(ctx, cm, ranges, top_k, lazy, &proven)) != STB_OK) return rc;
+    const uint32_t n_hits = k1_status(ctx->status_pin, top_k).n;
+    if (proven) return k1_copy_out(ctx, ctx->hits_pin, false, capped_hits(ctx->hits_pin, n_hits, has_max, max_distance), out_hits, cap, out_n);
+    if (!host) {
+      // the f32 scan's candidate margin is not provable: exact collect pass down to its k-th hit
       ctx->fallback_searches++;
-      float floor_cos = -INFINITY;
-      if (n_hits == top_k) floor_cos = (float)(1.0 - ctx->hits_pin[top_k - 1].distance - 2.0 * STB_SCORE_EPS);
+      const float floor_cos = n_hits == top_k ? k1_floor(ctx->hits_pin[top_k - 1].distance, 2.0 * STB_SCORE_EPS) : -INFINITY;
       uint64_t n_pass = 0;
-      if ((rc = collect_exact_sorted(ctx, corpus, floor_cos, has_max ? std::min(max_distance, STB_DEFAULT_MAX_DIST) : STB_DEFAULT_MAX_DIST,
-                                     ranges_dev, n_loc, n_virtual, &n_pass)) != STB_OK) return rc;
-      total = std::min<uint64_t>(n_pass, top_k);
-      src_dev = ctx->collect_hits;
-      answered = true;
+      if ((rc = collect_exact_sorted(ctx, corpus, floor_cos, limit, ranges, &n_pass)) != STB_OK) return rc;
+      return k1_copy_out(ctx, ctx->collect_hits, true, std::min<uint64_t>(n_pass, top_k), out_hits, cap, out_n);
     }
   }
-  if (!answered) {
-    // ---- threshold mode / top_k beyond the register lists (on host rows: any top-k no copy proved) -------
-    // collect -> exact -> sort
-    // When the int8 copy exists (or may be built: same lazy rule as the top-k tiers) the streaming
-    // passes read it instead of the f32 rows: its scores are upper bounds u >= c - 2e-5 of the exact
-    // cosine, so "u >= floor" collects a superset of "c >= floor" at a quarter of the bytes.
-    bool use_q8 = false;
-    if ((rc = k1_copy_ready(ctx, cm, STB_TIER_Q8, 0, lazy, &use_q8)) != STB_OK) return rc;
-    float floor_cos = -INFINITY;
-    double limit = STB_DEFAULT_MAX_DIST;
-    uint64_t n_pass = 0;
-    bool done = false;
-    if (threshold_all) {
-      limit = max_distance;
-      floor_cos = (float)(1.0 - max_distance - (use_q8 ? 2.0 * STB_Q8_SCAN_EPS : STB_SCORE_EPS));
-      if (!(max_distance == max_distance)) floor_cos = INFINITY;   // NaN threshold: nothing passes
-      if ((rc = collect_exact_sorted(ctx, corpus, floor_cos, limit, ranges_dev, n_loc, n_virtual, &n_pass,
-                                     use_q8 ? STB_TIER_Q8 : STB_TIER_F32)) != STB_OK) return rc;
-      done = true;
-    } else {
-      if (has_max) {
-        limit = std::min(max_distance, STB_DEFAULT_MAX_DIST);
-        if (!(max_distance == max_distance)) limit = -1.0;
-      }
-      // top_k beyond the register lists: histogram pass to find the score bin of the k-th
-      // best, then collect only rows at or above that bin (instead of the whole shard)
-      std::vector<unsigned int> hist(4096);
-      auto kth_bin = [&](int tier, int *bin) -> int {
-        int r;
-        if ((r = stb_launch_scan_hist(ctx, corpus, tier, ctx->q_dev, ranges_dev, n_loc, n_virtual, ctx->hist_dev)) != STB_OK) return r;
-        STB_CUDA(cudaMemcpyAsync(hist.data(), ctx->hist_dev, 4096 * sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
-        STB_CUDA(cudaStreamSynchronize(ctx->stream));
-        uint64_t cum = 0;
-        int b = 0;
-        for (; b < 4096; ++b) { cum += hist[b]; if (cum >= top_k) break; }
-        *bin = b;
-        return STB_OK;
-      };
-      if (use_q8) {
-        // q8: the histogram is over UPPER BOUNDS, which sit up to ~0.02-0.04 above the exact cosines, so the
-        // floor is put 0.04 below the k-th best bound and the result is PROVEN afterwards: every row that
-        // was not collected has c < floor + 2e-5; if the k-th exact distance found is below
-        // 1 - floor - 2e-5 nothing outside can enter or tie.  Otherwise the f32 passes below answer.
-        int b = 0;
-        if ((rc = kth_bin(STB_TIER_Q8, &b)) != STB_OK) return rc;
-        floor_cos = (b < 4095) ? (float)(1.0 - (double)(b + 1) / 2048.0 - 0.04) : -INFINITY;
-        if ((rc = collect_exact_sorted(ctx, corpus, floor_cos, limit, ranges_dev, n_loc, n_virtual, &n_pass, STB_TIER_Q8)) != STB_OK) return rc;
-        if (floor_cos == -INFINITY) done = true;             // everything was collected
-        else if (n_pass >= top_k) {
-          stb_hit kth;
-          STB_CUDA(cudaMemcpyAsync(&kth, ctx->collect_hits + (top_k - 1), sizeof(kth), cudaMemcpyDeviceToHost, ctx->stream));
-          STB_CUDA(cudaStreamSynchronize(ctx->stream));
-          done = kth.distance < 1.0 - (double)floor_cos - 2.0 * STB_Q8_SCAN_EPS;
-        }
-        if (!done) ctx->fallback_searches++;
-      }
-      if (!done) {
-        int b = 0;
-        if ((rc = kth_bin(STB_TIER_F32, &b)) != STB_OK) return rc;
-        floor_cos = (b < 4095) ? (float)(1.0 - (double)(b + 1) / 2048.0 - 2.0 * STB_SCORE_EPS) : -INFINITY;   // else: fewer than k rows, take all
-        if ((rc = collect_exact_sorted(ctx, corpus, floor_cos, limit, ranges_dev, n_loc, n_virtual, &n_pass)) != STB_OK) return rc;
-      }
-    }
-    total = threshold_all ? n_pass : std::min<uint64_t>(n_pass, top_k);
-    src_dev = ctx->collect_hits;
-  }
-  *out_n = total;
-  uint64_t ncopy = std::min(total, cap);
-  if (ncopy) {
-    STB_CUDA(cudaMemcpyAsync(out_hits, src_dev, ncopy * sizeof(stb_hit), cudaMemcpyDeviceToHost, ctx->stream));
-    STB_CUDA(cudaStreamSynchronize(ctx->stream));
-  }
-  if (total > cap) { stb_set_error("search: %llu hits, capacity %llu", (unsigned long long)total, (unsigned long long)cap); return STB_ERR_CAPACITY; }
-  return STB_OK;
+  // ---- threshold mode, or the k-th-bin route: collect -> exact -> sort
+  // When the int8 copy exists (or may be built: same lazy rule as the top-k tiers) the streaming
+  // passes read it instead of the f32 rows: its scores are upper bounds u >= c - 2e-5 of the exact
+  // cosine, so "u >= floor" collects a superset of "c >= floor" at a quarter of the bytes.
+  bool use_q8 = false;
+  if ((rc = k1_copy_ready(ctx, cm, STB_TIER_Q8, 0, lazy, &use_q8)) != STB_OK) return rc;
+  uint64_t n_pass = 0;
+  if (threshold_all)
+    rc = collect_exact_sorted(ctx, corpus, k1_floor(max_distance, use_q8 ? 2.0 * STB_Q8_SCAN_EPS : STB_SCORE_EPS), limit, ranges,
+                              &n_pass, use_q8 ? STB_TIER_Q8 : STB_TIER_F32);
+  else
+    rc = k1_kth_bin_collect(ctx, corpus, ranges, top_k, limit, use_q8, &n_pass);
+  if (rc != STB_OK) return rc;
+  return k1_copy_out(ctx, ctx->collect_hits, true, threshold_all ? n_pass : std::min<uint64_t>(n_pass, top_k), out_hits, cap, out_n);
 }
 
 int stb_search_topk_dev(stb_ctx *ctx, const stb_corpus *corpus, const float *q_dev, uint32_t top_k,
@@ -883,9 +873,9 @@ int stb_search_topk_dev(stb_ctx *ctx, const stb_corpus *corpus, const float *q_d
   if (corpus->n == 0) { stb_set_error("search_topk_dev: empty corpus"); return STB_ERR_STATE; }
   // candidates from the narrowest copy that already exists; status[1] says whether the result is
   // proven, the caller's fallback is unchanged
-  const int tier = best_built_tier(ctx, corpus, top_k);
-  if ((rc = host_rows_tier_check(corpus, tier, "search_topk_dev")) != STB_OK) return rc;
-  return stb_launch_scan_topk(ctx, corpus, tier, q_dev, top_k, nullptr, 0, corpus->n, out_hits_dev, out_status_dev, nullptr, true);
+  int tier;
+  if ((rc = k1_async_tier(ctx, corpus, top_k, kBuiltOnly, "search_topk_dev", &tier)) != STB_OK) return rc;
+  return stb_launch_scan_topk(ctx, corpus, tier, q_dev, top_k, {nullptr, 0, corpus->n}, out_hits_dev, out_status_dev, nullptr, true);
 }
 
 // ------------------------------------------------------------ peer-memory exchange ---
@@ -1010,14 +1000,15 @@ int stb_search_topk_xchg(stb_ctx *ctx, const stb_corpus *corpus, const float *q_
   if (!x->connected) { stb_set_error("search_topk_xchg: exchange not connected"); return STB_ERR_STATE; }
   if (x->dead) { stb_set_error("search_topk_xchg: this exchange saw a peer time-out; destroy it on every rank"); return STB_ERR_STATE; }
   if (top_k == 0 || top_k > x->max_k) { stb_set_error("search_topk_xchg: top_k must be 1..%u", x->max_k); return STB_ERR_ARG; }
+  int tier;
+  if ((rc = k1_async_tier(ctx, corpus, top_k, kBuiltOnly, "search_topk_xchg", &tier)) != STB_OK) return rc;
   StbXchgArgs a;
   memset(&a, 0, sizeof(a));
   for (uint32_t r = 0; r < x->world; ++r) a.base[r] = x->peers[r];
   a.world = x->world; a.rank = x->rank; a.max_k = x->max_k;
   a.seq = ++x->seq;
   a.slot = (uint32_t)(a.seq % STB_XCHG_SLOTS);
-  return stb_launch_scan_topk(ctx, corpus, best_built_tier(ctx, corpus, top_k), q_dev, top_k, nullptr, 0, corpus->n,
-                              out_hits_dev, out_status_dev, &a);
+  return stb_launch_scan_topk(ctx, corpus, tier, q_dev, top_k, {nullptr, 0, corpus->n}, out_hits_dev, out_status_dev, &a);
 }
 
 // ----------------------------------------------------------------- K2 batched search ---
@@ -2496,12 +2487,10 @@ static bool k1_copy_usable(const stb_corpus *c, int tier) {
 // Query and ranges staged like stb_search's; per-row device outputs: `floats` arrays of n f32 (NaN-filled) and one of
 // n u32 (zeroed), in the one buffer f_dev.
 static int k1_debug_stage(stb_ctx *ctx, const stb_corpus *c, const char *what, const float *q, const uint64_t *row_ranges,
-                          uint32_t n_ranges, int floats, StbBuf<float> &f_dev, unsigned int **u_dev, const uint64_t **ranges_dev,
-                          uint32_t *n_loc, uint64_t *n_virtual) {
+                          uint32_t n_ranges, int floats, StbBuf<float> &f_dev, unsigned int **u_dev, StbRowRanges *ranges) {
   int rc;
-  if ((rc = k1_upload_ranges(ctx, c, what, row_ranges, n_ranges, ranges_dev, n_loc, n_virtual)) != STB_OK) return rc;
-  memcpy(ctx->q_pin, q, STB_D * sizeof(float));
-  STB_CUDA(cudaMemcpyAsync(ctx->q_dev, ctx->q_pin, STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+  if ((rc = k1_upload_ranges(ctx, c, what, row_ranges, n_ranges, ranges)) != STB_OK) return rc;
+  if ((rc = k1_stage_query(ctx, q)) != STB_OK) return rc;
   const size_t n = c->n;
   if ((rc = f_dev.alloc(n * (floats + 1))) != STB_OK) return rc;
   *u_dev = (unsigned int *)(f_dev + n * floats);
@@ -2524,18 +2513,16 @@ int stb_debug_scan_scores(stb_ctx *ctx, const stb_corpus *corpus, int tier, cons
   if (corpus->n == 0) return STB_OK;
   StbBuf<float> d_score;
   unsigned int *d_seen = nullptr;
-  const uint64_t *ranges_dev = nullptr;
-  uint32_t n_loc = 0;
-  uint64_t n_virtual = 0;
-  if ((rc = k1_debug_stage(ctx, corpus, "debug_scan_scores", q, row_ranges, n_ranges, 1, d_score, &d_seen, &ranges_dev, &n_loc,
-                           &n_virtual)) == STB_OK && n_virtual) {
-    rc = stb_launch_debug_scan(ctx, corpus, tier, ctx->q_dev, ranges_dev, n_loc, n_virtual, d_score, d_seen);
-    if (rc == STB_OK && hist) rc = stb_launch_scan_hist(ctx, corpus, tier, ctx->q_dev, ranges_dev, n_loc, n_virtual, ctx->hist_dev);
+  StbRowRanges ranges = {nullptr, 0, 0};
+  if ((rc = k1_debug_stage(ctx, corpus, "debug_scan_scores", q, row_ranges, n_ranges, 1, d_score, &d_seen, &ranges)) == STB_OK &&
+      ranges.n_virtual) {
+    rc = stb_launch_debug_scan(ctx, corpus, tier, ctx->q_dev, ranges, d_score, d_seen);
+    if (rc == STB_OK && hist) rc = stb_launch_scan_hist(ctx, corpus, tier, ctx->q_dev, ranges, ctx->hist_dev);
   }
   cudaError_t e = cudaSuccess;
   if (rc == STB_OK) e = cudaMemcpyAsync(scores, d_score, corpus->n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream);
   if (rc == STB_OK && e == cudaSuccess) e = cudaMemcpyAsync(seen, d_seen, corpus->n * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream);
-  if (rc == STB_OK && e == cudaSuccess && hist && n_virtual)
+  if (rc == STB_OK && e == cudaSuccess && hist && ranges.n_virtual)
     e = cudaMemcpyAsync(hist, ctx->hist_dev, 4096 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
   if (rc == STB_OK && e != cudaSuccess) { stb_set_error("debug_scan_scores: %s", cudaGetErrorString(e)); cudaGetLastError(); return STB_ERR_CUDA; }
@@ -2561,16 +2548,14 @@ int stb_debug_q4_scan(stb_ctx *ctx, const stb_corpus *corpus, const float *q, ui
   StbBuf<float> d_f;
   unsigned int *d_seen = nullptr;
   StbBuf<unsigned long long> d_words;
-  const uint64_t *ranges_dev = nullptr;
-  uint32_t n_loc = 0;
-  uint64_t n_virtual = 0;
-  rc = k1_debug_stage(ctx, corpus, "debug_q4_scan", q, row_ranges, n_ranges, 4, d_f, &d_seen, &ranges_dev, &n_loc, &n_virtual);
+  StbRowRanges ranges = {nullptr, 0, 0};
+  rc = k1_debug_stage(ctx, corpus, "debug_q4_scan", q, row_ranges, n_ranges, 4, d_f, &d_seen, &ranges);
   cudaError_t e = cudaSuccess;
   if (rc == STB_OK && (rc = d_words.alloc(STB_Q4_WORDS + 1)) == STB_OK)   // the words, then the refined counter
     e = cudaMemsetAsync(d_words, 0, (STB_Q4_WORDS + 1) * sizeof(unsigned long long), ctx->stream);
-  if (rc == STB_OK && e == cudaSuccess && n_virtual)
-    rc = stb_launch_debug_q4(ctx, corpus, ctx->q_dev, top_k, ranges_dev, n_loc, n_virtual, d_words, d_words + STB_Q4_WORDS, pin,
-                             d_f, d_f + n, d_f + 2 * n, d_f + 3 * n, d_seen);
+  if (rc == STB_OK && e == cudaSuccess && ranges.n_virtual)
+    rc = stb_launch_debug_q4(ctx, corpus, ctx->q_dev, top_k, ranges, d_words, d_words + STB_Q4_WORDS, pin, d_f, d_f + n,
+                             d_f + 2 * n, d_f + 3 * n, d_seen);
   float *outs[4] = {u4, t, l8, u8};
   for (int i = 0; i < 4 && rc == STB_OK && e == cudaSuccess; ++i)
     e = cudaMemcpyAsync(outs[i], d_f + i * n, n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream);
@@ -2587,16 +2572,15 @@ int stb_search_xchg(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint
   if (rc) return rc;
   if (!q || !out_hits || !out_n || !out_complete) { stb_set_error("search_xchg: null argument"); return STB_ERR_ARG; }
   if ((rc = host_rows_refuse(corpus, "search_xchg")) != STB_OK) return rc;
-  memcpy(ctx->q_pin, q, STB_D * sizeof(float));
-  STB_CUDA(cudaMemcpyAsync(ctx->q_dev, ctx->q_pin, STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+  if ((rc = k1_stage_query(ctx, q)) != STB_OK) return rc;
   // the merge CTA stores the hits + status straight into pinned host memory
   if ((rc = stb_search_topk_xchg(ctx, corpus, ctx->q_dev, top_k, x, ctx->hits_pin, ctx->status_pin)) != STB_OK) return rc;
   STB_CUDA(cudaStreamSynchronize(ctx->stream));
-  const uint32_t n = std::min<uint32_t>(ctx->status_pin[0], top_k);
-  memcpy(out_hits, ctx->hits_pin, n * sizeof(stb_hit));
-  *out_n = n;
-  *out_complete = ctx->status_pin[1] ? 1 : 0;
-  if (ctx->status_pin[2] == 0xfffffffeu) { x->dead = true; stb_set_error("search_xchg: a peer rank never arrived (timeout)"); return STB_ERR_STATE; }
+  const K1Status st = k1_status(ctx->status_pin, top_k);
+  memcpy(out_hits, ctx->hits_pin, st.n * sizeof(stb_hit));
+  *out_n = st.n;
+  *out_complete = st.proven ? 1 : 0;
+  if (st.timeout) { x->dead = true; stb_set_error("search_xchg: a peer rank never arrived (timeout)"); return STB_ERR_STATE; }
   return STB_OK;
 }
 
@@ -2618,57 +2602,51 @@ int stb_search_many(stb_ctx *ctx, const stb_corpus *corpus, const float *q, uint
     if (x && corpus->n == 0) { stb_set_error("search_many: empty shard in a sharded search"); return STB_ERR_STATE; }
     return STB_OK;
   }
-  if (top_k > (x ? x->max_k : stb_scan_topk_max_k())) {
-    if (x) { stb_set_error("search_many: top_k must be 1..%u", x->max_k); return STB_ERR_ARG; }
-    for (uint32_t i = 0; i < nq; ++i) {                    // beyond the register lists: the general path, query by query
-      uint64_t n = 0;
-      rc = stb_search(ctx, corpus, q + (size_t)i * STB_D, top_k, 0, 0.0, STB_MODE_SEARCH_DOCUMENTS, nullptr, 0,
-                      out_hits + (size_t)i * top_k, top_k, &n);
-      if (rc != STB_OK) return rc;
-      out_n[i] = (uint32_t)n;
+  if (x && top_k > x->max_k) { stb_set_error("search_many: top_k must be 1..%u", x->max_k); return STB_ERR_ARG; }
+  const bool scan = top_k <= stb_scan_topk_max_k();   // beyond the register lists: every query takes stb_search
+  if (scan) {
+    // many queries amortise the int8 copy: build or extend it now (same size rule as the lazy build);
+    // otherwise the launches read the narrowest copy already built
+    const bool eager = nq >= 2 && corpus->n >= 32768;
+    int tier;
+    if ((rc = k1_async_tier(ctx, corpus, top_k, {eager, eager}, "search_many", &tier)) != STB_OK) return rc;
+    if ((rc = ctx->bq_dev.reserve((size_t)nq * STB_D)) != STB_OK) return rc;
+    if ((rc = ctx->hits_pin.reserve((size_t)nq * top_k, 2 * ctx->hits_pin.cap)) != STB_OK) return rc;
+    if ((size_t)nq * STB_D > ctx->many_q_pin.cap || (size_t)nq * 4 > ctx->many_status_pin.cap) {
+      const size_t cap = std::max<size_t>((size_t)nq, 64);
+      if ((rc = ctx->many_q_pin.alloc(cap * STB_D)) != STB_OK || (rc = ctx->many_status_pin.alloc(cap * 4)) != STB_OK) return rc;
     }
-    return STB_OK;
-  }
-  // many queries amortise the int8 copy: build or extend it now (same size rule as the lazy build);
-  // otherwise the launches read the narrowest copy already built
-  const bool eager = nq >= 2 && corpus->n >= 32768;
-  bool q8_ready = false;
-  if ((rc = k1_copy_ready(ctx, const_cast<stb_corpus *>(corpus), STB_TIER_Q8, top_k, {eager, eager}, &q8_ready)) != STB_OK) return rc;
-  const int tier = q8_ready ? STB_TIER_Q8 : best_built_tier(ctx, corpus, top_k);
-  if ((rc = host_rows_tier_check(corpus, tier, "search_many")) != STB_OK) return rc;
-  if ((rc = ctx->bq_dev.reserve((size_t)nq * STB_D)) != STB_OK) return rc;
-  if ((rc = ctx->hits_pin.reserve((size_t)nq * top_k, 2 * ctx->hits_pin.cap)) != STB_OK) return rc;
-  if ((size_t)nq * STB_D > ctx->many_q_pin.cap || (size_t)nq * 4 > ctx->many_status_pin.cap) {
-    const size_t cap = std::max<size_t>((size_t)nq, 64);
-    if ((rc = ctx->many_q_pin.alloc(cap * STB_D)) != STB_OK || (rc = ctx->many_status_pin.alloc(cap * 4)) != STB_OK) return rc;
-  }
-  memcpy(ctx->many_q_pin, q, (size_t)nq * STB_D * sizeof(float));
-  STB_CUDA(cudaMemcpyAsync(ctx->bq_dev, ctx->many_q_pin, (size_t)nq * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-  for (uint32_t i = 0; i < nq; ++i) {
-    stb_hit *oh = ctx->hits_pin + (size_t)i * top_k;
-    uint32_t *os = ctx->many_status_pin + 4 * (size_t)i;
-    if (x) rc = stb_search_topk_xchg(ctx, corpus, ctx->bq_dev + (size_t)i * STB_D, top_k, x, oh, os);
-    else rc = stb_launch_scan_topk(ctx, corpus, tier, ctx->bq_dev + (size_t)i * STB_D, top_k, nullptr, 0, corpus->n, oh, os, nullptr,
-                                   nq > 1);
-    if (rc != STB_OK) { cudaStreamSynchronize(ctx->stream); return rc; }
-  }
-  STB_CUDA(cudaStreamSynchronize(ctx->stream));
-  for (uint32_t i = 0; i < nq; ++i) {
-    const uint32_t *st = ctx->many_status_pin + 4 * (size_t)i;
-    if (x && st[2] == 0xfffffffeu) { x->dead = true; stb_set_error("search_many: a peer rank never arrived (timeout)"); return STB_ERR_STATE; }
-    if (st[1]) {
-      const uint32_t n = std::min<uint32_t>(st[0], top_k);
-      memcpy(out_hits + (size_t)i * top_k, ctx->hits_pin + (size_t)i * top_k, n * sizeof(stb_hit));
-      out_n[i] = n;
-    } else if (x) {
-      if (out_complete) out_complete[i] = 0;               // every rank sees the same flag: fall back together
-    } else {
-      uint64_t n = 0;                                      // tier ladder / collect path
-      rc = stb_search(ctx, corpus, q + (size_t)i * STB_D, top_k, 0, 0.0, STB_MODE_SEARCH_DOCUMENTS, nullptr, 0,
-                      out_hits + (size_t)i * top_k, top_k, &n);
-      if (rc != STB_OK) return rc;
-      out_n[i] = (uint32_t)n;
+    memcpy(ctx->many_q_pin, q, (size_t)nq * STB_D * sizeof(float));
+    STB_CUDA(cudaMemcpyAsync(ctx->bq_dev, ctx->many_q_pin, (size_t)nq * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    for (uint32_t i = 0; i < nq; ++i) {
+      stb_hit *oh = ctx->hits_pin + (size_t)i * top_k;
+      uint32_t *os = ctx->many_status_pin + 4 * (size_t)i;
+      if (x) rc = stb_search_topk_xchg(ctx, corpus, ctx->bq_dev + (size_t)i * STB_D, top_k, x, oh, os);
+      else rc = stb_launch_scan_topk(ctx, corpus, tier, ctx->bq_dev + (size_t)i * STB_D, top_k, {nullptr, 0, corpus->n}, oh, os,
+                                     nullptr, nq > 1);
+      if (rc != STB_OK) { cudaStreamSynchronize(ctx->stream); return rc; }
     }
+    STB_CUDA(cudaStreamSynchronize(ctx->stream));
+  }
+  for (uint32_t i = 0; i < nq; ++i) {
+    if (scan) {
+      const K1Status st = k1_status(ctx->many_status_pin + 4 * (size_t)i, top_k);
+      if (x && st.timeout) { x->dead = true; stb_set_error("search_many: a peer rank never arrived (timeout)"); return STB_ERR_STATE; }
+      if (st.proven) {
+        memcpy(out_hits + (size_t)i * top_k, ctx->hits_pin + (size_t)i * top_k, st.n * sizeof(stb_hit));
+        out_n[i] = st.n;
+        continue;
+      }
+      if (x) {
+        if (out_complete) out_complete[i] = 0;             // every rank sees the same flag: fall back together
+        continue;
+      }
+    }
+    uint64_t n = 0;                                        // tier ladder / collect path
+    rc = stb_search(ctx, corpus, q + (size_t)i * STB_D, top_k, 0, 0.0, STB_MODE_SEARCH_DOCUMENTS, nullptr, 0,
+                    out_hits + (size_t)i * top_k, top_k, &n);
+    if (rc != STB_OK) return rc;
+    out_n[i] = (uint32_t)n;
   }
   return STB_OK;
 }

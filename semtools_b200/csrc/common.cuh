@@ -203,7 +203,7 @@ struct stb_ctx {
   StbBuf<uint32_t> collect_rows;   // threshold/fallback compaction: local row ids
   StbBuf<unsigned long long> collect_count;
   StbBuf<stb_hit> collect_hits;    // exact hits of collected rows (sorted in place)
-  StbBuf<uint64_t> ranges_dev;     // [3 * n] : begin(local), end(local), vstart
+  StbBuf<uint64_t> ranges_dev;     // the clipped row ranges of the K1 passes (StbRowRanges)
   StbBuf<int> err_flag;            // device int: scratch flag of the copy builders, stb_embed and K2's query shadow; zeroed before each use
   StbBuf<unsigned int> hist_dev;   // 4096-bin score histogram (large-k path)
   // cudaFuncSetAttribute is per DEVICE: remembered per context, never in function statics
@@ -281,9 +281,11 @@ struct stb_ctx {
 
 // Spin-wait bound of the peer-memory exchanges (SM cycles, ~15 s): long enough that ranks entering a sharded
 // search a few seconds apart (first-call allocations, a busy host) still meet; a peer that is really gone
-// costs one bound, the call reports it (status 0xfffffffe / 2) and the caller must stop using the exchange:
-// ranks that disagree on whether an exchange happened no longer issue the same sequence of calls.
+// costs one bound, the call reports it (status STB_XCHG_STATUS_TIMEOUT / 2) and the caller must stop using the
+// exchange: ranks that disagree on whether an exchange happened no longer issue the same sequence of calls.
 #define STB_XCHG_TIMEOUT_CYCLES 30000000000ll
+// status[2] of a sharded top-k scan whose peers did not all arrive within that bound
+#define STB_XCHG_STATUS_TIMEOUT 0xfffffffeu
 #define STB_XCHG_SLOTS 4
 #define STB_XCHG_MAX_WORLD 8
 struct StbXchgArgs {
@@ -424,9 +426,16 @@ int stb_launch_corpus_gather(stb_ctx *ctx, const float *rows, const uint64_t *se
                              uint64_t m, float *stage);
 
 // ---- scan_topk.cu -------------------------------------------------------------
+// The rows a K1 pass scans, as k1_upload_ranges (api.cu) uploads them: with n > 0 ranges, dev holds vstart[n + 1]
+// (the virtual prefix of every range, then the total), then rbegin[n] (its first local row); the only decoder is
+// stb_scan_args (scan_topk.cu).  n = 0 and dev null: every row.  n_virtual: the rows scanned.
+struct StbRowRanges {
+  const uint64_t *dev;
+  uint32_t n;
+  uint64_t n_virtual;
+};
 // Fast path: one kernel = scan + per-warp running top-K' + CTA/tree merge +
 // exact f64 re-rank + completeness check.  q_dev: 256 f32 on device.
-// n_ranges > 0: ranges_dev holds local [begin,end,vstart] triples.
 // tier: STB_TIER_* -- which copy of `c` the streaming pass reads (must exist and be current).
 // overlapped: the launch is one of a pipelined single-GPU series (stb_search_topk_dev, stb_search_many
 // without an exchange) and takes no exchange or ranges: the grid is sized for ONE CTA per SM and
@@ -434,9 +443,8 @@ int stb_launch_corpus_gather(stb_ctx *ctx, const float *rows, const uint64_t *se
 // waiting for it to drain (scan_topk.cu: "overlapped launches").  It co-scans: it starts its pass where
 // its predecessor on the same corpus is reading, so the two scans share each tile's read through L2.
 int stb_launch_scan_topk(stb_ctx *ctx, const stb_corpus *c, int tier, const float *q_dev, uint32_t top_k,
-                         const uint64_t *ranges_dev, uint32_t n_ranges,
-                         uint64_t n_virtual, stb_hit *out_hits_dev,
-                         uint32_t *out_status_dev, const StbXchgArgs *xchg = nullptr, bool overlapped = false);
+                         const StbRowRanges &ranges, stb_hit *out_hits_dev, uint32_t *out_status_dev,
+                         const StbXchgArgs *xchg = nullptr, bool overlapped = false);
 // int8 codes + scales, nibble plane + {s, rho} of rows [first_row, n_rows) (q8 tier)
 // rows_first: the row rows_dev[0] holds (a staged chunk of a host-rows corpus), 0 for a whole matrix
 int stb_launch_q8_build(stb_ctx *ctx, const float *rows_dev, uint64_t first_row, uint64_t n_rows, uint8_t *out,
@@ -446,23 +454,21 @@ uint32_t stb_scan_topk_max_k(void);
 // Collect path: every row whose approximate cosine >= cos_floor (or that cannot be
 // scored safely) is appended to ctx->collect_rows; total count -> collect_count.
 // tier: STB_TIER_F32 (approximate cosine of the f32 rows) or STB_TIER_Q8 (upper bounds from the int8 copy)
-int stb_launch_scan_collect(stb_ctx *ctx, const stb_corpus *c, int tier,
-                            const float *q_dev, float cos_floor,
-                            const uint64_t *ranges_dev, uint32_t n_ranges,
-                            uint64_t n_virtual);
+int stb_launch_scan_collect(stb_ctx *ctx, const stb_corpus *c, int tier, const float *q_dev, float cos_floor,
+                            const StbRowRanges &ranges);
 // Large-k support: 4096-bin histogram of the approximate cosine over the scanned rows
 // (bin b: cos in (1-(b+1)/2048, 1-b/2048]).  hist_dev: 4096 u32 on device.
-int stb_launch_scan_hist(stb_ctx *ctx, const stb_corpus *c, int tier, const float *q_dev, const uint64_t *ranges_dev,
-                         uint32_t n_ranges, uint64_t n_virtual, unsigned int *hist_dev);
+int stb_launch_scan_hist(stb_ctx *ctx, const stb_corpus *c, int tier, const float *q_dev, const StbRowRanges &ranges,
+                         unsigned int *hist_dev);
 // Test hooks (stb_debug_scan_scores, stb_debug_q4_scan): the f32 / h16 / q8 pass, or the q8 tier's prefiltered
 // top-k scan, with a sink that stores each scanned local row's score into score[row] and counts it in seen[row].
 // The q4 form also stores u4 and T per row and l8 per refined row (pin != 0: T held at -inf); words: top_k
 // threshold words (zeroed; tag 1), refined: a zeroed counter.
-int stb_launch_debug_scan(stb_ctx *ctx, const stb_corpus *c, int tier, const float *q_dev, const uint64_t *ranges_dev,
-                          uint32_t n_ranges, uint64_t n_virtual, float *score, unsigned int *seen);
-int stb_launch_debug_q4(stb_ctx *ctx, const stb_corpus *c, const float *q_dev, uint32_t top_k, const uint64_t *ranges_dev,
-                        uint32_t n_ranges, uint64_t n_virtual, unsigned long long *words, unsigned long long *refined,
-                        int pin, float *u4, float *t, float *l8, float *u8, unsigned int *seen);
+int stb_launch_debug_scan(stb_ctx *ctx, const stb_corpus *c, int tier, const float *q_dev, const StbRowRanges &ranges,
+                          float *score, unsigned int *seen);
+int stb_launch_debug_q4(stb_ctx *ctx, const stb_corpus *c, const float *q_dev, uint32_t top_k, const StbRowRanges &ranges,
+                        unsigned long long *words, unsigned long long *refined, int pin, float *u4, float *t, float *l8,
+                        float *u8, unsigned int *seen);
 // Exact canonical distances of m collected rows -> hits (invalid/failing rows get
 // distance=+inf,row=UINT64_MAX); counts passing rows into pass_count.
 int stb_launch_exact(stb_ctx *ctx, const float *rows, uint64_t row_base,

@@ -55,17 +55,16 @@ struct ScanArgs {
   uint64_t t_bulk;               // tickets [0, t_bulk) cover STB_TICKET_TILES tiles each, later ones one tile
 };
 
-// A pass's ScanArgs over ranges_dev as k1_upload_ranges (api.cu) packs them: vstart[n_ranges + 1], then
-// rbegin[n_ranges]; the only decoder of that layout.  No tickets: the top-k launch sets its own.
-static ScanArgs stb_scan_args(const stb_corpus *c, const float *q_dev, const uint64_t *ranges_dev, uint32_t n_ranges,
-                              uint64_t n_virtual) {
+// A pass's ScanArgs over row ranges as k1_upload_ranges (api.cu) packs them: vstart[r.n + 1], then rbegin[r.n];
+// the only decoder of that layout.  No tickets: the top-k launch sets its own.
+static ScanArgs stb_scan_args(const stb_corpus *c, const float *q_dev, const StbRowRanges &r) {
   ScanArgs a;
   a.rows = reinterpret_cast<const float4 *>(c->rows);
-  a.n_virtual = n_virtual;
+  a.n_virtual = r.n_virtual;
   a.q = q_dev;
-  a.vstart = ranges_dev;
-  a.rbegin = ranges_dev ? ranges_dev + (n_ranges + 1) : nullptr;
-  a.n_ranges = n_ranges;
+  a.vstart = r.dev;
+  a.rbegin = r.dev ? r.dev + (r.n + 1) : nullptr;
+  a.n_ranges = r.n;
   a.tickets = nullptr; a.t_base = 0; a.t_bulk = 0;
   return a;
 }
@@ -1448,7 +1447,7 @@ __device__ __forceinline__ void stb_scan_topk_body(const TopkArgs &args) {
       }
       ts[0] = min(total, k);
       ts[1] = all_complete;
-      ts[2] = s_timeout ? 0xfffffffeu : (uint32_t)n_valid;
+      ts[2] = s_timeout ? STB_XCHG_STATUS_TIMEOUT : (uint32_t)n_valid;
       ts[3] = (uint32_t)KF | ((uint32_t)SRC << 16);
     }
   };
@@ -1639,12 +1638,11 @@ static int stb_launch_topk_r(stb_ctx *ctx, const TopkArgs &a, int tier, uint32_t
 }
 
 int stb_launch_scan_topk(stb_ctx *ctx, const stb_corpus *c, int tier, const float *q_dev, uint32_t top_k,
-                         const uint64_t *ranges_dev, uint32_t n_ranges,
-                         uint64_t n_virtual, stb_hit *out_hits_dev,
-                         uint32_t *out_status_dev, const StbXchgArgs *xchg, bool overlapped) {
-  if (overlapped && (xchg || n_ranges)) { stb_set_error("scan_topk: an overlapped launch takes no exchange or ranges"); return STB_ERR_ARG; }
+                         const StbRowRanges &ranges, stb_hit *out_hits_dev, uint32_t *out_status_dev,
+                         const StbXchgArgs *xchg, bool overlapped) {
+  if (overlapped && (xchg || ranges.n)) { stb_set_error("scan_topk: an overlapped launch takes no exchange or ranges"); return STB_ERR_ARG; }
   TopkArgs a;
-  a.scan = stb_scan_args(c, q_dev, ranges_dev, n_ranges, n_virtual);
+  a.scan = stb_scan_args(c, q_dev, ranges);
   memset(&a.co, 0, sizeof(a.co));
   a.row_base = c->row_base;
   a.keys = ctx->block_keys;
@@ -1666,7 +1664,7 @@ int stb_launch_scan_topk(stb_ctx *ctx, const stb_corpus *c, int tier, const floa
     a.q4.refined = ctx->q4_refined;
   }
   if (tier == STB_TIER_H16 && !c->shadow) { stb_set_error("scan_topk: h16 tier unavailable"); return STB_ERR_STATE; }
-  return n_ranges > 0 ? stb_launch_topk_r<1>(ctx, a, tier, top_k, overlapped) : stb_launch_topk_r<0>(ctx, a, tier, top_k, overlapped);
+  return ranges.n > 0 ? stb_launch_topk_r<1>(ctx, a, tier, top_k, overlapped) : stb_launch_topk_r<0>(ctx, a, tier, top_k, overlapped);
 }
 
 // ---- the series of top-k launches (StbScanSeries, common.cuh) ----------------------------------------------
@@ -1809,24 +1807,22 @@ stb_scan_collect_kernel(const CollectArgs args) {
   else stb_scan_rows<U, RANGES>(args.scan, sink);
 }
 
-int stb_launch_scan_collect(stb_ctx *ctx, const stb_corpus *c, int tier,
-                            const float *q_dev, float cos_floor,
-                            const uint64_t *ranges_dev, uint32_t n_ranges,
-                            uint64_t n_virtual) {
+int stb_launch_scan_collect(stb_ctx *ctx, const stb_corpus *c, int tier, const float *q_dev, float cos_floor,
+                            const StbRowRanges &ranges) {
   CollectArgs a;
-  a.scan = stb_scan_args(c, q_dev, ranges_dev, n_ranges, n_virtual);
+  a.scan = stb_scan_args(c, q_dev, ranges);
   a.q8 = c->q8; a.q8_scale = c->q8_scale;
   a.cos_floor = cos_floor;
   a.out = ctx->collect_rows;
   a.count = ctx->collect_count;
   a.cap = ctx->collect_rows.cap;
   STB_CUDA(cudaMemsetAsync(ctx->collect_count, 0, sizeof(unsigned long long), ctx->stream));
-  const unsigned grid = stb_scan_grid(ctx, n_virtual, tier == STB_TIER_Q8 ? STB_Q8_SCAN_U : STB_SCAN_U);
+  const unsigned grid = stb_scan_grid(ctx, ranges.n_virtual, tier == STB_TIER_Q8 ? STB_Q8_SCAN_U : STB_SCAN_U);
   if (tier == STB_TIER_Q8) {
     if (!c->q8) { stb_set_error("scan_collect: q8 tier unavailable"); return STB_ERR_STATE; }
-    if (n_ranges > 0) stb_scan_collect_kernel<STB_Q8_SCAN_U, true, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a);
+    if (ranges.n > 0) stb_scan_collect_kernel<STB_Q8_SCAN_U, true, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a);
     else stb_scan_collect_kernel<STB_Q8_SCAN_U, false, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a);
-  } else if (n_ranges > 0)
+  } else if (ranges.n > 0)
     stb_scan_collect_kernel<STB_SCAN_U, true><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a);
   else
     stb_scan_collect_kernel<STB_SCAN_U, false><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a);
@@ -1869,16 +1865,16 @@ stb_scan_hist_kernel(const ScanArgs scan, unsigned int *global_hist, const uint8
     if (s_hist[i]) atomicAdd(global_hist + i, s_hist[i]);
 }
 
-int stb_launch_scan_hist(stb_ctx *ctx, const stb_corpus *c, int tier, const float *q_dev, const uint64_t *ranges_dev,
-                         uint32_t n_ranges, uint64_t n_virtual, unsigned int *hist_dev) {
-  const ScanArgs a = stb_scan_args(c, q_dev, ranges_dev, n_ranges, n_virtual);
+int stb_launch_scan_hist(stb_ctx *ctx, const stb_corpus *c, int tier, const float *q_dev, const StbRowRanges &ranges,
+                         unsigned int *hist_dev) {
+  const ScanArgs a = stb_scan_args(c, q_dev, ranges);
   STB_CUDA(cudaMemsetAsync(hist_dev, 0, STB_HIST_BINS * sizeof(unsigned int), ctx->stream));
-  const unsigned grid = stb_scan_grid(ctx, n_virtual, tier == STB_TIER_Q8 ? STB_Q8_SCAN_U : STB_SCAN_U);
+  const unsigned grid = stb_scan_grid(ctx, ranges.n_virtual, tier == STB_TIER_Q8 ? STB_Q8_SCAN_U : STB_SCAN_U);
   if (tier == STB_TIER_Q8) {
     if (!c->q8) { stb_set_error("scan_hist: q8 tier unavailable"); return STB_ERR_STATE; }
-    if (n_ranges > 0) stb_scan_hist_kernel<STB_Q8_SCAN_U, true, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, hist_dev, c->q8, c->q8_scale);
+    if (ranges.n > 0) stb_scan_hist_kernel<STB_Q8_SCAN_U, true, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, hist_dev, c->q8, c->q8_scale);
     else stb_scan_hist_kernel<STB_Q8_SCAN_U, false, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, hist_dev, c->q8, c->q8_scale);
-  } else if (n_ranges > 0)
+  } else if (ranges.n > 0)
     stb_scan_hist_kernel<STB_SCAN_U, true><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, hist_dev, nullptr, nullptr);
   else
     stb_scan_hist_kernel<STB_SCAN_U, false><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, hist_dev, nullptr, nullptr);
@@ -1910,21 +1906,21 @@ stb_debug_scan_kernel(const ScanArgs scan, const uint8_t *shadow, const uint8_t 
   else stb_scan_rows<U, RANGES>(scan, sink);
 }
 
-int stb_launch_debug_scan(stb_ctx *ctx, const stb_corpus *c, int tier, const float *q_dev, const uint64_t *ranges_dev,
-                          uint32_t n_ranges, uint64_t n_virtual, float *score, unsigned int *seen) {
-  const ScanArgs a = stb_scan_args(c, q_dev, ranges_dev, n_ranges, n_virtual);
+int stb_launch_debug_scan(stb_ctx *ctx, const stb_corpus *c, int tier, const float *q_dev, const StbRowRanges &ranges,
+                          float *score, unsigned int *seen) {
+  const ScanArgs a = stb_scan_args(c, q_dev, ranges);
   const DumpSink sink{score, seen};
-  const bool r = n_ranges > 0;
+  const bool r = ranges.n > 0;
   if (tier == STB_TIER_Q8) {
-    const unsigned grid = stb_scan_grid(ctx, n_virtual, STB_Q8_SCAN_U);
+    const unsigned grid = stb_scan_grid(ctx, ranges.n_virtual, STB_Q8_SCAN_U);
     if (r) stb_debug_scan_kernel<STB_Q8_SCAN_U, true, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, nullptr, c->q8, c->q8_scale, sink);
     else stb_debug_scan_kernel<STB_Q8_SCAN_U, false, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, nullptr, c->q8, c->q8_scale, sink);
   } else if (tier == STB_TIER_H16) {
-    const unsigned grid = stb_scan_grid(ctx, n_virtual, STB_SHADOW_SCAN_U);
+    const unsigned grid = stb_scan_grid(ctx, ranges.n_virtual, STB_SHADOW_SCAN_U);
     if (r) stb_debug_scan_kernel<STB_SHADOW_SCAN_U, true, 1><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, c->shadow, nullptr, nullptr, sink);
     else stb_debug_scan_kernel<STB_SHADOW_SCAN_U, false, 1><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, c->shadow, nullptr, nullptr, sink);
   } else {
-    const unsigned grid = stb_scan_grid(ctx, n_virtual, STB_SCAN_U);
+    const unsigned grid = stb_scan_grid(ctx, ranges.n_virtual, STB_SCAN_U);
     if (r) stb_debug_scan_kernel<STB_SCAN_U, true, 0><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, nullptr, nullptr, nullptr, sink);
     else stb_debug_scan_kernel<STB_SCAN_U, false, 0><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, nullptr, nullptr, nullptr, sink);
   }
@@ -1944,10 +1940,10 @@ stb_debug_q4_kernel(const ScanArgs scan, const uint8_t *q8, const float *q8_scal
   stb_scan_q4<STB_Q4_SCAN_U, RANGES, 1>(scan, q8, q8_scale, q4a, scratch, scratch + STB_Q4_QUEUE, s, nullptr, &dump);
 }
 
-int stb_launch_debug_q4(stb_ctx *ctx, const stb_corpus *c, const float *q_dev, uint32_t top_k, const uint64_t *ranges_dev,
-                        uint32_t n_ranges, uint64_t n_virtual, unsigned long long *words, unsigned long long *refined,
-                        int pin, float *u4, float *t, float *l8, float *u8, unsigned int *seen) {
-  const ScanArgs a = stb_scan_args(c, q_dev, ranges_dev, n_ranges, n_virtual);
+int stb_launch_debug_q4(stb_ctx *ctx, const stb_corpus *c, const float *q_dev, uint32_t top_k, const StbRowRanges &ranges,
+                        unsigned long long *words, unsigned long long *refined, int pin, float *u4, float *t, float *l8,
+                        float *u8, unsigned int *seen) {
+  const ScanArgs a = stb_scan_args(c, q_dev, ranges);
   StbQ4Args q4a;
   q4a.plane = c->q4;
   q4a.sr = c->q4_sr;
@@ -1957,8 +1953,8 @@ int stb_launch_debug_q4(stb_ctx *ctx, const stb_corpus *c, const float *q_dev, u
   q4a.refined = refined;
   const DumpSink sink{u8, seen};
   const StbQ4Dump dump{u4, t, l8, pin};
-  const unsigned grid = stb_scan_grid(ctx, n_virtual, STB_Q4_SCAN_U);
-  if (n_ranges > 0) stb_debug_q4_kernel<true><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, c->q8, c->q8_scale, q4a, sink, dump);
+  const unsigned grid = stb_scan_grid(ctx, ranges.n_virtual, STB_Q4_SCAN_U);
+  if (ranges.n > 0) stb_debug_q4_kernel<true><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, c->q8, c->q8_scale, q4a, sink, dump);
   else stb_debug_q4_kernel<false><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, c->q8, c->q8_scale, q4a, sink, dump);
   STB_CUDA(cudaGetLastError());
   ctx->kernel_launches++;
