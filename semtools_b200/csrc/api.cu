@@ -1493,8 +1493,9 @@ static int k2_query_tiles(stb_ctx *ctx, K2Copy copy, const float *q_dev, uint32_
 // GEMM pass p of the m_tiles query tiles in ctx->bq_tiles over the corpus's `copy`
 static int k2_gemm(stb_ctx *ctx, const stb_corpus *corpus, K2Copy copy, uint32_t m_tiles, StbGemmPass p) {
   p.a_tiles = ctx->bq_tiles; p.m_tiles = m_tiles; p.n_rows = corpus->n;
-  return copy == K2Copy::kQ8 ? stb_launch_gemm_q8(ctx, p, corpus->q8, corpus->q8_scale, ctx->b_q8c)
-                             : stb_launch_gemm_shadow(ctx, p, corpus->shadow);
+  if (copy == K2Copy::kQ8) { p.copy = STB_GEMM_Q8; p.b_tiles = corpus->q8; p.q8_scale = corpus->q8_scale; p.qc = ctx->b_q8c; }
+  else p.b_tiles = corpus->shadow;
+  return stb_launch_gemm(ctx, p);
 }
 
 // The top-k passes of routes 2, 3, 7 and 8 (batch_scan.cu) on `copy`: query tiles -> sampled threshold ->
@@ -2406,8 +2407,9 @@ int stb_debug_batch_params(int *shadow_is_f16, double *eps) {
 }
 
 // ------------------------------------------------------------------- K2 debug hook ---
-// Runs shadow build + wgmma GEMM on host inputs and returns the FULL approximate score
-// matrix (tests only: validates descriptors / accumulator layout / epilogue against a reference matmul).
+// Runs shadow build + wgmma GEMM on host inputs and returns the FULL approximate score matrix (the debug pass) and
+// the per-32-row maxima (the sampling pass) (tests only: validates descriptors / accumulator layout / epilogues
+// against a reference matmul).
 int stb_debug_batch_gemm(stb_ctx *ctx, const float *q, uint32_t nq, const float *rows, uint64_t n,
                          float *out_full, float *out_submax) {
   int rc = ctx_use(ctx);
@@ -2430,8 +2432,11 @@ int stb_debug_batch_gemm(stb_ctx *ctx, const float *q, uint32_t nq, const float 
   if (e == cudaSuccess) rc = stb_launch_shadow_build(ctx, dq, nq, 128, da, dbad);
   if (e == cudaSuccess && rc == STB_OK) rc = stb_launch_shadow_build(ctx, dr, n, 256, db, dbad);
   StbGemmPass p;
-  p.a_tiles = da; p.m_tiles = m_tiles; p.n_tiles = n_tiles; p.submax = dsub; p.tilemax = dtile; p.full_out = dfull;
-  if (e == cudaSuccess && rc == STB_OK) rc = stb_launch_gemm_shadow(ctx, p, db);
+  p.epi = STB_EPI_DEBUG; p.a_tiles = da; p.b_tiles = db; p.m_tiles = m_tiles; p.n_tiles = n_tiles; p.n_rows = n;
+  p.full_out = dfull;
+  if (e == cudaSuccess && rc == STB_OK) rc = stb_launch_gemm(ctx, p);
+  p.epi = STB_EPI_SAMPLE; p.submax = dsub; p.tilemax = dtile;
+  if (e == cudaSuccess && rc == STB_OK) rc = stb_launch_gemm(ctx, p);
   if (e == cudaSuccess && rc == STB_OK) e = cudaMemcpyAsync(out_full, dfull, q_pad * n_pad * 4, cudaMemcpyDeviceToHost, ctx->stream);
   if (e == cudaSuccess && rc == STB_OK && out_submax) e = cudaMemcpyAsync(out_submax, dsub, (size_t)n_tiles * 8 * q_pad * 4, cudaMemcpyDeviceToHost, ctx->stream);
   if (e == cudaSuccess && rc == STB_OK) e = cudaStreamSynchronize(ctx->stream);
@@ -2462,11 +2467,12 @@ int stb_debug_batch_q8_gemm(stb_ctx *ctx, const stb_corpus *corpus_c, const floa
       (rc = ddot.alloc(q_pad * n_pad)) != STB_OK || (rc = du.alloc(q_pad * n_pad)) != STB_OK || (rc = dl.alloc(q_pad * n_pad)) != STB_OK)
     return rc;
   StbGemmPass p;
-  p.epi = STB_EPI_DEBUG; p.a_tiles = da; p.m_tiles = m_tiles; p.n_tiles = (uint32_t)(n_pad / 256); p.n_rows = n;
+  p.copy = STB_GEMM_Q8; p.epi = STB_EPI_DEBUG; p.a_tiles = da; p.m_tiles = m_tiles; p.n_tiles = (uint32_t)(n_pad / 256);
+  p.n_rows = n; p.b_tiles = corpus->q8; p.q8_scale = corpus->q8_scale; p.qc = dc;
   p.dot_out = ddot; p.u_out = du; p.l_out = dl;
   STB_CUDA(cudaMemcpyAsync(dq, q, (size_t)nq * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
   if ((rc = stb_launch_q8_query_tiles(ctx, dq, nq, (uint32_t)q_pad, da, dc, dbad, d16)) != STB_OK ||
-      (rc = stb_launch_gemm_q8(ctx, p, corpus->q8, corpus->q8_scale, dc)) != STB_OK)
+      (rc = stb_launch_gemm(ctx, p)) != STB_OK)
     return rc;
   STB_CUDA(cudaMemcpyAsync(q16, d16, (size_t)nq * STB_D * sizeof(int16_t), cudaMemcpyDeviceToHost, ctx->stream));
   STB_CUDA(cudaMemcpy2DAsync(dot, n * 4, ddot, n_pad * 4, n * 4, nq, cudaMemcpyDeviceToHost, ctx->stream));

@@ -19,6 +19,8 @@
 //                               L2 (64 KB streamed per 16.8 MFLOP).
 //                               Epilogue: max over each 32-row sub-tile of the accumulator
 //                               fragments (lane-quad shuffles) -> submax[subtile][query].
+//                               The same kernel serves pipeline v2, the filtered routes and
+//                               the q8 copy (route 7 below).
 //   3. stb_batch_select_kernel  per query: the 32 sub-tiles with the largest maxima.
 //   4. stb_batch_finish_kernel  per query: exact canonical f64 re-score of the 32x32
 //                               candidate rows, sort by (distance,row), top-k, and the
@@ -32,6 +34,7 @@
 #include <math_constants.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "common.cuh"
 #include "row_encode.cuh"
@@ -109,6 +112,10 @@ __device__ __forceinline__ void wg_reg_fence(float (&d)[128]) {
 #pragma unroll
   for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+__device__ __forceinline__ void wg_reg_fence(int32_t (&d)[128]) {
+#pragma unroll
+  for (int i = 0; i < 128; ++i) asm volatile("" : "+r"(d[i])::"memory");
+}
 __device__ __forceinline__ void wg_mma_m64n256k16(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
@@ -141,6 +148,53 @@ __device__ __forceinline__ void wg_mma_m64n256k16(float (&d)[128], uint64_t ades
         "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
         "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
       : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+__device__ __forceinline__ void wg_mma_m64n256k32_s8(int32_t (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k32.s32.s8.s8 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p;\n\t}"
+      :
+        "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+        "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+        "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+        "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+        "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+        "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+        "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+        "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]),
+        "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]),
+        "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79]),
+        "+r"(d[80]), "+r"(d[81]), "+r"(d[82]), "+r"(d[83]), "+r"(d[84]), "+r"(d[85]), "+r"(d[86]), "+r"(d[87]),
+        "+r"(d[88]), "+r"(d[89]), "+r"(d[90]), "+r"(d[91]), "+r"(d[92]), "+r"(d[93]), "+r"(d[94]), "+r"(d[95]),
+        "+r"(d[96]), "+r"(d[97]), "+r"(d[98]), "+r"(d[99]), "+r"(d[100]), "+r"(d[101]), "+r"(d[102]), "+r"(d[103]),
+        "+r"(d[104]), "+r"(d[105]), "+r"(d[106]), "+r"(d[107]), "+r"(d[108]), "+r"(d[109]), "+r"(d[110]), "+r"(d[111]),
+        "+r"(d[112]), "+r"(d[113]), "+r"(d[114]), "+r"(d[115]), "+r"(d[116]), "+r"(d[117]), "+r"(d[118]), "+r"(d[119]),
+        "+r"(d[120]), "+r"(d[121]), "+r"(d[122]), "+r"(d[123]), "+r"(d[124]), "+r"(d[125]), "+r"(d[126]), "+r"(d[127])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+__device__ __forceinline__ void tma_load_2d(void *dst_smem, const CUtensorMap *map, int x, int y, uint64_t *bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
+          smem_u32(dst_smem)),
+      "l"(reinterpret_cast<uint64_t>(map)), "r"(x), "r"(y), "r"(smem_u32(bar))
+      : "memory");
+}
+__device__ __forceinline__ void tma_load_1d(void *dst_smem, const CUtensorMap *map, int x, uint64_t *bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.1d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2}], [%3];" ::"r"(
+          smem_u32(dst_smem)),
+      "l"(reinterpret_cast<uint64_t>(map)), "r"(x), "r"(smem_u32(bar))
+      : "memory");
 }
 
 // Shared-memory matrix descriptor, K-major operand, 128-byte swizzle (sm_90 wgmma format):
@@ -178,104 +232,264 @@ stb_shadow_build_kernel(const float4 *__restrict__ rows, uint64_t first_row, uin
 }
 
 // ------------------------------------------------------------------- 2. wgmma GEMM ---
-struct GemmArgs {
-  const uint8_t *a_tiles;     // query shadow: m_tiles x (4 slabs x 16 KiB)
-  const uint8_t *b_tiles;     // corpus shadow: n_tiles x (4 slabs x 32 KiB)
-  uint32_t m_tiles;           // ceil(Q / 128)
-  uint32_t n_tiles;           // ceil(N / 256)
-  // maxima are stored [query tile][sub-tile or tile][128 queries]: the selection pass streams
-  // them contiguously
-  union {
-    float *submax;            // [m_tiles][n_tiles * 8][128]  per-32-row maxima
-    const uint4 *items;       // STB_GEMM_WORK (below)
-  };
-  union {
-    float *tilemax;           // [m_tiles][n_tiles][128]      per-256-row maxima (STB_GEMM_WORK: [m_tiles][tile_stride][128])
-    const uint32_t *slot_row; // STB_GEMM_WORK, EPI 1 (below)
-  };
-  union {
-    float *full_out;          // debug: full score matrix [m_tiles*128][n_tiles*256] or null
-    const uint32_t *item_off; // STB_GEMM_WORK (below)
-  };
-  uint32_t tile_stride;       // corpus tile t of this launch is shadow tile t * tile_stride (sampling pass)
-  // EPI == 1 (candidate-emitting epilogue, pipeline v2):
-  const float *thr;           // [q_pad] per-query score threshold (+inf for padding queries)
-  uint32_t *cand_cnt;         // [q_pad][grid] candidates emitted per (query, CTA) (> cand_cap: overflow marker)
-  uint64_t *cand_keys;        // [q_pad][grid][cand_cap] keys (score desc, local row)
-  uint32_t cand_cap;          // per-segment capacity
-  uint64_t n_rows;            // real corpus rows (padding rows of the last tile are never emitted)
-  // FILTER (stb_search_batch_filtered): tile t of the launch is shadow tile tile_ids[t * tile_stride]
-  const uint32_t *tile_ids;   // listed tiles: the shadow tiles holding an eligible row, ascending
-  const uint32_t *bitmap;     // eligible local rows, 1 bit each: 8 words per shadow tile
-  // EPI == 2 (stb_search_batch_threshold's re-emission): segment (q, CTA) is cand_keys[seg_off[q * grid + CTA],
-  // seg_off[q * grid + CTA + 1]), sized by the first pass's exact counts; cand_cnt holds the cursors
-  union {
-    const uint64_t *seg_off;  // [q_pad * grid + 1]
-    const uint32_t *cta_tiles;  // STB_GEMM_WORK (below)
-  };
-  // STB_GEMM_WORK (stb_search_batch_subsets; the unions keep the layout the other modes compile against): CTA b
-  // walks the corpus tiles u in [cta_tiles[b], cta_tiles[b + 1]) (shadow tile tile_ids[u]); tile u's work items
-  // are items[item_off[u], item_off[u + 1]), each {query tile, mask slot of half 0, mask slot of half 1, sample
-  // columns}: a mask slot is 8 bitmap words at bitmap + 8 * slot; the sample columns (EPI 0: low / high 16
-  // bits, 0xffff: none) index tilemax [m_tiles][tile_stride][128].  EPI 1 writes query slot s's keys and count
-  // at row slot_row[s] (~0: a padding slot, which never emits).
-};
-
-// Filter modes of the GEMM (STB_GEMM_ALL, _LISTED, _WORK: common.cuh): every tile, the listed tiles of one filter,
-// or a work list of (query tile, masks) per corpus tile, one filter per 64-query half
-
-// warpgroup 0: bulk-copy producer (one thread); warpgroups 1 and 2: wgmma + epilogue, each on
-// 64 of the 128 queries of a query tile (m64n256 accumulators, 128 f32 registers per thread)
+// One kernel for every pass of K2's GEMM (StbGemmPass, common.cuh): stb_batch_gemm_kernel<Copy, SELECT, EPI>.
+// Warpgroup 0 is the copy producer (one thread); warpgroups 1 and 2 run wgmma and the epilogue, each on 64 of the
+// 128 queries of a query tile (m64n256 accumulators, 128 registers per thread).  A corpus tile stays resident in
+// shared memory while the query tiles of its items stream through a 6-slab ring from L2.
+//   Copy    the corpus copy: ShadowCopy (16-bit shadow) or Q8Copy (q8 codes and scales)
+//   SELECT  the corpus tiles a CTA walks and the query tiles of each (TileWalk): STB_GEMM_ALL, _LISTED or _WORK
+//   EPI     StbGemmEpi: sampled maxima, emission into per-(query, CTA) segments, or the debug score matrix
 #define STB_GEMM_THREADS 384
 #define STB_GEMM_CONSUMER_WARPS 8
-#define STB_GEMM_SMEM (STB_N_SLABS * STB_B_SLAB_BYTES + STB_A_RING * STB_A_SLAB_BYTES + 1024 + 256)
-// STB_GEMM_WORK: three 64-byte mask buffers behind the barriers instead of two 32-byte ones
-#define STB_GEMM_SMEM_WORK (STB_GEMM_SMEM + 128)
-static_assert(STB_GEMM_SMEM_WORK <= 227 * 1024, "GEMM shared memory");
+// Shared memory: the corpus slabs, the query ring, the copy's per-tile extra, then 256 bytes for up to 24
+// barriers and the mask words behind them (STB_GEMM_WORK's three 64-byte mask buffers take 128 bytes more), and
+// the 1024 bytes of alignment slack.
+template <class Copy, int SELECT>
+constexpr int stb_gemm_smem() {
+  return Copy::kBSlabs * STB_B_SLAB_BYTES + STB_A_RING * STB_A_SLAB_BYTES + Copy::kExtraSmem + 256 +
+         (SELECT == STB_GEMM_WORK ? 128 : 0) + 1024;
+}
 
-// FILTER == STB_GEMM_WORK (EPI 0 or 1), the body of stb_batch_gemm_kernel below on its shared memory and
-// initialised barriers: the same pipeline and epilogues per 64-query half, over each corpus tile's work items
-// (GemmArgs) instead of every query tile.  Kept apart from the kernel body so the other modes compile as they
-// did.  An item's 2 x 8 mask words arrive with its first query slab; item i of a CTA uses mask buffer i % 3:
-// item i + 3's slab 0 reuses the ring slot of item i + 1's slab 2, which every consumer warp releases only
-// after the epilogue of item i.
-template <int EPI>
-__device__ __forceinline__ void stb_batch_gemm_work(const GemmArgs &args, uint8_t *sB, uint8_t *sA, uint64_t *bars) {
-  uint64_t *b_full = bars + 0, *b_empty = bars + STB_N_SLABS;
-  uint64_t *a_full = bars + 2 * STB_N_SLABS, *a_empty = a_full + STB_A_RING;
-  uint32_t *s_mask = reinterpret_cast<uint32_t *>(bars + 24);       // [3][2][8]
-  static_assert(24 * 8 + 3 * 16 * 4 <= 256 + (STB_GEMM_SMEM_WORK - STB_GEMM_SMEM), "work-item mask words must fit");
+// rows of the 32-row sub-tile at row r0 below n_rows, 1 bit each
+__device__ __forceinline__ uint32_t stb_rows_below(uint64_t r0, uint64_t n_rows) {
+  return r0 + 32 > n_rows ? (r0 < n_rows ? (1u << (uint32_t)(n_rows - r0)) - 1u : 0u) : 0xffffffffu;
+}
+
+// The 16-bit shadow: a corpus tile is four 32 KiB K-slabs, stored in HBM already in the swizzled tile layout and
+// fetched with plain bulk copies; query slab s multiplies corpus slab s with four wgmma m64n256k16 (f32
+// accumulators).  The scores are the accumulators.  The shadow's padding rows are zero rows and count in the
+// sampled maxima (pipeline v1's sub-tile maxima cover whole sub-tiles); they never emit.
+struct ShadowCopy {
+  using Acc = float;
+  static constexpr int kBSlabs = 4, kExtraSmem = 0, kExtraBytes = 0;
+  static constexpr bool kSampleBelowN = false;
+  const uint8_t *tiles;
+  __device__ explicit ShadowCopy(const StbGemmPass &a) : tiles(a.b_tiles) {}
+  __device__ void load_extra(uint8_t *, uint32_t, uint64_t, uint64_t *) const {}
+  __device__ void load_slab(uint8_t *dst, int s, uint64_t tile, uint64_t *bar) const {
+    bulk_g2s(dst, tiles + (tile * STB_N_SLABS + s) * STB_B_SLAB_BYTES, STB_B_SLAB_BYTES, bar);
+  }
+  __device__ static void mma(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+    wg_mma_m64n256k16(d, adesc, bdesc, acc);
+  }
+  __device__ static void before_slab(float (&)[128], int) {}
+  struct Scorer {
+    template <bool LOWER>
+    __device__ void scores(const float (&d)[128], int c, uint32_t, float (&v)[4][2][2]) const {
+#pragma unroll
+      for (int ii = 0; ii < 4; ++ii)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) v[ii][h][e] = d[16 * c + 4 * ii + 2 * h + e];
+    }
+    // the f32 scores, full_out [m_tiles * 128][n_tiles * 256]
+    __device__ void debug(const StbGemmPass &a, const float (&d)[128], int i, int, uint32_t, size_t o) const {
+      *reinterpret_cast<float2 *>(a.full_out + o) = make_float2(d[i], d[i + 1]);
+    }
+  };
+  __device__ Scorer scorer(const StbGemmPass &, const uint8_t *, uint32_t, uint32_t) const { return {}; }
+};
+
+// The q8 copy: a corpus tile is two K-slabs of codes (bytes 0-127 and 128-255 of each row, 32 KiB each) loaded
+// with the tensor maps of q8_tensor_maps, which apply the 128-byte swizzle on the way in (the q8 copy stays
+// row-major for K1 and zero-fills rows past n), and the tile's 256 scales (1 KiB) with slab 0, double-buffered by
+// tile parity: the producer refills buffer (it + 1) & 1 only after every consumer warp released slab 0 of tile it,
+// which it does after the epilogues of tile it - 1.  The query slabs are hi 0-127, hi 128-255, lo 0-127, lo
+// 128-255 (stb_q8_query_tiles_kernel): a consumer warpgroup runs the hi slabs on corpus slabs 0 and 1 (wgmma
+// m64n256k32 s8), waits, multiplies its s32 accumulators by 256 and accumulates the lo slabs on top, so corpus
+// slab 0 is free after the lo pass of query slab 2.  The scores are K1's bounds: l (sampling) and u (emission).
+struct Q8Copy {
+  using Acc = int32_t;
+  static constexpr int kBSlabs = 2, kExtraSmem = 2 * STB_B_TILE * 4, kExtraBytes = STB_B_TILE * 4;
+  static constexpr bool kSampleBelowN = true;    // each sampled maximum of l is a real row's
+  const CUtensorMap *codes_map, *scale_map;
+  __device__ Q8Copy(const StbGemmPass &, const CUtensorMap &codes, const CUtensorMap &scales)
+      : codes_map(&codes), scale_map(&scales) {}
+  __device__ void load_extra(uint8_t *extra, uint32_t it, uint64_t tile, uint64_t *bar) const {
+    tma_load_1d(extra + (it & 1) * (STB_B_TILE * 4), scale_map, (int)(tile * STB_B_TILE), bar);
+  }
+  __device__ void load_slab(uint8_t *dst, int s, uint64_t tile, uint64_t *bar) const {
+    tma_load_2d(dst, codes_map, s * 128, (int)(tile * STB_B_TILE), bar);
+  }
+  __device__ static void mma(int32_t (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+    wg_mma_m64n256k32_s8(d, adesc, bdesc, acc);
+  }
+  __device__ static void before_slab(int32_t (&d)[128], int s) {
+    if (s == 2) {
+      // the hi products are complete: dot = 256 hi.x8 + lo.x8 (|256 hi.x8| <= 256 * 127 * 127 * 256 < 2^31)
+      wg_wait<0>();
+      wg_reg_fence(d);
+#pragma unroll
+      for (int i = 0; i < 128; ++i) d[i] *= 256;
+      wg_reg_fence(d);
+    }
+  }
+  struct Scorer {
+    const float *sc;                     // the tile's scales
+    float4 qc[2];                        // {1/S, h_l1, e_q, S} of queries qrow and qrow + 8
+    // l (LOWER) or u of sub-tile c, with the expressions of K1's bounds (scan_topk.cu)
+    template <bool LOWER>
+    __device__ void scores(const int32_t (&d)[128], int c, uint32_t quad, float (&v)[4][2][2]) const {
+#pragma unroll
+      for (int ii = 0; ii < 4; ++ii) {
+        const float2 s2 = *reinterpret_cast<const float2 *>(sc + c * STB_SUB + ii * 8 + quad * 2);
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const float x = (float)d[16 * c + 4 * ii + 2 * h + e];
+            v[ii][h][e] = LOWER ? fmaf(e ? s2.y : s2.x, fmaf(x, qc[h].x, -qc[h].y), -qc[h].z) - (float)STB_Q8_SCAN_EPS
+                                : fmaf(e ? s2.y : s2.x, fmaf(x, qc[h].x, qc[h].y), qc[h].z);
+          }
+      }
+    }
+    // dot, u and l: dot_out, u_out, l_out [m_tiles * 128][n_tiles * 256]
+    __device__ void debug(const StbGemmPass &a, const int32_t (&d)[128], int i, int h, uint32_t col, size_t o) const {
+      const float2 s2 = *reinterpret_cast<const float2 *>(sc + col);
+      const int32_t d0 = d[i], d1 = d[i + 1];
+      *reinterpret_cast<int2 *>(a.dot_out + o) = make_int2(d0, d1);
+      *reinterpret_cast<float2 *>(a.u_out + o) =
+          make_float2(fmaf(s2.x, fmaf((float)d0, qc[h].x, qc[h].y), qc[h].z), fmaf(s2.y, fmaf((float)d1, qc[h].x, qc[h].y), qc[h].z));
+      *reinterpret_cast<float2 *>(a.l_out + o) =
+          make_float2(fmaf(s2.x, fmaf((float)d0, qc[h].x, -qc[h].y), -qc[h].z) - (float)STB_Q8_SCAN_EPS,
+                      fmaf(s2.y, fmaf((float)d1, qc[h].x, -qc[h].y), -qc[h].z) - (float)STB_Q8_SCAN_EPS);
+    }
+  };
+  __device__ Scorer scorer(const StbGemmPass &a, const uint8_t *extra, uint32_t it, uint32_t q0) const {
+    Scorer s;
+    s.sc = reinterpret_cast<const float *>(extra) + (it & 1) * STB_B_TILE;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) s.qc[h] = __ldg(a.qc + q0 + 8 * h);
+    return s;
+  }
+};
+
+// The corpus tiles a CTA walks and the items (query tiles) of each, the same for the producer and the consumers.
+//   STB_GEMM_ALL     launch tile t = blockIdx.x + it * gridDim.x is corpus tile t * tile_stride; its items are the
+//                    m_tiles query tiles.
+//   STB_GEMM_LISTED  launch tile t is corpus tile tile_ids[t * tile_stride], and only the eligible rows of bitmap
+//                    count.  The tile's 8 mask words arrive with corpus slab 0 into mask slot it & 1: the producer
+//                    refills the slot of tile it - 2 only after every consumer warp released slab 0 of tile it - 1,
+//                    which it does only after the epilogues of tile it - 2.
+//   STB_GEMM_WORK    CTA b walks u in [cta_tiles[b], cta_tiles[b + 1]), corpus tile tile_ids[u], whose items are
+//                    items[item_off[u], item_off[u + 1]): {query tile, mask slot of half 0, of half 1, sample
+//                    columns}.  A mask slot is 8 bitmap words at bitmap + 8 * slot, one filter per 64-query half;
+//                    an item's 2 x 8 words arrive with its first query slab, and item i of a CTA uses mask buffer
+//                    i % 3: item i + 3's slab 0 reuses the ring slot of item i + 1's slab 2, which every consumer
+//                    warp releases only after the epilogue of item i.  The sample columns (half 0: low 16 bits,
+//                    half 1: high, 0xffff: none) index tilemax [m_tiles][tile_stride][128], and query slot q's
+//                    output row is slot_row[q] (~0: a padding slot, which never emits).
+template <int SELECT>
+struct TileWalk {
+  const StbGemmPass &a;
+  uint32_t first, count;
+  __device__ explicit TileWalk(const StbGemmPass &a) : a(a) {
+    if constexpr (SELECT == STB_GEMM_WORK) {
+      first = __ldg(a.cta_tiles + blockIdx.x);
+      count = __ldg(a.cta_tiles + blockIdx.x + 1) - first;
+    } else {
+      first = blockIdx.x;
+      count = (a.n_tiles > blockIdx.x) ? (a.n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+    }
+  }
+  // the launch's tile of iteration it
+  __device__ uint64_t t(uint32_t it) const {
+    return SELECT == STB_GEMM_WORK ? (uint64_t)(first + it) : blockIdx.x + (uint64_t)it * gridDim.x;
+  }
+  __device__ uint64_t tile(uint32_t it) const {
+    if constexpr (SELECT == STB_GEMM_ALL) return t(it) * a.tile_stride;
+    if constexpr (SELECT == STB_GEMM_LISTED) return __ldg(a.tile_ids + t(it) * a.tile_stride);
+    return __ldg(a.tile_ids + t(it));
+  }
+  __device__ uint32_t item_begin(uint32_t it) const { return SELECT == STB_GEMM_WORK ? __ldg(a.item_off + t(it)) : 0u; }
+  __device__ uint32_t item_end(uint32_t it) const { return SELECT == STB_GEMM_WORK ? __ldg(a.item_off + t(it) + 1) : a.m_tiles; }
+  __device__ uint4 item(uint32_t w) const { return SELECT == STB_GEMM_WORK ? __ldg(a.items + w) : make_uint4(w, 0u, 0u, 0u); }
+  // the 8 mask words of this half of item n (the CTA's n-th) of tile it, sub-tile c at [c]; null for STB_GEMM_ALL
+  __device__ const uint32_t *mask(const uint32_t *s_mask, uint32_t it, uint32_t n, uint32_t half) const {
+    if constexpr (SELECT == STB_GEMM_LISTED) return s_mask + (it & 1) * 8;
+    if constexpr (SELECT == STB_GEMM_WORK) return s_mask + (n % 3) * 16 + half * 8;
+    return nullptr;
+  }
+  // the output row of query slot q: ~0 never emits
+  __device__ uint32_t out_row(uint32_t q) const { return SELECT == STB_GEMM_WORK ? __ldg(a.slot_row + q) : q; }
+  // where this half's sampled maxima of item it go (tilemax + 128 * column), or null
+  __device__ float *sample_at(uint32_t it, uint4 item, uint32_t half) const {
+    if constexpr (SELECT == STB_GEMM_WORK) {
+      const uint32_t col = half ? (item.w >> 16) : (item.w & 0xffffu);
+      return col == 0xffffu ? nullptr : a.tilemax + ((size_t)item.x * a.tile_stride + col) * STB_A_TILE;
+    }
+    return a.tilemax + ((size_t)item.x * a.n_tiles + t(it)) * STB_A_TILE;
+  }
+};
+
+__device__ __forceinline__ float quad_max(float x) {
+  x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 1));
+  return fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 2));
+}
+
+template <class Copy, int SELECT, int EPI, class... Maps>
+__global__ void __launch_bounds__(STB_GEMM_THREADS, 1)
+stb_batch_gemm_kernel(const StbGemmPass a, const __grid_constant__ Maps... maps) {
+  static_assert(SELECT == STB_GEMM_ALL || EPI == STB_EPI_SAMPLE || EPI == STB_EPI_EMIT, "filters run the sampling and the emitting pass");
+  static_assert(2 * Copy::kBSlabs + 2 * STB_A_RING <= 24, "barriers must fit");
+  static_assert(24 * 8 + 2 * 8 * 4 <= 256 && 24 * 8 + 3 * 16 * 4 <= 256 + 128, "mask words must fit behind the barriers");
   static_assert(STB_A_RING == 6 && STB_N_SLABS == 4, "the mask buffer rule (item % 3) assumes this ring");
+  extern __shared__ uint8_t smem_raw[];
+  // 1024-byte alignment required by the 128-byte swizzle atoms
+  uint8_t *sB = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint8_t *sA = sB + Copy::kBSlabs * STB_B_SLAB_BYTES;
+  uint8_t *extra = sA + STB_A_RING * STB_A_SLAB_BYTES;
+  uint64_t *bars = reinterpret_cast<uint64_t *>(extra + Copy::kExtraSmem);
+  uint64_t *b_full = bars + 0, *b_empty = bars + Copy::kBSlabs;      // one pair per corpus slab
+  uint64_t *a_full = bars + 2 * Copy::kBSlabs, *a_empty = a_full + STB_A_RING;
+  uint32_t *s_mask = reinterpret_cast<uint32_t *>(bars + 24);       // LISTED: [2][8], WORK: [3][2][8]
+  const Copy cp(a, maps...);
+  const TileWalk<SELECT> walk(a);
+
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t t0 = __ldg(args.cta_tiles + blockIdx.x), t1 = __ldg(args.cta_tiles + blockIdx.x + 1);
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < Copy::kBSlabs; ++i) { mbar_init(b_full + i, 1); mbar_init(b_empty + i, STB_GEMM_CONSUMER_WARPS); }
+    for (int i = 0; i < STB_A_RING; ++i) { mbar_init(a_full + i, 1); mbar_init(a_empty + i, STB_GEMM_CONSUMER_WARPS); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
 
   if (warp < 4) {
-    // ===== bulk-copy producer (one thread) =====
+    // ===== copy producer (one thread) =====
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (threadIdx.x == 0) {
       uint32_t a_cnt = 0;
-      for (uint32_t u = t0, it = 0; u < t1; ++u, ++it) {
-        const uint8_t *src = args.b_tiles + (uint64_t)__ldg(args.tile_ids + u) * (size_t)(STB_N_SLABS * STB_B_SLAB_BYTES);
-        for (int s = 0; s < STB_N_SLABS; ++s) {
+      for (uint32_t it = 0; it < walk.count; ++it) {
+        const uint64_t tile = walk.tile(it);
+        // corpus tile, slab by slab: slab s of the previous tile is released as soon as the last query slab on it
+        // retires, so the refill overlaps the remaining slabs
+        for (int s = 0; s < Copy::kBSlabs; ++s) {
           mbar_wait(b_empty + s, (it & 1) ^ 1);
-          mbar_expect_tx(b_full + s, STB_B_SLAB_BYTES);
-          bulk_g2s(sB + s * STB_B_SLAB_BYTES, src + (size_t)s * STB_B_SLAB_BYTES, STB_B_SLAB_BYTES, b_full + s);
+          if (s == 0) {
+            mbar_expect_tx(b_full, STB_B_SLAB_BYTES + Copy::kExtraBytes + (SELECT == STB_GEMM_LISTED ? 32 : 0));
+            if constexpr (SELECT == STB_GEMM_LISTED) bulk_g2s(s_mask + (it & 1) * 8, a.bitmap + tile * 8, 32, b_full);
+            cp.load_extra(extra, it, tile, b_full);
+          } else {
+            mbar_expect_tx(b_full + s, STB_B_SLAB_BYTES);
+          }
+          cp.load_slab(sB + s * STB_B_SLAB_BYTES, s, tile, b_full + s);
         }
-        const uint32_t w1 = __ldg(args.item_off + u + 1);
-        for (uint32_t w = __ldg(args.item_off + u); w < w1; ++w) {
-          const uint4 item = __ldg(args.items + w);
+        const uint32_t w1 = walk.item_end(it);
+        for (uint32_t w = walk.item_begin(it); w < w1; ++w) {
+          const uint4 item = walk.item(w);
           for (int s = 0; s < STB_N_SLABS; ++s, ++a_cnt) {
             const uint32_t slot = a_cnt % STB_A_RING;
             mbar_wait(a_empty + slot, ((a_cnt / STB_A_RING) & 1) ^ 1);
-            if (s == 0) {
+            if (SELECT == STB_GEMM_WORK && s == 0) {
               uint32_t *mk = s_mask + ((a_cnt / STB_N_SLABS) % 3) * 16;
               mbar_expect_tx(a_full + slot, STB_A_SLAB_BYTES + 64);
-              bulk_g2s(mk, args.bitmap + (size_t)item.y * 8, 32, a_full + slot);
-              bulk_g2s(mk + 8, args.bitmap + (size_t)item.z * 8, 32, a_full + slot);
+              bulk_g2s(mk, a.bitmap + (size_t)item.y * 8, 32, a_full + slot);
+              bulk_g2s(mk + 8, a.bitmap + (size_t)item.z * 8, 32, a_full + slot);
             } else {
               mbar_expect_tx(a_full + slot, STB_A_SLAB_BYTES);
             }
-            bulk_g2s(sA + slot * STB_A_SLAB_BYTES, args.a_tiles + ((size_t)item.x * STB_N_SLABS + s) * STB_A_SLAB_BYTES,
+            bulk_g2s(sA + slot * STB_A_SLAB_BYTES, a.a_tiles + ((size_t)item.x * STB_N_SLABS + s) * STB_A_SLAB_BYTES,
                      STB_A_SLAB_BYTES, a_full + slot);
           }
         }
@@ -284,242 +498,41 @@ __device__ __forceinline__ void stb_batch_gemm_work(const GemmArgs &args, uint8_
     return;
   }
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-  // ===== consumers (accumulator layout as in stb_batch_gemm_kernel) =====
-  const uint32_t half = (uint32_t)(warp >> 2) - 1u;
+  // ===== consumers: wgmma over one 64-query half of every item, then the epilogue =====
+  // Accumulator fragment of m64nN (PTX ISA, wgmma D layout): thread (warp w, lane l) of the warpgroup holds rows
+  // r = 16w + l/4 and r + 8; d[4i + e] is (r, 8i + 2(l%4) + e), d[4i + 2 + e] is (r + 8, same column).  So
+  // d[16c + 4ii + 2h + e] is query qrow + 8h, tile column 32c + 8ii + 2quad + e: a 32-row sub-tile c is
+  // d[16c .. 16c + 15], spread over a lane quad.
+  const uint32_t half = (uint32_t)(warp >> 2) - 1u;       // which 64 queries of the tile
   const uint32_t qrow = half * 64 + (warp & 3) * 16 + (lane >> 2);
   const uint32_t quad = lane & 3;
-  float d[128];
+  typename Copy::Acc d[128];
 #pragma unroll
-  for (int i = 0; i < 128; ++i) d[i] = 0.f;
+  for (int i = 0; i < 128; ++i) d[i] = 0;
   uint32_t a_cnt = 0;
-  for (uint32_t u = t0, it = 0; u < t1; ++u, ++it) {
-    const uint64_t tile_row0 = (uint64_t)__ldg(args.tile_ids + u) * STB_B_TILE;
-    const uint32_t w0 = __ldg(args.item_off + u), w1 = __ldg(args.item_off + u + 1);
+  for (uint32_t it = 0; it < walk.count; ++it) {
+    const uint32_t w0 = walk.item_begin(it), w1 = walk.item_end(it);
     for (uint32_t w = w0; w < w1; ++w, a_cnt += STB_N_SLABS) {
-      const uint4 item = __ldg(args.items + w);
-      const uint32_t m = item.x;
-      const uint32_t *mask = s_mask + ((a_cnt / STB_N_SLABS) % 3) * 16 + half * 8;   // this half's filter
-      const uint32_t q0 = m * STB_A_TILE + qrow;
+      const uint4 item = walk.item(w);
+      const uint32_t q0 = item.x * STB_A_TILE + qrow;
+      const bool last = w + 1 == w1;                      // the tile's last item releases its corpus slabs
+      // epilogue state, fetched while the MMAs run
+      const auto sco = cp.scorer(a, extra, it, q0);
       [[maybe_unused]] float thr[2];
-      [[maybe_unused]] uint32_t cnt[2], cnt0[2], qout[2];
-      if constexpr (EPI == 1) {
+      [[maybe_unused]] uint32_t qout[2], cnt[2], cnt0[2], seg_len[2];
+      [[maybe_unused]] uint64_t seg_base[2];
+      if constexpr (EPI == STB_EPI_EMIT || EPI == STB_EPI_EMIT_SIZED) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           // a padding slot never emits and owns no segment
-          const uint32_t r = __ldg(args.slot_row + q0 + 8 * h);
-          thr[h] = (r == 0xffffffffu) ? CUDART_INF_F : __ldg(args.thr + q0 + 8 * h);
-          qout[h] = (r == 0xffffffffu) ? 0u : r;
-          cnt0[h] = args.cand_cnt[(size_t)qout[h] * gridDim.x + blockIdx.x];
+          const uint32_t r = walk.out_row(q0 + 8 * h);
+          const bool pad = SELECT == STB_GEMM_WORK && r == 0xffffffffu;
+          thr[h] = pad ? CUDART_INF_F : __ldg(a.thr + q0 + 8 * h);
+          qout[h] = pad ? 0u : r;
+          cnt0[h] = a.cand_cnt[(size_t)qout[h] * gridDim.x + blockIdx.x];
           cnt[h] = cnt0[h];
-        }
-      }
-      wg_reg_fence(d);
-#pragma unroll
-      for (int s = 0; s < STB_N_SLABS; ++s) {
-        const uint32_t slot = (a_cnt + s) % STB_A_RING;
-        if (w == w0) mbar_wait(b_full + s, it & 1);
-        mbar_wait(a_full + slot, ((a_cnt + s) / STB_A_RING) & 1);
-        wg_fence();
-        const uint32_t a_addr = smem_u32(sA + slot * STB_A_SLAB_BYTES + half * (64 * 128));
-        const uint32_t b_addr = smem_u32(sB + s * STB_B_SLAB_BYTES);
-#pragma unroll
-        for (int k = 0; k < STB_SLAB_K / 16; ++k)
-          wg_mma_m64n256k16(d, wg_desc_sw128(a_addr + k * 32), wg_desc_sw128(b_addr + k * 32), (uint32_t)((s | k) != 0));
-        wg_commit();
-        if (s > 0) {
-          wg_wait<1>();
-          if (lane == 0) {
-            mbar_arrive(a_empty + (a_cnt + s - 1) % STB_A_RING);
-            if (w + 1 == w1) mbar_arrive(b_empty + s - 1);
-          }
-        }
-      }
-      wg_wait<0>();
-      wg_reg_fence(d);
-      if (lane == 0) {
-        mbar_arrive(a_empty + (a_cnt + STB_N_SLABS - 1) % STB_A_RING);
-        if (w + 1 == w1) mbar_arrive(b_empty + STB_N_SLABS - 1);
-      }
-
-      if constexpr (EPI == 0) {
-        // tile maximum over this half's eligible rows (ineligible scores -inf, as FILTER == STB_GEMM_LISTED),
-        // stored at the half's column of its group's sample (0xffff: the tile is not in that sample)
-        float tmx[2] = {-CUDART_INF_F, -CUDART_INF_F};
-#pragma unroll
-        for (int c = 0; c < STB_B_TILE / STB_SUB; ++c) {
-          const uint32_t mw = mask[c];
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            float mx = -CUDART_INF_F;
-#pragma unroll
-            for (int ii = 0; ii < 4; ++ii)
-#pragma unroll
-              for (int e = 0; e < 2; ++e)
-                mx = fmaxf(mx, ((mw >> (ii * 8 + quad * 2 + e)) & 1u) ? d[16 * c + 4 * ii + 2 * h + e] : -CUDART_INF_F);
-            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-            tmx[h] = fmaxf(tmx[h], mx);
-          }
-        }
-        const uint32_t col = half ? (item.w >> 16) : (item.w & 0xffffu);
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-          if (quad == (uint32_t)(2 + h) && col != 0xffffu)
-            args.tilemax[((size_t)m * args.tile_stride + col) * STB_A_TILE + qrow + 8 * h] = tmx[h];
-      } else {
-        // emission as stb_batch_gemm_kernel's EPI 1, into the segments of row qout
-#pragma unroll
-        for (int c = 0; c < STB_B_TILE / STB_SUB; ++c) {
-          const uint64_t row0 = tile_row0 + (uint64_t)c * STB_SUB;
-          const uint32_t mw = mask[c];
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            uint32_t hit = 0u;
-#pragma unroll
-            for (int ii = 0; ii < 4; ++ii)
-#pragma unroll
-              for (int e = 0; e < 2; ++e)
-                hit |= (d[16 * c + 4 * ii + 2 * h + e] >= thr[h] ? 1u : 0u) << (ii * 8 + quad * 2 + e);
-            hit |= __shfl_xor_sync(0xffffffffu, hit, 1);
-            hit |= __shfl_xor_sync(0xffffffffu, hit, 2);
-            if (row0 + 32 > args.n_rows) hit &= (row0 < args.n_rows) ? ((1u << (uint32_t)(args.n_rows - row0)) - 1u) : 0u;
-            hit &= mw;
-            uint64_t *seg = args.cand_keys + ((size_t)qout[h] * gridDim.x + blockIdx.x) * args.cand_cap;
-#pragma unroll
-            for (int ii = 0; ii < 4; ++ii)
-#pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const uint32_t b = ii * 8 + quad * 2 + e;
-                const uint32_t pos = cnt[h] + __popc(hit & ((1u << b) - 1u));
-                const uint64_t key = stb_make_key(d[16 * c + 4 * ii + 2 * h + e], (uint32_t)(row0 + b));
-                if (((hit >> b) & 1u) && pos < args.cand_cap) seg[pos] = key;
-              }
-            cnt[h] += __popc(hit);
-          }
-        }
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-          if (quad == 0 && cnt[h] != cnt0[h]) args.cand_cnt[(size_t)qout[h] * gridDim.x + blockIdx.x] = cnt[h];
-      }
-    }
-  }
-}
-
-// EPI 0: per-sub-tile / per-tile maxima (pipeline v1, and the sampling pass of v2).
-// EPI 1: emit every (query,row) whose approximate score reaches the query's threshold.
-// EPI 2: the same emission into exactly sized segments at args.seg_off (unfiltered only).
-// FILTER == STB_GEMM_LISTED: the CTAs walk the listed tiles (args.tile_ids) and only eligible rows count
-// (args.bitmap): EPI 0 takes each tile maximum over its eligible rows, EPI 1 emits eligible rows only.  The
-// tile's 8 bitmap words arrive with its first corpus slab, double-buffered behind the mbarriers.
-// FILTER == STB_GEMM_WORK: stb_batch_gemm_work above.
-template <int EPI, int FILTER>
-__global__ void __launch_bounds__(STB_GEMM_THREADS, 1)
-stb_batch_gemm_kernel(const GemmArgs args) {
-  extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment required by the 128-byte swizzle atoms
-  uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t *sB = smem;
-  uint8_t *sA = smem + STB_N_SLABS * STB_B_SLAB_BYTES;
-  uint64_t *bars = reinterpret_cast<uint64_t *>(sA + STB_A_RING * STB_A_SLAB_BYTES);
-  uint64_t *b_full = bars + 0, *b_empty = bars + STB_N_SLABS;      // one pair per K-slab
-  uint64_t *a_full = bars + 2 * STB_N_SLABS, *a_empty = a_full + STB_A_RING;
-  // FILTER: [2][8] bitmap words, slot it & 1 = the tile of iteration it (the 256 bytes behind the ring hold
-  // the 20 barriers, then these 64 bytes)
-  [[maybe_unused]] uint32_t *s_mask = reinterpret_cast<uint32_t *>(bars + 24);
-  static_assert(24 * 8 + 2 * 8 * 4 <= 256, "mask words must fit behind the barriers");
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < STB_N_SLABS; ++i) { mbar_init(b_full + i, 1); mbar_init(b_empty + i, STB_GEMM_CONSUMER_WARPS); }
-    for (int i = 0; i < STB_A_RING; ++i) { mbar_init(a_full + i, 1); mbar_init(a_empty + i, STB_GEMM_CONSUMER_WARPS); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  if constexpr (FILTER == STB_GEMM_WORK) {
-    static_assert(EPI == 0 || EPI == 1, "work lists serve v2's two passes");
-    stb_batch_gemm_work<EPI>(args, sB, sA, bars);
-    return;
-  }
-
-  const uint32_t my_tiles = (args.n_tiles > blockIdx.x) ? (args.n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-
-  if (warp < 4) {
-    // ===== bulk-copy producer (one thread) =====
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-    if (threadIdx.x == 0) {
-      uint32_t a_cnt = 0;
-      for (uint32_t it = 0; it < my_tiles; ++it) {
-        const uint64_t t = blockIdx.x + (uint64_t)it * gridDim.x;
-        // corpus tile, slab by slab: slab s of the previous tile is released as soon as the
-        // last query tile's MMAs on it retire, so the refill overlaps the remaining slabs
-        if constexpr (FILTER == STB_GEMM_LISTED) {
-          const uint64_t tile = __ldg(args.tile_ids + t * args.tile_stride);
-          const uint8_t *src = args.b_tiles + tile * (size_t)(STB_N_SLABS * STB_B_SLAB_BYTES);
-          for (int s = 0; s < STB_N_SLABS; ++s) {
-            mbar_wait(b_empty + s, (it & 1) ^ 1);
-            if (s == 0) {
-              // the mask slot of iteration it - 2 is free: every consumer warp released slab 0 of the tile
-              // of it - 1, which it does only after the epilogues of the tile of it - 2
-              mbar_expect_tx(b_full, STB_B_SLAB_BYTES + 32);
-              bulk_g2s(s_mask + (it & 1) * 8, args.bitmap + tile * 8, 32, b_full);
-            } else {
-              mbar_expect_tx(b_full + s, STB_B_SLAB_BYTES);
-            }
-            bulk_g2s(sB + s * STB_B_SLAB_BYTES, src + (size_t)s * STB_B_SLAB_BYTES, STB_B_SLAB_BYTES, b_full + s);
-          }
-        } else {
-          const uint8_t *src = args.b_tiles + t * args.tile_stride * (size_t)(STB_N_SLABS * STB_B_SLAB_BYTES);
-          for (int s = 0; s < STB_N_SLABS; ++s) {
-            mbar_wait(b_empty + s, (it & 1) ^ 1);
-            mbar_expect_tx(b_full + s, STB_B_SLAB_BYTES);
-            bulk_g2s(sB + s * STB_B_SLAB_BYTES, src + (size_t)s * STB_B_SLAB_BYTES, STB_B_SLAB_BYTES, b_full + s);
-          }
-        }
-        for (uint32_t m = 0; m < args.m_tiles; ++m) {
-          for (int s = 0; s < STB_N_SLABS; ++s, ++a_cnt) {
-            const uint32_t slot = a_cnt % STB_A_RING;
-            mbar_wait(a_empty + slot, ((a_cnt / STB_A_RING) & 1) ^ 1);
-            mbar_expect_tx(a_full + slot, STB_A_SLAB_BYTES);
-            bulk_g2s(sA + slot * STB_A_SLAB_BYTES,
-                     args.a_tiles + ((size_t)m * STB_N_SLABS + s) * STB_A_SLAB_BYTES, STB_A_SLAB_BYTES,
-                     a_full + slot);
-          }
-        }
-      }
-    }
-    return;
-  }
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-  // ===== consumers: wgmma over one 64-query half of every query tile, then the epilogue =====
-  // Accumulator fragment of m64nN (PTX ISA, wgmma D layout): thread (warp w, lane l) of the
-  // warpgroup holds rows r = 16w + l/4 and r + 8; d[4i + e] is (r, 8i + 2(l%4) + e), d[4i + 2 + e]
-  // is (r + 8, same column).  A 32-row sub-tile c is d[16c .. 16c + 15], spread over a lane quad.
-  const uint32_t half = (uint32_t)(warp >> 2) - 1u;       // which 64 queries of the tile
-  const uint32_t qrow = half * 64 + (warp & 3) * 16 + (lane >> 2);   // + 8 for the second row
-  const uint32_t quad = lane & 3;
-  const uint64_t n_sub = (uint64_t)args.n_tiles * (STB_B_TILE / STB_SUB);
-  float d[128];
-#pragma unroll
-  for (int i = 0; i < 128; ++i) d[i] = 0.f;
-  uint32_t a_cnt = 0;
-  for (uint32_t it = 0; it < my_tiles; ++it) {
-    const uint64_t t = blockIdx.x + (uint64_t)it * gridDim.x;
-    [[maybe_unused]] uint64_t tile_row0 = 0;                 // FILTER: first row of the shadow tile
-    if constexpr (FILTER == STB_GEMM_LISTED) tile_row0 = (uint64_t)__ldg(args.tile_ids + t * args.tile_stride) * STB_B_TILE;
-    for (uint32_t m = 0; m < args.m_tiles; ++m, a_cnt += STB_N_SLABS) {
-      const uint32_t q0 = m * STB_A_TILE + qrow;
-      [[maybe_unused]] float thr[2];
-      [[maybe_unused]] uint32_t cnt[2], cnt0[2];
-      [[maybe_unused]] uint64_t seg_base[2];
-      [[maybe_unused]] uint32_t seg_len[2];
-      if constexpr (EPI >= 1) {       // epilogue state, fetched while the MMAs run
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          thr[h] = __ldg(args.thr + q0 + 8 * h);
-          cnt0[h] = args.cand_cnt[(size_t)(q0 + 8 * h) * gridDim.x + blockIdx.x];
-          cnt[h] = cnt0[h];
-          if constexpr (EPI == 2) {
-            const uint64_t *so = args.seg_off + (size_t)(q0 + 8 * h) * gridDim.x + blockIdx.x;
+          if constexpr (EPI == STB_EPI_EMIT_SIZED) {
+            const uint64_t *so = a.seg_off + (size_t)qout[h] * gridDim.x + blockIdx.x;
             seg_base[h] = __ldg(so);
             seg_len[h] = (uint32_t)(__ldg(so + 1) - seg_base[h]);
           }
@@ -529,21 +542,23 @@ stb_batch_gemm_kernel(const GemmArgs args) {
 #pragma unroll
       for (int s = 0; s < STB_N_SLABS; ++s) {
         const uint32_t slot = (a_cnt + s) % STB_A_RING;
-        if (m == 0) mbar_wait(b_full + s, it & 1);
+        if (w == w0 && s < Copy::kBSlabs) mbar_wait(b_full + s, it & 1);
         mbar_wait(a_full + slot, ((a_cnt + s) / STB_A_RING) & 1);
+        Copy::before_slab(d, s);
         wg_fence();
         const uint32_t a_addr = smem_u32(sA + slot * STB_A_SLAB_BYTES + half * (64 * 128));
-        const uint32_t b_addr = smem_u32(sB + s * STB_B_SLAB_BYTES);
+        const uint32_t b_addr = smem_u32(sB + (s % Copy::kBSlabs) * STB_B_SLAB_BYTES);
 #pragma unroll
-        for (int k = 0; k < STB_SLAB_K / 16; ++k)   // advancing K by 16 elements = 32 bytes inside the swizzle atom
-          wg_mma_m64n256k16(d, wg_desc_sw128(a_addr + k * 32), wg_desc_sw128(b_addr + k * 32), (uint32_t)((s | k) != 0));
+        for (int k = 0; k < 4; ++k)   // advancing K by 32 bytes inside the swizzle atom
+          Copy::mma(d, wg_desc_sw128(a_addr + k * 32), wg_desc_sw128(b_addr + k * 32), (uint32_t)((s | k) != 0));
         wg_commit();
         if (s > 0) {
-          // slab s-1 has been read: free its query slot (and, after the last query tile, its corpus slab)
+          // query slab s-1 has been read: free its ring slot, and after the tile's last item the corpus slab it
+          // multiplied, if no later query slab multiplies that one
           wg_wait<1>();
           if (lane == 0) {
             mbar_arrive(a_empty + (a_cnt + s - 1) % STB_A_RING);
-            if (m + 1 == args.m_tiles) mbar_arrive(b_empty + s - 1);
+            if (last && s - 1 + Copy::kBSlabs >= STB_N_SLABS) mbar_arrive(b_empty + (s - 1) % Copy::kBSlabs);
           }
         }
       }
@@ -551,90 +566,81 @@ stb_batch_gemm_kernel(const GemmArgs args) {
       wg_reg_fence(d);
       if (lane == 0) {
         mbar_arrive(a_empty + (a_cnt + STB_N_SLABS - 1) % STB_A_RING);
-        if (m + 1 == args.m_tiles) mbar_arrive(b_empty + STB_N_SLABS - 1);
+        if (last) mbar_arrive(b_empty + Copy::kBSlabs - 1);
       }
 
-      if constexpr (EPI == 0) {
+      // (taken here, not before the MMAs: STB_GEMM_ALL's first row then stays in uniform registers)
+      const uint64_t row0 = walk.tile(it) * STB_B_TILE;
+      [[maybe_unused]] const uint32_t *mask = walk.mask(s_mask, it, a_cnt / STB_N_SLABS, half);
+      if constexpr (EPI == STB_EPI_SAMPLE) {
+        // Per query, the maximum of the copy's sampling score over the rows that count: the eligible rows, or
+        // (STB_GEMM_ALL) the rows below n_rows on the q8 copy and every row of the shadow.  A row that does not
+        // count scores -inf here (a select, no branch): the maximum is a counted row's score, which the
+        // threshold's sufficiency argument needs.
         float tmx[2] = {-CUDART_INF_F, -CUDART_INF_F};
 #pragma unroll
         for (int c = 0; c < STB_B_TILE / STB_SUB; ++c) {
-          [[maybe_unused]] uint32_t mw = 0;
-          if constexpr (FILTER == STB_GEMM_LISTED) mw = s_mask[(it & 1) * 8 + c];
+          uint32_t counted = 0xffffffffu;
+          if constexpr (SELECT != STB_GEMM_ALL) counted = mask[c];
+          else if constexpr (Copy::kSampleBelowN) counted = stb_rows_below(row0 + (uint64_t)c * STB_SUB, a.n_rows);
+          float v[4][2][2];
+          sco.template scores<true>(d, c, quad, v);
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            float mx;
-            if constexpr (FILTER == STB_GEMM_LISTED) {
-              // an ineligible row's score is -inf here (a select, no branch): the maximum is an eligible
-              // row's score, which the threshold's sufficiency argument needs
-              mx = -CUDART_INF_F;
-#pragma unroll
-              for (int ii = 0; ii < 4; ++ii)
-#pragma unroll
-                for (int e = 0; e < 2; ++e)
-                  mx = fmaxf(mx, ((mw >> (ii * 8 + quad * 2 + e)) & 1u) ? d[16 * c + 4 * ii + 2 * h + e] : -CUDART_INF_F);
-            } else {
-              mx = d[16 * c + 2 * h];
-#pragma unroll
-              for (int ii = 0; ii < 4; ++ii)
-                mx = fmaxf(mx, fmaxf(d[16 * c + 4 * ii + 2 * h], d[16 * c + 4 * ii + 2 * h + 1]));
-            }
-            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-            tmx[h] = fmaxf(tmx[h], mx);
-            if (args.submax && quad == (uint32_t)h)
-              args.submax[((size_t)m * n_sub + t * (STB_B_TILE / STB_SUB) + c) * STB_A_TILE + qrow + 8 * h] = mx;
-          }
-          if (args.full_out) {
+            float mx = -CUDART_INF_F;
 #pragma unroll
             for (int ii = 0; ii < 4; ++ii)
 #pragma unroll
-              for (int h = 0; h < 2; ++h) {
-                float *o = args.full_out + (size_t)(q0 + 8 * h) * ((size_t)args.n_tiles * STB_B_TILE) + t * STB_B_TILE +
-                           c * STB_SUB + ii * 8 + quad * 2;
-                *reinterpret_cast<float2 *>(o) = make_float2(d[16 * c + 4 * ii + 2 * h], d[16 * c + 4 * ii + 2 * h + 1]);
+              for (int e = 0; e < 2; ++e) mx = fmaxf(mx, ((counted >> (ii * 8 + quad * 2 + e)) & 1u) ? v[ii][h][e] : -CUDART_INF_F);
+            if constexpr (SELECT == STB_GEMM_ALL && std::is_same<Copy, ShadowCopy>::value) {
+              // pipeline v1 (on the shadow): the maximum of each 32-row sub-tile
+              if (a.submax) {
+                const float smx = quad_max(mx);
+                if (quad == (uint32_t)h)
+                  a.submax[((size_t)item.x * a.n_tiles * (STB_B_TILE / STB_SUB) + walk.t(it) * (STB_B_TILE / STB_SUB) + c) * STB_A_TILE + qrow + 8 * h] = smx;
               }
+            }
+            tmx[h] = fmaxf(tmx[h], mx);
           }
         }
+        float *at = walk.sample_at(it, item, half);
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
-          if (quad == (uint32_t)(2 + h)) args.tilemax[((size_t)m * args.n_tiles + t) * STB_A_TILE + qrow + 8 * h] = tmx[h];
-      } else {
-        // The threshold is the k-th best score of a ~1.5 % sample minus the rounding margin, so an
-        // emission is rare.  Each (query, CTA) pair owns a private segment of the candidate buffer
-        // and its own cursor, kept in step by the four lanes of the quad that hold the query's row:
-        // no atomics, and keys land in ascending row order within a 32-row sub-tile.
+        for (int h = 0; h < 2; ++h) {
+          tmx[h] = quad_max(tmx[h]);
+          if (at && quad == (uint32_t)(2 + h)) at[qrow + 8 * h] = tmx[h];
+        }
+      } else if constexpr (EPI == STB_EPI_EMIT || EPI == STB_EPI_EMIT_SIZED) {
+        // The threshold is the k-th best sampled score minus the rounding margin, so an emission is rare.  Each
+        // (query, CTA) pair owns a private segment of the candidate buffer and its own cursor, kept in step by the
+        // four lanes of the quad that hold the query's row: no atomics, and keys land in ascending row order
+        // within a 32-row sub-tile.  STB_EPI_EMIT_SIZED's segments are sized by a first pass's exact counts.
+        const bool ragged = row0 + STB_B_TILE > a.n_rows;         // a tile with padding rows
 #pragma unroll
         for (int c = 0; c < STB_B_TILE / STB_SUB; ++c) {
-          uint64_t row0;
-          [[maybe_unused]] uint32_t mw = 0;
-          if constexpr (FILTER == STB_GEMM_LISTED) {
-            row0 = tile_row0 + (uint64_t)c * STB_SUB;
-            mw = s_mask[(it & 1) * 8 + c];
-          } else {
-            row0 = t * STB_B_TILE + (uint64_t)c * STB_SUB;
-          }
+          const uint64_t r0 = row0 + (uint64_t)c * STB_SUB;
+          float v[4][2][2];
+          sco.template scores<false>(d, c, quad, v);
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            // Branch-free on purpose: an accumulator read on a divergent path makes the compiler
-            // serialise the wgmma of the next query tile behind it.
+            // Branch-free on purpose: an accumulator read on a divergent path makes the compiler serialise the
+            // wgmma of the next item behind it.
             uint32_t hit = 0u;
 #pragma unroll
             for (int ii = 0; ii < 4; ++ii)
 #pragma unroll
-              for (int e = 0; e < 2; ++e)
-                hit |= (d[16 * c + 4 * ii + 2 * h + e] >= thr[h] ? 1u : 0u) << (ii * 8 + quad * 2 + e);
+              for (int e = 0; e < 2; ++e) hit |= (v[ii][h][e] >= thr[h] ? 1u : 0u) << (ii * 8 + quad * 2 + e);
             hit |= __shfl_xor_sync(0xffffffffu, hit, 1);
             hit |= __shfl_xor_sync(0xffffffffu, hit, 2);
-            if (row0 + 32 > args.n_rows) hit &= (row0 < args.n_rows) ? ((1u << (uint32_t)(args.n_rows - row0)) - 1u) : 0u;   // padding rows
-            if constexpr (FILTER == STB_GEMM_LISTED) hit &= mw;                                                                                    // ineligible rows
+            if (ragged) hit &= stb_rows_below(r0, a.n_rows);           // padding rows
+            if constexpr (SELECT != STB_GEMM_ALL) hit &= mask[c];      // ineligible rows
             uint64_t *seg;
             uint32_t seg_cap;
-            if constexpr (EPI == 2) {
-              seg = args.cand_keys + seg_base[h];
+            if constexpr (EPI == STB_EPI_EMIT_SIZED) {
+              seg = a.cand_keys + seg_base[h];
               seg_cap = seg_len[h];
             } else {
-              seg = args.cand_keys + ((size_t)(q0 + 8 * h) * gridDim.x + blockIdx.x) * args.cand_cap;
-              seg_cap = args.cand_cap;
+              seg = a.cand_keys + ((size_t)qout[h] * gridDim.x + blockIdx.x) * a.cand_cap;
+              seg_cap = a.cand_cap;
             }
 #pragma unroll
             for (int ii = 0; ii < 4; ++ii)
@@ -642,15 +648,26 @@ stb_batch_gemm_kernel(const GemmArgs args) {
               for (int e = 0; e < 2; ++e) {
                 const uint32_t b = ii * 8 + quad * 2 + e;
                 const uint32_t pos = cnt[h] + __popc(hit & ((1u << b) - 1u));
-                const uint64_t key = stb_make_key(d[16 * c + 4 * ii + 2 * h + e], (uint32_t)(row0 + b));
+                const uint64_t key = stb_make_key(v[ii][h][e], (uint32_t)(r0 + b));
                 if (((hit >> b) & 1u) && pos < seg_cap) seg[pos] = key;
               }
-            cnt[h] += __popc(hit);                       // > cand_cap = overflow marker
+            cnt[h] += __popc(hit);                       // > seg_cap = overflow marker
           }
         }
 #pragma unroll
         for (int h = 0; h < 2; ++h)
-          if (quad == 0 && cnt[h] != cnt0[h]) args.cand_cnt[(size_t)(q0 + 8 * h) * gridDim.x + blockIdx.x] = cnt[h];
+          if (quad == 0 && cnt[h] != cnt0[h]) a.cand_cnt[(size_t)qout[h] * gridDim.x + blockIdx.x] = cnt[h];
+      } else {
+        // the score matrix the epilogues see, [m_tiles * 128][n_tiles * 256]
+        const size_t ld = (size_t)a.n_tiles * STB_B_TILE;
+#pragma unroll
+        for (int c = 0; c < STB_B_TILE / STB_SUB; ++c)
+#pragma unroll
+          for (int ii = 0; ii < 4; ++ii) {
+            const uint32_t col = c * STB_SUB + ii * 8 + quad * 2;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) sco.debug(a, d, 16 * c + 4 * ii + 2 * h, h, col, (size_t)(q0 + 8 * h) * ld + row0 + col);
+          }
       }
     }
   }
@@ -677,48 +694,6 @@ int stb_launch_shadow_build(stb_ctx *ctx, const float *rows_dev, uint64_t n_rows
   return STB_OK;
 }
 
-template <int EPI, int FILTER = STB_GEMM_ALL>
-static int launch_gemm(stb_ctx *ctx, const GemmArgs &a) {
-  const int attr = FILTER == STB_GEMM_WORK ? (EPI == 0 ? STB_ATTR_GEMM0W : STB_ATTR_GEMM1W)
-                   : FILTER == STB_GEMM_LISTED ? (EPI == 0 ? STB_ATTR_GEMM0F : STB_ATTR_GEMM1F)
-                   : (EPI == 0 ? STB_ATTR_GEMM0 : (EPI == 1 ? STB_ATTR_GEMM1 : STB_ATTR_GEMM2));
-  const int smem = FILTER == STB_GEMM_WORK ? STB_GEMM_SMEM_WORK : STB_GEMM_SMEM;
-  STB_ATTR_ONCE(ctx, attr,
-                cudaFuncSetAttribute(stb_batch_gemm_kernel<EPI, FILTER>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  // STB_GEMM_WORK: the same grid as the caller's cta_tiles (stb_batch_emit_grid)
-  unsigned grid = (unsigned)std::min<uint32_t>(a.n_tiles, (uint32_t)ctx->sm_count);
-  if (grid == 0) return STB_OK;
-  stb_batch_gemm_kernel<EPI, FILTER><<<grid, STB_GEMM_THREADS, smem, ctx->stream>>>(a);
-  STB_CUDA(cudaGetLastError());
-  ctx->kernel_launches++;
-  return STB_OK;
-}
-
-// The pass on the shadow: GemmArgs's unions hold the work list's arrays in STB_GEMM_WORK
-int stb_launch_gemm_shadow(stb_ctx *ctx, const StbGemmPass &p, const uint8_t *shadow) {
-  GemmArgs a{};
-  a.a_tiles = p.a_tiles; a.b_tiles = shadow; a.m_tiles = p.m_tiles; a.n_tiles = p.n_tiles; a.tile_stride = p.tile_stride;
-  a.thr = p.thr; a.cand_cnt = p.cand_cnt; a.cand_keys = p.cand_keys; a.cand_cap = p.cand_cap; a.n_rows = p.n_rows;
-  a.tile_ids = p.tile_ids; a.bitmap = p.bitmap;
-  if (p.select == STB_GEMM_WORK) {
-    a.items = p.items; a.item_off = p.item_off; a.cta_tiles = p.cta_tiles;
-    if (p.epi == STB_EPI_EMIT) a.slot_row = p.slot_row;
-    else a.tilemax = p.tilemax;
-  } else {
-    a.submax = p.submax; a.tilemax = p.tilemax; a.full_out = p.full_out; a.seg_off = p.seg_off;
-  }
-  switch (p.select * 4 + p.epi) {
-    case STB_GEMM_ALL * 4 + STB_EPI_SAMPLE: return launch_gemm<0>(ctx, a);
-    case STB_GEMM_ALL * 4 + STB_EPI_EMIT: return launch_gemm<1>(ctx, a);
-    case STB_GEMM_ALL * 4 + STB_EPI_EMIT_SIZED: return launch_gemm<2>(ctx, a);
-    case STB_GEMM_LISTED * 4 + STB_EPI_SAMPLE: return launch_gemm<0, STB_GEMM_LISTED>(ctx, a);
-    case STB_GEMM_LISTED * 4 + STB_EPI_EMIT: return launch_gemm<1, STB_GEMM_LISTED>(ctx, a);
-    case STB_GEMM_WORK * 4 + STB_EPI_SAMPLE: return launch_gemm<0, STB_GEMM_WORK>(ctx, a);
-    case STB_GEMM_WORK * 4 + STB_EPI_EMIT: return launch_gemm<1, STB_GEMM_WORK>(ctx, a);
-  }
-  stb_set_error("batch GEMM: no shadow kernel for epilogue %d over tile selection %d", p.epi, p.select);
-  return STB_ERR_ARG;
-}
 
 // stb_search_batch_subsets's query slots: slot s holds the f32 query row slot_row[s] of `rows` (zeros for a
 // padding slot, ~0) ...
@@ -1077,7 +1052,7 @@ struct Finish2Args {
   const uint32_t *q_bad;       // [nq] 1: the query could not be normalised (never proven)
   stb_hit *out_hits;           // [nq][top_k]
   uint32_t *out_status;        // [nq][2]: hits, complete
-  // route 7 (null on the shadow's routes): the keys hold q8 upper bounds u (stb_batch_q8_gemm_kernel); the q8
+  // route 7 (null on the shadow's routes): the keys hold q8 upper bounds u (stb_batch_gemm_kernel on Q8Copy); the q8
   // scales, the queries' {1/S, h_l1, e_q, S} and the emission thresholds the proof is checked against
   const float *q8_scale;
   const float4 *q8_qc;
@@ -1299,9 +1274,6 @@ int stb_launch_batch_finish2(stb_ctx *ctx, const uint64_t *cand_keys, const uint
 // that cannot win, re-scores the rest exactly and proves the query only if the k-th distance beats thr + eps.
 // =========================================================================================
 
-#define STB_Q8_B_SLAB_BYTES (STB_B_TILE * 128)            // 128 code bytes of 256 rows: 32 KiB
-#define STB_Q8_GEMM_SMEM (2 * STB_Q8_B_SLAB_BYTES + STB_A_RING * STB_A_SLAB_BYTES + 2 * STB_B_TILE * 4 + 256 + 1024)
-static_assert(STB_Q8_GEMM_SMEM <= 227 * 1024, "q8 GEMM shared memory");
 
 // 1. Query tiles.  One warp per query slot (all four lane groups compute the same query, as stb_q8_query's
 // reductions require); lane j < 8 writes its 16-byte chunk j of each of the tile's four K-slabs: hi bytes of
@@ -1353,329 +1325,6 @@ int stb_launch_q8_query_tiles(stb_ctx *ctx, const float *q_dev, uint32_t nq, uin
   return STB_OK;
 }
 
-// 2. The GEMM.  Corpus tile = 256 rows: two K-slabs of codes (bytes 0-127 and 128-255 of each row, 32 KiB each)
-// loaded with the tensor maps below, which apply the 128-byte swizzle on the way in (the q8 copy stays row-major
-// for K1 and zero-fills rows past n), and the tile's 256 scales (1 KiB) with slab 0, double-buffered by tile
-// parity: the producer refills buffer (it + 1) & 1 only after every consumer warp released slab 0 of tile it,
-// which it does after the epilogues of tile it - 1.  Query tiles stream through the 6-slab ring of
-// stb_batch_gemm_kernel.  Per (query tile, corpus tile) a consumer warpgroup runs the hi slabs (K = 256, 8
-// wgmma m64n256k32 s8), waits, multiplies its s32 accumulators by 256 and accumulates the lo slabs on top.
-__device__ __forceinline__ void wg_reg_fence_s32(int32_t (&d)[128]) {
-#pragma unroll
-  for (int i = 0; i < 128; ++i) asm volatile("" : "+r"(d[i])::"memory");
-}
-__device__ __forceinline__ void wg_mma_m64n256k32_s8(int32_t (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %130, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n256k32.s32.s8.s8 {"
-      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
-      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
-      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
-      "%128, %129, p;\n\t}"
-      :
-        "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
-        "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
-        "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
-        "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
-        "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
-        "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
-        "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
-        "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]),
-        "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]),
-        "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79]),
-        "+r"(d[80]), "+r"(d[81]), "+r"(d[82]), "+r"(d[83]), "+r"(d[84]), "+r"(d[85]), "+r"(d[86]), "+r"(d[87]),
-        "+r"(d[88]), "+r"(d[89]), "+r"(d[90]), "+r"(d[91]), "+r"(d[92]), "+r"(d[93]), "+r"(d[94]), "+r"(d[95]),
-        "+r"(d[96]), "+r"(d[97]), "+r"(d[98]), "+r"(d[99]), "+r"(d[100]), "+r"(d[101]), "+r"(d[102]), "+r"(d[103]),
-        "+r"(d[104]), "+r"(d[105]), "+r"(d[106]), "+r"(d[107]), "+r"(d[108]), "+r"(d[109]), "+r"(d[110]), "+r"(d[111]),
-        "+r"(d[112]), "+r"(d[113]), "+r"(d[114]), "+r"(d[115]), "+r"(d[116]), "+r"(d[117]), "+r"(d[118]), "+r"(d[119]),
-        "+r"(d[120]), "+r"(d[121]), "+r"(d[122]), "+r"(d[123]), "+r"(d[124]), "+r"(d[125]), "+r"(d[126]), "+r"(d[127])
-      : "l"(adesc), "l"(bdesc), "r"(accumulate));
-}
-__device__ __forceinline__ void tma_load_2d(void *dst_smem, const CUtensorMap *map, int x, int y, uint64_t *bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
-          smem_u32(dst_smem)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(x), "r"(y), "r"(smem_u32(bar))
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_1d(void *dst_smem, const CUtensorMap *map, int x, uint64_t *bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.1d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2}], [%3];" ::"r"(
-          smem_u32(dst_smem)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(x), "r"(smem_u32(bar))
-      : "memory");
-}
-
-struct Q8GemmArgs {
-  const uint8_t *a_tiles;     // m_tiles x 4 slabs x 16 KiB (stb_q8_query_tiles_kernel)
-  const float4 *qc;           // [q_pad] {1/S, h_l1, e_q, S}
-  uint32_t m_tiles;
-  uint32_t n_tiles;           // corpus tiles of this launch: tile t is corpus tile t * tile_stride
-  uint32_t tile_stride;
-  uint64_t n_rows;            // rows past n (the zero-filled tail of the last tile) never count
-  float *tilemax;             // EPI 0: [m_tiles][n_tiles][128] maximum of l per tile
-  const float *thr;           // EPI 1: [q_pad] emission thresholds on u ...
-  uint32_t *cand_cnt;         //        [q_pad][grid] counts (> cand_cap: overflow marker)
-  uint64_t *cand_keys;        //        [q_pad][grid][cand_cap] keys (u desc, local row)
-  uint32_t cand_cap;
-  int32_t *dot_out;           // EPI 2: [m_tiles * 128][n_tiles * 256] dot, u and l
-  float *u_out, *l_out;
-  // (appended, so the unfiltered EPI 0-2 kernels keep their parameter offsets)
-  // FILTER (route 8): tile t of the launch is corpus tile tile_ids[t * tile_stride], and only the eligible rows
-  // of `bitmap` (8 words per corpus tile, stb_launch_row_bitmap) count
-  const uint32_t *tile_ids;
-  const uint32_t *bitmap;
-  // EPI 3 (route 10's re-emission): segment (q, CTA) is cand_keys[seg_off[q * grid + CTA], seg_off[q * grid + CTA + 1]),
-  // sized by the first pass's exact counts; cand_cnt holds the cursors
-  const uint64_t *seg_off;
-};
-
-// EPI 0: sampling (tile maxima of l); EPI 1: emit every row whose u reaches the query's threshold; EPI 2: debug;
-// EPI 3: EPI 1 into exactly sized segments (unfiltered only).
-// FILTER: the CTAs walk the listed tiles and only eligible rows count: EPI 0 takes each tile maximum of l over
-// its eligible rows (an ineligible row's l is -inf, DESIGN §5), EPI 1 emits eligible rows only.  The tile's 8
-// bitmap words arrive with its scales, double-buffered by tile parity like them.
-template <int EPI, bool FILTER>
-__global__ void __launch_bounds__(STB_GEMM_THREADS, 1)
-stb_batch_q8_gemm_kernel(const __grid_constant__ CUtensorMap codes_map, const __grid_constant__ CUtensorMap scale_map,
-                         const Q8GemmArgs args) {
-  static_assert(!FILTER || EPI == 0 || EPI == 1, "route 8 runs the sampling and the emitting pass");
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t *sB = smem;                                          // 2 code slabs
-  uint8_t *sA = smem + 2 * STB_Q8_B_SLAB_BYTES;                // query ring
-  float *s_scale = reinterpret_cast<float *>(sA + STB_A_RING * STB_A_SLAB_BYTES);   // [2][256]
-  uint64_t *bars = reinterpret_cast<uint64_t *>(s_scale + 2 * STB_B_TILE);
-  uint64_t *b_full = bars + 0, *b_empty = bars + 2;
-  uint64_t *a_full = bars + 4, *a_empty = a_full + STB_A_RING;
-  // FILTER: [2][8] bitmap words behind the 16 barriers, slot it & 1 = the tile of iteration it
-  [[maybe_unused]] uint32_t *s_mask = reinterpret_cast<uint32_t *>(bars + 4 + 2 * STB_A_RING);
-  static_assert((4 + 2 * STB_A_RING) * 8 + 2 * 8 * 4 <= 256, "mask words must fit behind the barriers");
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < 2; ++i) { mbar_init(b_full + i, 1); mbar_init(b_empty + i, STB_GEMM_CONSUMER_WARPS); }
-    for (int i = 0; i < STB_A_RING; ++i) { mbar_init(a_full + i, 1); mbar_init(a_empty + i, STB_GEMM_CONSUMER_WARPS); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  const uint32_t my_tiles = (args.n_tiles > blockIdx.x) ? (args.n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-
-  if (warp < 4) {
-    // ===== producer (one thread) =====
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-    if (threadIdx.x == 0) {
-      uint32_t a_cnt = 0;
-      for (uint32_t it = 0; it < my_tiles; ++it) {
-        const uint64_t t = blockIdx.x + (uint64_t)it * gridDim.x;
-        const uint64_t tile = FILTER ? (uint64_t)__ldg(args.tile_ids + t * args.tile_stride) : t * args.tile_stride;
-        const int row0 = (int)(tile * STB_B_TILE);
-        for (int s = 0; s < 2; ++s) {
-          mbar_wait(b_empty + s, (it & 1) ^ 1);
-          if (s == 0) {
-            if constexpr (FILTER) {
-              mbar_expect_tx(b_full, STB_Q8_B_SLAB_BYTES + STB_B_TILE * 4 + 32);
-              bulk_g2s(s_mask + (it & 1) * 8, args.bitmap + tile * 8, 32, b_full);
-            } else {
-              mbar_expect_tx(b_full, STB_Q8_B_SLAB_BYTES + STB_B_TILE * 4);
-            }
-            tma_load_1d(s_scale + (it & 1) * STB_B_TILE, &scale_map, row0, b_full);
-          } else {
-            mbar_expect_tx(b_full + s, STB_Q8_B_SLAB_BYTES);
-          }
-          tma_load_2d(sB + s * STB_Q8_B_SLAB_BYTES, &codes_map, s * 128, row0, b_full + s);
-        }
-        for (uint32_t m = 0; m < args.m_tiles; ++m) {
-          for (int s = 0; s < 4; ++s, ++a_cnt) {
-            const uint32_t slot = a_cnt % STB_A_RING;
-            mbar_wait(a_empty + slot, ((a_cnt / STB_A_RING) & 1) ^ 1);
-            mbar_expect_tx(a_full + slot, STB_A_SLAB_BYTES);
-            bulk_g2s(sA + slot * STB_A_SLAB_BYTES, args.a_tiles + ((size_t)m * 4 + s) * STB_A_SLAB_BYTES, STB_A_SLAB_BYTES,
-                     a_full + slot);
-          }
-        }
-      }
-    }
-    return;
-  }
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-  // ===== consumers (accumulator layout as in stb_batch_gemm_kernel) =====
-  const uint32_t half = (uint32_t)(warp >> 2) - 1u;
-  const uint32_t qrow = half * 64 + (warp & 3) * 16 + (lane >> 2);
-  const uint32_t quad = lane & 3;
-  int32_t d[128];
-#pragma unroll
-  for (int i = 0; i < 128; ++i) d[i] = 0;
-  uint32_t a_cnt = 0;
-  for (uint32_t it = 0; it < my_tiles; ++it) {
-    const uint64_t t = blockIdx.x + (uint64_t)it * gridDim.x;
-    const uint64_t row0 = FILTER ? (uint64_t)__ldg(args.tile_ids + t * args.tile_stride) * STB_B_TILE
-                                 : t * args.tile_stride * STB_B_TILE;
-    const float *sc = s_scale + (it & 1) * STB_B_TILE;
-    [[maybe_unused]] const uint32_t *mk = s_mask + (it & 1) * 8;
-    for (uint32_t m = 0; m < args.m_tiles; ++m, a_cnt += 4) {
-      const uint32_t q0 = m * STB_A_TILE + qrow;
-      float4 qc[2];
-      [[maybe_unused]] float thr[2];
-      [[maybe_unused]] uint32_t cnt[2], cnt0[2];
-      [[maybe_unused]] uint64_t seg_base[2];
-      [[maybe_unused]] uint32_t seg_len[2];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        qc[h] = __ldg(args.qc + q0 + 8 * h);
-        if constexpr (EPI == 1 || EPI == 3) {
-          thr[h] = __ldg(args.thr + q0 + 8 * h);
-          cnt0[h] = args.cand_cnt[(size_t)(q0 + 8 * h) * gridDim.x + blockIdx.x];
-          cnt[h] = cnt0[h];
-          if constexpr (EPI == 3) {
-            const uint64_t *so = args.seg_off + (size_t)(q0 + 8 * h) * gridDim.x + blockIdx.x;
-            seg_base[h] = __ldg(so);
-            seg_len[h] = (uint32_t)(__ldg(so + 1) - seg_base[h]);
-          }
-        }
-      }
-      wg_reg_fence_s32(d);
-#pragma unroll
-      for (int s = 0; s < 4; ++s) {
-        const uint32_t slot = (a_cnt + s) % STB_A_RING;
-        if (m == 0 && s < 2) mbar_wait(b_full + s, it & 1);
-        mbar_wait(a_full + slot, ((a_cnt + s) / STB_A_RING) & 1);
-        if (s == 2) {
-          // the hi products are complete: dot = 256 hi.x8 + lo.x8 (|256 hi.x8| <= 256 * 127 * 127 * 256 < 2^31)
-          wg_wait<0>();
-          wg_reg_fence_s32(d);
-#pragma unroll
-          for (int i = 0; i < 128; ++i) d[i] *= 256;
-          wg_reg_fence_s32(d);
-        }
-        wg_fence();
-        const uint32_t a_addr = smem_u32(sA + slot * STB_A_SLAB_BYTES + half * (64 * 128));
-        const uint32_t b_addr = smem_u32(sB + (s & 1) * STB_Q8_B_SLAB_BYTES);
-#pragma unroll
-        for (int k = 0; k < 4; ++k)   // K by 32 bytes inside the swizzle atom
-          wg_mma_m64n256k32_s8(d, wg_desc_sw128(a_addr + k * 32), wg_desc_sw128(b_addr + k * 32), (uint32_t)((s | k) != 0));
-        wg_commit();
-        if (s > 0) {
-          wg_wait<1>();
-          if (lane == 0) {
-            mbar_arrive(a_empty + (a_cnt + s - 1) % STB_A_RING);
-            if (m + 1 == args.m_tiles && s == 3) mbar_arrive(b_empty);    // slab 0's lo pass has retired
-          }
-        }
-      }
-      wg_wait<0>();
-      wg_reg_fence_s32(d);
-      if (lane == 0) {
-        mbar_arrive(a_empty + (a_cnt + 3) % STB_A_RING);
-        if (m + 1 == args.m_tiles) mbar_arrive(b_empty + 1);
-      }
-
-      // d[16c + 4ii + 2h + e]: query qrow + 8h, tile column 32c + 8ii + 2quad + e
-      if constexpr (EPI == 0) {
-        const uint32_t n_real = args.n_rows > row0 + STB_B_TILE ? STB_B_TILE : (uint32_t)(args.n_rows > row0 ? args.n_rows - row0 : 0);
-        float tmx[2] = {-CUDART_INF_F, -CUDART_INF_F};
-#pragma unroll
-        for (int c = 0; c < STB_B_TILE / STB_SUB; ++c)
-#pragma unroll
-          for (int ii = 0; ii < 4; ++ii) {
-            const uint32_t col = c * STB_SUB + ii * 8 + quad * 2;
-            const float2 s2 = *reinterpret_cast<const float2 *>(sc + col);
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              // FILTER: the eligible rows (the bitmap holds no row past n)
-              const bool real = FILTER ? ((mk[c] >> (ii * 8 + quad * 2 + e)) & 1u) != 0u : col + e < n_real;
-#pragma unroll
-              for (int h = 0; h < 2; ++h) {
-                const float l = fmaf(e ? s2.y : s2.x, fmaf((float)d[16 * c + 4 * ii + 2 * h + e], qc[h].x, -qc[h].y), -qc[h].z) -
-                                (float)STB_Q8_SCAN_EPS;
-                tmx[h] = fmaxf(tmx[h], real ? l : -CUDART_INF_F);
-              }
-            }
-          }
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          tmx[h] = fmaxf(tmx[h], __shfl_xor_sync(0xffffffffu, tmx[h], 1));
-          tmx[h] = fmaxf(tmx[h], __shfl_xor_sync(0xffffffffu, tmx[h], 2));
-          if (quad == (uint32_t)h) args.tilemax[((size_t)m * args.n_tiles + t) * STB_A_TILE + qrow + 8 * h] = tmx[h];
-        }
-      } else if constexpr (EPI == 1 || EPI == 3) {
-        // as stb_batch_gemm_kernel's EPI 1 (EPI 3: its EPI 2): a private segment per (query, CTA), branch-free hit masks
-#pragma unroll
-        for (int c = 0; c < STB_B_TILE / STB_SUB; ++c) {
-          const uint64_t r0 = row0 + (uint64_t)c * STB_SUB;
-          float u[4][2][2];
-#pragma unroll
-          for (int ii = 0; ii < 4; ++ii) {
-            const float2 s2 = *reinterpret_cast<const float2 *>(sc + c * STB_SUB + ii * 8 + quad * 2);
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-#pragma unroll
-              for (int e = 0; e < 2; ++e)
-                u[ii][h][e] = fmaf(e ? s2.y : s2.x, fmaf((float)d[16 * c + 4 * ii + 2 * h + e], qc[h].x, qc[h].y), qc[h].z);
-          }
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            uint32_t hit = 0u;
-#pragma unroll
-            for (int ii = 0; ii < 4; ++ii)
-#pragma unroll
-              for (int e = 0; e < 2; ++e) hit |= (u[ii][h][e] >= thr[h] ? 1u : 0u) << (ii * 8 + quad * 2 + e);
-            hit |= __shfl_xor_sync(0xffffffffu, hit, 1);
-            hit |= __shfl_xor_sync(0xffffffffu, hit, 2);
-            if (r0 + 32 > args.n_rows) hit &= (r0 < args.n_rows) ? ((1u << (uint32_t)(args.n_rows - r0)) - 1u) : 0u;
-            if constexpr (FILTER) hit &= mk[c];                                    // ineligible rows
-            uint64_t *seg;
-            uint32_t seg_cap;
-            if constexpr (EPI == 3) {
-              seg = args.cand_keys + seg_base[h];
-              seg_cap = seg_len[h];
-            } else {
-              seg = args.cand_keys + ((size_t)(q0 + 8 * h) * gridDim.x + blockIdx.x) * args.cand_cap;
-              seg_cap = args.cand_cap;
-            }
-#pragma unroll
-            for (int ii = 0; ii < 4; ++ii)
-#pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const uint32_t b = ii * 8 + quad * 2 + e;
-                const uint32_t pos = cnt[h] + __popc(hit & ((1u << b) - 1u));
-                if (((hit >> b) & 1u) && pos < seg_cap) seg[pos] = stb_make_key(u[ii][h][e], (uint32_t)(r0 + b));
-              }
-            cnt[h] += __popc(hit);
-          }
-        }
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-          if (quad == 0 && cnt[h] != cnt0[h]) args.cand_cnt[(size_t)(q0 + 8 * h) * gridDim.x + blockIdx.x] = cnt[h];
-      } else {
-        const size_t ld = (size_t)args.n_tiles * STB_B_TILE;
-#pragma unroll
-        for (int c = 0; c < STB_B_TILE / STB_SUB; ++c)
-#pragma unroll
-          for (int ii = 0; ii < 4; ++ii) {
-            const uint32_t col = c * STB_SUB + ii * 8 + quad * 2;
-            const float2 s2 = *reinterpret_cast<const float2 *>(sc + col);
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const size_t o = (size_t)(q0 + 8 * h) * ld + row0 + col;
-              const int32_t d0 = d[16 * c + 4 * ii + 2 * h], d1 = d[16 * c + 4 * ii + 2 * h + 1];
-              *reinterpret_cast<int2 *>(args.dot_out + o) = make_int2(d0, d1);
-              *reinterpret_cast<float2 *>(args.u_out + o) =
-                  make_float2(fmaf(s2.x, fmaf((float)d0, qc[h].x, qc[h].y), qc[h].z), fmaf(s2.y, fmaf((float)d1, qc[h].x, qc[h].y), qc[h].z));
-              *reinterpret_cast<float2 *>(args.l_out + o) =
-                  make_float2(fmaf(s2.x, fmaf((float)d0, qc[h].x, -qc[h].y), -qc[h].z) - (float)STB_Q8_SCAN_EPS,
-                              fmaf(s2.y, fmaf((float)d1, qc[h].x, -qc[h].y), -qc[h].z) - (float)STB_Q8_SCAN_EPS);
-            }
-          }
-      }
-    }
-  }
-}
 
 // The q8 copy's tensor maps, encoded per launch (a map holds the buffer's address, which moves when the copy
 // grows): codes as [n_rows][256] u8 in [256 rows][128 B] boxes with the 128-byte swizzle, scales as [n_rows] f32
@@ -1707,38 +1356,56 @@ static int q8_tensor_maps(const uint8_t *codes, const float *scales, uint64_t n_
   return STB_OK;
 }
 
-template <int EPI, bool FILTER = false>
-static int launch_q8_gemm(stb_ctx *ctx, const uint8_t *codes, const float *scales, const Q8GemmArgs &a) {
-  if (a.n_rows == 0 || a.n_rows > 0x7fffff00ull) { stb_set_error("q8 GEMM: %llu rows", (unsigned long long)a.n_rows); return STB_ERR_ARG; }
-  CUtensorMap cm, sm;
-  int rc = q8_tensor_maps(codes, scales, a.n_rows, &cm, &sm);
-  if (rc != STB_OK) return rc;
-  const int attr = FILTER ? (EPI == 0 ? STB_ATTR_Q8GEMM0F : STB_ATTR_Q8GEMM1F)
-                          : (EPI == 0 ? STB_ATTR_Q8GEMM0 : EPI == 1 ? STB_ATTR_Q8GEMM1 : EPI == 2 ? STB_ATTR_Q8GEMM2 : STB_ATTR_Q8GEMM3);
-  STB_ATTR_ONCE(ctx, attr,
-                cudaFuncSetAttribute(stb_batch_q8_gemm_kernel<EPI, FILTER>, cudaFuncAttributeMaxDynamicSharedMemorySize, STB_Q8_GEMM_SMEM));
-  const unsigned grid = (unsigned)std::min<uint32_t>(a.n_tiles, (uint32_t)ctx->sm_count);   // = stb_batch_emit_grid
+// The GEMM kernels that exist, by (copy, tile selection, epilogue).  Entry i's shared-memory opt-in is made once
+// per context under attribute id STB_ATTR_GEMM + i.
+struct StbGemmKernel {
+  int copy, select, epi;
+  const void *fn;
+  int smem;
+};
+template <class Copy, int SELECT, int EPI, class... Maps>
+static StbGemmKernel gemm_kernel(int copy) {
+  static_assert(stb_gemm_smem<Copy, SELECT>() <= 227 * 1024, "GEMM shared memory");
+  return {copy, SELECT, EPI, reinterpret_cast<const void *>(&stb_batch_gemm_kernel<Copy, SELECT, EPI, Maps...>),
+          stb_gemm_smem<Copy, SELECT>()};
+}
+#define STB_SHADOW_GEMM(sel, epi) gemm_kernel<ShadowCopy, sel, epi>(STB_GEMM_SHADOW)
+#define STB_Q8_GEMM(sel, epi) gemm_kernel<Q8Copy, sel, epi, CUtensorMap, CUtensorMap>(STB_GEMM_Q8)
+static const StbGemmKernel kGemmKernels[] = {
+    STB_SHADOW_GEMM(STB_GEMM_ALL, STB_EPI_SAMPLE),    STB_SHADOW_GEMM(STB_GEMM_ALL, STB_EPI_EMIT),
+    STB_SHADOW_GEMM(STB_GEMM_ALL, STB_EPI_EMIT_SIZED), STB_SHADOW_GEMM(STB_GEMM_ALL, STB_EPI_DEBUG),
+    STB_SHADOW_GEMM(STB_GEMM_LISTED, STB_EPI_SAMPLE), STB_SHADOW_GEMM(STB_GEMM_LISTED, STB_EPI_EMIT),
+    STB_SHADOW_GEMM(STB_GEMM_WORK, STB_EPI_SAMPLE),   STB_SHADOW_GEMM(STB_GEMM_WORK, STB_EPI_EMIT),
+    STB_Q8_GEMM(STB_GEMM_ALL, STB_EPI_SAMPLE),        STB_Q8_GEMM(STB_GEMM_ALL, STB_EPI_EMIT),
+    STB_Q8_GEMM(STB_GEMM_ALL, STB_EPI_EMIT_SIZED),    STB_Q8_GEMM(STB_GEMM_ALL, STB_EPI_DEBUG),
+    STB_Q8_GEMM(STB_GEMM_LISTED, STB_EPI_SAMPLE),     STB_Q8_GEMM(STB_GEMM_LISTED, STB_EPI_EMIT),
+};
+#undef STB_SHADOW_GEMM
+#undef STB_Q8_GEMM
+static_assert(STB_ATTR_GEMM + sizeof(kGemmKernels) / sizeof(kGemmKernels[0]) <= 32, "func_attr_mask has 32 bits");
+
+int stb_launch_gemm(stb_ctx *ctx, const StbGemmPass &p) {
+  int i = 0;
+  const int n_kernels = (int)(sizeof(kGemmKernels) / sizeof(kGemmKernels[0]));
+  while (i < n_kernels && !(kGemmKernels[i].copy == p.copy && kGemmKernels[i].select == p.select && kGemmKernels[i].epi == p.epi)) ++i;
+  if (i == n_kernels) {
+    stb_set_error("batch GEMM: no %s kernel for epilogue %d over tile selection %d", p.copy == STB_GEMM_Q8 ? "q8" : "shadow",
+                  p.epi, p.select);
+    return STB_ERR_ARG;
+  }
+  const StbGemmKernel &k = kGemmKernels[i];
+  CUtensorMap maps[2];
+  void *args[3] = {const_cast<StbGemmPass *>(&p), &maps[0], &maps[1]};
+  if (p.copy == STB_GEMM_Q8) {
+    if (p.n_rows == 0 || p.n_rows > 0x7fffff00ull) { stb_set_error("q8 GEMM: %llu rows", (unsigned long long)p.n_rows); return STB_ERR_ARG; }
+    const int rc = q8_tensor_maps(p.b_tiles, p.q8_scale, p.n_rows, &maps[0], &maps[1]);
+    if (rc != STB_OK) return rc;
+  }
+  STB_ATTR_ONCE(ctx, STB_ATTR_GEMM + i, cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, k.smem));
+  // = stb_batch_emit_grid; STB_GEMM_WORK's cta_tiles are cut for this grid
+  const unsigned grid = (unsigned)std::min<uint32_t>(p.n_tiles, (uint32_t)ctx->sm_count);
   if (grid == 0) return STB_OK;
-  stb_batch_q8_gemm_kernel<EPI, FILTER><<<grid, STB_GEMM_THREADS, STB_Q8_GEMM_SMEM, ctx->stream>>>(cm, sm, a);
-  STB_CUDA(cudaGetLastError());
+  STB_CUDA(cudaLaunchKernel(k.fn, dim3(grid), dim3(STB_GEMM_THREADS), args, (size_t)k.smem, ctx->stream));
   ctx->kernel_launches++;
   return STB_OK;
-}
-
-int stb_launch_gemm_q8(stb_ctx *ctx, const StbGemmPass &p, const uint8_t *codes, const float *scales, const float4 *qc) {
-  Q8GemmArgs a{};
-  a.a_tiles = p.a_tiles; a.qc = qc; a.m_tiles = p.m_tiles; a.n_tiles = p.n_tiles; a.tile_stride = p.tile_stride;
-  a.n_rows = p.n_rows; a.tilemax = p.tilemax; a.thr = p.thr; a.cand_cnt = p.cand_cnt; a.cand_keys = p.cand_keys;
-  a.cand_cap = p.cand_cap; a.dot_out = p.dot_out; a.u_out = p.u_out; a.l_out = p.l_out; a.tile_ids = p.tile_ids;
-  a.bitmap = p.bitmap; a.seg_off = p.seg_off;
-  switch (p.select * 4 + p.epi) {
-    case STB_GEMM_ALL * 4 + STB_EPI_SAMPLE: return launch_q8_gemm<0>(ctx, codes, scales, a);
-    case STB_GEMM_ALL * 4 + STB_EPI_EMIT: return launch_q8_gemm<1>(ctx, codes, scales, a);
-    case STB_GEMM_ALL * 4 + STB_EPI_DEBUG: return launch_q8_gemm<2>(ctx, codes, scales, a);
-    case STB_GEMM_ALL * 4 + STB_EPI_EMIT_SIZED: return launch_q8_gemm<3>(ctx, codes, scales, a);
-    case STB_GEMM_LISTED * 4 + STB_EPI_SAMPLE: return launch_q8_gemm<0, true>(ctx, codes, scales, a);
-    case STB_GEMM_LISTED * 4 + STB_EPI_EMIT: return launch_q8_gemm<1, true>(ctx, codes, scales, a);
-  }
-  stb_set_error("batch GEMM: no q8 kernel for epilogue %d over tile selection %d", p.epi, p.select);
-  return STB_ERR_ARG;
 }

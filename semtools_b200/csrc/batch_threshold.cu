@@ -2,7 +2,7 @@
 //
 // Semantics: Q independent search_documents calls with max_distance set (reference src/search/mod.rs:88-89,
 // 115-116): every row with canonical distance < M, ordered by (distance, row).  The tensor-core pass is K2's
-// candidate-emitting wgmma GEMM (batch_scan.cu, EPI 1 and its exactly sized variant EPI 2); this file holds the
+// candidate-emitting wgmma GEMM (batch_scan.cu, STB_EPI_EMIT and its exactly sized variant STB_EPI_EMIT_SIZED); this file holds the
 // steps around it and the exact finish.
 #include <math_constants.h>
 
@@ -17,8 +17,8 @@
 // The emission threshold is given, not sampled (api.cu: thr_emission_value, DESIGN §5):
 //   thr = RD_f32(((1 - M) - EPS) - delta)  for the queries the tensor path answers, +inf for the rest.
 // A row with canonical d < M has exact cosine c > 1 - M - delta, so its score a >= c - EPS >= thr.
-// Pipeline: thresholds -> emitting GEMM (EPI 1, 64 keys per (query, CTA)) -> [queries with an overflowed
-// segment: EPI 2 into exactly sized segments] -> compact -> sort by row -> exact re-score, d < M ->
+// Pipeline: thresholds -> emitting GEMM (STB_EPI_EMIT, 64 keys per (query, CTA)) -> [queries with an overflowed
+// segment: STB_EPI_EMIT_SIZED into exactly sized segments] -> compact -> sort by row -> exact re-score, d < M ->
 // stable sort by distance -> hits.
 // =========================================================================================
 

@@ -496,10 +496,8 @@ int stb_launch_batch_xchg(stb_ctx *ctx, const StbBatchXchgArgs &a, const stb_hit
                           stb_hit *out_hits, uint32_t *out_status);
 
 // opt-in to > 48 KiB dynamic shared memory (or another function attribute) once per context
-enum { STB_ATTR_GEMM0 = 0, STB_ATTR_GEMM1, STB_ATTR_MERGE, STB_ATTR_IVF_V2, STB_ATTR_FINISH2,
-       STB_ATTR_IVF_BATCH, STB_ATTR_GEMM0F, STB_ATTR_GEMM1F, STB_ATTR_GEMM2, STB_ATTR_GEMM0W, STB_ATTR_GEMM1W,
-       STB_ATTR_Q8GEMM0, STB_ATTR_Q8GEMM1, STB_ATTR_Q8GEMM2, STB_ATTR_THRESH_BIG,
-       STB_ATTR_Q8GEMM0F, STB_ATTR_Q8GEMM1F, STB_ATTR_Q8GEMM3 };
+// (STB_ATTR_GEMM + i: entry i of K2's GEMM kernel table, batch_scan.cu)
+enum { STB_ATTR_MERGE = 0, STB_ATTR_IVF_V2, STB_ATTR_FINISH2, STB_ATTR_IVF_BATCH, STB_ATTR_THRESH_BIG, STB_ATTR_GEMM };
 #define STB_ATTR_ONCE(ctx, bit, call)                         \
   do {                                                        \
     if (!((ctx)->func_attr_mask & (1u << (bit)))) {           \
@@ -544,26 +542,32 @@ int stb_tok_chunk(stb_ctx *ctx, const stb_tokenizer *tok, const StbTextHost &h, 
 int stb_launch_shadow_build(stb_ctx *ctx, const float *rows_dev, uint64_t n_rows, int tile,
                             uint8_t *out, int *bad_flag_dev, uint64_t first_row = 0,
                             uint32_t *row_bad_dev = nullptr, uint64_t rows_first = 0);
-// One pass of K2's GEMM (batch_scan.cu) over either copy: the epilogue, the corpus tiles it covers, and what those
-// read and write.  Tile t of a pass is corpus tile t * tile_stride (STB_GEMM_ALL), listed tile tile_ids[t *
-// tile_stride] with the eligible rows of `bitmap` (STB_GEMM_LISTED), or, STB_GEMM_WORK (shadow only), the t-th
-// tile of a work list: per corpus tile tile_ids[u] its (query tile, mask slots, sample columns) items, one filter
-// per 64-query half (batch_scan.cu, GemmArgs).  Rows past n_rows never count.
+// One pass of K2's GEMM (batch_scan.cu, stb_batch_gemm_kernel) over either copy: the epilogue, the corpus tiles it
+// covers, and what those read and write.  Tile t of a pass is corpus tile t * tile_stride (STB_GEMM_ALL), listed
+// tile tile_ids[t * tile_stride] with the eligible rows of `bitmap` (STB_GEMM_LISTED), or, STB_GEMM_WORK (shadow
+// only), the t-th tile of a work list: per corpus tile tile_ids[u] its (query tile, mask slots, sample columns)
+// items, one filter per 64-query half (batch_scan.cu, TileWalk).  Rows past n_rows never emit.
+#define STB_GEMM_SHADOW 0             // the 16-bit shadow: b_tiles = its tiles
+#define STB_GEMM_Q8 1                 // the q8 copy: b_tiles = its codes, with q8_scale and the query constants qc
 #define STB_GEMM_ALL 0
 #define STB_GEMM_LISTED 1
 #define STB_GEMM_WORK 2
 enum StbGemmEpi {
-  STB_EPI_SAMPLE,             // tile maxima into tilemax [m_tiles][n_tiles][128] (shadow: per-32-row submax and the
-                              // full score matrix full_out too, if given; q8: of the lower bound l)
+  STB_EPI_SAMPLE,             // tile maxima into tilemax [m_tiles][n_tiles][128] (q8: of the lower bound l); the
+                              // shadow's STB_GEMM_ALL pass also takes per-32-row maxima into submax, if given
   STB_EPI_EMIT,               // every (query, row) whose score (q8: upper bound u) reaches thr[query], into the
                               // per-(query, CTA) segments cand_keys [q_pad][grid][cand_cap], counts cand_cnt
   STB_EPI_EMIT_SIZED,         // the same into exactly sized segments cand_keys[seg_off[i], seg_off[i+1]) (i = query *
                               // grid + CTA), cand_cnt the zeroed cursors; STB_GEMM_ALL only
-  STB_EPI_DEBUG               // q8, STB_GEMM_ALL: dot, u and l of every (query, row), [m_tiles * 128][n_tiles * 256]
+  STB_EPI_DEBUG               // STB_GEMM_ALL: the scores the epilogues see for every (query, row), [m_tiles * 128]
+                              // [n_tiles * 256]: the shadow's into full_out, the q8 copy's dot, u and l
 };
 struct StbGemmPass {
-  int epi = STB_EPI_SAMPLE, select = STB_GEMM_ALL;
+  int copy = STB_GEMM_SHADOW, epi = STB_EPI_SAMPLE, select = STB_GEMM_ALL;
   const uint8_t *a_tiles = nullptr;              // query tiles: m_tiles x 64 KiB
+  const uint8_t *b_tiles = nullptr;
+  const float *q8_scale = nullptr;
+  const float4 *qc = nullptr;                    // [q_pad] {1/S, h_l1, e_q, S} (stb_launch_q8_query_tiles)
   uint32_t m_tiles = 0, n_tiles = 0, tile_stride = 1;
   uint64_t n_rows = 0;
   const uint32_t *tile_ids = nullptr, *bitmap = nullptr;
@@ -578,10 +582,8 @@ struct StbGemmPass {
   int32_t *dot_out = nullptr;
   float *u_out = nullptr, *l_out = nullptr;
 };
-// The pass on the corpus shadow, or on the q8 copy (codes, scales) with the query constants qc of
-// stb_launch_q8_query_tiles; a combination no kernel is built for is refused with STB_ERR_ARG
-int stb_launch_gemm_shadow(stb_ctx *ctx, const StbGemmPass &p, const uint8_t *shadow);
-int stb_launch_gemm_q8(stb_ctx *ctx, const StbGemmPass &p, const uint8_t *codes, const float *scales, const float4 *qc);
+// Launches pass p; a combination no kernel is built for is refused with STB_ERR_ARG
+int stb_launch_gemm(stb_ctx *ctx, const StbGemmPass &p);
 // the query slots of the STB_GEMM_WORK passes: f32 rows gathered into slot order, then the per-row bad flags scattered
 // back and the sampled maxima preset to -inf
 int stb_launch_batch_slots_gather(stb_ctx *ctx, const float *rows, const uint32_t *slot_row, uint32_t n_slots, float *out);

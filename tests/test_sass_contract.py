@@ -36,6 +36,16 @@ def test_resource_usage_of_the_hot_kernels():
     assert embed and max(embed) <= 80, embed
 
 
+def test_resource_usage_of_the_gemm_kernels():
+    """K2's GEMM holds a 64x256 accumulator in 128 registers per consumer thread at 1 CTA/SM: every
+    instantiation (shadow: 4 + 2 + 2, q8: 4 + 2) stays at <= 168 registers with nothing on the stack."""
+    out = _run("--dump-resource-usage")
+    fns = re.findall(r"Function (\S+):\s*\n\s*REG:(\d+) STACK:(\d+) SHARED:(\d+)", out)
+    gemm = [(n, int(r), int(st)) for n, r, st, _ in fns if "stb_batch_gemm_kernel" in n]
+    assert len(gemm) == 14, gemm
+    assert all(r <= 168 and st == 0 for _, r, st in gemm), gemm
+
+
 def test_hopper_instructions_are_where_the_design_says():
     sass = _run("-sass")
     per_fn, cur = {}, None
@@ -48,6 +58,7 @@ def test_hopper_instructions_are_where_the_design_says():
     gemm = "".join(v for k, v in per_fn.items() if "stb_batch_gemm" in k)
     assert "HGMMA.64x256x16.F32" in gemm and "UBLKCP" in gemm and "SYNCS" in gemm   # wgmma m64n256k16, cp.async.bulk, mbarrier
     assert "HMMA" not in gemm.replace("HGMMA", "")                               # no legacy mma.sync in the tensor path
+    assert "IGMMA.64x256x32.S8.S8" in gemm and "UTMALDG" in gemm                  # the q8 copy: s8 wgmma, TMA tensor loads
     q8 = [v for k, v in per_fn.items() if "stb_scan_topk_kernel" in k and "IDP.4A" in v]
     assert q8                                                                    # the int8 tier scans with dp4a
     k1 = [v for k, v in per_fn.items() if "stb_scan_topk_kernel" in k]
