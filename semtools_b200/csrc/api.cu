@@ -220,48 +220,107 @@ static int copy_prefix(stb_ctx *ctx, void *dst, const void *src, size_t bytes) {
   return STB_OK;
 }
 
-// q8 copy of `cap` rows (int8 codes + scales, 260 B/row, and the top-k prefilter's nibble plane + {s, rho},
-// 136 B/row) with the first `keep` rows of the current one; nothing changes when an allocation fails.
-static int q8_realloc(stb_corpus *c, uint64_t cap, uint64_t keep) {
-  StbBuf<uint8_t> q8, q4;
-  StbBuf<float> scale;
-  StbBuf<float2> sr;
+}  // extern "C"
+// ---- the candidate copies (StbCopy, common.cuh) ----
+// What sets the two copies apart beyond their buffers: growth to room for `cap` rows that keeps the first `keep`
+// (nothing changes when an allocation fails), the builder of rows [r0, r1) from rows_dev, whose first row is
+// row rows_first, and the message of a copy that holds rows which cannot be normalised.
+static int copy_realloc(stb_ctx *ctx, StbShadowCopy &k, uint64_t cap, uint64_t keep) {
+  StbShadowBufs g;
   int rc;
-  if ((rc = q8.alloc(cap * 256ull)) != STB_OK || (rc = scale.alloc(cap)) != STB_OK ||
-      (rc = q4.alloc(stb_q4_plane_bytes(cap))) != STB_OK || (rc = sr.alloc(cap)) != STB_OK)
+  if ((rc = g.tiles.alloc(StbShadowBufs::bytes(cap))) != STB_OK ||
+      (rc = copy_prefix(ctx, g.tiles, k.tiles, StbShadowBufs::bytes(keep))) != STB_OK)   // keep: whole tiles
     return rc;
-  if (c->q8 && keep &&
-      ((rc = copy_prefix(c->ctx, q8, c->q8, keep * 256ull)) != STB_OK ||
-       (rc = copy_prefix(c->ctx, scale, c->q8_scale, keep * sizeof(float))) != STB_OK ||
-       (rc = copy_prefix(c->ctx, q4, c->q4, stb_q4_plane_bytes(keep))) != STB_OK ||   // whole tiles
-       (rc = copy_prefix(c->ctx, sr, c->q4_sr, keep * sizeof(float2))) != STB_OK))
+  static_cast<StbShadowBufs &>(k) = std::move(g);
+  return STB_OK;
+}
+// int8 codes + scales, 260 B/row, and the top-k prefilter's nibble plane + {s, rho}, 136 B/row
+static int copy_realloc(stb_ctx *ctx, StbQ8Copy &k, uint64_t cap, uint64_t keep) {
+  StbQ8Bufs g;
+  int rc;
+  if ((rc = g.codes.alloc(cap * 256ull)) != STB_OK || (rc = g.scale.alloc(cap)) != STB_OK ||
+      (rc = g.plane.alloc(stb_q4_plane_bytes(cap))) != STB_OK || (rc = g.sr.alloc(cap)) != STB_OK)
     return rc;
-  c->q8 = std::move(q8); c->q8_scale = std::move(scale); c->q4 = std::move(q4); c->q4_sr = std::move(sr);
+  if (k.allocated() && keep &&
+      ((rc = copy_prefix(ctx, g.codes, k.codes, keep * 256ull)) != STB_OK ||
+       (rc = copy_prefix(ctx, g.scale, k.scale, keep * sizeof(float))) != STB_OK ||
+       (rc = copy_prefix(ctx, g.plane, k.plane, stb_q4_plane_bytes(keep))) != STB_OK ||   // whole tiles
+       (rc = copy_prefix(ctx, g.sr, k.sr, keep * sizeof(float2))) != STB_OK))
+    return rc;
+  static_cast<StbQ8Bufs &>(k) = std::move(g);
+  return STB_OK;
+}
+static int copy_build(stb_ctx *ctx, StbShadowCopy &k, const float *rows_dev, uint64_t r0, uint64_t r1, uint64_t rows_first) {
+  return stb_launch_shadow_build(ctx, rows_dev, r1, 256, k.tiles, ctx->err_flag, r0, nullptr, rows_first);
+}
+static int copy_build(stb_ctx *ctx, StbQ8Copy &k, const float *rows_dev, uint64_t r0, uint64_t r1, uint64_t rows_first) {
+  return stb_launch_q8_build(ctx, rows_dev, r0, r1, k.codes, k.scale, k.plane, k.sr, ctx->err_flag, rows_first);
+}
+static const char *copy_bad_rows(const StbShadowCopy &) {
+  return "search_batch: corpus holds rows whose norm is not a normal fp32 number; use stb_search";
+}
+static const char *copy_bad_rows(const StbQ8Copy &) { return "q8 tier: corpus holds rows whose norm is not a normal fp32 number"; }
+
+// Rows [first, n) of a host-rows corpus for a copy builder: uploaded into the context's staging buffer in chunks
+// of at most STB_MUT_CHUNK_ROWS rows (a multiple of the shadow's 256-row tile), fn(stage, r0, r1, r0) per chunk.
+template <class F>
+static int host_rows_staged(stb_corpus *c, uint64_t first, F &&fn) {
+  stb_ctx *ctx = c->ctx;
+  if (first >= c->n) return STB_OK;
+  const uint64_t chunk = std::min<uint64_t>(c->n - first, STB_MUT_CHUNK_ROWS);
+  int rc;
+  if ((rc = ctx->mut_stage.reserve(chunk * STB_D)) != STB_OK) return rc;
+  for (uint64_t r0 = first; r0 < c->n; r0 += chunk) {
+    const uint64_t m = std::min(chunk, c->n - r0);
+    STB_CUDA(cudaMemcpyAsync(ctx->mut_stage, c->rows_host + r0 * STB_D, m * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    if ((rc = fn(ctx->mut_stage, r0, r0 + m, r0)) != STB_OK) return rc;
+  }
   return STB_OK;
 }
 
-// A host-rows corpus grows both halves together: new pinned rows and a new q8 copy, then the old ones are
+// The one build-or-extend of a copy: makes it cover every row, converting only the rows behind its usable prefix
+// (all of them when it has none or is bad), from HBM or, on a host-rows corpus, through the staging buffer.  A
+// host-rows corpus gets here for its shadow, or to re-encode a q8 copy a mutation dropped as unusable.
+// STB_ERR_STATE: the copy holds rows that cannot be normalised in fp32, and is unusable.
+template <class Copy>
+static int corpus_ensure(stb_ctx *ctx, stb_corpus *c, Copy &k) {
+  if (!k.covers(c->n)) {
+    const uint64_t first = k.prefix(c->n);
+    int rc;
+    if (!k.has_room(c->n) && (rc = copy_realloc(ctx, k, std::max<uint64_t>(c->n, c->capacity), first)) != STB_OK) return rc;
+    STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
+    const auto build = [&](const float *rows, uint64_t r0, uint64_t r1, uint64_t rows_first) {
+      return copy_build(ctx, k, rows, r0, r1, rows_first);
+    };
+    if ((rc = c->host_rows ? host_rows_staged(c, first, build) : build(c->rows, first, c->n, 0)) != STB_OK) return rc;
+    int flag = 0;
+    STB_CUDA(cudaMemcpyAsync(&flag, ctx->err_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
+    STB_CUDA(cudaStreamSynchronize(ctx->stream));
+    k.rows = c->n;
+    k.bad = flag != 0;
+  }
+  if (k.bad) { stb_set_error("%s", copy_bad_rows(k)); return STB_ERR_STATE; }
+  return STB_OK;
+}
+extern "C" {
+
+// A host-rows corpus grows both halves together: new mapped rows and a new q8 copy, then the old ones are
 // copied and freed (so growing briefly holds two host buffers).  A failed allocation changes nothing.
 static int host_corpus_reserve(stb_corpus *c, uint64_t ncap) {
   stb_ctx *ctx = c->ctx;
-  float *hp = nullptr, *dp = nullptr;
-  cudaError_t e = cudaHostAlloc((void **)&hp, ncap * STB_D * sizeof(float), cudaHostAllocMapped | cudaHostAllocPortable);
-  if (e == cudaSuccess) e = cudaHostGetDevicePointer((void **)&dp, hp, 0);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    if (hp) cudaFreeHost(hp);
+  StbBuf<float, STB_MEM_MAPPED> grown;
+  cudaError_t e = cudaSuccess;
+  if (grown.alloc(ncap * STB_D, &e) != STB_OK) {
     stb_set_error("corpus: cannot allocate %llu rows of page-locked host memory: %s", (unsigned long long)ncap, cudaGetErrorString(e));
     return STB_ERR_NOMEM;
   }
-  int rc = q8_realloc(c, ncap, c->n);
-  if (rc != STB_OK) { cudaFreeHost(hp); return rc; }
+  int rc = copy_realloc(ctx, c->q8, ncap, c->n);
+  if (rc != STB_OK) return rc;
   STB_CUDA(cudaStreamSynchronize(ctx->stream));   // kernels write the rows (update, remove)
-  if (c->rows_host) {
-    memcpy(hp, c->rows_host, c->n * STB_D * sizeof(float));
-    cudaFreeHost(c->rows_host);
-  }
-  c->rows_host = hp;
-  c->rows = dp;
+  if (c->rows_host) memcpy(grown, c->rows_host, c->n * STB_D * sizeof(float));
+  c->rows_host = std::move(grown);
+  c->rows = c->rows_host.dev;
   c->capacity = ncap;
   return STB_OK;
 }
@@ -314,20 +373,19 @@ int stb_corpus_destroy(stb_corpus *c) {
   if (!c) return STB_OK;
   if (c->ctx && ctx_alive(c->ctx)) { cudaSetDevice(c->ctx->device); cudaStreamSynchronize(c->ctx->stream); }
   else cudaDeviceSynchronize();
-  if (c->host_rows) cudaFreeHost(c->rows_host);
   cudaGetLastError();
   delete c;
   return STB_OK;
 }
 
 // The reduced-width copies (K2 shadow, K1 tiers) cover a PREFIX of the rows: an append leaves the
-// prefix valid and the next query / prepare only converts the new rows (q8_rows / shadow_rows < n);
+// prefix valid and the next query / prepare only converts the new rows (StbCopy::rows < n);
 // an update or a removal re-encodes the copies at the rows it writes, so they stay built; a clear drops
 // them.  Anything but an append starts a new epoch; an update or a removal also ends a co-scan series on
 // the corpus (the next asynchronous top-k query starts at tile 0).
 enum CorpusChange { CORPUS_APPEND, CORPUS_ROWS_REWRITTEN, CORPUS_CLEAR };
 static void corpus_changed(stb_corpus *c, CorpusChange kind) {
-  if (kind == CORPUS_CLEAR) { c->shadow_rows = 0; c->q8_rows = 0; c->shadow_bad = 0; c->q8_bad = 0; }
+  if (kind == CORPUS_CLEAR) { c->shadow.drop(); c->q8.drop(); }
   if (kind != CORPUS_APPEND) ++c->epoch;
   c->ctx->series.forget_rows(c->rows, kind == CORPUS_ROWS_REWRITTEN);
   c->searches_since_change = 0;
@@ -335,7 +393,21 @@ static void corpus_changed(stb_corpus *c, CorpusChange kind) {
   memset(c->tier_proven, 0, sizeof(c->tier_proven));
 }
 
-static StbCorpusWriteArgs corpus_write_args(stb_corpus *c, uint64_t q8_rows, uint64_t shadow_rows);
+// The commit kernel's arguments (corpus_update.cu): the rows, the staging buffer, and each allocated copy with the
+// rows of it the kernel keeps current; it raises flags[0] for a q8 row and flags[1] for a shadow row that cannot
+// be normalised.
+static StbCorpusWriteArgs corpus_write_args(stb_corpus *c, uint64_t q8_cover, uint64_t shadow_cover) {
+  StbCorpusWriteArgs a;
+  memset(&a, 0, sizeof(a));
+  a.rows = reinterpret_cast<float4 *>(c->rows);
+  a.stage = reinterpret_cast<const float4 *>(c->ctx->mut_stage.p);
+  a.q8 = c->q8.codes; a.q8_scale = c->q8.scale; a.q4 = c->q8.plane; a.q4_sr = c->q8.sr;
+  a.q8_rows = c->q8.allocated() ? q8_cover : 0;
+  a.shadow = c->shadow.tiles;
+  a.shadow_rows = c->shadow.allocated() ? shadow_cover : 0;
+  a.flags = c->ctx->mut_flags;
+  return a;
+}
 
 // Appending to a host-rows corpus: staged rows [0, m) become rows first .. first + m - 1.  The commit kernel of the
 // in-place mutations writes them to the host rows and encodes their q8 entries from HBM in the same pass; the
@@ -362,8 +434,8 @@ static int host_append_finish(stb_corpus *c, uint64_t n) {
   STB_CUDA(cudaMemcpyAsync(flags, c->ctx->mut_flags, sizeof(flags), cudaMemcpyDeviceToHost, c->ctx->stream));
   STB_CUDA(cudaStreamSynchronize(c->ctx->stream));
   c->n += n;
-  c->q8_rows = c->n;
-  if (flags[0]) c->q8_bad = 1;
+  c->q8.rows = c->n;
+  c->q8.mark_bad(flags[0]);
   corpus_changed(c, CORPUS_APPEND);
   return STB_OK;
 }
@@ -564,9 +636,6 @@ int stb_embed_status(stb_ctx *ctx) {
 }
 
 // --------------------------------------------------------------------- search ---
-static int corpus_ensure_shadow(stb_ctx *ctx, stb_corpus *c);   // defined with the K2 entry points
-static int corpus_ensure_q8(stb_ctx *ctx, stb_corpus *c);
-
 // STB_SCAN_TIER = f32 | h16 | q8: the narrowest candidate tier K1 may use (default q8).  Read per
 // call so one process can compare tiers; results are identical whatever the value.
 static int stb_env_max_tier() {
@@ -591,15 +660,14 @@ static const K1CopyPolicy kBuiltOnly = {false, false};
 static int k1_copy_ready(stb_ctx *ctx, stb_corpus *c, int tier, uint32_t top_k, K1CopyPolicy policy, bool *ready) {
   *ready = tier == STB_TIER_F32;
   if (*ready || tier > stb_env_max_tier() || (tier == STB_TIER_Q8 && top_k > STB_Q8_MAX_K)) return STB_OK;
-  const bool q8 = tier == STB_TIER_Q8;
-  const bool have = q8 ? c->q8 != nullptr : c->shadow != nullptr;
-  const uint64_t rows = q8 ? c->q8_rows : c->shadow_rows;
-  const bool bad = q8 ? c->q8_bad : c->shadow_bad;
-  if (have && rows == c->n) { *ready = !bad; return STB_OK; }
-  if (!policy.build && !(policy.extend && have && rows > 0 && !bad)) return STB_OK;
-  const int rc = q8 ? corpus_ensure_q8(ctx, c) : corpus_ensure_shadow(ctx, c);
-  *ready = rc == STB_OK;
-  return rc == STB_ERR_STATE ? STB_OK : rc;
+  const auto ready_or_build = [&](auto &k) -> int {
+    if (k.covers(c->n)) { *ready = k.usable(c->n); return STB_OK; }
+    if (!policy.build && !(policy.extend && k.built() > 0)) return STB_OK;
+    const int rc = corpus_ensure(ctx, c, k);
+    *ready = rc == STB_OK;
+    return rc == STB_ERR_STATE ? STB_OK : rc;
+  };
+  return tier == STB_TIER_Q8 ? ready_or_build(c->q8) : ready_or_build(c->shadow);
 }
 
 // The single-GPU asynchronous entry points (stb_search_topk_dev, stb_search_many without an exchange) always
@@ -1012,93 +1080,6 @@ int stb_search_topk_xchg(stb_ctx *ctx, const stb_corpus *corpus, const float *q_
 }
 
 // ----------------------------------------------------------------- K2 batched search ---
-// Rows [first, n) of a host-rows corpus for a copy builder: uploaded into the context's staging buffer in chunks
-// of at most STB_MUT_CHUNK_ROWS rows (a multiple of the shadow's 256-row tile), fn(stage, r0, r1) per chunk.
-}  // extern "C"
-template <class F>
-static int host_rows_staged(stb_corpus *c, uint64_t first, F &&fn) {
-  stb_ctx *ctx = c->ctx;
-  if (first >= c->n) return STB_OK;
-  const uint64_t chunk = std::min<uint64_t>(c->n - first, STB_MUT_CHUNK_ROWS);
-  int rc;
-  if ((rc = ctx->mut_stage.reserve(chunk * STB_D)) != STB_OK) return rc;
-  for (uint64_t r0 = first; r0 < c->n; r0 += chunk) {
-    const uint64_t m = std::min(chunk, c->n - r0);
-    STB_CUDA(cudaMemcpyAsync(ctx->mut_stage, c->rows_host + r0 * STB_D, m * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-    if ((rc = fn(ctx->mut_stage, r0, r0 + m)) != STB_OK) return rc;
-  }
-  return STB_OK;
-}
-extern "C" {
-
-// The bytes corpus_ensure_shadow allocates to cover every row (0: the shadow it holds already has room)
-static uint64_t shadow_grow_bytes(const stb_corpus *c) {
-  const uint64_t tiles = (c->n + 255) / 256;
-  if (c->shadow && tiles * 131072ull <= c->shadow.cap) return 0;
-  return std::max<uint64_t>(tiles, (c->capacity + 255) / 256) * 131072ull;
-}
-
-static int corpus_ensure_shadow(stb_ctx *ctx, stb_corpus *c) {
-  if (c->shadow && c->shadow_rows == c->n) {
-    if (c->shadow_bad) { stb_set_error("search_batch: corpus holds rows whose norm is not a normal fp32 number; use stb_search"); return STB_ERR_STATE; }
-    return STB_OK;
-  }
-  uint64_t first = (c->shadow && c->shadow_rows < c->n && !c->shadow_bad) ? (c->shadow_rows / 256) * 256 : 0;   // valid prefix, whole tiles
-  int rc;
-  if (const uint64_t bytes = shadow_grow_bytes(c)) {
-    StbBuf<uint8_t> grown;
-    if ((rc = grown.alloc(bytes)) != STB_OK ||
-        (rc = copy_prefix(ctx, grown, c->shadow, (first / 256) * 131072ull)) != STB_OK)
-      return rc;
-    c->shadow = std::move(grown);
-  }
-  STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
-  if (c->host_rows)
-    rc = host_rows_staged(c, first, [&](const float *stage, uint64_t r0, uint64_t r1) {
-      return stb_launch_shadow_build(ctx, stage, r1, 256, c->shadow, ctx->err_flag, r0, nullptr, r0);
-    });
-  else
-    rc = stb_launch_shadow_build(ctx, c->rows, c->n, 256, c->shadow, ctx->err_flag, first);
-  if (rc != STB_OK) return rc;
-  int flag = 0;
-  STB_CUDA(cudaMemcpyAsync(&flag, ctx->err_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
-  STB_CUDA(cudaStreamSynchronize(ctx->stream));
-  c->shadow_rows = c->n;
-  c->shadow_bad = (first ? c->shadow_bad : 0) | flag;
-  if (c->shadow_bad) { stb_set_error("search_batch: corpus holds rows whose norm is not a normal fp32 number; use stb_search"); return STB_ERR_STATE; }
-  return STB_OK;
-}
-
-static int corpus_ensure_q8(stb_ctx *ctx, stb_corpus *c) {
-  if (c->q8 && c->q8_rows == c->n) {
-    if (c->q8_bad) { stb_set_error("q8 tier: corpus holds rows whose norm is not a normal fp32 number"); return STB_ERR_STATE; }
-    return STB_OK;
-  }
-  uint64_t first = (c->q8 && c->q8_rows < c->n && !c->q8_bad) ? c->q8_rows : 0;      // valid prefix: convert only the new rows
-  int rc;
-  if (c->n > c->q8_scale.cap || !c->q8) {
-    if ((rc = q8_realloc(c, std::max<uint64_t>(c->n, c->capacity), first)) != STB_OK) return rc;
-  }
-  STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
-  // a host-rows corpus gets here only to re-encode a copy a mutation dropped as unusable
-  if (c->host_rows)
-    rc = host_rows_staged(c, first, [&](const float *stage, uint64_t r0, uint64_t r1) {
-      return stb_launch_q8_build(ctx, stage, r0, r1, c->q8, c->q8_scale, c->q4, c->q4_sr, ctx->err_flag, r0);
-    });
-  else
-    rc = stb_launch_q8_build(ctx, c->rows, first, c->n, c->q8, c->q8_scale, c->q4, c->q4_sr, ctx->err_flag);
-  if (rc != STB_OK) return rc;
-  int flag = 0;
-  STB_CUDA(cudaMemcpyAsync(&flag, ctx->err_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  STB_CUDA(cudaMemsetAsync(ctx->err_flag, 0, sizeof(int), ctx->stream));
-  STB_CUDA(cudaStreamSynchronize(ctx->stream));
-  c->q8_rows = c->n;
-  c->q8_bad = (first ? c->q8_bad : 0) | flag;
-  if (c->q8_bad) { stb_set_error("q8 tier: corpus holds rows whose norm is not a normal fp32 number"); return STB_ERR_STATE; }
-  return STB_OK;
-}
-
 int stb_corpus_prepare(stb_corpus *corpus, int what) {
   if (!corpus) { stb_set_error("null corpus"); return STB_ERR_ARG; }
   if (what & ~(STB_PREPARE_Q8 | STB_PREPARE_H16)) { stb_set_error("corpus_prepare: unknown flag"); return STB_ERR_ARG; }
@@ -1107,8 +1088,8 @@ int stb_corpus_prepare(stb_corpus *corpus, int what) {
   if (corpus->n == 0) return STB_OK;
   // rows that cannot be normalised in fp32 make a copy unusable (STB_ERR_STATE): not an error of
   // this call -- searches simply stay on the f32 rows
-  if (what & STB_PREPARE_Q8) { rc = corpus_ensure_q8(corpus->ctx, corpus); if (rc != STB_OK && rc != STB_ERR_STATE) return rc; }
-  if (what & STB_PREPARE_H16) { rc = corpus_ensure_shadow(corpus->ctx, corpus); if (rc != STB_OK && rc != STB_ERR_STATE) return rc; }
+  if (what & STB_PREPARE_Q8) { rc = corpus_ensure(corpus->ctx, corpus, corpus->q8); if (rc != STB_OK && rc != STB_ERR_STATE) return rc; }
+  if (what & STB_PREPARE_H16) { rc = corpus_ensure(corpus->ctx, corpus, corpus->shadow); if (rc != STB_OK && rc != STB_ERR_STATE) return rc; }
   return STB_OK;
 }
 
@@ -1120,8 +1101,8 @@ int stb_corpus_tier_stats(const stb_corpus *corpus, uint32_t tries[3], uint32_t 
   }
   if (built_rows) {
     built_rows[STB_TIER_F32] = corpus->n;
-    built_rows[STB_TIER_H16] = (corpus->shadow && !corpus->shadow_bad) ? corpus->shadow_rows : 0;   // < n after an append: a valid prefix
-    built_rows[STB_TIER_Q8] = (corpus->q8 && !corpus->q8_bad) ? corpus->q8_rows : 0;
+    built_rows[STB_TIER_H16] = corpus->shadow.built();   // < n after an append: a valid prefix
+    built_rows[STB_TIER_Q8] = corpus->q8.built();
   }
   return STB_OK;
 }
@@ -1139,21 +1120,8 @@ static int corpus_mutation_check(stb_corpus *c, const char *what) {
 }
 
 static void corpus_drop_bad_copies(stb_corpus *c) {
-  if (c->q8_bad) { c->q8_rows = 0; c->q8_bad = 0; }
-  if (c->shadow_bad) { c->shadow_rows = 0; c->shadow_bad = 0; }
-}
-
-static StbCorpusWriteArgs corpus_write_args(stb_corpus *c, uint64_t q8_rows, uint64_t shadow_rows) {
-  StbCorpusWriteArgs a;
-  memset(&a, 0, sizeof(a));
-  a.rows = reinterpret_cast<float4 *>(c->rows);
-  a.stage = reinterpret_cast<const float4 *>(c->ctx->mut_stage.p);
-  a.q8 = c->q8; a.q8_scale = c->q8_scale; a.q4 = c->q4; a.q4_sr = c->q4_sr;
-  a.q8_rows = c->q8 ? q8_rows : 0;
-  a.shadow = c->shadow;
-  a.shadow_rows = c->shadow ? shadow_rows : 0;
-  a.flags = c->ctx->mut_flags;
-  return a;
+  if (c->q8.bad) c->q8.drop();
+  if (c->shadow.bad) c->shadow.drop();
 }
 
 // reads the bad-row flags the call's kernels raised (synchronises) and books the change
@@ -1162,12 +1130,12 @@ static int corpus_mutation_finish(stb_corpus *c) {
   int flags[2] = {0, 0};
   STB_CUDA(cudaMemcpyAsync(flags, ctx->mut_flags, sizeof(flags), cudaMemcpyDeviceToHost, ctx->stream));
   STB_CUDA(cudaStreamSynchronize(ctx->stream));
-  if (flags[0]) c->q8_bad = 1;
-  if (flags[1]) c->shadow_bad = 1;
+  c->q8.mark_bad(flags[0]);
+  c->shadow.mark_bad(flags[1]);
   corpus_changed(c, CORPUS_ROWS_REWRITTEN);
   // a host-rows corpus keeps its q8 copy current: one dropped as unusable is re-encoded from the rows now
-  if (c->host_rows && c->q8_rows < c->n) {
-    const int rc = corpus_ensure_q8(ctx, c);
+  if (c->host_rows && c->q8.rows < c->n) {
+    const int rc = corpus_ensure(ctx, c, c->q8);
     if (rc != STB_OK && rc != STB_ERR_STATE) return rc;
   }
   return STB_OK;
@@ -1209,7 +1177,7 @@ int stb_corpus_update_impl(stb_corpus *c, const uint64_t *idx, const float *rows
   const bool staged = hook && hook->staged_rows && n <= chunk;
   corpus_drop_bad_copies(c);
   STB_CUDA(cudaMemsetAsync(ctx->mut_flags, 0, 2 * sizeof(int), ctx->stream));
-  StbCorpusWriteArgs a = corpus_write_args(c, c->q8_rows, c->shadow_rows);
+  StbCorpusWriteArgs a = corpus_write_args(c, c->q8.rows, c->shadow.rows);
   a.idx = ctx->mut_idx;
   std::vector<uint64_t> local(chunk);
   for (uint64_t i0 = 0; i0 < n; i0 += chunk) {
@@ -1249,23 +1217,21 @@ int stb_corpus_remove_impl(stb_corpus *c, const uint64_t *ranges, uint32_t n_ran
       return STB_ERR_RANGE;
     }
   stb_ctx *ctx = c->ctx;
-  // kept segments behind the first removed row, as {destination, source} local rows; removed rows inside the
-  // prefix each copy covers (a copy marked bad is dropped below: it covers none)
+  // kept segments behind the first removed row, as {destination, source} local rows; the rows each copy covers
+  // afterwards (a copy marked bad is dropped below: it covers none)
   std::vector<uint64_t> seg;
-  const uint64_t q8_had = c->q8_bad ? 0 : c->q8_rows, shadow_had = c->shadow_bad ? 0 : c->shadow_rows;
-  uint64_t removed = 0, removed_q8 = 0, removed_shadow = 0;
+  uint64_t removed = 0;
   const uint64_t first = ranges[0] - lo;
   uint64_t dst = first;
   for (uint32_t i = 0; i < n_ranges; ++i) {
     const uint64_t b = ranges[2 * i] - lo, e = ranges[2 * i + 1] - lo;
     const uint64_t next = (i + 1 < n_ranges) ? ranges[2 * i + 2] - lo : c->n;
     removed += e - b;
-    if (q8_had > b) removed_q8 += std::min(e, q8_had) - b;
-    if (shadow_had > b) removed_shadow += std::min(e, shadow_had) - b;
     if (next > e) { seg.push_back(dst); seg.push_back(e); dst += next - e; }
   }
   const uint64_t moved = dst - first;
-  const uint64_t q8_rows = q8_had - removed_q8, shadow_rows = shadow_had - removed_shadow;
+  const uint64_t q8_left = c->q8.covered_after_remove(ranges, n_ranges, lo);
+  const uint64_t shadow_left = c->shadow.covered_after_remove(ranges, n_ranges, lo);
   if ((rc = ctx->mut_flags.reserve(2)) != STB_OK) return rc;
   if (moved) {
     const uint64_t chunk = std::min<uint64_t>(moved, STB_MUT_CHUNK_ROWS);
@@ -1280,7 +1246,7 @@ int stb_corpus_remove_impl(stb_corpus *c, const uint64_t *ranges, uint32_t n_ran
     // reads rows no earlier chunk has overwritten, and it completes before the commit writes.
     STB_CUDA(cudaMemcpyAsync(ctx->mut_idx, seg.data(), seg.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->stream));
     const uint32_t n_seg = (uint32_t)(seg.size() / 2);
-    StbCorpusWriteArgs a = corpus_write_args(c, q8_rows, shadow_rows);
+    StbCorpusWriteArgs a = corpus_write_args(c, q8_left, shadow_left);
     for (uint64_t d0 = first; d0 < first + moved; d0 += STB_MUT_CHUNK_ROWS) {
       a.first = d0;
       a.m = std::min<uint64_t>(STB_MUT_CHUNK_ROWS, first + moved - d0);
@@ -1289,12 +1255,12 @@ int stb_corpus_remove_impl(stb_corpus *c, const uint64_t *ranges, uint32_t n_ran
     }
     STB_CUDA(cudaStreamSynchronize(ctx->stream));   // `seg` dies at scope end
   }
-  // the shadow's last covered tile ends in zero padding, as a build of `shadow_rows` rows leaves it
-  if (c->shadow && shadow_rows % 256 &&
-      (rc = stb_launch_shadow_build(ctx, c->rows, shadow_rows, 256, c->shadow, ctx->mut_flags + 1, shadow_rows)) != STB_OK) return rc;
+  // the shadow's last covered tile ends in zero padding, as a build of `shadow_left` rows leaves it
+  if (c->shadow.allocated() && shadow_left % 256 &&
+      (rc = stb_launch_shadow_build(ctx, c->rows, shadow_left, 256, c->shadow.tiles, ctx->mut_flags + 1, shadow_left)) != STB_OK) return rc;
   c->n -= removed;
-  c->q8_rows = q8_rows;
-  c->shadow_rows = shadow_rows;
+  c->q8.rows = q8_left;
+  c->shadow.rows = shadow_left;
   return corpus_mutation_finish(c);
 }
 
@@ -1310,14 +1276,14 @@ int stb_debug_corpus_copy(const stb_corpus *c, int which, uint64_t first, uint64
   if (rc) return rc;
   const void *src = nullptr;
   size_t unit = 0;
-  uint64_t rows = c->q8 ? c->q8_rows : 0, units = rows;
+  uint64_t rows = c->q8.covered(), units = rows;
   switch (which) {
-    case STB_COPY_Q8_CODES: src = c->q8; unit = 256; break;
-    case STB_COPY_Q8_SCALES: src = c->q8_scale; unit = sizeof(float); break;
-    case STB_COPY_Q8_PLANE: src = c->q4; unit = 128; break;
-    case STB_COPY_Q8_SR: src = c->q4_sr; unit = sizeof(float2); break;
+    case STB_COPY_Q8_CODES: src = c->q8.codes; unit = 256; break;
+    case STB_COPY_Q8_SCALES: src = c->q8.scale; unit = sizeof(float); break;
+    case STB_COPY_Q8_PLANE: src = c->q8.plane; unit = 128; break;
+    case STB_COPY_Q8_SR: src = c->q8.sr; unit = sizeof(float2); break;
     case STB_COPY_H16_TILES:
-      src = c->shadow; unit = 131072; rows = c->shadow ? c->shadow_rows : 0; units = (rows + 255) / 256; break;
+      src = c->shadow.tiles; unit = 131072; rows = c->shadow.covered(); units = (rows + 255) / 256; break;
     default: stb_set_error("debug_corpus_copy: unknown copy %d", which); return STB_ERR_ARG;
   }
   if (covered) *covered = rows;
@@ -1349,7 +1315,7 @@ int stb_corpus_prepare_batch(stb_corpus *corpus) {
   int rc = ctx_use(corpus->ctx);
   if (rc) return rc;
   if (corpus->n == 0) return STB_OK;
-  return corpus_ensure_shadow(corpus->ctx, corpus);
+  return corpus_ensure(corpus->ctx, corpus, corpus->shadow);
 }
 
 }  // extern "C"
@@ -1367,9 +1333,9 @@ static void k2_record(stb_ctx *ctx, K2Route route, uint32_t nq, uint32_t a = 0, 
   memcpy(ctx->b_last, words, sizeof(words));
 }
 
-// The shadow as every K2 search call sees it.  batch_shadow is corpus_ensure_shadow, for a call that then reads the
+// The shadow as every K2 search call sees it.  batch_shadow is corpus_ensure, for a call that then reads the
 // shadow.  batch_shadow_fits is for a call whose shadow plan does not fit but whose q8 plan does: it would not read
-// the shadow, so none is built; it asks only whether corpus_ensure_shadow could allocate it (STB_ERR_NOMEM if not),
+// the shadow, so none is built; it asks only whether corpus_ensure could allocate it (STB_ERR_NOMEM if not),
 // with a trial allocation of the same size, released at once.  STB_ERR_NOMEM is the trigger of the q8 routes.
 // While stb_debug_batch_no_shadow is on, both return STB_ERR_NOMEM without building or touching the shadow.
 static int batch_no_shadow_hook(const stb_ctx *ctx) {
@@ -1379,15 +1345,14 @@ static int batch_no_shadow_hook(const stb_ctx *ctx) {
 }
 static int batch_shadow(stb_ctx *ctx, stb_corpus *c) {
   const int rc = batch_no_shadow_hook(ctx);
-  return rc != STB_OK ? rc : corpus_ensure_shadow(ctx, c);
+  return rc != STB_OK ? rc : corpus_ensure(ctx, c, c->shadow);
 }
 static int batch_shadow_fits(stb_ctx *ctx, const stb_corpus *c) {
   const int rc = batch_no_shadow_hook(ctx);
   if (rc != STB_OK) return rc;
-  const uint64_t bytes = shadow_grow_bytes(c);
-  if (bytes == 0) return STB_OK;
+  if (c->shadow.has_room(c->n)) return STB_OK;
   StbBuf<uint8_t> trial;
-  return trial.alloc(bytes);
+  return trial.alloc(StbShadowBufs::bytes(std::max<uint64_t>(c->n, c->capacity)));
 }
 
 // The copy a K2 call reads: the 16-bit shadow, the q8 copy (where the shadow does not fit in HBM), or neither
@@ -1423,7 +1388,7 @@ static int k2_choose_copy(stb_ctx *ctx, stb_corpus *corpus, bool reads_shadow, b
   out->status = rc;
   out->shadow_err = stb_last_error();
   if (!q8_usable) return STB_OK;
-  if ((rc = corpus_ensure_q8(ctx, corpus)) == STB_OK) { out->copy = K2Copy::kQ8; return STB_OK; }
+  if ((rc = corpus_ensure(ctx, corpus, corpus->q8)) == STB_OK) { out->copy = K2Copy::kQ8; return STB_OK; }
   if (rc != STB_ERR_NOMEM && rc != STB_ERR_STATE) return rc;
   stb_set_error("%s", out->shadow_err.c_str());
   return STB_OK;
@@ -1493,8 +1458,8 @@ static int k2_query_tiles(stb_ctx *ctx, K2Copy copy, const float *q_dev, uint32_
 // GEMM pass p of the m_tiles query tiles in ctx->bq_tiles over the corpus's `copy`
 static int k2_gemm(stb_ctx *ctx, const stb_corpus *corpus, K2Copy copy, uint32_t m_tiles, StbGemmPass p) {
   p.a_tiles = ctx->bq_tiles; p.m_tiles = m_tiles; p.n_rows = corpus->n;
-  if (copy == K2Copy::kQ8) { p.copy = STB_GEMM_Q8; p.b_tiles = corpus->q8; p.q8_scale = corpus->q8_scale; p.qc = ctx->b_q8c; }
-  else p.b_tiles = corpus->shadow;
+  if (copy == K2Copy::kQ8) { p.copy = STB_GEMM_Q8; p.b_tiles = corpus->q8.codes; p.q8_scale = corpus->q8.scale; p.qc = ctx->b_q8c; }
+  else p.b_tiles = corpus->shadow.tiles;
   return stb_launch_gemm(ctx, p);
 }
 
@@ -1538,7 +1503,7 @@ static int k2_topk_run(stb_ctx *ctx, const stb_corpus *corpus, K2Copy copy, cons
   if ((rc = k2_gemm(ctx, corpus, copy, m_tiles, pass)) != STB_OK) return rc;
   return stb_launch_batch_finish2(ctx, ctx->b_keys, ctx->b_cnt, n_seg, kSegCap, nq, top_k, corpus->rows, corpus->n,
                                   corpus->row_base, q_dev, ctx->b_qbad, out_hits_dev, out_status_dev,
-                                  q8 ? (const float *)corpus->q8_scale : nullptr, q8 ? (const float4 *)ctx->b_q8c : nullptr,
+                                  q8 ? (const float *)corpus->q8.scale : nullptr, q8 ? (const float4 *)ctx->b_q8c : nullptr,
                                   q8 ? (const float *)ctx->b_thr : nullptr);
 }
 
@@ -1659,7 +1624,7 @@ static int batch_dev_impl(stb_ctx *ctx, const stb_corpus *corpus_c, const float 
   if (corpus->n == 0) { stb_set_error("search_batch_dev: empty corpus"); return STB_ERR_STATE; }
   K2Choice ch;
   if (q8_route) {
-    if ((rc = corpus_ensure_q8(ctx, corpus)) != STB_OK) return rc;
+    if ((rc = corpus_ensure(ctx, corpus, corpus->q8)) != STB_OK) return rc;
     ch.copy = K2Copy::kQ8;
   } else if ((rc = k2_choose_copy(ctx, corpus, true, true, &ch)) != STB_OK) {
     return rc;
@@ -2453,7 +2418,7 @@ int stb_debug_batch_q8_gemm(stb_ctx *ctx, const stb_corpus *corpus_c, const floa
   stb_corpus *corpus = const_cast<stb_corpus *>(corpus_c);
   if (!corpus || !q || !q16 || !dot || !u || !l || nq == 0 || corpus->n == 0) { stb_set_error("debug_batch_q8_gemm: bad argument"); return STB_ERR_ARG; }
   if (corpus->ctx != ctx) { stb_set_error("debug_batch_q8_gemm: corpus belongs to another context"); return STB_ERR_ARG; }
-  if ((rc = corpus_ensure_q8(ctx, corpus)) != STB_OK) return rc;
+  if ((rc = corpus_ensure(ctx, corpus, corpus->q8)) != STB_OK) return rc;
   const uint32_t m_tiles = (nq + 127) / 128;
   const size_t q_pad = (size_t)m_tiles * 128, n = corpus->n, n_pad = (n + 255) / 256 * 256;
   StbBuf<float> dq, du, dl;
@@ -2468,7 +2433,7 @@ int stb_debug_batch_q8_gemm(stb_ctx *ctx, const stb_corpus *corpus_c, const floa
     return rc;
   StbGemmPass p;
   p.copy = STB_GEMM_Q8; p.epi = STB_EPI_DEBUG; p.a_tiles = da; p.m_tiles = m_tiles; p.n_tiles = (uint32_t)(n_pad / 256);
-  p.n_rows = n; p.b_tiles = corpus->q8; p.q8_scale = corpus->q8_scale; p.qc = dc;
+  p.n_rows = n; p.b_tiles = corpus->q8.codes; p.q8_scale = corpus->q8.scale; p.qc = dc;
   p.dot_out = ddot; p.u_out = du; p.l_out = dl;
   STB_CUDA(cudaMemcpyAsync(dq, q, (size_t)nq * STB_D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
   if ((rc = stb_launch_q8_query_tiles(ctx, dq, nq, (uint32_t)q_pad, da, dc, dbad, d16)) != STB_OK ||
@@ -2484,11 +2449,6 @@ int stb_debug_batch_q8_gemm(stb_ctx *ctx, const stb_corpus *corpus_c, const floa
 
 // ------------------------------------------------------------------- K1 debug hooks ---
 // The scan passes' per-row scores, for tests that check each pass's contract row by row (DESIGN.md section 5).
-static bool k1_copy_usable(const stb_corpus *c, int tier) {
-  if (tier == STB_TIER_Q8) return c->q8 && c->q4 && c->q8_rows == c->n && !c->q8_bad;
-  if (tier == STB_TIER_H16) return c->shadow && c->shadow_rows == c->n && !c->shadow_bad;
-  return true;
-}
 
 // Query and ranges staged like stb_search's; per-row device outputs: `floats` arrays of n f32 (NaN-filled) and one of
 // n u32 (zeroed), in the one buffer f_dev.
@@ -2514,7 +2474,7 @@ int stb_debug_scan_scores(stb_ctx *ctx, const stb_corpus *corpus, int tier, cons
   if (tier < STB_TIER_F32 || tier > STB_TIER_Q8) { stb_set_error("debug_scan_scores: unknown tier %d", tier); return STB_ERR_ARG; }
   if (hist && tier == STB_TIER_H16) { stb_set_error("debug_scan_scores: no histogram pass reads the 16-bit shadow"); return STB_ERR_ARG; }
   if (cap < corpus->n) { stb_set_error("debug_scan_scores: outputs hold %llu rows, the corpus %llu", (unsigned long long)cap, (unsigned long long)corpus->n); return STB_ERR_ARG; }
-  if (!k1_copy_usable(corpus, tier)) { stb_set_error("debug_scan_scores: tier %d copy not built or unusable", tier); return STB_ERR_STATE; }
+  if (!corpus->tier_usable(tier)) { stb_set_error("debug_scan_scores: tier %d copy not built or unusable", tier); return STB_ERR_STATE; }
   if (hist) memset(hist, 0, 4096 * sizeof(uint32_t));
   if (corpus->n == 0) return STB_OK;
   StbBuf<float> d_score;
@@ -2547,7 +2507,7 @@ int stb_debug_q4_scan(stb_ctx *ctx, const stb_corpus *corpus, const float *q, ui
   if (corpus->ctx != ctx) { stb_set_error("debug_q4_scan: corpus belongs to another context"); return STB_ERR_ARG; }
   if (top_k < 1 || top_k > STB_Q8_MAX_K) { stb_set_error("debug_q4_scan: top_k must be 1..%d", STB_Q8_MAX_K); return STB_ERR_ARG; }
   if (cap < corpus->n) { stb_set_error("debug_q4_scan: outputs hold %llu rows, the corpus %llu", (unsigned long long)cap, (unsigned long long)corpus->n); return STB_ERR_ARG; }
-  if (!k1_copy_usable(corpus, STB_TIER_Q8)) { stb_set_error("debug_q4_scan: q8 copy not built or unusable"); return STB_ERR_STATE; }
+  if (!corpus->tier_usable(STB_TIER_Q8)) { stb_set_error("debug_q4_scan: q8 copy not built or unusable"); return STB_ERR_STATE; }
   memset(words, 0, top_k * sizeof(uint64_t));
   if (corpus->n == 0) return STB_OK;
   const size_t n = corpus->n;

@@ -66,62 +66,75 @@ void stb_set_error(const char *fmt, ...);
     }                                                                              \
   } while (0)
 
-// The one owner of every device (cudaMalloc) and page-locked host (cudaMallocHost) buffer of the library: cap
-// elements of T at p, freed by the destructor.  It converts to T *, so launches, copies and indexing read it as
-// the pointer.  alloc(n) frees what it holds, then allocates exactly n elements.  reserve(need, floor) keeps
-// the buffer if it holds need elements, else allocates max(need, floor, 1.5 cap) and only then frees the old
-// one.  Neither keeps the contents.  A failed allocation returns STB_ERR_NOMEM with the byte count in the
-// error message and leaves the buffer as it was (after alloc's free: empty).  Freeing an old buffer that a
-// kernel may still read is the caller's to order (stream synchronise).
-template <class T, bool PINNED = false>
+// The one owner of every device (cudaMalloc), page-locked host (cudaMallocHost) and device-mapped host
+// (cudaHostAlloc, mapped and portable) buffer of the library: cap elements of T at p, freed by the destructor.
+// It converts to T *, so launches, copies and indexing read it as the pointer; dev is the address kernels use
+// (the device alias of a mapped buffer, p otherwise).  alloc(n) frees what it holds, then allocates exactly n
+// elements.  reserve(need, floor) keeps the buffer if it holds need elements, else allocates
+// max(need, floor, 1.5 cap) and only then frees the old one.  Neither keeps the contents.  A failed allocation
+// returns STB_ERR_NOMEM with the byte count in the error message (and the CUDA error in *why, if given) and
+// leaves the buffer as it was (after alloc's free: empty).  Freeing an old buffer that a kernel may still read
+// is the caller's to order (stream synchronise).
+enum StbMem { STB_MEM_DEVICE, STB_MEM_PINNED, STB_MEM_MAPPED };
+template <class T, int MEM = STB_MEM_DEVICE>
 struct StbBuf {
   T *p = nullptr;
+  T *dev = nullptr;
   size_t cap = 0;
   StbBuf() = default;
   StbBuf(const StbBuf &) = delete;
   StbBuf &operator=(const StbBuf &) = delete;
-  StbBuf(StbBuf &&o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  StbBuf(StbBuf &&o) noexcept : p(o.p), dev(o.dev), cap(o.cap) { o.p = o.dev = nullptr; o.cap = 0; }
   StbBuf &operator=(StbBuf &&o) noexcept {
-    if (this != &o) { release(); p = o.p; cap = o.cap; o.p = nullptr; o.cap = 0; }
+    if (this != &o) { release(); p = o.p; dev = o.dev; cap = o.cap; o.p = o.dev = nullptr; o.cap = 0; }
     return *this;
   }
   ~StbBuf() { release(); }
   operator T *() const { return p; }
-  int alloc(size_t n) {
+  int alloc(size_t n, cudaError_t *why = nullptr) {
     release();
-    return take(n);
+    return take(n, why);
   }
   int reserve(size_t need, size_t floor = 0) {
     if (need <= cap && p) return STB_OK;
     size_t n = need > floor ? need : floor;
     if (cap + cap / 2 > n) n = cap + cap / 2;
-    return take(n);
+    return take(n, nullptr);
   }
 
  private:
-  int take(size_t n) {
-    void *np = nullptr;
-    const cudaError_t e = PINNED ? cudaMallocHost(&np, n * sizeof(T)) : cudaMalloc(&np, n * sizeof(T));
+  int take(size_t n, cudaError_t *why) {
+    void *np = nullptr, *dp = nullptr;
+    cudaError_t e = MEM == STB_MEM_PINNED ? cudaMallocHost(&np, n * sizeof(T))
+                  : MEM == STB_MEM_MAPPED ? cudaHostAlloc(&np, n * sizeof(T), cudaHostAllocMapped | cudaHostAllocPortable)
+                                          : cudaMalloc(&np, n * sizeof(T));
+    dp = np;
+    if (MEM == STB_MEM_MAPPED && e == cudaSuccess) e = cudaHostGetDevicePointer(&dp, np, 0);
     if (e != cudaSuccess) {
       cudaGetLastError();
-      stb_set_error("%s(%zu bytes) failed: %s", PINNED ? "cudaMallocHost" : "cudaMalloc", n * sizeof(T), cudaGetErrorString(e));
+      if (np) free_mem(np);
+      if (why) *why = e;
+      stb_set_error("%s(%zu bytes) failed: %s", MEM == STB_MEM_DEVICE ? "cudaMalloc" : MEM == STB_MEM_PINNED ? "cudaMallocHost" : "cudaHostAlloc",
+                    n * sizeof(T), cudaGetErrorString(e));
       return STB_ERR_NOMEM;
     }
     release();
     p = static_cast<T *>(np);
+    dev = static_cast<T *>(dp);
     cap = n;
     return STB_OK;
   }
+  static void free_mem(void *q) {
+    if (MEM == STB_MEM_DEVICE) cudaFree(q); else cudaFreeHost(q);
+    cudaGetLastError();
+  }
   void release() {
-    if (p) {
-      if (PINNED) cudaFreeHost(p); else cudaFree(p);
-      cudaGetLastError();
-    }
-    p = nullptr;
+    if (p) free_mem(p);
+    p = dev = nullptr;
     cap = 0;
   }
 };
-template <class T> using StbPinned = StbBuf<T, true>;
+template <class T> using StbPinned = StbBuf<T, STB_MEM_PINNED>;
 
 #define STB_TICKET_SLOTS 8
 #define STB_TICKET_TILES 4   // co-scan, 10M rows, q8: 4 and 2 tiles 0.434 ms/query, 1 tile 0.635 ms
@@ -323,35 +336,82 @@ struct stb_table {
   int normalize;
 };
 
+// The buffers of the corpus's two reduced-width candidate copies, and what tells them apart: the rows a build or
+// an extension starts on a multiple of (kUnit), and the rows the buffers have room for.
+struct StbShadowBufs {            // L2-normalised 16-bit rows in wgmma tile layout (K2's operand, K1's h16 tier)
+  static constexpr uint64_t kUnit = 256;
+  static uint64_t bytes(uint64_t rows) { return (rows + 255) / 256 * 131072ull; }   // whole tiles of 128 KiB
+  StbBuf<uint8_t> tiles;
+  const void *data() const { return tiles.p; }
+  uint64_t room() const { return tiles.cap / 131072 * 256; }
+};
+struct StbQ8Bufs {                // K1's q8 tier and its top-k prefilter, K2's q8 routes
+  static constexpr uint64_t kUnit = 1;
+  StbBuf<uint8_t> codes;          // int8 codes [room][256] + per-row scale
+  StbBuf<float> scale;
+  StbBuf<uint8_t> plane;          // nibble plane [room][128] (tile-interleaved) + per-row {s, rho}
+  StbBuf<float2> sr;
+  const void *data() const { return codes.p; }
+  uint64_t room() const { return scale.cap; }   // all four are allocated together, for the same rows
+};
+// A candidate copy (DESIGN.md section 3, "Candidate copies"): the one owner of its buffers and of its state.  It
+// covers the corpus's rows [0, rows); bad: one of those rows cannot be normalised in fp32, which makes the whole
+// copy unusable until it is dropped or rebuilt.
+template <class Bufs>
+struct StbCopy : Bufs {
+  uint64_t rows = 0;
+  bool bad = false;
+  bool allocated() const { return this->data() != nullptr; }
+  bool covers(uint64_t n) const { return allocated() && rows == n; }
+  bool has_room(uint64_t n) const { return allocated() && n <= Bufs::room(); }
+  // the one usability rule: a scan over a corpus of n rows may read it
+  bool usable(uint64_t n) const { return covers(n) && !bad; }
+  uint64_t covered() const { return allocated() ? rows : 0; }
+  // the rows it holds usable: all n, or a prefix after an append; 0 when bad
+  uint64_t built() const { return bad ? 0 : covered(); }
+  // where a build for n rows starts: the end of the usable prefix in whole units, 0 to build from nothing
+  uint64_t prefix(uint64_t n) const { return rows < n ? built() / Bufs::kUnit * Bufs::kUnit : 0; }
+  // the rows it covers once the rows of n_ranges ascending, disjoint ranges [b, e) (minus lo) are removed
+  uint64_t covered_after_remove(const uint64_t *ranges, uint32_t n_ranges, uint64_t lo) const {
+    const uint64_t had = built();
+    uint64_t left = had;
+    for (uint32_t i = 0; i < n_ranges; ++i) {
+      const uint64_t b = ranges[2 * i] - lo, e = ranges[2 * i + 1] - lo;
+      if (b < had) left -= (e < had ? e : had) - b;
+    }
+    return left;
+  }
+  void drop() { rows = 0; bad = false; }
+  void mark_bad(int flag) { bad = bad || flag != 0; }   // flag: a kernel's bad-row flag
+};
+using StbShadowCopy = StbCopy<StbShadowBufs>;
+using StbQ8Copy = StbCopy<StbQ8Bufs>;
+
 struct stb_corpus {
   stb_ctx *ctx;
-  float *rows;         // capacity x 256: dev_rows, or on a host-rows corpus the device address of rows_host
+  float *rows;         // capacity x 256: dev_rows, or on a host-rows corpus the device alias of rows_host
   StbBuf<float> dev_rows;   // a device corpus's rows
   // stb_corpus_create_host: the rows live in page-locked, device-mapped host memory (kernels read them over
   // the host link through `rows`) and the q8 copy is kept current by every call that writes rows
-  float *rows_host;    // null on a device corpus
+  StbBuf<float, STB_MEM_MAPPED> rows_host;   // empty on a device corpus
   int host_rows;
   uint64_t n;
   uint64_t capacity;
   uint64_t row_base;
   uint64_t epoch;            // bumped by every change that is not an append (an IVF-PQ index refuses to extend over it)
-  // K2: L2-normalised bf16 copy in wgmma tile layout (built lazily, rebuilt when n changes)
-  StbBuf<uint8_t> shadow;    // whole 256-row tiles of 128 KiB
-  uint64_t shadow_rows;      // rows covered by `shadow` (== n when valid)
-  int shadow_bad;            // 1: some row cannot be normalised in fp32 -> tensor path refused
-  // K1 tier q8: int8 codes [capacity][256] + per-row scale, built lazily / by stb_corpus_prepare
-  // (q8_scale.cap: the rows all four hold)
-  StbBuf<uint8_t> q8;
-  StbBuf<float> q8_scale;
-  StbBuf<uint8_t> q4;        // ... its nibble plane [capacity][128] and per-row {s, rho} (top-k prefilter)
-  StbBuf<float2> q4_sr;
-  uint64_t q8_rows;          // rows covered (== n when valid; also the plane's)
-  int q8_bad;
+  // the candidate copies, built lazily, by stb_corpus_prepare or by K2 (api.cu: corpus_ensure), kept current by
+  // the in-place mutations
+  StbShadowCopy shadow;
+  StbQ8Copy q8;
   // per-tier bookkeeping: a reduced-width tier is skipped once it proves fewer than half of its
   // results on this corpus (index = STB_TIER_*)
   uint32_t tier_tries[3], tier_proven[3];
   uint32_t searches_since_change;   // lazy builds wait for the second query on an unchanged corpus
   uint32_t ivfpq_live;       // IVF-PQ indexes built on this corpus and not yet destroyed: update / remove refuse
+  // StbCopy::usable for the copy K1's tier `tier` scans (the f32 rows always are)
+  bool tier_usable(int tier) const {
+    return tier == STB_TIER_Q8 ? q8.usable(n) : tier == STB_TIER_H16 ? shadow.usable(n) : true;
+  }
 };
 
 // Row ranges as stb_search takes them: n half-open [begin, end) pairs, ascending and disjoint (api.cu).

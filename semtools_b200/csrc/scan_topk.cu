@@ -1652,18 +1652,18 @@ int stb_launch_scan_topk(stb_ctx *ctx, const stb_corpus *c, int tier, const floa
   a.top_k = top_k;
   if (xchg) a.xchg = *xchg; else memset(&a.xchg, 0, sizeof(a.xchg));
   a.early_trigger = 0;
-  a.shadow = c->shadow;
-  a.q8 = c->q8;
-  a.q8_scale = c->q8_scale;
+  a.shadow = c->shadow.tiles;
+  a.q8 = c->q8.codes;
+  a.q8_scale = c->q8.scale;
   memset(&a.q4, 0, sizeof(a.q4));
-  if (tier == STB_TIER_Q8 && (top_k > STB_Q8_MAX_K || !c->q8 || !c->q4)) { stb_set_error("scan_topk: q8 tier unavailable"); return STB_ERR_STATE; }
+  if (tier == STB_TIER_Q8 && (top_k > STB_Q8_MAX_K || !c->tier_usable(tier))) { stb_set_error("scan_topk: q8 tier unavailable"); return STB_ERR_STATE; }
   if (tier == STB_TIER_Q8) {
-    a.q4.plane = c->q4;   // its threshold words and tag: the launch's slot of the series (stb_launch_topk_t)
-    a.q4.sr = c->q4_sr;
+    a.q4.plane = c->q8.plane;   // its threshold words and tag: the launch's slot of the series (stb_launch_topk_t)
+    a.q4.sr = c->q8.sr;
     a.q4.top_k = top_k > 0 ? top_k : 1;
     a.q4.refined = ctx->q4_refined;
   }
-  if (tier == STB_TIER_H16 && !c->shadow) { stb_set_error("scan_topk: h16 tier unavailable"); return STB_ERR_STATE; }
+  if (tier == STB_TIER_H16 && !c->tier_usable(tier)) { stb_set_error("scan_topk: h16 tier unavailable"); return STB_ERR_STATE; }
   return ranges.n > 0 ? stb_launch_topk_r<1>(ctx, a, tier, top_k, overlapped) : stb_launch_topk_r<0>(ctx, a, tier, top_k, overlapped);
 }
 
@@ -1811,7 +1811,7 @@ int stb_launch_scan_collect(stb_ctx *ctx, const stb_corpus *c, int tier, const f
                             const StbRowRanges &ranges) {
   CollectArgs a;
   a.scan = stb_scan_args(c, q_dev, ranges);
-  a.q8 = c->q8; a.q8_scale = c->q8_scale;
+  a.q8 = c->q8.codes; a.q8_scale = c->q8.scale;
   a.cos_floor = cos_floor;
   a.out = ctx->collect_rows;
   a.count = ctx->collect_count;
@@ -1819,7 +1819,7 @@ int stb_launch_scan_collect(stb_ctx *ctx, const stb_corpus *c, int tier, const f
   STB_CUDA(cudaMemsetAsync(ctx->collect_count, 0, sizeof(unsigned long long), ctx->stream));
   const unsigned grid = stb_scan_grid(ctx, ranges.n_virtual, tier == STB_TIER_Q8 ? STB_Q8_SCAN_U : STB_SCAN_U);
   if (tier == STB_TIER_Q8) {
-    if (!c->q8) { stb_set_error("scan_collect: q8 tier unavailable"); return STB_ERR_STATE; }
+    if (!c->tier_usable(tier)) { stb_set_error("scan_collect: q8 tier unavailable"); return STB_ERR_STATE; }
     if (ranges.n > 0) stb_scan_collect_kernel<STB_Q8_SCAN_U, true, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a);
     else stb_scan_collect_kernel<STB_Q8_SCAN_U, false, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a);
   } else if (ranges.n > 0)
@@ -1871,9 +1871,9 @@ int stb_launch_scan_hist(stb_ctx *ctx, const stb_corpus *c, int tier, const floa
   STB_CUDA(cudaMemsetAsync(hist_dev, 0, STB_HIST_BINS * sizeof(unsigned int), ctx->stream));
   const unsigned grid = stb_scan_grid(ctx, ranges.n_virtual, tier == STB_TIER_Q8 ? STB_Q8_SCAN_U : STB_SCAN_U);
   if (tier == STB_TIER_Q8) {
-    if (!c->q8) { stb_set_error("scan_hist: q8 tier unavailable"); return STB_ERR_STATE; }
-    if (ranges.n > 0) stb_scan_hist_kernel<STB_Q8_SCAN_U, true, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, hist_dev, c->q8, c->q8_scale);
-    else stb_scan_hist_kernel<STB_Q8_SCAN_U, false, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, hist_dev, c->q8, c->q8_scale);
+    if (!c->tier_usable(tier)) { stb_set_error("scan_hist: q8 tier unavailable"); return STB_ERR_STATE; }
+    if (ranges.n > 0) stb_scan_hist_kernel<STB_Q8_SCAN_U, true, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, hist_dev, c->q8.codes, c->q8.scale);
+    else stb_scan_hist_kernel<STB_Q8_SCAN_U, false, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, hist_dev, c->q8.codes, c->q8.scale);
   } else if (ranges.n > 0)
     stb_scan_hist_kernel<STB_SCAN_U, true><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, hist_dev, nullptr, nullptr);
   else
@@ -1913,12 +1913,12 @@ int stb_launch_debug_scan(stb_ctx *ctx, const stb_corpus *c, int tier, const flo
   const bool r = ranges.n > 0;
   if (tier == STB_TIER_Q8) {
     const unsigned grid = stb_scan_grid(ctx, ranges.n_virtual, STB_Q8_SCAN_U);
-    if (r) stb_debug_scan_kernel<STB_Q8_SCAN_U, true, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, nullptr, c->q8, c->q8_scale, sink);
-    else stb_debug_scan_kernel<STB_Q8_SCAN_U, false, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, nullptr, c->q8, c->q8_scale, sink);
+    if (r) stb_debug_scan_kernel<STB_Q8_SCAN_U, true, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, nullptr, c->q8.codes, c->q8.scale, sink);
+    else stb_debug_scan_kernel<STB_Q8_SCAN_U, false, 2><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, nullptr, c->q8.codes, c->q8.scale, sink);
   } else if (tier == STB_TIER_H16) {
     const unsigned grid = stb_scan_grid(ctx, ranges.n_virtual, STB_SHADOW_SCAN_U);
-    if (r) stb_debug_scan_kernel<STB_SHADOW_SCAN_U, true, 1><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, c->shadow, nullptr, nullptr, sink);
-    else stb_debug_scan_kernel<STB_SHADOW_SCAN_U, false, 1><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, c->shadow, nullptr, nullptr, sink);
+    if (r) stb_debug_scan_kernel<STB_SHADOW_SCAN_U, true, 1><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, c->shadow.tiles, nullptr, nullptr, sink);
+    else stb_debug_scan_kernel<STB_SHADOW_SCAN_U, false, 1><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, c->shadow.tiles, nullptr, nullptr, sink);
   } else {
     const unsigned grid = stb_scan_grid(ctx, ranges.n_virtual, STB_SCAN_U);
     if (r) stb_debug_scan_kernel<STB_SCAN_U, true, 0><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, nullptr, nullptr, nullptr, sink);
@@ -1945,8 +1945,8 @@ int stb_launch_debug_q4(stb_ctx *ctx, const stb_corpus *c, const float *q_dev, u
                         float *u8, unsigned int *seen) {
   const ScanArgs a = stb_scan_args(c, q_dev, ranges);
   StbQ4Args q4a;
-  q4a.plane = c->q4;
-  q4a.sr = c->q4_sr;
+  q4a.plane = c->q8.plane;
+  q4a.sr = c->q8.sr;
   q4a.thr = words;
   q4a.tag = 1u;
   q4a.top_k = top_k;
@@ -1954,8 +1954,8 @@ int stb_launch_debug_q4(stb_ctx *ctx, const stb_corpus *c, const float *q_dev, u
   const DumpSink sink{u8, seen};
   const StbQ4Dump dump{u4, t, l8, pin};
   const unsigned grid = stb_scan_grid(ctx, ranges.n_virtual, STB_Q4_SCAN_U);
-  if (ranges.n > 0) stb_debug_q4_kernel<true><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, c->q8, c->q8_scale, q4a, sink, dump);
-  else stb_debug_q4_kernel<false><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, c->q8, c->q8_scale, q4a, sink, dump);
+  if (ranges.n > 0) stb_debug_q4_kernel<true><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, c->q8.codes, c->q8.scale, q4a, sink, dump);
+  else stb_debug_q4_kernel<false><<<grid, STB_SCAN_THREADS, 0, ctx->stream>>>(a, c->q8.codes, c->q8.scale, q4a, sink, dump);
   STB_CUDA(cudaGetLastError());
   ctx->kernel_launches++;
   return STB_OK;
