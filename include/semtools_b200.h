@@ -254,9 +254,26 @@ int stb_embed_status(stb_ctx *ctx);
  * context scratch that grows on demand.
  *
  * stb_debug_tokenize returns the CSR stb_embed_text would pool (ids_offsets[n_lines + 1] always; ids while
- * they fit ids_cap, else STB_ERR_CAPACITY) and, if taken is not NULL, the rule's verdict. */
+ * they fit ids_cap, else STB_ERR_CAPACITY) and, if taken is not NULL, the rule's verdict.
+ *
+ * stb_tokenizer_load_ex(..., STB_TOKENIZER_UTF8, ...) loads a handle whose GPU rule is UTF-8 text (flags = 0 is
+ * stb_tokenizer_load).  For the same GPU shape, plus the Precompiled charsmaps, the grapheme-break properties and
+ * the lowercase map resident in HBM, stb_tokenizer_gpu_lines takes a line iff it
+ *   - is valid UTF-8 (shortest form, no surrogates, nothing above U+10FFFF) -- control characters, NUL, tab, the
+ *     Metaspace replacement and every script are allowed,
+ *   - contains no added token's content, neither as given nor (for normalized = true tokens) after normalisation.
+ * The kernels normalise such a line by the tokenizer's steps in order (Precompiled grapheme cluster by cluster,
+ * UAX #29), split it on spaces and on the replacement character, and run the Viterbi.  A line they cannot finish
+ * exactly is given back to the host tokenizer inside the same call: its normalised text outgrows twice its bytes
+ * plus the Prepend bytes, a Metaspace piece exceeds STB_TOKENIZER_PIECE_CAP, or -- under prepend_scheme "first" --
+ * the normaliser removed the line's leading characters (HF decides "first" by the original offset).  For such a
+ * handle stb_debug_tokenize's taken[i] = 1 means line i's ids came from the GPU (a subset of the rule's lines).
+ * Every line gets exactly the ids a flags-0 handle of the same tokenizer.json gives it, so rows, errors and
+ * "a failed call appends nothing" are the same; only where the work runs differs. */
 #define STB_TOKENIZER_PIECE_CAP 256u
+#define STB_TOKENIZER_UTF8 1u
 int stb_tokenizer_load(stb_ctx *ctx, const uint8_t *json, uint64_t len, stb_tokenizer **out);
+int stb_tokenizer_load_ex(stb_ctx *ctx, const uint8_t *json, uint64_t len, uint32_t flags, stb_tokenizer **out);
 int stb_tokenizer_destroy(stb_tokenizer *tok);
 int stb_tokenizer_gpu_lines(const stb_tokenizer *tok, const uint8_t *text, const uint64_t *text_offsets,
                             uint64_t n_lines, uint8_t *taken);

@@ -35,9 +35,10 @@ SYMBOLS = [
     "stb_debug_ivfpq_export",
     "stb_ivfpq_search_batch", "stb_ivfpq_search_batch_dev", "stb_debug_ivfpq_batch_last",
     "stb_ivfpq_search_filtered", "stb_ivfpq_search_subsets", "stb_ivfpq_update", "stb_ivfpq_remove",
-    "stb_tokenizer_load", "stb_tokenizer_destroy", "stb_tokenizer_gpu_lines", "stb_embed_text", "stb_debug_tokenize",
+    "stb_tokenizer_load", "stb_tokenizer_load_ex", "stb_tokenizer_destroy", "stb_tokenizer_gpu_lines", "stb_embed_text", "stb_debug_tokenize",
 ]
 STB_TOKENIZER_PIECE_CAP = 256
+STB_TOKENIZER_UTF8 = 1
 
 
 class StbHit(C.Structure):
@@ -151,6 +152,7 @@ def lib() -> C.CDLL:
     L.stb_ivfpq_search_filtered.argtypes = [vp, vp, u32, u32, u32, u32, i32, f64, vp, u32, vp, vp, vp]
     L.stb_ivfpq_search_subsets.argtypes = [vp, vp, u32, u32, u32, u32, i32, f64, u32, vp, vp, vp, vp, vp, vp]
     L.stb_tokenizer_load.argtypes = [vp, vp, u64, C.POINTER(vp)]
+    L.stb_tokenizer_load_ex.argtypes = [vp, vp, u64, u32, C.POINTER(vp)]
     L.stb_tokenizer_destroy.argtypes = [vp]
     L.stb_tokenizer_gpu_lines.argtypes = [vp, vp, vp, u64, vp]
     L.stb_embed_text.argtypes = [vp, vp, vp, vp, vp, u64, u32, vp, vp]
@@ -340,13 +342,15 @@ class Table:
 
 
 class Tokenizer:
-    """stb_tokenizer: a tokenizer.json loaded into the library (Unigram model resident in HBM)."""
+    """stb_tokenizer: a tokenizer.json loaded into the library (Unigram model resident in HBM).  utf8=True loads
+    it with STB_TOKENIZER_UTF8: the GPU takes valid UTF-8 lines, not only printable ASCII ones (same ids)."""
 
-    def __init__(self, ctx: Context, json_bytes: bytes):
+    def __init__(self, ctx: Context, json_bytes: bytes, utf8: bool = False):
         self.ctx = ctx
         self._h = vp()
         buf = np.frombuffer(json_bytes, dtype=np.uint8)
-        _check(lib().stb_tokenizer_load(ctx._h, _np_ptr(buf), buf.size, C.byref(self._h)))
+        flags = STB_TOKENIZER_UTF8 if utf8 else 0
+        _check(lib().stb_tokenizer_load_ex(ctx._h, _np_ptr(buf), buf.size, flags, C.byref(self._h)))
 
     def close(self):
         if getattr(self, "_h", None) is not None and self._h and _lib is not None:

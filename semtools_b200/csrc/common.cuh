@@ -274,6 +274,9 @@ struct stb_ctx {
   StbBuf<uint64_t> tok_off, tok_hoff;
   StbBuf<uint32_t> tok_hids, tok_nlen, tok_tmp, tok_cnt;
   StbBuf<int> tok_flag;            // device int: a piece past the cap (never set when the rule holds)
+  // UTF-8 handles: the second normalisation buffer, the regions' offsets, each candidate line's give-back status
+  StbBuf<uint8_t> tok_norm2, tok_status;
+  StbBuf<uint64_t> tok_roff;
   // in-place corpus mutations (stb_corpus_update / _remove): row staging (<= STB_MUT_CHUNK_ROWS rows),
   // row ids or kept-segment table, and the q8 / shadow bad-row flags
   StbBuf<float> mut_stage;
@@ -592,9 +595,10 @@ int stb_text_host(const stb_tokenizer *tok, const uint8_t *text, const uint64_t 
 // Grows the tokenizer scratch and K3's CSR staging to the largest chunk of the call, before its first chunk.
 int stb_tok_reserve(stb_ctx *ctx, const stb_tokenizer *tok, const StbTextHost &h, const uint64_t *offsets, uint32_t max_length);
 // Tokenises lines [l0, l0 + m) (one chunk) into the K3 CSR ctx->embed_off_dev[m + 1] / ctx->embed_ids_dev, on the
-// stream; the pieces-past-the-cap flag goes to ctx->tok_flag (zeroed by the caller).
+// stream; the pieces-past-the-cap flag goes to ctx->tok_flag (zeroed by the caller).  A UTF-8 handle synchronises
+// the stream once per chunk (its give-back) and clears h.taken for the lines it gave back.
 const stb_ctx *stb_tokenizer_ctx(const stb_tokenizer *tok);
-int stb_tok_chunk(stb_ctx *ctx, const stb_tokenizer *tok, const StbTextHost &h, const uint8_t *text,
+int stb_tok_chunk(stb_ctx *ctx, const stb_tokenizer *tok, StbTextHost &h, const uint8_t *text,
                   const uint64_t *offsets, uint64_t l0, uint64_t m, uint32_t max_length);
 
 // ---- batch_scan.cu (K2) ------------------------------------------------------------------

@@ -94,6 +94,15 @@ std::string to_lowercase(const std::string &s) { return to_lowercase_impl(s, tru
 // mapping WITHOUT the context-sensitive Final_Sigma rule of str::to_lowercase
 std::string to_lowercase_per_char(const std::string &s) { return to_lowercase_impl(s, false); }
 
+const std::vector<LowerEntry> &lower_table() {
+  static const std::vector<LowerEntry> t = [] {
+    std::vector<LowerEntry> v;
+    for (const LowerMap &m : kLower) v.push_back({m.cp, m.n, {m.to[0], m.to[1], m.to[2]}});
+    return v;
+  }();
+  return t;
+}
+
 static std::string to_lowercase_impl(const std::string &s, bool final_sigma) {
   std::vector<uint32_t> cps;
   cps.reserve(s.size());
@@ -294,9 +303,9 @@ void Searcher::load_table(const float *E, uint64_t V, bool normalize, const floa
                        normalize ? 1 : 0, &table_));
 }
 
-bool Searcher::load_text_tokenizer(const std::string &json) {
+bool Searcher::load_text_tokenizer(const std::string &json, uint32_t flags) {
   if (text_tok_) { stb_tokenizer_destroy(text_tok_); text_tok_ = nullptr; }
-  const int rc = stb_tokenizer_load(ctx_, reinterpret_cast<const uint8_t *>(json.data()), json.size(), &text_tok_);
+  const int rc = stb_tokenizer_load_ex(ctx_, reinterpret_cast<const uint8_t *>(json.data()), json.size(), flags, &text_tok_);
   if (rc == STB_ERR_ARG) { text_tok_ = nullptr; return false; }
   check(rc);
   return true;

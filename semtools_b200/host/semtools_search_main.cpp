@@ -118,6 +118,7 @@ static int selftest() {
 
 static int real_main(int argc, char **argv) {
   std::string vocab, tokenizer_json, table, model_dir, query;
+  uint32_t tok_flags = 0;                        // --gpu-tokenizer utf8: STB_TOKENIZER_UTF8
   std::vector<std::string> files;
   SearchConfig cfg;
   bool json = false, have_query = false;
@@ -214,6 +215,11 @@ static int real_main(int argc, char **argv) {
     else if (a == "--tokenizer") tokenizer_json = next();
     else if (a == "--table") table = next();
     else if (a == "--model") model_dir = next();
+    else if (a == "--gpu-tokenizer") {
+      const std::string g = next();
+      if (g != "ascii" && g != "utf8") { fprintf(stderr, "Error: --gpu-tokenizer takes ascii or utf8\n"); return 2; }
+      tok_flags = g == "utf8" ? STB_TOKENIZER_UTF8 : 0;
+    }
     else if (a == "-n" || a == "--n-lines" || a == "--context") cfg.n_lines = std::stoul(next());
     else if (a == "--top-k") cfg.top_k = std::stoul(next());
     else if (a == "-m" || a == "--max-distance" || a == "--threshold") cfg.max_distance = std::stod(next());
@@ -229,10 +235,13 @@ static int real_main(int argc, char **argv) {
   else if (!model_dir.empty()) { fprintf(stderr, "Error: --model replaces --tokenizer / --vocab / --table\n"); return 2; }
   if (!have_query || (vocab.empty() == tokenizer_json.empty()) || (table.empty() && model_dir.empty())) {
     fprintf(stderr, "usage: semtools_b200_search (--model DIR | (--tokenizer tokenizer.json | --vocab V) --table T) QUERY [FILES...] [-n N] [--top-k K] [-m D] [-i] [-j] [-w WORKSPACE]\n"
+                    "       [--gpu-tokenizer ascii|utf8]\n"
                     "  --model:     a local model2vec directory (tokenizer.json, model.safetensors, config.json), as StaticModel::from_pretrained reads it\n"
                     "               (default: $SEMTOOLS_B200_MODEL_DIR, like the Python CLI)\n"
                     "  --tokenizer: the model's HF tokenizer.json (Unigram + Metaspace subset, see semtools_tokenizer.hpp)\n"
-                    "  --vocab:     whitespace WordLevel vocabulary, one token per line (synthetic models)\n");
+                    "  --vocab:     whitespace WordLevel vocabulary, one token per line (synthetic models)\n"
+                    "  --gpu-tokenizer: which lines the GPU tokenises -- ascii (printable ASCII lines, the default) or utf8\n"
+                    "               (every valid UTF-8 line); the other lines are tokenised on the host, with the same ids\n");
     return 2;
   }
   try {
@@ -271,7 +280,7 @@ static int real_main(int argc, char **argv) {
     }
     auto load = [&](Searcher &s) {
       s.load_table(tab_E, tab_V, tab_norm, md.weights.data(), md.weights.size(), md.mapping.data(), md.mapping.size());
-      if (!tok_text.empty()) s.load_text_tokenizer(tok_text);
+      if (!tok_text.empty()) s.load_text_tokenizer(tok_text, tok_flags);
     };
     // identity of this host's embedder, recorded in the store so its vectors are never mixed with another
     // host's / model's (ADVICE r1): a model directory gets the Python host's fingerprint string, the

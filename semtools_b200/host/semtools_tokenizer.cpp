@@ -51,7 +51,7 @@ bool is_space_at(const std::string &s, size_t i, size_t *len) {
 }
 
 // ---- extended grapheme clusters (UAX #29) -------------------------------------------------------
-struct GbRange { uint32_t a, b; uint8_t v; };
+using GbRange = HfTokenizer::PropRange;
 #include "grapheme_break.inc"
 enum { GB_OTHER = 0, GB_CR, GB_LF, GB_CONTROL, GB_EXTEND, GB_ZWJ, GB_RI, GB_PREPEND, GB_SPACINGMARK, GB_L, GB_V, GB_T, GB_LV, GB_LVT };
 enum { INCB_NONE = 0, INCB_CONSONANT, INCB_EXTEND, INCB_LINKER };
@@ -71,14 +71,15 @@ inline uint8_t gcb_of(uint32_t cp) {
 inline uint8_t gb_props_slow(uint32_t cp) {
   return (uint8_t)(gcb_of(cp) | (gb_lookup(kExtPictRanges, cp) ? 0x10 : 0) | (gb_lookup(kInCbRanges, cp) << 5));
 }
-inline uint8_t gb_props(uint32_t cp) {
+const std::vector<uint8_t> &gb_bmp() {
   static const std::vector<uint8_t> bmp = [] {
     std::vector<uint8_t> t(0x10000);
     for (uint32_t c = 0; c < 0x10000; ++c) t[c] = gb_props_slow(c);
     return t;
   }();
-  return cp < 0x10000 ? bmp[cp] : gb_props_slow(cp);
+  return bmp;
 }
+inline uint8_t gb_props(uint32_t cp) { return cp < 0x10000 ? gb_bmp()[cp] : gb_props_slow(cp); }
 // one scalar value at s[i]; malformed sequences yield the single byte as an (unassigned-looking) code point
 inline uint32_t decode_at(const std::string &s, size_t i, size_t *len) {
   const unsigned char c = (unsigned char)s[i];
@@ -419,6 +420,29 @@ HfTokenizer::AsciiPlan HfTokenizer::ascii_plan() const {
   p.added_normalized = !added_norm_.empty();
   p.ok = true;
   return p;
+}
+
+HfTokenizer::Utf8View HfTokenizer::utf8_view() const {
+  Utf8View v;
+  for (const auto &st : norm_) {
+    switch (st.kind) {
+      case N_LOWER: v.ops.push_back({OP_LOWER, true, true, ""}); break;
+      case N_REPLACE_MULTISPACE: v.ops.push_back({OP_MULTISPACE, true, true, ""}); break;
+      case N_STRIP: v.ops.push_back({OP_STRIP, st.left, st.right, ""}); break;
+      case N_PREPEND: v.ops.push_back({OP_PREPEND, true, true, st.a}); break;
+      case N_PRECOMPILED:
+        if (!maps_[st.map].trie.empty()) v.ops.push_back({OP_PRECOMPILED, true, true, "", st.map});   // else the identity
+        break;
+      default: break;                                        // not a shape ascii_plan() accepts
+    }
+  }
+  for (const auto &m : maps_) v.maps.push_back({m.trie.data(), m.trie.size(), m.normalized.data(), m.normalized.size(), m.ascii_plain});
+  v.gb_bmp = gb_bmp().data();
+  v.gcb = kGcbRanges; v.n_gcb = sizeof(kGcbRanges) / sizeof(kGcbRanges[0]);
+  v.ext_pict = kExtPictRanges; v.n_ext_pict = sizeof(kExtPictRanges) / sizeof(kExtPictRanges[0]);
+  v.incb = kInCbRanges; v.n_incb = sizeof(kInCbRanges) / sizeof(kInCbRanges[0]);
+  v.lower = lower_table().data(); v.n_lower = lower_table().size();
+  return v;
 }
 
 HfTokenizer::TrieView HfTokenizer::trie() const {

@@ -76,6 +76,25 @@ class HfTokenizer : public Tokenizer {
     bool decline_leading_space = false;
   };
   AsciiPlan ascii_plan() const;
+  // What the UTF-8 GPU tokenizer (STB_TOKENIZER_UTF8) restates, for a shape ascii_plan() accepts: the normaliser
+  // steps in order, Precompiled included (kind OP_PRECOMPILED, charsmap maps[map]), and the host tables those steps
+  // read -- the charsmaps' darts-clone units and replacement blobs, the grapheme-break properties (BMP as one byte
+  // per code point: gcb | ext_pict << 4 | incb << 5; supplementary planes through the three range tables) and the
+  // per-character lowercase map.  Pointers stay valid for the tokenizer's lifetime.
+  enum { OP_PRECOMPILED = OP_PREPEND + 1 };
+  struct Utf8Op { int kind; bool left = true, right = true; std::string text; int map = -1; };
+  struct CharsmapView { const uint32_t *trie; size_t n_trie; const char *normalized; size_t n_normalized; const bool *ascii_plain; };
+  struct PropRange { uint32_t a, b; uint8_t v; };
+  struct Utf8View {
+    std::vector<Utf8Op> ops;
+    std::vector<CharsmapView> maps;
+    const uint8_t *gb_bmp;                                   // 0x10000 bytes
+    const PropRange *gcb, *ext_pict, *incb;
+    size_t n_gcb, n_ext_pict, n_incb;
+    const LowerEntry *lower;
+    size_t n_lower;
+  };
+  Utf8View utf8_view() const;
   // The Unigram model as unigram() reads it: root_[256], first_child_[n_nodes + 1], child_byte_ / child_node_
   // [n_edges], terminal_[n_nodes], scores_[vocab]
   struct TrieView {

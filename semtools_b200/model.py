@@ -33,11 +33,17 @@ class StaticModel:
         self._table = None
         self._tokenizer_json = None                              # tokenizer.json bytes (from_pretrained)
         self._text_tok = None
+        self.gpu_tokenizer = "ascii"                             # the GPU rule of text_tokenizer(): "ascii" | "utf8"
 
     # -- StaticModel::from_pretrained(path, token, normalize, subfolder) -----------------------
     @classmethod
     def from_pretrained(cls, repo_or_path: str, token=None, normalize=None, subfolder=None,
-                        ctx: capi.Context | None = None) -> "StaticModel":
+                        ctx: capi.Context | None = None, gpu_tokenizer: str = "ascii") -> "StaticModel":
+        """gpu_tokenizer: which lines the library's tokenizer takes on the GPU -- "ascii" (printable ASCII lines)
+        or "utf8" (every valid UTF-8 line; lines the kernels cannot finish exactly go back to the host inside
+        the call).  Both give the same ids."""
+        if gpu_tokenizer not in ("ascii", "utf8"):
+            raise ValueError(f"gpu_tokenizer must be 'ascii' or 'utf8', got {gpu_tokenizer!r}")
         from safetensors import safe_open
         from tokenizers import Tokenizer
         base = os.path.join(repo_or_path, subfolder) if subfolder else repo_or_path
@@ -71,6 +77,7 @@ class StaticModel:
         if emb.ndim != 2 or emb.shape[1] != capi.STB_DIM:
             raise ValueError(f"embedding table must be V x {capi.STB_DIM}, got {emb.shape}")
         m = cls(tokenizer, emb, weights, mapping, normalize, median, unk_id, ctx)
+        m.gpu_tokenizer = gpu_tokenizer
         with open(tok_path, "rb") as f:
             m._tokenizer_json = f.read()
         m._tokenizer_file_hash = capi.fnv1a64(m._tokenizer_json)     # the C++ host hashes the same bytes (load_model_dir)
@@ -131,7 +138,7 @@ class StaticModel:
         if self._text_tok is None and self._tokenizer_json is not None:
             self.table()
             try:
-                self._text_tok = capi.Tokenizer(self.ctx, self._tokenizer_json)
+                self._text_tok = capi.Tokenizer(self.ctx, self._tokenizer_json, utf8=self.gpu_tokenizer == "utf8")
             except capi.StbError as e:
                 if e.status != capi.STB_ERR_ARG:
                     raise
