@@ -682,6 +682,47 @@ int stb_ivfpq_search_subsets(stb_ivfpq *index, const float *q, uint32_t nq, uint
                              uint32_t rerank, int has_max, double max_distance,
                              uint32_t n_subsets, const uint64_t *subset_offsets, const uint64_t *row_ranges,
                              const uint32_t *subset_of, stb_hit *out_hits, uint32_t *out_n, uint64_t *out_scanned);
+/* Threshold mode of search_documents (src/search/mod.rs:88-89,115-119) on the index, for a batch: every row of
+ * the query's probed lists (and every forced row) under max_distance, with no top_k cap.
+ *  - Probe: for query i the coarse scores, probe list and LUT are bit for bit stb_ivfpq_search_batch's; nprobe is
+ *    clamped to [1, min(nlist, 1024)].  stb_debug_ivfpq_batch_last describes the call's last launch, with
+ *    info = {nq, nprobe, 0, 0}.
+ *  - Cutoff: t = RD_f32((1 - max_distance) - slack), computed in f64 and rounded toward -inf.
+ *  - Candidates: when t = -inf (max_distance or slack +inf), every code of the probed lists; otherwise every such
+ *    code whose ADC score s (stb_ivfpq_search_batch's fp32 sum, in the same order) satisfies s >= t, so a NaN
+ *    score is none.  Plus every forced row.
+ *  - Hits: the candidate rows whose canonical distance (as on every K5 path) is < max_distance (strict), GLOBAL
+ *    rows, each query's ordered by (distance, row).
+ *  - Output as stb_search_batch_threshold's: out_offsets has nq + 1 entries, out_offsets[0] = 0, the hits of all
+ *    queries concatenated in query order; if out_offsets[nq] > cap the first cap hits are written, every offset
+ *    is still written and the call returns STB_ERR_CAPACITY.  out_hits may be NULL only when cap == 0.
+ *  - Counts (either pointer may be NULL): out_scanned[i] = codes in the probed lists, as stb_ivfpq_search_batch
+ *    reports them; out_reranked[i] = candidate codes plus forced rows, the rows whose f32 row was read.
+ *  - Arguments: nq == 0 is a no-op; a NULL index, q or out_offsets is STB_ERR_ARG, as is a NaN or negative slack.
+ *    A max_distance that is NaN or <= 0 sets every offset and count to 0 and launches nothing.
+ *  - Launches: queries in chunks of at most 4096 (probe stage, one pass that counts each query's candidates per
+ *    block of 16384 probed codes, one synchronisation), then launches of at most STB_IVFPQ_THRESHOLD_KEYS
+ *    candidate keys (or one block, if a block alone holds more) that emit the keys and finish them as
+ *    stb_search_batch_threshold does (sort by row, canonical re-score, stable sort by distance).  A query with
+ *    more candidates than a launch holds is split at block boundaries and its pieces merged into (distance, row)
+ *    order, so a query's answer depends neither on the other queries, nor on the chunking, nor on the budget.
+ *    Scratch belongs to the index and grows on demand (the keys of a launch: 32 B each, plus the sorts').
+ * What follows:
+ *  - every returned hit is a threshold hit of stb_search for that query, with the same distance bits: only the
+ *    recall is approximate;
+ *  - with nprobe >= nlist (so nlist <= 1024) and slack = +inf every indexed row is re-scored, so the hits are
+ *    the canonical threshold answer over the indexed rows, forced rows included; for a query with finite
+ *    components (zero and huge ones included) they equal, bit for bit, those of
+ *      stb_search(ctx, corpus, q_i, 0, 1, max_distance, STB_MODE_SEARCH_DOCUMENTS, NULL, 0, ...)
+ *    and of stb_search_batch_threshold (for a query with a NaN or infinite component every canonical distance
+ *    is 0, and every indexed row is a hit);
+ *  - the hit set is monotone: raising nprobe (the probe list is a prefix of the coarse order) or slack never
+ *    removes a hit. */
+#define STB_IVFPQ_THRESHOLD_KEYS (1ull << 24)   /* candidate keys one launch holds (128 MiB) */
+int stb_ivfpq_search_threshold(stb_ivfpq *index, const float *q, uint32_t nq, uint32_t nprobe,
+                               double max_distance, double slack,
+                               stb_hit *out_hits, uint64_t cap, uint64_t *out_offsets,
+                               uint64_t *out_scanned, uint64_t *out_reranked);
 
 /* Host-buffer form of the fused multi-GPU search (the call a sharded host makes per query):
  * pinned H2D of the query, ONE kernel (scan + NVLink exchange + merge), D2H of the merged
@@ -821,6 +862,9 @@ int stb_debug_ivfpq_export(const stb_ivfpq *index, float *centroids, float *code
  * i >= nq. */
 int stb_debug_ivfpq_batch_last(const stb_ivfpq *index, uint32_t i, uint32_t info[4], float *coarse,
                                uint32_t *probe, float *lut);
+/* Test hook for K5's threshold search: candidate keys per launch for this index (0 = STB_IVFPQ_THRESHOLD_KEYS;
+ * more than that is STB_ERR_ARG).  Lowering it splits queries between launches without changing any answer. */
+int stb_debug_ivfpq_threshold_keys(stb_ivfpq *index, uint64_t keys);
 /* Test hook for K2: describes the most recent stb_search_batch_dev, stb_search_batch_filtered,
  * stb_search_batch_subsets or stb_search_batch_threshold on ctx (synchronises the stream).  info = {route, nq, a,
  * b, n_seg, seg_cap}; route 1 = v1, 2 = v2, 3 = filtered v2, 4 = a filtered call that launched nothing on the

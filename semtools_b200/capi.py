@@ -35,6 +35,7 @@ SYMBOLS = [
     "stb_debug_ivfpq_export",
     "stb_ivfpq_search_batch", "stb_ivfpq_search_batch_dev", "stb_debug_ivfpq_batch_last",
     "stb_ivfpq_search_filtered", "stb_ivfpq_search_subsets", "stb_ivfpq_update", "stb_ivfpq_remove",
+    "stb_ivfpq_search_threshold", "stb_debug_ivfpq_threshold_keys",
     "stb_tokenizer_load", "stb_tokenizer_load_ex", "stb_tokenizer_destroy", "stb_tokenizer_gpu_lines", "stb_embed_text", "stb_debug_tokenize",
 ]
 STB_TOKENIZER_PIECE_CAP = 256
@@ -151,6 +152,8 @@ def lib() -> C.CDLL:
     L.stb_debug_ivfpq_batch_last.argtypes = [vp, u32, vp, vp, vp, vp]
     L.stb_ivfpq_search_filtered.argtypes = [vp, vp, u32, u32, u32, u32, i32, f64, vp, u32, vp, vp, vp]
     L.stb_ivfpq_search_subsets.argtypes = [vp, vp, u32, u32, u32, u32, i32, f64, u32, vp, vp, vp, vp, vp, vp]
+    L.stb_ivfpq_search_threshold.argtypes = [vp, vp, u32, u32, f64, f64, vp, u64, vp, vp, vp]
+    L.stb_debug_ivfpq_threshold_keys.argtypes = [vp, u64]
     L.stb_tokenizer_load.argtypes = [vp, vp, u64, C.POINTER(vp)]
     L.stb_tokenizer_load_ex.argtypes = [vp, vp, u64, u32, C.POINTER(vp)]
     L.stb_tokenizer_destroy.argtypes = [vp]
@@ -824,6 +827,33 @@ class IvfPq:
                                               _np_ptr(offsets), _np_ptr(rr) if rr.size else None, _np_ptr(subset_of),
                                               _np_ptr(out) if out.size else None, _np_ptr(n), _np_ptr(scanned)))
         return out, n, scanned
+
+    def search_threshold(self, queries, nprobe: int = 64, max_distance: float = 0.5, slack: float = 0.0,
+                         cap: int | None = None):
+        """stb_ivfpq_search_threshold: for each query, every row of its probed lists (and every forced row) with
+        distance < max_distance whose ADC score reaches RD_f32((1 - max_distance) - slack).  Starts from a modest
+        capacity and retries once with the reported total.  Returns (list of HIT_DTYPE arrays, one per query,
+        scanned [nq] codes in the probed lists, reranked [nq] rows re-scored)."""
+        queries = np.ascontiguousarray(queries, dtype=np.float32).reshape(-1, STB_DIM)
+        nq = queries.shape[0]
+        if cap is None:
+            cap = max(nq, 1) * 64
+        offsets = np.zeros(nq + 1, dtype=np.uint64)
+        scanned = np.zeros(nq, dtype=np.uint64)
+        reranked = np.zeros(nq, dtype=np.uint64)
+        while True:
+            out = np.zeros(max(cap, 1), dtype=HIT_DTYPE)
+            rc = _check(lib().stb_ivfpq_search_threshold(self._h, _np_ptr(queries), nq, nprobe, float(max_distance),
+                                                         float(slack), _np_ptr(out), cap, _np_ptr(offsets),
+                                                         _np_ptr(scanned), _np_ptr(reranked)), allow_capacity=True)
+            if rc == STB_ERR_CAPACITY:
+                cap = int(offsets[nq])
+                continue
+            return [out[int(offsets[i]): int(offsets[i + 1])] for i in range(nq)], scanned, reranked
+
+    def set_threshold_keys(self, keys: int):
+        """stb_debug_ivfpq_threshold_keys: candidate keys per launch of search_threshold (0 = the default)."""
+        _check(lib().stb_debug_ivfpq_threshold_keys(self._h, keys))
 
     def search_batch_dev(self, q_dev: int, nq: int, nprobe: int, top_k: int, rerank: int, out_hits_dev: int,
                          out_status_dev: int):

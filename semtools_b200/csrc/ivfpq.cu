@@ -25,7 +25,9 @@
 #include <math_constants.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cub/device/device_radix_sort.cuh>
+#include <functional>
 #include <vector>
 
 #include "common.cuh"
@@ -93,6 +95,16 @@ struct stb_ivfpq {
   // subsets search (f_bitmap and f_elig then hold one bitmap and one count array per subset of a launch)
   StbBuf<uint64_t> f_set_off;        // [2 per subset of a launch]: its pairs [begin, end) in f_ranges
   StbBuf<uint32_t> f_slot_set;       // [query slot]: its subset within the launch
+  // threshold search scratch (see "threshold search"), grown on demand
+  uint64_t t_budget = 0;             // candidate keys per launch (0: STB_IVFPQ_THRESHOLD_KEYS)
+  StbBuf<uint32_t> t_cnt;            // [nq][blocks] candidates per block, then [nq] probed codes
+  StbBuf<uint4> t_items;             // the emit launch's CTAs: {query, block or IVF_NO_LIST, key offset, 0}
+  StbBuf<int> t_off;                 // [slots + 1] key segments
+  StbBuf<uint32_t> t_slot;           // [slots] query of each slot, then [slots] its hits
+  StbBuf<uint64_t> t_buf;            // 4 x keys: the finish's sort buffers
+  StbBuf<uint64_t> t_at;             // [slots] where each slot's hits go in t_hits
+  StbBuf<stb_hit> t_hits;
+  StbBuf<uint8_t> t_sort;
 };
 
 // ------------------------------------------------------------------ assignment GEMM ---
@@ -1184,6 +1196,94 @@ __global__ void ivff_elig_kernel(const uint32_t *list_off, const uint32_t *order
   if (lane == 0) elig[l] = cnt;
 }
 
+// ------------------------------------------------------------------ threshold search -----
+// stb_ivfpq_search_threshold: every probed code whose ADC score reaches a cutoff t, and the forced rows, re-scored
+// exactly.  After the batched probe stage (ivfb_probe), a query's probed codes v = 0 .. total-1 (probe order, as
+// ivfb_code_key numbers them) are cut into blocks of IVFT_BLOCK; one CTA scans one block.
+//   ivft_scan_kernel<false>  grid (blocks, nq): candidates per (query, block) and each query's probed codes.
+//   ivft_scan_kernel<true>   one CTA per item of a launch the host planned from those counts: a block's candidates,
+//                            or a query's forced rows, written as keys (local row in the low 32 bits) from the
+//                            item's offset, each exactly sized segment of a query's items one after the other.
+// Then K2 threshold's finish (batch_threshold.cu): sort by row, canonical re-score with the limit, stable sort by
+// distance, write.  A code is a candidate iff t = -inf (every probed code: its score is not even computed) or its
+// ADC score s >= t, so a NaN score is one only at t = -inf.
+#define IVFT_BLOCK 16384           // probed codes per CTA of the scan; the host splits a query at these
+#define IVFT_THREADS 256
+
+struct IvftArgs {
+  uint32_t nprobe, blocks;                   // blocks: the count grid's x
+  const uint32_t *list_off; const uint8_t *codes; const uint32_t *order;
+  const float *coarse; uint32_t nlist; const uint32_t *probe; const float *lut;
+  float t;
+  uint32_t *cnt, *total;                     // count: [nq][blocks] candidates, [nq] probed codes
+  const uint4 *items;                        // emit: {query, block or IVF_NO_LIST (the forced rows), key offset, 0}
+  const uint32_t *forced; uint32_t n_forced;
+  uint64_t *keys;
+};
+
+template <bool EMIT>
+__global__ void __launch_bounds__(IVFT_THREADS)
+ivft_scan_kernel(const IvftArgs a) {
+  __shared__ float s_lut[PQ_M * PQ_KSUB];      // 32 KiB
+  __shared__ uint32_t s_pref[1024], s_start[1024];
+  __shared__ float s_pc[1024];
+  __shared__ uint32_t s_n;
+  const uint32_t tid = threadIdx.x, lane = tid & 31;
+  uint32_t q = blockIdx.y, b = blockIdx.x, dst = 0;
+  if (EMIT) { const uint4 it = a.items[blockIdx.x]; q = it.x; b = it.y; dst = it.z; }
+  if (EMIT && b == IVF_NO_LIST) {
+    for (uint32_t i = tid; i < a.n_forced; i += IVFT_THREADS) a.keys[dst + i] = __ldg(a.forced + i);
+    return;
+  }
+  const uint32_t *pr = a.probe + (size_t)q * IVFB_PROBE_STRIDE(a.nprobe, false);
+  const uint32_t total = pr[2 * a.nprobe];
+  if (!EMIT && b == 0 && tid == 0) a.total[q] = total;
+  const uint64_t v0 = (uint64_t)b * IVFT_BLOCK;
+  const uint32_t v1 = (uint32_t)min((uint64_t)total, v0 + IVFT_BLOCK);
+  const bool all = a.t == -CUDART_INF_F;
+  if (!EMIT && (v0 >= total || all)) {
+    if (tid == 0) a.cnt[(size_t)q * a.blocks + b] = v0 < total ? v1 - (uint32_t)v0 : 0;
+    return;
+  }
+  if (!all)
+    for (uint32_t i = tid; i < PQ_M * PQ_KSUB; i += IVFT_THREADS) s_lut[i] = a.lut[(size_t)q * PQ_M * PQ_KSUB + i];
+  for (uint32_t p = tid; p < a.nprobe; p += IVFT_THREADS) {
+    const uint32_t l = pr[p];
+    s_pref[p] = pr[a.nprobe + p]; s_start[p] = __ldg(a.list_off + l); s_pc[p] = a.coarse[(size_t)q * a.nlist + l];
+  }
+  if (tid == 0) s_n = 0;
+  __syncthreads();
+  // whole warps step through the block, so each warp reserves its candidates' slots with one atomic
+  for (uint32_t w0 = (uint32_t)v0 + (tid & ~31u); w0 < v1; w0 += IVFT_THREADS) {
+    const uint32_t v = w0 + lane;
+    bool cand = false;
+    uint32_t pos = 0;
+    if (all) {
+      cand = v < v1;
+      if (EMIT && cand) {
+        uint32_t lo = 0, hi = a.nprobe;      // probe p with pref[p] <= v < pref[p+1], as ivfb_code_key finds it
+        while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (s_pref[mid] <= v) lo = mid; else hi = mid; }
+        pos = s_start[lo] + (v - s_pref[lo]);
+      }
+    } else if (v < v1) {
+      const uint64_t key = ivfb_code_key<false>(v, total, a.nprobe, s_pref, s_start, s_pc, s_lut, a.codes, a.order, nullptr);
+      cand = key != STB_KEY_INVALID && stb_key_score(key) >= a.t;
+      pos = stb_key_row(key);
+    }
+    const unsigned bal = __ballot_sync(0xffffffffu, cand);
+    uint32_t base = 0;
+    if (lane == 0 && bal) base = atomicAdd(&s_n, (uint32_t)__popc(bal));
+    if (EMIT) {
+      base = __shfl_sync(0xffffffffu, base, 0);
+      if (cand) a.keys[dst + base + __popc(bal & ((1u << lane) - 1u))] = __ldg(a.order + pos);
+    }
+  }
+  if (!EMIT) {
+    __syncthreads();
+    if (tid == 0) a.cnt[(size_t)q * a.blocks + b] = s_n;
+  }
+}
+
 // ------------------------------------------------------------------ host side ---------
 #define IVF_TRY(call)                      \
   do {                                     \
@@ -1825,15 +1925,150 @@ struct IvfbSubsets {
       : filter(true), max_dist(has_max ? std::min(max_distance, STB_DEFAULT_MAX_DIST) : STB_DEFAULT_MAX_DIST) {}
 };
 
+// A threshold search (stb_ivfpq_search_threshold) through the host loop: its cutoff, limit and outputs, and `at`,
+// the hits placed so far (the offset of the next query).
+struct IvftCall {
+  float t;
+  double max_dist;
+  uint64_t budget;
+  stb_hit *out_hits;
+  uint64_t cap, at = 0;
+  uint64_t *out_offsets, *out_scanned, *out_reranked;
+};
+
+// Queries i0 .. i0+m-1 of a threshold search, uploaded to b_q: the probe stage, the count pass, one synchronisation,
+// then launches planned from the counts.  Each query's units -- its forced rows, then each block with a candidate --
+// go to launches in order; a launch takes units while its keys stay within the budget (at least one unit), so a
+// query whose units do not fit is split between launches at block boundaries.  A slot is one query's units within
+// one launch: one key segment of the finish.  A split query's pieces are merged on the host into (distance, row)
+// order; the others' hits go to the output as the finish wrote them.
+static int ivft_chunk(stb_ivfpq *x, uint32_t m, uint32_t nprobe, uint32_t i0, IvftCall &c) {
+  stb_ctx *ctx = x->ctx;
+  cudaStream_t st = ctx->stream;
+  int rc;
+  if ((rc = ivfb_probe(x, x->b_q, m, nprobe, x->b_coarse, x->b_probe, x->b_lut, nullptr)) != STB_OK) return rc;
+  x->last_info[0] = m; x->last_info[1] = nprobe; x->last_info[2] = 0; x->last_info[3] = 0;
+  x->last_filtered = false;
+  // count grid: enough blocks for the most codes a query can probe, its nprobe longest lists
+  std::vector<uint32_t> sz(x->nlist);
+  for (uint32_t l = 0; l < x->nlist; ++l) sz[l] = x->list_off_h[l + 1] - x->list_off_h[l];
+  std::nth_element(sz.begin(), sz.begin() + (nprobe - 1), sz.end(), std::greater<uint32_t>());
+  uint64_t most = 0;
+  for (uint32_t p = 0; p < nprobe; ++p) most += sz[p];
+  const uint32_t blocks = (uint32_t)std::max<uint64_t>(1, (most + IVFT_BLOCK - 1) / IVFT_BLOCK);
+  if ((rc = x->t_cnt.reserve((size_t)m * (blocks + 1))) != STB_OK) return rc;
+  IvftArgs a;
+  a.nprobe = nprobe; a.blocks = blocks; a.list_off = x->list_off; a.codes = x->codes; a.order = x->order;
+  a.coarse = x->b_coarse; a.nlist = x->nlist; a.probe = x->b_probe; a.lut = x->b_lut; a.t = c.t;
+  a.cnt = x->t_cnt; a.total = x->t_cnt + (size_t)m * blocks; a.items = nullptr;
+  a.forced = x->forced; a.n_forced = x->n_forced; a.keys = nullptr;
+  ivft_scan_kernel<false><<<dim3(blocks, m), IVFT_THREADS, 0, st>>>(a);
+  STB_CUDA(cudaGetLastError());
+  ctx->kernel_launches += 1;
+  std::vector<uint32_t> cnt((size_t)m * (blocks + 1));
+  STB_CUDA(cudaMemcpyAsync(cnt.data(), x->t_cnt, cnt.size() * 4, cudaMemcpyDeviceToHost, st));
+  STB_CUDA(cudaStreamSynchronize(st));
+  const uint32_t *total = cnt.data() + (size_t)m * blocks;
+
+  std::vector<uint4> items;                 // the launch being planned
+  std::vector<uint32_t> slot_q, pass;
+  std::vector<int> slot_off;
+  std::vector<uint64_t> at;
+  std::vector<stb_hit> lh, pend;            // a launch's hits; the pieces of a split query
+  uint64_t keys = 0;
+  uint32_t next = 0;                        // queries [0, next) of the chunk have their end offset
+  const auto put = [&](const stb_hit *h, uint64_t n) {
+    if (c.at < c.cap) memcpy(c.out_hits + c.at, h, std::min(n, c.cap - c.at) * sizeof(stb_hit));
+    c.at += n;
+  };
+  const auto close_to = [&](uint32_t j) { for (; next < j; ++next) c.out_offsets[i0 + next + 1] = c.at; };
+  // one launch: emit, finish, hits to the host.  continues: its last slot's query has units left for the next one
+  const auto run = [&](bool continues) -> int {
+    const uint32_t n_slots = (uint32_t)slot_q.size();
+    const int K = (int)keys;
+    slot_off.push_back(K);
+    if ((rc = x->t_items.reserve(items.size(), 256)) != STB_OK || (rc = x->t_off.reserve(n_slots + 1, 256)) != STB_OK ||
+        (rc = x->t_slot.reserve(2 * (size_t)n_slots, 512)) != STB_OK || (rc = x->t_at.reserve(n_slots, 256)) != STB_OK ||
+        (rc = x->t_buf.reserve(4 * (size_t)K)) != STB_OK)
+      return rc;
+    size_t sort_bytes = 0;
+    if ((rc = stb_batch_thr_sort_bytes(ctx, K, n_slots, x->t_off, &sort_bytes)) != STB_OK) return rc;
+    if ((rc = x->t_sort.reserve(sort_bytes)) != STB_OK) return rc;
+    STB_CUDA(cudaMemcpyAsync(x->t_items, items.data(), items.size() * sizeof(uint4), cudaMemcpyHostToDevice, st));
+    STB_CUDA(cudaMemcpyAsync(x->t_off, slot_off.data(), slot_off.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    STB_CUDA(cudaMemcpyAsync(x->t_slot, slot_q.data(), n_slots * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    uint64_t *A = x->t_buf, *B = A + K, *C = B + K, *D = C + K;
+    a.items = x->t_items; a.keys = A;
+    ivft_scan_kernel<true><<<(unsigned)items.size(), IVFT_THREADS, 0, st>>>(a);
+    STB_CUDA(cudaGetLastError());
+    ctx->kernel_launches += 1;
+    uint32_t *d_pass = x->t_slot + n_slots;
+    if ((rc = stb_batch_thr_sort_rows(ctx, x->t_sort, sort_bytes, K, n_slots, x->t_off, A, B)) != STB_OK) return rc;
+    if ((rc = stb_launch_batch_thr_rescore(ctx, B, x->t_off, x->t_slot, n_slots, x->b_q, x->corpus->rows,
+                                           x->corpus->row_base, c.max_dist, C, D, d_pass)) != STB_OK) return rc;
+    if ((rc = stb_batch_thr_sort_dist(ctx, x->t_sort, sort_bytes, K, n_slots, x->t_off, C, A, D, B)) != STB_OK) return rc;
+    pass.resize(n_slots);
+    STB_CUDA(cudaMemcpyAsync(pass.data(), d_pass, n_slots * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    STB_CUDA(cudaStreamSynchronize(st));
+    at.resize(n_slots);
+    uint64_t n_hits = 0;
+    for (uint32_t s = 0; s < n_slots; ++s) { at[s] = n_hits; n_hits += pass[s]; }
+    lh.resize(n_hits);
+    if (n_hits) {
+      if ((rc = x->t_hits.reserve(n_hits)) != STB_OK) return rc;
+      STB_CUDA(cudaMemcpyAsync(x->t_at, at.data(), n_slots * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+      if ((rc = stb_launch_batch_thr_write(ctx, A, B, x->t_off, d_pass, n_slots, x->t_at, x->t_hits)) != STB_OK) return rc;
+      STB_CUDA(cudaMemcpyAsync(lh.data(), x->t_hits, n_hits * sizeof(stb_hit), cudaMemcpyDeviceToHost, st));
+      STB_CUDA(cudaStreamSynchronize(st));
+    }
+    for (uint32_t s = 0; s < n_slots; ++s) {
+      const uint32_t j = slot_q[s];
+      const stb_hit *h = lh.data() + at[s];
+      close_to(j);
+      const bool split = !pend.empty() || (continues && s == n_slots - 1);
+      if (!split) { put(h, pass[s]); continue; }
+      pend.insert(pend.end(), h, h + pass[s]);
+      if (continues && s == n_slots - 1) continue;
+      std::sort(pend.begin(), pend.end(), [](const stb_hit &u, const stb_hit &v) {
+        return u.distance < v.distance || (u.distance == v.distance && u.row < v.row);
+      });
+      put(pend.data(), pend.size());
+      pend.clear();
+    }
+    items.clear(); slot_q.clear(); slot_off.clear(); keys = 0;
+    return STB_OK;
+  };
+  for (uint32_t j = 0; j < m; ++j) {
+    const uint32_t nb = (total[j] + IVFT_BLOCK - 1) / IVFT_BLOCK;
+    uint64_t cand = 0;
+    for (uint32_t b = 0; b < nb; ++b) cand += cnt[(size_t)j * blocks + b];
+    if (c.out_scanned) c.out_scanned[i0 + j] = total[j];
+    if (c.out_reranked) c.out_reranked[i0 + j] = cand + x->n_forced;
+    for (uint32_t u = 0; u <= nb; ++u) {                          // unit 0: the forced rows; unit b + 1: block b
+      const uint32_t n_u = u == 0 ? x->n_forced : cnt[(size_t)j * blocks + u - 1];
+      if (n_u == 0) continue;
+      if (keys && keys + n_u > c.budget && (rc = run(slot_q.back() == j)) != STB_OK) return rc;
+      if (slot_q.empty() || slot_q.back() != j) { slot_q.push_back(j); slot_off.push_back((int)keys); }
+      items.push_back(make_uint4(j, u == 0 ? IVF_NO_LIST : u - 1, (uint32_t)keys, 0));
+      keys += n_u;
+    }
+  }
+  if (keys && (rc = run(false)) != STB_OK) return rc;
+  close_to(m);
+  return STB_OK;
+}
+
 // The host forms' one loop (arguments checked, subsets clipped).  Launches take the queries in caller order, at most
 // IVFB_MAX_NQ of them and as many distinct subsets as STB_IVFPQ_SUBSET_SCRATCH holds; a query of an empty subset is
 // answered here and takes no part.  Each launch: the eligibility pass of its subsets, the four batched kernels, one
 // synchronisation.  The pass is skipped when the previous launch of the call had the same subsets in the same slots,
 // whose bitmaps and counts the scratch still holds.  A launch of consecutive caller rows reads q and writes out_hits
-// in place; any other gathers its queries and scatters its hits.
+// in place; any other gathers its queries and scatters its hits.  thr != NULL: a threshold search (no subsets, top_k
+// and rerank 0), whose launches ivft_chunk answers after the query upload.
 static int ivfb_host_search(stb_ivfpq *x, const float *q, uint32_t nq, uint32_t nprobe, uint32_t top_k, uint32_t rerank,
-                            const IvfbSubsets &s, stb_hit *out_hits, uint32_t *out_n, uint64_t *out_scanned) {
-  if (top_k == 0) { ivf_answer_none(out_hits, out_n, out_scanned, 0, nq, 0); return STB_OK; }
+                            const IvfbSubsets &s, stb_hit *out_hits, uint32_t *out_n, uint64_t *out_scanned,
+                            IvftCall *thr = nullptr) {
+  if (top_k == 0 && !thr) { ivf_answer_none(out_hits, out_n, out_scanned, 0, nq, 0); return STB_OK; }
   stb_ctx *ctx = x->ctx;
   if (cudaSetDevice(ctx->device) != cudaSuccess) { stb_set_error("cudaSetDevice failed"); return STB_ERR_CUDA; }
   ivf_clamp(x, top_k, IVFB_RERANK_CAP, nprobe, rerank);
@@ -1900,6 +2135,10 @@ static int ivfb_host_search(stb_ivfpq *x, const float *q, uint32_t nq, uint32_t 
         STB_CUDA(cudaMemcpyAsync(x->f_slot_set, slot_set.data(), (size_t)m * 4, cudaMemcpyHostToDevice, st));
         f.slot_set = x->f_slot_set;
       }
+    }
+    if (thr) {
+      if ((rc = ivft_chunk(x, m, nprobe, qrow[0], *thr)) != STB_OK) return rc;
+      continue;
     }
     if ((rc = ivfb_launch(x, x->b_q, m, nprobe, top_k, rerank, x->b_hits, x->b_status, s.filter ? &f : nullptr)) != STB_OK)
       return rc;
@@ -1977,6 +2216,43 @@ int stb_ivfpq_search_subsets(stb_ivfpq *x, const float *q, uint32_t nq, uint32_t
   }
   sub.subset_of = subset_of;
   return ivfb_host_search(x, q, nq, nprobe, top_k, rerank, sub, out_hits, out_n, out_scanned);
+}
+
+int stb_ivfpq_search_threshold(stb_ivfpq *x, const float *q, uint32_t nq, uint32_t nprobe, double max_distance,
+                               double slack, stb_hit *out_hits, uint64_t cap, uint64_t *out_offsets,
+                               uint64_t *out_scanned, uint64_t *out_reranked) {
+  static const char *who = "ivfpq_search_threshold";
+  if (!x) { stb_set_error("%s: null index", who); return STB_ERR_ARG; }
+  if (nq == 0) return STB_OK;
+  if (!q || !out_offsets || (cap && !out_hits)) { stb_set_error("%s: null argument", who); return STB_ERR_ARG; }
+  if (!(slack >= 0.0)) { stb_set_error("%s: slack must be >= 0 (got %g)", who, slack); return STB_ERR_ARG; }
+  for (uint32_t i = 0; i <= nq; ++i) out_offsets[i] = 0;
+  for (uint32_t i = 0; i < nq; ++i) { if (out_scanned) out_scanned[i] = 0; if (out_reranked) out_reranked[i] = 0; }
+  if (!(max_distance > 0.0)) return STB_OK;                 // NaN or <= 0: no distance is below it
+  // the cutoff RD_f32((1 - M) - slack), rounded toward -inf from f64
+  const double t64 = (1.0 - max_distance) - slack;
+  float t = (float)t64;
+  if ((double)t > t64) t = std::nextafter(t, -INFINITY);
+  IvftCall c;
+  c.t = t; c.max_dist = max_distance; c.budget = x->t_budget ? x->t_budget : STB_IVFPQ_THRESHOLD_KEYS;
+  c.out_hits = out_hits; c.cap = cap; c.out_offsets = out_offsets; c.out_scanned = out_scanned; c.out_reranked = out_reranked;
+  const int rc = ivfb_host_search(x, q, nq, nprobe, 0, 0, IvfbSubsets(), nullptr, nullptr, nullptr, &c);
+  if (rc != STB_OK) return rc;
+  if (out_offsets[nq] > cap) {
+    stb_set_error("%s: %llu hits, capacity %llu", who, (unsigned long long)out_offsets[nq], (unsigned long long)cap);
+    return STB_ERR_CAPACITY;
+  }
+  return STB_OK;
+}
+
+int stb_debug_ivfpq_threshold_keys(stb_ivfpq *x, uint64_t keys) {
+  if (!x) { stb_set_error("ivfpq_threshold_keys: null index"); return STB_ERR_ARG; }
+  if (keys > STB_IVFPQ_THRESHOLD_KEYS) {
+    stb_set_error("ivfpq_threshold_keys: at most %llu keys", (unsigned long long)STB_IVFPQ_THRESHOLD_KEYS);
+    return STB_ERR_ARG;
+  }
+  x->t_budget = keys;
+  return STB_OK;
 }
 
 int stb_ivfpq_search(stb_ivfpq *x, const float *q, uint32_t nprobe, uint32_t top_k, uint32_t rerank,
