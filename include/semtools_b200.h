@@ -578,6 +578,58 @@ int stb_ivfpq_update(stb_ivfpq *index, const uint64_t *idx, const float *rows, u
 int stb_ivfpq_remove(stb_ivfpq *index, const uint64_t *ranges, uint32_t n_ranges);
 int stb_ivfpq_stats(const stb_ivfpq *index, uint64_t *rows, uint32_t *nlist, uint32_t *max_list,
                     uint64_t *index_bytes);
+/* Save an index to a file and load it onto its corpus in another process, without retraining or re-encoding.
+ * File format, version 1, little-endian.  A 216-byte header, then the six sections back to back, in order:
+ *     0  char     magic[8] = "STBIVFPQ"
+ *     8  u32      version = 1, d = 256, pq_m = 32, pq_ksub = 256, pq_dsub = 8, nlist
+ *    32  u64      n (rows indexed), n_listed, n_forced, rows_digest
+ *    64  6 x {u64 offset, u64 bytes, u64 checksum}, one per section
+ *   208  u64      header_checksum = digest(the header's bytes [0, 208))
+ *   216  centroids f32[nlist][256], codebooks f32[32][256][8], list_off u32[nlist + 1], order u32[n_listed],
+ *        codes u8[n_listed][32], forced u32[n_forced] -- exactly stb_debug_ivfpq_export's arrays.  Section k
+ *        starts where section k - 1 ends (the first at 216) and the file ends with the last one.
+ *   The checksum of a section is digest(its bytes); rows_digest = digest(the corpus rows [0, n) as stored: n x
+ *   256 f32, 1 KiB per row).  Nothing else is stored: no query scratch, batch state or tuning value.
+ * The digest of a byte string s of L bytes (all arithmetic mod 2^64):
+ *     mix(z):  z ^= z >> 30; z *= 0xBF58476D1CE4E5B9; z ^= z >> 27; z *= 0x94D049BB133111EB; z ^= z >> 31
+ *     s is zero-padded to whole 1 KiB blocks; w(b, i) = little-endian u64 at byte 1024 b + 8 i (i < 128)
+ *     h(b)     = sum over i of mix(w(b, i) ^ (i + 1) * 0x9E3779B97F4A7C15)
+ *     digest   = sum over b of mix(h(b) ^ (b + 1) * 0xC2B2AE3D27D4EB4F)  +  mix(L ^ 0x165667B19E3779F9)
+ *   It is order-sensitive (a word's position and its block's enter its term) and parallel over blocks: the GPU
+ *   computes every section checksum, after the section reached HBM, and rows_digest, a block per row.  It
+ *   detects a wrong corpus or accidental damage; it is NOT cryptographic and does not authenticate a file.
+ * stb_ivfpq_save: synchronous (waits for the index's enqueued work); the index is not changed.  Writes the
+ *   file through a 32 MiB pinned buffer (never a second host copy of the index) to a new file beside `path`
+ *   (path + ".tmp.<pid>.<k>", the next k while that name exists), fsyncs it and renames it over `path`, so a
+ *   reader sees the old file or the whole new one.  On any failure `path` is untouched and the temporary file removed.  The same index gives the same
+ *   bytes.  STB_ERR_ARG: a NULL argument, or a path that cannot be written.  STB_ERR_STATE: the corpus was
+ *   cleared since the index last read it (as stb_ivfpq_extend).
+ * stb_ivfpq_load: a new index on `corpus` equal to the saved one: stb_debug_ivfpq_export and stb_ivfpq_stats
+ *   return the saved values, every search, extend, update and remove behaves as on the original, bit for bit.
+ *   The corpus may have another row_base (hits carry this corpus's global rows) and rows appended after
+ *   [0, n): they stay outside the index until stb_ivfpq_extend.  The file is untrusted input; in order:
+ *    1. corpus of another context: STB_ERR_ARG; a host-rows corpus: STB_ERR_STATE (as stb_ivfpq_build);
+ *    2. before anything is allocated, STB_ERR_ARG with a message naming the field: the file cannot be read or is
+ *       shorter than the header; magic, version, shape constants; header_checksum; 1 <= nlist <= 8192;
+ *       n_forced <= 1024; n_listed + n_forced == n < 2^32; each section's offset and bytes as the counts give
+ *       them, and the file ends where the last section ends.  Then a corpus with fewer than n rows: STB_ERR_STATE;
+ *    3. the sections are read through the pinned buffer into the index's own buffers and their checksums
+ *       computed on the GPU: a mismatch is STB_ERR_ARG;
+ *    4. one GPU pass over the lists, STB_ERR_ARG unless list_off[0] == 0, list_off never decreases and
+ *       list_off[nlist] == n_listed; every order entry is < n and each list strictly ascending; forced is
+ *       strictly ascending and < n; no row appears twice across order and forced (a bitmap of n bits) -- with
+ *       the counts, every row of [0, n) appears exactly once;
+ *    5. one GPU pass over the corpus rows [0, n): their digest must equal rows_digest (else STB_ERR_STATE), and
+ *       forced must be exactly the rows that cannot be normalised (the build's rule; else STB_ERR_ARG).
+ *   Only then is the index installed (query scratch, corpus epoch, the corpus's live-index count).  On every
+ *   refusal nothing stays allocated, the corpus is not counted as indexed (stb_corpus_update still works), and
+ *   the context stays usable.  Checks 2 and 4 run before any kernel reads list_off, order or forced as indices.
+ *   The codes and list assignments are not re-derived (that is the build's add phase, which loading skips).
+ *   Guarantees: accidental damage is caught by the checksums and a different corpus by the digest; a crafted
+ *   file with consistent checksums can at worst lower recall -- every kernel stays in bounds and every returned
+ *   distance is still the exact canonical distance of its row. */
+int stb_ivfpq_save(const stb_ivfpq *index, const char *path);
+int stb_ivfpq_load(stb_ctx *ctx, const stb_corpus *corpus, const char *path, stb_ivfpq **out);
 int stb_ivfpq_search(stb_ivfpq *index, const float *q, uint32_t nprobe, uint32_t top_k,
                      uint32_t rerank, stb_hit *out_hits, uint32_t *out_n, uint64_t *out_scanned);
 /* Asynchronous device-resident form (query, hits and status stay in HBM, nothing synchronises): the
@@ -865,6 +917,9 @@ int stb_debug_ivfpq_batch_last(const stb_ivfpq *index, uint32_t i, uint32_t info
 /* Test hook for K5's threshold search: candidate keys per launch for this index (0 = STB_IVFPQ_THRESHOLD_KEYS;
  * more than that is STB_ERR_ARG).  Lowering it splits queries between launches without changing any answer. */
 int stb_debug_ivfpq_threshold_keys(stb_ivfpq *index, uint64_t keys);
+/* Test hook for K5's stb_ivfpq_load: host milliseconds of the load that made this index, ms[0] reading the file
+ * and uploading its sections, ms[1] the GPU verification (checksums, lists, rows); both 0 for a built index. */
+int stb_debug_ivfpq_load_ms(const stb_ivfpq *index, double ms[2]);
 /* Test hook for K2: describes the most recent stb_search_batch_dev, stb_search_batch_filtered,
  * stb_search_batch_subsets or stb_search_batch_threshold on ctx (synchronises the stream).  info = {route, nq, a,
  * b, n_seg, seg_cap}; route 1 = v1, 2 = v2, 3 = filtered v2, 4 = a filtered call that launched nothing on the

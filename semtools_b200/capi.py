@@ -35,7 +35,7 @@ SYMBOLS = [
     "stb_debug_ivfpq_export",
     "stb_ivfpq_search_batch", "stb_ivfpq_search_batch_dev", "stb_debug_ivfpq_batch_last",
     "stb_ivfpq_search_filtered", "stb_ivfpq_search_subsets", "stb_ivfpq_update", "stb_ivfpq_remove",
-    "stb_ivfpq_search_threshold", "stb_debug_ivfpq_threshold_keys",
+    "stb_ivfpq_search_threshold", "stb_debug_ivfpq_threshold_keys", "stb_ivfpq_save", "stb_ivfpq_load", "stb_debug_ivfpq_load_ms",
     "stb_tokenizer_load", "stb_tokenizer_load_ex", "stb_tokenizer_destroy", "stb_tokenizer_gpu_lines", "stb_embed_text", "stb_debug_tokenize",
 ]
 STB_TOKENIZER_PIECE_CAP = 256
@@ -154,6 +154,9 @@ def lib() -> C.CDLL:
     L.stb_ivfpq_search_subsets.argtypes = [vp, vp, u32, u32, u32, u32, i32, f64, u32, vp, vp, vp, vp, vp, vp]
     L.stb_ivfpq_search_threshold.argtypes = [vp, vp, u32, u32, f64, f64, vp, u64, vp, vp, vp]
     L.stb_debug_ivfpq_threshold_keys.argtypes = [vp, u64]
+    L.stb_ivfpq_save.argtypes = [vp, C.c_char_p]
+    L.stb_ivfpq_load.argtypes = [vp, vp, C.c_char_p, C.POINTER(vp)]
+    L.stb_debug_ivfpq_load_ms.argtypes = [vp, vp]
     L.stb_tokenizer_load.argtypes = [vp, vp, u64, C.POINTER(vp)]
     L.stb_tokenizer_load_ex.argtypes = [vp, vp, u64, u32, C.POINTER(vp)]
     L.stb_tokenizer_destroy.argtypes = [vp]
@@ -709,6 +712,25 @@ class IvfPq:
             self._h = None
 
     __del__ = close
+
+    def save(self, path):
+        """stb_ivfpq_save: write the index to `path` (atomically replaced); the corpus rows are not stored."""
+        _check(lib().stb_ivfpq_save(self._h, os.fsencode(path)))
+
+    @classmethod
+    def load(cls, corpus: "Corpus", path) -> "IvfPq":
+        """stb_ivfpq_load: the index saved at `path`, on a corpus whose first rows are the ones it was saved with."""
+        self = cls.__new__(cls)
+        self.corpus = corpus
+        self._h = vp()
+        _check(lib().stb_ivfpq_load(corpus.ctx._h, corpus._h, os.fsencode(path), C.byref(self._h)))
+        return self
+
+    def load_ms(self):
+        """stb_debug_ivfpq_load_ms: (read + upload, verification) milliseconds of the load that made this index."""
+        ms = np.zeros(2, dtype=np.float64)
+        _check(lib().stb_debug_ivfpq_load_ms(self._h, _np_ptr(ms)))
+        return float(ms[0]), float(ms[1])
 
     def extend(self) -> int:
         """stb_ivfpq_extend: index the rows appended to the corpus since the build or the last extend

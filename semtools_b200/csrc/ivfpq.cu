@@ -22,12 +22,18 @@
 // its cosine.  Such rows are kept out of the inverted lists and out of training; the build records
 // them in a side list (at most IVF_FORCED_CAP, usually empty) that every search re-ranks exactly
 // in addition to the ADC candidates.
+#include <fcntl.h>
 #include <math_constants.h>
+#include <sys/stat.h>
+#include <unistd.h>
 
 #include <algorithm>
+#include <atomic>
+#include <chrono>
 #include <cmath>
 #include <cub/device/device_radix_sort.cuh>
 #include <functional>
+#include <string>
 #include <vector>
 
 #include "common.cuh"
@@ -105,6 +111,7 @@ struct stb_ivfpq {
   StbBuf<uint64_t> t_at;             // [slots] where each slot's hits go in t_hits
   StbBuf<stb_hit> t_hits;
   StbBuf<uint8_t> t_sort;
+  double load_ms[2];                 // stb_ivfpq_load: read + upload, verification (0 for a built index)
 };
 
 // ------------------------------------------------------------------ assignment GEMM ---
@@ -1498,6 +1505,19 @@ static int ivf_add_rows(stb_ivfpq *x, uint64_t first, uint64_t m, const char *wh
   return ivf_edit_swap(x, e);
 }
 
+// The query scratch every search reads and the fused kernels' tickets (zeroed, enqueued): the last step of
+// stb_ivfpq_build and of stb_ivfpq_load, once the index's arrays are in place.
+static int ivf_alloc_query_scratch(stb_ivfpq *x) {
+  IVF_TRY(x->coarse.alloc(x->nlist));
+  IVF_TRY(x->lut.alloc((size_t)PQ_M * PQ_KSUB));
+  IVF_TRY(x->probe.alloc(2 * 1024 + 1));
+  IVF_TRY(x->cand_rows.alloc(IVF_HOST_TOPK_MAX + IVF_FORCED_CAP + 4));   // + the valid-row counter
+  IVF_TRY(x->keys2.alloc((size_t)ADC2_MAX_CTAS * ADC2_KEEP));
+  IVF_TRY(x->tickets.alloc(2));
+  STB_CUDA(cudaMemsetAsync(x->tickets, 0, 2 * sizeof(unsigned int), x->ctx->stream));
+  return STB_OK;
+}
+
 extern "C" {
 
 int stb_ivfpq_destroy(stb_ivfpq *x) {
@@ -1602,14 +1622,8 @@ int stb_ivfpq_build(stb_ctx *ctx, const stb_corpus *corpus, uint32_t nlist, uint
   x->list_off_h.assign(nlist + 1, 0);
   int rc = ivf_add_rows(x, 0, n, "ivfpq_build");
   if (rc != STB_OK) IVF_FAIL(rc);
-  // query scratch
-  IVF_ALLOC(x->coarse, nlist);
-  IVF_ALLOC(x->lut, (size_t)PQ_M * PQ_KSUB);
-  IVF_ALLOC(x->probe, 2 * 1024 + 1);
-  IVF_ALLOC(x->cand_rows, IVF_HOST_TOPK_MAX + IVF_FORCED_CAP + 4);   // + the valid-row counter
-  IVF_ALLOC(x->keys2, (size_t)ADC2_MAX_CTAS * ADC2_KEEP);
-  IVF_ALLOC(x->tickets, 2);
-  IVF_CUDA(cudaMemsetAsync(x->tickets, 0, 2 * sizeof(unsigned int), ctx->stream));
+  rc = ivf_alloc_query_scratch(x);
+  if (rc != STB_OK) IVF_FAIL(rc);
   IVF_CUDA(cudaGetLastError());
   IVF_CUDA(cudaStreamSynchronize(st));
   ctx->kernel_launches += 3 + iters * 8;                   // training (the add phase counts its own)
@@ -2370,6 +2384,476 @@ int stb_debug_ivfpq_batch_last(const stb_ivfpq *x, uint32_t i, uint32_t info[4],
   const size_t stride = x->last_filtered ? IVFB_PROBE_STRIDE(nprobe, true) : IVFB_PROBE_STRIDE(nprobe, false);
   if (probe) STB_CUDA(cudaMemcpy(probe, x->b_probe + (size_t)i * stride, (size_t)nprobe * 4, cudaMemcpyDeviceToHost));
   if (lut) STB_CUDA(cudaMemcpy(lut, x->b_lut + (size_t)i * PQ_M * PQ_KSUB, (size_t)PQ_M * PQ_KSUB * 4, cudaMemcpyDeviceToHost));
+  return STB_OK;
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------ saved index file ------
+// stb_ivfpq_save / stb_ivfpq_load (format and guarantees in the header).  One digest definition serves the
+// corpus rows and every section: ivf_digest_block is one 1 KiB block's term, computed by a warp whose lane l
+// holds the block's u64 words 4l .. 4l+3; ivf_digest_kernel sums the terms of a byte string's blocks and
+// ivf_rows_pass_kernel those of the corpus rows (one row = one block), the length term is added on the host.
+// The sums are mod 2^64 and commutative, so the result does not depend on which warp took which block.
+#define IVF_FILE_VERSION 1
+#define IVF_FILE_SECTIONS 6
+#define IVF_FILE_CHUNK (16ull << 20)     // bytes per half of the pinned buffer a save or load streams through
+#define IVF_DIGEST_K1 0x9E3779B97F4A7C15ull
+#define IVF_DIGEST_K2 0xC2B2AE3D27D4EB4Full
+#define IVF_DIGEST_K3 0x165667B19E3779F9ull
+// failures of the verification pass (bits of its status word)
+#define IVF_BAD_OFF 1u                   // list_off[0] != 0, a decreasing pair, or list_off[nlist] != n_listed
+#define IVF_BAD_ROW 2u                   // an order entry >= n
+#define IVF_BAD_ORDER 4u                 // a list not strictly ascending
+#define IVF_BAD_FORCED 8u                // a forced entry >= n, or forced not strictly ascending
+#define IVF_BAD_DUP 16u                  // a row in two places of order and forced
+
+struct IvfFileSection {
+  uint64_t offset, bytes, checksum;
+};
+struct IvfFileHeader {
+  char magic[8];                         // "STBIVFPQ"
+  uint32_t version, d, pq_m, pq_ksub, pq_dsub, nlist;
+  uint64_t n, n_listed, n_forced, rows_digest;
+  IvfFileSection sec[IVF_FILE_SECTIONS]; // centroids, codebooks, list_off, order, codes, forced
+  uint64_t header_checksum;              // digest of the 208 bytes before it
+};
+static_assert(sizeof(IvfFileHeader) == 216, "IvfFileHeader is the file's first 216 bytes");
+static const char *const ivf_section_name[IVF_FILE_SECTIONS] = {"centroids", "codebooks", "list_off", "order", "codes", "forced"};
+
+__host__ __device__ __forceinline__ uint64_t ivf_mix(uint64_t z) {
+  z ^= z >> 30; z *= 0xBF58476D1CE4E5B9ull;
+  z ^= z >> 27; z *= 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
+// Term of block b (warp-collective; every lane returns it): mix(h_b ^ (b + 1) K2), h_b = sum_i mix(w_i ^ (i + 1) K1).
+__device__ __forceinline__ uint64_t ivf_digest_block(const uint64_t (&w)[4], uint64_t b) {
+  const uint64_t lane = threadIdx.x & 31;
+  unsigned long long h = 0;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) h += ivf_mix(w[k] ^ ((4 * lane + k + 1) * IVF_DIGEST_K1));
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) h += __shfl_xor_sync(0xffffffffu, h, off);
+  return ivf_mix(h ^ ((b + 1) * IVF_DIGEST_K2));
+}
+
+// *out += the block terms of p[0, bytes) (zero-padded to whole blocks); warp per block
+__global__ void __launch_bounds__(256) ivf_digest_kernel(const uint8_t *__restrict__ p, uint64_t bytes, unsigned long long *out) {
+  const int lane = threadIdx.x & 31;
+  const uint64_t blocks = (bytes + 1023) / 1024;
+  unsigned long long acc = 0;
+  for (uint64_t b = (uint64_t)blockIdx.x * 8 + (threadIdx.x >> 5); b < blocks; b += (uint64_t)gridDim.x * 8) {
+    uint64_t w[4];
+    if ((b + 1) * 1024 <= bytes) {
+      const ulonglong2 *q = reinterpret_cast<const ulonglong2 *>(p + b * 1024) + 2 * lane;
+      const ulonglong2 a = __ldg(q), c = __ldg(q + 1);
+      w[0] = a.x; w[1] = a.y; w[2] = c.x; w[3] = c.y;
+    } else {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const uint64_t off = b * 1024 + 8 * (4 * lane + k);
+        w[k] = 0;
+        for (uint64_t j = 0; j < 8 && off + j < bytes; ++j) w[k] |= (uint64_t)p[off + j] << (8 * j);
+      }
+    }
+    acc += ivf_digest_block(w, b);
+  }
+  if (lane == 0 && acc) atomicAdd(out, acc);
+}
+
+// One read of rows [0, n): out[0] += their block terms, out[1] = rows with K1's forced flag (ivf_forced),
+// out[2] = those of them not in forced[0, n_forced) (ascending: binary search)
+__global__ void __launch_bounds__(256) ivf_rows_pass_kernel(const float4 *__restrict__ X, uint64_t n, const uint32_t *__restrict__ forced,
+                                                            uint32_t n_forced, unsigned long long *out) {
+  const int lane = threadIdx.x & 31;
+  unsigned long long acc = 0, flagged = 0, missing = 0;
+  for (uint64_t i = (uint64_t)blockIdx.x * 8 + (threadIdx.x >> 5); i < n; i += (uint64_t)gridDim.x * 8) {
+    const float4 v0 = __ldg(X + i * STB_ROW_F4 + 2 * lane), v1 = __ldg(X + i * STB_ROW_F4 + 2 * lane + 1);
+    const uint64_t w[4] = {__float_as_uint(v0.x) | (uint64_t)__float_as_uint(v0.y) << 32,
+                           __float_as_uint(v0.z) | (uint64_t)__float_as_uint(v0.w) << 32,
+                           __float_as_uint(v1.x) | (uint64_t)__float_as_uint(v1.y) << 32,
+                           __float_as_uint(v1.z) | (uint64_t)__float_as_uint(v1.w) << 32};
+    acc += ivf_digest_block(w, i);
+    if (ivf_forced(ivf_warp_ss(v0, v1)) && lane == 0) {
+      ++flagged;
+      uint32_t lo = 0, hi = n_forced;
+      while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (__ldg(forced + mid) < i) lo = mid + 1; else hi = mid; }
+      if (lo == n_forced || __ldg(forced + lo) != i) ++missing;
+    }
+  }
+  if (lane != 0) return;
+  if (acc) atomicAdd(out, acc);
+  if (flagged) atomicAdd(out + 1, flagged);
+  if (missing) atomicAdd(out + 2, missing);
+}
+
+// The loaded lists and forced list against n rows (seen: n bits, zeroed): a warp per list checks its own
+// [list_off[l], list_off[l + 1]) before it reads order there; threads past the lists' CTAs take forced.
+__global__ void __launch_bounds__(256) ivf_verify_lists_kernel(const uint32_t *__restrict__ list_off, uint32_t nlist, uint64_t n_listed,
+                                                               const uint32_t *__restrict__ order, const uint32_t *__restrict__ forced,
+                                                               uint32_t n_forced, uint64_t n, uint32_t *seen, uint32_t *bad) {
+  const uint32_t list_ctas = (nlist + 7) / 8;
+  uint32_t flags = 0;
+  if (blockIdx.x < list_ctas) {
+    const uint32_t lane = threadIdx.x & 31, l = blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (l >= nlist) return;
+    const uint32_t b = list_off[l], e = list_off[l + 1];
+    if ((l == 0 && b != 0) || (l == nlist - 1 && e != n_listed) || b > e || e > n_listed) {
+      if (lane == 0) atomicOr(bad, IVF_BAD_OFF);
+      return;
+    }
+    for (uint32_t i = b + lane; i < e; i += 32) {
+      const uint32_t r = order[i];
+      if (i > b && order[i - 1] >= r) flags |= IVF_BAD_ORDER;
+      if (r >= n) { flags |= IVF_BAD_ROW; continue; }
+      if (atomicOr(seen + (r >> 5), 1u << (r & 31)) & (1u << (r & 31))) flags |= IVF_BAD_DUP;
+    }
+  } else {
+    const uint32_t i = (blockIdx.x - list_ctas) * blockDim.x + threadIdx.x;
+    if (i >= n_forced) return;
+    const uint32_t r = forced[i];
+    if ((i > 0 && forced[i - 1] >= r) || r >= n) flags |= IVF_BAD_FORCED;
+    else if (atomicOr(seen + (r >> 5), 1u << (r & 31)) & (1u << (r & 31))) flags |= IVF_BAD_DUP;
+  }
+  if (flags) atomicOr(bad, flags);
+}
+
+// the digest of a host byte string (the header's checksum): the kernels' definition, block by block
+static uint64_t ivf_digest_host(const void *p, uint64_t bytes) {
+  const uint8_t *s = static_cast<const uint8_t *>(p);
+  uint64_t d = 0;
+  for (uint64_t b = 0; b * 1024 < bytes; ++b) {
+    uint64_t h = 0;
+    for (uint64_t i = 0; i < 128; ++i) {
+      uint64_t w = 0;
+      for (uint64_t j = 0; j < 8; ++j) {
+        const uint64_t o = b * 1024 + 8 * i + j;
+        if (o < bytes) w |= (uint64_t)s[o] << (8 * j);
+      }
+      h += ivf_mix(w ^ ((i + 1) * IVF_DIGEST_K1));
+    }
+    d += ivf_mix(h ^ ((b + 1) * IVF_DIGEST_K2));
+  }
+  return d + ivf_mix(bytes ^ IVF_DIGEST_K3);
+}
+
+static unsigned ivf_digest_ctas(const stb_ctx *ctx, uint64_t blocks) {
+  return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((blocks + 7) / 8, (uint64_t)ctx->sm_count * 16));
+}
+
+// section sizes for the counts, and their offsets: back to back after the header
+static void ivf_file_layout(uint32_t nlist, uint64_t n_listed, uint64_t n_forced, IvfFileSection sec[IVF_FILE_SECTIONS]) {
+  const uint64_t bytes[IVF_FILE_SECTIONS] = {(uint64_t)nlist * STB_D * 4, (uint64_t)PQ_M * PQ_KSUB * PQ_DSUB * 4,
+                                             ((uint64_t)nlist + 1) * 4, n_listed * 4, n_listed * PQ_M, n_forced * 4};
+  uint64_t off = sizeof(IvfFileHeader);
+  for (int k = 0; k < IVF_FILE_SECTIONS; ++k) { sec[k].offset = off; sec[k].bytes = bytes[k]; off += bytes[k]; }
+}
+
+static uint8_t *ivf_section_dev(const stb_ivfpq *x, int k) {
+  void *p[IVF_FILE_SECTIONS] = {x->centroids, x->codebooks, x->list_off, x->order, x->codes, x->forced};
+  return static_cast<uint8_t *>(p[k]);
+}
+
+// The checksums of x's sections laid out as sec (and, with `rows`, the digest of the corpus rows [0, n), the
+// forced flags it counts and those missing from forced) into sum[0 .. 5] and sum[6 .. 8]; synchronous.
+static int ivf_file_digests(const stb_ivfpq *x, const IvfFileSection sec[IVF_FILE_SECTIONS], bool rows,
+                            uint64_t sum[IVF_FILE_SECTIONS + 3]) {
+  stb_ctx *ctx = x->ctx;
+  cudaStream_t st = ctx->stream;
+  StbBuf<unsigned long long> d;
+  IVF_TRY(d.alloc(IVF_FILE_SECTIONS + 3));
+  STB_CUDA(cudaMemsetAsync(d, 0, (IVF_FILE_SECTIONS + 3) * 8, st));
+  for (int k = 0; k < IVF_FILE_SECTIONS; ++k) {
+    if (!sec[k].bytes) continue;
+    ivf_digest_kernel<<<ivf_digest_ctas(ctx, (sec[k].bytes + 1023) / 1024), 256, 0, st>>>(ivf_section_dev(x, k), sec[k].bytes, d + k);
+    ctx->kernel_launches += 1;
+  }
+  if (rows && x->n) {
+    ivf_rows_pass_kernel<<<ivf_digest_ctas(ctx, x->n), 256, 0, st>>>(reinterpret_cast<const float4 *>(x->corpus->rows), x->n,
+                                                                     x->forced, x->n_forced, d + IVF_FILE_SECTIONS);
+    ctx->kernel_launches += 1;
+  }
+  STB_CUDA(cudaGetLastError());
+  STB_CUDA(cudaMemcpyAsync(sum, d, (IVF_FILE_SECTIONS + 3) * 8, cudaMemcpyDeviceToHost, st));
+  STB_CUDA(cudaStreamSynchronize(st));
+  for (int k = 0; k < IVF_FILE_SECTIONS; ++k) sum[k] += ivf_mix(sec[k].bytes ^ IVF_DIGEST_K3);
+  sum[IVF_FILE_SECTIONS] += ivf_mix((x->n * STB_D * 4) ^ IVF_DIGEST_K3);
+  return STB_OK;
+}
+
+// A page-locked buffer of two halves and an event per half: the file side of one half overlaps the copy of
+// the other.
+struct IvfFilePipe {
+  StbPinned<uint8_t> buf;
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  int half = 0;
+  ~IvfFilePipe() {
+    for (cudaEvent_t e : ev) if (e) { cudaEventSynchronize(e); cudaEventDestroy(e); }
+  }
+  int init() {
+    IVF_TRY(buf.alloc(2 * IVF_FILE_CHUNK));
+    for (cudaEvent_t &e : ev) STB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    return STB_OK;
+  }
+};
+
+static bool ivf_pio(int fd, bool wr, uint8_t *p, uint64_t bytes, uint64_t off) {
+  while (bytes) {
+    const ssize_t r = wr ? pwrite(fd, p, bytes, (off_t)off) : pread(fd, p, bytes, (off_t)off);
+    if (r < 0 && errno == EINTR) continue;
+    if (r <= 0) return false;
+    p += r; bytes -= (uint64_t)r; off += (uint64_t)r;
+  }
+  return true;
+}
+
+// device -> file: chunk c is copied into one half while chunk c - 1 is written from the other
+static int ivf_file_write(stb_ctx *ctx, IvfFilePipe &pp, int fd, const uint8_t *src, uint64_t bytes, uint64_t off, const char *path) {
+  int pend = -1;
+  uint64_t pend_bytes = 0, pend_off = 0;
+  for (uint64_t done = 0;;) {
+    const uint64_t c = std::min<uint64_t>(bytes - done, IVF_FILE_CHUNK);
+    if (c) {
+      STB_CUDA(cudaMemcpyAsync(pp.buf + pp.half * IVF_FILE_CHUNK, src + done, c, cudaMemcpyDeviceToHost, ctx->stream));
+      STB_CUDA(cudaEventRecord(pp.ev[pp.half], ctx->stream));
+    }
+    if (pend >= 0) {
+      STB_CUDA(cudaEventSynchronize(pp.ev[pend]));
+      if (!ivf_pio(fd, true, pp.buf + pend * IVF_FILE_CHUNK, pend_bytes, pend_off)) {
+        stb_set_error("ivfpq_save: cannot write %s: %s", path, strerror(errno));
+        return STB_ERR_ARG;
+      }
+    }
+    if (!c) return STB_OK;
+    pend = pp.half; pend_bytes = c; pend_off = off + done;
+    pp.half ^= 1;
+    done += c;
+  }
+}
+
+// file -> device: a half is refilled once the copy that last read it is done
+static int ivf_file_read(stb_ctx *ctx, IvfFilePipe &pp, int fd, uint8_t *dst, uint64_t bytes, uint64_t off, const char *path) {
+  for (uint64_t done = 0; done < bytes;) {
+    const uint64_t c = std::min<uint64_t>(bytes - done, IVF_FILE_CHUNK);
+    uint8_t *h = pp.buf + pp.half * IVF_FILE_CHUNK;
+    STB_CUDA(cudaEventSynchronize(pp.ev[pp.half]));
+    if (!ivf_pio(fd, false, h, c, off + done)) {
+      stb_set_error("ivfpq_load: cannot read %s at byte %llu", path, (unsigned long long)(off + done));
+      return STB_ERR_ARG;
+    }
+    STB_CUDA(cudaMemcpyAsync(dst + done, h, c, cudaMemcpyHostToDevice, ctx->stream));
+    STB_CUDA(cudaEventRecord(pp.ev[pp.half], ctx->stream));
+    pp.half ^= 1;
+    done += c;
+  }
+  return STB_OK;
+}
+
+// the file's header after the checks of stb_ivfpq_load's step 2 that need no allocation (STB_ERR_ARG naming the field)
+static int ivf_file_check_header(const IvfFileHeader &h, uint64_t file_bytes, const char *path) {
+#define IVF_BAD_FILE(...)                                        \
+  do {                                                           \
+    stb_set_error("ivfpq_load: %s: " __VA_ARGS__);               \
+    return STB_ERR_ARG;                                          \
+  } while (0)
+  if (memcmp(h.magic, "STBIVFPQ", 8) != 0) IVF_BAD_FILE("magic is not STBIVFPQ", path);
+  if (h.version != IVF_FILE_VERSION) IVF_BAD_FILE("version %u (this library reads %u)", path, h.version, IVF_FILE_VERSION);
+  if (h.d != STB_D || h.pq_m != PQ_M || h.pq_ksub != PQ_KSUB || h.pq_dsub != PQ_DSUB)
+    IVF_BAD_FILE("shape constants d/pq_m/pq_ksub/pq_dsub = %u/%u/%u/%u (want 256/32/256/8)", path, h.d, h.pq_m, h.pq_ksub, h.pq_dsub);
+  if (h.header_checksum != ivf_digest_host(&h, offsetof(IvfFileHeader, header_checksum)))
+    IVF_BAD_FILE("header_checksum does not match the header", path);
+  if (h.nlist < 1 || h.nlist > 8192) IVF_BAD_FILE("nlist %u outside [1, 8192]", path, h.nlist);
+  if (h.n_forced > IVF_FORCED_CAP) IVF_BAD_FILE("n_forced %llu > %u", path, (unsigned long long)h.n_forced, (unsigned)IVF_FORCED_CAP);
+  if (h.n > 0xffffffffull || h.n_listed > h.n || h.n_listed + h.n_forced != h.n)
+    IVF_BAD_FILE("n_listed %llu + n_forced %llu != n %llu (or n >= 2^32)", path, (unsigned long long)h.n_listed,
+                 (unsigned long long)h.n_forced, (unsigned long long)h.n);
+  IvfFileSection want[IVF_FILE_SECTIONS];
+  ivf_file_layout(h.nlist, h.n_listed, h.n_forced, want);
+  for (int k = 0; k < IVF_FILE_SECTIONS; ++k)
+    if (h.sec[k].offset != want[k].offset || h.sec[k].bytes != want[k].bytes)
+      IVF_BAD_FILE("section %s at %llu, %llu bytes (the counts give %llu, %llu bytes)", path, ivf_section_name[k],
+                   (unsigned long long)h.sec[k].offset, (unsigned long long)h.sec[k].bytes, (unsigned long long)want[k].offset,
+                   (unsigned long long)want[k].bytes);
+  const uint64_t end = want[IVF_FILE_SECTIONS - 1].offset + want[IVF_FILE_SECTIONS - 1].bytes;
+  if (file_bytes != end) IVF_BAD_FILE("file is %llu bytes, its sections end at %llu", path, (unsigned long long)file_bytes, (unsigned long long)end);
+#undef IVF_BAD_FILE
+  return STB_OK;
+}
+
+static double ivf_ms_since(std::chrono::steady_clock::time_point t) {
+  return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count();
+}
+
+// rows [0, n) of the file's corpus are on this corpus's first n rows, the lists are a partition of them (the
+// steps of stb_ivfpq_load after the upload)
+static int ivf_file_verify(stb_ivfpq *x, const IvfFileHeader &h, const char *path) {
+  stb_ctx *ctx = x->ctx;
+  cudaStream_t st = ctx->stream;
+  uint64_t sum[IVF_FILE_SECTIONS + 3];
+  // section checksums before any kernel reads list_off, order or forced as indices
+  IVF_TRY(ivf_file_digests(x, h.sec, false, sum));
+  for (int k = 0; k < IVF_FILE_SECTIONS; ++k)
+    if (sum[k] != h.sec[k].checksum) {
+      stb_set_error("ivfpq_load: %s: section %s does not match its checksum", path, ivf_section_name[k]);
+      return STB_ERR_ARG;
+    }
+  StbBuf<uint32_t> seen;
+  IVF_TRY(seen.alloc((x->n + 31) / 32 + 1));                  // [0]: the status word, then the row bitmap
+  STB_CUDA(cudaMemsetAsync(seen, 0, ((x->n + 31) / 32 + 1) * 4, st));
+  const unsigned ctas = (x->nlist + 7) / 8 + (x->n_forced + 255) / 256;
+  ivf_verify_lists_kernel<<<ctas, 256, 0, st>>>(x->list_off, x->nlist, h.n_listed, x->order, x->forced, x->n_forced, x->n, seen + 1, seen);
+  STB_CUDA(cudaGetLastError());
+  ctx->kernel_launches += 1;
+  uint32_t bad = 0;
+  STB_CUDA(cudaMemcpyAsync(&bad, seen, 4, cudaMemcpyDeviceToHost, st));
+  STB_CUDA(cudaStreamSynchronize(st));
+  if (bad) {
+    stb_set_error("ivfpq_load: %s: the lists are not a partition of rows [0, %llu):%s%s%s%s%s", path, (unsigned long long)x->n,
+                  bad & IVF_BAD_OFF ? " list_off does not run from 0 to n_listed without decreasing;" : "",
+                  bad & IVF_BAD_ROW ? " an order entry is >= n;" : "", bad & IVF_BAD_ORDER ? " a list is not strictly ascending;" : "",
+                  bad & IVF_BAD_FORCED ? " forced is not strictly ascending below n;" : "",
+                  bad & IVF_BAD_DUP ? " a row appears twice in order and forced;" : "");
+    return STB_ERR_ARG;
+  }
+  IVF_TRY(ivf_file_digests(x, h.sec, true, sum));
+  if (sum[IVF_FILE_SECTIONS] != h.rows_digest) {
+    stb_set_error("ivfpq_load: %s: the corpus rows [0, %llu) are not the rows the index was saved with (rows_digest)", path,
+                  (unsigned long long)x->n);
+    return STB_ERR_STATE;
+  }
+  if (sum[IVF_FILE_SECTIONS + 1] != x->n_forced || sum[IVF_FILE_SECTIONS + 2] != 0) {
+    stb_set_error("ivfpq_load: %s: forced holds %u rows, the rows have %llu that cannot be normalised (%llu of them missing)", path,
+                  x->n_forced, (unsigned long long)sum[IVF_FILE_SECTIONS + 1], (unsigned long long)sum[IVF_FILE_SECTIONS + 2]);
+    return STB_ERR_ARG;
+  }
+  return STB_OK;
+}
+
+extern "C" {
+
+int stb_ivfpq_save(const stb_ivfpq *x, const char *path) {
+  if (!x || !path) { stb_set_error("ivfpq_save: null argument"); return STB_ERR_ARG; }
+  stb_ctx *ctx = x->ctx;
+  if (cudaSetDevice(ctx->device) != cudaSuccess) { stb_set_error("cudaSetDevice failed"); return STB_ERR_CUDA; }
+  const stb_corpus *c = x->corpus;
+  if (c->epoch != x->corpus_epoch || c->n < x->n) {
+    stb_set_error("ivfpq_save: the corpus was cleared since the index last read it (%llu rows, the index holds %llu)",
+                  (unsigned long long)c->n, (unsigned long long)x->n);
+    return STB_ERR_STATE;
+  }
+  STB_CUDA(cudaStreamSynchronize(ctx->stream));
+  IvfFileHeader h;
+  memset(&h, 0, sizeof(h));
+  memcpy(h.magic, "STBIVFPQ", 8);
+  h.version = IVF_FILE_VERSION; h.d = STB_D; h.pq_m = PQ_M; h.pq_ksub = PQ_KSUB; h.pq_dsub = PQ_DSUB; h.nlist = x->nlist;
+  h.n = x->n; h.n_listed = x->list_off_h[x->nlist]; h.n_forced = x->n_forced;
+  ivf_file_layout(h.nlist, h.n_listed, h.n_forced, h.sec);
+  uint64_t sum[IVF_FILE_SECTIONS + 3];
+  IVF_TRY(ivf_file_digests(x, h.sec, true, sum));
+  for (int k = 0; k < IVF_FILE_SECTIONS; ++k) h.sec[k].checksum = sum[k];
+  h.rows_digest = sum[IVF_FILE_SECTIONS];
+  h.header_checksum = ivf_digest_host(&h, offsetof(IvfFileHeader, header_checksum));
+  IvfFilePipe pp;
+  IVF_TRY(pp.init());
+  // a new file beside `path`, renamed over it once complete and on disk
+  // (a name taken, e.g. by a file a crashed process with the same pid left behind, moves on to the next serial)
+  static std::atomic<unsigned> serial{0};
+  std::string tmp;
+  int fd = -1;
+  for (int tries = 0; fd < 0 && tries < 1000; ++tries) {
+    tmp = std::string(path) + ".tmp." + std::to_string((long)getpid()) + "." + std::to_string(serial++);
+    fd = open(tmp.c_str(), O_WRONLY | O_CREAT | O_EXCL | O_CLOEXEC, 0666);
+    if (fd < 0 && errno != EEXIST) break;
+  }
+  if (fd < 0) { stb_set_error("ivfpq_save: cannot create %s: %s", tmp.c_str(), strerror(errno)); return STB_ERR_ARG; }
+  int rc = STB_OK;
+  if (!ivf_pio(fd, true, reinterpret_cast<uint8_t *>(&h), sizeof(h), 0)) {
+    stb_set_error("ivfpq_save: cannot write %s: %s", tmp.c_str(), strerror(errno));
+    rc = STB_ERR_ARG;
+  }
+  for (int k = 0; k < IVF_FILE_SECTIONS && rc == STB_OK; ++k)
+    rc = ivf_file_write(ctx, pp, fd, ivf_section_dev(x, k), h.sec[k].bytes, h.sec[k].offset, tmp.c_str());
+  if (rc == STB_OK && fsync(fd) != 0) { stb_set_error("ivfpq_save: fsync %s: %s", tmp.c_str(), strerror(errno)); rc = STB_ERR_ARG; }
+  if (close(fd) != 0 && rc == STB_OK) { stb_set_error("ivfpq_save: close %s: %s", tmp.c_str(), strerror(errno)); rc = STB_ERR_ARG; }
+  if (rc == STB_OK && rename(tmp.c_str(), path) != 0) {
+    stb_set_error("ivfpq_save: rename %s -> %s: %s", tmp.c_str(), path, strerror(errno));
+    rc = STB_ERR_ARG;
+  }
+  if (rc != STB_OK) { unlink(tmp.c_str()); return rc; }
+  // the rename itself reaches the disk with the directory
+  const std::string p(path);
+  const size_t slash = p.rfind('/');
+  const int dfd = open(slash == std::string::npos ? "." : slash == 0 ? "/" : p.substr(0, slash).c_str(), O_RDONLY | O_DIRECTORY | O_CLOEXEC);
+  if (dfd >= 0) { fsync(dfd); close(dfd); }
+  return STB_OK;
+}
+
+int stb_ivfpq_load(stb_ctx *ctx, const stb_corpus *corpus, const char *path, stb_ivfpq **out) {
+  if (!ctx || !corpus || !path || !out) { stb_set_error("ivfpq_load: null argument"); return STB_ERR_ARG; }
+  *out = nullptr;
+  if (corpus->ctx != ctx) { stb_set_error("ivfpq_load: corpus belongs to another context"); return STB_ERR_ARG; }
+  if (corpus->host_rows) { stb_set_error("ivfpq_load: not available on a corpus whose rows are in host memory"); return STB_ERR_STATE; }
+  if (cudaSetDevice(ctx->device) != cudaSuccess) { stb_set_error("cudaSetDevice failed"); return STB_ERR_CUDA; }
+  const auto t0 = std::chrono::steady_clock::now();
+  const int fd = open(path, O_RDONLY | O_CLOEXEC);
+  if (fd < 0) { stb_set_error("ivfpq_load: cannot open %s: %s", path, strerror(errno)); return STB_ERR_ARG; }
+  struct FdCloser { int fd; ~FdCloser() { close(fd); } } closer{fd};
+  struct stat sb;
+  IvfFileHeader h;
+  if (fstat(fd, &sb) != 0 || (uint64_t)sb.st_size < sizeof(h) || !ivf_pio(fd, false, reinterpret_cast<uint8_t *>(&h), sizeof(h), 0)) {
+    stb_set_error("ivfpq_load: %s: shorter than the %zu-byte header", path, sizeof(h));
+    return STB_ERR_ARG;
+  }
+  IVF_TRY(ivf_file_check_header(h, (uint64_t)sb.st_size, path));
+  if (corpus->n < h.n) {
+    stb_set_error("ivfpq_load: %s indexes %llu rows, the corpus holds %llu", path, (unsigned long long)h.n, (unsigned long long)corpus->n);
+    return STB_ERR_STATE;
+  }
+  stb_ivfpq *x = new (std::nothrow) stb_ivfpq();
+  if (!x) { stb_set_error("out of host memory"); return STB_ERR_NOMEM; }
+  // not counted in corpus->ivfpq_live until it is installed: a refusal deletes it without stb_ivfpq_destroy
+  cudaStream_t st = ctx->stream;
+  auto fail = [&](int rc) {
+    cudaStreamSynchronize(st);
+    cudaGetLastError();
+    delete x;
+    return rc;
+  };
+  x->ctx = ctx; x->corpus = corpus; x->nlist = h.nlist; x->n = h.n; x->n_forced = (uint32_t)h.n_forced;
+  int rc;
+  if ((rc = ivf_edit_buf(x->centroids, h.sec[0].bytes)) != STB_OK || (rc = ivf_edit_buf(x->codebooks, h.sec[1].bytes)) != STB_OK ||
+      (rc = ivf_edit_buf(x->list_off, h.sec[2].bytes)) != STB_OK || (rc = ivf_edit_buf(x->order, h.sec[3].bytes)) != STB_OK ||
+      (rc = ivf_edit_buf(x->codes, h.sec[4].bytes)) != STB_OK || (rc = ivf_edit_buf(x->forced, IVF_FORCED_CAP * 4)) != STB_OK)
+    return fail(rc);
+  {
+    IvfFilePipe pp;
+    if ((rc = pp.init()) != STB_OK) return fail(rc);
+    for (int k = 0; k < IVF_FILE_SECTIONS; ++k)
+      if ((rc = ivf_file_read(ctx, pp, fd, ivf_section_dev(x, k), h.sec[k].bytes, h.sec[k].offset, path)) != STB_OK)
+        return fail(rc);
+    if (cudaStreamSynchronize(st) != cudaSuccess) { stb_set_error("ivfpq_load: upload failed"); return fail(STB_ERR_CUDA); }
+  }
+  x->load_ms[0] = ivf_ms_since(t0);
+  const auto t1 = std::chrono::steady_clock::now();
+  if ((rc = ivf_file_verify(x, h, path)) != STB_OK) return fail(rc);
+  x->load_ms[1] = ivf_ms_since(t1);
+  x->list_off_h.resize(h.nlist + 1);
+  if (cudaMemcpy(x->list_off_h.data(), x->list_off, ((size_t)h.nlist + 1) * 4, cudaMemcpyDeviceToHost) != cudaSuccess) {
+    stb_set_error("ivfpq_load: list_off copy failed");
+    return fail(STB_ERR_CUDA);
+  }
+  if ((rc = ivf_alloc_query_scratch(x)) != STB_OK) return fail(rc);
+  if (cudaStreamSynchronize(st) != cudaSuccess) { stb_set_error("ivfpq_load: scratch set-up failed"); return fail(STB_ERR_CUDA); }
+  x->corpus_epoch = corpus->epoch;
+  const_cast<stb_corpus *>(corpus)->ivfpq_live++;
+  *out = x;
+  return STB_OK;
+}
+
+int stb_debug_ivfpq_load_ms(const stb_ivfpq *x, double ms[2]) {
+  if (!x || !ms) { stb_set_error("ivfpq_load_ms: null argument"); return STB_ERR_ARG; }
+  ms[0] = x->load_ms[0]; ms[1] = x->load_ms[1];
   return STB_OK;
 }
 
